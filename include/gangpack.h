@@ -419,7 +419,9 @@ typedef struct {
     int64_t pack_kernel_ns;    /* device time of the pack kernel (CUDA events on the launch stream) */
     int64_t prep_kernel_ns;    /* device time of the kernels before it (preparation / shape classification + capacity tables) */
     int64_t scan_path_apps;    /* independent tightly/evenly: applications decided by the node-order scan instead of the
-                                  per-shape capacity tables (all of them with GANGPACK_TABLES=0) */
+                                  per-shape capacity tables (all of them with GANGPACK_TABLES=0).
+                                  FIFO modes: applications decided by the whole CTA instead of warp 0 alone (every
+                                  evaluated one with GANGPACK_FIFO_WARP=0) */
     int64_t scan_path_nodes;   /* executor-order entries those scans visited (nodes_scanned also counts table probes) */
     int64_t reserved[1];
 } gp_stats;

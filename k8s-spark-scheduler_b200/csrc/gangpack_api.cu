@@ -354,6 +354,7 @@ struct gp_ctx {
     size_t one_bytes = 0;
     int zero_copy = 1;                            // GANGPACK_ZERO_COPY=0 disables reading/writing mapped host buffers in kernels
     int use_tables = 1;                           // GANGPACK_TABLES=0: every independent decision takes the node-order scan
+    int fifo_warp = 1;                            // GANGPACK_FIFO_WARP=0: every FIFO application is decided by the whole CTA
     bool async_snapshot = false;                  // gp_config.flags & GP_CFG_ASYNC_SNAPSHOT
     int chunk_apps = kChunkApps;                  // GANGPACK_CHUNK_APPS
     int trace = 0;                                // GANGPACK_TRACE=1: host-side phase timing on stderr
@@ -515,6 +516,7 @@ gp_status gp_create(gp_ctx** out, const gp_config* cfg) {
     c->async_snapshot = cfg && (cfg->flags & GP_CFG_ASYNC_SNAPSHOT);
     if (const char* z = std::getenv("GANGPACK_ZERO_COPY")) c->zero_copy = std::atoi(z);
     if (const char* z = std::getenv("GANGPACK_TABLES")) c->use_tables = std::atoi(z);
+    if (const char* z = std::getenv("GANGPACK_FIFO_WARP")) c->fifo_warp = std::atoi(z);
     if (const char* z = std::getenv("GANGPACK_GRAPHS")) c->use_graphs = std::atoi(z);
     if (const char* z = std::getenv("GANGPACK_CHUNK_APPS")) c->chunk_apps = std::max(1024, std::atoi(z));
     if (const char* z = std::getenv("GANGPACK_TRACE")) c->trace = std::atoi(z);
@@ -833,8 +835,10 @@ static void launch_pack(gp_ctx* c, gp_mode mode, const Snapshot& s, const PrepAp
         // FIFO: one persistent 1024-thread CTA per instance group, its slots staged in shared memory
         bool& attr_set = c->fifo_attr_set[ALGO];     // per device: function attributes live in the device's context
         if (!attr_set) {
-            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
-            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
+            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
+            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
+            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
+            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
             attr_set = true;
         }
         // small groups: fewer threads per CTA (the per-application fixed cost scales with the CTA size)
@@ -843,10 +847,9 @@ static void launch_pack(gp_ctx* c, gp_mode mode, const Snapshot& s, const PrepAp
         (void)avg_ne;
         int32_t* app_list = c->fifo_list.as<int32_t>();
         unsigned int* cursor = reinterpret_cast<unsigned int*>(c->dev_misc.as<char>() + 56);     // zeroed by pack_begin
-        if (mode == GP_MODE_FIFO_REFERENCE)
-            gp_pack_fifo_cta<ALGO, 1><<<s.n_groups, kFifoThreadsRt, kFifoSmemBytes, st>>>(s, prep, app_group, n_apps, driver_node, executor_nodes, scratch, stats, s.gmins, app_list, cursor);
-        else
-            gp_pack_fifo_cta<ALGO, 2><<<s.n_groups, kFifoThreadsRt, kFifoSmemBytes, st>>>(s, prep, app_group, n_apps, driver_node, executor_nodes, scratch, stats, s.gmins, app_list, cursor);
+        auto kern = mode == GP_MODE_FIFO_REFERENCE ? (c->fifo_warp ? gp_pack_fifo_cta<ALGO, 1, true> : gp_pack_fifo_cta<ALGO, 1, false>)
+                                                   : (c->fifo_warp ? gp_pack_fifo_cta<ALGO, 2, true> : gp_pack_fifo_cta<ALGO, 2, false>);
+        kern<<<s.n_groups, kFifoThreadsRt, kFifoSmemBytes, st>>>(s, prep, app_group, n_apps, driver_node, executor_nodes, scratch, stats, s.gmins, app_list, cursor);
         // the FIFO kernels subtract usage from `pair` in place: refresh the compact 32-bit view so that a later
         // independent pack on this context (the driver's own pack after fitEarlierDrivers, resource.go:255 then :321)
         // sees the charged availability

@@ -567,7 +567,10 @@ __device__ __forceinline__ int32_t fifo_app_warp(const Snapshot& s, const GroupD
     return slot_node[d1];
 }
 
-template <int ALGO, int FIFO_MODE>
+// WARP_FIRST = false (GANGPACK_FIFO_WARP=0): warp 0 keeps the queue and the dead prefixes but hands every application to
+// the whole CTA -- a second device implementation of the same decision (a template parameter: the default kernel carries
+// no extra branch)
+template <int ALGO, int FIFO_MODE, bool WARP_FIRST>
 __global__ void __launch_bounds__(kFifoThreads, 1) gp_pack_fifo_cta(Snapshot s, const PrepApp* __restrict__ prep,
                                                                     const int32_t* __restrict__ app_group, int32_t n_apps,
                                                                     int32_t* __restrict__ driver_node,
@@ -698,8 +701,8 @@ __global__ void __launch_bounds__(kFifoThreads, 1) gp_pack_fifo_cta(Snapshot s, 
                             start_d = min(g.nd, start_d + kWarp);
                         }
                     }
-                    int32_t r = kEscalate;                         // general arithmetic class: the CTA decides
-                    if (fl & kAppFast)
+                    int32_t r = kEscalate;                         // general arithmetic class (or !WARP_FIRST): the CTA decides
+                    if (WARP_FIRST && (fl & kAppFast))
                         r = view.all_smem ? fifo_app_warp<ALGO, FIFO_MODE>(s, g, view_s, pa, executor_nodes, cache, start_e, start_d, dcur, ecur, st, true, lane)
                                           : fifo_app_warp<ALGO, FIFO_MODE>(s, g, view, pa, executor_nodes, cache, start_e, start_d, dcur, ecur, st, drv_identity, lane);
                     if (r == kEscalate) {

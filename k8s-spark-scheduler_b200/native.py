@@ -619,6 +619,9 @@ class GangPacker:
         return bool(has.value), d.value, en[:count] if has.value else en[:0]
 
     def stats(self) -> dict:
+        """gp_last_stats of the last pack call.  scan_path_apps: independent tightly / evenly batches count the applications
+        the node-order scan decided instead of the capacity tables; the FIFO modes count the applications the whole CTA
+        decided instead of warp 0 alone (all evaluated ones with GANGPACK_FIFO_WARP=0)."""
         s = gp_stats()
         self._check(load().gp_last_stats(self._h, C.byref(s)))
         return {"nodes_scanned": s.nodes_scanned, "drivers_tried": s.drivers_tried, "kernel_launches": s.kernel_launches,

@@ -100,6 +100,36 @@ def literal_batch(oracle, algo, cpu, mem, gpu, drv_idx, exec_idx, apps, n_thread
     return dn, en, off
 
 
+def group_slices(dn, en, off, sel):
+    """The results of the applications `sel` (queue order) as their own batch: (driver_node, executor_nodes, off)."""
+    sel = np.asarray(sel, np.int64)
+    cnt = (off[sel + 1] - off[sel]).astype(np.int64)
+    sub_off = np.zeros(len(sel) + 1, np.int64)
+    np.cumsum(cnt, out=sub_off[1:])
+    idx = np.repeat(off[sel] - sub_off[:-1], cnt) + np.arange(int(sub_off[-1]), dtype=np.int64)
+    return np.asarray(dn)[sel], np.asarray(en)[idx], sub_off
+
+
+def fifo_vs_closed(oracle, algo, mode, cpu, mem, gpu, eorder, dorder, eoff, doff, apps, got, label=""):
+    """fitEarlierDrivers per instance group through the closed form: every driver_node (incl. -1 / -2) and every
+    ExecutorNodes slice of `got` must match, group by group (the groups are disjoint node sets, so the oracle runs them
+    one after the other on the availability the previous one left).  Returns the final (cpu, mem, gpu)."""
+    dn, en, off = got
+    group = np.asarray(apps.get("group", np.zeros(len(apps["count"]), np.int32)))
+    avail = (np.asarray(cpu, np.int64), np.asarray(mem, np.int64), np.asarray(gpu, np.int64))
+    for g in range(len(eoff) - 1):
+        sel = np.nonzero(group == g)[0]
+        if sel.size == 0:
+            continue
+        sub = {k: np.asarray(apps[k])[sel] for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu", "count", "young")}
+        drv = res_aos(sub["drv_cpu"], sub["drv_mem"], sub["drv_gpu"])
+        exe = res_aos(sub["exe_cpu"], sub["exe_mem"], sub["exe_gpu"])
+        _, wd, we, woff, avail = oracle.closed_batch(algo, mode, avail[0], avail[1], avail[2], dorder[doff[g]:doff[g + 1]],
+                                                     eorder[eoff[g]:eoff[g + 1]], drv, exe, sub["count"], sub["young"])
+        assert_same_results(group_slices(dn, en, off, sel), (wd, we, woff), f"{label} group {g}")
+    return avail
+
+
 def literal_fifo(oracle, algo, mode, cpu, mem, gpu, drv_idx, exec_idx, apps, young):
     """fitEarlierDrivers through the literal restatement -> ((driver_node, executor_nodes, off), final (cpu, mem, gpu))."""
     names = node_names(len(cpu))

@@ -4,7 +4,7 @@ clusters, the synthetic bench workload, and all FIFO modes including the final s
 import numpy as np
 import pytest
 
-from helpers import (ALGO_ID, MODE_ID, assert_same_results, case_arrays, order_indices, random_apps,
+from helpers import (ALGO_ID, MODE_ID, assert_same_results, case_arrays, fifo_vs_closed, order_indices, random_apps,
                      random_cluster, res_aos)
 
 pytestmark = pytest.mark.gpu
@@ -368,13 +368,14 @@ def test_device_resident_api(oracle, packer):
 
 
 @pytest.mark.parametrize("mode", [1, 2])
-def test_fifo_full_size_conservation(packer, mode):
+def test_fifo_full_size_conservation(oracle, packer, mode):
     """BASELINE configs[1] in FIFO mode at full size (10k nodes x 10k apps): size-independent properties.
     (i) conservation: initial - final availability equals the usage recomputed from the emitted placements under
     the mode's accounting (reference: each distinct executor node one executor, driver node charged the driver
     only if it hosts no executor -- EXT/sparkpods.go:139-146; exact: every pod); (ii) after the first blocking
     application nothing is evaluated; (iii) every placement respected the availability at its turn (no node
-    ever goes below its running balance by more than the accounting allows)."""
+    ever goes below its running balance by more than the accounting allows); (iv) every one of the 10 000 decisions and
+    the final snapshot equal the closed-form oracle's."""
     import k8s_spark_scheduler_b200.synth as synth
     N, Q = 10000, 10000
     nodes = synth.make_nodes(N)
@@ -414,6 +415,30 @@ def test_fifo_full_size_conservation(packer, mode):
         assert np.array_equal(nodes["avail_cpu"] - use_cpu, fc), (algo, mode)
         assert np.array_equal(nodes["avail_mem"] - use_mem, fm), (algo, mode)
         assert fits.sum() > 1000
+        # (iv) bit-exact against the oracle
+        final = fifo_vs_closed(oracle, algo, mode, nodes["avail_cpu"], nodes["avail_mem"], nodes["avail_gpu"], order, order,
+                               [0, N], [0, N], a, (dn, en, off), f"fifo full size algo {algo} mode {mode}")
+        fg = packer.get_snapshot()[2]
+        assert np.array_equal(fc, final[0]) and np.array_equal(fm, final[1]) and np.array_equal(fg, final[2]), (algo, mode)
+
+
+@pytest.mark.parametrize("mode", [1, 2])
+def test_fifo_da_50k_vs_oracle(oracle, packer, mode):
+    """bench.py's fifo-da-50k shape (BASELINE configs[3]: 10k nodes in 16 instance groups, 50 000 queued drivers of a
+    dynamic-allocation sweep), every decision and the final snapshot against the closed form, group by group."""
+    import k8s_spark_scheduler_b200.synth as synth
+    nodes = synth.make_nodes(10000, groups=16)
+    apps = synth.make_apps(50000, groups=16, da_sweep=True, young_frac=0.05)
+    eoff, eorder = synth.group_orders(nodes)
+    a = {k: apps[k] for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu", "count", "group", "young")}
+    for algo in (0, 1):
+        packer.set_snapshot(nodes["avail_cpu"], nodes["avail_mem"], nodes["avail_gpu"], eorder, eorder, eoff, eoff)
+        got = packer.pack_batch(a, algo, mode)
+        final = fifo_vs_closed(oracle, algo, mode, nodes["avail_cpu"], nodes["avail_mem"], nodes["avail_gpu"], eorder, eorder,
+                               eoff, eoff, a, got, f"fifo-da-50k algo {algo} mode {mode}")
+        fc, fm, fg = packer.get_snapshot()
+        assert np.array_equal(fc, final[0]) and np.array_equal(fm, final[1]) and np.array_equal(fg, final[2]), (algo, mode)
+        assert (got[0] >= 0).sum() > 10000
 
 
 def _potential_nodes_inputs(names, zones):

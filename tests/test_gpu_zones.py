@@ -247,3 +247,141 @@ def test_reschedule_availability_double_counts_overhead(oracle, packer):
     plain, _ = packer.build_availability(alloc, over, rnode, res)
     has = np.zeros(n, bool); has[rnode[rnode >= 0]] = True
     assert np.array_equal(plain[0] - got[0], over[0] * has)         # exactly one extra overhead where a reservation exists
+
+
+def _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, sc, sm, sg, zone_of, order_d, order_e, apps, fifo, label):
+    """Both single-AZ packers (and, for the FIFO loop, both accounting modes) on the device against the literal
+    restatement with efficiencies -> [(algo, mode, zone, driver_node)] of the device runs."""
+    n = len(cpu)
+    names = node_names(n)
+    labels = ["zone-%d" % z for z in zone_of]
+    zones, eo, do, eoff, doff = _zone_groups(order_d, order_e, zone_of)
+    drv = res_aos(apps["drv_cpu"], apps["drv_mem"], apps["drv_gpu"]); exe = res_aos(apps["exe_cpu"], apps["exe_mem"], apps["exe_gpu"])
+    runs = []
+    for algo, oalgo in ((0, 2), (2, 5)):
+        for mode in ((1, 2) if fifo else (0,)):
+            cl = oracle.Cluster(names, cpu, mem, gpu, sched=(sc, sm, sg), zone=labels)
+            packer.set_snapshot(cpu, mem, gpu, eo, do, eoff, doff)
+            packer.set_schedulable(sc, sm, sg)
+            if fifo:
+                _, wd, we, woff = cl.fifo(oalgo, mode, drv, exe, apps["count"], apps["young"], [names[i] for i in order_d],
+                                          [names[i] for i in order_e], with_efficiencies=True)
+                zone, gd, ge, goff, _ = packer.pack_fifo_zones(apps, algo, mode)
+            else:
+                wd, we, woff = cl.binpack_batch(oalgo, drv, exe, apps["count"], [names[i] for i in order_d], [names[i] for i in order_e],
+                                                with_efficiencies=True, n_threads=4)
+                zone, gd, ge, goff, _ = packer.pack_batch_zones(apps, algo)
+            assert np.array_equal(goff, woff)
+            bad = np.nonzero(gd != wd)[0]
+            assert bad.size == 0, (label, algo, mode, bad[:5], gd[bad[:5]], wd[bad[:5]], zone[bad[:5]])
+            for i in np.nonzero(wd >= 0)[0]:
+                assert np.array_equal(ge[goff[i]:goff[i + 1]], we[woff[i]:woff[i + 1]]), (label, algo, mode, i)
+                assert zone[i] == zones.index(zone_of[wd[i]]), (label, algo, mode, i)
+            assert (zone[wd < 0] == -1).all()
+            if fifo:
+                fc, fm, fg = packer.get_snapshot()
+                wc, wm, wg = cl.available()
+                assert np.array_equal(fc, wc) and np.array_equal(fm, wm) and np.array_equal(fg, wg), (label, algo, mode)
+            runs.append((algo, mode, zone, gd))
+    return runs
+
+
+def _many_zones(seed, Z, per, q):
+    rng = np.random.default_rng(seed)
+    n = Z * per
+    cpu, mem, gpu = random_cluster(rng, n)
+    sc = cpu + rng.integers(0, 9, n) * 250 + (rng.integers(0, 3, n) == 0) * 1
+    sm = mem + rng.integers(0, 17, n) * (1 << 28)
+    zone_of = rng.permutation(np.arange(n) % Z)               # every zone has nodes
+    order_e = [int(i) for i in rng.permutation(n)]
+    order_d = [int(i) for i in rng.permutation(n)]
+    rank = {z: r for r, z in enumerate(_zone_groups(order_d, order_e, zone_of)[0])}
+    late = np.array([rank[z] >= 32 for z in zone_of])         # more of these nodes in use: higher efficiencies, they win often
+    sc, sm = sc + late * 16000, sm + late * (64 << 30)
+    apps = random_apps(rng, q)
+    apps["young"] = (rng.random(q) < 0.97).astype(np.uint8)
+    return cpu, mem, gpu, sc, sm, gpu.clip(0), zone_of, order_d, order_e, apps
+
+
+@pytest.mark.parametrize("Z", [16, 17, 33, 64])
+def test_fifo_zones_beyond_one_warp(oracle, packer, Z):
+    """gp_pack_fifo_zones strides the zones over 16 warps: winners packed by a warp other than 0 and by the second stride
+    (z >= 16), up to the 64-zone limit of its shared-memory table."""
+    cpu, mem, gpu, sc, sm, sg, zone_of, order_d, order_e, apps = _many_zones(5000 + Z, Z, 6, 120)
+    runs = _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, sc, sm, sg, zone_of, order_d, order_e, apps, True, f"Z={Z}")
+    won = np.concatenate([zone[gd >= 0] for _, _, zone, gd in runs])
+    assert (won % 16 != 0).any()                              # a warp other than 0
+    if Z > 16:
+        assert (won >= 16).any()                              # the second stride
+
+
+@pytest.mark.parametrize("Z", [31, 32, 33, 70])
+def test_batch_zones_across_warp_steps(oracle, packer, Z):
+    """gp_zone_choose walks the zones 32 per warp step and applies the tie rule across steps."""
+    cpu, mem, gpu, sc, sm, sg, zone_of, order_d, order_e, apps = _many_zones(5100 + Z, Z, 5, 150)
+    runs = _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, sc, sm, sg, zone_of, order_d, order_e, apps, False, f"Z={Z}")
+    won = np.concatenate([zone[gd >= 0] for _, _, zone, gd in runs])
+    assert (won >= 32).any() if Z > 32 else (won >= 24).any()
+
+
+@pytest.mark.parametrize("first_fit_zone", [0, 31])
+def test_zone_ties_go_to_the_first_zone(oracle, packer, first_fit_zone):
+    """40 zones, identical from `first_fit_zone` on (the zones before it cannot host a driver): every tie of the averages
+    goes to the first zone (strict '<', single_az.go:91-94).  With 31, the tie spans the 32-zone step of gp_zone_choose
+    and the two warp strides of gp_pack_fifo_zones."""
+    Z, per = 40, 3
+    n = Z * per
+    zone_of = np.repeat(np.arange(Z), per)
+    cpu = np.where(zone_of < first_fit_zone, 200, np.tile([8000, 6000, 4000], Z)).astype(np.int64)
+    mem = np.tile([32 << 30, 24 << 30, 16 << 30], Z).astype(np.int64)
+    gpu = np.zeros(n, np.int64)
+    sc, sm = cpu + 8000, mem + (32 << 30)
+    order = list(range(n))
+    q = 24
+    i = np.arange(q)
+    apps = {"drv_cpu": np.full(q, 1000, np.int64), "drv_mem": np.full(q, 1 << 30, np.int64), "drv_gpu": np.zeros(q, np.int64),
+            "exe_cpu": 500 * (1 + i % 3), "exe_mem": (1 << 30) * (1 + i % 2), "exe_gpu": np.zeros(q, np.int64),
+            "count": (1 + i % 4).astype(np.int32), "young": np.ones(q, np.uint8)}
+    runs = _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, sc, sm, gpu, zone_of, order, order, apps, False, "ties batch")
+    for _, _, zone, gd in runs:
+        assert (gd >= 0).all() and (zone == first_fit_zone).all()
+    runs = _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, sc, sm, gpu, zone_of, order, order, apps, True, "ties fifo")
+    for _, _, zone, gd in runs:
+        assert zone[0] == first_fit_zone
+
+
+@pytest.mark.parametrize("young", [0, 1])
+def test_zero_efficiency_picks_no_zone(oracle, packer, young):
+    """A driver-only application with zero requests on untouched nodes packs with an average efficiency of exactly 0.0:
+    chooseBestResult keeps nothing (best starts at 0.0, strict '<'), so it fits nowhere; in the FIFO loop a non-young one
+    then blocks the queue."""
+    n = 12
+    cpu = np.full(n, 8000, np.int64); mem = np.full(n, 32 << 30, np.int64); gpu = np.zeros(n, np.int64)
+    zone_of = np.arange(n) % 3
+    order = list(range(n))
+    apps = {"drv_cpu": np.array([0, 1000, 1000], np.int64), "drv_mem": np.array([0, 1 << 30, 1 << 30], np.int64),
+            "drv_gpu": np.zeros(3, np.int64), "exe_cpu": np.array([1000, 2000, 1000], np.int64),
+            "exe_mem": np.full(3, 2 << 30, np.int64), "exe_gpu": np.zeros(3, np.int64),
+            "count": np.array([0, 2, 1], np.int32), "young": np.array([young, 0, 0], np.uint8)}
+    runs = _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, cpu, mem, gpu, zone_of, order, order, apps, True, "zero eff fifo")
+    for _, _, zone, gd in runs:
+        assert gd[0] == -1 and zone[0] == -1
+        assert (gd[1:] >= 0).all() if young else (gd[1:] == -2).all()
+    runs = _zone_literal_vs_device(oracle, packer, cpu, mem, gpu, cpu, mem, gpu, zone_of, order, order, apps, False, "zero eff batch")
+    for _, _, zone, gd in runs:
+        assert gd[0] == -1 and (gd[1:] >= 0).all()
+
+
+def test_fifo_zones_refuses_more_than_64(packer, gangpack):
+    n = 65 * 2
+    cpu = np.full(n, 8000, np.int64); mem = np.full(n, 32 << 30, np.int64); gpu = np.zeros(n, np.int64)
+    order = list(range(n))
+    _, eo, do, eoff, doff = _zone_groups(order, order, np.arange(n) % 65)
+    packer.set_snapshot(cpu, mem, gpu, eo, do, eoff, doff)
+    packer.set_schedulable(cpu, mem, gpu)
+    apps = random_apps(np.random.default_rng(1), 4)
+    with pytest.raises(gangpack.native.GangpackError) as e:
+        packer.pack_fifo_zones(apps, 0, 1)
+    assert e.value.status == 1
+    zone, gd, _, _, _ = packer.pack_batch_zones(apps, 0)          # the independent form has no zone limit
+    assert (gd >= 0).any() and (zone[gd >= 0] < 65).all()
