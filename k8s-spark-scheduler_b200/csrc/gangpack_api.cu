@@ -152,18 +152,6 @@ __device__ __forceinline__ int32_t find_group(const int32_t* off, int32_t n_grou
     return lo;
 }
 
-__global__ void gp_build_groups(int32_t n_groups, const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
-                                GroupDesc* __restrict__ groups) {
-    int32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= n_groups) return;
-    GroupDesc d;
-    d.sbase = exec_off[g] + drv_off[g];
-    d.ne = exec_off[g + 1] - exec_off[g];
-    d.dbase = drv_off[g];
-    d.nd = drv_off[g + 1] - drv_off[g];
-    groups[g] = d;
-}
-
 // snapshot-wide facts: negative gpu availability, per-dimension maxima (bounds for the fast class)
 // Called by the threads of a warp that own a node (`active` = their mask): the warp combines its values with
 // shuffles and issues at most one atomic per dimension.
@@ -188,51 +176,92 @@ __device__ __forceinline__ void note_node(SnapMeta* meta, int64_t cv, int64_t mv
     }
 }
 
-// executor-order entries -> slots [sbase, sbase+ne)
-__global__ void gp_build_exec_slots(int32_t n_exec, int32_t n_groups,
+// The slot layout is two launches (gp_set_snapshot, gp_set_snapshot_device, gp_prepare_cluster):
+// K1 gp_build_slots_exec: thread i writes group descriptor i, lays out executor-order entry i in its slot and notes the
+//    availability of driver-order entry i in the snapshot maxima / flags (a node's availability does not depend on its slot);
+// K2 gp_build_slots_drv: thread s owns slot s.  Executor slots get their compact view; the spare slot of driver-order
+//    entry j either receives that node (driver-only) or stays unused (-1: the node has an executor slot in the group);
+//    slots past the last group (the orders' lengths may be upper bounds) are -1 as well.  So no slot_node memset is needed.
+// n_exec / n_drv may be upper bounds of exec_off[n_groups] / drv_off[n_groups] (device-built orders).
+__global__ void gp_build_slots_exec(int32_t n_exec, int32_t n_drv, int32_t n_groups,
                                     const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
-                                    const int32_t* __restrict__ exec_order,
+                                    const int32_t* __restrict__ exec_order, const int32_t* __restrict__ drv_order,
                                     const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
-                                    longlong2* __restrict__ pair, int64_t* __restrict__ sgpu, int32_t* __restrict__ slot_node,
-                                    int32_t* __restrict__ node_slot, SnapMeta* __restrict__ meta) {
-    int32_t e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= n_exec || e >= exec_off[n_groups]) return;     // n_exec may be an upper bound (device-built orders)
-    int32_t g = find_group(exec_off, n_groups, e);
-    int32_t slot = exec_off[g] + drv_off[g] + (e - exec_off[g]);
-    int32_t node = exec_order[e];
-    const int64_t cv = cpu[node], mv = mem[node], gv = gpu ? gpu[node] : 0;
-    pair[slot] = make_longlong2(cv, mv);
-    sgpu[slot] = gv;
-    note_node(meta, cv, mv, gv);
-    slot_node[slot] = node;
-    node_slot[node] = slot;
-}
-
-// driver-order entries -> group-local slot (an executor slot, or the spare slot ne + j)
-__global__ void gp_build_driver_slots(int32_t n_drv, int32_t n_groups,
-                                      const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
-                                      const int32_t* __restrict__ drv_order,
-                                      const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
-                                      longlong2* __restrict__ pair, int64_t* __restrict__ sgpu, int32_t* __restrict__ slot_node,
-                                      int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_slot, SnapMeta* __restrict__ meta) {
-    int32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n_drv || j >= drv_off[n_groups]) return;       // n_drv may be an upper bound
-    int32_t g = find_group(drv_off, n_groups, j);
-    int32_t sbase = exec_off[g] + drv_off[g];
-    int32_t ne = exec_off[g + 1] - exec_off[g];
-    int32_t node = drv_order[j];
-    int32_t ns = node_slot[node];
-    if (ns >= sbase && ns < sbase + ne) {
-        drv_slot[j] = ns - sbase;
-    } else {
-        int32_t local = ne + (j - drv_off[g]);
-        int32_t slot = sbase + local;
+                                    GroupDesc* __restrict__ groups, longlong2* __restrict__ pair, int64_t* __restrict__ sgpu,
+                                    int32_t* __restrict__ slot_node, int32_t* __restrict__ node_slot, SnapMeta* __restrict__ meta) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_groups) {
+        GroupDesc d;
+        d.sbase = exec_off[i] + drv_off[i];
+        d.ne = exec_off[i + 1] - exec_off[i];
+        d.dbase = drv_off[i];
+        d.nd = drv_off[i + 1] - drv_off[i];
+        groups[i] = d;
+    }
+    if (i < n_exec && i < exec_off[n_groups]) {
+        const int32_t g = find_group(exec_off, n_groups, i);
+        const int32_t slot = exec_off[g] + drv_off[g] + (i - exec_off[g]);
+        const int32_t node = exec_order[i];
         const int64_t cv = cpu[node], mv = mem[node], gv = gpu ? gpu[node] : 0;
         pair[slot] = make_longlong2(cv, mv);
         sgpu[slot] = gv;
         note_node(meta, cv, mv, gv);
         slot_node[slot] = node;
-        node_slot[node] = slot;          // the node's availability lives in its spare slot (gp_reserve_placements / gp_apply_usage_delta)
+        node_slot[node] = slot;
+    }
+    if (i < n_drv && i < drv_off[n_groups]) {
+        const int32_t node = drv_order[i];
+        note_node(meta, cpu[node], mem[node], gpu ? gpu[node] : 0);
+    }
+}
+
+__device__ __forceinline__ int shift_for(long long mx);
+__device__ __forceinline__ uint2 compact_pair(longlong2 v, int s0, int s1);
+
+__global__ void gp_build_slots_drv(int32_t n_slots, int32_t n_groups,
+                                   const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
+                                   const int32_t* __restrict__ drv_order,
+                                   const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
+                                   longlong2* __restrict__ pair, int64_t* __restrict__ sgpu, int32_t* __restrict__ slot_node,
+                                   int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_slot, SnapMeta* __restrict__ meta,
+                                   uint2* __restrict__ pair32) {
+    const int s0 = shift_for(meta->max_avail[0]), s1 = shift_for(meta->max_avail[1]);
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s == 0) { meta->shift32[0] = s0; meta->shift32[1] = s1; }
+    if (s > n_slots) return;
+    if (s >= exec_off[n_groups] + drv_off[n_groups]) {       // past the last group
+        slot_node[s] = -1;
+        if (s < n_slots) pair32[s] = make_uint2(0u, 0u);
+        return;
+    }
+    // the group whose slots [exec_off[g] + drv_off[g], exec_off[g+1] + drv_off[g+1]) hold s
+    int32_t lo = 0, hi = n_groups - 1;
+    while (lo < hi) {
+        const int32_t mid = (lo + hi + 1) >> 1;
+        if (exec_off[mid] + drv_off[mid] <= s) lo = mid; else hi = mid - 1;
+    }
+    const int32_t g = lo;
+    const int32_t sbase = exec_off[g] + drv_off[g];
+    const int32_t ne = exec_off[g + 1] - exec_off[g];
+    const int32_t local = s - sbase;
+    if (local < ne) {                                        // executor slot, laid out by K1
+        pair32[s] = compact_pair(pair[s], s0, s1);
+        return;
+    }
+    const int32_t j = drv_off[g] + (local - ne);
+    const int32_t node = drv_order[j];
+    const int32_t ns = node_slot[node];
+    if (ns >= sbase && ns < sbase + ne) {
+        drv_slot[j] = ns - sbase;
+        slot_node[s] = -1;                                   // unused spare slot
+        pair32[s] = make_uint2(0u, 0u);
+    } else {
+        const longlong2 v = make_longlong2(cpu[node], mem[node]);
+        pair[s] = v;
+        sgpu[s] = gpu ? gpu[node] : 0;
+        pair32[s] = compact_pair(v, s0, s1);
+        slot_node[s] = node;
+        node_slot[node] = s;             // the node's availability lives in its spare slot (gp_reserve_placements / gp_apply_usage_delta)
         drv_slot[j] = local;
     }
 }
@@ -260,17 +289,20 @@ __device__ __forceinline__ int shift_for(long long mx) {
     const int bits = 64 - __clzll(mx);
     return bits > 32 ? bits - 32 : 0;
 }
+__device__ __forceinline__ uint2 compact_pair(longlong2 v, int s0, int s1) {
+    uint2 o;
+    o.x = v.x < 0 ? 0u : (uint32_t)((unsigned long long)v.x >> s0);
+    o.y = v.y < 0 ? 0u : (uint32_t)((unsigned long long)v.y >> s1);
+    return o;
+}
+// the compact view again after a kernel that charged `pair` (FIFO, reservations, usage deltas)
 __global__ void gp_fill_pair32(int32_t n_slots, const longlong2* __restrict__ pair, SnapMeta* __restrict__ meta,
                                uint2* __restrict__ pair32) {
     const int s0 = shift_for(meta->max_avail[0]), s1 = shift_for(meta->max_avail[1]);
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0) { meta->shift32[0] = s0; meta->shift32[1] = s1; }
     if (i >= n_slots) return;
-    const longlong2 v = pair[i];
-    uint2 o;
-    o.x = v.x < 0 ? 0u : (uint32_t)((unsigned long long)v.x >> s0);
-    o.y = v.y < 0 ? 0u : (uint32_t)((unsigned long long)v.y >> s1);
-    pair32[i] = o;
+    pair32[i] = compact_pair(pair[i], s0, s1);
 }
 
 // slots -> node-table order (gp_get_snapshot)
@@ -361,8 +393,8 @@ struct gp_ctx {
     int pack_ctas_per_sm[3] = {0, 0, 0};            // occupancy of gp_pack_independent<ALGO> on this device
     int tab_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_pack_tables<ALGO, OUT>
     bool tab_attr_set[2] = {false, false};
-    // per pipeline lane: shape hash + header, capacity tables, group totals, per-application shape slot
-    struct TableSet { DevBuf hdr, table, total, app_slot; } tabs[kLanes];
+    // per pipeline lane: shape hash + header, capacity tables, group totals, placement prefixes, per-application shape slot
+    struct TableSet { DevBuf hdr, table, total, place, app_slot; } tabs[kLanes];
     bool record_events = true;                    // CUDA events around the kernels (gp_last_stats); the pipelined host path skips them
     int use_graphs = 1;                           // GANGPACK_GRAPHS=0: always issue the launches one by one
     GraphCache g_chunk[kMaxChunks + 1];           // per pipelined chunk (+1: an unchunked batch on the context's own stream): classify .. scan
@@ -616,22 +648,20 @@ static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_
     void* bufs[8] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p};
     std::memcpy(key.buf, bufs, sizeof(bufs));
     gp_status rs = run_cached(c, c->g_snapshot, &key, sizeof(key), st, [&](int& launches) -> gp_status {
-        GP_CUDA(c, cudaMemsetAsync(c->slot_node.p, 0xFF, sizeof(int32_t) * (size_t)(n_slots + 1), st));
+        // node_slot must be -1 for every node outside the orders (K2 reads it for the driver-order nodes); every slot_node
+        // entry is written by K1 or K2
         GP_CUDA(c, cudaMemsetAsync(c->node_slot.p, 0xFF, sizeof(int32_t) * (size_t)(dn->n_nodes + 1), st));
         GP_CUDA(c, cudaMemsetAsync(c->snap_flags.p, 0, sizeof(SnapMeta), st));
         const int T = 256;
-        gp_build_groups<<<(dn->n_groups + T - 1) / T, T, 0, st>>>(dn->n_groups, dn->exec_off, dn->drv_off, c->groups.as<GroupDesc>());
-        if (n_exec > 0)
-            gp_build_exec_slots<<<(n_exec + T - 1) / T, T, 0, st>>>(
-                n_exec, dn->n_groups, dn->exec_off, dn->drv_off, dn->exec_order, dn->avail_cpu_milli, dn->avail_mem_bytes,
-                dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(), c->slot_node.as<int32_t>(),
-                c->node_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>());
-        if (n_drv > 0)
-            gp_build_driver_slots<<<(n_drv + T - 1) / T, T, 0, st>>>(
-                n_drv, dn->n_groups, dn->exec_off, dn->drv_off, dn->drv_order, dn->avail_cpu_milli, dn->avail_mem_bytes,
-                dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(), c->slot_node.as<int32_t>(),
-                c->node_slot.as<int32_t>(), c->drv_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>());
-        gp_fill_pair32<<<(n_slots + T) / T, T, 0, st>>>(n_slots, c->pair.as<longlong2>(), c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
+        const int32_t n1 = std::max(std::max(n_exec, n_drv), dn->n_groups);
+        gp_build_slots_exec<<<(n1 + T - 1) / T, T, 0, st>>>(
+            n_exec, n_drv, dn->n_groups, dn->exec_off, dn->drv_off, dn->exec_order, dn->drv_order, dn->avail_cpu_milli,
+            dn->avail_mem_bytes, dn->avail_gpu, c->groups.as<GroupDesc>(), c->pair.as<longlong2>(), c->sgpu.as<int64_t>(),
+            c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>());
+        gp_build_slots_drv<<<(n_slots + T) / T, T, 0, st>>>(
+            n_slots, dn->n_groups, dn->exec_off, dn->drv_off, dn->drv_order, dn->avail_cpu_milli, dn->avail_mem_bytes,
+            dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(), c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(),
+            c->drv_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
         GP_CUDA(c, cudaGetLastError());
         launches = 0;       // (the snapshot layout is not part of a pack call's launch count)
         return GP_OK;
@@ -919,6 +949,7 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         if (use_tables) {
             GP_CUDA(c, T.table.reserve(sizeof(uint32_t) * (size_t)kMaxShapes * (size_t)((c->n_slots + 4) & ~3)));
             GP_CUDA(c, T.total.reserve(3 * sizeof(uint32_t) * (size_t)kMaxShapes * (size_t)c->n_groups));   // total | firstfit | first_host
+            GP_CUDA(c, T.place.reserve(sizeof(int32_t) * (size_t)kMaxShapes * (size_t)c->n_groups * kPlaceLen));
         }
         ShapeTables tabs;
         tabs.hdr = T.hdr.as<ShapeHeader>();
@@ -927,6 +958,7 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         tabs.table = T.table.as<uint32_t>(); tabs.total = T.total.as<uint32_t>();
         tabs.firstfit = reinterpret_cast<int32_t*>(T.total.as<uint32_t>() + (size_t)kMaxShapes * (size_t)c->n_groups);
         tabs.first_host = tabs.firstfit + (size_t)kMaxShapes * (size_t)c->n_groups;
+        tabs.place = T.place.as<int32_t>();
         tabs.pitch = (c->n_slots + 4) & ~3; tabs.n_groups = c->n_groups;      // rows start 16-byte aligned
         int64_t* off_out = nullptr;
         if (!da.cols.off) {                       // derive the offsets on the device

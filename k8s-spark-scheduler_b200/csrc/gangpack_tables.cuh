@@ -18,16 +18,19 @@
 //                         into shared memory by TMA bulk copies (cp.async.bulk + mbarrier, double-buffered), every
 //                         thread evaluates 4 consecutive nodes, a block-wide exclusive scan turns capacities into the
 //                         prefix table  S[i] = sum_{n<i} min(cap(n|0), CLAMP)   (tightly-pack) or
-//                                       M[i] = #{n<i : cap(n|0) >= 1}            (distribute-evenly);
+//                                       M[i] = #{n<i : cap(n|0) >= 1}            (distribute-evenly),
+//                         and the first kPlaceLen entries of the driver-free placement P[t] = node of the t-th executor;
 //       (same launch, second half of the grid: one CTA per (driver shape, instance group) finds the first driver candidate
 //       the shape fits on);
 //   K3 gp_decide_tables   ONE THREAD per application (with the tables a decision is O(log N + k) scalar work -- a warp per
 //                         application, right for an O(N) scan, would idle 31 lanes): feasibility is
 //                         S[ne] - delta(d) >= k  per driver candidate d starting at the shape's first fit (delta = what the
 //                         driver displaces on its own node: O(1) per candidate, the reference's loop binpack.go:67-85
-//                         verbatim), the walk starts at the shape's first hosting node (one word per (shape, group), written
-//                         by K2), ExecutorNodes is emitted by walking the table from there with the next word always in
-//                         flight (zero-capacity runs are jumped by a galloping search).
+//                         verbatim).  ExecutorNodes is P shifted by delta past the driver's run, written by the whole warp
+//                         with coalesced stores, when its largest index k - 1 + delta is below kPlaceLen; otherwise it is
+//                         emitted by walking the table from the shape's first hosting node (one word per (shape, group),
+//                         written by K2) with the next word always in flight (zero-capacity runs are jumped by a galloping
+//                         search).
 // What the tables cannot answer exactly -- more than kMaxShapes distinct shapes in a batch, executor counts above the table
 // clamp, distribute-evenly placements that need more than one round -- is appended, already prepared (PrepApp), to a list
 // that the warp-per-application scan kernel gp_pack_listed (the node-order scan of gangpack_kernels.cuh) works off.
@@ -45,6 +48,7 @@ constexpr int kMaxShapes = 64;        // dense tables per batch
 constexpr int kTabThreads = 1024;
 constexpr int kTabPerThread = 4;
 constexpr int kTabTile = kTabThreads * kTabPerThread;     // 4096 nodes per tile: 64 KB of (cpu, mem)
+constexpr int kPlaceLen = 256;        // placement prefix per (shape, group): covers every count <= 128 whatever the driver takes
 
 struct __align__(16) ShapeEntry {     // 96 bytes
     unsigned long long key;           // fingerprint, never 0; 0 = empty (claimed with atomicCAS)
@@ -82,6 +86,8 @@ struct ShapeTables {
     uint32_t* total;                  // [kMaxShapes][n_groups]
     int32_t* firstfit;                // [kMaxShapes][n_groups] first driver-order position the driver shape fits on (nd: none)
     int32_t* first_host;              // [kMaxShapes][n_groups] first executor-order position with capacity > 0 for the shape (ne: none)
+    int32_t* place;                   // [kMaxShapes][n_groups][kPlaceLen] node receiving the t-th executor without a driver
+                                      // (entries t >= the group's total are not written)
     int32_t pitch;                    // row length (>= n_slots, multiple of 4)
     int32_t n_groups;
 };
@@ -277,6 +283,7 @@ __global__ void __launch_bounds__(kTabThreads, 1) gp_build_shape_tables(Snapshot
     const longlong2* gpair = s.pair + g.sbase;
     const int64_t* ggpu = s.gpu + g.sbase;
     uint32_t* out = tabs.table + (size_t)id * tabs.pitch + g.sbase;
+    int32_t* place = tabs.place + ((size_t)id * tabs.n_groups + grp) * kPlaceLen;
 
     if (tid == 0) { mbar_init(&sh.bar[0], 1); mbar_init(&sh.bar[1], 1); sh.first_host = ne; }
     __syncthreads();
@@ -335,6 +342,20 @@ __global__ void __launch_bounds__(kTabThreads, 1) gp_build_shape_tables(Snapshot
         } else {
 #pragma unroll
             for (int j = 0; j < kTabPerThread; ++j) if (i0 + j < ne) out[i0 + j] = base + v[j];
+        }
+        // placement prefix: a node whose first executor index is below kPlaceLen writes its run [S, min(S + c, kPlaceLen))
+        // (the CTA writes at most kPlaceLen words in all; only the first hosting nodes of the order do anything)
+        if (base < (uint32_t)kPlaceLen) {
+#pragma unroll
+            for (int j = 0; j < kTabPerThread; ++j) {
+                const uint32_t p0 = base + v[j];
+                const uint32_t p1 = base + (j + 1 < kTabPerThread ? v[j + 1] : sum);
+                if (p0 < p1 && p0 < (uint32_t)kPlaceLen) {
+                    const int32_t node = __ldg(s.slot_node + g.sbase + i0 + j);
+                    const uint32_t end = p1 < (uint32_t)kPlaceLen ? p1 : (uint32_t)kPlaceLen;
+                    for (uint32_t t = p0; t < end; ++t) place[t] = node;
+                }
+            }
         }
         carry += tile_total;
         __syncthreads();            // tile[t & 1] and part[t & 1] may be overwritten from here on
@@ -414,7 +435,11 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
                                                                    unsigned long long* __restrict__ stats, int* __restrict__ err,
                                                                    volatile int* __restrict__ err_host, int force_scan) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
     unsigned long long probes = 0, drivers = 0;
+    // this lane's share of the warp's coalesced emission (sh_k = 0: none): out[sh_dst + t] = place[sh_src + shifted t]
+    uint32_t sh_k = 0, sh_cut = 0, sh_delta = 0;
+    int64_t sh_dst = 0, sh_src = 0;
     if (i < n_apps) {
         const int64_t d_cpu = cols.load(0, i), d_mem = cols.load(1, i), d_gpu = cols.load(2, i);
         const int64_t e_cpu = cols.load(3, i), e_mem = cols.load(4, i), e_gpu = cols.load(5, i);
@@ -472,16 +497,16 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
                     }
                 }
                 int32_t dslot = -1;
-                uint32_t cd = 0, c0d = 0;
+                uint32_t cd = 0, c0d = 0, sd = 0;
                 for (; j < nd; ++j) {
                     ++drivers;
                     const int32_t ls = s.drv_slot[g.dbase + j];
                     const longlong2 v = __ldg(gpair + ls);
                     const int64_t gv = (drv_gpu || cap_gpu) ? __ldg(ggpu + ls) : 0;
                     if ((d_cpu > v.x) || (d_mem > v.y) || (drv_gpu && d_gpu > gv)) continue;
-                    uint32_t my_c0 = 0, my_cd = 0;
+                    uint32_t my_c0 = 0, my_cd = 0, sp = 0;
                     if (ls < ne && k != 0) {
-                        const uint32_t sp = __ldg(tab + ls);
+                        sp = __ldg(tab + ls);
                         my_c0 = tab_at(tab, ls + 1, ne, total) - sp;
                         probes += 2;
                         if (my_c0 != 0) {        // what the node can still take once the driver sits on it
@@ -493,17 +518,27 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
                         if (ALGO == 0 && total - (my_c0 - my_cd) < k) continue;       // the executors do not fit with this driver
                         // distribute-evenly: >= k+1 hosting nodes, the driver removes at most its own
                     }
-                    dslot = ls; cd = my_cd; c0d = my_c0;
+                    dslot = ls; cd = my_cd; c0d = my_c0; sd = sp;
                     break;
                 }
                 if (dslot >= 0) {
                     result = s.slot_node[g.sbase + dslot];
-                    if (k != 0) {
+                    // ---- emission by index shift: the driver's node takes cd instead of c0 executors, so every executor
+                    // after its run comes delta = c0 - cd places later in the driver-free placement P:
+                    //   out[t] = P[t < S(d) + cd ? t : t + delta]      (delta = 0 on a driver-only node: c0 = cd = 0)
+                    // The warp writes these after the branch, coalesced; larger indices walk the table below.
+                    const uint32_t delta = c0d - cd;
+                    if (k != 0 && (uint64_t)k - 1u + delta < (uint64_t)kPlaceLen) {
+                        sh_k = k; sh_delta = delta;
+                        sh_cut = min(sd + cd, (uint32_t)kPlaceLen);     // S(d) + cd <= total; >= kPlaceLen: no shift below k
+                        sh_dst = off;
+                        sh_src = ((int64_t)en->id * tabs.n_groups + grp) * kPlaceLen;
+                        probes += k;                            // one P word per executor
+                    } else if (k != 0) {
                         // ---- emission: walk the prefix table from the first hosting node ---------------------------------
                         OUT* out = executor_nodes + off;
                         const int32_t* slot_node = s.slot_node + g.sbase;
                         const int32_t dpos = (dslot < ne) ? dslot : 0x7fffffff;
-                        (void)c0d;
                         int32_t pos = __ldg(tabs.first_host + (size_t)en->id * tabs.n_groups + grp);    // first node with room for the shape
                         ++probes;
                         uint32_t prev = 0, placed = 0;
@@ -560,6 +595,25 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
             } else {
                 driver_node[i] = result;
             }
+        }
+    }
+    // ---- coalesced emission of the index-shift lanes: the warp's executor indices are concatenated in lane order, and
+    // every 32-index chunk is written by the whole warp (owner lane of index e: binary search over the inclusive scan)
+    {
+        const uint32_t incl = warp_incl_scan(sh_k, lane);
+        const uint32_t n_out = __shfl_sync(kFull, incl, 31);
+        const uint32_t excl = incl - sh_k;
+        const int64_t dst = sh_dst - (int64_t)excl, src = sh_src - (int64_t)excl;     // index e of the concatenation
+        const uint32_t cut = excl + sh_cut;
+        for (uint32_t e0 = 0; e0 < n_out; e0 += 32) {
+            const uint32_t e = e0 + (uint32_t)lane;
+            int owner = 0;                              // number of lanes whose indices all lie before e
+#pragma unroll
+            for (int step = 16; step >= 1; step >>= 1)
+                if (__shfl_sync(kFull, incl, owner + step - 1) <= e) owner += step;
+            const int64_t o_dst = __shfl_sync(kFull, dst, owner), o_src = __shfl_sync(kFull, src, owner);
+            const uint32_t o_cut = __shfl_sync(kFull, cut, owner), o_delta = __shfl_sync(kFull, sh_delta, owner);
+            if (e < n_out) executor_nodes[o_dst + e] = (OUT)__ldg(tabs.place + o_src + e + (e < o_cut ? 0u : o_delta));
         }
     }
     // statistics: one atomic per warp
