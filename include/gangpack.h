@@ -337,8 +337,9 @@ gp_status gp_synchronize(gp_ctx* ctx);
  * [driver] + ExecutorNodes, duplicates kept, sequential sums, cpu through Quantity.Value() -- and the zone with the highest
  * AvgPackingEfficiency.Max wins: the first among equals, and none when every average is 0 (:80, :91).  For
  * minimal-fragmentation the efficiencies see the driver only (minimalFragmentation never adds its executors to
- * SparkBinPack's reserved map) -- kept.  "az-aware-tightly-pack" (az_aware_pack_tightly.go:27-38) = this call, then plain
- * gp_pack_batch(GP_TIGHTLY_PACK) over the undivided orders for the applications that got zone -1.
+ * SparkBinPack's reserved map) -- kept.  "az-aware-tightly-pack" (az_aware_pack_tightly.go:27-38) for independent decisions =
+ * this call, then plain gp_pack_batch(GP_TIGHTLY_PACK) over the undivided orders for the applications that got zone -1;
+ * under FIFO it is gp_pack_fifo_az_aware below.
  * gp_set_schedulable: NodeSchedulingMetadata.SchedulableResources of the current snapshot's nodes (resources.go:61-100). */
 gp_status gp_set_schedulable(gp_ctx* ctx, const int64_t* sched_cpu_milli, const int64_t* sched_mem_bytes, const int64_t* sched_gpu /* or NULL */);
 typedef struct {
@@ -357,8 +358,35 @@ gp_status gp_pack_batch_zones(gp_ctx* ctx, const gp_apps* apps /* group, skip_if
  * driver_node -1 and -- unless skip_if_no_fit[i] -- blocks the queue: everything behind it reports driver_node -2
  * (never evaluated, resource.go:244-253).  The availability the device holds afterwards is what the loop left (read it
  * with gp_get_snapshot).  At most 64 zones; exec_out_off must be NULL or the prefix sum of exe_count.
- * ("az-aware-tightly-pack" needs the undivided orders for its fallback and stays a per-driver call sequence.) */
+ * ("az-aware-tightly-pack" needs the undivided orders for its fallback: gp_pack_fifo_az_aware.) */
 gp_status gp_pack_fifo_zones(gp_ctx* ctx, const gp_apps* apps /* group ignored */, gp_algo algo, gp_mode mode, gp_zone_results* out);
+
+/* The FIFO loop with "az-aware-tightly-pack" (AzAwareTightlyPack, LIB/binpack/az_aware_pack_tightly.go:27-38) in ONE launch.
+ * Each queued application is packed in every candidate zone with tightly-pack and the zone is chosen exactly like
+ * gp_pack_fifo_zones; when no zone wins, SparkBinPack(tightlyPackExecutors) runs over the UNDIVIDED driver / executor orders
+ * against the availability the loop holds at that point, on the device, before the next application is tried.  Either
+ * placement is charged like gp_pack_fifo_zones (mode GP_MODE_FIFO_REFERENCE or GP_MODE_FIFO_EXACT); an application that
+ * fits neither way blocks or is skipped like there.
+ * Snapshot (gp_set_snapshot, then gp_set_schedulable): groups 0..n_zones-1 are the candidate zones in driverZonesInOrder
+ * order (zones without executor candidates left out, single_az.go:38-41), each with the undivided orders restricted to its
+ * nodes; groups n_zones.. hold the other nodes of the two orders (a zone with driver candidates only, executor candidates of
+ * a zone without driver candidates), which only the fallback reaches.  With n_zones = 0 every application takes the
+ * fallback: the loop is then plain FIFO tightly-pack.
+ * Results as gp_pack_fifo_zones, plus: zone[i] == -1 && driver_node[i] >= 0 = the undivided fallback placed application i
+ * (its avg_efficiency is four zeros: the reference does not use the fallback's efficiencies).
+ * GP_ERR_INVALID (gp_last_error names the cause): an independent mode; n_zones above 64 or above n_groups; no
+ * gp_set_schedulable; a snapshot from gp_set_snapshot_device / gp_prepare_cluster (no host copy to check the orders
+ * against); order lengths other than exec_off[n_groups] / drv_off[n_groups]; an order entry out of range, repeated or not
+ * listed by the snapshot in that role; a zone group whose order is not the undivided order restricted to its nodes. */
+typedef struct {
+    int32_t n_zones;                 /* 0..64: snapshot groups 0..n_zones-1 are the candidate zones */
+    int32_t n_exec;
+    const int32_t* exec_order;       /* [n_exec] executorNodePriorityOrder, undivided, node indices */
+    int32_t n_drv;
+    const int32_t* drv_order;        /* [n_drv] driverNodePriorityOrder, undivided, node indices */
+} gp_az_orders;
+gp_status gp_pack_fifo_az_aware(gp_ctx* ctx, const gp_apps* apps /* group ignored */, gp_mode mode, const gp_az_orders* orders,
+                                gp_zone_results* out);
 
 /* ---- reservation table of a batch + a snapshot that stays on the device (SURVEY 8f rows f4 and f2) ---------------
  * gp_reserve_placements: newResourceReservation (internal/extender/resourcereservations.go:491-528) for every application
@@ -411,7 +439,8 @@ gp_status gp_multi_group_owner(gp_multi* m, int32_t* owner /* [n_groups] */);
 
 /* Statistics of the last gp_pack_batch* on this context (host call, synchronises the stream):
  * nodes_scanned = executor-order entries visited, drivers_tried = driver-order entries visited,
- * summed over apps -- the N_e / N_d of the algorithmic-bytes formula (DESIGN.md). */
+ * summed over apps -- the N_e / N_d of the algorithmic-bytes formula (DESIGN.md); gp_pack_fifo_az_aware includes the
+ * scans of its undivided fallback in both. */
 typedef struct {
     int64_t nodes_scanned;
     int64_t drivers_tried;
@@ -421,7 +450,8 @@ typedef struct {
     int64_t scan_path_apps;    /* independent tightly/evenly: applications decided by the node-order scan instead of the
                                   per-shape capacity tables (all of them with GANGPACK_TABLES=0).
                                   FIFO modes: applications decided by the whole CTA instead of warp 0 alone (every
-                                  evaluated one with GANGPACK_FIFO_WARP=0) */
+                                  evaluated one with GANGPACK_FIFO_WARP=0).
+                                  gp_pack_fifo_az_aware: applications for which the undivided fallback ran, placed or not */
     int64_t scan_path_nodes;   /* executor-order entries those scans visited (nodes_scanned also counts table probes) */
     int64_t reserved[1];
 } gp_stats;

@@ -380,6 +380,11 @@ struct gp_ctx {
     void* pinned_misc = nullptr;                         // 32 B pinned mirror of dev_misc
     std::vector<int64_t> host_off;
     std::vector<int32_t> v_owner;                 // gp_set_snapshot validation scratch (no per-call allocation)
+    // gp_set_snapshot's host copy of the layout, kept for gp_pack_fifo_az_aware's order checks: v_owner[v] (group, roles)
+    // and v_pos[v] / v_pos[n_nodes + v] (position of v in its group's executor / driver order).  host_layout: they
+    // describe the current snapshot (false after gp_set_snapshot_device / gp_prepare_cluster or a refused gp_set_snapshot)
+    std::vector<int32_t> v_pos;
+    bool host_layout = false;
     std::vector<uint8_t> v_seen_e, v_seen_d;
     std::vector<std::pair<const char*, size_t>> pinned_blocks;   // gp_alloc_pinned allocations (device-mapped under UVA)
     void* one_block = nullptr;                    // gp_pack_one staging (mapped pinned)
@@ -636,6 +641,7 @@ gp_status gp_synchronize(gp_ctx* ctx) {
 // Build the slot layout from DEVICE-resident gp_nodes arrays on `st`.
 static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, cudaStream_t st) {
     const int32_t n_slots = n_exec + n_drv;
+    c->host_layout = false;              // gp_set_snapshot sets it again once the layout it validated is in place
     GP_CUDA(c, c->pair.reserve(sizeof(longlong2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->pair32.reserve(sizeof(uint2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->sgpu.reserve(sizeof(int64_t) * (size_t)(n_slots + 1)));
@@ -691,15 +697,19 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot: order arrays missing");
     {
         // owner[v] = 4 * group + (bit0: listed as executor candidate, bit1: listed as driver candidate); -1 = unseen
+        c->host_layout = false;
         std::vector<int32_t>& owner = c->v_owner;
         owner.assign((size_t)n->n_nodes, -1);
         const uint32_t N = (uint32_t)n->n_nodes;
+        c->v_pos.resize(2 * (size_t)N);
+        int32_t* pos = c->v_pos.data();
         for (int32_t g = 0; g < G; ++g) {
             for (int32_t e = n->exec_off[g]; e < n->exec_off[g + 1]; ++e) {
                 const uint32_t v = (uint32_t)n->exec_order[e];
                 if (v >= N) return fail(c, GP_ERR_INVALID, "gp_set_snapshot: exec_order index out of range");
                 if (owner[v] >= 0) return fail(c, GP_ERR_INVALID, "gp_set_snapshot: node listed twice in executor orders");
                 owner[v] = 4 * g + 1;
+                pos[v] = e - n->exec_off[g];
             }
         }
         for (int32_t g = 0; g < G; ++g) {
@@ -710,6 +720,7 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
                 if (o >= 0 && (o & 2)) return fail(c, GP_ERR_INVALID, "gp_set_snapshot: node listed twice in driver orders");
                 if (o >= 0 && (o >> 2) != g) return fail(c, GP_ERR_INVALID, "gp_set_snapshot: node belongs to two instance groups");
                 owner[v] = 4 * g + (o >= 0 ? (o & 3) : 0) + 2;
+                pos[N + v] = d - n->drv_off[g];
             }
         }
         // exact-int64 domain: branch-free so that the loop vectorises
@@ -771,6 +782,7 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
     dn.exec_order = c->exec_order.as<int32_t>(); dn.drv_order = c->drv_order.as<int32_t>();
     gp_status s = build_snapshot_device(c, &dn, n_exec, n_drv, st);
     if (s != GP_OK) return s;
+    c->host_layout = true;
     // GP_CFG_ASYNC_SNAPSHOT with page-locked inputs: return while the device is still reading them -- the upload and the
     // slot layout then overlap the H2D copies of the gp_pack_* call that follows
     if (!(c->async_snapshot && all_mapped)) GP_CUDA(c, cudaStreamSynchronize(st));   // the caller may reuse its host buffers
@@ -1517,21 +1529,16 @@ static gp_status refresh_views(gp_ctx* c, bool raised, cudaStream_t st) {
     return GP_OK;
 }
 
-// the FIFO loop with a single-AZ packer in one launch (gangpack_zonefifo.cuh)
-gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode mode, gp_zone_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_zones: gp_set_snapshot first");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
-    if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: NULL apps/results");
-    if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
-        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: the single-AZ packers are tightly-pack and minimal-fragmentation");
-    if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
-        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones)");
-    const int32_t Q = a->n_apps, Z = c->n_groups;
-    if (Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
+// The FIFO loop over zones in one launch (gangpack_zonefifo.cuh), shared by gp_pack_fifo_zones (kind = 0 tightly-pack,
+// 2 minimal-fragmentation; the zones are every instance group) and gp_pack_fifo_az_aware (kind = kZoneAzAware; zones
+// 0..Z-1, plus the undivided orders `az` of the fallback, already validated).  Argument checks common to both are here.
+static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, int32_t Z, const gp_az_orders* az,
+                                gp_zone_results* out, const char* who) {
+    const std::string w(who);
+    const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
     if (!a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->zone || !out->driver_node)
-        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: missing app/result arrays");
+        return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
     std::vector<int64_t>& hoff = c->host_off;
     hoff.resize((size_t)Q + 1);
     int64_t acc = 0, pitch = 1;
@@ -1543,19 +1550,23 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
     hoff[(size_t)Q] = acc;
     if (a->exec_out_off)
         for (int32_t i = 0; i <= Q; ++i)
-            if (a->exec_out_off[i] != hoff[(size_t)i]) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: exec_out_off must be the prefix sum of exe_count (or NULL)");
+            if (a->exec_out_off[i] != hoff[(size_t)i]) return fail(c, GP_ERR_INVALID, w + ": exec_out_off must be the prefix sum of exe_count (or NULL)");
     const int64_t total = acc;
-    if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, "gp_pack_fifo_zones: executor_nodes_cap too small");
-    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: executor_nodes is NULL");
+    if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, w + ": executor_nodes_cap too small");
+    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, w + ": executor_nodes is NULL");
     pitch = (pitch + 3) & ~(int64_t)3;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
-    const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)Z * (size_t)pitch;
+    const bool azk = kind == kZoneAzAware;
+    const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)(Z + (azk ? 1 : 0)) * (size_t)pitch;   // az-aware: row Z = fallback
+    const size_t NE = azk ? (size_t)az->n_exec : 0, ND = azk ? (size_t)az->n_drv : 0, NN = azk ? (size_t)c->n_nodes : 0;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
     const size_t o_in = take(48 * q), o_cnt = take(4 * q), o_off = take(8 * (q + 1)), o_skip = take(q), o_rexe = take(4 * RP),
-                 o_rlist = take(algo == GP_MINIMAL_FRAGMENTATION ? 8 * RP : 0), o_zone = take(4 * q), o_drv = take(4 * q),
+                 o_rlist = take(kind == GP_MINIMAL_FRAGMENTATION ? 8 * RP : 0), o_zone = take(4 * q), o_drv = take(4 * q),
                  o_exe = take(4 * (T + 1)), o_avg = take(32 * q);
+    const size_t o_eord = take(4 * NE), o_dord = take(4 * ND), o_npos = take(4 * NN), o_fbe = take(4 * NE), o_fbd = take(4 * ND),
+                 o_fbp = take(4 * ND);
     GP_CUDA(c, c->zonebuf.reserve(o));
     char* b = c->zonebuf.as<char>();
     int2* unused = nullptr;
@@ -1584,16 +1595,30 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
     zi.sched[0] = c->sched.as<long long>(); zi.sched[1] = c->sched.as<long long>() + N; zi.sched[2] = c->sched.as<long long>() + 2 * N;
     zi.node_slot = c->node_slot.as<int32_t>();
     zi.row_exec = (int32_t*)(b + o_rexe);
-    zi.row_list = algo == GP_MINIMAL_FRAGMENTATION ? (int2*)(b + o_rlist) : nullptr;
+    zi.row_list = kind == GP_MINIMAL_FRAGMENTATION ? (int2*)(b + o_rlist) : nullptr;
     zi.row_pitch = pitch; zi.n_apps = Q; zi.n_zones = Z;
     double* avg = out->avg_efficiency ? (double*)(b + o_avg) : nullptr;
     int32_t* zo = (int32_t*)(b + o_zone); int32_t* dq = (int32_t*)(b + o_drv); int32_t* eo = (int32_t*)(b + o_exe);
-    if (algo == GP_TIGHTLY_PACK) {
+    GatherSlots fb{};
+    if (azk) {
+        if (NE) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * NE, cudaMemcpyHostToDevice, st));
+        if (ND) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * ND, cudaMemcpyHostToDevice, st));
+        gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)NE, (int32_t)ND, (const int32_t*)(b + o_eord), (const int32_t*)(b + o_dord),
+                                                   c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe),
+                                                   (int32_t*)(b + o_fbd), (int32_t*)(b + o_fbp));
+        c->last.kernel_launches += 1;
+        fb.exec_slot = (const int32_t*)(b + o_fbe); fb.drv_slot = (const int32_t*)(b + o_fbd); fb.drv_pos = (const int32_t*)(b + o_fbp);
+        fb.ne = (int32_t)NE; fb.nd = (int32_t)ND;
+    }
+    if (kind == GP_TIGHTLY_PACK) {
         if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
         else gp_pack_fifo_zones_cta<0, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-    } else {
+    } else if (kind == GP_MINIMAL_FRAGMENTATION) {
         if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<2, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
         else gp_pack_fifo_zones_cta<2, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+    } else {
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<kZoneAzAware, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
+        else gp_pack_fifo_zones_cta<kZoneAzAware, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
     }
     GP_CUDA(c, cudaGetLastError());
     c->last.kernel_launches += 2;
@@ -1605,6 +1630,70 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
     if (avg) GP_CUDA(c, cudaMemcpyAsync(out->avg_efficiency, avg, 32 * q, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
     return decode_device_error(c, *reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
+}
+
+// the FIFO loop with a single-AZ packer in one launch
+gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode mode, gp_zone_results* out) {
+    if (!c) return GP_ERR_INVALID;
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_zones: gp_set_snapshot first");
+    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: NULL apps/results");
+    if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
+        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: the single-AZ packers are tightly-pack and minimal-fragmentation");
+    if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
+        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones)");
+    const int32_t Z = c->n_groups;
+    if (Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
+    return fifo_zones_run(c, a, (int)algo, mode, Z, nullptr, out, "gp_pack_fifo_zones");
+}
+
+// the FIFO loop with az-aware-tightly-pack in one launch: the zone packs plus the undivided fallback on the device
+gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const gp_az_orders* o, gp_zone_results* out) {
+    if (!c) return GP_ERR_INVALID;
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_az_aware: gp_set_snapshot first");
+    if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
+        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones, "
+                                       "then gp_pack_batch over the undivided orders)");
+    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!a || !out || !o || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: NULL apps/orders/results");
+    const int32_t Z = o->n_zones;
+    if (Z < 0 || Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones must be 0..64");
+    if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones exceeds the snapshot's instance groups");
+    if (!c->host_layout)
+        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
+                                       "gp_prepare_cluster there is no host copy of the layout to check the undivided orders against)");
+    if (o->n_exec != c->n_exec || o->n_drv != c->n_drv)
+        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: order lengths must equal the snapshot's exec_off[n_groups] / drv_off[n_groups]");
+    if ((o->n_exec > 0 && !o->exec_order) || (o->n_drv > 0 && !o->drv_order))
+        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: order arrays missing");
+    // O(N): every entry a node of the snapshot in that role, once; every zone group's order = the undivided order
+    // restricted to that group's nodes (the fallback and the zone packs must see the same priorities)
+    const uint32_t N = (uint32_t)c->n_nodes;
+    const int32_t* owner = c->v_owner.data();
+    const int32_t* pos = c->v_pos.data();
+    for (int role = 0; role < 2; ++role) {
+        const int32_t n = role == 0 ? o->n_exec : o->n_drv;
+        const int32_t* ord = role == 0 ? o->exec_order : o->drv_order;
+        const char* name = role == 0 ? "exec_order" : "drv_order";
+        std::vector<uint8_t>& seen = role == 0 ? c->v_seen_e : c->v_seen_d;
+        seen.assign((size_t)N, 0);
+        int32_t next[kZoneFifoMaxZones] = {};
+        for (int32_t i = 0; i < n; ++i) {
+            const uint32_t v = (uint32_t)ord[i];
+            if (v >= N) return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: ") + name + " entry out of range");
+            if (seen[v]) return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: ") + name + " lists a node twice");
+            seen[v] = 1;
+            const int32_t ow = owner[v];
+            if (ow < 0 || !(ow & (1 << role)))
+                return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: ") + name + " lists a node the snapshot does not list as " +
+                                                   (role == 0 ? "an executor" : "a driver") + " candidate");
+            const int32_t g = ow >> 2;
+            if (g < Z && pos[(size_t)role * N + v] != next[g]++)
+                return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: zone group ") + std::to_string(g) + "'s " +
+                                                   (role == 0 ? "executor" : "driver") + " order is not " + name + " restricted to its nodes");
+        }
+    }
+    return fifo_zones_run(c, a, kZoneAzAware, mode, Z, o, out, "gp_pack_fifo_az_aware");
 }
 
 gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* placed, int32_t subtract, gp_reservation_table* out) {

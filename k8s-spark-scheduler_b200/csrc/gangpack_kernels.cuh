@@ -325,6 +325,22 @@ struct WarpStats { unsigned long long nodes; unsigned long long drivers; };
 
 constexpr int kCapCache = 1024;   // per-warp shared-memory cache of phase-1 capacities (uint16)
 
+// Where pack_app_impl finds the nodes it scans (slot-mapping policy).
+// GroupSlots: one instance group of the snapshot -- executor-order position i is slot g.sbase + i, driver candidate j has
+//   the group-local slot drv_slot[g.dbase + j] (>= ne: its spare slot).
+// GatherSlots: the undivided orders of az-aware-tightly-pack's fallback (gangpack_zonefifo.cuh), which run across instance
+//   groups -- position i is slot exec_slot[i], driver candidate j is slot drv_slot[j] and executor-order position
+//   drv_pos[j] (-1: not an executor candidate).  Every node has exactly one slot (node_slot), so a charge made through
+//   either view is seen by both.
+struct GroupSlots { static constexpr bool kGather = false; };
+struct GatherSlots {
+    static constexpr bool kGather = true;
+    const int32_t* exec_slot;   // [ne]
+    const int32_t* drv_slot;    // [nd]
+    const int32_t* drv_pos;     // [nd]
+    int32_t ne, nd;
+};
+
 // ---------------------------------------------------------------------------------------------
 // One application, one warp, against an immutable snapshot (GP_MODE_INDEPENDENT; the FIFO modes live in
 // gangpack_fifo.cuh).  Returns the driver's node index (>= 0) or -1.
@@ -333,19 +349,32 @@ constexpr int kCapCache = 1024;   // per-warp shared-memory cache of phase-1 cap
 // MUT: the snapshot changes inside the launch (zone-aware FIFO, gangpack_zones.cuh): coherent loads, never with C32 (the
 // compact view is not kept current).  grp_override / out_override: pack against another instance group than pa->group and
 // write ExecutorNodes (and the candidate list) at another offset than pa->out_off.
-template <int ALGO, bool FAST, bool NOGPU, bool C32, class OUT, bool MUT = false>
+// MAP: GroupSlots, or GatherSlots with `view` (tightly-pack, coherent loads only; grp_override and g0 are then unused).
+template <int ALGO, bool FAST, bool NOGPU, bool C32, class OUT, bool MUT = false, class MAP = GroupSlots>
 __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepApp* __restrict__ pa,
                                                  OUT* __restrict__ executor_nodes, int2* __restrict__ scratch,
                                                  uint16_t* __restrict__ wcache, WarpStats& st, int lane,
                                                  int snap_flags, const GroupDesc& g0,
-                                                 int32_t grp_override = -1, int64_t out_override = -1) {
+                                                 int32_t grp_override = -1, int64_t out_override = -1,
+                                                 const MAP* __restrict__ view = nullptr) {
     static_assert(!(MUT && C32), "the compact view is read-only");
+    static_assert(!MAP::kGather || (ALGO == 0 && MUT && !C32), "the gather scan is tightly-pack over the mutable slots");
     Caps<FAST> a;
     a.init(pa, (pa->flags & kAppUsesGpu) || (snap_flags & kSnapGpuNegative));
     const bool ug = NOGPU ? false : a.use_gpu;      // compile-time false on the hot instantiation
     if (C32) a.init32(s.meta);
-    const int32_t grp = grp_override >= 0 ? grp_override : pa->group;
-    const GroupDesc g = grp == 0 ? g0 : s.groups[grp];   // group 0's descriptor is kept in registers by the caller
+    GroupDesc g;
+    if constexpr (MAP::kGather) {
+        g.sbase = 0; g.ne = view->ne; g.dbase = 0; g.nd = view->nd;   // no group: only the lengths are used
+    } else {
+        const int32_t grp = grp_override >= 0 ? grp_override : pa->group;
+        g = grp == 0 ? g0 : s.groups[grp];                 // group 0's descriptor is kept in registers by the caller
+    }
+    // slot of executor-order position i
+    auto xslot = [&](int32_t i) -> int32_t {
+        if constexpr (MAP::kGather) return __ldg(view->exec_slot + i);
+        else return g.sbase + i;
+    };
     const uint32_t k = a.k;
     const uint32_t lmax = (uint32_t)pa->lmax;
     const int32_t ne = g.ne;
@@ -374,8 +403,8 @@ __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepAp
             if (i0 < ne) c0 = a.cap32(__ldg(s.pair32 + g.sbase + i0));
             if (i1 < ne) c1 = a.cap32(__ldg(s.pair32 + g.sbase + i1));
         } else {
-            if (i0 < ne) c0 = a.template cap0<MUT>(s, g.sbase + i0, ug);
-            if (i1 < ne) c1 = a.template cap0<MUT>(s, g.sbase + i1, ug);
+            if (i0 < ne) c0 = a.template cap0<MUT>(s, xslot(i0), ug);
+            if (i1 < ne) c1 = a.template cap0<MUT>(s, xslot(i1), ug);
         }
         if (cache_ok && i1 < kCapCache) { wcache[i0] = (uint16_t)c0; wcache[i1] = (uint16_t)c1; }
         const unsigned has0 = __ballot_sync(kFull, c0 != 0), has1 = __ballot_sync(kFull, c1 != 0);
@@ -401,29 +430,41 @@ __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepAp
     if (first_nz < 0) first_nz = 0;
 
     // ---- phase 2: first feasible driver candidate (binpack.go:67-85) ----------------------------
-    int32_t dslot = -1;
+    // dslot: the driver's executor-order position (>= ne: not an executor candidate); dglob: its slot
+    int32_t dslot = -1, dglob = -1;
     for (int32_t j0 = 0; j0 < g.nd && dslot < 0; j0 += kWarp) {
         int32_t j = j0 + lane;
         bool feasible = false;
-        int32_t ls = -1;
+        int32_t ls = -1, gs = -1;
         if (j < g.nd) {
-            ls = s.drv_slot[g.dbase + j];
-            feasible = driver_fits<MUT>(s, g.sbase + ls, a, ug);
+            if constexpr (MAP::kGather) {
+                const int32_t p = __ldg(view->drv_pos + j);
+                ls = p < 0 ? ne : p;
+                gs = __ldg(view->drv_slot + j);
+            } else {
+                ls = s.drv_slot[g.dbase + j];
+                gs = g.sbase + ls;
+            }
+            feasible = driver_fits<MUT>(s, gs, a, ug);
             if (feasible && exact_total && ls < ne) {
                 // the executor total with the driver on this node must still reach k
-                uint32_t c0 = a.template cap0<MUT>(s, g.sbase + ls, ug);
-                uint32_t cdl = a.template cap<MUT>(s, g.sbase + ls, a.d_cpu, a.d_mem, a.d_gpu, ug);
+                uint32_t c0 = a.template cap0<MUT>(s, gs, ug);
+                uint32_t cdl = a.template cap<MUT>(s, gs, a.d_cpu, a.d_mem, a.d_gpu, ug);
                 feasible = (P - c0 + cdl >= k);
             }
         }
         unsigned vote = __ballot_sync(kFull, feasible);
         st.drivers += (unsigned long long)((g.nd - j0) < kWarp ? (g.nd - j0) : kWarp);
-        if (vote) dslot = __shfl_sync(kFull, ls, __ffs(vote) - 1);
+        if (vote) {
+            dslot = __shfl_sync(kFull, ls, __ffs(vote) - 1);
+            if constexpr (MAP::kGather) dglob = __shfl_sync(kFull, gs, __ffs(vote) - 1);
+        }
     }
     if (dslot < 0) return -1;
-    const int32_t driver_node = s.slot_node[g.sbase + dslot];
+    if constexpr (!MAP::kGather) dglob = g.sbase + dslot;
+    const int32_t driver_node = s.slot_node[dglob];
     // cap(d | drv): only matters when the driver's node is an executor candidate
-    const uint32_t cd = (dslot < ne && k != 0) ? a.template cap<MUT>(s, g.sbase + dslot, a.d_cpu, a.d_mem, a.d_gpu, ug) : 0u;
+    const uint32_t cd = (dslot < ne && k != 0) ? a.template cap<MUT>(s, dglob, a.d_cpu, a.d_mem, a.d_gpu, ug) : 0u;
 
     // ---- phase 3: emit ExecutorNodes -------------------------------------------------------------
     if (k != 0) {
@@ -435,7 +476,7 @@ __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepAp
                 uint32_t c = 0;
                 if (i == dslot) c = cd;
                 else if (i < cached_end) c = wcache[i];
-                else if (i < ne) c = C32 ? a.cap32(__ldg(s.pair32 + g.sbase + i)) : a.template cap0<MUT>(s, g.sbase + i, ug);
+                else if (i < ne) c = C32 ? a.cap32(__ldg(s.pair32 + g.sbase + i)) : a.template cap0<MUT>(s, xslot(i), ug);
                 if (p0 >= cached_end) st.nodes += (unsigned long long)((ne - p0) < kWarp ? (ne - p0) : kWarp);
                 uint32_t incl = warp_incl_scan(c, lane);
                 uint32_t total = __shfl_sync(kFull, incl, kWarp - 1);
@@ -444,7 +485,7 @@ __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepAp
                 if (T != 0) {
                     uint32_t excl = incl - c;
                     uint32_t take = excl >= T ? 0u : ((c < T - excl) ? c : (T - excl));
-                    int32_t node = (take != 0) ? s.slot_node[g.sbase + i] : -1;
+                    int32_t node = (take != 0) ? s.slot_node[xslot(i)] : -1;
                     // cooperative expansion: output j belongs to the first lane with incl > j
                     for (uint32_t j = lane; j < ((T + kWarp - 1) & ~(uint32_t)(kWarp - 1)); j += kWarp) {
                         int lo = 0;

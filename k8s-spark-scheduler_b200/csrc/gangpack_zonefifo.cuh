@@ -16,6 +16,13 @@
 //      DISTINCT executor node once, the driver only when its node hosts no executor), 2 = every pod;
 //   4. __syncthreads, next application.  A driver that fits nowhere blocks the queue unless it is young
 //      (resource.go:244-253); the applications behind it report -2 like gp_pack_fifo_cta.
+//
+// az-aware-tightly-pack (ALGO kZoneAzAware, az_aware_pack_tightly.go:27-38) packs the zones with tightly-pack like 1. and,
+// when no zone wins in 2., falls back to SparkBinPack(tightlyPackExecutors) over the UNDIVIDED driver / executor orders
+// against the availability the loop holds at that point.  Those orders run across the snapshot's groups (zone groups plus
+// a trailing group with the nodes no candidate zone contains), so warp 0 scans them through a gather view built once per
+// call by gp_build_fallback_view (GatherSlots: position -> slot).  The fallback's placement lands in row Z and is emitted
+// and charged by the code of 3., so both accounting modes share it; it reports zone -1 and zero averages.
 #pragma once
 
 #include "gangpack_kernels.cuh"
@@ -27,6 +34,7 @@ namespace gp {
 constexpr int kZoneFifoWarps = 16;
 constexpr int kZoneFifoThreads = kZoneFifoWarps * 32;
 constexpr int kZoneFifoMaxZones = 64;
+constexpr int kZoneAzAware = 3;               // ALGO of az-aware-tightly-pack (0 and 2 are the single-AZ packers)
 
 struct ZoneFifoIn {
     const long long* sched[3];        // SchedulableResources, node-table order (gpu may be NULL = 0)
@@ -56,15 +64,43 @@ __device__ __forceinline__ void zone_charge(const Snapshot& s, int32_t slot, lon
     if (g != 0) s.gpu[slot] = load_gpu<true>(s.gpu + slot) - mult * g;
 }
 
-// ALGO: 0 tightly-pack, 2 minimal-fragmentation.  FIFO_MODE: 1 reference accounting, 2 exact.
-template <int ALGO, int FIFO_MODE>
+// The fallback view of az-aware-tightly-pack, once per call, in one CTA: fb_exec_slot[i] = node_slot[exec_order[i]],
+// fb_drv_slot[j] = node_slot[drv_order[j]], fb_drv_pos[j] = position of drv_order[j] in exec_order or -1 (node_pos:
+// [n_nodes] scratch for the node -> position scatter).
+__global__ void __launch_bounds__(1024) gp_build_fallback_view(int32_t n_nodes, int32_t n_exec, int32_t n_drv,
+                                                               const int32_t* __restrict__ exec_order, const int32_t* __restrict__ drv_order,
+                                                               const int32_t* __restrict__ node_slot, int32_t* __restrict__ node_pos,
+                                                               int32_t* __restrict__ fb_exec_slot, int32_t* __restrict__ fb_drv_slot,
+                                                               int32_t* __restrict__ fb_drv_pos) {
+    for (int32_t v = threadIdx.x; v < n_nodes; v += blockDim.x) node_pos[v] = -1;
+    __syncthreads();
+    for (int32_t i = threadIdx.x; i < n_exec; i += blockDim.x) {
+        const int32_t v = exec_order[i];
+        node_pos[v] = i;
+        fb_exec_slot[i] = node_slot[v];
+    }
+    __syncthreads();
+    for (int32_t j = threadIdx.x; j < n_drv; j += blockDim.x) {
+        const int32_t v = drv_order[j];
+        fb_drv_slot[j] = node_slot[v];
+        fb_drv_pos[j] = node_pos[v];
+    }
+}
+
+// ALGO: 0 tightly-pack, 2 minimal-fragmentation, kZoneAzAware az-aware-tightly-pack.  FIFO_MODE: 1 reference accounting,
+// 2 exact.  fb: the fallback view, one GatherSlots for kZoneAzAware (its row is Z of in.row_exec), none for the single-AZ
+// packers (so their parameter list, and code, stay what they were before the az-aware form existed).
+template <int ALGO, int FIFO_MODE, class... FB>
 __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Snapshot s, const PrepApp* __restrict__ prep, ZoneFifoIn in,
                                                                               int32_t* __restrict__ zone_out, int32_t* __restrict__ driver_out,
                                                                               int32_t* __restrict__ exec_out, double* __restrict__ avg_out,
-                                                                              unsigned long long* __restrict__ stats) {
+                                                                              unsigned long long* __restrict__ stats, FB... fb) {
+    constexpr bool kAz = ALGO == kZoneAzAware;
+    static_assert(sizeof...(FB) == (kAz ? 1 : 0), "the fallback view goes with az-aware-tightly-pack only");
     __shared__ uint16_t caches[kZoneFifoWarps][kCapCache];
     __shared__ double z_avg[kZoneFifoMaxZones][4];
     __shared__ int32_t z_drv[kZoneFifoMaxZones];
+    __shared__ int32_t fb_drv;                        // kAz: driver node of the fallback, -1 = it fits nowhere either
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int32_t Z = in.n_zones;
     const GroupDesc g0 = s.groups[0];
@@ -89,7 +125,7 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
         for (int32_t z = warp; z < Z; z += kZoneFifoWarps) {
             const int64_t row = (int64_t)z * in.row_pitch;
             int32_t d;
-            if (ALGO == 0)
+            if (ALGO == 0 || kAz)
                 d = pack_app_impl<0, false, false, false, int32_t, true>(s, pa, in.row_exec, nullptr, caches[warp], st, lane, snap_flags, g0, z, row);
             else
                 d = pack_app_minfrag<false, true>(s, pa, in.row_exec, in.row_list, st, lane, snap_flags, z, row);
@@ -98,7 +134,7 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
                 z_drv[z] = d;
                 if (d >= 0)
                     zone_row_average(av, in.sched, d, in.row_exec + row, k, pa->drv[0], pa->drv[1], pa->drv[2],
-                                     pa->div[0].e, pa->div[1].e, pa->div[2].e, ALGO == 0, z_avg[z]);
+                                     pa->div[0].e, pa->div[1].e, pa->div[2].e, ALGO == 0 || kAz, z_avg[z]);
             }
         }
         __syncthreads();
@@ -107,11 +143,28 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
         int32_t best_z = -1;
         for (int32_t z = 0; z < Z; ++z)
             if (z_drv[z] >= 0 && best < z_avg[z][3]) { best = z_avg[z][3]; best_z = z; }
+        // ---- 2b. az-aware: no zone won -> warp 0 packs over the undivided orders into row Z (az_aware_pack_tightly.go:33-37)
+        int32_t win = best_z;                                        // the row to emit: a zone, or Z for the fallback
+        if constexpr (kAz) {
+            if (best_z < 0) {
+                if (warp == 0) {
+                    const int32_t d = pack_app_impl<0, false, false, false, int32_t, true, GatherSlots>(
+                        s, pa, in.row_exec, nullptr, caches[0], st, lane, snap_flags, g0, 0, (int64_t)Z * in.row_pitch, &fb...);
+                    if (lane == 0) {
+                        fb_drv = d;
+                        if (stats) atomicAdd(stats + 2, 1ull);   // stats[2]: applications for which the fallback ran
+                    }
+                }
+                __syncthreads();
+                if (fb_drv >= 0) win = Z;
+            }
+        }
+        const bool fell_back = kAz && win == Z;
         // ---- 3. the winner's warp emits and charges ---------------------------------------------------------------------
-        if (best_z >= 0 && warp == best_z % kZoneFifoWarps) {
-            const int32_t* ex = in.row_exec + (int64_t)best_z * in.row_pitch;
+        if (win >= 0 && warp == win % kZoneFifoWarps) {
+            const int32_t* ex = in.row_exec + (int64_t)win * in.row_pitch;
             int32_t* out = exec_out + pa->out_off;
-            const int32_t d = z_drv[best_z];
+            const int32_t d = fell_back ? fb_drv : z_drv[win];
             const long long ec = pa->div[0].e, em = pa->div[1].e, eg = pa->div[2].e;
             bool hosts = false;                                      // the driver's node hosts an executor
             for (int32_t t0 = 0; t0 < k; t0 += 32) {
@@ -134,16 +187,16 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
             __syncwarp();
             if (lane == 0) {
                 if (FIFO_MODE == 2 || !hosts) zone_charge(s, in.node_slot[d], 1, pa->drv[0], pa->drv[1], pa->drv[2]);
-                zone_out[app] = best_z;
+                zone_out[app] = fell_back ? -1 : win;
                 driver_out[app] = d;
-                if (avg_out) for (int t = 0; t < 4; ++t) avg_out[4 * (int64_t)app + t] = z_avg[best_z][t];
+                if (avg_out) for (int t = 0; t < 4; ++t) avg_out[4 * (int64_t)app + t] = fell_back ? 0.0 : z_avg[win][t];
             }
-        } else if (best_z < 0 && threadIdx.x == 0) {
+        } else if (win < 0 && threadIdx.x == 0) {
             zone_out[app] = -1;
             driver_out[app] = -1;
             if (avg_out) for (int t = 0; t < 4; ++t) avg_out[4 * (int64_t)app + t] = 0.0;
         }
-        if (best_z < 0 && !(fl & kAppSkipIfNoFit)) blocked = true;    // resource.go:244-253
+        if (win < 0 && !(fl & kAppSkipIfNoFit)) blocked = true;       // resource.go:244-253
         __syncthreads();
     }
     if (lane == 0 && stats) { atomicAdd(stats + 0, st.nodes); atomicAdd(stats + 1, st.drivers); }

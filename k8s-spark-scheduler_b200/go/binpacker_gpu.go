@@ -629,3 +629,187 @@ func FitEarlierDriversSingleAZ(algo C.gp_algo, apps []QueuedApp, nodeNames, exec
 	}
 	return fits, true
 }
+
+// FitEarlierDriversAzAware is FitEarlierDriversSingleAZ for `binpack: az-aware-tightly-pack` (AzAwareTightlyPack,
+// LIB/binpack/az_aware_pack_tightly.go:27-38): the candidate zones become instance groups 0..Z-1 as there, one trailing
+// group holds the other nodes of the two orders (a zone with driver candidates only, executor candidates of a zone without
+// driver candidates), and the undivided orders go along as node indices.  ONE gp_pack_fifo_az_aware call runs the whole
+// queue: the zone packs, and when no zone wins the fallback over the undivided orders, both on the device.
+// ok=false: the caller must run the original Go loop instead (also above 64 candidate zones).
+func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []string,
+	metadata resources.NodeGroupSchedulingMetadata) (fits bool, ok bool) {
+	d, err := getDevice()
+	if err != nil {
+		return false, false
+	}
+	if len(apps) == 0 {
+		return true, true
+	}
+	// groupNodesByZone for both orders; zones without executor candidates are left out (single_az.go:38-41)
+	group := func(names []string) ([]string, map[string][]string) {
+		order, byZone := []string{}, map[string][]string{}
+		for _, n := range names {
+			m, present := metadata[n]
+			if !present {
+				continue
+			}
+			if _, seen := byZone[m.ZoneLabel]; !seen {
+				order = append(order, m.ZoneLabel)
+			}
+			byZone[m.ZoneLabel] = append(byZone[m.ZoneLabel], n)
+		}
+		return order, byZone
+	}
+	zones, dz := group(nodeNames)
+	_, ez := group(executorNodeNames)
+	s := &snapshot{}
+	index := map[string]int32{}
+	var sc, sm, sg []int64
+	intern := func(n string) (int32, bool) {
+		if i, seen := index[n]; seen {
+			return i, true
+		}
+		m := metadata[n]
+		c, mm, g, exact := toTriple(m.AvailableResources)
+		c2, m2, g2, exact2 := toTriple(m.SchedulableResources)
+		if !exact || !exact2 {
+			return -1, false
+		}
+		i := int32(len(s.names))
+		index[n] = i
+		s.names = append(s.names, n)
+		s.cpu, s.mem, s.gpu = append(s.cpu, c), append(s.mem, mm), append(s.gpu, g)
+		sc, sm, sg = append(sc, c2), append(sm, m2), append(sg, g2)
+		return i, true
+	}
+	eoff, doff := []int32{0}, []int32{0}
+	candidate := map[string]bool{}
+	for _, z := range zones {
+		eo, has := ez[z]
+		if !has {
+			continue
+		}
+		candidate[z] = true
+		for _, n := range eo {
+			i, exact := intern(n)
+			if !exact {
+				return false, false
+			}
+			s.execIdx = append(s.execIdx, i)
+		}
+		for _, n := range dz[z] {
+			i, exact := intern(n)
+			if !exact {
+				return false, false
+			}
+			s.drvIdx = append(s.drvIdx, i)
+		}
+		eoff, doff = append(eoff, int32(len(s.execIdx))), append(doff, int32(len(s.drvIdx)))
+	}
+	nZones := len(eoff) - 1
+	if nZones > 64 {
+		return false, false // gp_pack_fifo_az_aware takes at most 64 candidate zones: the Go loop decides
+	}
+	// the trailing group: every node of the two orders outside the candidate zones (only the fallback reaches it)
+	rest := func(names []string, dst *[]int32) bool {
+		for _, n := range names {
+			m, present := metadata[n]
+			if !present || candidate[m.ZoneLabel] {
+				continue
+			}
+			i, exact := intern(n)
+			if !exact {
+				return false
+			}
+			*dst = append(*dst, i)
+		}
+		return true
+	}
+	if !rest(executorNodeNames, &s.execIdx) || !rest(nodeNames, &s.drvIdx) {
+		return false, false
+	}
+	if nZones == 0 || int(eoff[nZones]) < len(s.execIdx) || int(doff[nZones]) < len(s.drvIdx) {
+		eoff, doff = append(eoff, int32(len(s.execIdx))), append(doff, int32(len(s.drvIdx)))
+	}
+	nGroups := len(eoff) - 1
+	// the undivided orders, as node indices of the same table (names absent from the metadata dropped)
+	undivided := func(names []string) []int32 {
+		out := make([]int32, 0, len(names))
+		for _, n := range names {
+			if i, seen := index[n]; seen {
+				out = append(out, i)
+			}
+		}
+		return out
+	}
+	ue, ud := undivided(executorNodeNames), undivided(nodeNames)
+	q := len(apps)
+	dc, dm, dg := make([]int64, q), make([]int64, q), make([]int64, q)
+	ec, em, eg := make([]int64, q), make([]int64, q), make([]int64, q)
+	cnt, skip := make([]int32, q), make([]uint8, q)
+	total := 0
+	for i, a := range apps {
+		var o1, o2 bool
+		dc[i], dm[i], dg[i], o1 = toTriple(a.Driver)
+		ec[i], em[i], eg[i], o2 = toTriple(a.Executor)
+		if !o1 || !o2 || a.MinExecutorCount < 0 {
+			return false, false
+		}
+		cnt[i] = int32(a.MinExecutorCount)
+		if a.SkipIfNoFit {
+			skip[i] = 1
+		}
+		total += a.MinExecutorCount
+	}
+	zone, driver := make([]int32, q), make([]int32, q)
+	exec := make([]int32, max(total, 1))
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []any{ptrOrNil(s.cpu), ptrOrNil(s.mem), ptrOrNil(s.gpu), ptrOrNil32(s.execIdx), ptrOrNil32(s.drvIdx),
+		ptrOrNil32(eoff), ptrOrNil32(doff), ptrOrNil(sc), ptrOrNil(sm), ptrOrNil(sg), ptrOrNil32(ue), ptrOrNil32(ud),
+		ptrOrNil(dc), ptrOrNil(dm), ptrOrNil(dg), ptrOrNil(ec), ptrOrNil(em), ptrOrNil(eg),
+		ptrOrNil32(cnt), ptrOrNil8(skip), ptrOrNil32(zone), ptrOrNil32(driver), ptrOrNil32(exec)} {
+		if p != nil {
+			pin.Pin(p)
+		}
+	}
+	gn := C.gp_nodes{
+		n_nodes: C.int32_t(len(s.names)), avail_cpu_milli: ptr64(s.cpu), avail_mem_bytes: ptr64(s.mem), avail_gpu: ptr64(s.gpu),
+		n_groups: C.int32_t(nGroups), exec_off: ptr32(eoff), exec_order: ptr32(s.execIdx), drv_off: ptr32(doff), drv_order: ptr32(s.drvIdx),
+	}
+	if st := C.gp_set_snapshot(d.ctx, &gn); st != C.GP_OK {
+		return false, false
+	}
+	if st := C.gp_set_schedulable(d.ctx, ptr64(sc), ptr64(sm), ptr64(sg)); st != C.GP_OK {
+		return false, false
+	}
+	ga := C.gp_apps{n_apps: C.int32_t(q), drv_cpu_milli: ptr64(dc), drv_mem_bytes: ptr64(dm), drv_gpu: ptr64(dg),
+		exe_cpu_milli: ptr64(ec), exe_mem_bytes: ptr64(em), exe_gpu: ptr64(eg), exe_count: ptr32(cnt), skip_if_no_fit: ptr8(skip)}
+	orders := C.gp_az_orders{n_zones: C.int32_t(nZones), n_exec: C.int32_t(len(ue)), exec_order: ptr32(ue),
+		n_drv: C.int32_t(len(ud)), drv_order: ptr32(ud)}
+	gz := C.gp_zone_results{zone: ptr32(zone), driver_node: ptr32(driver), executor_nodes: ptr32(exec), executor_nodes_cap: C.int64_t(len(exec))}
+	if st := C.gp_pack_fifo_az_aware(d.ctx, &ga, C.GP_MODE_FIFO_REFERENCE, &orders, &gz); st != C.GP_OK {
+		return false, false
+	}
+	cpu, mem, gpu := make([]int64, len(s.names)), make([]int64, len(s.names)), make([]int64, len(s.names))
+	if st := C.gp_get_snapshot(d.ctx, ptr64(cpu), ptr64(mem), ptr64(gpu)); st != C.GP_OK {
+		return false, false
+	}
+	for i, n := range s.names { // SubtractUsageIfExists (LIB/resources/resources.go:129-135), as the device left it
+		a := metadata[n].AvailableResources
+		a.CPU = *resource.NewMilliQuantity(cpu[i], resource.DecimalSI)
+		a.Memory = *resource.NewQuantity(mem[i], resource.BinarySI)
+		a.NvidiaGPU = *resource.NewQuantity(gpu[i], resource.DecimalSI)
+	}
+	fits = true
+	for i := range apps {
+		if driver[i] == -2 || (driver[i] == -1 && skip[i] == 0) { // EXT/resource.go:250-252
+			fits = false
+		}
+	}
+	return fits, true
+}

@@ -27,6 +27,7 @@
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "gangpack.h"
@@ -447,8 +448,9 @@ inline const char* const azAwareTightlyPack = "az-aware-tightly-pack";      // :
 inline const char* const SingleAzTightlyPack = "single-az-tightly-pack";    // :29
 inline const char* const SingleAzMinimalFragmentation = "single-az-minimal-fragmentation";   // :33
 
-// binpackFunctions (:43-49): all five `binpack:` values.  `algo` is the device packer behind the function; the
-// zone-aware ones (needsHostLoop) choose a zone per application on the host, so the FIFO loop calls them per driver.
+// binpackFunctions (:43-49): all five `binpack:` values.  `algo` is the device packer behind the function.  As a
+// SparkBinPackFunction the zone-aware ones (NeedsHostLoop) choose a zone per application; extender::FitEarlierDrivers runs
+// them as one device FIFO loop instead (az-aware-tightly-pack above 64 candidate zones: per driver).
 inline const std::map<std::string, Binpacker>& binpackFunctions() {
     static const std::map<std::string, Binpacker> m = {
         {tightlyPack, {tightlyPack, binpack::TightlyPack, false, GP_TIGHTLY_PACK}},
@@ -622,20 +624,38 @@ inline bool FitEarlierDrivers(const binpacker::Binpacker& packer, const std::vec
         if (!drivers[i].ParseError) live.push_back(i);
     if (results) results->assign(drivers.size(), binpack::EmptyPackingResult());
     if (live.empty()) return true;
-    if (packer.IsSingleAz) {
-        // single-AZ packers: the whole queue in ONE launch (gp_pack_fifo_zones) -- zone = instance group, the zone choice of
-        // driver i feeds driver i+1 on the device
+    const bool azAware = packer.Name == binpacker::azAwareTightlyPack;
+    std::vector<std::pair<std::vector<std::string>, std::vector<std::string>>> groups;
+    if (packer.IsSingleAz || azAware) {
         std::vector<std::string> dzOrder, ezOrder;
         std::unordered_map<std::string, std::vector<std::string>> dz, ez;
         binpack::groupNodesByZone(nodeNames, metadata, &dzOrder, &dz);
         binpack::groupNodesByZone(executorNodeNames, metadata, &ezOrder, &ez);
-        std::vector<std::pair<std::vector<std::string>, std::vector<std::string>>> groups;
         for (const auto& z : dzOrder)
             if (ez.count(z)) groups.emplace_back(dz[z], ez[z]);                 // single_az.go:36-41
+    }
+    // The single-AZ packers and az-aware-tightly-pack (up to 64 candidate zones): the whole queue in ONE launch -- zone =
+    // instance group, the zone choice (or az-aware's undivided fallback) of driver i feeds driver i+1 on the device.
+    // az-aware-tightly-pack with more zones keeps the per-driver loop below (gp_pack_fifo_az_aware takes at most 64).
+    if (packer.IsSingleAz || (azAware && groups.size() <= 64)) {
         const size_t q = live.size();
-        if (groups.empty()) {                                                   // EmptyPackingResult for every driver
+        const int32_t nZones = (int32_t)groups.size();
+        if (packer.IsSingleAz && groups.empty()) {                              // EmptyPackingResult for every driver
             for (size_t j = 0; j < q; ++j) if (!drivers[live[j]].SkipIfNoFit) return false;
             return true;
+        }
+        if (azAware) {
+            // one trailing group with the nodes of both orders that no candidate zone contains: only the undivided
+            // fallback (az_aware_pack_tightly.go:33-37) reaches them
+            std::unordered_set<std::string> inZone;
+            for (const auto& g : groups) {
+                inZone.insert(g.first.begin(), g.first.end());
+                inZone.insert(g.second.begin(), g.second.end());
+            }
+            std::pair<std::vector<std::string>, std::vector<std::string>> rest;
+            for (const auto& n : nodeNames) if (metadata.count(n) && !inZone.count(n)) rest.first.push_back(n);
+            for (const auto& n : executorNodeNames) if (metadata.count(n) && !inZone.count(n)) rest.second.push_back(n);
+            if (groups.empty() || !rest.first.empty() || !rest.second.empty()) groups.push_back(std::move(rest));
         }
         gangpack::Device& d = gangpack::Device::Get();
         d.SetSnapshotGroups(metadata, groups);
@@ -660,7 +680,18 @@ inline bool FitEarlierDrivers(const binpacker::Binpacker& packer, const std::vec
         a.exe_count = cnt.data(); a.skip_if_no_fit = skip.data();
         gp_zone_results r{};
         r.zone = zone.data(); r.driver_node = driver.data(); r.executor_nodes = exec.data(); r.executor_nodes_cap = (int64_t)exec.size();
-        d.check(gp_pack_fifo_zones(d.ctx(), &a, (gp_algo)packer.algo, GP_MODE_FIFO_REFERENCE, &r), "gp_pack_fifo_zones");
+        if (azAware) {
+            std::vector<int32_t> eo, dord;                                      // the undivided orders as node indices
+            for (const auto& n : executorNodeNames) { const int32_t i = d.index(n); if (i >= 0) eo.push_back(i); }
+            for (const auto& n : nodeNames) { const int32_t i = d.index(n); if (i >= 0) dord.push_back(i); }
+            gp_az_orders o{};
+            o.n_zones = nZones;
+            o.n_exec = (int32_t)eo.size(); o.exec_order = eo.data();
+            o.n_drv = (int32_t)dord.size(); o.drv_order = dord.data();
+            d.check(gp_pack_fifo_az_aware(d.ctx(), &a, GP_MODE_FIFO_REFERENCE, &o, &r), "gp_pack_fifo_az_aware");
+        } else {
+            d.check(gp_pack_fifo_zones(d.ctx(), &a, (gp_algo)packer.algo, GP_MODE_FIFO_REFERENCE, &r), "gp_pack_fifo_zones");
+        }
         std::vector<int64_t> cpu(d.n_nodes()), mem(d.n_nodes()), gpu(d.n_nodes());
         d.check(gp_get_snapshot(d.ctx(), cpu.data(), mem.data(), gpu.data()), "gp_get_snapshot");
         for (size_t i = 0; i < d.n_nodes(); ++i) {
@@ -682,9 +713,9 @@ inline bool FitEarlierDrivers(const binpacker::Binpacker& packer, const std::vec
         return ok;
     }
     if (binpacker::NeedsHostLoop(packer)) {
-        // az-aware-tightly-pack: the reference's own loop (:230-259), every BinpackFunc call being one device batch over
-        // the zones (+ the undivided fallback); usage is subtracted on the host between calls (SubtractUsageIfExists,
-        // resources.go:129-135)
+        // az-aware-tightly-pack with more than 64 candidate zones: the reference's own loop (:230-259), every BinpackFunc
+        // call being one device batch over the zones (+ the undivided fallback); usage is subtracted on the host between
+        // calls (SubtractUsageIfExists, resources.go:129-135)
         for (size_t i : live) {
             const auto& a = drivers[i];
             binpack::PackingResult pr = packer.BinpackFunc(a.Resources.DriverResources, a.Resources.ExecutorResources,
