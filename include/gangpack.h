@@ -337,9 +337,9 @@ gp_status gp_synchronize(gp_ctx* ctx);
  * [driver] + ExecutorNodes, duplicates kept, sequential sums, cpu through Quantity.Value() -- and the zone with the highest
  * AvgPackingEfficiency.Max wins: the first among equals, and none when every average is 0 (:80, :91).  For
  * minimal-fragmentation the efficiencies see the driver only (minimalFragmentation never adds its executors to
- * SparkBinPack's reserved map) -- kept.  "az-aware-tightly-pack" (az_aware_pack_tightly.go:27-38) for independent decisions =
- * this call, then plain gp_pack_batch(GP_TIGHTLY_PACK) over the undivided orders for the applications that got zone -1;
- * under FIFO it is gp_pack_fifo_az_aware below.
+ * SparkBinPack's reserved map) -- kept.  "az-aware-tightly-pack" (az_aware_pack_tightly.go:27-38), which falls back to the
+ * undivided orders when no zone wins, is gp_pack_batch_az_aware for independent decisions and gp_pack_fifo_az_aware under
+ * FIFO (both below).
  * gp_set_schedulable: NodeSchedulingMetadata.SchedulableResources of the current snapshot's nodes (resources.go:61-100). */
 gp_status gp_set_schedulable(gp_ctx* ctx, const int64_t* sched_cpu_milli, const int64_t* sched_mem_bytes, const int64_t* sched_gpu /* or NULL */);
 typedef struct {
@@ -379,7 +379,8 @@ gp_status gp_pack_fifo_zones(gp_ctx* ctx, const gp_apps* apps /* group ignored *
  * against); order lengths other than exec_off[n_groups] / drv_off[n_groups]; an order entry out of range, repeated or not
  * listed by the snapshot in that role; a zone group whose order is not the undivided order restricted to its nodes. */
 typedef struct {
-    int32_t n_zones;                 /* 0..64: snapshot groups 0..n_zones-1 are the candidate zones */
+    int32_t n_zones;                 /* snapshot groups 0..n_zones-1 are the candidate zones (0..64 under FIFO, 0..n_groups
+                                        for gp_pack_batch_az_aware) */
     int32_t n_exec;
     const int32_t* exec_order;       /* [n_exec] executorNodePriorityOrder, undivided, node indices */
     int32_t n_drv;
@@ -387,6 +388,24 @@ typedef struct {
 } gp_az_orders;
 gp_status gp_pack_fifo_az_aware(gp_ctx* ctx, const gp_apps* apps /* group ignored */, gp_mode mode, const gp_az_orders* orders,
                                 gp_zone_results* out);
+
+/* "az-aware-tightly-pack" (AzAwareTightlyPack, LIB/binpack/az_aware_pack_tightly.go:27-38) for a batch of INDEPENDENT
+ * decisions against the unmodified snapshot -- the Predicate's own pack (EXT/resource.go:321) with n_apps = 1, or the
+ * unschedulable marker's many decisions (EXT/unschedulablepods.go:132-166).  Each application is packed in every candidate
+ * zone with tightly-pack and the zone is chosen exactly like gp_pack_batch_zones; when no zone wins,
+ * SparkBinPack(tightlyPackExecutors) runs over the UNDIVIDED orders.  Everything stays on the device: one stream
+ * synchronise, at the end.  The device snapshot is not modified.
+ * Snapshot and orders: the layout of gp_pack_fifo_az_aware (candidate zones in groups 0..n_zones-1, the other nodes of the
+ * two orders in the groups after them, gp_set_schedulable required), with any n_zones from 0 to n_groups (no 64-zone
+ * bound).  With n_zones = 0 the call is gp_pack_batch(GP_TIGHTLY_PACK, GP_MODE_INDEPENDENT) over the undivided orders.
+ * Results: zone[i] >= 0 = that zone won, avg_efficiency its averages; zone[i] == -1 && driver_node[i] >= 0 = the fallback
+ * placed application i (four zero averages); zone[i] == -1 && driver_node[i] == -1 = it fits nowhere.  exec_out_off may be
+ * NULL or given, as in gp_pack_batch_zones; exe_count up to 2^24.
+ * gp_stats: scan_path_apps = applications for which the fallback ran; nodes_scanned / drivers_tried include its scans.
+ * GP_ERR_INVALID (gp_last_error names the cause): those of gp_pack_fifo_az_aware except the mode and the 64-zone bound
+ * (n_zones negative or above n_groups). */
+gp_status gp_pack_batch_az_aware(gp_ctx* ctx, const gp_apps* apps /* group, skip_if_no_fit ignored */, const gp_az_orders* orders,
+                                 gp_zone_results* out);
 
 /* ---- reservation table of a batch + a snapshot that stays on the device (SURVEY 8f rows f4 and f2) ---------------
  * gp_reserve_placements: newResourceReservation (internal/extender/resourcereservations.go:491-528) for every application
@@ -439,8 +458,8 @@ gp_status gp_multi_group_owner(gp_multi* m, int32_t* owner /* [n_groups] */);
 
 /* Statistics of the last gp_pack_batch* on this context (host call, synchronises the stream):
  * nodes_scanned = executor-order entries visited, drivers_tried = driver-order entries visited,
- * summed over apps -- the N_e / N_d of the algorithmic-bytes formula (DESIGN.md); gp_pack_fifo_az_aware includes the
- * scans of its undivided fallback in both. */
+ * summed over apps -- the N_e / N_d of the algorithmic-bytes formula (DESIGN.md); gp_pack_fifo_az_aware and
+ * gp_pack_batch_az_aware include the scans of their undivided fallback in both. */
 typedef struct {
     int64_t nodes_scanned;
     int64_t drivers_tried;
@@ -451,7 +470,8 @@ typedef struct {
                                   per-shape capacity tables (all of them with GANGPACK_TABLES=0).
                                   FIFO modes: applications decided by the whole CTA instead of warp 0 alone (every
                                   evaluated one with GANGPACK_FIFO_WARP=0).
-                                  gp_pack_fifo_az_aware: applications for which the undivided fallback ran, placed or not */
+                                  gp_pack_fifo_az_aware / gp_pack_batch_az_aware: applications for which the undivided
+                                  fallback ran, placed or not */
     int64_t scan_path_nodes;   /* executor-order entries those scans visited (nodes_scanned also counts table probes) */
     int64_t reserved[1];
 } gp_stats;

@@ -386,6 +386,8 @@ struct gp_ctx {
     std::vector<int32_t> v_pos;
     bool host_layout = false;
     std::vector<uint8_t> v_seen_e, v_seen_d;
+    std::vector<int32_t> v_zone_next;             // az-aware order check: next position per zone group
+    int az_fallback_ctas_per_sm = 0;              // occupancy of gp_pack_az_fallback (queried once)
     std::vector<std::pair<const char*, size_t>> pinned_blocks;   // gp_alloc_pinned allocations (device-mapped under UVA)
     void* one_block = nullptr;                    // gp_pack_one staging (mapped pinned)
     size_t one_bytes = 0;
@@ -1432,18 +1434,17 @@ gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, 
     return GP_OK;
 }
 
-gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_zones: gp_set_snapshot first");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
-    if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: NULL apps/results");
-    if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
-        return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: the single-AZ packers are tightly-pack and minimal-fragmentation (single_az_pack_tightly.go, single_az_minimal_fragmentation.go)");
-    const int32_t Q = a->n_apps, Z = c->n_groups;
+// Independent zone packs of a batch, shared by gp_pack_batch_zones (the zones are every instance group, no fallback) and
+// gp_pack_batch_az_aware (zones 0..Z-1 with tightly-pack, plus the undivided orders `az` of the fallback, already
+// validated).  Argument checks common to both are here.
+static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int32_t Z, const gp_az_orders* az, gp_zone_results* out,
+                                 const char* who) {
+    const std::string w(who);
+    const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
     if (!a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->zone || !out->driver_node)
-        return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: missing app/result arrays");
-    if ((int64_t)Q * Z > 0x7fffffffLL) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: n_apps x zones too large");
+        return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
+    if ((int64_t)Q * Z > 0x7fffffffLL) return fail(c, GP_ERR_INVALID, w + ": n_apps x zones too large");
     const int64_t* off = a->exec_out_off;
     if (!off) {
         c->host_off.resize((size_t)Q + 1);
@@ -1453,8 +1454,8 @@ gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone
         off = c->host_off.data();
     }
     const int64_t total = off[Q];
-    if (total < 0 || total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, "gp_pack_batch_zones: executor_nodes_cap too small");
-    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: executor_nodes is NULL");
+    if (total < 0 || total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, w + ": executor_nodes_cap too small");
+    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, w + ": executor_nodes is NULL");
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t q = (size_t)Q, R = q * (size_t)Z, T = (size_t)total;
@@ -1463,6 +1464,10 @@ gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone
     const size_t o_in = take(48 * q), o_cnt = take(4 * q), o_off = take(8 * (q + 1)), o_rows = take(48 * R), o_rcnt = take(4 * R), o_rgrp = take(4 * R),
                  o_roff = take(8 * (R + 1)), o_rdrv = take(4 * R), o_rexe = take(4 * ((size_t)Z * T + 1)), o_zone = take(4 * q), o_drv = take(4 * q),
                  o_exe = take(4 * (T + 1)), o_avg = take(32 * q);
+    // az-aware: the fallback's PrepApp records and list, the undivided orders and their gather view
+    const size_t QF = az ? q : 0, NE = az ? (size_t)az->n_exec : 0, ND = az ? (size_t)az->n_drv : 0, NN = az ? (size_t)c->n_nodes : 0;
+    const size_t o_prep = take(sizeof(PrepApp) * QF), o_list = take(4 * QF), o_eord = take(4 * NE), o_dord = take(4 * ND), o_npos = take(4 * NN),
+                 o_fbe = take(4 * NE), o_fbd = take(4 * ND), o_fbp = take(4 * ND);
     GP_CUDA(c, c->zonebuf.reserve(o));
     char* b = c->zonebuf.as<char>();
     const int64_t* hc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
@@ -1505,12 +1510,58 @@ gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone
                                                                        out->avg_efficiency ? (double*)(b + o_avg) : nullptr);
     GP_CUDA(c, cudaGetLastError());
     c->last.kernel_launches += 2;
+    if (az) {
+        // the applications no zone won: SparkBinPack(tightlyPackExecutors) over the undivided orders, still on the device
+        // (az_aware_pack_tightly.go:33-37).  dev_misc [40] = length of the list, [44] = the fallback's claim counter
+        // (both zeroed by pack_begin); stats [2..3] restart so that scan_path_apps / _nodes count the fallback alone.
+        unsigned int* n_listed = reinterpret_cast<unsigned int*>(c->dev_misc.as<char>() + 40);
+        unsigned long long* d_stats = reinterpret_cast<unsigned long long*>(c->dev_misc.as<char>() + 8);
+        GP_CUDA(c, cudaMemsetAsync(d_stats + 2, 0, 16, st));
+        int32_t* listed = (int32_t*)(b + o_list);
+        gp_az_fallback_list<<<(unsigned)((q + TH - 1) / TH), TH, 0, st>>>(Q, (const int32_t*)(b + o_zone), listed, n_listed);
+        AppColumns cols{};
+        for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
+        cols.count = (const int32_t*)(b + o_cnt); cols.group = nullptr; cols.off = (const int64_t*)(b + o_off); cols.bits = 64; cols.mem_shift = 0;
+        PrepApp* prep = (PrepApp*)(b + o_prep);
+        gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
+            Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, c->dev_misc.as<int>(),
+            reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
+        if (NE) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * NE, cudaMemcpyHostToDevice, st));
+        if (ND) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * ND, cudaMemcpyHostToDevice, st));
+        gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)NE, (int32_t)ND, (const int32_t*)(b + o_eord), (const int32_t*)(b + o_dord),
+                                                   c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe),
+                                                   (int32_t*)(b + o_fbd), (int32_t*)(b + o_fbp));
+        GatherSlots fb{};
+        fb.exec_slot = (const int32_t*)(b + o_fbe); fb.drv_slot = (const int32_t*)(b + o_fbd); fb.drv_pos = (const int32_t*)(b + o_fbp);
+        fb.ne = (int32_t)NE; fb.nd = (int32_t)ND;
+        int& per_sm = c->az_fallback_ctas_per_sm;
+        if (per_sm == 0) {
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_az_fallback, kAzFallbackThreads, 0);
+            if (per_sm < 1) per_sm = 1;
+        }
+        int64_t blocks = ((int64_t)Q * 32 + kAzFallbackThreads - 1) / kAzFallbackThreads;   // the list holds at most Q
+        if (blocks > (int64_t)c->sm_count * per_sm) blocks = (int64_t)c->sm_count * per_sm;
+        gp_pack_az_fallback<<<(unsigned)blocks, kAzFallbackThreads, 0, st>>>(make_snapshot(c), prep, listed, n_listed, fb, (int32_t*)(b + o_drv),
+                                                                            (int32_t*)(b + o_exe), d_stats, n_listed + 1);
+        GP_CUDA(c, cudaGetLastError());
+        c->last.kernel_launches += 4;
+    }
     GP_CUDA(c, cudaMemcpyAsync(out->zone, b + o_zone, 4 * q, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaMemcpyAsync(out->driver_node, b + o_drv, 4 * q, cudaMemcpyDeviceToHost, st));
     if (T) GP_CUDA(c, cudaMemcpyAsync(out->executor_nodes, b + o_exe, 4 * T, cudaMemcpyDeviceToHost, st));
     if (out->avg_efficiency) GP_CUDA(c, cudaMemcpyAsync(out->avg_efficiency, b + o_avg, 32 * q, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
     return decode_device_error(c, *reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
+}
+
+gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone_results* out) {
+    if (!c) return GP_ERR_INVALID;
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_zones: gp_set_snapshot first");
+    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: NULL apps/results");
+    if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
+        return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: the single-AZ packers are tightly-pack and minimal-fragmentation (single_az_pack_tightly.go, single_az_minimal_fragmentation.go)");
+    return batch_zones_run(c, a, algo, c->n_groups, nullptr, out, "gp_pack_batch_zones");
 }
 
 // ---- reservation table + device-resident snapshot upkeep (gangpack_zones.cuh) -------------------------------------------
@@ -1526,6 +1577,48 @@ static gp_status refresh_views(gp_ctx* c, bool raised, cudaStream_t st) {
                                                                &meta->flags, meta->max_avail);
     gp_fill_pair32<<<(c->n_slots + T) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), meta, c->pair32.as<uint2>());
     GP_CUDA(c, cudaGetLastError());
+    return GP_OK;
+}
+
+// The undivided orders of az-aware-tightly-pack against the snapshot gp_set_snapshot laid out, in O(N): every entry a node
+// of the snapshot in that role, once; every zone group's order = the undivided order restricted to that group's nodes
+// (the fallback and the zone packs must see the same priorities).  o->n_zones is already within 0..n_groups.
+static gp_status check_az_orders(gp_ctx* c, const gp_az_orders* o, const char* who) {
+    const std::string w(who);
+    if (!c->host_layout)
+        return fail(c, GP_ERR_INVALID, w + ": the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
+                                           "gp_prepare_cluster there is no host copy of the layout to check the undivided orders against)");
+    if (o->n_exec != c->n_exec || o->n_drv != c->n_drv)
+        return fail(c, GP_ERR_INVALID, w + ": order lengths must equal the snapshot's exec_off[n_groups] / drv_off[n_groups]");
+    if ((o->n_exec > 0 && !o->exec_order) || (o->n_drv > 0 && !o->drv_order))
+        return fail(c, GP_ERR_INVALID, w + ": order arrays missing");
+    const int32_t Z = o->n_zones;
+    const uint32_t N = (uint32_t)c->n_nodes;
+    const int32_t* owner = c->v_owner.data();
+    const int32_t* pos = c->v_pos.data();
+    for (int role = 0; role < 2; ++role) {
+        const int32_t n = role == 0 ? o->n_exec : o->n_drv;
+        const int32_t* ord = role == 0 ? o->exec_order : o->drv_order;
+        const char* name = role == 0 ? "exec_order" : "drv_order";
+        std::vector<uint8_t>& seen = role == 0 ? c->v_seen_e : c->v_seen_d;
+        seen.assign((size_t)N, 0);
+        std::vector<int32_t>& next = c->v_zone_next;     // next expected position in each zone group's order
+        next.assign((size_t)Z, 0);
+        for (int32_t i = 0; i < n; ++i) {
+            const uint32_t v = (uint32_t)ord[i];
+            if (v >= N) return fail(c, GP_ERR_INVALID, w + ": " + name + " entry out of range");
+            if (seen[v]) return fail(c, GP_ERR_INVALID, w + ": " + name + " lists a node twice");
+            seen[v] = 1;
+            const int32_t ow = owner[v];
+            if (ow < 0 || !(ow & (1 << role)))
+                return fail(c, GP_ERR_INVALID, w + ": " + name + " lists a node the snapshot does not list as " +
+                                                   (role == 0 ? "an executor" : "a driver") + " candidate");
+            const int32_t g = ow >> 2;
+            if (g < Z && pos[(size_t)role * N + v] != next[(size_t)g]++)
+                return fail(c, GP_ERR_INVALID, w + ": zone group " + std::to_string(g) + "'s " +
+                                                   (role == 0 ? "executor" : "driver") + " order is not " + name + " restricted to its nodes");
+        }
+    }
     return GP_OK;
 }
 
@@ -1659,41 +1752,24 @@ gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const
     const int32_t Z = o->n_zones;
     if (Z < 0 || Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones must be 0..64");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones exceeds the snapshot's instance groups");
-    if (!c->host_layout)
-        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
-                                       "gp_prepare_cluster there is no host copy of the layout to check the undivided orders against)");
-    if (o->n_exec != c->n_exec || o->n_drv != c->n_drv)
-        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: order lengths must equal the snapshot's exec_off[n_groups] / drv_off[n_groups]");
-    if ((o->n_exec > 0 && !o->exec_order) || (o->n_drv > 0 && !o->drv_order))
-        return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: order arrays missing");
-    // O(N): every entry a node of the snapshot in that role, once; every zone group's order = the undivided order
-    // restricted to that group's nodes (the fallback and the zone packs must see the same priorities)
-    const uint32_t N = (uint32_t)c->n_nodes;
-    const int32_t* owner = c->v_owner.data();
-    const int32_t* pos = c->v_pos.data();
-    for (int role = 0; role < 2; ++role) {
-        const int32_t n = role == 0 ? o->n_exec : o->n_drv;
-        const int32_t* ord = role == 0 ? o->exec_order : o->drv_order;
-        const char* name = role == 0 ? "exec_order" : "drv_order";
-        std::vector<uint8_t>& seen = role == 0 ? c->v_seen_e : c->v_seen_d;
-        seen.assign((size_t)N, 0);
-        int32_t next[kZoneFifoMaxZones] = {};
-        for (int32_t i = 0; i < n; ++i) {
-            const uint32_t v = (uint32_t)ord[i];
-            if (v >= N) return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: ") + name + " entry out of range");
-            if (seen[v]) return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: ") + name + " lists a node twice");
-            seen[v] = 1;
-            const int32_t ow = owner[v];
-            if (ow < 0 || !(ow & (1 << role)))
-                return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: ") + name + " lists a node the snapshot does not list as " +
-                                                   (role == 0 ? "an executor" : "a driver") + " candidate");
-            const int32_t g = ow >> 2;
-            if (g < Z && pos[(size_t)role * N + v] != next[g]++)
-                return fail(c, GP_ERR_INVALID, std::string("gp_pack_fifo_az_aware: zone group ") + std::to_string(g) + "'s " +
-                                                   (role == 0 ? "executor" : "driver") + " order is not " + name + " restricted to its nodes");
-        }
-    }
+    gp_status s = check_az_orders(c, o, "gp_pack_fifo_az_aware");
+    if (s != GP_OK) return s;
     return fifo_zones_run(c, a, kZoneAzAware, mode, Z, o, out, "gp_pack_fifo_az_aware");
+}
+
+// az-aware-tightly-pack for a batch of independent decisions: the zone packs, the zone choice and the undivided fallback
+// on the device, one stream synchronise
+gp_status gp_pack_batch_az_aware(gp_ctx* c, const gp_apps* a, const gp_az_orders* o, gp_zone_results* out) {
+    if (!c) return GP_ERR_INVALID;
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_az_aware: gp_set_snapshot first");
+    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!a || !out || !o || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: NULL apps/orders/results");
+    const int32_t Z = o->n_zones;
+    if (Z < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones is negative");
+    if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones exceeds the snapshot's instance groups");
+    gp_status s = check_az_orders(c, o, "gp_pack_batch_az_aware");
+    if (s != GP_OK) return s;
+    return batch_zones_run(c, a, GP_TIGHTLY_PACK, Z, o, out, "gp_pack_batch_az_aware");
 }
 
 gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* placed, int32_t subtract, gp_reservation_table* out) {

@@ -349,7 +349,9 @@ struct GatherSlots {
 // MUT: the snapshot changes inside the launch (zone-aware FIFO, gangpack_zones.cuh): coherent loads, never with C32 (the
 // compact view is not kept current).  grp_override / out_override: pack against another instance group than pa->group and
 // write ExecutorNodes (and the candidate list) at another offset than pa->out_off.
-// MAP: GroupSlots, or GatherSlots with `view` (tightly-pack, coherent loads only; grp_override and g0 are then unused).
+// MAP: GroupSlots, or GatherSlots with `view` (tightly-pack over the full-width slots; grp_override and g0 are then unused).
+// The gather view takes coherent loads (MUT) inside the FIFO loop and read-only loads in gp_pack_az_fallback, where
+// nothing writes the slots.
 template <int ALGO, bool FAST, bool NOGPU, bool C32, class OUT, bool MUT = false, class MAP = GroupSlots>
 __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepApp* __restrict__ pa,
                                                  OUT* __restrict__ executor_nodes, int2* __restrict__ scratch,
@@ -358,7 +360,7 @@ __device__ __forceinline__ int32_t pack_app_impl(const Snapshot& s, const PrepAp
                                                  int32_t grp_override = -1, int64_t out_override = -1,
                                                  const MAP* __restrict__ view = nullptr) {
     static_assert(!(MUT && C32), "the compact view is read-only");
-    static_assert(!MAP::kGather || (ALGO == 0 && MUT && !C32), "the gather scan is tightly-pack over the mutable slots");
+    static_assert(!MAP::kGather || (ALGO == 0 && !C32), "the gather scan is tightly-pack over the full-width slots");
     Caps<FAST> a;
     a.init(pa, (pa->flags & kAppUsesGpu) || (snap_flags & kSnapGpuNegative));
     const bool ug = NOGPU ? false : a.use_gpu;      // compile-time false on the hot instantiation

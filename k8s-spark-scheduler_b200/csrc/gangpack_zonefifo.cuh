@@ -202,4 +202,66 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
     if (lane == 0 && stats) { atomicAdd(stats + 0, st.nodes); atomicAdd(stats + 1, st.drivers); }
 }
 
+// ---- independent decisions (gp_pack_batch_az_aware) ------------------------------------------------------------------
+// Every application is decided against the unmodified snapshot: the zone packs and gp_zone_choose run like
+// gp_pack_batch_zones over groups 0..Z-1, then the applications no zone won are listed (in any order: nothing is charged)
+// and packed over the undivided orders through the same gather view as the FIFO form.
+
+// listed[0..*n_listed) = the applications with zone[i] == -1; *n_listed starts at 0
+__global__ void __launch_bounds__(256) gp_az_fallback_list(int32_t n_apps, const int32_t* __restrict__ zone, int32_t* __restrict__ listed,
+                                                            unsigned int* __restrict__ n_listed) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool fb = i < n_apps && zone[i] < 0;
+    const unsigned vote = __ballot_sync(kFull, fb);
+    if (vote == 0) return;                                     // warp-uniform
+    const int lane = threadIdx.x & 31;
+    unsigned int base = 0;
+    if (lane == 0) base = atomicAdd(n_listed, (unsigned int)__popc(vote));
+    base = __shfl_sync(kFull, base, 0);
+    if (fb) listed[base + __popc(vote & ((1u << lane) - 1u))] = i;
+}
+
+// SparkBinPack(tightlyPackExecutors) over the undivided orders for every listed application: a persistent grid, one warp
+// per application claimed from *next.  The driver and ExecutorNodes go straight to the application's own entries of the
+// final results (prep[i].out_off is its CSR offset).  MUT = false: nothing writes the slots during the call, so the scan
+// takes the read-only loads of the other independent kernels.  stats[2] / [3]: applications / executor-order entries of
+// these scans.
+constexpr int kAzFallbackThreads = 256;
+__global__ void __launch_bounds__(kAzFallbackThreads) gp_pack_az_fallback(Snapshot s, const PrepApp* __restrict__ prep,
+                                                                         const int32_t* __restrict__ listed,
+                                                                         const unsigned int* __restrict__ n_listed,
+                                                                         const __grid_constant__ GatherSlots view,
+                                                                         int32_t* __restrict__ drv_node, int32_t* __restrict__ exec_out,
+                                                                         unsigned long long* __restrict__ stats,
+                                                                         unsigned int* __restrict__ next) {
+    __shared__ uint16_t caches[kAzFallbackThreads / 32][kCapCache];
+    const unsigned int n = *n_listed;
+    if (n == 0) return;
+    const int lane = threadIdx.x & 31;
+    const int snap_flags = s.meta->flags;
+    const GroupDesc none{};                                    // the gather view has no group
+    WarpStats st{0, 0};
+    unsigned long long apps_done = 0;
+    for (;;) {
+        unsigned int i = 0;
+        if (lane == 0) i = atomicAdd(next, 1u);
+        i = __shfl_sync(kFull, i, 0);
+        if (i >= n) break;
+        const int32_t app = listed[i];
+        const PrepApp* pa = prep + app;
+        int32_t d = -1;
+        if (!(pa->flags & kAppInvalid))
+            d = pack_app_impl<0, false, false, false, int32_t, false, GatherSlots>(s, pa, exec_out, nullptr, caches[threadIdx.x >> 5], st,
+                                                                                  lane, snap_flags, none, -1, -1, &view);
+        if (lane == 0) drv_node[app] = d;
+        ++apps_done;
+    }
+    if (lane == 0) {
+        atomicAdd(stats + 0, st.nodes);
+        atomicAdd(stats + 1, st.drivers);
+        atomicAdd(stats + 2, apps_done);
+        atomicAdd(stats + 3, st.nodes);
+    }
+}
+
 }  // namespace gp

@@ -323,12 +323,64 @@ var (
 	SingleAZMinimalFragmentation = singleAZ(MinimalFragmentation)
 	AzAwareTightlyPack           = binpack.SparkBinPackFunction(func(ctx context.Context, d, e *resources.Resources, k int,
 		dord, eord []string, md resources.NodeGroupSchedulingMetadata) *binpack.PackingResult {
-		if r := SingleAZTightlyPack(ctx, d, e, k, dord, eord, md); r.HasCapacity { // az_aware_pack_tightly.go:33-37
+		if r, ok := azAwareTightlyPackDevice(d, e, k, dord, eord, md); ok {
 			return r
 		}
-		return TightlyPack(ctx, d, e, k, dord, eord, md)
+		return binpack.AzAwareTightlyPack(ctx, d, e, k, dord, eord, md)
 	})
 )
+
+// azAwareTightlyPackDevice is AzAwareTightlyPack (LIB/binpack/az_aware_pack_tightly.go:27-38) for one application as
+// ONE gp_pack_batch_az_aware call on the az-aware layout: the zone packs, the zone choice and, when no zone wins, the
+// fallback over the undivided orders all run on the device.  ok=false (no device, a quantity that is not an exact int64,
+// a device error): the caller runs the Go packer.
+func azAwareTightlyPackDevice(driverResources, executorResources *resources.Resources, executorCount int,
+	driverNodePriorityOrder, executorNodePriorityOrder []string,
+	md resources.NodeGroupSchedulingMetadata) (*binpack.PackingResult, bool) {
+	d, err := getDevice()
+	if err != nil {
+		return nil, false
+	}
+	dc, dm, dg, ok1 := toTriple(driverResources)
+	ec, em, eg, ok2 := toTriple(executorResources)
+	l, ok3 := azAwareLayout(driverNodePriorityOrder, executorNodePriorityOrder, md)
+	if !ok1 || !ok2 || !ok3 || executorCount < 0 {
+		return nil, false
+	}
+	cnt := []int32{int32(executorCount)}
+	zone, driver := []int32{-1}, []int32{-1}
+	exec := make([]int32, max(executorCount, 1))
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	l.pin(&pin)
+	for _, p := range []any{&dc, &dm, &dg, &ec, &em, &eg, ptrOrNil32(cnt), ptrOrNil32(zone), ptrOrNil32(driver), ptrOrNil32(exec)} {
+		pin.Pin(p)
+	}
+	if !l.upload(d) {
+		return nil, false
+	}
+	ga := C.gp_apps{n_apps: 1, drv_cpu_milli: (*C.int64_t)(unsafe.Pointer(&dc)), drv_mem_bytes: (*C.int64_t)(unsafe.Pointer(&dm)),
+		drv_gpu: (*C.int64_t)(unsafe.Pointer(&dg)), exe_cpu_milli: (*C.int64_t)(unsafe.Pointer(&ec)),
+		exe_mem_bytes: (*C.int64_t)(unsafe.Pointer(&em)), exe_gpu: (*C.int64_t)(unsafe.Pointer(&eg)), exe_count: ptr32(cnt)}
+	orders := l.orders()
+	gz := C.gp_zone_results{zone: ptr32(zone), driver_node: ptr32(driver), executor_nodes: ptr32(exec), executor_nodes_cap: C.int64_t(len(exec))}
+	if st := C.gp_pack_batch_az_aware(d.ctx, &ga, &orders, &gz); st != C.GP_OK {
+		return nil, false
+	}
+	if driver[0] < 0 {
+		return binpack.EmptyPackingResult(), true
+	}
+	res := &binpack.PackingResult{DriverNode: l.s.names[driver[0]], HasCapacity: true, ExecutorNodes: make([]string, executorCount)}
+	for i := 0; i < executorCount; i++ {
+		res.ExecutorNodes[i] = l.s.names[exec[i]]
+	}
+	res.PackingEfficiencies = efficienciesFor(md, driverResources, executorResources, res, true)
+	return res, true
+}
 
 // RescheduleExecutorNode is the node choice of rescheduleExecutor (EXT/resource.go:652-662, 675-705) on the device:
 // minFrag selects rescheduleExecutorWithMinimalFragmentation (`md` = availableNodesSchedulingMetadata of :640, `overhead`
@@ -630,22 +682,20 @@ func FitEarlierDriversSingleAZ(algo C.gp_algo, apps []QueuedApp, nodeNames, exec
 	return fits, true
 }
 
-// FitEarlierDriversAzAware is FitEarlierDriversSingleAZ for `binpack: az-aware-tightly-pack` (AzAwareTightlyPack,
-// LIB/binpack/az_aware_pack_tightly.go:27-38): the candidate zones become instance groups 0..Z-1 as there, one trailing
-// group holds the other nodes of the two orders (a zone with driver candidates only, executor candidates of a zone without
-// driver candidates), and the undivided orders go along as node indices.  ONE gp_pack_fifo_az_aware call runs the whole
-// queue: the zone packs, and when no zone wins the fallback over the undivided orders, both on the device.
-// ok=false: the caller must run the original Go loop instead (also above 64 candidate zones).
-func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []string,
-	metadata resources.NodeGroupSchedulingMetadata) (fits bool, ok bool) {
-	d, err := getDevice()
-	if err != nil {
-		return false, false
-	}
-	if len(apps) == 0 {
-		return true, true
-	}
-	// groupNodesByZone for both orders; zones without executor candidates are left out (single_az.go:38-41)
+// azLayout is the snapshot of az-aware-tightly-pack (gp_pack_batch_az_aware, gp_pack_fifo_az_aware): the candidate zones
+// become instance groups 0..nZones-1 (groupNodesByZone in driverZonesInOrder order, zones without executor candidates
+// left out, single_az.go:36-41), one trailing group holds the other nodes of the two orders (a zone with driver candidates
+// only, executor candidates of a zone without driver candidates), and the undivided orders go along as node indices of
+// the same table (ue, ud).  sc / sm / sg: SchedulableResources of the table's nodes.
+type azLayout struct {
+	s                  *snapshot
+	sc, sm, sg         []int64
+	eoff, doff, ue, ud []int32
+	nZones             int
+}
+
+// azAwareLayout marshals the layout; ok=false when a quantity is not an exact int64.
+func azAwareLayout(nodeNames, executorNodeNames []string, metadata resources.NodeGroupSchedulingMetadata) (*azLayout, bool) {
 	group := func(names []string) ([]string, map[string][]string) {
 		order, byZone := []string{}, map[string][]string{}
 		for _, n := range names {
@@ -662,9 +712,9 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 	}
 	zones, dz := group(nodeNames)
 	_, ez := group(executorNodeNames)
-	s := &snapshot{}
+	l := &azLayout{s: &snapshot{}, eoff: []int32{0}, doff: []int32{0}}
+	s := l.s
 	index := map[string]int32{}
-	var sc, sm, sg []int64
 	intern := func(n string) (int32, bool) {
 		if i, seen := index[n]; seen {
 			return i, true
@@ -679,10 +729,9 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 		index[n] = i
 		s.names = append(s.names, n)
 		s.cpu, s.mem, s.gpu = append(s.cpu, c), append(s.mem, mm), append(s.gpu, g)
-		sc, sm, sg = append(sc, c2), append(sm, m2), append(sg, g2)
+		l.sc, l.sm, l.sg = append(l.sc, c2), append(l.sm, m2), append(l.sg, g2)
 		return i, true
 	}
-	eoff, doff := []int32{0}, []int32{0}
 	candidate := map[string]bool{}
 	for _, z := range zones {
 		eo, has := ez[z]
@@ -693,23 +742,20 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 		for _, n := range eo {
 			i, exact := intern(n)
 			if !exact {
-				return false, false
+				return nil, false
 			}
 			s.execIdx = append(s.execIdx, i)
 		}
 		for _, n := range dz[z] {
 			i, exact := intern(n)
 			if !exact {
-				return false, false
+				return nil, false
 			}
 			s.drvIdx = append(s.drvIdx, i)
 		}
-		eoff, doff = append(eoff, int32(len(s.execIdx))), append(doff, int32(len(s.drvIdx)))
+		l.eoff, l.doff = append(l.eoff, int32(len(s.execIdx))), append(l.doff, int32(len(s.drvIdx)))
 	}
-	nZones := len(eoff) - 1
-	if nZones > 64 {
-		return false, false // gp_pack_fifo_az_aware takes at most 64 candidate zones: the Go loop decides
-	}
+	l.nZones = len(l.eoff) - 1
 	// the trailing group: every node of the two orders outside the candidate zones (only the fallback reaches it)
 	rest := func(names []string, dst *[]int32) bool {
 		for _, n := range names {
@@ -726,13 +772,12 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 		return true
 	}
 	if !rest(executorNodeNames, &s.execIdx) || !rest(nodeNames, &s.drvIdx) {
-		return false, false
+		return nil, false
 	}
-	if nZones == 0 || int(eoff[nZones]) < len(s.execIdx) || int(doff[nZones]) < len(s.drvIdx) {
-		eoff, doff = append(eoff, int32(len(s.execIdx))), append(doff, int32(len(s.drvIdx)))
+	if l.nZones == 0 || int(l.eoff[l.nZones]) < len(s.execIdx) || int(l.doff[l.nZones]) < len(s.drvIdx) {
+		l.eoff, l.doff = append(l.eoff, int32(len(s.execIdx))), append(l.doff, int32(len(s.drvIdx)))
 	}
-	nGroups := len(eoff) - 1
-	// the undivided orders, as node indices of the same table (names absent from the metadata dropped)
+	// the undivided orders (names absent from the metadata dropped)
 	undivided := func(names []string) []int32 {
 		out := make([]int32, 0, len(names))
 		for _, n := range names {
@@ -742,7 +787,56 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 		}
 		return out
 	}
-	ue, ud := undivided(executorNodeNames), undivided(nodeNames)
+	l.ue, l.ud = undivided(executorNodeNames), undivided(nodeNames)
+	return l, true
+}
+
+// pin keeps the layout's arrays in place while C holds pointers to them.
+func (l *azLayout) pin(pin *runtime.Pinner) {
+	for _, p := range []any{ptrOrNil(l.s.cpu), ptrOrNil(l.s.mem), ptrOrNil(l.s.gpu), ptrOrNil32(l.s.execIdx), ptrOrNil32(l.s.drvIdx),
+		ptrOrNil32(l.eoff), ptrOrNil32(l.doff), ptrOrNil(l.sc), ptrOrNil(l.sm), ptrOrNil(l.sg), ptrOrNil32(l.ue), ptrOrNil32(l.ud)} {
+		if p != nil {
+			pin.Pin(p)
+		}
+	}
+}
+
+// upload sets the snapshot and its SchedulableResources on the device (d.mu held, arrays pinned).
+func (l *azLayout) upload(d *device) bool {
+	gn := C.gp_nodes{
+		n_nodes: C.int32_t(len(l.s.names)), avail_cpu_milli: ptr64(l.s.cpu), avail_mem_bytes: ptr64(l.s.mem), avail_gpu: ptr64(l.s.gpu),
+		n_groups: C.int32_t(len(l.eoff) - 1), exec_off: ptr32(l.eoff), exec_order: ptr32(l.s.execIdx), drv_off: ptr32(l.doff),
+		drv_order: ptr32(l.s.drvIdx),
+	}
+	if st := C.gp_set_snapshot(d.ctx, &gn); st != C.GP_OK {
+		return false
+	}
+	return C.gp_set_schedulable(d.ctx, ptr64(l.sc), ptr64(l.sm), ptr64(l.sg)) == C.GP_OK
+}
+
+func (l *azLayout) orders() C.gp_az_orders {
+	return C.gp_az_orders{n_zones: C.int32_t(l.nZones), n_exec: C.int32_t(len(l.ue)), exec_order: ptr32(l.ue),
+		n_drv: C.int32_t(len(l.ud)), drv_order: ptr32(l.ud)}
+}
+
+// FitEarlierDriversAzAware is FitEarlierDriversSingleAZ for `binpack: az-aware-tightly-pack` (AzAwareTightlyPack,
+// LIB/binpack/az_aware_pack_tightly.go:27-38) on the az-aware layout (azAwareLayout).  ONE gp_pack_fifo_az_aware call
+// runs the whole queue: the zone packs, and when no zone wins the fallback over the undivided orders, both on the device.
+// ok=false: the caller must run the original Go loop instead (also above 64 candidate zones).
+func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []string,
+	metadata resources.NodeGroupSchedulingMetadata) (fits bool, ok bool) {
+	d, err := getDevice()
+	if err != nil {
+		return false, false
+	}
+	if len(apps) == 0 {
+		return true, true
+	}
+	l, exact := azAwareLayout(nodeNames, executorNodeNames, metadata)
+	if !exact || l.nZones > 64 {
+		return false, false // gp_pack_fifo_az_aware takes at most 64 candidate zones: the Go loop decides
+	}
+	s := l.s
 	q := len(apps)
 	dc, dm, dg := make([]int64, q), make([]int64, q), make([]int64, q)
 	ec, em, eg := make([]int64, q), make([]int64, q), make([]int64, q)
@@ -769,28 +863,19 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 	defer d.mu.Unlock()
 	var pin runtime.Pinner
 	defer pin.Unpin()
-	for _, p := range []any{ptrOrNil(s.cpu), ptrOrNil(s.mem), ptrOrNil(s.gpu), ptrOrNil32(s.execIdx), ptrOrNil32(s.drvIdx),
-		ptrOrNil32(eoff), ptrOrNil32(doff), ptrOrNil(sc), ptrOrNil(sm), ptrOrNil(sg), ptrOrNil32(ue), ptrOrNil32(ud),
-		ptrOrNil(dc), ptrOrNil(dm), ptrOrNil(dg), ptrOrNil(ec), ptrOrNil(em), ptrOrNil(eg),
+	l.pin(&pin)
+	for _, p := range []any{ptrOrNil(dc), ptrOrNil(dm), ptrOrNil(dg), ptrOrNil(ec), ptrOrNil(em), ptrOrNil(eg),
 		ptrOrNil32(cnt), ptrOrNil8(skip), ptrOrNil32(zone), ptrOrNil32(driver), ptrOrNil32(exec)} {
 		if p != nil {
 			pin.Pin(p)
 		}
 	}
-	gn := C.gp_nodes{
-		n_nodes: C.int32_t(len(s.names)), avail_cpu_milli: ptr64(s.cpu), avail_mem_bytes: ptr64(s.mem), avail_gpu: ptr64(s.gpu),
-		n_groups: C.int32_t(nGroups), exec_off: ptr32(eoff), exec_order: ptr32(s.execIdx), drv_off: ptr32(doff), drv_order: ptr32(s.drvIdx),
-	}
-	if st := C.gp_set_snapshot(d.ctx, &gn); st != C.GP_OK {
-		return false, false
-	}
-	if st := C.gp_set_schedulable(d.ctx, ptr64(sc), ptr64(sm), ptr64(sg)); st != C.GP_OK {
+	if !l.upload(d) {
 		return false, false
 	}
 	ga := C.gp_apps{n_apps: C.int32_t(q), drv_cpu_milli: ptr64(dc), drv_mem_bytes: ptr64(dm), drv_gpu: ptr64(dg),
 		exe_cpu_milli: ptr64(ec), exe_mem_bytes: ptr64(em), exe_gpu: ptr64(eg), exe_count: ptr32(cnt), skip_if_no_fit: ptr8(skip)}
-	orders := C.gp_az_orders{n_zones: C.int32_t(nZones), n_exec: C.int32_t(len(ue)), exec_order: ptr32(ue),
-		n_drv: C.int32_t(len(ud)), drv_order: ptr32(ud)}
+	orders := l.orders()
 	gz := C.gp_zone_results{zone: ptr32(zone), driver_node: ptr32(driver), executor_nodes: ptr32(exec), executor_nodes_cap: C.int64_t(len(exec))}
 	if st := C.gp_pack_fifo_az_aware(d.ctx, &ga, C.GP_MODE_FIFO_REFERENCE, &orders, &gz); st != C.GP_OK {
 		return false, false

@@ -345,6 +345,55 @@ inline void groupNodesByZone(const std::vector<std::string>& nodeNames, const re
     }
 }
 
+using ZoneGroupList = std::vector<std::pair<std::vector<std::string>, std::vector<std::string>>>;   // (driver order, executor order)
+
+// The candidate zones of the single-AZ packers in driverZonesInOrder order: one group per zone with both kinds of
+// candidates, each holding the two orders restricted to that zone (single_az.go:30-41).
+inline ZoneGroupList ZoneGroups(const std::vector<std::string>& driverOrder, const std::vector<std::string>& executorOrder,
+                                const resources::NodeGroupSchedulingMetadata& md) {
+    std::vector<std::string> dzOrder, ezOrder;
+    std::unordered_map<std::string, std::vector<std::string>> dz, ez;
+    groupNodesByZone(driverOrder, md, &dzOrder, &dz);
+    groupNodesByZone(executorOrder, md, &ezOrder, &ez);
+    ZoneGroupList groups;
+    for (const auto& z : dzOrder)
+        if (ez.count(z)) groups.emplace_back(dz[z], ez[z]);                         // :36-41
+    return groups;
+}
+
+// The snapshot layout of az-aware-tightly-pack (gp_pack_batch_az_aware, gp_pack_fifo_az_aware): the candidate zones, then
+// one trailing group with the nodes of both orders that no candidate zone contains -- only the undivided fallback
+// (az_aware_pack_tightly.go:33-37) reaches them.  Returns the number of candidate zones.
+inline int32_t AzAwareLayout(const std::vector<std::string>& driverOrder, const std::vector<std::string>& executorOrder,
+                             const resources::NodeGroupSchedulingMetadata& md, ZoneGroupList* groups) {
+    *groups = ZoneGroups(driverOrder, executorOrder, md);
+    const int32_t nZones = (int32_t)groups->size();
+    std::unordered_set<std::string> inZone;
+    for (const auto& g : *groups) {
+        inZone.insert(g.first.begin(), g.first.end());
+        inZone.insert(g.second.begin(), g.second.end());
+    }
+    std::pair<std::vector<std::string>, std::vector<std::string>> rest;
+    for (const auto& n : driverOrder) if (md.count(n) && !inZone.count(n)) rest.first.push_back(n);
+    for (const auto& n : executorOrder) if (md.count(n) && !inZone.count(n)) rest.second.push_back(n);
+    if (groups->empty() || !rest.first.empty() || !rest.second.empty()) groups->push_back(std::move(rest));
+    return nZones;
+}
+
+// The undivided orders of az-aware-tightly-pack as node indices of the snapshot `d` holds (names it does not know are
+// dropped, as in the groups).  eo / dord own the arrays the result points to.
+inline gp_az_orders UndividedOrders(const gangpack::Device& d, int32_t nZones, const std::vector<std::string>& driverOrder,
+                                    const std::vector<std::string>& executorOrder, std::vector<int32_t>* eo, std::vector<int32_t>* dord) {
+    eo->clear(); dord->clear();
+    for (const auto& n : executorOrder) { const int32_t i = d.index(n); if (i >= 0) eo->push_back(i); }
+    for (const auto& n : driverOrder) { const int32_t i = d.index(n); if (i >= 0) dord->push_back(i); }
+    gp_az_orders o{};
+    o.n_zones = nZones;
+    o.n_exec = (int32_t)eo->size(); o.exec_order = eo->data();
+    o.n_drv = (int32_t)dord->size(); o.drv_order = dord->data();
+    return o;
+}
+
 // getSingleAZSparkBinFunction(fn) + chooseBestResult, single_az.go:23-55,75-97, fn = tightlyPackExecutors or
 // minimalFragmentation: every candidate zone is packed in ONE device batch (zone = instance group), the best result
 // is chosen on the host by average packing efficiency over [driver] + ExecutorNodes.  The efficiencies come from
@@ -353,13 +402,7 @@ inline void groupNodesByZone(const std::vector<std::string>& nodeNames, const re
 inline PackingResult SingleAZPackImpl(gp_algo algo, const resources::Resources& drv, const resources::Resources& exe, int count,
                                       const std::vector<std::string>& driverOrder, const std::vector<std::string>& executorOrder,
                                       const resources::NodeGroupSchedulingMetadata& md) {
-    std::vector<std::string> dzOrder, ezOrder;
-    std::unordered_map<std::string, std::vector<std::string>> dz, ez;
-    groupNodesByZone(driverOrder, md, &dzOrder, &dz);
-    groupNodesByZone(executorOrder, md, &ezOrder, &ez);
-    std::vector<std::pair<std::vector<std::string>, std::vector<std::string>>> groups;
-    for (const auto& z : dzOrder)
-        if (ez.count(z)) groups.emplace_back(dz[z], ez[z]);                         // :36-41
+    const ZoneGroupList groups = ZoneGroups(driverOrder, executorOrder, md);
     if (groups.empty()) return EmptyPackingResult();
     gangpack::Device& d = gangpack::Device::Get();
     d.SetSnapshotGroups(md, groups);
@@ -397,14 +440,44 @@ inline PackingResult SingleAZPackImpl(gp_algo algo, const resources::Resources& 
     return best;
 }
 
+// AzAwareTightlyPack (az_aware_pack_tightly.go:27-38) for one application: one upload of the az-aware layout and one
+// gp_pack_batch_az_aware call -- the zone packs, the zone choice and, when no zone wins, the undivided fallback all run
+// on the device.
+inline PackingResult AzAwarePackImpl(const resources::Resources& drv, const resources::Resources& exe, int count,
+                                     const std::vector<std::string>& driverOrder, const std::vector<std::string>& executorOrder,
+                                     const resources::NodeGroupSchedulingMetadata& md) {
+    ZoneGroupList groups;
+    const int32_t nZones = AzAwareLayout(driverOrder, executorOrder, md, &groups);
+    gangpack::Device& d = gangpack::Device::Get();
+    d.SetSnapshotGroups(md, groups);
+    d.SetSchedulable(md);
+    std::vector<int32_t> eo, dord;
+    const gp_az_orders o = UndividedOrders(d, nZones, driverOrder, executorOrder, &eo, &dord);
+    int64_t dc = drv.CPU, dm = drv.Memory, dg = drv.NvidiaGPU, ec = exe.CPU, em = exe.Memory, eg = exe.NvidiaGPU;
+    int32_t cnt = count, zone = -1, driver = -1;
+    std::vector<int32_t> exec((size_t)std::max(count, 1));
+    gp_apps a{};
+    a.n_apps = 1;
+    a.drv_cpu_milli = &dc; a.drv_mem_bytes = &dm; a.drv_gpu = &dg;
+    a.exe_cpu_milli = &ec; a.exe_mem_bytes = &em; a.exe_gpu = &eg;
+    a.exe_count = &cnt;
+    gp_zone_results r{};
+    r.zone = &zone; r.driver_node = &driver; r.executor_nodes = exec.data(); r.executor_nodes_cap = (int64_t)exec.size();
+    d.check(gp_pack_batch_az_aware(d.ctx(), &a, &o, &r), "gp_pack_batch_az_aware");
+    if (driver < 0) return EmptyPackingResult();
+    PackingResult res;
+    res.HasCapacity = true;
+    res.DriverNode = d.name(driver);
+    for (int t = 0; t < count; ++t) res.ExecutorNodes.push_back(d.name(exec[(size_t)t]));
+    return res;
+}
+
 inline PackingResult GuardedSingleAZ(bool azAware, const resources::Resources& d, const resources::Resources& e, int c,
                                      const std::vector<std::string>& dord, const std::vector<std::string>& eord,
                                      const resources::NodeGroupSchedulingMetadata& md, gp_algo algo = GP_TIGHTLY_PACK) {
     const int key = algo == GP_MINIMAL_FRAGMENTATION ? 102 : (azAware ? 101 : 100);
     try {
-        PackingResult r = SingleAZPackImpl(algo, d, e, c, dord, eord, md);
-        if (r.HasCapacity || !azAware) return r;
-        return gangpack::PackOne(GP_TIGHTLY_PACK, d, e, c, dord, eord, md);          // az_aware_pack_tightly.go:33-37
+        return azAware ? AzAwarePackImpl(d, e, c, dord, eord, md) : SingleAZPackImpl(algo, d, e, c, dord, eord, md);
     } catch (const gangpack::Error&) {
         auto f = gangpack::Fallbacks().find(key);
         if (f != gangpack::Fallbacks().end() && f->second) return f->second(d, e, c, dord, eord, md);
@@ -625,37 +698,21 @@ inline bool FitEarlierDrivers(const binpacker::Binpacker& packer, const std::vec
     if (results) results->assign(drivers.size(), binpack::EmptyPackingResult());
     if (live.empty()) return true;
     const bool azAware = packer.Name == binpacker::azAwareTightlyPack;
-    std::vector<std::pair<std::vector<std::string>, std::vector<std::string>>> groups;
-    if (packer.IsSingleAz || azAware) {
-        std::vector<std::string> dzOrder, ezOrder;
-        std::unordered_map<std::string, std::vector<std::string>> dz, ez;
-        binpack::groupNodesByZone(nodeNames, metadata, &dzOrder, &dz);
-        binpack::groupNodesByZone(executorNodeNames, metadata, &ezOrder, &ez);
-        for (const auto& z : dzOrder)
-            if (ez.count(z)) groups.emplace_back(dz[z], ez[z]);                 // single_az.go:36-41
+    binpack::ZoneGroupList groups;
+    int32_t nZones = 0;
+    if (azAware) nZones = binpack::AzAwareLayout(nodeNames, executorNodeNames, metadata, &groups);
+    else if (packer.IsSingleAz) {
+        groups = binpack::ZoneGroups(nodeNames, executorNodeNames, metadata);
+        nZones = (int32_t)groups.size();
     }
     // The single-AZ packers and az-aware-tightly-pack (up to 64 candidate zones): the whole queue in ONE launch -- zone =
     // instance group, the zone choice (or az-aware's undivided fallback) of driver i feeds driver i+1 on the device.
     // az-aware-tightly-pack with more zones keeps the per-driver loop below (gp_pack_fifo_az_aware takes at most 64).
-    if (packer.IsSingleAz || (azAware && groups.size() <= 64)) {
+    if (packer.IsSingleAz || (azAware && nZones <= 64)) {
         const size_t q = live.size();
-        const int32_t nZones = (int32_t)groups.size();
         if (packer.IsSingleAz && groups.empty()) {                              // EmptyPackingResult for every driver
             for (size_t j = 0; j < q; ++j) if (!drivers[live[j]].SkipIfNoFit) return false;
             return true;
-        }
-        if (azAware) {
-            // one trailing group with the nodes of both orders that no candidate zone contains: only the undivided
-            // fallback (az_aware_pack_tightly.go:33-37) reaches them
-            std::unordered_set<std::string> inZone;
-            for (const auto& g : groups) {
-                inZone.insert(g.first.begin(), g.first.end());
-                inZone.insert(g.second.begin(), g.second.end());
-            }
-            std::pair<std::vector<std::string>, std::vector<std::string>> rest;
-            for (const auto& n : nodeNames) if (metadata.count(n) && !inZone.count(n)) rest.first.push_back(n);
-            for (const auto& n : executorNodeNames) if (metadata.count(n) && !inZone.count(n)) rest.second.push_back(n);
-            if (groups.empty() || !rest.first.empty() || !rest.second.empty()) groups.push_back(std::move(rest));
         }
         gangpack::Device& d = gangpack::Device::Get();
         d.SetSnapshotGroups(metadata, groups);
@@ -681,13 +738,8 @@ inline bool FitEarlierDrivers(const binpacker::Binpacker& packer, const std::vec
         gp_zone_results r{};
         r.zone = zone.data(); r.driver_node = driver.data(); r.executor_nodes = exec.data(); r.executor_nodes_cap = (int64_t)exec.size();
         if (azAware) {
-            std::vector<int32_t> eo, dord;                                      // the undivided orders as node indices
-            for (const auto& n : executorNodeNames) { const int32_t i = d.index(n); if (i >= 0) eo.push_back(i); }
-            for (const auto& n : nodeNames) { const int32_t i = d.index(n); if (i >= 0) dord.push_back(i); }
-            gp_az_orders o{};
-            o.n_zones = nZones;
-            o.n_exec = (int32_t)eo.size(); o.exec_order = eo.data();
-            o.n_drv = (int32_t)dord.size(); o.drv_order = dord.data();
+            std::vector<int32_t> eo, dord;
+            const gp_az_orders o = binpack::UndividedOrders(d, nZones, nodeNames, executorNodeNames, &eo, &dord);
             d.check(gp_pack_fifo_az_aware(d.ctx(), &a, GP_MODE_FIFO_REFERENCE, &o, &r), "gp_pack_fifo_az_aware");
         } else {
             d.check(gp_pack_fifo_zones(d.ctx(), &a, (gp_algo)packer.algo, GP_MODE_FIFO_REFERENCE, &r), "gp_pack_fifo_zones");

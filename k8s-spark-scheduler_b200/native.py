@@ -35,7 +35,7 @@ STATUS_NAMES = {0: "GP_OK", 1: "GP_ERR_INVALID", 2: "GP_ERR_CUDA", 3: "GP_ERR_NO
 
 # every symbol include/gangpack.h declares (tests assert the .so exports exactly these)
 EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_backend", "gp_alloc_pinned",
-           "gp_free_pinned", "gp_register_host", "gp_unregister_host", "gp_set_snapshot", "gp_get_snapshot", "gp_pack_batch", "gp_pack_batch_wire", "gp_pack_one", "gp_set_schedulable", "gp_pack_batch_zones", "gp_pack_fifo_zones", "gp_pack_fifo_az_aware", "gp_reserve_placements", "gp_apply_usage_delta",
+           "gp_free_pinned", "gp_register_host", "gp_unregister_host", "gp_set_snapshot", "gp_get_snapshot", "gp_pack_batch", "gp_pack_batch_wire", "gp_pack_one", "gp_set_schedulable", "gp_pack_batch_zones", "gp_pack_fifo_zones", "gp_pack_fifo_az_aware", "gp_pack_batch_az_aware", "gp_reserve_placements", "gp_apply_usage_delta",
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_reschedule_executors",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -192,6 +192,8 @@ def load():
     L.gp_pack_fifo_zones.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.c_int, C.POINTER(gp_zone_results)]
     L.gp_pack_fifo_az_aware.restype = C.c_int
     L.gp_pack_fifo_az_aware.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_az_orders), C.POINTER(gp_zone_results)]
+    L.gp_pack_batch_az_aware.restype = C.c_int
+    L.gp_pack_batch_az_aware.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_az_orders), C.POINTER(gp_zone_results)]
     L.gp_reserve_placements.restype = C.c_int
     L.gp_reserve_placements.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_results), C.c_int32, C.POINTER(gp_reservation_table)]
     L.gp_apply_usage_delta.restype = C.c_int
@@ -570,6 +572,28 @@ class GangPacker:
         self._check(load().gp_pack_fifo_az_aware(self._h, C.byref(a), mode, C.byref(o), C.byref(r)))
         return zone, drv, exe[:total], off, avg[:q]
 
+    def pack_batch_az_aware(self, apps: dict, exec_order, drv_order, n_zones: int):
+        """az-aware-tightly-pack for a batch of independent decisions against the unmodified snapshot, in one call.  The
+        snapshot layout is that of pack_fifo_az_aware (any n_zones up to the number of groups); exec_order / drv_order are
+        the undivided priority orders (node indices) of the fallback.  -> like pack_batch_zones; zone -1 with
+        driver_node >= 0 = placed by the fallback (zero averages)."""
+        q = len(apps["count"])
+        count = _np(apps["count"], np.int32)
+        off = np.zeros(q + 1, np.int64)
+        np.cumsum(np.maximum(count, 0), out=off[1:])
+        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
+        eo, do = _np(exec_order, np.int32), _np(drv_order, np.int32)
+        total = int(off[-1]) if q else 0
+        zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
+        exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
+        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
+                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
+                    exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
+        o = gp_az_orders(n_zones=int(n_zones), n_exec=len(eo), exec_order=_p(eo), n_drv=len(do), drv_order=_p(do))
+        r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
+        self._check(load().gp_pack_batch_az_aware(self._h, C.byref(a), C.byref(o), C.byref(r)))
+        return zone, drv, exe[:total], off, avg[:q]
+
     def reserve_placements(self, apps: dict, placed, subtract=True):
         """newResourceReservation for a packed batch -> dict of row arrays (app, slot, node, cpu, mem, gpu); with subtract the
         device-resident snapshot is charged with every reserved pod.  placed = (driver_node, executor_nodes, off)."""
@@ -650,8 +674,8 @@ class GangPacker:
     def stats(self) -> dict:
         """gp_last_stats of the last pack call.  scan_path_apps: independent tightly / evenly batches count the applications
         the node-order scan decided instead of the capacity tables; the FIFO modes count the applications the whole CTA
-        decided instead of warp 0 alone (all evaluated ones with GANGPACK_FIFO_WARP=0); pack_fifo_az_aware counts the
-        applications for which the undivided fallback ran."""
+        decided instead of warp 0 alone (all evaluated ones with GANGPACK_FIFO_WARP=0); pack_fifo_az_aware and
+        pack_batch_az_aware count the applications for which the undivided fallback ran."""
         s = gp_stats()
         self._check(load().gp_last_stats(self._h, C.byref(s)))
         return {"nodes_scanned": s.nodes_scanned, "drivers_tried": s.drivers_tried, "kernel_launches": s.kernel_launches,

@@ -8,7 +8,14 @@ Prints one JSON line; the two paths must agree bit for bit.
 holds the zone-grouped snapshot and runs gp_pack_batch_zones for the driver, the other the undivided snapshot and runs
 gp_pack_one when no zone wins; both are charged with gp_reserve_placements(subtract) after every placed driver.  3 000
 nodes in 4 zones of unequal size; every 250th application asks for more executors than the largest zone holds, so the
-undivided fallback runs (the JSON line reports how often and how many it placed)."""
+undivided fallback runs (the JSON line reports how often and how many it placed).
+
+--packer az-aware-tightly-pack --independent: a batch of independent decisions on the same cluster, one
+gp_pack_batch_az_aware call against the two-context recipe it replaces -- gp_pack_batch_zones on a context holding the
+zone-grouped snapshot, the zone -1 applications gathered on the host, gp_pack_batch(tightly-pack) over the undivided
+orders on a second context, the results merged on the host.  Both snapshots stay resident (no upload is timed); every
+50th application asks for more executors than the largest zone holds.  The two paths must agree bit for bit, and the
+JSON line names the card and its power limit."""
 import argparse
 import json
 import os
@@ -23,8 +30,9 @@ import k8s_spark_scheduler_b200 as g  # noqa: E402
 from k8s_spark_scheduler_b200 import synth  # noqa: E402
 
 
-def az_aware():
-    n, q, q_loop = 3000, 2000, 300
+def az_case(q, big_every):
+    """3 000 nodes in 4 zones of unequal size and q synth applications, every big_every-th larger than any zone holds."""
+    n = 3000
     nodes = synth.make_nodes(n)
     cpu, mem, gpu = nodes["avail_cpu"], nodes["avail_mem"], nodes["avail_gpu"]
     order = synth.priority_order(cpu, mem).astype(np.int32)
@@ -34,12 +42,84 @@ def az_aware():
     eo = np.concatenate([order[zone_of[order] == z] for z in range(Z)]).astype(np.int32)
     eoff = np.concatenate([[0], np.cumsum([(zone_of == z).sum() for z in range(Z)])]).astype(np.int32)
     apps = synth.make_apps(q, seed=11)
-    keys = ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu", "count")
-    a = {k: np.array(apps[k]) for k in keys}
+    a = {k: np.array(apps[k]) for k in KEYS}
     a["young"] = np.ones(q, np.uint8)
-    for i in range(0, q, 250):                                          # larger than any one zone holds
+    for i in range(0, q, big_every):                                    # larger than any one zone holds
         caps = np.minimum(np.maximum(cpu, 0) // max(int(a["exe_cpu"][i]), 1), np.maximum(mem, 0) // max(int(a["exe_mem"][i]), 1))
         a["count"][i] = int(max(caps[zone_of == z].sum() for z in range(Z)) * 1.1) + 1
+    return n, Z, cpu, mem, gpu, order, eo, eoff, a
+
+
+KEYS = ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu", "count")
+
+
+def card():
+    """name and power limit of the card, read in the same run as the measurement"""
+    import torch
+    import subprocess
+    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": out}
+
+
+def az_aware_independent():
+    q, reps = 4000, 20
+    n, Z, cpu, mem, gpu, order, eo, eoff, a = az_case(q, 50)
+    sc, sm, sg = cpu + 4000, mem + (8 << 30), gpu
+    p, pz, pu = g.GangPacker(), g.GangPacker(), g.GangPacker()
+    p.set_snapshot(cpu, mem, gpu, eo, eo, eoff, eoff)                   # every zone a candidate: no trailing group
+    p.set_schedulable(sc, sm, sg)
+    pz.set_snapshot(cpu, mem, gpu, eo, eo, eoff, eoff)
+    pz.set_schedulable(sc, sm, sg)
+    pu.set_snapshot(cpu, mem, gpu, order, order)
+
+    def one_call():
+        return p.pack_batch_az_aware(a, order, order, Z)
+
+    def recipe():
+        zone, drv, exe, off, avg = pz.pack_batch_zones(a, 0)
+        fb = np.nonzero(zone == -1)[0]
+        if fb.size:
+            d2, e2, o2 = pu.pack_batch({k: a[k][fb] for k in KEYS}, 0, 0)
+            drv[fb] = d2
+            for j in np.nonzero(d2 >= 0)[0]:
+                i = fb[j]
+                exe[off[i]:off[i + 1]] = e2[o2[j]:o2[j + 1]]
+        return zone, drv, exe, off, avg
+
+    t_one, t_two = [], []
+    for r in range(reps + 2):                                           # alternate the two paths; the first two are warm-up
+        for f, ts in ((one_call, t_one), (recipe, t_two)):
+            t0 = time.perf_counter()
+            res = f()
+            if r >= 2:
+                ts.append(time.perf_counter() - t0)
+        if r == 0:
+            got, want = one_call(), recipe()
+            fallbacks = p.stats()["scan_path_apps"]
+    zone, gd, ge, goff, avg = got
+    placed = np.zeros(len(ge), bool)
+    for i in np.nonzero(gd >= 0)[0]:
+        placed[goff[i]:goff[i + 1]] = True
+    won = zone >= 0
+    same = bool(np.array_equal(zone, want[0]) and np.array_equal(gd, want[1]) and np.array_equal(ge[placed], want[2][placed])
+                and np.array_equal(avg[won].view(np.uint64), want[4][won].view(np.uint64)) and (avg[~won] == 0.0).all())
+    del res
+    print(json.dumps(dict({"workload": "az-aware-tightly-pack, %d independent decisions, %d nodes in %d zones of unequal size"
+                                       % (q, n, Z),
+                           "one_call_ms": float(np.median(t_one)) * 1e3, "one_call_ms_min": float(np.min(t_one)) * 1e3,
+                           "two_context_recipe_ms": float(np.median(t_two)) * 1e3,
+                           "two_context_recipe_ms_min": float(np.min(t_two)) * 1e3, "reps": reps,
+                           "placed": int((gd >= 0).sum()), "fallback_ran": int(fallbacks),
+                           "fallback_placed": int(((zone == -1) & (gd >= 0)).sum()), "paths_agree": same}, **card())))
+    for x in (p, pz, pu):
+        x.close()
+
+
+def az_aware():
+    q, q_loop = 2000, 300
+    n, Z, cpu, mem, gpu, order, eo, eoff, a = az_case(q, 250)
+    keys = KEYS
     sc, sm, sg = cpu + 4000, mem + (8 << 30), gpu
     p, pz, pu = g.GangPacker(), g.GangPacker(), g.GangPacker()
 
@@ -94,8 +174,12 @@ def az_aware():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--packer", choices=("single-az-tightly-pack", "az-aware-tightly-pack"), default="single-az-tightly-pack")
-    if ap.parse_args().packer == "az-aware-tightly-pack":
-        return az_aware()
+    ap.add_argument("--independent", action="store_true", help="az-aware-tightly-pack: a batch of independent decisions")
+    args = ap.parse_args()
+    if args.independent and args.packer != "az-aware-tightly-pack":
+        ap.error("--independent goes with --packer az-aware-tightly-pack")
+    if args.packer == "az-aware-tightly-pack":
+        return az_aware_independent() if args.independent else az_aware()
     n, Z, q, q_loop = 3000, 3, 2000, 300
     nodes = synth.make_nodes(n)
     cpu, mem, gpu = nodes["avail_cpu"], nodes["avail_mem"], nodes["avail_gpu"]
