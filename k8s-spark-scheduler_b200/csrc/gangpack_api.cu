@@ -179,17 +179,24 @@ __device__ __forceinline__ void note_node(SnapMeta* meta, int64_t cv, int64_t mv
 // The slot layout is two launches (gp_set_snapshot, gp_set_snapshot_device, gp_prepare_cluster):
 // K1 gp_build_slots_exec: thread i writes group descriptor i, lays out executor-order entry i in its slot and notes the
 //    availability of driver-order entry i in the snapshot maxima / flags (a node's availability does not depend on its slot);
+//    with node_cpu != NULL it also copies node-table entry i into the context's node-table arrays (gp_get_snapshot);
 // K2 gp_build_slots_drv: thread s owns slot s.  Executor slots get their compact view; the spare slot of driver-order
 //    entry j either receives that node (driver-only) or stays unused (-1: the node has an executor slot in the group);
 //    slots past the last group (the orders' lengths may be upper bounds) are -1 as well.  So no slot_node memset is needed.
 // n_exec / n_drv may be upper bounds of exec_off[n_groups] / drv_off[n_groups] (device-built orders).
-__global__ void gp_build_slots_exec(int32_t n_exec, int32_t n_drv, int32_t n_groups,
+__global__ void gp_build_slots_exec(int32_t n_exec, int32_t n_drv, int32_t n_groups, int32_t n_nodes,
                                     const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
                                     const int32_t* __restrict__ exec_order, const int32_t* __restrict__ drv_order,
                                     const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
                                     GroupDesc* __restrict__ groups, longlong2* __restrict__ pair, int64_t* __restrict__ sgpu,
-                                    int32_t* __restrict__ slot_node, int32_t* __restrict__ node_slot, SnapMeta* __restrict__ meta) {
+                                    int32_t* __restrict__ slot_node, int32_t* __restrict__ node_slot, SnapMeta* __restrict__ meta,
+                                    int64_t* __restrict__ node_cpu, int64_t* __restrict__ node_mem, int64_t* __restrict__ node_gpu) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (node_cpu && i < n_nodes) {
+        node_cpu[i] = cpu[i];
+        node_mem[i] = mem[i];
+        node_gpu[i] = gpu ? gpu[i] : 0;
+    }
     if (i < n_groups) {
         GroupDesc d;
         d.sbase = exec_off[i] + drv_off[i];
@@ -398,8 +405,8 @@ struct gp_ctx {
     int chunk_apps = kChunkApps;                  // GANGPACK_CHUNK_APPS
     int trace = 0;                                // GANGPACK_TRACE=1: host-side phase timing on stderr
     int pack_ctas_per_sm[3] = {0, 0, 0};            // occupancy of gp_pack_independent<ALGO> on this device
-    int tab_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_pack_tables<ALGO, OUT>
-    bool tab_attr_set[2] = {false, false};
+    int tab_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_pack_listed<ALGO, OUT>
+    int dec_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_decide_tables<ALGO, OUT>
     // per pipeline lane: shape hash + header, capacity tables, group totals, placement prefixes, per-application shape slot
     struct TableSet { DevBuf hdr, table, total, place, app_slot; } tabs[kLanes];
     bool record_events = true;                    // CUDA events around the kernels (gp_last_stats); the pipelined host path skips them
@@ -640,8 +647,10 @@ gp_status gp_synchronize(gp_ctx* ctx) {
 
 // ---- snapshot ---------------------------------------------------------------------------------
 
-// Build the slot layout from DEVICE-resident gp_nodes arrays on `st`.
-static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, cudaStream_t st) {
+// Build the slot layout from DEVICE-resident gp_nodes arrays on `st`.  copy_nodes: the layout kernel also copies the node
+// table into node_cpu / node_mem / node_gpu (reserved by the caller; false when dn already points at them).
+static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, cudaStream_t st,
+                                       bool copy_nodes = false) {
     const int32_t n_slots = n_exec + n_drv;
     c->host_layout = false;              // gp_set_snapshot sets it again once the layout it validated is in place
     GP_CUDA(c, c->pair.reserve(sizeof(longlong2) * (size_t)(n_slots + 1)));
@@ -651,9 +660,11 @@ static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_
     GP_CUDA(c, c->node_slot.reserve(sizeof(int32_t) * (size_t)(dn->n_nodes + 1)));
     GP_CUDA(c, c->drv_slot.reserve(sizeof(int32_t) * (size_t)(n_drv + 1)));
     GP_CUDA(c, c->groups.reserve(sizeof(GroupDesc) * (size_t)dn->n_groups));
-    struct { gp_nodes dn; int32_t n_exec, n_drv; void* buf[8]; } key{};
+    int64_t* node_cpu = copy_nodes ? c->node_cpu.as<int64_t>() : nullptr;
+    struct { gp_nodes dn; int32_t n_exec, n_drv; void* buf[11]; } key{};
     key.dn = *dn; key.n_exec = n_exec; key.n_drv = n_drv;
-    void* bufs[8] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p};
+    void* bufs[11] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p,
+                      node_cpu, c->node_mem.p, c->node_gpu.p};
     std::memcpy(key.buf, bufs, sizeof(bufs));
     gp_status rs = run_cached(c, c->g_snapshot, &key, sizeof(key), st, [&](int& launches) -> gp_status {
         // node_slot must be -1 for every node outside the orders (K2 reads it for the driver-order nodes); every slot_node
@@ -661,11 +672,12 @@ static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_
         GP_CUDA(c, cudaMemsetAsync(c->node_slot.p, 0xFF, sizeof(int32_t) * (size_t)(dn->n_nodes + 1), st));
         GP_CUDA(c, cudaMemsetAsync(c->snap_flags.p, 0, sizeof(SnapMeta), st));
         const int T = 256;
-        const int32_t n1 = std::max(std::max(n_exec, n_drv), dn->n_groups);
+        const int32_t n1 = std::max(std::max(std::max(n_exec, n_drv), dn->n_groups), node_cpu ? dn->n_nodes : 0);
         gp_build_slots_exec<<<(n1 + T - 1) / T, T, 0, st>>>(
-            n_exec, n_drv, dn->n_groups, dn->exec_off, dn->drv_off, dn->exec_order, dn->drv_order, dn->avail_cpu_milli,
+            n_exec, n_drv, dn->n_groups, dn->n_nodes, dn->exec_off, dn->drv_off, dn->exec_order, dn->drv_order, dn->avail_cpu_milli,
             dn->avail_mem_bytes, dn->avail_gpu, c->groups.as<GroupDesc>(), c->pair.as<longlong2>(), c->sgpu.as<int64_t>(),
-            c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>());
+            c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>(), node_cpu, c->node_mem.as<int64_t>(),
+            c->node_gpu.as<int64_t>());
         gp_build_slots_drv<<<(n_slots + T) / T, T, 0, st>>>(
             n_slots, dn->n_groups, dn->exec_off, dn->drv_off, dn->drv_order, dn->avail_cpu_milli, dn->avail_mem_bytes,
             dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(), c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(),
@@ -798,16 +810,10 @@ gp_status gp_set_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, 
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot_device: missing arrays or bad sizes");
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : c->stream;
-    // keep a node-table copy so gp_get_snapshot can answer for nodes outside every group
-    const size_t nb = sizeof(int64_t) * (size_t)(dn->n_nodes + 1), vb = sizeof(int64_t) * (size_t)dn->n_nodes;
+    // keep a node-table copy so gp_get_snapshot can answer for nodes outside every group: the layout kernel makes it
+    const size_t nb = sizeof(int64_t) * (size_t)(dn->n_nodes + 1);
     GP_CUDA(c, c->node_cpu.reserve(nb)); GP_CUDA(c, c->node_mem.reserve(nb)); GP_CUDA(c, c->node_gpu.reserve(nb));
-    if (vb) {
-        GP_CUDA(c, cudaMemcpyAsync(c->node_cpu.p, dn->avail_cpu_milli, vb, cudaMemcpyDeviceToDevice, st));
-        GP_CUDA(c, cudaMemcpyAsync(c->node_mem.p, dn->avail_mem_bytes, vb, cudaMemcpyDeviceToDevice, st));
-        if (dn->avail_gpu) GP_CUDA(c, cudaMemcpyAsync(c->node_gpu.p, dn->avail_gpu, vb, cudaMemcpyDeviceToDevice, st));
-        else GP_CUDA(c, cudaMemsetAsync(c->node_gpu.p, 0, vb, st));
-    }
-    return build_snapshot_device(c, dn, n_exec, n_drv, st);
+    return build_snapshot_device(c, dn, n_exec, n_drv, st, dn->n_nodes > 0);
 }
 
 gp_status gp_get_snapshot(gp_ctx* c, int64_t* cpu, int64_t* mem, int64_t* gpu) {
@@ -903,32 +909,33 @@ static void launch_pack(gp_ctx* c, gp_mode mode, const Snapshot& s, const PrepAp
     }
 }
 
-// independent tightly-pack / distribute-evenly: classify -> capacity tables -> thread-per-application decisions ->
-// warp-per-application scan of whatever the tables could not decide (gangpack_tables.cuh)
+// independent tightly-pack / distribute-evenly: one launch for classify -> capacity tables -> thread-per-application
+// decisions, then the warp-per-application scan of whatever the tables could not decide (gangpack_tables.cuh)
 template <int ALGO, class OUT>
-static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs, const int32_t* app_slot,
-                               PrepApp* prep, int32_t* listed, int32_t q, const DevResults& dr, int32_t lo, int2* scratch,
-                               unsigned long long* stats, unsigned int* next_app, int* d_err, volatile int* err_host, bool use_tables,
-                               cudaStream_t st, int chunk) {
-    if (use_tables) {
-        bool& attr = c->tab_attr_set[ALGO];
-        if (!attr) {
-            GP_CUDA(c, cudaFuncSetAttribute(gp_build_shape_tables<ALGO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTabSmemBytes));
-            attr = true;
-        }
-        gp_build_shape_tables<ALGO><<<dim3(2 * kMaxShapes, (unsigned)c->n_groups), kTabThreads, kTabSmemBytes, st>>>(s, tabs);
-        c->last.kernel_launches += 1;
+static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs, int64_t off_base,
+                               int64_t* off_out, int32_t* app_slot, PrepApp* prep, int32_t* listed, int32_t q, const DevResults& dr,
+                               int32_t lo, int2* scratch, unsigned long long* stats, unsigned int* next_app, int* d_err,
+                               volatile int* err_host, bool use_tables, int64_t seg_bound, cudaStream_t st) {
+    int& dec_per_sm = c->dec_ctas_per_sm[ALGO][sizeof(OUT) == 2 ? 1 : 0];
+    if (dec_per_sm == 0) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&dec_per_sm, gp_decide_tables<ALGO, OUT>, kTabThreads, 0);
+        if (dec_per_sm < 1) dec_per_sm = 1;
     }
-    if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][1], st));
-    gp_decide_tables<ALGO, OUT><<<(q + kDecideThreads - 1) / kDecideThreads, kDecideThreads, 0, st>>>(
-        s, cols, tabs, app_slot, q, dr.cap, dr.driver + lo, static_cast<OUT*>(dr.exec), prep, listed, stats, d_err, err_host, use_tables ? 0 : 1);
+    // persistent grid: as many CTAs as fit on the device, or as many as there can be work items
+    const int64_t tiles = ((int64_t)q + kTabThreads - 1) / kTabThreads;
+    const int64_t shapes = std::min<int64_t>(q, kMaxShapes);
+    int64_t blocks = tiles * ((use_tables || off_out) ? 2 : 1) + (use_tables ? shapes * (seg_bound + c->n_groups) : 0);
+    blocks = std::min<int64_t>(blocks, (int64_t)c->sm_count * dec_per_sm);
+    gp_decide_tables<ALGO, OUT><<<(int)blocks, kTabThreads, 0, st>>>(s, cols, tabs, off_base, off_out, app_slot, q, dr.cap, dr.driver + lo,
+                                                                    static_cast<OUT*>(dr.exec), prep, listed, stats, d_err, err_host,
+                                                                    use_tables ? 0 : 1);
     int& per_sm = c->tab_ctas_per_sm[ALGO][sizeof(OUT) == 2 ? 1 : 0];
     if (per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_listed<ALGO, OUT>, kPackTabThreads, 0);
         if (per_sm < 1) per_sm = 1;
     }
     // persistent grid; with the tables on the list is normally short (or empty: the CTAs leave at once)
-    int64_t blocks = ((int64_t)q * 32 + kPackTabThreads - 1) / kPackTabThreads;
+    blocks = ((int64_t)q * 32 + kPackTabThreads - 1) / kPackTabThreads;
     const int64_t max_blocks = (int64_t)c->sm_count * (use_tables ? 2 : per_sm);
     if (blocks > max_blocks) blocks = max_blocks;
     if (blocks < 1) blocks = 1;
@@ -953,58 +960,58 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
 
     if (mode == GP_MODE_INDEPENDENT && algo != GP_MINIMAL_FRAGMENTATION) {
         gp_ctx::TableSet& T = c->tabs[chunk % gp_ctx::kLanes];
-        const size_t hdr_bytes = 1024 + (sizeof(ShapeEntry) + sizeof(DriverEntry)) * (size_t)kShapeSlots;
         const bool use_tables = c->use_tables && q >= 32;
-        GP_CUDA(c, T.hdr.reserve(hdr_bytes));
-        // [executor slot | driver slot | listed | block sums of the executor counts (K0)]
-        const size_t slot_words = (3 * (size_t)q + 1) & ~(size_t)1;             // keeps the block sums 8-byte aligned
-        const size_t n_blocks = ((size_t)q + kClassifyThreads - 1) / kClassifyThreads;
-        GP_CUDA(c, T.app_slot.reserve(sizeof(int32_t) * slot_words + sizeof(unsigned long long) * (n_blocks + 1)));
-        if (use_tables) {
-            GP_CUDA(c, T.table.reserve(sizeof(uint32_t) * (size_t)kMaxShapes * (size_t)((c->n_slots + 4) & ~3)));
-            GP_CUDA(c, T.total.reserve(3 * sizeof(uint32_t) * (size_t)kMaxShapes * (size_t)c->n_groups));   // total | firstfit | first_host
-            GP_CUDA(c, T.place.reserve(sizeof(int32_t) * (size_t)kMaxShapes * (size_t)c->n_groups * kPlaceLen));
-        }
-        ShapeTables tabs;
-        tabs.hdr = T.hdr.as<ShapeHeader>();
-        tabs.entries = reinterpret_cast<ShapeEntry*>(T.hdr.as<char>() + 1024);
-        tabs.dentries = reinterpret_cast<DriverEntry*>(T.hdr.as<char>() + 1024 + sizeof(ShapeEntry) * (size_t)kShapeSlots);
-        tabs.table = T.table.as<uint32_t>(); tabs.total = T.total.as<uint32_t>();
-        tabs.firstfit = reinterpret_cast<int32_t*>(T.total.as<uint32_t>() + (size_t)kMaxShapes * (size_t)c->n_groups);
-        tabs.first_host = tabs.firstfit + (size_t)kMaxShapes * (size_t)c->n_groups;
-        tabs.place = T.place.as<int32_t>();
-        tabs.pitch = (c->n_slots + 4) & ~3; tabs.n_groups = c->n_groups;      // rows start 16-byte aligned
         int64_t* off_out = nullptr;
         if (!da.cols.off) {                       // derive the offsets on the device
             off_out = c->off_dev.as<int64_t>() + lo;
             cols.off = off_out;
         }
+        // [header | look-back words of the classify tiles | executor hash | driver hash | look-back words of the table
+        // segments]: the memset that starts the call zeroes what the call uses of it (the header always: ticket, counters)
+        const size_t n_tiles = ((size_t)q + kTabThreads - 1) / kTabThreads;
+        const size_t cls_bytes = (sizeof(unsigned long long) * n_tiles + 15) & ~(size_t)15;
+        const size_t hash_bytes = (sizeof(ShapeEntry) + sizeof(DriverEntry)) * (size_t)kShapeSlots;
+        // sum over the groups of max(1, ceil(ne / kTabSeg)) <= n_slots / kTabSeg + n_groups
+        const int64_t seg_bound = (int64_t)c->n_slots / kTabSeg + c->n_groups + 1;
+        const size_t hdr_bytes = 1024 + cls_bytes + hash_bytes + sizeof(unsigned long long) * (size_t)kMaxShapes * (size_t)seg_bound;
+        const size_t zero_bytes = use_tables ? hdr_bytes : off_out ? 1024 + cls_bytes : 1024;
+        GP_CUDA(c, T.hdr.reserve(hdr_bytes));
+        // [executor slot | driver slot | listed]
+        GP_CUDA(c, T.app_slot.reserve(sizeof(int32_t) * (3 * (size_t)q + 1)));
+        if (use_tables) {
+            GP_CUDA(c, T.table.reserve(sizeof(uint32_t) * (size_t)kMaxShapes * (size_t)((c->n_slots + 4) & ~3)));
+            // total | firstfit | first_host | segments before each group
+            GP_CUDA(c, T.total.reserve(sizeof(uint32_t) * (3 * (size_t)kMaxShapes * (size_t)c->n_groups + (size_t)c->n_groups + 1)));
+            GP_CUDA(c, T.place.reserve(sizeof(int32_t) * (size_t)kMaxShapes * (size_t)c->n_groups * kPlaceLen));
+        }
+        ShapeTables tabs;
+        tabs.hdr = T.hdr.as<ShapeHeader>();
+        tabs.cls_status = reinterpret_cast<unsigned long long*>(T.hdr.as<char>() + 1024);
+        tabs.entries = reinterpret_cast<ShapeEntry*>(T.hdr.as<char>() + 1024 + cls_bytes);
+        tabs.dentries = reinterpret_cast<DriverEntry*>(T.hdr.as<char>() + 1024 + cls_bytes + sizeof(ShapeEntry) * (size_t)kShapeSlots);
+        tabs.seg_status = reinterpret_cast<unsigned long long*>(T.hdr.as<char>() + 1024 + cls_bytes + hash_bytes);
+        tabs.table = T.table.as<uint32_t>(); tabs.total = T.total.as<uint32_t>();
+        tabs.firstfit = reinterpret_cast<int32_t*>(T.total.as<uint32_t>() + (size_t)kMaxShapes * (size_t)c->n_groups);
+        tabs.first_host = tabs.firstfit + (size_t)kMaxShapes * (size_t)c->n_groups;
+        tabs.seg_pre = tabs.first_host + (size_t)kMaxShapes * (size_t)c->n_groups;
+        tabs.place = T.place.as<int32_t>();
+        tabs.pitch = (c->n_slots + 4) & ~3; tabs.n_groups = c->n_groups;      // rows start 16-byte aligned
         int32_t* app_slot = T.app_slot.as<int32_t>();
         int32_t* listed = app_slot + 2 * (size_t)q;
         PrepApp* prep = c->prep.as<PrepApp>() + lo;
         const bool o16 = dr.node_bits == 16;
         auto issue = [&](int& launches) -> gp_status {
             const int before = (int)c->last.kernel_launches;
-            // the hash tables and the header (listed counter) start from zero: the whole block when the tables are used
-            GP_CUDA(c, cudaMemsetAsync(T.hdr.p, 0, use_tables ? hdr_bytes : 1024, st));
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][0], st));
-            if (use_tables || off_out) {
-                unsigned long long* block_sums = reinterpret_cast<unsigned long long*>(app_slot + slot_words);
-                if (off_out) {
-                    gp_count_blocks<<<(unsigned)n_blocks, kClassifyThreads, 0, st>>>(q, cols.count, block_sums);
-                    c->last.kernel_launches += 1;
-                }
-                gp_classify_apps<<<(unsigned)n_blocks, kClassifyThreads, 0, st>>>(
-                    q, cols, tabs, c->snap_flags.as<SnapMeta>(), off_base, off_out, block_sums, app_slot, use_tables ? 1 : 0);
-                c->last.kernel_launches += 1;
-            }
+            GP_CUDA(c, cudaMemsetAsync(T.hdr.p, 0, zero_bytes, st));
+            if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][1], st));
             gp_status r;
             if (algo == GP_TIGHTLY_PACK)
-                r = o16 ? launch_tables<0, uint16_t>(c, s, cols, tabs, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, st, chunk)
-                        : launch_tables<0, int32_t>(c, s, cols, tabs, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, st, chunk);
+                r = o16 ? launch_tables<0, uint16_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st)
+                        : launch_tables<0, int32_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st);
             else
-                r = o16 ? launch_tables<1, uint16_t>(c, s, cols, tabs, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, st, chunk)
-                        : launch_tables<1, int32_t>(c, s, cols, tabs, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, st, chunk);
+                r = o16 ? launch_tables<1, uint16_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st)
+                        : launch_tables<1, int32_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st);
             if (r != GP_OK) return r;
             GP_CUDA(c, cudaGetLastError());
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][2], st));

@@ -10,26 +10,27 @@
 // Why tables.  Every application of an independent batch is packed against the SAME snapshot
 // (internal/extender/unschedulablepods.go:132-166; each Predicate's own pack, resource.go:321), and a node's executor
 // capacity depends only on the executor request -- the "shape" (cpu, mem, gpu).  Real queues hold few shapes (the
-// synthetic one: 12).  So instead of every application re-scanning the node order, each distinct shape is scanned ONCE:
-//   K1 gp_classify_apps   thread per application: intern its shape in a small hash table (atomicCAS on a 64-bit
+// synthetic one: 12).  So instead of every application re-scanning the node order, each distinct shape is scanned ONCE.
+// The three dependent phases run in ONE persistent launch, gp_decide_tables, as ticket-ordered work items (see there):
+//   1 gp_classify_apps    thread per application: intern its shape in a small hash table (atomicCAS on a 64-bit
 //                         fingerprint; the full tuple is verified again by the consumer, so a fingerprint collision costs
-//                         a fallback, never a wrong answer) and derive the ExecutorNodes offsets when the caller gave none;
-//   K2 gp_build_shape_tables  one CTA per (shape, instance group): the group's (cpu, mem) slots are staged tile by tile
-//                         into shared memory by TMA bulk copies (cp.async.bulk + mbarrier, double-buffered), every
-//                         thread evaluates 4 consecutive nodes, a block-wide exclusive scan turns capacities into the
-//                         prefix table  S[i] = sum_{n<i} min(cap(n|0), CLAMP)   (tightly-pack) or
+//                         a fallback, never a wrong answer) and derive the ExecutorNodes offsets when the caller gave none
+//                         (decoupled look-back over the tiles);
+//   2 gp_build_shape_tables  one item per kTabSeg-node segment of one (shape, instance group): every thread evaluates 4
+//                         consecutive nodes, a block-wide scan plus a look-back over the earlier segments of the same
+//                         (shape, group) turns capacities into the prefix table
+//                                       S[i] = sum_{n<i} min(cap(n|0), CLAMP)   (tightly-pack) or
 //                                       M[i] = #{n<i : cap(n|0) >= 1}            (distribute-evenly),
 //                         and the first kPlaceLen entries of the driver-free placement P[t] = node of the t-th executor;
-//       (same launch, second half of the grid: one CTA per (driver shape, instance group) finds the first driver candidate
-//       the shape fits on);
-//   K3 gp_decide_tables   ONE THREAD per application (with the tables a decision is O(log N + k) scalar work -- a warp per
+//                         one item per (driver shape, instance group) finds the first driver candidate the shape fits on;
+//   3 decide              ONE THREAD per application (with the tables a decision is O(log N + k) scalar work -- a warp per
 //                         application, right for an O(N) scan, would idle 31 lanes): feasibility is
 //                         S[ne] - delta(d) >= k  per driver candidate d starting at the shape's first fit (delta = what the
 //                         driver displaces on its own node: O(1) per candidate, the reference's loop binpack.go:67-85
 //                         verbatim).  ExecutorNodes is P shifted by delta past the driver's run, written by the whole warp
 //                         with coalesced stores, when its largest index k - 1 + delta is below kPlaceLen; otherwise it is
 //                         emitted by walking the table from the shape's first hosting node (one word per (shape, group),
-//                         written by K2) with the next word always in flight (zero-capacity runs are jumped by a galloping
+//                         written by phase 2) with the next word always in flight (zero-capacity runs are jumped by a galloping
 //                         search).
 // What the tables cannot answer exactly -- more than kMaxShapes distinct shapes in a batch, executor counts above the table
 // clamp, distribute-evenly placements that need more than one round -- is appended, already prepared (PrepApp), to a list
@@ -38,16 +39,15 @@
 #pragma once
 
 #include "gangpack_kernels.cuh"
-#include "gangpack_fifo.cuh"     // TMA / mbarrier helpers
 
 namespace gp {
 
 constexpr int kShapeSlots = 1024;     // hash slots (power of two)
 constexpr int kShapeProbes = 16;      // linear probes before giving up (-> scan path)
 constexpr int kMaxShapes = 64;        // dense tables per batch
-constexpr int kTabThreads = 1024;
+constexpr int kTabThreads = 256;      // every phase of gp_decide_tables; also the applications per classify tile
 constexpr int kTabPerThread = 4;
-constexpr int kTabTile = kTabThreads * kTabPerThread;     // 4096 nodes per tile: 64 KB of (cpu, mem)
+constexpr int kTabSeg = kTabThreads * kTabPerThread;      // nodes per table segment
 constexpr int kPlaceLen = 256;        // placement prefix per (shape, group): covers every count <= 128 whatever the driver takes
 
 struct __align__(16) ShapeEntry {     // 96 bytes
@@ -75,6 +75,10 @@ struct ShapeHeader {
     int32_t pad;
     int32_t id_slot[kMaxShapes];      // dense executor-shape id -> hash slot
     int32_t did_slot[kMaxShapes];     // dense driver-shape id -> hash slot
+    uint32_t ticket;                  // next work item of gp_decide_tables
+    uint32_t cls_done;                // classify tiles finished
+    uint32_t tab_done;                // table items finished
+    uint32_t dec_next;                // next 32-application chunk of the decide phase
 };
 static_assert(sizeof(ShapeHeader) <= 1024, "ShapeHeader");
 
@@ -82,6 +86,9 @@ struct ShapeTables {
     ShapeEntry* entries;              // [kShapeSlots]
     DriverEntry* dentries;            // [kShapeSlots]
     ShapeHeader* hdr;
+    unsigned long long* cls_status;   // [classify tiles] look-back words of the derived offsets (zeroed with the header)
+    unsigned long long* seg_status;   // [kMaxShapes * segments] look-back words of the table segments (zeroed with the header)
+    int32_t* seg_pre;                 // [n_groups + 1] table segments before each group (written by classify tile 0)
     uint32_t* table;                  // [kMaxShapes][pitch] exclusive prefix per instance group, indexed by slot
     uint32_t* total;                  // [kMaxShapes][n_groups]
     int32_t* firstfit;                // [kMaxShapes][n_groups] first driver-order position the driver shape fits on (nd: none)
@@ -126,31 +133,64 @@ struct AppColumns {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// K1: intern executor shapes, derive offsets
+// cross-CTA signalling inside the one launch
 // ---------------------------------------------------------------------------------------------------------------
-constexpr int kClassifyThreads = 256;
-
-// K0: executor counts per block of kClassifyThreads applications (the offsets K1 derives are an exclusive prefix sum: every
-// CTA of K1 adds up the <= n/256 block sums before its own block instead of re-reading every count before it -- the
-// redundant form moved q^2/512 words through L2)
-__global__ void __launch_bounds__(kClassifyThreads) gp_count_blocks(int32_t n_apps, const int32_t* __restrict__ count,
-                                                                    unsigned long long* __restrict__ block_sums) {
-    __shared__ unsigned long long s_part[kClassifyThreads / 32];
-    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const int32_t c = i < n_apps ? count[i] : 0;
-    unsigned long long v = c > 0 ? (unsigned long long)c : 0ull;
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) v += __shfl_xor_sync(kFull, v, d);
-    if (lane == 0) s_part[w] = v;
+__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long* p) {
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
+    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+// thread 0 of a CTA: wait until *ctr >= n (acquire: the producers' writes are visible to the whole CTA after the
+// __syncthreads that follows)
+__device__ __forceinline__ void wait_count(const uint32_t* ctr, uint32_t n) {
+    unsigned ns = 32;
+    while (ld_acquire_u32(ctr) < n) { __nanosleep(ns); if (ns < 1024) ns <<= 1; }
+    __threadfence();
+}
+// whole CTA after writing an item's output: count it done (release)
+__device__ __forceinline__ void signal_done(uint32_t* ctr) {
     __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-        for (int k = 0; k < kClassifyThreads / 32; ++k) t += s_part[k];
-        block_sums[blockIdx.x] = t;
+    if (threadIdx.x == 0) { __threadfence(); atomicAdd(ctr, 1u); }
+}
+
+// Look-back status word of a scanned item (classify tile, table segment): flag in bits 62-63, value below.
+constexpr unsigned long long kStAggregate = 1ull << 62;     // the item's own sum is published
+constexpr unsigned long long kStInclusive = 2ull << 62;     // the sum of every item of the chain up to and including it
+constexpr unsigned long long kStValue = (1ull << 62) - 1;
+
+// Decoupled look-back (Merrill & Garland 2016), called by one whole warp: the exclusive prefix of item `idx` of the chain
+// of status words [first, idx), idx > first.  Item `first` always publishes an inclusive word, so the walk ends there.
+// Every item it waits for has a smaller ticket (see gp_decide_tables).
+__device__ __forceinline__ unsigned long long lookback(const unsigned long long* status, int32_t first, int32_t idx, int lane) {
+    unsigned long long excl = 0;
+    for (int32_t end = idx;; end -= 32) {
+        const int32_t j = end - 1 - lane;                   // lane 0: the nearest predecessor
+        unsigned long long v = kStInclusive;                // before the chain: an inclusive 0
+        if (j >= first) {
+            unsigned ns = 32;
+            while (((v = ld_relaxed_u64(status + j)) >> 62) == 0) { __nanosleep(ns); if (ns < 512) ns <<= 1; }
+        }
+        const unsigned inc = __ballot_sync(kFull, (v >> 62) == 2);
+        const int stop = inc ? __ffs(inc) - 1 : 31;         // nearest inclusive word: nothing beyond it is needed
+        unsigned long long add = lane <= stop ? (v & kStValue) : 0ull;
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) add += __shfl_xor_sync(kFull, add, d);
+        excl += add;
+        if (inc) return excl;
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// phase 1 (classify): intern executor and driver shapes, derive offsets -- one tile of kTabThreads applications
+// ---------------------------------------------------------------------------------------------------------------
 // intern one request tuple (fingerprint fp) into the open-addressing table of ENTRY records; returns the slot or -1.
 // `init(entry, slot)` fills a freshly claimed entry.  Called by ONE lane per distinct fingerprint of a warp.
 template <class ENTRY, class INIT>
@@ -170,39 +210,56 @@ __device__ __forceinline__ int32_t intern_shape(ENTRY* table, unsigned long long
     return -1;
 }
 
-__global__ void __launch_bounds__(kClassifyThreads) gp_classify_apps(int32_t n_apps, AppColumns cols, ShapeTables tabs,
-                                                                     const SnapMeta* __restrict__ meta,
-                                                                     int64_t off_base, int64_t* __restrict__ off_out /* or NULL */,
-                                                                     const unsigned long long* __restrict__ block_sums /* with off_out */,
-                                                                     int32_t* __restrict__ app_slot, int use_tables) {
-    __shared__ unsigned long long s_part[kClassifyThreads / 32];
-    const int32_t block0 = blockIdx.x * blockDim.x;
-    const int32_t i = block0 + threadIdx.x;
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+struct OneScratch {
+    unsigned long long part[kTabThreads / 32];
+    unsigned long long base;
+    uint32_t ticket;
+    int32_t first_host;
+};
 
-    // ---- ExecutorNodes offsets = exclusive prefix sum of max(count, 0), when the caller passed none: the block sums of
-    // K0 before this block + a block-wide scan of this block's counts (no inter-CTA dependency inside this launch)
-    if (off_out) {
-        unsigned long long before = 0;
-        for (int32_t t = threadIdx.x; t < (int32_t)blockIdx.x; t += blockDim.x) before += block_sums[t];
-        const int32_t mine = (i < n_apps) ? max(cols.count[i], 0) : 0;
-        unsigned long long wb = before;
+// ExecutorNodes offsets = exclusive prefix sum of max(count, 0), when the caller passed none: a block scan of the tile +
+// the sum of every tile before it, by look-back over the tiles in ticket order
+__device__ __forceinline__ void classify_offsets(OneScratch& sh, int32_t tile, int32_t n_apps, const AppColumns& cols,
+                                                 const ShapeTables& tabs, int64_t off_base, int64_t* off_out) {
+    const int32_t i = tile * kTabThreads + (int32_t)threadIdx.x;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int32_t mine = (i < n_apps) ? max(cols.count[i], 0) : 0;
+    const uint32_t incl = warp_incl_scan((uint32_t)mine, lane);
+    unsigned long long wsum = (unsigned long long)mine;
 #pragma unroll
-        for (int d = 16; d >= 1; d >>= 1) wb += __shfl_xor_sync(kFull, wb, d);
-        uint32_t incl = warp_incl_scan((uint32_t)mine, lane);
-        __shared__ unsigned long long s_before[kClassifyThreads / 32];
-        if (lane == 31) s_part[w] = incl;
-        if (lane == 0) s_before[w] = wb;
-        __syncthreads();
-        unsigned long long base = (unsigned long long)off_base, prev = 0;
-        for (int t = 0; t < kClassifyThreads / 32; ++t) { base += s_before[t]; if (t < w) prev += s_part[t]; }
-        if (i < n_apps) off_out[i] = (int64_t)(base + prev + incl - (uint32_t)mine);
-        if (i == n_apps - 1) off_out[n_apps] = (int64_t)(base + prev + incl);
-        __syncthreads();
+    for (int d = 16; d >= 1; d >>= 1) wsum += __shfl_xor_sync(kFull, wsum, d);
+    if (lane == 31) sh.part[w] = incl;
+    __shared__ unsigned long long s_wsum[kTabThreads / 32];
+    if (lane == 0) s_wsum[w] = wsum;
+    __syncthreads();
+    if (w == 0) {
+        unsigned long long agg = lane < kTabThreads / 32 ? s_wsum[lane] : 0ull;
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) agg += __shfl_xor_sync(kFull, agg, d);
+        unsigned long long excl = 0;
+        if (tile == 0) {
+            if (lane == 0) st_relaxed_u64(tabs.cls_status, kStInclusive | agg);
+        } else {
+            if (lane == 0) st_relaxed_u64(tabs.cls_status + tile, kStAggregate | agg);
+            excl = lookback(tabs.cls_status, 0, tile, lane);
+            if (lane == 0) st_relaxed_u64(tabs.cls_status + tile, kStInclusive | ((excl + agg) & kStValue));
+        }
+        if (lane == 0) sh.base = excl;
     }
-    const unsigned act = __ballot_sync(kFull, i < n_apps);     // the lanes that intern (the whole warp except in the last block)
+    __syncthreads();
+    unsigned long long base = (unsigned long long)off_base + sh.base, prev = 0;
+    for (int t = 0; t < w; ++t) prev += sh.part[t];
+    if (i < n_apps) off_out[i] = (int64_t)(base + prev + incl - (uint32_t)mine);
+    if (i == n_apps - 1) off_out[n_apps] = (int64_t)(base + prev + incl);
+}
+
+// per thread: today's gp_classify_apps body
+__device__ __forceinline__ void gp_classify_apps(int32_t tile, int32_t n_apps, const AppColumns& cols, const ShapeTables& tabs,
+                                                 const SnapMeta* meta, int32_t* app_slot) {
+    const int32_t i = tile * kTabThreads + (int32_t)threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    const unsigned act = __ballot_sync(kFull, i < n_apps);     // the lanes that intern (the whole warp except in the last tile)
     if (i >= n_apps) return;
-    if (!use_tables) { app_slot[i] = -1; return; }
 
     // A queue has few distinct requests: the lanes of a warp that carry the same fingerprint elect ONE of them to probe /
     // claim the entry (100 000 threads doing their own CAS on a dozen lines serialise on those lines); the consumer
@@ -230,7 +287,7 @@ __global__ void __launch_bounds__(kClassifyThreads) gp_classify_apps(int32_t n_a
         app_slot[i] = __shfl_sync(act, found, leader);
     }
 
-    // ---- the driver request, interned the same way: its first fitting candidate is searched once per shape (K2d) ----
+    // ---- the driver request, interned the same way: its first fitting candidate is searched once per shape ----------
     const int64_t d0 = cols.load(0, i), d1 = cols.load(1, i), d2 = cols.load(2, i);
     const bool d_ok = d0 >= 0 && d1 >= 0 && d2 >= 0 && d0 < kMaxQuantity && d1 < kMaxQuantity && d2 < kMaxQuantity;
     const unsigned long long dfp = d_ok ? shape_fingerprint(d0 ^ 0x5bd1e995, d1, d2) : 0ull;
@@ -250,29 +307,38 @@ __global__ void __launch_bounds__(kClassifyThreads) gp_classify_apps(int32_t n_a
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// K2: capacity prefix tables, one CTA per (shape, instance group)
-// ---------------------------------------------------------------------------------------------------------------
-struct TabScratch {
-    unsigned long long bar[2];
-    uint32_t part[2][kTabThreads / 32];
-    int32_t first_host;
-};
-constexpr size_t kTabSmemBytes = 1024 + 2 * (size_t)kTabTile * sizeof(longlong2);      // 1 KB scratch + 2 x 64 KB tiles
+// seg_pre[g] = table segments of the groups before g (max(1, ceil(ne / kTabSeg)) each: an empty group still has the one
+// segment that writes its total and first_host); seg_pre[n_groups] = all of them
+__device__ __forceinline__ void segment_prefix(OneScratch& sh, const Snapshot& s, int32_t* seg_pre) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t carry = 0;
+    __syncthreads();            // sh.part may still be read by classify_offsets
+    for (int32_t g0 = 0; g0 < s.n_groups; g0 += kTabThreads) {
+        const int32_t g = g0 + (int32_t)threadIdx.x;
+        const uint32_t n = g < s.n_groups ? (uint32_t)max(1, (s.groups[g].ne + kTabSeg - 1) / kTabSeg) : 0u;
+        const uint32_t incl = warp_incl_scan(n, lane);
+        if (lane == 31) sh.part[w] = incl;
+        __syncthreads();
+        uint32_t before = carry, all = carry;
+        for (int t = 0; t < kTabThreads / 32; ++t) { if (t < w) before += (uint32_t)sh.part[t]; all += (uint32_t)sh.part[t]; }
+        if (g < s.n_groups) seg_pre[g] = (int32_t)(before + incl - n);
+        carry = all;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) seg_pre[s.n_groups] = (int32_t)carry;
+}
 
-__device__ __forceinline__ void driver_firstfit_block(const Snapshot& s, const ShapeTables& tabs, int id, int grp);
-
-// grid (2 * kMaxShapes, n_groups): blocks [0, kMaxShapes) build the capacity table of executor shape blockIdx.x, blocks
-// [kMaxShapes, 2 kMaxShapes) find the first fitting candidate of driver shape blockIdx.x - kMaxShapes (one launch for both)
+// ---------------------------------------------------------------------------------------------------------------
+// phase 2 (tables): capacity prefix of one segment of one (shape, instance group)
+// ---------------------------------------------------------------------------------------------------------------
+// Segment `seg` of `n_seg` covers executor-order positions [seg * kTabSeg, min(+kTabSeg, ne)) of group `grp`; every
+// thread evaluates kTabPerThread consecutive nodes.  `st` is the segment's look-back status word; the chain of the
+// (shape, group) is st - seg .. st - seg + n_seg - 1.  Together the segments write
+//     S[i] = sum_{n<i} min(cap(n|0), CLAMP)   (tightly-pack) or   M[i] = #{n<i : cap(n|0) >= 1}   (distribute-evenly),
+// total = S[ne], first_host (first position with capacity, ne: none) and the placement prefix P[t < min(total, kPlaceLen)].
 template <int ALGO>
-__global__ void __launch_bounds__(kTabThreads, 1) gp_build_shape_tables(Snapshot s, ShapeTables tabs) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    if (blockIdx.x >= kMaxShapes) { driver_firstfit_block(s, tabs, (int)blockIdx.x - kMaxShapes, (int)blockIdx.y); return; }
-    TabScratch& sh = *reinterpret_cast<TabScratch*>(smem_raw);
-    longlong2* tile[2] = {reinterpret_cast<longlong2*>(smem_raw + 1024), reinterpret_cast<longlong2*>(smem_raw + 1024) + kTabTile};
-    const int id = blockIdx.x, grp = blockIdx.y;
-    const int n_shapes = min(tabs.hdr->n_shapes, kMaxShapes);
-    if (id >= n_shapes) return;
+__device__ __forceinline__ void gp_build_shape_tables(OneScratch& sh, const Snapshot& s, const ShapeTables& tabs, int id, int grp,
+                                                      int32_t seg, int32_t n_seg, unsigned long long* st) {
     const ShapeEntry& en = tabs.entries[tabs.hdr->id_slot[id]];
     const DimDiv dc = en.div[0], dm = en.div[1], dg = en.div[2];
     const bool ug = (en.flags & 1u) || (s.meta->flags & kSnapGpuNegative);
@@ -285,94 +351,84 @@ __global__ void __launch_bounds__(kTabThreads, 1) gp_build_shape_tables(Snapshot
     uint32_t* out = tabs.table + (size_t)id * tabs.pitch + g.sbase;
     int32_t* place = tabs.place + ((size_t)id * tabs.n_groups + grp) * kPlaceLen;
 
-    if (tid == 0) { mbar_init(&sh.bar[0], 1); mbar_init(&sh.bar[1], 1); sh.first_host = ne; }
-    __syncthreads();
-    const int n_tiles = (ne + kTabTile - 1) / kTabTile;
-    auto issue = [&](int t) {          // thread 0: TMA bulk copies of tile t into buffer t & 1 (<= 32 KB per copy)
-        const int32_t lo = t * kTabTile;
-        const uint32_t bytes = (uint32_t)min(kTabTile, ne - lo) * (uint32_t)sizeof(longlong2);
-        mbar_expect_tx(&sh.bar[t & 1], bytes);
-        for (uint32_t off = 0; off < bytes; off += 32768u) {
-            const uint32_t n = bytes - off < 32768u ? bytes - off : 32768u;
-            tma_load_1d(reinterpret_cast<unsigned char*>(tile[t & 1]) + off, reinterpret_cast<const unsigned char*>(gpair + lo) + off, n,
-                        &sh.bar[t & 1]);
+    const int32_t i0 = seg * kTabSeg + tid * kTabPerThread;
+    uint32_t v[kTabPerThread];
+    uint32_t sum = 0;
+    int32_t my_first = 0x7fffffff;
+#pragma unroll
+    for (int j = 0; j < kTabPerThread; ++j) {
+        const int32_t i = i0 + j;
+        uint32_t c = 0;
+        if (i < ne) {
+            const longlong2 a = __ldg(gpair + i);
+            c = min(cap_dim(a.x, dc, clamp), cap_dim(a.y, dm, clamp));
+            if (ug) c = min(c, cap_dim(__ldg(ggpu + i), dg, clamp));
+            if (ALGO == 1) c = c != 0 ? 1u : 0u;
         }
-    };
-    if (tid == 0 && n_tiles > 0) issue(0);
-    uint32_t carry = 0;
-    for (int t = 0; t < n_tiles; ++t) {
-        if (tid == 0 && t + 1 < n_tiles) issue(t + 1);           // buffer (t+1)&1 was released by the barrier that ended tile t-1
-        mbar_wait(&sh.bar[t & 1], (uint32_t)((t >> 1) & 1));
-        const longlong2* tp = tile[t & 1];
-        const int32_t lo = t * kTabTile;
-        const int32_t i0 = lo + tid * kTabPerThread;
-        uint32_t v[kTabPerThread];
-        uint32_t sum = 0;
-        int32_t my_first = 0x7fffffff;
+        if (c != 0 && i < my_first) my_first = i;
+        v[j] = sum;             // exclusive within the thread
+        sum += c;
+    }
+    // block-wide exclusive scan of the per-thread sums, and the segment's first hosting node
+    if (tid == 0) sh.first_host = 0x7fffffff;
+    const uint32_t incl = warp_incl_scan(sum, lane);
+    if (lane == 31) sh.part[w] = incl;
+    __syncthreads();
+    {
+        const uint32_t wmin = __reduce_min_sync(kFull, (uint32_t)my_first);
+        if (lane == 0 && wmin != 0x7fffffffu) atomicMin(&sh.first_host, (int32_t)wmin);
+    }
+    uint32_t before = 0, seg_total = 0;
+    for (int t = 0; t < kTabThreads / 32; ++t) { if (t < w) before += (uint32_t)sh.part[t]; seg_total += (uint32_t)sh.part[t]; }
+    if (w == 0) {               // the segment's base: the sum of the segments before it in the same (shape, group)
+        unsigned long long base = 0;
+        if (seg == 0) {
+            if (lane == 0) st_relaxed_u64(st, kStInclusive | seg_total);
+        } else {
+            if (lane == 0) st_relaxed_u64(st, kStAggregate | seg_total);
+            base = lookback(st - seg, 0, seg, lane);
+            if (lane == 0) st_relaxed_u64(st, kStInclusive | (base + seg_total));
+        }
+        if (lane == 0) sh.base = base;
+    }
+    __syncthreads();
+    const uint32_t seg_base = (uint32_t)sh.base;
+    const uint32_t base = seg_base + before + incl - sum;
+    if (i0 + kTabPerThread <= ne && ((g.sbase + i0) & 3) == 0) {
+        *reinterpret_cast<uint4*>(out + i0) = make_uint4(base + v[0], base + v[1], base + v[2], base + v[3]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < kTabPerThread; ++j) if (i0 + j < ne) out[i0 + j] = base + v[j];
+    }
+    // placement prefix: a node whose first executor index is below kPlaceLen writes its run [S, min(S + c, kPlaceLen))
+    // (the (shape, group) writes at most kPlaceLen words in all; only the first hosting nodes of the order do anything)
+    if (base < (uint32_t)kPlaceLen) {
 #pragma unroll
         for (int j = 0; j < kTabPerThread; ++j) {
-            const int32_t i = i0 + j;
-            uint32_t c = 0;
-            if (i < ne) {
-                const longlong2 a = tp[i - lo];
-                c = min(cap_dim(a.x, dc, clamp), cap_dim(a.y, dm, clamp));
-                if (ug) c = min(c, cap_dim(__ldg(ggpu + i), dg, clamp));
-                if (ALGO == 1) c = c != 0 ? 1u : 0u;
-            }
-            if (c != 0 && i < my_first) my_first = i;
-            v[j] = sum;             // exclusive within the thread
-            sum += c;
-        }
-        // the first hosting node of the shape: every decision of the shape starts its walk there (no search per application)
-        {
-            const uint32_t wmin = __reduce_min_sync(kFull, (uint32_t)my_first);
-            if (lane == 0 && wmin != 0x7fffffffu) atomicMin(&sh.first_host, (int32_t)wmin);
-        }
-        // block-wide exclusive scan of the per-thread sums
-        const uint32_t incl = warp_incl_scan(sum, lane);
-        if (lane == 31) sh.part[t & 1][w] = incl;
-        __syncthreads();            // also: every thread is done reading tile[t & 1]... of the PREVIOUS use (see issue())
-        const uint32_t pt = sh.part[t & 1][lane];
-        const uint32_t pti = warp_incl_scan(pt, lane);
-        const uint32_t before = __shfl_sync(kFull, pti - pt, w);
-        const uint32_t tile_total = __shfl_sync(kFull, pti, 31);
-        const uint32_t base = carry + before + incl - sum;
-        if (i0 + kTabPerThread <= ne && ((g.sbase + i0) & 3) == 0) {
-            *reinterpret_cast<uint4*>(out + i0) = make_uint4(base + v[0], base + v[1], base + v[2], base + v[3]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < kTabPerThread; ++j) if (i0 + j < ne) out[i0 + j] = base + v[j];
-        }
-        // placement prefix: a node whose first executor index is below kPlaceLen writes its run [S, min(S + c, kPlaceLen))
-        // (the CTA writes at most kPlaceLen words in all; only the first hosting nodes of the order do anything)
-        if (base < (uint32_t)kPlaceLen) {
-#pragma unroll
-            for (int j = 0; j < kTabPerThread; ++j) {
-                const uint32_t p0 = base + v[j];
-                const uint32_t p1 = base + (j + 1 < kTabPerThread ? v[j + 1] : sum);
-                if (p0 < p1 && p0 < (uint32_t)kPlaceLen) {
-                    const int32_t node = __ldg(s.slot_node + g.sbase + i0 + j);
-                    const uint32_t end = p1 < (uint32_t)kPlaceLen ? p1 : (uint32_t)kPlaceLen;
-                    for (uint32_t t = p0; t < end; ++t) place[t] = node;
-                }
+            const uint32_t p0 = base + v[j];
+            const uint32_t p1 = base + (j + 1 < kTabPerThread ? v[j + 1] : sum);
+            if (p0 < p1 && p0 < (uint32_t)kPlaceLen) {
+                const int32_t node = __ldg(s.slot_node + g.sbase + i0 + j);
+                const uint32_t end = p1 < (uint32_t)kPlaceLen ? p1 : (uint32_t)kPlaceLen;
+                for (uint32_t t = p0; t < end; ++t) place[t] = node;
             }
         }
-        carry += tile_total;
-        __syncthreads();            // tile[t & 1] and part[t & 1] may be overwritten from here on
     }
+    // first_host: the one segment with nothing before it and something in it (or the last one, when the group hosts none);
+    // total: the last segment
     if (tid == 0) {
-        tabs.total[(size_t)id * tabs.n_groups + grp] = carry;
-        tabs.first_host[(size_t)id * tabs.n_groups + grp] = sh.first_host;     // ordered by the barrier that ended the last tile
+        const size_t at = (size_t)id * tabs.n_groups + grp;
+        if (seg_base == 0 && seg_total != 0) tabs.first_host[at] = sh.first_host;
+        if (seg == n_seg - 1) {
+            tabs.total[at] = seg_base + seg_total;
+            if (seg_base + seg_total == 0) tabs.first_host[at] = ne;
+        }
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// K2d: first fitting driver candidate per (driver shape, instance group)
-// ---------------------------------------------------------------------------------------------------------------
+// phase 2 (tables): first fitting driver candidate per (driver shape, instance group)
 __device__ __forceinline__ void driver_firstfit_block(const Snapshot& s, const ShapeTables& tabs, int id, int grp) {
     __shared__ int32_t s_first;
-    const int n = min(tabs.hdr->n_dshapes, kMaxShapes);
-    if (id >= n) return;
     const DriverEntry& en = tabs.dentries[tabs.hdr->did_slot[id]];
     const int64_t d0 = en.d[0], d1 = en.d[1], d2 = en.d[2];
     const GroupDesc g = s.groups[grp];
@@ -381,15 +437,26 @@ __device__ __forceinline__ void driver_firstfit_block(const Snapshot& s, const S
     const int64_t* ggpu = s.gpu + g.sbase;
     if (threadIdx.x == 0) s_first = g.nd;
     __syncthreads();
-    for (int32_t j0 = 0; j0 < g.nd; j0 += blockDim.x) {
-        const int32_t j = j0 + threadIdx.x;
-        bool fits = false;
-        if (j < g.nd) {
-            const int32_t ls = s.drv_slot[g.dbase + j];
-            const longlong2 v = __ldg(gpair + ls);
-            fits = !(d0 > v.x) && !(d1 > v.y) && !(ug && d2 > __ldg(ggpu + ls));     // driverResources.GreaterThan(available) == false
+    // kFitPerThread independent candidates per thread and step: a shape that fits late walks the order in few dependent
+    // load round trips
+    constexpr int kFitPerThread = 8;
+    for (int32_t j0 = 0; j0 < g.nd; j0 += kFitPerThread * kTabThreads) {
+        int32_t ls[kFitPerThread];
+#pragma unroll
+        for (int u = 0; u < kFitPerThread; ++u) {
+            const int32_t j = j0 + u * kTabThreads + (int32_t)threadIdx.x;
+            ls[u] = j < g.nd ? s.drv_slot[g.dbase + j] : -1;
         }
-        if (fits) atomicMin(&s_first, j);
+        int32_t mine = 0x7fffffff;
+#pragma unroll
+        for (int u = 0; u < kFitPerThread; ++u) {
+            if (ls[u] < 0) continue;
+            const longlong2 v = __ldg(gpair + ls[u]);
+            // driverResources.GreaterThan(available) == false
+            const bool fits = !(d0 > v.x) && !(d1 > v.y) && !(ug && d2 > __ldg(ggpu + ls[u]));
+            if (fits && mine == 0x7fffffff) mine = j0 + u * kTabThreads + (int32_t)threadIdx.x;
+        }
+        if (mine != 0x7fffffff) atomicMin(&s_first, mine);
         __syncthreads();
         if (s_first < g.nd) break;               // block-uniform
     }
@@ -397,14 +464,16 @@ __device__ __forceinline__ void driver_firstfit_block(const Snapshot& s, const S
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// K3: one thread per application
+// phase 3 (decide): one thread per application
 // ---------------------------------------------------------------------------------------------------------------
+// The tables are written earlier in the same launch: every load of them below is an ordinary (coherent) load, never the
+// read-only path.
 // prefix value S(i), i in [0, ne]
-__device__ __forceinline__ uint32_t tab_at(const uint32_t* __restrict__ tab, int32_t i, int32_t ne, uint32_t total) {
-    return i < ne ? __ldg(tab + i) : total;
+__device__ __forceinline__ uint32_t tab_at(const uint32_t* tab, int32_t i, int32_t ne, uint32_t total) {
+    return i < ne ? tab[i] : total;
 }
 // smallest p in (lo, ne] with S(p) > val; requires S(ne) = total > val
-__device__ __forceinline__ int32_t tab_next_above(const uint32_t* __restrict__ tab, int32_t lo, int32_t ne, uint32_t total, uint32_t val,
+__device__ __forceinline__ int32_t tab_next_above(const uint32_t* tab, int32_t lo, int32_t ne, uint32_t total, uint32_t val,
                                                   unsigned long long& probes) {
     int32_t a = lo + 1, b = ne;                     // answer in [a, b], S(b) > val
     // gallop first: the zero-capacity runs inside a walk are short (1-2 probes instead of log2(ne))
@@ -424,19 +493,16 @@ __device__ __forceinline__ int32_t tab_next_above(const uint32_t* __restrict__ t
     return a;
 }
 
-constexpr int kDecideThreads = 128;
-// cols: raw application columns; app_slot: [2][n_apps] executor / driver shape slots from K1.  Applications the tables
-// cannot decide are prepared (PrepApp) and appended to `listed`; force_scan appends every application.
+// cols: raw application columns; app_slot: [2][n_apps] executor / driver shape slots from phase 1.  Applications the
+// tables cannot decide are prepared (PrepApp) and appended to `listed`; force_scan appends every application.
 template <int ALGO, class OUT>
-__global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, AppColumns cols, ShapeTables tabs,
-                                                                   const int32_t* __restrict__ app_slot, int32_t n_apps, int64_t out_cap,
-                                                                   int32_t* __restrict__ driver_node, OUT* __restrict__ executor_nodes,
-                                                                   PrepApp* __restrict__ prep, int32_t* __restrict__ listed,
-                                                                   unsigned long long* __restrict__ stats, int* __restrict__ err,
-                                                                   volatile int* __restrict__ err_host, int force_scan) {
-    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs,
+                                            const int32_t* app_slot, int32_t n_apps, int64_t out_cap,
+                                            int32_t* __restrict__ driver_node, OUT* __restrict__ executor_nodes,
+                                            PrepApp* __restrict__ prep, int32_t* __restrict__ listed, int* __restrict__ err,
+                                            volatile int* __restrict__ err_host, int force_scan,
+                                            unsigned long long& probes, unsigned long long& drivers) {
     const int lane = threadIdx.x & 31;
-    unsigned long long probes = 0, drivers = 0;
     // this lane's share of the warp's coalesced emission (sh_k = 0: none): out[sh_dst + t] = place[sh_src + shifted t]
     uint32_t sh_k = 0, sh_cut = 0, sh_delta = 0;
     int64_t sh_dst = 0, sh_src = 0;
@@ -506,7 +572,7 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
                     if ((d_cpu > v.x) || (d_mem > v.y) || (drv_gpu && d_gpu > gv)) continue;
                     uint32_t my_c0 = 0, my_cd = 0, sp = 0;
                     if (ls < ne && k != 0) {
-                        sp = __ldg(tab + ls);
+                        sp = tab[ls];
                         my_c0 = tab_at(tab, ls + 1, ne, total) - sp;
                         probes += 2;
                         if (my_c0 != 0) {        // what the node can still take once the driver sits on it
@@ -539,14 +605,14 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
                         OUT* out = executor_nodes + off;
                         const int32_t* slot_node = s.slot_node + g.sbase;
                         const int32_t dpos = (dslot < ne) ? dslot : 0x7fffffff;
-                        int32_t pos = __ldg(tabs.first_host + (size_t)en->id * tabs.n_groups + grp);    // first node with room for the shape
+                        int32_t pos = tabs.first_host[(size_t)en->id * tabs.n_groups + grp];    // first node with room for the shape
                         ++probes;
                         uint32_t prev = 0, placed = 0;
                         uint32_t nxt = tab_at(tab, pos + 1, ne, total);
                         ++probes;
                         while (placed < k && pos < ne) {
                             // S(pos + 2) is requested before S(pos + 1) is consumed: the walk's dependent-load chain is
-                            // what bounds this kernel (one thread per application), so the next word is always in flight
+                            // what bounds this phase (one thread per application), so the next word is always in flight
                             const uint32_t nxt2 = tab_at(tab, pos + 2, ne, total);
                             ++probes;
                             uint32_t c = nxt - prev;
@@ -613,8 +679,97 @@ __global__ void __launch_bounds__(kDecideThreads) gp_decide_tables(Snapshot s, A
                 if (__shfl_sync(kFull, incl, owner + step - 1) <= e) owner += step;
             const int64_t o_dst = __shfl_sync(kFull, dst, owner), o_src = __shfl_sync(kFull, src, owner);
             const uint32_t o_cut = __shfl_sync(kFull, cut, owner), o_delta = __shfl_sync(kFull, sh_delta, owner);
-            if (e < n_out) executor_nodes[o_dst + e] = (OUT)__ldg(tabs.place + o_src + e + (e < o_cut ? 0u : o_delta));
+            if (e < n_out) executor_nodes[o_dst + e] = (OUT)tabs.place[o_src + e + (e < o_cut ? 0u : o_delta)];
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// the one launch: classify -> tables -> decide
+// ---------------------------------------------------------------------------------------------------------------
+// A persistent grid (sized by the occupancy query) works off one sequence of work items.  Every CTA claims the next
+// ticket with atomicAdd on hdr->ticket, runs the item, and claims again:
+//   tickets [0, n_cls)                  classify tiles of kTabThreads applications (n_cls = 0 when neither the tables nor
+//                                       the offsets are needed);
+//   [n_cls, n_cls + n_tab)              table items, known once every classify tile is done: per executor shape present
+//                                       and group, its segments in order (seg_pre), then per (driver shape, group) one
+//                                       first-fit item;
+//   any later ticket                    the CTA turns to the decide phase: each of its warps claims 32-application chunks
+//                                       from hdr->dec_next until none is left (the cost of a decision varies with its
+//                                       walk; warp-sized claims keep the SMs evenly loaded), then the CTA leaves.
+// Forward progress.  An item waits only for items with smaller tickets: a classify tile for the tiles before it (offset
+// look-back), a table item for every classify tile (hdr->cls_done) and for the earlier segments of its (shape, group)
+// (look-back), the decide phase for every table item (hdr->tab_done).  A ticket is claimed by a CTA that is running, and a
+// CTA claims its next ticket only after finishing the last one.  So by induction over the tickets, every claimed item
+// completes, whatever number of CTAs happens to be co-resident (other work on the GPU, the other pipeline lanes).
+// The ticket, the phase counters and every look-back word start from zero by the memset of the table header.
+template <int ALGO, class OUT>
+__global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppColumns cols, ShapeTables tabs, int64_t off_base,
+                                                                int64_t* off_out /* or NULL */, int32_t* app_slot, int32_t n_apps,
+                                                                int64_t out_cap, int32_t* __restrict__ driver_node,
+                                                                OUT* __restrict__ executor_nodes, PrepApp* __restrict__ prep,
+                                                                int32_t* __restrict__ listed, unsigned long long* __restrict__ stats,
+                                                                int* __restrict__ err, volatile int* __restrict__ err_host, int force_scan) {
+    __shared__ OneScratch sh;
+    ShapeHeader* hdr = tabs.hdr;
+    const int32_t n_tiles = (n_apps + kTabThreads - 1) / kTabThreads;
+    const int32_t n_cls = (!force_scan || off_out) ? n_tiles : 0;
+    int32_t n_es = 0, n_tab = -1, total_segs = 0;         // n_tab < 0: classify not yet seen complete by this CTA
+    unsigned long long probes = 0, drivers = 0;
+    for (;;) {
+        if (threadIdx.x == 0) sh.ticket = atomicAdd(&hdr->ticket, 1u);
+        __syncthreads();
+        const int32_t t = (int32_t)sh.ticket;
+        if (t < n_cls) {
+            if (off_out) classify_offsets(sh, t, n_apps, cols, tabs, off_base, off_out);
+            if (!force_scan) {
+                gp_classify_apps(t, n_apps, cols, tabs, s.meta, app_slot);
+                if (t == 0) segment_prefix(sh, s, tabs.seg_pre);
+            }
+            signal_done(&hdr->cls_done);
+            continue;
+        }
+        if (n_tab < 0) {
+            if (threadIdx.x == 0) wait_count(&hdr->cls_done, (uint32_t)n_cls);
+            __syncthreads();
+            n_tab = 0;
+            if (!force_scan) {
+                n_es = min(hdr->n_shapes, kMaxShapes);
+                total_segs = tabs.seg_pre[s.n_groups];
+                n_tab = n_es * total_segs + min(hdr->n_dshapes, kMaxShapes) * s.n_groups;
+            }
+        }
+        int32_t r = t - n_cls;
+        if (r < n_tab) {
+            if (r < n_es * total_segs) {
+                const int id = r / total_segs;
+                const int32_t gs = r - id * total_segs;
+                int32_t lo = 0, hi = s.n_groups - 1;          // the group whose segments [seg_pre[g], seg_pre[g+1]) hold gs
+                while (lo < hi) {
+                    const int32_t mid = (lo + hi + 1) >> 1;
+                    if (tabs.seg_pre[mid] <= gs) lo = mid; else hi = mid - 1;
+                }
+                const int32_t s0 = tabs.seg_pre[lo];
+                gp_build_shape_tables<ALGO>(sh, s, tabs, id, lo, gs - s0, tabs.seg_pre[lo + 1] - s0, tabs.seg_status + r);
+            } else {
+                const int32_t rd = r - n_es * total_segs;
+                driver_firstfit_block(s, tabs, rd / s.n_groups, rd % s.n_groups);
+            }
+            signal_done(&hdr->tab_done);
+            continue;
+        }
+        if (threadIdx.x == 0) wait_count(&hdr->tab_done, (uint32_t)n_tab);
+        __syncthreads();
+        const int lane = threadIdx.x & 31;
+        for (;;) {
+            uint32_t c = 0;
+            if (lane == 0) c = atomicAdd(&hdr->dec_next, 1u);
+            c = __shfl_sync(kFull, c, 0);
+            if (c >= (uint32_t)(n_apps + 31) / 32u) break;
+            decide_app<ALGO, OUT>((int32_t)c * 32 + lane, s, cols, tabs, app_slot, n_apps, out_cap, driver_node, executor_nodes, prep,
+                                  listed, err, err_host, force_scan, probes, drivers);
+        }
+        break;
     }
     // statistics: one atomic per warp
 #pragma unroll
