@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -89,28 +90,24 @@ __global__ void gp_prep_apps(int32_t n_apps, AppColumns cols, const uint8_t* __r
     for (int32_t t = threadIdx.x; t < n_block * kQ; t += blockDim.x) dst[t] = stage[t];
 }
 
-// Independent mode (GP_MODE_INDEPENDENT): one warp per application; warps claim applications from a
-// global counter (claim-then-broadcast, next index prefetched) so long scans do not leave a tail.
+// Independent minimal-fragmentation (GP_MODE_INDEPENDENT): one warp per application; warps claim applications from a
+// global counter (claim-then-broadcast, next index prefetched) so long scans do not leave a tail.  Independent
+// tightly-pack / distribute-evenly take gp_decide_tables instead.
 constexpr int kPackThreads = 256;
 template <int ALGO>
-#ifndef GP_PACK_MIN_BLOCKS
-#define GP_PACK_MIN_BLOCKS 4
-#endif
 #ifndef GP_MF_MIN_BLOCKS
 #define GP_MF_MIN_BLOCKS 4      // minimal-fragmentation: 64 registers (96 uncapped); occupancy hides its dependent multi-pass loads
 #endif
-__global__ void __launch_bounds__(kPackThreads, ALGO == 2 ? GP_MF_MIN_BLOCKS : GP_PACK_MIN_BLOCKS) gp_pack_independent(Snapshot s, const PrepApp* __restrict__ prep, int32_t n_apps,
+__global__ void __launch_bounds__(kPackThreads, GP_MF_MIN_BLOCKS) gp_pack_independent(Snapshot s, const PrepApp* __restrict__ prep, int32_t n_apps,
                                                                     int32_t* __restrict__ driver_node,
                                                                     int32_t* __restrict__ executor_nodes,
                                                                     int2* __restrict__ scratch,
                                                                     unsigned long long* __restrict__ stats,
                                                                     unsigned int* __restrict__ next_app) {
-    __shared__ uint16_t cap_cache[kPackThreads / 32][kCapCache];
+    static_assert(ALGO == 2, "gp_pack_independent is minimal-fragmentation only");
     const int lane = threadIdx.x & 31;
-    uint16_t* wcache = cap_cache[threadIdx.x >> 5];
     WarpStats st{0, 0};
     const int snap_flags = s.meta->flags;          // per-kernel facts stay in registers
-    const GroupDesc g0 = s.groups[0];
     // claim-then-broadcast, two applications ahead: while application i is packed, the index of i+2 is in
     // flight and the record of i+1 is being pulled into L1
     unsigned int i = 0, n1 = 0;
@@ -123,14 +120,10 @@ __global__ void __launch_bounds__(kPackThreads, ALGO == 2 ? GP_MF_MIN_BLOCKS : G
         if (lane == 0 && n1 < (unsigned int)n_apps) asm volatile("prefetch.global.L1 [%0];" ::"l"(prep + n1));
         const PrepApp* pa = prep + i;
         int32_t d = -1;
-        if (!(pa->flags & kAppInvalid)) {
-            if constexpr (ALGO == 2) {       // minimal-fragmentation: multi-pass, see gangpack_minfrag.cuh
-                const bool gpu_idle = !(pa->flags & kAppUsesGpu) && !(snap_flags & kSnapGpuNegative);
-                d = ((pa->flags & kAppFast32) && gpu_idle) ? pack_app_minfrag<true>(s, pa, executor_nodes, scratch, st, lane, snap_flags)
-                                                           : pack_app_minfrag<false>(s, pa, executor_nodes, scratch, st, lane, snap_flags);
-            } else {
-                d = pack_app<ALGO, int32_t>(s, pa, executor_nodes, scratch, wcache, st, lane, snap_flags, g0);
-            }
+        if (!(pa->flags & kAppInvalid)) {       // multi-pass, see gangpack_minfrag.cuh
+            const bool gpu_idle = !(pa->flags & kAppUsesGpu) && !(snap_flags & kSnapGpuNegative);
+            d = ((pa->flags & kAppFast32) && gpu_idle) ? pack_app_minfrag<true>(s, pa, executor_nodes, scratch, st, lane, snap_flags)
+                                                       : pack_app_minfrag<false>(s, pa, executor_nodes, scratch, st, lane, snap_flags);
         }
         if (lane == 0) driver_node[i] = d;
         i = n1;
@@ -328,9 +321,14 @@ __global__ void gp_scatter_slots(int32_t n_slots, const longlong2* __restrict__ 
 // host side
 // =============================================================================================
 
+// Device memory owned by the context: freed when the context is deleted.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     cudaError_t reserve(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -344,6 +342,15 @@ struct DevBuf {
     template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// One staging layout in one DevBuf: take() every piece (256-byte-aligned offsets), then reserve() once.
+struct Arena {
+    DevBuf& buf;
+    size_t size = 0;
+    size_t take(size_t bytes) { const size_t o = size; size += (bytes + 255) & ~(size_t)255; return o; }
+    cudaError_t reserve() { return buf.reserve(size); }
+    char* base() const { return buf.as<char>(); }
+};
+
 // A fixed sequence of kernel launches / memsets that repeats with identical arguments (one Predicate after the other:
 // same buffers, same batch shape) is captured ONCE into a CUDA graph and replayed with a single launch call -- the
 // pipelined host path is bound by how fast the host thread can issue its calls, not by the GPU.  The key is the byte image
@@ -352,20 +359,39 @@ struct GraphCache {
     cudaGraphExec_t exec = nullptr;
     std::vector<char> key, last_key;
     int launches = 0;
+    ~GraphCache() { reset(); }
     void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; key.clear(); last_key.clear(); }
 };
 
-// dev_misc layout: [0] error bits (int), [8..24) stats (2 x u64), [32..32+4*kMaxChunks) per-chunk work counters
-static constexpr size_t kMiscCounters = 64, kMiscBytes = 64 + 4 * 16;   // [0] err, [8..40) 4 x u64 statistics, [64..) counters
 static constexpr int32_t kChunkApps = 50000;        // apps per pipelined chunk of gp_pack_batch (~1.5 MB H2D)
 static constexpr int32_t kZeroCopyOutApps = 8192;  // batches up to this size write results straight into mapped host memory
+static constexpr int kMaxChunks = 16;
+
+// The head of the per-call status block: what gp_last_stats copies to the host
+struct StatusHead {
+    int err;                                // kErr* bits
+    unsigned long long stats[4];            // nodes_scanned, drivers_tried, scan_path_apps, scan_path_nodes (device atomics)
+};
+static_assert(offsetof(StatusHead, stats) % 8 == 0, "64-bit atomics on the statistics need 8-byte alignment");
+static_assert(sizeof(StatusHead) == 40, "gp_last_stats copies the error bits and the four statistics");
+
+// Device status words of one pack call, zeroed by pack_begin
+struct DevStatus {
+    StatusHead head;
+    unsigned int az_listed, az_claim;       // gp_pack_az_fallback: length of its application list, its claim counter
+    unsigned int fifo_cursor;               // FIFO kernels: instance-group cursor
+    unsigned int next_app[kMaxChunks];      // per pipelined chunk: application claim counter
+};
+static_assert(sizeof(DevStatus) <= 128, "pack_begin zeroes the block on every call");
+
+// Pinned host block: the mirror of StatusHead (gp_last_stats) and the error word the kernels write through its mapping
+struct PinnedStatus { StatusHead head; volatile int err_word; };
 
 struct gp_ctx {
     int device = 0;
     int sm_count = 0;
     cudaStream_t stream = nullptr;
     static constexpr int kLanes = 3;       // H2D / kernels / D2H of consecutive chunks overlap across lanes
-    static constexpr int kMaxChunks = 16;
     cudaStream_t lane[kLanes] = {nullptr, nullptr, nullptr};
     cudaEvent_t ev[kMaxChunks][3] = {};    // per chunk: prep start, pack start, pack end
     cudaEvent_t ev_ready = nullptr, ev_done[kLanes] = {nullptr, nullptr, nullptr};
@@ -380,11 +406,12 @@ struct gp_ctx {
     DevBuf exec_off, drv_off, exec_order, drv_order;
     DevBuf pair, pair32, sgpu, slot_node, node_slot, drv_slot, groups, snap_flags;
 
-    // batch staging
-    DevBuf a_dcpu, a_dmem, a_dgpu, a_ecpu, a_emem, a_egpu, a_count, a_group, a_skip, a_off;
+    // batch staging; a_rows: the six quantity rows in one pitched block (pack_batch_impl)
+    DevBuf a_rows, a_count, a_group, a_skip, a_off;
     DevBuf prep, r_driver, r_exec, scratch, dev_misc, gmin, sortbuf, usagebuf, reschedbuf;
-    std::vector<int32_t> iota;   // dev_misc: [0] err int, [2..3] stats u64 x2 (8B aligned at +8)
-    void* pinned_misc = nullptr;                         // 32 B pinned mirror of dev_misc
+    void* pinned_misc = nullptr;                  // PinnedStatus
+    DevStatus* status() const { return dev_misc.as<DevStatus>(); }
+    PinnedStatus* host_status() const { return static_cast<PinnedStatus*>(pinned_misc); }
     std::vector<int64_t> host_off;
     std::vector<int32_t> v_owner;                 // gp_set_snapshot validation scratch (no per-call allocation)
     // gp_set_snapshot's host copy of the layout, kept for gp_pack_fifo_az_aware's order checks: v_owner[v] (group, roles)
@@ -404,7 +431,7 @@ struct gp_ctx {
     bool async_snapshot = false;                  // gp_config.flags & GP_CFG_ASYNC_SNAPSHOT
     int chunk_apps = kChunkApps;                  // GANGPACK_CHUNK_APPS
     int trace = 0;                                // GANGPACK_TRACE=1: host-side phase timing on stderr
-    int pack_ctas_per_sm[3] = {0, 0, 0};            // occupancy of gp_pack_independent<ALGO> on this device
+    int pack_ctas_per_sm = 0;                       // occupancy of gp_pack_independent<2> on this device
     int tab_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_pack_listed<ALGO, OUT>
     int dec_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_decide_tables<ALGO, OUT>
     // per pipeline lane: shape hash + header, capacity tables, group totals, placement prefixes, per-application shape slot
@@ -415,7 +442,8 @@ struct gp_ctx {
     GraphCache g_snapshot;                        // slot layout of gp_set_snapshot
     DevBuf off_dev;                               // ExecutorNodes offsets derived on the device
     DevBuf fifo_list;                             // FIFO modes: per-instance-group application lists (queue order)
-    DevBuf sched, zonebuf;                        // SchedulableResources [3][n_nodes]; staging of gp_pack_batch_zones
+    DevBuf sched, zonebuf, fbview;                // SchedulableResources [3][n_nodes]; staging of the zone entry points;
+                                                  // the az-aware fallback's orders and gather view
     bool have_sched = false;
     bool sort_attr_set = false;
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
@@ -569,8 +597,8 @@ gp_status gp_create(gp_ctx** out, const gp_config* cfg) {
     if ((e = cudaSetDevice(dev)) != cudaSuccess ||
         (e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = create_aux(c)) != cudaSuccess ||
-        (e = cudaHostAlloc(&c->pinned_misc, 64, cudaHostAllocDefault)) != cudaSuccess ||
-        (e = c->dev_misc.reserve(kMiscBytes)) != cudaSuccess || (e = c->snap_flags.reserve(sizeof(SnapMeta))) != cudaSuccess) {
+        (e = cudaHostAlloc(&c->pinned_misc, sizeof(PinnedStatus), cudaHostAllocDefault)) != cudaSuccess ||
+        (e = c->dev_misc.reserve(sizeof(DevStatus))) != cudaSuccess || (e = c->snap_flags.reserve(sizeof(SnapMeta))) != cudaSuccess) {
         g_create_error = std::string("gp_create: ") + cudaGetErrorString(e);
         delete c;
         return GP_ERR_CUDA;
@@ -583,15 +611,6 @@ void gp_destroy(gp_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    DevBuf* bufs[] = {&c->node_cpu, &c->node_mem, &c->node_gpu, &c->exec_off, &c->drv_off, &c->exec_order, &c->drv_order,
-                      &c->pair, &c->pair32, &c->sgpu, &c->slot_node, &c->node_slot, &c->drv_slot, &c->groups, &c->snap_flags,
-                      &c->a_dcpu, &c->a_dmem, &c->a_dgpu, &c->a_ecpu, &c->a_emem, &c->a_egpu, &c->a_count, &c->a_group,
-                      &c->a_skip, &c->a_off, &c->prep, &c->r_driver, &c->r_exec, &c->scratch, &c->dev_misc, &c->gmin, &c->sortbuf, &c->usagebuf, &c->reschedbuf,
-                      &c->off_dev, &c->fifo_list, &c->sched, &c->zonebuf};
-    for (DevBuf* b : bufs) b->release();
-    for (auto& t : c->tabs) { t.hdr.release(); t.table.release(); t.total.release(); t.app_slot.release(); }
-    for (auto& g : c->g_chunk) g.reset();
-    c->g_snapshot.reset();
     if (c->pinned_misc) cudaFreeHost(c->pinned_misc);
     if (c->one_block) cudaFreeHost(c->one_block);
     for (auto& row : c->ev) for (cudaEvent_t e : row) if (e) cudaEventDestroy(e);
@@ -600,7 +619,7 @@ void gp_destroy(gp_ctx* c) {
     for (cudaEvent_t e : c->ev_done) if (e) cudaEventDestroy(e);
     for (cudaStream_t l : c->lane) if (l) cudaStreamDestroy(l);
     if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;                            // device buffers and graphs free themselves
 }
 
 gp_status gp_alloc_pinned(gp_ctx* ctx, size_t bytes, void** out) {
@@ -864,49 +883,44 @@ static AppColumns cols_at(const AppColumns& c, int32_t lo) {
     return r;
 }
 
-template <int ALGO>
-static void launch_pack(gp_ctx* c, gp_mode mode, const Snapshot& s, const PrepApp* prep, const int32_t* app_group, int32_t n_apps,
-                        int32_t* driver_node, int32_t* executor_nodes, int2* scratch, unsigned long long* stats,
-                        unsigned int* next_app, cudaStream_t st) {
-    if (mode == GP_MODE_INDEPENDENT) {
-        // persistent grid: as many CTAs as fit on the device (or fewer for small batches)
-        int& per_sm = c->pack_ctas_per_sm[ALGO];
-        if (per_sm == 0) {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_independent<ALGO>, kPackThreads, 0);
-            if (per_sm < 1) per_sm = 1;
-        }
-        int64_t blocks = ((int64_t)n_apps * 32 + kPackThreads - 1) / kPackThreads;
-        int64_t max_blocks = (int64_t)c->sm_count * per_sm;
-        if (blocks > max_blocks) blocks = max_blocks;
-        if (blocks < 1) blocks = 1;
-        gp_pack_independent<ALGO><<<(int)blocks, kPackThreads, 0, st>>>(s, prep, n_apps, driver_node, executor_nodes, scratch,
-                                                                       stats, next_app);
-    } else if constexpr (ALGO != 2) {     // (check_args rejects the FIFO modes for minimal-fragmentation)
-        // FIFO: one persistent 1024-thread CTA per instance group, its slots staged in shared memory
-        bool& attr_set = c->fifo_attr_set[ALGO];     // per device: function attributes live in the device's context
-        if (!attr_set) {
-            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
-            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
-            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
-            cudaFuncSetAttribute(gp_pack_fifo_cta<ALGO, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes);
-            attr_set = true;
-        }
-        // small groups: fewer threads per CTA (the per-application fixed cost scales with the CTA size)
-        const int avg_ne = c->n_groups > 0 ? c->n_exec / c->n_groups : 0;
-        const int kFifoThreadsRt = kFifoThreads;
-        (void)avg_ne;
-        int32_t* app_list = c->fifo_list.as<int32_t>();
-        unsigned int* cursor = reinterpret_cast<unsigned int*>(c->dev_misc.as<char>() + 56);     // zeroed by pack_begin
-        auto kern = mode == GP_MODE_FIFO_REFERENCE ? (c->fifo_warp ? gp_pack_fifo_cta<ALGO, 1, true> : gp_pack_fifo_cta<ALGO, 1, false>)
-                                                   : (c->fifo_warp ? gp_pack_fifo_cta<ALGO, 2, true> : gp_pack_fifo_cta<ALGO, 2, false>);
-        kern<<<s.n_groups, kFifoThreadsRt, kFifoSmemBytes, st>>>(s, prep, app_group, n_apps, driver_node, executor_nodes, scratch, stats, s.gmins, app_list, cursor);
-        // the FIFO kernels subtract usage from `pair` in place: refresh the compact 32-bit view so that a later
-        // independent pack on this context (the driver's own pack after fitEarlierDrivers, resource.go:255 then :321)
-        // sees the charged availability
-        const int T = 256;
-        gp_fill_pair32<<<(c->n_slots + T) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
-        c->last.kernel_launches += 1;
+// independent minimal-fragmentation: persistent grid, as many CTAs as fit on the device (or fewer for small batches)
+static void launch_minfrag(gp_ctx* c, const Snapshot& s, const PrepApp* prep, int32_t n_apps, int32_t* driver_node,
+                           int32_t* executor_nodes, int2* scratch, unsigned long long* stats, unsigned int* next_app, cudaStream_t st) {
+    int& per_sm = c->pack_ctas_per_sm;
+    if (per_sm == 0) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_independent<2>, kPackThreads, 0);
+        if (per_sm < 1) per_sm = 1;
     }
+    int64_t blocks = ((int64_t)n_apps * 32 + kPackThreads - 1) / kPackThreads;
+    int64_t max_blocks = (int64_t)c->sm_count * per_sm;
+    if (blocks > max_blocks) blocks = max_blocks;
+    if (blocks < 1) blocks = 1;
+    gp_pack_independent<2><<<(int)blocks, kPackThreads, 0, st>>>(s, prep, n_apps, driver_node, executor_nodes, scratch, stats, next_app);
+}
+
+// FIFO modes (tightly-pack / distribute-evenly): one persistent 1024-thread CTA per instance group, its slots staged in
+// shared memory
+template <int ALGO>
+static gp_status launch_fifo(gp_ctx* c, gp_mode mode, const Snapshot& s, const PrepApp* prep, const int32_t* app_group, int32_t n_apps,
+                             int32_t* driver_node, int32_t* executor_nodes, int2* scratch, unsigned long long* stats, cudaStream_t st) {
+    const auto kernels = {gp_pack_fifo_cta<ALGO, 1, true>, gp_pack_fifo_cta<ALGO, 2, true>, gp_pack_fifo_cta<ALGO, 1, false>,
+                          gp_pack_fifo_cta<ALGO, 2, false>};
+    bool& attr_set = c->fifo_attr_set[ALGO];     // per device: function attributes live in the device's context
+    if (!attr_set) {
+        for (auto k : kernels) GP_CUDA(c, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFifoSmemBytes));
+        attr_set = true;
+    }
+    auto kern = mode == GP_MODE_FIFO_REFERENCE ? (c->fifo_warp ? gp_pack_fifo_cta<ALGO, 1, true> : gp_pack_fifo_cta<ALGO, 1, false>)
+                                               : (c->fifo_warp ? gp_pack_fifo_cta<ALGO, 2, true> : gp_pack_fifo_cta<ALGO, 2, false>);
+    kern<<<s.n_groups, kFifoThreads, kFifoSmemBytes, st>>>(s, prep, app_group, n_apps, driver_node, executor_nodes, scratch, stats, s.gmins,
+                                                           c->fifo_list.as<int32_t>(), &c->status()->fifo_cursor);
+    // the FIFO kernels subtract usage from `pair` in place: refresh the compact 32-bit view so that a later
+    // independent pack on this context (the driver's own pack after fitEarlierDrivers, resource.go:255 then :321)
+    // sees the charged availability
+    const int T = 256;
+    gp_fill_pair32<<<(c->n_slots + T) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
+    c->last.kernel_launches += 1;
+    return GP_OK;
 }
 
 // independent tightly-pack / distribute-evenly: one launch for classify -> capacity tables -> thread-per-application
@@ -951,10 +965,10 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
                                    const DevResults& dr, int2* scratch, cudaStream_t st, int chunk) {
     const int32_t q = hi - lo;
     if (q <= 0) return GP_OK;
-    int* d_err = c->dev_misc.as<int>();
-    unsigned long long* d_stats = reinterpret_cast<unsigned long long*>(c->dev_misc.as<char>() + 8);
-    unsigned int* next_app = reinterpret_cast<unsigned int*>(c->dev_misc.as<char>() + kMiscCounters) + chunk;
-    volatile int* err_host = reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48);
+    int* d_err = &c->status()->head.err;
+    unsigned long long* d_stats = c->status()->head.stats;
+    unsigned int* next_app = &c->status()->next_app[chunk];
+    volatile int* err_host = &c->host_status()->err_word;
     Snapshot s = make_snapshot(c);
     AppColumns cols = cols_at(da.cols, lo);
 
@@ -1000,18 +1014,15 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         int32_t* listed = app_slot + 2 * (size_t)q;
         PrepApp* prep = c->prep.as<PrepApp>() + lo;
         const bool o16 = dr.node_bits == 16;
+        const auto launch = algo == GP_TIGHTLY_PACK ? (o16 ? launch_tables<0, uint16_t> : launch_tables<0, int32_t>)
+                                                    : (o16 ? launch_tables<1, uint16_t> : launch_tables<1, int32_t>);
         auto issue = [&](int& launches) -> gp_status {
             const int before = (int)c->last.kernel_launches;
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][0], st));
             GP_CUDA(c, cudaMemsetAsync(T.hdr.p, 0, zero_bytes, st));
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][1], st));
-            gp_status r;
-            if (algo == GP_TIGHTLY_PACK)
-                r = o16 ? launch_tables<0, uint16_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st)
-                        : launch_tables<0, int32_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st);
-            else
-                r = o16 ? launch_tables<1, uint16_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st)
-                        : launch_tables<1, int32_t>(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app, d_err, err_host, use_tables, seg_bound, st);
+            const gp_status r = launch(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app,
+                                       d_err, err_host, use_tables, seg_bound, st);
             if (r != GP_OK) return r;
             GP_CUDA(c, cudaGetLastError());
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][2], st));
@@ -1031,7 +1042,7 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         key.cols = cols; key.tabs = tabs; key.snap = s; key.cap = dr.cap;
         const void* ptrs[10] = {app_slot, prep, listed, dr.driver, dr.exec, scratch, d_stats, next_app, d_err, off_out};
         std::memcpy(key.p, ptrs, sizeof(ptrs));
-        return run_cached(c, c->g_chunk[st == c->stream ? gp_ctx::kMaxChunks : chunk], &key, sizeof(key), st, issue);
+        return run_cached(c, c->g_chunk[st == c->stream ? kMaxChunks : chunk], &key, sizeof(key), st, issue);
     }
 
     // ---- FIFO modes and minimal-fragmentation: prepared records + the pack kernel ------------------------------------
@@ -1049,12 +1060,13 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
     s.gmins = c->gmin.as<GroupMin>();
     if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][1], st));
     int32_t* exec32 = static_cast<int32_t*>(dr.exec);
-    if (algo == GP_TIGHTLY_PACK)
-        launch_pack<0>(c, mode, s, prep, cols.group, q, dr.driver + lo, exec32, scratch, d_stats, next_app, st);
-    else if (algo == GP_MINIMAL_FRAGMENTATION)
-        launch_pack<2>(c, mode, s, prep, cols.group, q, dr.driver + lo, exec32, scratch, d_stats, next_app, st);
-    else
-        launch_pack<1>(c, mode, s, prep, cols.group, q, dr.driver + lo, exec32, scratch, d_stats, next_app, st);
+    if (mode == GP_MODE_INDEPENDENT) {
+        launch_minfrag(c, s, prep, q, dr.driver + lo, exec32, scratch, d_stats, next_app, st);
+    } else {                              // (check_args rejects the FIFO modes for minimal-fragmentation)
+        const gp_status r = algo == GP_TIGHTLY_PACK ? launch_fifo<0>(c, mode, s, prep, cols.group, q, dr.driver + lo, exec32, scratch, d_stats, st)
+                                                    : launch_fifo<1>(c, mode, s, prep, cols.group, q, dr.driver + lo, exec32, scratch, d_stats, st);
+        if (r != GP_OK) return r;
+    }
     GP_CUDA(c, cudaGetLastError());
     if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][2], st));
     c->last.kernel_launches += 2;
@@ -1065,8 +1077,8 @@ static bool fused_path(gp_algo algo, gp_mode mode) { return mode == GP_MODE_INDE
 
 // common prologue: buffers, counters
 static gp_status pack_begin(gp_ctx* c, int32_t q, gp_algo algo, gp_mode mode, int64_t exec_cap, bool derive_off, int2** scratch, cudaStream_t st) {
-    GP_CUDA(c, cudaMemsetAsync(c->dev_misc.p, 0, kMiscBytes, st));
-    *reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48) = 0;   // host-visible error word
+    GP_CUDA(c, cudaMemsetAsync(c->status(), 0, sizeof(DevStatus), st));
+    c->host_status()->err_word = 0;
     c->last = gp_stats{};
     c->ev_chunks = 0;
     *scratch = nullptr;
@@ -1120,6 +1132,9 @@ static gp_status decode_device_error(gp_ctx* c, int err) {
     return fail(c, GP_ERR_CAPACITY, "pack: exec_out_off inconsistent with exe_count or executor_nodes_cap too small");
 }
 
+// after a synchronise: the validation errors the kernels reported through the mapped error word
+static gp_status host_error(gp_ctx* c) { return decode_device_error(c, c->host_status()->err_word); }
+
 static gp_apps_wire widen(const gp_apps* a) {
     gp_apps_wire w{};
     w.n_apps = a->n_apps; w.quantity_bits = 64; w.mem_shift = 0;
@@ -1157,17 +1172,16 @@ gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mo
 gp_status gp_last_stats(gp_ctx* c, gp_stats* out) {
     if (!c || !out) return GP_ERR_INVALID;
     GP_CUDA(c, cudaSetDevice(c->device));
-    GP_CUDA(c, cudaMemcpyAsync(c->pinned_misc, c->dev_misc.p, 40, cudaMemcpyDeviceToHost, c->stream));
+    StatusHead& h = c->host_status()->head;
+    GP_CUDA(c, cudaMemcpyAsync(&h, &c->status()->head, sizeof(StatusHead), cudaMemcpyDeviceToHost, c->stream));
     GP_CUDA(c, cudaStreamSynchronize(c->stream));
-    const unsigned long long* s = reinterpret_cast<const unsigned long long*>((const char*)c->pinned_misc + 8);
-    c->last.nodes_scanned = (int64_t)s[0];
-    c->last.drivers_tried = (int64_t)s[1];
-    c->last.scan_path_apps = (int64_t)s[2];
-    c->last.scan_path_nodes = (int64_t)s[3];
+    c->last.nodes_scanned = (int64_t)h.stats[0];
+    c->last.drivers_tried = (int64_t)h.stats[1];
+    c->last.scan_path_apps = (int64_t)h.stats[2];
+    c->last.scan_path_nodes = (int64_t)h.stats[3];
     fill_kernel_times(c);
     *out = c->last;
-    int err = *reinterpret_cast<const int*>(c->pinned_misc);
-    return decode_device_error(c, err);
+    return decode_device_error(c, h.err);
 }
 
 static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, gp_results_wire* out);
@@ -1216,7 +1230,7 @@ static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo,
     // the quantity columns are staged in ONE pitched device block (rows: drv cpu, drv mem, exe cpu, exe mem, drv gpu,
     // exe gpu) so that equally spaced host columns can be moved by a single 2-D DMA per chunk
     const size_t dpitch = (bq + 255) & ~(size_t)255;
-    GP_CUDA(c, c->a_dcpu.reserve(dpitch * 6));
+    GP_CUDA(c, c->a_rows.reserve(dpitch * 6));
     GP_CUDA(c, c->a_count.reserve(b32));
     if (off) GP_CUDA(c, c->a_off.reserve(sizeof(int64_t) * (size_t)(q + 1)));
     GP_CUDA(c, c->r_driver.reserve(b32));
@@ -1230,7 +1244,7 @@ static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo,
     void* mo_driver = small ? const_cast<void*>(mapped_ptr(c, out->driver_node, b32)) : nullptr;
     void* mo_exec = (small && out->executor_nodes) ? const_cast<void*>(mapped_ptr(c, out->executor_nodes, os * (size_t)out->executor_nodes_cap)) : nullptr;
     const bool out_mapped = small && mo_driver && (out->executor_nodes_cap == 0 || !out->executor_nodes || mo_exec);
-    char* blk = c->a_dcpu.as<char>();
+    char* blk = c->a_rows.as<char>();
     DevApps dv{};
     const void* hq[6] = {a->drv_cpu, a->drv_mem, a->exe_cpu, a->exe_mem, a->drv_gpu, a->exe_gpu};    // staging row order
     dv.cols.q[0] = blk + 0 * dpitch; dv.cols.q[1] = blk + 1 * dpitch; dv.cols.q[3] = blk + 2 * dpitch; dv.cols.q[4] = blk + 3 * dpitch;
@@ -1254,7 +1268,7 @@ static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo,
     int n_chunks = 1;
     if (mode == GP_MODE_INDEPENDENT && q >= 2 * c->chunk_apps) {
         n_chunks = (q + c->chunk_apps - 1) / c->chunk_apps;
-        if (n_chunks > gp_ctx::kMaxChunks) n_chunks = gp_ctx::kMaxChunks;
+        if (n_chunks > kMaxChunks) n_chunks = kMaxChunks;
     }
     int2* scratch = nullptr;
     s = pack_begin(c, q, algo, mode, out->executor_nodes_cap, !off, &scratch, st);
@@ -1369,9 +1383,8 @@ static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo,
                      a->quantity_bits, out->node_bits, (int)out_mapped, std::chrono::duration<double, std::micro>(t_issued - t_begin).count(),
                      std::chrono::duration<double, std::micro>(t_done - t_issued).count());
     }
-    // validation errors arrive through the mapped error word; scan statistics stay on the device until
-    // gp_last_stats asks for them
-    return decode_device_error(c, *reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
+    // scan statistics stay on the device until gp_last_stats asks for them
+    return host_error(c);
 }
 
 gp_status gp_pack_one(gp_ctx* c, gp_algo algo, int64_t drv_cpu, int64_t drv_mem, int64_t drv_gpu, int64_t exe_cpu,
@@ -1441,6 +1454,59 @@ gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, 
     return GP_OK;
 }
 
+// ---- staging shared by the zone entry points ------------------------------------------------------------------------
+// the arrays a non-empty batch of a zone entry point needs
+static bool has_zone_arrays(const gp_apps* a, const gp_zone_results* out) {
+    return a->drv_cpu_milli && a->drv_mem_bytes && a->exe_cpu_milli && a->exe_mem_bytes && a->exe_count && out->zone && out->driver_node;
+}
+
+// The six int64 quantity columns (6 x n_apps from o_in; absent gpu columns stay NULL = 0 in `six`), exe_count to o_cnt
+// and the ExecutorNodes offsets `off` to o_off
+static gp_status upload_app_columns(gp_ctx* c, const gp_apps* a, const int64_t* off, char* b, size_t o_in, size_t o_cnt, size_t o_off,
+                                    cudaStream_t st, SixCols* six) {
+    const size_t q = (size_t)a->n_apps;
+    const int64_t* hc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
+    *six = SixCols{};
+    for (int k = 0; k < 6; ++k) {
+        if (!hc[k]) continue;
+        int64_t* d = reinterpret_cast<int64_t*>(b + o_in) + q * (size_t)k;
+        GP_CUDA(c, cudaMemcpyAsync(d, hc[k], 8 * q, cudaMemcpyHostToDevice, st));
+        six->p[k] = d;
+    }
+    GP_CUDA(c, cudaMemcpyAsync(b + o_cnt, a->exe_count, 4 * q, cudaMemcpyHostToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(b + o_off, off, 8 * (q + 1), cudaMemcpyHostToDevice, st));
+    return GP_OK;
+}
+
+// az-aware-tightly-pack: upload the undivided orders and build the fallback's gather view of them (gp_build_fallback_view)
+static gp_status stage_fallback_view(gp_ctx* c, const gp_az_orders* az, cudaStream_t st, GatherSlots* fb) {
+    const size_t ne = (size_t)az->n_exec, nd = (size_t)az->n_drv;
+    Arena ar{c->fbview};
+    const size_t o_eord = ar.take(4 * ne), o_dord = ar.take(4 * nd), o_npos = ar.take(4 * (size_t)c->n_nodes), o_fbe = ar.take(4 * ne),
+                 o_fbd = ar.take(4 * nd), o_fbp = ar.take(4 * nd);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    if (ne) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * ne, cudaMemcpyHostToDevice, st));
+    if (nd) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * nd, cudaMemcpyHostToDevice, st));
+    gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)ne, (int32_t)nd, (const int32_t*)(b + o_eord), (const int32_t*)(b + o_dord),
+                                               c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe), (int32_t*)(b + o_fbd),
+                                               (int32_t*)(b + o_fbp));
+    c->last.kernel_launches += 1;
+    *fb = GatherSlots{(const int32_t*)(b + o_fbe), (const int32_t*)(b + o_fbd), (const int32_t*)(b + o_fbp), (int32_t)ne, (int32_t)nd};
+    return GP_OK;
+}
+
+// zone / driver / ExecutorNodes (T entries) / averages to the host, one synchronise, then the kernels' validation errors
+static gp_status finish_zone_results(gp_ctx* c, gp_zone_results* out, const int32_t* zone, const int32_t* drv, const int32_t* exe,
+                                     const double* avg, size_t q, size_t T, cudaStream_t st) {
+    GP_CUDA(c, cudaMemcpyAsync(out->zone, zone, 4 * q, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaMemcpyAsync(out->driver_node, drv, 4 * q, cudaMemcpyDeviceToHost, st));
+    if (T) GP_CUDA(c, cudaMemcpyAsync(out->executor_nodes, exe, 4 * T, cudaMemcpyDeviceToHost, st));
+    if (out->avg_efficiency) GP_CUDA(c, cudaMemcpyAsync(out->avg_efficiency, avg, 32 * q, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    return host_error(c);
+}
+
 // Independent zone packs of a batch, shared by gp_pack_batch_zones (the zones are every instance group, no fallback) and
 // gp_pack_batch_az_aware (zones 0..Z-1 with tightly-pack, plus the undivided orders `az` of the fallback, already
 // validated).  Argument checks common to both are here.
@@ -1449,8 +1515,7 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
     const std::string w(who);
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
-    if (!a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->zone || !out->driver_node)
-        return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
+    if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
     if ((int64_t)Q * Z > 0x7fffffffLL) return fail(c, GP_ERR_INVALID, w + ": n_apps x zones too large");
     const int64_t* off = a->exec_out_off;
     if (!off) {
@@ -1466,26 +1531,18 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t q = (size_t)Q, R = q * (size_t)Z, T = (size_t)total;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-    const size_t o_in = take(48 * q), o_cnt = take(4 * q), o_off = take(8 * (q + 1)), o_rows = take(48 * R), o_rcnt = take(4 * R), o_rgrp = take(4 * R),
-                 o_roff = take(8 * (R + 1)), o_rdrv = take(4 * R), o_rexe = take(4 * ((size_t)Z * T + 1)), o_zone = take(4 * q), o_drv = take(4 * q),
-                 o_exe = take(4 * (T + 1)), o_avg = take(32 * q);
-    // az-aware: the fallback's PrepApp records and list, the undivided orders and their gather view
-    const size_t QF = az ? q : 0, NE = az ? (size_t)az->n_exec : 0, ND = az ? (size_t)az->n_drv : 0, NN = az ? (size_t)c->n_nodes : 0;
-    const size_t o_prep = take(sizeof(PrepApp) * QF), o_list = take(4 * QF), o_eord = take(4 * NE), o_dord = take(4 * ND), o_npos = take(4 * NN),
-                 o_fbe = take(4 * NE), o_fbd = take(4 * ND), o_fbp = take(4 * ND);
-    GP_CUDA(c, c->zonebuf.reserve(o));
-    char* b = c->zonebuf.as<char>();
-    const int64_t* hc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
-    SixCols six{};
-    for (int k = 0; k < 6; ++k) {
-        if (!hc[k]) continue;
-        GP_CUDA(c, cudaMemcpyAsync(b + o_in + 8 * q * (size_t)k, hc[k], 8 * q, cudaMemcpyHostToDevice, st));
-        six.p[k] = reinterpret_cast<const int64_t*>(b + o_in + 8 * q * (size_t)k);
-    }
-    GP_CUDA(c, cudaMemcpyAsync(b + o_cnt, a->exe_count, 4 * q, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_off, off, 8 * (q + 1), cudaMemcpyHostToDevice, st));
+    Arena ar{c->zonebuf};
+    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_rows = ar.take(48 * R), o_rcnt = ar.take(4 * R),
+                 o_rgrp = ar.take(4 * R), o_roff = ar.take(8 * (R + 1)), o_rdrv = ar.take(4 * R), o_rexe = ar.take(4 * ((size_t)Z * T + 1)),
+                 o_zone = ar.take(4 * q), o_drv = ar.take(4 * q), o_exe = ar.take(4 * (T + 1)), o_avg = ar.take(32 * q);
+    // az-aware: the fallback's PrepApp records and list
+    const size_t QF = az ? q : 0;
+    const size_t o_prep = ar.take(sizeof(PrepApp) * QF), o_list = ar.take(4 * QF);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    SixCols six;
+    gp_status s = upload_app_columns(c, a, off, b, o_in, o_cnt, o_off, st, &six);
+    if (s != GP_OK) return s;
     const int TH = 256;
     // the efficiencies read the availability in node-table order: refresh that copy from the slots (a FIFO batch may
     // have charged them since gp_set_snapshot)
@@ -1495,7 +1552,7 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
     gp_zone_expand<<<(unsigned)((R + 1 + TH - 1) / TH), TH, 0, st>>>(Q, Z, six, (const int32_t*)(b + o_cnt), (const int64_t*)(b + o_off),
                                                                       (int64_t*)(b + o_rows), (int32_t*)(b + o_rcnt), (int32_t*)(b + o_rgrp), (int64_t*)(b + o_roff));
     int2* scratch = nullptr;
-    gp_status s = pack_begin(c, (int32_t)R, algo, GP_MODE_INDEPENDENT, (int64_t)Z * total, false, &scratch, st);
+    s = pack_begin(c, (int32_t)R, algo, GP_MODE_INDEPENDENT, (int64_t)Z * total, false, &scratch, st);
     if (s != GP_OK) return s;
     DevApps dv{};
     for (int k = 0; k < 6; ++k) dv.cols.q[k] = b + o_rows + 8 * R * (size_t)k;
@@ -1519,28 +1576,22 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
     c->last.kernel_launches += 2;
     if (az) {
         // the applications no zone won: SparkBinPack(tightlyPackExecutors) over the undivided orders, still on the device
-        // (az_aware_pack_tightly.go:33-37).  dev_misc [40] = length of the list, [44] = the fallback's claim counter
-        // (both zeroed by pack_begin); stats [2..3] restart so that scan_path_apps / _nodes count the fallback alone.
-        unsigned int* n_listed = reinterpret_cast<unsigned int*>(c->dev_misc.as<char>() + 40);
-        unsigned long long* d_stats = reinterpret_cast<unsigned long long*>(c->dev_misc.as<char>() + 8);
+        // (az_aware_pack_tightly.go:33-37).  The list length and the fallback's claim counter are zeroed by pack_begin;
+        // stats [2..3] restart so that scan_path_apps / _nodes count the fallback alone.
+        DevStatus* ds = c->status();
+        unsigned long long* d_stats = ds->head.stats;
         GP_CUDA(c, cudaMemsetAsync(d_stats + 2, 0, 16, st));
         int32_t* listed = (int32_t*)(b + o_list);
-        gp_az_fallback_list<<<(unsigned)((q + TH - 1) / TH), TH, 0, st>>>(Q, (const int32_t*)(b + o_zone), listed, n_listed);
+        gp_az_fallback_list<<<(unsigned)((q + TH - 1) / TH), TH, 0, st>>>(Q, (const int32_t*)(b + o_zone), listed, &ds->az_listed);
         AppColumns cols{};
         for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
         cols.count = (const int32_t*)(b + o_cnt); cols.group = nullptr; cols.off = (const int64_t*)(b + o_off); cols.bits = 64; cols.mem_shift = 0;
         PrepApp* prep = (PrepApp*)(b + o_prep);
         gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
-            Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, c->dev_misc.as<int>(),
-            reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
-        if (NE) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * NE, cudaMemcpyHostToDevice, st));
-        if (ND) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * ND, cudaMemcpyHostToDevice, st));
-        gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)NE, (int32_t)ND, (const int32_t*)(b + o_eord), (const int32_t*)(b + o_dord),
-                                                   c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe),
-                                                   (int32_t*)(b + o_fbd), (int32_t*)(b + o_fbp));
-        GatherSlots fb{};
-        fb.exec_slot = (const int32_t*)(b + o_fbe); fb.drv_slot = (const int32_t*)(b + o_fbd); fb.drv_pos = (const int32_t*)(b + o_fbp);
-        fb.ne = (int32_t)NE; fb.nd = (int32_t)ND;
+            Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, &ds->head.err, &c->host_status()->err_word);
+        GatherSlots fb;
+        s = stage_fallback_view(c, az, st, &fb);
+        if (s != GP_OK) return s;
         int& per_sm = c->az_fallback_ctas_per_sm;
         if (per_sm == 0) {
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_az_fallback, kAzFallbackThreads, 0);
@@ -1548,17 +1599,13 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
         }
         int64_t blocks = ((int64_t)Q * 32 + kAzFallbackThreads - 1) / kAzFallbackThreads;   // the list holds at most Q
         if (blocks > (int64_t)c->sm_count * per_sm) blocks = (int64_t)c->sm_count * per_sm;
-        gp_pack_az_fallback<<<(unsigned)blocks, kAzFallbackThreads, 0, st>>>(make_snapshot(c), prep, listed, n_listed, fb, (int32_t*)(b + o_drv),
-                                                                            (int32_t*)(b + o_exe), d_stats, n_listed + 1);
+        gp_pack_az_fallback<<<(unsigned)blocks, kAzFallbackThreads, 0, st>>>(make_snapshot(c), prep, listed, &ds->az_listed, fb, (int32_t*)(b + o_drv),
+                                                                            (int32_t*)(b + o_exe), d_stats, &ds->az_claim);
         GP_CUDA(c, cudaGetLastError());
-        c->last.kernel_launches += 4;
+        c->last.kernel_launches += 3;
     }
-    GP_CUDA(c, cudaMemcpyAsync(out->zone, b + o_zone, 4 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaMemcpyAsync(out->driver_node, b + o_drv, 4 * q, cudaMemcpyDeviceToHost, st));
-    if (T) GP_CUDA(c, cudaMemcpyAsync(out->executor_nodes, b + o_exe, 4 * T, cudaMemcpyDeviceToHost, st));
-    if (out->avg_efficiency) GP_CUDA(c, cudaMemcpyAsync(out->avg_efficiency, b + o_avg, 32 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    return decode_device_error(c, *reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
+    return finish_zone_results(c, out, (const int32_t*)(b + o_zone), (const int32_t*)(b + o_drv), (const int32_t*)(b + o_exe),
+                               (const double*)(b + o_avg), q, T, st);
 }
 
 gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone_results* out) {
@@ -1572,16 +1619,12 @@ gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone
 }
 
 // ---- reservation table + device-resident snapshot upkeep (gangpack_zones.cuh) -------------------------------------------
-static gp_status refresh_views(gp_ctx* c, bool raised, cudaStream_t st) {
+static gp_status refresh_views(gp_ctx* c, cudaStream_t st) {
     const int T = 256;
     if (c->n_slots <= 0) return GP_OK;
     SnapMeta* meta = c->snap_flags.as<SnapMeta>();
-    if (raised)
-        gp_refresh_meta<<<(c->n_slots + T - 1) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->slot_node.as<int32_t>(),
-                                                               &meta->flags, meta->max_avail);
-    else   // availabilities only went down: a negative gpu value may have appeared
-        gp_refresh_meta<<<(c->n_slots + T - 1) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->slot_node.as<int32_t>(),
-                                                               &meta->flags, meta->max_avail);
+    gp_refresh_meta<<<(c->n_slots + T - 1) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->slot_node.as<int32_t>(),
+                                                           &meta->flags, meta->max_avail);
     gp_fill_pair32<<<(c->n_slots + T) / T, T, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), meta, c->pair32.as<uint2>());
     GP_CUDA(c, cudaGetLastError());
     return GP_OK;
@@ -1637,8 +1680,7 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     const std::string w(who);
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
-    if (!a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->zone || !out->driver_node)
-        return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
+    if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
     std::vector<int64_t>& hoff = c->host_off;
     hoff.resize((size_t)Q + 1);
     int64_t acc = 0, pitch = 1;
@@ -1659,36 +1701,28 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     cudaStream_t st = c->stream;
     const bool azk = kind == kZoneAzAware;
     const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)(Z + (azk ? 1 : 0)) * (size_t)pitch;   // az-aware: row Z = fallback
-    const size_t NE = azk ? (size_t)az->n_exec : 0, ND = azk ? (size_t)az->n_drv : 0, NN = azk ? (size_t)c->n_nodes : 0;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-    const size_t o_in = take(48 * q), o_cnt = take(4 * q), o_off = take(8 * (q + 1)), o_skip = take(q), o_rexe = take(4 * RP),
-                 o_rlist = take(kind == GP_MINIMAL_FRAGMENTATION ? 8 * RP : 0), o_zone = take(4 * q), o_drv = take(4 * q),
-                 o_exe = take(4 * (T + 1)), o_avg = take(32 * q);
-    const size_t o_eord = take(4 * NE), o_dord = take(4 * ND), o_npos = take(4 * NN), o_fbe = take(4 * NE), o_fbd = take(4 * ND),
-                 o_fbp = take(4 * ND);
-    GP_CUDA(c, c->zonebuf.reserve(o));
-    char* b = c->zonebuf.as<char>();
+    Arena ar{c->zonebuf};
+    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_skip = ar.take(q), o_rexe = ar.take(4 * RP),
+                 o_rlist = ar.take(kind == GP_MINIMAL_FRAGMENTATION ? 8 * RP : 0), o_zone = ar.take(4 * q), o_drv = ar.take(4 * q),
+                 o_exe = ar.take(4 * (T + 1)), o_avg = ar.take(32 * q);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
     int2* unused = nullptr;
     gp_status s = pack_begin(c, Q, GP_TIGHTLY_PACK, mode, total, false, &unused, st);
     if (s != GP_OK) return s;
-    const int64_t* hc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
-    AppColumns cols{};
-    for (int k = 0; k < 6; ++k) {
-        if (!hc[k]) continue;
-        GP_CUDA(c, cudaMemcpyAsync(b + o_in + 8 * q * (size_t)k, hc[k], 8 * q, cudaMemcpyHostToDevice, st));
-        cols.q[k] = b + o_in + 8 * q * (size_t)k;
-    }
-    GP_CUDA(c, cudaMemcpyAsync(b + o_cnt, a->exe_count, 4 * q, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_off, hoff.data(), 8 * (q + 1), cudaMemcpyHostToDevice, st));
+    SixCols six;
+    s = upload_app_columns(c, a, hoff.data(), b, o_in, o_cnt, o_off, st, &six);
+    if (s != GP_OK) return s;
     if (a->skip_if_no_fit) GP_CUDA(c, cudaMemcpyAsync(b + o_skip, a->skip_if_no_fit, q, cudaMemcpyHostToDevice, st));
+    AppColumns cols{};
+    for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
     cols.count = (const int32_t*)(b + o_cnt); cols.group = nullptr; cols.off = (const int64_t*)(b + o_off); cols.bits = 64; cols.mem_shift = 0;
-    int* d_err = c->dev_misc.as<int>();
-    volatile int* err_host = reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48);
-    unsigned long long* d_stats = reinterpret_cast<unsigned long long*>(c->dev_misc.as<char>() + 8);
+    DevStatus* ds = c->status();
+    unsigned long long* d_stats = ds->head.stats;
     PrepApp* prep = c->prep.as<PrepApp>();
     gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
-        Q, cols, a->skip_if_no_fit ? (const uint8_t*)(b + o_skip) : nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, d_err, err_host);
+        Q, cols, a->skip_if_no_fit ? (const uint8_t*)(b + o_skip) : nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep,
+        &ds->head.err, &c->host_status()->err_word);
     Snapshot snap = make_snapshot(c);
     ZoneFifoIn zi{};
     const size_t N = (size_t)c->n_nodes;
@@ -1701,14 +1735,8 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     int32_t* zo = (int32_t*)(b + o_zone); int32_t* dq = (int32_t*)(b + o_drv); int32_t* eo = (int32_t*)(b + o_exe);
     GatherSlots fb{};
     if (azk) {
-        if (NE) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * NE, cudaMemcpyHostToDevice, st));
-        if (ND) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * ND, cudaMemcpyHostToDevice, st));
-        gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)NE, (int32_t)ND, (const int32_t*)(b + o_eord), (const int32_t*)(b + o_dord),
-                                                   c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe),
-                                                   (int32_t*)(b + o_fbd), (int32_t*)(b + o_fbp));
-        c->last.kernel_launches += 1;
-        fb.exec_slot = (const int32_t*)(b + o_fbe); fb.drv_slot = (const int32_t*)(b + o_fbd); fb.drv_pos = (const int32_t*)(b + o_fbp);
-        fb.ne = (int32_t)NE; fb.nd = (int32_t)ND;
+        s = stage_fallback_view(c, az, st, &fb);
+        if (s != GP_OK) return s;
     }
     if (kind == GP_TIGHTLY_PACK) {
         if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
@@ -1722,14 +1750,9 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     }
     GP_CUDA(c, cudaGetLastError());
     c->last.kernel_launches += 2;
-    s = refresh_views(c, false, st);                   // the compact view follows the charged slots
+    s = refresh_views(c, st);                          // the compact view follows the charged slots
     if (s != GP_OK) return s;
-    GP_CUDA(c, cudaMemcpyAsync(out->zone, zo, 4 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaMemcpyAsync(out->driver_node, dq, 4 * q, cudaMemcpyDeviceToHost, st));
-    if (T) GP_CUDA(c, cudaMemcpyAsync(out->executor_nodes, eo, 4 * T, cudaMemcpyDeviceToHost, st));
-    if (avg) GP_CUDA(c, cudaMemcpyAsync(out->avg_efficiency, avg, 32 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    return decode_device_error(c, *reinterpret_cast<volatile int*>(static_cast<char*>(c->pinned_misc) + 48));
+    return finish_zone_results(c, out, zo, dq, eo, avg, q, T, st);
 }
 
 // the FIFO loop with a single-AZ packer in one launch
@@ -1819,21 +1842,15 @@ gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* p
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t q = (size_t)Q, T = (size_t)(total > 0 ? total : 0), R = (size_t)rows;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-    const size_t o_in = take(48 * q), o_cnt = take(4 * q), o_off = take(8 * (q + 1)), o_roff = take(8 * (q + 1)), o_drv = take(4 * q), o_exe = take(4 * (T + 1)),
-                 o_ra = take(4 * (R + 1)), o_rs = take(4 * (R + 1)), o_rn = take(4 * (R + 1)), o_rc = take(8 * (R + 1)), o_rm = take(8 * (R + 1)), o_rg = take(8 * (R + 1));
-    GP_CUDA(c, c->zonebuf.reserve(o));
-    char* b = c->zonebuf.as<char>();
-    const int64_t* hc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
+    Arena ar{c->zonebuf};
+    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_roff = ar.take(8 * (q + 1)), o_drv = ar.take(4 * q),
+                 o_exe = ar.take(4 * (T + 1)), o_ra = ar.take(4 * (R + 1)), o_rs = ar.take(4 * (R + 1)), o_rn = ar.take(4 * (R + 1)),
+                 o_rc = ar.take(8 * (R + 1)), o_rm = ar.take(8 * (R + 1)), o_rg = ar.take(8 * (R + 1));
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
     ReserveIn ri{};
-    for (int k = 0; k < 6; ++k) {
-        if (!hc[k]) continue;
-        GP_CUDA(c, cudaMemcpyAsync(b + o_in + 8 * q * (size_t)k, hc[k], 8 * q, cudaMemcpyHostToDevice, st));
-        ri.cols.p[k] = reinterpret_cast<const int64_t*>(b + o_in + 8 * q * (size_t)k);
-    }
-    GP_CUDA(c, cudaMemcpyAsync(b + o_cnt, a->exe_count, 4 * q, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_off, off.data(), 8 * (q + 1), cudaMemcpyHostToDevice, st));
+    gp_status s = upload_app_columns(c, a, off.data(), b, o_in, o_cnt, o_off, st, &ri.cols);
+    if (s != GP_OK) return s;
     GP_CUDA(c, cudaMemcpyAsync(b + o_roff, roff, 8 * (q + 1), cudaMemcpyHostToDevice, st));
     GP_CUDA(c, cudaMemcpyAsync(b + o_drv, placed->driver_node, 4 * q, cudaMemcpyHostToDevice, st));
     if (T) GP_CUDA(c, cudaMemcpyAsync(b + o_exe, placed->executor_nodes, 4 * T, cudaMemcpyHostToDevice, st));
@@ -1844,7 +1861,7 @@ gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* p
     gp_reserve_rows<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(ri, ro, c->node_slot.as<int32_t>(), c->pair.as<longlong2>(), c->sgpu.as<long long>(),
                                                                         c->node_cpu.as<long long>(), c->node_mem.as<long long>(), c->node_gpu.as<long long>());
     GP_CUDA(c, cudaGetLastError());
-    if (subtract) { gp_status s = refresh_views(c, false, st); if (s != GP_OK) return s; }
+    if (subtract) { s = refresh_views(c, st); if (s != GP_OK) return s; }
     if (out && R) {
         GP_CUDA(c, cudaMemcpyAsync(out->app, ro.app, 4 * R, cudaMemcpyDeviceToHost, st));
         GP_CUDA(c, cudaMemcpyAsync(out->slot, ro.slot, 4 * R, cudaMemcpyDeviceToHost, st));
@@ -1870,9 +1887,10 @@ gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, c
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t R = (size_t)n_rows;
-    GP_CUDA(c, c->zonebuf.reserve(28 * R + 1024));
-    char* b = c->zonebuf.as<char>();
-    const size_t o_c = 0, o_m = 8 * R, o_g = 16 * R, o_n = 24 * R;
+    Arena ar{c->zonebuf};
+    const size_t o_c = ar.take(8 * R), o_m = ar.take(8 * R), o_g = ar.take(8 * R), o_n = ar.take(4 * R);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
     GP_CUDA(c, cudaMemcpyAsync(b + o_c, cpu, 8 * R, cudaMemcpyHostToDevice, st));
     GP_CUDA(c, cudaMemcpyAsync(b + o_m, mem, 8 * R, cudaMemcpyHostToDevice, st));
     if (gpu) GP_CUDA(c, cudaMemcpyAsync(b + o_g, gpu, 8 * R, cudaMemcpyHostToDevice, st));
@@ -1883,7 +1901,7 @@ gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, c
                                                                   c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->node_cpu.as<long long>(),
                                                                   c->node_mem.as<long long>(), c->node_gpu.as<long long>());
     GP_CUDA(c, cudaGetLastError());
-    gp_status s = refresh_views(c, sign < 0, st);
+    gp_status s = refresh_views(c, st);
     if (s != GP_OK) return s;
     GP_CUDA(c, cudaStreamSynchronize(st));
     return GP_OK;
@@ -1897,13 +1915,13 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
                                     long long** d_resched = nullptr) {
     const int32_t n = in->n_nodes;
     const size_t N = (size_t)n, R = (size_t)in->n_reservations;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_alloc = take(24 * N), o_over = take(24 * N), o_usage = take(24 * N + 4 * N), o_avail = take(24 * N), o_sched = take(24 * N),
-                 o_resched = take(24 * N), o_rn = take(4 * R), o_rc = take(8 * R), o_rm = take(8 * R), o_rg = take(8 * R);
+    Arena ar{c->usagebuf};
+    const size_t o_alloc = ar.take(24 * N), o_over = ar.take(24 * N), o_usage = ar.take(24 * N + 4 * N), o_avail = ar.take(24 * N),
+                 o_sched = ar.take(24 * N), o_resched = ar.take(24 * N), o_rn = ar.take(4 * R), o_rc = ar.take(8 * R), o_rm = ar.take(8 * R),
+                 o_rg = ar.take(8 * R);
     const size_t o_has = o_usage + 24 * N;      // zeroed together with the usage sums
-    GP_CUDA(c, c->usagebuf.reserve(off));
-    char* b = c->usagebuf.as<char>();
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
     auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
     GP_CUDA(c, up(o_alloc, in->alloc_cpu_milli, 8 * N));
     GP_CUDA(c, up(o_alloc + 8 * N, in->alloc_mem_bytes, 8 * N));
@@ -1949,15 +1967,15 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
         if (in->name_rank[i] < 0 || in->name_rank[i] >= n) return fail(c, GP_ERR_INVALID, "gp_potential_nodes: name_rank out of range");
     // one scratch block
     const size_t N = (size_t)n, Z = (size_t)in->n_zones;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_cpu = take(8 * N), o_mem = take(8 * N), o_gpu = take(8 * N), o_keys = take(sizeof(SortKey) * N), o_sorted = take(sizeof(SortKey) * N),
-                 o_tot = take(16 * Z), o_zone = take(4 * N), o_nr = take(4 * N), o_prio = take(4 * Z), o_pos = take(4 * N), o_order = take(4 * N),
-                 o_drv = take(4 * N), o_exe = take(4 * N), o_drv2 = take(4 * N), o_exe2 = take(4 * N), o_lrd = take(4 * N),
-                 o_lre = take(4 * N), o_lk = take(sizeof(LabelKey) * N), o_lks = take(sizeof(LabelKey) * N), o_cnt = take(16),
-                 o_fc = take(N), o_fu = take(N), o_fr = take(N);
-    GP_CUDA(c, c->sortbuf.reserve(off));
-    char* b = c->sortbuf.as<char>();
+    Arena ar{c->sortbuf};
+    const size_t o_cpu = ar.take(8 * N), o_mem = ar.take(8 * N), o_gpu = ar.take(8 * N), o_keys = ar.take(sizeof(SortKey) * N),
+                 o_sorted = ar.take(sizeof(SortKey) * N), o_tot = ar.take(16 * Z), o_zone = ar.take(4 * N), o_nr = ar.take(4 * N),
+                 o_prio = ar.take(4 * Z), o_pos = ar.take(4 * N), o_order = ar.take(4 * N), o_drv = ar.take(4 * N), o_exe = ar.take(4 * N),
+                 o_drv2 = ar.take(4 * N), o_exe2 = ar.take(4 * N), o_lrd = ar.take(4 * N), o_lre = ar.take(4 * N),
+                 o_lk = ar.take(sizeof(LabelKey) * N), o_lks = ar.take(sizeof(LabelKey) * N), o_cnt = ar.take(16),
+                 o_fc = ar.take(N), o_fu = ar.take(N), o_fr = ar.take(N);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
     auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
     if (!d_cpu) { GP_CUDA(c, up(o_cpu, in->avail_cpu_milli, 8 * N)); d_cpu = (const long long*)(b + o_cpu); }
     if (!d_mem) { GP_CUDA(c, up(o_mem, in->avail_mem_bytes, 8 * N)); d_mem = (const long long*)(b + o_mem); }
@@ -2172,12 +2190,12 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
     }
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
-    // one staging buffer: [exe 3q i64 | reserved 3N i64 | host_off (q+1) i64 | group q i32 | host_nodes H i32 | out q i32 | err i32]
     const size_t Q = (size_t)q, N = (size_t)c->n_nodes, H = (size_t)hosted;
-    const size_t o_exe = 0, o_res = o_exe + 8 * 3 * Q, o_hoff = o_res + 8 * 3 * N, o_grp = o_hoff + 8 * (Q + 1),
-                 o_hn = o_grp + 4 * Q, o_out = o_hn + 4 * (H + 1), o_err = o_out + 4 * Q, total = o_err + 8;
-    GP_CUDA(c, c->reschedbuf.reserve(total));
-    char* base = c->reschedbuf.as<char>();
+    Arena ar{c->reschedbuf};
+    const size_t o_exe = ar.take(8 * 3 * Q), o_res = ar.take(8 * 3 * N), o_hoff = ar.take(8 * (Q + 1)), o_grp = ar.take(4 * Q),
+                 o_hn = ar.take(4 * (H + 1)), o_out = ar.take(4 * Q), o_err = ar.take(8);
+    GP_CUDA(c, ar.reserve());
+    char* base = ar.base();
     int64_t* d_exe = reinterpret_cast<int64_t*>(base + o_exe);
     int64_t* d_res = reinterpret_cast<int64_t*>(base + o_res);
     int64_t* d_hoff = reinterpret_cast<int64_t*>(base + o_hoff);
