@@ -235,6 +235,38 @@ gp_status gp_potential_nodes(gp_ctx* ctx, const gp_sort_input* in,
 gp_status gp_prepare_cluster(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort,
                              int32_t* n_driver /* may be NULL */, int32_t* n_executor /* may be NULL */);
 
+/* The same chain for the zone-aware packers (SURVEY 8f rows f1/f2/f3): gp_prepare_cluster's availability and priority orders
+ * (label re-sort and undefined_ties included), then both orders grouped by sort->zone_id on the device -- groupNodesByZone
+ * (LIB/binpack/single_az.go:57-73).  Candidate zones have at least one driver and one executor candidate (:36-41); they are
+ * ordered by the first position at which each appears in the driver order AFTER the label re-sort (driverZonesInOrder), and
+ * each group's orders are the undivided orders restricted to that zone.  zone_id NULL or n_zones == 1: one zone.
+ *   GP_LAYOUT_SINGLE_AZ  the groups are the candidate zones, every other node is dropped; no candidate zone = ONE empty group
+ *                        (every gp_pack_*_zones result is then zone -1, the EmptyPackingResult of :31-33).  For
+ *                        gp_pack_batch_zones / gp_pack_fifo_zones.
+ *   GP_LAYOUT_AZ_AWARE   the candidate zones, then one trailing group with every other node of either order in undivided order
+ *                        (present when non-empty or when no zone is a candidate): the layout of gp_pack_fifo_az_aware /
+ *                        gp_pack_batch_az_aware, which then take orders == NULL to mean the undivided orders and n_zones this
+ *                        call left on the device (az_aware_pack_tightly.go:27-38).
+ * SchedulableResources (allocatable - overhead) are kept as if gp_set_schedulable had been called with them, and gp_get_snapshot
+ * works as after gp_prepare_cluster.  The layout stays valid across FIFO calls, gp_reserve_placements and gp_apply_usage_delta
+ * (they change availability, not orders); gp_set_snapshot, gp_set_snapshot_device, gp_prepare_cluster or another
+ * gp_prepare_cluster_zones replaces it.  One stream synchronise for the counts; the optional arrays cost one more copy. */
+typedef enum { GP_LAYOUT_SINGLE_AZ = 0, GP_LAYOUT_AZ_AWARE = 1 } gp_zone_layout_kind;
+typedef struct {
+    int32_t kind;              /* in: gp_zone_layout_kind */
+    int32_t n_zones;           /* out: candidate zones = instance groups 0..n_zones-1, in driverZonesInOrder order */
+    int32_t n_groups;          /* out: instance groups of the snapshot laid out */
+    int32_t n_driver;          /* out: length of the undivided driver order (PotentialNodes' driverNodes) */
+    int32_t n_executor;        /* out: length of the undivided executor order */
+    int32_t reserved;
+    int32_t* zone_of_group;    /* out, or NULL: [sort->n_zones + 1] zone id of each group, -1 = trailing / empty group */
+    int32_t* exec_off;         /* out, or NULL: [n_groups + 1]   } the grouped layout as gp_nodes would carry it; */
+    int32_t* exec_order;       /* out, or NULL: [n_nodes]        } copied back only when asked (logging, tests)  */
+    int32_t* drv_off;          /* out, or NULL: [n_groups + 1] */
+    int32_t* drv_order;        /* out, or NULL: [n_nodes] */
+} gp_zone_layout;
+gp_status gp_prepare_cluster_zones(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout);
+
 /* ---- executors without a usable reservation (the step after the hot path; SURVEY 8f row f4) --- */
 /* rescheduleExecutor's node choice (internal/extender/resource.go:594-673) for a BATCH of executor pods, every
  * decision independent against the current snapshot (its executor priority orders and availabilities):
@@ -377,7 +409,9 @@ gp_status gp_pack_fifo_zones(gp_ctx* ctx, const gp_apps* apps /* group ignored *
  * GP_ERR_INVALID (gp_last_error names the cause): an independent mode; n_zones above 64 or above n_groups; no
  * gp_set_schedulable; a snapshot from gp_set_snapshot_device / gp_prepare_cluster (no host copy to check the orders
  * against); order lengths other than exec_off[n_groups] / drv_off[n_groups]; an order entry out of range, repeated or not
- * listed by the snapshot in that role; a zone group whose order is not the undivided order restricted to its nodes. */
+ * listed by the snapshot in that role; a zone group whose order is not the undivided order restricted to its nodes.
+ * orders == NULL: right after gp_prepare_cluster_zones(GP_LAYOUT_AZ_AWARE) only -- the undivided orders and n_zones that call
+ * left on the device (more than 64 candidate zones: GP_ERR_INVALID as above); after any other snapshot GP_ERR_INVALID. */
 typedef struct {
     int32_t n_zones;                 /* snapshot groups 0..n_zones-1 are the candidate zones (0..64 under FIFO, 0..n_groups
                                         for gp_pack_batch_az_aware) */
@@ -403,7 +437,7 @@ gp_status gp_pack_fifo_az_aware(gp_ctx* ctx, const gp_apps* apps /* group ignore
  * NULL or given, as in gp_pack_batch_zones; exe_count up to 2^24.
  * gp_stats: scan_path_apps = applications for which the fallback ran; nodes_scanned / drivers_tried include its scans.
  * GP_ERR_INVALID (gp_last_error names the cause): those of gp_pack_fifo_az_aware except the mode and the 64-zone bound
- * (n_zones negative or above n_groups). */
+ * (n_zones negative or above n_groups).  orders == NULL as in gp_pack_fifo_az_aware, without the 64-zone bound. */
 gp_status gp_pack_batch_az_aware(gp_ctx* ctx, const gp_apps* apps /* group, skip_if_no_fit ignored */, const gp_az_orders* orders,
                                  gp_zone_results* out);
 

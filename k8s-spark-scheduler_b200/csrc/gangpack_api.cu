@@ -9,6 +9,7 @@
 #include "gangpack_zonefifo.cuh"
 #include "gangpack_resched.cuh"
 #include "gangpack_sort.cuh"
+#include "gangpack_zonelayout.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -445,6 +446,12 @@ struct gp_ctx {
     DevBuf sched, zonebuf, fbview;                // SchedulableResources [3][n_nodes]; staging of the zone entry points;
                                                   // the az-aware fallback's orders and gather view
     bool have_sched = false;
+    // gp_prepare_cluster_zones: the undivided orders it sorted (in zoneprep, which also holds that call's scratch), their
+    // lengths and n_zones as DEVICE pointers for gp_pack_*_az_aware(orders == NULL); zone_kind = the gp_zone_layout_kind of the
+    // current snapshot, -1 when another entry laid it out
+    DevBuf zoneprep;
+    int zone_kind = -1;
+    gp_az_orders zone_orders{};
     bool sort_attr_set = false;
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
 
@@ -672,6 +679,7 @@ static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_
                                        bool copy_nodes = false) {
     const int32_t n_slots = n_exec + n_drv;
     c->host_layout = false;              // gp_set_snapshot sets it again once the layout it validated is in place
+    c->zone_kind = -1;                   // gp_prepare_cluster_zones sets it again once its layout is in place
     GP_CUDA(c, c->pair.reserve(sizeof(longlong2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->pair32.reserve(sizeof(uint2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->sgpu.reserve(sizeof(int64_t) * (size_t)(n_slots + 1)));
@@ -1478,17 +1486,20 @@ static gp_status upload_app_columns(gp_ctx* c, const gp_apps* a, const int64_t* 
     return GP_OK;
 }
 
-// az-aware-tightly-pack: upload the undivided orders and build the fallback's gather view of them (gp_build_fallback_view)
-static gp_status stage_fallback_view(gp_ctx* c, const gp_az_orders* az, cudaStream_t st, GatherSlots* fb) {
+// az-aware-tightly-pack: upload the undivided orders and build the fallback's gather view of them (gp_build_fallback_view).
+// on_device: az's orders are device arrays (gp_prepare_cluster_zones' held orders) and are read in place.
+static gp_status stage_fallback_view(gp_ctx* c, const gp_az_orders* az, bool on_device, cudaStream_t st, GatherSlots* fb) {
     const size_t ne = (size_t)az->n_exec, nd = (size_t)az->n_drv;
     Arena ar{c->fbview};
-    const size_t o_eord = ar.take(4 * ne), o_dord = ar.take(4 * nd), o_npos = ar.take(4 * (size_t)c->n_nodes), o_fbe = ar.take(4 * ne),
-                 o_fbd = ar.take(4 * nd), o_fbp = ar.take(4 * nd);
+    const size_t o_eord = ar.take(on_device ? 0 : 4 * ne), o_dord = ar.take(on_device ? 0 : 4 * nd), o_npos = ar.take(4 * (size_t)c->n_nodes),
+                 o_fbe = ar.take(4 * ne), o_fbd = ar.take(4 * nd), o_fbp = ar.take(4 * nd);
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
-    if (ne) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * ne, cudaMemcpyHostToDevice, st));
-    if (nd) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * nd, cudaMemcpyHostToDevice, st));
-    gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)ne, (int32_t)nd, (const int32_t*)(b + o_eord), (const int32_t*)(b + o_dord),
+    const int32_t* eord = on_device ? az->exec_order : (const int32_t*)(b + o_eord);
+    const int32_t* dord = on_device ? az->drv_order : (const int32_t*)(b + o_dord);
+    if (!on_device && ne) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * ne, cudaMemcpyHostToDevice, st));
+    if (!on_device && nd) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * nd, cudaMemcpyHostToDevice, st));
+    gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)ne, (int32_t)nd, eord, dord,
                                                c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe), (int32_t*)(b + o_fbd),
                                                (int32_t*)(b + o_fbp));
     c->last.kernel_launches += 1;
@@ -1509,9 +1520,9 @@ static gp_status finish_zone_results(gp_ctx* c, gp_zone_results* out, const int3
 
 // Independent zone packs of a batch, shared by gp_pack_batch_zones (the zones are every instance group, no fallback) and
 // gp_pack_batch_az_aware (zones 0..Z-1 with tightly-pack, plus the undivided orders `az` of the fallback, already
-// validated).  Argument checks common to both are here.
-static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int32_t Z, const gp_az_orders* az, gp_zone_results* out,
-                                 const char* who) {
+// validated; az_dev: they are device arrays).  Argument checks common to both are here.
+static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int32_t Z, const gp_az_orders* az, bool az_dev,
+                                 gp_zone_results* out, const char* who) {
     const std::string w(who);
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
@@ -1590,7 +1601,7 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
         gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
             Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, &ds->head.err, &c->host_status()->err_word);
         GatherSlots fb;
-        s = stage_fallback_view(c, az, st, &fb);
+        s = stage_fallback_view(c, az, az_dev, st, &fb);
         if (s != GP_OK) return s;
         int& per_sm = c->az_fallback_ctas_per_sm;
         if (per_sm == 0) {
@@ -1615,7 +1626,7 @@ gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: NULL apps/results");
     if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
         return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: the single-AZ packers are tightly-pack and minimal-fragmentation (single_az_pack_tightly.go, single_az_minimal_fragmentation.go)");
-    return batch_zones_run(c, a, algo, c->n_groups, nullptr, out, "gp_pack_batch_zones");
+    return batch_zones_run(c, a, algo, c->n_groups, nullptr, false, out, "gp_pack_batch_zones");
 }
 
 // ---- reservation table + device-resident snapshot upkeep (gangpack_zones.cuh) -------------------------------------------
@@ -1672,10 +1683,23 @@ static gp_status check_az_orders(gp_ctx* c, const gp_az_orders* o, const char* w
     return GP_OK;
 }
 
+// The az-aware entries' NULL arguments.  orders == NULL stands for the undivided orders and n_zones gp_prepare_cluster_zones
+// (GP_LAYOUT_AZ_AWARE) left on the device -- *o then points at them; after any other snapshot it is refused.
+static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_results* out, const gp_az_orders** o, const char* who) {
+    const std::string w(who);
+    if (!*o && c->zone_kind == GP_LAYOUT_SINGLE_AZ)
+        return fail(c, GP_ERR_INVALID, w + ": orders == NULL needs a gp_prepare_cluster_zones(GP_LAYOUT_AZ_AWARE) snapshot; this one is "
+                                           "GP_LAYOUT_SINGLE_AZ (no trailing group, no undivided orders)");
+    if (!a || !out || (!*o && c->zone_kind != GP_LAYOUT_AZ_AWARE) || a->n_apps < 0) return fail(c, GP_ERR_INVALID, w + ": NULL apps/orders/results");
+    if (!*o) *o = &c->zone_orders;
+    return GP_OK;
+}
+
 // The FIFO loop over zones in one launch (gangpack_zonefifo.cuh), shared by gp_pack_fifo_zones (kind = 0 tightly-pack,
 // 2 minimal-fragmentation; the zones are every instance group) and gp_pack_fifo_az_aware (kind = kZoneAzAware; zones
-// 0..Z-1, plus the undivided orders `az` of the fallback, already validated).  Argument checks common to both are here.
-static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, int32_t Z, const gp_az_orders* az,
+// 0..Z-1, plus the undivided orders `az` of the fallback, already validated; az_dev: they are device arrays).  Argument
+// checks common to both are here.
+static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, int32_t Z, const gp_az_orders* az, bool az_dev,
                                 gp_zone_results* out, const char* who) {
     const std::string w(who);
     const int32_t Q = a->n_apps;
@@ -1735,7 +1759,7 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     int32_t* zo = (int32_t*)(b + o_zone); int32_t* dq = (int32_t*)(b + o_drv); int32_t* eo = (int32_t*)(b + o_exe);
     GatherSlots fb{};
     if (azk) {
-        s = stage_fallback_view(c, az, st, &fb);
+        s = stage_fallback_view(c, az, az_dev, st, &fb);
         if (s != GP_OK) return s;
     }
     if (kind == GP_TIGHTLY_PACK) {
@@ -1767,7 +1791,7 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones)");
     const int32_t Z = c->n_groups;
     if (Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
-    return fifo_zones_run(c, a, (int)algo, mode, Z, nullptr, out, "gp_pack_fifo_zones");
+    return fifo_zones_run(c, a, (int)algo, mode, Z, nullptr, false, out, "gp_pack_fifo_zones");
 }
 
 // the FIFO loop with az-aware-tightly-pack in one launch: the zone packs plus the undivided fallback on the device
@@ -1778,13 +1802,15 @@ gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones, "
                                        "then gp_pack_batch over the undivided orders)");
     if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
-    if (!a || !out || !o || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: NULL apps/orders/results");
+    gp_status s = held_az_orders(c, a, out, &o, "gp_pack_fifo_az_aware");
+    if (s != GP_OK) return s;
+    const bool held = o == &c->zone_orders;
     const int32_t Z = o->n_zones;
     if (Z < 0 || Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones must be 0..64");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones exceeds the snapshot's instance groups");
-    gp_status s = check_az_orders(c, o, "gp_pack_fifo_az_aware");
+    if (!held) s = check_az_orders(c, o, "gp_pack_fifo_az_aware");
     if (s != GP_OK) return s;
-    return fifo_zones_run(c, a, kZoneAzAware, mode, Z, o, out, "gp_pack_fifo_az_aware");
+    return fifo_zones_run(c, a, kZoneAzAware, mode, Z, o, held, out, "gp_pack_fifo_az_aware");
 }
 
 // az-aware-tightly-pack for a batch of independent decisions: the zone packs, the zone choice and the undivided fallback
@@ -1793,13 +1819,15 @@ gp_status gp_pack_batch_az_aware(gp_ctx* c, const gp_apps* a, const gp_az_orders
     if (!c) return GP_ERR_INVALID;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_az_aware: gp_set_snapshot first");
     if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
-    if (!a || !out || !o || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: NULL apps/orders/results");
+    gp_status s = held_az_orders(c, a, out, &o, "gp_pack_batch_az_aware");
+    if (s != GP_OK) return s;
+    const bool held = o == &c->zone_orders;
     const int32_t Z = o->n_zones;
     if (Z < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones is negative");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones exceeds the snapshot's instance groups");
-    gp_status s = check_az_orders(c, o, "gp_pack_batch_az_aware");
+    if (!held) s = check_az_orders(c, o, "gp_pack_batch_az_aware");
     if (s != GP_OK) return s;
-    return batch_zones_run(c, a, GP_TIGHTLY_PACK, Z, o, out, "gp_pack_batch_az_aware");
+    return batch_zones_run(c, a, GP_TIGHTLY_PACK, Z, o, held, out, "gp_pack_batch_az_aware");
 }
 
 gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* placed, int32_t subtract, gp_reservation_table* out) {
@@ -1953,10 +1981,23 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
     return GP_OK;
 }
 
-struct SortStage { const int32_t* drv; const int32_t* exe; const int32_t* counts; };
+struct SortStage { const int32_t* drv; const int32_t* exe; const int32_t* counts; const int32_t* zone; };
 
-// f1 stage: d_cpu / d_mem / d_gpu are device arrays (NULL: uploaded from `in`; gpu optional); leaves the two orders and
-// counts[3] = {#driver candidates, #executor candidates, #undefined ties} on the device.
+// Stable re-sort of list[0..*cnt) by rank[node] (-1 last): out[k] = the k-th node in (rank, position) order.  The label
+// re-sort of PotentialNodes, and the zone partition of gp_prepare_cluster_zones.
+static void launch_label_resort(int32_t n, const int32_t* cnt, const int32_t* list, const int32_t* rank, LabelKey* lk, LabelKey* lks,
+                                int32_t* pos, int32_t* out, cudaStream_t st) {
+    const int T = 256;
+    const int nb = (n + T - 1) / T;
+    const int ntile = (n + kSortTile - 1) / kSortTile;
+    gp_label_keys<<<nb, T, 0, st>>>(cnt, list, rank, lk);
+    gp_sort_tiles<LabelKey><<<ntile, kSortThreads, kSortTile * sizeof(LabelKey), st>>>(n, cnt, lk, lks);
+    gp_rank_by_search<LabelKey><<<nb, T, 0, st>>>(n, cnt, lk, lks, pos);
+    gp_label_scatter<<<nb, T, 0, st>>>(cnt, list, pos, out);
+}
+
+// f1 stage: d_cpu / d_mem / d_gpu are device arrays (NULL: uploaded from `in`; gpu optional); leaves the two orders,
+// counts[3] = {#driver candidates, #executor candidates, #undefined ties} and the zone ids (NULL: one zone) on the device.
 static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long* d_cpu, const long long* d_mem, const long long* d_gpu,
                             cudaStream_t st, SortStage* out) {
     const int32_t n = in->n_nodes;
@@ -2014,13 +2055,10 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
     out->drv = (const int32_t*)(b + o_drv);
     out->exe = (const int32_t*)(b + o_exe);
     out->counts = (const int32_t*)(b + o_cnt);
+    out->zone = zoned ? (const int32_t*)(b + o_zone) : nullptr;
     auto label_sort = [&](const int32_t* cnt, const int32_t* list, size_t o_rank, size_t o_out) {
-        LabelKey* lk = (LabelKey*)(b + o_lk);
-        LabelKey* lks = (LabelKey*)(b + o_lks);
-        gp_label_keys<<<nb, T, 0, st>>>(cnt, list, (const int32_t*)(b + o_rank), lk);
-        gp_sort_tiles<LabelKey><<<ntile, kSortThreads, kSortTile * sizeof(LabelKey), st>>>(n, cnt, lk, lks);
-        gp_rank_by_search<LabelKey><<<nb, T, 0, st>>>(n, cnt, lk, lks, pos);
-        gp_label_scatter<<<nb, T, 0, st>>>(cnt, list, pos, (int32_t*)(b + o_out));
+        launch_label_resort(n, cnt, list, (const int32_t*)(b + o_rank), (LabelKey*)(b + o_lk), (LabelKey*)(b + o_lks), pos,
+                            (int32_t*)(b + o_out), st);
         return (const int32_t*)(b + o_out);
     };
     if (in->driver_label_rank) out->drv = label_sort(out->counts, out->drv, o_lrd, o_drv2);
@@ -2146,6 +2184,108 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
     if (sort->undefined_ties) *sort->undefined_ties = counts[2];
     if (n_driver) *n_driver = counts[0];
     if (n_executor) *n_executor = counts[1];
+    return GP_OK;
+}
+
+// reservations -> availability -> priority orders -> zone-grouped slot layout, without leaving the device
+gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout) {
+    if (!c) return GP_ERR_INVALID;
+    if (!usage || !sort || !layout || usage->n_nodes != sort->n_nodes || usage->n_nodes < 0 || sort->n_zones < 1 || usage->n_reservations < 0 ||
+        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes)) ||
+        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)))
+        return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: missing arrays or mismatched sizes");
+    const int32_t kind = layout->kind;
+    if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
+        return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: layout->kind must be GP_LAYOUT_SINGLE_AZ or GP_LAYOUT_AZ_AWARE");
+    if (sort->n_zones == 0x7fffffff) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: n_zones too large");
+    const int32_t n = usage->n_nodes;
+    layout->n_zones = 0; layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
+    if (n == 0) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: empty node table");
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    c->zone_kind = -1;                                  // the held orders are overwritten below
+    long long *d_avail = nullptr, *d_sched = nullptr;
+    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched);
+    if (s != GP_OK) return s;
+    const size_t N = (size_t)n;
+    SortStage so{};
+    s = stage_sort(c, sort, d_avail, d_avail + N, d_avail + 2 * N, st, &so);
+    if (s != GP_OK) return s;
+    // g_bound = sort->n_zones + 1 groups bound every layout; the slots are laid out for that many (the groups past the
+    // last one are empty) so that the group count can stay on the device until the one synchronise below
+    const size_t Zs = (size_t)sort->n_zones;
+    const int32_t g_bound = sort->n_zones + 1;
+    Arena ar{c->zoneprep};
+    const size_t o_udrv = ar.take(4 * N), o_uexe = ar.take(4 * N), o_first = ar.take(4 * Zs), o_has = ar.take(Zs), o_zg = ar.take(4 * Zs),
+                 o_zog = ar.take(4 * (Zs + 1)), o_rank = ar.take(4 * N), o_lk = ar.take(sizeof(LabelKey) * N), o_lks = ar.take(sizeof(LabelKey) * N),
+                 o_pos = ar.take(4 * N), o_info = ar.take(4 * kZiWords);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    int32_t* udrv = (int32_t*)(b + o_udrv);
+    int32_t* uexe = (int32_t*)(b + o_uexe);
+    int32_t* info = (int32_t*)(b + o_info);
+    int32_t* rank = (int32_t*)(b + o_rank);
+    // the undivided orders outlive the sort's scratch, which the next gp_potential_nodes / gp_prepare_cluster reuses
+    GP_CUDA(c, cudaMemcpyAsync(udrv, so.drv, 4 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(uexe, so.exe, 4 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_first, 0x7f, 4 * Zs, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_has, 0, Zs, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_zg, 0xff, 4 * Zs, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_zog, 0xff, 4 * (Zs + 1), st));
+    GP_CUDA(c, cudaMemsetAsync(info, 0, 4 * kZiWords, st));
+    const int T = 256;
+    const int nb = (n + T - 1) / T;
+    const int32_t az = kind == GP_LAYOUT_AZ_AWARE ? 1 : 0;
+    gp_zone_mark<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, (int32_t*)(b + o_first), (uint8_t*)(b + o_has));
+    gp_zone_candidates<<<1, 1024, 0, st>>>(so.counts, udrv, so.zone, (const int32_t*)(b + o_first), (const uint8_t*)(b + o_has),
+                                           (int32_t*)(b + o_zg), (int32_t*)(b + o_zog), info);
+    gp_group_rank<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, (const int32_t*)(b + o_zg), az, info, rank);
+    GP_CUDA(c, cudaGetLastError());
+    // node-table copy (gp_get_snapshot), the grouped orders and their offsets, then the usual slot layout
+    const size_t nbytes = sizeof(int64_t) * (N + 1);
+    GP_CUDA(c, c->node_cpu.reserve(nbytes)); GP_CUDA(c, c->node_mem.reserve(nbytes)); GP_CUDA(c, c->node_gpu.reserve(nbytes));
+    GP_CUDA(c, cudaMemcpyAsync(c->node_cpu.p, d_avail, 8 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(c->node_mem.p, d_avail + N, 8 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(c->node_gpu.p, d_avail + 2 * N, 8 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, c->exec_order.reserve(4 * (N + 1))); GP_CUDA(c, c->drv_order.reserve(4 * (N + 1)));
+    GP_CUDA(c, c->exec_off.reserve(4 * ((size_t)g_bound + 1))); GP_CUDA(c, c->drv_off.reserve(4 * ((size_t)g_bound + 1)));
+    LabelKey* lk = (LabelKey*)(b + o_lk);
+    LabelKey* lks = (LabelKey*)(b + o_lks);
+    int32_t* pos = (int32_t*)(b + o_pos);
+    launch_label_resort(n, so.counts, udrv, rank, lk, lks, pos, c->drv_order.as<int32_t>(), st);
+    launch_label_resort(n, so.counts + 1, uexe, rank, lk, lks, pos, c->exec_order.as<int32_t>(), st);
+    gp_group_offsets<<<(unsigned)((g_bound + T) / T), T, 0, st>>>(g_bound, so.counts, c->drv_order.as<int32_t>(), c->exec_order.as<int32_t>(),
+                                                                  rank, az, c->exec_off.as<int32_t>(), c->drv_off.as<int32_t>(), info);
+    GP_CUDA(c, cudaGetLastError());
+    gp_nodes dn{};
+    dn.n_nodes = n;
+    dn.avail_cpu_milli = c->node_cpu.as<int64_t>(); dn.avail_mem_bytes = c->node_mem.as<int64_t>(); dn.avail_gpu = c->node_gpu.as<int64_t>();
+    dn.n_groups = g_bound;
+    dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = c->exec_order.as<int32_t>();
+    dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = c->drv_order.as<int32_t>();
+    s = build_snapshot_device(c, &dn, n, n, st);      // n bounds both order lengths
+    if (s != GP_OK) return s;
+    GP_CUDA(c, c->sched.reserve(24 * (N + 1)));
+    GP_CUDA(c, cudaMemcpyAsync(c->sched.p, d_sched, 24 * N, cudaMemcpyDeviceToDevice, st));
+    int32_t counts[3] = {0, 0, 0}, hinfo[kZiWords] = {};
+    GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaMemcpyAsync(hinfo, info, sizeof(hinfo), cudaMemcpyDeviceToHost, st));
+    if (layout->zone_of_group) GP_CUDA(c, cudaMemcpyAsync(layout->zone_of_group, b + o_zog, 4 * (Zs + 1), cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    c->n_groups = hinfo[kZiGroups]; c->n_exec = hinfo[kZiExec]; c->n_drv = hinfo[kZiDrv];
+    c->have_sched = true;
+    c->zone_orders = gp_az_orders{hinfo[kZiZones], counts[1], uexe, counts[0], udrv};
+    c->zone_kind = kind;
+    if (sort->undefined_ties) *sort->undefined_ties = counts[2];
+    layout->n_zones = hinfo[kZiZones]; layout->n_groups = hinfo[kZiGroups];
+    layout->n_driver = counts[0]; layout->n_executor = counts[1];
+    // the grouped layout itself only when asked: its sizes are known now
+    const size_t ob = 4 * (size_t)(hinfo[kZiGroups] + 1);
+    if (layout->exec_off) GP_CUDA(c, cudaMemcpyAsync(layout->exec_off, c->exec_off.p, ob, cudaMemcpyDeviceToHost, st));
+    if (layout->drv_off) GP_CUDA(c, cudaMemcpyAsync(layout->drv_off, c->drv_off.p, ob, cudaMemcpyDeviceToHost, st));
+    if (layout->exec_order && c->n_exec) GP_CUDA(c, cudaMemcpyAsync(layout->exec_order, c->exec_order.p, 4 * (size_t)c->n_exec, cudaMemcpyDeviceToHost, st));
+    if (layout->drv_order && c->n_drv) GP_CUDA(c, cudaMemcpyAsync(layout->drv_order, c->drv_order.p, 4 * (size_t)c->n_drv, cudaMemcpyDeviceToHost, st));
+    if (layout->exec_off || layout->drv_off || layout->exec_order || layout->drv_order) GP_CUDA(c, cudaStreamSynchronize(st));
     return GP_OK;
 }
 

@@ -17,7 +17,7 @@ _ROOT = os.path.dirname(_PKG)
 LIB_PATH = os.environ.get("GANGPACK_LIB") or os.path.join(_PKG, "libgangpack.so")   # GANGPACK_LIB: experimental builds
 _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack_kernels.cuh", "gangpack_fifo.cuh", "gangpack_minfrag.cuh",
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
-                                                    "gangpack_zones.cuh", "gangpack_zonefifo.cuh")] + [
+                                                    "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -37,7 +37,8 @@ STATUS_NAMES = {0: "GP_OK", 1: "GP_ERR_INVALID", 2: "GP_ERR_CUDA", 3: "GP_ERR_NO
 EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_backend", "gp_alloc_pinned",
            "gp_free_pinned", "gp_register_host", "gp_unregister_host", "gp_set_snapshot", "gp_get_snapshot", "gp_pack_batch", "gp_pack_batch_wire", "gp_pack_one", "gp_set_schedulable", "gp_pack_batch_zones", "gp_pack_fifo_zones", "gp_pack_fifo_az_aware", "gp_pack_batch_az_aware", "gp_reserve_placements", "gp_apply_usage_delta",
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
-           "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_reschedule_executors",
+           "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
+           "gp_reschedule_executors",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -134,6 +135,16 @@ class gp_usage_input(C.Structure):
                 ("res_mem_bytes", C.c_void_p), ("res_gpu", C.c_void_p)]
 
 
+LAYOUT_SINGLE_AZ = 0
+LAYOUT_AZ_AWARE = 1
+
+
+class gp_zone_layout(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("n_zones", C.c_int32), ("n_groups", C.c_int32), ("n_driver", C.c_int32),
+                ("n_executor", C.c_int32), ("reserved", C.c_int32), ("zone_of_group", C.c_void_p), ("exec_off", C.c_void_p),
+                ("exec_order", C.c_void_p), ("drv_off", C.c_void_p), ("drv_order", C.c_void_p)]
+
+
 class gp_reschedule(C.Structure):
     _fields_ = [("n_execs", C.c_int32), ("exe_cpu_milli", C.c_void_p), ("exe_mem_bytes", C.c_void_p), ("exe_gpu", C.c_void_p),
                 ("group", C.c_void_p), ("min_frag", C.c_int32), ("reserved_cpu_milli", C.c_void_p),
@@ -218,6 +229,8 @@ def load():
     L.gp_prepare_cluster.restype = C.c_int
     L.gp_prepare_cluster.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input), C.POINTER(C.c_int32),
                                      C.POINTER(C.c_int32)]
+    L.gp_prepare_cluster_zones.restype = C.c_int
+    L.gp_prepare_cluster_zones.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input), C.POINTER(gp_zone_layout)]
     L.gp_potential_nodes.restype = C.c_int
     L.gp_potential_nodes.argtypes = [C.c_void_p, C.POINTER(gp_sort_input), C.c_void_p, C.POINTER(C.c_int32),
                                      C.c_void_p, C.POINTER(C.c_int32)]
@@ -251,6 +264,16 @@ def _np(a, dtype):
 
 def _p(a):
     return None if a is None else a.ctypes.data
+
+
+def _az_orders(exec_order, drv_order, n_zones):
+    """-> (pointer argument, kept arrays): a gp_az_orders, or NULL when all three are None (the orders
+    prepare_cluster_zones(LAYOUT_AZ_AWARE) left on the device)."""
+    if exec_order is None and drv_order is None and n_zones is None:
+        return None, None
+    eo, do = _np(exec_order, np.int32), _np(drv_order, np.int32)
+    o = gp_az_orders(n_zones=int(n_zones), n_exec=len(eo), exec_order=_p(eo), n_drv=len(do), drv_order=_p(do))
+    return C.byref(o), (o, eo, do)
 
 
 def compact_apps(apps: dict, mem_shift: int = 20):
@@ -437,6 +460,40 @@ class GangPacker:
         self.n_nodes = n
         return nd.value, ne.value
 
+    def prepare_cluster_zones(self, alloc, overhead, res_node, res, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
+                              unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None, kind=LAYOUT_AZ_AWARE,
+                              layout=True):
+        """reservations -> availability -> priority orders -> zone-grouped snapshot (kind LAYOUT_SINGLE_AZ or LAYOUT_AZ_AWARE),
+        chained on the device, SchedulableResources included.  -> dict with n_zones, n_groups, n_driver, n_executor,
+        zone_of_group, undefined_ties and, with `layout`, the grouped exec_off / exec_order / drv_off / drv_order."""
+        al = [_np(x, np.int64) for x in alloc]
+        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
+        rn = _np(res_node, np.int32)
+        rs = [_np(x, np.int64) for x in res]
+        n = len(al[0])
+        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
+                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
+                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
+        arrs = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(is_driver_candidate, np.uint8), _np(unschedulable, np.uint8),
+                _np(ready, np.uint8), _np(driver_label_rank, np.int32), _np(executor_label_rank, np.int32)]
+        ties = C.c_int32(0)
+        si = gp_sort_input(n_nodes=n, avail_cpu_milli=None, avail_mem_bytes=None, n_zones=n_zones, zone_id=_p(arrs[0]),
+                           name_rank=_p(arrs[1]), is_driver_candidate=_p(arrs[2]), unschedulable=_p(arrs[3]), ready=_p(arrs[4]),
+                           driver_label_rank=_p(arrs[5]), executor_label_rank=_p(arrs[6]), undefined_ties=C.addressof(ties))
+        zog = np.full(n_zones + 1, -9, np.int32)
+        bufs = {k: np.full(max(n, 1) if k.endswith("order") else n_zones + 2, -9, np.int32)
+                for k in ("exec_off", "exec_order", "drv_off", "drv_order")} if layout else {}
+        lo = gp_zone_layout(kind=int(kind), zone_of_group=_p(zog), **{k: _p(v) for k, v in bufs.items()})
+        self._check(load().gp_prepare_cluster_zones(self._h, C.byref(ui), C.byref(si), C.byref(lo)))
+        self.n_nodes = n
+        out = dict(n_zones=lo.n_zones, n_groups=lo.n_groups, n_driver=lo.n_driver, n_executor=lo.n_executor, zone_of_group=zog,
+                   undefined_ties=ties.value)
+        if layout:
+            G = lo.n_groups
+            out.update(exec_off=bufs["exec_off"][:G + 1].copy(), drv_off=bufs["drv_off"][:G + 1].copy())
+            out.update(exec_order=bufs["exec_order"][:out["exec_off"][G]].copy(), drv_order=bufs["drv_order"][:out["drv_off"][G]].copy())
+        return out
+
     # ---- node priority order (NodeSorter.PotentialNodes) ---------------------------------------
     def potential_nodes(self, avail_cpu, avail_mem, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None, avail_gpu=None):
@@ -550,48 +607,47 @@ class GangPacker:
         self._check(load().gp_pack_fifo_zones(self._h, C.byref(a), algo, mode, C.byref(r)))
         return zone, drv, exe[:total], off, avg[:q]
 
-    def pack_fifo_az_aware(self, apps: dict, mode: int, exec_order, drv_order, n_zones: int):
+    def pack_fifo_az_aware(self, apps: dict, mode: int, exec_order=None, drv_order=None, n_zones=None):
         """fitEarlierDrivers with az-aware-tightly-pack in one launch.  The snapshot's groups 0..n_zones-1 are the candidate
         zones, the groups after them the remaining nodes; exec_order / drv_order are the undivided priority orders (node
-        indices) of the fallback.  -> like pack_fifo_zones; zone -1 with driver_node >= 0 = placed by the fallback."""
+        indices) of the fallback -- all three None (orders == NULL): the ones prepare_cluster_zones(LAYOUT_AZ_AWARE) left on
+        the device.  -> like pack_fifo_zones; zone -1 with driver_node >= 0 = placed by the fallback."""
         q = len(apps["count"])
         count = _np(apps["count"], np.int32)
         off = np.zeros(q + 1, np.int64)
         np.cumsum(np.maximum(count, 0), out=off[1:])
         arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
         young = _np(apps.get("young"), np.uint8)
-        eo, do = _np(exec_order, np.int32), _np(drv_order, np.int32)
+        o = _az_orders(exec_order, drv_order, n_zones)
         total = int(off[-1]) if q else 0
         zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
         exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
         a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
                     exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
                     exe_count=_p(count), group=None, skip_if_no_fit=_p(young), exec_out_off=_p(off))
-        o = gp_az_orders(n_zones=int(n_zones), n_exec=len(eo), exec_order=_p(eo), n_drv=len(do), drv_order=_p(do))
         r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
-        self._check(load().gp_pack_fifo_az_aware(self._h, C.byref(a), mode, C.byref(o), C.byref(r)))
+        self._check(load().gp_pack_fifo_az_aware(self._h, C.byref(a), mode, o[0], C.byref(r)))
         return zone, drv, exe[:total], off, avg[:q]
 
-    def pack_batch_az_aware(self, apps: dict, exec_order, drv_order, n_zones: int):
+    def pack_batch_az_aware(self, apps: dict, exec_order=None, drv_order=None, n_zones=None):
         """az-aware-tightly-pack for a batch of independent decisions against the unmodified snapshot, in one call.  The
         snapshot layout is that of pack_fifo_az_aware (any n_zones up to the number of groups); exec_order / drv_order are
-        the undivided priority orders (node indices) of the fallback.  -> like pack_batch_zones; zone -1 with
-        driver_node >= 0 = placed by the fallback (zero averages)."""
+        the undivided priority orders (node indices) of the fallback, or all three None as in pack_fifo_az_aware.
+        -> like pack_batch_zones; zone -1 with driver_node >= 0 = placed by the fallback (zero averages)."""
         q = len(apps["count"])
         count = _np(apps["count"], np.int32)
         off = np.zeros(q + 1, np.int64)
         np.cumsum(np.maximum(count, 0), out=off[1:])
         arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
-        eo, do = _np(exec_order, np.int32), _np(drv_order, np.int32)
+        o = _az_orders(exec_order, drv_order, n_zones)
         total = int(off[-1]) if q else 0
         zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
         exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
         a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
                     exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
                     exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
-        o = gp_az_orders(n_zones=int(n_zones), n_exec=len(eo), exec_order=_p(eo), n_drv=len(do), drv_order=_p(do))
         r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
-        self._check(load().gp_pack_batch_az_aware(self._h, C.byref(a), C.byref(o), C.byref(r)))
+        self._check(load().gp_pack_batch_az_aware(self._h, C.byref(a), o[0], C.byref(r)))
         return zone, drv, exe[:total], off, avg[:q]
 
     def reserve_placements(self, apps: dict, placed, subtract=True):
