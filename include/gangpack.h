@@ -295,6 +295,44 @@ typedef struct {
 /* node_out[i] = node index, or -1 ("not enough capacity to reschedule the executor", :672) */
 gp_status gp_reschedule_executors(gp_ctx* ctx, const gp_reschedule* in, int32_t* node_out /* [n_execs] */);
 
+/* The whole of rescheduleExecutor (internal/extender/resource.go:594-673) minus pod and lister I/O, from the reservations to
+ * the node choice in ONE device call, for a batch of executors decided independently against the same state.  The node table
+ * is availableNodes (getNodes(nodeNames), :604) as gp_prepare_cluster takes it:
+ *   scope       NULL or keep_topology_zone == -1: every node.  keep_topology_zone >= 0: filterNodesToZone (:463-478) first --
+ *               only nodes whose topology_zone equals it are kept, and zone totals, availabilities and the executor order
+ *               see only them.  A node with topology_zone == -1 (label missing) is GP_ERR_INVALID, whatever its zone, as in
+ *               the reference.  Choosing the zone (getCommonZoneForExecutorsApplication, :493-533) stays with the caller.
+ *   order       the executor order PotentialNodes would build from the metadata availability alloc - (reservations + overhead):
+ *               zone priority by (memory, cpu) totals over the kept nodes (equal totals by zone id; sort->zone_id is the
+ *               sorter's zone, NodeSchedulingMetadata.ZoneLabel = failure-domain.beta.kubernetes.io/zone or "default",
+ *               LIB/resources/resources.go:78-81 -- NOT the topology label of the scope, SURVEY App. B5), then (available memory,
+ *               available cpu, name rank), schedulable && ready nodes only, stable label re-sort by executor_label_rank when
+ *               given.  No sort runs: a node's position is the rank of its unique key, and each decision is an arg-min.
+ *   first fit   (in->min_frag == 0, :657-662) the first node of that order with !GreaterThan against
+ *               alloc - (reservations + overhead * (node carries a reservation ? 2 : 1)) -- gp_build_reschedule_availability.
+ *   min-frag    (:675-705) capacities from the metadata availability with usage->overhead_* as "reserved" (:682); the hosting set
+ *               is in->host_off / host_nodes in node-table indices (hosting nodes that are not kept executor candidates are
+ *               ignored); a hosting node with capacity >= 1 wins, then the smallest capacity, then the order.
+ *   node_out[i] = node-table index, or -1 ("not enough capacity", :672).
+ *   ambiguous[i] = 1 when the reference's own choice is unspecified: another node qualifies equally well (first fit: it fits;
+ *               min-frag: same hosting class and capacity) but scheduleContextLessThan (internal/sort/nodesorting.go:83-93)
+ *               does not order it against the winner -- same label key, zone priority, memory and cpu, different gpu (SURVEY
+ *               App. B6).  A shim that wants the reference's choice then falls back to Go.
+ * sort->avail_*, is_driver_candidate, driver_label_rank and undefined_ties are ignored; in->reserved_* must be NULL and
+ * in->group NULL or all 0.  The context's snapshot, schedulable resources, zone layout and held az-aware orders are left
+ * untouched (the call has scratch of its own), so it may be interleaved with a resident driver snapshot.  Validation as in
+ * gp_prepare_cluster and gp_reschedule_executors; one stream synchronise, at the end. */
+typedef struct {
+    int32_t keep_topology_zone;      /* -1: every node; >= 0: keep only nodes whose topology_zone equals it */
+    int32_t reserved;
+    const int32_t* topology_zone;    /* [n_nodes] id of the node's topology.kubernetes.io/zone label, -1 = label missing;
+                                        required when keep_topology_zone >= 0 */
+} gp_reschedule_scope;
+gp_status gp_reschedule_from_reservations(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort,
+                                          const gp_reschedule_scope* scope /* NULL = every node */,
+                                          const gp_reschedule* in, int32_t* node_out /* [n_execs] */,
+                                          uint8_t* ambiguous /* [n_execs] or NULL */);
+
 /* ---- packing ------------------------------------------------------------------------------- */
 /* One batch through the hot path with HOST buffers: H2D of the app SoA, kernels, D2H of the
  * results; returns when the results are in host memory.  FIFO modes mutate the device snapshot. */

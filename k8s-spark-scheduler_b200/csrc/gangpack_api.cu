@@ -10,6 +10,7 @@
 #include "gangpack_resched.cuh"
 #include "gangpack_sort.cuh"
 #include "gangpack_zonelayout.cuh"
+#include "gangpack_reschedprep.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -450,6 +451,7 @@ struct gp_ctx {
     // lengths and n_zones as DEVICE pointers for gp_pack_*_az_aware(orders == NULL); zone_kind = the gp_zone_layout_kind of the
     // current snapshot, -1 when another entry laid it out
     DevBuf zoneprep;
+    DevBuf reschedprep;                           // gp_reschedule_from_reservations' own scratch (no state points into it)
     int zone_kind = -1;
     gp_az_orders zone_orders{};
     bool sort_attr_set = false;
@@ -1939,8 +1941,9 @@ gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, c
 }  // extern "C"
 
 // f2 stage: uploads the inputs, leaves avail[3][N] / sched[3][N] on the device (usagebuf).
+// d_over (optional, [3]): the uploaded overhead columns, NULL where the caller gave none.
 static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStream_t st, long long** d_avail, long long** d_sched,
-                                    long long** d_resched = nullptr) {
+                                    long long** d_resched = nullptr, const long long** d_over = nullptr) {
     const int32_t n = in->n_nodes;
     const size_t N = (size_t)n, R = (size_t)in->n_reservations;
     Arena ar{c->usagebuf};
@@ -1975,6 +1978,11 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
                                                    (const unsigned long long*)(b + o_usage), (long long*)(b + o_avail), (long long*)(b + o_sched),
                                                    (const unsigned int*)(b + o_has), d_resched ? (long long*)(b + o_resched) : nullptr);
     if (d_resched) *d_resched = (long long*)(b + o_resched);
+    if (d_over) {
+        d_over[0] = in->overhead_cpu_milli ? ov : nullptr;
+        d_over[1] = in->overhead_mem_bytes ? ov + N : nullptr;
+        d_over[2] = in->overhead_gpu ? ov + 2 * N : nullptr;
+    }
     GP_CUDA(c, cudaGetLastError());
     *d_avail = (long long*)(b + o_avail);
     *d_sched = (long long*)(b + o_sched);
@@ -2378,6 +2386,125 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
     GP_CUDA(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
     if (err) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: instance group out of range");
+    return GP_OK;
+}
+
+// rescheduleExecutor from the reservations to the node choice (SURVEY 8f row f4); see gangpack_reschedprep.cuh
+gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const gp_reschedule_scope* scope,
+                                          const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous) {
+    if (!c) return GP_ERR_INVALID;
+    static const char* who = "gp_reschedule_from_reservations";
+    auto bad = [&](gp_status st, const char* what) { return fail(c, st, std::string(who) + ": " + what); };
+    if (!usage || !sort || !in || usage->n_nodes != sort->n_nodes || usage->n_nodes < 0 || sort->n_zones < 1 || usage->n_reservations < 0 ||
+        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes)) ||
+        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)) ||
+        in->n_execs < 0 || (in->n_execs > 0 && (!in->exe_cpu_milli || !in->exe_mem_bytes || !node_out)))
+        return bad(GP_ERR_INVALID, "missing arrays or mismatched sizes");
+    const int32_t n = usage->n_nodes, q = in->n_execs;
+    if (n == 0) return bad(GP_ERR_INVALID, "empty node table");
+    if (in->reserved_cpu_milli || in->reserved_mem_bytes || in->reserved_gpu)
+        return bad(GP_ERR_INVALID, "reserved_* must be NULL (the overhead of the node table is the reserved amount)");
+    const int32_t keep = scope ? scope->keep_topology_zone : -1;
+    if (keep < -1) return bad(GP_ERR_INVALID, "scope->keep_topology_zone must be -1 or a zone id");
+    if (keep >= 0) {
+        if (!scope->topology_zone) return bad(GP_ERR_INVALID, "scope->topology_zone missing");
+        for (int32_t i = 0; i < n; ++i)
+            if (scope->topology_zone[i] < 0)
+                return bad(GP_ERR_INVALID, "filterNodesToZone: a node has no topology.kubernetes.io/zone label (topology_zone == -1), "
+                                           "unable to make scheduling decisions based on AZ");
+    }
+    if (sort->zone_id) for (int32_t i = 0; i < n; ++i)
+        if (sort->zone_id[i] < 0 || sort->zone_id[i] >= sort->n_zones) return bad(GP_ERR_INVALID, "zone_id out of range");
+    if (sort->name_rank) for (int32_t i = 0; i < n; ++i)
+        if (sort->name_rank[i] < 0 || sort->name_rank[i] >= n) return bad(GP_ERR_INVALID, "name_rank out of range");
+    const bool mf = in->min_frag != 0;
+    const bool has_host = mf && in->host_off;
+    for (int32_t i = 0; i < q; ++i) {
+        const int64_t v[3] = {in->exe_cpu_milli[i], in->exe_mem_bytes[i], in->exe_gpu ? in->exe_gpu[i] : 0};
+        for (int64_t x : v) {
+            if (x < 0) return bad(GP_ERR_INVALID, "negative resource request");
+            if (x >= kMaxQuantity) return bad(GP_ERR_UNREPRESENTABLE, "quantity >= 2^61");
+        }
+        if (in->group && in->group[i] != 0) return bad(GP_ERR_INVALID, "instance group out of range (one node table: group must be 0)");
+    }
+    int64_t hosted = 0;
+    if (has_host) {
+        if (in->host_off[0] != 0) return bad(GP_ERR_INVALID, "host_off must start at 0");
+        for (int32_t i = 0; i < q; ++i)
+            if (in->host_off[i + 1] < in->host_off[i]) return bad(GP_ERR_INVALID, "host_off not monotone");
+        hosted = in->host_off[q];
+        if (hosted > 0 && !in->host_nodes) return bad(GP_ERR_INVALID, "host_nodes missing");
+        for (int64_t t = 0; t < hosted; ++t)
+            if (in->host_nodes[t] < 0 || in->host_nodes[t] >= n) return bad(GP_ERR_INVALID, "host_nodes index out of range");
+    }
+    if (q == 0) return GP_OK;
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    // availability: one scatter of the reservations, one pass per node (usagebuf is scratch of the f2 stage only)
+    long long *d_avail = nullptr, *d_sched = nullptr, *d_ff = nullptr;
+    const long long* d_over[3] = {nullptr, nullptr, nullptr};
+    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched, mf ? nullptr : &d_ff, d_over);
+    if (s != GP_OK) return s;
+    const size_t N = (size_t)n, Q = (size_t)q, H = (size_t)hosted, Z = (size_t)sort->n_zones;
+    const bool zoned = sort->zone_id != nullptr && sort->n_zones > 1;
+    Arena ar{c->reschedprep};
+    const size_t o_tot = ar.take(16 * Z), o_prio = ar.take(4 * Z), o_zone = ar.take(4 * N), o_nr = ar.take(4 * N), o_fu = ar.take(N),
+                 o_fr = ar.take(N), o_lr = ar.take(4 * N), o_tz = ar.take(4 * N), o_rec = ar.take(sizeof(RpNode) * N), o_exe = ar.take(24 * Q),
+                 o_hoff = ar.take(8 * (Q + 1)), o_hn = ar.take(4 * (H + 1)), o_out = ar.take(4 * Q), o_amb = ar.take(Q);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
+    if (zoned) GP_CUDA(c, up(o_zone, sort->zone_id, 4 * N));
+    if (sort->name_rank) GP_CUDA(c, up(o_nr, sort->name_rank, 4 * N));
+    if (sort->unschedulable) GP_CUDA(c, up(o_fu, sort->unschedulable, N));
+    if (sort->ready) GP_CUDA(c, up(o_fr, sort->ready, N));
+    if (sort->executor_label_rank) GP_CUDA(c, up(o_lr, sort->executor_label_rank, 4 * N));
+    if (keep >= 0) GP_CUDA(c, up(o_tz, scope->topology_zone, 4 * N));
+    GP_CUDA(c, up(o_exe, in->exe_cpu_milli, 8 * Q));
+    GP_CUDA(c, up(o_exe + 8 * Q, in->exe_mem_bytes, 8 * Q));
+    if (in->exe_gpu) GP_CUDA(c, up(o_exe + 16 * Q, in->exe_gpu, 8 * Q));
+    else GP_CUDA(c, cudaMemsetAsync(b + o_exe + 16 * Q, 0, 8 * Q, st));
+    if (has_host) {
+        GP_CUDA(c, up(o_hoff, in->host_off, 8 * (Q + 1)));
+        if (H) GP_CUDA(c, up(o_hn, in->host_nodes, 4 * H));
+    }
+    const int T = 256;
+    const int nb = (n + T - 1) / T;
+    const int32_t* tz = keep >= 0 ? (const int32_t*)(b + o_tz) : nullptr;
+    if (zoned) {
+        GP_CUDA(c, cudaMemsetAsync(b + o_tot, 0, 16 * Z, st));
+        gp_rp_zone_totals<<<nb, T, 0, st>>>(n, d_avail, d_avail + N, (const int32_t*)(b + o_zone), keep, tz, (unsigned long long*)(b + o_tot));
+        gp_zone_priority<<<(sort->n_zones + T - 1) / T, T, 0, st>>>(sort->n_zones, (const unsigned long long*)(b + o_tot), (int32_t*)(b + o_prio));
+    }
+    RpNodeIn ni{};
+    ni.avail = d_avail; ni.ff = d_ff;
+    for (int d = 0; d < 3; ++d) ni.over[d] = d_over[d];
+    ni.zone = zoned ? (const int32_t*)(b + o_zone) : nullptr;
+    ni.prio = (const int32_t*)(b + o_prio);
+    ni.name_rank = sort->name_rank ? (const int32_t*)(b + o_nr) : nullptr;
+    ni.unschedulable = sort->unschedulable ? (const uint8_t*)(b + o_fu) : nullptr;
+    ni.ready = sort->ready ? (const uint8_t*)(b + o_fr) : nullptr;
+    ni.label_rank = sort->executor_label_rank ? (const int32_t*)(b + o_lr) : nullptr;
+    ni.tz = tz; ni.keep = keep; ni.n = n;
+    RpNode* rec = (RpNode*)(b + o_rec);
+    gp_rp_nodes<<<nb, T, 0, st>>>(ni, rec);
+    RpDecideIn di{};
+    di.exe = (const int64_t*)(b + o_exe);
+    di.host_off = has_host ? (const int64_t*)(b + o_hoff) : nullptr;
+    di.host_nodes = (const int32_t*)(b + o_hn);
+    di.n = n; di.q = q;
+    // one CTA per executor; the grid is capped at 8 CTAs per SM's worth of executors and grid-strides over the rest.  The cap
+    // only sizes the grid: registers bound residency (gp_rp_decide<true>: 78 x 256 threads -> 3 CTAs per SM; <false>: 48 -> 5),
+    // so the CTAs beyond that wait for a free slot
+    const int blocks = (int)std::min<int64_t>(q, (int64_t)c->sm_count * 8);
+    int32_t* d_out = (int32_t*)(b + o_out);
+    uint8_t* d_amb = ambiguous ? (uint8_t*)(b + o_amb) : nullptr;
+    if (mf) gp_rp_decide<true><<<blocks, kRpThreads, 0, st>>>(rec, di, d_out, d_amb);
+    else gp_rp_decide<false><<<blocks, kRpThreads, 0, st>>>(rec, di, d_out, d_amb);
+    GP_CUDA(c, cudaGetLastError());
+    GP_CUDA(c, cudaMemcpyAsync(node_out, d_out, 4 * Q, cudaMemcpyDeviceToHost, st));
+    if (ambiguous) GP_CUDA(c, cudaMemcpyAsync(ambiguous, d_amb, Q, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
     return GP_OK;
 }
 

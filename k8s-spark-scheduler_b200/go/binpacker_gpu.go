@@ -22,6 +22,7 @@ import (
 	"context"
 	"fmt"
 	"runtime"
+	"sort"
 	"sync"
 	"unsafe"
 
@@ -446,6 +447,164 @@ func RescheduleExecutorNode(minFrag bool, executorResources *resources.Resources
 		return "", false, true // failureFit, :672
 	}
 	return s.names[out], true, true
+}
+
+// The two zone labels rescheduleExecutor reads, and they differ (SURVEY App. B5): PotentialNodes sorts by
+// NodeSchedulingMetadata.ZoneLabel, the BETA label with the placeholder "default" when it is absent
+// (LIB/resources/resources.go:27,78-81); filterNodesToZone and getAzsOfPods read the GA label (EXT/resource.go:466,526).
+const (
+	labelZoneFailureDomain = "failure-domain.beta.kubernetes.io/zone" // corev1.LabelZoneFailureDomain
+	labelTopologyZone      = "topology.kubernetes.io/zone"            // v1.LabelTopologyZone
+)
+
+// RescheduleNode is one node of availableNodes (getNodes(nodeNames), EXT/resource.go:604) as rescheduleExecutor reads it.
+type RescheduleNode struct {
+	Name          string
+	Allocatable   *resources.Resources // node.Status.Allocatable
+	Labels        map[string]string    // node.Labels: both zone labels are read from here
+	Unschedulable bool
+	Ready         bool
+	ExecutorRank  int32 // rank of the node's executor-prioritized-node-label value, -1 unknown
+}
+
+// ReservationRow is one hard or soft reservation (GetReservedResources, EXT/resourcereservations.go:258-263).
+type ReservationRow struct {
+	Node      string
+	Resources *resources.Resources
+}
+
+// RescheduleExecutorFromReservations is the whole of rescheduleExecutor (EXT/resource.go:594-673) minus pod and lister I/O in
+// ONE gp_reschedule_from_reservations call: the reservations, both availabilities, PotentialNodes' executor order and the
+// first-fit / minimal-fragmentation choice stay on the device, and the resident driver snapshot is left alone.  commonZone:
+// the zone getCommonZoneForExecutorsApplication returned, or nil.  labelRanked: executor-prioritized-node-label configured.
+// ok=false (any non-OK status, an inexact quantity, or a choice the reference leaves to its unstable sort): run the Go code.
+func RescheduleExecutorFromReservations(minFrag bool, executorResources *resources.Resources, nodes []RescheduleNode,
+	reservations []ReservationRow, overhead resources.NodeGroupResources, labelRanked bool, commonZone *string,
+	hosting map[string]bool) (node string, found, ok bool) {
+	d, err := getDevice()
+	if err != nil || len(nodes) == 0 {
+		return "", false, false
+	}
+	ec, em, eg, exact := toTriple(executorResources)
+	if !exact {
+		return "", false, false
+	}
+	n := len(nodes)
+	index := make(map[string]int32, n)
+	zoneID, topoID := make(map[string]int32), make(map[string]int32) // sorter zones and topology zones, interned separately
+	ac, am, ag := make([]int64, n), make([]int64, n), make([]int64, n)
+	oc, om, og := make([]int64, n), make([]int64, n), make([]int64, n)
+	zone, topo, nameRank, labelRank := make([]int32, n), make([]int32, n), make([]int32, n), make([]int32, n)
+	unsched, ready := make([]uint8, n), make([]uint8, n)
+	names := make([]string, n)
+	for i, nd := range nodes {
+		index[nd.Name] = int32(i)
+		names[i] = nd.Name
+		if ac[i], am[i], ag[i], exact = toTriple(nd.Allocatable); !exact {
+			return "", false, false
+		}
+		if o, has := overhead[nd.Name]; has {
+			if oc[i], om[i], og[i], exact = toTriple(o); !exact {
+				return "", false, false
+			}
+		}
+		sortZone, has := nd.Labels[labelZoneFailureDomain] // NodeSchedulingMetadataForNodes, resources.go:78-81
+		if !has {
+			sortZone = "default"
+		}
+		z, seen := zoneID[sortZone]
+		if !seen {
+			z = int32(len(zoneID))
+			zoneID[sortZone] = z
+		}
+		zone[i], topo[i] = z, -1
+		if ga, has := nd.Labels[labelTopologyZone]; has { // filterNodesToZone, EXT/resource.go:466
+			t, seen := topoID[ga]
+			if !seen {
+				t = int32(len(topoID))
+				topoID[ga] = t
+			}
+			topo[i] = t
+		}
+		if nd.Unschedulable {
+			unsched[i] = 1
+		}
+		if nd.Ready {
+			ready[i] = 1
+		}
+		labelRank[i] = nd.ExecutorRank
+	}
+	byName := make([]int32, n)
+	for i := range byName {
+		byName[i] = int32(i)
+	}
+	sort.Slice(byName, func(a, b int) bool { return names[byName[a]] < names[byName[b]] })
+	for r, i := range byName {
+		nameRank[i] = int32(r)
+	}
+	R := len(reservations)
+	rn, rc, rm, rg := make([]int32, R), make([]int64, R), make([]int64, R), make([]int64, R)
+	for t, r := range reservations {
+		rn[t] = -1 // a reservation on a node outside the table is ignored (LIB/resources/resources.go:72-75)
+		if i, known := index[r.Node]; known {
+			rn[t] = i
+		}
+		if rc[t], rm[t], rg[t], exact = toTriple(r.Resources); !exact {
+			return "", false, false
+		}
+	}
+	hostNodes, hostOff := []int32{}, []int64{0, 0}
+	for h, yes := range hosting {
+		if i, known := index[h]; known && yes {
+			hostNodes = append(hostNodes, i)
+		}
+	}
+	hostOff[1] = int64(len(hostNodes))
+	u := C.gp_usage_input{n_nodes: C.int32_t(n), alloc_cpu_milli: ptr64(ac), alloc_mem_bytes: ptr64(am), alloc_gpu: ptr64(ag),
+		overhead_cpu_milli: ptr64(oc), overhead_mem_bytes: ptr64(om), overhead_gpu: ptr64(og), n_reservations: C.int64_t(R),
+		res_node: ptr32(rn), res_cpu_milli: ptr64(rc), res_mem_bytes: ptr64(rm), res_gpu: ptr64(rg)}
+	s := C.gp_sort_input{n_nodes: C.int32_t(n), n_zones: C.int32_t(len(zoneID)), zone_id: ptr32(zone), name_rank: ptr32(nameRank),
+		unschedulable: ptr8(unsched), ready: ptr8(ready)}
+	if labelRanked {
+		s.executor_label_rank = ptr32(labelRank)
+	}
+	scope := C.gp_reschedule_scope{keep_topology_zone: -1, topology_zone: ptr32(topo)}
+	var scopeArg *C.gp_reschedule_scope
+	if commonZone != nil {
+		scope.keep_topology_zone = C.int32_t(len(topoID)) // a zone no node carries: nothing is kept
+		if z, seen := topoID[*commonZone]; seen {
+			scope.keep_topology_zone = C.int32_t(z)
+		}
+		scopeArg = &scope
+	}
+	in := C.gp_reschedule{n_execs: 1, exe_cpu_milli: (*C.int64_t)(unsafe.Pointer(&ec)), exe_mem_bytes: (*C.int64_t)(unsafe.Pointer(&em)),
+		exe_gpu: (*C.int64_t)(unsafe.Pointer(&eg))}
+	if minFrag {
+		in.min_frag = 1
+		in.host_off, in.host_nodes = ptr64(hostOff), ptr32(hostNodes)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	var out C.int32_t = -1
+	var ambiguous C.uint8_t
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []any{&ec, &em, &eg, &hostOff[0], ptrOrNil32(hostNodes), ptrOrNil(ac), ptrOrNil(am), ptrOrNil(ag), ptrOrNil(oc),
+		ptrOrNil(om), ptrOrNil(og), ptrOrNil32(rn), ptrOrNil(rc), ptrOrNil(rm), ptrOrNil(rg), ptrOrNil32(zone), ptrOrNil32(topo),
+		ptrOrNil32(nameRank), ptrOrNil32(labelRank), ptrOrNil8(unsched), ptrOrNil8(ready)} {
+		if p != nil {
+			pin.Pin(p)
+		}
+	}
+	if st := C.gp_reschedule_from_reservations(d.ctx, &u, &s, scopeArg, &in, &out, &ambiguous); st != C.GP_OK || ambiguous != 0 {
+		return "", false, false // a missing zone label under a scope is refused here too: the Go code returns filterNodesToZone's error
+	}
+	if out < 0 {
+		return "", false, true // failureFit, :672
+	}
+	return names[out], true, true
 }
 
 // QueuedApp is what fitEarlierDrivers reads from one earlier driver pod (EXT/resource.go:230-243).

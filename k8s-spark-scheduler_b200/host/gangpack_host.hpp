@@ -870,4 +870,114 @@ inline std::pair<std::string, bool> RescheduleExecutorNode(const binpacker::Binp
     return {d.name(node), true};
 }
 
+// The two zone labels rescheduleExecutor reads, and they differ (SURVEY App. B5): PotentialNodes sorts by
+// NodeSchedulingMetadata.ZoneLabel, the BETA label with the placeholder "default" when it is absent
+// (LIB/resources/resources.go:27,78-81); filterNodesToZone and getAzsOfPods read the GA label (resource.go:466,526).
+inline const char* const LabelZoneFailureDomain = "failure-domain.beta.kubernetes.io/zone";   // corev1.LabelZoneFailureDomain
+inline const char* const LabelTopologyZone = "topology.kubernetes.io/zone";                   // v1.LabelTopologyZone
+
+// One node of availableNodes (getNodes(nodeNames), resource.go:604) as rescheduleExecutor reads it.
+struct RescheduleNode {
+    std::string Name;
+    resources::Resources Allocatable;                  // node.Status.Allocatable
+    bool Unschedulable = false;
+    bool Ready = true;
+    std::map<std::string, std::string> AllLabels;      // node.Labels: both zone labels and the executor label priority
+};
+struct ReservationRow {                                // one hard or soft reservation (GetReservedResources, resourcereservations.go:258-263)
+    std::string Node;
+    resources::Resources Resources;
+};
+struct RescheduleOutcome {
+    std::string Node;                                  // chosen node, "" = failureFit (:672)
+    bool Found = false;
+    bool Ambiguous = false;                            // the reference's own choice is unspecified (SURVEY App. B6)
+};
+
+// rescheduleExecutor (resource.go:594-673) minus pod and lister I/O, in ONE device call (gp_reschedule_from_reservations):
+// GetReservedResources -> NodeSchedulingMetadataForNodes -> AvailableForNodes (overhead counted twice, App. B7) ->
+// PotentialNodes -> first fit or rescheduleExecutorWithMinimalFragmentation.  commonZone: the zone
+// getCommonZoneForExecutorsApplication returned (filterNodesToZone then runs first over LabelTopologyZone; a node without that
+// label throws, as the reference errors), or nullptr.  The executor order's zone priority comes from LabelZoneFailureDomain
+// ("default" when absent), as in the reference.  The device context's resident snapshot is not touched.
+inline RescheduleOutcome RescheduleExecutor(const binpacker::Binpacker& packer, const resources::Resources& executorResources,
+                                            const std::vector<RescheduleNode>& availableNodes, const std::vector<ReservationRow>& reservations,
+                                            const resources::NodeGroupResources& overhead, const sort::LabelPriorityOrder* executorLabel,
+                                            const std::string* commonZone,
+                                            const std::set<std::string>& nodesWithExecutorsBelongingToThisApp) {
+    RescheduleOutcome out;
+    const size_t N = availableNodes.size();
+    if (N == 0) return out;
+    std::unordered_map<std::string, int32_t> index, zoneId, topoId;   // sorter zones and topology zones, interned separately
+    std::vector<int64_t> ac(N), am(N), ag(N), oc(N, 0), om(N, 0), og(N, 0);
+    std::vector<int32_t> zone(N), topo(N), nameRank(N), labelRank(N, -1);
+    std::vector<uint8_t> unsched(N), ready(N);
+    std::unordered_map<std::string, int> rankOfValue;
+    if (executorLabel)
+        for (size_t i = 0; i < executorLabel->DescendingPriorityValues.size(); ++i) rankOfValue[executorLabel->DescendingPriorityValues[i]] = (int)i;
+    for (size_t i = 0; i < N; ++i) {
+        const RescheduleNode& n = availableNodes[i];
+        index[n.Name] = (int32_t)i;
+        ac[i] = n.Allocatable.CPU; am[i] = n.Allocatable.Memory; ag[i] = n.Allocatable.NvidiaGPU;
+        auto o = overhead.find(n.Name);                                                   // GetOverhead(availableNodes)
+        if (o != overhead.end()) { oc[i] = o->second.CPU; om[i] = o->second.Memory; og[i] = o->second.NvidiaGPU; }
+        auto beta = n.AllLabels.find(LabelZoneFailureDomain);                            // the sorter's zone (resources.go:78-81)
+        const std::string& sortZone = beta == n.AllLabels.end() ? std::string("default") : beta->second;
+        zone[i] = zoneId.emplace(sortZone, (int32_t)zoneId.size()).first->second;       // interned in first-seen order
+        auto ga = n.AllLabels.find(LabelTopologyZone);                                  // filterNodesToZone's label (:466)
+        topo[i] = ga == n.AllLabels.end() ? -1 : topoId.emplace(ga->second, (int32_t)topoId.size()).first->second;
+        unsched[i] = n.Unschedulable ? 1 : 0; ready[i] = n.Ready ? 1 : 0;
+        if (executorLabel) {
+            auto v = n.AllLabels.find(executorLabel->Name);
+            if (v != n.AllLabels.end()) { auto r = rankOfValue.find(v->second); if (r != rankOfValue.end()) labelRank[i] = r->second; }
+        }
+    }
+    std::vector<size_t> byName(N);
+    for (size_t i = 0; i < N; ++i) byName[i] = i;
+    std::sort(byName.begin(), byName.end(), [&](size_t a, size_t b) { return availableNodes[a].Name < availableNodes[b].Name; });
+    for (size_t r = 0; r < N; ++r) nameRank[byName[r]] = (int32_t)r;
+    std::vector<int32_t> rn;
+    std::vector<int64_t> rc, rm, rg;
+    rn.reserve(reservations.size()); rc.reserve(reservations.size()); rm.reserve(reservations.size()); rg.reserve(reservations.size());
+    for (const auto& r : reservations) {
+        auto it = index.find(r.Node);
+        rn.push_back(it == index.end() ? -1 : it->second);                                // not in the table: ignored (resources.go:72-75)
+        rc.push_back(r.Resources.CPU); rm.push_back(r.Resources.Memory); rg.push_back(r.Resources.NvidiaGPU);
+    }
+    gp_usage_input u{};
+    u.n_nodes = (int32_t)N;
+    u.alloc_cpu_milli = ac.data(); u.alloc_mem_bytes = am.data(); u.alloc_gpu = ag.data();
+    u.overhead_cpu_milli = oc.data(); u.overhead_mem_bytes = om.data(); u.overhead_gpu = og.data();
+    u.n_reservations = (int64_t)rn.size();
+    u.res_node = rn.data(); u.res_cpu_milli = rc.data(); u.res_mem_bytes = rm.data(); u.res_gpu = rg.data();
+    gp_sort_input s{};
+    s.n_nodes = (int32_t)N;
+    s.n_zones = (int32_t)zoneId.size();
+    s.zone_id = zone.data(); s.name_rank = nameRank.data(); s.unschedulable = unsched.data(); s.ready = ready.data();
+    s.executor_label_rank = executorLabel ? labelRank.data() : nullptr;
+    gp_reschedule_scope scope{};
+    scope.keep_topology_zone = -1;
+    scope.topology_zone = topo.data();
+    if (commonZone) {
+        auto z = topoId.find(*commonZone);
+        scope.keep_topology_zone = z == topoId.end() ? (int32_t)topoId.size() : z->second;   // a zone no node has: nothing kept
+    }
+    const bool minFrag = packer.Name == binpacker::SingleAzMinimalFragmentation;             // :652
+    int64_t ec = executorResources.CPU, em = executorResources.Memory, eg = executorResources.NvidiaGPU;
+    std::vector<int32_t> hosting;
+    for (const auto& n : nodesWithExecutorsBelongingToThisApp) { auto it = index.find(n); if (it != index.end()) hosting.push_back(it->second); }
+    int64_t hoff[2] = {0, (int64_t)hosting.size()};
+    gp_reschedule in{};
+    in.n_execs = 1; in.exe_cpu_milli = &ec; in.exe_mem_bytes = &em; in.exe_gpu = &eg; in.min_frag = minFrag ? 1 : 0;
+    if (minFrag) { in.host_off = hoff; in.host_nodes = hosting.data(); }
+    int32_t node = -1;
+    uint8_t ambiguous = 0;
+    gangpack::Device& d = gangpack::Device::Get();
+    d.check(gp_reschedule_from_reservations(d.ctx(), &u, &s, commonZone ? &scope : nullptr, &in, &node, &ambiguous),
+            "gp_reschedule_from_reservations");
+    out.Ambiguous = ambiguous != 0;
+    if (node >= 0) { out.Node = availableNodes[(size_t)node].Name; out.Found = true; }
+    return out;
+}
+
 }  // namespace extender

@@ -17,7 +17,8 @@ _ROOT = os.path.dirname(_PKG)
 LIB_PATH = os.environ.get("GANGPACK_LIB") or os.path.join(_PKG, "libgangpack.so")   # GANGPACK_LIB: experimental builds
 _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack_kernels.cuh", "gangpack_fifo.cuh", "gangpack_minfrag.cuh",
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
-                                                    "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh")] + [
+                                                    "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
+                                                    "gangpack_reschedprep.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -38,7 +39,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_free_pinned", "gp_register_host", "gp_unregister_host", "gp_set_snapshot", "gp_get_snapshot", "gp_pack_batch", "gp_pack_batch_wire", "gp_pack_one", "gp_set_schedulable", "gp_pack_batch_zones", "gp_pack_fifo_zones", "gp_pack_fifo_az_aware", "gp_pack_batch_az_aware", "gp_reserve_placements", "gp_apply_usage_delta",
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
-           "gp_reschedule_executors",
+           "gp_reschedule_executors", "gp_reschedule_from_reservations",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -152,6 +153,10 @@ class gp_reschedule(C.Structure):
                 ("host_nodes", C.c_void_p)]
 
 
+class gp_reschedule_scope(C.Structure):
+    _fields_ = [("keep_topology_zone", C.c_int32), ("reserved", C.c_int32), ("topology_zone", C.c_void_p)]
+
+
 class gp_stats(C.Structure):
     _fields_ = [("nodes_scanned", C.c_int64), ("drivers_tried", C.c_int64), ("kernel_launches", C.c_int64),
                 ("pack_kernel_ns", C.c_int64), ("prep_kernel_ns", C.c_int64), ("scan_path_apps", C.c_int64),
@@ -236,6 +241,9 @@ def load():
                                      C.c_void_p, C.POINTER(C.c_int32)]
     L.gp_reschedule_executors.restype = C.c_int
     L.gp_reschedule_executors.argtypes = [C.c_void_p, C.POINTER(gp_reschedule), C.c_void_p]
+    L.gp_reschedule_from_reservations.restype = C.c_int
+    L.gp_reschedule_from_reservations.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input),
+                                                  C.POINTER(gp_reschedule_scope), C.POINTER(gp_reschedule), C.c_void_p, C.c_void_p]
     L.gp_multi_create.restype = C.c_int
     L.gp_multi_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32]
     L.gp_multi_destroy.restype = None
@@ -438,6 +446,46 @@ class GangPacker:
         outs = [np.empty(max(n, 1), np.int64) for _ in range(3)]
         self._check(load().gp_build_reschedule_availability(self._h, C.byref(ui), *[_p(o) for o in outs]))
         return [o[:n] for o in outs]
+
+    def reschedule_from_reservations(self, alloc, overhead, res_node, res, exe, min_frag=False, hosting=None, zone_id=None,
+                                     n_zones=1, name_rank=None, unschedulable=None, ready=None, executor_label_rank=None,
+                                     keep_topology_zone=None, topology_zone=None):
+        """rescheduleExecutor from the reservations to the node choice in one device call, for a batch of executors.
+        alloc / overhead / res / exe: (cpu, mem, gpu) triples (overhead and the gpu entries may be None); hosting: per-executor
+        lists of node indices already hosting executors of the same application, or None; keep_topology_zone: None (every
+        node) or the zone id filterNodesToZone keeps, with topology_zone[n] the node's zone id (-1 = label missing).
+        The context's snapshot is not touched.  -> (node index per executor or -1, ambiguous flag per executor)."""
+        al = [_np(x, np.int64) for x in alloc]
+        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
+        rn = _np(res_node, np.int32)
+        rs = [_np(x, np.int64) for x in res]
+        n = len(al[0])
+        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
+                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
+                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
+        arrs = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(unschedulable, np.uint8), _np(ready, np.uint8),
+                _np(executor_label_rank, np.int32)]
+        si = gp_sort_input(n_nodes=n, n_zones=n_zones, zone_id=_p(arrs[0]), name_rank=_p(arrs[1]), unschedulable=_p(arrs[2]),
+                           ready=_p(arrs[3]), executor_label_rank=_p(arrs[4]))
+        tz = _np(topology_zone, np.int32)
+        scope = None
+        if keep_topology_zone is not None:
+            scope = gp_reschedule_scope(keep_topology_zone=int(keep_topology_zone), topology_zone=_p(tz))
+        ec, em = _np(exe[0], np.int64), _np(exe[1], np.int64)
+        eg = _np(exe[2], np.int64) if len(exe) > 2 else None
+        q = len(ec)
+        hoff = hn = None
+        if hosting is not None:
+            hoff = np.zeros(q + 1, np.int64)
+            np.cumsum([len(h) for h in hosting], out=hoff[1:])
+            hn = np.array([v for h in hosting for v in h] or [0], np.int32)
+        r = gp_reschedule(n_execs=q, exe_cpu_milli=_p(ec), exe_mem_bytes=_p(em), exe_gpu=_p(eg), min_frag=1 if min_frag else 0,
+                          host_off=_p(hoff), host_nodes=_p(hn))
+        out = np.full(max(q, 1), -9, np.int32)
+        amb = np.full(max(q, 1), 9, np.uint8)
+        self._check(load().gp_reschedule_from_reservations(self._h, C.byref(ui), C.byref(si), C.byref(scope) if scope is not None else None,
+                                                           C.byref(r), _p(out), _p(amb)))
+        return out[:q], amb[:q]
 
     def prepare_cluster(self, alloc, overhead, res_node, res, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None):
