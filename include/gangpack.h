@@ -124,7 +124,8 @@ typedef struct {
  *   executor_nodes[exec_out_off[i] .. +exe_count[i]) : ExecutorNodes, in the reference's order
  *     (reservation names executor-1..k follow it, resourcereservations.go:501-510); its contents are
  *     UNDEFINED unless driver_node[i] >= 0 (the FIFO kernels emit optimistically before feasibility is known).
- * PackingEfficiencies are not produced on the device (metrics by-product, SURVEY §8a A7). */
+ * The per-node PackingEfficiencies map is not returned; its cluster-wide average, the Predicate's metric, is
+ * gp_packing_efficiency (SURVEY §8a A7). */
 typedef struct {
     int32_t* driver_node;            /* [n_apps] */
     int32_t* executor_nodes;         /* [executor_nodes_cap] */
@@ -503,6 +504,36 @@ gp_status gp_reserve_placements(gp_ctx* ctx, const gp_apps* apps, const gp_resul
                                 int32_t subtract_from_snapshot, gp_reservation_table* out /* may be NULL with subtract */);
 gp_status gp_apply_usage_delta(gp_ctx* ctx, int64_t n_rows, const int32_t* node, const int64_t* cpu_milli, const int64_t* mem_bytes,
                                const int64_t* gpu /* or NULL */, int32_t sign /* +1 reserve, -1 release */);
+
+/* ---- the Predicate's packing-efficiency metric (EXT/resource.go:329, 352) ---------------------------------------------
+ * computeAvgPackingEfficiencyForResult (internal/extender/resource.go:372-381) of placed applications: ComputePackingEfficiencies
+ * over EVERY node of the context's node table (LIB/binpack/efficiency.go:66-102, binpack.go:72-77) averaged like
+ * ComputeAvgPackingEfficiency (:114-156), against the availability the device holds and the SchedulableResources of
+ * gp_set_schedulable / gp_prepare_cluster / gp_prepare_cluster_zones.  avg_out[4*i..] = {CPU, Memory, GPU, Max}.
+ * (internal/metrics/binpack.go:66 reports max(CPU, Memory) of it; that step stays with the caller.)
+ *   placed     HOST gp_results as gp_pack_batch returns them: driver_node, executor_nodes in CSR by apps->exec_out_off (or the
+ *              prefix sum of exe_count).  Zone results are wrapped: gp_results{zone_results.driver_node, .executor_nodes, cap}.
+ *   reserved   per node, the driver plus every executor placed there (SparkBinPack's map, binpack.go:72-75 + pack_tightly.go:50:
+ *              tightly-pack, distribute-evenly, the az-aware zone winner or its fallback); algo GP_MINIMAL_FRAGMENTATION (also
+ *              for single-az-minimal-fragmentation winners): the driver only -- minimalFragmentation never adds its executors.
+ *   charged    GP_MODE_INDEPENDENT: every row against the current device availability (what SparkBinPack saw for an
+ *              independent batch on this snapshot).  GP_MODE_FIFO_REFERENCE / GP_MODE_FIFO_EXACT: n_apps must be 1 and that
+ *              application's usage under that mode is already in the availability (the driver as the last entry of a FIFO
+ *              call; gp_reserve_placements(subtract = 1) charges like FIFO_EXACT); it is added back first -- FIFO_REFERENCE:
+ *              sparkResourceUsage's map (EXT/sparkpods.go:139-146: one executor per distinct executor node, a driver node
+ *              that hosts an executor the executor only), FIFO_EXACT: every pod.
+ *   driver_node[i] < 0: WorstAvgPackingEfficiency (four zeros).
+ * Exact sums: the CPU, Memory and Max sums over every node and the GPU sum over the nodes whose schedulable GPU is non-zero are
+ * each rounded ONCE, to nearest-even, from their exact real value (math.fsum of the reference's per-node terms; an empty or
+ * all-zero sum is +0.0).  Then CPU, Memory and Max are divided by max(float64(n_nodes), 1) and GPU is gpuSum / nodesWithGPU, or
+ * 1.0 when no node has GPUs.  The reference sums in Go map order, which changes from call to call; this result does not
+ * depend on any order and lies within the recursive-summation bound of every order the reference can take.
+ * Device availability, slots, zone layout, held az-aware orders and gp_last_stats are left untouched; one stream synchronise,
+ * at the end.  GP_ERR_NO_SNAPSHOT: no snapshot.  GP_ERR_INVALID: no SchedulableResources, a node index out of range, a FIFO
+ * charged mode with n_apps != 1, a negative request.  GP_ERR_CAPACITY: executor_nodes_cap too small.  GP_ERR_UNREPRESENTABLE:
+ * a request, or a per-node reserved or added-back amount, >= 2^61. */
+gp_status gp_packing_efficiency(gp_ctx* ctx, const gp_apps* apps, gp_algo algo, const gp_results* placed /* host */,
+                                gp_mode charged, double* avg_out /* [n_apps][4] */);
 
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets

@@ -11,6 +11,7 @@
 #include "gangpack_sort.cuh"
 #include "gangpack_zonelayout.cuh"
 #include "gangpack_reschedprep.cuh"
+#include "gangpack_efficiency.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -447,6 +448,9 @@ struct gp_ctx {
     DevBuf sched, zonebuf, fbview;                // SchedulableResources [3][n_nodes]; staging of the zone entry points;
                                                   // the az-aware fallback's orders and gather view
     bool have_sched = false;
+    // SchedulableResources for gp_packing_efficiency alone: also set by gp_prepare_cluster, whose one-group snapshot the zone
+    // entry points keep refusing (have_sched stays false there)
+    bool have_eff_sched = false;
     // gp_prepare_cluster_zones: the undivided orders it sorted (in zoneprep, which also holds that call's scratch), their
     // lengths and n_zones as DEVICE pointers for gp_pack_*_az_aware(orders == NULL); zone_kind = the gp_zone_layout_kind of the
     // current snapshot, -1 when another entry laid it out
@@ -719,6 +723,7 @@ static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_
     c->n_nodes = dn->n_nodes; c->n_groups = dn->n_groups; c->n_exec = n_exec; c->n_drv = n_drv; c->n_slots = n_slots;
     c->have_snapshot = true;
     c->have_sched = false;               // SchedulableResources belong to a node table
+    c->have_eff_sched = false;
     return GP_OK;
 }
 
@@ -1461,6 +1466,7 @@ gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, 
     }
     GP_CUDA(c, cudaStreamSynchronize(c->stream));
     c->have_sched = true;
+    c->have_eff_sched = true;
     return GP_OK;
 }
 
@@ -1937,6 +1943,95 @@ gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, c
     return GP_OK;
 }
 
+// ---- computeAvgPackingEfficiencyForResult over the whole node table, exactly summed (gangpack_efficiency.cuh) ----------
+gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, double* avg_out) {
+    if (!c) return GP_ERR_INVALID;
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_packing_efficiency: no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)");
+    if (!c->have_eff_sched)
+        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: no SchedulableResources (gp_set_schedulable, gp_prepare_cluster or gp_prepare_cluster_zones first)");
+    if (!a || !placed || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: NULL apps/placed");
+    if (algo != GP_TIGHTLY_PACK && algo != GP_DISTRIBUTE_EVENLY && algo != GP_MINIMAL_FRAGMENTATION)
+        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: unknown algo");
+    if (charged != GP_MODE_INDEPENDENT && charged != GP_MODE_FIFO_REFERENCE && charged != GP_MODE_FIFO_EXACT)
+        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: unknown charged mode");
+    if (charged != GP_MODE_INDEPENDENT && a->n_apps != 1)
+        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: a FIFO charged mode adds back ONE application's usage: n_apps must be 1");
+    const int32_t Q = a->n_apps;
+    if (Q == 0) return GP_OK;
+    if (!avg_out || !a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !placed->driver_node)
+        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: missing app/result arrays");
+    // host pass over the placed rows: offsets, request domain, node indices (a caller-supplied placement need not be feasible)
+    std::vector<int64_t>& off = c->host_off;
+    off.resize((size_t)Q + 1);
+    const int64_t* qc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
+    int64_t acc = 0;
+    for (int32_t i = 0; i < Q; ++i) {
+        const int64_t k = a->exe_count[i] > 0 ? a->exe_count[i] : 0;
+        off[(size_t)i] = a->exec_out_off ? a->exec_out_off[i] : acc;
+        acc += k;
+        const int32_t d = placed->driver_node[i];
+        if (d >= c->n_nodes) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: driver_node out of range");
+        if (d < 0) continue;
+        for (const int64_t* col : qc) {
+            if (!col) continue;
+            if (col[i] < 0) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: negative request");
+            if (col[i] >= kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, "gp_packing_efficiency: request >= 2^61");
+        }
+        if (k > 0 && !placed->executor_nodes) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: executor_nodes is NULL");
+        if (off[(size_t)i] < 0 || off[(size_t)i] + k > placed->executor_nodes_cap)
+            return fail(c, GP_ERR_CAPACITY, "gp_packing_efficiency: offsets exceed executor_nodes_cap");
+        for (int64_t t = 0; t < k; ++t) {
+            const int32_t n = placed->executor_nodes[off[(size_t)i] + t];
+            if (n < 0 || n >= c->n_nodes) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: executor node out of range");
+        }
+    }
+    off[(size_t)Q] = a->exec_out_off ? a->exec_out_off[Q] : acc;
+    const int64_t total = placed->executor_nodes_cap < off[(size_t)Q] ? placed->executor_nodes_cap : off[(size_t)Q];
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    const size_t q = (size_t)Q, T = (size_t)(total > 0 ? total : 0), N = (size_t)c->n_nodes;
+    const int TH = kEffThreads;
+    const int n_part = (int)std::max<size_t>(1, std::min<size_t>((N + TH - 1) / TH, (size_t)c->sm_count * 4));
+    Arena ar{c->zonebuf};
+    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_drv = ar.take(4 * q), o_exe = ar.take(4 * (T + 1)),
+                 o_part = ar.take(sizeof(EffAcc) * (size_t)n_part), o_base = ar.take(sizeof(EffAcc)), o_avg = ar.take(32 * q), o_err = ar.take(4);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    EffRowsIn ri{};
+    gp_status s = upload_app_columns(c, a, off.data(), b, o_in, o_cnt, o_off, st, &ri.cols);
+    if (s != GP_OK) return s;
+    GP_CUDA(c, cudaMemcpyAsync(b + o_drv, placed->driver_node, 4 * q, cudaMemcpyHostToDevice, st));
+    if (T) GP_CUDA(c, cudaMemcpyAsync(b + o_exe, placed->executor_nodes, 4 * T, cudaMemcpyHostToDevice, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_err, 0, 4, st));
+    int* d_err = (int*)(b + o_err);
+    EffBaseIn bi{};
+    bi.av = SnapshotAvail{c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->node_slot.as<int32_t>(), c->node_cpu.as<long long>(),
+                      c->node_mem.as<long long>(), c->node_gpu.as<long long>()};
+    bi.sched[0] = c->sched.as<long long>(); bi.sched[1] = c->sched.as<long long>() + N; bi.sched[2] = c->sched.as<long long>() + 2 * N;
+    bi.n_nodes = c->n_nodes;
+    EffAcc* base = (EffAcc*)(b + o_base);
+    gp_eff_base<<<n_part, TH, 0, st>>>(bi, (EffAcc*)(b + o_part), d_err);
+    gp_eff_finish<<<1, TH, 0, st>>>((const EffAcc*)(b + o_part), n_part, base);
+    ri.av = bi.av;
+    for (int k = 0; k < 3; ++k) ri.sched[k] = bi.sched[k];
+    ri.count = (const int32_t*)(b + o_cnt); ri.off = (const int64_t*)(b + o_off);
+    ri.driver = (const int32_t*)(b + o_drv); ri.exec = (const int32_t*)(b + o_exe); ri.base = base;
+    ri.n_apps = Q; ri.n_nodes = c->n_nodes;
+    ri.executors_reserved = algo == GP_MINIMAL_FRAGMENTATION ? 0 : 1;
+    ri.charged = (int32_t)charged;
+    gp_eff_rows<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(ri, (double*)(b + o_avg), d_err);
+    GP_CUDA(c, cudaGetLastError());
+    int herr = 0;
+    GP_CUDA(c, cudaMemcpyAsync(avg_out, b + o_avg, 32 * q, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    if (herr & kEffErrQuantity)
+        return fail(c, GP_ERR_UNREPRESENTABLE, "gp_packing_efficiency: a per-node reserved amount is >= 2^61");
+    if (herr & kEffErrRange)
+        return fail(c, GP_ERR_UNREPRESENTABLE, "gp_packing_efficiency: an efficiency term outside the exact accumulator's range");
+    return GP_OK;
+}
+
 // ---- node priority order (f1) and availability snapshot (f2): device stages + the entries built on them ----
 }  // extern "C"
 
@@ -2185,10 +2280,14 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
     dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = so.drv;
     s = build_snapshot_device(c, &dn, n, n, st);      // n is the upper bound of both order lengths
     if (s != GP_OK) return s;
+    // SchedulableResources for gp_packing_efficiency (the zone entry points still want gp_set_schedulable)
+    GP_CUDA(c, c->sched.reserve(24 * (N + 1)));
+    GP_CUDA(c, cudaMemcpyAsync(c->sched.p, d_sched, 24 * N, cudaMemcpyDeviceToDevice, st));
     int32_t counts[3] = {0, 0, 0};
     GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
     c->n_drv = counts[0]; c->n_exec = counts[1];
+    c->have_eff_sched = true;
     if (sort->undefined_ties) *sort->undefined_ties = counts[2];
     if (n_driver) *n_driver = counts[0];
     if (n_executor) *n_executor = counts[1];
@@ -2282,6 +2381,7 @@ gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const
     GP_CUDA(c, cudaStreamSynchronize(st));
     c->n_groups = hinfo[kZiGroups]; c->n_exec = hinfo[kZiExec]; c->n_drv = hinfo[kZiDrv];
     c->have_sched = true;
+    c->have_eff_sched = true;
     c->zone_orders = gp_az_orders{hinfo[kZiZones], counts[1], uexe, counts[0], udrv};
     c->zone_kind = kind;
     if (sort->undefined_ties) *sort->undefined_ties = counts[2];

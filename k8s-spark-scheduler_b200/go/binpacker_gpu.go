@@ -264,6 +264,99 @@ func efficienciesFor(md resources.NodeGroupSchedulingMetadata, drv, exe *resourc
 	return binpack.ComputePackingEfficiencies(md, reserved)
 }
 
+// AvgPackingEfficiencyForResult is computeAvgPackingEfficiencyForResult (EXT/resource.go:372-381), the metric the
+// Predicate reports at :352, over EVERY node of nodesSchedulingMetadata -- the metadata the packer saw -- with `reserved`
+// rebuilt from the placement (minimalFragmentation: the driver only).  It marshals the whole node table (availability and
+// SchedulableResources, every node as an executor candidate so the snapshot covers them all), uploads it and makes ONE
+// gp_packing_efficiency call; it never relies on a snapshot an earlier call left on the context, whose node table may be
+// another one (the packers here upload only the nodes of their priority orders).  The sums are rounded once from their
+// exact value: the Go loop sums in map order, so the two agree within the recursive-summation bound (bit for bit when
+// every partial sum is exact).  A shim that keeps a gp_prepare_cluster / gp_prepare_cluster_zones snapshot resident calls
+// gp_packing_efficiency on it directly instead (INTEGRATION.md, the Predicate recipe's step 4).
+// ok=false (no device, a name outside the metadata, an inexact quantity, a device error): the caller runs the Go
+// computeAvgPackingEfficiencyForResult on the PackingEfficiencies the Go packer returns.
+func AvgPackingEfficiencyForResult(nodesSchedulingMetadata resources.NodeGroupSchedulingMetadata,
+	driverResources, executorResources *resources.Resources, result *binpack.PackingResult,
+	minimalFragmentation bool) (binpack.AvgPackingEfficiency, bool) {
+	if result == nil || !result.HasCapacity {
+		return binpack.WorstAvgPackingEfficiency(), true
+	}
+	d, err := getDevice()
+	if err != nil {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	dc, dm, dg, ok1 := toTriple(driverResources)
+	ec, em, eg, ok2 := toTriple(executorResources)
+	if !ok1 || !ok2 {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	all := make([]string, 0, len(nodesSchedulingMetadata))
+	for n := range nodesSchedulingMetadata {
+		all = append(all, n)
+	}
+	s, ok := marshal(nodesSchedulingMetadata, nil, all)
+	if !ok {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	index := make(map[string]int32, len(s.names))
+	sc, sm, sg := make([]int64, len(s.names)+1), make([]int64, len(s.names)+1), make([]int64, len(s.names)+1)
+	for i, n := range s.names {
+		index[n] = int32(i)
+		c, m, g, exact := toTriple(nodesSchedulingMetadata[n].SchedulableResources)
+		if !exact {
+			return binpack.AvgPackingEfficiency{}, false
+		}
+		sc[i], sm[i], sg[i] = c, m, g
+	}
+	driver, ok := index[result.DriverNode]
+	if !ok {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	execs := make([]int32, max(len(result.ExecutorNodes), 1))
+	for i, n := range result.ExecutorNodes {
+		v, ok := index[n]
+		if !ok {
+			return binpack.AvgPackingEfficiency{}, false
+		}
+		execs[i] = v
+	}
+	drv := []int64{dc, dm, dg}
+	exe := []int64{ec, em, eg}
+	count := []int32{int32(len(result.ExecutorNodes))}
+	off := []int64{0, int64(len(result.ExecutorNodes))}
+	drvNode := []int32{driver}
+	avg := make([]float64, 4)
+	algo := C.gp_algo(C.GP_TIGHTLY_PACK)
+	if minimalFragmentation {
+		algo = C.GP_MINIMAL_FRAGMENTATION
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	if err := d.setSnapshot(s); err != nil {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	if st := C.gp_set_schedulable(d.ctx, ptr64(sc), ptr64(sm), ptr64(sg)); st != C.GP_OK {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	// gp_apps / gp_results hold Go pointers: every slice base is pinned for the duration of the call
+	// (cgocheck: "Go pointer to unpinned Go pointer"), exactly as setSnapshot does for the node table.
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []any{&drv[0], &exe[0], &count[0], &off[0], &drvNode[0], &execs[0]} {
+		pin.Pin(p)
+	}
+	a := C.gp_apps{n_apps: 1, drv_cpu_milli: ptr64(drv[0:1]), drv_mem_bytes: ptr64(drv[1:2]), drv_gpu: ptr64(drv[2:3]),
+		exe_cpu_milli: ptr64(exe[0:1]), exe_mem_bytes: ptr64(exe[1:2]), exe_gpu: ptr64(exe[2:3]), exe_count: ptr32(count),
+		exec_out_off: ptr64(off)}
+	placed := C.gp_results{driver_node: ptr32(drvNode), executor_nodes: ptr32(execs), executor_nodes_cap: C.int64_t(len(execs))}
+	if C.gp_packing_efficiency(d.ctx, &a, algo, &placed, C.GP_MODE_INDEPENDENT, (*C.double)(unsafe.Pointer(&avg[0]))) != C.GP_OK {
+		return binpack.AvgPackingEfficiency{}, false
+	}
+	return binpack.AvgPackingEfficiency{CPU: avg[0], Memory: avg[1], GPU: avg[2], Max: avg[3]}, true
+}
+
 // TightlyPack / DistributeEvenly / MinimalFragmentation are drop-in values for binpack.TightlyPack /
 // binpack.DistributeEvenly / binpack.MinimalFragmentation.
 var (

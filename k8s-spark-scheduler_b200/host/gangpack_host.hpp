@@ -191,6 +191,29 @@ public:
         }
         check(gp_set_schedulable(ctx_, c.data(), m.data(), g.data()), "gp_set_schedulable");
     }
+    // Every node of the metadata in one executor-only group (no driver candidates): the node table of the
+    // cluster-wide packing efficiency (gp_packing_efficiency), with its SchedulableResources
+    void SetSnapshotAll(const resources::NodeGroupSchedulingMetadata& md) {
+        names_.clear(); index_.clear();
+        cpu_.clear(); mem_.clear(); gpu_.clear(); exec_.clear(); drv_.clear();
+        for (const auto& kv : md) {
+            index_.emplace(kv.first, (int32_t)names_.size());
+            exec_.push_back((int32_t)names_.size());
+            names_.push_back(kv.first);
+            cpu_.push_back(kv.second.AvailableResources.CPU);
+            mem_.push_back(kv.second.AvailableResources.Memory);
+            gpu_.push_back(kv.second.AvailableResources.NvidiaGPU);
+        }
+        int32_t eoff[2] = {0, (int32_t)exec_.size()}, doff[2] = {0, 0};
+        gp_nodes n{};
+        n.n_nodes = (int32_t)names_.size();
+        n.avail_cpu_milli = cpu_.data(); n.avail_mem_bytes = mem_.data(); n.avail_gpu = gpu_.data();
+        n.n_groups = 1;
+        n.exec_off = eoff; n.exec_order = exec_.data();
+        n.drv_off = doff; n.drv_order = drv_.data();
+        check(gp_set_snapshot(ctx_, &n), "gp_set_snapshot");
+        SetSchedulable(md);
+    }
     const std::string& name(int32_t i) const { return names_.at((size_t)i); }
     size_t n_nodes() const { return names_.size(); }
     int32_t index(const std::string& n) const { auto it = index_.find(n); return it == index_.end() ? -1 : it->second; }
@@ -868,6 +891,48 @@ inline std::pair<std::string, bool> RescheduleExecutorNode(const binpacker::Binp
     d.check(gp_reschedule_executors(d.ctx(), &in, &node), "gp_reschedule_executors");
     if (node < 0) return {std::string(), false};
     return {d.name(node), true};
+}
+
+// computeAvgPackingEfficiencyForResult (internal/extender/resource.go:372-381): the Predicate's packing-efficiency metric,
+// ComputeAvgPackingEfficiency over the PackingEfficiencies of EVERY node of nodesSchedulingMetadata, with `reserved` rebuilt
+// from the placement (binpack.go:72-77: driver + every executor; minimal-fragmentation -- algo GP_MINIMAL_FRAGMENTATION,
+// also for single-az-minimal-fragmentation winners -- the driver only).  Computed by one gp_packing_efficiency call; its
+// sums are rounded once from their exact value, so it agrees with the Go loop (map order) within the recursive-summation
+// bound and bit for bit where every partial sum is exact.  The Go function reads packingResult.PackingEfficiencies; this
+// layer's PackingResult does not carry them, so the resources of the placed application are passed instead.
+// EmptyPackingResult -> WorstAvgPackingEfficiency.
+inline binpack::AvgPackingEfficiency ComputeAvgPackingEfficiencyForResult(const resources::NodeGroupSchedulingMetadata& nodesSchedulingMetadata,
+                                                                           const binpack::PackingResult& packingResult,
+                                                                           const resources::Resources& driverResources,
+                                                                           const resources::Resources& executorResources,
+                                                                           gp_algo algo = GP_TIGHTLY_PACK) {
+    if (!packingResult.HasCapacity) return binpack::WorstAvgPackingEfficiency();
+    gangpack::Device& d = gangpack::Device::Get();
+    d.SetSnapshotAll(nodesSchedulingMetadata);
+    auto idx = [&](const std::string& n) {
+        const int32_t i = d.index(n);
+        if (i < 0) throw gangpack::Error(GP_ERR_INVALID, "ComputeAvgPackingEfficiencyForResult: node not in the metadata: " + n);
+        return i;
+    };
+    int32_t driver = idx(packingResult.DriverNode);
+    std::vector<int32_t> execs;
+    for (const auto& n : packingResult.ExecutorNodes) execs.push_back(idx(n));
+    const int32_t count = (int32_t)execs.size();
+    if (execs.empty()) execs.push_back(0);
+    const int64_t drv[3] = {driverResources.CPU, driverResources.Memory, driverResources.NvidiaGPU};
+    const int64_t exe[3] = {executorResources.CPU, executorResources.Memory, executorResources.NvidiaGPU};
+    const int64_t off[2] = {0, count};
+    gp_apps a{};
+    a.n_apps = 1;
+    a.drv_cpu_milli = &drv[0]; a.drv_mem_bytes = &drv[1]; a.drv_gpu = &drv[2];
+    a.exe_cpu_milli = &exe[0]; a.exe_mem_bytes = &exe[1]; a.exe_gpu = &exe[2];
+    a.exe_count = &count; a.exec_out_off = off;
+    gp_results r{&driver, execs.data(), (int64_t)execs.size()};
+    double avg[4] = {0, 0, 0, 0};
+    d.check(gp_packing_efficiency(d.ctx(), &a, algo, &r, GP_MODE_INDEPENDENT, avg), "gp_packing_efficiency");
+    binpack::AvgPackingEfficiency out;
+    out.CPU = avg[0]; out.Memory = avg[1]; out.GPU = avg[2]; out.Max = avg[3];
+    return out;
 }
 
 // The two zone labels rescheduleExecutor reads, and they differ (SURVEY App. B5): PotentialNodes sorts by

@@ -18,7 +18,7 @@ LIB_PATH = os.environ.get("GANGPACK_LIB") or os.path.join(_PKG, "libgangpack.so"
 _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack_kernels.cuh", "gangpack_fifo.cuh", "gangpack_minfrag.cuh",
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
                                                     "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
-                                                    "gangpack_reschedprep.cuh")] + [
+                                                    "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -39,7 +39,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_free_pinned", "gp_register_host", "gp_unregister_host", "gp_set_snapshot", "gp_get_snapshot", "gp_pack_batch", "gp_pack_batch_wire", "gp_pack_one", "gp_set_schedulable", "gp_pack_batch_zones", "gp_pack_fifo_zones", "gp_pack_fifo_az_aware", "gp_pack_batch_az_aware", "gp_reserve_placements", "gp_apply_usage_delta",
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
-           "gp_reschedule_executors", "gp_reschedule_from_reservations",
+           "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -214,6 +214,8 @@ def load():
     L.gp_reserve_placements.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_results), C.c_int32, C.POINTER(gp_reservation_table)]
     L.gp_apply_usage_delta.restype = C.c_int
     L.gp_apply_usage_delta.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
+    L.gp_packing_efficiency.restype = C.c_int
+    L.gp_packing_efficiency.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_results), C.c_int, C.c_void_p]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -721,6 +723,26 @@ class GangPacker:
     def apply_usage_delta(self, node, cpu, mem, gpu=None, sign=1):
         n, c, m, g = _np(node, np.int32), _np(cpu, np.int64), _np(mem, np.int64), _np(gpu, np.int64)
         self._check(load().gp_apply_usage_delta(self._h, len(n), _p(n), _p(c), _p(m), _p(g), sign))
+
+    def packing_efficiency(self, apps: dict, placed, algo: int, charged: int = MODE_INDEPENDENT) -> np.ndarray:
+        """computeAvgPackingEfficiencyForResult of each placed application over EVERY node of the snapshot, exactly summed
+        -> (n_apps, 4) float64 {CPU, Memory, GPU, Max}.  placed = (driver_node, executor_nodes, off) as pack_batch returns
+        them (zone results: (driver_node, executor_nodes, off) of the zone call).  algo decides what counts as reserved
+        (MINIMAL_FRAGMENTATION: the driver only); charged = MODE_FIFO_* adds that one application's charged usage back first."""
+        q = len(apps["count"])
+        count = _np(apps["count"], np.int32)
+        driver, execn, off = placed
+        driver = _np(driver, np.int32); execn = _np(execn, np.int32); off = _np(off, np.int64)
+        if execn is None or len(execn) == 0:
+            execn = np.zeros(1, np.int32)
+        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
+        avg = np.zeros((max(q, 1), 4), np.float64)
+        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
+                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
+                    exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
+        r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
+        self._check(load().gp_packing_efficiency(self._h, C.byref(a), algo, C.byref(r), charged, _p(avg)))
+        return avg[:q]
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
