@@ -535,6 +535,46 @@ gp_status gp_apply_usage_delta(gp_ctx* ctx, int64_t n_rows, const int32_t* node,
 gp_status gp_packing_efficiency(gp_ctx* ctx, const gp_apps* apps, gp_algo algo, const gp_results* placed /* host */,
                                 gp_mode charged, double* avg_out /* [n_apps][4] */);
 
+/* ---- the unschedulable-pod marker's capacity checks (EXT/unschedulablepods.go:93-166) ------------------------------------
+ * DoesPodExceedClusterCapacity (:132-166) for a batch of stale drivers, under any `binpack:` value, in one call.  Each driver is
+ * packed against the nodes of its affinity class with zero usage -- NodeSchedulingMetadataForNodes(nodes, zero usage, overhead)
+ * (LIB/resources/resources.go:61-100), so available = schedulable = allocatable - overhead on every node, unschedulable and
+ * not-ready nodes included -- and the affinity nodes in lister order as both priority orders; exceeds[i] = !HasCapacity.
+ * The answer depends on neither that order nor any placement (DESIGN §2.2): no sort, no layout and no placement is computed.
+ *   nodes       allocatable and GetNonSchedulableOverhead per node; zone_id = ZoneLabel (failure-domain.beta.kubernetes.io/zone,
+ *               "default" when absent) interned to 0..n_zones-1, NULL = one zone (only the single-AZ packers look at it);
+ *               node_group = the affinity class of each node (0..n_groups-1), -1 = in none, NULL = every node in class 0.
+ *   drivers     gp_apps with group = the driver's affinity class, -1 = its required affinity matches every node, NULL = 0;
+ *               exe_count any int32 >= 0 (no 2^24 bound); skip_if_no_fit and exec_out_off are ignored.
+ *   An affinity class with no nodes gives exceeds = 1.
+ * The call is stateless with respect to the context: the snapshot, SchedulableResources, the zone layout, the held az-aware
+ * orders and gp_last_stats are left untouched; it has scratch of its own and synchronises the stream once, at the end.
+ * GP_ERR_INVALID (gp_last_error names the cause): a negative request or exe_count, a group or zone id out of range, an unknown
+ * packer, n_groups < 1.  GP_ERR_UNREPRESENTABLE: a request, |allocatable| or |overhead| >= 2^61.  The node table is
+ * validated with n_apps == 0 too.  On an error exceeds is undefined. */
+typedef enum {
+    GP_BP_TIGHTLY_PACK = 0,                    /* "tightly-pack" */
+    GP_BP_DISTRIBUTE_EVENLY = 1,               /* "distribute-evenly" */
+    GP_BP_AZ_AWARE_TIGHTLY_PACK = 2,           /* "az-aware-tightly-pack" */
+    GP_BP_SINGLE_AZ_TIGHTLY_PACK = 3,          /* "single-az-tightly-pack" */
+    GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION = 4  /* "single-az-minimal-fragmentation" */
+} gp_binpacker;
+typedef struct {
+    int32_t n_nodes;
+    const int64_t* alloc_cpu_milli;      /* [n_nodes] node.Status.Allocatable */
+    const int64_t* alloc_mem_bytes;
+    const int64_t* alloc_gpu;            /* or NULL (= 0) */
+    const int64_t* overhead_cpu_milli;   /* [n_nodes] GetNonSchedulableOverhead, or NULL (= 0) */
+    const int64_t* overhead_mem_bytes;   /* or NULL */
+    const int64_t* overhead_gpu;         /* or NULL */
+    int32_t n_zones;                     /* >= 1 when zone_id is given */
+    const int32_t* zone_id;              /* [n_nodes] or NULL (one zone) */
+    int32_t n_groups;                    /* >= 1 */
+    const int32_t* node_group;           /* [n_nodes] affinity class, -1 = none; or NULL (all 0) */
+} gp_capacity_nodes;
+gp_status gp_exceeds_cluster_capacity(gp_ctx* ctx, const gp_capacity_nodes* nodes, const gp_apps* drivers, gp_binpacker packer,
+                                      uint8_t* exceeds /* [n_apps] */);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

@@ -12,6 +12,7 @@
 #include "gangpack_zonelayout.cuh"
 #include "gangpack_reschedprep.cuh"
 #include "gangpack_efficiency.cuh"
+#include "gangpack_capacity.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -456,6 +457,7 @@ struct gp_ctx {
     // current snapshot, -1 when another entry laid it out
     DevBuf zoneprep;
     DevBuf reschedprep;                           // gp_reschedule_from_reservations' own scratch (no state points into it)
+    DevBuf capprep;                               // gp_exceeds_cluster_capacity's own scratch (no state points into it)
     int zone_kind = -1;
     gp_az_orders zone_orders{};
     bool sort_attr_set = false;
@@ -2608,5 +2610,116 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     return GP_OK;
 }
 
+// DoesPodExceedClusterCapacity for a batch of stale drivers, any packer (EXT/unschedulablepods.go:132-166); see
+// gangpack_capacity.cuh and DESIGN §2.2
+gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds) {
+    if (!c) return GP_ERR_INVALID;
+    static const char* who = "gp_exceeds_cluster_capacity";
+    auto bad = [&](gp_status st, const char* what) { return fail(c, st, std::string(who) + ": " + what); };
+    if (!nodes || !a || nodes->n_nodes < 0 || a->n_apps < 0 || nodes->n_groups < 1 || (nodes->zone_id && nodes->n_zones < 1) ||
+        (nodes->n_nodes > 0 && (!nodes->alloc_cpu_milli || !nodes->alloc_mem_bytes)) ||
+        (a->n_apps > 0 && (!a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !exceeds)))
+        return bad(GP_ERR_INVALID, "missing arrays or bad sizes (n_groups >= 1; n_zones >= 1 with zone_id)");
+    if ((int)packer < GP_BP_TIGHTLY_PACK || (int)packer > GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) return bad(GP_ERR_INVALID, "unknown packer");
+    const int32_t n = nodes->n_nodes, Q = a->n_apps;
+    const int32_t Z = nodes->zone_id ? nodes->n_zones : 1, G = nodes->n_groups;
+    if ((int64_t)(G + 1) * Z > (int64_t)INT32_MAX / 2) return bad(GP_ERR_INVALID, "(n_groups + 1) * n_zones too large");
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    const size_t N = (size_t)n, q = (size_t)Q, B = (size_t)(G + 1) * (size_t)Z;
+    size_t H = 64;
+    while (H < 2 * q) H <<= 1;                          // more slots than drivers: every probe ends
+    // every node sits in its class's bucket and in a bucket of class slot G: 2N entries
+    const size_t n_segs = 2 * N / kCapSeg + B + 1;
+    // buckets of more than kCapSeg nodes: at most 2N / (kCapSeg + 1), whatever the number of zones
+    const int32_t ms_stride = (int32_t)std::max<size_t>(1, 2 * N / ((size_t)kCapSeg + 1));
+    const int32_t pairs_per_chunk = (int32_t)std::max<int64_t>(1, std::min<int64_t>(std::max(Q, 1), kCapSlotEntries / ms_stride));
+    const size_t A = (size_t)pairs_per_chunk * (size_t)ms_stride;
+    const size_t q1 = std::max<size_t>(q, 1);
+    Arena ar{c->capprep};
+    const size_t o_alloc = ar.take(24 * N), o_over = ar.take(24 * N), o_zone = ar.take(4 * N), o_grp = ar.take(4 * N), o_key = ar.take(8 * N),
+                 o_rank = ar.take(8 * N), o_staged = ar.take(24 * N), o_sched = ar.take(48 * N), o_bcnt = ar.take(4 * B),
+                 o_boff = ar.take(4 * (B + 1)), o_soff = ar.take(4 * (B + 1)), o_moff = ar.take(4 * (B + 1)), o_segs = ar.take(sizeof(CapSeg) * n_segs),
+                 o_q = ar.take(48 * q), o_cnt = ar.take(4 * q), o_ag = ar.take(4 * q), o_hash = ar.take(sizeof(CapEntry) * H),
+                 o_pairs = ar.take(sizeof(CapPair) * q), o_np = ar.take(8), o_err = ar.take(8), o_ap = ar.take(4 * q),
+                 o_pref = ar.take(8 * (q + 1)), o_slots = ar.take(sizeof(CapSlot) * A), o_T = ar.take(8 * q1),
+                 o_M = ar.take(8 * q1), o_zb = ar.take(8 * q1), o_out = ar.take(q1);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
+    // n_pairs and the error word are adjacent: one memset clears both
+    GP_CUDA(c, cudaMemsetAsync(b + o_bcnt, 0, 4 * B, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_hash, 0, sizeof(CapEntry) * H, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_np, 0, o_ap - o_np, st));
+    CapScratch s{};
+    s.key = (int32_t*)(b + o_key); s.rank = (int32_t*)(b + o_rank); s.bucket_cnt = (int32_t*)(b + o_bcnt);
+    s.bucket_off = (int32_t*)(b + o_boff); s.seg_off = (int32_t*)(b + o_soff); s.ms_off = (int32_t*)(b + o_moff);
+    for (int d = 0; d < 3; ++d) { s.staged[d] = (long long*)(b + o_staged) + d * N; s.sched[d] = (long long*)(b + o_sched) + 2 * d * N; }
+    s.segs = (CapSeg*)(b + o_segs); s.err = (int*)(b + o_err);
+    s.B = (int32_t)B; s.Z = Z; s.G = G; s.n = n;
+    const int T = 256;
+    if (n > 0) {
+        CapNodesIn ni{};
+        ni.n = n;
+        const int64_t* cols[6] = {nodes->alloc_cpu_milli, nodes->alloc_mem_bytes, nodes->alloc_gpu,
+                                  nodes->overhead_cpu_milli, nodes->overhead_mem_bytes, nodes->overhead_gpu};
+        for (int d = 0; d < 6; ++d) {
+            if (!cols[d]) continue;
+            const size_t o = (d < 3 ? o_alloc : o_over) + 8 * N * (size_t)(d % 3);
+            GP_CUDA(c, up(o, cols[d], 8 * N));
+            (d < 3 ? ni.alloc : ni.over)[d % 3] = (const long long*)(b + o);
+        }
+        if (nodes->zone_id) { GP_CUDA(c, up(o_zone, nodes->zone_id, 4 * N)); ni.zone = (const int32_t*)(b + o_zone); }
+        if (nodes->node_group) { GP_CUDA(c, up(o_grp, nodes->node_group, 4 * N)); ni.group = (const int32_t*)(b + o_grp); }
+        gp_cc_nodes<<<(unsigned)((N + T - 1) / T), T, 0, st>>>(ni, s);
+    }
+    gp_cc_bucket_scan<<<1, 1024, 0, st>>>(s);
+    if (n > 0) gp_cc_scatter<<<(unsigned)((2 * N + T - 1) / T), T, 0, st>>>(s);
+    CapAppsIn ai{};
+    ai.n = Q;
+    const int64_t* qcols[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
+    for (int t = 0; t < 6; ++t) {
+        if (!qcols[t]) continue;
+        GP_CUDA(c, up(o_q + 8 * q * (size_t)t, qcols[t], 8 * q));
+        ai.q[t] = (const long long*)(b + o_q) + q * (size_t)t;
+    }
+    if (Q > 0) GP_CUDA(c, up(o_cnt, a->exe_count, 4 * q));
+    ai.count = (const int32_t*)(b + o_cnt);
+    if (a->group && Q > 0) { GP_CUDA(c, up(o_ag, a->group, 4 * q)); ai.group = (const int32_t*)(b + o_ag); }
+    ai.n_groups = G;
+    ai.hash_mask = (uint32_t)(H - 1);
+    CapPair* pairs = (CapPair*)(b + o_pairs);
+    int32_t* n_pairs = (int32_t*)(b + o_np);
+    int32_t* app_pair = (int32_t*)(b + o_ap);
+    if (Q > 0) gp_cc_intern<<<(unsigned)((q + T - 1) / T), T, 0, st>>>(ai, (CapEntry*)(b + o_hash), pairs, n_pairs, app_pair, s.err);
+    long long* pref = (long long*)(b + o_pref);
+    CapPairOut po{(unsigned long long*)(b + o_T), (long long*)(b + o_M), (long long*)(b + o_zb)};
+    gp_cc_pair_scan<<<1, 1024, 0, st>>>(s, pairs, n_pairs, pref, po);
+    CapPassIn pi{};
+    pi.s = s; pi.pairs = pairs; pi.n_pairs = n_pairs; pi.pref = pref; pi.out = po;
+    pi.slots = (CapSlot*)(b + o_slots); pi.ms_stride = ms_stride;
+    // The number of pairs is only known on the device; chunks beyond it return at once.  One chunk unless the pairs times
+    // the multi-segment buckets exceed kCapSlotEntries (100 000 pairs over 50 000 nodes: 2.4 million slots, two chunks).
+    const int pass_blocks = c->sm_count * 8;
+    for (int32_t p0 = 0; p0 < Q; p0 += pairs_per_chunk) {
+        pi.p0 = p0; pi.p1 = (int32_t)std::min<int64_t>((int64_t)p0 + pairs_per_chunk, Q);
+        if (2 * N > (size_t)kCapSeg) gp_cc_clear<<<(unsigned)std::min<size_t>((A + T - 1) / T, (size_t)c->sm_count * 16), T, 0, st>>>(pi);
+        gp_cc_pass<<<pass_blocks, kCapThreads, 0, st>>>(pi);
+    }
+    uint8_t* d_out = (uint8_t*)(b + o_out);
+    if (Q > 0) gp_cc_decide<<<(unsigned)((q + T - 1) / T), T, 0, st>>>(Q, ai.count, app_pair, pairs, po, (int32_t)packer, d_out);
+    GP_CUDA(c, cudaGetLastError());
+    int herr = 0;
+    if (Q > 0) GP_CUDA(c, cudaMemcpyAsync(exceeds, d_out, q, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaMemcpyAsync(&herr, s.err, 4, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    if (herr & kCcErrNegative) return bad(GP_ERR_INVALID, "negative resource request or exe_count");
+    if (herr & kCcErrGroup) return bad(GP_ERR_INVALID, "driver group out of range (-1 or 0..n_groups-1)");
+    if (herr & kCcErrZone) return bad(GP_ERR_INVALID, "zone_id out of range");
+    if (herr & kCcErrNodeGroup) return bad(GP_ERR_INVALID, "node_group out of range (-1 or 0..n_groups-1)");
+    if (herr & kCcErrUnrepresentable) return bad(GP_ERR_UNREPRESENTABLE, "request >= 2^61");
+    if (herr & kCcErrNodeQuantity) return bad(GP_ERR_UNREPRESENTABLE, "|allocatable| or |overhead| >= 2^61");
+    return GP_OK;
+}
 
 }  // extern "C"

@@ -21,6 +21,7 @@ import "C"
 import (
 	"context"
 	"fmt"
+	"math"
 	"runtime"
 	"sort"
 	"sync"
@@ -1149,4 +1150,108 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 		}
 	}
 	return fits, true
+}
+
+// StaleDriver is one driver the unschedulable-pod marker checks (scanForUnschedulablePods, EXT/unschedulablepods.go:93-129):
+// its application resources and the affinity class of its required node affinity, an index into the classes the caller
+// assigns to the nodes (-1: the affinity matches every node).
+type StaleDriver struct {
+	DriverResources, ExecutorResources *resources.Resources
+	MinExecutorCount                   int
+	AffinityClass                      int32
+}
+
+// gpBinpacker maps a `binpack:` value to the device packer; unknown names select distribute-evenly, like SelectBinpacker
+// (internal/binpacker/binpack.go:52-58).
+func gpBinpacker(name string) C.gp_binpacker {
+	switch name {
+	case "tightly-pack":
+		return C.GP_BP_TIGHTLY_PACK
+	case "az-aware-tightly-pack":
+		return C.GP_BP_AZ_AWARE_TIGHTLY_PACK
+	case "single-az-tightly-pack":
+		return C.GP_BP_SINGLE_AZ_TIGHTLY_PACK
+	case "single-az-minimal-fragmentation":
+		return C.GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION
+	}
+	return C.GP_BP_DISTRIBUTE_EVENLY
+}
+
+// DoesPodsExceedClusterCapacity is DoesPodExceedClusterCapacity (EXT/unschedulablepods.go:132-166) for every stale driver of
+// one marker sweep in ONE gp_exceeds_cluster_capacity call, whatever the `binpack:` value.  nodesSchedulingMetadata is
+// NodeSchedulingMetadataForNodes(every node, zero usage, GetNonSchedulableOverhead): only SchedulableResources and ZoneLabel
+// are read.  nodeClass gives the affinity class of each node (absent: in none of the nClasses classes).  The device context's
+// resident snapshot is not touched.  ok=false (no device, an inexact quantity, a count outside int32, any non-OK status):
+// the caller runs DoesPodExceedClusterCapacity per driver in Go.  Cost: one evaluation per node of a class per distinct
+// (executor shape, driver shape) pair; for tightly-pack / distribute-evenly sweeps with thousands of distinct pairs,
+// gp_pack_batch with one instance group per class is faster (INTEGRATION.md, the marker's "Cost" note).
+func DoesPodsExceedClusterCapacity(binpackerName string, nodesSchedulingMetadata resources.NodeGroupSchedulingMetadata,
+	nodeClass map[string]int32, nClasses int32, drivers []StaleDriver) ([]bool, bool) {
+	d, err := getDevice()
+	if err != nil {
+		return nil, false
+	}
+	n, q := len(nodesSchedulingMetadata), len(drivers)
+	sc, sm, sg := make([]int64, n+1), make([]int64, n+1), make([]int64, n+1)
+	zone, group := make([]int32, n+1), make([]int32, n+1)
+	zoneID := map[string]int32{}
+	i := 0
+	for name, md := range nodesSchedulingMetadata {
+		c, m, g, exact := toTriple(md.SchedulableResources)
+		if !exact {
+			return nil, false
+		}
+		sc[i], sm[i], sg[i] = c, m, g
+		z, seen := zoneID[md.ZoneLabel]
+		if !seen {
+			z = int32(len(zoneID))
+			zoneID[md.ZoneLabel] = z
+		}
+		zone[i] = z
+		group[i] = -1
+		if cls, in := nodeClass[name]; in {
+			group[i] = cls
+		}
+		i++
+	}
+	var cols [6][]int64
+	for t := range cols {
+		cols[t] = make([]int64, q+1)
+	}
+	count, class := make([]int32, q+1), make([]int32, q+1)
+	for j, drv := range drivers {
+		dc, dm, dg, ok1 := toTriple(drv.DriverResources)
+		ec, em, eg, ok2 := toTriple(drv.ExecutorResources)
+		if !ok1 || !ok2 || drv.MinExecutorCount < 0 || drv.MinExecutorCount > math.MaxInt32 {
+			return nil, false
+		}
+		cols[0][j], cols[1][j], cols[2][j], cols[3][j], cols[4][j], cols[5][j] = dc, dm, dg, ec, em, eg
+		count[j], class[j] = int32(drv.MinExecutorCount), drv.AffinityClass
+	}
+	exceeds := make([]uint8, q+1)
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	// the two C structs hold Go pointers: every slice base is pinned for the duration of the call
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []any{&sc[0], &sm[0], &sg[0], &zone[0], &group[0], &count[0], &class[0], &exceeds[0]} {
+		pin.Pin(p)
+	}
+	for t := range cols {
+		pin.Pin(&cols[t][0])
+	}
+	nodes := C.gp_capacity_nodes{n_nodes: C.int32_t(n), alloc_cpu_milli: ptr64(sc), alloc_mem_bytes: ptr64(sm), alloc_gpu: ptr64(sg),
+		n_zones: C.int32_t(max(len(zoneID), 1)), zone_id: ptr32(zone), n_groups: C.int32_t(max(nClasses, 1)), node_group: ptr32(group)}
+	a := C.gp_apps{n_apps: C.int32_t(q), drv_cpu_milli: ptr64(cols[0]), drv_mem_bytes: ptr64(cols[1]), drv_gpu: ptr64(cols[2]),
+		exe_cpu_milli: ptr64(cols[3]), exe_mem_bytes: ptr64(cols[4]), exe_gpu: ptr64(cols[5]), exe_count: ptr32(count), group: ptr32(class)}
+	if C.gp_exceeds_cluster_capacity(d.ctx, &nodes, &a, gpBinpacker(binpackerName), ptr8(exceeds)) != C.GP_OK {
+		return nil, false
+	}
+	out := make([]bool, q)
+	for j := range out {
+		out[j] = exceeds[j] != 0
+	}
+	return out, true
 }

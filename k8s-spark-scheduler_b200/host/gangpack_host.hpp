@@ -1045,4 +1045,70 @@ inline RescheduleOutcome RescheduleExecutor(const binpacker::Binpacker& packer, 
     return out;
 }
 
+// The unschedulable-pod marker's capacity checks (scanForUnschedulablePods, internal/extender/unschedulablepods.go:93-129) for
+// ALL stale drivers in one device call (gp_exceeds_cluster_capacity) instead of one DoesPodExceedClusterCapacity (:132-166) each.
+class UnschedulablePodMarker {
+public:
+    struct StaleDriver {
+        resources::Resources DriverResources;
+        resources::Resources ExecutorResources;
+        int MinExecutorCount = 0;
+        int AffinityClass = -1;        // index into the caller's affinity classes; -1 = the required affinity matches every node
+    };
+    explicit UnschedulablePodMarker(const binpacker::Binpacker& packer) : packer_(packer) {}
+
+    // nodesSchedulingMetadata: NodeSchedulingMetadataForNodes(every node, zero usage, GetNonSchedulableOverhead) -- only
+    // SchedulableResources and ZoneLabel are read.  nodeClass: the affinity class of each node (absent = in none);
+    // nClasses: the number of classes.  -> exceeds[i] for drivers[i].  The device context's resident snapshot is not touched.
+    std::vector<bool> DoesPodsExceedClusterCapacity(const resources::NodeGroupSchedulingMetadata& nodesSchedulingMetadata,
+                                                    const std::unordered_map<std::string, int32_t>& nodeClass, int32_t nClasses,
+                                                    const std::vector<StaleDriver>& drivers) const {
+        const size_t N = nodesSchedulingMetadata.size(), Q = drivers.size();
+        std::vector<int64_t> sc, sm, sg;
+        std::vector<int32_t> zone, group;
+        sc.reserve(N); sm.reserve(N); sg.reserve(N); zone.reserve(N); group.reserve(N);
+        std::unordered_map<std::string, int32_t> zoneId;
+        for (const auto& kv : nodesSchedulingMetadata) {
+            const auto& s = kv.second.SchedulableResources;
+            sc.push_back(s.CPU); sm.push_back(s.Memory); sg.push_back(s.NvidiaGPU);
+            zone.push_back(zoneId.emplace(kv.second.ZoneLabel, (int32_t)zoneId.size()).first->second);
+            auto c = nodeClass.find(kv.first);
+            group.push_back(c == nodeClass.end() ? -1 : c->second);
+        }
+        std::vector<int64_t> q[6];
+        std::vector<int32_t> count(Q), cls(Q);
+        for (auto& col : q) col.resize(Q);
+        for (size_t i = 0; i < Q; ++i) {
+            const StaleDriver& d = drivers[i];
+            q[0][i] = d.DriverResources.CPU; q[1][i] = d.DriverResources.Memory; q[2][i] = d.DriverResources.NvidiaGPU;
+            q[3][i] = d.ExecutorResources.CPU; q[4][i] = d.ExecutorResources.Memory; q[5][i] = d.ExecutorResources.NvidiaGPU;
+            count[i] = d.MinExecutorCount; cls[i] = d.AffinityClass;
+        }
+        gp_capacity_nodes n{};
+        n.n_nodes = (int32_t)N;
+        n.alloc_cpu_milli = sc.data(); n.alloc_mem_bytes = sm.data(); n.alloc_gpu = sg.data();   // schedulable = alloc - overhead
+        n.n_zones = std::max<int32_t>(1, (int32_t)zoneId.size()); n.zone_id = zone.data();
+        n.n_groups = std::max<int32_t>(1, nClasses); n.node_group = group.data();
+        gp_apps a{};
+        a.n_apps = (int32_t)Q;
+        a.drv_cpu_milli = q[0].data(); a.drv_mem_bytes = q[1].data(); a.drv_gpu = q[2].data();
+        a.exe_cpu_milli = q[3].data(); a.exe_mem_bytes = q[4].data(); a.exe_gpu = q[5].data();
+        a.exe_count = count.data(); a.group = cls.data();
+        std::vector<uint8_t> out(std::max<size_t>(Q, 1));
+        gangpack::Device& dev = gangpack::Device::Get();
+        dev.check(gp_exceeds_cluster_capacity(dev.ctx(), &n, &a, Packer(), out.data()), "gp_exceeds_cluster_capacity");
+        return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
+    }
+
+private:
+    gp_binpacker Packer() const {
+        if (packer_.Name == binpacker::tightlyPack) return GP_BP_TIGHTLY_PACK;
+        if (packer_.Name == binpacker::azAwareTightlyPack) return GP_BP_AZ_AWARE_TIGHTLY_PACK;
+        if (packer_.Name == binpacker::SingleAzTightlyPack) return GP_BP_SINGLE_AZ_TIGHTLY_PACK;
+        if (packer_.Name == binpacker::SingleAzMinimalFragmentation) return GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION;
+        return GP_BP_DISTRIBUTE_EVENLY;                 // SelectBinpacker's default
+    }
+    binpacker::Binpacker packer_;
+};
+
 }  // namespace extender

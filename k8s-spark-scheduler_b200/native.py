@@ -18,7 +18,7 @@ LIB_PATH = os.environ.get("GANGPACK_LIB") or os.path.join(_PKG, "libgangpack.so"
 _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack_kernels.cuh", "gangpack_fifo.cuh", "gangpack_minfrag.cuh",
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
                                                     "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
-                                                    "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh")] + [
+                                                    "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh", "gangpack_capacity.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -39,7 +39,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_free_pinned", "gp_register_host", "gp_unregister_host", "gp_set_snapshot", "gp_get_snapshot", "gp_pack_batch", "gp_pack_batch_wire", "gp_pack_one", "gp_set_schedulable", "gp_pack_batch_zones", "gp_pack_fifo_zones", "gp_pack_fifo_az_aware", "gp_pack_batch_az_aware", "gp_reserve_placements", "gp_apply_usage_delta",
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
-           "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency",
+           "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -157,6 +157,23 @@ class gp_reschedule_scope(C.Structure):
     _fields_ = [("keep_topology_zone", C.c_int32), ("reserved", C.c_int32), ("topology_zone", C.c_void_p)]
 
 
+# gp_binpacker: the `binpack:` config values (internal/binpacker/binpack.go:21-24, 43-49)
+BP_TIGHTLY_PACK = 0
+BP_DISTRIBUTE_EVENLY = 1
+BP_AZ_AWARE_TIGHTLY_PACK = 2
+BP_SINGLE_AZ_TIGHTLY_PACK = 3
+BP_SINGLE_AZ_MINIMAL_FRAGMENTATION = 4
+BINPACKERS = {"tightly-pack": BP_TIGHTLY_PACK, "distribute-evenly": BP_DISTRIBUTE_EVENLY,
+              "az-aware-tightly-pack": BP_AZ_AWARE_TIGHTLY_PACK, "single-az-tightly-pack": BP_SINGLE_AZ_TIGHTLY_PACK,
+              "single-az-minimal-fragmentation": BP_SINGLE_AZ_MINIMAL_FRAGMENTATION}
+
+
+class gp_capacity_nodes(C.Structure):
+    _fields_ = [("n_nodes", C.c_int32), ("alloc_cpu_milli", C.c_void_p), ("alloc_mem_bytes", C.c_void_p), ("alloc_gpu", C.c_void_p),
+                ("overhead_cpu_milli", C.c_void_p), ("overhead_mem_bytes", C.c_void_p), ("overhead_gpu", C.c_void_p),
+                ("n_zones", C.c_int32), ("zone_id", C.c_void_p), ("n_groups", C.c_int32), ("node_group", C.c_void_p)]
+
+
 class gp_stats(C.Structure):
     _fields_ = [("nodes_scanned", C.c_int64), ("drivers_tried", C.c_int64), ("kernel_launches", C.c_int64),
                 ("pack_kernel_ns", C.c_int64), ("prep_kernel_ns", C.c_int64), ("scan_path_apps", C.c_int64),
@@ -216,6 +233,8 @@ def load():
     L.gp_apply_usage_delta.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
     L.gp_packing_efficiency.restype = C.c_int
     L.gp_packing_efficiency.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_results), C.c_int, C.c_void_p]
+    L.gp_exceeds_cluster_capacity.restype = C.c_int
+    L.gp_exceeds_cluster_capacity.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.POINTER(gp_apps), C.c_int, C.c_void_p]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -743,6 +762,30 @@ class GangPacker:
         r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
         self._check(load().gp_packing_efficiency(self._h, C.byref(a), algo, C.byref(r), charged, _p(avg)))
         return avg[:q]
+
+    def exceeds_cluster_capacity(self, alloc, apps: dict, packer: int, overhead=None, zone_id=None, n_zones=1, node_group=None,
+                                 n_groups=1) -> np.ndarray:
+        """DoesPodExceedClusterCapacity for a batch of stale drivers under one `binpack:` packer (BP_*), in one device call.
+        alloc / overhead: (cpu, mem, gpu-or-None) per node; zone_id: interned ZoneLabel (None = one zone); node_group: affinity
+        class per node, -1 = none (None = all 0).  apps: drv_*, exe_*, count and group (the driver's class, -1 = every node).
+        -> uint8[n_apps], 1 = exceeds cluster capacity.  Leaves the context's snapshot and statistics untouched."""
+        q = len(apps["count"])
+        count = _np(apps["count"], np.int32)
+        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
+        group = _np(apps.get("group"), np.int32)
+        al = [_np(v, np.int64) for v in alloc]
+        ov = [_np(v, np.int64) for v in overhead] if overhead is not None else [None, None, None]
+        zid, grp = _np(zone_id, np.int32), _np(node_group, np.int32)
+        nd = gp_capacity_nodes(n_nodes=len(al[0]), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]),
+                               alloc_gpu=_p(al[2] if len(al) > 2 else None), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]),
+                               overhead_gpu=_p(ov[2] if len(ov) > 2 else None), n_zones=int(n_zones), zone_id=_p(zid),
+                               n_groups=int(n_groups), node_group=_p(grp))
+        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
+                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
+                    exe_count=_p(count), group=_p(group), skip_if_no_fit=None, exec_out_off=None)
+        out = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity(self._h, C.byref(nd), C.byref(a), int(packer), _p(out)))
+        return out[:q]
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
