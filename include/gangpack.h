@@ -575,6 +575,50 @@ typedef struct {
 gp_status gp_exceeds_cluster_capacity(gp_ctx* ctx, const gp_capacity_nodes* nodes, const gp_apps* drivers, gp_binpacker packer,
                                       uint8_t* exceeds /* [n_apps] */);
 
+/* ---- the failover reconciler's node choice (EXT/failover.go:43-82, 286-436) ------------------------------------------------
+ * syncResourceReservationsAndDemands minus pod, lister and CRD I/O: availableResourcesPerInstanceGroup (:286-323), then for each
+ * stale driver in call order constructResourceReservation's findNodes (:348-390, 409-436) and the charge of :159, in one call.
+ *   usage       the node table with every hard and soft reservation row and GetOverhead, exactly as gp_build_availability takes
+ *               it: available = allocatable - (reservations + overhead).
+ *   nodes       node_group = the interned value of the node's instanceGroupLabel ("" is a group like any other); creation orders
+ *               like metav1.Time.Before (UnixNano); unschedulable / not-ready nodes belong to no group's order.  Each group's
+ *               order is its schedulable, ready nodes by (creation descending, node-table index) -- the reference's newest-first
+ *               sort.Slice when the lister returns the nodes in that order (DESIGN §2.3).
+ *   stale       exe_cpu/mem/gpu, group (NULL = 0) and exe_count = max(0, MinExecutorCount - running executors) per driver, in the
+ *               order the reservations are written; drv_* and skip_if_no_fit are ignored; exec_out_off NULL or the prefix sum.
+ *   placed[i]   -1: the driver's group has no schedulable, ready node ("instance group not found", :358-362; nothing charged,
+ *               even with exe_count 0); otherwise len(reservedNodeNames), 0..exe_count (less: the group ran out of room).
+ *   executor_nodes[exec_out_off[i] ..) the reservedNodeNames as node indices, node-major; entries past placed[i] undefined.
+ *   Each node the walk reaches is charged (t + 1) x exe when it took t executors and the walk went on, t x exe when it completed
+ *   the driver there (DESIGN §2.3); the running driver and executors of a stale application are never charged.
+ * The context is left alone: snapshot, SchedulableResources, zone layout, held az-aware orders and gp_last_stats stay as they
+ * were; the call has scratch of its own and synchronises the stream once, at the end.
+ * GP_ERR_INVALID: missing arrays, n_groups < 1, a node or driver group out of range, a negative request or exe_count, an
+ * exec_out_off that is not the prefix sum.  GP_ERR_UNREPRESENTABLE: a request >= 2^61, exe_count > 2^24, or an availability the
+ * loop reads or charges outside the exact-int64 domain (|v| >= 2^61; the reference's quantities have no bound, so repeated
+ * overshoot charges can leave it) -- the whole call is refused, nothing wraps.  GP_ERR_CAPACITY: executor_nodes_cap too small.
+ * On an error the outputs are undefined. */
+typedef struct {
+    int32_t n_groups;              /* instance-group ids 0..n_groups-1 (instanceGroupLabel values interned; "" included) */
+    int32_t reserved;
+    const int32_t* node_group;     /* [usage->n_nodes] */
+    const int64_t* creation;       /* [n_nodes] ordered like metav1.Time.Before (UnixNano) */
+    const uint8_t* unschedulable;  /* or NULL */
+    const uint8_t* ready;          /* or NULL (= all) */
+} gp_reconcile_nodes;
+typedef struct {
+    int32_t* placed;               /* [n_apps] len(reservedNodeNames), 0..exe_count; -1 = instance group not found */
+    int32_t* executor_nodes;       /* node-major at exec_out_off[i]; entries past placed[i] undefined */
+    int64_t executor_nodes_cap;
+    int64_t* avail_cpu_milli;      /* out or NULL: [n_nodes] availability after the loop (the only direct */
+    int64_t* avail_mem_bytes;      /*   observable of the overshoot charge; tests and logging)            */
+    int64_t* avail_gpu;
+} gp_reconcile_results;
+gp_status gp_reconcile_find_nodes(gp_ctx* ctx, const gp_usage_input* usage, const gp_reconcile_nodes* nodes,
+                                  const gp_apps* stale /* exe_*, group, exe_count = max(0, Min - running);
+                                                          drv_* and skip_if_no_fit ignored; call order = processing order */,
+                                  gp_reconcile_results* out);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

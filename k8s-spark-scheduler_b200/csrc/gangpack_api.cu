@@ -13,6 +13,7 @@
 #include "gangpack_reschedprep.cuh"
 #include "gangpack_efficiency.cuh"
 #include "gangpack_capacity.cuh"
+#include "gangpack_reconcile.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -458,9 +459,11 @@ struct gp_ctx {
     DevBuf zoneprep;
     DevBuf reschedprep;                           // gp_reschedule_from_reservations' own scratch (no state points into it)
     DevBuf capprep;                               // gp_exceeds_cluster_capacity's own scratch (no state points into it)
+    DevBuf reconbuf;                              // gp_reconcile_find_nodes' own scratch (no state points into it)
     int zone_kind = -1;
     gp_az_orders zone_orders{};
     bool sort_attr_set = false;
+    bool recon_attr_set = false;                  // dynamic shared-memory opt-in of gp_sort_tiles<ReconKey> done on this device
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
 
     gp_stats last{};
@@ -2719,6 +2722,135 @@ gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes,
     if (herr & kCcErrNodeGroup) return bad(GP_ERR_INVALID, "node_group out of range (-1 or 0..n_groups-1)");
     if (herr & kCcErrUnrepresentable) return bad(GP_ERR_UNREPRESENTABLE, "request >= 2^61");
     if (herr & kCcErrNodeQuantity) return bad(GP_ERR_UNREPRESENTABLE, "|allocatable| or |overhead| >= 2^61");
+    return GP_OK;
+}
+
+// the failover reconciler's findNodes loop for a batch of stale drivers (EXT/failover.go:43-82, 286-436); see
+// gangpack_reconcile.cuh and DESIGN §2.3
+gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
+                                  gp_reconcile_results* out) {
+    if (!c) return GP_ERR_INVALID;
+    static const char* who = "gp_reconcile_find_nodes";
+    auto bad = [&](gp_status st, const char* what) { return fail(c, st, std::string(who) + ": " + what); };
+    if (!usage || !nodes || !a || !out || usage->n_nodes < 0 || usage->n_reservations < 0 || nodes->n_groups < 1 || a->n_apps < 0 ||
+        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes || !nodes->node_group || !nodes->creation)) ||
+        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)) ||
+        (a->n_apps > 0 && (!a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->placed)))
+        return bad(GP_ERR_INVALID, "missing arrays or bad sizes (n_groups >= 1)");
+    const int32_t n = usage->n_nodes, q = a->n_apps, G = nodes->n_groups;
+    for (int32_t i = 0; i < n; ++i)
+        if (nodes->node_group[i] < 0 || nodes->node_group[i] >= G) return bad(GP_ERR_INVALID, "node_group out of range");
+    int64_t total = 0;
+    for (int32_t i = 0; i < q; ++i) {
+        const int64_t v[3] = {a->exe_cpu_milli[i], a->exe_mem_bytes[i], a->exe_gpu ? a->exe_gpu[i] : 0};
+        for (int64_t x : v) {
+            if (x < 0) return bad(GP_ERR_INVALID, "negative resource request");
+            if (x >= kMaxQuantity) return bad(GP_ERR_UNREPRESENTABLE, "quantity >= 2^61");
+        }
+        const int32_t k = a->exe_count[i];
+        if (k < 0) return bad(GP_ERR_INVALID, "negative exe_count");
+        if (k > kMaxCount) return bad(GP_ERR_UNREPRESENTABLE, "exe_count > 2^24");
+        if (a->group && (a->group[i] < 0 || a->group[i] >= G)) return bad(GP_ERR_INVALID, "instance group out of range");
+        if (a->exec_out_off && a->exec_out_off[i] != total) return bad(GP_ERR_INVALID, "exec_out_off is not the prefix sum of exe_count");
+        total += k;
+    }
+    if (a->exec_out_off && a->exec_out_off[q] != total) return bad(GP_ERR_INVALID, "exec_out_off is not the prefix sum of exe_count");
+    if (total > 0 && (!out->executor_nodes || out->executor_nodes_cap < total))
+        return bad(GP_ERR_CAPACITY, "executor_nodes_cap below the sum of exe_count");
+    const bool want_avail = out->avail_cpu_milli || out->avail_mem_bytes || out->avail_gpu;
+    if (n == 0) {                                       // every group is missing from orderedNodes
+        for (int32_t i = 0; i < q; ++i) out->placed[i] = -1;
+        return GP_OK;
+    }
+    if (q == 0 && !want_avail) return GP_OK;
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    long long *d_avail = nullptr, *d_sched = nullptr;   // usagebuf: scratch of the availability stage, charged in place below
+    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched);
+    if (s != GP_OK) return s;
+    const size_t N = (size_t)n, Q = (size_t)q, Gs = (size_t)G, E = (size_t)total;
+    Arena ar{c->reconbuf};
+    const size_t o_grp = ar.take(4 * N), o_cre = ar.take(8 * N), o_fu = ar.take(N), o_fr = ar.take(N), o_keys = ar.take(sizeof(ReconKey) * N),
+                 o_sorted = ar.take(sizeof(ReconKey) * N), o_pos = ar.take(4 * N), o_order = ar.take(4 * N), o_ngrp = ar.take(4 * N),
+                 o_noff = ar.take(4 * (Gs + 1)), o_aoff = ar.take(4 * (Gs + 1)), o_exe = ar.take(24 * Q), o_cnt = ar.take(4 * Q),
+                 o_agrp = ar.take(4 * Q), o_off = ar.take(8 * Q), o_list = ar.take(4 * Q), o_lk = ar.take(sizeof(LabelKey) * Q),
+                 o_lks = ar.take(sizeof(LabelKey) * Q), o_apos = ar.take(4 * Q), o_apps = ar.take(4 * Q), o_placed = ar.take(4 * Q),
+                 o_exn = ar.take(4 * E), o_word = ar.take(16);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
+    GP_CUDA(c, up(o_grp, nodes->node_group, 4 * N));
+    GP_CUDA(c, up(o_cre, nodes->creation, 8 * N));
+    if (nodes->unschedulable) GP_CUDA(c, up(o_fu, nodes->unschedulable, N));
+    if (nodes->ready) GP_CUDA(c, up(o_fr, nodes->ready, N));
+    GP_CUDA(c, cudaMemsetAsync(b + o_word, 0, 16, st));  // claim counter, error word
+    if (!c->recon_attr_set) {
+        GP_CUDA(c, cudaFuncSetAttribute(gp_sort_tiles<ReconKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSortTile * sizeof(ReconKey))));
+        c->recon_attr_set = true;
+    }
+    const int T = 256;
+    const int nb = (n + T - 1) / T;
+    ReconKey* keys = (ReconKey*)(b + o_keys);
+    int32_t* pos = (int32_t*)(b + o_pos);
+    int32_t* order = (int32_t*)(b + o_order);
+    int32_t* ngrp = (int32_t*)(b + o_ngrp);
+    gp_rc_node_keys<<<nb, T, 0, st>>>(n, G, (const int32_t*)(b + o_grp), (const long long*)(b + o_cre),
+                                      nodes->unschedulable ? (const uint8_t*)(b + o_fu) : nullptr, nodes->ready ? (const uint8_t*)(b + o_fr) : nullptr,
+                                      keys, ngrp);
+    gp_sort_tiles<ReconKey><<<(n + kSortTile - 1) / kSortTile, kSortThreads, kSortTile * sizeof(ReconKey), st>>>(n, nullptr, keys, (ReconKey*)(b + o_sorted));
+    gp_rank_by_search<ReconKey><<<nb, T, 0, st>>>(n, nullptr, keys, (const ReconKey*)(b + o_sorted), pos);
+    gp_scatter_order<<<nb, T, 0, st>>>(n, pos, order);
+    int32_t* apps = (int32_t*)(b + o_apps);
+    int32_t* agrp = (int32_t*)(b + o_agrp);
+    int32_t* cnt = (int32_t*)(b + o_word + 8);
+    if (q > 0) {
+        // exe cpu, mem, gpu columns, counts, groups and offsets
+        GP_CUDA(c, up(o_exe, a->exe_cpu_milli, 8 * Q));
+        GP_CUDA(c, up(o_exe + 8 * Q, a->exe_mem_bytes, 8 * Q));
+        if (a->exe_gpu) GP_CUDA(c, up(o_exe + 16 * Q, a->exe_gpu, 8 * Q));
+        else GP_CUDA(c, cudaMemsetAsync(b + o_exe + 16 * Q, 0, 8 * Q, st));
+        GP_CUDA(c, up(o_cnt, a->exe_count, 4 * Q));
+        if (a->group) GP_CUDA(c, up(o_agrp, a->group, 4 * Q));
+        else GP_CUDA(c, cudaMemsetAsync(agrp, 0, 4 * Q, st));
+        if (a->exec_out_off) GP_CUDA(c, up(o_off, a->exec_out_off, 8 * Q));
+        else {
+            std::vector<int64_t>& off = c->host_off;
+            off.resize(Q);
+            int64_t run = 0;
+            for (int32_t i = 0; i < q; ++i) { off[i] = run; run += a->exe_count[i]; }
+            GP_CUDA(c, up(o_off, off.data(), 8 * Q));
+        }
+        // the stale drivers partitioned by group, call order kept inside each group
+        const int qb = (q + T - 1) / T;
+        gp_rc_app_list<<<qb, T, 0, st>>>(q, (int32_t*)(b + o_list), cnt);
+        launch_label_resort(q, cnt, (const int32_t*)(b + o_list), agrp, (LabelKey*)(b + o_lk), (LabelKey*)(b + o_lks), (int32_t*)(b + o_apos),
+                            apps, st);
+    }
+    gp_rc_offsets<<<(unsigned)((Gs + T) / T), T, 0, st>>>(G, n, order, ngrp, q, apps, agrp, (int32_t*)(b + o_noff), (int32_t*)(b + o_aoff));
+    if (q > 0) {
+        RcLoopIn li{};
+        li.avail = d_avail; li.order = order; li.noff = (const int32_t*)(b + o_noff);
+        li.apps = apps; li.aoff = (const int32_t*)(b + o_aoff);
+        li.exe = (const long long*)(b + o_exe); li.count = (const int32_t*)(b + o_cnt); li.out_off = (const long long*)(b + o_off);
+        li.placed = (int32_t*)(b + o_placed); li.exec_nodes = (int32_t*)(b + o_exn);
+        li.claim = (unsigned int*)(b + o_word); li.err = (int*)(b + o_word + 4);
+        li.n = n; li.q = q; li.n_groups = G;
+        // one CTA per instance group; CTAs that find no group left return at once
+        const int blocks = (int)std::min<int64_t>(G, (int64_t)c->sm_count * 8);
+        gp_rc_loop<<<blocks, kRcThreads, 0, st>>>(li);
+    }
+    GP_CUDA(c, cudaGetLastError());
+    int herr = 0;
+    if (q > 0) {
+        GP_CUDA(c, cudaMemcpyAsync(out->placed, b + o_placed, 4 * Q, cudaMemcpyDeviceToHost, st));
+        if (E) GP_CUDA(c, cudaMemcpyAsync(out->executor_nodes, b + o_exn, 4 * E, cudaMemcpyDeviceToHost, st));
+        GP_CUDA(c, cudaMemcpyAsync(&herr, b + o_word + 4, 4, cudaMemcpyDeviceToHost, st));
+    }
+    int64_t* outs[3] = {out->avail_cpu_milli, out->avail_mem_bytes, out->avail_gpu};
+    for (int d = 0; d < 3; ++d)
+        if (outs[d]) GP_CUDA(c, cudaMemcpyAsync(outs[d], d_avail + N * (size_t)d, 8 * N, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    if (herr & kRcErrDomain) return bad(GP_ERR_UNREPRESENTABLE, "an availability the loop charged lies outside the exact-int64 domain (|v| >= 2^61)");
     return GP_OK;
 }
 

@@ -1255,3 +1255,150 @@ func DoesPodsExceedClusterCapacity(binpackerName string, nodesSchedulingMetadata
 	}
 	return out, true
 }
+
+// ReconcileNode is one lister node as the failover reconciler sees it (EXT/failover.go:286-314).
+type ReconcileNode struct {
+	Name             string
+	Allocatable      *resources.Resources // from node.Status.Allocatable
+	InstanceGroup    string               // n.Labels[instanceGroupLabel]; "" when the label is missing
+	Unschedulable    bool                 // n.Spec.Unschedulable
+	Ready            bool                 // NodeReady == True
+	CreationUnixNano int64                // n.CreationTimestamp.UnixNano(): ordered like metav1.Time.Before
+}
+
+// ReconcileRow is one reservation of an RR, or one soft reservation: UsageForNodes + UsedSoftReservationResources (:315-317).
+type ReconcileRow struct {
+	Node      string
+	Resources *resources.Resources
+}
+
+// ReconcileDriver is one stale driver, in the order its RR is written.
+type ReconcileDriver struct {
+	InstanceGroup     string // internal.FindInstanceGroupFromPodSpec
+	ExecutorResources *resources.Resources
+	MinExecutorCount  int
+	RunningExecutors  int // len(sp.inconsistentExecutors); capped at MinExecutorCount as at :141-143
+}
+
+// ReconcileResult is what constructResourceReservation learns from findNodes for one driver.
+type ReconcileResult struct {
+	InstanceGroupFound bool     // false: "instance group not found" (:358-362), no RR and no charge
+	ReservedNodeNames  []string // findNodes' result, possibly shorter than Min - running
+}
+
+// ReconcileFindNodes runs availableResourcesPerInstanceGroup and every stale driver's findNodes with the charge of :159 in one
+// gp_reconcile_find_nodes call (DESIGN §2.3).  ok = false on any refusal or inexact quantity: the caller then runs the Go loop.
+// The node slice is the lister's order; equal creation times keep it.
+func ReconcileFindNodes(nodes []ReconcileNode, rows []ReconcileRow, overhead resources.NodeGroupResources, drivers []ReconcileDriver) ([]ReconcileResult, bool) {
+	d, err := getDevice()
+	if err != nil {
+		return nil, false
+	}
+	n, r, q := len(nodes), len(rows), len(drivers)
+	index := make(map[string]int32, n)
+	groupID := map[string]int32{}
+	intern := func(g string) int32 {
+		id, seen := groupID[g]
+		if !seen {
+			id = int32(len(groupID))
+			groupID[g] = id
+		}
+		return id
+	}
+	var al, ov [3][]int64
+	for t := 0; t < 3; t++ {
+		al[t], ov[t] = make([]int64, n+1), make([]int64, n+1)
+	}
+	grp, cre := make([]int32, n+1), make([]int64, n+1)
+	unsched, ready := make([]uint8, n+1), make([]uint8, n+1)
+	for i, nd := range nodes {
+		index[nd.Name] = int32(i)
+		var ok bool
+		if al[0][i], al[1][i], al[2][i], ok = toTriple(nd.Allocatable); !ok {
+			return nil, false
+		}
+		if o, in := overhead[nd.Name]; in {
+			if ov[0][i], ov[1][i], ov[2][i], ok = toTriple(o); !ok {
+				return nil, false
+			}
+		}
+		grp[i], cre[i] = intern(nd.InstanceGroup), nd.CreationUnixNano
+		if nd.Unschedulable {
+			unsched[i] = 1
+		}
+		if nd.Ready {
+			ready[i] = 1
+		}
+	}
+	rn := make([]int32, r+1)
+	var rc [3][]int64
+	for t := 0; t < 3; t++ {
+		rc[t] = make([]int64, r+1)
+	}
+	for j, row := range rows {
+		rn[j] = -1 // a reservation on a node the lister no longer returns: AvailableForNodes never reads it
+		if v, in := index[row.Node]; in {
+			rn[j] = v
+		}
+		var ok bool
+		if rc[0][j], rc[1][j], rc[2][j], ok = toTriple(row.Resources); !ok {
+			return nil, false
+		}
+	}
+	var ec [3][]int64
+	for t := 0; t < 3; t++ {
+		ec[t] = make([]int64, q+1)
+	}
+	count, dg, off := make([]int32, q+1), make([]int32, q+1), make([]int64, q+1)
+	for j, drv := range drivers {
+		var ok bool
+		if ec[0][j], ec[1][j], ec[2][j], ok = toTriple(drv.ExecutorResources); !ok {
+			return nil, false
+		}
+		k := drv.MinExecutorCount - min(drv.RunningExecutors, drv.MinExecutorCount) // :366
+		if k < 0 {
+			k = 0
+		}
+		if k > 1<<24 {
+			return nil, false
+		}
+		count[j], dg[j] = int32(k), intern(drv.InstanceGroup)
+		off[j+1] = off[j] + int64(k)
+	}
+	placed, exe := make([]int32, q+1), make([]int32, off[q]+1)
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	// the C structs hold Go pointers: every slice base is pinned for the duration of the call
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []any{&grp[0], &cre[0], &unsched[0], &ready[0], &rn[0], &count[0], &dg[0], &off[0], &placed[0], &exe[0]} {
+		pin.Pin(p)
+	}
+	for t := 0; t < 3; t++ {
+		pin.Pin(&al[t][0])
+		pin.Pin(&ov[t][0])
+		pin.Pin(&rc[t][0])
+		pin.Pin(&ec[t][0])
+	}
+	u := C.gp_usage_input{n_nodes: C.int32_t(n), alloc_cpu_milli: ptr64(al[0]), alloc_mem_bytes: ptr64(al[1]), alloc_gpu: ptr64(al[2]),
+		overhead_cpu_milli: ptr64(ov[0]), overhead_mem_bytes: ptr64(ov[1]), overhead_gpu: ptr64(ov[2]),
+		n_reservations: C.int64_t(r), res_node: ptr32(rn), res_cpu_milli: ptr64(rc[0]), res_mem_bytes: ptr64(rc[1]), res_gpu: ptr64(rc[2])}
+	nd := C.gp_reconcile_nodes{n_groups: C.int32_t(max(len(groupID), 1)), node_group: ptr32(grp), creation: ptr64(cre),
+		unschedulable: ptr8(unsched), ready: ptr8(ready)}
+	a := C.gp_apps{n_apps: C.int32_t(q), exe_cpu_milli: ptr64(ec[0]), exe_mem_bytes: ptr64(ec[1]), exe_gpu: ptr64(ec[2]),
+		exe_count: ptr32(count), group: ptr32(dg), exec_out_off: ptr64(off)}
+	out := C.gp_reconcile_results{placed: ptr32(placed), executor_nodes: ptr32(exe), executor_nodes_cap: C.int64_t(off[q])}
+	if C.gp_reconcile_find_nodes(d.ctx, &u, &nd, &a, &out) != C.GP_OK {
+		return nil, false
+	}
+	res := make([]ReconcileResult, q)
+	for j := range res {
+		res[j].InstanceGroupFound = placed[j] >= 0
+		for t := int32(0); t < placed[j]; t++ {
+			res[j].ReservedNodeNames = append(res[j].ReservedNodeNames, nodes[exe[off[j]+int64(t)]].Name)
+		}
+	}
+	return res, true
+}

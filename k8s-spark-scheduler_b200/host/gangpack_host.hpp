@@ -1111,4 +1111,93 @@ private:
     binpacker::Binpacker packer_;
 };
 
+// The failover reconciler's node choice (syncResourceReservationsAndDemands, internal/extender/failover.go:43-82):
+// availableResourcesPerInstanceGroup (:286-323) and, per stale driver, constructResourceReservation's findNodes (:348-390,
+// 409-436) with the charge of :159 -- one gp_reconcile_find_nodes call for every stale driver.  Pod and reservation listing,
+// the RR writes and syncDemands / syncSoftReservations stay with the caller.
+struct ReconcileNode {
+    std::string Name;
+    resources::Resources Allocatable;
+    std::unordered_map<std::string, std::string> Labels;
+    bool Unschedulable = false;
+    bool Ready = true;
+    int64_t CreationUnixNano = 0;          // metav1.Time, ordered like Before
+};
+struct ReconcileRow {                      // one RR reservation or one soft reservation
+    std::string Node;
+    resources::Resources Resources;
+};
+struct StaleDriver {
+    std::string InstanceGroup;             // FindInstanceGroupFromPodSpec; "" when the driver names none
+    resources::Resources ExecutorResources;
+    int MinExecutorCount = 0;
+    int RunningExecutors = 0;              // inconsistent executors already running; capped at MinExecutorCount (:141-143)
+};
+struct ReconcileResult {
+    bool InstanceGroupFound = false;       // false: constructResourceReservation errs (:358-362) and nothing is charged
+    std::vector<std::string> ReservedNodeNames;
+};
+
+// nodes: the lister's nodes (their order is the tie order among equal creation times, DESIGN §2.3); rows: every RR and soft
+// reservation; overhead: GetOverhead by node name; drivers: in the order their RRs are written.
+inline std::vector<ReconcileResult> ReconcileFindNodes(const std::vector<ReconcileNode>& nodes, const std::vector<ReconcileRow>& rows,
+                                                       const resources::NodeGroupResources& overhead, const std::string& instanceGroupLabel,
+                                                       const std::vector<StaleDriver>& drivers) {
+    const size_t N = nodes.size(), R = rows.size(), Q = drivers.size();
+    std::unordered_map<std::string, int32_t> index, groupId;
+    auto intern = [&](const std::string& g) { return groupId.emplace(g, (int32_t)groupId.size()).first->second; };
+    std::vector<int64_t> ac(N), am(N), ag(N), oc(N), om(N), og(N), cr(N);
+    std::vector<int32_t> grp(N);
+    std::vector<uint8_t> unsched(N), ready(N);
+    for (size_t i = 0; i < N; ++i) {
+        const ReconcileNode& n = nodes[i];
+        index.emplace(n.Name, (int32_t)i);
+        ac[i] = n.Allocatable.CPU; am[i] = n.Allocatable.Memory; ag[i] = n.Allocatable.NvidiaGPU;
+        auto o = overhead.find(n.Name);
+        if (o != overhead.end()) { oc[i] = o->second.CPU; om[i] = o->second.Memory; og[i] = o->second.NvidiaGPU; }
+        auto l = n.Labels.find(instanceGroupLabel);
+        grp[i] = intern(l == n.Labels.end() ? std::string() : l->second);      // n.Labels[label]: "" when missing
+        unsched[i] = n.Unschedulable; ready[i] = n.Ready; cr[i] = n.CreationUnixNano;
+    }
+    std::vector<int32_t> rn(R);
+    std::vector<int64_t> rc(R), rm(R), rg(R);
+    for (size_t r = 0; r < R; ++r) {
+        auto it = index.find(rows[r].Node);
+        rn[r] = it == index.end() ? -1 : it->second;
+        rc[r] = rows[r].Resources.CPU; rm[r] = rows[r].Resources.Memory; rg[r] = rows[r].Resources.NvidiaGPU;
+    }
+    std::vector<int64_t> ec(Q), em(Q), eg(Q), off(Q + 1, 0);
+    std::vector<int32_t> count(Q), dg(Q);
+    for (size_t i = 0; i < Q; ++i) {
+        const StaleDriver& d = drivers[i];
+        ec[i] = d.ExecutorResources.CPU; em[i] = d.ExecutorResources.Memory; eg[i] = d.ExecutorResources.NvidiaGPU;
+        count[i] = std::max(0, d.MinExecutorCount - std::min(d.RunningExecutors, d.MinExecutorCount));   // :366
+        dg[i] = intern(d.InstanceGroup);
+        off[i + 1] = off[i] + count[i];
+    }
+    gp_usage_input u{};
+    u.n_nodes = (int32_t)N;
+    u.alloc_cpu_milli = ac.data(); u.alloc_mem_bytes = am.data(); u.alloc_gpu = ag.data();
+    u.overhead_cpu_milli = oc.data(); u.overhead_mem_bytes = om.data(); u.overhead_gpu = og.data();
+    u.n_reservations = (int64_t)R; u.res_node = rn.data(); u.res_cpu_milli = rc.data(); u.res_mem_bytes = rm.data(); u.res_gpu = rg.data();
+    gp_reconcile_nodes nd{};
+    nd.n_groups = std::max<int32_t>(1, (int32_t)groupId.size());
+    nd.node_group = grp.data(); nd.creation = cr.data(); nd.unschedulable = unsched.data(); nd.ready = ready.data();
+    gp_apps a{};
+    a.n_apps = (int32_t)Q;
+    a.exe_cpu_milli = ec.data(); a.exe_mem_bytes = em.data(); a.exe_gpu = eg.data();
+    a.exe_count = count.data(); a.group = dg.data(); a.exec_out_off = off.data();
+    std::vector<int32_t> placed(std::max<size_t>(Q, 1)), exe(std::max<int64_t>(off[Q], 1));
+    gp_reconcile_results out{};
+    out.placed = placed.data(); out.executor_nodes = exe.data(); out.executor_nodes_cap = off[Q];
+    gangpack::Device& dev = gangpack::Device::Get();
+    dev.check(gp_reconcile_find_nodes(dev.ctx(), &u, &nd, &a, &out), "gp_reconcile_find_nodes");
+    std::vector<ReconcileResult> res(Q);
+    for (size_t i = 0; i < Q; ++i) {
+        res[i].InstanceGroupFound = placed[i] >= 0;
+        for (int32_t j = 0; j < placed[i]; ++j) res[i].ReservedNodeNames.push_back(nodes[(size_t)exe[(size_t)off[i] + (size_t)j]].Name);
+    }
+    return res;
+}
+
 }  // namespace extender

@@ -18,7 +18,8 @@ LIB_PATH = os.environ.get("GANGPACK_LIB") or os.path.join(_PKG, "libgangpack.so"
 _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack_kernels.cuh", "gangpack_fifo.cuh", "gangpack_minfrag.cuh",
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
                                                     "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
-                                                    "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh", "gangpack_capacity.cuh")] + [
+                                                    "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh", "gangpack_capacity.cuh",
+                                                    "gangpack_reconcile.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -40,6 +41,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
+           "gp_reconcile_find_nodes",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -174,6 +176,16 @@ class gp_capacity_nodes(C.Structure):
                 ("n_zones", C.c_int32), ("zone_id", C.c_void_p), ("n_groups", C.c_int32), ("node_group", C.c_void_p)]
 
 
+class gp_reconcile_nodes(C.Structure):
+    _fields_ = [("n_groups", C.c_int32), ("reserved", C.c_int32), ("node_group", C.c_void_p), ("creation", C.c_void_p),
+                ("unschedulable", C.c_void_p), ("ready", C.c_void_p)]
+
+
+class gp_reconcile_results(C.Structure):
+    _fields_ = [("placed", C.c_void_p), ("executor_nodes", C.c_void_p), ("executor_nodes_cap", C.c_int64),
+                ("avail_cpu_milli", C.c_void_p), ("avail_mem_bytes", C.c_void_p), ("avail_gpu", C.c_void_p)]
+
+
 class gp_stats(C.Structure):
     _fields_ = [("nodes_scanned", C.c_int64), ("drivers_tried", C.c_int64), ("kernel_launches", C.c_int64),
                 ("pack_kernel_ns", C.c_int64), ("prep_kernel_ns", C.c_int64), ("scan_path_apps", C.c_int64),
@@ -235,6 +247,9 @@ def load():
     L.gp_packing_efficiency.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_results), C.c_int, C.c_void_p]
     L.gp_exceeds_cluster_capacity.restype = C.c_int
     L.gp_exceeds_cluster_capacity.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.POINTER(gp_apps), C.c_int, C.c_void_p]
+    L.gp_reconcile_find_nodes.restype = C.c_int
+    L.gp_reconcile_find_nodes.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_reconcile_nodes), C.POINTER(gp_apps),
+                                          C.POINTER(gp_reconcile_results)]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -786,6 +801,43 @@ class GangPacker:
         out = np.full(max(q, 1), 255, np.uint8)
         self._check(load().gp_exceeds_cluster_capacity(self._h, C.byref(nd), C.byref(a), int(packer), _p(out)))
         return out[:q]
+
+    def reconcile_find_nodes(self, alloc, overhead, res_node, res, node_group, creation, apps: dict, n_groups: int,
+                             unschedulable=None, ready=None, exec_cap=None, want_avail=True):
+        """The failover reconciler's findNodes loop for a batch of stale drivers in one device call (gp_reconcile_find_nodes).
+        alloc / overhead / res: (cpu, mem, gpu-or-None) triples (overhead may be None); res_node: node index per reservation row
+        (hard and soft alike, -1 = unknown node); node_group: interned instanceGroupLabel per node; creation: int64 per node
+        (UnixNano); apps: exe_cpu, exe_mem, exe_gpu (optional), count = max(0, Min - running) and group, in call order.
+        -> (placed[q] (-1 = instance group not found), executor_nodes (CSR by off), off[q + 1], (cpu, mem, gpu) availability after
+        the loop or None).  Leaves the context's snapshot and statistics untouched."""
+        al = [_np(x, np.int64) for x in alloc]
+        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
+        rn = _np(res_node, np.int32)
+        rs = [_np(x, np.int64) for x in res]
+        n = len(al[0])
+        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2] if len(al) > 2 else None),
+                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2] if len(ov) > 2 else None),
+                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]),
+                            res_gpu=_p(rs[2] if len(rs) > 2 else None))
+        ng, cr = _np(node_group, np.int32), _np(creation, np.int64)
+        fu, fr = _np(unschedulable, np.uint8), _np(ready, np.uint8)
+        nd = gp_reconcile_nodes(n_groups=int(n_groups), node_group=_p(ng), creation=_p(cr), unschedulable=_p(fu), ready=_p(fr))
+        count = _np(apps["count"], np.int32)
+        q = len(count)
+        arrs = {k: _np(apps.get(k), np.int64) for k in ("exe_cpu", "exe_mem", "exe_gpu")}
+        group = _np(apps.get("group"), np.int32)
+        off = np.zeros(q + 1, np.int64)
+        np.cumsum(count, out=off[1:])
+        a = gp_apps(n_apps=q, exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
+                    exe_count=_p(count), group=_p(group), exec_out_off=_p(off))
+        placed = np.full(max(q, 1), -9, np.int32)
+        cap = int(off[q]) if exec_cap is None else int(exec_cap)
+        execn = np.full(max(cap, 1), -9, np.int32)
+        av = [np.empty(max(n, 1), np.int64) for _ in range(3)] if want_avail else [None] * 3
+        r = gp_reconcile_results(placed=_p(placed), executor_nodes=_p(execn), executor_nodes_cap=cap,
+                                 avail_cpu_milli=_p(av[0]), avail_mem_bytes=_p(av[1]), avail_gpu=_p(av[2]))
+        self._check(load().gp_reconcile_find_nodes(self._h, C.byref(ui), C.byref(nd), C.byref(a), C.byref(r)))
+        return placed[:q], execn[:int(off[q])], off, (tuple(x[:n] for x in av) if want_avail else None)
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
