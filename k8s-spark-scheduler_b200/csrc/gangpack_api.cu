@@ -354,6 +354,9 @@ struct Arena {
     size_t take(size_t bytes) { const size_t o = size; size += (bytes + 255) & ~(size_t)255; return o; }
     cudaError_t reserve() { return buf.reserve(size); }
     char* base() const { return buf.as<char>(); }
+    cudaError_t upload(size_t off, const void* src, size_t bytes, cudaStream_t st) const {
+        return cudaMemcpyAsync(base() + off, src, bytes, cudaMemcpyHostToDevice, st);
+    }
 };
 
 // A fixed sequence of kernel launches / memsets that repeats with identical arguments (one Predicate after the other:
@@ -2040,6 +2043,51 @@ gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const
 // ---- node priority order (f1) and availability snapshot (f2): device stages + the entries built on them ----
 }  // extern "C"
 
+// Host checks shared by the entries below; `who` (the entry's name) prefixes every message.  The shape of a gp_usage_input:
+// sizes non-negative, the allocatable columns for nodes, the reservation columns for rows.
+static gp_status check_usage(gp_ctx* c, const gp_usage_input* in, const char* who) {
+    if (!in || in->n_nodes < 0 || in->n_reservations < 0 || (in->n_nodes > 0 && (!in->alloc_cpu_milli || !in->alloc_mem_bytes)) ||
+        (in->n_reservations > 0 && (!in->res_node || !in->res_cpu_milli || !in->res_mem_bytes)))
+        return fail(c, GP_ERR_INVALID, std::string(who) + ": missing arrays or bad sizes");
+    return GP_OK;
+}
+
+// The two id arrays of a gp_sort_input the kernels index with.
+static gp_status check_sort_ids(gp_ctx* c, const gp_sort_input* in, const char* who) {
+    const int32_t n = in->n_nodes;
+    if (in->zone_id) for (int32_t i = 0; i < n; ++i)
+        if (in->zone_id[i] < 0 || in->zone_id[i] >= in->n_zones) return fail(c, GP_ERR_INVALID, std::string(who) + ": zone_id out of range");
+    if (in->name_rank) for (int32_t i = 0; i < n; ++i)
+        if (in->name_rank[i] < 0 || in->name_rank[i] >= n) return fail(c, GP_ERR_INVALID, std::string(who) + ": name_rank out of range");
+    return GP_OK;
+}
+
+// Executor requests (gpu optional): non-negative and inside the exact-int64 domain.
+static gp_status check_requests(gp_ctx* c, int32_t q, const int64_t* cpu, const int64_t* mem, const int64_t* gpu, const char* who) {
+    for (int32_t i = 0; i < q; ++i) {
+        const int64_t v[3] = {cpu[i], mem[i], gpu ? gpu[i] : 0};
+        for (int64_t x : v) {
+            if (x < 0) return fail(c, GP_ERR_INVALID, std::string(who) + ": negative resource request");
+            if (x >= kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, std::string(who) + ": quantity >= 2^61");
+        }
+    }
+    return GP_OK;
+}
+
+// The host_off / host_nodes CSR of a gp_reschedule (host_off given): monotone from 0, node indices below n_nodes.
+// *hosted = host_off[n_execs].
+static gp_status check_hosting(gp_ctx* c, const gp_reschedule* in, int32_t n_nodes, int64_t* hosted, const char* who) {
+    const std::string w(who);
+    if (in->host_off[0] != 0) return fail(c, GP_ERR_INVALID, w + ": host_off must start at 0");
+    for (int32_t i = 0; i < in->n_execs; ++i)
+        if (in->host_off[i + 1] < in->host_off[i]) return fail(c, GP_ERR_INVALID, w + ": host_off not monotone");
+    *hosted = in->host_off[in->n_execs];
+    if (*hosted > 0 && !in->host_nodes) return fail(c, GP_ERR_INVALID, w + ": host_nodes missing");
+    for (int64_t t = 0; t < *hosted; ++t)
+        if (in->host_nodes[t] < 0 || in->host_nodes[t] >= n_nodes) return fail(c, GP_ERR_INVALID, w + ": host_nodes index out of range");
+    return GP_OK;
+}
+
 // f2 stage: uploads the inputs, leaves avail[3][N] / sched[3][N] on the device (usagebuf).
 // d_over (optional, [3]): the uploaded overhead columns, NULL where the caller gave none.
 static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStream_t st, long long** d_avail, long long** d_sched,
@@ -2053,20 +2101,19 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
     const size_t o_has = o_usage + 24 * N;      // zeroed together with the usage sums
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
-    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
-    GP_CUDA(c, up(o_alloc, in->alloc_cpu_milli, 8 * N));
-    GP_CUDA(c, up(o_alloc + 8 * N, in->alloc_mem_bytes, 8 * N));
-    if (in->alloc_gpu) GP_CUDA(c, up(o_alloc + 16 * N, in->alloc_gpu, 8 * N));
-    if (in->overhead_cpu_milli) GP_CUDA(c, up(o_over, in->overhead_cpu_milli, 8 * N));
-    if (in->overhead_mem_bytes) GP_CUDA(c, up(o_over + 8 * N, in->overhead_mem_bytes, 8 * N));
-    if (in->overhead_gpu) GP_CUDA(c, up(o_over + 16 * N, in->overhead_gpu, 8 * N));
+    GP_CUDA(c, ar.upload(o_alloc, in->alloc_cpu_milli, 8 * N, st));
+    GP_CUDA(c, ar.upload(o_alloc + 8 * N, in->alloc_mem_bytes, 8 * N, st));
+    if (in->alloc_gpu) GP_CUDA(c, ar.upload(o_alloc + 16 * N, in->alloc_gpu, 8 * N, st));
+    if (in->overhead_cpu_milli) GP_CUDA(c, ar.upload(o_over, in->overhead_cpu_milli, 8 * N, st));
+    if (in->overhead_mem_bytes) GP_CUDA(c, ar.upload(o_over + 8 * N, in->overhead_mem_bytes, 8 * N, st));
+    if (in->overhead_gpu) GP_CUDA(c, ar.upload(o_over + 16 * N, in->overhead_gpu, 8 * N, st));
     GP_CUDA(c, cudaMemsetAsync(b + o_usage, 0, 28 * N, st));
     const int T = 256;
     if (R) {
-        GP_CUDA(c, up(o_rn, in->res_node, 4 * R));
-        GP_CUDA(c, up(o_rc, in->res_cpu_milli, 8 * R));
-        GP_CUDA(c, up(o_rm, in->res_mem_bytes, 8 * R));
-        if (in->res_gpu) GP_CUDA(c, up(o_rg, in->res_gpu, 8 * R));
+        GP_CUDA(c, ar.upload(o_rn, in->res_node, 4 * R, st));
+        GP_CUDA(c, ar.upload(o_rc, in->res_cpu_milli, 8 * R, st));
+        GP_CUDA(c, ar.upload(o_rm, in->res_mem_bytes, 8 * R, st));
+        if (in->res_gpu) GP_CUDA(c, ar.upload(o_rg, in->res_gpu, 8 * R, st));
         gp_usage_scatter<<<(unsigned)((R + T - 1) / T), T, 0, st>>>((long long)R, (const int32_t*)(b + o_rn), (const long long*)(b + o_rc),
                                                                    (const long long*)(b + o_rm), in->res_gpu ? (const long long*)(b + o_rg) : nullptr,
                                                                    n, (unsigned long long*)(b + o_usage), d_resched ? (unsigned int*)(b + o_has) : nullptr);
@@ -2106,14 +2153,10 @@ static void launch_label_resort(int32_t n, const int32_t* cnt, const int32_t* li
 
 // f1 stage: d_cpu / d_mem / d_gpu are device arrays (NULL: uploaded from `in`; gpu optional); leaves the two orders,
 // counts[3] = {#driver candidates, #executor candidates, #undefined ties} and the zone ids (NULL: one zone) on the device.
+// The caller has run check_sort_ids.
 static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long* d_cpu, const long long* d_mem, const long long* d_gpu,
                             cudaStream_t st, SortStage* out) {
     const int32_t n = in->n_nodes;
-    // cheap host validation of the two id arrays the kernels index with
-    if (in->zone_id) for (int32_t i = 0; i < n; ++i)
-        if (in->zone_id[i] < 0 || in->zone_id[i] >= in->n_zones) return fail(c, GP_ERR_INVALID, "gp_potential_nodes: zone_id out of range");
-    if (in->name_rank) for (int32_t i = 0; i < n; ++i)
-        if (in->name_rank[i] < 0 || in->name_rank[i] >= n) return fail(c, GP_ERR_INVALID, "gp_potential_nodes: name_rank out of range");
     // one scratch block
     const size_t N = (size_t)n, Z = (size_t)in->n_zones;
     Arena ar{c->sortbuf};
@@ -2125,18 +2168,17 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
                  o_fc = ar.take(N), o_fu = ar.take(N), o_fr = ar.take(N);
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
-    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
-    if (!d_cpu) { GP_CUDA(c, up(o_cpu, in->avail_cpu_milli, 8 * N)); d_cpu = (const long long*)(b + o_cpu); }
-    if (!d_mem) { GP_CUDA(c, up(o_mem, in->avail_mem_bytes, 8 * N)); d_mem = (const long long*)(b + o_mem); }
-    if (!d_gpu && in->avail_gpu) { GP_CUDA(c, up(o_gpu, in->avail_gpu, 8 * N)); d_gpu = (const long long*)(b + o_gpu); }
+    if (!d_cpu) { GP_CUDA(c, ar.upload(o_cpu, in->avail_cpu_milli, 8 * N, st)); d_cpu = (const long long*)(b + o_cpu); }
+    if (!d_mem) { GP_CUDA(c, ar.upload(o_mem, in->avail_mem_bytes, 8 * N, st)); d_mem = (const long long*)(b + o_mem); }
+    if (!d_gpu && in->avail_gpu) { GP_CUDA(c, ar.upload(o_gpu, in->avail_gpu, 8 * N, st)); d_gpu = (const long long*)(b + o_gpu); }
     const bool zoned = in->zone_id != nullptr && in->n_zones > 1;       // one zone: priority 0 for every node, nothing to total
-    if (zoned) GP_CUDA(c, up(o_zone, in->zone_id, 4 * N));
-    if (in->name_rank) GP_CUDA(c, up(o_nr, in->name_rank, 4 * N));
-    if (in->is_driver_candidate) GP_CUDA(c, up(o_fc, in->is_driver_candidate, N));
-    if (in->unschedulable) GP_CUDA(c, up(o_fu, in->unschedulable, N));
-    if (in->ready) GP_CUDA(c, up(o_fr, in->ready, N));
-    if (in->driver_label_rank) GP_CUDA(c, up(o_lrd, in->driver_label_rank, 4 * N));
-    if (in->executor_label_rank) GP_CUDA(c, up(o_lre, in->executor_label_rank, 4 * N));
+    if (zoned) GP_CUDA(c, ar.upload(o_zone, in->zone_id, 4 * N, st));
+    if (in->name_rank) GP_CUDA(c, ar.upload(o_nr, in->name_rank, 4 * N, st));
+    if (in->is_driver_candidate) GP_CUDA(c, ar.upload(o_fc, in->is_driver_candidate, N, st));
+    if (in->unschedulable) GP_CUDA(c, ar.upload(o_fu, in->unschedulable, N, st));
+    if (in->ready) GP_CUDA(c, ar.upload(o_fr, in->ready, N, st));
+    if (in->driver_label_rank) GP_CUDA(c, ar.upload(o_lrd, in->driver_label_rank, 4 * N, st));
+    if (in->executor_label_rank) GP_CUDA(c, ar.upload(o_lre, in->executor_label_rank, 4 * N, st));
     if (zoned) GP_CUDA(c, cudaMemsetAsync(b + o_tot, 0, 16 * Z, st));
     if (!c->sort_attr_set) {
         GP_CUDA(c, cudaFuncSetAttribute(gp_sort_tiles<SortKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSortTile * sizeof(SortKey))));
@@ -2180,6 +2222,63 @@ __global__ void gp_offsets_from_counts(const int32_t* __restrict__ counts, int32
     if (threadIdx.x == 0) { drv_off[0] = 0; drv_off[1] = counts[0]; exec_off[0] = 0; exec_off[1] = counts[1]; }
 }
 
+// gp_prepare_cluster and gp_prepare_cluster_zones up to their layout step: the checks both make, then reservations ->
+// availability (d_avail / d_sched: [3][n_nodes]) -> priority orders on the context's stream.
+static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const char* who,
+                                long long** d_avail, long long** d_sched, SortStage* so) {
+    gp_status s = check_usage(c, usage, who);
+    if (s != GP_OK) return s;
+    if (!sort || usage->n_nodes != sort->n_nodes || sort->n_zones < 1)
+        return fail(c, GP_ERR_INVALID, std::string(who) + ": missing arrays or mismatched sizes");
+    if (usage->n_nodes == 0) return fail(c, GP_ERR_INVALID, std::string(who) + ": empty node table");
+    if ((s = check_sort_ids(c, sort, who)) != GP_OK) return s;
+    GP_CUDA(c, cudaSetDevice(c->device));
+    if ((s = stage_availability(c, usage, c->stream, d_avail, d_sched)) != GP_OK) return s;
+    const size_t N = (size_t)usage->n_nodes;
+    return stage_sort(c, sort, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so);
+}
+
+// gp_prepare_cluster and gp_prepare_cluster_zones after their layout step, which set dn's groups, offsets and orders: the
+// node-table copy (gp_get_snapshot), the usual slot layout with n_nodes bounding both order lengths, SchedulableResources,
+// and counts[3] of the sort read back (the caller synchronises).
+static gp_status prepare_snapshot(gp_ctx* c, gp_nodes* dn, const long long* d_avail, const long long* d_sched, const SortStage& so,
+                                  int32_t* counts) {
+    cudaStream_t st = c->stream;
+    const int32_t n = dn->n_nodes;
+    const size_t N = (size_t)n, nb = sizeof(int64_t) * (N + 1);
+    GP_CUDA(c, c->node_cpu.reserve(nb)); GP_CUDA(c, c->node_mem.reserve(nb)); GP_CUDA(c, c->node_gpu.reserve(nb));
+    GP_CUDA(c, cudaMemcpyAsync(c->node_cpu.p, d_avail, 8 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(c->node_mem.p, d_avail + N, 8 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(c->node_gpu.p, d_avail + 2 * N, 8 * N, cudaMemcpyDeviceToDevice, st));
+    dn->avail_cpu_milli = c->node_cpu.as<int64_t>(); dn->avail_mem_bytes = c->node_mem.as<int64_t>(); dn->avail_gpu = c->node_gpu.as<int64_t>();
+    gp_status s = build_snapshot_device(c, dn, n, n, st);
+    if (s != GP_OK) return s;
+    GP_CUDA(c, c->sched.reserve(24 * (N + 1)));
+    GP_CUDA(c, cudaMemcpyAsync(c->sched.p, d_sched, 24 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
+    return GP_OK;
+}
+
+// The two gp_build_*availability entries: the availability stage, then every non-NULL outs[k] gets row k % 3 of
+// availableResources for k < 3 (first_fit: that of rescheduleExecutor's first-fit branch), of SchedulableResources for k >= 3.
+static gp_status availability_out(gp_ctx* c, const gp_usage_input* in, bool first_fit, int64_t* const* outs, const char* who) {
+    gp_status s = check_usage(c, in, who);
+    if (s != GP_OK) return s;
+    const int32_t n = in->n_nodes;
+    if (n == 0) return GP_OK;
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    long long *d_avail = nullptr, *d_sched = nullptr, *d_ff = nullptr;
+    s = stage_availability(c, in, st, &d_avail, &d_sched, first_fit ? &d_ff : nullptr);
+    if (s != GP_OK) return s;
+    const size_t N = (size_t)n;
+    const long long* src[2] = {first_fit ? d_ff : d_avail, d_sched};
+    for (int k = 0; k < 6; ++k)
+        if (outs[k]) GP_CUDA(c, cudaMemcpyAsync(outs[k], src[k / 3] + N * (size_t)(k % 3), 8 * N, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    return GP_OK;
+}
+
 extern "C" {
 
 gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver_order, int32_t* n_driver,
@@ -2191,10 +2290,12 @@ gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver
     const int32_t n = in->n_nodes;
     *n_driver = 0; *n_executor = 0;
     if (n == 0) return GP_OK;
+    gp_status s = check_sort_ids(c, in, "gp_potential_nodes");
+    if (s != GP_OK) return s;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     SortStage so{};
-    gp_status s = stage_sort(c, in, nullptr, nullptr, nullptr, st, &so);
+    s = stage_sort(c, in, nullptr, nullptr, nullptr, st, &so);
     if (s != GP_OK) return s;
     int32_t counts[3] = {0, 0, 0};
     GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
@@ -2210,89 +2311,40 @@ gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver
 gp_status gp_build_availability(gp_ctx* c, const gp_usage_input* in, int64_t* avail_cpu, int64_t* avail_mem, int64_t* avail_gpu,
                                 int64_t* sched_cpu, int64_t* sched_mem, int64_t* sched_gpu) {
     if (!c) return GP_ERR_INVALID;
-    if (!in || in->n_nodes < 0 || in->n_reservations < 0 || (in->n_nodes > 0 && (!in->alloc_cpu_milli || !in->alloc_mem_bytes)) ||
-        (in->n_reservations > 0 && (!in->res_node || !in->res_cpu_milli || !in->res_mem_bytes)))
-        return fail(c, GP_ERR_INVALID, "gp_build_availability: missing arrays or bad sizes");
-    const int32_t n = in->n_nodes;
-    if (n == 0) return GP_OK;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    cudaStream_t st = c->stream;
-    long long *d_avail = nullptr, *d_sched = nullptr;
-    gp_status s = stage_availability(c, in, st, &d_avail, &d_sched);
-    if (s != GP_OK) return s;
-    const size_t N = (size_t)n;
-    int64_t* outs[6] = {avail_cpu, avail_mem, avail_gpu, sched_cpu, sched_mem, sched_gpu};
-    for (int k = 0; k < 6; ++k)
-        if (outs[k]) GP_CUDA(c, cudaMemcpyAsync(outs[k], (k < 3 ? d_avail : d_sched) + N * (size_t)(k % 3), 8 * N, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    return GP_OK;
+    int64_t* const outs[6] = {avail_cpu, avail_mem, avail_gpu, sched_cpu, sched_mem, sched_gpu};
+    return availability_out(c, in, false, outs, "gp_build_availability");
 }
 
 // availableResources of rescheduleExecutor's first-fit branch: the availability to upload before gp_reschedule_executors(min_frag = 0)
 gp_status gp_build_reschedule_availability(gp_ctx* c, const gp_usage_input* in, int64_t* avail_cpu, int64_t* avail_mem, int64_t* avail_gpu) {
     if (!c) return GP_ERR_INVALID;
-    if (!in || in->n_nodes < 0 || in->n_reservations < 0 || (in->n_nodes > 0 && (!in->alloc_cpu_milli || !in->alloc_mem_bytes)) ||
-        (in->n_reservations > 0 && (!in->res_node || !in->res_cpu_milli || !in->res_mem_bytes)))
-        return fail(c, GP_ERR_INVALID, "gp_build_reschedule_availability: missing arrays or bad sizes");
-    const int32_t n = in->n_nodes;
-    if (n == 0) return GP_OK;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    cudaStream_t st = c->stream;
-    long long *d_avail = nullptr, *d_sched = nullptr, *d_re = nullptr;
-    gp_status s = stage_availability(c, in, st, &d_avail, &d_sched, &d_re);
-    if (s != GP_OK) return s;
-    const size_t N = (size_t)n;
-    int64_t* outs[3] = {avail_cpu, avail_mem, avail_gpu};
-    for (int k = 0; k < 3; ++k)
-        if (outs[k]) GP_CUDA(c, cudaMemcpyAsync(outs[k], d_re + N * (size_t)k, 8 * N, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    return GP_OK;
+    int64_t* const outs[6] = {avail_cpu, avail_mem, avail_gpu, nullptr, nullptr, nullptr};
+    return availability_out(c, in, true, outs, "gp_build_reschedule_availability");
 }
 
 // reservations -> availability -> priority orders -> slot layout, without leaving the device
 gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, int32_t* n_driver, int32_t* n_executor) {
     if (!c) return GP_ERR_INVALID;
-    if (!usage || !sort || usage->n_nodes != sort->n_nodes || usage->n_nodes < 0 || sort->n_zones < 1 || usage->n_reservations < 0 ||
-        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes)) ||
-        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)))
-        return fail(c, GP_ERR_INVALID, "gp_prepare_cluster: missing arrays or mismatched sizes");
-    const int32_t n = usage->n_nodes;
     if (n_driver) *n_driver = 0;
     if (n_executor) *n_executor = 0;
-    if (n == 0) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster: empty node table");
-    GP_CUDA(c, cudaSetDevice(c->device));
-    cudaStream_t st = c->stream;
     long long *d_avail = nullptr, *d_sched = nullptr;
-    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched);
-    if (s != GP_OK) return s;
-    const size_t N = (size_t)n;
     SortStage so{};
-    s = stage_sort(c, sort, d_avail, d_avail + N, d_avail + 2 * N, st, &so);
+    gp_status s = prepare_orders(c, usage, sort, "gp_prepare_cluster", &d_avail, &d_sched, &so);
     if (s != GP_OK) return s;
-    // node-table copy (gp_get_snapshot) and the one-group offsets, then the usual slot layout with N as the upper bound
-    const size_t nb = sizeof(int64_t) * (N + 1);
-    GP_CUDA(c, c->node_cpu.reserve(nb)); GP_CUDA(c, c->node_mem.reserve(nb)); GP_CUDA(c, c->node_gpu.reserve(nb));
-    GP_CUDA(c, cudaMemcpyAsync(c->node_cpu.p, d_avail, 8 * N, cudaMemcpyDeviceToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(c->node_mem.p, d_avail + N, 8 * N, cudaMemcpyDeviceToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(c->node_gpu.p, d_avail + 2 * N, 8 * N, cudaMemcpyDeviceToDevice, st));
+    cudaStream_t st = c->stream;
     GP_CUDA(c, c->exec_off.reserve(8)); GP_CUDA(c, c->drv_off.reserve(8));
     gp_offsets_from_counts<<<1, 32, 0, st>>>(so.counts, c->exec_off.as<int32_t>(), c->drv_off.as<int32_t>());
     gp_nodes dn{};
-    dn.n_nodes = n;
-    dn.avail_cpu_milli = c->node_cpu.as<int64_t>(); dn.avail_mem_bytes = c->node_mem.as<int64_t>(); dn.avail_gpu = c->node_gpu.as<int64_t>();
+    dn.n_nodes = usage->n_nodes;
     dn.n_groups = 1;
     dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = so.exe;
     dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = so.drv;
-    s = build_snapshot_device(c, &dn, n, n, st);      // n is the upper bound of both order lengths
-    if (s != GP_OK) return s;
-    // SchedulableResources for gp_packing_efficiency (the zone entry points still want gp_set_schedulable)
-    GP_CUDA(c, c->sched.reserve(24 * (N + 1)));
-    GP_CUDA(c, cudaMemcpyAsync(c->sched.p, d_sched, 24 * N, cudaMemcpyDeviceToDevice, st));
     int32_t counts[3] = {0, 0, 0};
-    GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
+    s = prepare_snapshot(c, &dn, d_avail, d_sched, so, counts);
+    if (s != GP_OK) return s;
     GP_CUDA(c, cudaStreamSynchronize(st));
     c->n_drv = counts[0]; c->n_exec = counts[1];
-    c->have_eff_sched = true;
+    c->have_eff_sched = true;           // SchedulableResources for gp_packing_efficiency (the zone entry points still want gp_set_schedulable)
     if (sort->undefined_ties) *sort->undefined_ties = counts[2];
     if (n_driver) *n_driver = counts[0];
     if (n_executor) *n_executor = counts[1];
@@ -2302,27 +2354,20 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
 // reservations -> availability -> priority orders -> zone-grouped slot layout, without leaving the device
 gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout) {
     if (!c) return GP_ERR_INVALID;
-    if (!usage || !sort || !layout || usage->n_nodes != sort->n_nodes || usage->n_nodes < 0 || sort->n_zones < 1 || usage->n_reservations < 0 ||
-        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes)) ||
-        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)))
-        return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: missing arrays or mismatched sizes");
+    if (!layout) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: missing arrays or mismatched sizes");
     const int32_t kind = layout->kind;
     if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
         return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: layout->kind must be GP_LAYOUT_SINGLE_AZ or GP_LAYOUT_AZ_AWARE");
-    if (sort->n_zones == 0x7fffffff) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: n_zones too large");
-    const int32_t n = usage->n_nodes;
+    if (sort && sort->n_zones == 0x7fffffff) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: n_zones too large");
     layout->n_zones = 0; layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
-    if (n == 0) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: empty node table");
-    GP_CUDA(c, cudaSetDevice(c->device));
+    long long *d_avail = nullptr, *d_sched = nullptr;
+    SortStage so{};
+    gp_status s = prepare_orders(c, usage, sort, "gp_prepare_cluster_zones", &d_avail, &d_sched, &so);
+    if (s != GP_OK) return s;
     cudaStream_t st = c->stream;
     c->zone_kind = -1;                                  // the held orders are overwritten below
-    long long *d_avail = nullptr, *d_sched = nullptr;
-    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched);
-    if (s != GP_OK) return s;
+    const int32_t n = usage->n_nodes;
     const size_t N = (size_t)n;
-    SortStage so{};
-    s = stage_sort(c, sort, d_avail, d_avail + N, d_avail + 2 * N, st, &so);
-    if (s != GP_OK) return s;
     // g_bound = sort->n_zones + 1 groups bound every layout; the slots are laid out for that many (the groups past the
     // last one are empty) so that the group count can stay on the device until the one synchronise below
     const size_t Zs = (size_t)sort->n_zones;
@@ -2353,12 +2398,7 @@ gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const
                                            (int32_t*)(b + o_zg), (int32_t*)(b + o_zog), info);
     gp_group_rank<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, (const int32_t*)(b + o_zg), az, info, rank);
     GP_CUDA(c, cudaGetLastError());
-    // node-table copy (gp_get_snapshot), the grouped orders and their offsets, then the usual slot layout
-    const size_t nbytes = sizeof(int64_t) * (N + 1);
-    GP_CUDA(c, c->node_cpu.reserve(nbytes)); GP_CUDA(c, c->node_mem.reserve(nbytes)); GP_CUDA(c, c->node_gpu.reserve(nbytes));
-    GP_CUDA(c, cudaMemcpyAsync(c->node_cpu.p, d_avail, 8 * N, cudaMemcpyDeviceToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(c->node_mem.p, d_avail + N, 8 * N, cudaMemcpyDeviceToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(c->node_gpu.p, d_avail + 2 * N, 8 * N, cudaMemcpyDeviceToDevice, st));
+    // the grouped orders and their offsets
     GP_CUDA(c, c->exec_order.reserve(4 * (N + 1))); GP_CUDA(c, c->drv_order.reserve(4 * (N + 1)));
     GP_CUDA(c, c->exec_off.reserve(4 * ((size_t)g_bound + 1))); GP_CUDA(c, c->drv_off.reserve(4 * ((size_t)g_bound + 1)));
     LabelKey* lk = (LabelKey*)(b + o_lk);
@@ -2371,16 +2411,12 @@ gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const
     GP_CUDA(c, cudaGetLastError());
     gp_nodes dn{};
     dn.n_nodes = n;
-    dn.avail_cpu_milli = c->node_cpu.as<int64_t>(); dn.avail_mem_bytes = c->node_mem.as<int64_t>(); dn.avail_gpu = c->node_gpu.as<int64_t>();
     dn.n_groups = g_bound;
     dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = c->exec_order.as<int32_t>();
     dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = c->drv_order.as<int32_t>();
-    s = build_snapshot_device(c, &dn, n, n, st);      // n bounds both order lengths
-    if (s != GP_OK) return s;
-    GP_CUDA(c, c->sched.reserve(24 * (N + 1)));
-    GP_CUDA(c, cudaMemcpyAsync(c->sched.p, d_sched, 24 * N, cudaMemcpyDeviceToDevice, st));
     int32_t counts[3] = {0, 0, 0}, hinfo[kZiWords] = {};
-    GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
+    s = prepare_snapshot(c, &dn, d_avail, d_sched, so, counts);
+    if (s != GP_OK) return s;
     GP_CUDA(c, cudaMemcpyAsync(hinfo, info, sizeof(hinfo), cudaMemcpyDeviceToHost, st));
     if (layout->zone_of_group) GP_CUDA(c, cudaMemcpyAsync(layout->zone_of_group, b + o_zog, 4 * (Zs + 1), cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
@@ -2415,15 +2451,10 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
     const bool has_host = mf && in->host_off;
     if (has_res && !in->reserved_mem_bytes) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: reserved_mem_bytes missing");
     // host validation (O(q + n_nodes + hosted)): the exact-int64 domain, non-negative requests, CSR shape
-    for (int32_t i = 0; i < q; ++i) {
-        const int64_t v[3] = {in->exe_cpu_milli[i], in->exe_mem_bytes[i], in->exe_gpu ? in->exe_gpu[i] : 0};
-        for (int64_t x : v) {
-            if (x < 0) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: negative resource request");
-            if (x >= kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, "gp_reschedule_executors: quantity >= 2^61");
-        }
-        if (in->group && (in->group[i] < 0 || in->group[i] >= c->n_groups))
-            return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: instance group out of range");
-    }
+    gp_status chk = check_requests(c, q, in->exe_cpu_milli, in->exe_mem_bytes, in->exe_gpu, "gp_reschedule_executors");
+    if (chk != GP_OK) return chk;
+    for (int32_t i = 0; i < q; ++i)
+        if (in->group && (in->group[i] < 0 || in->group[i] >= c->n_groups)) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: instance group out of range");
     if (has_res)
         for (int32_t n = 0; n < c->n_nodes; ++n) {
             const int64_t v[3] = {in->reserved_cpu_milli[n], in->reserved_mem_bytes[n], in->reserved_gpu ? in->reserved_gpu[n] : 0};
@@ -2431,16 +2462,7 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
                 if (x >= kMaxQuantity || x <= -kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, "gp_reschedule_executors: |reserved| >= 2^61");
         }
     int64_t hosted = 0;
-    if (has_host) {
-        if (in->host_off[0] != 0) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: host_off must start at 0");
-        for (int32_t i = 0; i < q; ++i)
-            if (in->host_off[i + 1] < in->host_off[i]) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: host_off not monotone");
-        hosted = in->host_off[q];
-        if (hosted > 0 && !in->host_nodes) return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: host_nodes missing");
-        for (int64_t t = 0; t < hosted; ++t)
-            if (in->host_nodes[t] < 0 || in->host_nodes[t] >= c->n_nodes)
-                return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: host_nodes index out of range");
-    }
+    if (has_host && (chk = check_hosting(c, in, c->n_nodes, &hosted, "gp_reschedule_executors")) != GP_OK) return chk;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t Q = (size_t)q, N = (size_t)c->n_nodes, H = (size_t)hosted;
@@ -2500,9 +2522,9 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     if (!c) return GP_ERR_INVALID;
     static const char* who = "gp_reschedule_from_reservations";
     auto bad = [&](gp_status st, const char* what) { return fail(c, st, std::string(who) + ": " + what); };
-    if (!usage || !sort || !in || usage->n_nodes != sort->n_nodes || usage->n_nodes < 0 || sort->n_zones < 1 || usage->n_reservations < 0 ||
-        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes)) ||
-        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)) ||
+    gp_status s = check_usage(c, usage, who);
+    if (s != GP_OK) return s;
+    if (!sort || !in || usage->n_nodes != sort->n_nodes || sort->n_zones < 1 ||
         in->n_execs < 0 || (in->n_execs > 0 && (!in->exe_cpu_milli || !in->exe_mem_bytes || !node_out)))
         return bad(GP_ERR_INVALID, "missing arrays or mismatched sizes");
     const int32_t n = usage->n_nodes, q = in->n_execs;
@@ -2518,37 +2540,21 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
                 return bad(GP_ERR_INVALID, "filterNodesToZone: a node has no topology.kubernetes.io/zone label (topology_zone == -1), "
                                            "unable to make scheduling decisions based on AZ");
     }
-    if (sort->zone_id) for (int32_t i = 0; i < n; ++i)
-        if (sort->zone_id[i] < 0 || sort->zone_id[i] >= sort->n_zones) return bad(GP_ERR_INVALID, "zone_id out of range");
-    if (sort->name_rank) for (int32_t i = 0; i < n; ++i)
-        if (sort->name_rank[i] < 0 || sort->name_rank[i] >= n) return bad(GP_ERR_INVALID, "name_rank out of range");
+    if ((s = check_sort_ids(c, sort, who)) != GP_OK) return s;
     const bool mf = in->min_frag != 0;
     const bool has_host = mf && in->host_off;
-    for (int32_t i = 0; i < q; ++i) {
-        const int64_t v[3] = {in->exe_cpu_milli[i], in->exe_mem_bytes[i], in->exe_gpu ? in->exe_gpu[i] : 0};
-        for (int64_t x : v) {
-            if (x < 0) return bad(GP_ERR_INVALID, "negative resource request");
-            if (x >= kMaxQuantity) return bad(GP_ERR_UNREPRESENTABLE, "quantity >= 2^61");
-        }
+    if ((s = check_requests(c, q, in->exe_cpu_milli, in->exe_mem_bytes, in->exe_gpu, who)) != GP_OK) return s;
+    for (int32_t i = 0; i < q; ++i)
         if (in->group && in->group[i] != 0) return bad(GP_ERR_INVALID, "instance group out of range (one node table: group must be 0)");
-    }
     int64_t hosted = 0;
-    if (has_host) {
-        if (in->host_off[0] != 0) return bad(GP_ERR_INVALID, "host_off must start at 0");
-        for (int32_t i = 0; i < q; ++i)
-            if (in->host_off[i + 1] < in->host_off[i]) return bad(GP_ERR_INVALID, "host_off not monotone");
-        hosted = in->host_off[q];
-        if (hosted > 0 && !in->host_nodes) return bad(GP_ERR_INVALID, "host_nodes missing");
-        for (int64_t t = 0; t < hosted; ++t)
-            if (in->host_nodes[t] < 0 || in->host_nodes[t] >= n) return bad(GP_ERR_INVALID, "host_nodes index out of range");
-    }
+    if (has_host && (s = check_hosting(c, in, n, &hosted, who)) != GP_OK) return s;
     if (q == 0) return GP_OK;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     // availability: one scatter of the reservations, one pass per node (usagebuf is scratch of the f2 stage only)
     long long *d_avail = nullptr, *d_sched = nullptr, *d_ff = nullptr;
     const long long* d_over[3] = {nullptr, nullptr, nullptr};
-    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched, mf ? nullptr : &d_ff, d_over);
+    s = stage_availability(c, usage, st, &d_avail, &d_sched, mf ? nullptr : &d_ff, d_over);
     if (s != GP_OK) return s;
     const size_t N = (size_t)n, Q = (size_t)q, H = (size_t)hosted, Z = (size_t)sort->n_zones;
     const bool zoned = sort->zone_id != nullptr && sort->n_zones > 1;
@@ -2558,20 +2564,19 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
                  o_hoff = ar.take(8 * (Q + 1)), o_hn = ar.take(4 * (H + 1)), o_out = ar.take(4 * Q), o_amb = ar.take(Q);
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
-    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
-    if (zoned) GP_CUDA(c, up(o_zone, sort->zone_id, 4 * N));
-    if (sort->name_rank) GP_CUDA(c, up(o_nr, sort->name_rank, 4 * N));
-    if (sort->unschedulable) GP_CUDA(c, up(o_fu, sort->unschedulable, N));
-    if (sort->ready) GP_CUDA(c, up(o_fr, sort->ready, N));
-    if (sort->executor_label_rank) GP_CUDA(c, up(o_lr, sort->executor_label_rank, 4 * N));
-    if (keep >= 0) GP_CUDA(c, up(o_tz, scope->topology_zone, 4 * N));
-    GP_CUDA(c, up(o_exe, in->exe_cpu_milli, 8 * Q));
-    GP_CUDA(c, up(o_exe + 8 * Q, in->exe_mem_bytes, 8 * Q));
-    if (in->exe_gpu) GP_CUDA(c, up(o_exe + 16 * Q, in->exe_gpu, 8 * Q));
+    if (zoned) GP_CUDA(c, ar.upload(o_zone, sort->zone_id, 4 * N, st));
+    if (sort->name_rank) GP_CUDA(c, ar.upload(o_nr, sort->name_rank, 4 * N, st));
+    if (sort->unschedulable) GP_CUDA(c, ar.upload(o_fu, sort->unschedulable, N, st));
+    if (sort->ready) GP_CUDA(c, ar.upload(o_fr, sort->ready, N, st));
+    if (sort->executor_label_rank) GP_CUDA(c, ar.upload(o_lr, sort->executor_label_rank, 4 * N, st));
+    if (keep >= 0) GP_CUDA(c, ar.upload(o_tz, scope->topology_zone, 4 * N, st));
+    GP_CUDA(c, ar.upload(o_exe, in->exe_cpu_milli, 8 * Q, st));
+    GP_CUDA(c, ar.upload(o_exe + 8 * Q, in->exe_mem_bytes, 8 * Q, st));
+    if (in->exe_gpu) GP_CUDA(c, ar.upload(o_exe + 16 * Q, in->exe_gpu, 8 * Q, st));
     else GP_CUDA(c, cudaMemsetAsync(b + o_exe + 16 * Q, 0, 8 * Q, st));
     if (has_host) {
-        GP_CUDA(c, up(o_hoff, in->host_off, 8 * (Q + 1)));
-        if (H) GP_CUDA(c, up(o_hn, in->host_nodes, 4 * H));
+        GP_CUDA(c, ar.upload(o_hoff, in->host_off, 8 * (Q + 1), st));
+        if (H) GP_CUDA(c, ar.upload(o_hn, in->host_nodes, 4 * H, st));
     }
     const int T = 256;
     const int nb = (n + T - 1) / T;
@@ -2649,7 +2654,6 @@ gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes,
                  o_M = ar.take(8 * q1), o_zb = ar.take(8 * q1), o_out = ar.take(q1);
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
-    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
     // n_pairs and the error word are adjacent: one memset clears both
     GP_CUDA(c, cudaMemsetAsync(b + o_bcnt, 0, 4 * B, st));
     GP_CUDA(c, cudaMemsetAsync(b + o_hash, 0, sizeof(CapEntry) * H, st));
@@ -2669,11 +2673,11 @@ gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes,
         for (int d = 0; d < 6; ++d) {
             if (!cols[d]) continue;
             const size_t o = (d < 3 ? o_alloc : o_over) + 8 * N * (size_t)(d % 3);
-            GP_CUDA(c, up(o, cols[d], 8 * N));
+            GP_CUDA(c, ar.upload(o, cols[d], 8 * N, st));
             (d < 3 ? ni.alloc : ni.over)[d % 3] = (const long long*)(b + o);
         }
-        if (nodes->zone_id) { GP_CUDA(c, up(o_zone, nodes->zone_id, 4 * N)); ni.zone = (const int32_t*)(b + o_zone); }
-        if (nodes->node_group) { GP_CUDA(c, up(o_grp, nodes->node_group, 4 * N)); ni.group = (const int32_t*)(b + o_grp); }
+        if (nodes->zone_id) { GP_CUDA(c, ar.upload(o_zone, nodes->zone_id, 4 * N, st)); ni.zone = (const int32_t*)(b + o_zone); }
+        if (nodes->node_group) { GP_CUDA(c, ar.upload(o_grp, nodes->node_group, 4 * N, st)); ni.group = (const int32_t*)(b + o_grp); }
         gp_cc_nodes<<<(unsigned)((N + T - 1) / T), T, 0, st>>>(ni, s);
     }
     gp_cc_bucket_scan<<<1, 1024, 0, st>>>(s);
@@ -2683,12 +2687,12 @@ gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes,
     const int64_t* qcols[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
     for (int t = 0; t < 6; ++t) {
         if (!qcols[t]) continue;
-        GP_CUDA(c, up(o_q + 8 * q * (size_t)t, qcols[t], 8 * q));
+        GP_CUDA(c, ar.upload(o_q + 8 * q * (size_t)t, qcols[t], 8 * q, st));
         ai.q[t] = (const long long*)(b + o_q) + q * (size_t)t;
     }
-    if (Q > 0) GP_CUDA(c, up(o_cnt, a->exe_count, 4 * q));
+    if (Q > 0) GP_CUDA(c, ar.upload(o_cnt, a->exe_count, 4 * q, st));
     ai.count = (const int32_t*)(b + o_cnt);
-    if (a->group && Q > 0) { GP_CUDA(c, up(o_ag, a->group, 4 * q)); ai.group = (const int32_t*)(b + o_ag); }
+    if (a->group && Q > 0) { GP_CUDA(c, ar.upload(o_ag, a->group, 4 * q, st)); ai.group = (const int32_t*)(b + o_ag); }
     ai.n_groups = G;
     ai.hash_mask = (uint32_t)(H - 1);
     CapPair* pairs = (CapPair*)(b + o_pairs);
@@ -2732,21 +2736,17 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
     if (!c) return GP_ERR_INVALID;
     static const char* who = "gp_reconcile_find_nodes";
     auto bad = [&](gp_status st, const char* what) { return fail(c, st, std::string(who) + ": " + what); };
-    if (!usage || !nodes || !a || !out || usage->n_nodes < 0 || usage->n_reservations < 0 || nodes->n_groups < 1 || a->n_apps < 0 ||
-        (usage->n_nodes > 0 && (!usage->alloc_cpu_milli || !usage->alloc_mem_bytes || !nodes->node_group || !nodes->creation)) ||
-        (usage->n_reservations > 0 && (!usage->res_node || !usage->res_cpu_milli || !usage->res_mem_bytes)) ||
+    gp_status s = check_usage(c, usage, who);
+    if (s != GP_OK) return s;
+    if (!nodes || !a || !out || nodes->n_groups < 1 || a->n_apps < 0 || (usage->n_nodes > 0 && (!nodes->node_group || !nodes->creation)) ||
         (a->n_apps > 0 && (!a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->placed)))
         return bad(GP_ERR_INVALID, "missing arrays or bad sizes (n_groups >= 1)");
     const int32_t n = usage->n_nodes, q = a->n_apps, G = nodes->n_groups;
     for (int32_t i = 0; i < n; ++i)
         if (nodes->node_group[i] < 0 || nodes->node_group[i] >= G) return bad(GP_ERR_INVALID, "node_group out of range");
+    if ((s = check_requests(c, q, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu, who)) != GP_OK) return s;
     int64_t total = 0;
     for (int32_t i = 0; i < q; ++i) {
-        const int64_t v[3] = {a->exe_cpu_milli[i], a->exe_mem_bytes[i], a->exe_gpu ? a->exe_gpu[i] : 0};
-        for (int64_t x : v) {
-            if (x < 0) return bad(GP_ERR_INVALID, "negative resource request");
-            if (x >= kMaxQuantity) return bad(GP_ERR_UNREPRESENTABLE, "quantity >= 2^61");
-        }
         const int32_t k = a->exe_count[i];
         if (k < 0) return bad(GP_ERR_INVALID, "negative exe_count");
         if (k > kMaxCount) return bad(GP_ERR_UNREPRESENTABLE, "exe_count > 2^24");
@@ -2766,7 +2766,7 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     long long *d_avail = nullptr, *d_sched = nullptr;   // usagebuf: scratch of the availability stage, charged in place below
-    gp_status s = stage_availability(c, usage, st, &d_avail, &d_sched);
+    s = stage_availability(c, usage, st, &d_avail, &d_sched);
     if (s != GP_OK) return s;
     const size_t N = (size_t)n, Q = (size_t)q, Gs = (size_t)G, E = (size_t)total;
     Arena ar{c->reconbuf};
@@ -2778,11 +2778,10 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
                  o_exn = ar.take(4 * E), o_word = ar.take(16);
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
-    auto up = [&](size_t o, const void* src, size_t bytes) { return cudaMemcpyAsync(b + o, src, bytes, cudaMemcpyHostToDevice, st); };
-    GP_CUDA(c, up(o_grp, nodes->node_group, 4 * N));
-    GP_CUDA(c, up(o_cre, nodes->creation, 8 * N));
-    if (nodes->unschedulable) GP_CUDA(c, up(o_fu, nodes->unschedulable, N));
-    if (nodes->ready) GP_CUDA(c, up(o_fr, nodes->ready, N));
+    GP_CUDA(c, ar.upload(o_grp, nodes->node_group, 4 * N, st));
+    GP_CUDA(c, ar.upload(o_cre, nodes->creation, 8 * N, st));
+    if (nodes->unschedulable) GP_CUDA(c, ar.upload(o_fu, nodes->unschedulable, N, st));
+    if (nodes->ready) GP_CUDA(c, ar.upload(o_fr, nodes->ready, N, st));
     GP_CUDA(c, cudaMemsetAsync(b + o_word, 0, 16, st));  // claim counter, error word
     if (!c->recon_attr_set) {
         GP_CUDA(c, cudaFuncSetAttribute(gp_sort_tiles<ReconKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSortTile * sizeof(ReconKey))));
@@ -2805,20 +2804,20 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
     int32_t* cnt = (int32_t*)(b + o_word + 8);
     if (q > 0) {
         // exe cpu, mem, gpu columns, counts, groups and offsets
-        GP_CUDA(c, up(o_exe, a->exe_cpu_milli, 8 * Q));
-        GP_CUDA(c, up(o_exe + 8 * Q, a->exe_mem_bytes, 8 * Q));
-        if (a->exe_gpu) GP_CUDA(c, up(o_exe + 16 * Q, a->exe_gpu, 8 * Q));
+        GP_CUDA(c, ar.upload(o_exe, a->exe_cpu_milli, 8 * Q, st));
+        GP_CUDA(c, ar.upload(o_exe + 8 * Q, a->exe_mem_bytes, 8 * Q, st));
+        if (a->exe_gpu) GP_CUDA(c, ar.upload(o_exe + 16 * Q, a->exe_gpu, 8 * Q, st));
         else GP_CUDA(c, cudaMemsetAsync(b + o_exe + 16 * Q, 0, 8 * Q, st));
-        GP_CUDA(c, up(o_cnt, a->exe_count, 4 * Q));
-        if (a->group) GP_CUDA(c, up(o_agrp, a->group, 4 * Q));
+        GP_CUDA(c, ar.upload(o_cnt, a->exe_count, 4 * Q, st));
+        if (a->group) GP_CUDA(c, ar.upload(o_agrp, a->group, 4 * Q, st));
         else GP_CUDA(c, cudaMemsetAsync(agrp, 0, 4 * Q, st));
-        if (a->exec_out_off) GP_CUDA(c, up(o_off, a->exec_out_off, 8 * Q));
+        if (a->exec_out_off) GP_CUDA(c, ar.upload(o_off, a->exec_out_off, 8 * Q, st));
         else {
             std::vector<int64_t>& off = c->host_off;
             off.resize(Q);
             int64_t run = 0;
             for (int32_t i = 0; i < q; ++i) { off[i] = run; run += a->exe_count[i]; }
-            GP_CUDA(c, up(o_off, off.data(), 8 * Q));
+            GP_CUDA(c, ar.upload(o_off, off.data(), 8 * Q, st));
         }
         // the stale drivers partitioned by group, call order kept inside each group
         const int qb = (q + T - 1) / T;

@@ -310,6 +310,60 @@ def _p(a):
     return None if a is None else a.ctypes.data
 
 
+def _triple(t):
+    """(cpu, mem[, gpu]) columns, the gpu one absent or None -> three int64 arrays (gpu None when not given)."""
+    return [_np(t[i], np.int64) if i < len(t) else None for i in range(3)]
+
+
+def _usage_input(alloc, overhead, res_node, res):
+    """gp_usage_input over (cpu, mem[, gpu]) triples; overhead may be None.  The struct keeps its arrays alive."""
+    al, rs = _triple(alloc), _triple(res)
+    ov = _triple(overhead) if overhead is not None else [None] * 3
+    rn = _np(res_node, np.int32)
+    ui = gp_usage_input(n_nodes=len(al[0]), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
+                        overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
+                        n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
+    ui._keep = (al, ov, rn, rs)
+    return ui
+
+
+def _sort_input(n, n_zones, zone_id=None, name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None,
+                driver_label_rank=None, executor_label_rank=None, avail=(None, None, None), ties=None):
+    """gp_sort_input over n nodes.  avail: the host (cpu, mem, gpu) availability, None where the availability stage
+    supplies it on the device; ties: a c_int32 receiving undefined_ties, or None.  The struct keeps its arrays alive."""
+    ids = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(is_driver_candidate, np.uint8), _np(unschedulable, np.uint8),
+           _np(ready, np.uint8), _np(driver_label_rank, np.int32), _np(executor_label_rank, np.int32)]
+    av = [_np(x, np.int64) for x in avail]
+    si = gp_sort_input(n_nodes=n, avail_cpu_milli=_p(av[0]), avail_mem_bytes=_p(av[1]), n_zones=n_zones, zone_id=_p(ids[0]),
+                       name_rank=_p(ids[1]), is_driver_candidate=_p(ids[2]), unschedulable=_p(ids[3]), ready=_p(ids[4]),
+                       driver_label_rank=_p(ids[5]), executor_label_rank=_p(ids[6]), avail_gpu=_p(av[2]),
+                       undefined_ties=None if ties is None else C.addressof(ties))
+    si._keep = (ids, av)
+    return si
+
+
+def _hosting(hosting, q):
+    """Per-executor lists of node indices -> the (host_off[q + 1], host_nodes) CSR, or (None, None) without `hosting`."""
+    if hosting is None:
+        return None, None
+    hoff = np.zeros(q + 1, np.int64)
+    np.cumsum([len(h) for h in hosting], out=hoff[1:])
+    return hoff, np.array([v for h in hosting for v in h] or [0], np.int32)
+
+
+def _apps(apps, off, group=None, skip=None):
+    """gp_apps over the six quantity columns and count of `apps`, with these offsets, group and skip_if_no_fit columns (each
+    may be None).  The struct keeps its arrays alive."""
+    cols = [_np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")]
+    count, off = _np(apps["count"], np.int32), _np(off, np.int64)
+    group, skip = _np(group, np.int32), _np(skip, np.uint8)
+    a = gp_apps(n_apps=len(count), drv_cpu_milli=_p(cols[0]), drv_mem_bytes=_p(cols[1]), drv_gpu=_p(cols[2]),
+                exe_cpu_milli=_p(cols[3]), exe_mem_bytes=_p(cols[4]), exe_gpu=_p(cols[5]), exe_count=_p(count), group=_p(group),
+                skip_if_no_fit=_p(skip), exec_out_off=_p(off))
+    a._keep = (cols, count, off, group, skip)
+    return a
+
+
 def _az_orders(exec_order, drv_order, n_zones):
     """-> (pointer argument, kept arrays): a gp_az_orders, or NULL when all three are None (the orders
     prepare_cluster_zones(LAYOUT_AZ_AWARE) left on the device)."""
@@ -442,11 +496,7 @@ class GangPacker:
         q = len(ec)
         grp = _np(group, np.int32)
         rs = [_np(x, np.int64) for x in reserved] if reserved is not None else [None] * 3
-        hoff = hn = None
-        if hosting is not None:
-            hoff = np.zeros(q + 1, np.int64)
-            np.cumsum([len(h) for h in hosting], out=hoff[1:])
-            hn = np.array([n for h in hosting for n in h] or [0], np.int32)
+        hoff, hn = _hosting(hosting, q)
         out = np.full(max(q, 1), -9, np.int32)
         r = gp_reschedule(n_execs=q, exe_cpu_milli=_p(ec), exe_mem_bytes=_p(em), exe_gpu=_p(eg), group=_p(grp),
                           min_frag=1 if min_frag else 0, reserved_cpu_milli=_p(rs[0]), reserved_mem_bytes=_p(rs[1]),
@@ -457,28 +507,16 @@ class GangPacker:
     # ---- availability snapshot from reservations (NodeSchedulingMetadataForNodes) ----------------
     def build_availability(self, alloc, overhead, res_node, res):
         """alloc / overhead / res: (cpu, mem, gpu) triples (overhead may be None) -> (avail triple, sched triple)."""
-        al = [_np(x, np.int64) for x in alloc]
-        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
-        rn = _np(res_node, np.int32)
-        rs = [_np(x, np.int64) for x in res]
-        n = len(al[0])
-        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
-                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
-                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
         outs = [np.empty(max(n, 1), np.int64) for _ in range(6)]
         self._check(load().gp_build_availability(self._h, C.byref(ui), *[_p(o) for o in outs]))
         return [o[:n] for o in outs[:3]], [o[:n] for o in outs[3:]]
 
     def build_reschedule_availability(self, alloc, overhead, res_node, res):
         """availableResources of rescheduleExecutor's first-fit branch (overhead counted twice on nodes with reservations)."""
-        al = [_np(x, np.int64) for x in alloc]
-        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
-        rn = _np(res_node, np.int32)
-        rs = [_np(x, np.int64) for x in res]
-        n = len(al[0])
-        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
-                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
-                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
         outs = [np.empty(max(n, 1), np.int64) for _ in range(3)]
         self._check(load().gp_build_reschedule_availability(self._h, C.byref(ui), *[_p(o) for o in outs]))
         return [o[:n] for o in outs]
@@ -491,18 +529,10 @@ class GangPacker:
         lists of node indices already hosting executors of the same application, or None; keep_topology_zone: None (every
         node) or the zone id filterNodesToZone keeps, with topology_zone[n] the node's zone id (-1 = label missing).
         The context's snapshot is not touched.  -> (node index per executor or -1, ambiguous flag per executor)."""
-        al = [_np(x, np.int64) for x in alloc]
-        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
-        rn = _np(res_node, np.int32)
-        rs = [_np(x, np.int64) for x in res]
-        n = len(al[0])
-        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
-                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
-                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
-        arrs = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(unschedulable, np.uint8), _np(ready, np.uint8),
-                _np(executor_label_rank, np.int32)]
-        si = gp_sort_input(n_nodes=n, n_zones=n_zones, zone_id=_p(arrs[0]), name_rank=_p(arrs[1]), unschedulable=_p(arrs[2]),
-                           ready=_p(arrs[3]), executor_label_rank=_p(arrs[4]))
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
+        si = _sort_input(n, n_zones, zone_id=zone_id, name_rank=name_rank, unschedulable=unschedulable, ready=ready,
+                         executor_label_rank=executor_label_rank)
         tz = _np(topology_zone, np.int32)
         scope = None
         if keep_topology_zone is not None:
@@ -510,11 +540,7 @@ class GangPacker:
         ec, em = _np(exe[0], np.int64), _np(exe[1], np.int64)
         eg = _np(exe[2], np.int64) if len(exe) > 2 else None
         q = len(ec)
-        hoff = hn = None
-        if hosting is not None:
-            hoff = np.zeros(q + 1, np.int64)
-            np.cumsum([len(h) for h in hosting], out=hoff[1:])
-            hn = np.array([v for h in hosting for v in h] or [0], np.int32)
+        hoff, hn = _hosting(hosting, q)
         r = gp_reschedule(n_execs=q, exe_cpu_milli=_p(ec), exe_mem_bytes=_p(em), exe_gpu=_p(eg), min_frag=1 if min_frag else 0,
                           host_off=_p(hoff), host_nodes=_p(hn))
         out = np.full(max(q, 1), -9, np.int32)
@@ -526,19 +552,10 @@ class GangPacker:
     def prepare_cluster(self, alloc, overhead, res_node, res, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None):
         """reservations -> availability -> priority orders -> snapshot, chained on the device.  -> (n_driver, n_executor)."""
-        al = [_np(x, np.int64) for x in alloc]
-        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
-        rn = _np(res_node, np.int32)
-        rs = [_np(x, np.int64) for x in res]
-        n = len(al[0])
-        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
-                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
-                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
-        arrs = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(is_driver_candidate, np.uint8), _np(unschedulable, np.uint8),
-                _np(ready, np.uint8), _np(driver_label_rank, np.int32), _np(executor_label_rank, np.int32)]
-        si = gp_sort_input(n_nodes=n, avail_cpu_milli=None, avail_mem_bytes=None, n_zones=n_zones, zone_id=_p(arrs[0]),
-                           name_rank=_p(arrs[1]), is_driver_candidate=_p(arrs[2]), unschedulable=_p(arrs[3]), ready=_p(arrs[4]),
-                           driver_label_rank=_p(arrs[5]), executor_label_rank=_p(arrs[6]))
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
+        si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
+                         executor_label_rank)
         nd, ne = C.c_int32(0), C.c_int32(0)
         self._check(load().gp_prepare_cluster(self._h, C.byref(ui), C.byref(si), C.byref(nd), C.byref(ne)))
         self.n_nodes = n
@@ -550,20 +567,11 @@ class GangPacker:
         """reservations -> availability -> priority orders -> zone-grouped snapshot (kind LAYOUT_SINGLE_AZ or LAYOUT_AZ_AWARE),
         chained on the device, SchedulableResources included.  -> dict with n_zones, n_groups, n_driver, n_executor,
         zone_of_group, undefined_ties and, with `layout`, the grouped exec_off / exec_order / drv_off / drv_order."""
-        al = [_np(x, np.int64) for x in alloc]
-        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
-        rn = _np(res_node, np.int32)
-        rs = [_np(x, np.int64) for x in res]
-        n = len(al[0])
-        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
-                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]),
-                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]), res_gpu=_p(rs[2]))
-        arrs = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(is_driver_candidate, np.uint8), _np(unschedulable, np.uint8),
-                _np(ready, np.uint8), _np(driver_label_rank, np.int32), _np(executor_label_rank, np.int32)]
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
         ties = C.c_int32(0)
-        si = gp_sort_input(n_nodes=n, avail_cpu_milli=None, avail_mem_bytes=None, n_zones=n_zones, zone_id=_p(arrs[0]),
-                           name_rank=_p(arrs[1]), is_driver_candidate=_p(arrs[2]), unschedulable=_p(arrs[3]), ready=_p(arrs[4]),
-                           driver_label_rank=_p(arrs[5]), executor_label_rank=_p(arrs[6]), undefined_ties=C.addressof(ties))
+        si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
+                         executor_label_rank, ties=ties)
         zog = np.full(n_zones + 1, -9, np.int32)
         bufs = {k: np.full(max(n, 1) if k.endswith("order") else n_zones + 2, -9, np.int32)
                 for k in ("exec_off", "exec_order", "drv_off", "drv_order")} if layout else {}
@@ -583,16 +591,10 @@ class GangPacker:
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None, avail_gpu=None):
         """-> (driver_order, executor_order) as int32 node-index arrays.  With avail_gpu given, self.undefined_ties is the
         number of adjacent pairs the reference's comparator leaves undefined (SURVEY App. B6)."""
-        cpu, mem = _np(avail_cpu, np.int64), _np(avail_mem, np.int64)
-        gpu = _np(avail_gpu, np.int64)
-        n = len(cpu)
-        arrs = [_np(zone_id, np.int32), _np(name_rank, np.int32), _np(is_driver_candidate, np.uint8), _np(unschedulable, np.uint8),
-                _np(ready, np.uint8), _np(driver_label_rank, np.int32), _np(executor_label_rank, np.int32)]
+        n = len(avail_cpu)
         ties = C.c_int32(0)
-        si = gp_sort_input(n_nodes=n, avail_cpu_milli=_p(cpu), avail_mem_bytes=_p(mem), n_zones=n_zones, zone_id=_p(arrs[0]),
-                           name_rank=_p(arrs[1]), is_driver_candidate=_p(arrs[2]), unschedulable=_p(arrs[3]), ready=_p(arrs[4]),
-                           driver_label_rank=_p(arrs[5]), executor_label_rank=_p(arrs[6]), avail_gpu=_p(gpu),
-                           undefined_ties=C.addressof(ties))
+        si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
+                         executor_label_rank, avail=(avail_cpu, avail_mem, avail_gpu), ties=ties)
         d = np.empty(max(n, 1), np.int32); e = np.empty(max(n, 1), np.int32)
         nd, ne = C.c_int32(0), C.c_int32(0)
         self._check(load().gp_potential_nodes(self._h, C.byref(si), _p(d), C.byref(nd), _p(e), C.byref(ne)))
@@ -654,85 +656,44 @@ class GangPacker:
         c, m, g = _np(sched_cpu, np.int64), _np(sched_mem, np.int64), _np(sched_gpu, np.int64)
         self._check(load().gp_set_schedulable(self._h, _p(c), _p(m), _p(g)))
 
-    def pack_batch_zones(self, apps: dict, algo: int):
-        """single-az-tightly-pack / single-az-minimal-fragmentation for a batch: the snapshot's instance groups are the
-        candidate zones.  -> (zone[q], driver_node[q], executor_nodes, off[q+1], avg_efficiency[q,4])."""
+    def _pack_zones(self, apps: dict, skip, fn, *args):
+        """The zone packs' shared body: fn(ctx, apps, *args, results) -> (zone, driver_node, executor_nodes, off, avg_efficiency)."""
         q = len(apps["count"])
-        count = _np(apps["count"], np.int32)
         off = np.zeros(q + 1, np.int64)
-        np.cumsum(np.maximum(count, 0), out=off[1:])
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
+        np.cumsum(np.maximum(_np(apps["count"], np.int32), 0), out=off[1:])
         total = int(off[-1]) if q else 0
         zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
         exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
+        a = _apps(apps, off, skip=skip)
         r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
-        self._check(load().gp_pack_batch_zones(self._h, C.byref(a), algo, C.byref(r)))
+        self._check(fn(self._h, C.byref(a), *args, C.byref(r)))
         return zone, drv, exe[:total], off, avg[:q]
+
+    def pack_batch_zones(self, apps: dict, algo: int):
+        """single-az-tightly-pack / single-az-minimal-fragmentation for a batch: the snapshot's instance groups are the
+        candidate zones.  -> (zone[q], driver_node[q], executor_nodes, off[q+1], avg_efficiency[q,4])."""
+        return self._pack_zones(apps, None, load().gp_pack_batch_zones, algo)
 
     def pack_fifo_zones(self, apps: dict, algo: int, mode: int = 1):
         """fitEarlierDrivers with a single-AZ packer in one launch: `apps` is the queue in order (optional "young" = skip the
         driver instead of blocking the queue when it fits nowhere).  -> like pack_batch_zones; driver_node -2 = never evaluated."""
-        q = len(apps["count"])
-        count = _np(apps["count"], np.int32)
-        off = np.zeros(q + 1, np.int64)
-        np.cumsum(np.maximum(count, 0), out=off[1:])
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
-        young = _np(apps.get("young"), np.uint8)
-        total = int(off[-1]) if q else 0
-        zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
-        exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=None, skip_if_no_fit=_p(young), exec_out_off=_p(off))
-        r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
-        self._check(load().gp_pack_fifo_zones(self._h, C.byref(a), algo, mode, C.byref(r)))
-        return zone, drv, exe[:total], off, avg[:q]
+        return self._pack_zones(apps, apps.get("young"), load().gp_pack_fifo_zones, algo, mode)
 
     def pack_fifo_az_aware(self, apps: dict, mode: int, exec_order=None, drv_order=None, n_zones=None):
         """fitEarlierDrivers with az-aware-tightly-pack in one launch.  The snapshot's groups 0..n_zones-1 are the candidate
         zones, the groups after them the remaining nodes; exec_order / drv_order are the undivided priority orders (node
         indices) of the fallback -- all three None (orders == NULL): the ones prepare_cluster_zones(LAYOUT_AZ_AWARE) left on
         the device.  -> like pack_fifo_zones; zone -1 with driver_node >= 0 = placed by the fallback."""
-        q = len(apps["count"])
-        count = _np(apps["count"], np.int32)
-        off = np.zeros(q + 1, np.int64)
-        np.cumsum(np.maximum(count, 0), out=off[1:])
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
-        young = _np(apps.get("young"), np.uint8)
-        o = _az_orders(exec_order, drv_order, n_zones)
-        total = int(off[-1]) if q else 0
-        zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
-        exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=None, skip_if_no_fit=_p(young), exec_out_off=_p(off))
-        r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
-        self._check(load().gp_pack_fifo_az_aware(self._h, C.byref(a), mode, o[0], C.byref(r)))
-        return zone, drv, exe[:total], off, avg[:q]
+        o, _keep = _az_orders(exec_order, drv_order, n_zones)
+        return self._pack_zones(apps, apps.get("young"), load().gp_pack_fifo_az_aware, mode, o)
 
     def pack_batch_az_aware(self, apps: dict, exec_order=None, drv_order=None, n_zones=None):
         """az-aware-tightly-pack for a batch of independent decisions against the unmodified snapshot, in one call.  The
         snapshot layout is that of pack_fifo_az_aware (any n_zones up to the number of groups); exec_order / drv_order are
         the undivided priority orders (node indices) of the fallback, or all three None as in pack_fifo_az_aware.
         -> like pack_batch_zones; zone -1 with driver_node >= 0 = placed by the fallback (zero averages)."""
-        q = len(apps["count"])
-        count = _np(apps["count"], np.int32)
-        off = np.zeros(q + 1, np.int64)
-        np.cumsum(np.maximum(count, 0), out=off[1:])
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
-        o = _az_orders(exec_order, drv_order, n_zones)
-        total = int(off[-1]) if q else 0
-        zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
-        exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
-        r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
-        self._check(load().gp_pack_batch_az_aware(self._h, C.byref(a), o[0], C.byref(r)))
-        return zone, drv, exe[:total], off, avg[:q]
+        o, _keep = _az_orders(exec_order, drv_order, n_zones)
+        return self._pack_zones(apps, None, load().gp_pack_batch_az_aware, o)
 
     def reserve_placements(self, apps: dict, placed, subtract=True):
         """newResourceReservation for a packed batch -> dict of row arrays (app, slot, node, cpu, mem, gpu); with subtract the
@@ -740,14 +701,11 @@ class GangPacker:
         q = len(apps["count"])
         count = _np(apps["count"], np.int32)
         driver, execn, off = placed
-        driver = _np(driver, np.int32); execn = _np(execn, np.int32); off = _np(off, np.int64)
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
+        driver = _np(driver, np.int32); execn = _np(execn, np.int32)
         rows = int(((driver >= 0) * (1 + np.maximum(count, 0).astype(np.int64))).sum()) if q else 0
         t = {k: np.zeros(max(rows, 1), np.int32) for k in ("app", "slot", "node")}
         t.update({k: np.zeros(max(rows, 1), np.int64) for k in ("cpu", "mem", "gpu")})
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
+        a = _apps(apps, off)
         r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
         tab = gp_reservation_table(rows_cap=len(t["app"]), app=_p(t["app"]), slot=_p(t["slot"]), node=_p(t["node"]),
                                    cpu_milli=_p(t["cpu"]), mem_bytes=_p(t["mem"]), gpu=_p(t["gpu"]), n_rows=0)
@@ -764,16 +722,12 @@ class GangPacker:
         them (zone results: (driver_node, executor_nodes, off) of the zone call).  algo decides what counts as reserved
         (MINIMAL_FRAGMENTATION: the driver only); charged = MODE_FIFO_* adds that one application's charged usage back first."""
         q = len(apps["count"])
-        count = _np(apps["count"], np.int32)
         driver, execn, off = placed
-        driver = _np(driver, np.int32); execn = _np(execn, np.int32); off = _np(off, np.int64)
+        driver = _np(driver, np.int32); execn = _np(execn, np.int32)
         if execn is None or len(execn) == 0:
             execn = np.zeros(1, np.int32)
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
         avg = np.zeros((max(q, 1), 4), np.float64)
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=None, skip_if_no_fit=None, exec_out_off=_p(off))
+        a = _apps(apps, off)
         r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
         self._check(load().gp_packing_efficiency(self._h, C.byref(a), algo, C.byref(r), charged, _p(avg)))
         return avg[:q]
@@ -785,9 +739,6 @@ class GangPacker:
         class per node, -1 = none (None = all 0).  apps: drv_*, exe_*, count and group (the driver's class, -1 = every node).
         -> uint8[n_apps], 1 = exceeds cluster capacity.  Leaves the context's snapshot and statistics untouched."""
         q = len(apps["count"])
-        count = _np(apps["count"], np.int32)
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")}
-        group = _np(apps.get("group"), np.int32)
         al = [_np(v, np.int64) for v in alloc]
         ov = [_np(v, np.int64) for v in overhead] if overhead is not None else [None, None, None]
         zid, grp = _np(zone_id, np.int32), _np(node_group, np.int32)
@@ -795,9 +746,7 @@ class GangPacker:
                                alloc_gpu=_p(al[2] if len(al) > 2 else None), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]),
                                overhead_gpu=_p(ov[2] if len(ov) > 2 else None), n_zones=int(n_zones), zone_id=_p(zid),
                                n_groups=int(n_groups), node_group=_p(grp))
-        a = gp_apps(n_apps=q, drv_cpu_milli=_p(arrs["drv_cpu"]), drv_mem_bytes=_p(arrs["drv_mem"]), drv_gpu=_p(arrs["drv_gpu"]),
-                    exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=_p(group), skip_if_no_fit=None, exec_out_off=None)
+        a = _apps(apps, None, group=apps.get("group"))
         out = np.full(max(q, 1), 255, np.uint8)
         self._check(load().gp_exceeds_cluster_capacity(self._h, C.byref(nd), C.byref(a), int(packer), _p(out)))
         return out[:q]
@@ -810,26 +759,16 @@ class GangPacker:
         (UnixNano); apps: exe_cpu, exe_mem, exe_gpu (optional), count = max(0, Min - running) and group, in call order.
         -> (placed[q] (-1 = instance group not found), executor_nodes (CSR by off), off[q + 1], (cpu, mem, gpu) availability after
         the loop or None).  Leaves the context's snapshot and statistics untouched."""
-        al = [_np(x, np.int64) for x in alloc]
-        ov = [_np(x, np.int64) for x in overhead] if overhead is not None else [None] * 3
-        rn = _np(res_node, np.int32)
-        rs = [_np(x, np.int64) for x in res]
-        n = len(al[0])
-        ui = gp_usage_input(n_nodes=n, alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2] if len(al) > 2 else None),
-                            overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2] if len(ov) > 2 else None),
-                            n_reservations=len(rn), res_node=_p(rn), res_cpu_milli=_p(rs[0]), res_mem_bytes=_p(rs[1]),
-                            res_gpu=_p(rs[2] if len(rs) > 2 else None))
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
         ng, cr = _np(node_group, np.int32), _np(creation, np.int64)
         fu, fr = _np(unschedulable, np.uint8), _np(ready, np.uint8)
         nd = gp_reconcile_nodes(n_groups=int(n_groups), node_group=_p(ng), creation=_p(cr), unschedulable=_p(fu), ready=_p(fr))
         count = _np(apps["count"], np.int32)
         q = len(count)
-        arrs = {k: _np(apps.get(k), np.int64) for k in ("exe_cpu", "exe_mem", "exe_gpu")}
-        group = _np(apps.get("group"), np.int32)
         off = np.zeros(q + 1, np.int64)
         np.cumsum(count, out=off[1:])
-        a = gp_apps(n_apps=q, exe_cpu_milli=_p(arrs["exe_cpu"]), exe_mem_bytes=_p(arrs["exe_mem"]), exe_gpu=_p(arrs["exe_gpu"]),
-                    exe_count=_p(count), group=_p(group), exec_out_off=_p(off))
+        a = _apps(apps, off, group=apps.get("group"))
         placed = np.full(max(q, 1), -9, np.int32)
         cap = int(off[q]) if exec_cap is None else int(exec_cap)
         execn = np.full(max(cap, 1), -9, np.int32)
