@@ -653,8 +653,8 @@ typedef struct {
     int64_t kernel_launches;   /* launches of this library's kernels in that call */
     int64_t pack_kernel_ns;    /* device time of the pack kernels (CUDA events on the launch stream; independent tightly/evenly:
                                   the one classify + capacity tables + decide launch and the scan of the listed applications) */
-    int64_t prep_kernel_ns;    /* device time of the work before them (preparation kernel; independent tightly/evenly: the
-                                  memset of the shape-table header) */
+    int64_t prep_kernel_ns;    /* device time of the work before them (preparation kernel; independent tightly/evenly: 0, the
+                                  one launch prepares the applications itself and nothing runs before it) */
     int64_t scan_path_apps;    /* independent tightly/evenly: applications decided by the node-order scan instead of the
                                   per-shape capacity tables (all of them with GANGPACK_TABLES=0).
                                   FIFO modes: applications decided by the whole CTA instead of warp 0 alone (every

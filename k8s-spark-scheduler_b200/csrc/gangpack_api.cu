@@ -150,46 +150,65 @@ __device__ __forceinline__ int32_t find_group(const int32_t* off, int32_t n_grou
     return lo;
 }
 
-// snapshot-wide facts: negative gpu availability, per-dimension maxima (bounds for the fast class)
-// Called by the threads of a warp that own a node (`active` = their mask): the warp combines its values with
-// shuffles and issues at most one atomic per dimension.
-__device__ __forceinline__ long long warp_max_ll(unsigned active, long long v) {
+// snapshot-wide facts: negative gpu availability, per-dimension maxima (bounds for the fast class).  A CTA of
+// gp_build_slots_exec reduces its nodes' values to one SnapPart; every CTA of gp_build_slots_drv folds all parts.
+struct SnapPart { long long max_avail[3]; int flags; int pad; };
+static_assert(sizeof(SnapPart) == 32, "SnapPart layout");
+constexpr int kSnapThreads = 256;       // threads per CTA of both layout kernels
+// Block-wide max of (c, m, g) and OR of f, called by every thread of the CTA; the result is valid in thread 0.
+__device__ __forceinline__ void block_fold(long long& c, long long& m, long long& g, int& f) {
+    __shared__ SnapPart s_part[kSnapThreads / 32];
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) {
-        long long o = __shfl_xor_sync(active, v, d);     // lanes outside `active` return their own value: harmless for max
-        v = o > v ? o : v;
+        c = max(c, __shfl_xor_sync(kFull, c, d));
+        m = max(m, __shfl_xor_sync(kFull, m, d));
+        g = max(g, __shfl_xor_sync(kFull, g, d));
+        f |= __shfl_xor_sync(kFull, f, d);
     }
-    return v;
-}
-__device__ __forceinline__ void note_node(SnapMeta* meta, int64_t cv, int64_t mv, int64_t gv) {
-    const unsigned active = __activemask();
-    const bool full = active == 0xffffffffu;
-    if (__any_sync(active, gv < 0) && (threadIdx.x & 31) == (__ffs(active) - 1)) atomicOr(&meta->flags, kSnapGpuNegative);
-    long long c = cv, m = mv, g = gv;
-    if (full) { c = warp_max_ll(active, c); m = warp_max_ll(active, m); g = warp_max_ll(active, g); }
-    if (!full || (threadIdx.x & 31) == 0) {
-        if (c > 0 && c > meta->max_avail[0]) atomicMax(&meta->max_avail[0], c);
-        if (m > 0 && m > meta->max_avail[1]) atomicMax(&meta->max_avail[1], m);
-        if (g > 0 && g > meta->max_avail[2]) atomicMax(&meta->max_avail[2], g);
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    __syncthreads();                    // s_part may still be read by an earlier call
+    if (lane == 0) { s_part[w].max_avail[0] = c; s_part[w].max_avail[1] = m; s_part[w].max_avail[2] = g; s_part[w].flags = f; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int t = 1; t < kSnapThreads / 32; ++t) {
+            c = max(c, s_part[t].max_avail[0]); m = max(m, s_part[t].max_avail[1]); g = max(g, s_part[t].max_avail[2]);
+            f |= s_part[t].flags;
+        }
     }
 }
 
-// The slot layout is two launches (gp_set_snapshot, gp_set_snapshot_device, gp_prepare_cluster):
-// K1 gp_build_slots_exec: thread i writes group descriptor i, lays out executor-order entry i in its slot and notes the
-//    availability of driver-order entry i in the snapshot maxima / flags (a node's availability does not depend on its slot);
-//    with node_cpu != NULL it also copies node-table entry i into the context's node-table arrays (gp_get_snapshot);
-// K2 gp_build_slots_drv: thread s owns slot s.  Executor slots get their compact view; the spare slot of driver-order
+// The slot layout is two launches (gp_set_snapshot, gp_set_snapshot_device, gp_prepare_cluster), and no memset: every
+// word they leave behind is written by one of them.
+// K1 gp_build_slots_exec: thread i writes group descriptor i, lays out executor-order entry i in its slot, scatters
+//    drv_pos[node] = i for driver-order entry i, and takes the availability of both entries into its CTA's SnapPart (a
+//    node's availability does not depend on its slot); with node_cpu != NULL it also copies node-table entry i into the
+//    context's node-table arrays (gp_get_snapshot).  Every CTA writes its part, zeros included, so nothing needs a reset.
+// K2 gp_build_slots_drv: every CTA first folds K1's parts (written by the previous launch on the stream: no fence or
+//    counter needed) into the maxima its compact views shift by; CTA 0 publishes them in SnapMeta (flags, max_avail,
+//    shift32).  Thread s <= n_slots owns slot s.  Executor slots get their compact view; the spare slot of driver-order
 //    entry j either receives that node (driver-only) or stays unused (-1: the node has an executor slot in the group);
 //    slots past the last group (the orders' lengths may be upper bounds) are -1 as well.  So no slot_node memset is needed.
+//    Thread n_slots + 1 + v owns node v: it writes node_slot[v] = -1 when v is in neither order.
+// node_slot and drv_pos keep whatever an earlier layout left (garbage after a reallocation), so membership is tested
+// against the arrays K1 has just rewritten, with every stale index range-checked before it is followed:
+//   v is in the driver order     iff  p = drv_pos[v] lies in [0, drv_off[n_groups]) and drv_order[p] == v;
+//   v has executor slot ns       iff  ns = node_slot[v] is an executor slot of its group and slot_node[ns] == v.
+// Race freedom of K2: node_slot[v] is written by K1 (executor nodes), by the slot thread of v's driver-order entry
+// (driver-only nodes) or by node thread v (nodes in neither order) -- one writer per entry.  The slot thread reads
+// node_slot[v] only for its own node, and the node thread only when v is not in the driver order, so neither reads an
+// entry another K2 thread writes.  slot_node is read at executor slots only, which K1 wrote and K2 does not touch.
 // n_exec / n_drv may be upper bounds of exec_off[n_groups] / drv_off[n_groups] (device-built orders).
-__global__ void gp_build_slots_exec(int32_t n_exec, int32_t n_drv, int32_t n_groups, int32_t n_nodes,
+__global__ void __launch_bounds__(kSnapThreads) gp_build_slots_exec(int32_t n_exec, int32_t n_drv, int32_t n_groups, int32_t n_nodes,
                                     const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
                                     const int32_t* __restrict__ exec_order, const int32_t* __restrict__ drv_order,
                                     const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
                                     GroupDesc* __restrict__ groups, longlong2* __restrict__ pair, int64_t* __restrict__ sgpu,
-                                    int32_t* __restrict__ slot_node, int32_t* __restrict__ node_slot, SnapMeta* __restrict__ meta,
+                                    int32_t* __restrict__ slot_node, int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_pos,
+                                    SnapPart* __restrict__ parts,
                                     int64_t* __restrict__ node_cpu, int64_t* __restrict__ node_mem, int64_t* __restrict__ node_gpu) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    long long c = 0, m = 0, gm = 0;      // only positive availabilities raise the maxima
+    int neg = 0;
     if (node_cpu && i < n_nodes) {
         node_cpu[i] = cpu[i];
         node_mem[i] = mem[i];
@@ -210,42 +229,86 @@ __global__ void gp_build_slots_exec(int32_t n_exec, int32_t n_drv, int32_t n_gro
         const int64_t cv = cpu[node], mv = mem[node], gv = gpu ? gpu[node] : 0;
         pair[slot] = make_longlong2(cv, mv);
         sgpu[slot] = gv;
-        note_node(meta, cv, mv, gv);
+        c = max(c, (long long)cv); m = max(m, (long long)mv); gm = max(gm, (long long)gv); neg |= gv < 0;
         slot_node[slot] = node;
         node_slot[node] = slot;
     }
     if (i < n_drv && i < drv_off[n_groups]) {
         const int32_t node = drv_order[i];
-        note_node(meta, cpu[node], mem[node], gpu ? gpu[node] : 0);
+        const long long gv = gpu ? gpu[node] : 0;
+        c = max(c, (long long)cpu[node]); m = max(m, (long long)mem[node]); gm = max(gm, gv); neg |= gv < 0;
+        drv_pos[node] = i;
+    }
+    block_fold(c, m, gm, neg);
+    if (threadIdx.x == 0) {
+        SnapPart p;
+        p.max_avail[0] = c; p.max_avail[1] = m; p.max_avail[2] = gm; p.flags = neg ? kSnapGpuNegative : 0; p.pad = 0;
+        parts[blockIdx.x] = p;
     }
 }
 
 __device__ __forceinline__ int shift_for(long long mx);
 __device__ __forceinline__ uint2 compact_pair(longlong2 v, int s0, int s1);
 
-__global__ void gp_build_slots_drv(int32_t n_slots, int32_t n_groups,
-                                   const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
-                                   const int32_t* __restrict__ drv_order,
-                                   const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
-                                   longlong2* __restrict__ pair, int64_t* __restrict__ sgpu, int32_t* __restrict__ slot_node,
-                                   int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_slot, SnapMeta* __restrict__ meta,
-                                   uint2* __restrict__ pair32) {
-    const int s0 = shift_for(meta->max_avail[0]), s1 = shift_for(meta->max_avail[1]);
-    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s == 0) { meta->shift32[0] = s0; meta->shift32[1] = s1; }
-    if (s > n_slots) return;
-    if (s >= exec_off[n_groups] + drv_off[n_groups]) {       // past the last group
-        slot_node[s] = -1;
-        if (s < n_slots) pair32[s] = make_uint2(0u, 0u);
-        return;
-    }
-    // the group whose slots [exec_off[g] + drv_off[g], exec_off[g+1] + drv_off[g+1]) hold s
+// the group whose slots [exec_off[g] + drv_off[g], exec_off[g+1] + drv_off[g+1]) hold slot s (s below the last group's end)
+__device__ __forceinline__ int32_t slot_group(const int32_t* exec_off, const int32_t* drv_off, int32_t n_groups, int32_t s) {
     int32_t lo = 0, hi = n_groups - 1;
     while (lo < hi) {
         const int32_t mid = (lo + hi + 1) >> 1;
         if (exec_off[mid] + drv_off[mid] <= s) lo = mid; else hi = mid - 1;
     }
-    const int32_t g = lo;
+    return lo;
+}
+
+__global__ void __launch_bounds__(kSnapThreads) gp_build_slots_drv(int32_t n_slots, int32_t n_groups, int32_t n_nodes, int32_t n_drv,
+                                   const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
+                                   const int32_t* __restrict__ drv_order, const int32_t* __restrict__ drv_pos,
+                                   const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
+                                   longlong2* __restrict__ pair, int64_t* __restrict__ sgpu, int32_t* __restrict__ slot_node,
+                                   int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_slot, const SnapPart* __restrict__ parts,
+                                   int32_t n_parts, SnapMeta* __restrict__ meta, uint2* __restrict__ pair32) {
+    __shared__ long long s_max[2];
+    {
+        long long c = 0, m = 0, g = 0;
+        int f = 0;
+        for (int32_t b = threadIdx.x; b < n_parts; b += blockDim.x) {
+            const SnapPart p = parts[b];
+            c = max(c, p.max_avail[0]); m = max(m, p.max_avail[1]); g = max(g, p.max_avail[2]); f |= p.flags;
+        }
+        block_fold(c, m, g, f);
+        if (threadIdx.x == 0) {
+            s_max[0] = c; s_max[1] = m;
+            if (blockIdx.x == 0) {
+                meta->flags = f; meta->pad = 0;
+                meta->max_avail[0] = c; meta->max_avail[1] = m; meta->max_avail[2] = g;
+                meta->shift32[0] = shift_for(c); meta->shift32[1] = shift_for(m);
+            }
+        }
+        __syncthreads();
+    }
+    const int s0 = shift_for(s_max[0]), s1 = shift_for(s_max[1]);
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    const int32_t used = exec_off[n_groups] + drv_off[n_groups];
+    if (s > n_slots) {                                       // node v: -1 when it is in neither order
+        const int32_t v = s - n_slots - 1;
+        if (v > n_nodes) return;
+        const int32_t p = drv_pos[v];
+        if (p >= 0 && p < drv_off[n_groups] && p < n_drv && drv_order[p] == v) return;
+        const int32_t ns = node_slot[v];
+        bool exec = false;
+        if (ns >= 0 && ns < used) {
+            const int32_t g = slot_group(exec_off, drv_off, n_groups, ns);
+            exec = ns - (exec_off[g] + drv_off[g]) < exec_off[g + 1] - exec_off[g] && slot_node[ns] == v;
+        }
+        if (!exec) node_slot[v] = -1;
+        return;
+    }
+    if (s >= used) {                                         // past the last group
+        slot_node[s] = -1;
+        if (s < n_slots) pair32[s] = make_uint2(0u, 0u);
+        return;
+    }
+    const int32_t g = slot_group(exec_off, drv_off, n_groups, s);
     const int32_t sbase = exec_off[g] + drv_off[g];
     const int32_t ne = exec_off[g + 1] - exec_off[g];
     const int32_t local = s - sbase;
@@ -256,7 +319,7 @@ __global__ void gp_build_slots_drv(int32_t n_slots, int32_t n_groups,
     const int32_t j = drv_off[g] + (local - ne);
     const int32_t node = drv_order[j];
     const int32_t ns = node_slot[node];
-    if (ns >= sbase && ns < sbase + ne) {
+    if (ns >= sbase && ns < sbase + ne && slot_node[ns] == node) {
         drv_slot[j] = ns - sbase;
         slot_node[s] = -1;                                   // unused spare slot
         pair32[s] = make_uint2(0u, 0u);
@@ -343,6 +406,12 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
+    // reserve() for state the kernels leave zeroed after every use: a new allocation starts out all zero
+    cudaError_t reserve_zeroed(size_t bytes, cudaStream_t st) {
+        if (bytes <= cap) return cudaSuccess;
+        const cudaError_t e = reserve(bytes);
+        return e != cudaSuccess ? e : cudaMemsetAsync(p, 0, cap, st);
+    }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
@@ -383,14 +452,15 @@ struct StatusHead {
 static_assert(offsetof(StatusHead, stats) % 8 == 0, "64-bit atomics on the statistics need 8-byte alignment");
 static_assert(sizeof(StatusHead) == 40, "gp_last_stats copies the error bits and the four statistics");
 
-// Device status words of one pack call, zeroed by pack_begin
+// Device status words of one pack call, zeroed by pack_begin or by gp_decide_tables' first classify tile
 struct DevStatus {
     StatusHead head;
     unsigned int az_listed, az_claim;       // gp_pack_az_fallback: length of its application list, its claim counter
     unsigned int fifo_cursor;               // FIFO kernels: instance-group cursor
     unsigned int next_app[kMaxChunks];      // per pipelined chunk: application claim counter
+    unsigned int spare[3];
 };
-static_assert(sizeof(DevStatus) <= 128, "pack_begin zeroes the block on every call");
+static_assert(sizeof(DevStatus) == 4 * kStatusWords, "gp_decide_tables zeroes the whole block");
 
 // Pinned host block: the mirror of StatusHead (gp_last_stats) and the error word the kernels write through its mapping
 struct PinnedStatus { StatusHead head; volatile int err_word; };
@@ -413,6 +483,8 @@ struct gp_ctx {
     DevBuf node_cpu, node_mem, node_gpu;        // node-table order (as given)
     DevBuf exec_off, drv_off, exec_order, drv_order;
     DevBuf pair, pair32, sgpu, slot_node, node_slot, drv_slot, groups, snap_flags;
+    DevBuf drv_pos;                             // node -> driver-order position, scattered by the layout (gp_build_slots_exec)
+    DevBuf snap_part;                           // SnapPart per CTA of gp_build_slots_exec
 
     // batch staging; a_rows: the six quantity rows in one pitched block (pack_batch_impl)
     DevBuf a_rows, a_count, a_group, a_skip, a_off;
@@ -445,6 +517,7 @@ struct gp_ctx {
     // per pipeline lane: shape hash + header, capacity tables, group totals, placement prefixes, per-application shape slot
     struct TableSet { DevBuf hdr, table, total, place, app_slot; } tabs[kLanes];
     bool record_events = true;                    // CUDA events around the kernels (gp_last_stats); the pipelined host path skips them
+    bool ev_prep = false;                         // the last pack recorded a prep interval ev[i][0] .. ev[i][1] (not the tables path)
     int use_graphs = 1;                           // GANGPACK_GRAPHS=0: always issue the launches one by one
     GraphCache g_chunk[kMaxChunks + 1];           // per pipelined chunk (+1: an unchunked batch on the context's own stream): classify .. scan
     GraphCache g_snapshot;                        // slot layout of gp_set_snapshot
@@ -619,7 +692,10 @@ gp_status gp_create(gp_ctx** out, const gp_config* cfg) {
         (e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = create_aux(c)) != cudaSuccess ||
         (e = cudaHostAlloc(&c->pinned_misc, sizeof(PinnedStatus), cudaHostAllocDefault)) != cudaSuccess ||
-        (e = c->dev_misc.reserve(sizeof(DevStatus))) != cudaSuccess || (e = c->snap_flags.reserve(sizeof(SnapMeta))) != cudaSuccess) {
+        (e = c->dev_misc.reserve(sizeof(DevStatus))) != cudaSuccess || (e = c->snap_flags.reserve(sizeof(SnapMeta))) != cudaSuccess ||
+        // the layout writes every SnapMeta word but the padding
+        (e = cudaMemsetAsync(c->snap_flags.p, 0, sizeof(SnapMeta), c->stream)) != cudaSuccess ||
+        (e = cudaStreamSynchronize(c->stream)) != cudaSuccess) {
         g_create_error = std::string("gp_create: ") + cudaGetErrorString(e);
         delete c;
         return GP_ERR_CUDA;
@@ -701,28 +777,30 @@ static gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_
     GP_CUDA(c, c->node_slot.reserve(sizeof(int32_t) * (size_t)(dn->n_nodes + 1)));
     GP_CUDA(c, c->drv_slot.reserve(sizeof(int32_t) * (size_t)(n_drv + 1)));
     GP_CUDA(c, c->groups.reserve(sizeof(GroupDesc) * (size_t)dn->n_groups));
+    GP_CUDA(c, c->drv_pos.reserve(sizeof(int32_t) * (size_t)(dn->n_nodes + 1)));
     int64_t* node_cpu = copy_nodes ? c->node_cpu.as<int64_t>() : nullptr;
-    struct { gp_nodes dn; int32_t n_exec, n_drv; void* buf[11]; } key{};
+    const int T = kSnapThreads;
+    const int32_t n1 = std::max(std::max(std::max(n_exec, n_drv), dn->n_groups), node_cpu ? dn->n_nodes : 0);
+    const int32_t blocks1 = (n1 + T - 1) / T;
+    GP_CUDA(c, c->snap_part.reserve(sizeof(SnapPart) * (size_t)blocks1));
+    SnapPart* parts = c->snap_part.as<SnapPart>();
+    struct { gp_nodes dn; int32_t n_exec, n_drv; void* buf[13]; } key{};
     key.dn = *dn; key.n_exec = n_exec; key.n_drv = n_drv;
-    void* bufs[11] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p,
-                      node_cpu, c->node_mem.p, c->node_gpu.p};
+    void* bufs[13] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p,
+                      node_cpu, c->node_mem.p, c->node_gpu.p, c->drv_pos.p, c->snap_part.p};
     std::memcpy(key.buf, bufs, sizeof(bufs));
     gp_status rs = run_cached(c, c->g_snapshot, &key, sizeof(key), st, [&](int& launches) -> gp_status {
-        // node_slot must be -1 for every node outside the orders (K2 reads it for the driver-order nodes); every slot_node
-        // entry is written by K1 or K2
-        GP_CUDA(c, cudaMemsetAsync(c->node_slot.p, 0xFF, sizeof(int32_t) * (size_t)(dn->n_nodes + 1), st));
-        GP_CUDA(c, cudaMemsetAsync(c->snap_flags.p, 0, sizeof(SnapMeta), st));
-        const int T = 256;
-        const int32_t n1 = std::max(std::max(std::max(n_exec, n_drv), dn->n_groups), node_cpu ? dn->n_nodes : 0);
-        gp_build_slots_exec<<<(n1 + T - 1) / T, T, 0, st>>>(
+        gp_build_slots_exec<<<blocks1, T, 0, st>>>(
             n_exec, n_drv, dn->n_groups, dn->n_nodes, dn->exec_off, dn->drv_off, dn->exec_order, dn->drv_order, dn->avail_cpu_milli,
             dn->avail_mem_bytes, dn->avail_gpu, c->groups.as<GroupDesc>(), c->pair.as<longlong2>(), c->sgpu.as<int64_t>(),
-            c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>(), node_cpu, c->node_mem.as<int64_t>(),
-            c->node_gpu.as<int64_t>());
-        gp_build_slots_drv<<<(n_slots + T) / T, T, 0, st>>>(
-            n_slots, dn->n_groups, dn->exec_off, dn->drv_off, dn->drv_order, dn->avail_cpu_milli, dn->avail_mem_bytes,
-            dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(), c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(),
-            c->drv_slot.as<int32_t>(), c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
+            c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->drv_pos.as<int32_t>(), parts, node_cpu,
+            c->node_mem.as<int64_t>(), c->node_gpu.as<int64_t>());
+        // threads [0, n_slots]: slots; [n_slots + 1, n_slots + 1 + n_nodes]: nodes
+        gp_build_slots_drv<<<(n_slots + dn->n_nodes + 1 + T) / T, T, 0, st>>>(
+            n_slots, dn->n_groups, dn->n_nodes, n_drv, dn->exec_off, dn->drv_off, dn->drv_order, c->drv_pos.as<int32_t>(),
+            dn->avail_cpu_milli, dn->avail_mem_bytes, dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(),
+            c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->drv_slot.as<int32_t>(), parts, blocks1,
+            c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
         GP_CUDA(c, cudaGetLastError());
         launches = 0;       // (the snapshot layout is not part of a pack call's launch count)
         return GP_OK;
@@ -952,7 +1030,7 @@ template <int ALGO, class OUT>
 static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs, int64_t off_base,
                                int64_t* off_out, int32_t* app_slot, PrepApp* prep, int32_t* listed, int32_t q, const DevResults& dr,
                                int32_t lo, int2* scratch, unsigned long long* stats, unsigned int* next_app, int* d_err,
-                               volatile int* err_host, bool use_tables, int64_t seg_bound, cudaStream_t st) {
+                               volatile int* err_host, bool use_tables, int64_t seg_bound, unsigned int* status_zero, cudaStream_t st) {
     int& dec_per_sm = c->dec_ctas_per_sm[ALGO][sizeof(OUT) == 2 ? 1 : 0];
     if (dec_per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&dec_per_sm, gp_decide_tables<ALGO, OUT>, kTabThreads, 0);
@@ -965,7 +1043,7 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
     blocks = std::min<int64_t>(blocks, (int64_t)c->sm_count * dec_per_sm);
     gp_decide_tables<ALGO, OUT><<<(int)blocks, kTabThreads, 0, st>>>(s, cols, tabs, off_base, off_out, app_slot, q, dr.cap, dr.driver + lo,
                                                                     static_cast<OUT*>(dr.exec), prep, listed, stats, d_err, err_host,
-                                                                    use_tables ? 0 : 1);
+                                                                    use_tables ? 0 : 1, status_zero);
     int& per_sm = c->tab_ctas_per_sm[ALGO][sizeof(OUT) == 2 ? 1 : 0];
     if (per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_listed<ALGO, OUT>, kPackTabThreads, 0);
@@ -976,7 +1054,9 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
     const int64_t max_blocks = (int64_t)c->sm_count * (use_tables ? 2 : per_sm);
     if (blocks > max_blocks) blocks = max_blocks;
     if (blocks < 1) blocks = 1;
-    gp_pack_listed<ALGO, OUT><<<(int)blocks, kPackTabThreads, 0, st>>>(s, tabs.hdr, prep, listed, dr.driver + lo, static_cast<OUT*>(dr.exec), scratch,
+    // it also zeroes the classify tiles' and the table segments' look-back words (see there)
+    gp_pack_listed<ALGO, OUT><<<(int)blocks, kPackTabThreads, 0, st>>>(s, tabs, (int32_t)tiles, use_tables ? kMaxShapes * (int32_t)seg_bound : 0,
+                                                                      prep, listed, dr.driver + lo, static_cast<OUT*>(dr.exec), scratch,
                                                                       stats, next_app);
     c->last.kernel_launches += 2;
     return GP_OK;
@@ -984,8 +1064,9 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
 
 // Device-resident apps [lo, hi): enqueue the kernels on `st`; chunk index selects the timing events and the table lane.
 // off_base: ExecutorNodes offset of application `lo` (only used when the offsets are derived on the device).
+// status_in_kernel: pack_begin left the status block to this range's decide kernel (kernel_zeroes_status(), one range only).
 static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi, int64_t off_base, gp_algo algo, gp_mode mode,
-                                   const DevResults& dr, int2* scratch, cudaStream_t st, int chunk) {
+                                   const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel = false) {
     const int32_t q = hi - lo;
     if (q <= 0) return GP_OK;
     int* d_err = &c->status()->head.err;
@@ -1003,16 +1084,16 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
             off_out = c->off_dev.as<int64_t>() + lo;
             cols.off = off_out;
         }
-        // [header | look-back words of the classify tiles | executor hash | driver hash | look-back words of the table
-        // segments]: the memset that starts the call zeroes what the call uses of it (the header always: ticket, counters)
+        // [header | executor hash | driver hash | look-back words of the classify tiles | look-back words of the table
+        // segments]: zeroed when allocated, and gp_pack_listed zeroes what each call used of it.  The hash entries sit at
+        // the same place whatever q is, so the words a later call expects zero never overlap the fields a claimer wrote.
         const size_t n_tiles = ((size_t)q + kTabThreads - 1) / kTabThreads;
         const size_t cls_bytes = (sizeof(unsigned long long) * n_tiles + 15) & ~(size_t)15;
         const size_t hash_bytes = (sizeof(ShapeEntry) + sizeof(DriverEntry)) * (size_t)kShapeSlots;
         // sum over the groups of max(1, ceil(ne / kTabSeg)) <= n_slots / kTabSeg + n_groups
         const int64_t seg_bound = (int64_t)c->n_slots / kTabSeg + c->n_groups + 1;
-        const size_t hdr_bytes = 1024 + cls_bytes + hash_bytes + sizeof(unsigned long long) * (size_t)kMaxShapes * (size_t)seg_bound;
-        const size_t zero_bytes = use_tables ? hdr_bytes : off_out ? 1024 + cls_bytes : 1024;
-        GP_CUDA(c, T.hdr.reserve(hdr_bytes));
+        const size_t hdr_bytes = 1024 + hash_bytes + cls_bytes + sizeof(unsigned long long) * (size_t)kMaxShapes * (size_t)seg_bound;
+        GP_CUDA(c, T.hdr.reserve_zeroed(hdr_bytes, st));
         // [executor slot | driver slot | listed]
         GP_CUDA(c, T.app_slot.reserve(sizeof(int32_t) * (3 * (size_t)q + 1)));
         if (use_tables) {
@@ -1023,10 +1104,10 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         }
         ShapeTables tabs;
         tabs.hdr = T.hdr.as<ShapeHeader>();
-        tabs.cls_status = reinterpret_cast<unsigned long long*>(T.hdr.as<char>() + 1024);
-        tabs.entries = reinterpret_cast<ShapeEntry*>(T.hdr.as<char>() + 1024 + cls_bytes);
-        tabs.dentries = reinterpret_cast<DriverEntry*>(T.hdr.as<char>() + 1024 + cls_bytes + sizeof(ShapeEntry) * (size_t)kShapeSlots);
-        tabs.seg_status = reinterpret_cast<unsigned long long*>(T.hdr.as<char>() + 1024 + cls_bytes + hash_bytes);
+        tabs.entries = reinterpret_cast<ShapeEntry*>(T.hdr.as<char>() + 1024);
+        tabs.dentries = reinterpret_cast<DriverEntry*>(T.hdr.as<char>() + 1024 + sizeof(ShapeEntry) * (size_t)kShapeSlots);
+        tabs.cls_status = reinterpret_cast<unsigned long long*>(T.hdr.as<char>() + 1024 + hash_bytes);
+        tabs.seg_status = reinterpret_cast<unsigned long long*>(T.hdr.as<char>() + 1024 + hash_bytes + cls_bytes);
         tabs.table = T.table.as<uint32_t>(); tabs.total = T.total.as<uint32_t>();
         tabs.firstfit = reinterpret_cast<int32_t*>(T.total.as<uint32_t>() + (size_t)kMaxShapes * (size_t)c->n_groups);
         tabs.first_host = tabs.firstfit + (size_t)kMaxShapes * (size_t)c->n_groups;
@@ -1039,13 +1120,13 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         const bool o16 = dr.node_bits == 16;
         const auto launch = algo == GP_TIGHTLY_PACK ? (o16 ? launch_tables<0, uint16_t> : launch_tables<0, int32_t>)
                                                     : (o16 ? launch_tables<1, uint16_t> : launch_tables<1, int32_t>);
+        unsigned int* status_zero = status_in_kernel ? reinterpret_cast<unsigned int*>(c->status()) : nullptr;
+        c->ev_prep = false;                            // one launch prepares and packs: no separate prep interval
         auto issue = [&](int& launches) -> gp_status {
             const int before = (int)c->last.kernel_launches;
-            if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][0], st));
-            GP_CUDA(c, cudaMemsetAsync(T.hdr.p, 0, zero_bytes, st));
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][1], st));
             const gp_status r = launch(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app,
-                                       d_err, err_host, use_tables, seg_bound, st);
+                                       d_err, err_host, use_tables, seg_bound, status_zero, st);
             if (r != GP_OK) return r;
             GP_CUDA(c, cudaGetLastError());
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][2], st));
@@ -1060,10 +1141,10 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
             return r;
         }
         struct { int32_t algo, o16, use_tables, q, lo, chunk; int64_t off_base; AppColumns cols; ShapeTables tabs; Snapshot snap;
-                 const void* p[10]; int64_t cap; } key{};
+                 const void* p[11]; int64_t cap; } key{};
         key.algo = (int32_t)algo; key.o16 = o16; key.use_tables = use_tables; key.q = q; key.lo = lo; key.chunk = chunk; key.off_base = off_base;
         key.cols = cols; key.tabs = tabs; key.snap = s; key.cap = dr.cap;
-        const void* ptrs[10] = {app_slot, prep, listed, dr.driver, dr.exec, scratch, d_stats, next_app, d_err, off_out};
+        const void* ptrs[11] = {app_slot, prep, listed, dr.driver, dr.exec, scratch, d_stats, next_app, d_err, off_out, status_zero};
         std::memcpy(key.p, ptrs, sizeof(ptrs));
         return run_cached(c, c->g_chunk[st == c->stream ? kMaxChunks : chunk], &key, sizeof(key), st, issue);
     }
@@ -1076,6 +1157,7 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
         GP_CUDA(c, c->gmin.reserve(sizeof(GroupMin) * (size_t)c->n_groups));
         GP_CUDA(c, cudaMemsetAsync(c->gmin.p, 0x7f, sizeof(GroupMin) * (size_t)c->n_groups, st));   // +inf-ish
     }
+    c->ev_prep = true;
     if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][0], st));
     gp_prep_apps<<<(q + T - 1) / T, T, 0, st>>>(
         q, cols, da.skip ? da.skip + lo : nullptr, c->n_groups, dr.cap,
@@ -1098,9 +1180,15 @@ static gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int
 
 static bool fused_path(gp_algo algo, gp_mode mode) { return mode == GP_MODE_INDEPENDENT && algo != GP_MINIMAL_FRAGMENTATION; }
 
+// One range of q > 0 independent tightly-pack / distribute-evenly applications on one stream: the first classify tile of
+// its decide kernel zeroes the status block (gp_decide_tables), so pack_begin leaves out its memset.  Calls that pack
+// several ranges or take other kernels keep the memset.
+static bool kernel_zeroes_status(int32_t q, gp_algo algo, gp_mode mode) { return q > 0 && fused_path(algo, mode); }
+
 // common prologue: buffers, counters
-static gp_status pack_begin(gp_ctx* c, int32_t q, gp_algo algo, gp_mode mode, int64_t exec_cap, bool derive_off, int2** scratch, cudaStream_t st) {
-    GP_CUDA(c, cudaMemsetAsync(c->status(), 0, sizeof(DevStatus), st));
+static gp_status pack_begin(gp_ctx* c, int32_t q, gp_algo algo, gp_mode mode, int64_t exec_cap, bool derive_off, int2** scratch, cudaStream_t st,
+                            bool status_in_kernel = false) {
+    if (!status_in_kernel) GP_CUDA(c, cudaMemsetAsync(c->status(), 0, sizeof(DevStatus), st));
     c->host_status()->err_word = 0;
     c->last = gp_stats{};
     c->ev_chunks = 0;
@@ -1142,7 +1230,7 @@ static void fill_kernel_times(gp_ctx* c) {
     c->last.prep_kernel_ns = 0; c->last.pack_kernel_ns = 0;
     for (int i = 0; i < c->ev_chunks; ++i) {
         float a = 0.f, b = 0.f;
-        if (cudaEventElapsedTime(&a, c->ev[i][0], c->ev[i][1]) == cudaSuccess) c->last.prep_kernel_ns += (int64_t)(a * 1.0e6);
+        if (c->ev_prep && cudaEventElapsedTime(&a, c->ev[i][0], c->ev[i][1]) == cudaSuccess) c->last.prep_kernel_ns += (int64_t)(a * 1.0e6);
         if (cudaEventElapsedTime(&b, c->ev[i][1], c->ev[i][2]) == cudaSuccess) c->last.pack_kernel_ns += (int64_t)(b * 1.0e6);
     }
 }
@@ -1179,7 +1267,8 @@ gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mo
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : c->stream;
     int2* scratch = nullptr;
-    s = pack_begin(c, w.n_apps, algo, mode, ow.executor_nodes_cap, !w.exec_out_off, &scratch, st);
+    const bool zero_in_kernel = kernel_zeroes_status(w.n_apps, algo, mode);
+    s = pack_begin(c, w.n_apps, algo, mode, ow.executor_nodes_cap, !w.exec_out_off, &scratch, st, zero_in_kernel);
     if (s != GP_OK || w.n_apps == 0) return s;
     DevApps dv{};
     dv.cols.q[0] = w.drv_cpu; dv.cols.q[1] = w.drv_mem; dv.cols.q[2] = w.drv_gpu;
@@ -1187,7 +1276,7 @@ gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mo
     dv.cols.count = w.exe_count; dv.cols.group = w.group; dv.cols.off = w.exec_out_off; dv.cols.bits = 64; dv.cols.mem_shift = 0;
     dv.skip = w.skip_if_no_fit; dv.n = w.n_apps;
     DevResults dr{ow.driver_node, ow.executor_nodes, ow.executor_nodes_cap, 32};
-    s = pack_device_range(c, dv, 0, w.n_apps, 0, algo, mode, dr, scratch, st, 0);
+    s = pack_device_range(c, dv, 0, w.n_apps, 0, algo, mode, dr, scratch, st, 0, zero_in_kernel);
     if (s == GP_OK) c->ev_chunks = 1;
     return s;
 }

@@ -67,7 +67,9 @@ struct __align__(16) DriverEntry {    // 48 bytes: interned driver request
 };
 static_assert(sizeof(DriverEntry) == 48, "DriverEntry layout");
 
-// device-side header of one table set
+// device-side header of one table set.  The counters, the hash keys and the look-back words are zero when a call starts:
+// the buffer is zeroed when it is allocated, and gp_pack_listed, the last kernel of every call, zeroes what the call used
+// (n_listed excepted: gp_pack_listed reads it, and the first classify tile of the next call zeroes it).
 struct ShapeHeader {
     int32_t n_shapes;                 // executor shapes claimed so far (may exceed kMaxShapes)
     int32_t n_dshapes;                // driver shapes claimed so far
@@ -86,8 +88,8 @@ struct ShapeTables {
     ShapeEntry* entries;              // [kShapeSlots]
     DriverEntry* dentries;            // [kShapeSlots]
     ShapeHeader* hdr;
-    unsigned long long* cls_status;   // [classify tiles] look-back words of the derived offsets (zeroed with the header)
-    unsigned long long* seg_status;   // [kMaxShapes * segments] look-back words of the table segments (zeroed with the header)
+    unsigned long long* cls_status;   // [classify tiles] look-back words of the derived offsets (zero at the start of a call)
+    unsigned long long* seg_status;   // [kMaxShapes * segments] look-back words of the table segments (zero at the start of a call)
     int32_t* seg_pre;                 // [n_groups + 1] table segments before each group (written by classify tile 0)
     uint32_t* table;                  // [kMaxShapes][pitch] exclusive prefix per instance group, indexed by slot
     uint32_t* total;                  // [kMaxShapes][n_groups]
@@ -702,18 +704,25 @@ __device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const A
 // (look-back), the decide phase for every table item (hdr->tab_done).  A ticket is claimed by a CTA that is running, and a
 // CTA claims its next ticket only after finishing the last one.  So by induction over the tickets, every claimed item
 // completes, whatever number of CTAs happens to be co-resident (other work on the GPU, the other pipeline lanes).
-// The ticket, the phase counters and every look-back word start from zero by the memset of the table header.
+// The ticket, the phase counters and every look-back word start from zero: the previous call's gp_pack_listed left them so.
+// The item with ticket 0 is always a classify tile (one tile with nothing to classify when neither the tables nor the
+// offsets are needed).  It zeroes hdr->n_listed and, with status_zero != NULL, the call's status block (kStatusWords
+// words: error bits, statistics, claim counters) instead of a memset before the launch.  It finishes before cls_done can
+// count every tile, and every CTA waits for that count before it appends to the list, writes the error word or adds to
+// the statistics, so no write of the call is lost to the zeroing.
+constexpr int kStatusWords = 32;
 template <int ALGO, class OUT>
 __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppColumns cols, ShapeTables tabs, int64_t off_base,
                                                                 int64_t* off_out /* or NULL */, int32_t* app_slot, int32_t n_apps,
                                                                 int64_t out_cap, int32_t* __restrict__ driver_node,
                                                                 OUT* __restrict__ executor_nodes, PrepApp* __restrict__ prep,
                                                                 int32_t* __restrict__ listed, unsigned long long* __restrict__ stats,
-                                                                int* __restrict__ err, volatile int* __restrict__ err_host, int force_scan) {
+                                                                int* __restrict__ err, volatile int* __restrict__ err_host, int force_scan,
+                                                                unsigned int* __restrict__ status_zero) {
     __shared__ OneScratch sh;
     ShapeHeader* hdr = tabs.hdr;
     const int32_t n_tiles = (n_apps + kTabThreads - 1) / kTabThreads;
-    const int32_t n_cls = (!force_scan || off_out) ? n_tiles : 0;
+    const int32_t n_cls = (!force_scan || off_out) ? n_tiles : 1;
     int32_t n_es = 0, n_tab = -1, total_segs = 0;         // n_tab < 0: classify not yet seen complete by this CTA
     unsigned long long probes = 0, drivers = 0;
     for (;;) {
@@ -721,6 +730,10 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
         __syncthreads();
         const int32_t t = (int32_t)sh.ticket;
         if (t < n_cls) {
+            if (t == 0) {
+                if (threadIdx.x == 0) hdr->n_listed = 0;
+                if (status_zero && threadIdx.x < kStatusWords) status_zero[threadIdx.x] = 0u;
+            }
             if (off_out) classify_offsets(sh, t, n_apps, cols, tabs, off_base, off_out);
             if (!force_scan) {
                 gp_classify_apps(t, n_apps, cols, tabs, s.meta, app_slot);
@@ -784,8 +797,13 @@ constexpr int kPackTabThreads = 256;
 #ifndef GP_TAB_MIN_BLOCKS
 #define GP_TAB_MIN_BLOCKS 4
 #endif
+// It is the last kernel of every call on its table set, so it also leaves the set clean for the next call: its CTAs zero
+// the counters, the hash keys and the n_cls_words / n_seg_words look-back words the call used (a claimer writes every
+// other field of a hash entry).  gp_decide_tables, which uses all of these, has finished: the two launches are
+// stream-ordered.  No CTA sizes its share from a header word, and n_listed, which they read, is left to the next call.
 template <int ALGO, class OUT>
-__global__ void __launch_bounds__(kPackTabThreads, GP_TAB_MIN_BLOCKS) gp_pack_listed(Snapshot s, const ShapeHeader* __restrict__ hdr,
+__global__ void __launch_bounds__(kPackTabThreads, GP_TAB_MIN_BLOCKS) gp_pack_listed(Snapshot s, ShapeTables tabs, int32_t n_cls_words,
+                                                                                     int32_t n_seg_words,
                                                                                      const PrepApp* __restrict__ prep,
                                                                                      const int32_t* __restrict__ listed,
                                                                                      int32_t* __restrict__ driver_node,
@@ -794,34 +812,46 @@ __global__ void __launch_bounds__(kPackTabThreads, GP_TAB_MIN_BLOCKS) gp_pack_li
                                                                                      unsigned long long* __restrict__ stats,
                                                                                      unsigned int* __restrict__ next_app) {
     __shared__ uint16_t cap_cache[kPackTabThreads / 32][kCapCache];
+    ShapeHeader* hdr = tabs.hdr;
     const int n = hdr->n_listed;
-    if (n == 0) return;
-    const int lane = threadIdx.x & 31;
-    uint16_t* wcache = cap_cache[threadIdx.x >> 5];
-    WarpStats st{0, 0};
-    const int snap_flags = s.meta->flags;
-    const GroupDesc g0 = s.groups[0];
-    unsigned int i = 0, n1 = 0;
-    if (lane == 0) { i = atomicAdd(next_app, 1u); n1 = atomicAdd(next_app, 1u); }
-    i = __shfl_sync(kFull, i, 0);
-    n1 = __shfl_sync(kFull, n1, 0);
-    unsigned long long apps_done = 0;
-    while (i < (unsigned int)n) {
-        unsigned int n2 = 0;
-        if (lane == 0) n2 = atomicAdd(next_app, 1u);
-        if (lane == 0 && n1 < (unsigned int)n) asm volatile("prefetch.global.L1 [%0];" ::"l"(prep + n1));
-        const PrepApp* pa = prep + i;
-        const int32_t d = pack_app<ALGO, OUT>(s, pa, executor_nodes, scratch, wcache, st, lane, snap_flags, g0);
-        if (lane == 0) driver_node[listed[i]] = d;
-        ++apps_done;
-        i = n1;
-        n1 = __shfl_sync(kFull, n2, 0);
+    {
+        const int32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
+        if (tid == 0) {
+            hdr->n_shapes = 0; hdr->n_dshapes = 0;
+            hdr->ticket = 0; hdr->cls_done = 0; hdr->tab_done = 0; hdr->dec_next = 0;
+        }
+        for (int32_t k = tid; k < kShapeSlots; k += nth) { tabs.entries[k].key = 0ull; tabs.dentries[k].key = 0ull; }
+        for (int32_t k = tid; k < n_cls_words; k += nth) tabs.cls_status[k] = 0ull;
+        for (int32_t k = tid; k < n_seg_words; k += nth) tabs.seg_status[k] = 0ull;
     }
-    if (lane == 0) {
-        atomicAdd(stats + 0, st.nodes);
-        atomicAdd(stats + 1, st.drivers);
-        atomicAdd(stats + 2, apps_done);
-        atomicAdd(stats + 3, st.nodes);
+    if (n != 0) {
+        const int lane = threadIdx.x & 31;
+        uint16_t* wcache = cap_cache[threadIdx.x >> 5];
+        WarpStats st{0, 0};
+        const int snap_flags = s.meta->flags;
+        const GroupDesc g0 = s.groups[0];
+        unsigned int i = 0, n1 = 0;
+        if (lane == 0) { i = atomicAdd(next_app, 1u); n1 = atomicAdd(next_app, 1u); }
+        i = __shfl_sync(kFull, i, 0);
+        n1 = __shfl_sync(kFull, n1, 0);
+        unsigned long long apps_done = 0;
+        while (i < (unsigned int)n) {
+            unsigned int n2 = 0;
+            if (lane == 0) n2 = atomicAdd(next_app, 1u);
+            if (lane == 0 && n1 < (unsigned int)n) asm volatile("prefetch.global.L1 [%0];" ::"l"(prep + n1));
+            const PrepApp* pa = prep + i;
+            const int32_t d = pack_app<ALGO, OUT>(s, pa, executor_nodes, scratch, wcache, st, lane, snap_flags, g0);
+            if (lane == 0) driver_node[listed[i]] = d;
+            ++apps_done;
+            i = n1;
+            n1 = __shfl_sync(kFull, n2, 0);
+        }
+        if (lane == 0) {
+            atomicAdd(stats + 0, st.nodes);
+            atomicAdd(stats + 1, st.drivers);
+            atomicAdd(stats + 2, apps_done);
+            atomicAdd(stats + 3, st.nodes);
+        }
     }
 }
 
