@@ -575,6 +575,87 @@ typedef struct {
 gp_status gp_exceeds_cluster_capacity(gp_ctx* ctx, const gp_capacity_nodes* nodes, const gp_apps* drivers, gp_binpacker packer,
                                       uint8_t* exceeds /* [n_apps] */);
 
+/* ---- required node affinity (K8S = vendor/k8s.io) ------------------------------------------------------------------------
+ * GetRequiredNodeAffinity(pod).Match(node) (K8S/component-helpers/scheduling/corev1/nodeaffinity/nodeaffinity.go:297-324) for
+ * every (distinct affinity, node), as utils.ListWithPredicate runs it in selectDriverNode (EXT/resource.go:292-298) and in
+ * DoesPodExceedClusterCapacity (EXT/unschedulablepods.go:133-139).  Outcome per node: match, no match or error:
+ *   1. nodeSelector: every (key, value) must be a label of the node, else no match (even when the terms would have errored);
+ *   2. no requiredDuringScheduling...: match;
+ *   3. terms in order (nodeaffinity.go:56-103, 152-201): a term with a parse error records an error and is skipped, a term
+ *      without requirements is skipped, a term matches when all its label and field requirements match; the first match wins;
+ *   4. no term matched: no match, an error when a term recorded one.  A required affinity whose terms are all empty matches
+ *      no node.
+ * Label requirements (K8S/apimachinery/pkg/labels/selector.go:218-262): In = key present and value in the set; NotIn = key
+ * absent or value not in the set; Exists / DoesNotExist = presence; Gt / Lt = key present, its value parses
+ * (strconv.ParseInt(v, 10, 64)) and is strictly greater / less than the bound -- a value that does not parse is no match.
+ * Field requirements: metadata.name In / NotIn one value, given as a node index (-1: no node has that name).  A field key other
+ * than metadata.name reads "" (extractNodeFields sets no other field): the caller encodes In "" / NotIn v != "" as NotIn -1
+ * (always true) and In v != "" / NotIn "" as In -1 (never true).
+ * Strings never cross the boundary: the caller interns label keys and values to dense ids, and does what needs the strings --
+ * NewRequirement's validation (an operator that is not one of the six, a key that is not a qualified name, a value that is not
+ * a label value, In / NotIn without values, Exists / DoesNotExist with values, Gt / Lt without exactly one integer value;
+ * matchFields other than In / NotIn with exactly one value) becomes the term's parse_error flag, ParseInt of a node's label value
+ * becomes label_int_ok / label_int, metadata.name becomes a node index. */
+typedef enum {
+    GP_AFF_IN = 0, GP_AFF_NOT_IN = 1, GP_AFF_EXISTS = 2, GP_AFF_DOES_NOT_EXIST = 3, GP_AFF_GT = 4, GP_AFF_LT = 5,
+    GP_AFF_FIELD_NAME_IN = 6, GP_AFF_FIELD_NAME_NOT_IN = 7
+} gp_aff_op;
+typedef struct {
+    int32_t n_nodes;
+    int32_t n_keys;                      /* label key ids 0..n_keys-1 */
+    int32_t n_values;                    /* label value ids 0..n_values-1 */
+    int32_t reserved;
+    const int64_t* label_off;            /* [n_nodes+1] CSR: node i's labels are [label_off[i], label_off[i+1]); label_off[0] = 0 */
+    const int32_t* label_key;            /* strictly ascending within a node (node.Labels is a map) */
+    const int32_t* label_val;
+    const uint8_t* label_int_ok;         /* ParseInt(value, 10, 64) succeeded; or NULL (no value parses) */
+    const int64_t* label_int;            /* its result where label_int_ok; or NULL with label_int_ok */
+} gp_node_labels;
+typedef struct {
+    int32_t n_aff;                       /* distinct required affinities (nodeSelector + requiredDuringScheduling...) */
+    int32_t reserved;
+    const int64_t* sel_off;              /* [n_aff+1] nodeSelector of affinity a: [sel_off[a], sel_off[a+1]) */
+    const int32_t* sel_key;              /*   key id = value id, each */
+    const int32_t* sel_val;
+    const uint8_t* has_required;         /* [n_aff] requiredDuringScheduling... is not nil */
+    const int64_t* term_off;             /* [n_aff+1] affinity a's terms, in order: [term_off[a], term_off[a+1]) */
+    const int64_t* term_req_off;         /* [n_terms+1] term t's requirements: [term_req_off[t], term_req_off[t+1]) */
+    const uint8_t* term_parse_error;     /* [n_terms] or NULL (none) */
+    const int32_t* req_op;               /* [n_req] gp_aff_op */
+    const int32_t* req_key;              /* [n_req] label key id (ignored by the field operators) */
+    const int64_t* req_int;              /* [n_req] GT / LT: the bound; FIELD_NAME_*: node index or -1; else ignored */
+    const int64_t* req_val_off;          /* [n_req+1] IN / NOT_IN value set: [req_val_off[r], req_val_off[r+1]) */
+    const int32_t* req_val;              /*   value ids, strictly ascending within a requirement */
+} gp_node_affinities;
+typedef struct {
+    uint32_t* member;                    /* [n_aff][(n_nodes+31)/32]: bit j%32 of word j/32 = node j matches; or NULL */
+    int32_t* n_match;                    /* [n_aff] nodes that match; or NULL */
+    int32_t* n_error;                    /* [n_aff] nodes whose outcome is an error (ListWithPredicate returns it: the
+                                            Predicate fails with failureInternal); or NULL */
+} gp_affinity_match;
+/* The match of every affinity against every node, in one call.  An error node is not a member.
+ * The context is left alone (snapshot, SchedulableResources, zone layout, held az-aware orders, gp_last_stats); scratch of its
+ * own, one stream synchronise.  GP_ERR_INVALID (gp_last_error names the cause): missing arrays or negative sizes; offsets
+ * that do not start at 0 or decrease; a label key or value id out of range; the keys of a node not strictly ascending; an
+ * operator out of range; a selector or requirement key or value id out of range; a value set not strictly ascending; a field
+ * node index outside [-1, n_nodes).  On an error the outputs are undefined. */
+gp_status gp_match_node_affinity(gp_ctx* ctx, const gp_node_labels* labels, const gp_node_affinities* affinities,
+                                 gp_affinity_match* out);
+
+/* gp_exceeds_cluster_capacity with each driver's node set = the nodes its required affinity matches, evaluated in the same
+ * call: any subsets of the nodes, overlapping freely (DoesPodExceedClusterCapacity, EXT/unschedulablepods.go:132-166).
+ *   nodes       as for gp_exceeds_cluster_capacity, with node_group NULL and n_groups ignored; labels->n_nodes = nodes->n_nodes.
+ *   drivers     group = the driver's affinity id, 0..n_aff-1 (required); exe_count any int32 >= 0.
+ *   exceeds[i]  = !HasCapacity over driver i's matched nodes: the T + M criterion (DESIGN §2.2), per zone for the single-AZ
+ *               packers; an empty match gives 1.
+ *   affinity_error[i] = 1 when driver i's affinity gives an error on some node (ListWithPredicate fails: the marker's scan
+ *               returns at that driver, unschedulablepods.go:113-117); exceeds[i] is then undefined.  May be NULL.
+ * The scratch is bounded whatever the total membership: the affinities are processed in chunks. Context left alone, one
+ * stream synchronise.  Refusals: those of both calls, and node_group not NULL, a driver group outside [0, n_aff). */
+gp_status gp_exceeds_cluster_capacity_affinity(gp_ctx* ctx, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
+                                               const gp_node_affinities* affinities, const gp_apps* drivers, gp_binpacker packer,
+                                               uint8_t* exceeds /* [n_apps] */, uint8_t* affinity_error /* [n_apps] or NULL */);
+
 /* ---- the failover reconciler's node choice (EXT/failover.go:43-82, 286-436) ------------------------------------------------
  * syncResourceReservationsAndDemands minus pod, lister and CRD I/O: availableResourcesPerInstanceGroup (:286-323), then for each
  * stale driver in call order constructResourceReservation's findNodes (:348-390, 409-436) and the charge of :159, in one call.

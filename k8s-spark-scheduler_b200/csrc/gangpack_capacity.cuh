@@ -13,16 +13,27 @@
 // alike; az-aware-tightly-pack is that over the whole set; the two single-AZ packers need it in one zone and a positive
 // average packing efficiency, which under zero usage depends on the requests alone.
 //
+// A driver's node set is a class.  Two layouts of the classes:
+//   gp_exceeds_cluster_capacity           one class per node (node_group) plus the class of every node, for class -1 drivers:
+//                                         entry k = 0 of node i is its class, k = 1 the all-nodes class (slot G);
+//   gp_exceeds_cluster_capacity_affinity  class a = the nodes affinity a matches (gangpack_affinity.cuh), any subsets of the
+//                                         nodes, overlapping freely: entry k of node i is affinity a0 + k when it matches.
+// The entries of one chunk of classes are (k, node) for k < K; K x n_nodes stays below kCapEntries, so the scratch is bounded
+// whatever the number of memberships: more affinities take more chunks, never a refusal.  The pair results are kept across
+// chunks; each chunk resets and fills only the pairs of its own classes.
+//
 // Kernels (one stream, no host round trip between them):
-//   gp_cc_nodes        thread per node: validate, schedulable = alloc - overhead, buckets (class, zone) and (all, zone)
-//   gp_cc_bucket_scan  one CTA: node, segment and multi-segment offsets of the buckets
-//   gp_cc_scatter      thread per node: nodes grouped by bucket; the first node of every segment writes the segment
+//   gp_cc_nodes        thread per node: validate, schedulable = alloc - overhead, zone
 //   gp_cc_intern       thread per driver: validate, intern (class, executor shape, driver shape) -> dense pair id
-//   gp_cc_pair_scan    one CTA: prefix over the pairs of the number of segments each one visits; per-pair results reset
-//   per chunk of pairs (one chunk unless pairs x multi-segment buckets exceed kCapSlotEntries):
-//     gp_cc_clear      zero the chunk's (pair, multi-segment bucket) slots
-//     gp_cc_pass       CTA per (pair, segment): T and M of the segment, warp -> CTA -> global atomics on the pair; a zone's
-//                      T_z + M_z is complete in the CTA that holds its only segment, or in the last of its segments to arrive
+//   per chunk of classes [a0, a0 + K):
+//     gp_cc_keys         thread per entry: its bucket (class k, zone), -1 = the node is not in class k
+//     gp_cc_bucket_scan  one CTA: node, segment and multi-segment offsets of the buckets
+//     gp_cc_scatter      thread per entry: nodes grouped by bucket; the first node of every segment writes the segment
+//     gp_cc_pair_scan    one CTA: prefix over the pairs of the number of segments each one visits; the chunk's pairs reset
+//     per chunk of pairs (one chunk unless pairs x multi-segment buckets exceed kCapSlotEntries):
+//       gp_cc_clear      zero the chunk's (pair, multi-segment bucket) slots
+//       gp_cc_pass       CTA per (pair, segment): T and M of the segment, warp -> CTA -> global atomics on the pair; a zone's
+//                        T_z + M_z is complete in the CTA that holds its only segment, or in the last of its segments to arrive
 //   gp_cc_decide       thread per driver: O(1)
 #pragma once
 
@@ -39,9 +50,11 @@ constexpr int32_t kCapSeg = 16 * kCapThreads;         // nodes of one bucket per
 constexpr uint32_t kCapClamp = 1u << 31;               // C: above every int32 exe_count
 constexpr long long kCapNone = -0x7fffffffffffffffLL - 1;         // INT64_MIN: "no driver fits"
 // Scratch bound: a bucket of more than kCapSeg nodes is split over several CTAs, which combine its (T_z, M_z) in a slot per
-// (pair, such bucket).  There are at most 2 n_nodes / (kCapSeg + 1) such buckets, whatever the number of zones; a chunk of
+// (pair, such bucket).  There are at most K n_nodes / (kCapSeg + 1) such buckets in a chunk of K classes, whatever the number of zones; a chunk of
 // pairs owns at most kCapSlotEntries slots (24 bytes each, 48 MiB in all), more pairs take more chunks, never a refusal.
 constexpr int64_t kCapSlotEntries = (int64_t)1 << 21;
+// Entries of one chunk of affinity classes (K x n_nodes, 32 bytes each: 64 MiB); one chunk holds at least one class.
+constexpr int64_t kCapEntries = (int64_t)1 << 21;
 
 enum : int {
     kCcErrNegative = 1,         // negative request or exe_count
@@ -78,6 +91,13 @@ struct CapNodesIn {
     const int32_t* group;       // NULL = class 0
 };
 
+// The classes of one chunk: member == NULL -> node_group classes (K = 2), else the affinity bitmap of gangpack_affinity.cuh
+struct CapClassesIn {
+    const int32_t* group;       // [n] node_group, NULL = class 0
+    const uint32_t* member;     // [K][words]: row k = affinity a0 + k
+    int32_t words;
+};
+
 // kCapSeg consecutive nodes (or fewer, at the end) of one bucket
 struct CapSeg {
     int32_t first, len;
@@ -86,17 +106,20 @@ struct CapSeg {
 };
 
 struct CapScratch {
-    int32_t* key;               // [2n] per node: its class's bucket (-1 = in no class) and its bucket of class slot G (every
-    int32_t* rank;              // [2n] node, for class -1 drivers; -1 = invalid node), and the node's position in each
+    int32_t* key;               // [K n] entry k n + i: node i's bucket in class k of the chunk, -1 = not in it (or invalid)
+    int32_t* rank;              // [K n] the node's position in that bucket
+    int32_t* zone;              // [n] the node's zone, -1 = invalid node
     int32_t* bucket_cnt;        // [B]
     int32_t* bucket_off;        // [B + 1]
     int32_t* seg_off;           // [B + 1]
     int32_t* ms_off;            // [B + 1]
     long long* staged[3];       // [n] schedulable resources in node-table order
-    long long* sched[3];        // [2n] the same, nodes grouped by bucket (a node of a class appears twice)
+    long long* sched[3];        // [K n] the same, nodes grouped by bucket (once per class of the chunk it is in)
     CapSeg* segs;               // [n_segs]
     int* err;
     int32_t B, Z, G, n;
+    int32_t K;                  // classes in the chunk: 2 for node_group (slot G = every node), <= n_aff for affinities
+    int32_t a0;                 // affinity layout: the chunk's first class; -1 = node_group layout
 };
 
 // (pair, multi-segment bucket): the bucket's partial T_z and M_z, and how many of its segments have added theirs
@@ -161,16 +184,25 @@ __global__ void gp_cc_nodes(CapNodesIn in, CapScratch s) {
     const int32_t z = in.zone ? in.zone[i] : 0;
     const int32_t g = in.group ? in.group[i] : 0;
     if (z < 0 || z >= s.Z) bad |= kCcErrZone;
-    if (g < -1 || g >= s.G) bad |= kCcErrNodeGroup;
-    if (bad) { atomicOr(s.err, bad); s.key[i] = s.key[s.n + i] = -1; return; }
-    // class slot G holds every node by zone: a class -1 driver's zone is one bucket, whatever the classes of its nodes
-    const int32_t key = g < 0 ? -1 : g * s.Z + z, all = s.G * s.Z + z;
-    s.key[i] = key;
-    s.key[s.n + i] = all;
-    if (key >= 0) s.rank[i] = atomicAdd(s.bucket_cnt + key, 1);
-    s.rank[s.n + i] = atomicAdd(s.bucket_cnt + all, 1);
+    if (in.group && (g < -1 || g >= s.G)) bad |= kCcErrNodeGroup;     // NULL: every node in class 0
+    if (bad) { atomicOr(s.err, bad); s.zone[i] = -1; return; }
+    s.zone[i] = z;
 #pragma unroll
     for (int d = 0; d < 3; ++d) s.staged[d][i] = v[d];
+}
+
+// entry j = k n + i: node i in class k of the chunk -> bucket k Z + zone
+__global__ void gp_cc_keys(CapClassesIn in, CapScratch s) {
+    const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (j >= (long long)s.K * s.n) return;
+    const int32_t k = (int32_t)(j / s.n), i = (int32_t)(j - (long long)k * s.n), z = s.zone[i];
+    int32_t cls;                // the entry's bucket row, -1 = node i is not in class k
+    if (in.member) cls = (in.member[(long long)k * in.words + (i >> 5)] >> (i & 31)) & 1u ? k : -1;
+    else if (k == 1) cls = s.G;  // class slot G holds every node by zone: a class -1 driver's zone is one bucket
+    else cls = in.group ? in.group[i] : 0;
+    const int32_t key = z >= 0 && cls >= 0 ? cls * s.Z + z : -1;
+    s.key[j] = key;
+    if (key >= 0) s.rank[j] = atomicAdd(s.bucket_cnt + key, 1);
 }
 
 __global__ void __launch_bounds__(1024) gp_cc_bucket_scan(CapScratch s) {
@@ -190,9 +222,9 @@ __global__ void __launch_bounds__(1024) gp_cc_bucket_scan(CapScratch s) {
 }
 
 __global__ void gp_cc_scatter(CapScratch s) {
-    const int32_t j = blockIdx.x * blockDim.x + threadIdx.x;     // [0, n): class buckets, [n, 2n): class slot G
-    if (j >= 2 * s.n) return;
-    const int32_t key = s.key[j], i = j < s.n ? j : j - s.n;
+    const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;     // entry k n + i
+    if (j >= (long long)s.K * s.n) return;
+    const int32_t key = s.key[j], i = (int32_t)(j % s.n);
     if (key < 0) return;
     const int32_t r = s.rank[j], pos = s.bucket_off[key] + r;
     s.sched[0][pos] = s.staged[0][i]; s.sched[1][pos] = s.staged[1][i]; s.sched[2][pos] = s.staged[2][i];
@@ -212,6 +244,7 @@ struct CapAppsIn {
     const int32_t* count;
     const int32_t* group;       // NULL = class 0
     int32_t n_groups;
+    int32_t min_group;          // -1: node_group classes (-1 = every node); 0: affinity ids
     uint32_t hash_mask;         // table size - 1; the size is a power of two >= 2 n
 };
 
@@ -271,7 +304,7 @@ __global__ void gp_cc_intern(CapAppsIn in, CapEntry* table, CapPair* pairs, int3
     }
     if (in.count[i] < 0) bad |= kCcErrNegative;
     const int32_t g = in.group ? in.group[i] : 0;
-    if (g < -1 || g >= in.n_groups) bad |= kCcErrGroup;
+    if (g < in.min_group || g >= in.n_groups) bad |= kCcErrGroup;
     if (bad) atomicOr(err, bad);
     // chained, so that no exchange of fields between the two shapes or the class leaves the fingerprint unchanged
     unsigned long long fp = shape_fingerprint(q[3], q[4], q[5]);
@@ -298,9 +331,17 @@ __global__ void gp_cc_intern(CapAppsIn in, CapEntry* table, CapPair* pairs, int3
     app_pair[i] = bad ? -1 : id;
 }
 
-// the segments a pair visits: class c -> those of buckets [c Z, (c+1) Z), class -1 -> those of class slot G
+// the pair's class is one of the chunk's
+__device__ __forceinline__ bool cc_in_chunk(const CapScratch& s, int32_t cls) {
+    return s.a0 < 0 || (cls >= s.a0 && cls - s.a0 < s.K);
+}
+
+// the segments a pair visits: class c -> those of buckets [c Z, (c+1) Z), class -1 -> those of class slot G; an affinity
+// class a -> those of row a - a0, none outside the chunk
 __device__ __forceinline__ void cc_class_segs(const CapScratch& s, int32_t cls, int32_t& first, int32_t& cnt) {
-    if (cls < 0) cls = s.G;
+    if (!cc_in_chunk(s, cls)) { first = 0; cnt = 0; return; }
+    if (s.a0 >= 0) cls -= s.a0;
+    else if (cls < 0) cls = s.G;
     first = s.seg_off[cls * s.Z];
     cnt = s.seg_off[(cls + 1) * s.Z] - first;
 }
@@ -319,7 +360,7 @@ __global__ void __launch_bounds__(1024) gp_cc_pair_scan(CapScratch s, const CapP
     for (int32_t p0 = 0; p0 < np; p0 += 1024) {
         const int32_t p = p0 + (int32_t)threadIdx.x;
         int32_t first = 0, cnt = 0;
-        if (p < np) {
+        if (p < np && cc_in_chunk(s, pairs[p].cls)) {
             cc_class_segs(s, pairs[p].cls, first, cnt);
             out.T[p] = 0ull; out.M[p] = kCapNone; out.zone_best[p] = kCapNone;
         }

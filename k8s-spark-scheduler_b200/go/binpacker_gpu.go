@@ -24,12 +24,16 @@ import (
 	"math"
 	"runtime"
 	"sort"
+	"strconv"
 	"sync"
 	"unsafe"
 
 	"github.com/palantir/k8s-spark-scheduler-lib/pkg/binpack"
 	"github.com/palantir/k8s-spark-scheduler-lib/pkg/resources"
+	v1 "k8s.io/api/core/v1"
 	"k8s.io/apimachinery/pkg/api/resource"
+	"k8s.io/apimachinery/pkg/labels"
+	"k8s.io/apimachinery/pkg/selection"
 )
 
 // Names under which the GPU packers are registered next to the reference's own entries in
@@ -1152,15 +1156,6 @@ func FitEarlierDriversAzAware(apps []QueuedApp, nodeNames, executorNodeNames []s
 	return fits, true
 }
 
-// StaleDriver is one driver the unschedulable-pod marker checks (scanForUnschedulablePods, EXT/unschedulablepods.go:93-129):
-// its application resources and the affinity class of its required node affinity, an index into the classes the caller
-// assigns to the nodes (-1: the affinity matches every node).
-type StaleDriver struct {
-	DriverResources, ExecutorResources *resources.Resources
-	MinExecutorCount                   int
-	AffinityClass                      int32
-}
-
 // gpBinpacker maps a `binpack:` value to the device packer; unknown names select distribute-evenly, like SelectBinpacker
 // (internal/binpacker/binpack.go:52-58).
 func gpBinpacker(name string) C.gp_binpacker {
@@ -1177,29 +1172,265 @@ func gpBinpacker(name string) C.gp_binpacker {
 	return C.GP_BP_DISTRIBUTE_EVENLY
 }
 
-// DoesPodsExceedClusterCapacity is DoesPodExceedClusterCapacity (EXT/unschedulablepods.go:132-166) for every stale driver of
-// one marker sweep in ONE gp_exceeds_cluster_capacity call, whatever the `binpack:` value.  nodesSchedulingMetadata is
-// NodeSchedulingMetadataForNodes(every node, zero usage, GetNonSchedulableOverhead): only SchedulableResources and ZoneLabel
-// are read.  nodeClass gives the affinity class of each node (absent: in none of the nClasses classes).  The device context's
-// resident snapshot is not touched.  ok=false (no device, an inexact quantity, a count outside int32, any non-OK status):
-// the caller runs DoesPodExceedClusterCapacity per driver in Go.  Cost: one evaluation per node of a class per distinct
-// (executor shape, driver shape) pair; for tightly-pack / distribute-evenly sweeps with thousands of distinct pairs,
-// gp_pack_batch with one instance group per class is faster (INTEGRATION.md, the marker's "Cost" note).
-func DoesPodsExceedClusterCapacity(binpackerName string, nodesSchedulingMetadata resources.NodeGroupSchedulingMetadata,
-	nodeClass map[string]int32, nClasses int32, drivers []StaleDriver) ([]bool, bool) {
+// StaleDriver is one driver the unschedulable-pod marker checks (scanForUnschedulablePods, EXT/unschedulablepods.go:93-129):
+// its application resources and its required node affinity, an index into the distinct affinities of the sweep.
+type StaleDriver struct {
+	DriverResources, ExecutorResources *resources.Resources
+	MinExecutorCount                   int
+	Affinity                           int32
+}
+
+// NodeAffinity is one distinct required node affinity: what GetRequiredNodeAffinity(pod) reads
+// (K8S/component-helpers/scheduling/corev1/nodeaffinity/nodeaffinity.go:297-324).
+type NodeAffinity struct {
+	NodeSelector map[string]string
+	Required     *v1.NodeSelector // pod.Spec.Affinity.NodeAffinity.RequiredDuringSchedulingIgnoredDuringExecution; nil = none
+}
+
+// RequiredNodeAffinityOf reads a pod's NodeAffinity.
+func RequiredNodeAffinityOf(pod *v1.Pod) NodeAffinity {
+	a := NodeAffinity{NodeSelector: pod.Spec.NodeSelector}
+	if pod.Spec.Affinity != nil && pod.Spec.Affinity.NodeAffinity != nil {
+		a.Required = pod.Spec.Affinity.NodeAffinity.RequiredDuringSchedulingIgnoredDuringExecution
+	}
+	return a
+}
+
+// affinityArrays holds gp_node_labels and gp_node_affinities.  Label keys and values become dense ids; every rule that needs
+// the strings is applied here with the reference's own functions: labels.NewRequirement (the operator mapping of
+// nodeSelectorRequirementsAsSelector, nodeaffinity.go:203-241) and the In / NotIn-with-one-value rule of
+// nodeSelectorRequirementsAsFieldSelector (:248-280) set a term's parse_error flag, strconv.ParseInt(v, 10, 64) gives
+// label_int_ok / label_int, metadata.name becomes a node index (-1: no such node) and any other field key, which reads ""
+// (extractNodeFields), a constant requirement.  The same rules as affinity.encode() in the Python package.
+type affinityArrays struct {
+	nKeys, nValues                                          int32
+	labelOff, labelInt, selOff, termOff, termReqOff         []int64
+	reqInt, reqValOff                                       []int64
+	labelKey, labelVal, selKey, selVal, reqOp, reqKey, reqVal []int32
+	labelIntOK, hasRequired, termParseError                 []uint8
+}
+
+var labelOps = map[v1.NodeSelectorOperator]struct {
+	sel selection.Operator
+	op  C.int32_t
+}{
+	v1.NodeSelectorOpIn: {selection.In, C.GP_AFF_IN}, v1.NodeSelectorOpNotIn: {selection.NotIn, C.GP_AFF_NOT_IN},
+	v1.NodeSelectorOpExists: {selection.Exists, C.GP_AFF_EXISTS}, v1.NodeSelectorOpDoesNotExist: {selection.DoesNotExist, C.GP_AFF_DOES_NOT_EXIST},
+	v1.NodeSelectorOpGt: {selection.GreaterThan, C.GP_AFF_GT}, v1.NodeSelectorOpLt: {selection.LessThan, C.GP_AFF_LT},
+}
+
+func internAffinities(nodes []*v1.Node, affinities []NodeAffinity) *affinityArrays {
+	e := &affinityArrays{labelOff: []int64{0}, selOff: []int64{0}, termOff: []int64{0}, termReqOff: []int64{0}, reqValOff: []int64{0}}
+	keys, vals, nodeIndex := map[string]int32{}, map[string]int32{}, map[string]int64{}
+	id := func(m map[string]int32, s string) int32 {
+		v, seen := m[s]
+		if !seen {
+			v = int32(len(m))
+			m[s] = v
+		}
+		return v
+	}
+	for i, n := range nodes {
+		nodeIndex[n.Name] = int64(i)
+	}
+	for _, n := range nodes {
+		type ent struct {
+			k int32
+			v string
+		}
+		ents := make([]ent, 0, len(n.Labels))
+		for k, v := range n.Labels {
+			ents = append(ents, ent{id(keys, k), v})
+		}
+		sort.Slice(ents, func(a, b int) bool { return ents[a].k < ents[b].k })
+		for _, en := range ents {
+			iv, err := strconv.ParseInt(en.v, 10, 64)
+			ok := uint8(0)
+			if err == nil {
+				ok = 1
+			} else {
+				iv = 0
+			}
+			e.labelKey, e.labelVal = append(e.labelKey, en.k), append(e.labelVal, id(vals, en.v))
+			e.labelIntOK, e.labelInt = append(e.labelIntOK, ok), append(e.labelInt, iv)
+		}
+		e.labelOff = append(e.labelOff, int64(len(e.labelKey)))
+	}
+	addReq := func(op C.int32_t, key int32, bound int64, vs []int32) {
+		sort.Slice(vs, func(a, b int) bool { return vs[a] < vs[b] })
+		e.reqOp, e.reqKey, e.reqInt = append(e.reqOp, int32(op)), append(e.reqKey, key), append(e.reqInt, bound)
+		for j, v := range vs {
+			if j == 0 || v != vs[j-1] {
+				e.reqVal = append(e.reqVal, v)
+			}
+		}
+		e.reqValOff = append(e.reqValOff, int64(len(e.reqVal)))
+	}
+	for _, a := range affinities {
+		for k, v := range a.NodeSelector {
+			e.selKey, e.selVal = append(e.selKey, id(keys, k)), append(e.selVal, id(vals, v))
+		}
+		e.selOff = append(e.selOff, int64(len(e.selKey)))
+		has := uint8(0)
+		var terms []v1.NodeSelectorTerm
+		if a.Required != nil {
+			has, terms = 1, a.Required.NodeSelectorTerms
+		}
+		e.hasRequired = append(e.hasRequired, has)
+		for _, t := range terms {
+			bad := false
+			for _, r := range t.MatchExpressions {
+				o, known := labelOps[r.Operator]
+				if !known {
+					bad = true
+				} else if _, err := labels.NewRequirement(r.Key, o.sel, r.Values); err != nil {
+					bad = true
+				}
+			}
+			for _, r := range t.MatchFields {
+				if (r.Operator != v1.NodeSelectorOpIn && r.Operator != v1.NodeSelectorOpNotIn) || len(r.Values) != 1 {
+					bad = true
+				}
+			}
+			flag := uint8(0)
+			if bad {
+				flag = 1
+			} else {
+				for _, r := range t.MatchExpressions {
+					o := labelOps[r.Operator]
+					var bound int64
+					var vs []int32
+					switch o.op {
+					case C.GP_AFF_GT, C.GP_AFF_LT:
+						bound, _ = strconv.ParseInt(r.Values[0], 10, 64)
+					case C.GP_AFF_IN, C.GP_AFF_NOT_IN:
+						for _, v := range r.Values {
+							vs = append(vs, id(vals, v))
+						}
+					}
+					addReq(o.op, id(keys, r.Key), bound, vs)
+				}
+				for _, r := range t.MatchFields {
+					in := r.Operator == v1.NodeSelectorOpIn
+					if r.Key == "metadata.name" {
+						idx, found := nodeIndex[r.Values[0]]
+						if !found {
+							idx = -1
+						}
+						op := C.int32_t(C.GP_AFF_FIELD_NAME_NOT_IN)
+						if in {
+							op = C.GP_AFF_FIELD_NAME_IN
+						}
+						addReq(op, 0, idx, nil)
+					} else if (r.Values[0] == "") == in { // any other field reads "": always true
+						addReq(C.GP_AFF_FIELD_NAME_NOT_IN, 0, -1, nil)
+					} else { // never true
+						addReq(C.GP_AFF_FIELD_NAME_IN, 0, -1, nil)
+					}
+				}
+			}
+			e.termParseError = append(e.termParseError, flag)
+			e.termReqOff = append(e.termReqOff, int64(len(e.reqOp)))
+		}
+		e.termOff = append(e.termOff, int64(len(e.termParseError)))
+	}
+	e.nKeys, e.nValues = int32(len(keys)), int32(len(vals))
+	// one spare element each: no slice base is nil and every one can be pinned
+	e.labelKey, e.labelVal, e.selKey, e.selVal = append(e.labelKey, 0), append(e.labelVal, 0), append(e.selKey, 0), append(e.selVal, 0)
+	e.reqOp, e.reqKey, e.reqVal, e.labelInt, e.reqInt = append(e.reqOp, 0), append(e.reqKey, 0), append(e.reqVal, 0), append(e.labelInt, 0), append(e.reqInt, 0)
+	e.labelIntOK, e.hasRequired, e.termParseError = append(e.labelIntOK, 0), append(e.hasRequired, 0), append(e.termParseError, 0)
+	return e
+}
+
+// structs pins every slice base and returns the two C structs over them.
+func (e *affinityArrays) structs(pin *runtime.Pinner, nNodes, nAff int) (C.gp_node_labels, C.gp_node_affinities) {
+	for _, s := range [][]int64{e.labelOff, e.labelInt, e.selOff, e.termOff, e.termReqOff, e.reqInt, e.reqValOff} {
+		pin.Pin(&s[0])
+	}
+	for _, s := range [][]int32{e.labelKey, e.labelVal, e.selKey, e.selVal, e.reqOp, e.reqKey, e.reqVal} {
+		pin.Pin(&s[0])
+	}
+	for _, s := range [][]uint8{e.labelIntOK, e.hasRequired, e.termParseError} {
+		pin.Pin(&s[0])
+	}
+	l := C.gp_node_labels{n_nodes: C.int32_t(nNodes), n_keys: C.int32_t(e.nKeys), n_values: C.int32_t(e.nValues),
+		label_off: ptr64(e.labelOff), label_key: ptr32(e.labelKey), label_val: ptr32(e.labelVal), label_int_ok: ptr8(e.labelIntOK),
+		label_int: ptr64(e.labelInt)}
+	a := C.gp_node_affinities{n_aff: C.int32_t(nAff), sel_off: ptr64(e.selOff), sel_key: ptr32(e.selKey), sel_val: ptr32(e.selVal),
+		has_required: ptr8(e.hasRequired), term_off: ptr64(e.termOff), term_req_off: ptr64(e.termReqOff),
+		term_parse_error: ptr8(e.termParseError), req_op: ptr32(e.reqOp), req_key: ptr32(e.reqKey), req_int: ptr64(e.reqInt),
+		req_val_off: ptr64(e.reqValOff), req_val: ptr32(e.reqVal)}
+	return l, a
+}
+
+// MatchRequiredNodeAffinity is utils.ListWithPredicate(nodes, GetRequiredNodeAffinity(pod).Match) (internal/common/utils/
+// pods.go:110-127) for every distinct affinity at once, in one gp_match_node_affinity call: selectDriverNode's
+// availableNodes (EXT/resource.go:292-298).  matched[a] lists the nodes affinity a matches, in node order; failed[a] =
+// some node gave an error -- ListWithPredicate's error, on which the Predicate fails with failureInternal.  ok=false (no
+// device, any non-OK status): the caller runs ListWithPredicate in Go.
+func MatchRequiredNodeAffinity(nodes []*v1.Node, affinities []NodeAffinity) (matched [][]*v1.Node, failed []bool, ok bool) {
 	d, err := getDevice()
 	if err != nil {
-		return nil, false
+		return nil, nil, false
 	}
-	n, q := len(nodesSchedulingMetadata), len(drivers)
+	n, nAff := len(nodes), len(affinities)
+	e := internAffinities(nodes, affinities)
+	words := (n + 31) / 32
+	member := make([]uint32, nAff*words+1)
+	nMatch, nError := make([]int32, nAff+1), make([]int32, nAff+1)
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	l, a := e.structs(&pin, n, nAff)
+	pin.Pin(&member[0])
+	pin.Pin(&nMatch[0])
+	pin.Pin(&nError[0])
+	out := C.gp_affinity_match{member: (*C.uint32_t)(unsafe.Pointer(&member[0])), n_match: ptr32(nMatch), n_error: ptr32(nError)}
+	if C.gp_match_node_affinity(d.ctx, &l, &a, &out) != C.GP_OK {
+		return nil, nil, false
+	}
+	matched, failed = make([][]*v1.Node, nAff), make([]bool, nAff)
+	for p := 0; p < nAff; p++ {
+		failed[p] = nError[p] > 0
+		matched[p] = make([]*v1.Node, 0, nMatch[p])
+		for i := 0; i < n; i++ {
+			if member[p*words+i/32]>>(i%32)&1 != 0 {
+				matched[p] = append(matched[p], nodes[i])
+			}
+		}
+	}
+	return matched, failed, true
+}
+
+// DoesPodsExceedClusterCapacity is DoesPodExceedClusterCapacity (EXT/unschedulablepods.go:132-166) for every stale driver of
+// one marker sweep in ONE gp_exceeds_cluster_capacity_affinity call, whatever the `binpack:` value.  nodes is the node
+// lister's list; nodesSchedulingMetadata is NodeSchedulingMetadataForNodes(nodes, zero usage, GetNonSchedulableOverhead):
+// only SchedulableResources and ZoneLabel are read.  affinities holds each distinct required affinity of the stale drivers
+// once and drivers[i].Affinity indexes it; the affinities' node sets may overlap freely.  affinityError[i]: the driver's
+// affinity gave ListWithPredicate's error, on which the reference's scan returns (:113-117); exceeds[i] is then meaningless.
+// The device context's resident snapshot is not touched.  ok=false (no device, an inexact quantity, a count outside int32,
+// a node without metadata, any non-OK status): the caller runs DoesPodExceedClusterCapacity per driver in Go.
+func DoesPodsExceedClusterCapacity(binpackerName string, nodes []*v1.Node, nodesSchedulingMetadata resources.NodeGroupSchedulingMetadata,
+	affinities []NodeAffinity, drivers []StaleDriver) (exceeds, affinityError []bool, ok bool) {
+	d, err := getDevice()
+	if err != nil {
+		return nil, nil, false
+	}
+	n, q := len(nodes), len(drivers)
 	sc, sm, sg := make([]int64, n+1), make([]int64, n+1), make([]int64, n+1)
-	zone, group := make([]int32, n+1), make([]int32, n+1)
+	zone := make([]int32, n+1)
 	zoneID := map[string]int32{}
-	i := 0
-	for name, md := range nodesSchedulingMetadata {
+	for i, node := range nodes {
+		md, found := nodesSchedulingMetadata[node.Name]
+		if !found {
+			return nil, nil, false
+		}
 		c, m, g, exact := toTriple(md.SchedulableResources)
 		if !exact {
-			return nil, false
+			return nil, nil, false
 		}
 		sc[i], sm[i], sg[i] = c, m, g
 		z, seen := zoneID[md.ZoneLabel]
@@ -1208,52 +1439,49 @@ func DoesPodsExceedClusterCapacity(binpackerName string, nodesSchedulingMetadata
 			zoneID[md.ZoneLabel] = z
 		}
 		zone[i] = z
-		group[i] = -1
-		if cls, in := nodeClass[name]; in {
-			group[i] = cls
-		}
-		i++
 	}
 	var cols [6][]int64
 	for t := range cols {
 		cols[t] = make([]int64, q+1)
 	}
-	count, class := make([]int32, q+1), make([]int32, q+1)
+	count, prog := make([]int32, q+1), make([]int32, q+1)
 	for j, drv := range drivers {
 		dc, dm, dg, ok1 := toTriple(drv.DriverResources)
 		ec, em, eg, ok2 := toTriple(drv.ExecutorResources)
 		if !ok1 || !ok2 || drv.MinExecutorCount < 0 || drv.MinExecutorCount > math.MaxInt32 {
-			return nil, false
+			return nil, nil, false
 		}
 		cols[0][j], cols[1][j], cols[2][j], cols[3][j], cols[4][j], cols[5][j] = dc, dm, dg, ec, em, eg
-		count[j], class[j] = int32(drv.MinExecutorCount), drv.AffinityClass
+		count[j], prog[j] = int32(drv.MinExecutorCount), drv.Affinity
 	}
-	exceeds := make([]uint8, q+1)
+	e := internAffinities(nodes, affinities)
+	out, errs := make([]uint8, q+1), make([]uint8, q+1)
 	runtime.LockOSThread()
 	defer runtime.UnlockOSThread()
 	d.mu.Lock()
 	defer d.mu.Unlock()
-	// the two C structs hold Go pointers: every slice base is pinned for the duration of the call
+	// the C structs hold Go pointers: every slice base is pinned for the duration of the call
 	var pin runtime.Pinner
 	defer pin.Unpin()
-	for _, p := range []any{&sc[0], &sm[0], &sg[0], &zone[0], &group[0], &count[0], &class[0], &exceeds[0]} {
+	for _, p := range []any{&sc[0], &sm[0], &sg[0], &zone[0], &count[0], &prog[0], &out[0], &errs[0]} {
 		pin.Pin(p)
 	}
 	for t := range cols {
 		pin.Pin(&cols[t][0])
 	}
-	nodes := C.gp_capacity_nodes{n_nodes: C.int32_t(n), alloc_cpu_milli: ptr64(sc), alloc_mem_bytes: ptr64(sm), alloc_gpu: ptr64(sg),
-		n_zones: C.int32_t(max(len(zoneID), 1)), zone_id: ptr32(zone), n_groups: C.int32_t(max(nClasses, 1)), node_group: ptr32(group)}
-	a := C.gp_apps{n_apps: C.int32_t(q), drv_cpu_milli: ptr64(cols[0]), drv_mem_bytes: ptr64(cols[1]), drv_gpu: ptr64(cols[2]),
-		exe_cpu_milli: ptr64(cols[3]), exe_mem_bytes: ptr64(cols[4]), exe_gpu: ptr64(cols[5]), exe_count: ptr32(count), group: ptr32(class)}
-	if C.gp_exceeds_cluster_capacity(d.ctx, &nodes, &a, gpBinpacker(binpackerName), ptr8(exceeds)) != C.GP_OK {
-		return nil, false
+	l, a := e.structs(&pin, n, len(affinities))
+	cn := C.gp_capacity_nodes{n_nodes: C.int32_t(n), alloc_cpu_milli: ptr64(sc), alloc_mem_bytes: ptr64(sm), alloc_gpu: ptr64(sg),
+		n_zones: C.int32_t(max(len(zoneID), 1)), zone_id: ptr32(zone)}
+	apps := C.gp_apps{n_apps: C.int32_t(q), drv_cpu_milli: ptr64(cols[0]), drv_mem_bytes: ptr64(cols[1]), drv_gpu: ptr64(cols[2]),
+		exe_cpu_milli: ptr64(cols[3]), exe_mem_bytes: ptr64(cols[4]), exe_gpu: ptr64(cols[5]), exe_count: ptr32(count), group: ptr32(prog)}
+	if C.gp_exceeds_cluster_capacity_affinity(d.ctx, &cn, &l, &a, &apps, gpBinpacker(binpackerName), ptr8(out), ptr8(errs)) != C.GP_OK {
+		return nil, nil, false
 	}
-	out := make([]bool, q)
-	for j := range out {
-		out[j] = exceeds[j] != 0
+	exceeds, affinityError = make([]bool, q), make([]bool, q)
+	for j := range exceeds {
+		exceeds[j], affinityError[j] = out[j] != 0, errs[j] != 0
 	}
-	return out, true
+	return exceeds, affinityError, true
 }
 
 // ReconcileNode is one lister node as the failover reconciler sees it (EXT/failover.go:286-314).

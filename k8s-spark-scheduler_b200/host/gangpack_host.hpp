@@ -662,6 +662,201 @@ private:
 }  // namespace sort
 
 // ------------------------------------------------------------------------------------------------
+// ---- required node affinity (K8S = vendor/k8s.io) ---------------------------------------------------------------------
+// GetRequiredNodeAffinity(pod) as strings, and their interning into gp_node_labels / gp_node_affinities: label keys and values
+// become dense ids, and every rule that needs the strings is applied here -- labels.NewRequirement's validation
+// (K8S/apimachinery/pkg/labels/selector.go:156-196) and the field-selector conversion (K8S/component-helpers/scheduling/corev1/
+// nodeaffinity/nodeaffinity.go:203-280) become a term's parse_error flag, strconv.ParseInt of a node's label value becomes
+// label_int_ok / label_int, metadata.name becomes a node index.  The same rules as affinity.encode() of the Python package.
+namespace affinity {
+
+struct Requirement { std::string Key, Operator; std::vector<std::string> Values; };   // v1.NodeSelectorRequirement
+struct Term { std::vector<Requirement> MatchExpressions, MatchFields; };              // v1.NodeSelectorTerm
+struct Program {                                   // pod.Spec.NodeSelector + RequiredDuringSchedulingIgnoredDuringExecution
+    std::map<std::string, std::string> NodeSelector;
+    bool HasRequired = false;                      // the required node selector is not nil
+    std::vector<Term> Terms;
+};
+struct Node { std::string Name; std::map<std::string, std::string> Labels; };
+
+// strconv.ParseInt(s, 10, 64): an optional sign, then one or more ASCII digits, within int64
+inline bool ParseInt(const std::string& s, int64_t* out) {
+    size_t i = (!s.empty() && (s[0] == '+' || s[0] == '-')) ? 1 : 0;
+    if (i == s.size()) return false;
+    const bool neg = s[0] == '-';
+    unsigned long long v = 0;
+    const unsigned long long lim = neg ? (1ull << 63) : (1ull << 63) - 1;
+    for (; i < s.size(); ++i) {
+        if (s[i] < '0' || s[i] > '9') return false;
+        const unsigned d = (unsigned)(s[i] - '0');
+        if (v > (lim - d) / 10) return false;      // out of range
+        v = v * 10 + d;
+    }
+    *out = neg ? (int64_t)(0 - v) : (int64_t)v;
+    return true;
+}
+inline bool AlNum(char c) { return (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || (c >= '0' && c <= '9'); }
+// ([A-Za-z0-9][-A-Za-z0-9_.]*)?[A-Za-z0-9], at most 63 characters
+inline bool QualifiedNamePart(const std::string& s) {
+    if (s.empty() || s.size() > 63 || !AlNum(s.front()) || !AlNum(s.back())) return false;
+    for (char c : s) if (!AlNum(c) && c != '-' && c != '_' && c != '.') return false;
+    return true;
+}
+// validation.IsDNS1123Subdomain: dot-separated [a-z0-9]([-a-z0-9]*[a-z0-9])?, at most 253 characters
+inline bool DNS1123Subdomain(const std::string& s) {
+    if (s.empty() || s.size() > 253) return false;
+    size_t b = 0;
+    for (;;) {
+        const size_t e = std::min(s.find('.', b), s.size());
+        if (e == b) return false;
+        auto lower = [](char c) { return (c >= 'a' && c <= 'z') || (c >= '0' && c <= '9'); };
+        if (!lower(s[b]) || !lower(s[e - 1])) return false;
+        for (size_t i = b; i < e; ++i) if (!lower(s[i]) && s[i] != '-') return false;
+        if (e == s.size()) return true;
+        b = e + 1;
+    }
+}
+// validation.IsQualifiedName
+inline bool ValidLabelKey(const std::string& k) {
+    const size_t slash = k.find('/');
+    if (slash == std::string::npos) return QualifiedNamePart(k);
+    if (k.find('/', slash + 1) != std::string::npos) return false;
+    return DNS1123Subdomain(k.substr(0, slash)) && QualifiedNamePart(k.substr(slash + 1));
+}
+// validation.IsValidLabelValue
+inline bool ValidLabelValue(const std::string& v) { return v.empty() || QualifiedNamePart(v); }
+
+inline bool LabelRequirementOk(const Requirement& r) {
+    static const std::set<std::string> ops = {"In", "NotIn", "Exists", "DoesNotExist", "Gt", "Lt"};
+    if (!ops.count(r.Operator) || !ValidLabelKey(r.Key)) return false;
+    if ((r.Operator == "In" || r.Operator == "NotIn") && r.Values.empty()) return false;
+    if ((r.Operator == "Exists" || r.Operator == "DoesNotExist") && !r.Values.empty()) return false;
+    int64_t v;
+    if ((r.Operator == "Gt" || r.Operator == "Lt") && (r.Values.size() != 1 || !ParseInt(r.Values[0], &v))) return false;
+    for (const auto& s : r.Values) if (!ValidLabelValue(s)) return false;
+    return true;
+}
+
+// The arrays of gp_node_labels / gp_node_affinities; the structs point into this object
+struct Encoded {
+    int32_t n_nodes = 0, n_keys = 0, n_values = 0, n_aff = 0;
+    std::vector<int64_t> label_off{0}, label_int, sel_off{0}, term_off{0}, term_req_off{0}, req_int, req_val_off{0};
+    std::vector<int32_t> label_key, label_val, sel_key, sel_val, req_op, req_key, req_val;
+    std::vector<uint8_t> label_int_ok, has_required, term_parse_error;
+    gp_node_labels Labels() const {
+        gp_node_labels l{};
+        l.n_nodes = n_nodes; l.n_keys = n_keys; l.n_values = n_values;
+        l.label_off = label_off.data(); l.label_key = label_key.data(); l.label_val = label_val.data();
+        l.label_int_ok = label_int_ok.data(); l.label_int = label_int.data();
+        return l;
+    }
+    gp_node_affinities Programs() const {
+        gp_node_affinities a{};
+        a.n_aff = n_aff; a.sel_off = sel_off.data(); a.sel_key = sel_key.data(); a.sel_val = sel_val.data();
+        a.has_required = has_required.data(); a.term_off = term_off.data(); a.term_req_off = term_req_off.data();
+        a.term_parse_error = term_parse_error.data(); a.req_op = req_op.data(); a.req_key = req_key.data(); a.req_int = req_int.data();
+        a.req_val_off = req_val_off.data(); a.req_val = req_val.data();
+        return a;
+    }
+};
+
+inline Encoded Encode(const std::vector<Node>& nodes, const std::vector<Program>& programs) {
+    Encoded e;
+    std::unordered_map<std::string, int32_t> keys, vals, nodeIndex;
+    auto key = [&](const std::string& s) { return keys.emplace(s, (int32_t)keys.size()).first->second; };
+    auto val = [&](const std::string& s) { return vals.emplace(s, (int32_t)vals.size()).first->second; };
+    for (size_t i = 0; i < nodes.size(); ++i)
+        if (nodes[i].Name.empty() || !nodeIndex.emplace(nodes[i].Name, (int32_t)i).second)
+            throw std::invalid_argument("affinity::Encode: node names must be unique and non-empty");
+    for (const Node& n : nodes) {
+        std::vector<std::pair<int32_t, const std::string*>> ent;
+        for (const auto& kv : n.Labels) ent.emplace_back(key(kv.first), &kv.second);
+        std::sort(ent.begin(), ent.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+        for (const auto& kv : ent) {
+            int64_t v = 0;
+            const bool ok = ParseInt(*kv.second, &v);
+            e.label_key.push_back(kv.first); e.label_val.push_back(val(*kv.second));
+            e.label_int_ok.push_back(ok ? 1 : 0); e.label_int.push_back(ok ? v : 0);
+        }
+        e.label_off.push_back((int64_t)e.label_key.size());
+    }
+    auto addReq = [&](int32_t op, int32_t k, int64_t bound, std::vector<int32_t> vs) {
+        std::sort(vs.begin(), vs.end());
+        vs.erase(std::unique(vs.begin(), vs.end()), vs.end());
+        e.req_op.push_back(op); e.req_key.push_back(k); e.req_int.push_back(bound);
+        e.req_val.insert(e.req_val.end(), vs.begin(), vs.end());
+        e.req_val_off.push_back((int64_t)e.req_val.size());
+    };
+    static const std::map<std::string, int32_t> opId = {{"In", GP_AFF_IN}, {"NotIn", GP_AFF_NOT_IN}, {"Exists", GP_AFF_EXISTS},
+                                                        {"DoesNotExist", GP_AFF_DOES_NOT_EXIST}, {"Gt", GP_AFF_GT}, {"Lt", GP_AFF_LT}};
+    for (const Program& p : programs) {
+        for (const auto& kv : p.NodeSelector) { e.sel_key.push_back(key(kv.first)); e.sel_val.push_back(val(kv.second)); }
+        e.sel_off.push_back((int64_t)e.sel_key.size());
+        e.has_required.push_back(p.HasRequired ? 1 : 0);
+        for (const Term& t : p.HasRequired ? p.Terms : std::vector<Term>{}) {
+            bool bad = false;
+            for (const auto& r : t.MatchExpressions) bad = bad || !LabelRequirementOk(r);
+            for (const auto& r : t.MatchFields) bad = bad || !((r.Operator == "In" || r.Operator == "NotIn") && r.Values.size() == 1);
+            e.term_parse_error.push_back(bad ? 1 : 0);
+            if (!bad) {
+                for (const auto& r : t.MatchExpressions) {
+                    const int32_t op = opId.at(r.Operator);
+                    int64_t bound = 0;
+                    std::vector<int32_t> vs;
+                    if (op == GP_AFF_GT || op == GP_AFF_LT) ParseInt(r.Values[0], &bound);
+                    if (op == GP_AFF_IN || op == GP_AFF_NOT_IN) for (const auto& s : r.Values) vs.push_back(val(s));
+                    addReq(op, key(r.Key), bound, vs);
+                }
+                for (const auto& r : t.MatchFields) {
+                    const bool in = r.Operator == "In";
+                    if (r.Key == "metadata.name") {
+                        auto it = nodeIndex.find(r.Values[0]);
+                        addReq(in ? GP_AFF_FIELD_NAME_IN : GP_AFF_FIELD_NAME_NOT_IN, 0, it == nodeIndex.end() ? -1 : it->second, {});
+                    } else {                       // extractNodeFields sets metadata.name only: any other field reads ""
+                        const bool always = (r.Values[0].empty()) == in;
+                        addReq(always ? GP_AFF_FIELD_NAME_NOT_IN : GP_AFF_FIELD_NAME_IN, 0, -1, {});
+                    }
+                }
+            }
+            e.term_req_off.push_back((int64_t)e.req_op.size());
+        }
+        e.term_off.push_back((int64_t)e.term_parse_error.size());
+    }
+    e.n_nodes = (int32_t)nodes.size(); e.n_keys = (int32_t)keys.size(); e.n_values = (int32_t)vals.size();
+    e.n_aff = (int32_t)programs.size();
+    // never hand a NULL pointer for an empty column
+    for (auto* v : {&e.label_key, &e.label_val, &e.sel_key, &e.sel_val, &e.req_op, &e.req_key, &e.req_val}) v->reserve(1);
+    for (auto* v : {&e.label_int, &e.req_int}) v->reserve(1);
+    for (auto* v : {&e.label_int_ok, &e.has_required, &e.term_parse_error}) v->reserve(1);
+    return e;
+}
+
+// utils.ListWithPredicate(nodes, GetRequiredNodeAffinity(pod).Match) for every program at once (gp_match_node_affinity):
+// matched[a] = the indices of the nodes program a matches, in node order; failed[a] = some node gave an error (the Predicate's
+// failureInternal).
+struct MatchResult { std::vector<std::vector<int32_t>> Matched; std::vector<bool> Failed; };
+inline MatchResult MatchRequiredNodeAffinity(const std::vector<Node>& nodes, const std::vector<Program>& programs) {
+    const Encoded e = Encode(nodes, programs);
+    const gp_node_labels l = e.Labels();
+    const gp_node_affinities a = e.Programs();
+    const size_t words = (nodes.size() + 31) / 32, A = programs.size();
+    std::vector<uint32_t> member(std::max<size_t>(A * words, 1));
+    std::vector<int32_t> nMatch(std::max<size_t>(A, 1)), nError(std::max<size_t>(A, 1));
+    gp_affinity_match out{member.data(), nMatch.data(), nError.data()};
+    gangpack::Device& dev = gangpack::Device::Get();
+    dev.check(gp_match_node_affinity(dev.ctx(), &l, &a, &out), "gp_match_node_affinity");
+    MatchResult r;
+    r.Matched.resize(A); r.Failed.resize(A);
+    for (size_t p = 0; p < A; ++p) {
+        r.Failed[p] = nError[p] > 0;
+        for (size_t i = 0; i < nodes.size(); ++i)
+            if ((member[p * words + i / 32] >> (i % 32)) & 1u) r.Matched[p].push_back((int32_t)i);
+    }
+    return r;
+}
+
+}  // namespace affinity
+
 namespace extender {
 
 struct SparkApplicationResources {        // internal/types/types.go:22-27
@@ -1097,6 +1292,60 @@ public:
         std::vector<uint8_t> out(std::max<size_t>(Q, 1));
         gangpack::Device& dev = gangpack::Device::Get();
         dev.check(gp_exceeds_cluster_capacity(dev.ctx(), &n, &a, Packer(), out.data()), "gp_exceeds_cluster_capacity");
+        return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
+    }
+
+    // The same sweep with each driver's node set = the nodes its required affinity matches (gp_exceeds_cluster_capacity_affinity):
+    // the sets may overlap freely.  nodes: the node table with labels, every node in nodesSchedulingMetadata; programs: one
+    // per distinct required affinity; drivers[i].Affinity indexes programs.  affinityError[i] = ListWithPredicate failed for
+    // driver i's affinity (the reference's scan returns at that driver, unschedulablepods.go:113-117); exceeds[i] is then
+    // meaningless.
+    struct AffinityStaleDriver {
+        resources::Resources DriverResources;
+        resources::Resources ExecutorResources;
+        int MinExecutorCount = 0;
+        int Affinity = 0;              // index into programs
+    };
+    std::vector<bool> DoesPodsExceedClusterCapacity(const resources::NodeGroupSchedulingMetadata& nodesSchedulingMetadata,
+                                                    const std::vector<affinity::Node>& nodes,
+                                                    const std::vector<affinity::Program>& programs,
+                                                    const std::vector<AffinityStaleDriver>& drivers,
+                                                    std::vector<bool>* affinityError) const {
+        const size_t N = nodes.size(), Q = drivers.size();
+        std::vector<int64_t> sc(N + 1), sm(N + 1), sg(N + 1);
+        std::vector<int32_t> zone(N + 1);
+        std::unordered_map<std::string, int32_t> zoneId;
+        for (size_t i = 0; i < N; ++i) {
+            const auto& m = nodesSchedulingMetadata.at(nodes[i].Name);
+            sc[i] = m.SchedulableResources.CPU; sm[i] = m.SchedulableResources.Memory; sg[i] = m.SchedulableResources.NvidiaGPU;
+            zone[i] = zoneId.emplace(m.ZoneLabel, (int32_t)zoneId.size()).first->second;
+        }
+        std::vector<int64_t> q[6];
+        std::vector<int32_t> count(Q + 1), prog(Q + 1);
+        for (auto& col : q) col.resize(Q + 1);
+        for (size_t i = 0; i < Q; ++i) {
+            const AffinityStaleDriver& d = drivers[i];
+            q[0][i] = d.DriverResources.CPU; q[1][i] = d.DriverResources.Memory; q[2][i] = d.DriverResources.NvidiaGPU;
+            q[3][i] = d.ExecutorResources.CPU; q[4][i] = d.ExecutorResources.Memory; q[5][i] = d.ExecutorResources.NvidiaGPU;
+            count[i] = d.MinExecutorCount; prog[i] = d.Affinity;
+        }
+        const affinity::Encoded e = affinity::Encode(nodes, programs);
+        const gp_node_labels l = e.Labels();
+        const gp_node_affinities p = e.Programs();
+        gp_capacity_nodes n{};
+        n.n_nodes = (int32_t)N;
+        n.alloc_cpu_milli = sc.data(); n.alloc_mem_bytes = sm.data(); n.alloc_gpu = sg.data();   // schedulable = alloc - overhead
+        n.n_zones = std::max<int32_t>(1, (int32_t)zoneId.size()); n.zone_id = zone.data();
+        gp_apps a{};
+        a.n_apps = (int32_t)Q;
+        a.drv_cpu_milli = q[0].data(); a.drv_mem_bytes = q[1].data(); a.drv_gpu = q[2].data();
+        a.exe_cpu_milli = q[3].data(); a.exe_mem_bytes = q[4].data(); a.exe_gpu = q[5].data();
+        a.exe_count = count.data(); a.group = prog.data();
+        std::vector<uint8_t> out(Q + 1), err(Q + 1);
+        gangpack::Device& dev = gangpack::Device::Get();
+        dev.check(gp_exceeds_cluster_capacity_affinity(dev.ctx(), &n, &l, &p, &a, Packer(), out.data(), err.data()),
+                  "gp_exceeds_cluster_capacity_affinity");
+        if (affinityError) affinityError->assign(err.begin(), err.begin() + (std::ptrdiff_t)Q);
         return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
     }
 

@@ -19,6 +19,7 @@ _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
                                                     "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
                                                     "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh", "gangpack_capacity.cuh",
+                                                    "gangpack_affinity.cuh",
                                                     "gangpack_reconcile.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
@@ -41,7 +42,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_set_snapshot_device", "gp_pack_batch_device", "gp_stream", "gp_synchronize", "gp_last_stats",
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
-           "gp_reconcile_find_nodes",
+           "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -176,6 +177,23 @@ class gp_capacity_nodes(C.Structure):
                 ("n_zones", C.c_int32), ("zone_id", C.c_void_p), ("n_groups", C.c_int32), ("node_group", C.c_void_p)]
 
 
+class gp_node_labels(C.Structure):
+    _fields_ = [("n_nodes", C.c_int32), ("n_keys", C.c_int32), ("n_values", C.c_int32), ("reserved", C.c_int32),
+                ("label_off", C.c_void_p), ("label_key", C.c_void_p), ("label_val", C.c_void_p), ("label_int_ok", C.c_void_p),
+                ("label_int", C.c_void_p)]
+
+
+class gp_node_affinities(C.Structure):
+    _fields_ = [("n_aff", C.c_int32), ("reserved", C.c_int32), ("sel_off", C.c_void_p), ("sel_key", C.c_void_p),
+                ("sel_val", C.c_void_p), ("has_required", C.c_void_p), ("term_off", C.c_void_p), ("term_req_off", C.c_void_p),
+                ("term_parse_error", C.c_void_p), ("req_op", C.c_void_p), ("req_key", C.c_void_p), ("req_int", C.c_void_p),
+                ("req_val_off", C.c_void_p), ("req_val", C.c_void_p)]
+
+
+class gp_affinity_match(C.Structure):
+    _fields_ = [("member", C.c_void_p), ("n_match", C.c_void_p), ("n_error", C.c_void_p)]
+
+
 class gp_reconcile_nodes(C.Structure):
     _fields_ = [("n_groups", C.c_int32), ("reserved", C.c_int32), ("node_group", C.c_void_p), ("creation", C.c_void_p),
                 ("unschedulable", C.c_void_p), ("ready", C.c_void_p)]
@@ -248,6 +266,12 @@ def load():
     L.gp_exceeds_cluster_capacity.restype = C.c_int
     L.gp_exceeds_cluster_capacity.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.POINTER(gp_apps), C.c_int, C.c_void_p]
     L.gp_reconcile_find_nodes.restype = C.c_int
+    L.gp_match_node_affinity.restype = C.c_int
+    L.gp_match_node_affinity.argtypes = [C.c_void_p, C.POINTER(gp_node_labels), C.POINTER(gp_node_affinities), C.POINTER(gp_affinity_match)]
+    L.gp_exceeds_cluster_capacity_affinity.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_affinity.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.POINTER(gp_node_labels),
+                                                       C.POINTER(gp_node_affinities), C.POINTER(gp_apps), C.c_int, C.c_void_p,
+                                                       C.c_void_p]
     L.gp_reconcile_find_nodes.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_reconcile_nodes), C.POINTER(gp_apps),
                                           C.POINTER(gp_reconcile_results)]
     L.gp_pack_one.restype = C.c_int
@@ -372,6 +396,25 @@ def _az_orders(exec_order, drv_order, n_zones):
     eo, do = _np(exec_order, np.int32), _np(drv_order, np.int32)
     o = gp_az_orders(n_zones=int(n_zones), n_exec=len(eo), exec_order=_p(eo), n_drv=len(do), drv_order=_p(do))
     return C.byref(o), (o, eo, do)
+
+
+_LABEL_COLS = {"label_off": np.int64, "label_key": np.int32, "label_val": np.int32, "label_int_ok": np.uint8, "label_int": np.int64}
+_AFF_COLS = {"sel_off": np.int64, "sel_key": np.int32, "sel_val": np.int32, "has_required": np.uint8, "term_off": np.int64,
+             "term_req_off": np.int64, "term_parse_error": np.uint8, "req_op": np.int32, "req_key": np.int32, "req_int": np.int64,
+             "req_val_off": np.int64, "req_val": np.int32}
+
+
+def _affinity_input(enc: dict):
+    """(gp_node_labels, gp_node_affinities) over the arrays of affinity.encode() (or the same keys given by hand; a missing
+    optional column is NULL).  The structs keep their arrays alive."""
+    lc = {k: _np(enc.get(k), t) for k, t in _LABEL_COLS.items()}
+    ac = {k: _np(enc.get(k), t) for k, t in _AFF_COLS.items()}
+    n = int(enc["n_nodes"]) if "n_nodes" in enc else len(lc["label_off"]) - 1
+    lab = gp_node_labels(n_nodes=n, n_keys=int(enc["n_keys"]), n_values=int(enc["n_values"]), **{k: _p(v) for k, v in lc.items()})
+    n_aff = int(enc["n_aff"]) if "n_aff" in enc else len(ac["sel_off"]) - 1
+    aff = gp_node_affinities(n_aff=n_aff, **{k: _p(v) for k, v in ac.items()})
+    lab._keep, aff._keep = lc, ac
+    return lab, aff
 
 
 def compact_apps(apps: dict, mem_shift: int = 20):
@@ -750,6 +793,39 @@ class GangPacker:
         out = np.full(max(q, 1), 255, np.uint8)
         self._check(load().gp_exceeds_cluster_capacity(self._h, C.byref(nd), C.byref(a), int(packer), _p(out)))
         return out[:q]
+
+    def match_node_affinity(self, enc: dict):
+        """GetRequiredNodeAffinity(...).Match for every (affinity, node) of an affinity.encode() result, in one device call
+        (gp_match_node_affinity).  -> (member uint32[n_aff][ceil(n / 32)], n_match int32[n_aff], n_error int32[n_aff]);
+        a non-zero n_error is ListWithPredicate's error (the Predicate's failureInternal)."""
+        lab, aff = _affinity_input(enc)
+        words = (lab.n_nodes + 31) // 32
+        member = np.zeros((max(aff.n_aff, 1), max(words, 1)), np.uint32)
+        n_match = np.zeros(max(aff.n_aff, 1), np.int32)
+        n_error = np.zeros(max(aff.n_aff, 1), np.int32)
+        out = gp_affinity_match(member=_p(member), n_match=_p(n_match), n_error=_p(n_error))
+        self._check(load().gp_match_node_affinity(self._h, C.byref(lab), C.byref(aff), C.byref(out)))
+        return member[:aff.n_aff, :words], n_match[:aff.n_aff], n_error[:aff.n_aff]
+
+    def exceeds_cluster_capacity_affinity(self, alloc, enc: dict, apps: dict, packer: int, overhead=None, zone_id=None, n_zones=1):
+        """exceeds_cluster_capacity with each driver's node set = the nodes its required affinity matches
+        (gp_exceeds_cluster_capacity_affinity): enc from affinity.encode(); apps["group"] = the driver's affinity id.
+        -> (exceeds uint8[n_apps], affinity_error uint8[n_apps]); exceeds[i] is undefined where affinity_error[i] = 1."""
+        q = len(apps["count"])
+        al = [_np(v, np.int64) for v in alloc]
+        ov = [_np(v, np.int64) for v in overhead] if overhead is not None else [None, None, None]
+        zid = _np(zone_id, np.int32)
+        nd = gp_capacity_nodes(n_nodes=len(al[0]), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]),
+                               alloc_gpu=_p(al[2] if len(al) > 2 else None), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]),
+                               overhead_gpu=_p(ov[2] if len(ov) > 2 else None), n_zones=int(n_zones), zone_id=_p(zid),
+                               n_groups=0, node_group=None)
+        lab, aff = _affinity_input(enc)
+        a = _apps(apps, None, group=apps.get("group"))
+        out = np.full(max(q, 1), 255, np.uint8)
+        err = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity_affinity(self._h, C.byref(nd), C.byref(lab), C.byref(aff), C.byref(a),
+                                                                int(packer), _p(out), _p(err)))
+        return out[:q], err[:q]
 
     def reconcile_find_nodes(self, alloc, overhead, res_node, res, node_group, creation, apps: dict, n_groups: int,
                              unschedulable=None, ready=None, exec_cap=None, want_avail=True):
