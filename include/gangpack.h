@@ -700,6 +700,67 @@ gp_status gp_reconcile_find_nodes(gp_ctx* ctx, const gp_usage_input* usage, cons
                                                           drv_* and skip_if_no_fit ignored; call order = processing order */,
                                   gp_reconcile_results* out);
 
+/* ---- node overhead (EXT/overhead.go) ---------------------------------------------------------------------------------------
+ * OverheadComputer.getOverheadByNode (overhead.go:105-153) for a list of nodes, in one call: GetOverhead and
+ * GetNonSchedulableOverhead together.  The event side stays with the caller: one record slot per pod the informer added
+ * (addPodRequests, :163-174: spec.nodeName set, podToResources at that event -- containers summed, then a per-dimension max
+ * with each init container), removed by deletePodRequests (:176-193).  Per call, for each recorded pod on a listed node:
+ *   1. listed = 0 (the pod lister has no pod of the record's namespace/name): skipped (:131-138).  Everything below reads the
+ *      lister's CURRENT pod.
+ *   2. PodHasReservation (EXT/resourcereservations.go:115-132): false without a spark-app-id label; true when the
+ *      ResourceReservation (namespace, appID) exists and lists the pod's name in Status.Pods; else true when spark-role is
+ *      "executor" and the soft store's entry for appID (keyed by appID alone, no namespace) has the pod's name as a key.
+ *   3. no reservation: the requests go to overhead[node] and, unless spec.schedulerName is "spark-scheduler", to
+ *      nonsched[node]; a spark-scheduler pod whose application has a ResourceReservation is one the reference logs a
+ *      warning for (:140-145), counted in n_warned.
+ *   4. a listed node without recorded pods gets zero; records on nodes outside the list are ignored.
+ * A node's value does not depend on which other nodes are listed.  Strings never cross the boundary: the caller interns node
+ * names, (namespace, spark-app-id) pairs, spark-app-ids and pod names to dense ids. */
+typedef struct {
+    int64_t n_pods;                  /* record slots, < 2^31; a free slot has node_id = -1 and is ignored entirely */
+    int32_t n_node_ids, n_app_keys, n_app_ids, n_names;
+    const int32_t* node_id;          /* [n_pods] interned spec.nodeName at the add event, -1 = free slot */
+    const int64_t* req_cpu_milli;    /* [n_pods] podToResources at the add event: >= 0, < 2^61 */
+    const int64_t* req_mem_bytes;
+    const int64_t* req_gpu;          /* or NULL (= 0) */
+    const uint8_t* listed;           /* [n_pods] the lister holds a pod of this namespace/name; or NULL (= all).  The fields
+                                        below describe that pod and are ignored where listed = 0 */
+    const int32_t* app_key;          /* [n_pods] interned (namespace, spark-app-id), -1 = no spark-app-id label */
+    const int32_t* app_id;           /* [n_pods] interned spark-app-id, -1 exactly where app_key is -1 */
+    const int32_t* name_id;          /* [n_pods] interned pod name */
+    const uint8_t* is_executor;      /* [n_pods] spark-role == "executor"; or NULL (= none) */
+    const uint8_t* spark_scheduler;  /* [n_pods] spec.schedulerName == "spark-scheduler"; or NULL (= none) */
+} gp_overhead_pods;
+typedef struct {
+    int32_t n_rr;                    /* ResourceReservations: distinct rr_app_key, each with its Status.Pods values */
+    int32_t n_soft;                  /* soft-store entries: distinct soft_app_id, each with its Reservations keys */
+    const int32_t* rr_app_key;       /* [n_rr] */
+    const int64_t* rr_pod_off;       /* [n_rr + 1] CSR, starts at 0, non-decreasing */
+    const int32_t* rr_pod_name;      /* name ids */
+    const int32_t* soft_app_id;      /* [n_soft] */
+    const int64_t* soft_pod_off;     /* [n_soft + 1] */
+    const int32_t* soft_pod_name;
+} gp_overhead_reservations;
+typedef struct {
+    int64_t* overhead_cpu_milli;     /* [n_nodes] GetOverhead, or NULL */
+    int64_t* overhead_mem_bytes;
+    int64_t* overhead_gpu;
+    int64_t* nonsched_cpu_milli;     /* [n_nodes] GetNonSchedulableOverhead, or NULL */
+    int64_t* nonsched_mem_bytes;
+    int64_t* nonsched_gpu;
+    uint8_t* has_reservation;        /* [n_pods] PodHasReservation of every listed record (0 for free and unlisted slots), or NULL */
+    int64_t* n_warned;               /* pods on listed nodes counted by step 3's warning, or NULL */
+} gp_overhead_out;
+/* The outputs are in the order of node_ids (the caller's node table) and can be passed unchanged as gp_usage_input.overhead_*
+ * or gp_capacity_nodes.overhead_*.  The context is left alone (snapshot, SchedulableResources, zone layout, held az-aware
+ * orders, gp_last_stats); scratch of its own, one stream synchronise.
+ * GP_ERR_INVALID (gp_last_error names the cause): missing arrays or negative sizes; a node, app-key, app-id or name id out of
+ * range; app_key and app_id disagreeing on -1; a node id listed twice in node_ids, or an rr_app_key / soft_app_id given twice;
+ * CSR offsets that do not start at 0 or decrease; a negative request.  GP_ERR_UNREPRESENTABLE: a request >= 2^61 or a
+ * per-node sum >= 2^61 (the whole call is refused, nothing wraps).  On an error the outputs are undefined. */
+gp_status gp_node_overhead(gp_ctx* ctx, const gp_overhead_pods* pods, const gp_overhead_reservations* rsv, int32_t n_nodes,
+                           const int32_t* node_ids /* [n_nodes] the listed nodes, in node-table order */, gp_overhead_out* out);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

@@ -15,6 +15,7 @@
 #include "gangpack_affinity.cuh"
 #include "gangpack_capacity.cuh"
 #include "gangpack_reconcile.cuh"
+#include "gangpack_overhead.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -537,6 +538,7 @@ struct gp_ctx {
     DevBuf reschedprep;                           // gp_reschedule_from_reservations' own scratch (no state points into it)
     DevBuf capprep;                               // gp_exceeds_cluster_capacity's own scratch (no state points into it)
     DevBuf reconbuf;                              // gp_reconcile_find_nodes' own scratch (no state points into it)
+    DevBuf overbuf;                               // gp_node_overhead's own scratch (no state points into it)
     int zone_kind = -1;
     gp_az_orders zone_orders{};
     bool sort_attr_set = false;
@@ -3142,6 +3144,109 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
         if (outs[d]) GP_CUDA(c, cudaMemcpyAsync(outs[d], d_avail + N * (size_t)d, 8 * N, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
     if (herr & kRcErrDomain) return bad(GP_ERR_UNREPRESENTABLE, "an availability the loop charged lies outside the exact-int64 domain (|v| >= 2^61)");
+    return GP_OK;
+}
+
+// The overhead computer's per-call side (EXT/overhead.go:105-153) for a list of nodes; see gangpack_overhead.cuh
+gp_status gp_node_overhead(gp_ctx* c, const gp_overhead_pods* p, const gp_overhead_reservations* r, int32_t n_nodes,
+                           const int32_t* node_ids, gp_overhead_out* out) {
+    if (!c) return GP_ERR_INVALID;
+    static const char* who = "gp_node_overhead";
+    auto bad = [&](gp_status st, const char* what) { return fail(c, st, std::string(who) + ": " + what); };
+    if (!p || !r || !out || p->n_pods < 0 || p->n_node_ids < 0 || p->n_app_keys < 0 || p->n_app_ids < 0 || p->n_names < 0 ||
+        r->n_rr < 0 || r->n_soft < 0 || n_nodes < 0 || (n_nodes > 0 && !node_ids) ||
+        (p->n_pods > 0 && (!p->node_id || !p->req_cpu_milli || !p->req_mem_bytes || !p->app_key || !p->app_id || !p->name_id)) ||
+        (r->n_rr > 0 && (!r->rr_app_key || !r->rr_pod_off)) || (r->n_soft > 0 && (!r->soft_app_id || !r->soft_pod_off)))
+        return bad(GP_ERR_INVALID, "missing arrays or negative sizes");
+    if (p->n_pods > INT32_MAX) return bad(GP_ERR_INVALID, "n_pods must be below 2^31");
+    // CSR offsets (one per reservation: host-sized); the entries themselves are checked on the device
+    auto entries = [](const int64_t* off, int32_t n, int64_t* total) {
+        if (n == 0) { *total = 0; return !off || off[0] == 0; }
+        if (off[0] != 0) return false;
+        for (int32_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
+        *total = off[n];
+        return true;
+    };
+    int64_t er = 0, es = 0;
+    if (!entries(r->rr_pod_off, r->n_rr, &er) || !entries(r->soft_pod_off, r->n_soft, &es))
+        return bad(GP_ERR_INVALID, "rr_pod_off or soft_pod_off does not start at 0 or decreases");
+    if ((er > 0 && !r->rr_pod_name) || (es > 0 && !r->soft_pod_name)) return bad(GP_ERR_INVALID, "missing arrays or negative sizes");
+    if (er + es > ((int64_t)1 << 30)) return bad(GP_ERR_INVALID, "more than 2^30 reservation entries");
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    const size_t P = (size_t)p->n_pods, N = (size_t)n_nodes, R = (size_t)r->n_rr, S = (size_t)r->n_soft;
+    size_t H = 64;
+    while (H < 2 * (size_t)(er + es)) H <<= 1;           // at most half full: every probe ends
+    Arena ar{c->overbuf};
+    const size_t o_node = ar.take(4 * P), o_req = ar.take(24 * P), o_listed = ar.take(P), o_ak = ar.take(4 * P), o_ai = ar.take(4 * P),
+                 o_name = ar.take(4 * P), o_exe = ar.take(P), o_spark = ar.take(P), o_has = ar.take(P),
+                 o_rkey = ar.take(4 * R), o_roff = ar.take(8 * (R + 1)), o_rname = ar.take(4 * (size_t)er),
+                 o_skey = ar.take(4 * S), o_soff = ar.take(8 * (S + 1)), o_sname = ar.take(4 * (size_t)es), o_qn = ar.take(4 * N),
+                 o_rok = ar.take(4 * (size_t)p->n_app_keys), o_soa = ar.take(4 * (size_t)p->n_app_ids),
+                 o_ron = ar.take(4 * (size_t)p->n_node_ids), o_set = ar.take(8 * H),
+                 o_acc = ar.take(96 * N), o_word = ar.take(16), o_out = ar.take(48 * N);
+    GP_CUDA(c, ar.reserve());
+    char* b = ar.base();
+    // the directories and the hash set start at -1 / empty; the sums, n_warned and the error word at 0
+    GP_CUDA(c, cudaMemsetAsync(b + o_rok, 0xff, o_set + 8 * H - o_rok, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_acc, 0, o_word + 16 - o_acc, st));
+    struct Piece { size_t o; const void* src; size_t bytes; };
+    const Piece pieces[] = {
+        {o_node, p->node_id, 4 * P}, {o_req, p->req_cpu_milli, 8 * P}, {o_req + 8 * P, p->req_mem_bytes, 8 * P},
+        {o_req + 16 * P, p->req_gpu, 8 * P}, {o_listed, p->listed, P}, {o_ak, p->app_key, 4 * P}, {o_ai, p->app_id, 4 * P},
+        {o_name, p->name_id, 4 * P}, {o_exe, p->is_executor, P}, {o_spark, p->spark_scheduler, P},
+        {o_rkey, r->rr_app_key, 4 * R}, {o_roff, r->rr_pod_off, R ? 8 * (R + 1) : 0}, {o_rname, r->rr_pod_name, 4 * (size_t)er},
+        {o_skey, r->soft_app_id, 4 * S}, {o_soff, r->soft_pod_off, S ? 8 * (S + 1) : 0}, {o_sname, r->soft_pod_name, 4 * (size_t)es},
+        {o_qn, node_ids, 4 * N}};
+    for (const Piece& pc : pieces)
+        if (pc.src && pc.bytes) GP_CUDA(c, ar.upload(pc.o, pc.src, pc.bytes, st));
+    OhMaps M{(int32_t*)(b + o_rok), (int32_t*)(b + o_soa), (int32_t*)(b + o_ron), (unsigned long long*)(b + o_set), (uint32_t)(H - 1),
+             r->n_rr};
+    int* d_err = (int*)(b + o_word + 8);
+    const int T = 256, cap = c->sm_count * 8;
+    const long long n_dir = (long long)R + (long long)S + (long long)N;
+    if (n_dir > 0) {
+        OhDirIn D{r->n_rr, r->n_soft, n_nodes, p->n_app_keys, p->n_app_ids, p->n_node_ids,
+                  (const int32_t*)(b + o_rkey), (const int32_t*)(b + o_skey), (const int32_t*)(b + o_qn)};
+        gp_oh_dir<<<(unsigned)std::min<long long>((n_dir + T - 1) / T, cap), T, 0, st>>>(D, M, d_err);
+    }
+    if (er + es > 0) {
+        OhSetIn si{(const long long*)(b + o_roff), (const int32_t*)(b + o_rname), (const long long*)(b + o_soff),
+                   (const int32_t*)(b + o_sname), r->n_rr, r->n_soft, p->n_names, (long long)er, (long long)es};
+        gp_oh_insert<<<(unsigned)std::min<long long>((er + es + T - 1) / T, cap), T, 0, st>>>(si, M, d_err);
+    }
+    OhAcc A{(unsigned long long*)(b + o_acc), (unsigned long long*)(b + o_word), n_nodes};
+    if (P > 0) {
+        OhPodsIn pi{};
+        pi.n = (long long)P; pi.n_node_ids = p->n_node_ids; pi.n_app_keys = p->n_app_keys; pi.n_app_ids = p->n_app_ids; pi.n_names = p->n_names;
+        pi.node_id = (const int32_t*)(b + o_node);
+        for (int d = 0; d < 3; ++d) pi.req[d] = (d < 2 || p->req_gpu) ? (const long long*)(b + o_req) + P * (size_t)d : nullptr;
+        pi.listed = p->listed ? (const uint8_t*)(b + o_listed) : nullptr;
+        pi.app_key = (const int32_t*)(b + o_ak); pi.app_id = (const int32_t*)(b + o_ai); pi.name_id = (const int32_t*)(b + o_name);
+        pi.is_executor = p->is_executor ? (const uint8_t*)(b + o_exe) : nullptr;
+        pi.spark_scheduler = p->spark_scheduler ? (const uint8_t*)(b + o_spark) : nullptr;
+        pi.has_reservation = (uint8_t*)(b + o_has);
+        gp_oh_pods<<<(unsigned)((P + kOhThreads - 1) / kOhThreads), kOhThreads, 0, st>>>(pi, M, A, d_err);
+    }
+    long long* d_out = (long long*)(b + o_out);
+    if (N > 0) gp_oh_finish<<<(unsigned)((N + T - 1) / T), T, 0, st>>>(A, d_out, d_err);
+    GP_CUDA(c, cudaGetLastError());
+    int64_t* outs[6] = {out->overhead_cpu_milli, out->overhead_mem_bytes, out->overhead_gpu,
+                        out->nonsched_cpu_milli, out->nonsched_mem_bytes, out->nonsched_gpu};
+    for (int k = 0; k < 6; ++k)
+        if (outs[k] && N) GP_CUDA(c, cudaMemcpyAsync(outs[k], d_out + N * (size_t)k, 8 * N, cudaMemcpyDeviceToHost, st));
+    if (out->has_reservation && P) GP_CUDA(c, cudaMemcpyAsync(out->has_reservation, b + o_has, P, cudaMemcpyDeviceToHost, st));
+    unsigned long long word[2] = {0, 0};                 // n_warned, error bits
+    GP_CUDA(c, cudaMemcpyAsync(word, b + o_word, 16, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    const int herr = (int)word[1];
+    if (herr & kOhErrRange) return bad(GP_ERR_INVALID, "an id out of its range (node, app key, app id, name or query node)");
+    if (herr & kOhErrAppPair) return bad(GP_ERR_INVALID, "app_key and app_id disagree on -1");
+    if (herr & kOhErrDuplicate) return bad(GP_ERR_INVALID, "a query node id, rr_app_key or soft_app_id given twice");
+    if (herr & kOhErrNegative) return bad(GP_ERR_INVALID, "negative request");
+    if (herr & kOhErrRequest) return bad(GP_ERR_UNREPRESENTABLE, "request >= 2^61");
+    if (herr & kOhErrSum) return bad(GP_ERR_UNREPRESENTABLE, "a per-node sum >= 2^61");
+    if (out->n_warned) *out->n_warned = (int64_t)word[0];
     return GP_OK;
 }
 

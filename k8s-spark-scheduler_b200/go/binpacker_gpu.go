@@ -30,10 +30,12 @@ import (
 
 	"github.com/palantir/k8s-spark-scheduler-lib/pkg/binpack"
 	"github.com/palantir/k8s-spark-scheduler-lib/pkg/resources"
+	"github.com/palantir/k8s-spark-scheduler/internal/common"
 	v1 "k8s.io/api/core/v1"
 	"k8s.io/apimachinery/pkg/api/resource"
 	"k8s.io/apimachinery/pkg/labels"
 	"k8s.io/apimachinery/pkg/selection"
+	clientcache "k8s.io/client-go/tools/cache"
 )
 
 // Names under which the GPU packers are registered next to the reference's own entries in
@@ -1629,4 +1631,256 @@ func ReconcileFindNodes(nodes []ReconcileNode, rows []ReconcileRow, overhead res
 		}
 	}
 	return res, true
+}
+
+// ---- the overhead computer (internal/extender/overhead.go) ---------------------------------------------------------------
+
+// OverheadRecords is the event side of the overhead computer kept as record slots for gp_node_overhead: register OnAdd,
+// OnUpdate and OnDelete on the pod informer in place of NewOverheadComputer's handlers.  A slot per (node, UID) -- the
+// reference's ClusterRequests map -- holds the pod's namespace, name and podToResources at its add event; deletes free the
+// slot onto a free list.  Strings are interned once, when a record is written.
+type OverheadRecords struct {
+	mu       sync.Mutex
+	at       map[[2]string]int // (nodeName, UID) -> slot
+	free     []int
+	ns       []string
+	name     []string
+	nodeID   []int32 // -1: free slot
+	req      [3][]int64
+	inexact  []bool // a quantity outside the exact-int64 model (sub-millicore cpu ...): every call falls back while one is held
+	nInexact int
+	nodeIx   map[string]int32
+	nodes    []string
+}
+
+func NewOverheadRecords() *OverheadRecords {
+	return &OverheadRecords{at: map[[2]string]int{}, nodeIx: map[string]int32{}}
+}
+
+func podToResources(pod *v1.Pod) *resources.Resources { // overhead.go:195-209
+	res := resources.Zero()
+	for _, c := range pod.Spec.Containers {
+		res.AddFromResourceList(c.Resources.Requests)
+	}
+	for _, c := range pod.Spec.InitContainers {
+		res.SetMaxResource(c.Resources.Requests)
+	}
+	return res
+}
+
+// OnAdd / OnUpdate / OnDelete: clientcache.FilteringResourceEventHandler{FilterFunc: spec.nodeName != ""} around
+// addPodRequests / deletePodRequests -- the update that binds a pod is an add, the one that unbinds it a delete.
+func (o *OverheadRecords) OnAdd(obj interface{}) {
+	if pod, ok := obj.(*v1.Pod); ok && pod.Spec.NodeName != "" {
+		o.record(pod)
+	}
+}
+
+func (o *OverheadRecords) OnUpdate(oldObj, newObj interface{}) {
+	oldPod, ok1 := oldObj.(*v1.Pod)
+	newPod, ok2 := newObj.(*v1.Pod)
+	if !ok1 || !ok2 {
+		return
+	}
+	if newPod.Spec.NodeName != "" && oldPod.Spec.NodeName == "" {
+		o.record(newPod)
+	} else if newPod.Spec.NodeName == "" && oldPod.Spec.NodeName != "" {
+		o.remove(oldPod)
+	}
+}
+
+func (o *OverheadRecords) OnDelete(obj interface{}) {
+	pod, ok := obj.(*v1.Pod)
+	if !ok {
+		if t, isTomb := obj.(clientcache.DeletedFinalStateUnknown); isTomb {
+			pod, ok = t.Obj.(*v1.Pod)
+		}
+	}
+	if ok && pod.Spec.NodeName != "" {
+		o.remove(pod)
+	}
+}
+
+func (o *OverheadRecords) record(pod *v1.Pod) {
+	o.mu.Lock()
+	defer o.mu.Unlock()
+	key := [2]string{pod.Spec.NodeName, string(pod.UID)}
+	i, ok := o.at[key]
+	if !ok {
+		if n := len(o.free); n > 0 {
+			i, o.free = o.free[n-1], o.free[:n-1]
+		} else {
+			i = len(o.nodeID)
+			o.ns, o.name, o.nodeID, o.inexact = append(o.ns, ""), append(o.name, ""), append(o.nodeID, -1), append(o.inexact, false)
+			for d := range o.req {
+				o.req[d] = append(o.req[d], 0)
+			}
+		}
+		o.at[key] = i
+	}
+	id, known := o.nodeIx[pod.Spec.NodeName]
+	if !known {
+		id = int32(len(o.nodes))
+		o.nodeIx[pod.Spec.NodeName] = id
+		o.nodes = append(o.nodes, pod.Spec.NodeName)
+	}
+	cpu, mem, gpu, exact := toTriple(podToResources(pod))
+	o.setInexact(i, !exact)
+	o.ns[i], o.name[i], o.nodeID[i] = pod.Namespace, pod.Name, id
+	o.req[0][i], o.req[1][i], o.req[2][i] = cpu, mem, gpu
+}
+
+func (o *OverheadRecords) remove(pod *v1.Pod) {
+	o.mu.Lock()
+	defer o.mu.Unlock()
+	key := [2]string{pod.Spec.NodeName, string(pod.UID)}
+	i, ok := o.at[key]
+	if !ok {
+		return
+	}
+	delete(o.at, key)
+	o.setInexact(i, false)
+	o.nodeID[i], o.ns[i], o.name[i] = -1, "", ""
+	o.free = append(o.free, i)
+}
+
+func (o *OverheadRecords) setInexact(i int, v bool) {
+	if o.inexact[i] != v {
+		if v {
+			o.nInexact++
+		} else {
+			o.nInexact--
+		}
+		o.inexact[i] = v
+	}
+}
+
+// OverheadForNodes answers GetOverhead and GetNonSchedulableOverhead for `nodes` from one gp_node_overhead call: the
+// driver and executor Predicates (EXT/resource.go:301, :639), the failover reconciler (failover.go:53) and the
+// unschedulable marker (unschedulablepods.go:150, one call for the whole scan).  getPod is the pod lister's Get; rrPods
+// the ResourceReservation cache as (namespace, appID) -> Status.Pods values; softPods the soft store as appID ->
+// Reservations keys.  ok = false (no device, a record with an inexact quantity, any non-OK status): use the Go
+// OverheadComputer.
+func (o *OverheadRecords) OverheadForNodes(nodes []*v1.Node, getPod func(namespace, name string) (*v1.Pod, bool),
+	rrPods map[[2]string][]string, softPods map[string][]string) (overhead, nonSchedulable resources.NodeGroupResources, warned int64, ok bool) {
+	d, err := getDevice()
+	if err != nil {
+		return nil, nil, 0, false
+	}
+	o.mu.Lock()
+	defer o.mu.Unlock()
+	if o.nInexact > 0 {
+		return nil, nil, 0, false
+	}
+	nodeIx := make(map[string]int32, len(o.nodeIx)+len(nodes)) // the record table's ids, plus listed nodes without records
+	for k, v := range o.nodeIx {
+		nodeIx[k] = v
+	}
+	query := make([]int32, len(nodes)+1)
+	for i, n := range nodes {
+		id, known := nodeIx[n.Name]
+		if !known {
+			id = int32(len(nodeIx))
+			nodeIx[n.Name] = id
+		}
+		query[i] = id
+	}
+	keyIx, appIx, nameIx := map[[2]string]int32{}, map[string]int32{}, map[string]int32{}
+	internName := func(s string) int32 {
+		v, seen := nameIx[s]
+		if !seen {
+			v = int32(len(nameIx))
+			nameIx[s] = v
+		}
+		return v
+	}
+	rrKey, rrName, rrOff := []int32{}, []int32{}, []int64{0}
+	for k, names := range rrPods {
+		keyIx[k] = int32(len(keyIx))
+		rrKey = append(rrKey, keyIx[k])
+		for _, s := range names {
+			rrName = append(rrName, internName(s))
+		}
+		rrOff = append(rrOff, int64(len(rrName)))
+	}
+	softApp, softName, softOff := []int32{}, []int32{}, []int64{0}
+	for app, names := range softPods {
+		appIx[app] = int32(len(appIx))
+		softApp = append(softApp, appIx[app])
+		for _, s := range names {
+			softName = append(softName, internName(s))
+		}
+		softOff = append(softOff, int64(len(softName)))
+	}
+	p := len(o.nodeID)
+	listed, exe, spark := make([]uint8, p+1), make([]uint8, p+1), make([]uint8, p+1)
+	ak, ai, nm := make([]int32, p+1), make([]int32, p+1), make([]int32, p+1)
+	for i := 0; i < p; i++ {
+		ak[i], ai[i] = -1, -1
+		if o.nodeID[i] < 0 {
+			continue
+		}
+		pod, found := getPod(o.ns[i], o.name[i])
+		if !found {
+			continue // overhead.go:131-138
+		}
+		listed[i] = 1
+		if app, has := pod.Labels[common.SparkAppIDLabel]; has {
+			k := [2]string{pod.Namespace, app}
+			if _, seen := keyIx[k]; !seen {
+				keyIx[k] = int32(len(keyIx))
+			}
+			if _, seen := appIx[app]; !seen {
+				appIx[app] = int32(len(appIx))
+			}
+			ak[i], ai[i] = keyIx[k], appIx[app]
+		}
+		nm[i] = internName(pod.Name)
+		if pod.Labels[common.SparkRoleLabel] == common.Executor {
+			exe[i] = 1
+		}
+		if pod.Spec.SchedulerName == common.SparkSchedulerName {
+			spark[i] = 1
+		}
+	}
+	rrKey, rrName, softApp, softName = append(rrKey, 0), append(rrName, 0), append(softApp, 0), append(softName, 0) // non-empty bases
+	nodeID := append(o.nodeID, -1)
+	req := [3][]int64{append(o.req[0], 0), append(o.req[1], 0), append(o.req[2], 0)}
+	n := len(nodes)
+	outs := make([][]int64, 6)
+	for k := range outs {
+		outs[k] = make([]int64, n+1)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	d.mu.Lock()
+	defer d.mu.Unlock()
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, x := range []any{&nodeID[0], &listed[0], &exe[0], &spark[0], &ak[0], &ai[0], &nm[0], &query[0], &rrKey[0], &rrName[0],
+		&rrOff[0], &softApp[0], &softName[0], &softOff[0], &req[0][0], &req[1][0], &req[2][0], &warned} {
+		pin.Pin(x)
+	}
+	for k := range outs {
+		pin.Pin(&outs[k][0])
+	}
+	pods := C.gp_overhead_pods{n_pods: C.int64_t(p), n_node_ids: C.int32_t(len(nodeIx)), n_app_keys: C.int32_t(len(keyIx)),
+		n_app_ids: C.int32_t(len(appIx)), n_names: C.int32_t(len(nameIx)), node_id: ptr32(nodeID), req_cpu_milli: ptr64(req[0]),
+		req_mem_bytes: ptr64(req[1]), req_gpu: ptr64(req[2]), listed: ptr8(listed), app_key: ptr32(ak), app_id: ptr32(ai),
+		name_id: ptr32(nm), is_executor: ptr8(exe), spark_scheduler: ptr8(spark)}
+	rsv := C.gp_overhead_reservations{n_rr: C.int32_t(len(rrOff) - 1), n_soft: C.int32_t(len(softOff) - 1),
+		rr_app_key: ptr32(rrKey), rr_pod_off: ptr64(rrOff), rr_pod_name: ptr32(rrName),
+		soft_app_id: ptr32(softApp), soft_pod_off: ptr64(softOff), soft_pod_name: ptr32(softName)}
+	out := C.gp_overhead_out{overhead_cpu_milli: ptr64(outs[0]), overhead_mem_bytes: ptr64(outs[1]), overhead_gpu: ptr64(outs[2]),
+		nonsched_cpu_milli: ptr64(outs[3]), nonsched_mem_bytes: ptr64(outs[4]), nonsched_gpu: ptr64(outs[5]),
+		n_warned: (*C.int64_t)(unsafe.Pointer(&warned))}
+	if C.gp_node_overhead(d.ctx, &pods, &rsv, C.int32_t(n), ptr32(query), &out) != C.GP_OK {
+		return nil, nil, 0, false
+	}
+	overhead, nonSchedulable = resources.NodeGroupResources{}, resources.NodeGroupResources{}
+	for i, node := range nodes {
+		overhead[node.Name] = resources.CreateResources(outs[0][i], outs[1][i], outs[2][i])
+		nonSchedulable[node.Name] = resources.CreateResources(outs[3][i], outs[4][i], outs[5][i])
+	}
+	return overhead, nonSchedulable, warned, true
 }

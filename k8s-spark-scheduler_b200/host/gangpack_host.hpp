@@ -1449,4 +1449,138 @@ inline std::vector<ReconcileResult> ReconcileFindNodes(const std::vector<Reconci
     return res;
 }
 
+// The overhead computer (internal/extender/overhead.go): the event side on the host, the per-call side in one
+// gp_node_overhead call.  Only the fields the computer reads are kept.
+struct Container { resources::Resources Requests; };  // cpu, memory and nvidia.com/gpu of Resources.Requests
+struct Pod {
+    std::string UID, Namespace, Name, NodeName, SchedulerName;
+    std::map<std::string, std::string> Labels;
+    std::vector<Container> Containers, InitContainers;
+};
+
+// podToResources (overhead.go:195-209): the containers summed, then a per-dimension max with each init container
+inline resources::Resources PodToResources(const Pod& pod) {
+    resources::Resources r;
+    for (const Container& c : pod.Containers) r.Add(c.Requests);
+    for (const Container& c : pod.InitContainers) {
+        r.CPU = std::max(r.CPU, c.Requests.CPU);
+        r.Memory = std::max(r.Memory, c.Requests.Memory);
+        r.NvidiaGPU = std::max(r.NvidiaGPU, c.Requests.NvidiaGPU);
+    }
+    return r;
+}
+
+// The lister and reservation views the per-call side reads: the pod lister by (namespace, name), the ResourceReservation
+// cache by (namespace, appID) with its Status.Pods values, the soft store by appID with its Reservations keys.
+struct OverheadView {
+    std::map<std::pair<std::string, std::string>, Pod> Pods;
+    std::map<std::pair<std::string, std::string>, std::vector<std::string>> ResourceReservations;
+    std::map<std::string, std::vector<std::string>> SoftReservations;
+};
+
+class OverheadComputer {
+public:
+    // FilteringResourceEventHandler{podHasNodeName}: an add of a bound pod, the update that binds a pod, and the update that
+    // unbinds one (a delete) change the records; other updates change nothing
+    void AddPod(const Pod& p) { if (!p.NodeName.empty()) record(p); }
+    void UpdatePod(const Pod& oldPod, const Pod& newPod) {
+        if (!newPod.NodeName.empty() && oldPod.NodeName.empty()) record(newPod);
+        else if (newPod.NodeName.empty() && !oldPod.NodeName.empty()) remove(oldPod);
+    }
+    void DeletePod(const Pod& p) { if (!p.NodeName.empty()) remove(p); }
+
+    resources::NodeGroupResources GetOverhead(const OverheadView& v, const std::vector<std::string>& nodes) const {
+        return compute(v, nodes).first;
+    }
+    resources::NodeGroupResources GetNonSchedulableOverhead(const OverheadView& v, const std::vector<std::string>& nodes) const {
+        return compute(v, nodes).second;
+    }
+    // getOverheadByNode (overhead.go:105-117): both maps from one device call; *warned = pods the reference logs a warning for
+    std::pair<resources::NodeGroupResources, resources::NodeGroupResources> compute(const OverheadView& v, const std::vector<std::string>& nodes,
+                                                                                    int64_t* warned = nullptr) const {
+        std::map<std::string, int32_t> nodeIx, keyIx, appIx, nameIx;
+        auto id = [](std::map<std::string, int32_t>& m, const std::string& s) { return m.emplace(s, (int32_t)m.size()).first->second; };
+        auto key = [](const std::string& ns, const std::string& app) { return ns + '\x00' + app; };
+        std::vector<int32_t> query;
+        for (const auto& n : nodes) query.push_back(id(nodeIx, n));
+        std::vector<int32_t> rrKey, rrName, softApp, softName;
+        std::vector<int64_t> rrOff{0}, softOff{0};
+        for (const auto& kv : v.ResourceReservations) {
+            rrKey.push_back(id(keyIx, key(kv.first.first, kv.first.second)));
+            for (const auto& s : kv.second) rrName.push_back(id(nameIx, s));
+            rrOff.push_back((int64_t)rrName.size());
+        }
+        for (const auto& kv : v.SoftReservations) {
+            softApp.push_back(id(appIx, kv.first));
+            for (const auto& s : kv.second) softName.push_back(id(nameIx, s));
+            softOff.push_back((int64_t)softName.size());
+        }
+        const size_t P = slots_.size();
+        std::vector<int32_t> node(P, -1), ak(P, -1), ai(P, -1), nm(P, 0);
+        std::vector<int64_t> cpu(P), mem(P), gpu(P);
+        std::vector<uint8_t> listed(P), exe(P), spark(P);
+        for (size_t i = 0; i < P; ++i) {
+            const Slot& s = slots_[i];
+            if (!s.used) continue;
+            node[i] = id(nodeIx, s.node);
+            cpu[i] = s.requests.CPU; mem[i] = s.requests.Memory; gpu[i] = s.requests.NvidiaGPU;
+            auto it = v.Pods.find({s.ns, s.name});
+            if (it == v.Pods.end()) continue;
+            const Pod& pod = it->second;
+            listed[i] = 1;
+            auto app = pod.Labels.find("spark-app-id");
+            if (app != pod.Labels.end()) { ak[i] = id(keyIx, key(pod.Namespace, app->second)); ai[i] = id(appIx, app->second); }
+            nm[i] = id(nameIx, pod.Name);
+            auto role = pod.Labels.find("spark-role");
+            exe[i] = role != pod.Labels.end() && role->second == "executor";
+            spark[i] = pod.SchedulerName == "spark-scheduler";
+        }
+        gp_overhead_pods in{};
+        in.n_pods = (int64_t)P; in.n_node_ids = (int32_t)nodeIx.size(); in.n_app_keys = (int32_t)keyIx.size();
+        in.n_app_ids = (int32_t)appIx.size(); in.n_names = (int32_t)nameIx.size();
+        in.node_id = node.data(); in.req_cpu_milli = cpu.data(); in.req_mem_bytes = mem.data(); in.req_gpu = gpu.data();
+        in.listed = listed.data(); in.app_key = ak.data(); in.app_id = ai.data(); in.name_id = nm.data();
+        in.is_executor = exe.data(); in.spark_scheduler = spark.data();
+        gp_overhead_reservations rsv{};
+        rsv.n_rr = (int32_t)rrKey.size(); rsv.n_soft = (int32_t)softApp.size();
+        rsv.rr_app_key = rrKey.data(); rsv.rr_pod_off = rrOff.data(); rsv.rr_pod_name = rrName.data();
+        rsv.soft_app_id = softApp.data(); rsv.soft_pod_off = softOff.data(); rsv.soft_pod_name = softName.data();
+        const size_t N = nodes.size();
+        std::vector<int64_t> o(6 * std::max<size_t>(N, 1));
+        int64_t nw = 0;
+        gp_overhead_out out{o.data(), o.data() + N, o.data() + 2 * N, o.data() + 3 * N, o.data() + 4 * N, o.data() + 5 * N, nullptr, &nw};
+        gangpack::Device& dev = gangpack::Device::Get();
+        dev.check(gp_node_overhead(dev.ctx(), &in, &rsv, (int32_t)N, query.data(), &out), "gp_node_overhead");
+        std::pair<resources::NodeGroupResources, resources::NodeGroupResources> res;
+        for (size_t i = 0; i < N; ++i) {
+            res.first[nodes[i]] = resources::CreateResources(o[i], o[N + i], o[2 * N + i]);
+            res.second[nodes[i]] = resources::CreateResources(o[3 * N + i], o[4 * N + i], o[5 * N + i]);
+        }
+        if (warned) *warned = nw;
+        return res;
+    }
+
+private:
+    struct Slot { bool used = false; std::string ns, name, node; resources::Resources requests; };
+    void record(const Pod& p) {                            // addPodRequests (overhead.go:163-174)
+        auto k = std::make_pair(p.NodeName, p.UID);
+        auto it = at_.find(k);
+        size_t i;
+        if (it != at_.end()) i = it->second;
+        else if (!free_.empty()) { i = free_.back(); free_.pop_back(); at_.emplace(k, i); }
+        else { i = slots_.size(); slots_.emplace_back(); at_.emplace(k, i); }
+        slots_[i] = Slot{true, p.Namespace, p.Name, p.NodeName, PodToResources(p)};
+    }
+    void remove(const Pod& p) {                            // deletePodRequests (:176-193)
+        auto it = at_.find({p.NodeName, p.UID});
+        if (it == at_.end()) return;
+        slots_[it->second] = Slot{};
+        free_.push_back(it->second);
+        at_.erase(it);
+    }
+    std::vector<Slot> slots_;
+    std::vector<size_t> free_;
+    std::map<std::pair<std::string, std::string>, size_t> at_;   // (node, UID) -> slot: the reference's ClusterRequests
+};
+
 }  // namespace extender

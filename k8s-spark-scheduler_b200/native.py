@@ -19,7 +19,7 @@ _SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack
                                                     "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
                                                     "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
                                                     "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh", "gangpack_capacity.cuh",
-                                                    "gangpack_affinity.cuh",
+                                                    "gangpack_affinity.cuh", "gangpack_overhead.cuh",
                                                     "gangpack_reconcile.cuh")] + [
     os.path.join(_ROOT, "include", "gangpack.h")]
 
@@ -43,6 +43,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
+           "gp_node_overhead",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -204,6 +205,24 @@ class gp_reconcile_results(C.Structure):
                 ("avail_cpu_milli", C.c_void_p), ("avail_mem_bytes", C.c_void_p), ("avail_gpu", C.c_void_p)]
 
 
+class gp_overhead_pods(C.Structure):
+    _fields_ = [("n_pods", C.c_int64), ("n_node_ids", C.c_int32), ("n_app_keys", C.c_int32), ("n_app_ids", C.c_int32),
+                ("n_names", C.c_int32), ("node_id", C.c_void_p), ("req_cpu_milli", C.c_void_p), ("req_mem_bytes", C.c_void_p),
+                ("req_gpu", C.c_void_p), ("listed", C.c_void_p), ("app_key", C.c_void_p), ("app_id", C.c_void_p),
+                ("name_id", C.c_void_p), ("is_executor", C.c_void_p), ("spark_scheduler", C.c_void_p)]
+
+
+class gp_overhead_reservations(C.Structure):
+    _fields_ = [("n_rr", C.c_int32), ("n_soft", C.c_int32), ("rr_app_key", C.c_void_p), ("rr_pod_off", C.c_void_p),
+                ("rr_pod_name", C.c_void_p), ("soft_app_id", C.c_void_p), ("soft_pod_off", C.c_void_p), ("soft_pod_name", C.c_void_p)]
+
+
+class gp_overhead_out(C.Structure):
+    _fields_ = [("overhead_cpu_milli", C.c_void_p), ("overhead_mem_bytes", C.c_void_p), ("overhead_gpu", C.c_void_p),
+                ("nonsched_cpu_milli", C.c_void_p), ("nonsched_mem_bytes", C.c_void_p), ("nonsched_gpu", C.c_void_p),
+                ("has_reservation", C.c_void_p), ("n_warned", C.c_void_p)]
+
+
 class gp_stats(C.Structure):
     _fields_ = [("nodes_scanned", C.c_int64), ("drivers_tried", C.c_int64), ("kernel_launches", C.c_int64),
                 ("pack_kernel_ns", C.c_int64), ("prep_kernel_ns", C.c_int64), ("scan_path_apps", C.c_int64),
@@ -274,6 +293,9 @@ def load():
                                                        C.c_void_p]
     L.gp_reconcile_find_nodes.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_reconcile_nodes), C.POINTER(gp_apps),
                                           C.POINTER(gp_reconcile_results)]
+    L.gp_node_overhead.restype = C.c_int
+    L.gp_node_overhead.argtypes = [C.c_void_p, C.POINTER(gp_overhead_pods), C.POINTER(gp_overhead_reservations), C.c_int32,
+                                   C.c_void_p, C.POINTER(gp_overhead_out)]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -402,6 +424,12 @@ _LABEL_COLS = {"label_off": np.int64, "label_key": np.int32, "label_val": np.int
 _AFF_COLS = {"sel_off": np.int64, "sel_key": np.int32, "sel_val": np.int32, "has_required": np.uint8, "term_off": np.int64,
              "term_req_off": np.int64, "term_parse_error": np.uint8, "req_op": np.int32, "req_key": np.int32, "req_int": np.int64,
              "req_val_off": np.int64, "req_val": np.int32}
+
+
+_OVERHEAD_COLS = {"node_id": np.int32, "req_cpu_milli": np.int64, "req_mem_bytes": np.int64, "req_gpu": np.int64, "listed": np.uint8,
+                  "app_key": np.int32, "app_id": np.int32, "name_id": np.int32, "is_executor": np.uint8, "spark_scheduler": np.uint8,
+                  "rr_app_key": np.int32, "rr_pod_off": np.int64, "rr_pod_name": np.int32, "soft_app_id": np.int32,
+                  "soft_pod_off": np.int64, "soft_pod_name": np.int32, "node_ids": np.int32}
 
 
 def _affinity_input(enc: dict):
@@ -853,6 +881,29 @@ class GangPacker:
                                  avail_cpu_milli=_p(av[0]), avail_mem_bytes=_p(av[1]), avail_gpu=_p(av[2]))
         self._check(load().gp_reconcile_find_nodes(self._h, C.byref(ui), C.byref(nd), C.byref(a), C.byref(r)))
         return placed[:q], execn[:int(off[q])], off, (tuple(x[:n] for x in av) if want_avail else None)
+
+    def node_overhead(self, enc: dict):
+        """GetOverhead and GetNonSchedulableOverhead for the listed nodes in one device call (gp_node_overhead), over an
+        overhead.encode() result (or the same keys given by hand; a missing optional column is NULL).
+        -> (overhead (cpu, mem, gpu), nonsched (cpu, mem, gpu), has_reservation uint8[n_pods], n_warned): the triples in
+        enc["node_ids"] order, as build_availability, prepare_cluster, exceeds_cluster_capacity and reconcile_find_nodes
+        take them.  Leaves the context's snapshot and statistics untouched."""
+        col = {k: _np(enc.get(k), t) for k, t in _OVERHEAD_COLS.items()}
+        n_pods = int(enc["n_pods"]) if "n_pods" in enc else len(col["node_id"])
+        pods = gp_overhead_pods(n_pods=n_pods, n_node_ids=int(enc["n_node_ids"]), n_app_keys=int(enc["n_app_keys"]),
+                                n_app_ids=int(enc["n_app_ids"]), n_names=int(enc["n_names"]),
+                                **{k: _p(col[k]) for k in _OVERHEAD_COLS if k in gp_overhead_pods.__dict__})
+        rsv = gp_overhead_reservations(n_rr=int(enc["n_rr"]) if "n_rr" in enc else len(col["rr_app_key"]),
+                                       n_soft=int(enc["n_soft"]) if "n_soft" in enc else len(col["soft_app_id"]),
+                                       **{k: _p(col[k]) for k in _OVERHEAD_COLS if k in gp_overhead_reservations.__dict__})
+        qn = col["node_ids"]
+        n = 0 if qn is None else len(qn)
+        res = [np.zeros(max(n, 1), np.int64) for _ in range(6)]
+        has = np.zeros(max(n_pods, 1), np.uint8)
+        warned = C.c_int64(-1)
+        out = gp_overhead_out(*[_p(x) for x in res], _p(has), C.addressof(warned))
+        self._check(load().gp_node_overhead(self._h, C.byref(pods), C.byref(rsv), n, _p(qn), C.byref(out)))
+        return tuple(x[:n] for x in res[:3]), tuple(x[:n] for x in res[3:]), has[:n_pods], warned.value
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
