@@ -1299,6 +1299,17 @@ gp_status gp_last_stats(gp_ctx* c, gp_stats* out) {
     return decode_device_error(c, h.err);
 }
 
+#ifdef GP_DECIDE_TIMELINE
+// Diagnostic build only (not in gangpack.h): copy the phase timeline of the last gp_decide_tables launch on the context's
+// device (gp::TlBuf) into `out`, after the context's stream has finished.  -> the bytes needed; copies only if bytes suffices.
+int64_t gp_decide_timeline(gp_ctx* c, void* out, int64_t bytes) {
+    if (!c) return -1;
+    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -1;
+    if (out && bytes >= (int64_t)sizeof(gp::TlBuf) && cudaMemcpyFromSymbol(out, gp::g_tl, sizeof(gp::TlBuf)) != cudaSuccess) return -1;
+    return (int64_t)sizeof(gp::TlBuf);
+}
+#endif
+
 static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, gp_results_wire* out);
 
 gp_status gp_pack_batch_wire(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, gp_results_wire* out) {

@@ -80,7 +80,7 @@ struct ShapeHeader {
     uint32_t ticket;                  // next work item of gp_decide_tables
     uint32_t cls_done;                // classify tiles finished
     uint32_t tab_done;                // table items finished
-    uint32_t dec_next;                // next 32-application chunk of the decide phase
+    uint32_t dec_next;                // decide chunks claimed past the grid's warp count (the first chunk of a warp is fixed)
 };
 static_assert(sizeof(ShapeHeader) <= 1024, "ShapeHeader");
 
@@ -142,6 +142,11 @@ __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
+__device__ __forceinline__ uint32_t ld_relaxed_u32(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
 __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long* p) {
     unsigned long long v;
     asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
@@ -150,13 +155,50 @@ __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long
 __device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
+// Polling back-off cap (ns) of the phase waits and the look-back.  A waiter notices a completion up to one sleep late,
+// and a phase hand-off is on the critical path of the whole launch; one poller per CTA (per warp in the look-back) keeps
+// the polling traffic small even at this cap.
+constexpr unsigned kPollMaxNs = 128;
 // thread 0 of a CTA: wait until *ctr >= n (acquire: the producers' writes are visible to the whole CTA after the
 // __syncthreads that follows)
 __device__ __forceinline__ void wait_count(const uint32_t* ctr, uint32_t n) {
     unsigned ns = 32;
-    while (ld_acquire_u32(ctr) < n) { __nanosleep(ns); if (ns < 1024) ns <<= 1; }
+    while (ld_acquire_u32(ctr) < n) { __nanosleep(ns); if (ns < kPollMaxNs) ns <<= 1; }
     __threadfence();
 }
+// ---- phase timeline of gp_decide_tables (diagnostic build, -DGP_DECIDE_TIMELINE; tools/decide_timeline.py) ----------
+// Thread 0 of every CTA stamps %globaltimer when it claims a ticket and when the item is counted done, and when its
+// cls_done / tab_done waits return; every warp stamps the start and end of its decide chunks.  Each CTA and warp writes
+// its own slots (no shared counter that would itself serialise), and each launch overwrites the previous one's.  The
+// shipped build compiles none of this.
+#ifdef GP_DECIDE_TIMELINE
+enum TlKind : uint32_t { kTlCls = 0, kTlSeg = 1, kTlFirstFit = 2, kTlClsWait = 3, kTlTabWait = 4 };
+constexpr int kTlCtas = 1024;           // CTAs recorded
+constexpr int kTlPerCta = 48;           // records per CTA (further ones are counted, not stored)
+constexpr int kTlWarps = kTlCtas * (kTabThreads / 32);
+struct TlRec { unsigned long long t0, t1; uint32_t kind, item, pad0, pad1; };     // t0: claim / wait start, t1: done / return
+struct TlBuf {
+    uint32_t grid, n_cls, n_tab, n_chunks;
+    uint32_t n[kTlCtas];
+    TlRec rec[kTlCtas][kTlPerCta];
+    unsigned long long warp[kTlWarps][2];                    // first decide chunk starts, last one ends (0: no chunk)
+    uint32_t warp_chunks[kTlWarps];
+};
+__device__ TlBuf g_tl;
+__device__ __forceinline__ unsigned long long tl_now() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ void tl_rec(uint32_t& n, uint32_t kind, uint32_t item, unsigned long long t0) {
+    if (blockIdx.x < kTlCtas && n < kTlPerCta) g_tl.rec[blockIdx.x][n] = TlRec{t0, tl_now(), kind, item, 0u, 0u};
+    ++n;
+}
+#define GP_TL(...) __VA_ARGS__
+#else
+#define GP_TL(...)
+#endif
+
 // whole CTA after writing an item's output: count it done (release)
 __device__ __forceinline__ void signal_done(uint32_t* ctr) {
     __syncthreads();
@@ -178,7 +220,7 @@ __device__ __forceinline__ unsigned long long lookback(const unsigned long long*
         unsigned long long v = kStInclusive;                // before the chain: an inclusive 0
         if (j >= first) {
             unsigned ns = 32;
-            while (((v = ld_relaxed_u64(status + j)) >> 62) == 0) { __nanosleep(ns); if (ns < 512) ns <<= 1; }
+            while (((v = ld_relaxed_u64(status + j)) >> 62) == 0) { __nanosleep(ns); if (ns < kPollMaxNs) ns <<= 1; }
         }
         const unsigned inc = __ballot_sync(kFull, (v >> 62) == 2);
         const int stop = inc ? __ffs(inc) - 1 : 31;         // nearest inclusive word: nothing beyond it is needed
@@ -495,60 +537,89 @@ __device__ __forceinline__ int32_t tab_next_above(const uint32_t* tab, int32_t l
     return a;
 }
 
-// cols: raw application columns; app_slot: [2][n_apps] executor / driver shape slots from phase 1.  Applications the
-// tables cannot decide are prepared (PrepApp) and appended to `listed`; force_scan appends every application.
+// What the decide phase reads of one application before the tables exist: its columns, the validation, and the shape
+// slots phase 1 interned (with their full tuples checked).  Everything here was written before cls_done, so a warp loads
+// it while its CTA still waits for tab_done, and the decision itself starts from the table loads.
+struct AppIn {
+    int64_t d[3];                     // driver request
+    int64_t off;                      // ExecutorNodes offset
+    int32_t k, grp;                   // executor count, instance group
+    int32_t slot;                     // executor-shape hash slot whose table decides; -1: the scan decides
+    int32_t did;                      // dense driver-shape id with this exact request; -1: the driver loop starts at 0
+    int32_t bad;                      // validation error bits
+    bool live;                        // i < n_apps
+};
+__device__ __forceinline__ AppIn decide_load(int32_t i, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs,
+                                             const int32_t* app_slot, int32_t n_apps, int64_t out_cap, int force_scan) {
+    AppIn a;
+    a.live = i < n_apps;
+    a.d[0] = a.d[1] = a.d[2] = 0; a.off = 0; a.k = 0; a.grp = 0; a.slot = -1; a.did = -1; a.bad = 0;
+    if (!a.live) return a;
+    const int64_t d_cpu = cols.load(0, i), d_mem = cols.load(1, i), d_gpu = cols.load(2, i);
+    const int64_t e_cpu = cols.load(3, i), e_mem = cols.load(4, i), e_gpu = cols.load(5, i);
+    const int32_t kk = cols.count[i];
+    const int32_t grp = cols.group ? cols.group[i] : 0;
+    const int64_t off = cols.off[i], off1 = cols.off[i + 1];
+    // ---- validation (types.SparkApplicationResources must be non-negative and inside the exact-int64 domain) ----
+    int bad = 0;
+    if (d_cpu < 0 || d_mem < 0 || d_gpu < 0 || e_cpu < 0 || e_mem < 0 || e_gpu < 0 || kk < 0) bad |= kErrNegativeRequest;
+    if (d_cpu >= kMaxQuantity || d_mem >= kMaxQuantity || d_gpu >= kMaxQuantity || e_cpu >= kMaxQuantity || e_mem >= kMaxQuantity ||
+        e_gpu >= kMaxQuantity || kk > kMaxCount) bad |= kErrUnrepresentable;
+    if (grp < 0 || grp >= s.n_groups) bad |= kErrBadGroup;
+    if (off < 0 || off1 - off != (int64_t)(kk > 0 ? kk : 0) || off1 > out_cap) bad |= kErrBadOffsets;
+    a.d[0] = d_cpu; a.d[1] = d_mem; a.d[2] = d_gpu; a.off = off; a.k = kk; a.grp = grp; a.bad = bad;
+    if (bad || force_scan) return a;
+    const int32_t slot = app_slot[i];
+    if (slot >= 0) {
+        const ShapeEntry* en = tabs.entries + slot;         // the full tuple decides, not the fingerprint
+        if (en->id >= 0 && en->div[0].e == e_cpu && en->div[1].e == e_mem && en->div[2].e == e_gpu &&
+            (uint32_t)kk <= table_clamp(s.groups[grp].ne)) a.slot = slot;
+    }
+    const int32_t ds = app_slot[n_apps + i];
+    if (ds >= 0) {
+        const DriverEntry& de = tabs.dentries[ds];
+        if (de.id >= 0 && de.d[0] == d_cpu && de.d[1] == d_mem && de.d[2] == d_gpu) a.did = de.id;
+    }
+    return a;
+}
+
+// i: the application of this lane, a: what decide_load read of it.  Applications the tables cannot decide are prepared
+// (PrepApp) and appended to `listed`; force_scan appends every application.
 template <int ALGO, class OUT>
-__device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs,
-                                            const int32_t* app_slot, int32_t n_apps, int64_t out_cap,
-                                            int32_t* __restrict__ driver_node, OUT* __restrict__ executor_nodes,
-                                            PrepApp* __restrict__ prep, int32_t* __restrict__ listed, int* __restrict__ err,
-                                            volatile int* __restrict__ err_host, int force_scan,
+__device__ __forceinline__ void decide_app(int32_t i, const AppIn& a, const Snapshot& s, const AppColumns& cols,
+                                            const ShapeTables& tabs, int32_t* __restrict__ driver_node,
+                                            OUT* __restrict__ executor_nodes, PrepApp* __restrict__ prep,
+                                            int32_t* __restrict__ listed, int* __restrict__ err, volatile int* __restrict__ err_host,
                                             unsigned long long& probes, unsigned long long& drivers) {
     const int lane = threadIdx.x & 31;
     // this lane's share of the warp's coalesced emission (sh_k = 0: none): out[sh_dst + t] = place[sh_src + shifted t]
     uint32_t sh_k = 0, sh_cut = 0, sh_delta = 0;
     int64_t sh_dst = 0, sh_src = 0;
-    if (i < n_apps) {
-        const int64_t d_cpu = cols.load(0, i), d_mem = cols.load(1, i), d_gpu = cols.load(2, i);
-        const int64_t e_cpu = cols.load(3, i), e_mem = cols.load(4, i), e_gpu = cols.load(5, i);
-        const int32_t kk = cols.count[i];
-        const int32_t grp = cols.group ? cols.group[i] : 0;
-        const int64_t off = cols.off[i], off1 = cols.off[i + 1];
-        // ---- validation (types.SparkApplicationResources must be non-negative and inside the exact-int64 domain) ----
-        int bad = 0;
-        if (d_cpu < 0 || d_mem < 0 || d_gpu < 0 || e_cpu < 0 || e_mem < 0 || e_gpu < 0 || kk < 0) bad |= kErrNegativeRequest;
-        if (d_cpu >= kMaxQuantity || d_mem >= kMaxQuantity || d_gpu >= kMaxQuantity || e_cpu >= kMaxQuantity || e_mem >= kMaxQuantity ||
-            e_gpu >= kMaxQuantity || kk > kMaxCount) bad |= kErrUnrepresentable;
-        if (grp < 0 || grp >= s.n_groups) bad |= kErrBadGroup;
-        if (off < 0 || off1 - off != (int64_t)(kk > 0 ? kk : 0) || off1 > out_cap) bad |= kErrBadOffsets;
-        if (bad) {
-            atomicOr(err, bad); *err_host = bad;
+    if (a.live) {
+        const int64_t d_cpu = a.d[0], d_mem = a.d[1], d_gpu = a.d[2];
+        const int32_t kk = a.k, grp = a.grp;
+        const int64_t off = a.off;
+        if (a.bad) {
+            atomicOr(err, a.bad); *err_host = a.bad;
             driver_node[i] = -1;
         } else {
             const GroupDesc g = s.groups[grp];
             const int32_t ne = g.ne, nd = g.nd;
             const uint32_t k = (uint32_t)kk;
             const int snap_flags = s.meta->flags;
-            bool need_scan = force_scan != 0;
+            bool need_scan = a.slot < 0;
             int32_t result = -1;
             const ShapeEntry* en = nullptr;
             const uint32_t* tab = nullptr;
             uint32_t total = 0;
             const uint32_t clamp = table_clamp(ne);
             if (!need_scan) {
-                const int32_t slot = app_slot[i];
-                if (slot < 0) need_scan = true;
-                else {
-                    en = tabs.entries + slot;       // the full tuple decides, not the fingerprint
-                    if (en->id < 0 || en->div[0].e != e_cpu || en->div[1].e != e_mem || en->div[2].e != e_gpu || k > clamp) need_scan = true;
-                    else {
-                        tab = tabs.table + (size_t)en->id * tabs.pitch + g.sbase;
-                        total = tabs.total[(size_t)en->id * tabs.n_groups + grp];
-                        // distribute-evenly: no hosting node at all -> no executor can be placed (distribute_evenly.go:72);
-                        // 1..k hosting nodes: several rounds or an exact per-candidate test -> the scan decides
-                        if (ALGO == 1 && k != 0 && total != 0 && total < k + 1) need_scan = true;
-                    }
-                }
+                en = tabs.entries + a.slot;
+                tab = tabs.table + (size_t)en->id * tabs.pitch + g.sbase;
+                total = tabs.total[(size_t)en->id * tabs.n_groups + grp];
+                // distribute-evenly: no hosting node at all -> no executor can be placed (distribute_evenly.go:72);
+                // 1..k hosting nodes: several rounds or an exact per-candidate test -> the scan decides
+                if (ALGO == 1 && k != 0 && total != 0 && total < k + 1) need_scan = true;
             }
             if (!need_scan && !(k != 0 && (ALGO == 0 ? total < k : total == 0))) {   // not even without a driver (pack_tightly.go:62, distribute_evenly.go:72)
                 const bool drv_gpu = d_gpu != 0 || (snap_flags & kSnapGpuNegative);
@@ -556,14 +627,7 @@ __device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const A
                 const longlong2* gpair = s.pair + g.sbase;
                 const int64_t* ggpu = s.gpu + g.sbase;
                 // ---- driver loop (binpack.go:67-85) from the shape's first fitting candidate ---------------------------
-                int32_t j = 0;
-                {
-                    const int32_t ds = app_slot[n_apps + i];
-                    if (ds >= 0) {
-                        const DriverEntry& de = tabs.dentries[ds];
-                        if (de.id >= 0 && de.d[0] == d_cpu && de.d[1] == d_mem && de.d[2] == d_gpu) j = tabs.firstfit[(size_t)de.id * tabs.n_groups + grp];
-                    }
-                }
+                int32_t j = a.did >= 0 ? tabs.firstfit[(size_t)a.did * tabs.n_groups + grp] : 0;
                 int32_t dslot = -1;
                 uint32_t cd = 0, c0d = 0, sd = 0;
                 for (; j < nd; ++j) {
@@ -643,7 +707,8 @@ __device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const A
                 const int32_t at = atomicAdd(&tabs.hdr->n_listed, 1);
                 PrepApp p;
                 int b2 = 0; uint64_t lmax = 0; bool fast = true;
-                const int64_t dd[3] = {d_cpu, d_mem, d_gpu}, ee[3] = {e_cpu, e_mem, e_gpu};
+                const int64_t e_gpu = cols.load(5, i);
+                const int64_t dd[3] = {d_cpu, d_mem, d_gpu}, ee[3] = {cols.load(3, i), cols.load(4, i), e_gpu};
 #pragma unroll
                 for (int t = 0; t < 3; ++t) {
                     uint64_t l;
@@ -666,22 +731,37 @@ __device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const A
         }
     }
     // ---- coalesced emission of the index-shift lanes: the warp's executor indices are concatenated in lane order, and
-    // every 32-index chunk is written by the whole warp (owner lane of index e: binary search over the inclusive scan)
+    // every 32-index chunk is written by the whole warp (owner lane of index e: binary search over the inclusive scan).
+    // kEmitBatch chunks per round: their owner searches are independent shuffle chains, and all their P loads are issued
+    // before the first store, so a round costs one load round trip instead of one per chunk.
     {
+        constexpr int kEmitBatch = 4;
         const uint32_t incl = warp_incl_scan(sh_k, lane);
         const uint32_t n_out = __shfl_sync(kFull, incl, 31);
         const uint32_t excl = incl - sh_k;
         const int64_t dst = sh_dst - (int64_t)excl, src = sh_src - (int64_t)excl;     // index e of the concatenation
         const uint32_t cut = excl + sh_cut;
-        for (uint32_t e0 = 0; e0 < n_out; e0 += 32) {
-            const uint32_t e = e0 + (uint32_t)lane;
-            int owner = 0;                              // number of lanes whose indices all lie before e
+        for (uint32_t e0 = 0; e0 < n_out; e0 += 32 * kEmitBatch) {
+            int owner[kEmitBatch];                      // number of lanes whose indices all lie before e
+            int32_t node[kEmitBatch];
 #pragma unroll
-            for (int step = 16; step >= 1; step >>= 1)
-                if (__shfl_sync(kFull, incl, owner + step - 1) <= e) owner += step;
-            const int64_t o_dst = __shfl_sync(kFull, dst, owner), o_src = __shfl_sync(kFull, src, owner);
-            const uint32_t o_cut = __shfl_sync(kFull, cut, owner), o_delta = __shfl_sync(kFull, sh_delta, owner);
-            if (e < n_out) executor_nodes[o_dst + e] = (OUT)tabs.place[o_src + e + (e < o_cut ? 0u : o_delta)];
+            for (int b = 0; b < kEmitBatch; ++b) {
+                const uint32_t e = e0 + 32u * b + (uint32_t)lane;
+                int o = 0;
+#pragma unroll
+                for (int step = 16; step >= 1; step >>= 1)
+                    if (__shfl_sync(kFull, incl, o + step - 1) <= e) o += step;
+                const int64_t o_src = __shfl_sync(kFull, src, o);
+                const uint32_t o_cut = __shfl_sync(kFull, cut, o), o_delta = __shfl_sync(kFull, sh_delta, o);
+                owner[b] = o;
+                node[b] = e < n_out ? tabs.place[o_src + e + (e < o_cut ? 0u : o_delta)] : 0;
+            }
+#pragma unroll
+            for (int b = 0; b < kEmitBatch; ++b) {
+                const uint32_t e = e0 + 32u * b + (uint32_t)lane;
+                const int64_t o_dst = __shfl_sync(kFull, dst, owner[b]);
+                if (e < n_out) executor_nodes[o_dst + e] = (OUT)node[b];
+            }
         }
     }
 }
@@ -696,14 +776,18 @@ __device__ __forceinline__ void decide_app(int32_t i, const Snapshot& s, const A
 //   [n_cls, n_cls + n_tab)              table items, known once every classify tile is done: per executor shape present
 //                                       and group, its segments in order (seg_pre), then per (driver shape, group) one
 //                                       first-fit item;
-//   any later ticket                    the CTA turns to the decide phase: each of its warps claims 32-application chunks
-//                                       from hdr->dec_next until none is left (the cost of a decision varies with its
-//                                       walk; warp-sized claims keep the SMs evenly loaded), then the CTA leaves.
+//   any later ticket                    the CTA turns to the decide phase: warp w of CTA b first takes 32-application chunk
+//                                       b * 8 + w, with no claim; chunks past the grid's warp count are claimed one per
+//                                       warp from hdr->dec_next until none is left (the cost of a decision varies with
+//                                       its walk; warp-sized claims keep the SMs evenly loaded), then the CTA leaves.
 // Forward progress.  An item waits only for items with smaller tickets: a classify tile for the tiles before it (offset
 // look-back), a table item for every classify tile (hdr->cls_done) and for the earlier segments of its (shape, group)
 // (look-back), the decide phase for every table item (hdr->tab_done).  A ticket is claimed by a CTA that is running, and a
 // CTA claims its next ticket only after finishing the last one.  So by induction over the tickets, every claimed item
 // completes, whatever number of CTAs happens to be co-resident (other work on the GPU, the other pipeline lanes).
+// A decide chunk waits on nothing once the tables are done, so giving each warp a fixed first chunk by blockIdx is safe:
+// every CTA of the grid runs eventually and reaches the decide phase.  Tickets stay dynamic: CTAs are not dispatched
+// in index order, and a fixed ticket could make a running CTA wait for one that has not started.
 // The ticket, the phase counters and every look-back word start from zero: the previous call's gp_pack_listed left them so.
 // The item with ticket 0 is always a classify tile (one tile with nothing to classify when neither the tables nor the
 // offsets are needed).  It zeroes hdr->n_listed and, with status_zero != NULL, the call's status block (kStatusWords
@@ -725,8 +809,10 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
     const int32_t n_cls = (!force_scan || off_out) ? n_tiles : 1;
     int32_t n_es = 0, n_tab = -1, total_segs = 0;         // n_tab < 0: classify not yet seen complete by this CTA
     unsigned long long probes = 0, drivers = 0;
+    GP_TL(uint32_t tl_n = 0; unsigned long long tl_t0 = 0;)
     for (;;) {
         if (threadIdx.x == 0) sh.ticket = atomicAdd(&hdr->ticket, 1u);
+        GP_TL(if (threadIdx.x == 0) tl_t0 = tl_now();)
         __syncthreads();
         const int32_t t = (int32_t)sh.ticket;
         if (t < n_cls) {
@@ -740,10 +826,15 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
                 if (t == 0) segment_prefix(sh, s, tabs.seg_pre);
             }
             signal_done(&hdr->cls_done);
+            GP_TL(if (threadIdx.x == 0) tl_rec(tl_n, kTlCls, (uint32_t)t, tl_t0);)
             continue;
         }
         if (n_tab < 0) {
-            if (threadIdx.x == 0) wait_count(&hdr->cls_done, (uint32_t)n_cls);
+            if (threadIdx.x == 0) {
+                GP_TL(const unsigned long long w0 = tl_now();)
+                wait_count(&hdr->cls_done, (uint32_t)n_cls);
+                GP_TL(tl_rec(tl_n, kTlClsWait, 0u, w0);)
+            }
             __syncthreads();
             n_tab = 0;
             if (!force_scan) {
@@ -769,19 +860,43 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
                 driver_firstfit_block(s, tabs, rd / s.n_groups, rd % s.n_groups);
             }
             signal_done(&hdr->tab_done);
+            GP_TL(if (threadIdx.x == 0) tl_rec(tl_n, r < n_es * total_segs ? kTlSeg : kTlFirstFit, (uint32_t)r, tl_t0);)
             continue;
         }
-        if (threadIdx.x == 0) wait_count(&hdr->tab_done, (uint32_t)n_tab);
-        __syncthreads();
+        // The warp's first chunk is fixed, and everything decide_load reads was written before cls_done (which this CTA
+        // has seen): its loads are in flight while thread 0 waits for the tables.
         const int lane = threadIdx.x & 31;
-        for (;;) {
-            uint32_t c = 0;
-            if (lane == 0) c = atomicAdd(&hdr->dec_next, 1u);
-            c = __shfl_sync(kFull, c, 0);
-            if (c >= (uint32_t)(n_apps + 31) / 32u) break;
-            decide_app<ALGO, OUT>((int32_t)c * 32 + lane, s, cols, tabs, app_slot, n_apps, out_cap, driver_node, executor_nodes, prep,
-                                  listed, err, err_host, force_scan, probes, drivers);
+        GP_TL(unsigned long long tl_w0 = 0; uint32_t tl_chunks = 0;)
+        const uint32_t n_chunks = (uint32_t)(n_apps + 31) / 32u, n_warps = gridDim.x * (kTabThreads / 32u);
+        uint32_t c = blockIdx.x * (kTabThreads / 32u) + (threadIdx.x >> 5);
+        AppIn a = decide_load((int32_t)c * 32 + lane, s, cols, tabs, app_slot, n_apps, out_cap, force_scan);
+        if (threadIdx.x == 0) {
+            GP_TL(const unsigned long long w0 = tl_now();)
+            wait_count(&hdr->tab_done, (uint32_t)n_tab);
+            GP_TL(tl_rec(tl_n, kTlTabWait, 0u, w0);)
         }
+        __syncthreads();
+        while (c < n_chunks) {
+            GP_TL(if (tl_chunks++ == 0) tl_w0 = tl_now();)
+            decide_app<ALGO, OUT>((int32_t)c * 32 + lane, a, s, cols, tabs, driver_node, executor_nodes, prep, listed, err, err_host,
+                                  probes, drivers);
+            // the chunks past the grid's warps: claimed one at a time (their cost varies with the walks), and only while
+            // the counter says some are left
+            c = n_chunks;
+            if (n_warps < n_chunks) {
+                if (lane == 0 && n_warps + ld_relaxed_u32(&hdr->dec_next) < n_chunks) c = n_warps + atomicAdd(&hdr->dec_next, 1u);
+                c = __shfl_sync(kFull, c, 0);
+                if (c < n_chunks) a = decide_load((int32_t)c * 32 + lane, s, cols, tabs, app_slot, n_apps, out_cap, force_scan);
+            }
+        }
+        GP_TL(if (lane == 0 && blockIdx.x < kTlCtas) {
+            const uint32_t gw = blockIdx.x * (kTabThreads / 32) + (threadIdx.x >> 5);
+            g_tl.warp[gw][0] = tl_w0; g_tl.warp[gw][1] = tl_chunks ? tl_now() : 0ull; g_tl.warp_chunks[gw] = tl_chunks;
+        })
+        GP_TL(if (threadIdx.x == 0) {
+            if (blockIdx.x < kTlCtas) g_tl.n[blockIdx.x] = tl_n;
+            if (blockIdx.x == 0) { g_tl.grid = gridDim.x; g_tl.n_cls = (uint32_t)n_cls; g_tl.n_tab = (uint32_t)n_tab; g_tl.n_chunks = (uint32_t)(n_apps + 31) / 32u; }
+        })
         break;
     }
     // statistics: one atomic per warp

@@ -61,17 +61,19 @@ def _nvcc() -> str:
     raise RuntimeError("nvcc not found; cannot build libgangpack.so")
 
 
-def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_90a into k8s-spark-scheduler_b200/libgangpack.so (in-tree)."""
-    stale = force or not os.path.exists(LIB_PATH) or any(
-        os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in _SOURCES)
+def build(force: bool = False, verbose: bool = False, out: str | None = None, defines=()) -> str:
+    """Compile csrc/*.cu for sm_90a into k8s-spark-scheduler_b200/libgangpack.so (in-tree), or into `out` with extra
+    preprocessor `defines` (diagnostic builds such as GP_DECIDE_TIMELINE; never the in-tree library)."""
+    path = out or LIB_PATH
+    stale = force or not os.path.exists(path) or any(
+        os.path.getmtime(s) > os.path.getmtime(path) for s in _SOURCES)
     if stale:
-        cmd = [_nvcc()] + NVCC_FLAGS + ["-I", os.path.join(_ROOT, "include"), "-o", LIB_PATH, _SOURCES[0],
-                                        os.path.join(_PKG, "csrc", "gangpack_multi.cu")]
+        cmd = [_nvcc()] + NVCC_FLAGS + [f"-D{d}" for d in defines] + [
+            "-I", os.path.join(_ROOT, "include"), "-o", path, _SOURCES[0], os.path.join(_PKG, "csrc", "gangpack_multi.cu")]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         subprocess.check_call(cmd)
-    return LIB_PATH
+    return path
 
 
 class gp_config(C.Structure):
