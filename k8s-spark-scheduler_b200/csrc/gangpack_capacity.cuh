@@ -41,7 +41,6 @@
 #include <stdint.h>
 
 #include "gangpack_kernels.cuh"
-#include "gangpack_tables.cuh"
 
 namespace gp {
 

@@ -1,0 +1,273 @@
+// gangpack_ctx.cuh -- private to libgangpack: the context (gp_ctx) with its device buffers, status blocks and CUDA-graph
+// cache, and what more than one translation unit of csrc/ shares.  The functions and kernels declared here are defined in
+// the .cu file named above them; a helper that one file uses stays static there.
+#pragma once
+
+#include "gangpack.h"
+#include "gangpack_kernels.cuh"
+
+#include <cstddef>
+#include <cstring>
+#include <string>
+#include <utility>
+#include <vector>
+
+using namespace gp;
+
+// Device memory owned by the context: freed when the context is deleted.
+struct DevBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
+    cudaError_t reserve(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        if (p) cudaFree(p);
+        p = nullptr; cap = 0;
+        size_t want = bytes + bytes / 4 + 256;
+        cudaError_t e = cudaMalloc(&p, want);
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+    // reserve() for state the kernels leave zeroed after every use: a new allocation starts out all zero
+    cudaError_t reserve_zeroed(size_t bytes, cudaStream_t st) {
+        if (bytes <= cap) return cudaSuccess;
+        const cudaError_t e = reserve(bytes);
+        return e != cudaSuccess ? e : cudaMemsetAsync(p, 0, cap, st);
+    }
+    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+// One staging layout in one DevBuf: take() every piece (256-byte-aligned offsets), then reserve() once.
+struct Arena {
+    DevBuf& buf;
+    size_t size = 0;
+    size_t take(size_t bytes) { const size_t o = size; size += (bytes + 255) & ~(size_t)255; return o; }
+    cudaError_t reserve() { return buf.reserve(size); }
+    char* base() const { return buf.as<char>(); }
+    cudaError_t upload(size_t off, const void* src, size_t bytes, cudaStream_t st) const {
+        return cudaMemcpyAsync(base() + off, src, bytes, cudaMemcpyHostToDevice, st);
+    }
+};
+
+// A fixed sequence of kernel launches / memsets that repeats with identical arguments (one Predicate after the other:
+// same buffers, same batch shape) is captured ONCE into a CUDA graph and replayed with a single launch call -- the
+// pipelined host path is bound by how fast the host thread can issue its calls, not by the GPU.  The key is the byte image
+// of every argument of the sequence; it is captured when the same key is seen twice in a row.
+struct GraphCache {
+    cudaGraphExec_t exec = nullptr;
+    std::vector<char> key, last_key;
+    int launches = 0;
+    ~GraphCache() { reset(); }
+    void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; key.clear(); last_key.clear(); }
+};
+
+static constexpr int32_t kChunkApps = 50000;        // apps per pipelined chunk of gp_pack_batch (~1.5 MB H2D)
+static constexpr int32_t kZeroCopyOutApps = 8192;  // batches up to this size write results straight into mapped host memory
+static constexpr int kMaxChunks = 16;
+
+// The head of the per-call status block: what gp_last_stats copies to the host
+struct StatusHead {
+    int err;                                // kErr* bits
+    unsigned long long stats[4];            // nodes_scanned, drivers_tried, scan_path_apps, scan_path_nodes (device atomics)
+};
+static_assert(offsetof(StatusHead, stats) % 8 == 0, "64-bit atomics on the statistics need 8-byte alignment");
+static_assert(sizeof(StatusHead) == 40, "gp_last_stats copies the error bits and the four statistics");
+
+// Device status words of one pack call, zeroed by pack_begin or by gp_decide_tables' first classify tile
+struct DevStatus {
+    StatusHead head;
+    unsigned int az_listed, az_claim;       // gp_pack_az_fallback: length of its application list, its claim counter
+    unsigned int fifo_cursor;               // FIFO kernels: instance-group cursor
+    unsigned int next_app[kMaxChunks];      // per pipelined chunk: application claim counter
+    unsigned int spare[3];
+};
+static_assert(sizeof(DevStatus) == 4 * kStatusWords, "gp_decide_tables zeroes the whole block");
+
+// Pinned host block: the mirror of StatusHead (gp_last_stats) and the error word the kernels write through its mapping
+struct PinnedStatus { StatusHead head; volatile int err_word; };
+
+struct gp_ctx {
+    int device = 0;
+    int sm_count = 0;
+    cudaStream_t stream = nullptr;
+    static constexpr int kLanes = 3;       // H2D / kernels / D2H of consecutive chunks overlap across lanes
+    cudaStream_t lane[kLanes] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev[kMaxChunks][3] = {};    // per chunk: prep start, pack start, pack end
+    cudaEvent_t ev_ready = nullptr, ev_done[kLanes] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev_t0 = nullptr;           // GANGPACK_TRACE=2: start of the pipelined batch (timeline of the chunks on stderr)
+    int ev_chunks = 0;
+    std::string err;
+
+    // snapshot
+    bool have_snapshot = false;
+    int32_t n_nodes = 0, n_groups = 0, n_exec = 0, n_drv = 0, n_slots = 0;
+    DevBuf node_cpu, node_mem, node_gpu;        // node-table order (as given)
+    DevBuf exec_off, drv_off, exec_order, drv_order;
+    DevBuf pair, pair32, sgpu, slot_node, node_slot, drv_slot, groups, snap_flags;
+    DevBuf drv_pos;                             // node -> driver-order position, scattered by the layout (gp_build_slots_exec)
+    DevBuf snap_part;                           // SnapPart per CTA of gp_build_slots_exec
+
+    // batch staging; a_rows: the six quantity rows in one pitched block (pack_batch_impl)
+    DevBuf a_rows, a_count, a_group, a_skip, a_off;
+    DevBuf prep, r_driver, r_exec, scratch, dev_misc, gmin, sortbuf, usagebuf, reschedbuf;
+    void* pinned_misc = nullptr;                  // PinnedStatus
+    DevStatus* status() const { return dev_misc.as<DevStatus>(); }
+    PinnedStatus* host_status() const { return static_cast<PinnedStatus*>(pinned_misc); }
+    std::vector<int64_t> host_off;
+    std::vector<int32_t> v_owner;                 // gp_set_snapshot validation scratch (no per-call allocation)
+    // gp_set_snapshot's host copy of the layout, kept for gp_pack_fifo_az_aware's order checks: v_owner[v] (group, roles)
+    // and v_pos[v] / v_pos[n_nodes + v] (position of v in its group's executor / driver order).  host_layout: they
+    // describe the current snapshot (false after gp_set_snapshot_device / gp_prepare_cluster or a refused gp_set_snapshot)
+    std::vector<int32_t> v_pos;
+    bool host_layout = false;
+    std::vector<uint8_t> v_seen_e, v_seen_d;
+    std::vector<int32_t> v_zone_next;             // az-aware order check: next position per zone group
+    int az_fallback_ctas_per_sm = 0;              // occupancy of gp_pack_az_fallback (queried once)
+    std::vector<std::pair<const char*, size_t>> pinned_blocks;   // gp_alloc_pinned allocations (device-mapped under UVA)
+    void* one_block = nullptr;                    // gp_pack_one staging (mapped pinned)
+    size_t one_bytes = 0;
+    int zero_copy = 1;                            // GANGPACK_ZERO_COPY=0 disables reading/writing mapped host buffers in kernels
+    int use_tables = 1;                           // GANGPACK_TABLES=0: every independent decision takes the node-order scan
+    int fifo_warp = 1;                            // GANGPACK_FIFO_WARP=0: every FIFO application is decided by the whole CTA
+    bool async_snapshot = false;                  // gp_config.flags & GP_CFG_ASYNC_SNAPSHOT
+    int chunk_apps = kChunkApps;                  // GANGPACK_CHUNK_APPS
+    int trace = 0;                                // GANGPACK_TRACE=1: host-side phase timing on stderr
+    int pack_ctas_per_sm = 0;                       // occupancy of gp_pack_independent<2> on this device
+    int tab_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_pack_listed<ALGO, OUT>
+    int dec_ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // occupancy of gp_decide_tables<ALGO, OUT>
+    // per pipeline lane: shape hash + header, capacity tables, group totals, placement prefixes, per-application shape slot
+    struct TableSet { DevBuf hdr, table, total, place, app_slot; } tabs[kLanes];
+    bool record_events = true;                    // CUDA events around the kernels (gp_last_stats); the pipelined host path skips them
+    bool ev_prep = false;                         // the last pack recorded a prep interval ev[i][0] .. ev[i][1] (not the tables path)
+    int use_graphs = 1;                           // GANGPACK_GRAPHS=0: always issue the launches one by one
+    GraphCache g_chunk[kMaxChunks + 1];           // per pipelined chunk (+1: an unchunked batch on the context's own stream): classify .. scan
+    GraphCache g_snapshot;                        // slot layout of gp_set_snapshot
+    DevBuf off_dev;                               // ExecutorNodes offsets derived on the device
+    DevBuf fifo_list;                             // FIFO modes: per-instance-group application lists (queue order)
+    DevBuf sched, zonebuf, fbview;                // SchedulableResources [3][n_nodes]; staging of the zone entry points;
+                                                  // the az-aware fallback's orders and gather view
+    bool have_sched = false;
+    // SchedulableResources for gp_packing_efficiency alone: also set by gp_prepare_cluster, whose one-group snapshot the zone
+    // entry points keep refusing (have_sched stays false there)
+    bool have_eff_sched = false;
+    // gp_prepare_cluster_zones: the undivided orders it sorted (in zoneprep, which also holds that call's scratch), their
+    // lengths and n_zones as DEVICE pointers for gp_pack_*_az_aware(orders == NULL); zone_kind = the gp_zone_layout_kind of the
+    // current snapshot, -1 when another entry laid it out
+    DevBuf zoneprep;
+    DevBuf reschedprep;                           // gp_reschedule_from_reservations' own scratch (no state points into it)
+    DevBuf capprep;                               // gp_exceeds_cluster_capacity's own scratch (no state points into it)
+    DevBuf reconbuf;                              // gp_reconcile_find_nodes' own scratch (no state points into it)
+    DevBuf overbuf;                               // gp_node_overhead's own scratch (no state points into it)
+    int zone_kind = -1;
+    gp_az_orders zone_orders{};
+    bool sort_attr_set = false;
+    bool recon_attr_set = false;                  // dynamic shared-memory opt-in of gp_sort_tiles<ReconKey> done on this device
+    bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
+
+    gp_stats last{};
+};
+
+#define GP_CUDA(ctx, expr)                                                                     \
+    do {                                                                                       \
+        cudaError_t _e = (expr);                                                               \
+        if (_e != cudaSuccess) {                                                               \
+            (ctx)->err = std::string(#expr) + ": " + cudaGetErrorString(_e);                   \
+            return GP_ERR_CUDA;                                                                \
+        }                                                                                      \
+    } while (0)
+
+// issue(): enqueues the sequence on `st` and returns (status, launches).  See GraphCache.
+template <class F>
+static gp_status run_cached(gp_ctx* c, GraphCache& gc, const void* key, size_t kn, cudaStream_t st, F&& issue) {
+    const char* kb = static_cast<const char*>(key);
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (!c->use_graphs || cudaStreamIsCapturing(st, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
+        cudaGetLastError();
+        int n = 0;
+        gp_status s = issue(n);
+        c->last.kernel_launches += n;
+        return s;
+    }
+    if (gc.exec && gc.key.size() == kn && std::memcmp(gc.key.data(), kb, kn) == 0) {
+        GP_CUDA(c, cudaGraphLaunch(gc.exec, st));
+        c->last.kernel_launches += gc.launches;
+        return GP_OK;
+    }
+    if (gc.last_key.size() == kn && std::memcmp(gc.last_key.data(), kb, kn) == 0 &&
+        cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed) == cudaSuccess) {
+        int n = 0;
+        const gp_status s = issue(n);
+        cudaGraph_t g = nullptr;
+        const cudaError_t e = cudaStreamEndCapture(st, &g);
+        if (s == GP_OK && e == cudaSuccess && g) {
+            cudaGraphExec_t ex = nullptr;
+            if (cudaGraphInstantiate(&ex, g, 0) == cudaSuccess) {
+                if (gc.exec) cudaGraphExecDestroy(gc.exec);
+                gc.exec = ex; gc.key.assign(kb, kb + kn); gc.launches = n;
+                cudaGraphDestroy(g);
+                GP_CUDA(c, cudaGraphLaunch(gc.exec, st));
+                c->last.kernel_launches += n;
+                return GP_OK;
+            }
+        }
+        if (g) cudaGraphDestroy(g);
+        cudaGetLastError();                 // capture did not work out: issue directly below
+        if (s != GP_OK) return s;
+    } else {
+        cudaGetLastError();
+    }
+    gc.last_key.assign(kb, kb + kn);
+    int n = 0;
+    gp_status s = issue(n);
+    c->last.kernel_launches += n;
+    return s;
+}
+
+// ---- gangpack_api.cu -------------------------------------------------------------------------------------------------
+
+// gp_multi_copy's jobs: up to 8 host->device copies in one launch
+struct CopyJob { const void* src; void* dst; unsigned long long bytes; };
+struct CopyJobs { CopyJob j[8]; int n; };
+__global__ void gp_multi_copy(CopyJobs jobs);
+__global__ void gp_fill_pair32(int32_t n_slots, const longlong2* __restrict__ pair, SnapMeta* __restrict__ meta,
+                               uint2* __restrict__ pair32);
+__global__ void gp_scatter_slots(int32_t n_slots, const longlong2* __restrict__ pair, const int64_t* __restrict__ sgpu,
+                                 const int32_t* __restrict__ slot_node,
+                                 int64_t* __restrict__ cpu, int64_t* __restrict__ mem, int64_t* __restrict__ gpu);
+
+const void* mapped_ptr(gp_ctx* c, const void* p, size_t bytes);
+gp_status fail(gp_ctx* ctx, gp_status st, const std::string& msg);
+Snapshot make_snapshot(const gp_ctx* c);
+gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, cudaStream_t st,
+                                bool copy_nodes = false);
+
+// ---- gangpack_pack.cu ------------------------------------------------------------------------------------------------
+
+constexpr int kPrepThreads = 256;
+__global__ void gp_prep_apps(int32_t n_apps, AppColumns cols, const uint8_t* __restrict__ skip,
+                             int32_t n_groups, int64_t out_cap, const SnapMeta* __restrict__ meta,
+                             GroupMin* __restrict__ gmins, PrepApp* __restrict__ prep, int* __restrict__ err,
+                             volatile int* __restrict__ err_host);
+
+// device views of one batch
+struct DevApps {
+    AppColumns cols;                 // device pointers; cols.off may be NULL (derived on the device)
+    const uint8_t* skip;
+    int32_t n;
+};
+struct DevResults {
+    int32_t* driver;
+    void* exec;                      // int32 or uint16
+    int64_t cap;
+    int node_bits;
+};
+
+gp_status pack_begin(gp_ctx* c, int32_t q, gp_algo algo, gp_mode mode, int64_t exec_cap, bool derive_off, int2** scratch, cudaStream_t st,
+                     bool status_in_kernel = false);
+gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi, int64_t off_base, gp_algo algo, gp_mode mode,
+                            const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel = false);
+gp_status host_error(gp_ctx* c);

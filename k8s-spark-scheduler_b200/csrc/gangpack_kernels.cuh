@@ -109,6 +109,37 @@ struct Snapshot {
     int32_t n_slots;
 };
 
+// ---- raw application columns in either wire width --------------------------------------------------------------
+// 64-bit layout: exact int64 quantities (gp_apps).  32-bit layout (gp_apps_wire.quantity_bits == 32): int32 millicores /
+// int32 (bytes >> mem_shift) / int32 gpu units -- 28 bytes per application instead of 60.
+struct AppColumns {
+    const void* q[6];                 // drv cpu, drv mem, drv gpu, exe cpu, exe mem, exe gpu (gpu columns may be NULL = 0)
+    const int32_t* count;
+    const int32_t* group;             // or NULL (= 0)
+    const int64_t* off;               // [n+1] ExecutorNodes offsets (the caller's, or the ones K1 derived)
+    int32_t bits;                     // 64 or 32
+    int32_t mem_shift;                // 32-bit layout only
+    __device__ __forceinline__ int64_t load(int c, int32_t i) const {
+        const void* p = q[c];
+        if (!p) return 0;
+        if (bits == 64) return static_cast<const int64_t*>(p)[i];
+        const int64_t v = static_cast<const int32_t*>(p)[i];
+        return (c == 1 || c == 4) ? (v < 0 ? v : (v << mem_shift)) : v;     // negative stays negative -> validation error
+    }
+};
+
+// words of a pack call's status block (the host's DevStatus), which gp_decide_tables can zero in place of a memset
+constexpr int kStatusWords = 32;
+
+// fingerprint of a (cpu, mem, gpu) request, never 0: the shape hashes of gp_decide_tables and gp_cc_intern
+__device__ __forceinline__ unsigned long long shape_fingerprint(int64_t a, int64_t b, int64_t c) {
+    unsigned long long z = (unsigned long long)a * 0x9E3779B97F4A7C15ull;
+    z ^= ((unsigned long long)b + 0xBF58476D1CE4E5B9ull) * 0x94D049BB133111EBull;
+    z ^= ((unsigned long long)c + 0x2545F4914F6CDD1Dull) * 0xD6E8FEB86659FD93ull;
+    z ^= z >> 29; z *= 0xBF58476D1CE4E5B9ull; z ^= z >> 32;
+    return z ? z : 1ull;
+}
+
 // ---------------------------------------------------------------------------------------------
 // capacity arithmetic
 // ---------------------------------------------------------------------------------------------
@@ -118,7 +149,8 @@ struct Snapshot {
 // for xs = a >> sh < 2^32 and e' < 2^32, floor(xs/e') = mulhi64(magic, xs) with
 // magic = floor((2^64-1)/e') + 1 (Lemire, Kaser, Kurz 2019, N = 32).
 
-__device__ __noinline__ uint64_t udiv64(uint64_t a, uint64_t b) { return a / b; }
+// static: not inline, and several translation units of the library include this header
+static __device__ __noinline__ uint64_t udiv64(uint64_t a, uint64_t b) { return a / b; }
 
 // ---- general class: any int64 request ----------------------------------------------------------
 __device__ __forceinline__ uint32_t cap_dim(int64_t a, const DimDiv& p, uint32_t k) {

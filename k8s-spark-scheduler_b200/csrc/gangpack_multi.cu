@@ -11,7 +11,7 @@
 //     whole instance groups are assigned to devices (longest-processing-time first on apps_g x nodes_g), every device
 //     runs the queues of its groups in order against its copy of the snapshot, results are scattered back into queue
 //     order; gp_multi_get_snapshot reads every node from the device that owns its group.
-// Host code only: the kernels live in gangpack_api.cu.
+// Host code only: it calls the public gp_* entry points and launches no kernel of its own.
 #include "gangpack.h"
 
 #include <algorithm>

@@ -107,33 +107,6 @@ __device__ __forceinline__ uint32_t table_clamp(int32_t ne) {
     return by_len < (uint32_t)kMaxCount ? by_len : (uint32_t)kMaxCount;
 }
 
-__device__ __forceinline__ unsigned long long shape_fingerprint(int64_t a, int64_t b, int64_t c) {
-    unsigned long long z = (unsigned long long)a * 0x9E3779B97F4A7C15ull;
-    z ^= ((unsigned long long)b + 0xBF58476D1CE4E5B9ull) * 0x94D049BB133111EBull;
-    z ^= ((unsigned long long)c + 0x2545F4914F6CDD1Dull) * 0xD6E8FEB86659FD93ull;
-    z ^= z >> 29; z *= 0xBF58476D1CE4E5B9ull; z ^= z >> 32;
-    return z ? z : 1ull;
-}
-
-// ---- raw application columns in either wire width --------------------------------------------------------------
-// 64-bit layout: exact int64 quantities (gp_apps).  32-bit layout (gp_apps_wire.quantity_bits == 32): int32 millicores /
-// int32 (bytes >> mem_shift) / int32 gpu units -- 28 bytes per application instead of 60.
-struct AppColumns {
-    const void* q[6];                 // drv cpu, drv mem, drv gpu, exe cpu, exe mem, exe gpu (gpu columns may be NULL = 0)
-    const int32_t* count;
-    const int32_t* group;             // or NULL (= 0)
-    const int64_t* off;               // [n+1] ExecutorNodes offsets (the caller's, or the ones K1 derived)
-    int32_t bits;                     // 64 or 32
-    int32_t mem_shift;                // 32-bit layout only
-    __device__ __forceinline__ int64_t load(int c, int32_t i) const {
-        const void* p = q[c];
-        if (!p) return 0;
-        if (bits == 64) return static_cast<const int64_t*>(p)[i];
-        const int64_t v = static_cast<const int32_t*>(p)[i];
-        return (c == 1 || c == 4) ? (v < 0 ? v : (v << mem_shift)) : v;     // negative stays negative -> validation error
-    }
-};
-
 // ---------------------------------------------------------------------------------------------------------------
 // cross-CTA signalling inside the one launch
 // ---------------------------------------------------------------------------------------------------------------
@@ -794,7 +767,6 @@ __device__ __forceinline__ void decide_app(int32_t i, const AppIn& a, const Snap
 // words: error bits, statistics, claim counters) instead of a memset before the launch.  It finishes before cls_done can
 // count every tile, and every CTA waits for that count before it appends to the list, writes the error word or adds to
 // the statistics, so no write of the call is lost to the zeroing.
-constexpr int kStatusWords = 32;
 template <int ALGO, class OUT>
 __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppColumns cols, ShapeTables tabs, int64_t off_base,
                                                                 int64_t* off_out /* or NULL */, int32_t* app_slot, int32_t n_apps,

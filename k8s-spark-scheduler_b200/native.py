@@ -6,6 +6,7 @@ usable, loading / context creation raises.
 from __future__ import annotations
 
 import ctypes as C
+import glob
 import os
 import shutil
 import subprocess
@@ -15,13 +16,6 @@ import numpy as np
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
 LIB_PATH = os.environ.get("GANGPACK_LIB") or os.path.join(_PKG, "libgangpack.so")   # GANGPACK_LIB: experimental builds
-_SOURCES = [os.path.join(_PKG, "csrc", f) for f in ("gangpack_api.cu", "gangpack_kernels.cuh", "gangpack_fifo.cuh", "gangpack_minfrag.cuh",
-                                                    "gangpack_sort.cuh", "gangpack_tables.cuh", "gangpack_resched.cuh", "gangpack_multi.cu",
-                                                    "gangpack_zones.cuh", "gangpack_zonefifo.cuh", "gangpack_zonelayout.cuh",
-                                                    "gangpack_reschedprep.cuh", "gangpack_efficiency.cuh", "gangpack_capacity.cuh",
-                                                    "gangpack_affinity.cuh", "gangpack_overhead.cuh",
-                                                    "gangpack_reconcile.cuh")] + [
-    os.path.join(_ROOT, "include", "gangpack.h")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
@@ -65,11 +59,14 @@ def build(force: bool = False, verbose: bool = False, out: str | None = None, de
     """Compile csrc/*.cu for sm_90a into k8s-spark-scheduler_b200/libgangpack.so (in-tree), or into `out` with extra
     preprocessor `defines` (diagnostic builds such as GP_DECIDE_TIMELINE; never the in-tree library)."""
     path = out or LIB_PATH
+    csrc = os.path.join(_PKG, "csrc")
+    units = sorted(glob.glob(os.path.join(csrc, "*.cu")))
+    inputs = units + glob.glob(os.path.join(csrc, "*.cuh")) + [os.path.join(_ROOT, "include", "gangpack.h")]
     stale = force or not os.path.exists(path) or any(
-        os.path.getmtime(s) > os.path.getmtime(path) for s in _SOURCES)
+        os.path.getmtime(s) > os.path.getmtime(path) for s in inputs)
     if stale:
         cmd = [_nvcc()] + NVCC_FLAGS + [f"-D{d}" for d in defines] + [
-            "-I", os.path.join(_ROOT, "include"), "-o", path, _SOURCES[0], os.path.join(_PKG, "csrc", "gangpack_multi.cu")]
+            "-I", os.path.join(_ROOT, "include"), "-o", path] + units
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         subprocess.check_call(cmd)
