@@ -567,7 +567,9 @@ __device__ __noinline__ int32_t pack_app_general(const Snapshot& s, const PrepAp
     return pack_app_impl<ALGO, false, false, false, OUT>(s, pa, executor_nodes, scratch, wcache, st, lane, snap_flags, g0);
 }
 
-// fast class whose request shifts are below the compact view's shift (e.g. byte-granular memory requests)
+// fast class that cannot use the compact view: a cpu or memory request shift 32 or more above the view's shift (a fast
+// request never has a shift below it, since max_avail >> sh < 2^32 forces sh >= S).  Such a request exceeds every
+// availability of the snapshot, so its capacities here are all 0.
 template <int ALGO, class OUT>
 __device__ __noinline__ int32_t pack_app_fast64(const Snapshot& s, const PrepApp* __restrict__ pa,
                                                 OUT* __restrict__ executor_nodes, int2* __restrict__ scratch,
