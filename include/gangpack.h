@@ -166,7 +166,20 @@ gp_status gp_get_snapshot(gp_ctx* ctx, int64_t* avail_cpu_milli, int64_t* avail_
  *   available[n]   = allocatable[n] - (sum of reservations on n + overhead[n])
  *   schedulable[n] = allocatable[n] - overhead[n]
  * One entry of res_* per reservation (hard and soft alike); res_node = index into the node table, or -1 for a
- * reservation whose node is not in the table (ignored, like the map lookup at resources.go:72-75). */
+ * reservation whose node is not in the table (ignored, like the map lookup at resources.go:72-75; any index outside
+ * [0, n_nodes) is treated so).
+ *
+ * Domain.  The reference's quantities have no bound; this library computes in the exact-int64 domain |v| < 2^61, and every
+ * entry that takes a gp_usage_input (gp_build_availability, gp_build_reschedule_availability, gp_prepare_cluster,
+ * gp_prepare_cluster_zones, gp_reschedule_from_reservations, gp_reconcile_find_nodes) returns either the exact result or
+ * GP_ERR_UNREPRESENTABLE, never a wrapped one.  Refused: |allocatable|, |overhead| or a counted |reservation| >= 2^61; a
+ * node whose reservations add up, exactly, to a sum outside the domain (the sum is not taken modulo 2^64: reservations that
+ * add up to 2^64 are refused, not read as 0); an available, schedulable or -- where the entry computes it -- first-fit
+ * availability outside the domain, or gp_reschedule_from_reservations' availability - overhead of the minimal-fragmentation
+ * branch.  n_reservations >= 2^31 is GP_ERR_INVALID.  A refused call writes none of its outputs, except that
+ * gp_reschedule_from_reservations and gp_reconcile_find_nodes leave theirs undefined, and it replaces nothing in the
+ * context: after a refused gp_prepare_cluster or gp_prepare_cluster_zones the snapshot, layout, schedulable resources and
+ * held az-aware orders are those of the last successful call (both synchronise the stream once, after the sort, to know). */
 typedef struct {
     int32_t n_nodes;
     const int64_t* alloc_cpu_milli;      /* [n_nodes] node.Status.Allocatable */
@@ -202,14 +215,19 @@ gp_status gp_build_reschedule_availability(gp_ctx* ctx, const gp_usage_input* in
  * :55-57), each optionally re-sorted stably by the rank of a configured label value (:61-62,161-200).
  * The outputs are node indices and can be passed straight to gp_nodes.drv_order / exec_order.
  * Where the reference's comparators leave the order undefined (equal zone totals; equal (memory, cpu) with
- * different gpu, SURVEY App. B6) zones are ordered by id and nodes by name. */
+ * different gpu, SURVEY App. B6) zones are ordered by id and nodes by name.
+ * avail_* may hold any int64: keys are compared as signed 64-bit values, and the zone totals are summed and compared
+ * exactly, beyond 64 bits where they get there (a zone id without nodes totals (0, 0) and takes its rank among all n_zones
+ * ids like any other).  GP_ERR_INVALID: zone_id outside [0, n_zones), name_rank outside [0, n_nodes) or not a permutation
+ * (a rank given twice) -- in every entry that takes a gp_sort_input. */
 typedef struct {
     int32_t n_nodes;
     const int64_t* avail_cpu_milli;      /* [n_nodes] */
     const int64_t* avail_mem_bytes;      /* [n_nodes] */
     int32_t n_zones;                     /* >= 1 */
     const int32_t* zone_id;              /* [n_nodes] dense ids 0..n_zones-1 (ZoneLabel interned in first-seen order), or NULL (one zone) */
-    const int32_t* name_rank;            /* [n_nodes] rank of the node name in ascending byte order (unique), or NULL (= index order) */
+    const int32_t* name_rank;            /* [n_nodes] rank of the node name in ascending byte order: a permutation of 0..n_nodes-1
+                                            (checked), or NULL (= index order) */
     const uint8_t* is_driver_candidate;  /* [n_nodes] member of ExtenderArgs.NodeNames, or NULL (= all) */
     const uint8_t* unschedulable;        /* [n_nodes] node.Spec.Unschedulable, or NULL (= none) */
     const uint8_t* ready;                /* [n_nodes] NodeReady == True, or NULL (= all) */

@@ -21,21 +21,41 @@ __global__ void gp_offsets_from_counts(const int32_t* __restrict__ counts, int32
 }
 
 // Host checks shared by the entries below; `who` (the entry's name) prefixes every message.  The shape of a gp_usage_input:
-// sizes non-negative, the allocatable columns for nodes, the reservation columns for rows.
+// sizes non-negative, the allocatable columns for nodes, the reservation columns for rows, fewer than 2^31 rows (the bound
+// the exact usage sums rest on).  The quantities themselves are checked where they are read, on the device (usage_refusal).
 static gp_status check_usage(gp_ctx* c, const gp_usage_input* in, const char* who) {
-    if (!in || in->n_nodes < 0 || in->n_reservations < 0 || (in->n_nodes > 0 && (!in->alloc_cpu_milli || !in->alloc_mem_bytes)) ||
+    if (!in || in->n_nodes < 0 || in->n_reservations < 0 || in->n_reservations > 0x7fffffffLL ||
+        (in->n_nodes > 0 && (!in->alloc_cpu_milli || !in->alloc_mem_bytes)) ||
         (in->n_reservations > 0 && (!in->res_node || !in->res_cpu_milli || !in->res_mem_bytes)))
         return fail(c, GP_ERR_INVALID, std::string(who) + ": missing arrays or bad sizes");
     return GP_OK;
 }
 
-// The two id arrays of a gp_sort_input the kernels index with.
+// The status word of the availability stage (kFeErr* bits), read back by the entry: the refusal it stands for.
+static gp_status usage_refusal(gp_ctx* c, int err, const char* who) {
+    if (err & kFeErrInput)
+        return fail(c, GP_ERR_UNREPRESENTABLE, std::string(who) + ": |allocatable|, |overhead| or |reservation| >= 2^61");
+    if (err & kFeErrResult)
+        return fail(c, GP_ERR_UNREPRESENTABLE, std::string(who) + ": a node's reservation sum or availability lies outside the exact-int64 domain (|v| >= 2^61)");
+    return GP_OK;
+}
+
+// The two id arrays of a gp_sort_input the kernels index with: zone ids in range, name ranks a permutation of 0..n-1 (a rank
+// given twice would leave a position of the order unwritten).
 static gp_status check_sort_ids(gp_ctx* c, const gp_sort_input* in, const char* who) {
     const int32_t n = in->n_nodes;
     if (in->zone_id) for (int32_t i = 0; i < n; ++i)
         if (in->zone_id[i] < 0 || in->zone_id[i] >= in->n_zones) return fail(c, GP_ERR_INVALID, std::string(who) + ": zone_id out of range");
-    if (in->name_rank) for (int32_t i = 0; i < n; ++i)
-        if (in->name_rank[i] < 0 || in->name_rank[i] >= n) return fail(c, GP_ERR_INVALID, std::string(who) + ": name_rank out of range");
+    if (in->name_rank) {
+        std::vector<uint8_t>& seen = c->v_seen_e;       // host scratch of the order checks
+        seen.assign((size_t)n, 0);
+        for (int32_t i = 0; i < n; ++i) {
+            const int32_t r = in->name_rank[i];
+            if (r < 0 || r >= n) return fail(c, GP_ERR_INVALID, std::string(who) + ": name_rank out of range");
+            if (seen[r]) return fail(c, GP_ERR_INVALID, std::string(who) + ": name_rank is not a permutation (a rank is given twice)");
+            seen[r] = 1;
+        }
+    }
     return GP_OK;
 }
 
@@ -65,17 +85,18 @@ static gp_status check_hosting(gp_ctx* c, const gp_reschedule* in, int32_t n_nod
     return GP_OK;
 }
 
-// f2 stage: uploads the inputs, leaves avail[3][N] / sched[3][N] on the device (usagebuf).
+// f2 stage: uploads the inputs, leaves avail[3][N] / sched[3][N] and the stage's status word (*d_err: kFeErr* bits, for
+// usage_refusal once the stream has been synchronised) on the device (usagebuf).
 // d_over (optional, [3]): the uploaded overhead columns, NULL where the caller gave none.
-static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStream_t st, long long** d_avail, long long** d_sched,
+static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStream_t st, long long** d_avail, long long** d_sched, int** d_err,
                                     long long** d_resched = nullptr, const long long** d_over = nullptr) {
     const int32_t n = in->n_nodes;
     const size_t N = (size_t)n, R = (size_t)in->n_reservations;
     Arena ar{c->usagebuf};
-    const size_t o_alloc = ar.take(24 * N), o_over = ar.take(24 * N), o_usage = ar.take(24 * N + 4 * N), o_avail = ar.take(24 * N),
+    const size_t o_alloc = ar.take(24 * N), o_over = ar.take(24 * N), o_usage = ar.take(48 * N + 4 * N + 4), o_avail = ar.take(24 * N),
                  o_sched = ar.take(24 * N), o_resched = ar.take(24 * N), o_rn = ar.take(4 * R), o_rc = ar.take(8 * R), o_rm = ar.take(8 * R),
                  o_rg = ar.take(8 * R);
-    const size_t o_has = o_usage + 24 * N;      // zeroed together with the usage sums
+    const size_t o_has = o_usage + 48 * N, o_err = o_has + 4 * N;      // zeroed together with the usage sums
     GP_CUDA(c, ar.reserve());
     char* b = ar.base();
     GP_CUDA(c, ar.upload(o_alloc, in->alloc_cpu_milli, 8 * N, st));
@@ -84,8 +105,9 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
     if (in->overhead_cpu_milli) GP_CUDA(c, ar.upload(o_over, in->overhead_cpu_milli, 8 * N, st));
     if (in->overhead_mem_bytes) GP_CUDA(c, ar.upload(o_over + 8 * N, in->overhead_mem_bytes, 8 * N, st));
     if (in->overhead_gpu) GP_CUDA(c, ar.upload(o_over + 16 * N, in->overhead_gpu, 8 * N, st));
-    GP_CUDA(c, cudaMemsetAsync(b + o_usage, 0, 28 * N, st));
+    GP_CUDA(c, cudaMemsetAsync(b + o_usage, 0, 52 * N + 4, st));
     const int T = 256;
+    int* err = (int*)(b + o_err);
     if (R) {
         GP_CUDA(c, ar.upload(o_rn, in->res_node, 4 * R, st));
         GP_CUDA(c, ar.upload(o_rc, in->res_cpu_milli, 8 * R, st));
@@ -93,13 +115,13 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
         if (in->res_gpu) GP_CUDA(c, ar.upload(o_rg, in->res_gpu, 8 * R, st));
         gp_usage_scatter<<<(unsigned)((R + T - 1) / T), T, 0, st>>>((long long)R, (const int32_t*)(b + o_rn), (const long long*)(b + o_rc),
                                                                    (const long long*)(b + o_rm), in->res_gpu ? (const long long*)(b + o_rg) : nullptr,
-                                                                   n, (unsigned long long*)(b + o_usage), d_resched ? (unsigned int*)(b + o_has) : nullptr);
+                                                                   n, (unsigned long long*)(b + o_usage), d_resched ? (unsigned int*)(b + o_has) : nullptr, err);
     }
     const long long* al = (const long long*)(b + o_alloc);
     const long long* ov = (const long long*)(b + o_over);
     gp_availability<<<(n + T - 1) / T, T, 0, st>>>(n, al, al + N, in->alloc_gpu ? al + 2 * N : nullptr, in->overhead_cpu_milli ? ov : nullptr,
                                                    in->overhead_mem_bytes ? ov + N : nullptr, in->overhead_gpu ? ov + 2 * N : nullptr,
-                                                   (const unsigned long long*)(b + o_usage), (long long*)(b + o_avail), (long long*)(b + o_sched),
+                                                   (const unsigned long long*)(b + o_usage), (long long*)(b + o_avail), (long long*)(b + o_sched), err,
                                                    (const unsigned int*)(b + o_has), d_resched ? (long long*)(b + o_resched) : nullptr);
     if (d_resched) *d_resched = (long long*)(b + o_resched);
     if (d_over) {
@@ -110,6 +132,7 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
     GP_CUDA(c, cudaGetLastError());
     *d_avail = (long long*)(b + o_avail);
     *d_sched = (long long*)(b + o_sched);
+    *d_err = err;
     return GP_OK;
 }
 
@@ -138,7 +161,7 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
     const size_t N = (size_t)n, Z = (size_t)in->n_zones;
     Arena ar{c->sortbuf};
     const size_t o_cpu = ar.take(8 * N), o_mem = ar.take(8 * N), o_gpu = ar.take(8 * N), o_keys = ar.take(sizeof(SortKey) * N),
-                 o_sorted = ar.take(sizeof(SortKey) * N), o_tot = ar.take(16 * Z), o_zone = ar.take(4 * N), o_nr = ar.take(4 * N),
+                 o_sorted = ar.take(sizeof(SortKey) * N), o_tot = ar.take(8 * kZoneTotWords * Z), o_zone = ar.take(4 * N), o_nr = ar.take(4 * N),
                  o_prio = ar.take(4 * Z), o_pos = ar.take(4 * N), o_order = ar.take(4 * N), o_drv = ar.take(4 * N), o_exe = ar.take(4 * N),
                  o_drv2 = ar.take(4 * N), o_exe2 = ar.take(4 * N), o_lrd = ar.take(4 * N), o_lre = ar.take(4 * N),
                  o_lk = ar.take(sizeof(LabelKey) * N), o_lks = ar.take(sizeof(LabelKey) * N), o_cnt = ar.take(16),
@@ -156,7 +179,7 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
     if (in->ready) GP_CUDA(c, ar.upload(o_fr, in->ready, N, st));
     if (in->driver_label_rank) GP_CUDA(c, ar.upload(o_lrd, in->driver_label_rank, 4 * N, st));
     if (in->executor_label_rank) GP_CUDA(c, ar.upload(o_lre, in->executor_label_rank, 4 * N, st));
-    if (zoned) GP_CUDA(c, cudaMemsetAsync(b + o_tot, 0, 16 * Z, st));
+    if (zoned) GP_CUDA(c, cudaMemsetAsync(b + o_tot, 0, 8 * kZoneTotWords * Z, st));
     if (!c->sort_attr_set) {
         GP_CUDA(c, cudaFuncSetAttribute(gp_sort_tiles<SortKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSortTile * sizeof(SortKey))));
         c->sort_attr_set = true;
@@ -195,7 +218,8 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
 }
 
 // gp_prepare_cluster and gp_prepare_cluster_zones up to their layout step: the checks both make, then reservations ->
-// availability (d_avail / d_sched: [3][n_nodes]) -> priority orders on the context's stream.
+// availability (d_avail / d_sched: [3][n_nodes]) -> priority orders on the context's stream.  Synchronises once for the
+// availability stage's status word: a refusal returns before anything of the context's snapshot has been replaced.
 static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const char* who,
                                 long long** d_avail, long long** d_sched, SortStage* so) {
     gp_status s = check_usage(c, usage, who);
@@ -205,9 +229,14 @@ static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp
     if (usage->n_nodes == 0) return fail(c, GP_ERR_INVALID, std::string(who) + ": empty node table");
     if ((s = check_sort_ids(c, sort, who)) != GP_OK) return s;
     GP_CUDA(c, cudaSetDevice(c->device));
-    if ((s = stage_availability(c, usage, c->stream, d_avail, d_sched)) != GP_OK) return s;
+    int* d_err = nullptr;
+    if ((s = stage_availability(c, usage, c->stream, d_avail, d_sched, &d_err)) != GP_OK) return s;
     const size_t N = (size_t)usage->n_nodes;
-    return stage_sort(c, sort, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so);
+    if ((s = stage_sort(c, sort, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so)) != GP_OK) return s;
+    int err = 0;
+    GP_CUDA(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, c->stream));
+    GP_CUDA(c, cudaStreamSynchronize(c->stream));
+    return usage_refusal(c, err, who);
 }
 
 // gp_prepare_cluster and gp_prepare_cluster_zones after their layout step, which set dn's groups, offsets and orders: the
@@ -233,6 +262,7 @@ static gp_status prepare_snapshot(gp_ctx* c, gp_nodes* dn, const long long* d_av
 
 // The two gp_build_*availability entries: the availability stage, then every non-NULL outs[k] gets row k % 3 of
 // availableResources for k < 3 (first_fit: that of rescheduleExecutor's first-fit branch), of SchedulableResources for k >= 3.
+// The stage's status word is read first: a refused call writes to none of them.
 static gp_status availability_out(gp_ctx* c, const gp_usage_input* in, bool first_fit, int64_t* const* outs, const char* who) {
     gp_status s = check_usage(c, in, who);
     if (s != GP_OK) return s;
@@ -241,8 +271,13 @@ static gp_status availability_out(gp_ctx* c, const gp_usage_input* in, bool firs
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     long long *d_avail = nullptr, *d_sched = nullptr, *d_ff = nullptr;
-    s = stage_availability(c, in, st, &d_avail, &d_sched, first_fit ? &d_ff : nullptr);
+    int* d_err = nullptr;
+    s = stage_availability(c, in, st, &d_avail, &d_sched, &d_err, first_fit ? &d_ff : nullptr);
     if (s != GP_OK) return s;
+    int err = 0;
+    GP_CUDA(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    if ((s = usage_refusal(c, err, who)) != GP_OK) return s;           // the outputs are left as they were
     const size_t N = (size_t)n;
     const long long* src[2] = {first_fit ? d_ff : d_avail, d_sched};
     for (int k = 0; k < 6; ++k)
@@ -526,12 +561,13 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     // availability: one scatter of the reservations, one pass per node (usagebuf is scratch of the f2 stage only)
     long long *d_avail = nullptr, *d_sched = nullptr, *d_ff = nullptr;
     const long long* d_over[3] = {nullptr, nullptr, nullptr};
-    s = stage_availability(c, usage, st, &d_avail, &d_sched, mf ? nullptr : &d_ff, d_over);
+    int* d_err = nullptr;
+    s = stage_availability(c, usage, st, &d_avail, &d_sched, &d_err, mf ? nullptr : &d_ff, d_over);
     if (s != GP_OK) return s;
     const size_t N = (size_t)n, Q = (size_t)q, H = (size_t)hosted, Z = (size_t)sort->n_zones;
     const bool zoned = sort->zone_id != nullptr && sort->n_zones > 1;
     Arena ar{c->reschedprep};
-    const size_t o_tot = ar.take(16 * Z), o_prio = ar.take(4 * Z), o_zone = ar.take(4 * N), o_nr = ar.take(4 * N), o_fu = ar.take(N),
+    const size_t o_tot = ar.take(8 * kZoneTotWords * Z), o_prio = ar.take(4 * Z), o_zone = ar.take(4 * N), o_nr = ar.take(4 * N), o_fu = ar.take(N),
                  o_fr = ar.take(N), o_lr = ar.take(4 * N), o_tz = ar.take(4 * N), o_rec = ar.take(sizeof(RpNode) * N), o_exe = ar.take(24 * Q),
                  o_hoff = ar.take(8 * (Q + 1)), o_hn = ar.take(4 * (H + 1)), o_out = ar.take(4 * Q), o_amb = ar.take(Q);
     GP_CUDA(c, ar.reserve());
@@ -554,7 +590,7 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     const int nb = (n + T - 1) / T;
     const int32_t* tz = keep >= 0 ? (const int32_t*)(b + o_tz) : nullptr;
     if (zoned) {
-        GP_CUDA(c, cudaMemsetAsync(b + o_tot, 0, 16 * Z, st));
+        GP_CUDA(c, cudaMemsetAsync(b + o_tot, 0, 8 * kZoneTotWords * Z, st));
         gp_rp_zone_totals<<<nb, T, 0, st>>>(n, d_avail, d_avail + N, (const int32_t*)(b + o_zone), keep, tz, (unsigned long long*)(b + o_tot));
         gp_zone_priority<<<(sort->n_zones + T - 1) / T, T, 0, st>>>(sort->n_zones, (const unsigned long long*)(b + o_tot), (int32_t*)(b + o_prio));
     }
@@ -567,7 +603,7 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     ni.unschedulable = sort->unschedulable ? (const uint8_t*)(b + o_fu) : nullptr;
     ni.ready = sort->ready ? (const uint8_t*)(b + o_fr) : nullptr;
     ni.label_rank = sort->executor_label_rank ? (const int32_t*)(b + o_lr) : nullptr;
-    ni.tz = tz; ni.keep = keep; ni.n = n;
+    ni.tz = tz; ni.keep = keep; ni.n = n; ni.err = d_err;
     RpNode* rec = (RpNode*)(b + o_rec);
     gp_rp_nodes<<<nb, T, 0, st>>>(ni, rec);
     RpDecideIn di{};
@@ -586,8 +622,10 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     GP_CUDA(c, cudaGetLastError());
     GP_CUDA(c, cudaMemcpyAsync(node_out, d_out, 4 * Q, cudaMemcpyDeviceToHost, st));
     if (ambiguous) GP_CUDA(c, cudaMemcpyAsync(ambiguous, d_amb, Q, cudaMemcpyDeviceToHost, st));
+    int err = 0;
+    GP_CUDA(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
-    return GP_OK;
+    return usage_refusal(c, err, who);                  // refused: node_out / ambiguous hold no decision
 }
 
 // the failover reconciler's findNodes loop for a batch of stale drivers (EXT/failover.go:43-82, 286-436); see
@@ -627,7 +665,8 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     long long *d_avail = nullptr, *d_sched = nullptr;   // usagebuf: scratch of the availability stage, charged in place below
-    s = stage_availability(c, usage, st, &d_avail, &d_sched);
+    int* d_err = nullptr;
+    s = stage_availability(c, usage, st, &d_avail, &d_sched, &d_err);
     if (s != GP_OK) return s;
     const size_t N = (size_t)n, Q = (size_t)q, Gs = (size_t)G, E = (size_t)total;
     Arena ar{c->reconbuf};
@@ -709,7 +748,10 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
     int64_t* outs[3] = {out->avail_cpu_milli, out->avail_mem_bytes, out->avail_gpu};
     for (int d = 0; d < 3; ++d)
         if (outs[d]) GP_CUDA(c, cudaMemcpyAsync(outs[d], d_avail + N * (size_t)d, 8 * N, cudaMemcpyDeviceToHost, st));
+    int uerr = 0;
+    GP_CUDA(c, cudaMemcpyAsync(&uerr, d_err, 4, cudaMemcpyDeviceToHost, st));
     GP_CUDA(c, cudaStreamSynchronize(st));
+    if ((s = usage_refusal(c, uerr, who)) != GP_OK) return s;
     if (herr & kRcErrDomain) return bad(GP_ERR_UNREPRESENTABLE, "an availability the loop charged lies outside the exact-int64 domain (|v| >= 2^61)");
     return GP_OK;
 }

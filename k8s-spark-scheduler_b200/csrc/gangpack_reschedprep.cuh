@@ -49,12 +49,10 @@ __device__ __forceinline__ bool rp_member(int32_t i, int32_t keep, const int32_t
 // getAvailableResourcesByAZ (nodesorting.go:124-134) over the nodes filterNodesToZone keeps
 __global__ void gp_rp_zone_totals(int32_t n, const long long* __restrict__ cpu, const long long* __restrict__ mem,
                                   const int32_t* __restrict__ zone, int32_t keep, const int32_t* __restrict__ tz,
-                                  unsigned long long* __restrict__ tot /* [2*Z]: mem, cpu */) {
+                                  unsigned long long* __restrict__ tot /* [kZoneTotWords * Z] */) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || !rp_member(i, keep, tz)) return;
-    const int32_t z = zone[i];
-    atomicAdd(tot + 2 * z + 0, (unsigned long long)mem[i]);     // two's complement: signed sums wrap correctly
-    atomicAdd(tot + 2 * z + 1, (unsigned long long)cpu[i]);
+    zone_total_add(tot, zone[i], mem[i], cpu[i]);
 }
 
 struct RpNodeIn {
@@ -70,6 +68,7 @@ struct RpNodeIn {
     const int32_t* tz;               // topology zone per node (scope), read when keep >= 0
     int32_t keep;
     int32_t n;
+    int* err;                        // kFeErr* bits of the availability stage
 };
 
 __global__ void gp_rp_nodes(RpNodeIn in, RpNode* __restrict__ out) {
@@ -81,6 +80,8 @@ __global__ void gp_rp_nodes(RpNodeIn in, RpNode* __restrict__ out) {
 #pragma unroll
     for (int d = 0; d < 3; ++d)
         r.v[d] = in.ff ? in.ff[(size_t)d * N + i] : in.avail[(size_t)d * N + i] - (in.over[d] ? in.over[d][i] : 0);
+    // availability and overhead are inside the domain (or *err is set already), so the difference did not wrap
+    if (!in_domain(r.v[0]) || !in_domain(r.v[1]) || !in_domain(r.v[2])) atomicOr(in.err, kFeErrResult);
     const int32_t lr = in.label_rank ? in.label_rank[i] : 0;
     r.L = lr < 0 ? 0x7fffffffu : (uint32_t)lr;
     r.P = in.zone ? in.prio[in.zone[i]] : 0;

@@ -23,7 +23,46 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "gangpack_kernels.cuh"
+
 namespace gp {
+
+// ---- exact sums of signed 64-bit terms ------------------------------------------------------------------------------
+// The reference adds resource.Quantity values, which have no bound; a 64-bit atomicAdd wraps.  As in gangpack_overhead.cuh a
+// sum is kept in two words, each with an atomicAdd of its own: `lo` sums the terms' low 32 bits, `hi` their (arithmetic) high
+// halves.  With fewer than 2^31 terms lo < 2^63 and |hi| < 2^62 for ANY int64 terms, so neither word wraps, and
+// sum = hi * 2^32 + lo exactly.
+__device__ __forceinline__ void exact_add(unsigned long long* lo, unsigned long long* hi, long long v) {
+    const unsigned long long l = (unsigned long long)v & 0xffffffffull;
+    const long long h = v >> 32;
+    if (l) atomicAdd(lo, l);
+    if (h) atomicAdd(hi, (unsigned long long)h);
+}
+struct ExactSum {          // hi * 2^32 + lo, normalised: comparing (hi, lo) compares the sums
+    long long hi;
+    uint32_t lo;
+};
+__device__ __forceinline__ ExactSum exact_sum(unsigned long long lo, unsigned long long hi) {
+    ExactSum s; s.hi = (long long)hi + (long long)(lo >> 32); s.lo = (uint32_t)lo;
+    return s;
+}
+__device__ __forceinline__ int exact_cmp(const ExactSum& a, const ExactSum& b) {
+    return a.hi != b.hi ? (a.hi < b.hi ? -1 : 1) : (a.lo != b.lo ? (a.lo < b.lo ? -1 : 1) : 0);
+}
+__device__ __forceinline__ bool in_domain(long long v) { return v > -kMaxQuantity && v < kMaxQuantity; }
+// *v = the sum when it lies inside the exact-int64 domain (|sum| < 2^61)
+__device__ __forceinline__ bool exact_value(const ExactSum& s, long long* v) {
+    constexpr long long lim = kMaxQuantity >> 32;
+    if (s.hi < -lim || s.hi >= lim || (s.hi == -lim && s.lo == 0)) return false;
+    *v = s.hi * 4294967296LL + (long long)s.lo;
+    return true;
+}
+
+// status bits of the availability stage (f2) and of what is derived from it
+enum : int {
+    kFeErrInput = 1,        // |allocatable|, |overhead| or |a counted reservation| >= 2^61
+    kFeErrResult = 2,       // a usage sum or an availability outside the exact-int64 domain
+};
 
 struct SortKey {          // 24 bytes
     long long mem;
@@ -39,25 +78,33 @@ __device__ __forceinline__ bool key_less(const SortKey& a, const SortKey& b) {
     return a.name_rank < b.name_rank;
 }
 
-// per-zone totals of available memory / cpu (getAvailableResourcesByAZ, :124-134)
+// per-zone totals of available memory / cpu (getAvailableResourcesByAZ, :124-134), exact whatever the node quantities:
+// tot[4 * z ..] = memory (lo, hi), cpu (lo, hi) as exact_add keeps them
+constexpr int kZoneTotWords = 4;
+__device__ __forceinline__ void zone_total_add(unsigned long long* __restrict__ tot, int32_t z, long long mem, long long cpu) {
+    unsigned long long* t = tot + (size_t)kZoneTotWords * z;
+    exact_add(t + 0, t + 1, mem);
+    exact_add(t + 2, t + 3, cpu);
+}
 __global__ void gp_zone_totals(int32_t n, const long long* __restrict__ cpu, const long long* __restrict__ mem,
-                               const int32_t* __restrict__ zone, unsigned long long* __restrict__ tot /* [2*Z]: mem, cpu */) {
+                               const int32_t* __restrict__ zone, unsigned long long* __restrict__ tot /* [kZoneTotWords * Z] */) {
     int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int32_t z = zone[i];
-    atomicAdd(tot + 2 * z + 0, (unsigned long long)mem[i]);     // two's complement: signed sums wrap correctly
-    atomicAdd(tot + 2 * z + 1, (unsigned long long)cpu[i]);
+    zone_total_add(tot, zone[i], mem[i], cpu[i]);
 }
 
 // AZ priority = number of zones with smaller (mem, cpu, id)   (sort.Slice over zones, :102-104; ties by zone id)
 __global__ void gp_zone_priority(int32_t n_zones, const unsigned long long* __restrict__ tot, int32_t* __restrict__ prio) {
     int32_t z = blockIdx.x * blockDim.x + threadIdx.x;
     if (z >= n_zones) return;
-    const long long m = (long long)tot[2 * z], c = (long long)tot[2 * z + 1];
+    const unsigned long long* t = tot + (size_t)kZoneTotWords * z;
+    const ExactSum m = exact_sum(t[0], t[1]), c = exact_sum(t[2], t[3]);
     int32_t p = 0;
     for (int32_t o = 0; o < n_zones; ++o) {
-        const long long om = (long long)tot[2 * o], oc = (long long)tot[2 * o + 1];
-        const bool less = (om != m) ? (om < m) : ((oc != c) ? (oc < c) : (o < z));
+        const unsigned long long* u = tot + (size_t)kZoneTotWords * o;
+        const ExactSum om = exact_sum(u[0], u[1]), oc = exact_sum(u[2], u[3]);
+        const int by_mem = exact_cmp(om, m), by_cpu = exact_cmp(oc, c);
+        const bool less = by_mem ? by_mem < 0 : (by_cpu ? by_cpu < 0 : o < z);
         p += less ? 1 : 0;
     }
     prio[z] = p;
@@ -226,41 +273,60 @@ __global__ void gp_label_scatter(const int32_t* __restrict__ count_ptr, const in
 // usage[node] = sum of the resources of every (hard or soft) reservation on that node: UsageForNodes
 // (LIB/resources/resources.go:31-43) + UsedSoftReservationResources (internal/cache/softreservations.go:155-170),
 // summed as in GetReservedResources (EXT/resourcereservations.go:258-263).  A segmented reduction over
-// (reservation -> node) pairs: thread per reservation, 64-bit atomics (integer adds commute: exact).
+// (reservation -> node) pairs: thread per reservation, exact_add per dimension (integer adds commute: exact, and no
+// sum wraps).  usage[(2 * d + half) * n_nodes + node]: dimension d, half 0 = lo, 1 = hi.
 __global__ void gp_usage_scatter(long long n_res, const int32_t* __restrict__ res_node, const long long* __restrict__ res_cpu,
                                  const long long* __restrict__ res_mem, const long long* __restrict__ res_gpu, int32_t n_nodes,
-                                 unsigned long long* __restrict__ usage /* [3][n_nodes] */, unsigned int* __restrict__ has_entry /* [n_nodes] or NULL */) {
+                                 unsigned long long* __restrict__ usage /* [6][n_nodes] */, unsigned int* __restrict__ has_entry /* [n_nodes] or NULL */,
+                                 int* __restrict__ err) {
     const long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (r >= n_res) return;
     const int32_t node = res_node[r];
     if (node < 0 || node >= n_nodes) return;            // reservation on a node that is not in the list: ignored (:67-75)
     if (has_entry) has_entry[node] = 1u;                // the usage map has an entry for this node (whatever its value)
-    atomicAdd(usage + node, (unsigned long long)res_cpu[r]);
-    atomicAdd(usage + n_nodes + node, (unsigned long long)res_mem[r]);
-    if (res_gpu) atomicAdd(usage + 2 * (size_t)n_nodes + node, (unsigned long long)res_gpu[r]);
+    const long long v[3] = {res_cpu[r], res_mem[r], res_gpu ? res_gpu[r] : 0};
+    const size_t N = (size_t)n_nodes;
+    bool bad = false;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        bad |= !in_domain(v[d]);
+        exact_add(usage + (size_t)(2 * d) * N + node, usage + (size_t)(2 * d + 1) * N + node, v[d]);
+    }
+    if (bad) atomicOr(err, kFeErrInput);
 }
 
 // NodeSchedulingMetadataForNodes (resources.go:61-100): available = allocatable - (usage + overhead),
-// schedulable = allocatable - overhead.
+// schedulable = allocatable - overhead.  Inputs and usage sums inside the domain keep every expression below 2^63, so
+// nothing wraps before it is checked; whatever leaves the domain is reported in *err and the rows written are then not results.
 __global__ void gp_availability(int32_t n, const long long* __restrict__ alloc_cpu, const long long* __restrict__ alloc_mem,
                                 const long long* __restrict__ alloc_gpu, const long long* __restrict__ over_cpu,
                                 const long long* __restrict__ over_mem, const long long* __restrict__ over_gpu,
-                                const unsigned long long* __restrict__ usage, long long* __restrict__ avail /* [3][n] */,
-                                long long* __restrict__ sched /* [3][n] */, const unsigned int* __restrict__ has_entry = nullptr,
-                                long long* __restrict__ resched /* [3][n] or NULL */ = nullptr) {
+                                const unsigned long long* __restrict__ usage /* [6][n] */, long long* __restrict__ avail /* [3][n] */,
+                                long long* __restrict__ sched /* [3][n] */, int* __restrict__ err,
+                                const unsigned int* __restrict__ has_entry = nullptr, long long* __restrict__ resched /* [3][n] or NULL */ = nullptr) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const long long a[3] = {alloc_cpu[i], alloc_mem[i], alloc_gpu ? alloc_gpu[i] : 0};
     const long long o[3] = {over_cpu ? over_cpu[i] : 0, over_mem ? over_mem[i] : 0, over_gpu ? over_gpu[i] : 0};
+    int bad = 0;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-        const long long u = (long long)usage[(size_t)d * n + i];
-        avail[(size_t)d * n + i] = a[d] - (u + o[d]);
-        sched[(size_t)d * n + i] = a[d] - o[d];
-        // availableResources of rescheduleExecutor (EXT/resource.go:638-643): NodeSchedulingMetadataForNodes has already added
-        // the overhead into the usage map's EXISTING entries in place when usage.Add(overhead) adds it again (SURVEY App. B7)
-        if (resched) resched[(size_t)d * n + i] = a[d] - (u + o[d] * (has_entry[i] ? 2 : 1));
+        long long u = 0, av = 0, sc = 0, rs = 0;
+        if (!in_domain(a[d]) || !in_domain(o[d])) bad |= kFeErrInput;
+        else if (!exact_value(exact_sum(usage[(size_t)(2 * d) * n + i], usage[(size_t)(2 * d + 1) * n + i]), &u)) bad |= kFeErrResult;
+        else {
+            av = a[d] - (u + o[d]);
+            sc = a[d] - o[d];
+            // availableResources of rescheduleExecutor (EXT/resource.go:638-643): NodeSchedulingMetadataForNodes has already added
+            // the overhead into the usage map's EXISTING entries in place when usage.Add(overhead) adds it again (SURVEY App. B7)
+            rs = resched ? a[d] - (u + o[d] * (has_entry[i] ? 2 : 1)) : 0;
+            if (!in_domain(av) || !in_domain(sc) || !in_domain(rs)) bad |= kFeErrResult;
+        }
+        avail[(size_t)d * n + i] = av;
+        sched[(size_t)d * n + i] = sc;
+        if (resched) resched[(size_t)d * n + i] = rs;
     }
+    if (bad) atomicOr(err, bad);
 }
 
 }  // namespace gp

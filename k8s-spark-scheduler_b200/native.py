@@ -576,7 +576,9 @@ class GangPacker:
 
     # ---- availability snapshot from reservations (NodeSchedulingMetadataForNodes) ----------------
     def build_availability(self, alloc, overhead, res_node, res):
-        """alloc / overhead / res: (cpu, mem, gpu) triples (overhead may be None) -> (avail triple, sched triple)."""
+        """alloc / overhead / res: (cpu, mem, gpu) triples (overhead may be None) -> (avail triple, sched triple).
+        Exact or refused: |allocatable|, |overhead|, a counted |reservation|, a node's exact reservation sum or a result
+        >= 2^61 raises GangpackError with GP_ERR_UNREPRESENTABLE; nothing is computed modulo 2^64."""
         ui = _usage_input(alloc, overhead, res_node, res)
         n = ui.n_nodes
         outs = [np.empty(max(n, 1), np.int64) for _ in range(6)]
@@ -584,7 +586,8 @@ class GangPacker:
         return [o[:n] for o in outs[:3]], [o[:n] for o in outs[3:]]
 
     def build_reschedule_availability(self, alloc, overhead, res_node, res):
-        """availableResources of rescheduleExecutor's first-fit branch (overhead counted twice on nodes with reservations)."""
+        """availableResources of rescheduleExecutor's first-fit branch (overhead counted twice on nodes with a reservation row,
+        whatever its resources).  The domain and its refusal as in build_availability."""
         ui = _usage_input(alloc, overhead, res_node, res)
         n = ui.n_nodes
         outs = [np.empty(max(n, 1), np.int64) for _ in range(3)]
@@ -598,7 +601,8 @@ class GangPacker:
         alloc / overhead / res / exe: (cpu, mem, gpu) triples (overhead and the gpu entries may be None); hosting: per-executor
         lists of node indices already hosting executors of the same application, or None; keep_topology_zone: None (every
         node) or the zone id filterNodesToZone keeps, with topology_zone[n] the node's zone id (-1 = label missing).
-        The context's snapshot is not touched.  -> (node index per executor or -1, ambiguous flag per executor)."""
+        The context's snapshot is not touched.  The domain and its refusal as in build_availability; name_rank must be a
+        permutation (GP_ERR_INVALID).  -> (node index per executor or -1, ambiguous flag per executor)."""
         ui = _usage_input(alloc, overhead, res_node, res)
         n = ui.n_nodes
         si = _sort_input(n, n_zones, zone_id=zone_id, name_rank=name_rank, unschedulable=unschedulable, ready=ready,
@@ -621,7 +625,9 @@ class GangPacker:
 
     def prepare_cluster(self, alloc, overhead, res_node, res, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None):
-        """reservations -> availability -> priority orders -> snapshot, chained on the device.  -> (n_driver, n_executor)."""
+        """reservations -> availability -> priority orders -> snapshot, chained on the device.  -> (n_driver, n_executor).
+        A quantity, reservation sum or availability outside the exact-int64 domain (|v| >= 2^61) raises GangpackError
+        (GP_ERR_UNREPRESENTABLE) and the snapshot the context held stays in place."""
         ui = _usage_input(alloc, overhead, res_node, res)
         n = ui.n_nodes
         si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
@@ -636,7 +642,8 @@ class GangPacker:
                               layout=True):
         """reservations -> availability -> priority orders -> zone-grouped snapshot (kind LAYOUT_SINGLE_AZ or LAYOUT_AZ_AWARE),
         chained on the device, SchedulableResources included.  -> dict with n_zones, n_groups, n_driver, n_executor,
-        zone_of_group, undefined_ties and, with `layout`, the grouped exec_off / exec_order / drv_off / drv_order."""
+        zone_of_group, undefined_ties and, with `layout`, the grouped exec_off / exec_order / drv_off / drv_order.
+        The domain and its refusal as in prepare_cluster: a refused call leaves the context as it was."""
         ui = _usage_input(alloc, overhead, res_node, res)
         n = ui.n_nodes
         ties = C.c_int32(0)
@@ -660,7 +667,8 @@ class GangPacker:
     def potential_nodes(self, avail_cpu, avail_mem, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None, avail_gpu=None):
         """-> (driver_order, executor_order) as int32 node-index arrays.  With avail_gpu given, self.undefined_ties is the
-        number of adjacent pairs the reference's comparator leaves undefined (SURVEY App. B6)."""
+        number of adjacent pairs the reference's comparator leaves undefined (SURVEY App. B6).  Any int64 availability is
+        ordered exactly (zone totals included); name_rank must be a permutation of 0..n-1 (GP_ERR_INVALID)."""
         n = len(avail_cpu)
         ties = C.c_int32(0)
         si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,

@@ -140,6 +140,8 @@ SORT_CASES = {
     "negative zone_id": (dict(zone_id=(0, -1, 1, 0)), "zone_id out of range"),
     "name_rank >= n_nodes": (dict(name_rank=(0, 4, 1, 2)), "name_rank out of range"),
     "negative name_rank": (dict(name_rank=(0, -1, 1, 2)), "name_rank out of range"),
+    "name_rank given twice": (dict(name_rank=(0, 1, 1, 2)), "name_rank is not a permutation"),
+    "name_rank all equal": (dict(name_rank=(3, 3, 3, 3)), "name_rank is not a permutation"),
 }
 
 
