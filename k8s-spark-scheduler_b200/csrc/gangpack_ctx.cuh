@@ -41,17 +41,61 @@ struct DevBuf {
     template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-// One staging layout in one DevBuf: take() every piece (256-byte-aligned offsets), then reserve() once.
+// n elements of T at an offset of an Arena
+template <typename T> struct Piece {
+    size_t off, n;
+    Piece part(size_t first, size_t count) const { return {off + sizeof(T) * first, count}; }   // elements [first, first + count)
+};
+
+// One staging layout in one DevBuf, enqueued on one stream: take() every piece (256-byte-aligned offsets), then reserve()
+// once.  The first CUDA error of a helper is kept and every later helper does nothing: the entry calls check() (or sync())
+// before its first launch and before it reads anything back.  A piece of 0 elements issues no copy or memset.
 struct Arena {
     DevBuf& buf;
+    cudaStream_t st;
     size_t size = 0;
-    size_t take(size_t bytes) { const size_t o = size; size += (bytes + 255) & ~(size_t)255; return o; }
-    cudaError_t reserve() { return buf.reserve(size); }
-    char* base() const { return buf.as<char>(); }
-    cudaError_t upload(size_t off, const void* src, size_t bytes, cudaStream_t st) const {
-        return cudaMemcpyAsync(base() + off, src, bytes, cudaMemcpyHostToDevice, st);
+    cudaError_t err = cudaSuccess;
+    const char* op = nullptr;                    // the helper that met err
+
+    template <typename T> Piece<T> take(size_t n) {
+        const Piece<T> p{size, n};
+        size += (sizeof(T) * n + 255) & ~(size_t)255;
+        return p;
     }
+    void reserve() { if (!err) keep(buf.reserve(size), "reserve"); }
+    template <typename T> T* ptr(Piece<T> p) const { return reinterpret_cast<T*>(buf.as<char>() + p.off); }
+    // the device copy of `host`, or NULL when host is NULL (an absent optional column).  U differs from T only in name
+    // (int64_t columns staged as the kernels' long long).
+    template <typename T, typename U> T* put(Piece<T> p, const U* host) {
+        static_assert(sizeof(T) == sizeof(U), "a piece is uploaded from elements of its own size");
+        if (!host) return nullptr;
+        if (!err && p.n) keep(cudaMemcpyAsync(ptr(p), host, sizeof(T) * p.n, cudaMemcpyHostToDevice, st), "upload");
+        return ptr(p);
+    }
+    template <typename T, typename U> T* put_or_zero(Piece<T> p, const U* host) { return host ? put(p, host) : zero(p); }
+    template <typename T> T* fill(Piece<T> p, int byte) { return fill(p, p, byte); }
+    template <typename T> T* zero(Piece<T> p) { return fill(p, p, 0); }
+    // one memset over the pieces first .. last (taken in that order) and the padding between them
+    template <typename T, typename U> T* fill(Piece<T> first, Piece<U> last, int byte) {
+        const size_t bytes = last.off + sizeof(U) * last.n - first.off;
+        if (!err && bytes) keep(cudaMemsetAsync(ptr(first), byte, bytes, st), "memset");
+        return ptr(first);
+    }
+    // n elements of device memory to `host`; nothing when host is NULL or n is 0
+    template <typename U, typename T> void get(U* host, const T* dev, size_t n) {
+        static_assert(sizeof(T) == sizeof(U), "a piece is downloaded into elements of its own size");
+        if (!err && host && n) keep(cudaMemcpyAsync(host, dev, sizeof(T) * n, cudaMemcpyDeviceToHost, st), "download");
+    }
+    template <typename U, typename T> void get(U* host, Piece<T> p) { get(host, ptr(p), p.n); }
+    gp_status check(gp_ctx* c) const;
+    gp_status sync(gp_ctx* c) { if (!err) keep(cudaStreamSynchronize(st), "synchronise"); return check(c); }
+
+private:
+    void keep(cudaError_t e, const char* what) { if (e != cudaSuccess) { err = e; op = what; } }
 };
+
+// A status word's bit family decoded by refuse(): the first entry of a table, in table order, whose bits are set
+struct Refusal { int bits; gp_status status; const char* what; };
 
 // A fixed sequence of kernel launches / memsets that repeats with identical arguments (one Predicate after the other:
 // same buffers, same batch shape) is captured ONCE into a CUDA graph and replayed with a single launch call -- the
@@ -113,7 +157,7 @@ struct gp_ctx {
 
     // batch staging; a_rows: the six quantity rows in one pitched block (pack_batch_impl)
     DevBuf a_rows, a_count, a_group, a_skip, a_off;
-    DevBuf prep, r_driver, r_exec, scratch, dev_misc, gmin, sortbuf, usagebuf, reschedbuf;
+    DevBuf prep, r_driver, r_exec, scratch, dev_misc, gmin, sortbuf, usagebuf;
     void* pinned_misc = nullptr;                  // PinnedStatus
     DevStatus* status() const { return dev_misc.as<DevStatus>(); }
     PinnedStatus* host_status() const { return static_cast<PinnedStatus*>(pinned_misc); }
@@ -158,10 +202,10 @@ struct gp_ctx {
     // lengths and n_zones as DEVICE pointers for gp_pack_*_az_aware(orders == NULL); zone_kind = the gp_zone_layout_kind of the
     // current snapshot, -1 when another entry laid it out
     DevBuf zoneprep;
-    DevBuf reschedprep;                           // gp_reschedule_from_reservations' own scratch (no state points into it)
-    DevBuf capprep;                               // gp_exceeds_cluster_capacity's own scratch (no state points into it)
-    DevBuf reconbuf;                              // gp_reconcile_find_nodes' own scratch (no state points into it)
-    DevBuf overbuf;                               // gp_node_overhead's own scratch (no state points into it)
+    // The own scratch of one call of gp_reschedule_executors, gp_reschedule_from_reservations, gp_exceeds_cluster_capacity*,
+    // gp_match_node_affinity, gp_reconcile_find_nodes or gp_node_overhead: no state points into it, and the next call's
+    // use is ordered after this one's kernels on the context's stream
+    DevBuf callbuf;
     int zone_kind = -1;
     gp_az_orders zone_orders{};
     bool sort_attr_set = false;
@@ -179,6 +223,31 @@ struct gp_ctx {
             return GP_ERR_CUDA;                                                                \
         }                                                                                      \
     } while (0)
+
+#define GP_TRY(expr)                                                                           \
+    do {                                                                                       \
+        const gp_status _s = (expr);                                                           \
+        if (_s != GP_OK) return _s;                                                            \
+    } while (0)
+
+gp_status fail(gp_ctx* ctx, gp_status st, const std::string& msg);
+static inline gp_status fail(gp_ctx* c, gp_status st, const char* who, const char* what) {
+    return fail(c, st, std::string(who) + ": " + what);
+}
+
+inline gp_status Arena::check(gp_ctx* c) const {
+    if (!err) return GP_OK;
+    c->err = std::string("staging ") + op + ": " + cudaGetErrorString(err);
+    return GP_ERR_CUDA;
+}
+
+// `who: what` of the first entry of `table` whose bits are set in `word`; GP_OK when there is none
+template <size_t K>
+static gp_status refuse(gp_ctx* c, int word, const Refusal (&table)[K], const char* who) {
+    for (const Refusal& r : table)
+        if (word & r.bits) return fail(c, r.status, who, r.what);
+    return GP_OK;
+}
 
 // issue(): enqueues the sequence on `st` and returns (status, launches).  See GraphCache.
 template <class F>
@@ -240,7 +309,6 @@ __global__ void gp_scatter_slots(int32_t n_slots, const longlong2* __restrict__ 
                                  int64_t* __restrict__ cpu, int64_t* __restrict__ mem, int64_t* __restrict__ gpu);
 
 const void* mapped_ptr(gp_ctx* c, const void* p, size_t bytes);
-gp_status fail(gp_ctx* ctx, gp_status st, const std::string& msg);
 Snapshot make_snapshot(const gp_ctx* c);
 gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, cudaStream_t st,
                                 bool copy_nodes = false);

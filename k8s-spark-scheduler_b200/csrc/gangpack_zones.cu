@@ -23,15 +23,13 @@ gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, 
         const int64_t v[3] = {cpu[i], mem[i], gpu ? gpu[i] : 0};
         for (int64_t x : v) if (x >= kMaxQuantity || x <= -kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, "gp_set_schedulable: |quantity| >= 2^61");
     }
-    GP_CUDA(c, c->sched.reserve(24 * (N + 1)));
-    char* b = c->sched.as<char>();
-    if (N) {
-        GP_CUDA(c, cudaMemcpyAsync(b, cpu, 8 * N, cudaMemcpyHostToDevice, c->stream));
-        GP_CUDA(c, cudaMemcpyAsync(b + 8 * N, mem, 8 * N, cudaMemcpyHostToDevice, c->stream));
-        if (gpu) GP_CUDA(c, cudaMemcpyAsync(b + 16 * N, gpu, 8 * N, cudaMemcpyHostToDevice, c->stream));
-        else GP_CUDA(c, cudaMemsetAsync(b + 16 * N, 0, 8 * N, c->stream));
-    }
-    GP_CUDA(c, cudaStreamSynchronize(c->stream));
+    Arena ar{c->sched, c->stream};
+    const auto sched = ar.take<long long>(3 * (N + 1));
+    ar.reserve();
+    ar.put(sched.part(0, N), cpu);
+    ar.put(sched.part(N, N), mem);
+    ar.put_or_zero(sched.part(2 * N, N), gpu);
+    GP_TRY(ar.sync(c));
     c->have_sched = true;
     c->have_eff_sched = true;
     return GP_OK;
@@ -43,53 +41,48 @@ static bool has_zone_arrays(const gp_apps* a, const gp_zone_results* out) {
     return a->drv_cpu_milli && a->drv_mem_bytes && a->exe_cpu_milli && a->exe_mem_bytes && a->exe_count && out->zone && out->driver_node;
 }
 
-// The six int64 quantity columns (6 x n_apps from o_in; absent gpu columns stay NULL = 0 in `six`), exe_count to o_cnt
-// and the ExecutorNodes offsets `off` to o_off
-static gp_status upload_app_columns(gp_ctx* c, const gp_apps* a, const int64_t* off, char* b, size_t o_in, size_t o_cnt, size_t o_off,
-                                    cudaStream_t st, SixCols* six) {
+// Uploads the six int64 quantity columns (6 x n_apps of `in`; absent gpu columns stay NULL = 0 in the result), exe_count
+// and the ExecutorNodes offsets `off`
+static SixCols upload_app_columns(Arena& ar, const gp_apps* a, const int64_t* off, Piece<int64_t> in, Piece<int32_t> cnt,
+                                  Piece<int64_t> d_off) {
     const size_t q = (size_t)a->n_apps;
     const int64_t* hc[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
-    *six = SixCols{};
-    for (int k = 0; k < 6; ++k) {
-        if (!hc[k]) continue;
-        int64_t* d = reinterpret_cast<int64_t*>(b + o_in) + q * (size_t)k;
-        GP_CUDA(c, cudaMemcpyAsync(d, hc[k], 8 * q, cudaMemcpyHostToDevice, st));
-        six->p[k] = d;
-    }
-    GP_CUDA(c, cudaMemcpyAsync(b + o_cnt, a->exe_count, 4 * q, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_off, off, 8 * (q + 1), cudaMemcpyHostToDevice, st));
-    return GP_OK;
+    SixCols six{};
+    for (int k = 0; k < 6; ++k) six.p[k] = ar.put(in.part(q * k, q), hc[k]);
+    ar.put(cnt, a->exe_count);
+    ar.put(d_off, off);
+    return six;
 }
 
 // az-aware-tightly-pack: upload the undivided orders and build the fallback's gather view of them (gp_build_fallback_view).
 // on_device: az's orders are device arrays (gp_prepare_cluster_zones' held orders) and are read in place.
 static gp_status stage_fallback_view(gp_ctx* c, const gp_az_orders* az, bool on_device, cudaStream_t st, GatherSlots* fb) {
     const size_t ne = (size_t)az->n_exec, nd = (size_t)az->n_drv;
-    Arena ar{c->fbview};
-    const size_t o_eord = ar.take(on_device ? 0 : 4 * ne), o_dord = ar.take(on_device ? 0 : 4 * nd), o_npos = ar.take(4 * (size_t)c->n_nodes),
-                 o_fbe = ar.take(4 * ne), o_fbd = ar.take(4 * nd), o_fbp = ar.take(4 * nd);
-    GP_CUDA(c, ar.reserve());
-    char* b = ar.base();
-    const int32_t* eord = on_device ? az->exec_order : (const int32_t*)(b + o_eord);
-    const int32_t* dord = on_device ? az->drv_order : (const int32_t*)(b + o_dord);
-    if (!on_device && ne) GP_CUDA(c, cudaMemcpyAsync(b + o_eord, az->exec_order, 4 * ne, cudaMemcpyHostToDevice, st));
-    if (!on_device && nd) GP_CUDA(c, cudaMemcpyAsync(b + o_dord, az->drv_order, 4 * nd, cudaMemcpyHostToDevice, st));
-    gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)ne, (int32_t)nd, eord, dord,
-                                               c->node_slot.as<int32_t>(), (int32_t*)(b + o_npos), (int32_t*)(b + o_fbe), (int32_t*)(b + o_fbd),
-                                               (int32_t*)(b + o_fbp));
+    Arena ar{c->fbview, st};
+    const auto eord = ar.take<int32_t>(on_device ? 0 : ne), dord = ar.take<int32_t>(on_device ? 0 : nd),
+               npos = ar.take<int32_t>((size_t)c->n_nodes), fbe = ar.take<int32_t>(ne), fbd = ar.take<int32_t>(nd), fbp = ar.take<int32_t>(nd);
+    ar.reserve();
+    if (!on_device) {
+        ar.put(eord, az->exec_order);
+        ar.put(dord, az->drv_order);
+    }
+    GP_TRY(ar.check(c));
+    gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)ne, (int32_t)nd, on_device ? az->exec_order : ar.ptr(eord),
+                                               on_device ? az->drv_order : ar.ptr(dord), c->node_slot.as<int32_t>(), ar.ptr(npos),
+                                               ar.ptr(fbe), ar.ptr(fbd), ar.ptr(fbp));
     c->last.kernel_launches += 1;
-    *fb = GatherSlots{(const int32_t*)(b + o_fbe), (const int32_t*)(b + o_fbd), (const int32_t*)(b + o_fbp), (int32_t)ne, (int32_t)nd};
+    *fb = GatherSlots{ar.ptr(fbe), ar.ptr(fbd), ar.ptr(fbp), (int32_t)ne, (int32_t)nd};
     return GP_OK;
 }
 
 // zone / driver / ExecutorNodes (T entries) / averages to the host, one synchronise, then the kernels' validation errors
-static gp_status finish_zone_results(gp_ctx* c, gp_zone_results* out, const int32_t* zone, const int32_t* drv, const int32_t* exe,
-                                     const double* avg, size_t q, size_t T, cudaStream_t st) {
-    GP_CUDA(c, cudaMemcpyAsync(out->zone, zone, 4 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaMemcpyAsync(out->driver_node, drv, 4 * q, cudaMemcpyDeviceToHost, st));
-    if (T) GP_CUDA(c, cudaMemcpyAsync(out->executor_nodes, exe, 4 * T, cudaMemcpyDeviceToHost, st));
-    if (out->avg_efficiency) GP_CUDA(c, cudaMemcpyAsync(out->avg_efficiency, avg, 32 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaStreamSynchronize(st));
+static gp_status finish_zone_results(gp_ctx* c, Arena& ar, gp_zone_results* out, Piece<int32_t> zone, Piece<int32_t> drv,
+                                     Piece<int32_t> exe, Piece<double> avg, size_t T) {
+    ar.get(out->zone, zone);
+    ar.get(out->driver_node, drv);
+    ar.get(out->executor_nodes, exe.part(0, T));
+    ar.get(out->avg_efficiency, avg);
+    GP_TRY(ar.sync(c));
     return host_error(c);
 }
 
@@ -98,11 +91,10 @@ static gp_status finish_zone_results(gp_ctx* c, gp_zone_results* out, const int3
 // validated; az_dev: they are device arrays).  Argument checks common to both are here.
 static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int32_t Z, const gp_az_orders* az, bool az_dev,
                                  gp_zone_results* out, const char* who) {
-    const std::string w(who);
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
-    if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
-    if ((int64_t)Q * Z > 0x7fffffffLL) return fail(c, GP_ERR_INVALID, w + ": n_apps x zones too large");
+    if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, who, "missing app/result arrays");
+    if ((int64_t)Q * Z > 0x7fffffffLL) return fail(c, GP_ERR_INVALID, who, "n_apps x zones too large");
     const int64_t* off = a->exec_out_off;
     if (!off) {
         c->host_off.resize((size_t)Q + 1);
@@ -112,52 +104,54 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
         off = c->host_off.data();
     }
     const int64_t total = off[Q];
-    if (total < 0 || total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, w + ": executor_nodes_cap too small");
-    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, w + ": executor_nodes is NULL");
+    if (total < 0 || total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, who, "executor_nodes_cap too small");
+    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, who, "executor_nodes is NULL");
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t q = (size_t)Q, R = q * (size_t)Z, T = (size_t)total;
-    Arena ar{c->zonebuf};
-    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_rows = ar.take(48 * R), o_rcnt = ar.take(4 * R),
-                 o_rgrp = ar.take(4 * R), o_roff = ar.take(8 * (R + 1)), o_rdrv = ar.take(4 * R), o_rexe = ar.take(4 * ((size_t)Z * T + 1)),
-                 o_zone = ar.take(4 * q), o_drv = ar.take(4 * q), o_exe = ar.take(4 * (T + 1)), o_avg = ar.take(32 * q);
+    Arena ar{c->zonebuf, st};
+    const auto in = ar.take<int64_t>(6 * q);
+    const auto cnt = ar.take<int32_t>(q);
+    const auto off_p = ar.take<int64_t>(q + 1), rows = ar.take<int64_t>(6 * R);
+    const auto rcnt = ar.take<int32_t>(R), rgrp = ar.take<int32_t>(R);
+    const auto roff = ar.take<int64_t>(R + 1);
+    const auto rdrv = ar.take<int32_t>(R), rexe = ar.take<int32_t>((size_t)Z * T + 1), zone = ar.take<int32_t>(q), drv = ar.take<int32_t>(q),
+               exe = ar.take<int32_t>(T + 1);
+    const auto avg = ar.take<double>(4 * q);
     // az-aware: the fallback's PrepApp records and list
     const size_t QF = az ? q : 0;
-    const size_t o_prep = ar.take(sizeof(PrepApp) * QF), o_list = ar.take(4 * QF);
-    GP_CUDA(c, ar.reserve());
-    char* b = ar.base();
-    SixCols six;
-    gp_status s = upload_app_columns(c, a, off, b, o_in, o_cnt, o_off, st, &six);
-    if (s != GP_OK) return s;
+    const auto prep = ar.take<PrepApp>(QF);
+    const auto list = ar.take<int32_t>(QF);
+    ar.reserve();
+    const SixCols six = upload_app_columns(ar, a, off, in, cnt, off_p);
+    GP_TRY(ar.check(c));
     const int TH = 256;
     // the efficiencies read the availability in node-table order: refresh that copy from the slots (a FIFO batch may
     // have charged them since gp_set_snapshot)
     if (c->n_slots > 0)
         gp_scatter_slots<<<(c->n_slots + TH - 1) / TH, TH, 0, st>>>(c->n_slots, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(), c->slot_node.as<int32_t>(),
                                                                    c->node_cpu.as<int64_t>(), c->node_mem.as<int64_t>(), c->node_gpu.as<int64_t>());
-    gp_zone_expand<<<(unsigned)((R + 1 + TH - 1) / TH), TH, 0, st>>>(Q, Z, six, (const int32_t*)(b + o_cnt), (const int64_t*)(b + o_off),
-                                                                      (int64_t*)(b + o_rows), (int32_t*)(b + o_rcnt), (int32_t*)(b + o_rgrp), (int64_t*)(b + o_roff));
+    gp_zone_expand<<<(unsigned)((R + 1 + TH - 1) / TH), TH, 0, st>>>(Q, Z, six, ar.ptr(cnt), ar.ptr(off_p), ar.ptr(rows), ar.ptr(rcnt),
+                                                                      ar.ptr(rgrp), ar.ptr(roff));
     int2* scratch = nullptr;
-    s = pack_begin(c, (int32_t)R, algo, GP_MODE_INDEPENDENT, (int64_t)Z * total, false, &scratch, st);
-    if (s != GP_OK) return s;
+    GP_TRY(pack_begin(c, (int32_t)R, algo, GP_MODE_INDEPENDENT, (int64_t)Z * total, false, &scratch, st));
     DevApps dv{};
-    for (int k = 0; k < 6; ++k) dv.cols.q[k] = b + o_rows + 8 * R * (size_t)k;
-    dv.cols.count = (const int32_t*)(b + o_rcnt); dv.cols.group = (const int32_t*)(b + o_rgrp); dv.cols.off = (const int64_t*)(b + o_roff);
+    for (int k = 0; k < 6; ++k) dv.cols.q[k] = ar.ptr(rows) + R * (size_t)k;
+    dv.cols.count = ar.ptr(rcnt); dv.cols.group = ar.ptr(rgrp); dv.cols.off = ar.ptr(roff);
     dv.cols.bits = 64; dv.cols.mem_shift = 0; dv.skip = nullptr; dv.n = (int32_t)R;
-    DevResults dr{(int32_t*)(b + o_rdrv), b + o_rexe, (int64_t)Z * total, 32};
-    s = pack_device_range(c, dv, 0, (int32_t)R, 0, algo, GP_MODE_INDEPENDENT, dr, scratch, st, 0);
-    if (s != GP_OK) return s;
+    DevResults dr{ar.ptr(rdrv), ar.ptr(rexe), (int64_t)Z * total, 32};
+    GP_TRY(pack_device_range(c, dv, 0, (int32_t)R, 0, algo, GP_MODE_INDEPENDENT, dr, scratch, st, 0));
     c->ev_chunks = 1;
     ZoneChooseIn zi{};
     const size_t N = (size_t)c->n_nodes;
     zi.avail[0] = c->node_cpu.as<long long>(); zi.avail[1] = c->node_mem.as<long long>(); zi.avail[2] = c->node_gpu.as<long long>();
     zi.sched[0] = c->sched.as<long long>(); zi.sched[1] = c->sched.as<long long>() + N; zi.sched[2] = c->sched.as<long long>() + 2 * N;
     for (int k = 0; k < 3; ++k) { zi.drv[k] = six.p[k]; zi.exe[k] = six.p[3 + k]; }
-    zi.count = (const int32_t*)(b + o_cnt); zi.out_off = (const int64_t*)(b + o_off);
-    zi.row_driver = (const int32_t*)(b + o_rdrv); zi.row_exec = (const int32_t*)(b + o_rexe);
+    zi.count = ar.ptr(cnt); zi.out_off = ar.ptr(off_p);
+    zi.row_driver = ar.ptr(rdrv); zi.row_exec = ar.ptr(rexe);
     zi.n_apps = Q; zi.n_zones = Z; zi.executors_reserved = algo == GP_TIGHTLY_PACK ? 1 : 0;
-    gp_zone_choose<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(zi, (int32_t*)(b + o_zone), (int32_t*)(b + o_drv), (int32_t*)(b + o_exe),
-                                                                       out->avg_efficiency ? (double*)(b + o_avg) : nullptr);
+    gp_zone_choose<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(zi, ar.ptr(zone), ar.ptr(drv), ar.ptr(exe),
+                                                                       out->avg_efficiency ? ar.ptr(avg) : nullptr);
     GP_CUDA(c, cudaGetLastError());
     c->last.kernel_launches += 2;
     if (az) {
@@ -167,17 +161,15 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
         DevStatus* ds = c->status();
         unsigned long long* d_stats = ds->head.stats;
         GP_CUDA(c, cudaMemsetAsync(d_stats + 2, 0, 16, st));
-        int32_t* listed = (int32_t*)(b + o_list);
-        gp_az_fallback_list<<<(unsigned)((q + TH - 1) / TH), TH, 0, st>>>(Q, (const int32_t*)(b + o_zone), listed, &ds->az_listed);
+        int32_t* listed = ar.ptr(list);
+        gp_az_fallback_list<<<(unsigned)((q + TH - 1) / TH), TH, 0, st>>>(Q, ar.ptr(zone), listed, &ds->az_listed);
         AppColumns cols{};
         for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
-        cols.count = (const int32_t*)(b + o_cnt); cols.group = nullptr; cols.off = (const int64_t*)(b + o_off); cols.bits = 64; cols.mem_shift = 0;
-        PrepApp* prep = (PrepApp*)(b + o_prep);
+        cols.count = ar.ptr(cnt); cols.group = nullptr; cols.off = ar.ptr(off_p); cols.bits = 64; cols.mem_shift = 0;
         gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
-            Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, &ds->head.err, &c->host_status()->err_word);
+            Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, ar.ptr(prep), &ds->head.err, &c->host_status()->err_word);
         GatherSlots fb;
-        s = stage_fallback_view(c, az, az_dev, st, &fb);
-        if (s != GP_OK) return s;
+        GP_TRY(stage_fallback_view(c, az, az_dev, st, &fb));
         int& per_sm = c->az_fallback_ctas_per_sm;
         if (per_sm == 0) {
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_az_fallback, kAzFallbackThreads, 0);
@@ -185,13 +177,12 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
         }
         int64_t blocks = ((int64_t)Q * 32 + kAzFallbackThreads - 1) / kAzFallbackThreads;   // the list holds at most Q
         if (blocks > (int64_t)c->sm_count * per_sm) blocks = (int64_t)c->sm_count * per_sm;
-        gp_pack_az_fallback<<<(unsigned)blocks, kAzFallbackThreads, 0, st>>>(make_snapshot(c), prep, listed, &ds->az_listed, fb, (int32_t*)(b + o_drv),
-                                                                            (int32_t*)(b + o_exe), d_stats, &ds->az_claim);
+        gp_pack_az_fallback<<<(unsigned)blocks, kAzFallbackThreads, 0, st>>>(make_snapshot(c), ar.ptr(prep), listed, &ds->az_listed, fb, ar.ptr(drv),
+                                                                            ar.ptr(exe), d_stats, &ds->az_claim);
         GP_CUDA(c, cudaGetLastError());
         c->last.kernel_launches += 3;
     }
-    return finish_zone_results(c, out, (const int32_t*)(b + o_zone), (const int32_t*)(b + o_drv), (const int32_t*)(b + o_exe),
-                               (const double*)(b + o_avg), q, T, st);
+    return finish_zone_results(c, ar, out, zone, drv, exe, avg, T);
 }
 
 gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone_results* out) {
@@ -261,11 +252,10 @@ static gp_status check_az_orders(gp_ctx* c, const gp_az_orders* o, const char* w
 // The az-aware entries' NULL arguments.  orders == NULL stands for the undivided orders and n_zones gp_prepare_cluster_zones
 // (GP_LAYOUT_AZ_AWARE) left on the device -- *o then points at them; after any other snapshot it is refused.
 static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_results* out, const gp_az_orders** o, const char* who) {
-    const std::string w(who);
     if (!*o && c->zone_kind == GP_LAYOUT_SINGLE_AZ)
-        return fail(c, GP_ERR_INVALID, w + ": orders == NULL needs a gp_prepare_cluster_zones(GP_LAYOUT_AZ_AWARE) snapshot; this one is "
+        return fail(c, GP_ERR_INVALID, who, "orders == NULL needs a gp_prepare_cluster_zones(GP_LAYOUT_AZ_AWARE) snapshot; this one is "
                                            "GP_LAYOUT_SINGLE_AZ (no trailing group, no undivided orders)");
-    if (!a || !out || (!*o && c->zone_kind != GP_LAYOUT_AZ_AWARE) || a->n_apps < 0) return fail(c, GP_ERR_INVALID, w + ": NULL apps/orders/results");
+    if (!a || !out || (!*o && c->zone_kind != GP_LAYOUT_AZ_AWARE) || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/orders/results");
     if (!*o) *o = &c->zone_orders;
     return GP_OK;
 }
@@ -276,10 +266,9 @@ static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_resul
 // checks common to both are here.
 static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, int32_t Z, const gp_az_orders* az, bool az_dev,
                                 gp_zone_results* out, const char* who) {
-    const std::string w(who);
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
-    if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, w + ": missing app/result arrays");
+    if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, who, "missing app/result arrays");
     std::vector<int64_t>& hoff = c->host_off;
     hoff.resize((size_t)Q + 1);
     int64_t acc = 0, pitch = 1;
@@ -291,52 +280,51 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     hoff[(size_t)Q] = acc;
     if (a->exec_out_off)
         for (int32_t i = 0; i <= Q; ++i)
-            if (a->exec_out_off[i] != hoff[(size_t)i]) return fail(c, GP_ERR_INVALID, w + ": exec_out_off must be the prefix sum of exe_count (or NULL)");
+            if (a->exec_out_off[i] != hoff[(size_t)i]) return fail(c, GP_ERR_INVALID, who, "exec_out_off must be the prefix sum of exe_count (or NULL)");
     const int64_t total = acc;
-    if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, w + ": executor_nodes_cap too small");
-    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, w + ": executor_nodes is NULL");
+    if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, who, "executor_nodes_cap too small");
+    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, who, "executor_nodes is NULL");
     pitch = (pitch + 3) & ~(int64_t)3;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const bool azk = kind == kZoneAzAware;
     const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)(Z + (azk ? 1 : 0)) * (size_t)pitch;   // az-aware: row Z = fallback
-    Arena ar{c->zonebuf};
-    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_skip = ar.take(q), o_rexe = ar.take(4 * RP),
-                 o_rlist = ar.take(kind == GP_MINIMAL_FRAGMENTATION ? 8 * RP : 0), o_zone = ar.take(4 * q), o_drv = ar.take(4 * q),
-                 o_exe = ar.take(4 * (T + 1)), o_avg = ar.take(32 * q);
-    GP_CUDA(c, ar.reserve());
-    char* b = ar.base();
+    Arena ar{c->zonebuf, st};
+    const auto in = ar.take<int64_t>(6 * q);
+    const auto cnt = ar.take<int32_t>(q);
+    const auto off_p = ar.take<int64_t>(q + 1);
+    const auto skip = ar.take<uint8_t>(q);
+    const auto rexe = ar.take<int32_t>(RP);
+    const auto rlist = ar.take<int2>(kind == GP_MINIMAL_FRAGMENTATION ? RP : 0);
+    const auto zone = ar.take<int32_t>(q), drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1);
+    const auto avg_p = ar.take<double>(4 * q);
+    ar.reserve();
+    GP_TRY(ar.check(c));
     int2* unused = nullptr;
-    gp_status s = pack_begin(c, Q, GP_TIGHTLY_PACK, mode, total, false, &unused, st);
-    if (s != GP_OK) return s;
-    SixCols six;
-    s = upload_app_columns(c, a, hoff.data(), b, o_in, o_cnt, o_off, st, &six);
-    if (s != GP_OK) return s;
-    if (a->skip_if_no_fit) GP_CUDA(c, cudaMemcpyAsync(b + o_skip, a->skip_if_no_fit, q, cudaMemcpyHostToDevice, st));
+    GP_TRY(pack_begin(c, Q, GP_TIGHTLY_PACK, mode, total, false, &unused, st));
     AppColumns cols{};
+    const SixCols six = upload_app_columns(ar, a, hoff.data(), in, cnt, off_p);
+    const uint8_t* d_skip = ar.put(skip, a->skip_if_no_fit);
+    GP_TRY(ar.check(c));
     for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
-    cols.count = (const int32_t*)(b + o_cnt); cols.group = nullptr; cols.off = (const int64_t*)(b + o_off); cols.bits = 64; cols.mem_shift = 0;
+    cols.count = ar.ptr(cnt); cols.group = nullptr; cols.off = ar.ptr(off_p); cols.bits = 64; cols.mem_shift = 0;
     DevStatus* ds = c->status();
     unsigned long long* d_stats = ds->head.stats;
     PrepApp* prep = c->prep.as<PrepApp>();
     gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
-        Q, cols, a->skip_if_no_fit ? (const uint8_t*)(b + o_skip) : nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep,
-        &ds->head.err, &c->host_status()->err_word);
+        Q, cols, d_skip, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, &ds->head.err, &c->host_status()->err_word);
     Snapshot snap = make_snapshot(c);
     ZoneFifoIn zi{};
     const size_t N = (size_t)c->n_nodes;
     zi.sched[0] = c->sched.as<long long>(); zi.sched[1] = c->sched.as<long long>() + N; zi.sched[2] = c->sched.as<long long>() + 2 * N;
     zi.node_slot = c->node_slot.as<int32_t>();
-    zi.row_exec = (int32_t*)(b + o_rexe);
-    zi.row_list = kind == GP_MINIMAL_FRAGMENTATION ? (int2*)(b + o_rlist) : nullptr;
+    zi.row_exec = ar.ptr(rexe);
+    zi.row_list = kind == GP_MINIMAL_FRAGMENTATION ? ar.ptr(rlist) : nullptr;
     zi.row_pitch = pitch; zi.n_apps = Q; zi.n_zones = Z;
-    double* avg = out->avg_efficiency ? (double*)(b + o_avg) : nullptr;
-    int32_t* zo = (int32_t*)(b + o_zone); int32_t* dq = (int32_t*)(b + o_drv); int32_t* eo = (int32_t*)(b + o_exe);
+    double* avg = out->avg_efficiency ? ar.ptr(avg_p) : nullptr;
+    int32_t* zo = ar.ptr(zone); int32_t* dq = ar.ptr(drv); int32_t* eo = ar.ptr(exe);
     GatherSlots fb{};
-    if (azk) {
-        s = stage_fallback_view(c, az, az_dev, st, &fb);
-        if (s != GP_OK) return s;
-    }
+    if (azk) GP_TRY(stage_fallback_view(c, az, az_dev, st, &fb));
     if (kind == GP_TIGHTLY_PACK) {
         if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
         else gp_pack_fifo_zones_cta<0, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
@@ -349,9 +337,8 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     }
     GP_CUDA(c, cudaGetLastError());
     c->last.kernel_launches += 2;
-    s = refresh_views(c, st);                          // the compact view follows the charged slots
-    if (s != GP_OK) return s;
-    return finish_zone_results(c, out, zo, dq, eo, avg, q, T, st);
+    GP_TRY(refresh_views(c, st));                       // the compact view follows the charged slots
+    return finish_zone_results(c, ar, out, zone, drv, exe, avg_p, T);
 }
 
 // the FIFO loop with a single-AZ packer in one launch
@@ -445,35 +432,36 @@ gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* p
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t q = (size_t)Q, T = (size_t)(total > 0 ? total : 0), R = (size_t)rows;
-    Arena ar{c->zonebuf};
-    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_roff = ar.take(8 * (q + 1)), o_drv = ar.take(4 * q),
-                 o_exe = ar.take(4 * (T + 1)), o_ra = ar.take(4 * (R + 1)), o_rs = ar.take(4 * (R + 1)), o_rn = ar.take(4 * (R + 1)),
-                 o_rc = ar.take(8 * (R + 1)), o_rm = ar.take(8 * (R + 1)), o_rg = ar.take(8 * (R + 1));
-    GP_CUDA(c, ar.reserve());
-    char* b = ar.base();
+    Arena ar{c->zonebuf, st};
+    const auto in = ar.take<int64_t>(6 * q);
+    const auto cnt = ar.take<int32_t>(q);
+    const auto off_p = ar.take<int64_t>(q + 1), roff_p = ar.take<int64_t>(q + 1);
+    const auto drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1), ra = ar.take<int32_t>(R + 1), rs = ar.take<int32_t>(R + 1),
+               rn = ar.take<int32_t>(R + 1);
+    const auto rc = ar.take<long long>(R + 1), rm = ar.take<long long>(R + 1), rg = ar.take<long long>(R + 1);
+    ar.reserve();
     ReserveIn ri{};
-    gp_status s = upload_app_columns(c, a, off.data(), b, o_in, o_cnt, o_off, st, &ri.cols);
-    if (s != GP_OK) return s;
-    GP_CUDA(c, cudaMemcpyAsync(b + o_roff, roff, 8 * (q + 1), cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_drv, placed->driver_node, 4 * q, cudaMemcpyHostToDevice, st));
-    if (T) GP_CUDA(c, cudaMemcpyAsync(b + o_exe, placed->executor_nodes, 4 * T, cudaMemcpyHostToDevice, st));
-    ri.count = (const int32_t*)(b + o_cnt); ri.off = (const int64_t*)(b + o_off); ri.row_off = (const int64_t*)(b + o_roff);
-    ri.driver = (const int32_t*)(b + o_drv); ri.exec = (const int32_t*)(b + o_exe); ri.n_apps = Q; ri.subtract = subtract ? 1 : 0;
-    ReserveOut ro{(int32_t*)(b + o_ra), (int32_t*)(b + o_rs), (int32_t*)(b + o_rn), (long long*)(b + o_rc), (long long*)(b + o_rm), (long long*)(b + o_rg)};
+    ri.cols = upload_app_columns(ar, a, off.data(), in, cnt, off_p);
+    ri.row_off = ar.put(roff_p, roff);
+    ri.driver = ar.put(drv, placed->driver_node);
+    ar.put(exe.part(0, T), placed->executor_nodes);
+    GP_TRY(ar.check(c));
+    ri.count = ar.ptr(cnt); ri.off = ar.ptr(off_p); ri.exec = ar.ptr(exe); ri.n_apps = Q; ri.subtract = subtract ? 1 : 0;
+    ReserveOut ro{ar.ptr(ra), ar.ptr(rs), ar.ptr(rn), ar.ptr(rc), ar.ptr(rm), ar.ptr(rg)};
     const int TH = 256;
     gp_reserve_rows<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(ri, ro, c->node_slot.as<int32_t>(), c->pair.as<longlong2>(), c->sgpu.as<long long>(),
                                                                         c->node_cpu.as<long long>(), c->node_mem.as<long long>(), c->node_gpu.as<long long>());
     GP_CUDA(c, cudaGetLastError());
-    if (subtract) { s = refresh_views(c, st); if (s != GP_OK) return s; }
-    if (out && R) {
-        GP_CUDA(c, cudaMemcpyAsync(out->app, ro.app, 4 * R, cudaMemcpyDeviceToHost, st));
-        GP_CUDA(c, cudaMemcpyAsync(out->slot, ro.slot, 4 * R, cudaMemcpyDeviceToHost, st));
-        GP_CUDA(c, cudaMemcpyAsync(out->node, ro.node, 4 * R, cudaMemcpyDeviceToHost, st));
-        GP_CUDA(c, cudaMemcpyAsync(out->cpu_milli, ro.cpu, 8 * R, cudaMemcpyDeviceToHost, st));
-        GP_CUDA(c, cudaMemcpyAsync(out->mem_bytes, ro.mem, 8 * R, cudaMemcpyDeviceToHost, st));
-        if (out->gpu) GP_CUDA(c, cudaMemcpyAsync(out->gpu, ro.gpu, 8 * R, cudaMemcpyDeviceToHost, st));
+    if (subtract) GP_TRY(refresh_views(c, st));
+    if (out) {
+        ar.get(out->app, ra.part(0, R));
+        ar.get(out->slot, rs.part(0, R));
+        ar.get(out->node, rn.part(0, R));
+        ar.get(out->cpu_milli, rc.part(0, R));
+        ar.get(out->mem_bytes, rm.part(0, R));
+        ar.get(out->gpu, rg.part(0, R));
     }
-    GP_CUDA(c, cudaStreamSynchronize(st));
+    GP_TRY(ar.sync(c));
     if (out) out->n_rows = rows;
     return GP_OK;
 }
@@ -490,27 +478,31 @@ gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, c
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t R = (size_t)n_rows;
-    Arena ar{c->zonebuf};
-    const size_t o_c = ar.take(8 * R), o_m = ar.take(8 * R), o_g = ar.take(8 * R), o_n = ar.take(4 * R);
-    GP_CUDA(c, ar.reserve());
-    char* b = ar.base();
-    GP_CUDA(c, cudaMemcpyAsync(b + o_c, cpu, 8 * R, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_m, mem, 8 * R, cudaMemcpyHostToDevice, st));
-    if (gpu) GP_CUDA(c, cudaMemcpyAsync(b + o_g, gpu, 8 * R, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(b + o_n, node, 4 * R, cudaMemcpyHostToDevice, st));
+    Arena ar{c->zonebuf, st};
+    const auto cp = ar.take<long long>(R), mp = ar.take<long long>(R), gp = ar.take<long long>(R);
+    const auto np = ar.take<int32_t>(R);
+    ar.reserve();
+    const long long* d_cpu = ar.put(cp, cpu);
+    const long long* d_mem = ar.put(mp, mem);
+    const long long* d_gpu = ar.put(gp, gpu);
+    const int32_t* d_node = ar.put(np, node);
+    GP_TRY(ar.check(c));
     const int TH = 256;
-    gp_usage_delta<<<(unsigned)((R + TH - 1) / TH), TH, 0, st>>>(n_rows, (const int32_t*)(b + o_n), (const long long*)(b + o_c), (const long long*)(b + o_m),
-                                                                  gpu ? (const long long*)(b + o_g) : nullptr, sign, c->n_nodes, c->node_slot.as<int32_t>(),
+    gp_usage_delta<<<(unsigned)((R + TH - 1) / TH), TH, 0, st>>>(n_rows, d_node, d_cpu, d_mem, d_gpu, sign, c->n_nodes, c->node_slot.as<int32_t>(),
                                                                   c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->node_cpu.as<long long>(),
                                                                   c->node_mem.as<long long>(), c->node_gpu.as<long long>());
     GP_CUDA(c, cudaGetLastError());
-    gp_status s = refresh_views(c, st);
-    if (s != GP_OK) return s;
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    return GP_OK;
+    GP_TRY(refresh_views(c, st));
+    return ar.sync(c);
 }
 
 // ---- computeAvgPackingEfficiencyForResult over the whole node table, exactly summed (gangpack_efficiency.cuh) ----------
+// The efficiency kernels' status word (kEffErr* bits)
+static const Refusal kEffRefusals[] = {
+    {kEffErrQuantity, GP_ERR_UNREPRESENTABLE, "a per-node reserved amount is >= 2^61"},
+    {kEffErrRange, GP_ERR_UNREPRESENTABLE, "an efficiency term outside the exact accumulator's range"},
+};
+
 gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, double* avg_out) {
     if (!c) return GP_ERR_INVALID;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_packing_efficiency: no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)");
@@ -559,43 +551,40 @@ gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const
     const size_t q = (size_t)Q, T = (size_t)(total > 0 ? total : 0), N = (size_t)c->n_nodes;
     const int TH = kEffThreads;
     const int n_part = (int)std::max<size_t>(1, std::min<size_t>((N + TH - 1) / TH, (size_t)c->sm_count * 4));
-    Arena ar{c->zonebuf};
-    const size_t o_in = ar.take(48 * q), o_cnt = ar.take(4 * q), o_off = ar.take(8 * (q + 1)), o_drv = ar.take(4 * q), o_exe = ar.take(4 * (T + 1)),
-                 o_part = ar.take(sizeof(EffAcc) * (size_t)n_part), o_base = ar.take(sizeof(EffAcc)), o_avg = ar.take(32 * q), o_err = ar.take(4);
-    GP_CUDA(c, ar.reserve());
-    char* b = ar.base();
+    Arena ar{c->zonebuf, st};
+    const auto in = ar.take<int64_t>(6 * q);
+    const auto cnt = ar.take<int32_t>(q);
+    const auto off_p = ar.take<int64_t>(q + 1);
+    const auto drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1);
+    const auto part = ar.take<EffAcc>((size_t)n_part), base = ar.take<EffAcc>(1);
+    const auto avg = ar.take<double>(4 * q);
+    const auto err = ar.take<int>(1);
+    ar.reserve();
     EffRowsIn ri{};
-    gp_status s = upload_app_columns(c, a, off.data(), b, o_in, o_cnt, o_off, st, &ri.cols);
-    if (s != GP_OK) return s;
-    GP_CUDA(c, cudaMemcpyAsync(b + o_drv, placed->driver_node, 4 * q, cudaMemcpyHostToDevice, st));
-    if (T) GP_CUDA(c, cudaMemcpyAsync(b + o_exe, placed->executor_nodes, 4 * T, cudaMemcpyHostToDevice, st));
-    GP_CUDA(c, cudaMemsetAsync(b + o_err, 0, 4, st));
-    int* d_err = (int*)(b + o_err);
+    ri.cols = upload_app_columns(ar, a, off.data(), in, cnt, off_p);
+    ri.driver = ar.put(drv, placed->driver_node);
+    ar.put(exe.part(0, T), placed->executor_nodes);
+    int* d_err = ar.zero(err);
+    GP_TRY(ar.check(c));
     EffBaseIn bi{};
     bi.av = SnapshotAvail{c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->node_slot.as<int32_t>(), c->node_cpu.as<long long>(),
                       c->node_mem.as<long long>(), c->node_gpu.as<long long>()};
     bi.sched[0] = c->sched.as<long long>(); bi.sched[1] = c->sched.as<long long>() + N; bi.sched[2] = c->sched.as<long long>() + 2 * N;
     bi.n_nodes = c->n_nodes;
-    EffAcc* base = (EffAcc*)(b + o_base);
-    gp_eff_base<<<n_part, TH, 0, st>>>(bi, (EffAcc*)(b + o_part), d_err);
-    gp_eff_finish<<<1, TH, 0, st>>>((const EffAcc*)(b + o_part), n_part, base);
+    gp_eff_base<<<n_part, TH, 0, st>>>(bi, ar.ptr(part), d_err);
+    gp_eff_finish<<<1, TH, 0, st>>>(ar.ptr(part), n_part, ar.ptr(base));
     ri.av = bi.av;
     for (int k = 0; k < 3; ++k) ri.sched[k] = bi.sched[k];
-    ri.count = (const int32_t*)(b + o_cnt); ri.off = (const int64_t*)(b + o_off);
-    ri.driver = (const int32_t*)(b + o_drv); ri.exec = (const int32_t*)(b + o_exe); ri.base = base;
+    ri.count = ar.ptr(cnt); ri.off = ar.ptr(off_p); ri.exec = ar.ptr(exe); ri.base = ar.ptr(base);
     ri.n_apps = Q; ri.n_nodes = c->n_nodes;
     ri.executors_reserved = algo == GP_MINIMAL_FRAGMENTATION ? 0 : 1;
     ri.charged = (int32_t)charged;
-    gp_eff_rows<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(ri, (double*)(b + o_avg), d_err);
+    gp_eff_rows<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(ri, ar.ptr(avg), d_err);
     GP_CUDA(c, cudaGetLastError());
     int herr = 0;
-    GP_CUDA(c, cudaMemcpyAsync(avg_out, b + o_avg, 32 * q, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, st));
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    if (herr & kEffErrQuantity)
-        return fail(c, GP_ERR_UNREPRESENTABLE, "gp_packing_efficiency: a per-node reserved amount is >= 2^61");
-    if (herr & kEffErrRange)
-        return fail(c, GP_ERR_UNREPRESENTABLE, "gp_packing_efficiency: an efficiency term outside the exact accumulator's range");
-    return GP_OK;
+    ar.get(avg_out, avg);
+    ar.get(&herr, err);
+    GP_TRY(ar.sync(c));
+    return refuse(c, herr, kEffRefusals, "gp_packing_efficiency");
 }
 }  // extern "C"
