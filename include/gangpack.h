@@ -593,6 +593,39 @@ typedef struct {
 gp_status gp_exceeds_cluster_capacity(gp_ctx* ctx, const gp_capacity_nodes* nodes, const gp_apps* drivers, gp_binpacker packer,
                                       uint8_t* exceeds /* [n_apps] */);
 
+/* ---- the FIFO loop of every instance group with a zone-aware packer, in ONE launch ---------------------------------------
+ * fitEarlierDrivers (internal/extender/resource.go:224-262) walks one instance group's queue against that group's nodes
+ * (resource.go:292-295); queues of different instance groups are independent.  gp_pack_fifo_zones_groups runs all of them at
+ * once, one CTA per instance group, with packer GP_BP_SINGLE_AZ_TIGHTLY_PACK / GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION (as
+ * gp_pack_fifo_zones) or GP_BP_AZ_AWARE_TIGHTLY_PACK (as gp_pack_fifo_az_aware), mode GP_MODE_FIFO_REFERENCE or
+ * GP_MODE_FIFO_EXACT.
+ * Snapshot (gp_set_snapshot, then gp_set_schedulable): the groups of instance group i are group_off[i] .. group_off[i+1]-1,
+ * laid out for its packer as gp_pack_fifo_zones / gp_pack_fifo_az_aware expect them (single-AZ: every one a candidate zone,
+ * at most 64; az-aware: the first n_zones[i] (at most 64) its candidate zones, the rest its trailing group, exec_order /
+ * drv_order its undivided orders in CSR by exec_off / drv_off).  The queue of instance group i is the applications j with
+ * apps->group[j] == i (group NULL: every application in instance group 0), in index order; skip_if_no_fit as there.
+ * For every instance group each output -- zone (local to the instance group: 0 = its first candidate zone), driver_node
+ * (-1 / -2 included: a blocked queue blocks its own instance group only), ExecutorNodes, avg_efficiency and the availability
+ * left behind -- is what gp_pack_fifo_zones / gp_pack_fifo_az_aware return on a context holding only that instance group's
+ * groups and applications.  gp_stats sums over the instance groups (scan_path_apps: the az-aware fallbacks).
+ * GP_ERR_INVALID (gp_last_error names the cause; a refused call changes nothing): another packer or mode; no
+ * gp_set_schedulable; a snapshot from gp_set_snapshot_device / gp_prepare_cluster* (no host copy of the layout); group_off
+ * not monotone from 0 to the snapshot's n_groups; an application's group outside [0, n_instance_groups); more than 64
+ * candidate zones in an instance group, or n_zones[i] above its group count; az-aware orders missing, with offsets not
+ * monotone from 0 to the snapshot's executor / driver candidate counts, listing a node out of range, twice, of another
+ * instance group or not in that role, or a zone group whose order is not its instance group's order restricted to it. */
+typedef struct {
+    int32_t n_instance_groups;
+    const int32_t* group_off;        /* [n_instance_groups + 1] snapshot groups of each instance group */
+    const int32_t* n_zones;          /* az-aware: [n_instance_groups] candidate zones of each; NULL for the single-AZ packers */
+    const int32_t* exec_off;         /* az-aware: [n_instance_groups + 1] CSR of exec_order; else NULL */
+    const int32_t* exec_order;       /* az-aware: executorNodePriorityOrder of each instance group, undivided, node indices */
+    const int32_t* drv_off;          /* az-aware: [n_instance_groups + 1] CSR of drv_order; else NULL */
+    const int32_t* drv_order;        /* az-aware: driverNodePriorityOrder of each instance group, undivided, node indices */
+} gp_instance_groups;
+gp_status gp_pack_fifo_zones_groups(gp_ctx* ctx, const gp_apps* apps /* group = instance group */, gp_binpacker packer, gp_mode mode,
+                                    const gp_instance_groups* groups, gp_zone_results* out);
+
 /* ---- required node affinity (K8S = vendor/k8s.io) ------------------------------------------------------------------------
  * GetRequiredNodeAffinity(pod).Match(node) (K8S/component-helpers/scheduling/corev1/nodeaffinity/nodeaffinity.go:297-324) for
  * every (distinct affinity, node), as utils.ListWithPredicate runs it in selectDriverNode (EXT/resource.go:292-298) and in

@@ -170,6 +170,8 @@ struct gp_ctx {
     bool host_layout = false;
     std::vector<uint8_t> v_seen_e, v_seen_d;
     std::vector<int32_t> v_zone_next;             // az-aware order check: next position per zone group
+    std::vector<ZoneFifoGroup> zone_groups;       // zone FIFO: per instance group its zones, queue range and scratch rows
+    std::vector<int32_t> zone_queue;              // zone FIFO: application indices by instance group (stable counting sort)
     int az_fallback_ctas_per_sm = 0;              // occupancy of gp_pack_az_fallback (queried once)
     std::vector<std::pair<const char*, size_t>> pinned_blocks;   // gp_alloc_pinned allocations (device-mapped under UVA)
     void* one_block = nullptr;                    // gp_pack_one staging (mapped pinned)

@@ -373,6 +373,15 @@ struct GatherSlots {
     int32_t ne, nd;
 };
 
+// One instance group of the zone FIFO loop (gp_pack_fifo_zones_cta, gangpack_zonefifo.cuh): CTA b runs the b-th
+struct ZoneFifoGroup {
+    int64_t row_base;                 // its scratch rows start at entry row_base of the row arrays
+    int64_t row_pitch;                // >= max exe_count of its applications, a multiple of 4
+    int32_t zone0, n_zones;           // its candidate zones: snapshot groups zone0 .. zone0 + n_zones - 1
+    int32_t q_begin, q_end;           // its queue: ZoneFifoIn::queue[q_begin .. q_end)
+    int32_t e0, ne, d0, nd;           // az-aware: its undivided orders, entries e0 .. e0+ne-1 / d0 .. d0+nd-1 of the fallback view
+};
+
 // ---------------------------------------------------------------------------------------------
 // One application, one warp, against an immutable snapshot (GP_MODE_INDEPENDENT; the FIFO modes live in
 // gangpack_fifo.cuh).  Returns the driver's node index (>= 0) or -1.

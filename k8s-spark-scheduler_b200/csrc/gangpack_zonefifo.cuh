@@ -7,7 +7,9 @@
 // SubtractUsageIfExists, LIB/resources/resources.go:129-135).  The zone choice of driver i therefore feeds driver i+1:
 // the queue is one sequential chain over the whole cluster (zones are NOT independent queues).
 //
-// One persistent CTA walks the queue.  Per application:
+// One persistent CTA walks the queue of one instance group (fitEarlierDrivers runs per instance group, resource.go:292-295;
+// instance groups share no node, so their CTAs never wait on each other).  CTA b takes ZoneFifoGroup b: its zones, its
+// queue and its scratch rows.  Per application:
 //   1. warp w packs it in zones w, w + W, ... (snapshot instance group = zone) with the warp-per-application scan of the
 //      independent kernels -- here with coherent loads, the availabilities change inside the launch -- into a scratch row
 //      per zone; lane 0 of the warp then walks its row for the float64 averages in the reference's operation order;
@@ -21,8 +23,9 @@
 // when no zone wins in 2., falls back to SparkBinPack(tightlyPackExecutors) over the UNDIVIDED driver / executor orders
 // against the availability the loop holds at that point.  Those orders run across the snapshot's groups (zone groups plus
 // a trailing group with the nodes no candidate zone contains), so warp 0 scans them through a gather view built once per
-// call by gp_build_fallback_view (GatherSlots: position -> slot).  The fallback's placement lands in row Z and is emitted
-// and charged by the code of 3., so both accounting modes share it; it reports zone -1 and zero averages.
+// call by gp_build_fallback_view (GatherSlots: position -> slot; CTA b sees the entries of its instance group's orders).
+// The fallback's placement lands in row Z and is emitted and charged by the code of 3., so both accounting modes share
+// it; it reports zone -1 and zero averages.
 #pragma once
 
 #include "gangpack_kernels.cuh"
@@ -39,10 +42,10 @@ constexpr int kZoneAzAware = 3;               // ALGO of az-aware-tightly-pack (
 struct ZoneFifoIn {
     const long long* sched[3];        // SchedulableResources, node-table order (gpu may be NULL = 0)
     const int32_t* node_slot;         // node -> global slot
-    int32_t* row_exec;                // [Z][row_pitch] ExecutorNodes of the application in every zone
-    int2* row_list;                   // [Z][row_pitch] consumed-node list of minimal-fragmentation, NULL for tightly-pack
-    int64_t row_pitch;                // >= max exe_count of the batch
-    int32_t n_apps, n_zones;
+    int32_t* row_exec;                // per instance group [n_zones (+1 az-aware)][row_pitch] at row_base: ExecutorNodes per zone
+    int2* row_list;                   // the same rows: consumed-node list of minimal-fragmentation, NULL for tightly-pack
+    const ZoneFifoGroup* groups;      // [gridDim.x]
+    const int32_t* queue;             // application indices, instance group after instance group, queue order within each
 };
 
 // AvailableResources of a node as the loop currently holds them (the slots are charged inside the launch)
@@ -64,32 +67,43 @@ __device__ __forceinline__ void zone_charge(const Snapshot& s, int32_t slot, lon
     if (g != 0) s.gpu[slot] = load_gpu<true>(s.gpu + slot) - mult * g;
 }
 
-// The fallback view of az-aware-tightly-pack, once per call, in one CTA: fb_exec_slot[i] = node_slot[exec_order[i]],
-// fb_drv_slot[j] = node_slot[drv_order[j]], fb_drv_pos[j] = position of drv_order[j] in exec_order or -1 (node_pos:
-// [n_nodes] scratch for the node -> position scatter).
-__global__ void __launch_bounds__(1024) gp_build_fallback_view(int32_t n_nodes, int32_t n_exec, int32_t n_drv,
+// The fallback view of az-aware-tightly-pack, once per call, one CTA per instance group b, whose undivided orders are
+// exec_order[exec_off[b] .. exec_off[b+1]) and drv_order[drv_off[b] .. drv_off[b+1]) (offsets NULL: one instance group,
+// the whole orders): fb_exec_slot[i] = node_slot[exec_order[i]], fb_drv_slot[j] = node_slot[drv_order[j]], fb_drv_pos[j]
+// = position of drv_order[j] in its instance group's executor order, or -1.  node_pos: [n_nodes] scratch for the node ->
+// position scatter; a CTA writes and reads only the entries of its own nodes, and instance groups share no node.
+__global__ void __launch_bounds__(1024) gp_build_fallback_view(int32_t n_exec, int32_t n_drv, const int32_t* __restrict__ exec_off,
+                                                               const int32_t* __restrict__ drv_off,
                                                                const int32_t* __restrict__ exec_order, const int32_t* __restrict__ drv_order,
                                                                const int32_t* __restrict__ node_slot, int32_t* __restrict__ node_pos,
                                                                int32_t* __restrict__ fb_exec_slot, int32_t* __restrict__ fb_drv_slot,
                                                                int32_t* __restrict__ fb_drv_pos) {
-    for (int32_t v = threadIdx.x; v < n_nodes; v += blockDim.x) node_pos[v] = -1;
+    const int32_t e0 = exec_off ? exec_off[blockIdx.x] : 0, e1 = exec_off ? exec_off[blockIdx.x + 1] : n_exec;
+    const int32_t d0 = drv_off ? drv_off[blockIdx.x] : 0, d1 = drv_off ? drv_off[blockIdx.x + 1] : n_drv;
+    for (int32_t j = d0 + threadIdx.x; j < d1; j += blockDim.x) node_pos[drv_order[j]] = -1;
     __syncthreads();
-    for (int32_t i = threadIdx.x; i < n_exec; i += blockDim.x) {
+    for (int32_t i = e0 + threadIdx.x; i < e1; i += blockDim.x) {
         const int32_t v = exec_order[i];
-        node_pos[v] = i;
+        node_pos[v] = i - e0;
         fb_exec_slot[i] = node_slot[v];
     }
     __syncthreads();
-    for (int32_t j = threadIdx.x; j < n_drv; j += blockDim.x) {
+    for (int32_t j = d0 + threadIdx.x; j < d1; j += blockDim.x) {
         const int32_t v = drv_order[j];
         fb_drv_slot[j] = node_slot[v];
         fb_drv_pos[j] = node_pos[v];
     }
 }
 
+// The part of the fallback view `all` that instance group ig's orders cover
+__device__ __forceinline__ GatherSlots group_view(const ZoneFifoGroup& ig, const GatherSlots& all) {
+    return GatherSlots{all.exec_slot + ig.e0, all.drv_slot + ig.d0, all.drv_pos + ig.d0, ig.ne, ig.nd};
+}
+
 // ALGO: 0 tightly-pack, 2 minimal-fragmentation, kZoneAzAware az-aware-tightly-pack.  FIFO_MODE: 1 reference accounting,
-// 2 exact.  fb: the fallback view, one GatherSlots for kZoneAzAware (its row is Z of in.row_exec), none for the single-AZ
-// packers (so their parameter list, and code, stay what they were before the az-aware form existed).
+// 2 exact.  One CTA per instance group (in.groups).  fb: the fallback view of every instance group, one GatherSlots for
+// kZoneAzAware (the row after an instance group's zones is its fallback row), none for the single-AZ packers (so their
+// parameter list, and code, stay what they were before the az-aware form existed).
 template <int ALGO, int FIFO_MODE, class... FB>
 __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Snapshot s, const PrepApp* __restrict__ prep, ZoneFifoIn in,
                                                                               int32_t* __restrict__ zone_out, int32_t* __restrict__ driver_out,
@@ -102,14 +116,20 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
     __shared__ int32_t z_drv[kZoneFifoMaxZones];
     __shared__ int32_t fb_drv;                        // kAz: driver node of the fallback, -1 = it fits nowhere either
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int32_t Z = in.n_zones;
+    const ZoneFifoGroup ig = in.groups[blockIdx.x];
+    const int32_t Z = ig.n_zones;
+    int32_t* const row_exec = in.row_exec + ig.row_base;
+    int2* const row_list = in.row_list ? in.row_list + ig.row_base : nullptr;
+    GatherSlots view{};
+    if constexpr (kAz) view = group_view(ig, fb...);
     const GroupDesc g0 = s.groups[0];
     SlotAvail av;
     av.pair = s.pair; av.gpu = s.gpu; av.node_slot = in.node_slot;
     WarpStats st{0, 0};
     const int snap_flags = s.meta->flags;     // a placement only lands where it fits: no availability turns negative inside the loop
     bool blocked = false;
-    for (int32_t app = 0; app < in.n_apps; ++app) {
+    for (int32_t qi = ig.q_begin; qi < ig.q_end; ++qi) {
+        const int32_t app = in.queue[qi];
         const PrepApp* pa = prep + app;
         const uint32_t fl = pa->flags;
         if (blocked || (fl & kAppInvalid)) {
@@ -123,17 +143,18 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
         const int32_t k = pa->count;
         // ---- 1. every zone: pack + averages ---------------------------------------------------------------------------
         for (int32_t z = warp; z < Z; z += kZoneFifoWarps) {
-            const int64_t row = (int64_t)z * in.row_pitch;
+            const int64_t row = (int64_t)z * ig.row_pitch;
             int32_t d;
             if (ALGO == 0 || kAz)
-                d = pack_app_impl<0, false, false, false, int32_t, true>(s, pa, in.row_exec, nullptr, caches[warp], st, lane, snap_flags, g0, z, row);
+                d = pack_app_impl<0, false, false, false, int32_t, true>(s, pa, row_exec, nullptr, caches[warp], st, lane, snap_flags, g0,
+                                                                         ig.zone0 + z, row);
             else
-                d = pack_app_minfrag<false, true>(s, pa, in.row_exec, in.row_list, st, lane, snap_flags, z, row);
+                d = pack_app_minfrag<false, true>(s, pa, row_exec, row_list, st, lane, snap_flags, ig.zone0 + z, row);
             __syncwarp();
             if (lane == 0) {
                 z_drv[z] = d;
                 if (d >= 0)
-                    zone_row_average(av, in.sched, d, in.row_exec + row, k, pa->drv[0], pa->drv[1], pa->drv[2],
+                    zone_row_average(av, in.sched, d, row_exec + row, k, pa->drv[0], pa->drv[1], pa->drv[2],
                                      pa->div[0].e, pa->div[1].e, pa->div[2].e, ALGO == 0 || kAz, z_avg[z]);
             }
         }
@@ -149,7 +170,7 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
             if (best_z < 0) {
                 if (warp == 0) {
                     const int32_t d = pack_app_impl<0, false, false, false, int32_t, true, GatherSlots>(
-                        s, pa, in.row_exec, nullptr, caches[0], st, lane, snap_flags, g0, 0, (int64_t)Z * in.row_pitch, &fb...);
+                        s, pa, row_exec, nullptr, caches[0], st, lane, snap_flags, g0, 0, (int64_t)Z * ig.row_pitch, &view);
                     if (lane == 0) {
                         fb_drv = d;
                         if (stats) atomicAdd(stats + 2, 1ull);   // stats[2]: applications for which the fallback ran
@@ -162,7 +183,7 @@ __global__ void __launch_bounds__(kZoneFifoThreads, 1) gp_pack_fifo_zones_cta(Sn
         const bool fell_back = kAz && win == Z;
         // ---- 3. the winner's warp emits and charges ---------------------------------------------------------------------
         if (win >= 0 && warp == win % kZoneFifoWarps) {
-            const int32_t* ex = in.row_exec + (int64_t)win * in.row_pitch;
+            const int32_t* ex = row_exec + (int64_t)win * ig.row_pitch;
             int32_t* out = exec_out + pa->out_off;
             const int32_t d = fell_back ? fb_drv : z_drv[win];
             const long long ec = pa->div[0].e, em = pa->div[1].e, eg = pa->div[2].e;

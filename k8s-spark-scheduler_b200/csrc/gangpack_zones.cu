@@ -1,5 +1,5 @@
 // gangpack_zones.cu -- the single-AZ and az-aware-tightly-pack packers (gp_pack_batch_zones, gp_pack_fifo_zones,
-// gp_pack_fifo_az_aware, gp_pack_batch_az_aware) with gp_set_schedulable, the reservation table and usage deltas of the
+// gp_pack_fifo_az_aware, gp_pack_batch_az_aware, gp_pack_fifo_zones_groups) with gp_set_schedulable, the reservation table and usage deltas of the
 // resident snapshot (gp_reserve_placements, gp_apply_usage_delta), and gp_packing_efficiency.
 #include "gangpack_ctx.cuh"
 #include "gangpack_zones.cuh"
@@ -54,22 +54,41 @@ static SixCols upload_app_columns(Arena& ar, const gp_apps* a, const int64_t* of
     return six;
 }
 
-// az-aware-tightly-pack: upload the undivided orders and build the fallback's gather view of them (gp_build_fallback_view).
-// on_device: az's orders are device arrays (gp_prepare_cluster_zones' held orders) and are read in place.
-static gp_status stage_fallback_view(gp_ctx* c, const gp_az_orders* az, bool on_device, cudaStream_t st, GatherSlots* fb) {
-    const size_t ne = (size_t)az->n_exec, nd = (size_t)az->n_drv;
+// One instance group over the whole snapshot (gp_pack_fifo_zones, gp_pack_*_az_aware) in the layout of
+// gp_pack_fifo_zones_groups; o: the az-aware orders, NULL for the single-AZ packers
+struct OneInstanceGroup {
+    int32_t group_off[2], n_zones, exec_off[2], drv_off[2];
+    gp_instance_groups ig;
+    OneInstanceGroup(int32_t n_groups, const gp_az_orders* o)
+        : group_off{0, n_groups}, n_zones(o ? o->n_zones : 0), exec_off{0, o ? o->n_exec : 0}, drv_off{0, o ? o->n_drv : 0},
+          ig{1, group_off, o ? &n_zones : nullptr, o ? exec_off : nullptr, o ? o->exec_order : nullptr, o ? drv_off : nullptr,
+             o ? o->drv_order : nullptr} {}
+    OneInstanceGroup(const OneInstanceGroup&) = delete;
+    OneInstanceGroup& operator=(const OneInstanceGroup&) = delete;
+};
+
+// az-aware-tightly-pack: upload the undivided orders of the instance groups `ig` and build the fallback's gather view of
+// them (gp_build_fallback_view, one CTA per instance group).  on_device: the orders are device arrays
+// (gp_prepare_cluster_zones' held orders) and are read in place.
+static gp_status stage_fallback_view(gp_ctx* c, const gp_instance_groups& ig, bool on_device, cudaStream_t st, GatherSlots* fb) {
+    const int32_t G = ig.n_instance_groups;
+    const size_t ne = (size_t)ig.exec_off[G], nd = (size_t)ig.drv_off[G];
+    const size_t n_off = G == 1 ? 0 : (size_t)G + 1;          // one instance group: the whole orders, no offsets
     Arena ar{c->fbview, st};
     const auto eord = ar.take<int32_t>(on_device ? 0 : ne), dord = ar.take<int32_t>(on_device ? 0 : nd),
                npos = ar.take<int32_t>((size_t)c->n_nodes), fbe = ar.take<int32_t>(ne), fbd = ar.take<int32_t>(nd), fbp = ar.take<int32_t>(nd);
+    const auto eoff = ar.take<int32_t>(n_off), doff = ar.take<int32_t>(n_off);
     ar.reserve();
     if (!on_device) {
-        ar.put(eord, az->exec_order);
-        ar.put(dord, az->drv_order);
+        ar.put(eord, ig.exec_order);
+        ar.put(dord, ig.drv_order);
     }
+    const int32_t* d_eoff = n_off ? ar.put(eoff, ig.exec_off) : nullptr;
+    const int32_t* d_doff = n_off ? ar.put(doff, ig.drv_off) : nullptr;
     GP_TRY(ar.check(c));
-    gp_build_fallback_view<<<1, 1024, 0, st>>>(c->n_nodes, (int32_t)ne, (int32_t)nd, on_device ? az->exec_order : ar.ptr(eord),
-                                               on_device ? az->drv_order : ar.ptr(dord), c->node_slot.as<int32_t>(), ar.ptr(npos),
-                                               ar.ptr(fbe), ar.ptr(fbd), ar.ptr(fbp));
+    gp_build_fallback_view<<<(unsigned)G, 1024, 0, st>>>((int32_t)ne, (int32_t)nd, d_eoff, d_doff, on_device ? ig.exec_order : ar.ptr(eord),
+                                                         on_device ? ig.drv_order : ar.ptr(dord), c->node_slot.as<int32_t>(), ar.ptr(npos),
+                                                         ar.ptr(fbe), ar.ptr(fbd), ar.ptr(fbp));
     c->last.kernel_launches += 1;
     *fb = GatherSlots{ar.ptr(fbe), ar.ptr(fbd), ar.ptr(fbp), (int32_t)ne, (int32_t)nd};
     return GP_OK;
@@ -169,7 +188,8 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
         gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
             Q, cols, nullptr, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, ar.ptr(prep), &ds->head.err, &c->host_status()->err_word);
         GatherSlots fb;
-        GP_TRY(stage_fallback_view(c, az, az_dev, st, &fb));
+        const OneInstanceGroup one(c->n_groups, az);
+        GP_TRY(stage_fallback_view(c, one.ig, az_dev, st, &fb));
         int& per_sm = c->az_fallback_ctas_per_sm;
         if (per_sm == 0) {
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_az_fallback, kAzFallbackThreads, 0);
@@ -207,43 +227,54 @@ static gp_status refresh_views(gp_ctx* c, cudaStream_t st) {
     return GP_OK;
 }
 
-// The undivided orders of az-aware-tightly-pack against the snapshot gp_set_snapshot laid out, in O(N): every entry a node
-// of the snapshot in that role, once; every zone group's order = the undivided order restricted to that group's nodes
-// (the fallback and the zone packs must see the same priorities).  o->n_zones is already within 0..n_groups.
-static gp_status check_az_orders(gp_ctx* c, const gp_az_orders* o, const char* who) {
+// The undivided orders of az-aware-tightly-pack against the snapshot gp_set_snapshot laid out, in O(N): every entry of
+// instance group b's orders a node of b's groups in that role, every node once over all instance groups (so b's orders are
+// a permutation of b's nodes in that role); every zone group's order = its instance group's undivided order restricted to
+// that group's nodes (the fallback and the zone packs must see the same priorities).  ig.group_off and ig.n_zones are
+// already checked; ig.exec_off / ig.drv_off are present.
+static gp_status check_az_orders(gp_ctx* c, const gp_instance_groups& ig, const char* who) {
     const std::string w(who);
     if (!c->host_layout)
         return fail(c, GP_ERR_INVALID, w + ": the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
                                            "gp_prepare_cluster there is no host copy of the layout to check the undivided orders against)");
-    if (o->n_exec != c->n_exec || o->n_drv != c->n_drv)
+    const int32_t G = ig.n_instance_groups;
+    if (ig.exec_off[G] != c->n_exec || ig.drv_off[G] != c->n_drv)
         return fail(c, GP_ERR_INVALID, w + ": order lengths must equal the snapshot's exec_off[n_groups] / drv_off[n_groups]");
-    if ((o->n_exec > 0 && !o->exec_order) || (o->n_drv > 0 && !o->drv_order))
+    for (int32_t b = 0; b < G; ++b)
+        if (ig.exec_off[0] != 0 || ig.drv_off[0] != 0 || ig.exec_off[b + 1] < ig.exec_off[b] || ig.drv_off[b + 1] < ig.drv_off[b])
+            return fail(c, GP_ERR_INVALID, w + ": exec_off / drv_off must be monotone from 0");
+    if ((c->n_exec > 0 && !ig.exec_order) || (c->n_drv > 0 && !ig.drv_order))
         return fail(c, GP_ERR_INVALID, w + ": order arrays missing");
-    const int32_t Z = o->n_zones;
     const uint32_t N = (uint32_t)c->n_nodes;
     const int32_t* owner = c->v_owner.data();
     const int32_t* pos = c->v_pos.data();
     for (int role = 0; role < 2; ++role) {
-        const int32_t n = role == 0 ? o->n_exec : o->n_drv;
-        const int32_t* ord = role == 0 ? o->exec_order : o->drv_order;
+        const int32_t* off = role == 0 ? ig.exec_off : ig.drv_off;
+        const int32_t* ord = role == 0 ? ig.exec_order : ig.drv_order;
         const char* name = role == 0 ? "exec_order" : "drv_order";
         std::vector<uint8_t>& seen = role == 0 ? c->v_seen_e : c->v_seen_d;
         seen.assign((size_t)N, 0);
         std::vector<int32_t>& next = c->v_zone_next;     // next expected position in each zone group's order
-        next.assign((size_t)Z, 0);
-        for (int32_t i = 0; i < n; ++i) {
-            const uint32_t v = (uint32_t)ord[i];
-            if (v >= N) return fail(c, GP_ERR_INVALID, w + ": " + name + " entry out of range");
-            if (seen[v]) return fail(c, GP_ERR_INVALID, w + ": " + name + " lists a node twice");
-            seen[v] = 1;
-            const int32_t ow = owner[v];
-            if (ow < 0 || !(ow & (1 << role)))
-                return fail(c, GP_ERR_INVALID, w + ": " + name + " lists a node the snapshot does not list as " +
-                                                   (role == 0 ? "an executor" : "a driver") + " candidate");
-            const int32_t g = ow >> 2;
-            if (g < Z && pos[(size_t)role * N + v] != next[(size_t)g]++)
-                return fail(c, GP_ERR_INVALID, w + ": zone group " + std::to_string(g) + "'s " +
-                                                   (role == 0 ? "executor" : "driver") + " order is not " + name + " restricted to its nodes");
+        next.assign((size_t)c->n_groups, 0);
+        for (int32_t b = 0; b < G; ++b) {
+            const int32_t g_lo = ig.group_off[b], g_hi = ig.group_off[b + 1], z_hi = g_lo + ig.n_zones[b];
+            for (int32_t i = off[b]; i < off[b + 1]; ++i) {
+                const uint32_t v = (uint32_t)ord[i];
+                if (v >= N) return fail(c, GP_ERR_INVALID, w + ": " + name + " entry out of range");
+                if (seen[v]) return fail(c, GP_ERR_INVALID, w + ": " + name + " lists a node twice");
+                seen[v] = 1;
+                const int32_t ow = owner[v];
+                if (ow < 0 || !(ow & (1 << role)))
+                    return fail(c, GP_ERR_INVALID, w + ": " + name + " lists a node the snapshot does not list as " +
+                                                       (role == 0 ? "an executor" : "a driver") + " candidate");
+                const int32_t g = ow >> 2;
+                if (g < g_lo || g >= g_hi)
+                    return fail(c, GP_ERR_INVALID, w + ": " + name + " of instance group " + std::to_string(b) +
+                                                       " lists a node of another instance group");
+                if (g < z_hi && pos[(size_t)role * N + v] != next[(size_t)g]++)
+                    return fail(c, GP_ERR_INVALID, w + ": zone group " + std::to_string(g) + "'s " +
+                                                       (role == 0 ? "executor" : "driver") + " order is not " + name + " restricted to its nodes");
+            }
         }
     }
     return GP_OK;
@@ -260,22 +291,33 @@ static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_resul
     return GP_OK;
 }
 
-// The FIFO loop over zones in one launch (gangpack_zonefifo.cuh), shared by gp_pack_fifo_zones (kind = 0 tightly-pack,
-// 2 minimal-fragmentation; the zones are every instance group) and gp_pack_fifo_az_aware (kind = kZoneAzAware; zones
-// 0..Z-1, plus the undivided orders `az` of the fallback, already validated; az_dev: they are device arrays).  Argument
-// checks common to both are here.
-static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, int32_t Z, const gp_az_orders* az, bool az_dev,
-                                gp_zone_results* out, const char* who) {
+// The FIFO loop over zones in one launch (gangpack_zonefifo.cuh), one CTA per instance group of `ig` (already validated),
+// shared by gp_pack_fifo_zones (kind = 0 tightly-pack, 2 minimal-fragmentation; one instance group whose zones are every
+// snapshot group), gp_pack_fifo_az_aware (kind = kZoneAzAware; one instance group, zones 0..n_zones-1, plus the undivided
+// orders of the fallback; az_dev: they are device arrays) and gp_pack_fifo_zones_groups (either, per instance group).
+// group: the instance group of every application, NULL = 0.  Argument checks common to all three are here.
+static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, const int32_t* group, int kind, gp_mode mode, const gp_instance_groups& ig,
+                                bool az_dev, gp_zone_results* out, const char* who) {
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
     if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, who, "missing app/result arrays");
+    const bool azk = kind == kZoneAzAware;
+    const int32_t G = ig.n_instance_groups;
+    // one pass over the queue: ExecutorNodes offsets, and per instance group its application count (in q_end) and its
+    // largest exe_count (in row_pitch)
+    std::vector<ZoneFifoGroup>& grp = c->zone_groups;
+    grp.assign((size_t)G, ZoneFifoGroup{});
     std::vector<int64_t>& hoff = c->host_off;
     hoff.resize((size_t)Q + 1);
-    int64_t acc = 0, pitch = 1;
+    int64_t acc = 0;
     for (int32_t i = 0; i < Q; ++i) {
         const int64_t k = a->exe_count[i] > 0 ? a->exe_count[i] : 0;
         hoff[(size_t)i] = acc; acc += k;
-        if (k > pitch) pitch = k;
+        const int32_t b = group ? group[i] : 0;
+        if (b < 0 || b >= G) return fail(c, GP_ERR_INVALID, who, "an application's group is outside [0, n_instance_groups)");
+        ZoneFifoGroup& g = grp[(size_t)b];
+        ++g.q_end;
+        if (k > g.row_pitch) g.row_pitch = k;
     }
     hoff[(size_t)Q] = acc;
     if (a->exec_out_off)
@@ -284,16 +326,37 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     const int64_t total = acc;
     if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, who, "executor_nodes_cap too small");
     if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, who, "executor_nodes is NULL");
-    pitch = (pitch + 3) & ~(int64_t)3;
+    // per instance group: its zones, its queue range and its scratch rows (n_zones, az-aware: + the fallback row)
+    int32_t qb = 0;
+    int64_t rows = 0;
+    for (int32_t b = 0; b < G; ++b) {
+        ZoneFifoGroup& g = grp[(size_t)b];
+        g.zone0 = ig.group_off[b];
+        g.n_zones = azk ? ig.n_zones[b] : ig.group_off[b + 1] - ig.group_off[b];
+        const int32_t n = g.q_end;
+        g.q_begin = g.q_end = qb;                          // q_end: the cursor of the fill below
+        qb += n;
+        g.row_pitch = (std::max<int64_t>(g.row_pitch, 1) + 3) & ~(int64_t)3;
+        g.row_base = rows;
+        rows += (int64_t)(g.n_zones + (azk ? 1 : 0)) * g.row_pitch;
+        if (azk) {
+            g.e0 = ig.exec_off[b]; g.ne = ig.exec_off[b + 1] - g.e0;
+            g.d0 = ig.drv_off[b]; g.nd = ig.drv_off[b + 1] - g.d0;
+        }
+    }
+    std::vector<int32_t>& queue = c->zone_queue;            // stable counting sort of the applications by instance group
+    queue.resize((size_t)Q);
+    for (int32_t i = 0; i < Q; ++i) queue[(size_t)grp[(size_t)(group ? group[i] : 0)].q_end++] = i;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
-    const bool azk = kind == kZoneAzAware;
-    const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)(Z + (azk ? 1 : 0)) * (size_t)pitch;   // az-aware: row Z = fallback
+    const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)rows;
     Arena ar{c->zonebuf, st};
     const auto in = ar.take<int64_t>(6 * q);
     const auto cnt = ar.take<int32_t>(q);
     const auto off_p = ar.take<int64_t>(q + 1);
     const auto skip = ar.take<uint8_t>(q);
+    const auto gdesc = ar.take<ZoneFifoGroup>((size_t)G);
+    const auto qidx = ar.take<int32_t>(q);
     const auto rexe = ar.take<int32_t>(RP);
     const auto rlist = ar.take<int2>(kind == GP_MINIMAL_FRAGMENTATION ? RP : 0);
     const auto zone = ar.take<int32_t>(q), drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1);
@@ -305,6 +368,8 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     AppColumns cols{};
     const SixCols six = upload_app_columns(ar, a, hoff.data(), in, cnt, off_p);
     const uint8_t* d_skip = ar.put(skip, a->skip_if_no_fit);
+    ar.put(gdesc, grp.data());
+    ar.put(qidx, queue.data());
     GP_TRY(ar.check(c));
     for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
     cols.count = ar.ptr(cnt); cols.group = nullptr; cols.off = ar.ptr(off_p); cols.bits = 64; cols.mem_shift = 0;
@@ -320,20 +385,21 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode m
     zi.node_slot = c->node_slot.as<int32_t>();
     zi.row_exec = ar.ptr(rexe);
     zi.row_list = kind == GP_MINIMAL_FRAGMENTATION ? ar.ptr(rlist) : nullptr;
-    zi.row_pitch = pitch; zi.n_apps = Q; zi.n_zones = Z;
+    zi.groups = ar.ptr(gdesc); zi.queue = ar.ptr(qidx);
     double* avg = out->avg_efficiency ? ar.ptr(avg_p) : nullptr;
     int32_t* zo = ar.ptr(zone); int32_t* dq = ar.ptr(drv); int32_t* eo = ar.ptr(exe);
     GatherSlots fb{};
-    if (azk) GP_TRY(stage_fallback_view(c, az, az_dev, st, &fb));
+    if (azk) GP_TRY(stage_fallback_view(c, ig, az_dev, st, &fb));
+    const unsigned ctas = (unsigned)G;                 // one per instance group
     if (kind == GP_TIGHTLY_PACK) {
-        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-        else gp_pack_fifo_zones_cta<0, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+        else gp_pack_fifo_zones_cta<0, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
     } else if (kind == GP_MINIMAL_FRAGMENTATION) {
-        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<2, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-        else gp_pack_fifo_zones_cta<2, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<2, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+        else gp_pack_fifo_zones_cta<2, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
     } else {
-        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<kZoneAzAware, 1><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
-        else gp_pack_fifo_zones_cta<kZoneAzAware, 2><<<1, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<kZoneAzAware, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
+        else gp_pack_fifo_zones_cta<kZoneAzAware, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
     }
     GP_CUDA(c, cudaGetLastError());
     c->last.kernel_launches += 2;
@@ -351,9 +417,9 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: the single-AZ packers are tightly-pack and minimal-fragmentation");
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones)");
-    const int32_t Z = c->n_groups;
-    if (Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
-    return fifo_zones_run(c, a, (int)algo, mode, Z, nullptr, false, out, "gp_pack_fifo_zones");
+    if (c->n_groups > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
+    const OneInstanceGroup one(c->n_groups, nullptr);
+    return fifo_zones_run(c, a, nullptr, (int)algo, mode, one.ig, false, out, "gp_pack_fifo_zones");
 }
 
 // the FIFO loop with az-aware-tightly-pack in one launch: the zone packs plus the undivided fallback on the device
@@ -370,9 +436,47 @@ gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const
     const int32_t Z = o->n_zones;
     if (Z < 0 || Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones must be 0..64");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones exceeds the snapshot's instance groups");
-    if (!held) s = check_az_orders(c, o, "gp_pack_fifo_az_aware");
+    const OneInstanceGroup one(c->n_groups, o);
+    if (!held) s = check_az_orders(c, one.ig, "gp_pack_fifo_az_aware");
     if (s != GP_OK) return s;
-    return fifo_zones_run(c, a, kZoneAzAware, mode, Z, o, held, out, "gp_pack_fifo_az_aware");
+    return fifo_zones_run(c, a, nullptr, kZoneAzAware, mode, one.ig, held, out, "gp_pack_fifo_az_aware");
+}
+
+// the FIFO loop of every instance group with a zone-aware packer, one CTA per instance group, in one launch
+gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker packer, gp_mode mode, const gp_instance_groups* ig,
+                                    gp_zone_results* out) {
+    const char* who = "gp_pack_fifo_zones_groups";
+    if (!c) return GP_ERR_INVALID;
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, who, "gp_set_snapshot first");
+    int kind;
+    if (packer == GP_BP_SINGLE_AZ_TIGHTLY_PACK) kind = GP_TIGHTLY_PACK;
+    else if (packer == GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) kind = GP_MINIMAL_FRAGMENTATION;
+    else if (packer == GP_BP_AZ_AWARE_TIGHTLY_PACK) kind = kZoneAzAware;
+    else return fail(c, GP_ERR_INVALID, who, "packer must be GP_BP_SINGLE_AZ_TIGHTLY_PACK, GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION or "
+                                             "GP_BP_AZ_AWARE_TIGHTLY_PACK");
+    if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
+        return fail(c, GP_ERR_INVALID, who, "mode must be one of the FIFO modes");
+    if (!c->have_sched) return fail(c, GP_ERR_INVALID, who, "gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!c->host_layout)
+        return fail(c, GP_ERR_INVALID, who, "the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
+                                            "gp_prepare_cluster* there is no host copy of the layout to check the instance groups against)");
+    if (!a || !out || !ig || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/groups/results");
+    const int32_t G = ig->n_instance_groups;
+    const int32_t* goff = ig->group_off;
+    if (G < 0 || !goff) return fail(c, GP_ERR_INVALID, who, "n_instance_groups is negative or group_off is NULL");
+    if (goff[0] != 0 || goff[G] != c->n_groups) return fail(c, GP_ERR_INVALID, who, "group_off must run from 0 to the snapshot's n_groups");
+    const bool azk = kind == kZoneAzAware;
+    if (azk && (!ig->n_zones || !ig->exec_off || !ig->drv_off))
+        return fail(c, GP_ERR_INVALID, who, "az-aware-tightly-pack needs n_zones, exec_off and drv_off");
+    for (int32_t b = 0; b < G; ++b) {
+        const int64_t n = (int64_t)goff[b + 1] - goff[b];
+        if (n < 0) return fail(c, GP_ERR_INVALID, who, "group_off is not monotone");
+        const int64_t Z = azk ? ig->n_zones[b] : n;
+        if (Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, who, "more than 64 candidate zones in an instance group");
+        if (Z < 0 || Z > n) return fail(c, GP_ERR_INVALID, who, "n_zones[i] must be 0 .. the number of groups of instance group i");
+    }
+    if (azk) GP_TRY(check_az_orders(c, *ig, who));
+    return fifo_zones_run(c, a, a->group, kind, mode, *ig, false, out, who);
 }
 
 // az-aware-tightly-pack for a batch of independent decisions: the zone packs, the zone choice and the undivided fallback
@@ -387,7 +491,8 @@ gp_status gp_pack_batch_az_aware(gp_ctx* c, const gp_apps* a, const gp_az_orders
     const int32_t Z = o->n_zones;
     if (Z < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones is negative");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones exceeds the snapshot's instance groups");
-    if (!held) s = check_az_orders(c, o, "gp_pack_batch_az_aware");
+    const OneInstanceGroup one(c->n_groups, o);
+    if (!held) s = check_az_orders(c, one.ig, "gp_pack_batch_az_aware");
     if (s != GP_OK) return s;
     return batch_zones_run(c, a, GP_TIGHTLY_PACK, Z, o, held, out, "gp_pack_batch_az_aware");
 }

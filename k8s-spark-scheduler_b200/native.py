@@ -37,7 +37,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
-           "gp_node_overhead",
+           "gp_node_overhead", "gp_pack_fifo_zones_groups",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -113,6 +113,11 @@ class gp_zone_results(C.Structure):
 class gp_az_orders(C.Structure):
     _fields_ = [("n_zones", C.c_int32), ("n_exec", C.c_int32), ("exec_order", C.c_void_p), ("n_drv", C.c_int32),
                 ("drv_order", C.c_void_p)]
+
+
+class gp_instance_groups(C.Structure):
+    _fields_ = [("n_instance_groups", C.c_int32), ("group_off", C.c_void_p), ("n_zones", C.c_void_p), ("exec_off", C.c_void_p),
+                ("exec_order", C.c_void_p), ("drv_off", C.c_void_p), ("drv_order", C.c_void_p)]
 
 
 class gp_reservation_table(C.Structure):
@@ -275,6 +280,9 @@ def load():
     L.gp_pack_fifo_az_aware.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_az_orders), C.POINTER(gp_zone_results)]
     L.gp_pack_batch_az_aware.restype = C.c_int
     L.gp_pack_batch_az_aware.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_az_orders), C.POINTER(gp_zone_results)]
+    L.gp_pack_fifo_zones_groups.restype = C.c_int
+    L.gp_pack_fifo_zones_groups.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.c_int, C.POINTER(gp_instance_groups),
+                                            C.POINTER(gp_zone_results)]
     L.gp_reserve_placements.restype = C.c_int
     L.gp_reserve_placements.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_results), C.c_int32, C.POINTER(gp_reservation_table)]
     L.gp_apply_usage_delta.restype = C.c_int
@@ -417,6 +425,13 @@ def _az_orders(exec_order, drv_order, n_zones):
     eo, do = _np(exec_order, np.int32), _np(drv_order, np.int32)
     o = gp_az_orders(n_zones=int(n_zones), n_exec=len(eo), exec_order=_p(eo), n_drv=len(do), drv_order=_p(do))
     return C.byref(o), (o, eo, do)
+
+
+def _instance_groups(group_off, n_zones=None, exec_off=None, exec_order=None, drv_off=None, drv_order=None):
+    """-> (gp_instance_groups, kept arrays) over int32 copies of the given columns (None stays NULL)."""
+    cols = [_np(x, np.int32) for x in (group_off, n_zones, exec_off, exec_order, drv_off, drv_order)]
+    ig = gp_instance_groups(len(cols[0]) - 1, *[_p(x) for x in cols])
+    return ig, cols
 
 
 _LABEL_COLS = {"label_off": np.int64, "label_key": np.int32, "label_val": np.int32, "label_int_ok": np.uint8, "label_int": np.int64}
@@ -734,7 +749,7 @@ class GangPacker:
         c, m, g = _np(sched_cpu, np.int64), _np(sched_mem, np.int64), _np(sched_gpu, np.int64)
         self._check(load().gp_set_schedulable(self._h, _p(c), _p(m), _p(g)))
 
-    def _pack_zones(self, apps: dict, skip, fn, *args):
+    def _pack_zones(self, apps: dict, skip, fn, *args, group=None):
         """The zone packs' shared body: fn(ctx, apps, *args, results) -> (zone, driver_node, executor_nodes, off, avg_efficiency)."""
         q = len(apps["count"])
         off = np.zeros(q + 1, np.int64)
@@ -742,7 +757,7 @@ class GangPacker:
         total = int(off[-1]) if q else 0
         zone = np.full(q, -9, np.int32); drv = np.full(q, -9, np.int32)
         exe = np.full(max(total, 1), -9, np.int32); avg = np.zeros((max(q, 1), 4), np.float64)
-        a = _apps(apps, off, skip=skip)
+        a = _apps(apps, off, group=group, skip=skip)
         r = gp_zone_results(zone=_p(zone), driver_node=_p(drv), executor_nodes=_p(exe), executor_nodes_cap=len(exe), avg_efficiency=_p(avg))
         self._check(fn(self._h, C.byref(a), *args, C.byref(r)))
         return zone, drv, exe[:total], off, avg[:q]
@@ -772,6 +787,18 @@ class GangPacker:
         -> like pack_batch_zones; zone -1 with driver_node >= 0 = placed by the fallback (zero averages)."""
         o, _keep = _az_orders(exec_order, drv_order, n_zones)
         return self._pack_zones(apps, None, load().gp_pack_batch_az_aware, o)
+
+    def pack_fifo_zones_groups(self, apps: dict, packer: int, mode: int, group_off, n_zones=None, exec_off=None, exec_order=None,
+                               drv_off=None, drv_order=None):
+        """fitEarlierDrivers of every instance group in one launch, one CTA per instance group, with packer
+        BP_SINGLE_AZ_TIGHTLY_PACK / BP_SINGLE_AZ_MINIMAL_FRAGMENTATION (instance group i's snapshot groups group_off[i] ..
+        group_off[i+1]-1 are its zones) or BP_AZ_AWARE_TIGHTLY_PACK (the first n_zones[i] of them its zones, the rest its
+        trailing group; exec_order / drv_order its undivided orders in CSR by exec_off / drv_off).  apps["group"] is each
+        application's instance group (absent: 0), "young" as in pack_fifo_zones.  -> like pack_fifo_zones, with zone local to
+        the application's instance group."""
+        ig, _keep = _instance_groups(group_off, n_zones, exec_off, exec_order, drv_off, drv_order)
+        return self._pack_zones(apps, apps.get("young"), load().gp_pack_fifo_zones_groups, packer, mode, C.byref(ig),
+                                group=apps.get("group"))
 
     def reserve_placements(self, apps: dict, placed, subtract=True):
         """newResourceReservation for a packed batch -> dict of row arrays (app, slot, node, cpu, mem, gpu); with subtract the
