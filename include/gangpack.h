@@ -73,7 +73,11 @@ typedef enum {
 #define GP_CFG_ASYNC_SNAPSHOT 1  /* gp_set_snapshot with page-locked (gp_alloc_pinned / gp_register_host) inputs returns while the
                                     device is still reading them: the buffers must stay unchanged until the next gp_pack_* /
                                     gp_get_snapshot / gp_synchronize call on the context has returned.  The upload then overlaps the
-                                    input copies of that call (one Predicate = snapshot + pack, back to back) */
+                                    input copies of that call (one Predicate = snapshot + pack, back to back).
+                                    Also: a gp_pack_batch_device that directly follows gp_set_snapshot_device on the same stream
+                                    (no other call on the context in between) may start before the slot layout has ended, so
+                                    its inputs (application columns, offsets) must be ready before gp_set_snapshot_device is
+                                    enqueued: a caller's kernel that writes them between the two calls would race with it */
 typedef struct {
     int32_t device;          /* CUDA device ordinal; -1 = current device */
     int32_t flags;           /* GP_CFG_* */

@@ -58,8 +58,8 @@ __device__ __forceinline__ void block_fold(long long& c, long long& m, long long
 //    drv_pos[node] = i for driver-order entry i, and takes the availability of both entries into its CTA's SnapPart (a
 //    node's availability does not depend on its slot); with node_cpu != NULL it also copies node-table entry i into the
 //    context's node-table arrays (gp_get_snapshot).  Every CTA writes its part, zeros included, so nothing needs a reset.
-// K2 gp_build_slots_drv: every CTA first folds K1's parts (written by the previous launch on the stream: no fence or
-//    counter needed) into the maxima its compact views shift by; CTA 0 publishes them in SnapMeta (flags, max_avail,
+// K2 gp_build_slots_drv: every CTA first folds K1's parts (visible once its pdl_wait has returned: no fence or counter
+//    needed) into the maxima its compact views shift by; CTA 0 publishes them in SnapMeta (flags, max_avail,
 //    shift32).  Thread s <= n_slots owns slot s.  Executor slots get their compact view; the spare slot of driver-order
 //    entry j either receives that node (driver-only) or stays unused (-1: the node has an executor slot in the group);
 //    slots past the last group (the orders' lengths may be upper bounds) are -1 as well.  So no slot_node memset is needed.
@@ -81,6 +81,7 @@ __global__ void __launch_bounds__(kSnapThreads) gp_build_slots_exec(int32_t n_ex
                                     int32_t* __restrict__ slot_node, int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_pos,
                                     SnapPart* __restrict__ parts,
                                     int64_t* __restrict__ node_cpu, int64_t* __restrict__ node_mem, int64_t* __restrict__ node_gpu) {
+    pdl_trigger();                       // K2 may start: it waits for this launch before it reads anything of it
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     long long c = 0, m = 0, gm = 0;      // only positive availabilities raise the maxima
     int neg = 0;
@@ -135,14 +136,42 @@ __device__ __forceinline__ int32_t slot_group(const int32_t* exec_off, const int
     return lo;
 }
 
+// seg_pre[g] = table segments (gangpack_tables.cuh) of the groups before g, max(1, ceil(ne / kTabSeg)) each: an empty group
+// still has the one segment that writes its total and first_host; seg_pre[n_groups] = all of them.  Called by a whole CTA.
+__device__ __forceinline__ void segment_prefix(int32_t n_groups, const int32_t* __restrict__ exec_off, int32_t* __restrict__ seg_pre) {
+    __shared__ uint32_t part[kSnapThreads / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t carry = 0;
+    for (int32_t g0 = 0; g0 < n_groups; g0 += kSnapThreads) {
+        const int32_t g = g0 + (int32_t)threadIdx.x;
+        const uint32_t n = g < n_groups ? (uint32_t)max(1, (exec_off[g + 1] - exec_off[g] + kTabSeg - 1) / kTabSeg) : 0u;
+        const uint32_t incl = warp_incl_scan(n, lane);
+        if (lane == 31) part[w] = incl;
+        __syncthreads();
+        uint32_t before = carry, all = carry;
+        for (int t = 0; t < kSnapThreads / 32; ++t) { if (t < w) before += part[t]; all += part[t]; }
+        if (g < n_groups) seg_pre[g] = (int32_t)(before + incl - n);
+        carry = all;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) seg_pre[n_groups] = (int32_t)carry;
+}
+
+// Launched as K1's dependent: it may start once every CTA of K1 has started, and waits for K1 to end (pdl_wait) before it
+// reads anything K1 writes.  Its last CTA first writes the snapshot's segment prefix, which gp_decide_tables reads after
+// the layout; it reads only exec_off, an input of the layout, complete before K1 started.
 __global__ void __launch_bounds__(kSnapThreads) gp_build_slots_drv(int32_t n_slots, int32_t n_groups, int32_t n_nodes, int32_t n_drv,
                                    const int32_t* __restrict__ exec_off, const int32_t* __restrict__ drv_off,
                                    const int32_t* __restrict__ drv_order, const int32_t* __restrict__ drv_pos,
                                    const int64_t* __restrict__ cpu, const int64_t* __restrict__ mem, const int64_t* __restrict__ gpu,
                                    longlong2* __restrict__ pair, int64_t* __restrict__ sgpu, int32_t* __restrict__ slot_node,
                                    int32_t* __restrict__ node_slot, int32_t* __restrict__ drv_slot, const SnapPart* __restrict__ parts,
-                                   int32_t n_parts, SnapMeta* __restrict__ meta, uint2* __restrict__ pair32) {
+                                   int32_t n_parts, SnapMeta* __restrict__ meta, uint2* __restrict__ pair32,
+                                   int32_t* __restrict__ seg_pre) {
     __shared__ long long s_max[2];
+    pdl_trigger();                       // a pack call's gp_decide_tables may start: it waits for this launch (see there)
+    if (blockIdx.x == gridDim.x - 1) segment_prefix(n_groups, exec_off, seg_pre);
+    pdl_wait();
     {
         long long c = 0, m = 0, g = 0;
         int f = 0;
@@ -324,16 +353,17 @@ gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, i
     GP_CUDA(c, c->drv_slot.reserve(sizeof(int32_t) * (size_t)(n_drv + 1)));
     GP_CUDA(c, c->groups.reserve(sizeof(GroupDesc) * (size_t)dn->n_groups));
     GP_CUDA(c, c->drv_pos.reserve(sizeof(int32_t) * (size_t)(dn->n_nodes + 1)));
+    GP_CUDA(c, c->seg_pre.reserve(sizeof(int32_t) * (size_t)(dn->n_groups + 1)));
     int64_t* node_cpu = copy_nodes ? c->node_cpu.as<int64_t>() : nullptr;
     const int T = kSnapThreads;
     const int32_t n1 = std::max(std::max(std::max(n_exec, n_drv), dn->n_groups), node_cpu ? dn->n_nodes : 0);
     const int32_t blocks1 = (n1 + T - 1) / T;
     GP_CUDA(c, c->snap_part.reserve(sizeof(SnapPart) * (size_t)blocks1));
     SnapPart* parts = c->snap_part.as<SnapPart>();
-    struct { gp_nodes dn; int32_t n_exec, n_drv; void* buf[13]; } key{};
+    struct { gp_nodes dn; int32_t n_exec, n_drv; void* buf[14]; } key{};
     key.dn = *dn; key.n_exec = n_exec; key.n_drv = n_drv;
-    void* bufs[13] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p,
-                      node_cpu, c->node_mem.p, c->node_gpu.p, c->drv_pos.p, c->snap_part.p};
+    void* bufs[14] = {c->pair.p, c->pair32.p, c->sgpu.p, c->slot_node.p, c->node_slot.p, c->drv_slot.p, c->groups.p, c->snap_flags.p,
+                      node_cpu, c->node_mem.p, c->node_gpu.p, c->drv_pos.p, c->snap_part.p, c->seg_pre.p};
     std::memcpy(key.buf, bufs, sizeof(bufs));
     gp_status rs = run_cached(c, c->g_snapshot, &key, sizeof(key), st, [&](int& launches) -> gp_status {
         gp_build_slots_exec<<<blocks1, T, 0, st>>>(
@@ -342,11 +372,11 @@ gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, i
             c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->drv_pos.as<int32_t>(), parts, node_cpu,
             c->node_mem.as<int64_t>(), c->node_gpu.as<int64_t>());
         // threads [0, n_slots]: slots; [n_slots + 1, n_slots + 1 + n_nodes]: nodes
-        gp_build_slots_drv<<<(n_slots + dn->n_nodes + 1 + T) / T, T, 0, st>>>(
+        GP_CUDA(c, launch_pdl(true, (n_slots + dn->n_nodes + 1 + T) / T, T, st, gp_build_slots_drv,
             n_slots, dn->n_groups, dn->n_nodes, n_drv, dn->exec_off, dn->drv_off, dn->drv_order, c->drv_pos.as<int32_t>(),
             dn->avail_cpu_milli, dn->avail_mem_bytes, dn->avail_gpu, c->pair.as<longlong2>(), c->sgpu.as<int64_t>(),
             c->slot_node.as<int32_t>(), c->node_slot.as<int32_t>(), c->drv_slot.as<int32_t>(), parts, blocks1,
-            c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>());
+            c->snap_flags.as<SnapMeta>(), c->pair32.as<uint2>(), c->seg_pre.as<int32_t>()));
         GP_CUDA(c, cudaGetLastError());
         launches = 0;       // (the snapshot layout is not part of a pack call's launch count)
         return GP_OK;
@@ -474,6 +504,7 @@ gp_status gp_synchronize(gp_ctx* ctx) {
 
 gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!n || n->n_nodes < 0 || n->n_groups < 1 || !n->exec_off || !n->drv_off ||
         (n->n_nodes > 0 && (!n->avail_cpu_milli || !n->avail_mem_bytes)))
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot: missing arrays or bad sizes");
@@ -582,6 +613,7 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
 
 gp_status gp_set_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, void* stream) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!dn || dn->n_nodes < 0 || dn->n_groups < 1 || !dn->exec_off || !dn->drv_off || n_exec < 0 || n_drv < 0 ||
         (n_exec > 0 && !dn->exec_order) || (n_drv > 0 && !dn->drv_order))
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot_device: missing arrays or bad sizes");
@@ -590,11 +622,14 @@ gp_status gp_set_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, 
     // keep a node-table copy so gp_get_snapshot can answer for nodes outside every group: the layout kernel makes it
     const size_t nb = sizeof(int64_t) * (size_t)(dn->n_nodes + 1);
     GP_CUDA(c, c->node_cpu.reserve(nb)); GP_CUDA(c, c->node_mem.reserve(nb)); GP_CUDA(c, c->node_gpu.reserve(nb));
-    return build_snapshot_device(c, dn, n_exec, n_drv, st, dn->n_nodes > 0);
+    const gp_status s = build_snapshot_device(c, dn, n_exec, n_drv, st, dn->n_nodes > 0);
+    if (s == GP_OK && c->async_snapshot) c->layout_tail = st;      // the layout is the last work on st
+    return s;
 }
 
 gp_status gp_get_snapshot(gp_ctx* c, int64_t* cpu, int64_t* mem, int64_t* gpu) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_get_snapshot: no snapshot");
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;

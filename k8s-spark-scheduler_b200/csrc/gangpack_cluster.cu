@@ -277,6 +277,7 @@ extern "C" {
 gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver_order, int32_t* n_driver,
                              int32_t* executor_order, int32_t* n_executor) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!in || in->n_nodes < 0 || in->n_zones < 1 || !n_driver || !n_executor ||
         (in->n_nodes > 0 && (!in->avail_cpu_milli || !in->avail_mem_bytes || !driver_order || !executor_order)))
         return fail(c, GP_ERR_INVALID, "gp_potential_nodes: missing arrays or bad sizes");
@@ -304,6 +305,7 @@ gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver
 gp_status gp_build_availability(gp_ctx* c, const gp_usage_input* in, int64_t* avail_cpu, int64_t* avail_mem, int64_t* avail_gpu,
                                 int64_t* sched_cpu, int64_t* sched_mem, int64_t* sched_gpu) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     int64_t* const outs[6] = {avail_cpu, avail_mem, avail_gpu, sched_cpu, sched_mem, sched_gpu};
     return availability_out(c, in, false, outs, "gp_build_availability");
 }
@@ -311,6 +313,7 @@ gp_status gp_build_availability(gp_ctx* c, const gp_usage_input* in, int64_t* av
 // availableResources of rescheduleExecutor's first-fit branch: the availability to upload before gp_reschedule_executors(min_frag = 0)
 gp_status gp_build_reschedule_availability(gp_ctx* c, const gp_usage_input* in, int64_t* avail_cpu, int64_t* avail_mem, int64_t* avail_gpu) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     int64_t* const outs[6] = {avail_cpu, avail_mem, avail_gpu, nullptr, nullptr, nullptr};
     return availability_out(c, in, true, outs, "gp_build_reschedule_availability");
 }
@@ -318,6 +321,7 @@ gp_status gp_build_reschedule_availability(gp_ctx* c, const gp_usage_input* in, 
 // reservations -> availability -> priority orders -> slot layout, without leaving the device
 gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, int32_t* n_driver, int32_t* n_executor) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (n_driver) *n_driver = 0;
     if (n_executor) *n_executor = 0;
     long long *d_avail = nullptr, *d_sched = nullptr;
@@ -347,6 +351,7 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
 // reservations -> availability -> priority orders -> zone-grouped slot layout, without leaving the device
 gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!layout) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: missing arrays or mismatched sizes");
     const int32_t kind = layout->kind;
     if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
@@ -432,6 +437,7 @@ gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const
 // rescheduleExecutor's node choice for a batch of executors (SURVEY 8f row f4); see gangpack_resched.cuh
 gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* node_out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_reschedule_executors: gp_set_snapshot first");
     if (!in || in->n_execs < 0 || (in->n_execs > 0 && (!in->exe_cpu_milli || !in->exe_mem_bytes || !node_out)))
         return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: missing arrays or bad sizes");
@@ -501,6 +507,7 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
 gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const gp_reschedule_scope* scope,
                                           const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     static const char* who = "gp_reschedule_from_reservations";
     GP_TRY(check_usage(c, usage, who));
     if (!sort || !in || usage->n_nodes != sort->n_nodes || sort->n_zones < 1 ||
@@ -598,6 +605,7 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
 gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
                                   gp_reconcile_results* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     static const char* who = "gp_reconcile_find_nodes";
     GP_TRY(check_usage(c, usage, who));
     if (!nodes || !a || !out || nodes->n_groups < 1 || a->n_apps < 0 || (usage->n_nodes > 0 && (!nodes->node_group || !nodes->creation)) ||

@@ -154,6 +154,7 @@ struct gp_ctx {
     DevBuf pair, pair32, sgpu, slot_node, node_slot, drv_slot, groups, snap_flags;
     DevBuf drv_pos;                             // node -> driver-order position, scattered by the layout (gp_build_slots_exec)
     DevBuf snap_part;                           // SnapPart per CTA of gp_build_slots_exec
+    DevBuf seg_pre;                             // [n_groups + 1] table segments before each group (gp_build_slots_drv)
 
     // batch staging; a_rows: the six quantity rows in one pitched block (pack_batch_impl)
     DevBuf a_rows, a_count, a_group, a_skip, a_off;
@@ -180,6 +181,10 @@ struct gp_ctx {
     int use_tables = 1;                           // GANGPACK_TABLES=0: every independent decision takes the node-order scan
     int fifo_warp = 1;                            // GANGPACK_FIFO_WARP=0: every FIFO application is decided by the whole CTA
     bool async_snapshot = false;                  // gp_config.flags & GP_CFG_ASYNC_SNAPSHOT
+    // With async_snapshot: the stream on which the context's last call, gp_set_snapshot_device, enqueued the slot layout
+    // (nullptr: none).  Every other entry point that enqueues device work clears it.  While it is set, a
+    // gp_pack_batch_device on that stream may start its gp_decide_tables before the layout ends (pack_device_range).
+    cudaStream_t layout_tail = nullptr;
     int chunk_apps = kChunkApps;                  // GANGPACK_CHUNK_APPS
     int trace = 0;                                // GANGPACK_TRACE=1: host-side phase timing on stderr
     int pack_ctas_per_sm = 0;                       // occupancy of gp_pack_independent<2> on this device
@@ -249,6 +254,18 @@ static gp_status refuse(gp_ctx* c, int word, const Refusal (&table)[K], const ch
     for (const Refusal& r : table)
         if (word & r.bits) return fail(c, r.status, who, r.what);
     return GP_OK;
+}
+
+// Launch kernel k on st; with early, as a programmatic dependent of the kernel before it on st (pdl_wait, pdl_trigger).
+template <class... P, class... A>
+static cudaError_t launch_pdl(bool early, dim3 grid, dim3 block, cudaStream_t st, void (*k)(P...), A&&... args) {
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = early ? 1 : 0;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, k, std::forward<A>(args)...);
 }
 
 // issue(): enqueues the sequence on `st` and returns (status, launches).  See GraphCache.
@@ -339,5 +356,6 @@ struct DevResults {
 gp_status pack_begin(gp_ctx* c, int32_t q, gp_algo algo, gp_mode mode, int64_t exec_cap, bool derive_off, int2** scratch, cudaStream_t st,
                      bool status_in_kernel = false);
 gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi, int64_t off_base, gp_algo algo, gp_mode mode,
-                            const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel = false);
+                            const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel = false,
+                            bool after_layout = false);
 gp_status host_error(gp_ctx* c);

@@ -94,6 +94,18 @@ struct GroupDesc {
     int32_t nd;      // driver-order length
 };
 
+// Independent-mode capacity tables (gangpack_tables.cuh) are built in segments of kTabSeg executor-order positions.  The
+// slot layout counts each group's segments once per snapshot (gp_build_slots_drv), so a pack call need not.
+constexpr int kTabThreads = 256;      // every phase of gp_decide_tables; also the applications per classify tile
+constexpr int kTabPerThread = 4;
+constexpr int kTabSeg = kTabThreads * kTabPerThread;      // nodes per table segment
+
+// Programmatic dependent launch (sm_90).  A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may
+// start once every CTA of the kernel before it on the stream has run pdl_trigger() or exited; its pdl_wait() returns once
+// that kernel has completed and its writes are visible.  Without the attribute pdl_wait() returns at once.
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // Device snapshot: "slots" = per group the executor order followed by one spare slot per driver
 // candidate (used only when that candidate is not an executor candidate).
 struct Snapshot {

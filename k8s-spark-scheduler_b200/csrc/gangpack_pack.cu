@@ -178,7 +178,8 @@ template <int ALGO, class OUT>
 static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& cols, const ShapeTables& tabs, int64_t off_base,
                                int64_t* off_out, int32_t* app_slot, PrepApp* prep, int32_t* listed, int32_t q, const DevResults& dr,
                                int32_t lo, int2* scratch, unsigned long long* stats, unsigned int* next_app, int* d_err,
-                               volatile int* err_host, bool use_tables, int64_t seg_bound, unsigned int* status_zero, cudaStream_t st) {
+                               volatile int* err_host, bool use_tables, int64_t seg_bound, unsigned int* status_zero, bool early_start,
+                               cudaStream_t st) {
     int& dec_per_sm = c->dec_ctas_per_sm[ALGO][sizeof(OUT) == 2 ? 1 : 0];
     if (dec_per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&dec_per_sm, gp_decide_tables<ALGO, OUT>, kTabThreads, 0);
@@ -189,9 +190,10 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
     const int64_t shapes = std::min<int64_t>(q, kMaxShapes);
     int64_t blocks = tiles * ((use_tables || off_out) ? 2 : 1) + (use_tables ? shapes * (seg_bound + c->n_groups) : 0);
     blocks = std::min<int64_t>(blocks, (int64_t)c->sm_count * dec_per_sm);
-    gp_decide_tables<ALGO, OUT><<<(int)blocks, kTabThreads, 0, st>>>(s, cols, tabs, off_base, off_out, app_slot, q, dr.cap, dr.driver + lo,
-                                                                    static_cast<OUT*>(dr.exec), prep, listed, stats, d_err, err_host,
-                                                                    use_tables ? 0 : 1, status_zero);
+    // early_start: it may start while the slot layout before it on st still runs (see gp_decide_tables)
+    GP_CUDA(c, launch_pdl(early_start, (int)blocks, kTabThreads, st, gp_decide_tables<ALGO, OUT>, s, cols, tabs, off_base, off_out, app_slot,
+                          q, dr.cap, dr.driver + lo, static_cast<OUT*>(dr.exec), prep, listed, stats, d_err, err_host,
+                          use_tables ? 0 : 1, status_zero));
     int& per_sm = c->tab_ctas_per_sm[ALGO][sizeof(OUT) == 2 ? 1 : 0];
     if (per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_pack_listed<ALGO, OUT>, kPackTabThreads, 0);
@@ -202,10 +204,11 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
     const int64_t max_blocks = (int64_t)c->sm_count * (use_tables ? 2 : per_sm);
     if (blocks > max_blocks) blocks = max_blocks;
     if (blocks < 1) blocks = 1;
-    // it also zeroes the classify tiles' and the table segments' look-back words (see there)
-    gp_pack_listed<ALGO, OUT><<<(int)blocks, kPackTabThreads, 0, st>>>(s, tabs, (int32_t)tiles, use_tables ? kMaxShapes * (int32_t)seg_bound : 0,
-                                                                      prep, listed, dr.driver + lo, static_cast<OUT*>(dr.exec), scratch,
-                                                                      stats, next_app);
+    // it also zeroes the classify tiles' and the table segments' look-back words (see there); it waits for
+    // gp_decide_tables before it reads or writes anything
+    GP_CUDA(c, launch_pdl(true, (int)blocks, kPackTabThreads, st, gp_pack_listed<ALGO, OUT>, s, tabs, (int32_t)tiles,
+                          use_tables ? kMaxShapes * (int32_t)seg_bound : 0, prep, listed, dr.driver + lo, static_cast<OUT*>(dr.exec),
+                          scratch, stats, next_app));
     c->last.kernel_launches += 2;
     return GP_OK;
 }
@@ -213,8 +216,10 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
 // Device-resident apps [lo, hi): enqueue the kernels on `st`; chunk index selects the timing events and the table lane.
 // off_base: ExecutorNodes offset of application `lo` (only used when the offsets are derived on the device).
 // status_in_kernel: pack_begin left the status block to this range's decide kernel (kernel_zeroes_status(), one range only).
+// after_layout: the last work on st is this context's slot layout, and the caller's inputs were ready before it was
+// enqueued (gp_ctx::layout_tail).
 gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi, int64_t off_base, gp_algo algo, gp_mode mode,
-                            const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel) {
+                            const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel, bool after_layout) {
     const int32_t q = hi - lo;
     if (q <= 0) return GP_OK;
     int* d_err = &c->status()->head.err;
@@ -241,13 +246,17 @@ gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi
         // sum over the groups of max(1, ceil(ne / kTabSeg)) <= n_slots / kTabSeg + n_groups
         const int64_t seg_bound = (int64_t)c->n_slots / kTabSeg + c->n_groups + 1;
         const size_t hdr_bytes = 1024 + hash_bytes + cls_bytes + sizeof(unsigned long long) * (size_t)kMaxShapes * (size_t)seg_bound;
+        const size_t hdr_cap = T.hdr.cap;
         GP_CUDA(c, T.hdr.reserve_zeroed(hdr_bytes, st));
+        // gp_decide_tables may start before the layout ends only when it is the first work this call enqueues: neither
+        // pack_begin's status memset nor the header's zeroing above (a timing event is no work)
+        const bool early_start = after_layout && status_in_kernel && T.hdr.cap == hdr_cap;
         // [executor slot | driver slot | listed]
         GP_CUDA(c, T.app_slot.reserve(sizeof(int32_t) * (3 * (size_t)q + 1)));
         if (use_tables) {
             GP_CUDA(c, T.table.reserve(sizeof(uint32_t) * (size_t)kMaxShapes * (size_t)((c->n_slots + 4) & ~3)));
-            // total | firstfit | first_host | segments before each group
-            GP_CUDA(c, T.total.reserve(sizeof(uint32_t) * (3 * (size_t)kMaxShapes * (size_t)c->n_groups + (size_t)c->n_groups + 1)));
+            // total | firstfit | first_host
+            GP_CUDA(c, T.total.reserve(sizeof(uint32_t) * 3 * (size_t)kMaxShapes * (size_t)c->n_groups));
             GP_CUDA(c, T.place.reserve(sizeof(int32_t) * (size_t)kMaxShapes * (size_t)c->n_groups * kPlaceLen));
         }
         ShapeTables tabs;
@@ -259,7 +268,7 @@ gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi
         tabs.table = T.table.as<uint32_t>(); tabs.total = T.total.as<uint32_t>();
         tabs.firstfit = reinterpret_cast<int32_t*>(T.total.as<uint32_t>() + (size_t)kMaxShapes * (size_t)c->n_groups);
         tabs.first_host = tabs.firstfit + (size_t)kMaxShapes * (size_t)c->n_groups;
-        tabs.seg_pre = tabs.first_host + (size_t)kMaxShapes * (size_t)c->n_groups;
+        tabs.seg_pre = c->seg_pre.as<int32_t>();
         tabs.place = T.place.as<int32_t>();
         tabs.pitch = (c->n_slots + 4) & ~3; tabs.n_groups = c->n_groups;      // rows start 16-byte aligned
         int32_t* app_slot = T.app_slot.as<int32_t>();
@@ -274,7 +283,7 @@ gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi
             const int before = (int)c->last.kernel_launches;
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][1], st));
             const gp_status r = launch(c, s, cols, tabs, off_base, off_out, app_slot, prep, listed, q, dr, lo, scratch, d_stats, next_app,
-                                       d_err, err_host, use_tables, seg_bound, status_zero, st);
+                                       d_err, err_host, use_tables, seg_bound, status_zero, early_start, st);
             if (r != GP_OK) return r;
             GP_CUDA(c, cudaGetLastError());
             if (c->record_events) GP_CUDA(c, cudaEventRecord(c->ev[chunk][2], st));
@@ -288,9 +297,9 @@ gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi
             c->last.kernel_launches += n;
             return r;
         }
-        struct { int32_t algo, o16, use_tables, q, lo, chunk; int64_t off_base; AppColumns cols; ShapeTables tabs; Snapshot snap;
+        struct { int32_t algo, o16, use_tables, q, lo, chunk, early_start; int64_t off_base; AppColumns cols; ShapeTables tabs; Snapshot snap;
                  const void* p[11]; int64_t cap; } key{};
-        key.algo = (int32_t)algo; key.o16 = o16; key.use_tables = use_tables; key.q = q; key.lo = lo; key.chunk = chunk; key.off_base = off_base;
+        key.algo = (int32_t)algo; key.o16 = o16; key.use_tables = use_tables; key.q = q; key.lo = lo; key.chunk = chunk; key.early_start = early_start; key.off_base = off_base;
         key.cols = cols; key.tabs = tabs; key.snap = s; key.cap = dr.cap;
         const void* ptrs[11] = {app_slot, prep, listed, dr.driver, dr.exec, scratch, d_stats, next_app, d_err, off_out, status_zero};
         std::memcpy(key.p, ptrs, sizeof(ptrs));
@@ -407,6 +416,8 @@ extern "C" {
 
 gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mode mode, gp_results* dout, void* stream) {
     if (!c) return GP_ERR_INVALID;
+    const cudaStream_t layout_tail = c->layout_tail;
+    c->layout_tail = nullptr;
     if (!da || !dout) return fail(c, GP_ERR_INVALID, "gp_pack_batch_device: NULL apps/results");
     const gp_apps_wire w = widen(da);
     gp_results_wire ow{dout->driver_node, dout->executor_nodes, dout->executor_nodes_cap, 32, 0};
@@ -416,6 +427,7 @@ gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mo
     cudaStream_t st = stream ? (cudaStream_t)stream : c->stream;
     int2* scratch = nullptr;
     const bool zero_in_kernel = kernel_zeroes_status(w.n_apps, algo, mode);
+    const bool after_layout = layout_tail == st;
     s = pack_begin(c, w.n_apps, algo, mode, ow.executor_nodes_cap, !w.exec_out_off, &scratch, st, zero_in_kernel);
     if (s != GP_OK || w.n_apps == 0) return s;
     DevApps dv{};
@@ -424,13 +436,14 @@ gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mo
     dv.cols.count = w.exe_count; dv.cols.group = w.group; dv.cols.off = w.exec_out_off; dv.cols.bits = 64; dv.cols.mem_shift = 0;
     dv.skip = w.skip_if_no_fit; dv.n = w.n_apps;
     DevResults dr{ow.driver_node, ow.executor_nodes, ow.executor_nodes_cap, 32};
-    s = pack_device_range(c, dv, 0, w.n_apps, 0, algo, mode, dr, scratch, st, 0, zero_in_kernel);
+    s = pack_device_range(c, dv, 0, w.n_apps, 0, algo, mode, dr, scratch, st, 0, zero_in_kernel, after_layout);
     if (s == GP_OK) c->ev_chunks = 1;
     return s;
 }
 
 gp_status gp_last_stats(gp_ctx* c, gp_stats* out) {
     if (!c || !out) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     GP_CUDA(c, cudaSetDevice(c->device));
     StatusHead& h = c->host_status()->head;
     GP_CUDA(c, cudaMemcpyAsync(&h, &c->status()->head, sizeof(StatusHead), cudaMemcpyDeviceToHost, c->stream));
@@ -459,6 +472,7 @@ static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo,
 
 gp_status gp_pack_batch_wire(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, gp_results_wire* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     gp_status s = pack_batch_impl(c, a, algo, mode, out);
     if (s != GP_OK) {
         // Whatever was enqueued before the failure may still read the caller's buffers or write its results:
@@ -662,6 +676,7 @@ gp_status gp_pack_one(gp_ctx* c, gp_algo algo, int64_t drv_cpu, int64_t drv_mem,
                       int64_t exe_mem, int64_t exe_gpu, int32_t exe_count, int32_t* has_capacity, int32_t* driver_node,
                       int32_t* executor_nodes) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!has_capacity || !driver_node) return fail(c, GP_ERR_INVALID, "gp_pack_one: NULL outputs");
     if (exe_count > 0 && !executor_nodes) return fail(c, GP_ERR_INVALID, "gp_pack_one: executor_nodes is NULL");
     // The tuple and the result travel through a context-owned mapped pinned block: no DMA copies at all

@@ -45,9 +45,6 @@ namespace gp {
 constexpr int kShapeSlots = 1024;     // hash slots (power of two)
 constexpr int kShapeProbes = 16;      // linear probes before giving up (-> scan path)
 constexpr int kMaxShapes = 64;        // dense tables per batch
-constexpr int kTabThreads = 256;      // every phase of gp_decide_tables; also the applications per classify tile
-constexpr int kTabPerThread = 4;
-constexpr int kTabSeg = kTabThreads * kTabPerThread;      // nodes per table segment
 constexpr int kPlaceLen = 256;        // placement prefix per (shape, group): covers every count <= 128 whatever the driver takes
 
 struct __align__(16) ShapeEntry {     // 96 bytes
@@ -90,7 +87,7 @@ struct ShapeTables {
     ShapeHeader* hdr;
     unsigned long long* cls_status;   // [classify tiles] look-back words of the derived offsets (zero at the start of a call)
     unsigned long long* seg_status;   // [kMaxShapes * segments] look-back words of the table segments (zero at the start of a call)
-    int32_t* seg_pre;                 // [n_groups + 1] table segments before each group (written by classify tile 0)
+    const int32_t* seg_pre;           // [n_groups + 1] table segments before each group (the snapshot's, gp_build_slots_drv)
     uint32_t* table;                  // [kMaxShapes][pitch] exclusive prefix per instance group, indexed by slot
     uint32_t* total;                  // [kMaxShapes][n_groups]
     int32_t* firstfit;                // [kMaxShapes][n_groups] first driver-order position the driver shape fits on (nd: none)
@@ -271,8 +268,9 @@ __device__ __forceinline__ void classify_offsets(OneScratch& sh, int32_t tile, i
 }
 
 // per thread: today's gp_classify_apps body
+// It reads nothing of the snapshot: gp_decide_tables runs it before the slot layout has ended.
 __device__ __forceinline__ void gp_classify_apps(int32_t tile, int32_t n_apps, const AppColumns& cols, const ShapeTables& tabs,
-                                                 const SnapMeta* meta, int32_t* app_slot) {
+                                                 int32_t* app_slot) {
     const int32_t i = tile * kTabThreads + (int32_t)threadIdx.x;
     const int lane = threadIdx.x & 31;
     const unsigned act = __ballot_sync(kFull, i < n_apps);     // the lanes that intern (the whole warp except in the last tile)
@@ -290,13 +288,14 @@ __device__ __forceinline__ void gp_classify_apps(int32_t tile, int32_t n_apps, c
         int32_t found = -1;
         if (lane == leader && e_ok)
             found = intern_shape(tabs.entries, efp, [&](ShapeEntry* en, int32_t slot) {
-                // this lane owns the entry: dense id, division recipes (verified by every consumer against its own tuple)
+                // this lane owns the entry: dense id, division recipes (verified by every consumer against its own tuple).
+                // A recipe depends on the request alone; prep_dim's max_avail only decides `fast`, which is not kept here.
                 int32_t id = atomicAdd(&tabs.hdr->n_shapes, 1);
                 if (id >= kMaxShapes) id = -1;
                 int bad = 0; uint64_t l; bool fast = true;
-                en->div[0] = prep_dim(0, e0, 0, meta->max_avail[0], bad, l, fast);
-                en->div[1] = prep_dim(0, e1, 1, meta->max_avail[1], bad, l, fast);
-                en->div[2] = prep_dim(0, e2, 2, meta->max_avail[2], bad, l, fast);
+                en->div[0] = prep_dim(0, e0, 0, 0, bad, l, fast);
+                en->div[1] = prep_dim(0, e1, 1, 0, bad, l, fast);
+                en->div[2] = prep_dim(0, e2, 2, 0, bad, l, fast);
                 en->flags = e2 != 0 ? 1u : 0u;
                 en->id = id;
                 if (id >= 0) tabs.hdr->id_slot[id] = slot;
@@ -322,27 +321,6 @@ __device__ __forceinline__ void gp_classify_apps(int32_t tile, int32_t n_apps, c
             });
         app_slot[n_apps + i] = __shfl_sync(act, dfound, leader);         // second half of the array: driver-shape slots
     }
-}
-
-// seg_pre[g] = table segments of the groups before g (max(1, ceil(ne / kTabSeg)) each: an empty group still has the one
-// segment that writes its total and first_host); seg_pre[n_groups] = all of them
-__device__ __forceinline__ void segment_prefix(OneScratch& sh, const Snapshot& s, int32_t* seg_pre) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    uint32_t carry = 0;
-    __syncthreads();            // sh.part may still be read by classify_offsets
-    for (int32_t g0 = 0; g0 < s.n_groups; g0 += kTabThreads) {
-        const int32_t g = g0 + (int32_t)threadIdx.x;
-        const uint32_t n = g < s.n_groups ? (uint32_t)max(1, (s.groups[g].ne + kTabSeg - 1) / kTabSeg) : 0u;
-        const uint32_t incl = warp_incl_scan(n, lane);
-        if (lane == 31) sh.part[w] = incl;
-        __syncthreads();
-        uint32_t before = carry, all = carry;
-        for (int t = 0; t < kTabThreads / 32; ++t) { if (t < w) before += (uint32_t)sh.part[t]; all += (uint32_t)sh.part[t]; }
-        if (g < s.n_groups) seg_pre[g] = (int32_t)(before + incl - n);
-        carry = all;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) seg_pre[s.n_groups] = (int32_t)carry;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -767,6 +745,15 @@ __device__ __forceinline__ void decide_app(int32_t i, const AppIn& a, const Snap
 // words: error bits, statistics, claim counters) instead of a memset before the launch.  It finishes before cls_done can
 // count every tile, and every CTA waits for that count before it appends to the list, writes the error word or adds to
 // the statistics, so no write of the call is lost to the zeroing.
+// Early start (programmatic dependent launch).  The host may launch this kernel while the slot layout that precedes it
+// on the stream (gp_build_slots_drv) is still running (launch_tables, early_start).  So the classify tiles read nothing
+// of the snapshot: they read the application columns and offsets, and write app_slot, the hash entries, the look-back
+// words, the ticket, n_listed and the status block, none of which the layout kernels touch.  Every CTA runs pdl_wait()
+// right after its cls_done wait, before its first read of seg_pre, s.groups or anything else of the snapshot; every
+// table item and every decide chunk comes after it.  The host allows the early start only when the application columns
+// were ready before the layout was enqueued (gangpack.h, GP_CFG_ASYNC_SNAPSHOT).  Forward progress is as above: this
+// kernel starts only once every CTA of gp_build_slots_drv has run pdl_trigger(), so every CTA it waits for is already
+// resident and finishes whatever this grid occupies.  Each CTA runs pdl_trigger() as it leaves, for gp_pack_listed.
 template <int ALGO, class OUT>
 __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppColumns cols, ShapeTables tabs, int64_t off_base,
                                                                 int64_t* off_out /* or NULL */, int32_t* app_slot, int32_t n_apps,
@@ -793,10 +780,7 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
                 if (status_zero && threadIdx.x < kStatusWords) status_zero[threadIdx.x] = 0u;
             }
             if (off_out) classify_offsets(sh, t, n_apps, cols, tabs, off_base, off_out);
-            if (!force_scan) {
-                gp_classify_apps(t, n_apps, cols, tabs, s.meta, app_slot);
-                if (t == 0) segment_prefix(sh, s, tabs.seg_pre);
-            }
+            if (!force_scan) gp_classify_apps(t, n_apps, cols, tabs, app_slot);
             signal_done(&hdr->cls_done);
             GP_TL(if (threadIdx.x == 0) tl_rec(tl_n, kTlCls, (uint32_t)t, tl_t0);)
             continue;
@@ -808,6 +792,7 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
                 GP_TL(tl_rec(tl_n, kTlClsWait, 0u, w0);)
             }
             __syncthreads();
+            pdl_wait();                 // the slot layout has ended: everything below may read the snapshot
             n_tab = 0;
             if (!force_scan) {
                 n_es = min(hdr->n_shapes, kMaxShapes);
@@ -875,6 +860,7 @@ __global__ void __launch_bounds__(kTabThreads) gp_decide_tables(Snapshot s, AppC
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) { probes += __shfl_xor_sync(kFull, probes, d); drivers += __shfl_xor_sync(kFull, drivers, d); }
     if ((threadIdx.x & 31) == 0 && (probes | drivers)) { atomicAdd(stats + 0, probes); atomicAdd(stats + 1, drivers); }
+    pdl_trigger();
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -886,8 +872,9 @@ constexpr int kPackTabThreads = 256;
 #endif
 // It is the last kernel of every call on its table set, so it also leaves the set clean for the next call: its CTAs zero
 // the counters, the hash keys and the n_cls_words / n_seg_words look-back words the call used (a claimer writes every
-// other field of a hash entry).  gp_decide_tables, which uses all of these, has finished: the two launches are
-// stream-ordered.  No CTA sizes its share from a header word, and n_listed, which they read, is left to the next call.
+// other field of a hash entry).  It is launched as gp_decide_tables' dependent and may start while that kernel's last CTAs
+// are leaving; every CTA waits for gp_decide_tables to finish (pdl_wait) before it reads n_listed or zeroes anything.  No
+// CTA sizes its share from a header word, and n_listed, which they read, is left to the next call.
 template <int ALGO, class OUT>
 __global__ void __launch_bounds__(kPackTabThreads, GP_TAB_MIN_BLOCKS) gp_pack_listed(Snapshot s, ShapeTables tabs, int32_t n_cls_words,
                                                                                      int32_t n_seg_words,
@@ -900,6 +887,7 @@ __global__ void __launch_bounds__(kPackTabThreads, GP_TAB_MIN_BLOCKS) gp_pack_li
                                                                                      unsigned int* __restrict__ next_app) {
     __shared__ uint16_t cap_cache[kPackTabThreads / 32][kCapCache];
     ShapeHeader* hdr = tabs.hdr;
+    pdl_wait();
     const int n = hdr->n_listed;
     {
         const int32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;

@@ -15,6 +15,7 @@ extern "C" {
 // ---- single-AZ packers: pack every zone, choose by packing efficiency on the device (gangpack_zones.cuh) ----------
 gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, const int64_t* gpu) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_set_schedulable: gp_set_snapshot first");
     if (c->n_nodes > 0 && (!cpu || !mem)) return fail(c, GP_ERR_INVALID, "gp_set_schedulable: missing arrays");
     GP_CUDA(c, cudaSetDevice(c->device));
@@ -207,6 +208,7 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
 
 gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone_results* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_zones: gp_set_snapshot first");
     if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: NULL apps/results");
@@ -410,6 +412,7 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, const int32_t* grou
 // the FIFO loop with a single-AZ packer in one launch
 gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode mode, gp_zone_results* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_zones: gp_set_snapshot first");
     if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: NULL apps/results");
@@ -425,6 +428,7 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
 // the FIFO loop with az-aware-tightly-pack in one launch: the zone packs plus the undivided fallback on the device
 gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const gp_az_orders* o, gp_zone_results* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_az_aware: gp_set_snapshot first");
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones, "
@@ -447,6 +451,7 @@ gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker pa
                                     gp_zone_results* out) {
     const char* who = "gp_pack_fifo_zones_groups";
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, who, "gp_set_snapshot first");
     int kind;
     if (packer == GP_BP_SINGLE_AZ_TIGHTLY_PACK) kind = GP_TIGHTLY_PACK;
@@ -483,6 +488,7 @@ gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker pa
 // on the device, one stream synchronise
 gp_status gp_pack_batch_az_aware(gp_ctx* c, const gp_apps* a, const gp_az_orders* o, gp_zone_results* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_az_aware: gp_set_snapshot first");
     if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
     gp_status s = held_az_orders(c, a, out, &o, "gp_pack_batch_az_aware");
@@ -499,6 +505,7 @@ gp_status gp_pack_batch_az_aware(gp_ctx* c, const gp_apps* a, const gp_az_orders
 
 gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* placed, int32_t subtract, gp_reservation_table* out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_reserve_placements: gp_set_snapshot first");
     if (!a || !placed || a->n_apps < 0 || (!out && !subtract)) return fail(c, GP_ERR_INVALID, "gp_reserve_placements: NULL arguments");
     const int32_t Q = a->n_apps;
@@ -573,6 +580,7 @@ gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* p
 
 gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, const int64_t* cpu, const int64_t* mem, const int64_t* gpu, int32_t sign) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_apply_usage_delta: gp_set_snapshot first");
     if (n_rows < 0 || (sign != 1 && sign != -1) || (n_rows > 0 && (!node || !cpu || !mem))) return fail(c, GP_ERR_INVALID, "gp_apply_usage_delta: bad arguments");
     if (n_rows == 0) return GP_OK;
@@ -610,6 +618,7 @@ static const Refusal kEffRefusals[] = {
 
 gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, double* avg_out) {
     if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
     if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_packing_efficiency: no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)");
     if (!c->have_eff_sched)
         return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: no SchedulableResources (gp_set_schedulable, gp_prepare_cluster or gp_prepare_cluster_zones first)");
