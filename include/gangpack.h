@@ -290,6 +290,60 @@ typedef struct {
 } gp_zone_layout;
 gp_status gp_prepare_cluster_zones(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout);
 
+/* gp_prepare_cluster_zones for every instance group at once: the snapshot gp_pack_fifo_zones_groups drains, built on the
+ * device.  selectDriverNode ranks the nodes of ONE instance group (PotentialNodes over the affinity-filtered node set,
+ * internal/extender/resource.go:292-304; zone priority over that set's zones only, internal/sort/nodesorting.go:95-121).
+ *   instance_group  [n_nodes] the instance group of each node -- its instance-group-label value interned by the caller, or
+ *                   the driver affinity of each instance group matched with gp_match_node_affinity -- in
+ *                   [0, n_instance_groups), -1 = in none; NULL = every node in instance group 0.  Instance groups are
+ *                   disjoint node sets.  A node in none is in no order, but its availability is computed and gp_get_snapshot
+ *                   returns it.
+ *   availability    computed once for every node, exactly as gp_prepare_cluster_zones computes it (GetReservedResources and
+ *                   the overhead are per node, resource.go:300-303), with the same domain and GP_ERR_UNREPRESENTABLE refusal.
+ *   per instance group i: the driver and executor orders are PotentialNodes over i's nodes alone -- zone priority from
+ *                   per-(instance group, zone) exact totals, the candidate / schedulable / ready filters, the stable label
+ *                   re-sort within i, the undefined-tie rule -- grouped by zone exactly as gp_prepare_cluster_zones groups
+ *                   them (candidate zones in driverZonesInOrder order; GP_LAYOUT_SINGLE_AZ: they, or one empty group when
+ *                   there is none; GP_LAYOUT_AZ_AWARE: plus the trailing group, LIB/binpack/single_az.go:36-41,57-73,
+ *                   az_aware_pack_tightly.go:27-38).
+ * Identity: instance group i's slice -- its groups group_off[i] .. group_off[i+1]-1, their zone_of_group, offsets and orders,
+ * its undivided orders, n_zones[i] and undefined_ties[i] -- equals what gp_prepare_cluster_zones returns on a node table holding
+ * only i's nodes (with their reservations), node indices mapped back to this table.  An instance group without nodes gets
+ * the layout of "no candidate zone".  Instance groups are laid out in id order, so their groups are contiguous: the
+ * two-level layout of gp_instance_groups.  sort->undefined_ties (if given) is the total.
+ * The context then holds this layout: gp_pack_fifo_zones_groups(groups == NULL) drains every instance group's queue from it.
+ * It survives FIFO calls, gp_reserve_placements and gp_apply_usage_delta like gp_prepare_cluster_zones' layout; any other
+ * snapshot-setting call replaces it.  With n_instance_groups == 1 the context is also exactly as after
+ * gp_prepare_cluster_zones; with more, gp_pack_fifo_zones, gp_pack_batch_zones and gp_pack_*_az_aware(orders == NULL) are
+ * refused (they would treat every instance group's zones as one instance group's).
+ * GP_ERR_INVALID (gp_last_error names the cause): what gp_prepare_cluster_zones refuses; n_instance_groups < 1; an
+ * instance_group value outside [-1, n_instance_groups); n_instance_groups > 1 with n_instance_groups x (sort->n_zones + 1)
+ * above 2^22 (the per-(instance group, zone) scratch).  A refused call replaces nothing (one synchronise after the
+ * availability stage, as gp_prepare_cluster_zones).  One synchronise more for the counts and the per-instance-group words;
+ * the optional arrays below other than group_off, n_zones, exec_off, drv_off and undefined_ties cost one more copy. */
+typedef struct {
+    int32_t kind;                /* in: gp_zone_layout_kind */
+    int32_t n_groups;            /* out: snapshot groups over every instance group */
+    int32_t n_driver;            /* out: driver candidates over every instance group */
+    int32_t n_executor;          /* out: executor candidates over every instance group */
+    int32_t* group_off;          /* out, or NULL: [n_instance_groups + 1] snapshot groups of each instance group */
+    int32_t* n_zones;            /* out, or NULL: [n_instance_groups] its candidate zones (its first groups) */
+    int32_t* exec_off;           /* out, or NULL: [n_instance_groups + 1] CSR of exec_order */
+    int32_t* exec_order;         /* out, or NULL: [n_nodes] undivided executor orders, instance group by instance group */
+    int32_t* drv_off;            /* out, or NULL: [n_instance_groups + 1] CSR of drv_order */
+    int32_t* drv_order;          /* out, or NULL: [n_nodes] undivided driver orders */
+    int32_t* group_exec_off;     /* out, or NULL: [n_groups + 1] } the grouped layout as gp_nodes would carry it */
+    int32_t* group_exec_order;   /* out, or NULL: [n_nodes]      } */
+    int32_t* group_drv_off;      /* out, or NULL: [n_groups + 1] */
+    int32_t* group_drv_order;    /* out, or NULL: [n_nodes] */
+    int32_t* zone_of_group;      /* out, or NULL: [n_groups] zone id of each group, -1 = trailing / empty group; n_groups <=
+                                    n_instance_groups + min(n_nodes, n_instance_groups x sort->n_zones) */
+    int32_t* undefined_ties;     /* out, or NULL: [n_instance_groups] undefined ties of each instance group's order */
+} gp_instance_group_layout;
+gp_status gp_prepare_cluster_zones_groups(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort,
+                                          const int32_t* instance_group /* [n_nodes], or NULL = every node in group 0 */,
+                                          int32_t n_instance_groups, gp_instance_group_layout* layout);
+
 /* ---- executors without a usable reservation (the step after the hot path; SURVEY 8f row f4) --- */
 /* rescheduleExecutor's node choice (internal/extender/resource.go:594-673) for a BATCH of executor pods, every
  * decision independent against the current snapshot (its executor priority orders and availabilities):
@@ -613,11 +667,16 @@ gp_status gp_exceeds_cluster_capacity(gp_ctx* ctx, const gp_capacity_nodes* node
  * left behind -- is what gp_pack_fifo_zones / gp_pack_fifo_az_aware return on a context holding only that instance group's
  * groups and applications.  gp_stats sums over the instance groups (scan_path_apps: the az-aware fallbacks).
  * GP_ERR_INVALID (gp_last_error names the cause; a refused call changes nothing): another packer or mode; no
- * gp_set_schedulable; a snapshot from gp_set_snapshot_device / gp_prepare_cluster* (no host copy of the layout); group_off
+ * gp_set_schedulable; explicit groups on a snapshot from gp_set_snapshot_device / gp_prepare_cluster* (no host copy of the layout); group_off
  * not monotone from 0 to the snapshot's n_groups; an application's group outside [0, n_instance_groups); more than 64
  * candidate zones in an instance group, or n_zones[i] above its group count; az-aware orders missing, with offsets not
  * monotone from 0 to the snapshot's executor / driver candidate counts, listing a node out of range, twice, of another
- * instance group or not in that role, or a zone group whose order is not its instance group's order restricted to it. */
+ * instance group or not in that role, or a zone group whose order is not its instance group's order restricted to it.
+ * groups == NULL: the layout gp_prepare_cluster_zones_groups left on the context (its per-instance-group words kept on the
+ * host, its undivided orders read on the device, no order check: the library built them).  Refused (GP_ERR_INVALID) after
+ * any other snapshot-setting call (gp_set_snapshot, gp_set_snapshot_device, gp_prepare_cluster, gp_prepare_cluster_zones),
+ * with a packer that does not match the layout's kind (single-AZ packers: GP_LAYOUT_SINGLE_AZ; az-aware:
+ * GP_LAYOUT_AZ_AWARE), and with more than 64 candidate zones in an instance group. */
 typedef struct {
     int32_t n_instance_groups;
     const int32_t* group_off;        /* [n_instance_groups + 1] snapshot groups of each instance group */

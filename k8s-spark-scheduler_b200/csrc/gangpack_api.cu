@@ -344,7 +344,8 @@ gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, i
                                 bool copy_nodes) {
     const int32_t n_slots = n_exec + n_drv;
     c->host_layout = false;              // gp_set_snapshot sets it again once the layout it validated is in place
-    c->zone_kind = -1;                   // gp_prepare_cluster_zones sets it again once its layout is in place
+    c->zone_kind = -1;                   // gp_prepare_cluster_zones* set it again once their layout is in place
+    c->zone_igs = 0;
     GP_CUDA(c, c->pair.reserve(sizeof(longlong2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->pair32.reserve(sizeof(uint2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->sgpu.reserve(sizeof(int64_t) * (size_t)(n_slots + 1)));

@@ -1,5 +1,5 @@
 // gangpack_cluster.cu -- the entry points driven by the reservations: node priority orders (gp_potential_nodes),
-// availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster, gp_prepare_cluster_zones), executor
+// availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster, gp_prepare_cluster_zones[_groups]), executor
 // reschedule (gp_reschedule_executors, gp_reschedule_from_reservations) and the failover reconciler (gp_reconcile_find_nodes),
 // with the input checks and device staging they share.
 #include "gangpack_ctx.cuh"
@@ -127,45 +127,66 @@ static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStr
     return GP_OK;
 }
 
-struct SortStage { const int32_t* drv; const int32_t* exe; const int32_t* counts; const int32_t* zone; };
+// The sort's results on the device.  ig: the instance group of each node (NULL: one); n_zones: the stride of the (instance
+// group, zone) pairs (1 when zone is NULL); ig_ties: per instance group undefined ties (NULL without ig).
+struct SortStage { const int32_t* drv; const int32_t* exe; const int32_t* counts; const int32_t* zone; const int32_t* ig; int32_t n_zones;
+                   const int32_t* ig_ties; };
+
+static void launch_label_keys(int nb, const int32_t* cnt, const int32_t* list, const int32_t* rank, const int32_t*, LabelKey* lk,
+                              cudaStream_t st) {
+    gp_label_keys<<<nb, 256, 0, st>>>(cnt, list, rank, lk);
+}
+static void launch_label_keys(int nb, const int32_t* cnt, const int32_t* list, const int32_t* rank, const int32_t* seg, SegLabelKey* lk,
+                              cudaStream_t st) {
+    gp_seg_label_keys<<<nb, 256, 0, st>>>(cnt, list, rank, seg, lk);
+}
 
 // Stable re-sort of list[0..*cnt) by rank[node] (-1 last): out[k] = the k-th node in (rank, position) order.  The label
-// re-sort of PotentialNodes, and the zone partition of gp_prepare_cluster_zones.
-static void launch_label_resort(int32_t n, const int32_t* cnt, const int32_t* list, const int32_t* rank, LabelKey* lk, LabelKey* lks,
-                                int32_t* pos, int32_t* out, cudaStream_t st) {
+// re-sort of PotentialNodes, and the zone partition of gp_prepare_cluster_zones.  K = SegLabelKey: by (seg[node], rank,
+// position), the label re-sort of an instance-group-major list.
+template <class K>
+static void launch_label_resort(int32_t n, const int32_t* cnt, const int32_t* list, const int32_t* rank, K* lk, K* lks, int32_t* pos,
+                                int32_t* out, cudaStream_t st, const int32_t* seg = nullptr) {
     const int T = 256;
     const int nb = (n + T - 1) / T;
     const int ntile = (n + kSortTile - 1) / kSortTile;
-    gp_label_keys<<<nb, T, 0, st>>>(cnt, list, rank, lk);
-    gp_sort_tiles<LabelKey><<<ntile, kSortThreads, kSortTile * sizeof(LabelKey), st>>>(n, cnt, lk, lks);
-    gp_rank_by_search<LabelKey><<<nb, T, 0, st>>>(n, cnt, lk, lks, pos);
+    launch_label_keys(nb, cnt, list, rank, seg, lk, st);
+    gp_sort_tiles<K><<<ntile, kSortThreads, kSortTile * sizeof(K), st>>>(n, cnt, lk, lks);
+    gp_rank_by_search<K><<<nb, T, 0, st>>>(n, cnt, lk, lks, pos);
     gp_label_scatter<<<nb, T, 0, st>>>(cnt, list, pos, out);
 }
 
 // f1 stage: d_cpu / d_mem / d_gpu are device arrays (NULL: uploaded from `in`; gpu optional); leaves the two orders,
 // counts[3] = {#driver candidates, #executor candidates, #undefined ties} and the zone ids (NULL: one zone) on the device.
-// The caller has run check_sort_ids.
-static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long* d_cpu, const long long* d_mem, const long long* d_gpu,
-                            cudaStream_t st, SortStage* out) {
+// ig (host, [n_nodes] in [-1, n_ig), or NULL): PotentialNodes per instance group, instance-group-major (the instance group
+// is the leading key; nodes in none are dropped).  The caller has run check_sort_ids and checked ig.
+static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const int32_t* ig, int32_t n_ig, const long long* d_cpu, const long long* d_mem,
+                            const long long* d_gpu, cudaStream_t st, SortStage* out) {
     const int32_t n = in->n_nodes;
-    // one scratch block
-    const size_t N = (size_t)n, Z = (size_t)in->n_zones;
+    const bool zoned = in->zone_id != nullptr && in->n_zones > 1;       // one zone: priority 0 for every node, nothing to total
+    // one scratch block; the zone totals and priorities are per (instance group, zone) pair
+    const int32_t nzk = zoned ? in->n_zones : 1;
+    const size_t N = (size_t)n, P = (size_t)n_ig * (size_t)nzk, NI = ig ? N : 0;
+    const bool seg_labels = ig && (in->driver_label_rank || in->executor_label_rank);
     Arena ar{c->sortbuf, st};
     const auto cpu = ar.take<long long>(N), mem = ar.take<long long>(N), gpu = ar.take<long long>(N);
     const auto keys = ar.take<SortKey>(N), sorted = ar.take<SortKey>(N);
-    const auto tot = ar.take<unsigned long long>(kZoneTotWords * Z);
-    const auto zone = ar.take<int32_t>(N), nr = ar.take<int32_t>(N), prio = ar.take<int32_t>(Z), pos = ar.take<int32_t>(N),
+    const auto tot = ar.take<unsigned long long>(kZoneTotWords * P);
+    const auto zone = ar.take<int32_t>(N), nr = ar.take<int32_t>(N), prio = ar.take<int32_t>(P), pos = ar.take<int32_t>(N),
                order = ar.take<int32_t>(N), drv = ar.take<int32_t>(N), exe = ar.take<int32_t>(N), drv2 = ar.take<int32_t>(N),
                exe2 = ar.take<int32_t>(N), lrd = ar.take<int32_t>(N), lre = ar.take<int32_t>(N);
-    const auto lk = ar.take<LabelKey>(N), lks = ar.take<LabelKey>(N);
+    const auto lk = ar.take<LabelKey>(seg_labels ? 0 : N), lks = ar.take<LabelKey>(seg_labels ? 0 : N);
+    const auto slk = ar.take<SegLabelKey>(seg_labels ? N : 0), slks = ar.take<SegLabelKey>(seg_labels ? N : 0);
     const auto cnt = ar.take<int32_t>(4);
     const auto fc = ar.take<uint8_t>(N), fu = ar.take<uint8_t>(N), fr = ar.take<uint8_t>(N);
+    const auto igp = ar.take<int32_t>(NI), ties = ar.take<int32_t>(ig ? (size_t)n_ig : 0);
     ar.reserve();
     if (!d_cpu) d_cpu = ar.put(cpu, in->avail_cpu_milli);
     if (!d_mem) d_mem = ar.put(mem, in->avail_mem_bytes);
     if (!d_gpu) d_gpu = ar.put(gpu, in->avail_gpu);
-    const bool zoned = in->zone_id != nullptr && in->n_zones > 1;       // one zone: priority 0 for every node, nothing to total
     const int32_t* d_zone = zoned ? ar.put(zone, in->zone_id) : nullptr;
+    const int32_t* d_ig = ar.put(igp, ig);
+    int32_t* d_ties = ig ? ar.zero(ties) : nullptr;
     const int32_t* d_nr = ar.put(nr, in->name_rank);
     const uint8_t* d_fc = ar.put(fc, in->is_driver_candidate);
     const uint8_t* d_fu = ar.put(fu, in->unschedulable);
@@ -182,20 +203,27 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
     const int nb = (n + T - 1) / T;
     const int ntile = (n + kSortTile - 1) / kSortTile;
     if (zoned) {
-        gp_zone_totals<<<nb, T, 0, st>>>(n, d_cpu, d_mem, d_zone, ar.ptr(tot));
-        gp_zone_priority<<<(in->n_zones + T - 1) / T, T, 0, st>>>(in->n_zones, ar.ptr(tot), ar.ptr(prio));
+        gp_zone_totals<<<nb, T, 0, st>>>(n, d_cpu, d_mem, d_zone, d_ig, nzk, ar.ptr(tot));
+        gp_zone_priority<<<(unsigned)((P + T - 1) / T), T, 0, st>>>((int32_t)P, nzk, ar.ptr(tot), ar.ptr(prio));
     }
-    gp_make_keys<<<nb, T, 0, st>>>(n, d_cpu, d_mem, d_zone, ar.ptr(prio), d_nr, ar.ptr(keys));
+    gp_make_keys<<<nb, T, 0, st>>>(n, d_cpu, d_mem, d_zone, ar.ptr(prio), d_ig, n_ig, nzk, d_nr, ar.ptr(keys));
     gp_sort_tiles<SortKey><<<ntile, kSortThreads, kSortTile * sizeof(SortKey), st>>>(n, nullptr, ar.ptr(keys), ar.ptr(sorted));
     gp_rank_by_search<SortKey><<<nb, T, 0, st>>>(n, nullptr, ar.ptr(keys), ar.ptr(sorted), ar.ptr(pos));
     gp_scatter_order<<<nb, T, 0, st>>>(n, ar.ptr(pos), ar.ptr(order));
-    gp_split_candidates<<<1, 1024, 0, st>>>(n, ar.ptr(order), d_fc, d_fu, d_fr, ar.ptr(keys), d_gpu, ar.ptr(drv), ar.ptr(exe), ar.ptr(cnt));
+    if (d_ig) gp_split_candidates<true><<<1, 1024, 0, st>>>(n, ar.ptr(order), d_fc, d_fu, d_fr, ar.ptr(keys), d_gpu, d_ig, d_ties, ar.ptr(drv),
+                                                            ar.ptr(exe), ar.ptr(cnt));
+    else gp_split_candidates<false><<<1, 1024, 0, st>>>(n, ar.ptr(order), d_fc, d_fu, d_fr, ar.ptr(keys), d_gpu, nullptr, nullptr, ar.ptr(drv),
+                                                        ar.ptr(exe), ar.ptr(cnt));
     out->drv = ar.ptr(drv);
     out->exe = ar.ptr(exe);
     out->counts = ar.ptr(cnt);
     out->zone = d_zone;
+    out->ig = d_ig;
+    out->n_zones = nzk;
+    out->ig_ties = d_ties;
     auto label_sort = [&](const int32_t* count, const int32_t* list, const int32_t* rank, Piece<int32_t> to) {
-        launch_label_resort(n, count, list, rank, ar.ptr(lk), ar.ptr(lks), ar.ptr(pos), ar.ptr(to), st);
+        if (seg_labels) launch_label_resort(n, count, list, rank, ar.ptr(slk), ar.ptr(slks), ar.ptr(pos), ar.ptr(to), st, d_ig);
+        else launch_label_resort(n, count, list, rank, ar.ptr(lk), ar.ptr(lks), ar.ptr(pos), ar.ptr(to), st);
         return (const int32_t*)ar.ptr(to);
     };
     if (d_lrd) out->drv = label_sort(out->counts, out->drv, d_lrd, drv2);
@@ -207,8 +235,9 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const long long*
 // gp_prepare_cluster and gp_prepare_cluster_zones up to their layout step: the checks both make, then reservations ->
 // availability (d_avail / d_sched: [3][n_nodes]) -> priority orders on the context's stream.  Synchronises once for the
 // availability stage's status word: a refusal returns before anything of the context's snapshot has been replaced.
-static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const char* who,
-                                long long** d_avail, long long** d_sched, SortStage* so) {
+// ig / n_ig: the instance groups of stage_sort, already checked.
+static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+                                const char* who, long long** d_avail, long long** d_sched, SortStage* so) {
     GP_TRY(check_usage(c, usage, who));
     if (!sort || usage->n_nodes != sort->n_nodes || sort->n_zones < 1)
         return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
@@ -218,7 +247,7 @@ static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp
     int* d_err = nullptr;
     GP_TRY(stage_availability(c, usage, c->stream, d_avail, d_sched, &d_err));
     const size_t N = (size_t)usage->n_nodes;
-    GP_TRY(stage_sort(c, sort, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so));
+    GP_TRY(stage_sort(c, sort, ig, n_ig, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so));
     int err = 0;
     GP_CUDA(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, c->stream));
     GP_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -272,6 +301,107 @@ static gp_status availability_out(gp_ctx* c, const gp_usage_input* in, bool firs
     return GP_OK;
 }
 
+// What prepare_zones leaves for its entry: the sort's counts[3], the ZoneInfo words and the device zone_of_group.
+struct ZonePrep {
+    int32_t counts[3];
+    int32_t info[kZiWords];
+    const int32_t* zone_of_group;
+};
+
+// gp_prepare_cluster_zones (ig NULL, n_ig 1) and gp_prepare_cluster_zones_groups up to their optional outputs: the checks,
+// reservations -> availability -> instance-group-major priority orders (prepare_orders, which synchronises once and refuses
+// before anything of the context is replaced) -> the zone-grouped layout (gangpack_zonelayout.cuh) -> the slot layout, then
+// one synchronise that reads back the counts.  zog_now (or NULL): zone_of_group [sort->n_zones + 1] read back in that
+// synchronise; ig_ties (or NULL): the undefined ties [n_ig] likewise.  keep_ig (gp_prepare_cluster_zones_groups): the
+// per-instance-group words (group_off, n_zones, undivided exec_off / drv_off) are kept on the host (zone_ig_words) and
+// zone_igs = n_ig.  ig NULL with n_ig > 1: every node in instance group 0, the others empty.
+static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+                               int32_t kind, bool keep_ig, const char* who, int32_t* zog_now, int32_t* ig_ties, ZonePrep* zp) {
+    if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
+        return fail(c, GP_ERR_INVALID, who, "layout->kind must be GP_LAYOUT_SINGLE_AZ or GP_LAYOUT_AZ_AWARE");
+    if (sort && sort->n_zones == 0x7fffffff) return fail(c, GP_ERR_INVALID, who, "n_zones too large");
+    long long *d_avail = nullptr, *d_sched = nullptr;
+    SortStage so{};
+    GP_TRY(prepare_orders(c, usage, sort, ig, n_ig, who, &d_avail, &d_sched, &so));
+    cudaStream_t st = c->stream;
+    c->zone_kind = -1;                                  // the held orders are overwritten below
+    c->zone_igs = 0;
+    const int32_t n = usage->n_nodes;
+    const size_t N = (size_t)n, G1 = (size_t)n_ig + 1;
+    // the (instance group, zone) pairs; g_bound groups bound every layout (each instance group: its candidate zones plus
+    // one; a candidate zone holds a node).  The slots are laid out for that many (the groups past the last one are empty)
+    // so that the group count can stay on the device until the one synchronise below.
+    const size_t P = (size_t)n_ig * (size_t)so.n_zones;
+    const int32_t g_bound = (int32_t)std::min<int64_t>((int64_t)P + n_ig, (int64_t)n + n_ig);
+    Arena ar{c->zoneprep, st};
+    const auto udrv_p = ar.take<int32_t>(N), uexe_p = ar.take<int32_t>(N), first = ar.take<int32_t>(P);
+    const auto has = ar.take<uint8_t>(P);
+    const auto zg = ar.take<int32_t>(P), zog = ar.take<int32_t>(std::max<size_t>((size_t)g_bound, (size_t)sort->n_zones + 1)),
+               rank_p = ar.take<int32_t>(N);
+    const auto lk = ar.take<LabelKey>(N), lks = ar.take<LabelKey>(N);
+    const auto pos = ar.take<int32_t>(N), info_p = ar.take<int32_t>(kZiWords), igw = ar.take<int32_t>(6 * G1);
+    ar.reserve();
+    GP_TRY(ar.check(c));
+    int32_t* udrv = ar.ptr(udrv_p);
+    int32_t* uexe = ar.ptr(uexe_p);
+    int32_t* info = ar.ptr(info_p);
+    int32_t* rank = ar.ptr(rank_p);
+    int32_t* wb = ar.ptr(igw);
+    // group_off, n_zones, exec_off, drv_off adjacent: the host copy is one read
+    const IgWords w{wb + G1, wb + 4 * G1, wb, wb + 5 * G1, wb + 2 * G1, wb + 3 * G1};
+    // the undivided orders outlive the sort's scratch, which the next gp_potential_nodes / gp_prepare_cluster reuses
+    GP_CUDA(c, cudaMemcpyAsync(udrv, so.drv, 4 * N, cudaMemcpyDeviceToDevice, st));
+    GP_CUDA(c, cudaMemcpyAsync(uexe, so.exe, 4 * N, cudaMemcpyDeviceToDevice, st));
+    ar.fill(first, 0x7f);
+    ar.zero(has);
+    ar.fill(zg, zog, 0xff);
+    ar.fill(info_p, igw, 0);
+    GP_TRY(ar.check(c));
+    const int T = 256;
+    const int nb = (n + T - 1) / T;
+    const int32_t az = kind == GP_LAYOUT_AZ_AWARE ? 1 : 0;
+    gp_zone_mark<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, so.ig, so.n_zones, ar.ptr(first), ar.ptr(has));
+    gp_zone_candidates<<<1, 1024, 0, st>>>(so.counts, udrv, so.zone, so.ig, so.n_zones, n_ig, az, ar.ptr(first), ar.ptr(has), ar.ptr(zg),
+                                           ar.ptr(zog), w, info);
+    gp_group_rank<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, so.ig, so.n_zones, ar.ptr(zg), az, w, rank);
+    GP_CUDA(c, cudaGetLastError());
+    // the grouped orders and their offsets
+    GP_CUDA(c, c->exec_order.reserve(4 * (N + 1))); GP_CUDA(c, c->drv_order.reserve(4 * (N + 1)));
+    GP_CUDA(c, c->exec_off.reserve(4 * ((size_t)g_bound + 1))); GP_CUDA(c, c->drv_off.reserve(4 * ((size_t)g_bound + 1)));
+    launch_label_resort(n, so.counts, udrv, rank, ar.ptr(lk), ar.ptr(lks), ar.ptr(pos), c->drv_order.as<int32_t>(), st);
+    launch_label_resort(n, so.counts + 1, uexe, rank, ar.ptr(lk), ar.ptr(lks), ar.ptr(pos), c->exec_order.as<int32_t>(), st);
+    gp_group_offsets<<<(unsigned)((g_bound + T) / T), T, 0, st>>>(g_bound, so.counts, c->drv_order.as<int32_t>(), c->exec_order.as<int32_t>(),
+                                                                  rank, az, c->exec_off.as<int32_t>(), c->drv_off.as<int32_t>(), info, n_ig,
+                                                                  so.ig, udrv, uexe, w);
+    GP_CUDA(c, cudaGetLastError());
+    gp_nodes dn{};
+    dn.n_nodes = n;
+    dn.n_groups = g_bound;
+    dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = c->exec_order.as<int32_t>();
+    dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = c->drv_order.as<int32_t>();
+    GP_TRY(prepare_snapshot(c, &dn, d_avail, d_sched, so, zp->counts));
+    ar.get(zp->info, info_p);
+    ar.get(zog_now, zog.part(0, (size_t)sort->n_zones + 1));
+    if (keep_ig) {
+        c->zone_ig_words.resize(4 * G1);
+        ar.get(c->zone_ig_words.data(), wb, 4 * G1);
+    }
+    if (so.ig_ties) ar.get(ig_ties, so.ig_ties, (size_t)n_ig);
+    GP_TRY(ar.sync(c));
+    if (!so.ig_ties && ig_ties) {                       // one instance group holds every node: its ties are the total
+        std::fill(ig_ties, ig_ties + n_ig, 0);
+        ig_ties[0] = zp->counts[2];
+    }
+    c->n_groups = zp->info[kZiGroups]; c->n_exec = zp->info[kZiExec]; c->n_drv = zp->info[kZiDrv];
+    c->have_sched = true;
+    c->have_eff_sched = true;
+    c->zone_orders = gp_az_orders{zp->info[kZiZones], zp->counts[1], uexe, zp->counts[0], udrv};
+    c->zone_kind = kind;
+    if (keep_ig) c->zone_igs = n_ig;
+    zp->zone_of_group = ar.ptr(zog);
+    return GP_OK;
+}
+
 extern "C" {
 
 gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver_order, int32_t* n_driver,
@@ -289,7 +419,7 @@ gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     SortStage so{};
-    s = stage_sort(c, in, nullptr, nullptr, nullptr, st, &so);
+    s = stage_sort(c, in, nullptr, 1, nullptr, nullptr, nullptr, st, &so);
     if (s != GP_OK) return s;
     int32_t counts[3] = {0, 0, 0};
     GP_CUDA(c, cudaMemcpyAsync(counts, so.counts, 12, cudaMemcpyDeviceToHost, st));
@@ -326,7 +456,7 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
     if (n_executor) *n_executor = 0;
     long long *d_avail = nullptr, *d_sched = nullptr;
     SortStage so{};
-    gp_status s = prepare_orders(c, usage, sort, "gp_prepare_cluster", &d_avail, &d_sched, &so);
+    gp_status s = prepare_orders(c, usage, sort, nullptr, 1, "gp_prepare_cluster", &d_avail, &d_sched, &so);
     if (s != GP_OK) return s;
     cudaStream_t st = c->stream;
     GP_CUDA(c, c->exec_off.reserve(8)); GP_CUDA(c, c->drv_off.reserve(8));
@@ -350,87 +480,67 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
 
 // reservations -> availability -> priority orders -> zone-grouped slot layout, without leaving the device
 gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout) {
+    const char* who = "gp_prepare_cluster_zones";
     if (!c) return GP_ERR_INVALID;
     c->layout_tail = nullptr;
-    if (!layout) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: missing arrays or mismatched sizes");
-    const int32_t kind = layout->kind;
-    if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
-        return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: layout->kind must be GP_LAYOUT_SINGLE_AZ or GP_LAYOUT_AZ_AWARE");
-    if (sort && sort->n_zones == 0x7fffffff) return fail(c, GP_ERR_INVALID, "gp_prepare_cluster_zones: n_zones too large");
+    if (!layout) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     layout->n_zones = 0; layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
-    long long *d_avail = nullptr, *d_sched = nullptr;
-    SortStage so{};
-    gp_status s = prepare_orders(c, usage, sort, "gp_prepare_cluster_zones", &d_avail, &d_sched, &so);
-    if (s != GP_OK) return s;
-    cudaStream_t st = c->stream;
-    c->zone_kind = -1;                                  // the held orders are overwritten below
-    const int32_t n = usage->n_nodes;
-    const size_t N = (size_t)n;
-    // g_bound = sort->n_zones + 1 groups bound every layout; the slots are laid out for that many (the groups past the
-    // last one are empty) so that the group count can stay on the device until the one synchronise below
-    const size_t Zs = (size_t)sort->n_zones;
-    const int32_t g_bound = sort->n_zones + 1;
-    Arena ar{c->zoneprep, st};
-    const auto udrv_p = ar.take<int32_t>(N), uexe_p = ar.take<int32_t>(N), first = ar.take<int32_t>(Zs);
-    const auto has = ar.take<uint8_t>(Zs);
-    const auto zg = ar.take<int32_t>(Zs), zog = ar.take<int32_t>(Zs + 1), rank_p = ar.take<int32_t>(N);
-    const auto lk = ar.take<LabelKey>(N), lks = ar.take<LabelKey>(N);
-    const auto pos = ar.take<int32_t>(N), info_p = ar.take<int32_t>(kZiWords);
-    ar.reserve();
-    GP_TRY(ar.check(c));
-    int32_t* udrv = ar.ptr(udrv_p);
-    int32_t* uexe = ar.ptr(uexe_p);
-    int32_t* info = ar.ptr(info_p);
-    int32_t* rank = ar.ptr(rank_p);
-    // the undivided orders outlive the sort's scratch, which the next gp_potential_nodes / gp_prepare_cluster reuses
-    GP_CUDA(c, cudaMemcpyAsync(udrv, so.drv, 4 * N, cudaMemcpyDeviceToDevice, st));
-    GP_CUDA(c, cudaMemcpyAsync(uexe, so.exe, 4 * N, cudaMemcpyDeviceToDevice, st));
-    ar.fill(first, 0x7f);
-    ar.zero(has);
-    ar.fill(zg, 0xff);
-    ar.fill(zog, 0xff);
-    ar.zero(info_p);
-    GP_TRY(ar.check(c));
-    const int T = 256;
-    const int nb = (n + T - 1) / T;
-    const int32_t az = kind == GP_LAYOUT_AZ_AWARE ? 1 : 0;
-    gp_zone_mark<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, ar.ptr(first), ar.ptr(has));
-    gp_zone_candidates<<<1, 1024, 0, st>>>(so.counts, udrv, so.zone, ar.ptr(first), ar.ptr(has), ar.ptr(zg), ar.ptr(zog), info);
-    gp_group_rank<<<nb, T, 0, st>>>(n, so.counts, udrv, uexe, so.zone, ar.ptr(zg), az, info, rank);
-    GP_CUDA(c, cudaGetLastError());
-    // the grouped orders and their offsets
-    GP_CUDA(c, c->exec_order.reserve(4 * (N + 1))); GP_CUDA(c, c->drv_order.reserve(4 * (N + 1)));
-    GP_CUDA(c, c->exec_off.reserve(4 * ((size_t)g_bound + 1))); GP_CUDA(c, c->drv_off.reserve(4 * ((size_t)g_bound + 1)));
-    launch_label_resort(n, so.counts, udrv, rank, ar.ptr(lk), ar.ptr(lks), ar.ptr(pos), c->drv_order.as<int32_t>(), st);
-    launch_label_resort(n, so.counts + 1, uexe, rank, ar.ptr(lk), ar.ptr(lks), ar.ptr(pos), c->exec_order.as<int32_t>(), st);
-    gp_group_offsets<<<(unsigned)((g_bound + T) / T), T, 0, st>>>(g_bound, so.counts, c->drv_order.as<int32_t>(), c->exec_order.as<int32_t>(),
-                                                                  rank, az, c->exec_off.as<int32_t>(), c->drv_off.as<int32_t>(), info);
-    GP_CUDA(c, cudaGetLastError());
-    gp_nodes dn{};
-    dn.n_nodes = n;
-    dn.n_groups = g_bound;
-    dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = c->exec_order.as<int32_t>();
-    dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = c->drv_order.as<int32_t>();
-    int32_t counts[3] = {0, 0, 0}, hinfo[kZiWords] = {};
-    GP_TRY(prepare_snapshot(c, &dn, d_avail, d_sched, so, counts));
-    ar.get(hinfo, info_p);
-    ar.get(layout->zone_of_group, zog);
-    GP_TRY(ar.sync(c));
-    c->n_groups = hinfo[kZiGroups]; c->n_exec = hinfo[kZiExec]; c->n_drv = hinfo[kZiDrv];
-    c->have_sched = true;
-    c->have_eff_sched = true;
-    c->zone_orders = gp_az_orders{hinfo[kZiZones], counts[1], uexe, counts[0], udrv};
-    c->zone_kind = kind;
-    if (sort->undefined_ties) *sort->undefined_ties = counts[2];
-    layout->n_zones = hinfo[kZiZones]; layout->n_groups = hinfo[kZiGroups];
-    layout->n_driver = counts[0]; layout->n_executor = counts[1];
+    ZonePrep zp{};
+    GP_TRY(prepare_zones(c, usage, sort, nullptr, 1, layout->kind, false, who, layout->zone_of_group, nullptr, &zp));
+    if (sort->undefined_ties) *sort->undefined_ties = zp.counts[2];
+    layout->n_zones = zp.info[kZiZones]; layout->n_groups = zp.info[kZiGroups];
+    layout->n_driver = zp.counts[0]; layout->n_executor = zp.counts[1];
     // the grouped layout itself only when asked: its sizes are known now
-    const size_t n_off = (size_t)hinfo[kZiGroups] + 1;
+    Arena ar{c->zoneprep, c->stream};
+    const size_t n_off = (size_t)zp.info[kZiGroups] + 1;
     ar.get(layout->exec_off, c->exec_off.as<int32_t>(), n_off);
     ar.get(layout->drv_off, c->drv_off.as<int32_t>(), n_off);
     ar.get(layout->exec_order, c->exec_order.as<int32_t>(), (size_t)c->n_exec);
     ar.get(layout->drv_order, c->drv_order.as<int32_t>(), (size_t)c->n_drv);
     if (layout->exec_off || layout->drv_off || layout->exec_order || layout->drv_order) GP_TRY(ar.sync(c));
+    return GP_OK;
+}
+
+// the same chain for every instance group at once: the layout of each one is gp_prepare_cluster_zones' on its nodes alone
+gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
+                                          int32_t n_instance_groups, gp_instance_group_layout* layout) {
+    const char* who = "gp_prepare_cluster_zones_groups";
+    if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
+    if (!layout) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
+    layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
+    const int32_t G = n_instance_groups;
+    if (G < 1) return fail(c, GP_ERR_INVALID, who, "n_instance_groups must be >= 1");
+    if (sort && G > 1 && (int64_t)G * ((int64_t)sort->n_zones + 1) > kZoneLayoutMaxPairs)
+        return fail(c, GP_ERR_INVALID, who, "n_instance_groups x (n_zones + 1) above 2^22");
+    if (instance_group && usage && sort && usage->n_nodes == sort->n_nodes)
+        for (int32_t i = 0; i < usage->n_nodes; ++i)
+            if (instance_group[i] < -1 || instance_group[i] >= G)
+                return fail(c, GP_ERR_INVALID, who, "instance_group outside [-1, n_instance_groups)");
+    ZonePrep zp{};
+    GP_TRY(prepare_zones(c, usage, sort, instance_group, G, layout->kind, true, who, nullptr, layout->undefined_ties, &zp));
+    if (sort->undefined_ties) *sort->undefined_ties = zp.counts[2];
+    const int32_t n_groups = zp.info[kZiGroups];
+    layout->n_groups = n_groups; layout->n_driver = zp.counts[0]; layout->n_executor = zp.counts[1];
+    // the per-instance-group words are on the host already; the rest only when asked
+    const size_t g1 = (size_t)G + 1;
+    const int32_t* words = c->zone_ig_words.data();
+    if (layout->group_off) std::copy(words, words + g1, layout->group_off);
+    if (layout->n_zones) std::copy(words + g1, words + g1 + G, layout->n_zones);
+    if (layout->exec_off) std::copy(words + 2 * g1, words + 3 * g1, layout->exec_off);
+    if (layout->drv_off) std::copy(words + 3 * g1, words + 4 * g1, layout->drv_off);
+    Arena ar{c->zoneprep, c->stream};
+    const size_t n_off = (size_t)n_groups + 1;
+    ar.get(layout->exec_order, c->zone_orders.exec_order, (size_t)zp.counts[1]);
+    ar.get(layout->drv_order, c->zone_orders.drv_order, (size_t)zp.counts[0]);
+    ar.get(layout->group_exec_off, c->exec_off.as<int32_t>(), n_off);
+    ar.get(layout->group_drv_off, c->drv_off.as<int32_t>(), n_off);
+    ar.get(layout->group_exec_order, c->exec_order.as<int32_t>(), (size_t)c->n_exec);
+    ar.get(layout->group_drv_order, c->drv_order.as<int32_t>(), (size_t)c->n_drv);
+    ar.get(layout->zone_of_group, zp.zone_of_group, (size_t)n_groups);
+    if (layout->exec_order || layout->drv_order || layout->group_exec_off || layout->group_drv_off || layout->group_exec_order ||
+        layout->group_drv_order || layout->zone_of_group)
+        GP_TRY(ar.sync(c));
     return GP_OK;
 }
 
@@ -575,7 +685,7 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     const int nb = (n + T - 1) / T;
     if (zoned) {
         gp_rp_zone_totals<<<nb, T, 0, st>>>(n, d_avail, d_avail + N, ni.zone, keep, ni.tz, ar.ptr(tot));
-        gp_zone_priority<<<(sort->n_zones + T - 1) / T, T, 0, st>>>(sort->n_zones, ar.ptr(tot), ar.ptr(prio));
+        gp_zone_priority<<<(sort->n_zones + T - 1) / T, T, 0, st>>>(sort->n_zones, sort->n_zones, ar.ptr(tot), ar.ptr(prio));
     }
     ni.avail = d_avail; ni.ff = d_ff;
     for (int d = 0; d < 3; ++d) ni.over[d] = d_over[d];

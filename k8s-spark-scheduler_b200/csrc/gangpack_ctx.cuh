@@ -215,6 +215,12 @@ struct gp_ctx {
     DevBuf callbuf;
     int zone_kind = -1;
     gp_az_orders zone_orders{};
+    // gp_prepare_cluster_zones_groups: zone_igs = its n_instance_groups while its layout is held (0 otherwise, also after
+    // gp_prepare_cluster_zones), and zone_ig_words its per-instance-group words read back by that call, [n + 1] each:
+    // group_off, n_zones (n used), undivided exec_off, undivided drv_off -- what gp_pack_fifo_zones_groups(groups == NULL)
+    // builds its descriptors from
+    int32_t zone_igs = 0;
+    std::vector<int32_t> zone_ig_words;
     bool sort_attr_set = false;
     bool recon_attr_set = false;                  // dynamic shared-memory opt-in of gp_sort_tiles<ReconKey> done on this device
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device

@@ -86,18 +86,28 @@ __device__ __forceinline__ void zone_total_add(unsigned long long* __restrict__ 
     exact_add(t + 0, t + 1, mem);
     exact_add(t + 2, t + 3, cpu);
 }
+// Instance groups (gp_prepare_cluster_zones_groups): ig[i] = the instance group of node i, -1 = none (NULL: every node in
+// instance group 0).  Zones are then totalled and ranked per (instance group, zone) pair, pair = ig * n_zones + zone: a zone
+// is ranked only against the zones of its own instance group, as PotentialNodes over that instance group's nodes ranks it.
 __global__ void gp_zone_totals(int32_t n, const long long* __restrict__ cpu, const long long* __restrict__ mem,
-                               const int32_t* __restrict__ zone, unsigned long long* __restrict__ tot /* [kZoneTotWords * Z] */) {
+                               const int32_t* __restrict__ zone, const int32_t* __restrict__ ig, int32_t n_zones,
+                               unsigned long long* __restrict__ tot /* [kZoneTotWords * pairs] */) {
     int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    zone_total_add(tot, zone[i], mem[i], cpu[i]);
+    const int32_t g = ig ? ig[i] : 0;
+    if (g < 0) return;
+    zone_total_add(tot, g * n_zones + zone[i], mem[i], cpu[i]);
 }
 
-// AZ priority = number of zones with smaller (mem, cpu, id)   (sort.Slice over zones, :102-104; ties by zone id)
-__global__ void gp_zone_priority(int32_t n_zones, const unsigned long long* __restrict__ tot, int32_t* __restrict__ prio) {
+// AZ priority = number of zones of the same instance group with smaller (mem, cpu, id)   (sort.Slice over zones, :102-104;
+// ties by zone id); one thread per (instance group, zone) pair
+__global__ void gp_zone_priority(int32_t n_pairs, int32_t n_zones, const unsigned long long* __restrict__ tot, int32_t* __restrict__ prio) {
     int32_t z = blockIdx.x * blockDim.x + threadIdx.x;
-    if (z >= n_zones) return;
+    if (z >= n_pairs) return;
     const unsigned long long* t = tot + (size_t)kZoneTotWords * z;
+    const int32_t base = z - z % n_zones;
+    z -= base;
+    tot += (size_t)kZoneTotWords * base;
     const ExactSum m = exact_sum(t[0], t[1]), c = exact_sum(t[2], t[3]);
     int32_t p = 0;
     for (int32_t o = 0; o < n_zones; ++o) {
@@ -107,17 +117,22 @@ __global__ void gp_zone_priority(int32_t n_zones, const unsigned long long* __re
         const bool less = by_mem ? by_mem < 0 : (by_cpu ? by_cpu < 0 : o < z);
         p += less ? 1 : 0;
     }
-    prio[z] = p;
+    prio[base + z] = p;
 }
 
-// zone == NULL: one zone (priority 0); name_rank == NULL: index order
+// zone == NULL: one zone (priority 0, n_zones 1); name_rank == NULL: index order.  With instance groups the instance group
+// is the leading key, folded into az = ig * n_zones + zone priority; nodes in no instance group sort last (az = n_ig *
+// n_zones) and gp_split_candidates drops them.
 __global__ void gp_make_keys(int32_t n, const long long* __restrict__ cpu, const long long* __restrict__ mem,
-                             const int32_t* __restrict__ zone, const int32_t* __restrict__ zone_prio,
-                             const int32_t* __restrict__ name_rank, SortKey* __restrict__ keys) {
+                             const int32_t* __restrict__ zone, const int32_t* __restrict__ zone_prio, const int32_t* __restrict__ ig,
+                             int32_t n_ig, int32_t n_zones, const int32_t* __restrict__ name_rank, SortKey* __restrict__ keys) {
     int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     SortKey k;
-    k.mem = mem[i]; k.cpu = cpu[i]; k.az = zone ? zone_prio[zone[i]] : 0; k.name_rank = name_rank ? name_rank[i] : i;
+    const int32_t g = ig ? ig[i] : 0;
+    k.mem = mem[i]; k.cpu = cpu[i];
+    k.az = g < 0 ? n_ig * n_zones : g * n_zones + (zone ? zone_prio[g * n_zones + zone[i]] : 0);
+    k.name_rank = name_rank ? name_rank[i] : i;
     keys[i] = k;
 }
 
@@ -130,8 +145,19 @@ struct LabelKey {          // stable re-sort by label rank: (rank, position in t
     int32_t pos;
 };
 __device__ __forceinline__ bool key_less(const LabelKey& a, const LabelKey& b) { return a.rank != b.rank ? a.rank < b.rank : a.pos < b.pos; }
+// the label re-sort of instance-group-major candidate lists: stable within each instance group (seg), 12 bytes (a tile is
+// exactly 48 KB, the default dynamic shared-memory limit)
+struct SegLabelKey {
+    uint32_t seg;
+    uint32_t rank;
+    int32_t pos;
+};
+__device__ __forceinline__ bool key_less(const SegLabelKey& a, const SegLabelKey& b) {
+    return a.seg != b.seg ? a.seg < b.seg : (a.rank != b.rank ? a.rank < b.rank : a.pos < b.pos);
+}
 __device__ __forceinline__ SortKey key_max(const SortKey*) { SortKey k; k.mem = 0x7fffffffffffffffLL; k.cpu = 0x7fffffffffffffffLL; k.az = 0x7fffffff; k.name_rank = 0x7fffffff; return k; }
 __device__ __forceinline__ LabelKey key_max(const LabelKey*) { LabelKey k; k.rank = 0xffffffffu; k.pos = 0x7fffffff; return k; }
+__device__ __forceinline__ SegLabelKey key_max(const SegLabelKey*) { SegLabelKey k; k.seg = 0xffffffffu; k.rank = 0xffffffffu; k.pos = 0x7fffffff; return k; }
 
 // (1) sorted[tile] = the tile's keys in ascending order.  count_ptr: the number of keys lives on the device (candidate
 // lists) or is `n` when NULL.  Dynamic shared memory: kSortTile * sizeof(K).
@@ -190,12 +216,16 @@ __global__ void gp_scatter_order(int32_t n, const int32_t* __restrict__ pos, int
 // Order-preserving compaction of the priority order into the driver and executor candidate lists (one CTA, every
 // thread owns 8 consecutive positions per step).  counts[0] = #driver candidates, counts[1] = #executor candidates,
 // counts[2] = #adjacent pairs of the order that the reference's comparator leaves undefined (same zone priority, memory
-// and cpu but different gpu: SURVEY App. B6) -- 0 when no gpu column was given.
+// and cpu but different gpu: SURVEY App. B6) -- 0 when no gpu column was given.  ig (NULL: one instance group): a node in
+// no instance group is neither candidate nor part of a tie; ig_ties[g] (pre-zeroed, or NULL) counts instance group g's ties
+// (the az key holds the instance group, so a tie never spans two).  IG: ig is given (the one-group call reads no ig).
 constexpr int kSplitItems = 8;
+template <bool IG>
 __global__ void __launch_bounds__(1024) gp_split_candidates(int32_t n, const int32_t* __restrict__ order,
                                                             const uint8_t* __restrict__ is_candidate,
                                                             const uint8_t* __restrict__ unschedulable, const uint8_t* __restrict__ ready,
                                                             const SortKey* __restrict__ keys, const long long* __restrict__ gpu,
+                                                            const int32_t* __restrict__ ig, int32_t* __restrict__ ig_ties,
                                                             int32_t* __restrict__ drv, int32_t* __restrict__ exe, int32_t* __restrict__ counts) {
     __shared__ int32_t wsum[2][32];
     __shared__ int32_t base[2];
@@ -214,12 +244,17 @@ __global__ void __launch_bounds__(1024) gp_split_candidates(int32_t n, const int
             node[t] = -1;
             if (p < n) {
                 node[t] = order[p];
-                if (is_candidate ? is_candidate[node[t]] != 0 : true) fd |= 1u << t;
-                if (!(unschedulable && unschedulable[node[t]]) && (ready ? ready[node[t]] != 0 : true)) fe |= 1u << t;
-                if (gpu && p > 0) {
+                const int32_t g = IG ? ig[node[t]] : 0;
+                const uint32_t in = g >= 0 ? 1u : 0u;
+                if (is_candidate ? is_candidate[node[t]] != 0 : true) fd |= in << t;
+                if (!(unschedulable && unschedulable[node[t]]) && (ready ? ready[node[t]] != 0 : true)) fe |= in << t;
+                if (in && gpu && p > 0) {
                     const int32_t prev = t > 0 ? node[t - 1] : order[p - 1];
                     const SortKey a = keys[prev], b = keys[node[t]];
-                    if (a.az == b.az && a.mem == b.mem && a.cpu == b.cpu && gpu[prev] != gpu[node[t]]) ++my_ties;
+                    if (a.az == b.az && a.mem == b.mem && a.cpu == b.cpu && gpu[prev] != gpu[node[t]]) {
+                        ++my_ties;
+                        if (IG) atomicAdd(ig_ties + g, 1);
+                    }
                 }
             }
         }
@@ -261,6 +296,15 @@ __global__ void gp_label_keys(const int32_t* __restrict__ count_ptr, const int32
     if (i >= *count_ptr) return;
     const int32_t lr = label_rank[list[i]];
     LabelKey k; k.rank = lr < 0 ? 0x7fffffffu : (uint32_t)lr; k.pos = i;
+    keys[i] = k;
+}
+// the same within each instance group: (ig, rank, position)
+__global__ void gp_seg_label_keys(const int32_t* __restrict__ count_ptr, const int32_t* __restrict__ list,
+                                  const int32_t* __restrict__ label_rank, const int32_t* __restrict__ ig, SegLabelKey* __restrict__ keys) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= *count_ptr) return;
+    const int32_t v = list[i], lr = label_rank[v];
+    SegLabelKey k; k.seg = (uint32_t)ig[v]; k.rank = lr < 0 ? 0x7fffffffu : (uint32_t)lr; k.pos = i;
     keys[i] = k;
 }
 __global__ void gp_label_scatter(const int32_t* __restrict__ count_ptr, const int32_t* __restrict__ list,

@@ -42,6 +42,15 @@ static bool has_zone_arrays(const gp_apps* a, const gp_zone_results* out) {
     return a->drv_cpu_milli && a->drv_mem_bytes && a->exe_cpu_milli && a->exe_mem_bytes && a->exe_count && out->zone && out->driver_node;
 }
 
+// The single-instance-group zone entries read the whole snapshot as one instance group's zones: refused while it holds the
+// layout of gp_prepare_cluster_zones_groups over several instance groups.
+static gp_status one_instance_group(gp_ctx* c, const char* who) {
+    if (c->zone_igs > 1)
+        return fail(c, GP_ERR_INVALID, who, "the snapshot holds several instance groups (gp_prepare_cluster_zones_groups): drain them "
+                                            "with gp_pack_fifo_zones_groups(groups == NULL)");
+    return GP_OK;
+}
+
 // Uploads the six int64 quantity columns (6 x n_apps of `in`; absent gpu columns stay NULL = 0 in the result), exe_count
 // and the ExecutorNodes offsets `off`
 static SixCols upload_app_columns(Arena& ar, const gp_apps* a, const int64_t* off, Piece<int64_t> in, Piece<int32_t> cnt,
@@ -214,6 +223,7 @@ gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: NULL apps/results");
     if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
         return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: the single-AZ packers are tightly-pack and minimal-fragmentation (single_az_pack_tightly.go, single_az_minimal_fragmentation.go)");
+    GP_TRY(one_instance_group(c, "gp_pack_batch_zones"));
     return batch_zones_run(c, a, algo, c->n_groups, nullptr, false, out, "gp_pack_batch_zones");
 }
 
@@ -285,6 +295,7 @@ static gp_status check_az_orders(gp_ctx* c, const gp_instance_groups& ig, const 
 // The az-aware entries' NULL arguments.  orders == NULL stands for the undivided orders and n_zones gp_prepare_cluster_zones
 // (GP_LAYOUT_AZ_AWARE) left on the device -- *o then points at them; after any other snapshot it is refused.
 static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_results* out, const gp_az_orders** o, const char* who) {
+    if (!*o) GP_TRY(one_instance_group(c, who));
     if (!*o && c->zone_kind == GP_LAYOUT_SINGLE_AZ)
         return fail(c, GP_ERR_INVALID, who, "orders == NULL needs a gp_prepare_cluster_zones(GP_LAYOUT_AZ_AWARE) snapshot; this one is "
                                            "GP_LAYOUT_SINGLE_AZ (no trailing group, no undivided orders)");
@@ -420,6 +431,7 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: the single-AZ packers are tightly-pack and minimal-fragmentation");
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones)");
+    GP_TRY(one_instance_group(c, "gp_pack_fifo_zones"));
     if (c->n_groups > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
     const OneInstanceGroup one(c->n_groups, nullptr);
     return fifo_zones_run(c, a, nullptr, (int)algo, mode, one.ig, false, out, "gp_pack_fifo_zones");
@@ -446,6 +458,28 @@ gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const
     return fifo_zones_run(c, a, nullptr, kZoneAzAware, mode, one.ig, held, out, "gp_pack_fifo_az_aware");
 }
 
+// gp_pack_fifo_zones_groups(groups == NULL): the layout gp_prepare_cluster_zones_groups left, from its host words and its
+// device orders (built by the library: no order check)
+static gp_status held_groups_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, gp_zone_results* out, const char* who) {
+    if (c->zone_igs < 1)
+        return fail(c, GP_ERR_INVALID, who, "groups == NULL needs the layout of gp_prepare_cluster_zones_groups; the snapshot was laid "
+                                            "out by another call since");
+    const bool azk = kind == kZoneAzAware;
+    if (azk != (c->zone_kind == GP_LAYOUT_AZ_AWARE))
+        return fail(c, GP_ERR_INVALID, who, azk ? "az-aware-tightly-pack needs a GP_LAYOUT_AZ_AWARE layout; the held one is GP_LAYOUT_SINGLE_AZ"
+                                                : "the single-AZ packers need a GP_LAYOUT_SINGLE_AZ layout; the held one is GP_LAYOUT_AZ_AWARE");
+    const int32_t G = c->zone_igs;
+    const int32_t* words = c->zone_ig_words.data();
+    const size_t g1 = (size_t)G + 1;
+    const int32_t *goff = words, *nz = words + g1;
+    for (int32_t b = 0; b < G; ++b)
+        if ((azk ? nz[b] : goff[b + 1] - goff[b]) > kZoneFifoMaxZones)
+            return fail(c, GP_ERR_INVALID, who, "more than 64 candidate zones in an instance group");
+    const gp_instance_groups held{G, goff, azk ? nz : nullptr, azk ? words + 2 * g1 : nullptr, azk ? c->zone_orders.exec_order : nullptr,
+                                  azk ? words + 3 * g1 : nullptr, azk ? c->zone_orders.drv_order : nullptr};
+    return fifo_zones_run(c, a, a->group, kind, mode, held, azk, out, who);
+}
+
 // the FIFO loop of every instance group with a zone-aware packer, one CTA per instance group, in one launch
 gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker packer, gp_mode mode, const gp_instance_groups* ig,
                                     gp_zone_results* out) {
@@ -462,6 +496,10 @@ gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker pa
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, who, "mode must be one of the FIFO modes");
     if (!c->have_sched) return fail(c, GP_ERR_INVALID, who, "gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!ig) {
+        if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/results");
+        return held_groups_run(c, a, kind, mode, out, who);
+    }
     if (!c->host_layout)
         return fail(c, GP_ERR_INVALID, who, "the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
                                             "gp_prepare_cluster* there is no host copy of the layout to check the instance groups against)");

@@ -37,7 +37,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
-           "gp_node_overhead", "gp_pack_fifo_zones_groups",
+           "gp_node_overhead", "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -152,6 +152,12 @@ class gp_zone_layout(C.Structure):
     _fields_ = [("kind", C.c_int32), ("n_zones", C.c_int32), ("n_groups", C.c_int32), ("n_driver", C.c_int32),
                 ("n_executor", C.c_int32), ("reserved", C.c_int32), ("zone_of_group", C.c_void_p), ("exec_off", C.c_void_p),
                 ("exec_order", C.c_void_p), ("drv_off", C.c_void_p), ("drv_order", C.c_void_p)]
+
+
+class gp_instance_group_layout(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("n_groups", C.c_int32), ("n_driver", C.c_int32), ("n_executor", C.c_int32)] + \
+        [(k, C.c_void_p) for k in ("group_off", "n_zones", "exec_off", "exec_order", "drv_off", "drv_order", "group_exec_off",
+                                   "group_exec_order", "group_drv_off", "group_drv_order", "zone_of_group", "undefined_ties")]
 
 
 class gp_reschedule(C.Structure):
@@ -325,6 +331,9 @@ def load():
                                      C.POINTER(C.c_int32)]
     L.gp_prepare_cluster_zones.restype = C.c_int
     L.gp_prepare_cluster_zones.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input), C.POINTER(gp_zone_layout)]
+    L.gp_prepare_cluster_zones_groups.restype = C.c_int
+    L.gp_prepare_cluster_zones_groups.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input), C.c_void_p, C.c_int32,
+                                                  C.POINTER(gp_instance_group_layout)]
     L.gp_potential_nodes.restype = C.c_int
     L.gp_potential_nodes.argtypes = [C.c_void_p, C.POINTER(gp_sort_input), C.c_void_p, C.POINTER(C.c_int32),
                                      C.c_void_p, C.POINTER(C.c_int32)]
@@ -678,6 +687,44 @@ class GangPacker:
             out.update(exec_order=bufs["exec_order"][:out["exec_off"][G]].copy(), drv_order=bufs["drv_order"][:out["drv_off"][G]].copy())
         return out
 
+    def prepare_cluster_zones_groups(self, alloc, overhead, res_node, res, instance_group, n_instance_groups, zone_id=None, n_zones=1,
+                                     name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None, driver_label_rank=None,
+                                     executor_label_rank=None, kind=LAYOUT_AZ_AWARE, layout=True):
+        """prepare_cluster_zones for every instance group at once: instance_group[v] = node v's instance group (0 ..
+        n_instance_groups-1, -1 = none; None = every node in 0).  Each instance group's orders are PotentialNodes over its own
+        nodes, grouped by zone; its groups follow those of the instance groups before it.  -> dict with n_groups, n_driver,
+        n_executor, undefined_ties (the total), group_off, n_zones, exec_off, drv_off, ig_undefined_ties (per instance group)
+        and, with `layout`, the undivided exec_order / drv_order, the grouped group_exec_off / group_exec_order /
+        group_drv_off / group_drv_order and zone_of_group.  The context then holds the layout pack_fifo_zones_groups drains
+        when its layout arguments are all None.  A refused call leaves the context as it was."""
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
+        G = int(n_instance_groups)
+        ig = _np(instance_group, np.int32)
+        ties = C.c_int32(0)
+        si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
+                         executor_label_rank, ties=ties)
+        g1 = max(G, 0) + 1
+        bufs = {k: np.full(g1, -9, np.int32) for k in ("group_off", "n_zones", "exec_off", "drv_off", "undefined_ties")}
+        if layout:
+            n_groups_max = g1 + min(n, max(G, 0) * n_zones)
+            bufs.update({k: np.full(max(n, 1), -9, np.int32) for k in ("exec_order", "drv_order", "group_exec_order", "group_drv_order")})
+            bufs.update({k: np.full(n_groups_max + 1, -9, np.int32) for k in ("group_exec_off", "group_drv_off", "zone_of_group")})
+        lo = gp_instance_group_layout(kind=int(kind), **{k: _p(v) for k, v in bufs.items()})
+        self._check(load().gp_prepare_cluster_zones_groups(self._h, C.byref(ui), C.byref(si), _p(ig), G, C.byref(lo)))
+        self.n_nodes = n
+        out = dict(n_groups=lo.n_groups, n_driver=lo.n_driver, n_executor=lo.n_executor, undefined_ties=ties.value,
+                   group_off=bufs["group_off"].copy(), n_zones=bufs["n_zones"][:G].copy(), exec_off=bufs["exec_off"].copy(),
+                   drv_off=bufs["drv_off"].copy(), ig_undefined_ties=bufs["undefined_ties"][:G].copy())
+        if layout:
+            ng = lo.n_groups
+            out.update(exec_order=bufs["exec_order"][:lo.n_executor].copy(), drv_order=bufs["drv_order"][:lo.n_driver].copy(),
+                       group_exec_off=bufs["group_exec_off"][:ng + 1].copy(), group_drv_off=bufs["group_drv_off"][:ng + 1].copy(),
+                       zone_of_group=bufs["zone_of_group"][:ng].copy())
+            out.update(group_exec_order=bufs["group_exec_order"][:out["group_exec_off"][ng]].copy(),
+                       group_drv_order=bufs["group_drv_order"][:out["group_drv_off"][ng]].copy())
+        return out
+
     # ---- node priority order (NodeSorter.PotentialNodes) ---------------------------------------
     def potential_nodes(self, avail_cpu, avail_mem, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None, avail_gpu=None):
@@ -788,17 +835,19 @@ class GangPacker:
         o, _keep = _az_orders(exec_order, drv_order, n_zones)
         return self._pack_zones(apps, None, load().gp_pack_batch_az_aware, o)
 
-    def pack_fifo_zones_groups(self, apps: dict, packer: int, mode: int, group_off, n_zones=None, exec_off=None, exec_order=None,
+    def pack_fifo_zones_groups(self, apps: dict, packer: int, mode: int, group_off=None, n_zones=None, exec_off=None, exec_order=None,
                                drv_off=None, drv_order=None):
         """fitEarlierDrivers of every instance group in one launch, one CTA per instance group, with packer
         BP_SINGLE_AZ_TIGHTLY_PACK / BP_SINGLE_AZ_MINIMAL_FRAGMENTATION (instance group i's snapshot groups group_off[i] ..
         group_off[i+1]-1 are its zones) or BP_AZ_AWARE_TIGHTLY_PACK (the first n_zones[i] of them its zones, the rest its
         trailing group; exec_order / drv_order its undivided orders in CSR by exec_off / drv_off).  apps["group"] is each
         application's instance group (absent: 0), "young" as in pack_fifo_zones.  -> like pack_fifo_zones, with zone local to
-        the application's instance group."""
-        ig, _keep = _instance_groups(group_off, n_zones, exec_off, exec_order, drv_off, drv_order)
-        return self._pack_zones(apps, apps.get("young"), load().gp_pack_fifo_zones_groups, packer, mode, C.byref(ig),
-                                group=apps.get("group"))
+        the application's instance group.  All six layout arguments None (groups == NULL): the layout
+        prepare_cluster_zones_groups left on the device."""
+        cols = (group_off, n_zones, exec_off, exec_order, drv_off, drv_order)
+        ig, _keep = _instance_groups(*cols) if any(x is not None for x in cols) else (None, None)
+        return self._pack_zones(apps, apps.get("young"), load().gp_pack_fifo_zones_groups, packer, mode,
+                                C.byref(ig) if ig is not None else None, group=apps.get("group"))
 
     def reserve_placements(self, apps: dict, placed, subtract=True):
         """newResourceReservation for a packed batch -> dict of row arrays (app, slot, node, cpu, mem, gpu); with subtract the
