@@ -258,6 +258,41 @@ gp_status gp_potential_nodes(gp_ctx* ctx, const gp_sort_input* in,
 gp_status gp_prepare_cluster(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort,
                              int32_t* n_driver /* may be NULL */, int32_t* n_executor /* may be NULL */);
 
+/* gp_prepare_cluster for every instance group at once: the snapshot gp_pack_batch drains one FIFO queue per instance group
+ * from (tightly-pack, distribute-evenly; apps->group = the instance group), built on the device.
+ *   instance_group  [n_nodes] as in gp_prepare_cluster_zones_groups: in [0, n_instance_groups), -1 = in none, NULL = every node
+ *                   in instance group 0.  Instance groups are disjoint node sets.  A node in none is in no order, but its
+ *                   availability is computed and gp_get_snapshot returns it.
+ *   availability    computed once for every node, exactly as gp_prepare_cluster computes it, with the same domain and
+ *                   GP_ERR_UNREPRESENTABLE refusal.
+ *   snapshot group i = instance group i: its driver and executor orders are PotentialNodes over i's nodes alone -- zone
+ *                   priority from i's own (instance group, zone) exact totals, the candidate / schedulable / ready filters, the
+ *                   stable label re-sort within i, the undefined-tie rule.
+ * Identity: instance group i's orders, counts and undefined ties equal gp_prepare_cluster + gp_potential_nodes on a node table
+ * holding only i's nodes (with their reservations), node indices mapped back to this table; an instance group without nodes
+ * gets empty orders.  With instance_group == NULL or n_instance_groups == 1 (every node in 0) the context is exactly as after
+ * gp_prepare_cluster.  sort->undefined_ties (if given) is the total.
+ * SchedulableResources are kept as after gp_prepare_cluster.  The context is then ready for gp_pack_batch /
+ * gp_pack_batch_device in every mode, gp_reserve_placements, gp_apply_usage_delta and gp_packing_efficiency[_groups]; the
+ * snapshot survives FIFO calls, gp_reserve_placements and gp_apply_usage_delta.  A held zone layout is cleared, so the zone
+ * entries' orders == NULL / groups == NULL forms are refused afterwards.
+ * GP_ERR_INVALID (gp_last_error names the cause): what gp_prepare_cluster refuses; n_instance_groups < 1; an instance_group value
+ * outside [-1, n_instance_groups); n_instance_groups > 1 with n_instance_groups x (sort->n_zones + 1) above 2^22 (the
+ * per-(instance group, zone) zone totals).  A refused call replaces nothing (one synchronise after the availability stage, as
+ * gp_prepare_cluster).  One synchronise more for the counts and undefined_ties; the four order arrays cost one more copy. */
+typedef struct {
+    int32_t n_driver;            /* out: driver candidates over every instance group */
+    int32_t n_executor;          /* out: executor candidates over every instance group */
+    int32_t* exec_off;           /* out, or NULL: [n_instance_groups + 1] CSR of exec_order (= the snapshot's exec_off) */
+    int32_t* exec_order;         /* out, or NULL: [n_nodes] executor orders, instance group by instance group */
+    int32_t* drv_off;            /* out, or NULL: [n_instance_groups + 1] CSR of drv_order (= the snapshot's drv_off) */
+    int32_t* drv_order;          /* out, or NULL: [n_nodes] driver orders */
+    int32_t* undefined_ties;     /* out, or NULL: [n_instance_groups] undefined ties of each instance group's order */
+} gp_instance_group_orders;
+gp_status gp_prepare_cluster_groups(gp_ctx* ctx, const gp_usage_input* usage, const gp_sort_input* sort,
+                                    const int32_t* instance_group /* [n_nodes], or NULL = every node in group 0 */,
+                                    int32_t n_instance_groups, gp_instance_group_orders* out);
+
 /* The same chain for the zone-aware packers (SURVEY 8f rows f1/f2/f3): gp_prepare_cluster's availability and priority orders
  * (label re-sort and undefined_ties included), then both orders grouped by sort->zone_id on the device -- groupNodesByZone
  * (LIB/binpack/single_az.go:57-73).  Candidate zones have at least one driver and one executor candidate (:36-41); they are
@@ -610,6 +645,27 @@ gp_status gp_apply_usage_delta(gp_ctx* ctx, int64_t n_rows, const int32_t* node,
  * a request, or a per-node reserved or added-back amount, >= 2^61. */
 gp_status gp_packing_efficiency(gp_ctx* ctx, const gp_apps* apps, gp_algo algo, const gp_results* placed /* host */,
                                 gp_mode charged, double* avg_out /* [n_apps][4] */);
+
+/* gp_packing_efficiency averaged per instance group: the Predicate's metric as the reference computes it when a snapshot holds
+ * several instance groups.  selectDriverNode builds its metadata from the nodes of the driver's instance group
+ * (ListWithPredicate(driver affinity), EXT/resource.go:292-303), and ComputePackingEfficiencies runs over that metadata
+ * (LIB/binpack/binpack.go:72-77, efficiency.go:66-156).  Row i is exactly gp_packing_efficiency's computation with "every node
+ * of the table" replaced by {v : instance_group[v] == apps->group[i]} -- the per-node terms, the exact once-rounded sums, the
+ * max(n, 1) divisor with n that instance group's node count, the nodesWithGPU rule, four zeros for driver_node < 0.
+ *   instance_group  [n_nodes] in [0, n_instance_groups), -1 = in none (such a node counts in no row's average); instance
+ *                   groups are disjoint.  Any snapshot works: gp_set_snapshot with several groups, gp_prepare_cluster_groups,
+ *                   gp_prepare_cluster_zones_groups.
+ *   apps->group     each row's instance group (NULL = 0).
+ *   charged         as in gp_packing_efficiency, except that the FIFO modes allow at most ONE row per instance group (its
+ *                   add-back then touches only its own instance group's nodes, and every row stays exact).
+ * With n_instance_groups == 1 and every node in instance group 0 the result equals gp_packing_efficiency's, bit for bit.
+ * Refusals: gp_packing_efficiency's, plus GP_ERR_INVALID for instance_group NULL (with nodes), n_instance_groups < 1, a value
+ * outside [-1, n_instance_groups), a row's group outside [0, n_instance_groups), two rows of one instance group under a FIFO
+ * charged mode, and a placed row whose driver or executor node lies outside its instance group.  One stream synchronise. */
+gp_status gp_packing_efficiency_groups(gp_ctx* ctx, const gp_apps* apps /* group = instance group */, gp_algo algo,
+                                       const gp_results* placed /* host */, gp_mode charged,
+                                       const int32_t* instance_group /* [n_nodes] */, int32_t n_instance_groups,
+                                       double* avg_out /* [n_apps][4] */);
 
 /* ---- the unschedulable-pod marker's capacity checks (EXT/unschedulablepods.go:93-166) ------------------------------------
  * DoesPodExceedClusterCapacity (:132-166) for a batch of stale drivers, under any `binpack:` value, in one call.  Each driver is

@@ -1,5 +1,5 @@
 // gangpack_cluster.cu -- the entry points driven by the reservations: node priority orders (gp_potential_nodes),
-// availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster, gp_prepare_cluster_zones[_groups]), executor
+// availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster[_groups], gp_prepare_cluster_zones[_groups]), executor
 // reschedule (gp_reschedule_executors, gp_reschedule_from_reservations) and the failover reconciler (gp_reconcile_find_nodes),
 // with the input checks and device staging they share.
 #include "gangpack_ctx.cuh"
@@ -15,9 +15,15 @@
 
 // ---- node priority order (f1) and availability snapshot (f2): device stages + the entries built on them ----
 
-// offsets of the single instance group from the device-resident candidate counts
-__global__ void gp_offsets_from_counts(const int32_t* __restrict__ counts, int32_t* __restrict__ exec_off, int32_t* __restrict__ drv_off) {
-    if (threadIdx.x == 0) { drv_off[0] = 0; drv_off[1] = counts[0]; exec_off[0] = 0; exec_off[1] = counts[1]; }
+// exec_off / drv_off [n_ig + 1] of the plain multi-group snapshot: instance group g's range of the instance-group-major
+// candidate orders (ig NULL: every node in instance group 0, so [0, count, count, ...])
+__global__ void gp_ig_offsets(int32_t n_ig, const int32_t* __restrict__ counts, const int32_t* __restrict__ drv,
+                              const int32_t* __restrict__ exe, const int32_t* __restrict__ ig, int32_t* __restrict__ exec_off,
+                              int32_t* __restrict__ drv_off) {
+    const int32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g > n_ig) return;
+    drv_off[g] = ig_lower_bound(drv, counts[0], ig, g);
+    exec_off[g] = ig_lower_bound(exe, counts[1], ig, g);
 }
 
 // Host checks shared by the entries below; `who` (the entry's name) prefixes every message.  The shape of a gp_usage_input:
@@ -275,6 +281,56 @@ static gp_status prepare_snapshot(gp_ctx* c, gp_nodes* dn, const long long* d_av
     return GP_OK;
 }
 
+// The instance-group arguments of gp_prepare_cluster_groups and gp_prepare_cluster_zones_groups: n_ig >= 1, values in
+// [-1, n_ig), and with several instance groups at most 2^22 (instance group, zone + 1) pairs (stage_sort's zone totals are
+// per pair).  The other arguments are checked by prepare_orders.
+static gp_status check_instance_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+                                       const char* who) {
+    if (n_ig < 1) return fail(c, GP_ERR_INVALID, who, "n_instance_groups must be >= 1");
+    if (sort && n_ig > 1 && (int64_t)n_ig * ((int64_t)sort->n_zones + 1) > kZoneLayoutMaxPairs)
+        return fail(c, GP_ERR_INVALID, who, "n_instance_groups x (n_zones + 1) above 2^22");
+    if (ig && usage && sort && usage->n_nodes == sort->n_nodes)
+        for (int32_t i = 0; i < usage->n_nodes; ++i)
+            if (ig[i] < -1 || ig[i] >= n_ig) return fail(c, GP_ERR_INVALID, who, "instance_group outside [-1, n_instance_groups)");
+    return GP_OK;
+}
+
+// gp_prepare_cluster (ig NULL, n_ig 1) and gp_prepare_cluster_groups: the checks, reservations -> availability ->
+// instance-group-major priority orders (prepare_orders, which synchronises once and refuses before anything of the context
+// is replaced) -> snapshot group g = instance group g's range of those orders (gp_ig_offsets) -> the slot layout, then one
+// synchronise that reads back counts[3] and, when ig_ties is given, the undefined ties [n_ig] of each instance group.
+// ig NULL with n_ig > 1: every node in instance group 0, the others empty.
+static gp_status prepare_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+                                const char* who, int32_t* counts, int32_t* ig_ties, SortStage* so_out = nullptr) {
+    long long *d_avail = nullptr, *d_sched = nullptr;
+    SortStage so{};
+    GP_TRY(prepare_orders(c, usage, sort, ig, ig ? n_ig : 1, who, &d_avail, &d_sched, &so));
+    cudaStream_t st = c->stream;
+    const size_t G1 = (size_t)n_ig + 1;
+    GP_CUDA(c, c->exec_off.reserve(4 * G1)); GP_CUDA(c, c->drv_off.reserve(4 * G1));
+    const int T = 256;
+    gp_ig_offsets<<<(unsigned)((G1 + T - 1) / T), T, 0, st>>>(n_ig, so.counts, so.drv, so.exe, so.ig, c->exec_off.as<int32_t>(),
+                                                               c->drv_off.as<int32_t>());
+    GP_CUDA(c, cudaGetLastError());
+    gp_nodes dn{};
+    dn.n_nodes = usage->n_nodes;
+    dn.n_groups = n_ig;
+    dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = so.exe;
+    dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = so.drv;
+    GP_TRY(prepare_snapshot(c, &dn, d_avail, d_sched, so, counts));
+    if (ig_ties && so.ig_ties) GP_CUDA(c, cudaMemcpyAsync(ig_ties, so.ig_ties, 4 * (size_t)n_ig, cudaMemcpyDeviceToHost, st));
+    GP_CUDA(c, cudaStreamSynchronize(st));
+    if (ig_ties && !so.ig_ties) {                       // one instance group holds every node: its ties are the total
+        std::fill(ig_ties, ig_ties + n_ig, 0);
+        ig_ties[0] = counts[2];
+    }
+    c->n_drv = counts[0]; c->n_exec = counts[1];
+    c->have_eff_sched = true;           // SchedulableResources for gp_packing_efficiency (the zone entry points still want gp_set_schedulable)
+    if (sort->undefined_ties) *sort->undefined_ties = counts[2];
+    if (so_out) *so_out = so;
+    return GP_OK;
+}
+
 // The two gp_build_*availability entries: the availability stage, then every non-NULL outs[k] gets row k % 3 of
 // availableResources for k < 3 (first_fit: that of rescheduleExecutor's first-fit branch), of SchedulableResources for k >= 3.
 // The stage's status word is read first: a refused call writes to none of them.
@@ -454,27 +510,36 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
     c->layout_tail = nullptr;
     if (n_driver) *n_driver = 0;
     if (n_executor) *n_executor = 0;
-    long long *d_avail = nullptr, *d_sched = nullptr;
-    SortStage so{};
-    gp_status s = prepare_orders(c, usage, sort, nullptr, 1, "gp_prepare_cluster", &d_avail, &d_sched, &so);
-    if (s != GP_OK) return s;
-    cudaStream_t st = c->stream;
-    GP_CUDA(c, c->exec_off.reserve(8)); GP_CUDA(c, c->drv_off.reserve(8));
-    gp_offsets_from_counts<<<1, 32, 0, st>>>(so.counts, c->exec_off.as<int32_t>(), c->drv_off.as<int32_t>());
-    gp_nodes dn{};
-    dn.n_nodes = usage->n_nodes;
-    dn.n_groups = 1;
-    dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = so.exe;
-    dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = so.drv;
     int32_t counts[3] = {0, 0, 0};
-    s = prepare_snapshot(c, &dn, d_avail, d_sched, so, counts);
-    if (s != GP_OK) return s;
-    GP_CUDA(c, cudaStreamSynchronize(st));
-    c->n_drv = counts[0]; c->n_exec = counts[1];
-    c->have_eff_sched = true;           // SchedulableResources for gp_packing_efficiency (the zone entry points still want gp_set_schedulable)
-    if (sort->undefined_ties) *sort->undefined_ties = counts[2];
+    GP_TRY(prepare_groups(c, usage, sort, nullptr, 1, "gp_prepare_cluster", counts, nullptr));
     if (n_driver) *n_driver = counts[0];
     if (n_executor) *n_executor = counts[1];
+    return GP_OK;
+}
+
+// the same chain for every instance group at once: snapshot group i holds instance group i's PotentialNodes orders
+gp_status gp_prepare_cluster_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
+                                    int32_t n_instance_groups, gp_instance_group_orders* out) {
+    const char* who = "gp_prepare_cluster_groups";
+    if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
+    if (!out) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
+    out->n_driver = 0; out->n_executor = 0;
+    const int32_t G = n_instance_groups;
+    GP_TRY(check_instance_groups(c, usage, sort, instance_group, G, who));
+    int32_t counts[3] = {0, 0, 0};
+    SortStage so{};
+    GP_TRY(prepare_groups(c, usage, sort, instance_group, G, who, counts, out->undefined_ties, &so));
+    out->n_driver = counts[0]; out->n_executor = counts[1];
+    // the orders and their offsets only when asked: the snapshot's own exec_off / drv_off, and the sort's orders, which stay
+    // in its scratch until the next sort
+    Arena ar{c->zoneprep, c->stream};
+    const size_t g1 = (size_t)G + 1;
+    ar.get(out->exec_off, c->exec_off.as<int32_t>(), g1);
+    ar.get(out->drv_off, c->drv_off.as<int32_t>(), g1);
+    ar.get(out->exec_order, so.exe, (size_t)counts[1]);
+    ar.get(out->drv_order, so.drv, (size_t)counts[0]);
+    if (out->exec_off || out->drv_off || out->exec_order || out->drv_order) GP_TRY(ar.sync(c));
     return GP_OK;
 }
 
@@ -510,13 +575,7 @@ gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage
     if (!layout) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
     const int32_t G = n_instance_groups;
-    if (G < 1) return fail(c, GP_ERR_INVALID, who, "n_instance_groups must be >= 1");
-    if (sort && G > 1 && (int64_t)G * ((int64_t)sort->n_zones + 1) > kZoneLayoutMaxPairs)
-        return fail(c, GP_ERR_INVALID, who, "n_instance_groups x (n_zones + 1) above 2^22");
-    if (instance_group && usage && sort && usage->n_nodes == sort->n_nodes)
-        for (int32_t i = 0; i < usage->n_nodes; ++i)
-            if (instance_group[i] < -1 || instance_group[i] >= G)
-                return fail(c, GP_ERR_INVALID, who, "instance_group outside [-1, n_instance_groups)");
+    GP_TRY(check_instance_groups(c, usage, sort, instance_group, G, who));
     ZonePrep zp{};
     GP_TRY(prepare_zones(c, usage, sort, instance_group, G, layout->kind, true, who, nullptr, layout->undefined_ties, &zp));
     if (sort->undefined_ties) *sort->undefined_ties = zp.counts[2];

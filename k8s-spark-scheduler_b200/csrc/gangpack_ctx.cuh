@@ -163,6 +163,7 @@ struct gp_ctx {
     DevStatus* status() const { return dev_misc.as<DevStatus>(); }
     PinnedStatus* host_status() const { return static_cast<PinnedStatus*>(pinned_misc); }
     std::vector<int64_t> host_off;
+    std::vector<int32_t> eff_seg;                 // gp_packing_efficiency_groups: seg_off [G + 1], then the bucketed nodes
     std::vector<int32_t> v_owner;                 // gp_set_snapshot validation scratch (no per-call allocation)
     // gp_set_snapshot's host copy of the layout, kept for gp_pack_fifo_az_aware's order checks: v_owner[v] (group, roles)
     // and v_pos[v] / v_pos[n_nodes + v] (position of v in its group's executor / driver order).  host_layout: they

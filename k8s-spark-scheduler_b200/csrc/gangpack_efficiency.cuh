@@ -29,6 +29,10 @@
 // [driver] + ExecutorNodes (first-occurrence election as in the FIFO kernels, so node-major and round-major lists alike),
 // swaps each such node's unreserved terms for its reserved ones in the exact accumulator and rounds once: O(k) per row
 // after one O(N) pass per call.
+// Segmented (gp_packing_efficiency_groups): the nodes are bucketed by instance group in CSR (seg_off / nodes), n_part CTAs
+// of the base pass per segment, gp_eff_finish reduces each segment's partials in a CTA of its own, and a row reads its
+// instance group's base and node count.  The whole table is the one-segment case (nodes and seg_off NULL); the sums are
+// exact, so the split does not change a bit.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -227,15 +231,21 @@ struct EffBaseIn {
     SnapshotAvail av;
     const long long* sched[3];       // SchedulableResources [3][n_nodes]
     int32_t n_nodes;
+    const int32_t* nodes;            // segmented: the nodes bucketed by segment, or NULL (every node, one segment)
+    const int32_t* seg_off;          // segmented: [segments + 1] CSR of nodes, or NULL
+    int32_t n_part;                  // CTAs per segment (the grid is segments x n_part)
 };
 
-// unreserved terms of every node -> partial[blockIdx.x]
+// unreserved terms of every node of segment blockIdx.x / n_part -> partial[blockIdx.x]
 __global__ void __launch_bounds__(kEffThreads) gp_eff_base(EffBaseIn in, EffAcc* __restrict__ partial, int* __restrict__ err) {
     EffAcc a;
     acc_zero(a);
     bool ok = true;
     const long long zero[3] = {0, 0, 0};
-    for (int32_t n = blockIdx.x * kEffThreads + threadIdx.x; n < in.n_nodes; n += gridDim.x * kEffThreads) {
+    const int32_t sg = blockIdx.x / in.n_part, part = blockIdx.x - sg * in.n_part;
+    const int32_t lo = in.seg_off ? in.seg_off[sg] : 0, hi = in.seg_off ? in.seg_off[sg + 1] : in.n_nodes;
+    for (int32_t t = lo + part * kEffThreads + threadIdx.x; t < hi; t += in.n_part * kEffThreads) {
+        const int32_t n = in.nodes ? in.nodes[t] : t;
         long long av[3];
         in.av.load(n, av[0], av[1], av[2]);
         const long long* sc[3] = {in.sched[0] + n, in.sched[1] + n, in.sched[2] + n};
@@ -247,13 +257,14 @@ __global__ void __launch_bounds__(kEffThreads) gp_eff_base(EffBaseIn in, EffAcc*
     if (threadIdx.x == 0) partial[blockIdx.x] = a;
 }
 
-// partial[0 .. n_partial) -> *base
+// one CTA per segment: partial[blockIdx.x * n_partial ..][0 .. n_partial) -> base[blockIdx.x]
 __global__ void __launch_bounds__(kEffThreads) gp_eff_finish(const EffAcc* __restrict__ partial, int32_t n_partial, EffAcc* __restrict__ base) {
     EffAcc a;
     acc_zero(a);
+    partial += (size_t)blockIdx.x * n_partial;
     for (int32_t i = threadIdx.x; i < n_partial; i += kEffThreads) acc_add(a, partial[i]);
     acc_block_reduce(a);
-    if (threadIdx.x == 0) *base = a;
+    if (threadIdx.x == 0) base[blockIdx.x] = a;
 }
 
 struct EffRowsIn {
@@ -264,7 +275,9 @@ struct EffRowsIn {
     const int64_t* off;               // ExecutorNodes offsets
     const int32_t* driver;
     const int32_t* exec;
-    const EffAcc* base;
+    const EffAcc* base;               // [segments]
+    const int32_t* group;             // segmented: each row's segment (instance group), or NULL (segment 0)
+    const int32_t* seg_off;           // segmented: [segments + 1], a segment's node count is its length; NULL: n_nodes
     int32_t n_apps;
     int32_t n_nodes;
     int32_t executors_reserved;       // 0: minimal-fragmentation (the driver alone is in `reserved`)
@@ -329,9 +342,10 @@ __global__ void __launch_bounds__(kEffThreads) gp_eff_rows(EffRowsIn in, double*
     if (!ok) atomicOr(err, kEffErrRange);
     acc_warp_reduce(delta);
     if (lane == 0) {
-        EffAcc t = *in.base;
+        const int32_t g = in.group ? in.group[i] : 0;
+        EffAcc t = in.base[g];
         acc_add(t, delta);
-        const double length = fmax((double)in.n_nodes, 1.0);
+        const double length = fmax((double)(in.seg_off ? in.seg_off[g + 1] - in.seg_off[g] : in.n_nodes), 1.0);
         double* o = avg_out + 4 * (int64_t)i;
         o[0] = fx_to_double(t.s[0]) / length;
         o[1] = fx_to_double(t.s[1]) / length;

@@ -1,6 +1,6 @@
 // gangpack_zones.cu -- the single-AZ and az-aware-tightly-pack packers (gp_pack_batch_zones, gp_pack_fifo_zones,
 // gp_pack_fifo_az_aware, gp_pack_batch_az_aware, gp_pack_fifo_zones_groups) with gp_set_schedulable, the reservation table and usage deltas of the
-// resident snapshot (gp_reserve_placements, gp_apply_usage_delta), and gp_packing_efficiency.
+// resident snapshot (gp_reserve_placements, gp_apply_usage_delta), and gp_packing_efficiency[_groups].
 #include "gangpack_ctx.cuh"
 #include "gangpack_zones.cuh"
 #include "gangpack_zonefifo.cuh"
@@ -654,23 +654,50 @@ static const Refusal kEffRefusals[] = {
     {kEffErrRange, GP_ERR_UNREPRESENTABLE, "an efficiency term outside the exact accumulator's range"},
 };
 
-gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, double* avg_out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_packing_efficiency: no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)");
+}  // extern "C"
+
+// gp_packing_efficiency (ig NULL: every node of the table, one segment) and gp_packing_efficiency_groups (row i over the nodes
+// v with ig[v] == a->group[i]): the host pass over the rows, the (segmented) base pass and the row pass.
+static gp_status packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, const int32_t* ig,
+                                    int32_t n_ig, double* avg_out, const char* who) {
+    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, who, "no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)");
     if (!c->have_eff_sched)
-        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: no SchedulableResources (gp_set_schedulable, gp_prepare_cluster or gp_prepare_cluster_zones first)");
-    if (!a || !placed || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: NULL apps/placed");
+        return fail(c, GP_ERR_INVALID, who, "no SchedulableResources (gp_set_schedulable, gp_prepare_cluster or gp_prepare_cluster_zones first)");
+    if (!a || !placed || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/placed");
     if (algo != GP_TIGHTLY_PACK && algo != GP_DISTRIBUTE_EVENLY && algo != GP_MINIMAL_FRAGMENTATION)
-        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: unknown algo");
+        return fail(c, GP_ERR_INVALID, who, "unknown algo");
     if (charged != GP_MODE_INDEPENDENT && charged != GP_MODE_FIFO_REFERENCE && charged != GP_MODE_FIFO_EXACT)
-        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: unknown charged mode");
-    if (charged != GP_MODE_INDEPENDENT && a->n_apps != 1)
-        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: a FIFO charged mode adds back ONE application's usage: n_apps must be 1");
-    const int32_t Q = a->n_apps;
+        return fail(c, GP_ERR_INVALID, who, "unknown charged mode");
+    if (!ig && charged != GP_MODE_INDEPENDENT && a->n_apps != 1)
+        return fail(c, GP_ERR_INVALID, who, "a FIFO charged mode adds back ONE application's usage: n_apps must be 1");
+    const int32_t Q = a->n_apps, N32 = c->n_nodes;
+    // instance groups: the nodes bucketed by instance group (stable counting sort), seg[0 .. G] their CSR offsets
+    std::vector<int32_t>& seg = c->eff_seg;
+    if (ig) {
+        if (n_ig < 1) return fail(c, GP_ERR_INVALID, who, "n_instance_groups must be >= 1");
+        seg.assign((size_t)n_ig + 1, 0);
+        for (int32_t v = 0; v < N32; ++v) {
+            if (ig[v] < -1 || ig[v] >= n_ig) return fail(c, GP_ERR_INVALID, who, "instance_group outside [-1, n_instance_groups)");
+            if (ig[v] >= 0) ++seg[(size_t)ig[v] + 1];
+        }
+        for (int32_t g = 0; g < n_ig; ++g) seg[(size_t)g + 1] += seg[(size_t)g];
+        for (int32_t i = 0; i < Q; ++i) {
+            const int32_t g = a->group ? a->group[i] : 0;
+            if (g < 0 || g >= n_ig) return fail(c, GP_ERR_INVALID, who, "apps->group outside [0, n_instance_groups)");
+        }
+        if (charged != GP_MODE_INDEPENDENT) {           // each row adds back usage on its own instance group's nodes only
+            std::vector<uint8_t>& seen = c->v_seen_e;
+            seen.assign((size_t)n_ig, 0);
+            for (int32_t i = 0; i < Q; ++i) {
+                const int32_t g = a->group ? a->group[i] : 0;
+                if (seen[(size_t)g]) return fail(c, GP_ERR_INVALID, who, "a FIFO charged mode adds back ONE application's usage per instance group: two rows name one instance group");
+                seen[(size_t)g] = 1;
+            }
+        }
+    }
     if (Q == 0) return GP_OK;
     if (!avg_out || !a->drv_cpu_milli || !a->drv_mem_bytes || !a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !placed->driver_node)
-        return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: missing app/result arrays");
+        return fail(c, GP_ERR_INVALID, who, "missing app/result arrays");
     // host pass over the placed rows: offsets, request domain, node indices (a caller-supplied placement need not be feasible)
     std::vector<int64_t>& off = c->host_off;
     off.resize((size_t)Q + 1);
@@ -681,54 +708,75 @@ gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const
         off[(size_t)i] = a->exec_out_off ? a->exec_out_off[i] : acc;
         acc += k;
         const int32_t d = placed->driver_node[i];
-        if (d >= c->n_nodes) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: driver_node out of range");
+        if (d >= N32) return fail(c, GP_ERR_INVALID, who, "driver_node out of range");
         if (d < 0) continue;
+        const int32_t g = ig && a->group ? a->group[i] : 0;
+        if (ig && ig[d] != g) return fail(c, GP_ERR_INVALID, who, "driver_node outside the application's instance group");
         for (const int64_t* col : qc) {
             if (!col) continue;
-            if (col[i] < 0) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: negative request");
-            if (col[i] >= kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, "gp_packing_efficiency: request >= 2^61");
+            if (col[i] < 0) return fail(c, GP_ERR_INVALID, who, "negative request");
+            if (col[i] >= kMaxQuantity) return fail(c, GP_ERR_UNREPRESENTABLE, who, "request >= 2^61");
         }
-        if (k > 0 && !placed->executor_nodes) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: executor_nodes is NULL");
+        if (k > 0 && !placed->executor_nodes) return fail(c, GP_ERR_INVALID, who, "executor_nodes is NULL");
         if (off[(size_t)i] < 0 || off[(size_t)i] + k > placed->executor_nodes_cap)
-            return fail(c, GP_ERR_CAPACITY, "gp_packing_efficiency: offsets exceed executor_nodes_cap");
+            return fail(c, GP_ERR_CAPACITY, who, "offsets exceed executor_nodes_cap");
         for (int64_t t = 0; t < k; ++t) {
             const int32_t n = placed->executor_nodes[off[(size_t)i] + t];
-            if (n < 0 || n >= c->n_nodes) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency: executor node out of range");
+            if (n < 0 || n >= N32) return fail(c, GP_ERR_INVALID, who, "executor node out of range");
+            if (ig && ig[n] != g) return fail(c, GP_ERR_INVALID, who, "executor node outside the application's instance group");
         }
     }
     off[(size_t)Q] = a->exec_out_off ? a->exec_out_off[Q] : acc;
     const int64_t total = placed->executor_nodes_cap < off[(size_t)Q] ? placed->executor_nodes_cap : off[(size_t)Q];
+    const size_t G = ig ? (size_t)n_ig : 1, NS = ig ? (size_t)seg[G] : 0;
+    if (ig) {                                           // bucket the nodes: seg[G + 1 ..] = the nodes of each instance group
+        seg.resize(G + 1 + NS);
+        std::vector<int32_t> cur(seg.begin(), seg.begin() + (ptrdiff_t)G);      // next free position of each bucket
+        for (int32_t v = 0; v < N32; ++v)
+            if (ig[v] >= 0) seg[G + 1 + (size_t)cur[(size_t)ig[v]]++] = v;
+    }
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
-    const size_t q = (size_t)Q, T = (size_t)(total > 0 ? total : 0), N = (size_t)c->n_nodes;
+    const size_t q = (size_t)Q, T = (size_t)(total > 0 ? total : 0), N = (size_t)N32;
     const int TH = kEffThreads;
-    const int n_part = (int)std::max<size_t>(1, std::min<size_t>((N + TH - 1) / TH, (size_t)c->sm_count * 4));
+    // CTAs per segment: up to four per SM over all segments together, at most one per 256 nodes of the largest segment
+    size_t longest = ig ? 0 : N;
+    for (size_t g = 0; ig && g < G; ++g) longest = std::max<size_t>(longest, (size_t)(seg[g + 1] - seg[g]));
+    const size_t per_seg = ((size_t)c->sm_count * 4 + G - 1) / G;
+    const int n_part = (int)std::max<size_t>(1, std::min<size_t>((longest + TH - 1) / TH, per_seg));
     Arena ar{c->zonebuf, st};
     const auto in = ar.take<int64_t>(6 * q);
     const auto cnt = ar.take<int32_t>(q);
     const auto off_p = ar.take<int64_t>(q + 1);
     const auto drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1);
-    const auto part = ar.take<EffAcc>((size_t)n_part), base = ar.take<EffAcc>(1);
+    const auto part = ar.take<EffAcc>((size_t)n_part * G), base = ar.take<EffAcc>(G);
     const auto avg = ar.take<double>(4 * q);
     const auto err = ar.take<int>(1);
+    const auto segp = ar.take<int32_t>(ig ? G + 1 + NS : 0), grp = ar.take<int32_t>(ig && a->group ? q : 0);
     ar.reserve();
     EffRowsIn ri{};
     ri.cols = upload_app_columns(ar, a, off.data(), in, cnt, off_p);
     ri.driver = ar.put(drv, placed->driver_node);
     ar.put(exe.part(0, T), placed->executor_nodes);
     int* d_err = ar.zero(err);
+    const int32_t* d_seg = ig ? ar.put(segp, seg.data()) : nullptr;
+    ri.group = ig ? ar.put(grp, a->group) : nullptr;
     GP_TRY(ar.check(c));
     EffBaseIn bi{};
     bi.av = SnapshotAvail{c->pair.as<longlong2>(), c->sgpu.as<long long>(), c->node_slot.as<int32_t>(), c->node_cpu.as<long long>(),
                       c->node_mem.as<long long>(), c->node_gpu.as<long long>()};
     bi.sched[0] = c->sched.as<long long>(); bi.sched[1] = c->sched.as<long long>() + N; bi.sched[2] = c->sched.as<long long>() + 2 * N;
-    bi.n_nodes = c->n_nodes;
-    gp_eff_base<<<n_part, TH, 0, st>>>(bi, ar.ptr(part), d_err);
-    gp_eff_finish<<<1, TH, 0, st>>>(ar.ptr(part), n_part, ar.ptr(base));
+    bi.n_nodes = N32;
+    bi.seg_off = d_seg;
+    bi.nodes = d_seg ? d_seg + G + 1 : nullptr;
+    bi.n_part = n_part;
+    gp_eff_base<<<(unsigned)((size_t)n_part * G), TH, 0, st>>>(bi, ar.ptr(part), d_err);
+    gp_eff_finish<<<(unsigned)G, TH, 0, st>>>(ar.ptr(part), n_part, ar.ptr(base));
     ri.av = bi.av;
     for (int k = 0; k < 3; ++k) ri.sched[k] = bi.sched[k];
     ri.count = ar.ptr(cnt); ri.off = ar.ptr(off_p); ri.exec = ar.ptr(exe); ri.base = ar.ptr(base);
-    ri.n_apps = Q; ri.n_nodes = c->n_nodes;
+    ri.seg_off = d_seg;
+    ri.n_apps = Q; ri.n_nodes = N32;
     ri.executors_reserved = algo == GP_MINIMAL_FRAGMENTATION ? 0 : 1;
     ri.charged = (int32_t)charged;
     gp_eff_rows<<<(unsigned)((q * 32 + TH - 1) / TH), TH, 0, st>>>(ri, ar.ptr(avg), d_err);
@@ -737,6 +785,25 @@ gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const
     ar.get(avg_out, avg);
     ar.get(&herr, err);
     GP_TRY(ar.sync(c));
-    return refuse(c, herr, kEffRefusals, "gp_packing_efficiency");
+    return refuse(c, herr, kEffRefusals, who);
+}
+
+extern "C" {
+
+gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, double* avg_out) {
+    if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
+    return packing_efficiency(c, a, algo, placed, charged, nullptr, 1, avg_out, "gp_packing_efficiency");
+}
+
+// the same metric with row i averaged over its instance group's nodes (selectDriverNode's metadata) instead of the table's
+gp_status gp_packing_efficiency_groups(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged,
+                                       const int32_t* instance_group, int32_t n_instance_groups, double* avg_out) {
+    if (!c) return GP_ERR_INVALID;
+    c->layout_tail = nullptr;
+    if (!instance_group && c->n_nodes > 0) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency_groups: instance_group is NULL");
+    static const int32_t none = -1;                     // an empty node table: no node in any instance group
+    return packing_efficiency(c, a, algo, placed, charged, instance_group ? instance_group : &none, n_instance_groups, avg_out,
+                              "gp_packing_efficiency_groups");
 }
 }  // extern "C"

@@ -38,6 +38,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
            "gp_node_overhead", "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
+           "gp_prepare_cluster_groups", "gp_packing_efficiency_groups",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -158,6 +159,11 @@ class gp_instance_group_layout(C.Structure):
     _fields_ = [("kind", C.c_int32), ("n_groups", C.c_int32), ("n_driver", C.c_int32), ("n_executor", C.c_int32)] + \
         [(k, C.c_void_p) for k in ("group_off", "n_zones", "exec_off", "exec_order", "drv_off", "drv_order", "group_exec_off",
                                    "group_exec_order", "group_drv_off", "group_drv_order", "zone_of_group", "undefined_ties")]
+
+
+class gp_instance_group_orders(C.Structure):
+    _fields_ = [("n_driver", C.c_int32), ("n_executor", C.c_int32)] + \
+        [(k, C.c_void_p) for k in ("exec_off", "exec_order", "drv_off", "drv_order", "undefined_ties")]
 
 
 class gp_reschedule(C.Structure):
@@ -295,6 +301,9 @@ def load():
     L.gp_apply_usage_delta.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
     L.gp_packing_efficiency.restype = C.c_int
     L.gp_packing_efficiency.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_results), C.c_int, C.c_void_p]
+    L.gp_packing_efficiency_groups.restype = C.c_int
+    L.gp_packing_efficiency_groups.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_results), C.c_int, C.c_void_p,
+                                               C.c_int32, C.c_void_p]
     L.gp_exceeds_cluster_capacity.restype = C.c_int
     L.gp_exceeds_cluster_capacity.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.POINTER(gp_apps), C.c_int, C.c_void_p]
     L.gp_reconcile_find_nodes.restype = C.c_int
@@ -334,6 +343,9 @@ def load():
     L.gp_prepare_cluster_zones_groups.restype = C.c_int
     L.gp_prepare_cluster_zones_groups.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input), C.c_void_p, C.c_int32,
                                                   C.POINTER(gp_instance_group_layout)]
+    L.gp_prepare_cluster_groups.restype = C.c_int
+    L.gp_prepare_cluster_groups.argtypes = [C.c_void_p, C.POINTER(gp_usage_input), C.POINTER(gp_sort_input), C.c_void_p, C.c_int32,
+                                            C.POINTER(gp_instance_group_orders)]
     L.gp_potential_nodes.restype = C.c_int
     L.gp_potential_nodes.argtypes = [C.c_void_p, C.POINTER(gp_sort_input), C.c_void_p, C.POINTER(C.c_int32),
                                      C.c_void_p, C.POINTER(C.c_int32)]
@@ -725,6 +737,36 @@ class GangPacker:
                        group_drv_order=bufs["group_drv_order"][:out["group_drv_off"][ng]].copy())
         return out
 
+    def prepare_cluster_groups(self, alloc, overhead, res_node, res, instance_group, n_instance_groups, zone_id=None, n_zones=1,
+                               name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None, driver_label_rank=None,
+                               executor_label_rank=None, orders=True):
+        """prepare_cluster for every instance group at once: instance_group[v] = node v's instance group (0 ..
+        n_instance_groups-1, -1 = none; None = every node in 0).  Snapshot group i holds instance group i's PotentialNodes
+        orders over its own nodes, ready for pack_batch with apps["group"] = the instance group.  -> dict with n_driver,
+        n_executor, undefined_ties (the total), ig_undefined_ties (per instance group) and, with `orders`, exec_off / drv_off
+        ([n_instance_groups + 1]) and the instance-group-major exec_order / drv_order.  A refused call leaves the context as
+        it was."""
+        ui = _usage_input(alloc, overhead, res_node, res)
+        n = ui.n_nodes
+        G = int(n_instance_groups)
+        ig = _np(instance_group, np.int32)
+        ties = C.c_int32(0)
+        si = _sort_input(n, n_zones, zone_id, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
+                         executor_label_rank, ties=ties)
+        bufs = {"undefined_ties": np.full(max(G, 0) + 1, -9, np.int32)}
+        if orders:
+            bufs.update({k: np.full(max(G, 0) + 1, -9, np.int32) for k in ("exec_off", "drv_off")})
+            bufs.update({k: np.full(max(n, 1), -9, np.int32) for k in ("exec_order", "drv_order")})
+        o = gp_instance_group_orders(**{k: _p(v) for k, v in bufs.items()})
+        self._check(load().gp_prepare_cluster_groups(self._h, C.byref(ui), C.byref(si), _p(ig), G, C.byref(o)))
+        self.n_nodes = n
+        out = dict(n_driver=o.n_driver, n_executor=o.n_executor, undefined_ties=ties.value,
+                   ig_undefined_ties=bufs["undefined_ties"][:G].copy())
+        if orders:
+            out.update(exec_off=bufs["exec_off"].copy(), drv_off=bufs["drv_off"].copy(),
+                       exec_order=bufs["exec_order"][:o.n_executor].copy(), drv_order=bufs["drv_order"][:o.n_driver].copy())
+        return out
+
     # ---- node priority order (NodeSorter.PotentialNodes) ---------------------------------------
     def potential_nodes(self, avail_cpu, avail_mem, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
                         unschedulable=None, ready=None, driver_label_rank=None, executor_label_rank=None, avail_gpu=None):
@@ -884,6 +926,25 @@ class GangPacker:
         a = _apps(apps, off)
         r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
         self._check(load().gp_packing_efficiency(self._h, C.byref(a), algo, C.byref(r), charged, _p(avg)))
+        return avg[:q]
+
+    def packing_efficiency_groups(self, apps: dict, placed, algo: int, instance_group, n_instance_groups: int,
+                                  charged: int = MODE_INDEPENDENT) -> np.ndarray:
+        """packing_efficiency with row i averaged over the nodes v with instance_group[v] == apps["group"][i] (absent: 0)
+        instead of every node of the snapshot -- the reference's metric over the driver's instance group.  The FIFO charged
+        modes allow at most one row per instance group; a placed node outside its row's instance group is refused.
+        -> (n_apps, 4) float64 {CPU, Memory, GPU, Max}."""
+        q = len(apps["count"])
+        driver, execn, off = placed
+        driver = _np(driver, np.int32); execn = _np(execn, np.int32)
+        if execn is None or len(execn) == 0:
+            execn = np.zeros(1, np.int32)
+        ig = _np(instance_group, np.int32)
+        avg = np.zeros((max(q, 1), 4), np.float64)
+        a = _apps(apps, off, group=apps.get("group"))
+        r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
+        self._check(load().gp_packing_efficiency_groups(self._h, C.byref(a), algo, C.byref(r), charged, _p(ig),
+                                                        int(n_instance_groups), _p(avg)))
         return avg[:q]
 
     def exceeds_cluster_capacity(self, alloc, apps: dict, packer: int, overhead=None, zone_id=None, n_zones=1, node_group=None,
