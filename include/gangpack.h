@@ -667,6 +667,67 @@ gp_status gp_packing_efficiency_groups(gp_ctx* ctx, const gp_apps* apps /* group
                                        const int32_t* instance_group /* [n_nodes] */, int32_t n_instance_groups,
                                        double* avg_out /* [n_apps][4] */);
 
+/* ---- the Predicate's placement metrics (EXT/resource.go:352-357) ------------------------------------------------------------
+ * What selectDriverNode reports about a successful pack besides the packing efficiency, for a batch of placed applications:
+ * ReportInitialDriverExecutorCollocationMetric (internal/metrics/metrics.go:223-252), ReportInitialNodeCountMetrics (:254-275)
+ * and ReportCrossZoneMetric with crossZoneTraffic (:277-318, 322-330).  Row i is one application: driver_node d,
+ * ExecutorNodes e[0..k) (k = exe_count[i], in any order: node-major, round-major, capacity order or a zone result) and its
+ * instance group.  The reference returns before these metrics when !HasCapacity (:347-350): a row with d < 0 (-1 and the FIFO
+ * -2 alike) gets the "not reported" record {collocation -1, every other field 0}.  For d >= 0, with E the set of e:
+ *   collocation          0 "no-collocation" when d is not in E (k = 0 included); 1 "driver-collocated-with-all-executors"
+ *                        when d is in E and |E| = 1; 2 "driver-collocated-with-some-executors" otherwise.
+ *   distinct_exec_nodes  |E|.
+ *   execs_per_node       k / |E| with Go's integer division; -1 when k = 0 (ReportInitialNodeCountMetrics returns early).
+ *   n_zones, cross_zone_pairs, total_pairs
+ *                        pods per node: the driver's node 1, plus one per executor entry (a driver node that hosts executors
+ *                        counts 1 + its executors); T = k + 1.  c_z = the pods on nodes of availableNodes whose metric zone is z;
+ *                        pods on other nodes count in T and in no zone.  n_zones = #{z : c_z > 0}; total_pairs = T (T - 1) / 2;
+ *                        cross_zone_pairs = T S - (S^2 + sum_z c_z^2) / 2 with S = sum_z c_z (exact: the numerator is even),
+ *                        which is crossZoneTraffic for every iteration order of its map (DESIGN.md §2.8).  With k <= 2^24 (the
+ *                        gp_apps bound) every value fits in int64.
+ *   metric_zone          [n_nodes] the node's zone as the metric reads it, interned to 0..n_metric_zones-1: the label
+ *                        failure-domain.beta.kubernetes.io/zone (v1.LabelZoneFailureDomain, :290) with a missing label
+ *                        interned as the string "unknown-zone" -- so it merges with a node literally labelled unknown-zone.
+ *                        NodeSchedulingMetadata.ZoneLabel reads the same key but maps a missing label to "default"
+ *                        (LIB/resources/resources.go:27, 78-81), and the single-AZ packers and rescheduling read
+ *                        topology.kubernetes.io/zone: none of their zone columns can be passed here as is.
+ *   instance_group       [n_nodes] or NULL.  availableNodes is the driver's instance group (ListWithPredicate(driver affinity),
+ *                        EXT/resource.go:292-295): node v is in row i's scope when instance_group[v] == apps->group[i] (NULL
+ *                        group = 0), -1 = in no instance group.  NULL: every node of the table is in scope (the one-group
+ *                        Predicate; apps->group and n_instance_groups are ignored).  A placed node outside the scope is allowed.
+ * Emitting the counters, histograms, gauges and Mean() stays with the caller.
+ * The call is stateless: it needs no snapshot and leaves the device availability, slots, zone layout, held az-aware orders and
+ * gp_last_stats untouched.  apps: exe_count, group and exec_out_off are read (NULL exec_out_off = the prefix sum of exe_count).
+ * GP_ERR_INVALID (gp_last_error names the cause): NULL arrays or negative sizes; n_metric_zones above max(n_nodes, 1) (an
+ * interned id comes from some node); a driver or executor node of a placed row
+ * outside [0, n_nodes); a metric_zone value outside [0, n_metric_zones); with instance_group, n_instance_groups < 1, a value
+ * outside [-1, n_instance_groups) or a row's group outside [0, n_instance_groups); a negative exe_count.  GP_ERR_CAPACITY: a
+ * placed row's ExecutorNodes outside [0, executor_nodes_cap).  GP_ERR_UNREPRESENTABLE: an exe_count above 2^24.  A refused call
+ * writes no record.  One stream synchronise. */
+typedef struct {
+    int32_t collocation;             /* -1 not reported, 0 / 1 / 2 as above */
+    int32_t distinct_exec_nodes;
+    int32_t execs_per_node;
+    int32_t n_zones;
+    int64_t cross_zone_pairs;
+    int64_t total_pairs;
+} gp_placement_record;
+gp_status gp_placement_metrics(gp_ctx* ctx, const gp_apps* apps, const gp_results* placed /* host */, int32_t n_nodes,
+                               const int32_t* metric_zone /* [n_nodes] */, int32_t n_metric_zones,
+                               const int32_t* instance_group /* [n_nodes] or NULL */, int32_t n_instance_groups,
+                               gp_placement_record* out /* [n_apps] */);
+/* The same on device arrays, enqueued on `stream` (a cudaStream_t; NULL = the context's stream) with no synchronise and no
+ * host copy, like gp_pack_batch_device, whose outputs (driver_node, executor_nodes, and the apps it read) it reads in place.
+ * Every array pointer inside apps / placed, metric_zone, instance_group and out is a device pointer on ctx's device;
+ * exec_out_off may be NULL (derived on the device).  The checks above run on the device: *dev_status (one device int32, or
+ * NULL) receives GP_OK, GP_ERR_INVALID, GP_ERR_UNREPRESENTABLE or GP_ERR_CAPACITY once the work has run, and the records are meaningful only when it
+ * is GP_OK.  Arguments that need no device data (NULL pointers, negative sizes) are refused at once.  The call's scratch
+ * belongs to the context: the next gp_placement_metrics* call on it must be ordered after this one (same stream, or an
+ * event). */
+gp_status gp_placement_metrics_device(gp_ctx* ctx, const gp_apps* dev_apps, const gp_results* dev_placed, int32_t n_nodes,
+                                      const int32_t* metric_zone, int32_t n_metric_zones, const int32_t* instance_group,
+                                      int32_t n_instance_groups, gp_placement_record* dev_out, int32_t* dev_status, void* stream);
+
 /* ---- the unschedulable-pod marker's capacity checks (EXT/unschedulablepods.go:93-166) ------------------------------------
  * DoesPodExceedClusterCapacity (:132-166) for a batch of stale drivers, under any `binpack:` value, in one call.  Each driver is
  * packed against the nodes of its affinity class with zero usage -- NodeSchedulingMetadataForNodes(nodes, zero usage, overhead)

@@ -214,6 +214,12 @@ struct gp_ctx {
     // gp_match_node_affinity, gp_reconcile_find_nodes or gp_node_overhead: no state points into it, and the next call's
     // use is ordered after this one's kernels on the context's stream
     DevBuf callbuf;
+    // gp_placement_metrics[_device]: staging and scratch of one call; the two words of PmState (zeroed at the start of every
+    // call); the host form's records before its refusal check; the dynamic shared memory its kernels may take (0 until the
+    // first call on this device)
+    DevBuf metricbuf, metricstate;
+    std::vector<gp_placement_record> pm_records;
+    int pm_smem_limit = 0;
     int zone_kind = -1;
     gp_az_orders zone_orders{};
     // gp_prepare_cluster_zones_groups: zone_igs = its n_instance_groups while its layout is held (0 otherwise, also after

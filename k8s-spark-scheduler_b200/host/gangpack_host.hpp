@@ -1584,3 +1584,85 @@ private:
 };
 
 }  // namespace extender
+
+// ------------------------------------------------------------------------------------------------
+namespace metrics {
+
+// One node of availableNodes (EXT/resource.go:292-295) as ReportCrossZoneMetric reads it: its name and labels.
+struct Node {
+    std::string Name;
+    std::map<std::string, std::string> Labels;
+};
+
+// What the three placement reporters selectDriverNode calls after a successful pack (EXT/resource.go:354-356) would emit:
+// ReportInitialDriverExecutorCollocationMetric (internal/metrics/metrics.go:223-252), ReportInitialNodeCountMetrics
+// (:254-275, nothing when ExecutorNodes is empty) and ReportCrossZoneMetric (:277-318).  Reported is false for an
+// EmptyPackingResult, for which selectDriverNode returns before the metrics.
+struct PlacementMetricsResult {
+    bool Reported = false;
+    std::string CollocationType;           // "no-collocation", "driver-collocated-with-all-executors" or "-some-executors"
+    bool NodeCountReported = false;        // ReportInitialNodeCountMetrics returns early when there are no executors
+    int64_t ExecutorsPerNode = 0;          // initialExecutorsPerNode
+    int64_t NodeCount = 0;                 // initialNodeCount
+    int64_t CrossZonePairs = 0;            // crossAzTraffic
+    int64_t TotalPairs = 0;                // totalTraffic
+    int64_t NumberOfZones = 0;             // applicationZonesCount
+};
+
+// The three reporters' inputs for one PackingResult, computed by one gp_placement_metrics call.  availableNodes is the
+// Predicate's node list; a driver or executor node that is not in it counts in the pod total and in no zone, as in the
+// reference.  The metric zone is the failure-domain.beta.kubernetes.io/zone label, a missing one interned as
+// "unknown-zone" (metrics.go:290-294), so it merges with a node literally labelled unknown-zone.  Emitting the counters,
+// histograms and gauges stays with the caller.
+inline PlacementMetricsResult PlacementMetrics(const binpack::PackingResult& packingResult, const std::vector<Node>& availableNodes) {
+    PlacementMetricsResult out;
+    if (!packingResult.HasCapacity) return out;
+    // node table: availableNodes (instance group 0) then the placed names outside it (instance group -1, zone 0)
+    std::unordered_map<std::string, int32_t> index;
+    std::unordered_map<std::string, int32_t> zones;
+    std::vector<int32_t> zone, group;
+    for (const Node& n : availableNodes) {
+        if (!index.emplace(n.Name, (int32_t)zone.size()).second) continue;       // a lister's names are unique
+        auto it = n.Labels.find(extender::LabelZoneFailureDomain);
+        const std::string z = it == n.Labels.end() ? "unknown-zone" : it->second;
+        zone.push_back(zones.emplace(z, (int32_t)zones.size()).first->second);
+        group.push_back(0);
+    }
+    auto idx = [&](const std::string& name) {
+        auto it = index.find(name);
+        if (it != index.end()) return it->second;
+        const int32_t i = (int32_t)zone.size();
+        index.emplace(name, i);
+        zone.push_back(0);
+        group.push_back(-1);
+        return i;
+    };
+    int32_t driver = idx(packingResult.DriverNode);
+    std::vector<int32_t> execs;
+    for (const auto& n : packingResult.ExecutorNodes) execs.push_back(idx(n));
+    const int32_t count = (int32_t)execs.size();
+    if (execs.empty()) execs.push_back(0);
+    const int64_t off[2] = {0, count};
+    gp_apps a{};
+    a.n_apps = 1;
+    a.exe_count = &count;
+    a.exec_out_off = off;
+    gp_results r{&driver, execs.data(), (int64_t)execs.size()};
+    const int32_t n_zones = std::max<int32_t>((int32_t)zones.size(), 1);
+    gp_placement_record rec{};
+    gangpack::Device& d = gangpack::Device::Get();
+    d.check(gp_placement_metrics(d.ctx(), &a, &r, (int32_t)zone.size(), zone.data(), n_zones, group.data(), 1, &rec),
+            "gp_placement_metrics");
+    static const char* const kTags[3] = {"no-collocation", "driver-collocated-with-all-executors", "driver-collocated-with-some-executors"};
+    out.Reported = true;
+    out.CollocationType = kTags[rec.collocation];
+    out.NodeCountReported = rec.execs_per_node >= 0;
+    out.ExecutorsPerNode = out.NodeCountReported ? rec.execs_per_node : 0;
+    out.NodeCount = out.NodeCountReported ? rec.distinct_exec_nodes : 0;
+    out.CrossZonePairs = rec.cross_zone_pairs;
+    out.TotalPairs = rec.total_pairs;
+    out.NumberOfZones = rec.n_zones;
+    return out;
+}
+
+}  // namespace metrics

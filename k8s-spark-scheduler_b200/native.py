@@ -38,7 +38,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
            "gp_node_overhead", "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
-           "gp_prepare_cluster_groups", "gp_packing_efficiency_groups",
+           "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
 
@@ -239,6 +239,17 @@ class gp_overhead_out(C.Structure):
                 ("has_reservation", C.c_void_p), ("n_warned", C.c_void_p)]
 
 
+class gp_placement_record(C.Structure):
+    _fields_ = [("collocation", C.c_int32), ("distinct_exec_nodes", C.c_int32), ("execs_per_node", C.c_int32), ("n_zones", C.c_int32),
+                ("cross_zone_pairs", C.c_int64), ("total_pairs", C.c_int64)]
+
+
+# numpy view of gp_placement_record[]: collocation -1 = not reported (driver_node < 0), 0 no-collocation,
+# 1 driver-collocated-with-all-executors, 2 driver-collocated-with-some-executors
+PLACEMENT_DTYPE = np.dtype([(f, np.int32 if t is C.c_int32 else np.int64) for f, t in gp_placement_record._fields_])
+COLLOCATION_TAGS = {0: "no-collocation", 1: "driver-collocated-with-all-executors", 2: "driver-collocated-with-some-executors"}
+
+
 class gp_stats(C.Structure):
     _fields_ = [("nodes_scanned", C.c_int64), ("drivers_tried", C.c_int64), ("kernel_launches", C.c_int64),
                 ("pack_kernel_ns", C.c_int64), ("prep_kernel_ns", C.c_int64), ("scan_path_apps", C.c_int64),
@@ -305,6 +316,12 @@ def load():
     L.gp_packing_efficiency_groups.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.c_int, C.POINTER(gp_results), C.c_int, C.c_void_p,
                                                C.c_int32, C.c_void_p]
     L.gp_exceeds_cluster_capacity.restype = C.c_int
+    L.gp_placement_metrics.restype = C.c_int
+    L.gp_placement_metrics.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_results), C.c_int32, C.c_void_p, C.c_int32,
+                                       C.c_void_p, C.c_int32, C.c_void_p]
+    L.gp_placement_metrics_device.restype = C.c_int
+    L.gp_placement_metrics_device.argtypes = [C.c_void_p, C.POINTER(gp_apps), C.POINTER(gp_results), C.c_int32, C.c_void_p,
+                                              C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.gp_exceeds_cluster_capacity.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.POINTER(gp_apps), C.c_int, C.c_void_p]
     L.gp_reconcile_find_nodes.restype = C.c_int
     L.gp_match_node_affinity.restype = C.c_int
@@ -947,6 +964,29 @@ class GangPacker:
                                                         int(n_instance_groups), _p(avg)))
         return avg[:q]
 
+    def placement_metrics(self, apps: dict, placed, metric_zone, instance_group=None, n_instance_groups: int = 1,
+                          n_metric_zones=None) -> np.ndarray:
+        """What selectDriverNode reports about each placed application besides its packing efficiency: driver-executor
+        collocation, executor node count and cross-zone pod pairs -> a PLACEMENT_DTYPE array of n_apps records.
+        apps: count, [group], [off]; placed = (driver_node, executor_nodes, off) as pack_batch returns them; metric_zone: the
+        interned failure-domain.beta.kubernetes.io/zone of each node (a missing label interned as "unknown-zone");
+        instance_group: each node's instance group, -1 = none (None: every node is in every row's scope); n_metric_zones
+        defaults to max(metric_zone) + 1."""
+        q = len(apps["count"])
+        driver, execn, off = placed
+        driver = _np(driver, np.int32); execn = _np(execn, np.int32)
+        if execn is None or len(execn) == 0:
+            execn = np.zeros(1, np.int32)
+        zone, ig = _np(metric_zone, np.int32), _np(instance_group, np.int32)
+        out = np.zeros(max(q, 1), PLACEMENT_DTYPE)
+        a = _apps(apps, off, group=apps.get("group"))
+        r = gp_results(driver_node=_p(driver), executor_nodes=_p(execn), executor_nodes_cap=len(execn))
+        if n_metric_zones is None:
+            n_metric_zones = int(zone.max()) + 1 if len(zone) else 0
+        self._check(load().gp_placement_metrics(self._h, C.byref(a), C.byref(r), len(zone), _p(zone), int(n_metric_zones), _p(ig),
+                                                 int(n_instance_groups), _p(out)))
+        return out[:q]
+
     def exceeds_cluster_capacity(self, alloc, apps: dict, packer: int, overhead=None, zone_id=None, n_zones=1, node_group=None,
                                  n_groups=1) -> np.ndarray:
         """DoesPodExceedClusterCapacity for a batch of stale drivers under one `binpack:` packer (BP_*), in one device call.
@@ -1143,6 +1183,20 @@ class GangPacker:
         r = gp_results(driver_node=driver_node.data_ptr(), executor_nodes=executor_nodes.data_ptr(),
                        executor_nodes_cap=executor_nodes.numel())
         self._check(load().gp_pack_batch_device(self._h, C.byref(a), algo, mode, C.byref(r), stream or None))
+
+    def placement_metrics_device(self, t: dict, driver_node, executor_nodes, metric_zone, out, n_metric_zones: int,
+                                 instance_group=None, n_instance_groups: int = 1, status=None, stream: int = 0):
+        """placement_metrics on torch CUDA tensors, e.g. pack_batch_device's inputs and outputs in place: t as there (count,
+        [group], [off]), out a uint8 tensor of PLACEMENT_DTYPE.itemsize * n_apps bytes (view it with PLACEMENT_DTYPE), status an int32 tensor of one
+        element receiving the call's status (0 = ok) once the work has run.  Asynchronous on `stream` (0 = the context's)."""
+        def dp(v):
+            return v.data_ptr() if v is not None else None
+        a = gp_apps(n_apps=t["count"].numel(), exe_count=dp(t["count"]), group=dp(t.get("group")), exec_out_off=dp(t.get("off")))
+        r = gp_results(driver_node=driver_node.data_ptr(), executor_nodes=executor_nodes.data_ptr(),
+                       executor_nodes_cap=executor_nodes.numel())
+        self._check(load().gp_placement_metrics_device(self._h, C.byref(a), C.byref(r), metric_zone.numel(), dp(metric_zone),
+                                                        int(n_metric_zones), dp(instance_group), int(n_instance_groups), dp(out),
+                                                        dp(status), stream or None))
 
 
 class MultiGangPacker:
