@@ -144,7 +144,7 @@ struct AppColumns {
 constexpr int kStatusWords = 32;
 
 // fingerprint of a (cpu, mem, gpu) request, never 0: the shape hashes of gp_decide_tables and gp_cc_intern
-__device__ __forceinline__ unsigned long long shape_fingerprint(int64_t a, int64_t b, int64_t c) {
+__host__ __device__ __forceinline__ unsigned long long shape_fingerprint(int64_t a, int64_t b, int64_t c) {
     unsigned long long z = (unsigned long long)a * 0x9E3779B97F4A7C15ull;
     z ^= ((unsigned long long)b + 0xBF58476D1CE4E5B9ull) * 0x94D049BB133111EBull;
     z ^= ((unsigned long long)c + 0x2545F4914F6CDD1Dull) * 0xD6E8FEB86659FD93ull;

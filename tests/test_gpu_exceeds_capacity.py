@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 
 import capacity_ref as cr
+import fingerprint_ref as fr
+from k8s_spark_scheduler_b200 import affinity as aff
 
 pytestmark = pytest.mark.gpu
 
@@ -343,37 +345,36 @@ def test_refusals(gangpack, packer):
     assert run().tolist() == [0]                          # the context still works after every refusal
 
 
-# ---- interning: drivers of one warp whose fingerprints collide ---------------------------------------------------------
-def _xor_fingerprint(q, g):
-    """the fingerprint an earlier form of gp_cc_intern used: F(exe) ^ F(drv0 ^ c, drv1 + g K, drv2), symmetric in the shapes"""
-    M = (1 << 64) - 1
-
-    def f(a, b, c):
-        z = (a * 0x9E3779B97F4A7C15) & M
-        z ^= (((b + 0xBF58476D1CE4E5B9) & M) * 0x94D049BB133111EB) & M
-        z ^= (((c + 0x2545F4914F6CDD1D) & M) * 0xD6E8FEB86659FD93) & M
-        z ^= z >> 29; z = (z * 0xBF58476D1CE4E5B9) & M; z ^= z >> 32
-        return z or 1
-    return f(q[3], q[4], q[5]) ^ f(q[0] ^ 0x5bd1e995, (q[1] + g * 0x632BE59BD9B4E019) & M, q[2])
-
-
+# ---- interning: drivers whose fingerprints collide -----------------------------------------------------------------------
 def test_same_fingerprint_in_one_warp(packer):
-    # A and B swap the executor shape with the transformed driver shape: equal fingerprints under the symmetric hash.  A's
-    # 100 GiB driver fits no 8 GiB node, B's 100 GiB executors are not needed (k = 0); interleaved, every warp holds both.
-    x = 1000 ^ 0x5bd1e995
-    A = (1000, 100 * GI, 0, x, 0, 0)
-    B = (1000, 0, 0, x, 100 * GI, 0)
-    assert _xor_fingerprint(A, 0) == _xor_fingerprint(B, 0)
-    q = 96
-    rows = [A if i % 3 else B for i in range(q)]
-    cols = list(zip(*rows))
-    apps = dict(drv_cpu=cols[0], drv_mem=cols[1], drv_gpu=cols[2], exe_cpu=cols[3], exe_mem=cols[4], exe_gpu=cols[5],
-                count=[0] * q, group=[0] * q)
-    alloc = [np.full(4, 8000), np.full(4, 8 * GI), np.zeros(4, np.int64)]
-    for name in cr.PACKERS:
-        got = packer.exceeds_cluster_capacity(alloc, apps, BP[name])
-        want = [1 if r is A else 0 for r in rows]                # B: driver 1 CPU > 0, so positive efficiency too
-        assert got.tolist() == want, name
+    # Rows whose chained fingerprints F(F(F(exe), drv cpu, drv mem), drv gpu, class) collide (tests/fingerprint_ref.py): A
+    # fits (answer 0); B (class 0, like A) and C (A's requests in another class) ask for 2^50 or more driver GPUs (answer
+    # 1), so a row given another row's pair flips its answer.  A and B interleaved inside warps: the multi-round match loop;
+    # in warps and CTAs of their own: a probe passing an entry of equal fingerprint and another tuple.
+    A, B, C, ga, gc = fr.marker_rows()
+    assert fr.marker_fingerprint(A, 0) == fr.marker_fingerprint(B, 0) and fr.marker_fingerprint(A, ga) == fr.marker_fingerprint(C, gc)
+    n_groups = max(ga, gc) + 1
+    n = 4 * n_groups
+    alloc = [np.full(n, 8000), np.full(n, 8 * GI), np.zeros(n, np.int64)]
+    group = (np.arange(n) % n_groups).astype(np.int32)
+    zone = np.zeros(n, np.int32)
+    nodes = [{"name": f"n{i}", "labels": {"ig": f"g{group[i]}"}} for i in range(n)]
+    enc = aff.encode(nodes, [{"nodeSelector": {"ig": f"g{k}"}} for k in range(n_groups)])
+    within = [(A, 0) if i % 3 else (B, 0) for i in range(96)]
+    across = [(B, 0) if i // 256 == 0 or (i // 32) % 2 else (A, 0) for i in range(1024)]
+    classes = [[(A, ga), (C, gc), (A, gc)][i % 3] for i in range(96)] + [(C, gc)] * 64 + [(A, ga)] * 64
+    for rows in (within, across, classes):
+        cols = list(zip(*[r for r, _ in rows]))
+        apps = dict(drv_cpu=cols[0], drv_mem=cols[1], drv_gpu=cols[2], exe_cpu=cols[3], exe_mem=cols[4], exe_gpu=cols[5],
+                    count=np.full(len(rows), 3, np.int32), group=np.array([g for _, g in rows], np.int32))
+        apps = {k: np.asarray(v) for k, v in apps.items()}
+        cache = class_terms(alloc, [np.zeros(n, np.int64)] * 3, zone, 1, group, apps)
+        want = [0 if r == A else 1 for r, _ in rows]
+        for name in cr.PACKERS:
+            assert model_all(name, apps, cache).tolist() == want, name
+            assert call(packer, alloc, None, zone, 1, group, n_groups, apps, name).tolist() == want, name
+            got, err = packer.exceeds_cluster_capacity_affinity(alloc, enc, apps, BP[name], zone_id=zone)
+            assert not err.any() and got.tolist() == want, name
 
 
 # ---- buckets of more than one segment (4 096 nodes) and one zone per node ----------------------------------------------
