@@ -343,9 +343,6 @@ Snapshot make_snapshot(const gp_ctx* c) {
 gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, cudaStream_t st,
                                 bool copy_nodes) {
     const int32_t n_slots = n_exec + n_drv;
-    c->host_layout = false;              // gp_set_snapshot sets it again once the layout it validated is in place
-    c->zone_kind = -1;                   // gp_prepare_cluster_zones* set it again once their layout is in place
-    c->zone_igs = 0;
     GP_CUDA(c, c->pair.reserve(sizeof(longlong2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->pair32.reserve(sizeof(uint2) * (size_t)(n_slots + 1)));
     GP_CUDA(c, c->sgpu.reserve(sizeof(int64_t) * (size_t)(n_slots + 1)));
@@ -384,9 +381,6 @@ gp_status build_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, i
     });
     if (rs != GP_OK) return rs;
     c->n_nodes = dn->n_nodes; c->n_groups = dn->n_groups; c->n_exec = n_exec; c->n_drv = n_drv; c->n_slots = n_slots;
-    c->have_snapshot = true;
-    c->have_sched = false;               // SchedulableResources belong to a node table
-    c->have_eff_sched = false;
     return GP_OK;
 }
 
@@ -504,8 +498,7 @@ gp_status gp_synchronize(gp_ctx* ctx) {
 }
 
 gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!n || n->n_nodes < 0 || n->n_groups < 1 || !n->exec_off || !n->drv_off ||
         (n->n_nodes > 0 && (!n->avail_cpu_milli || !n->avail_mem_bytes)))
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot: missing arrays or bad sizes");
@@ -520,7 +513,7 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot: order arrays missing");
     {
         // owner[v] = 4 * group + (bit0: listed as executor candidate, bit1: listed as driver candidate); -1 = unseen
-        c->host_layout = false;
+        c->held.host_copy_overwritten();
         std::vector<int32_t>& owner = c->v_owner;
         owner.assign((size_t)n->n_nodes, -1);
         const uint32_t N = (uint32_t)n->n_nodes;
@@ -556,6 +549,7 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
         }
         if (out_of_domain) return fail(c, GP_ERR_UNREPRESENTABLE, "gp_set_snapshot: |quantity| >= 2^61");
     }
+    c->held.commit();
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t nb = sizeof(int64_t) * (size_t)(n->n_nodes + 1);
@@ -603,9 +597,8 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
     dn.avail_gpu = c->node_gpu.as<int64_t>();
     dn.exec_off = c->exec_off.as<int32_t>(); dn.drv_off = c->drv_off.as<int32_t>();
     dn.exec_order = c->exec_order.as<int32_t>(); dn.drv_order = c->drv_order.as<int32_t>();
-    gp_status s = build_snapshot_device(c, &dn, n_exec, n_drv, st);
-    if (s != GP_OK) return s;
-    c->host_layout = true;
+    GP_TRY(build_snapshot_device(c, &dn, n_exec, n_drv, st));
+    c->held.laid_out_snapshot();
     // GP_CFG_ASYNC_SNAPSHOT with page-locked inputs: return while the device is still reading them -- the upload and the
     // slot layout then overlap the H2D copies of the gp_pack_* call that follows
     if (!(c->async_snapshot && all_mapped)) GP_CUDA(c, cudaStreamSynchronize(st));   // the caller may reuse its host buffers
@@ -613,25 +606,24 @@ gp_status gp_set_snapshot(gp_ctx* c, const gp_nodes* n) {
 }
 
 gp_status gp_set_snapshot_device(gp_ctx* c, const gp_nodes* dn, int32_t n_exec, int32_t n_drv, void* stream) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!dn || dn->n_nodes < 0 || dn->n_groups < 1 || !dn->exec_off || !dn->drv_off || n_exec < 0 || n_drv < 0 ||
         (n_exec > 0 && !dn->exec_order) || (n_drv > 0 && !dn->drv_order))
         return fail(c, GP_ERR_INVALID, "gp_set_snapshot_device: missing arrays or bad sizes");
+    c->held.commit();
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : c->stream;
     // keep a node-table copy so gp_get_snapshot can answer for nodes outside every group: the layout kernel makes it
     const size_t nb = sizeof(int64_t) * (size_t)(dn->n_nodes + 1);
     GP_CUDA(c, c->node_cpu.reserve(nb)); GP_CUDA(c, c->node_mem.reserve(nb)); GP_CUDA(c, c->node_gpu.reserve(nb));
-    const gp_status s = build_snapshot_device(c, dn, n_exec, n_drv, st, dn->n_nodes > 0);
-    if (s == GP_OK && c->async_snapshot) c->layout_tail = st;      // the layout is the last work on st
-    return s;
+    GP_TRY(build_snapshot_device(c, dn, n_exec, n_drv, st, dn->n_nodes > 0));
+    c->held.laid_out_device(c->async_snapshot ? st : nullptr);      // the layout is the last work on st
+    return GP_OK;
 }
 
 gp_status gp_get_snapshot(gp_ctx* c, int64_t* cpu, int64_t* mem, int64_t* gpu) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_get_snapshot: no snapshot");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot("no snapshot"), "gp_get_snapshot"));
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const int T = 256;

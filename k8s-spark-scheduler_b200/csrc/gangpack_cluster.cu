@@ -305,6 +305,7 @@ static gp_status prepare_groups(gp_ctx* c, const gp_usage_input* usage, const gp
     long long *d_avail = nullptr, *d_sched = nullptr;
     SortStage so{};
     GP_TRY(prepare_orders(c, usage, sort, ig, ig ? n_ig : 1, who, &d_avail, &d_sched, &so));
+    c->held.commit();
     cudaStream_t st = c->stream;
     const size_t G1 = (size_t)n_ig + 1;
     GP_CUDA(c, c->exec_off.reserve(4 * G1)); GP_CUDA(c, c->drv_off.reserve(4 * G1));
@@ -325,7 +326,7 @@ static gp_status prepare_groups(gp_ctx* c, const gp_usage_input* usage, const gp
         ig_ties[0] = counts[2];
     }
     c->n_drv = counts[0]; c->n_exec = counts[1];
-    c->have_eff_sched = true;           // SchedulableResources for gp_packing_efficiency (the zone entry points still want gp_set_schedulable)
+    c->held.laid_out_cluster();
     if (sort->undefined_ties) *sort->undefined_ties = counts[2];
     if (so_out) *so_out = so;
     return GP_OK;
@@ -357,11 +358,12 @@ static gp_status availability_out(gp_ctx* c, const gp_usage_input* in, bool firs
     return GP_OK;
 }
 
-// What prepare_zones leaves for its entry: the sort's counts[3], the ZoneInfo words and the device zone_of_group.
+// What prepare_zones leaves for its entry: the sort's counts[3], the ZoneInfo words, the device zone_of_group, the IgWords read back.
 struct ZonePrep {
     int32_t counts[3];
     int32_t info[kZiWords];
     const int32_t* zone_of_group;
+    std::vector<int32_t> ig_words;
 };
 
 // gp_prepare_cluster_zones (ig NULL, n_ig 1) and gp_prepare_cluster_zones_groups up to their optional outputs: the checks,
@@ -369,8 +371,7 @@ struct ZonePrep {
 // before anything of the context is replaced) -> the zone-grouped layout (gangpack_zonelayout.cuh) -> the slot layout, then
 // one synchronise that reads back the counts.  zog_now (or NULL): zone_of_group [sort->n_zones + 1] read back in that
 // synchronise; ig_ties (or NULL): the undefined ties [n_ig] likewise.  keep_ig (gp_prepare_cluster_zones_groups): the
-// per-instance-group words (group_off, n_zones, undivided exec_off / drv_off) are kept on the host (zone_ig_words) and
-// zone_igs = n_ig.  ig NULL with n_ig > 1: every node in instance group 0, the others empty.
+// per-instance-group words are held (Held::groups).  ig NULL with n_ig > 1: every node in instance group 0, the others empty.
 static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
                                int32_t kind, bool keep_ig, const char* who, int32_t* zog_now, int32_t* ig_ties, ZonePrep* zp) {
     if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
@@ -379,9 +380,8 @@ static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_
     long long *d_avail = nullptr, *d_sched = nullptr;
     SortStage so{};
     GP_TRY(prepare_orders(c, usage, sort, ig, n_ig, who, &d_avail, &d_sched, &so));
+    c->held.commit();                                   // the held orders are overwritten below
     cudaStream_t st = c->stream;
-    c->zone_kind = -1;                                  // the held orders are overwritten below
-    c->zone_igs = 0;
     const int32_t n = usage->n_nodes;
     const size_t N = (size_t)n, G1 = (size_t)n_ig + 1;
     // the (instance group, zone) pairs; g_bound groups bound every layout (each instance group: its candidate zones plus
@@ -438,10 +438,8 @@ static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_
     GP_TRY(prepare_snapshot(c, &dn, d_avail, d_sched, so, zp->counts));
     ar.get(zp->info, info_p);
     ar.get(zog_now, zog.part(0, (size_t)sort->n_zones + 1));
-    if (keep_ig) {
-        c->zone_ig_words.resize(4 * G1);
-        ar.get(c->zone_ig_words.data(), wb, 4 * G1);
-    }
+    zp->ig_words.resize(4 * G1);
+    ar.get(zp->ig_words.data(), wb, 4 * G1);
     if (so.ig_ties) ar.get(ig_ties, so.ig_ties, (size_t)n_ig);
     GP_TRY(ar.sync(c));
     if (!so.ig_ties && ig_ties) {                       // one instance group holds every node: its ties are the total
@@ -449,11 +447,7 @@ static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_
         ig_ties[0] = zp->counts[2];
     }
     c->n_groups = zp->info[kZiGroups]; c->n_exec = zp->info[kZiExec]; c->n_drv = zp->info[kZiDrv];
-    c->have_sched = true;
-    c->have_eff_sched = true;
-    c->zone_orders = gp_az_orders{zp->info[kZiZones], zp->counts[1], uexe, zp->counts[0], udrv};
-    c->zone_kind = kind;
-    if (keep_ig) c->zone_igs = n_ig;
+    c->held.laid_out_zones(kind, gp_az_orders{zp->info[kZiZones], zp->counts[1], uexe, zp->counts[0], udrv}, keep_ig ? n_ig : 0, zp->ig_words.data());
     zp->zone_of_group = ar.ptr(zog);
     return GP_OK;
 }
@@ -462,8 +456,7 @@ extern "C" {
 
 gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver_order, int32_t* n_driver,
                              int32_t* executor_order, int32_t* n_executor) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!in || in->n_nodes < 0 || in->n_zones < 1 || !n_driver || !n_executor ||
         (in->n_nodes > 0 && (!in->avail_cpu_milli || !in->avail_mem_bytes || !driver_order || !executor_order)))
         return fail(c, GP_ERR_INVALID, "gp_potential_nodes: missing arrays or bad sizes");
@@ -490,24 +483,21 @@ gp_status gp_potential_nodes(gp_ctx* c, const gp_sort_input* in, int32_t* driver
 
 gp_status gp_build_availability(gp_ctx* c, const gp_usage_input* in, int64_t* avail_cpu, int64_t* avail_mem, int64_t* avail_gpu,
                                 int64_t* sched_cpu, int64_t* sched_mem, int64_t* sched_gpu) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     int64_t* const outs[6] = {avail_cpu, avail_mem, avail_gpu, sched_cpu, sched_mem, sched_gpu};
     return availability_out(c, in, false, outs, "gp_build_availability");
 }
 
 // availableResources of rescheduleExecutor's first-fit branch: the availability to upload before gp_reschedule_executors(min_frag = 0)
 gp_status gp_build_reschedule_availability(gp_ctx* c, const gp_usage_input* in, int64_t* avail_cpu, int64_t* avail_mem, int64_t* avail_gpu) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     int64_t* const outs[6] = {avail_cpu, avail_mem, avail_gpu, nullptr, nullptr, nullptr};
     return availability_out(c, in, true, outs, "gp_build_reschedule_availability");
 }
 
 // reservations -> availability -> priority orders -> slot layout, without leaving the device
 gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, int32_t* n_driver, int32_t* n_executor) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (n_driver) *n_driver = 0;
     if (n_executor) *n_executor = 0;
     int32_t counts[3] = {0, 0, 0};
@@ -521,8 +511,7 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
 gp_status gp_prepare_cluster_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
                                     int32_t n_instance_groups, gp_instance_group_orders* out) {
     const char* who = "gp_prepare_cluster_groups";
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!out) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     out->n_driver = 0; out->n_executor = 0;
     const int32_t G = n_instance_groups;
@@ -546,8 +535,7 @@ gp_status gp_prepare_cluster_groups(gp_ctx* c, const gp_usage_input* usage, cons
 // reservations -> availability -> priority orders -> zone-grouped slot layout, without leaving the device
 gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, gp_zone_layout* layout) {
     const char* who = "gp_prepare_cluster_zones";
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!layout) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     layout->n_zones = 0; layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
     ZonePrep zp{};
@@ -570,8 +558,7 @@ gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const
 gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
                                           int32_t n_instance_groups, gp_instance_group_layout* layout) {
     const char* who = "gp_prepare_cluster_zones_groups";
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!layout) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
     const int32_t G = n_instance_groups;
@@ -583,15 +570,15 @@ gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage
     layout->n_groups = n_groups; layout->n_driver = zp.counts[0]; layout->n_executor = zp.counts[1];
     // the per-instance-group words are on the host already; the rest only when asked
     const size_t g1 = (size_t)G + 1;
-    const int32_t* words = c->zone_ig_words.data();
-    if (layout->group_off) std::copy(words, words + g1, layout->group_off);
-    if (layout->n_zones) std::copy(words + g1, words + g1 + G, layout->n_zones);
-    if (layout->exec_off) std::copy(words + 2 * g1, words + 3 * g1, layout->exec_off);
-    if (layout->drv_off) std::copy(words + 3 * g1, words + 4 * g1, layout->drv_off);
+    const gp_instance_groups held = c->held.groups();
+    if (layout->group_off) std::copy(held.group_off, held.group_off + g1, layout->group_off);
+    if (layout->n_zones) std::copy(held.n_zones, held.n_zones + G, layout->n_zones);
+    if (layout->exec_off) std::copy(held.exec_off, held.exec_off + g1, layout->exec_off);
+    if (layout->drv_off) std::copy(held.drv_off, held.drv_off + g1, layout->drv_off);
     Arena ar{c->zoneprep, c->stream};
     const size_t n_off = (size_t)n_groups + 1;
-    ar.get(layout->exec_order, c->zone_orders.exec_order, (size_t)zp.counts[1]);
-    ar.get(layout->drv_order, c->zone_orders.drv_order, (size_t)zp.counts[0]);
+    ar.get(layout->exec_order, held.exec_order, (size_t)zp.counts[1]);
+    ar.get(layout->drv_order, held.drv_order, (size_t)zp.counts[0]);
     ar.get(layout->group_exec_off, c->exec_off.as<int32_t>(), n_off);
     ar.get(layout->group_drv_off, c->drv_off.as<int32_t>(), n_off);
     ar.get(layout->group_exec_order, c->exec_order.as<int32_t>(), (size_t)c->n_exec);
@@ -605,9 +592,8 @@ gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage
 
 // rescheduleExecutor's node choice for a batch of executors (SURVEY 8f row f4); see gangpack_resched.cuh
 gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* node_out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_reschedule_executors: gp_set_snapshot first");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), "gp_reschedule_executors"));
     if (!in || in->n_execs < 0 || (in->n_execs > 0 && (!in->exe_cpu_milli || !in->exe_mem_bytes || !node_out)))
         return fail(c, GP_ERR_INVALID, "gp_reschedule_executors: missing arrays or bad sizes");
     const int32_t q = in->n_execs;
@@ -675,8 +661,7 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
 // rescheduleExecutor from the reservations to the node choice (SURVEY 8f row f4); see gangpack_reschedprep.cuh
 gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const gp_reschedule_scope* scope,
                                           const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_reschedule_from_reservations";
     GP_TRY(check_usage(c, usage, who));
     if (!sort || !in || usage->n_nodes != sort->n_nodes || sort->n_zones < 1 ||
@@ -773,8 +758,7 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
 // gangpack_reconcile.cuh and DESIGN §2.3
 gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
                                   gp_reconcile_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_reconcile_find_nodes";
     GP_TRY(check_usage(c, usage, who));
     if (!nodes || !a || !out || nodes->n_groups < 1 || a->n_apps < 0 || (usage->n_nodes > 0 && (!nodes->node_group || !nodes->creation)) ||

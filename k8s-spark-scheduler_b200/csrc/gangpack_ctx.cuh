@@ -4,6 +4,7 @@
 #pragma once
 
 #include "gangpack.h"
+#include "gangpack_held.cuh"
 #include "gangpack_kernels.cuh"
 
 #include <cstddef>
@@ -147,7 +148,7 @@ struct gp_ctx {
     std::string err;
 
     // snapshot
-    bool have_snapshot = false;
+    Held held;
     int32_t n_nodes = 0, n_groups = 0, n_exec = 0, n_drv = 0, n_slots = 0;
     DevBuf node_cpu, node_mem, node_gpu;        // node-table order (as given)
     DevBuf exec_off, drv_off, exec_order, drv_order;
@@ -164,12 +165,9 @@ struct gp_ctx {
     PinnedStatus* host_status() const { return static_cast<PinnedStatus*>(pinned_misc); }
     std::vector<int64_t> host_off;
     std::vector<int32_t> eff_seg;                 // gp_packing_efficiency_groups: seg_off [G + 1], then the bucketed nodes
-    std::vector<int32_t> v_owner;                 // gp_set_snapshot validation scratch (no per-call allocation)
-    // gp_set_snapshot's host copy of the layout, kept for gp_pack_fifo_az_aware's order checks: v_owner[v] (group, roles)
-    // and v_pos[v] / v_pos[n_nodes + v] (position of v in its group's executor / driver order).  host_layout: they
-    // describe the current snapshot (false after gp_set_snapshot_device / gp_prepare_cluster or a refused gp_set_snapshot)
-    std::vector<int32_t> v_pos;
-    bool host_layout = false;
+    // gp_set_snapshot's host copy of the layout (Held::host_copy), kept for the az-aware order checks: v_owner[v] (group,
+    // roles) and v_pos[v] / v_pos[n_nodes + v] (position of v in its group's executor / driver order)
+    std::vector<int32_t> v_owner, v_pos;
     std::vector<uint8_t> v_seen_e, v_seen_d;
     std::vector<int32_t> v_zone_next;             // az-aware order check: next position per zone group
     std::vector<ZoneFifoGroup> zone_groups;       // zone FIFO: per instance group its zones, queue range and scratch rows
@@ -182,10 +180,6 @@ struct gp_ctx {
     int use_tables = 1;                           // GANGPACK_TABLES=0: every independent decision takes the node-order scan
     int fifo_warp = 1;                            // GANGPACK_FIFO_WARP=0: every FIFO application is decided by the whole CTA
     bool async_snapshot = false;                  // gp_config.flags & GP_CFG_ASYNC_SNAPSHOT
-    // With async_snapshot: the stream on which the context's last call, gp_set_snapshot_device, enqueued the slot layout
-    // (nullptr: none).  Every other entry point that enqueues device work clears it.  While it is set, a
-    // gp_pack_batch_device on that stream may start its gp_decide_tables before the layout ends (pack_device_range).
-    cudaStream_t layout_tail = nullptr;
     int chunk_apps = kChunkApps;                  // GANGPACK_CHUNK_APPS
     int trace = 0;                                // GANGPACK_TRACE=1: host-side phase timing on stderr
     int pack_ctas_per_sm = 0;                       // occupancy of gp_pack_independent<2> on this device
@@ -202,14 +196,7 @@ struct gp_ctx {
     DevBuf fifo_list;                             // FIFO modes: per-instance-group application lists (queue order)
     DevBuf sched, zonebuf, fbview;                // SchedulableResources [3][n_nodes]; staging of the zone entry points;
                                                   // the az-aware fallback's orders and gather view
-    bool have_sched = false;
-    // SchedulableResources for gp_packing_efficiency alone: also set by gp_prepare_cluster, whose one-group snapshot the zone
-    // entry points keep refusing (have_sched stays false there)
-    bool have_eff_sched = false;
-    // gp_prepare_cluster_zones: the undivided orders it sorted (in zoneprep, which also holds that call's scratch), their
-    // lengths and n_zones as DEVICE pointers for gp_pack_*_az_aware(orders == NULL); zone_kind = the gp_zone_layout_kind of the
-    // current snapshot, -1 when another entry laid it out
-    DevBuf zoneprep;
+    DevBuf zoneprep;                              // gp_prepare_cluster_zones*: the undivided orders (Held::orders) and scratch
     // The own scratch of one call of gp_reschedule_executors, gp_reschedule_from_reservations, gp_exceeds_cluster_capacity*,
     // gp_match_node_affinity, gp_reconcile_find_nodes or gp_node_overhead: no state points into it, and the next call's
     // use is ordered after this one's kernels on the context's stream
@@ -220,14 +207,6 @@ struct gp_ctx {
     DevBuf metricbuf, metricstate;
     std::vector<gp_placement_record> pm_records;
     int pm_smem_limit = 0;
-    int zone_kind = -1;
-    gp_az_orders zone_orders{};
-    // gp_prepare_cluster_zones_groups: zone_igs = its n_instance_groups while its layout is held (0 otherwise, also after
-    // gp_prepare_cluster_zones), and zone_ig_words its per-instance-group words read back by that call, [n + 1] each:
-    // group_off, n_zones (n used), undivided exec_off, undivided drv_off -- what gp_pack_fifo_zones_groups(groups == NULL)
-    // builds its descriptors from
-    int32_t zone_igs = 0;
-    std::vector<int32_t> zone_ig_words;
     bool sort_attr_set = false;
     bool recon_attr_set = false;                  // dynamic shared-memory opt-in of gp_sort_tiles<ReconKey> done on this device
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
@@ -254,6 +233,17 @@ gp_status fail(gp_ctx* ctx, gp_status st, const std::string& msg);
 static inline gp_status fail(gp_ctx* c, gp_status st, const char* who, const char* what) {
     return fail(c, st, std::string(who) + ": " + what);
 }
+
+// The prologue of the C ABI entries that enqueue device work: false for a NULL context; takes the tail (into *tail if given)
+static inline bool enter(gp_ctx* c, const void** tail = nullptr) {
+    const void* t = c ? c->held.take_tail() : nullptr;
+    if (tail) *tail = t;
+    return c != nullptr;
+}
+
+// GP_OK when the requirements are met, otherwise the first one's refusal as `who: what`
+static inline gp_status require(gp_ctx* c, Need n, const char* who) { return n.status == GP_OK ? GP_OK : fail(c, n.status, who, n.what); }
+static inline gp_status require(gp_ctx* c, Need a, Need b, const char* who) { return a.status != GP_OK ? require(c, a, who) : require(c, b, who); }
 
 inline gp_status Arena::check(gp_ctx* c) const {
     if (!err) return GP_OK;

@@ -269,8 +269,7 @@ extern "C" {
 // DoesPodExceedClusterCapacity for a batch of stale drivers, any packer (EXT/unschedulablepods.go:132-166); see
 // gangpack_capacity.cuh and DESIGN §2.2
 gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     return capacity_run(c, "gp_exceeds_cluster_capacity", nodes, nullptr, nullptr, a, packer, exceeds, nullptr);
 }
 
@@ -278,8 +277,7 @@ gp_status gp_exceeds_cluster_capacity(gp_ctx* c, const gp_capacity_nodes* nodes,
 gp_status gp_exceeds_cluster_capacity_affinity(gp_ctx* c, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
                                                const gp_node_affinities* affinities, const gp_apps* a, gp_binpacker packer,
                                                uint8_t* exceeds, uint8_t* affinity_error) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_exceeds_cluster_capacity_affinity";
     if (!affinities) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
     return capacity_run(c, who, nodes, labels, affinities, a, packer, exceeds, affinity_error);
@@ -287,8 +285,7 @@ gp_status gp_exceeds_cluster_capacity_affinity(gp_ctx* c, const gp_capacity_node
 
 // GetRequiredNodeAffinity(...).Match for every (affinity, node); see gangpack_affinity.cuh
 gp_status gp_match_node_affinity(gp_ctx* c, const gp_node_labels* labels, const gp_node_affinities* affinities, gp_affinity_match* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_match_node_affinity";
     gp_status s = check_affinity(c, labels, affinities, who);
     if (s != GP_OK) return s;
@@ -325,8 +322,7 @@ static const Refusal kOhRefusals[] = {
 // The overhead computer's per-call side (EXT/overhead.go:105-153) for a list of nodes; see gangpack_overhead.cuh
 gp_status gp_node_overhead(gp_ctx* c, const gp_overhead_pods* p, const gp_overhead_reservations* r, int32_t n_nodes,
                            const int32_t* node_ids, gp_overhead_out* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_node_overhead";
     if (!p || !r || !out || p->n_pods < 0 || p->n_node_ids < 0 || p->n_app_keys < 0 || p->n_app_ids < 0 || p->n_names < 0 ||
         r->n_rr < 0 || r->n_soft < 0 || n_nodes < 0 || (n_nodes > 0 && !node_ids) ||

@@ -217,7 +217,7 @@ static gp_status launch_tables(gp_ctx* c, const Snapshot& s, const AppColumns& c
 // off_base: ExecutorNodes offset of application `lo` (only used when the offsets are derived on the device).
 // status_in_kernel: pack_begin left the status block to this range's decide kernel (kernel_zeroes_status(), one range only).
 // after_layout: the last work on st is this context's slot layout, and the caller's inputs were ready before it was
-// enqueued (gp_ctx::layout_tail).
+// enqueued (Held::take_tail).
 gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi, int64_t off_base, gp_algo algo, gp_mode mode,
                             const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel, bool after_layout) {
     const int32_t q = hi - lo;
@@ -361,7 +361,7 @@ gp_status pack_begin(gp_ctx* c, int32_t q, gp_algo algo, gp_mode mode, int64_t e
 }
 
 static gp_status check_args(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, const gp_results_wire* out, const char* who) {
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, std::string(who) + ": gp_set_snapshot first");
+    GP_TRY(require(c, c->held.snapshot(), who));
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, std::string(who) + ": NULL apps/results");
     if (algo != GP_TIGHTLY_PACK && algo != GP_DISTRIBUTE_EVENLY && algo != GP_MINIMAL_FRAGMENTATION)
         return fail(c, GP_ERR_INVALID, std::string(who) + ": unknown algo");
@@ -415,9 +415,8 @@ static gp_apps_wire widen(const gp_apps* a) {
 extern "C" {
 
 gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mode mode, gp_results* dout, void* stream) {
-    if (!c) return GP_ERR_INVALID;
-    const cudaStream_t layout_tail = c->layout_tail;
-    c->layout_tail = nullptr;
+    const void* layout_tail = nullptr;
+    if (!enter(c, &layout_tail)) return GP_ERR_INVALID;
     if (!da || !dout) return fail(c, GP_ERR_INVALID, "gp_pack_batch_device: NULL apps/results");
     const gp_apps_wire w = widen(da);
     gp_results_wire ow{dout->driver_node, dout->executor_nodes, dout->executor_nodes_cap, 32, 0};
@@ -442,8 +441,7 @@ gp_status gp_pack_batch_device(gp_ctx* c, const gp_apps* da, gp_algo algo, gp_mo
 }
 
 gp_status gp_last_stats(gp_ctx* c, gp_stats* out) {
-    if (!c || !out) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!out || !enter(c)) return GP_ERR_INVALID;
     GP_CUDA(c, cudaSetDevice(c->device));
     StatusHead& h = c->host_status()->head;
     GP_CUDA(c, cudaMemcpyAsync(&h, &c->status()->head, sizeof(StatusHead), cudaMemcpyDeviceToHost, c->stream));
@@ -471,8 +469,7 @@ int64_t gp_decide_timeline(gp_ctx* c, void* out, int64_t bytes) {
 static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, gp_results_wire* out);
 
 gp_status gp_pack_batch_wire(gp_ctx* c, const gp_apps_wire* a, gp_algo algo, gp_mode mode, gp_results_wire* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     gp_status s = pack_batch_impl(c, a, algo, mode, out);
     if (s != GP_OK) {
         // Whatever was enqueued before the failure may still read the caller's buffers or write its results:
@@ -675,8 +672,7 @@ static gp_status pack_batch_impl(gp_ctx* c, const gp_apps_wire* a, gp_algo algo,
 gp_status gp_pack_one(gp_ctx* c, gp_algo algo, int64_t drv_cpu, int64_t drv_mem, int64_t drv_gpu, int64_t exe_cpu,
                       int64_t exe_mem, int64_t exe_gpu, int32_t exe_count, int32_t* has_capacity, int32_t* driver_node,
                       int32_t* executor_nodes) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!has_capacity || !driver_node) return fail(c, GP_ERR_INVALID, "gp_pack_one: NULL outputs");
     if (exe_count > 0 && !executor_nodes) return fail(c, GP_ERR_INVALID, "gp_pack_one: executor_nodes is NULL");
     // The tuple and the result travel through a context-owned mapped pinned block: no DMA copies at all

@@ -99,8 +99,7 @@ extern "C" {
 
 gp_status gp_placement_metrics(gp_ctx* c, const gp_apps* a, const gp_results* placed, int32_t N, const int32_t* zone, int32_t Z,
                                const int32_t* ig, int32_t G, gp_placement_record* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     const char* who = "gp_placement_metrics";
     GP_TRY(pm_check(c, a, placed, N, zone, Z, ig, G, out, who));
     const int32_t Q = a->n_apps;
@@ -167,8 +166,7 @@ gp_status gp_placement_metrics(gp_ctx* c, const gp_apps* a, const gp_results* pl
 
 gp_status gp_placement_metrics_device(gp_ctx* c, const gp_apps* da, const gp_results* dp, int32_t N, const int32_t* zone, int32_t Z,
                                       const int32_t* ig, int32_t G, gp_placement_record* dout, int32_t* dev_status, void* stream) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     const char* who = "gp_placement_metrics_device";
     GP_TRY(pm_check(c, da, dp, N, zone, Z, ig, G, dout, who));
     GP_CUDA(c, cudaSetDevice(c->device));

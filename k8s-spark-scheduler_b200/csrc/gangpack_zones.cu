@@ -14,9 +14,8 @@ extern "C" {
 
 // ---- single-AZ packers: pack every zone, choose by packing efficiency on the device (gangpack_zones.cuh) ----------
 gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, const int64_t* gpu) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_set_schedulable: gp_set_snapshot first");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), "gp_set_schedulable"));
     if (c->n_nodes > 0 && (!cpu || !mem)) return fail(c, GP_ERR_INVALID, "gp_set_schedulable: missing arrays");
     GP_CUDA(c, cudaSetDevice(c->device));
     const size_t N = (size_t)c->n_nodes;
@@ -31,8 +30,7 @@ gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, 
     ar.put(sched.part(N, N), mem);
     ar.put_or_zero(sched.part(2 * N, N), gpu);
     GP_TRY(ar.sync(c));
-    c->have_sched = true;
-    c->have_eff_sched = true;
+    c->held.schedulable_set();
     return GP_OK;
 }
 
@@ -40,15 +38,6 @@ gp_status gp_set_schedulable(gp_ctx* c, const int64_t* cpu, const int64_t* mem, 
 // the arrays a non-empty batch of a zone entry point needs
 static bool has_zone_arrays(const gp_apps* a, const gp_zone_results* out) {
     return a->drv_cpu_milli && a->drv_mem_bytes && a->exe_cpu_milli && a->exe_mem_bytes && a->exe_count && out->zone && out->driver_node;
-}
-
-// The single-instance-group zone entries read the whole snapshot as one instance group's zones: refused while it holds the
-// layout of gp_prepare_cluster_zones_groups over several instance groups.
-static gp_status one_instance_group(gp_ctx* c, const char* who) {
-    if (c->zone_igs > 1)
-        return fail(c, GP_ERR_INVALID, who, "the snapshot holds several instance groups (gp_prepare_cluster_zones_groups): drain them "
-                                            "with gp_pack_fifo_zones_groups(groups == NULL)");
-    return GP_OK;
 }
 
 // Uploads the six int64 quantity columns (6 x n_apps of `in`; absent gpu columns stay NULL = 0 in the result), exe_count
@@ -216,14 +205,12 @@ static gp_status batch_zones_run(gp_ctx* c, const gp_apps* a, gp_algo algo, int3
 }
 
 gp_status gp_pack_batch_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_zone_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_zones: gp_set_snapshot first");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), c->held.full_sched(), "gp_pack_batch_zones"));
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: NULL apps/results");
     if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
         return fail(c, GP_ERR_INVALID, "gp_pack_batch_zones: the single-AZ packers are tightly-pack and minimal-fragmentation (single_az_pack_tightly.go, single_az_minimal_fragmentation.go)");
-    GP_TRY(one_instance_group(c, "gp_pack_batch_zones"));
+    GP_TRY(require(c, c->held.one_instance_group(), "gp_pack_batch_zones"));
     return batch_zones_run(c, a, algo, c->n_groups, nullptr, false, out, "gp_pack_batch_zones");
 }
 
@@ -245,10 +232,8 @@ static gp_status refresh_views(gp_ctx* c, cudaStream_t st) {
 // that group's nodes (the fallback and the zone packs must see the same priorities).  ig.group_off and ig.n_zones are
 // already checked; ig.exec_off / ig.drv_off are present.
 static gp_status check_az_orders(gp_ctx* c, const gp_instance_groups& ig, const char* who) {
+    GP_TRY(require(c, c->held.host_copy(false), who));
     const std::string w(who);
-    if (!c->host_layout)
-        return fail(c, GP_ERR_INVALID, w + ": the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
-                                           "gp_prepare_cluster there is no host copy of the layout to check the undivided orders against)");
     const int32_t G = ig.n_instance_groups;
     if (ig.exec_off[G] != c->n_exec || ig.drv_off[G] != c->n_drv)
         return fail(c, GP_ERR_INVALID, w + ": order lengths must equal the snapshot's exec_off[n_groups] / drv_off[n_groups]");
@@ -295,12 +280,9 @@ static gp_status check_az_orders(gp_ctx* c, const gp_instance_groups& ig, const 
 // The az-aware entries' NULL arguments.  orders == NULL stands for the undivided orders and n_zones gp_prepare_cluster_zones
 // (GP_LAYOUT_AZ_AWARE) left on the device -- *o then points at them; after any other snapshot it is refused.
 static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_results* out, const gp_az_orders** o, const char* who) {
-    if (!*o) GP_TRY(one_instance_group(c, who));
-    if (!*o && c->zone_kind == GP_LAYOUT_SINGLE_AZ)
-        return fail(c, GP_ERR_INVALID, who, "orders == NULL needs a gp_prepare_cluster_zones(GP_LAYOUT_AZ_AWARE) snapshot; this one is "
-                                           "GP_LAYOUT_SINGLE_AZ (no trailing group, no undivided orders)");
-    if (!a || !out || (!*o && c->zone_kind != GP_LAYOUT_AZ_AWARE) || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/orders/results");
-    if (!*o) *o = &c->zone_orders;
+    if (!*o) GP_TRY(require(c, c->held.az_orders(), who));
+    if (!*o) *o = c->held.orders();
+    if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/orders/results");
     return GP_OK;
 }
 
@@ -422,16 +404,14 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, const int32_t* grou
 
 // the FIFO loop with a single-AZ packer in one launch
 gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode mode, gp_zone_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_zones: gp_set_snapshot first");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), c->held.full_sched(), "gp_pack_fifo_zones"));
     if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: NULL apps/results");
     if (algo != GP_TIGHTLY_PACK && algo != GP_MINIMAL_FRAGMENTATION)
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: the single-AZ packers are tightly-pack and minimal-fragmentation");
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones)");
-    GP_TRY(one_instance_group(c, "gp_pack_fifo_zones"));
+    GP_TRY(require(c, c->held.one_instance_group(), "gp_pack_fifo_zones"));
     if (c->n_groups > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_zones: more than 64 zones");
     const OneInstanceGroup one(c->n_groups, nullptr);
     return fifo_zones_run(c, a, nullptr, (int)algo, mode, one.ig, false, out, "gp_pack_fifo_zones");
@@ -439,44 +419,31 @@ gp_status gp_pack_fifo_zones(gp_ctx* c, const gp_apps* a, gp_algo algo, gp_mode 
 
 // the FIFO loop with az-aware-tightly-pack in one launch: the zone packs plus the undivided fallback on the device
 gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const gp_az_orders* o, gp_zone_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_fifo_az_aware: gp_set_snapshot first");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), "gp_pack_fifo_az_aware"));
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: mode must be one of the FIFO modes (independent decisions: gp_pack_batch_zones, "
                                        "then gp_pack_batch over the undivided orders)");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
-    gp_status s = held_az_orders(c, a, out, &o, "gp_pack_fifo_az_aware");
-    if (s != GP_OK) return s;
-    const bool held = o == &c->zone_orders;
+    GP_TRY(require(c, c->held.full_sched(), "gp_pack_fifo_az_aware"));
+    GP_TRY(held_az_orders(c, a, out, &o, "gp_pack_fifo_az_aware"));
+    const bool held = o == c->held.orders();
     const int32_t Z = o->n_zones;
     if (Z < 0 || Z > kZoneFifoMaxZones) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones must be 0..64");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_fifo_az_aware: n_zones exceeds the snapshot's instance groups");
     const OneInstanceGroup one(c->n_groups, o);
-    if (!held) s = check_az_orders(c, one.ig, "gp_pack_fifo_az_aware");
-    if (s != GP_OK) return s;
+    if (!held) GP_TRY(check_az_orders(c, one.ig, "gp_pack_fifo_az_aware"));
     return fifo_zones_run(c, a, nullptr, kZoneAzAware, mode, one.ig, held, out, "gp_pack_fifo_az_aware");
 }
 
 // gp_pack_fifo_zones_groups(groups == NULL): the layout gp_prepare_cluster_zones_groups left, from its host words and its
 // device orders (built by the library: no order check)
 static gp_status held_groups_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, gp_zone_results* out, const char* who) {
-    if (c->zone_igs < 1)
-        return fail(c, GP_ERR_INVALID, who, "groups == NULL needs the layout of gp_prepare_cluster_zones_groups; the snapshot was laid "
-                                            "out by another call since");
     const bool azk = kind == kZoneAzAware;
-    if (azk != (c->zone_kind == GP_LAYOUT_AZ_AWARE))
-        return fail(c, GP_ERR_INVALID, who, azk ? "az-aware-tightly-pack needs a GP_LAYOUT_AZ_AWARE layout; the held one is GP_LAYOUT_SINGLE_AZ"
-                                                : "the single-AZ packers need a GP_LAYOUT_SINGLE_AZ layout; the held one is GP_LAYOUT_AZ_AWARE");
-    const int32_t G = c->zone_igs;
-    const int32_t* words = c->zone_ig_words.data();
-    const size_t g1 = (size_t)G + 1;
-    const int32_t *goff = words, *nz = words + g1;
-    for (int32_t b = 0; b < G; ++b)
-        if ((azk ? nz[b] : goff[b + 1] - goff[b]) > kZoneFifoMaxZones)
+    GP_TRY(require(c, c->held.groups_layout(azk), who));
+    const gp_instance_groups held = c->held.groups();
+    for (int32_t b = 0; b < held.n_instance_groups; ++b)
+        if ((azk ? held.n_zones[b] : held.group_off[b + 1] - held.group_off[b]) > kZoneFifoMaxZones)
             return fail(c, GP_ERR_INVALID, who, "more than 64 candidate zones in an instance group");
-    const gp_instance_groups held{G, goff, azk ? nz : nullptr, azk ? words + 2 * g1 : nullptr, azk ? c->zone_orders.exec_order : nullptr,
-                                  azk ? words + 3 * g1 : nullptr, azk ? c->zone_orders.drv_order : nullptr};
     return fifo_zones_run(c, a, a->group, kind, mode, held, azk, out, who);
 }
 
@@ -484,9 +451,8 @@ static gp_status held_groups_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode 
 gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker packer, gp_mode mode, const gp_instance_groups* ig,
                                     gp_zone_results* out) {
     const char* who = "gp_pack_fifo_zones_groups";
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, who, "gp_set_snapshot first");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), who));
     int kind;
     if (packer == GP_BP_SINGLE_AZ_TIGHTLY_PACK) kind = GP_TIGHTLY_PACK;
     else if (packer == GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) kind = GP_MINIMAL_FRAGMENTATION;
@@ -495,14 +461,12 @@ gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker pa
                                              "GP_BP_AZ_AWARE_TIGHTLY_PACK");
     if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
         return fail(c, GP_ERR_INVALID, who, "mode must be one of the FIFO modes");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, who, "gp_set_schedulable first (the efficiencies need SchedulableResources)");
+    GP_TRY(require(c, c->held.full_sched(), who));
     if (!ig) {
         if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/results");
         return held_groups_run(c, a, kind, mode, out, who);
     }
-    if (!c->host_layout)
-        return fail(c, GP_ERR_INVALID, who, "the snapshot must be laid out by gp_set_snapshot (after gp_set_snapshot_device / "
-                                            "gp_prepare_cluster* there is no host copy of the layout to check the instance groups against)");
+    GP_TRY(require(c, c->held.host_copy(true), who));
     if (!a || !out || !ig || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/groups/results");
     const int32_t G = ig->n_instance_groups;
     const int32_t* goff = ig->group_off;
@@ -525,26 +489,21 @@ gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker pa
 // az-aware-tightly-pack for a batch of independent decisions: the zone packs, the zone choice and the undivided fallback
 // on the device, one stream synchronise
 gp_status gp_pack_batch_az_aware(gp_ctx* c, const gp_apps* a, const gp_az_orders* o, gp_zone_results* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_pack_batch_az_aware: gp_set_snapshot first");
-    if (!c->have_sched) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: gp_set_schedulable first (the efficiencies need SchedulableResources)");
-    gp_status s = held_az_orders(c, a, out, &o, "gp_pack_batch_az_aware");
-    if (s != GP_OK) return s;
-    const bool held = o == &c->zone_orders;
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), c->held.full_sched(), "gp_pack_batch_az_aware"));
+    GP_TRY(held_az_orders(c, a, out, &o, "gp_pack_batch_az_aware"));
+    const bool held = o == c->held.orders();
     const int32_t Z = o->n_zones;
     if (Z < 0) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones is negative");
     if (Z > c->n_groups) return fail(c, GP_ERR_INVALID, "gp_pack_batch_az_aware: n_zones exceeds the snapshot's instance groups");
     const OneInstanceGroup one(c->n_groups, o);
-    if (!held) s = check_az_orders(c, one.ig, "gp_pack_batch_az_aware");
-    if (s != GP_OK) return s;
+    if (!held) GP_TRY(check_az_orders(c, one.ig, "gp_pack_batch_az_aware"));
     return batch_zones_run(c, a, GP_TIGHTLY_PACK, Z, o, held, out, "gp_pack_batch_az_aware");
 }
 
 gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* placed, int32_t subtract, gp_reservation_table* out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_reserve_placements: gp_set_snapshot first");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), "gp_reserve_placements"));
     if (!a || !placed || a->n_apps < 0 || (!out && !subtract)) return fail(c, GP_ERR_INVALID, "gp_reserve_placements: NULL arguments");
     const int32_t Q = a->n_apps;
     if (out) out->n_rows = 0;
@@ -617,9 +576,8 @@ gp_status gp_reserve_placements(gp_ctx* c, const gp_apps* a, const gp_results* p
 }
 
 gp_status gp_apply_usage_delta(gp_ctx* c, int64_t n_rows, const int32_t* node, const int64_t* cpu, const int64_t* mem, const int64_t* gpu, int32_t sign) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, "gp_apply_usage_delta: gp_set_snapshot first");
+    if (!enter(c)) return GP_ERR_INVALID;
+    GP_TRY(require(c, c->held.snapshot(), "gp_apply_usage_delta"));
     if (n_rows < 0 || (sign != 1 && sign != -1) || (n_rows > 0 && (!node || !cpu || !mem))) return fail(c, GP_ERR_INVALID, "gp_apply_usage_delta: bad arguments");
     if (n_rows == 0) return GP_OK;
     for (int64_t r = 0; r < n_rows; ++r) {
@@ -660,9 +618,8 @@ static const Refusal kEffRefusals[] = {
 // v with ig[v] == a->group[i]): the host pass over the rows, the (segmented) base pass and the row pass.
 static gp_status packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, const int32_t* ig,
                                     int32_t n_ig, double* avg_out, const char* who) {
-    if (!c->have_snapshot) return fail(c, GP_ERR_NO_SNAPSHOT, who, "no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)");
-    if (!c->have_eff_sched)
-        return fail(c, GP_ERR_INVALID, who, "no SchedulableResources (gp_set_schedulable, gp_prepare_cluster or gp_prepare_cluster_zones first)");
+    GP_TRY(require(c, c->held.snapshot("no snapshot (gp_set_snapshot, gp_prepare_cluster or gp_prepare_cluster_zones first)"),
+                   c->held.efficiency_sched(), who));
     if (!a || !placed || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/placed");
     if (algo != GP_TIGHTLY_PACK && algo != GP_DISTRIBUTE_EVENLY && algo != GP_MINIMAL_FRAGMENTATION)
         return fail(c, GP_ERR_INVALID, who, "unknown algo");
@@ -791,16 +748,14 @@ static gp_status packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, c
 extern "C" {
 
 gp_status gp_packing_efficiency(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged, double* avg_out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     return packing_efficiency(c, a, algo, placed, charged, nullptr, 1, avg_out, "gp_packing_efficiency");
 }
 
 // the same metric with row i averaged over its instance group's nodes (selectDriverNode's metadata) instead of the table's
 gp_status gp_packing_efficiency_groups(gp_ctx* c, const gp_apps* a, gp_algo algo, const gp_results* placed, gp_mode charged,
                                        const int32_t* instance_group, int32_t n_instance_groups, double* avg_out) {
-    if (!c) return GP_ERR_INVALID;
-    c->layout_tail = nullptr;
+    if (!enter(c)) return GP_ERR_INVALID;
     if (!instance_group && c->n_nodes > 0) return fail(c, GP_ERR_INVALID, "gp_packing_efficiency_groups: instance_group is NULL");
     static const int32_t none = -1;                     // an empty node table: no node in any instance group
     return packing_efficiency(c, a, algo, placed, charged, instance_group ? instance_group : &none, n_instance_groups, avg_out,
