@@ -992,6 +992,64 @@ typedef struct {
 gp_status gp_node_overhead(gp_ctx* ctx, const gp_overhead_pods* pods, const gp_overhead_reservations* rsv, int32_t n_nodes,
                            const int32_t* node_ids /* [n_nodes] the listed nodes, in node-table order */, gp_overhead_out* out);
 
+/* ---- the resident overhead table ------------------------------------------------------------------------------------------
+ * The same computation as gp_node_overhead over state the context keeps on the device and changes only by deltas, so a
+ * Predicate uploads the listed node ids alone instead of every record and reservation entry.  The state:
+ *   record slots   [n_slots] rows with the columns of gp_overhead_pods; node_id = -1 marks a free slot
+ *   RR flags       one per app key: the ResourceReservation (namespace, spark-app-id) exists
+ *   member set     (kind, app, name) triples: kind 0 = (app key, pod name) for a name in a ResourceReservation's Status.Pods,
+ *                  kind 1 = (app id, pod name) for a key in the soft store entry of that app id
+ * A query answers exactly what gp_node_overhead answers for: the slots as gp_overhead_pods, rr_app_key = the app keys whose RR
+ * flag is set, each listing its kind-0 members, soft_app_id = the app ids that have kind-1 members.  Kind-0 members of an app
+ * key whose flag is clear are never read; as in gp_node_overhead, free slots are ignored and the pod fields of a slot with
+ * listed = 0 are not read.  The table belongs to the context (freed by gp_destroy); no other entry reads or changes it. */
+typedef struct {
+    int64_t n_slots;                                        /* slot capacity, < 2^31 */
+    int32_t n_node_ids, n_app_keys, n_app_ids, n_names;     /* id capacities */
+} gp_overhead_table_size;
+/* Replace the context's table with an empty one of these capacities: every slot free, no RR flag, no member.
+ * GP_ERR_INVALID: NULL size, a negative capacity or n_slots >= 2^31 (the table held before is kept).  After a CUDA error
+ * the context holds no table. */
+gp_status gp_overhead_table_reset(gp_ctx* ctx, const gp_overhead_table_size* size);
+
+typedef struct {
+    int64_t n_write;                 /* slot writes: each the slot's whole new row; node_id = -1 frees the slot */
+    const int32_t* slot;             /* [n_write] distinct, < n_slots */
+    const int32_t* node_id;          /* [n_write] the columns of gp_overhead_pods, with its NULL conventions: */
+    const int64_t* req_cpu_milli;    /*   req_gpu NULL = 0, listed NULL = all, is_executor and spark_scheduler NULL = none */
+    const int64_t* req_mem_bytes;
+    const int64_t* req_gpu;
+    const uint8_t* listed;
+    const int32_t* app_key;
+    const int32_t* app_id;
+    const int32_t* name_id;
+    const uint8_t* is_executor;
+    const uint8_t* spark_scheduler;
+    int32_t n_rr;                    /* RR flag writes */
+    const int32_t* rr_app_key;       /* [n_rr] distinct */
+    const uint8_t* rr_exists;        /* [n_rr] nonzero = the flag is set */
+    int64_t n_member;                /* member writes: present nonzero inserts (a present triple: no-op), 0 removes (an absent
+                                        one: no-op) */
+    const uint8_t* member_kind;      /* [n_member] 0 = RR (member_app is an app key), 1 = soft (member_app is an app id) */
+    const int32_t* member_app;
+    const int32_t* member_name;
+    const uint8_t* member_present;   /* the triples (kind, app, name) are distinct */
+} gp_overhead_delta;
+/* Apply one delta.  The whole delta is checked on the device before anything is written: a refused delta leaves the table
+ * exactly as it was.  The order in which the writes of one delta apply is not observable.  One stream synchronise.
+ * GP_ERR_INVALID: no table (gp_overhead_table_reset first), missing arrays or negative counts; a slot or id outside its
+ * capacity or a member kind other than 0 and 1; a slot, rr_app_key or member triple given twice; app_key and app_id disagreeing
+ * on -1 (listed rows); a negative request (rows with node_id != -1).  GP_ERR_UNREPRESENTABLE: a request >= 2^61, so no table
+ * ever holds one.  GP_ERR_CAPACITY: more than 2^29 members.  A refusal, or a CUDA error while the delta is staged, leaves the
+ * table as it was; a CUDA error once the update writes the table's buffers leaves no table (GP_ERR_INVALID "no overhead
+ * table" until the next reset), and the caller resets and replays its whole state. */
+gp_status gp_overhead_table_update(gp_ctx* ctx, const gp_overhead_delta* delta);
+/* GetOverhead and GetNonSchedulableOverhead of the listed nodes from the table: node_ids is the only upload, and only the
+ * outputs asked for come back (48 bytes per listed node, has_reservation [n_slots], n_warned).  The outputs are those of
+ * gp_node_overhead on the equivalent arrays.  GP_ERR_INVALID: no table, missing arrays or a negative count, a node id out of
+ * range or listed twice.  GP_ERR_UNREPRESENTABLE: a per-node sum >= 2^61.  A query never changes the table. */
+gp_status gp_overhead_table_query(gp_ctx* ctx, int32_t n_nodes, const int32_t* node_ids, gp_overhead_out* out);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

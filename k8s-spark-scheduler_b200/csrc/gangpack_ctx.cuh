@@ -211,6 +211,18 @@ struct gp_ctx {
     bool recon_attr_set = false;                  // dynamic shared-memory opt-in of gp_sort_tiles<ReconKey> done on this device
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
 
+    // the resident overhead table (gangpack_overhead_table.cu); no other entry reads or changes it
+    struct OverheadTable {
+        bool live = false;                        // reset and not broken by a CUDA error since
+        gp_overhead_table_size size{};
+        DevBuf cols;                              // slot columns, RR flags and the duplicate stamps in one block
+        DevBuf set[2];                            // member set: set[cur] is live, the other the target of the next rehash
+        int cur = 0;
+        uint32_t cells = 0;                       // cells of set[cur], a power of two
+        long long keys = 0, used = 0;             // live keys; cells holding a key or a tombstone
+        uint32_t seq = 0;                         // the last update's stamp
+    } oht;
+
     gp_stats last{};
 };
 

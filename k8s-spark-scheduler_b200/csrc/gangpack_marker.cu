@@ -402,7 +402,7 @@ gp_status gp_node_overhead(gp_ctx* c, const gp_overhead_pods* p, const gp_overhe
     OhAcc A{ar.ptr(acc), &ar.ptr(word)->n_warned, n_nodes};
     if (P > 0) {
         pi.n = (long long)P; pi.n_node_ids = p->n_node_ids; pi.n_app_keys = p->n_app_keys; pi.n_app_ids = p->n_app_ids; pi.n_names = p->n_names;
-        gp_oh_pods<<<(unsigned)((P + kOhThreads - 1) / kOhThreads), kOhThreads, 0, st>>>(pi, M, A, d_err);
+        gp_oh_pods<<<(unsigned)((P + kOhThreads - 1) / kOhThreads), kOhThreads, 0, st>>>(pi, OhCallLookup{M}, A, d_err);
     }
     if (N > 0) gp_oh_finish<<<(unsigned)((N + T - 1) / T), T, 0, st>>>(A, ar.ptr(d_out), d_err);
     GP_CUDA(c, cudaGetLastError());

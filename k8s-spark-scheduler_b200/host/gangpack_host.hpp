@@ -26,6 +26,7 @@
 #include <set>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -1581,6 +1582,300 @@ private:
     std::vector<Slot> slots_;
     std::vector<size_t> free_;
     std::map<std::pair<std::string, std::string>, size_t> at_;   // (node, UID) -> slot: the reference's ClusterRequests
+};
+
+// The overhead computer over the context's resident overhead table (gp_overhead_table_*): the pod events of
+// OverheadComputer plus the pod lister's, the ResourceReservation cache's and the soft store's, as the informer handlers
+// deliver them.  compute() sends what changed since the last call as at most one gp_overhead_table_update and answers with
+// one gp_overhead_table_query.  Ids come from reference-counted interners, so the ids of names that are gone are reused; a
+// capacity that would be exceeded is doubled and the whole state replayed after a reset.  The table belongs to the
+// device context, so one instance per context.
+class ResidentOverheadComputer {
+public:
+    explicit ResidentOverheadComputer(gp_overhead_table_size initial = {64, 64, 64, 64, 64}) : size_(initial) {}
+    ResidentOverheadComputer(const ResidentOverheadComputer&) = delete;            // rows hold pointers to its interners
+    ResidentOverheadComputer& operator=(const ResidentOverheadComputer&) = delete;
+
+    void AddPod(const Pod& p) { if (!p.NodeName.empty()) record(p); }
+    void UpdatePod(const Pod& oldPod, const Pod& newPod) {
+        if (!newPod.NodeName.empty() && oldPod.NodeName.empty()) record(newPod);
+        else if (newPod.NodeName.empty() && !oldPod.NodeName.empty()) remove(oldPod);
+    }
+    void DeletePod(const Pod& p) { if (!p.NodeName.empty()) remove(p); }
+
+    // the pod lister: the pod now at (namespace, name), or none
+    void SetListerPod(const Pod& p) {
+        const auto k = std::make_pair(p.Namespace, p.Name);
+        lister_[k] = p;
+        refreshPod(k);
+    }
+    void DeleteListerPod(const std::string& ns, const std::string& name) {
+        if (lister_.erase({ns, name})) refreshPod({ns, name});
+    }
+    // the ResourceReservation (namespace, appID) with its Status.Pods values (they may repeat), and its deletion
+    void SetResourceReservation(const std::string& ns, const std::string& app, const std::vector<std::string>& pods) {
+        const int32_t k = keys_.acquire(appKey(ns, app));
+        touchFlag(k);
+        flags_.insert(k);
+        hold(0, k, pods);
+        dropReservation(ns, app);
+        rrs_[{ns, app}] = pods;
+    }
+    void DeleteResourceReservation(const std::string& ns, const std::string& app) {
+        if (!rrs_.count({ns, app})) return;
+        const int32_t k = keys_.id.at(appKey(ns, app));
+        touchFlag(k);
+        flags_.erase(k);
+        dropReservation(ns, app);
+    }
+    // the soft store's entry of appID with its Reservations keys, and its deletion
+    void SetSoftReservation(const std::string& app, const std::vector<std::string>& pods) {
+        hold(1, apps_.acquire(app), pods);
+        dropSoft(app);
+        soft_[app] = pods;
+    }
+    void DeleteSoftReservation(const std::string& app) { if (soft_.count(app)) dropSoft(app); }
+
+    resources::NodeGroupResources GetOverhead(const std::vector<std::string>& nodes) { return compute(nodes).first; }
+    resources::NodeGroupResources GetNonSchedulableOverhead(const std::vector<std::string>& nodes) { return compute(nodes).second; }
+    // getOverheadByNode (overhead.go:105-117): both maps; *warned = pods the reference logs a warning for.  A node without an
+    // id has no records: it answers zero without being sent.
+    std::pair<resources::NodeGroupResources, resources::NodeGroupResources> compute(const std::vector<std::string>& nodes,
+                                                                                    int64_t* warned = nullptr) {
+        gangpack::Device& dev = gangpack::Device::Get();
+        flush(dev);
+        std::vector<int32_t> query;
+        std::vector<size_t> at;
+        for (size_t i = 0; i < nodes.size(); ++i) {
+            auto it = nodes_.id.find(nodes[i]);
+            if (it != nodes_.id.end()) { query.push_back(it->second); at.push_back(i); }
+        }
+        const size_t Q = query.size();
+        std::vector<int64_t> o(6 * std::max<size_t>(Q, 1));
+        int64_t nw = 0;
+        gp_overhead_out out{o.data(), o.data() + Q, o.data() + 2 * Q, o.data() + 3 * Q, o.data() + 4 * Q, o.data() + 5 * Q, nullptr, &nw};
+        dev.check(gp_overhead_table_query(dev.ctx(), (int32_t)Q, query.data(), &out), "gp_overhead_table_query");
+        std::pair<resources::NodeGroupResources, resources::NodeGroupResources> res;
+        for (const auto& n : nodes) res.first[n] = res.second[n] = resources::Zero();
+        for (size_t j = 0; j < Q; ++j) {
+            res.first[nodes[at[j]]] = resources::CreateResources(o[j], o[Q + j], o[2 * Q + j]);
+            res.second[nodes[at[j]]] = resources::CreateResources(o[3 * Q + j], o[4 * Q + j], o[5 * Q + j]);
+        }
+        if (warned) *warned = nw;
+        return res;
+    }
+
+private:
+    struct Ids {                                   // dense ids with reference counts
+        std::unordered_map<std::string, int32_t> id;
+        std::vector<int32_t> count, freed;
+        int32_t acquire(const std::string& k) {
+            auto it = id.find(k);
+            int32_t i;
+            if (it != id.end()) i = it->second;
+            else {
+                if (!freed.empty()) { i = freed.back(); freed.pop_back(); }
+                else { i = (int32_t)count.size(); count.push_back(0); }
+                id.emplace(k, i);
+            }
+            ++count[(size_t)i];
+            return i;
+        }
+        void release(const std::string& k) {
+            auto it = id.find(k);
+            const int32_t i = it->second;
+            if (--count[(size_t)i] == 0) { id.erase(it); freed.push_back(i); }
+        }
+        int32_t bound() const { return (int32_t)count.size(); }
+    };
+    struct Row {                                   // one slot's columns as the table holds them
+        int32_t node = -1;
+        int64_t req[3] = {0, 0, 0};
+        uint8_t listed = 0;
+        int32_t ak = -1, ai = -1, nm = 0;
+        uint8_t exe = 0, spark = 0;
+        bool operator==(const Row& o) const {
+            return node == o.node && req[0] == o.req[0] && req[1] == o.req[1] && req[2] == o.req[2] && listed == o.listed &&
+                   ak == o.ak && ai == o.ai && nm == o.nm && exe == o.exe && spark == o.spark;
+        }
+        bool operator!=(const Row& o) const { return !(*this == o); }
+    };
+    struct Slot { bool used = false; std::string ns, name, node; resources::Resources requests; };
+    using Member = std::tuple<int, int32_t, int32_t>;   // (kind, app, name)
+    using PodKey = std::pair<std::string, std::string>;
+
+    static std::string appKey(const std::string& ns, const std::string& app) { return ns + '\x00' + app; }
+
+    void record(const Pod& p) {                    // addPodRequests (overhead.go:163-174), the slots of OverheadComputer
+        auto k = std::make_pair(p.NodeName, p.UID);
+        auto it = at_.find(k);
+        size_t i;
+        if (it != at_.end()) i = it->second;
+        else if (!free_.empty()) { i = free_.back(); free_.pop_back(); at_.emplace(k, i); }
+        else { i = slots_.size(); slots_.emplace_back(); at_.emplace(k, i); }
+        slots_[i] = Slot{true, p.Namespace, p.Name, p.NodeName, PodToResources(p)};
+        refresh(i);
+    }
+    void remove(const Pod& p) {                    // deletePodRequests (:176-193)
+        auto it = at_.find({p.NodeName, p.UID});
+        if (it == at_.end()) return;
+        const size_t i = it->second;
+        slots_[i] = Slot{};
+        free_.push_back(i);
+        at_.erase(it);
+        refresh(i);
+    }
+    void refreshPod(const PodKey& k) {
+        auto it = byPod_.find(k);
+        if (it == byPod_.end()) return;
+        const std::vector<size_t> at(it->second.begin(), it->second.end());
+        for (size_t i : at) refresh(i);
+    }
+    // the slot's row from its record and the lister's current pod; the references of the new row are taken before the old
+    // row's are released
+    void refresh(size_t i) {
+        if (rows_.size() < slots_.size()) { rows_.resize(slots_.size()); refs_.resize(slots_.size()); podOf_.resize(slots_.size()); }
+        const Slot& s = slots_[i];
+        Row r;
+        std::vector<std::pair<Ids*, std::string>> refs;
+        auto take = [&](Ids& ids, const std::string& k) { refs.emplace_back(&ids, k); return ids.acquire(k); };
+        if (s.used) {
+            r.node = take(nodes_, s.node);
+            r.req[0] = s.requests.CPU; r.req[1] = s.requests.Memory; r.req[2] = s.requests.NvidiaGPU;
+            auto it = lister_.find({s.ns, s.name});
+            if (it != lister_.end()) {
+                const Pod& pod = it->second;
+                r.listed = 1;
+                auto app = pod.Labels.find("spark-app-id");
+                if (app != pod.Labels.end()) { r.ak = take(keys_, appKey(pod.Namespace, app->second)); r.ai = take(apps_, app->second); }
+                r.nm = take(names_, pod.Name);
+                auto role = pod.Labels.find("spark-role");
+                r.exe = role != pod.Labels.end() && role->second == "executor";
+                r.spark = pod.SchedulerName == "spark-scheduler";
+            }
+        }
+        for (auto& ref : refs_[i]) ref.first->release(ref.second);
+        dirty_.emplace(i, rows_[i]);
+        rows_[i] = r;
+        refs_[i] = std::move(refs);
+        const PodKey now = s.used ? PodKey{s.ns, s.name} : PodKey{};
+        if (podOf_[i] != now) {
+            if (!podOf_[i].second.empty() || !podOf_[i].first.empty()) {
+                auto& set = byPod_[podOf_[i]];
+                set.erase(i);
+                if (set.empty()) byPod_.erase(podOf_[i]);
+            }
+            if (s.used) byPod_[now].insert(i);
+            podOf_[i] = now;
+        }
+    }
+    void touchFlag(int32_t k) { flagTouched_.emplace(k, flags_.count(k) > 0); }
+    // one holder of (kind, app, name) per distinct name; each holds a reference on the name's id
+    void hold(int kind, int32_t app, const std::vector<std::string>& pods) {
+        for (const auto& n : std::set<std::string>(pods.begin(), pods.end())) {
+            const Member m{kind, app, names_.acquire(n)};
+            int32_t& c = members_[m];
+            memberTouched_.emplace(m, c > 0);
+            ++c;
+        }
+    }
+    void release(int kind, int32_t app, const std::vector<std::string>& pods) {
+        for (const auto& n : std::set<std::string>(pods.begin(), pods.end())) {
+            const Member m{kind, app, names_.id.at(n)};
+            auto it = members_.find(m);
+            memberTouched_.emplace(m, it->second > 0);
+            if (--it->second == 0) members_.erase(it);
+            names_.release(n);
+        }
+    }
+    void dropReservation(const std::string& ns, const std::string& app) {
+        auto it = rrs_.find({ns, app});
+        if (it == rrs_.end()) return;
+        release(0, keys_.id.at(appKey(ns, app)), it->second);
+        keys_.release(appKey(ns, app));
+        rrs_.erase(it);
+    }
+    void dropSoft(const std::string& app) {
+        auto it = soft_.find(app);
+        if (it == soft_.end()) return;
+        release(1, apps_.id.at(app), it->second);
+        apps_.release(app);
+        soft_.erase(it);
+    }
+
+    // The changes since the last update (everything after a reset) as one gp_overhead_table_update
+    void flush(gangpack::Device& dev) {
+        auto grow = [&](int64_t& cap, int64_t need) { while (cap < need) { cap = std::max<int64_t>(2 * cap, 1); replay_ = true; } };
+        int64_t caps[5] = {size_.n_slots, size_.n_node_ids, size_.n_app_keys, size_.n_app_ids, size_.n_names};
+        grow(caps[0], (int64_t)slots_.size());
+        grow(caps[1], nodes_.bound()); grow(caps[2], keys_.bound()); grow(caps[3], apps_.bound()); grow(caps[4], names_.bound());
+        size_ = gp_overhead_table_size{caps[0], (int32_t)caps[1], (int32_t)caps[2], (int32_t)caps[3], (int32_t)caps[4]};
+        std::vector<int32_t> slot, node, ak, ai, nm, rrKey, mApp, mName;
+        std::vector<int64_t> cpu, mem, gpu;
+        std::vector<uint8_t> listed, exe, spark, rrOn, mKind, mPresent;
+        auto row = [&](size_t i) {
+            const Row& r = rows_[i];
+            slot.push_back((int32_t)i); node.push_back(r.node);
+            cpu.push_back(r.req[0]); mem.push_back(r.req[1]); gpu.push_back(r.req[2]);
+            listed.push_back(r.listed); ak.push_back(r.ak); ai.push_back(r.ai); nm.push_back(r.nm);
+            exe.push_back(r.exe); spark.push_back(r.spark);
+        };
+        auto member = [&](const Member& m, bool present) {
+            mKind.push_back((uint8_t)std::get<0>(m)); mApp.push_back(std::get<1>(m)); mName.push_back(std::get<2>(m));
+            mPresent.push_back(present);
+        };
+        if (replay_) {
+            for (size_t i = 0; i < rows_.size(); ++i) if (rows_[i] != Row{}) row(i);
+            for (int32_t k : flags_) { rrKey.push_back(k); rrOn.push_back(1); }
+            for (const auto& kv : members_) member(kv.first, true);
+        } else {
+            for (const auto& kv : dirty_) if (rows_[kv.first] != kv.second) row(kv.first);
+            for (const auto& kv : flagTouched_) {
+                const bool on = flags_.count(kv.first) > 0;
+                if (on != kv.second) { rrKey.push_back(kv.first); rrOn.push_back(on); }
+            }
+            for (const auto& kv : memberTouched_) {
+                auto it = members_.find(kv.first);
+                const bool on = it != members_.end() && it->second > 0;
+                if (on != kv.second) member(kv.first, on);
+            }
+        }
+        const bool reset = replay_;
+        replay_ = true;                            // until the table holds this state: a failed call replays next time
+        if (reset) dev.check(gp_overhead_table_reset(dev.ctx(), &size_), "gp_overhead_table_reset");
+        if (reset || !slot.empty() || !rrKey.empty() || !mKind.empty()) {
+            gp_overhead_delta d{};
+            d.n_write = (int64_t)slot.size();
+            d.slot = slot.data(); d.node_id = node.data(); d.req_cpu_milli = cpu.data(); d.req_mem_bytes = mem.data(); d.req_gpu = gpu.data();
+            d.listed = listed.data(); d.app_key = ak.data(); d.app_id = ai.data(); d.name_id = nm.data();
+            d.is_executor = exe.data(); d.spark_scheduler = spark.data();
+            d.n_rr = (int32_t)rrKey.size(); d.rr_app_key = rrKey.data(); d.rr_exists = rrOn.data();
+            d.n_member = (int64_t)mKind.size();
+            d.member_kind = mKind.data(); d.member_app = mApp.data(); d.member_name = mName.data(); d.member_present = mPresent.data();
+            dev.check(gp_overhead_table_update(dev.ctx(), &d), "gp_overhead_table_update");
+        }
+        replay_ = false;
+        dirty_.clear(); flagTouched_.clear(); memberTouched_.clear();
+    }
+
+    gp_overhead_table_size size_;
+    bool replay_ = true;
+    std::vector<Slot> slots_;
+    std::vector<size_t> free_;
+    std::map<std::pair<std::string, std::string>, size_t> at_;   // (node, UID) -> slot
+    std::vector<Row> rows_;
+    std::vector<std::vector<std::pair<Ids*, std::string>>> refs_;
+    std::vector<PodKey> podOf_;
+    std::map<PodKey, std::set<size_t>> byPod_;                    // (namespace, name) -> slots whose record names that pod
+    Ids nodes_, keys_, apps_, names_;
+    std::map<PodKey, Pod> lister_;
+    std::map<PodKey, std::vector<std::string>> rrs_;
+    std::map<std::string, std::vector<std::string>> soft_;
+    std::set<int32_t> flags_;
+    std::map<Member, int32_t> members_;
+    std::map<size_t, Row> dirty_;                                 // -> the row the table holds
+    std::map<int32_t, bool> flagTouched_;
+    std::map<Member, bool> memberTouched_;
 };
 
 }  // namespace extender

@@ -37,7 +37,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_potential_nodes", "gp_build_availability", "gp_build_reschedule_availability", "gp_prepare_cluster", "gp_prepare_cluster_zones",
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
-           "gp_node_overhead", "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
+           "gp_node_overhead", "gp_overhead_table_reset", "gp_overhead_table_update", "gp_overhead_table_query",
+           "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
            "gp_multi_set_snapshot", "gp_multi_pack_batch", "gp_multi_get_snapshot", "gp_multi_group_owner"]
@@ -239,6 +240,19 @@ class gp_overhead_out(C.Structure):
                 ("has_reservation", C.c_void_p), ("n_warned", C.c_void_p)]
 
 
+class gp_overhead_table_size(C.Structure):
+    _fields_ = [("n_slots", C.c_int64), ("n_node_ids", C.c_int32), ("n_app_keys", C.c_int32), ("n_app_ids", C.c_int32),
+                ("n_names", C.c_int32)]
+
+
+class gp_overhead_delta(C.Structure):
+    _fields_ = [("n_write", C.c_int64), ("slot", C.c_void_p), ("node_id", C.c_void_p), ("req_cpu_milli", C.c_void_p),
+                ("req_mem_bytes", C.c_void_p), ("req_gpu", C.c_void_p), ("listed", C.c_void_p), ("app_key", C.c_void_p),
+                ("app_id", C.c_void_p), ("name_id", C.c_void_p), ("is_executor", C.c_void_p), ("spark_scheduler", C.c_void_p),
+                ("n_rr", C.c_int32), ("rr_app_key", C.c_void_p), ("rr_exists", C.c_void_p), ("n_member", C.c_int64),
+                ("member_kind", C.c_void_p), ("member_app", C.c_void_p), ("member_name", C.c_void_p), ("member_present", C.c_void_p)]
+
+
 class gp_placement_record(C.Structure):
     _fields_ = [("collocation", C.c_int32), ("distinct_exec_nodes", C.c_int32), ("execs_per_node", C.c_int32), ("n_zones", C.c_int32),
                 ("cross_zone_pairs", C.c_int64), ("total_pairs", C.c_int64)]
@@ -335,6 +349,12 @@ def load():
     L.gp_node_overhead.restype = C.c_int
     L.gp_node_overhead.argtypes = [C.c_void_p, C.POINTER(gp_overhead_pods), C.POINTER(gp_overhead_reservations), C.c_int32,
                                    C.c_void_p, C.POINTER(gp_overhead_out)]
+    L.gp_overhead_table_reset.restype = C.c_int
+    L.gp_overhead_table_reset.argtypes = [C.c_void_p, C.POINTER(gp_overhead_table_size)]
+    L.gp_overhead_table_update.restype = C.c_int
+    L.gp_overhead_table_update.argtypes = [C.c_void_p, C.POINTER(gp_overhead_delta)]
+    L.gp_overhead_table_query.restype = C.c_int
+    L.gp_overhead_table_query.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(gp_overhead_out)]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -477,6 +497,12 @@ _AFF_COLS = {"sel_off": np.int64, "sel_key": np.int32, "sel_val": np.int32, "has
              "term_req_off": np.int64, "term_parse_error": np.uint8, "req_op": np.int32, "req_key": np.int32, "req_int": np.int64,
              "req_val_off": np.int64, "req_val": np.int32}
 
+
+# gp_overhead_delta's columns (overhead.OverheadTable.delta() keys)
+_DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "req_cpu_milli": np.int64, "req_mem_bytes": np.int64, "req_gpu": np.int64,
+               "listed": np.uint8, "app_key": np.int32, "app_id": np.int32, "name_id": np.int32, "is_executor": np.uint8,
+               "spark_scheduler": np.uint8, "rr_app_key": np.int32, "rr_exists": np.uint8, "member_kind": np.uint8,
+               "member_app": np.int32, "member_name": np.int32, "member_present": np.uint8}
 
 _OVERHEAD_COLS = {"node_id": np.int32, "req_cpu_milli": np.int64, "req_mem_bytes": np.int64, "req_gpu": np.int64, "listed": np.uint8,
                   "app_key": np.int32, "app_id": np.int32, "name_id": np.int32, "is_executor": np.uint8, "spark_scheduler": np.uint8,
@@ -1088,6 +1114,38 @@ class GangPacker:
         out = gp_overhead_out(*[_p(x) for x in res], _p(has), C.addressof(warned))
         self._check(load().gp_node_overhead(self._h, C.byref(pods), C.byref(rsv), n, _p(qn), C.byref(out)))
         return tuple(x[:n] for x in res[:3]), tuple(x[:n] for x in res[3:]), has[:n_pods], warned.value
+
+    # ---- the resident overhead table (gp_overhead_table_*) ---------------------------------------------------------------
+    def overhead_table_reset(self, n_slots, n_node_ids, n_app_keys, n_app_ids, n_names):
+        """Replace the context's overhead table with an empty one of these capacities."""
+        z = gp_overhead_table_size(int(n_slots), int(n_node_ids), int(n_app_keys), int(n_app_ids), int(n_names))
+        # recorded once the library holds the new table: a refused reset keeps the table and size held before, and after a
+        # reset that fails with a CUDA error every query is refused before anything is downloaded
+        self._check(load().gp_overhead_table_reset(self._h, C.byref(z)))
+        self._oht_slots = int(n_slots)
+
+    def overhead_table_update(self, delta: dict):
+        """One gp_overhead_table_update over the arrays of overhead.OverheadTable.delta() (or the same keys given by hand; a
+        missing optional column is NULL; the "reset" entry is not read here)."""
+        col = {k: _np(delta.get(k), t) for k, t in _DELTA_COLS.items()}
+        n = lambda k: 0 if col[k] is None else len(col[k])
+        d = gp_overhead_delta(n_write=int(delta.get("n_write", n("slot"))), n_rr=int(delta.get("n_rr", n("rr_app_key"))),
+                              n_member=int(delta.get("n_member", n("member_kind"))), **{k: _p(v) for k, v in col.items()})
+        self._check(load().gp_overhead_table_update(self._h, C.byref(d)))
+
+    def overhead_table_query(self, node_ids, has_reservation=True):
+        """The table's GetOverhead and GetNonSchedulableOverhead for the listed node ids -> the tuple of node_overhead, with
+        has_reservation over every slot of the table (None when not asked for)."""
+        qn = _np(node_ids, np.int32)
+        n = len(qn)
+        res = [np.zeros(max(n, 1), np.int64) for _ in range(6)]
+        slots = getattr(self, "_oht_slots", 0)          # [n_slots] of the table held; before any reset the query is refused
+        has = np.zeros(max(slots, 1), np.uint8) if has_reservation else None
+        warned = C.c_int64(-1)
+        out = gp_overhead_out(*[_p(x) for x in res], _p(has), C.addressof(warned))
+        self._check(load().gp_overhead_table_query(self._h, n, _p(qn), C.byref(out)))
+        return (tuple(x[:n] for x in res[:3]), tuple(x[:n] for x in res[3:]),
+                None if has is None else has[:slots], warned.value)
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)

@@ -254,3 +254,294 @@ def synthetic_cluster(seed: int, n_nodes: int, n_pods: int, big_apps: int = 0, b
             soft.setdefault(app, []).extend(names[1 + (execs * 3) // 4:] + ([names[0]] if kind == 4 else []))
         a += 1
     return nodes, records, lister, rrs, soft, pods
+
+
+# ---- the resident table (gp_overhead_table_*) -------------------------------------------------------------------------------
+_FREE_ROW = (-1, 0, 0, 0, 0, -1, -1, 0, 0, 0)     # node_id, cpu, mem, gpu, listed, app_key, app_id, name_id, is_executor, spark
+_ROW_COLS = (("node_id", np.int32), ("req_cpu_milli", np.int64), ("req_mem_bytes", np.int64), ("req_gpu", np.int64),
+             ("listed", np.uint8), ("app_key", np.int32), ("app_id", np.int32), ("name_id", np.int32),
+             ("is_executor", np.uint8), ("spark_scheduler", np.uint8))
+_SIZE_KEYS = ("n_slots", "n_node_ids", "n_app_keys", "n_app_ids", "n_names")
+
+
+class _CountedInterner:
+    """Dense ids with reference counts: the id of a key whose last reference is released goes to the next new key."""
+
+    def __init__(self):
+        self.ids, self.count, self._free = {}, [], []
+
+    def acquire(self, key) -> int:
+        i = self.ids.get(key)
+        if i is None:
+            if self._free:
+                i = self._free.pop()
+            else:
+                i = len(self.count)
+                self.count.append(0)
+            self.ids[key] = i
+        self.count[i] += 1
+        return i
+
+    def release(self, key):
+        i = self.ids[key]
+        self.count[i] -= 1
+        if not self.count[i]:
+            del self.ids[key]
+            self._free.append(i)
+
+    @property
+    def bound(self) -> int:
+        """every id in use is below this"""
+        return len(self.count)
+
+
+class OverheadTable(PodRecords):
+    """The host side of the resident overhead table: PodRecords' slots (same numbering), the pod lister, the
+    ResourceReservation cache and the soft store, kept as the shim's informer handlers see them, and turned into the deltas of
+    gp_overhead_table_update.  Ids come from reference-counted interners over the slots' rows, the RR flags and the members,
+    so the ids of nodes, apps and pod names that are gone are reused.
+
+    Events: add / update / delete (the pod informer through the nodeName filter, as PodRecords), lister_set(pod) /
+    lister_delete(namespace, name), rr_set((namespace, appID), Status.Pods values) / rr_delete, soft_set(appID, Reservations
+    keys) / soft_delete.  delta() -> the arrays of one update; when it carries "reset" (the first one, whenever a capacity
+    would be exceeded: it is doubled and the whole state replayed, and after replay()), gp_overhead_table_reset(**delta["reset"])
+    goes first."""
+
+    def __init__(self, n_slots=64, n_node_ids=64, n_app_keys=64, n_app_ids=64, n_names=64):
+        super().__init__()
+        self.size = dict(n_slots=n_slots, n_node_ids=n_node_ids, n_app_keys=n_app_keys, n_app_ids=n_app_ids, n_names=n_names)
+        self.lister, self.rrs, self.soft = {}, {}, {}
+        self._nodes, self._keys, self._apps, self._names = (_CountedInterner() for _ in range(4))
+        self._row, self._refs = [], []                  # per slot: its row (ids), the interner references the row holds
+        self._by_pod, self._pod_of = {}, {}              # (namespace, name) -> slots whose record names that pod, and back
+        self._flags = set()                              # app key ids with a ResourceReservation
+        self._members = {}                               # (kind, app, name) ids -> holders (0: absent)
+        self._dirty, self._flag_touched, self._member_touched = {}, {}, {}   # -> what the device holds since the last delta
+        self._replay = True
+
+    # ---- pod records (PodRecords' add / update / delete land here)
+    def _record(self, pod):
+        super()._record(pod)
+        self._refresh(self._at[(pod["nodeName"], pod["uid"])])
+
+    def _remove(self, pod):
+        at = self._at.get((pod["nodeName"], pod["uid"]))
+        super()._remove(pod)
+        if at is not None:
+            self._refresh(at)
+
+    # ---- the lister
+    def lister_set(self, pod):
+        key = (pod["namespace"], pod["name"])
+        self.lister[key] = pod
+        for at in list(self._by_pod.get(key, ())):
+            self._refresh(at)
+
+    def lister_delete(self, namespace, name):
+        if self.lister.pop((namespace, name), None) is not None:
+            for at in list(self._by_pod.get((namespace, name), ())):
+                self._refresh(at)
+
+    # ---- ResourceReservations and the soft store
+    def rr_set(self, key, names):
+        kid = self._keys.acquire(key)
+        self._touch_flag(kid)
+        self._flags.add(kid)
+        self._hold(0, kid, names)
+        self._drop_rr(key)
+        self.rrs[key] = list(names)
+
+    def rr_delete(self, key):
+        if key in self.rrs:
+            kid = self._keys.ids[key]
+            self._touch_flag(kid)
+            self._flags.discard(kid)
+            self._drop_rr(key)
+
+    def soft_set(self, app, names):
+        aid = self._apps.acquire(app)
+        self._hold(1, aid, names)
+        self._drop_soft(app)
+        self.soft[app] = list(names)
+
+    def soft_delete(self, app):
+        if app in self.soft:
+            self._drop_soft(app)
+
+    # ---- queries
+    def node_ids(self, nodes) -> np.ndarray:
+        """the table's ids of these node names; -1 for a node without one (it has no records: its overhead is zero)"""
+        return np.array([self._nodes.ids.get(n, -1) for n in nodes], np.int32)
+
+    def answer(self, nodes, query):
+        """GetOverhead / GetNonSchedulableOverhead of `nodes` in their order through query(node_ids) -- a device query or
+        evaluate(to_encoding(mirror, node_ids)) -- asked for the nodes that have an id; the others are zero.
+        -> (overhead (cpu, mem, gpu), nonsched (cpu, mem, gpu), has_reservation, n_warned)"""
+        ids = self.node_ids(nodes)
+        known = ids >= 0
+        ov, ns, has, warned = query(ids[known])
+        cols = [np.zeros(len(nodes), np.int64) for _ in range(6)]
+        for c, v in zip(cols, tuple(ov) + tuple(ns)):
+            c[known] = v
+        return tuple(cols[:3]), tuple(cols[3:]), has, warned
+
+    def replay(self):
+        """The next delta resets the table and resends the whole state.  delta() takes its changes as sent, so after an
+        update the library refused (a request >= 2^61 is refused when it arrives) or that failed, call this: otherwise the
+        host and the device disagree for good."""
+        self._replay = True
+
+    def delta(self) -> dict:
+        """The arrays of one gp_overhead_table_update: what changed since the last delta (everything after a reset).  The
+        changes count as sent; see replay() for an update that does not go through."""
+        bounds = dict(n_slots=len(self.slots), n_node_ids=self._nodes.bound, n_app_keys=self._keys.bound,
+                      n_app_ids=self._apps.bound, n_names=self._names.bound)
+        for k, b in bounds.items():
+            while self.size[k] < b:
+                self.size[k] = max(2 * self.size[k], 1)
+                self._replay = True
+        if self._replay:
+            slots = [at for at, row in enumerate(self._row) if row != _FREE_ROW]
+            flags = sorted(self._flags)
+            members = sorted(t for t, n in self._members.items() if n)
+        else:
+            slots = sorted(at for at, was in self._dirty.items() if self._row[at] != was)
+            flags = sorted(k for k, was in self._flag_touched.items() if (k in self._flags) != was)
+            members = sorted(t for t, was in self._member_touched.items() if (self._members.get(t, 0) > 0) != was)
+        rows = [self._row[at] for at in slots]
+        d = {"reset": dict(self.size) if self._replay else None, "slot": np.array(slots, np.int32)}
+        for j, (name, t) in enumerate(_ROW_COLS):
+            d[name] = np.array([r[j] for r in rows], t)
+        d["rr_app_key"] = np.array(flags, np.int32)
+        d["rr_exists"] = np.array([k in self._flags for k in flags], np.uint8)
+        d["member_kind"] = np.array([t[0] for t in members], np.uint8)
+        d["member_app"] = np.array([t[1] for t in members], np.int32)
+        d["member_name"] = np.array([t[2] for t in members], np.int32)
+        d["member_present"] = np.array([self._members.get(t, 0) > 0 for t in members], np.uint8)
+        self._dirty, self._flag_touched, self._member_touched = {}, {}, {}
+        self._replay = False
+        return d
+
+    # ---- internals
+    def _refresh(self, at):
+        while len(self._row) < len(self.slots):
+            self._row.append(_FREE_ROW)
+            self._refs.append(())
+        rec = self.slots[at]
+        refs, row = [], _FREE_ROW
+
+        def acquire(interner, key):
+            refs.append((interner, key))
+            return interner.acquire(key)
+
+        if rec is not None:
+            ns, name, node, req = rec
+            pod = self.lister.get((ns, name))
+            if pod is None:
+                row = (acquire(self._nodes, node),) + tuple(req) + (0, -1, -1, 0, 0, 0)
+            else:
+                labels = pod.get("labels") or {}
+                app = labels.get(SPARK_APP_ID_LABEL)
+                ak, ai = (-1, -1) if app is None else (acquire(self._keys, (pod["namespace"], app)), acquire(self._apps, app))
+                row = (acquire(self._nodes, node),) + tuple(req) + (
+                    1, ak, ai, acquire(self._names, pod["name"]), int(labels.get(SPARK_ROLE_LABEL) == EXECUTOR),
+                    int(pod.get("schedulerName") == SPARK_SCHEDULER_NAME))
+        for interner, key in self._refs[at]:
+            interner.release(key)
+        old = self._row[at]
+        self._dirty.setdefault(at, old)
+        self._row[at], self._refs[at] = row, tuple(refs)
+        self._index(at, self._pod_of.get(at), None if rec is None else (rec[0], rec[1]))
+
+    def _index(self, at, old_pod, new_pod):
+        if old_pod == new_pod:
+            return
+        if old_pod is not None:
+            self._by_pod[old_pod].discard(at)
+            if not self._by_pod[old_pod]:
+                del self._by_pod[old_pod]
+            del self._pod_of[at]
+        if new_pod is not None:
+            self._by_pod.setdefault(new_pod, set()).add(at)
+            self._pod_of[at] = new_pod
+
+    def _touch_flag(self, kid):
+        self._flag_touched.setdefault(kid, kid in self._flags)
+
+    def _hold(self, kind, app, names):
+        """one holder of (kind, app, name) per distinct name (Status.Pods values may repeat); each holds a name id"""
+        for name in dict.fromkeys(names):
+            t = (kind, app, self._names.acquire(name))
+            self._member_touched.setdefault(t, self._members.get(t, 0) > 0)
+            self._members[t] = self._members.get(t, 0) + 1
+
+    def _release(self, kind, app, names):
+        for name in dict.fromkeys(names):
+            t = (kind, app, self._names.ids[name])
+            self._member_touched.setdefault(t, self._members[t] > 0)
+            self._members[t] -= 1
+            if not self._members[t]:
+                del self._members[t]
+            self._names.release(name)
+
+    def _drop_rr(self, key):
+        old = self.rrs.pop(key, None)
+        if old is not None:
+            self._release(0, self._keys.ids[key], old)
+            self._keys.release(key)
+
+    def _drop_soft(self, app):
+        old = self.soft.pop(app, None)
+        if old is not None:
+            self._release(1, self._apps.ids[app], old)
+            self._apps.release(app)
+
+
+class TableMirror:
+    """What gp_overhead_table_update leaves on the device, with numpy: apply(delta) in the order the library would, so
+    evaluate(to_encoding(mirror, node_ids)) is the device's answer without a device."""
+
+    def __init__(self):
+        self.size = None
+
+    def apply(self, d: dict):
+        if d.get("reset"):
+            self.size = dict(d["reset"])
+            n = self.size["n_slots"]
+            self.cols = {name: np.full(n, free, t) for (name, t), free in zip(_ROW_COLS, _FREE_ROW)}
+            self.rr = np.zeros(self.size["n_app_keys"], np.uint8)
+            self.members = set()
+        s = np.asarray(d["slot"], np.int64)
+        for name, t in _ROW_COLS:
+            v = d.get(name)
+            default = {"listed": 1, "req_gpu": 0, "is_executor": 0, "spark_scheduler": 0}.get(name)
+            self.cols[name][s] = np.asarray(v, t) if v is not None else default
+        self.rr[np.asarray(d["rr_app_key"], np.int64)] = np.asarray(d["rr_exists"], np.uint8) != 0
+        for k, a, nm, p in zip(*(np.asarray(d[x]).tolist() for x in ("member_kind", "member_app", "member_name", "member_present"))):
+            (self.members.add if p else self.members.discard)((k, a, nm))
+
+
+def to_encoding(mirror: TableMirror, node_ids) -> dict:
+    """The gp_node_overhead arrays of the table's state: its slots, rr_app_key = the app keys whose RR flag is set with their
+    kind-0 members, soft_app_id = the app ids with kind-1 members."""
+    by = ({}, {})
+    for k, a, nm in sorted(mirror.members):
+        by[k].setdefault(a, []).append(nm)
+    rr_keys = [int(k) for k in np.nonzero(mirror.rr)[0]]
+    rr_names = [by[0].get(k, []) for k in rr_keys]
+    soft_ids = sorted(by[1])
+    soft_names = [by[1][a] for a in soft_ids]
+
+    def csr(lists):
+        off = np.zeros(len(lists) + 1, np.int64)
+        np.cumsum([len(x) for x in lists], out=off[1:])
+        return off, np.array([v for x in lists for v in x], np.int32)
+
+    rr_off, rr_name = csr(rr_names)
+    soft_off, soft_name = csr(soft_names)
+    enc = {name: mirror.cols[name].copy() for name, _ in _ROW_COLS}
+    enc.update(n_pods=mirror.size["n_slots"], **{k: mirror.size[k] for k in _SIZE_KEYS[1:]},
+               n_rr=len(rr_keys), rr_app_key=np.array(rr_keys, np.int32), rr_pod_off=rr_off, rr_pod_name=rr_name,
+               n_soft=len(soft_ids), soft_app_id=np.array(soft_ids, np.int32), soft_pod_off=soft_off, soft_pod_name=soft_name,
+               node_ids=np.asarray(node_ids, np.int32))
+    return enc
