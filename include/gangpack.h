@@ -1050,6 +1050,69 @@ gp_status gp_overhead_table_update(gp_ctx* ctx, const gp_overhead_delta* delta);
  * range or listed twice.  GP_ERR_UNREPRESENTABLE: a per-node sum >= 2^61.  A query never changes the table. */
 gp_status gp_overhead_table_query(gp_ctx* ctx, int32_t n_nodes, const int32_t* node_ids, gp_overhead_out* out);
 
+/* ---- the resident reservation table ---------------------------------------------------------------------------------------
+ * GetReservedResources' rows (every ResourceReservation's Spec.Reservations entry and every soft reservation, hard and soft
+ * alike) kept on the device and changed only by deltas, so a Predicate no longer uploads one gp_usage_input row per
+ * reservation.  The state: [n_slots] slots, each a reservation-table node id (-1 = free slot) and cpu / mem / gpu.  Node ids are
+ * the caller's interned node names; a row whose node has left the cluster keeps its id and is ignored where no node-table
+ * entry carries that id, like the map lookup at resources.go:72-75.  The table belongs to the context (freed by gp_destroy);
+ * updates change no snapshot, layout, schedulable resources or statistics. */
+typedef struct {
+    int64_t n_slots;                 /* slot capacity, < 2^31 */
+    int32_t n_node_ids;              /* node id capacity */
+} gp_reservation_table_size;
+/* Replace the context's reservation table with an empty one (every slot free).  GP_ERR_INVALID: NULL size, a negative
+ * capacity or n_slots >= 2^31 (the table held before is kept).  After a CUDA error the context holds no table. */
+gp_status gp_reservation_table_reset(gp_ctx* ctx, const gp_reservation_table_size* size);
+
+typedef struct {
+    int64_t n_write;                 /* whole-row slot writes; node_id = -1 frees the slot */
+    const int32_t* slot;             /* [n_write] distinct, < n_slots */
+    const int32_t* node_id;          /* [n_write] in [-1, n_node_ids) */
+    const int64_t* cpu_milli;        /* [n_write] any value with |v| < 2^61 (negative included, as gp_usage_input accepts) */
+    const int64_t* mem_bytes;
+    const int64_t* gpu;              /* or NULL (= 0) */
+} gp_reservation_delta;
+/* Apply one delta.  The whole delta is checked on the device before anything is written: a refused delta leaves the table
+ * exactly as it was.  One stream synchronise.  GP_ERR_INVALID: no table (gp_reservation_table_reset first), missing arrays or
+ * a negative count; a slot or node id out of range; a slot given twice.  GP_ERR_UNREPRESENTABLE: |cpu|, |mem| or |gpu| >= 2^61
+ * on a row with node_id != -1.  A refusal, or a CUDA error while the delta is staged, leaves the table as it was; a CUDA error
+ * once the update writes the table leaves no table (GP_ERR_INVALID "no reservation table" until the next reset), and the
+ * caller resets and replays its whole state. */
+gp_status gp_reservation_table_update(gp_ctx* ctx, const gp_reservation_delta* delta);
+
+/* The node table of the resident Predicate front ends: allocatable and overhead as in gp_usage_input, and the reservations
+ * from the resident table.  Overhead comes either from the host arrays (NULL = 0) or, with overhead_node_id given, from the
+ * resident overhead table on the device (GetOverhead, gp_overhead_table_query's overhead_*), never crossing to the host. */
+typedef struct {
+    int32_t n_nodes;
+    const int32_t* node_id;            /* [n_nodes] reservation-table id of each node-table entry, distinct, -1 = none */
+    const int64_t* alloc_cpu_milli;    /* [n_nodes] as gp_usage_input */
+    const int64_t* alloc_mem_bytes;
+    const int64_t* alloc_gpu;          /* or NULL (= 0) */
+    const int32_t* overhead_node_id;   /* [n_nodes] overhead-table ids (distinct, -1 = no records), or NULL = overhead_* below */
+    const int64_t* overhead_cpu_milli; /* as gp_usage_input (ignored when overhead_node_id is given) */
+    const int64_t* overhead_mem_bytes;
+    const int64_t* overhead_gpu;
+} gp_resident_usage;
+/* The resident forms of gp_prepare_cluster_groups, gp_prepare_cluster_zones_groups and gp_reschedule_from_reservations: the
+ * same arguments with a gp_resident_usage in place of the gp_usage_input, and the same result -- outputs bit for bit, status,
+ * and the context afterwards -- as the per-call entry given the equivalent gp_usage_input: the same n_nodes and allocatable;
+ * as overhead the host arrays, or gp_overhead_table_query(overhead_node_id)'s GetOverhead; one row per occupied slot with
+ * res_node = the index i where node_id[i] equals the slot's id, or -1 when no entry has that id.  instance_group == NULL
+ * gives gp_prepare_cluster / gp_prepare_cluster_zones, as for the per-call forms.  Uploads: the two id arrays, allocatable
+ * and host overhead; the slots are read where they are.  Refusals, besides the per-call entry's (a refused call replaces
+ * nothing): GP_ERR_INVALID for no reservation table, overhead_node_id without a live overhead table, an id out of range or
+ * given twice; GP_ERR_UNREPRESENTABLE for a per-node overhead sum >= 2^61 (gp_overhead_table_query's refusal). */
+gp_status gp_prepare_cluster_groups_resident(gp_ctx* ctx, const gp_resident_usage* usage, const gp_sort_input* sort,
+                                             const int32_t* instance_group, int32_t n_instance_groups, gp_instance_group_orders* out);
+gp_status gp_prepare_cluster_zones_groups_resident(gp_ctx* ctx, const gp_resident_usage* usage, const gp_sort_input* sort,
+                                                   const int32_t* instance_group, int32_t n_instance_groups,
+                                                   gp_instance_group_layout* layout);
+gp_status gp_reschedule_from_reservations_resident(gp_ctx* ctx, const gp_resident_usage* usage, const gp_sort_input* sort,
+                                                   const gp_reschedule_scope* scope, const gp_reschedule* in,
+                                                   int32_t* node_out, uint8_t* ambiguous);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

@@ -1,7 +1,8 @@
 // gangpack_cluster.cu -- the entry points driven by the reservations: node priority orders (gp_potential_nodes),
 // availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster[_groups], gp_prepare_cluster_zones[_groups]), executor
 // reschedule (gp_reschedule_executors, gp_reschedule_from_reservations) and the failover reconciler (gp_reconcile_find_nodes),
-// with the input checks and device staging they share.
+// with the input checks and device staging they share; and the *_resident forms of gp_prepare_cluster_groups,
+// gp_prepare_cluster_zones_groups and gp_reschedule_from_reservations, which take the reservations from the resident table.
 #include "gangpack_ctx.cuh"
 #include "gangpack_sort.cuh"
 #include "gangpack_zonelayout.cuh"
@@ -39,9 +40,43 @@ static gp_status check_usage(gp_ctx* c, const gp_usage_input* in, const char* wh
 
 // The status word of the availability stage (kFeErr* bits), read back by the entry: the refusal it stands for.
 static const Refusal kFeRefusals[] = {
+    {kFeErrId, GP_ERR_INVALID, "a reservation-table or overhead-table node id out of range or given twice"},
     {kFeErrInput, GP_ERR_UNREPRESENTABLE, "|allocatable|, |overhead| or |reservation| >= 2^61"},
     {kFeErrResult, GP_ERR_UNREPRESENTABLE, "a node's reservation sum or availability lies outside the exact-int64 domain (|v| >= 2^61)"},
 };
+
+// Where an availability stage takes its usage from: the per-call rows of a gp_usage_input, or the resident reservation table
+// through a gp_resident_usage (the *_resident entries).  Everything else of the stage is the same for both.
+struct UsageIn {
+    const gp_usage_input* rows = nullptr;
+    const gp_resident_usage* res = nullptr;
+    UsageIn(const gp_usage_input* u) : rows(u) {}
+    UsageIn(const gp_resident_usage* r) : res(r) {}
+    bool given() const { return rows || res; }
+    int32_t n_nodes() const { return rows ? rows->n_nodes : res ? res->n_nodes : 0; }
+    // overhead from the resident overhead table, on the device
+    bool table_overhead() const { return res && res->overhead_node_id; }
+};
+
+// check_usage for either source.  The resident form: the node table's columns, a live reservation table, and a live overhead
+// table when overhead_node_id is given; the ids themselves are checked on the device (kFeErrId).
+static gp_status check_source(gp_ctx* c, const UsageIn& u, const char* who) {
+    if (!u.res) return check_usage(c, u.rows, who);
+    const gp_resident_usage* r = u.res;
+    if (r->n_nodes < 0 || (r->n_nodes > 0 && (!r->node_id || !r->alloc_cpu_milli || !r->alloc_mem_bytes)))
+        return fail(c, GP_ERR_INVALID, who, "missing arrays or bad sizes");
+    if (!c->rt.live) return fail(c, GP_ERR_INVALID, who, "no reservation table (gp_reservation_table_reset first)");
+    if (r->overhead_node_id && !c->oht.live) return fail(c, GP_ERR_INVALID, who, "overhead_node_id without an overhead table");
+    return GP_OK;
+}
+
+// The two status words of the availability stage once the stream has been synchronised: err[0] kFeErr* bits, err[1] the
+// overhead query's bits (resident overhead only).  Ids first, then the overhead sums, then the domain of the stage itself.
+static gp_status stage_refusal(gp_ctx* c, const int* err, const char* who) {
+    GP_TRY(refuse(c, err[0] & kFeErrId, kFeRefusals, who));
+    GP_TRY(oht_sum_refusal(c, err[1], who));
+    return refuse(c, err[0], kFeRefusals, who);
+}
 
 // The failover loop's status word (kRcErr* bits)
 static const Refusal kRcRefusals[] = {
@@ -92,36 +127,71 @@ static gp_status check_hosting(gp_ctx* c, const gp_reschedule* in, int32_t n_nod
     return GP_OK;
 }
 
-// f2 stage: uploads the inputs, leaves avail[3][N] / sched[3][N] and the stage's status word (*d_err: kFeErr* bits, for
-// kFeRefusals once the stream has been synchronised) on the device (usagebuf).
-// d_over (optional, [3]): the uploaded overhead columns, NULL where the caller gave none.
-static gp_status stage_availability(gp_ctx* c, const gp_usage_input* in, cudaStream_t st, long long** d_avail, long long** d_sched, int** d_err,
+// f2 stage: uploads the inputs, leaves avail[3][N] / sched[3][N] and the stage's two status words (*d_err: [2], for
+// stage_refusal once the stream has been synchronised) on the device (usagebuf).
+// d_over (optional, [3]): the device overhead columns, NULL where the caller gave none.
+// The usage sums come from the per-call rows (gp_usage_scatter<UsageRowIndex>) or from the reservation table's slots through a
+// directory built from node_id (gp_resident_dirs, gp_usage_scatter<UsageSlotDir>); resident overhead is the overhead table's
+// GetOverhead written straight into the overhead piece (oht_enqueue_sums).  From the sums on, both are the same kernels.
+static gp_status stage_availability(gp_ctx* c, const UsageIn& in, cudaStream_t st, long long** d_avail, long long** d_sched, int** d_err,
                                     long long** d_resched = nullptr, const long long** d_over = nullptr) {
-    const int32_t n = in->n_nodes;
-    const size_t N = (size_t)n, R = (size_t)in->n_reservations;
+    const int32_t n = in.n_nodes();
+    const gp_usage_input* rows = in.rows;
+    const gp_resident_usage* res = in.res;
+    const bool tab = in.table_overhead();
+    const size_t N = (size_t)n, R = rows ? (size_t)rows->n_reservations : 0;
+    const size_t S = res ? (size_t)c->rt.size.n_slots : 0;
+    const size_t RI = res ? (size_t)c->rt.size.n_node_ids : 0, OI = tab ? (size_t)c->oht.size.n_node_ids : 0;
+    const int64_t* const alloc_h[3] = {rows ? rows->alloc_cpu_milli : res->alloc_cpu_milli, rows ? rows->alloc_mem_bytes : res->alloc_mem_bytes,
+                                       rows ? rows->alloc_gpu : res->alloc_gpu};
+    const int64_t* const over_h[3] = {rows ? rows->overhead_cpu_milli : res->overhead_cpu_milli,
+                                      rows ? rows->overhead_mem_bytes : res->overhead_mem_bytes,
+                                      rows ? rows->overhead_gpu : res->overhead_gpu};
     Arena ar{c->usagebuf, st};
-    const auto alloc = ar.take<long long>(3 * N), over = ar.take<long long>(3 * N);
+    // resident overhead: the query's six columns, GetOverhead first
+    const auto alloc = ar.take<long long>(3 * N), over = ar.take<long long>((tab ? 6 : 3) * N);
     const auto usage = ar.take<unsigned long long>(6 * N);
     const auto has = ar.take<unsigned int>(N);
-    const auto err = ar.take<int>(1);
+    const auto err = ar.take<int>(2);
     const auto avail = ar.take<long long>(3 * N), sched = ar.take<long long>(3 * N), resched = ar.take<long long>(3 * N);
     const auto rn = ar.take<int32_t>(R);
     const auto rc = ar.take<long long>(R), rm = ar.take<long long>(R), rg = ar.take<long long>(R);
+    const auto ids = ar.take<int32_t>(res ? N : 0), oids = ar.take<int32_t>(tab ? N : 0);
+    const auto rdir = ar.take<int32_t>(RI), odir = ar.take<int32_t>(OI);
+    const auto acc = ar.take<unsigned long long>(tab ? 12 * N : 0), warned = ar.take<unsigned long long>(tab ? 1 : 0);
     ar.reserve();
-    const long long* al[3] = {ar.put(alloc.part(0, N), in->alloc_cpu_milli), ar.put(alloc.part(N, N), in->alloc_mem_bytes),
-                              ar.put(alloc.part(2 * N, N), in->alloc_gpu)};
-    const long long* ov[3] = {ar.put(over.part(0, N), in->overhead_cpu_milli), ar.put(over.part(N, N), in->overhead_mem_bytes),
-                              ar.put(over.part(2 * N, N), in->overhead_gpu)};
-    ar.fill(usage, err, 0);                             // the usage sums, the has-an-entry flags and the status word
-    const int32_t* r_node = ar.put(rn, in->res_node);
-    const long long* r_cpu = ar.put(rc, in->res_cpu_milli);
-    const long long* r_mem = ar.put(rm, in->res_mem_bytes);
-    const long long* r_gpu = ar.put(rg, in->res_gpu);
-    GP_TRY(ar.check(c));
+    const long long* al[3];
+    const long long* ov[3];
+    for (int d = 0; d < 3; ++d) {
+        al[d] = ar.put(alloc.part(N * d, N), alloc_h[d]);
+        ov[d] = tab ? ar.ptr(over.part(N * d, N)) : ar.put(over.part(N * d, N), over_h[d]);
+    }
+    ar.fill(usage, err, 0);                             // the usage sums, the has-an-entry flags and the status words
     const int T = 256;
-    if (R)
-        gp_usage_scatter<<<(unsigned)((R + T - 1) / T), T, 0, st>>>((long long)R, r_node, r_cpu, r_mem, r_gpu, n, ar.ptr(usage),
-                                                                   d_resched ? ar.ptr(has) : nullptr, ar.ptr(err));
+    if (rows) {
+        const int32_t* r_node = ar.put(rn, rows->res_node);
+        const long long* r_cpu = ar.put(rc, rows->res_cpu_milli);
+        const long long* r_mem = ar.put(rm, rows->res_mem_bytes);
+        const long long* r_gpu = ar.put(rg, rows->res_gpu);
+        GP_TRY(ar.check(c));
+        if (R)
+            gp_usage_scatter<<<(unsigned)((R + T - 1) / T), T, 0, st>>>((long long)R, UsageRowIndex{r_node, n}, r_cpu, r_mem, r_gpu, n,
+                                                                       ar.ptr(usage), d_resched ? ar.ptr(has) : nullptr, ar.ptr(err));
+    } else {
+        const int32_t* d_ids = ar.put(ids, res->node_id);
+        const int32_t* d_oids = tab ? ar.put(oids, res->overhead_node_id) : nullptr;
+        ar.fill(rdir, odir, 0xff);
+        if (tab) ar.fill(acc, warned, 0);
+        GP_TRY(ar.check(c));
+        int* e = ar.ptr(err);
+        gp_resident_dirs<<<(n + T - 1) / T, T, 0, st>>>(n, d_ids, c->rt.size.n_node_ids, ar.ptr(rdir), d_oids, c->oht.size.n_node_ids,
+                                                        ar.ptr(odir), e);
+        if (tab) oht_enqueue_sums(c, st, ar.ptr(odir), n, ar.ptr(acc), ar.ptr(warned), ar.ptr(over), nullptr, e + 1);
+        const RtCols tc = rt_cols(c);
+        if (S)
+            gp_usage_scatter<<<(unsigned)((S + T - 1) / T), T, 0, st>>>((long long)S, UsageSlotDir{tc.node, ar.ptr(rdir)}, tc.v[0], tc.v[1],
+                                                                       tc.v[2], n, ar.ptr(usage), d_resched ? ar.ptr(has) : nullptr, ar.ptr(err));
+    }
     gp_availability<<<(n + T - 1) / T, T, 0, st>>>(n, al[0], al[1], al[2], ov[0], ov[1], ov[2], ar.ptr(usage), ar.ptr(avail), ar.ptr(sched),
                                                    ar.ptr(err), ar.ptr(has), d_resched ? ar.ptr(resched) : nullptr);
     if (d_resched) *d_resched = ar.ptr(resched);
@@ -242,22 +312,22 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const int32_t* i
 // availability (d_avail / d_sched: [3][n_nodes]) -> priority orders on the context's stream.  Synchronises once for the
 // availability stage's status word: a refusal returns before anything of the context's snapshot has been replaced.
 // ig / n_ig: the instance groups of stage_sort, already checked.
-static gp_status prepare_orders(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+static gp_status prepare_orders(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
                                 const char* who, long long** d_avail, long long** d_sched, SortStage* so) {
-    GP_TRY(check_usage(c, usage, who));
-    if (!sort || usage->n_nodes != sort->n_nodes || sort->n_zones < 1)
+    GP_TRY(check_source(c, usage, who));
+    if (!sort || usage.n_nodes() != sort->n_nodes || sort->n_zones < 1)
         return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
-    if (usage->n_nodes == 0) return fail(c, GP_ERR_INVALID, who, "empty node table");
+    if (usage.n_nodes() == 0) return fail(c, GP_ERR_INVALID, who, "empty node table");
     GP_TRY(check_sort_ids(c, sort, who));
     GP_CUDA(c, cudaSetDevice(c->device));
     int* d_err = nullptr;
     GP_TRY(stage_availability(c, usage, c->stream, d_avail, d_sched, &d_err));
-    const size_t N = (size_t)usage->n_nodes;
+    const size_t N = (size_t)usage.n_nodes();
     GP_TRY(stage_sort(c, sort, ig, n_ig, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so));
-    int err = 0;
-    GP_CUDA(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, c->stream));
+    int err[2] = {0, 0};
+    GP_CUDA(c, cudaMemcpyAsync(err, d_err, sizeof err, cudaMemcpyDeviceToHost, c->stream));
     GP_CUDA(c, cudaStreamSynchronize(c->stream));
-    return refuse(c, err, kFeRefusals, who);
+    return stage_refusal(c, err, who);
 }
 
 // gp_prepare_cluster and gp_prepare_cluster_zones after their layout step, which set dn's groups, offsets and orders: the
@@ -284,13 +354,13 @@ static gp_status prepare_snapshot(gp_ctx* c, gp_nodes* dn, const long long* d_av
 // The instance-group arguments of gp_prepare_cluster_groups and gp_prepare_cluster_zones_groups: n_ig >= 1, values in
 // [-1, n_ig), and with several instance groups at most 2^22 (instance group, zone + 1) pairs (stage_sort's zone totals are
 // per pair).  The other arguments are checked by prepare_orders.
-static gp_status check_instance_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+static gp_status check_instance_groups(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
                                        const char* who) {
     if (n_ig < 1) return fail(c, GP_ERR_INVALID, who, "n_instance_groups must be >= 1");
     if (sort && n_ig > 1 && (int64_t)n_ig * ((int64_t)sort->n_zones + 1) > kZoneLayoutMaxPairs)
         return fail(c, GP_ERR_INVALID, who, "n_instance_groups x (n_zones + 1) above 2^22");
-    if (ig && usage && sort && usage->n_nodes == sort->n_nodes)
-        for (int32_t i = 0; i < usage->n_nodes; ++i)
+    if (ig && usage.given() && sort && usage.n_nodes() == sort->n_nodes)
+        for (int32_t i = 0; i < usage.n_nodes(); ++i)
             if (ig[i] < -1 || ig[i] >= n_ig) return fail(c, GP_ERR_INVALID, who, "instance_group outside [-1, n_instance_groups)");
     return GP_OK;
 }
@@ -300,7 +370,7 @@ static gp_status check_instance_groups(gp_ctx* c, const gp_usage_input* usage, c
 // is replaced) -> snapshot group g = instance group g's range of those orders (gp_ig_offsets) -> the slot layout, then one
 // synchronise that reads back counts[3] and, when ig_ties is given, the undefined ties [n_ig] of each instance group.
 // ig NULL with n_ig > 1: every node in instance group 0, the others empty.
-static gp_status prepare_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+static gp_status prepare_groups(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
                                 const char* who, int32_t* counts, int32_t* ig_ties, SortStage* so_out = nullptr) {
     long long *d_avail = nullptr, *d_sched = nullptr;
     SortStage so{};
@@ -314,7 +384,7 @@ static gp_status prepare_groups(gp_ctx* c, const gp_usage_input* usage, const gp
                                                                c->drv_off.as<int32_t>());
     GP_CUDA(c, cudaGetLastError());
     gp_nodes dn{};
-    dn.n_nodes = usage->n_nodes;
+    dn.n_nodes = usage.n_nodes();
     dn.n_groups = n_ig;
     dn.exec_off = c->exec_off.as<int32_t>(); dn.exec_order = so.exe;
     dn.drv_off = c->drv_off.as<int32_t>(); dn.drv_order = so.drv;
@@ -372,7 +442,7 @@ struct ZonePrep {
 // one synchronise that reads back the counts.  zog_now (or NULL): zone_of_group [sort->n_zones + 1] read back in that
 // synchronise; ig_ties (or NULL): the undefined ties [n_ig] likewise.  keep_ig (gp_prepare_cluster_zones_groups): the
 // per-instance-group words are held (Held::groups).  ig NULL with n_ig > 1: every node in instance group 0, the others empty.
-static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
+static gp_status prepare_zones(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const int32_t* ig, int32_t n_ig,
                                int32_t kind, bool keep_ig, const char* who, int32_t* zog_now, int32_t* ig_ties, ZonePrep* zp) {
     if (kind != GP_LAYOUT_SINGLE_AZ && kind != GP_LAYOUT_AZ_AWARE)
         return fail(c, GP_ERR_INVALID, who, "layout->kind must be GP_LAYOUT_SINGLE_AZ or GP_LAYOUT_AZ_AWARE");
@@ -382,7 +452,7 @@ static gp_status prepare_zones(gp_ctx* c, const gp_usage_input* usage, const gp_
     GP_TRY(prepare_orders(c, usage, sort, ig, n_ig, who, &d_avail, &d_sched, &so));
     c->held.commit();                                   // the held orders are overwritten below
     cudaStream_t st = c->stream;
-    const int32_t n = usage->n_nodes;
+    const int32_t n = usage.n_nodes();
     const size_t N = (size_t)n, G1 = (size_t)n_ig + 1;
     // the (instance group, zone) pairs; g_bound groups bound every layout (each instance group: its candidate zones plus
     // one; a candidate zone holds a node).  The slots are laid out for that many (the groups past the last one are empty)
@@ -507,10 +577,11 @@ gp_status gp_prepare_cluster(gp_ctx* c, const gp_usage_input* usage, const gp_so
     return GP_OK;
 }
 
-// the same chain for every instance group at once: snapshot group i holds instance group i's PotentialNodes orders
-gp_status gp_prepare_cluster_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
-                                    int32_t n_instance_groups, gp_instance_group_orders* out) {
-    const char* who = "gp_prepare_cluster_groups";
+}  // extern "C"
+
+// gp_prepare_cluster_groups[_resident]
+static gp_status prepare_cluster_groups(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const int32_t* instance_group,
+                                        int32_t n_instance_groups, gp_instance_group_orders* out, const char* who) {
     if (!enter(c)) return GP_ERR_INVALID;
     if (!out) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     out->n_driver = 0; out->n_executor = 0;
@@ -530,6 +601,20 @@ gp_status gp_prepare_cluster_groups(gp_ctx* c, const gp_usage_input* usage, cons
     ar.get(out->drv_order, so.drv, (size_t)counts[0]);
     if (out->exec_off || out->drv_off || out->exec_order || out->drv_order) GP_TRY(ar.sync(c));
     return GP_OK;
+}
+
+extern "C" {
+
+// the same chain for every instance group at once: snapshot group i holds instance group i's PotentialNodes orders
+gp_status gp_prepare_cluster_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
+                                    int32_t n_instance_groups, gp_instance_group_orders* out) {
+    return prepare_cluster_groups(c, usage, sort, instance_group, n_instance_groups, out, "gp_prepare_cluster_groups");
+}
+
+// the same with the reservations (and optionally the overhead) from the context's resident tables
+gp_status gp_prepare_cluster_groups_resident(gp_ctx* c, const gp_resident_usage* usage, const gp_sort_input* sort,
+                                             const int32_t* instance_group, int32_t n_instance_groups, gp_instance_group_orders* out) {
+    return prepare_cluster_groups(c, usage, sort, instance_group, n_instance_groups, out, "gp_prepare_cluster_groups_resident");
 }
 
 // reservations -> availability -> priority orders -> zone-grouped slot layout, without leaving the device
@@ -554,10 +639,11 @@ gp_status gp_prepare_cluster_zones(gp_ctx* c, const gp_usage_input* usage, const
     return GP_OK;
 }
 
-// the same chain for every instance group at once: the layout of each one is gp_prepare_cluster_zones' on its nodes alone
-gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
-                                          int32_t n_instance_groups, gp_instance_group_layout* layout) {
-    const char* who = "gp_prepare_cluster_zones_groups";
+}  // extern "C"
+
+// gp_prepare_cluster_zones_groups[_resident]
+static gp_status prepare_cluster_zones_groups(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const int32_t* instance_group,
+                                              int32_t n_instance_groups, gp_instance_group_layout* layout, const char* who) {
     if (!enter(c)) return GP_ERR_INVALID;
     if (!layout) return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     layout->n_groups = 0; layout->n_driver = 0; layout->n_executor = 0;
@@ -588,6 +674,20 @@ gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage
         layout->group_drv_order || layout->zone_of_group)
         GP_TRY(ar.sync(c));
     return GP_OK;
+}
+
+extern "C" {
+
+// the same chain for every instance group at once: the layout of each one is gp_prepare_cluster_zones' on its nodes alone
+gp_status gp_prepare_cluster_zones_groups(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const int32_t* instance_group,
+                                          int32_t n_instance_groups, gp_instance_group_layout* layout) {
+    return prepare_cluster_zones_groups(c, usage, sort, instance_group, n_instance_groups, layout, "gp_prepare_cluster_zones_groups");
+}
+
+// the same with the reservations (and optionally the overhead) from the context's resident tables
+gp_status gp_prepare_cluster_zones_groups_resident(gp_ctx* c, const gp_resident_usage* usage, const gp_sort_input* sort,
+                                                   const int32_t* instance_group, int32_t n_instance_groups, gp_instance_group_layout* layout) {
+    return prepare_cluster_zones_groups(c, usage, sort, instance_group, n_instance_groups, layout, "gp_prepare_cluster_zones_groups_resident");
 }
 
 // rescheduleExecutor's node choice for a batch of executors (SURVEY 8f row f4); see gangpack_resched.cuh
@@ -658,16 +758,17 @@ gp_status gp_reschedule_executors(gp_ctx* c, const gp_reschedule* in, int32_t* n
     return GP_OK;
 }
 
-// rescheduleExecutor from the reservations to the node choice (SURVEY 8f row f4); see gangpack_reschedprep.cuh
-gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const gp_reschedule_scope* scope,
-                                          const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous) {
+}  // extern "C"
+
+// gp_reschedule_from_reservations[_resident]
+static gp_status reschedule_from_reservations(gp_ctx* c, const UsageIn& usage, const gp_sort_input* sort, const gp_reschedule_scope* scope,
+                                              const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous, const char* who) {
     if (!enter(c)) return GP_ERR_INVALID;
-    static const char* who = "gp_reschedule_from_reservations";
-    GP_TRY(check_usage(c, usage, who));
-    if (!sort || !in || usage->n_nodes != sort->n_nodes || sort->n_zones < 1 ||
+    GP_TRY(check_source(c, usage, who));
+    if (!sort || !in || usage.n_nodes() != sort->n_nodes || sort->n_zones < 1 ||
         in->n_execs < 0 || (in->n_execs > 0 && (!in->exe_cpu_milli || !in->exe_mem_bytes || !node_out)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
-    const int32_t n = usage->n_nodes, q = in->n_execs;
+    const int32_t n = usage.n_nodes(), q = in->n_execs;
     if (n == 0) return fail(c, GP_ERR_INVALID, who, "empty node table");
     if (in->reserved_cpu_milli || in->reserved_mem_bytes || in->reserved_gpu)
         return fail(c, GP_ERR_INVALID, who, "reserved_* must be NULL (the overhead of the node table is the reserved amount)");
@@ -748,10 +849,25 @@ gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage
     GP_CUDA(c, cudaGetLastError());
     ar.get(node_out, d_out);
     ar.get(ambiguous, amb);
-    int err = 0;
-    ar.get(&err, d_err, 1);
+    int err[2] = {0, 0};
+    ar.get(err, d_err, 2);
     GP_TRY(ar.sync(c));
-    return refuse(c, err, kFeRefusals, who);            // refused: node_out / ambiguous hold no decision
+    return stage_refusal(c, err, who);                  // refused: node_out / ambiguous hold no decision
+}
+
+extern "C" {
+
+// rescheduleExecutor from the reservations to the node choice (SURVEY 8f row f4); see gangpack_reschedprep.cuh
+gp_status gp_reschedule_from_reservations(gp_ctx* c, const gp_usage_input* usage, const gp_sort_input* sort, const gp_reschedule_scope* scope,
+                                          const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous) {
+    return reschedule_from_reservations(c, usage, sort, scope, in, node_out, ambiguous, "gp_reschedule_from_reservations");
+}
+
+// the same with the reservations (and optionally the overhead) from the context's resident tables
+gp_status gp_reschedule_from_reservations_resident(gp_ctx* c, const gp_resident_usage* usage, const gp_sort_input* sort,
+                                                   const gp_reschedule_scope* scope, const gp_reschedule* in, int32_t* node_out,
+                                                   uint8_t* ambiguous) {
+    return reschedule_from_reservations(c, usage, sort, scope, in, node_out, ambiguous, "gp_reschedule_from_reservations_resident");
 }
 
 // the failover reconciler's findNodes loop for a batch of stale drivers (EXT/failover.go:43-82, 286-436); see

@@ -223,6 +223,14 @@ struct gp_ctx {
         uint32_t seq = 0;                         // the last update's stamp
     } oht;
 
+    // the resident reservation table (gangpack_reservation_table.cu); read by the *_resident entries, changed only by its own
+    struct ReservationTable {
+        bool live = false;                        // reset and not broken by a CUDA error since
+        gp_reservation_table_size size{};
+        DevBuf cols;                              // node id [n_slots], cpu / mem / gpu [3][n_slots], duplicate stamps [n_slots]
+        uint32_t seq = 0;                         // the last update's stamp
+    } rt;
+
     gp_stats last{};
 };
 
@@ -374,3 +382,19 @@ gp_status pack_device_range(gp_ctx* c, const DevApps& da, int32_t lo, int32_t hi
                             const DevResults& dr, int2* scratch, cudaStream_t st, int chunk, bool status_in_kernel = false,
                             bool after_layout = false);
 gp_status host_error(gp_ctx* c);
+
+// ---- gangpack_overhead_table.cu --------------------------------------------------------------------------------------
+
+// Enqueue GetOverhead and GetNonSchedulableOverhead of the live overhead table into out[6][n_rows] (overhead cpu, mem, gpu,
+// then non-schedulable), a slot counting towards row_of_node[its node id] (-1: none).  Scratch is the caller's: acc
+// [12 * n_rows] and *n_warned zeroed, has_reservation [n_slots] or NULL.  *d_err receives the query's bits, decoded by
+// oht_sum_refusal once the stream has been synchronised.
+void oht_enqueue_sums(gp_ctx* c, cudaStream_t st, const int32_t* row_of_node, int32_t n_rows, unsigned long long* acc,
+                      unsigned long long* n_warned, long long* out, uint8_t* has_reservation, int* d_err);
+gp_status oht_sum_refusal(gp_ctx* c, int word, const char* who);
+
+// ---- gangpack_reservation_table.cu -----------------------------------------------------------------------------------
+
+// The live reservation table's columns on the device: node id [n_slots] (-1 = free) and cpu / mem / gpu [n_slots] each
+struct RtCols { const int32_t* node; const long long* v[3]; };
+RtCols rt_cols(gp_ctx* c);

@@ -68,6 +68,33 @@ static uint32_t pow2_at_least(long long n, uint32_t lo) {
     return h;
 }
 
+void oht_enqueue_sums(gp_ctx* c, cudaStream_t st, const int32_t* row_of_node, int32_t n_rows, unsigned long long* acc,
+                      unsigned long long* n_warned, long long* out, uint8_t* has_reservation, int* d_err) {
+    auto& t = c->oht;
+    const size_t S = (size_t)t.size.n_slots;
+    Arena tc{t.cols, st};
+    const OhtPieces p = take_cols(tc, t.size);
+    const OhtCols T = cols_of(tc, p, S);
+    const OhAcc A{acc, n_warned, n_rows};
+    if (S > 0) {
+        OhPodsIn pi{};
+        pi.n = (long long)S;
+        pi.n_node_ids = t.size.n_node_ids; pi.n_app_keys = t.size.n_app_keys; pi.n_app_ids = t.size.n_app_ids; pi.n_names = t.size.n_names;
+        pi.node_id = T.node_id;
+        for (int d = 0; d < 3; ++d) pi.req[d] = T.req[d];
+        pi.listed = T.listed;
+        pi.app_key = T.app_key; pi.app_id = T.app_id; pi.name_id = T.name_id;
+        pi.is_executor = T.is_executor; pi.spark_scheduler = T.spark_scheduler;
+        pi.has_reservation = has_reservation;
+        const OhTableLookup L{T.rr, OhtSet{t.set[t.cur].as<unsigned long long>(), t.cells - 1}, row_of_node};
+        gp_oh_pods<<<(unsigned)((S + kOhThreads - 1) / kOhThreads), kOhThreads, 0, st>>>(pi, L, A, d_err);
+    }
+    const int B = 256;
+    if (n_rows > 0) gp_oh_finish<<<(unsigned)((n_rows + B - 1) / B), B, 0, st>>>(A, out, d_err);
+}
+
+gp_status oht_sum_refusal(gp_ctx* c, int word, const char* who) { return refuse(c, word, kOhtQueryRefusals, who); }
+
 extern "C" {
 
 gp_status gp_overhead_table_reset(gp_ctx* c, const gp_overhead_table_size* z) {
@@ -225,9 +252,6 @@ gp_status gp_overhead_table_query(gp_ctx* c, int32_t n_nodes, const int32_t* nod
     ar.fill(acc, word, 0);
     ar.put(qn, node_ids);
     GP_TRY(ar.check(c));
-    Arena tc{t.cols, st};
-    const OhtPieces p = take_cols(tc, t.size);
-    const OhtCols T = cols_of(tc, p, S);
     int* d_err = &ar.ptr(word)->err;
     const int B = 256, cap = c->sm_count * 8;
     OhMaps M{nullptr, nullptr, ar.ptr(ron), nullptr, 0, 0};
@@ -235,21 +259,8 @@ gp_status gp_overhead_table_query(gp_ctx* c, int32_t n_nodes, const int32_t* nod
         OhDirIn D{0, 0, n_nodes, 0, 0, t.size.n_node_ids, nullptr, nullptr, ar.ptr(qn)};
         gp_oh_dir<<<(unsigned)std::min<long long>(((long long)N + B - 1) / B, cap), B, 0, st>>>(D, M, d_err);
     }
-    OhAcc A{ar.ptr(acc), &ar.ptr(word)->n_warned, n_nodes};
-    if (S > 0) {
-        OhPodsIn pi{};
-        pi.n = (long long)S;
-        pi.n_node_ids = t.size.n_node_ids; pi.n_app_keys = t.size.n_app_keys; pi.n_app_ids = t.size.n_app_ids; pi.n_names = t.size.n_names;
-        pi.node_id = T.node_id;
-        for (int d = 0; d < 3; ++d) pi.req[d] = T.req[d];
-        pi.listed = T.listed;
-        pi.app_key = T.app_key; pi.app_id = T.app_id; pi.name_id = T.name_id;
-        pi.is_executor = T.is_executor; pi.spark_scheduler = T.spark_scheduler;
-        pi.has_reservation = out->has_reservation ? ar.ptr(has) : nullptr;
-        const OhTableLookup L{T.rr, OhtSet{t.set[t.cur].as<unsigned long long>(), t.cells - 1}, ar.ptr(ron)};
-        gp_oh_pods<<<(unsigned)((S + kOhThreads - 1) / kOhThreads), kOhThreads, 0, st>>>(pi, L, A, d_err);
-    }
-    if (N > 0) gp_oh_finish<<<(unsigned)((N + B - 1) / B), B, 0, st>>>(A, ar.ptr(d_out), d_err);
+    oht_enqueue_sums(c, st, ar.ptr(ron), n_nodes, ar.ptr(acc), &ar.ptr(word)->n_warned, ar.ptr(d_out),
+                     out->has_reservation ? ar.ptr(has) : nullptr, d_err);
     GP_CUDA(c, cudaGetLastError());
     int64_t* outs[6] = {out->overhead_cpu_milli, out->overhead_mem_bytes, out->overhead_gpu,
                         out->nonsched_cpu_milli, out->nonsched_mem_bytes, out->nonsched_gpu};

@@ -62,7 +62,25 @@ __device__ __forceinline__ bool exact_value(const ExactSum& s, long long* v) {
 enum : int {
     kFeErrInput = 1,        // |allocatable|, |overhead| or |a counted reservation| >= 2^61
     kFeErrResult = 2,       // a usage sum or an availability outside the exact-int64 domain
+    kFeErrId = 4,           // resident forms: a reservation-table or overhead-table node id out of range or given twice
 };
+
+// The resident forms' directories: dir[id] = i for every node-table entry i with ids[i] != -1 (the directory is memset to -1
+// first); atomicCAS from -1, so an id given twice is a refusal, not an overwrite.  Thread per entry of each of the two arrays
+// (b_ids NULL: one).
+__global__ void gp_resident_dirs(int32_t n, const int32_t* __restrict__ a_ids, int32_t a_lim, int32_t* __restrict__ a_dir,
+                                 const int32_t* __restrict__ b_ids, int32_t b_lim, int32_t* __restrict__ b_dir, int* __restrict__ err) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    bool bad = false;
+    const int32_t a = a_ids[i];
+    if (a != -1) bad |= a < 0 || a >= a_lim || atomicCAS(a_dir + a, -1, i) != -1;
+    if (b_ids) {
+        const int32_t b = b_ids[i];
+        if (b != -1) bad |= b < 0 || b >= b_lim || atomicCAS(b_dir + b, -1, i) != -1;
+    }
+    if (bad) atomicOr(err, kFeErrId);
+}
 
 struct SortKey {          // 24 bytes
     long long mem;
@@ -319,14 +337,33 @@ __global__ void gp_label_scatter(const int32_t* __restrict__ count_ptr, const in
 // summed as in GetReservedResources (EXT/resourcereservations.go:258-263).  A segmented reduction over
 // (reservation -> node) pairs: thread per reservation, exact_add per dimension (integer adds commute: exact, and no
 // sum wraps).  usage[(2 * d + half) * n_nodes + node]: dimension d, half 0 = lo, 1 = hi.
-__global__ void gp_usage_scatter(long long n_res, const int32_t* __restrict__ res_node, const long long* __restrict__ res_cpu,
+// Where finds the node-table index of row r (-1: the row is not counted): UsageRowIndex for the per-call rows, UsageSlotDir for
+// the slots of the resident reservation table.
+struct UsageRowIndex {                  // gp_usage_input.res_node: an index outside [0, n_nodes) is not in the list
+    const int32_t* res_node;
+    int32_t n_nodes;
+    __device__ int32_t operator()(long long r) const {
+        const int32_t node = res_node[r];
+        return node < 0 || node >= n_nodes ? -1 : node;
+    }
+};
+struct UsageSlotDir {                   // a slot's node id through the per-call directory (node id -> node-table index, -1 = none)
+    const int32_t* slot_node;           // [n_slots] -1 = free slot; occupied slots hold ids in [0, n_node_ids), checked when written
+    const int32_t* dir;                 // [n_node_ids]
+    __device__ int32_t operator()(long long r) const {
+        const int32_t id = slot_node[r];
+        return id < 0 ? -1 : dir[id];
+    }
+};
+template <class Where>
+__global__ void gp_usage_scatter(long long n_res, Where where, const long long* __restrict__ res_cpu,
                                  const long long* __restrict__ res_mem, const long long* __restrict__ res_gpu, int32_t n_nodes,
                                  unsigned long long* __restrict__ usage /* [6][n_nodes] */, unsigned int* __restrict__ has_entry /* [n_nodes] or NULL */,
                                  int* __restrict__ err) {
     const long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (r >= n_res) return;
-    const int32_t node = res_node[r];
-    if (node < 0 || node >= n_nodes) return;            // reservation on a node that is not in the list: ignored (:67-75)
+    const int32_t node = where(r);
+    if (node < 0) return;                               // reservation on a node that is not in the list: ignored (:67-75)
     if (has_entry) has_entry[node] = 1u;                // the usage map has an entry for this node (whatever its value)
     const long long v[3] = {res_cpu[r], res_mem[r], res_gpu ? res_gpu[r] : 0};
     const size_t N = (size_t)n_nodes;

@@ -1878,6 +1878,143 @@ private:
     std::map<Member, bool> memberTouched_;
 };
 
+// GetReservedResources' rows (resourcereservations.go:258-263) over the context's resident reservation table
+// (gp_reservation_table_*): the ResourceReservation cache's and the soft store's events as their handlers deliver them, one
+// slot per Spec.Reservations entry or soft reservation.  Flush() sends what changed since the last one as at most one
+// gp_reservation_table_update -- call it once per Predicate, before gp_prepare_cluster_*_resident or
+// gp_reschedule_from_reservations_resident with NodeIDs(nodes).  Freed slots are reused and node ids are reference-counted;
+// a capacity that would be exceeded is doubled, and after a reset, a refused or a failed update the whole state is sent
+// again until an update succeeds.  The table belongs to the device context, so one instance per context.
+class ResidentReservations {
+public:
+    struct Reservation { std::string Node; resources::Resources Res; };
+    using Entries = std::map<std::string, Reservation>;           // name (reservation entry or pod) -> reservation
+
+    explicit ResidentReservations(gp_reservation_table_size initial = {64, 64}) : size_(initial) {}
+
+    // a ResourceReservation created, updated or rewritten by compaction (its Spec.Reservations), and its deletion
+    void SetResourceReservation(const std::string& ns, const std::string& app, const Entries& e) { set(0, ns + '\x00' + app, e, rrs_); }
+    void DeleteResourceReservation(const std::string& ns, const std::string& app) { set(0, ns + '\x00' + app, {}, rrs_); }
+    // the soft store's reservations of appID (pod name -> reservation), and their removal
+    void SetSoftReservations(const std::string& app, const Entries& e) { set(1, app, e, soft_); }
+    void DeleteSoftReservations(const std::string& app) { set(1, app, {}, soft_); }
+
+    // the table's id of each node name, -1 for a node no reservation names
+    std::vector<int32_t> NodeIDs(const std::vector<std::string>& nodes) const {
+        std::vector<int32_t> ids(nodes.size(), -1);
+        for (size_t i = 0; i < nodes.size(); ++i) {
+            auto it = nodes_.find(nodes[i]);
+            if (it != nodes_.end()) ids[i] = it->second;
+        }
+        return ids;
+    }
+
+    void Flush(gangpack::Device& dev) {
+        auto grow = [&](int64_t& cap, int64_t need) { while (cap < need) { cap = std::max<int64_t>(2 * cap, 1); replay_ = true; } };
+        int64_t caps[2] = {size_.n_slots, size_.n_node_ids};
+        grow(caps[0], (int64_t)rows_.size());
+        grow(caps[1], (int64_t)nodeCount_.size());
+        size_ = gp_reservation_table_size{caps[0], (int32_t)caps[1]};
+        std::vector<int32_t> slot, node;
+        std::vector<int64_t> cpu, mem, gpu;
+        auto row = [&](size_t i) {
+            slot.push_back((int32_t)i); node.push_back(rows_[i].node);
+            cpu.push_back(rows_[i].v[0]); mem.push_back(rows_[i].v[1]); gpu.push_back(rows_[i].v[2]);
+        };
+        if (replay_) {
+            for (size_t i = 0; i < rows_.size(); ++i) if (rows_[i].node != -1) row(i);
+        } else {
+            for (const auto& kv : dirty_) if (rows_[kv.first] != kv.second) row(kv.first);
+        }
+        const bool reset = replay_;
+        replay_ = true;                            // until the table holds this state: a failed call replays next time
+        if (reset) dev.check(gp_reservation_table_reset(dev.ctx(), &size_), "gp_reservation_table_reset");
+        if (!slot.empty()) {
+            gp_reservation_delta d{(int64_t)slot.size(), slot.data(), node.data(), cpu.data(), mem.data(), gpu.data()};
+            dev.check(gp_reservation_table_update(dev.ctx(), &d), "gp_reservation_table_update");
+        }
+        replay_ = false;
+        dirty_.clear();
+    }
+
+private:
+    struct Row {
+        int32_t node = -1;
+        int64_t v[3] = {0, 0, 0};
+        bool operator!=(const Row& o) const { return node != o.node || v[0] != o.v[0] || v[1] != o.v[1] || v[2] != o.v[2]; }
+    };
+    using Key = std::tuple<int, std::string, std::string>;       // (kind, owner, name)
+
+    void set(int kind, const std::string& owner, const Entries& now, std::map<std::string, Entries>& store) {
+        Entries old;
+        auto it = store.find(owner);
+        if (it != store.end()) { old = std::move(it->second); store.erase(it); }
+        if (!now.empty()) store[owner] = now;
+        for (const auto& kv : old)
+            if (!now.count(kv.first)) {
+                auto s = slot_.find(Key{kind, owner, kv.first});
+                write(s->second, nullptr);
+                slot_.erase(s);
+            }
+        for (const auto& kv : now) {
+            const Key k{kind, owner, kv.first};
+            auto s = slot_.find(k);
+            size_t at;
+            if (s == slot_.end()) {
+                if (!free_.empty()) { at = free_.back(); free_.pop_back(); }
+                else { at = rows_.size(); rows_.emplace_back(); nodeOf_.emplace_back(); }
+                slot_.emplace(k, at);
+            } else {
+                at = s->second;
+                auto o = old.find(kv.first);
+                if (o != old.end() && o->second.Node == kv.second.Node && o->second.Res.Eq(kv.second.Res)) continue;
+            }
+            write(at, &kv.second);
+        }
+    }
+    // slot at := r, or free it (r NULL); the node reference of the new row is taken before the old row's is released
+    void write(size_t at, const Reservation* r) {
+        dirty_.emplace(at, rows_[at]);
+        Row row;
+        if (r) {
+            row.node = acquire(r->Node);
+            row.v[0] = r->Res.CPU; row.v[1] = r->Res.Memory; row.v[2] = r->Res.NvidiaGPU;
+        }
+        if (!nodeOf_[at].empty()) release(nodeOf_[at]);
+        rows_[at] = row;
+        nodeOf_[at] = r ? r->Node : std::string();
+        if (!r) free_.push_back(at);
+    }
+    int32_t acquire(const std::string& n) {
+        auto it = nodes_.find(n);
+        int32_t i;
+        if (it != nodes_.end()) i = it->second;
+        else {
+            if (!freeIds_.empty()) { i = freeIds_.back(); freeIds_.pop_back(); }
+            else { i = (int32_t)nodeCount_.size(); nodeCount_.push_back(0); }
+            nodes_.emplace(n, i);
+        }
+        ++nodeCount_[(size_t)i];
+        return i;
+    }
+    void release(const std::string& n) {
+        auto it = nodes_.find(n);
+        const int32_t i = it->second;
+        if (--nodeCount_[(size_t)i] == 0) { nodes_.erase(it); freeIds_.push_back(i); }
+    }
+
+    gp_reservation_table_size size_;
+    bool replay_ = true;
+    std::map<std::string, Entries> rrs_, soft_;
+    std::map<Key, size_t> slot_;
+    std::vector<Row> rows_;
+    std::vector<std::string> nodeOf_;                             // per slot: the node name its row holds ("" = free)
+    std::vector<size_t> free_;
+    std::unordered_map<std::string, int32_t> nodes_;
+    std::vector<int32_t> nodeCount_, freeIds_;
+    std::map<size_t, Row> dirty_;                                 // -> the row the table holds
+};
+
 }  // namespace extender
 
 // ------------------------------------------------------------------------------------------------

@@ -38,6 +38,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_reschedule_executors", "gp_reschedule_from_reservations", "gp_packing_efficiency", "gp_exceeds_cluster_capacity",
            "gp_reconcile_find_nodes", "gp_match_node_affinity", "gp_exceeds_cluster_capacity_affinity",
            "gp_node_overhead", "gp_overhead_table_reset", "gp_overhead_table_update", "gp_overhead_table_query",
+           "gp_reservation_table_reset", "gp_reservation_table_update", "gp_prepare_cluster_groups_resident",
+           "gp_prepare_cluster_zones_groups_resident", "gp_reschedule_from_reservations_resident",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -253,6 +255,21 @@ class gp_overhead_delta(C.Structure):
                 ("member_kind", C.c_void_p), ("member_app", C.c_void_p), ("member_name", C.c_void_p), ("member_present", C.c_void_p)]
 
 
+class gp_reservation_table_size(C.Structure):
+    _fields_ = [("n_slots", C.c_int64), ("n_node_ids", C.c_int32)]
+
+
+class gp_reservation_delta(C.Structure):
+    _fields_ = [("n_write", C.c_int64), ("slot", C.c_void_p), ("node_id", C.c_void_p), ("cpu_milli", C.c_void_p),
+                ("mem_bytes", C.c_void_p), ("gpu", C.c_void_p)]
+
+
+class gp_resident_usage(C.Structure):
+    _fields_ = [("n_nodes", C.c_int32), ("node_id", C.c_void_p), ("alloc_cpu_milli", C.c_void_p), ("alloc_mem_bytes", C.c_void_p),
+                ("alloc_gpu", C.c_void_p), ("overhead_node_id", C.c_void_p), ("overhead_cpu_milli", C.c_void_p),
+                ("overhead_mem_bytes", C.c_void_p), ("overhead_gpu", C.c_void_p)]
+
+
 class gp_placement_record(C.Structure):
     _fields_ = [("collocation", C.c_int32), ("distinct_exec_nodes", C.c_int32), ("execs_per_node", C.c_int32), ("n_zones", C.c_int32),
                 ("cross_zone_pairs", C.c_int64), ("total_pairs", C.c_int64)]
@@ -355,6 +372,20 @@ def load():
     L.gp_overhead_table_update.argtypes = [C.c_void_p, C.POINTER(gp_overhead_delta)]
     L.gp_overhead_table_query.restype = C.c_int
     L.gp_overhead_table_query.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(gp_overhead_out)]
+    L.gp_reservation_table_reset.restype = C.c_int
+    L.gp_reservation_table_reset.argtypes = [C.c_void_p, C.POINTER(gp_reservation_table_size)]
+    L.gp_reservation_table_update.restype = C.c_int
+    L.gp_reservation_table_update.argtypes = [C.c_void_p, C.POINTER(gp_reservation_delta)]
+    L.gp_prepare_cluster_groups_resident.restype = C.c_int
+    L.gp_prepare_cluster_groups_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input), C.c_void_p,
+                                                     C.c_int32, C.POINTER(gp_instance_group_orders)]
+    L.gp_prepare_cluster_zones_groups_resident.restype = C.c_int
+    L.gp_prepare_cluster_zones_groups_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input),
+                                                           C.c_void_p, C.c_int32, C.POINTER(gp_instance_group_layout)]
+    L.gp_reschedule_from_reservations_resident.restype = C.c_int
+    L.gp_reschedule_from_reservations_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input),
+                                                           C.POINTER(gp_reschedule_scope), C.POINTER(gp_reschedule), C.c_void_p,
+                                                           C.c_void_p]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -438,6 +469,18 @@ def _usage_input(alloc, overhead, res_node, res):
     return ui
 
 
+def _resident_usage(node_id, alloc, overhead=None, overhead_node_id=None):
+    """gp_resident_usage: node_id[n] reservation-table ids, alloc / overhead (cpu, mem[, gpu]) triples (overhead may be None),
+    overhead_node_id[n] overhead-table ids or None (overhead from the host arrays).  The struct keeps its arrays alive."""
+    ids, al = _np(node_id, np.int32), _triple(alloc)
+    ov = _triple(overhead) if overhead is not None else [None] * 3
+    oid = _np(overhead_node_id, np.int32)
+    ru = gp_resident_usage(n_nodes=len(ids), node_id=_p(ids), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]), alloc_gpu=_p(al[2]),
+                           overhead_node_id=_p(oid), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]))
+    ru._keep = (ids, al, ov, oid)
+    return ru
+
+
 def _sort_input(n, n_zones, zone_id=None, name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None,
                 driver_label_rank=None, executor_label_rank=None, avail=(None, None, None), ties=None):
     """gp_sort_input over n nodes.  avail: the host (cpu, mem, gpu) availability, None where the availability stage
@@ -503,6 +546,9 @@ _DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "req_cpu_milli": np.int64,
                "listed": np.uint8, "app_key": np.int32, "app_id": np.int32, "name_id": np.int32, "is_executor": np.uint8,
                "spark_scheduler": np.uint8, "rr_app_key": np.int32, "rr_exists": np.uint8, "member_kind": np.uint8,
                "member_app": np.int32, "member_name": np.int32, "member_present": np.uint8}
+
+# gp_reservation_delta's columns (reservations.ReservationTable.delta() keys)
+_RT_DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "cpu_milli": np.int64, "mem_bytes": np.int64, "gpu": np.int64}
 
 _OVERHEAD_COLS = {"node_id": np.int32, "req_cpu_milli": np.int64, "req_mem_bytes": np.int64, "req_gpu": np.int64, "listed": np.uint8,
                   "app_key": np.int32, "app_id": np.int32, "name_id": np.int32, "is_executor": np.uint8, "spark_scheduler": np.uint8,
@@ -682,7 +728,22 @@ class GangPacker:
         node) or the zone id filterNodesToZone keeps, with topology_zone[n] the node's zone id (-1 = label missing).
         The context's snapshot is not touched.  The domain and its refusal as in build_availability; name_rank must be a
         permutation (GP_ERR_INVALID).  -> (node index per executor or -1, ambiguous flag per executor)."""
-        ui = _usage_input(alloc, overhead, res_node, res)
+        return self._reschedule(load().gp_reschedule_from_reservations, _usage_input(alloc, overhead, res_node, res), exe, min_frag,
+                                hosting, zone_id, n_zones, name_rank, unschedulable, ready, executor_label_rank, keep_topology_zone,
+                                topology_zone)
+
+    def reschedule_from_reservations_resident(self, node_id, alloc, overhead, exe, min_frag=False, hosting=None, zone_id=None,
+                                              n_zones=1, name_rank=None, unschedulable=None, ready=None, executor_label_rank=None,
+                                              keep_topology_zone=None, topology_zone=None, overhead_node_id=None):
+        """reschedule_from_reservations with the reservations from the resident reservation table: node_id[n] = each node's
+        reservation-table id (-1 = none); overhead from the host triple (or None), or with overhead_node_id[n] from the
+        resident overhead table.  Returns what reschedule_from_reservations returns on the equivalent rows."""
+        return self._reschedule(load().gp_reschedule_from_reservations_resident, _resident_usage(node_id, alloc, overhead, overhead_node_id),
+                                exe, min_frag, hosting, zone_id, n_zones, name_rank, unschedulable, ready, executor_label_rank,
+                                keep_topology_zone, topology_zone)
+
+    def _reschedule(self, fn, ui, exe, min_frag, hosting, zone_id, n_zones, name_rank, unschedulable, ready, executor_label_rank,
+                    keep_topology_zone, topology_zone):
         n = ui.n_nodes
         si = _sort_input(n, n_zones, zone_id=zone_id, name_rank=name_rank, unschedulable=unschedulable, ready=ready,
                          executor_label_rank=executor_label_rank)
@@ -698,8 +759,7 @@ class GangPacker:
                           host_off=_p(hoff), host_nodes=_p(hn))
         out = np.full(max(q, 1), -9, np.int32)
         amb = np.full(max(q, 1), 9, np.uint8)
-        self._check(load().gp_reschedule_from_reservations(self._h, C.byref(ui), C.byref(si), C.byref(scope) if scope is not None else None,
-                                                           C.byref(r), _p(out), _p(amb)))
+        self._check(fn(self._h, C.byref(ui), C.byref(si), C.byref(scope) if scope is not None else None, C.byref(r), _p(out), _p(amb)))
         return out[:q], amb[:q]
 
     def prepare_cluster(self, alloc, overhead, res_node, res, zone_id=None, n_zones=1, name_rank=None, is_driver_candidate=None,
@@ -752,7 +812,24 @@ class GangPacker:
         and, with `layout`, the undivided exec_order / drv_order, the grouped group_exec_off / group_exec_order /
         group_drv_off / group_drv_order and zone_of_group.  The context then holds the layout pack_fifo_zones_groups drains
         when its layout arguments are all None.  A refused call leaves the context as it was."""
-        ui = _usage_input(alloc, overhead, res_node, res)
+        return self._prepare_zones_groups(load().gp_prepare_cluster_zones_groups, _usage_input(alloc, overhead, res_node, res),
+                                          instance_group, n_instance_groups, zone_id, n_zones, name_rank, is_driver_candidate,
+                                          unschedulable, ready, driver_label_rank, executor_label_rank, kind, layout)
+
+    def prepare_cluster_zones_groups_resident(self, node_id, alloc, overhead, instance_group, n_instance_groups, zone_id=None, n_zones=1,
+                                              name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None,
+                                              driver_label_rank=None, executor_label_rank=None, kind=LAYOUT_AZ_AWARE, layout=True,
+                                              overhead_node_id=None):
+        """prepare_cluster_zones_groups with the reservations from the resident reservation table (node_id, overhead and
+        overhead_node_id as in reschedule_from_reservations_resident).  Returns what prepare_cluster_zones_groups returns on
+        the equivalent rows, and leaves the context as it would."""
+        return self._prepare_zones_groups(load().gp_prepare_cluster_zones_groups_resident,
+                                          _resident_usage(node_id, alloc, overhead, overhead_node_id), instance_group, n_instance_groups,
+                                          zone_id, n_zones, name_rank, is_driver_candidate, unschedulable, ready, driver_label_rank,
+                                          executor_label_rank, kind, layout)
+
+    def _prepare_zones_groups(self, fn, ui, instance_group, n_instance_groups, zone_id, n_zones, name_rank, is_driver_candidate,
+                              unschedulable, ready, driver_label_rank, executor_label_rank, kind, layout):
         n = ui.n_nodes
         G = int(n_instance_groups)
         ig = _np(instance_group, np.int32)
@@ -766,7 +843,7 @@ class GangPacker:
             bufs.update({k: np.full(max(n, 1), -9, np.int32) for k in ("exec_order", "drv_order", "group_exec_order", "group_drv_order")})
             bufs.update({k: np.full(n_groups_max + 1, -9, np.int32) for k in ("group_exec_off", "group_drv_off", "zone_of_group")})
         lo = gp_instance_group_layout(kind=int(kind), **{k: _p(v) for k, v in bufs.items()})
-        self._check(load().gp_prepare_cluster_zones_groups(self._h, C.byref(ui), C.byref(si), _p(ig), G, C.byref(lo)))
+        self._check(fn(self._h, C.byref(ui), C.byref(si), _p(ig), G, C.byref(lo)))
         self.n_nodes = n
         out = dict(n_groups=lo.n_groups, n_driver=lo.n_driver, n_executor=lo.n_executor, undefined_ties=ties.value,
                    group_off=bufs["group_off"].copy(), n_zones=bufs["n_zones"][:G].copy(), exec_off=bufs["exec_off"].copy(),
@@ -789,7 +866,22 @@ class GangPacker:
         n_executor, undefined_ties (the total), ig_undefined_ties (per instance group) and, with `orders`, exec_off / drv_off
         ([n_instance_groups + 1]) and the instance-group-major exec_order / drv_order.  A refused call leaves the context as
         it was."""
-        ui = _usage_input(alloc, overhead, res_node, res)
+        return self._prepare_groups(load().gp_prepare_cluster_groups, _usage_input(alloc, overhead, res_node, res), instance_group,
+                                    n_instance_groups, zone_id, n_zones, name_rank, is_driver_candidate, unschedulable, ready,
+                                    driver_label_rank, executor_label_rank, orders)
+
+    def prepare_cluster_groups_resident(self, node_id, alloc, overhead, instance_group, n_instance_groups, zone_id=None, n_zones=1,
+                                        name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None, driver_label_rank=None,
+                                        executor_label_rank=None, orders=True, overhead_node_id=None):
+        """prepare_cluster_groups with the reservations from the resident reservation table (node_id, overhead and
+        overhead_node_id as in reschedule_from_reservations_resident).  Returns what prepare_cluster_groups returns on the
+        equivalent rows, and leaves the context as it would."""
+        return self._prepare_groups(load().gp_prepare_cluster_groups_resident, _resident_usage(node_id, alloc, overhead, overhead_node_id),
+                                    instance_group, n_instance_groups, zone_id, n_zones, name_rank, is_driver_candidate, unschedulable,
+                                    ready, driver_label_rank, executor_label_rank, orders)
+
+    def _prepare_groups(self, fn, ui, instance_group, n_instance_groups, zone_id, n_zones, name_rank, is_driver_candidate, unschedulable,
+                        ready, driver_label_rank, executor_label_rank, orders):
         n = ui.n_nodes
         G = int(n_instance_groups)
         ig = _np(instance_group, np.int32)
@@ -801,7 +893,7 @@ class GangPacker:
             bufs.update({k: np.full(max(G, 0) + 1, -9, np.int32) for k in ("exec_off", "drv_off")})
             bufs.update({k: np.full(max(n, 1), -9, np.int32) for k in ("exec_order", "drv_order")})
         o = gp_instance_group_orders(**{k: _p(v) for k, v in bufs.items()})
-        self._check(load().gp_prepare_cluster_groups(self._h, C.byref(ui), C.byref(si), _p(ig), G, C.byref(o)))
+        self._check(fn(self._h, C.byref(ui), C.byref(si), _p(ig), G, C.byref(o)))
         self.n_nodes = n
         out = dict(n_driver=o.n_driver, n_executor=o.n_executor, undefined_ties=ties.value,
                    ig_undefined_ties=bufs["undefined_ties"][:G].copy())
@@ -1146,6 +1238,18 @@ class GangPacker:
         self._check(load().gp_overhead_table_query(self._h, n, _p(qn), C.byref(out)))
         return (tuple(x[:n] for x in res[:3]), tuple(x[:n] for x in res[3:]),
                 None if has is None else has[:slots], warned.value)
+
+    # ---- the resident reservation table (gp_reservation_table_*) ---------------------------------------------------------
+    def reservation_table_reset(self, n_slots, n_node_ids):
+        """Replace the context's reservation table with an empty one of these capacities."""
+        self._check(load().gp_reservation_table_reset(self._h, C.byref(gp_reservation_table_size(int(n_slots), int(n_node_ids)))))
+
+    def reservation_table_update(self, delta: dict):
+        """One gp_reservation_table_update over the arrays of reservations.ReservationTable.delta() (slot, node_id, cpu_milli,
+        mem_bytes and optionally gpu; the "reset" entry is not read here)."""
+        col = {k: _np(delta.get(k), t) for k, t in _RT_DELTA_COLS.items()}
+        d = gp_reservation_delta(n_write=0 if col["slot"] is None else len(col["slot"]), **{k: _p(v) for k, v in col.items()})
+        self._check(load().gp_reservation_table_update(self._h, C.byref(d)))
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
