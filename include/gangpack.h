@@ -1112,6 +1112,29 @@ gp_status gp_prepare_cluster_zones_groups_resident(gp_ctx* ctx, const gp_residen
 gp_status gp_reschedule_from_reservations_resident(gp_ctx* ctx, const gp_resident_usage* usage, const gp_sort_input* sort,
                                                    const gp_reschedule_scope* scope, const gp_reschedule* in,
                                                    int32_t* node_out, uint8_t* ambiguous);
+/* The failover reconciler's resident form: gp_reconcile_find_nodes with a gp_resident_usage in place of the gp_usage_input, on
+ * the same terms as the three entries above -- placed, executor_nodes, the avail_* outputs, the status and the gp_last_error
+ * category are those of gp_reconcile_find_nodes given the equivalent gp_usage_input, and the context (reservation table,
+ * overhead table, snapshot, zone layout, held az-aware orders, gp_last_stats) is left as it was.  Its refusals are
+ * gp_reconcile_find_nodes' and the resident ones listed above; n_nodes == 0 still gives placed = -1 for every driver without
+ * reading either table (a live reservation table is still required). */
+gp_status gp_reconcile_find_nodes_resident(gp_ctx* ctx, const gp_resident_usage* usage, const gp_reconcile_nodes* nodes,
+                                           const gp_apps* stale, gp_reconcile_results* out);
+/* The unschedulable-pod marker's resident forms: gp_exceeds_cluster_capacity[_affinity] with GetNonSchedulableOverhead from the
+ * resident overhead table in place of nodes->overhead_* (ignored).  overhead_node_id [n_nodes]: the overhead-table id of each
+ * node-table entry, distinct, -1 = no records (overhead 0); NULL only with n_nodes == 0.  The result -- exceeds,
+ * affinity_error and the status -- is that of the per-call entry given overhead_* = gp_overhead_table_query(overhead_node_id)'s
+ * nonsched_* (0 where the id is -1); the overhead is summed on the device into the call's scratch and never crosses to the
+ * host.  The context, the overhead table included, is left as it was.  Refusals, besides the per-call entry's: GP_ERR_INVALID
+ * for no overhead table, overhead_node_id missing, an id out of range or given twice; GP_ERR_UNREPRESENTABLE for a per-node
+ * sum >= 2^61 (gp_overhead_table_query's refusal). */
+gp_status gp_exceeds_cluster_capacity_resident(gp_ctx* ctx, const gp_capacity_nodes* nodes /* overhead_* ignored */,
+                                               const int32_t* overhead_node_id, const gp_apps* drivers, gp_binpacker packer,
+                                               uint8_t* exceeds /* [n_apps] */);
+gp_status gp_exceeds_cluster_capacity_affinity_resident(gp_ctx* ctx, const gp_capacity_nodes* nodes, const int32_t* overhead_node_id,
+                                                        const gp_node_labels* labels, const gp_node_affinities* affinities,
+                                                        const gp_apps* drivers, gp_binpacker packer, uint8_t* exceeds /* [n_apps] */,
+                                                        uint8_t* affinity_error /* [n_apps] or NULL */);
 
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets

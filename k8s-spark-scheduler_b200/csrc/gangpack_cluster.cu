@@ -2,7 +2,8 @@
 // availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster[_groups], gp_prepare_cluster_zones[_groups]), executor
 // reschedule (gp_reschedule_executors, gp_reschedule_from_reservations) and the failover reconciler (gp_reconcile_find_nodes),
 // with the input checks and device staging they share; and the *_resident forms of gp_prepare_cluster_groups,
-// gp_prepare_cluster_zones_groups and gp_reschedule_from_reservations, which take the reservations from the resident table.
+// gp_prepare_cluster_zones_groups, gp_reschedule_from_reservations and gp_reconcile_find_nodes, which take the reservations
+// from the resident table.
 #include "gangpack_ctx.cuh"
 #include "gangpack_sort.cuh"
 #include "gangpack_zonelayout.cuh"
@@ -76,6 +77,11 @@ static gp_status stage_refusal(gp_ctx* c, const int* err, const char* who) {
     GP_TRY(refuse(c, err[0] & kFeErrId, kFeRefusals, who));
     GP_TRY(oht_sum_refusal(c, err[1], who));
     return refuse(c, err[0], kFeRefusals, who);
+}
+
+void enqueue_resident_dir(cudaStream_t st, int32_t n, const int32_t* ids, int32_t lim, int32_t* dir, int* d_err) {
+    const int T = 256;
+    if (n > 0) gp_resident_dirs<<<(n + T - 1) / T, T, 0, st>>>(n, ids, lim, dir, nullptr, 0, nullptr, d_err);
 }
 
 // The failover loop's status word (kRcErr* bits)
@@ -870,17 +876,18 @@ gp_status gp_reschedule_from_reservations_resident(gp_ctx* c, const gp_resident_
     return reschedule_from_reservations(c, usage, sort, scope, in, node_out, ambiguous, "gp_reschedule_from_reservations_resident");
 }
 
-// the failover reconciler's findNodes loop for a batch of stale drivers (EXT/failover.go:43-82, 286-436); see
-// gangpack_reconcile.cuh and DESIGN §2.3
-gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
-                                  gp_reconcile_results* out) {
+}  // extern "C"
+
+// gp_reconcile_find_nodes[_resident]
+static gp_status reconcile_find_nodes(gp_ctx* c, const UsageIn& usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
+                                      gp_reconcile_results* out, const char* who) {
     if (!enter(c)) return GP_ERR_INVALID;
-    static const char* who = "gp_reconcile_find_nodes";
-    GP_TRY(check_usage(c, usage, who));
-    if (!nodes || !a || !out || nodes->n_groups < 1 || a->n_apps < 0 || (usage->n_nodes > 0 && (!nodes->node_group || !nodes->creation)) ||
+    GP_TRY(check_source(c, usage, who));
+    const int32_t n = usage.n_nodes();
+    if (!nodes || !a || !out || nodes->n_groups < 1 || a->n_apps < 0 || (n > 0 && (!nodes->node_group || !nodes->creation)) ||
         (a->n_apps > 0 && (!a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->placed)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or bad sizes (n_groups >= 1)");
-    const int32_t n = usage->n_nodes, q = a->n_apps, G = nodes->n_groups;
+    const int32_t q = a->n_apps, G = nodes->n_groups;
     for (int32_t i = 0; i < n; ++i)
         if (nodes->node_group[i] < 0 || nodes->node_group[i] >= G) return fail(c, GP_ERR_INVALID, who, "node_group out of range");
     GP_TRY(check_requests(c, q, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu, who));
@@ -985,11 +992,26 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
     }
     int64_t* outs[3] = {out->avail_cpu_milli, out->avail_mem_bytes, out->avail_gpu};
     for (int d = 0; d < 3; ++d) ar.get(outs[d], d_avail + N * (size_t)d, N);
-    int uerr = 0;
-    ar.get(&uerr, d_err, 1);
+    int uerr[2] = {0, 0};
+    ar.get(uerr, d_err, 2);
     GP_TRY(ar.sync(c));
-    GP_TRY(refuse(c, uerr, kFeRefusals, who));
+    GP_TRY(stage_refusal(c, uerr, who));
     return refuse(c, herr, kRcRefusals, who);
+}
+
+extern "C" {
+
+// the failover reconciler's findNodes loop for a batch of stale drivers (EXT/failover.go:43-82, 286-436); see
+// gangpack_reconcile.cuh and DESIGN §2.3
+gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
+                                  gp_reconcile_results* out) {
+    return reconcile_find_nodes(c, usage, nodes, a, out, "gp_reconcile_find_nodes");
+}
+
+// the same with the reservations (and optionally the overhead) from the context's resident tables
+gp_status gp_reconcile_find_nodes_resident(gp_ctx* c, const gp_resident_usage* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
+                                           gp_reconcile_results* out) {
+    return reconcile_find_nodes(c, usage, nodes, a, out, "gp_reconcile_find_nodes_resident");
 }
 
 }  // extern "C"

@@ -393,6 +393,12 @@ void oht_enqueue_sums(gp_ctx* c, cudaStream_t st, const int32_t* row_of_node, in
                       unsigned long long* n_warned, long long* out, uint8_t* has_reservation, int* d_err);
 gp_status oht_sum_refusal(gp_ctx* c, int word, const char* who);
 
+// ---- gangpack_cluster.cu ---------------------------------------------------------------------------------------------
+
+// Enqueue gp_resident_dirs over one id array: dir[ids[i]] = i for every ids[i] != -1 (dir [lim] memset to -1 by the caller);
+// an id out of [0, lim) or given twice sets *d_err nonzero.  The marker's overhead-table directory.
+void enqueue_resident_dir(cudaStream_t st, int32_t n, const int32_t* ids, int32_t lim, int32_t* dir, int* d_err);
+
 // ---- gangpack_reservation_table.cu -----------------------------------------------------------------------------------
 
 // The live reservation table's columns on the device: node id [n_slots] (-1 = free) and cpu / mem / gpu [n_slots] each

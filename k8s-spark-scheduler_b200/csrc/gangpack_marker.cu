@@ -1,5 +1,6 @@
 // gangpack_marker.cu -- the unschedulable-pod marker's capacity checks (gp_exceeds_cluster_capacity, with required node
-// affinity gp_exceeds_cluster_capacity_affinity), gp_match_node_affinity, and the overhead computer (gp_node_overhead).
+// affinity gp_exceeds_cluster_capacity_affinity, and their *_resident forms over the overhead table), gp_match_node_affinity,
+// and the overhead computer (gp_node_overhead).
 #include "gangpack_ctx.cuh"
 #include "gangpack_affinity.cuh"
 #include "gangpack_capacity.cuh"
@@ -112,10 +113,11 @@ struct AffStage {
 };
 
 // DoesPodExceedClusterCapacity for a batch of stale drivers, any packer; the node sets are the node_group classes (aff ==
-// NULL) or the affinities' matches
+// NULL) or the affinities' matches.  The overhead is nodes->overhead_* (resident false) or, resident, GetNonSchedulableOverhead
+// of the overhead table's records on node id over_ids[i] (-1: none), summed into this call's scratch by the query's kernels.
 static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
                               const gp_node_affinities* aff, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds,
-                              uint8_t* affinity_error) {
+                              uint8_t* affinity_error, bool resident = false, const int32_t* over_ids = nullptr) {
     if (!aff) {
         if (!nodes || !a || nodes->n_nodes < 0 || a->n_apps < 0 || nodes->n_groups < 1 || (nodes->zone_id && nodes->n_zones < 1) ||
             (nodes->n_nodes > 0 && (!nodes->alloc_cpu_milli || !nodes->alloc_mem_bytes)) ||
@@ -137,6 +139,8 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     const int32_t Z = nodes->zone_id ? nodes->n_zones : 1, G = aff ? aff->n_aff : nodes->n_groups;
     if (!aff && (int64_t)(G + 1) * Z > (int64_t)INT32_MAX / 2) return fail(c, GP_ERR_INVALID, who, "(n_groups + 1) * n_zones too large");
     if (aff && (int64_t)Z > (int64_t)INT32_MAX / 2) return fail(c, GP_ERR_INVALID, who, "n_zones too large");
+    if (resident && n > 0 && !over_ids) return fail(c, GP_ERR_INVALID, who, "overhead_node_id missing");
+    if (resident && !c->oht.live) return fail(c, GP_ERR_INVALID, who, "no overhead table (gp_overhead_table_reset first)");
     // classes per chunk: node_group -> its own class and the all-nodes class; affinities -> as many as keep K n and K Z
     // within kCapEntries (at least one)
     const int32_t K = !aff ? 2 : (int32_t)std::max<int64_t>(1, std::min<int64_t>(std::max(G, 1), kCapEntries / std::max<int64_t>({(int64_t)n, (int64_t)Z, 1})));
@@ -152,7 +156,8 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     const size_t A = (size_t)pairs_per_chunk * (size_t)ms_stride;
     const size_t q1 = std::max<size_t>(q, 1);
     Arena ar{c->callbuf, st};
-    const auto alloc = ar.take<long long>(3 * N), over = ar.take<long long>(3 * N);
+    // resident overhead: the query's six columns, GetNonSchedulableOverhead last
+    const auto alloc = ar.take<long long>(3 * N), over = ar.take<long long>((resident ? 6 : 3) * N);
     const auto zone = ar.take<int32_t>(N), grp = ar.take<int32_t>(N), key = ar.take<int32_t>(E), rank = ar.take<int32_t>(E),
                zst = ar.take<int32_t>(N);
     const auto staged = ar.take<long long>(3 * N), sched = ar.take<long long>(3 * E);
@@ -173,9 +178,17 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     AffStage as{};
     Piece<uint32_t> member{0, 0};
     if (aff) { as.take(ar, labels, aff); member = ar.take<uint32_t>((size_t)K * (size_t)as.words); }
+    const size_t NR = resident ? N : 0;
+    const auto oids = ar.take<int32_t>(NR), odir = ar.take<int32_t>(resident ? (size_t)c->oht.size.n_node_ids : 0);
+    const auto oacc = ar.take<unsigned long long>(12 * NR), owarned = ar.take<unsigned long long>(resident ? 1 : 0);
+    const auto oerr = ar.take<int>(resident ? 2 : 0);   // the directory's word, then the overhead query's
     ar.reserve();
     ar.zero(hash);
     ar.fill(n_pairs, err, 0);                           // adjacent: one memset clears both
+    if (resident) {
+        ar.fill(odir, 0xff);
+        ar.fill(oacc, oerr, 0);
+    }
     if (aff) GP_TRY(as.upload(c, ar, labels, aff));
     CapScratch s{};
     s.key = ar.ptr(key); s.rank = ar.ptr(rank); s.zone = ar.ptr(zst); s.bucket_cnt = ar.ptr(bcnt);
@@ -191,11 +204,19 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         const int64_t* cols[2][3] = {{nodes->alloc_cpu_milli, nodes->alloc_mem_bytes, nodes->alloc_gpu},
                                      {nodes->overhead_cpu_milli, nodes->overhead_mem_bytes, nodes->overhead_gpu}};
         for (int d = 0; d < 3; ++d) ni.alloc[d] = ar.put(alloc.part(d * N, N), cols[0][d]);
-        for (int d = 0; d < 3; ++d) ni.over[d] = ar.put(over.part(d * N, N), cols[1][d]);
+        if (!resident)
+            for (int d = 0; d < 3; ++d) ni.over[d] = ar.put(over.part(d * N, N), cols[1][d]);
+        const int32_t* d_oids = ar.put(oids, resident ? over_ids : nullptr);
         ni.zone = ar.put(zone, nodes->zone_id);
         ni.group = ar.put(grp, nodes->node_group);
         ci.group = ni.group;
         GP_TRY(ar.check(c));
+        if (resident) {
+            int* e = ar.ptr(oerr);
+            enqueue_resident_dir(st, n, d_oids, c->oht.size.n_node_ids, ar.ptr(odir), e);
+            oht_enqueue_sums(c, st, ar.ptr(odir), n, ar.ptr(oacc), ar.ptr(owarned), ar.ptr(over), nullptr, e + 1);
+            for (int d = 0; d < 3; ++d) ni.over[d] = ar.ptr(over.part((3 + d) * N, N));
+        }
         gp_cc_nodes<<<(unsigned)((N + T - 1) / T), T, 0, st>>>(ni, s);
     }
     CapAppsIn ai{};
@@ -241,7 +262,7 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     }
     if (Q > 0) gp_cc_decide<<<(unsigned)((q + T - 1) / T), T, 0, st>>>(Q, ai.count, ar.ptr(app_pair), ar.ptr(pairs), po, (int32_t)packer, ar.ptr(d_out));
     GP_CUDA(c, cudaGetLastError());
-    int herr = 0, aerr = 0;
+    int herr = 0, aerr = 0, oerr_h[2] = {0, 0};
     std::vector<int32_t> n_error(aff ? (size_t)G : 0);
     ar.get(exceeds, ar.ptr(d_out), q);
     ar.get(&herr, s.err, 1);
@@ -249,7 +270,10 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         ar.get(&aerr, ar.ptr(as.err), 1);
         ar.get(n_error.data(), as.ne);
     }
+    ar.get(oerr_h, oerr);
     GP_TRY(ar.sync(c));
+    if (oerr_h[0]) return fail(c, GP_ERR_INVALID, who, "an overhead_node_id out of range or given twice");
+    GP_TRY(oht_sum_refusal(c, oerr_h[1], who));
     if (aff) GP_TRY(refuse(c, aerr, kAffRefusals, who));
     const Refusal cc_refusals[] = {                     // the capacity kernels' status word (kCcErr* bits)
         {kCcErrNegative, GP_ERR_INVALID, "negative resource request or exe_count"},
@@ -281,6 +305,22 @@ gp_status gp_exceeds_cluster_capacity_affinity(gp_ctx* c, const gp_capacity_node
     static const char* who = "gp_exceeds_cluster_capacity_affinity";
     if (!affinities) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
     return capacity_run(c, who, nodes, labels, affinities, a, packer, exceeds, affinity_error);
+}
+
+// the two with GetNonSchedulableOverhead from the context's resident overhead table, on the device (nodes->overhead_* ignored)
+gp_status gp_exceeds_cluster_capacity_resident(gp_ctx* c, const gp_capacity_nodes* nodes, const int32_t* overhead_node_id, const gp_apps* a,
+                                               gp_binpacker packer, uint8_t* exceeds) {
+    if (!enter(c)) return GP_ERR_INVALID;
+    return capacity_run(c, "gp_exceeds_cluster_capacity_resident", nodes, nullptr, nullptr, a, packer, exceeds, nullptr, true, overhead_node_id);
+}
+
+gp_status gp_exceeds_cluster_capacity_affinity_resident(gp_ctx* c, const gp_capacity_nodes* nodes, const int32_t* overhead_node_id,
+                                                        const gp_node_labels* labels, const gp_node_affinities* affinities, const gp_apps* a,
+                                                        gp_binpacker packer, uint8_t* exceeds, uint8_t* affinity_error) {
+    if (!enter(c)) return GP_ERR_INVALID;
+    static const char* who = "gp_exceeds_cluster_capacity_affinity_resident";
+    if (!affinities) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    return capacity_run(c, who, nodes, labels, affinities, a, packer, exceeds, affinity_error, true, overhead_node_id);
 }
 
 // GetRequiredNodeAffinity(...).Match for every (affinity, node); see gangpack_affinity.cuh

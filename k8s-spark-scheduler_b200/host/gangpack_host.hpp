@@ -1241,10 +1241,17 @@ inline RescheduleOutcome RescheduleExecutor(const binpacker::Binpacker& packer, 
     return out;
 }
 
+class ResidentOverheadComputer;
+
 // The unschedulable-pod marker's capacity checks (scanForUnschedulablePods, internal/extender/unschedulablepods.go:93-129) for
 // ALL stale drivers in one device call (gp_exceeds_cluster_capacity) instead of one DoesPodExceedClusterCapacity (:132-166) each.
 class UnschedulablePodMarker {
 public:
+    struct CapacityNode {              // what the resident sweep reads of a node: allocatable and zone, the overhead is the table's
+        std::string Name;
+        resources::Resources Allocatable;
+        std::string ZoneLabel = "default";
+    };
     struct StaleDriver {
         resources::Resources DriverResources;
         resources::Resources ExecutorResources;
@@ -1295,6 +1302,13 @@ public:
         dev.check(gp_exceeds_cluster_capacity(dev.ctx(), &n, &a, Packer(), out.data()), "gp_exceeds_cluster_capacity");
         return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
     }
+
+    // The same sweep with GetNonSchedulableOverhead read in place from the resident overhead table: the table's pending delta
+    // is flushed once, then one gp_exceeds_cluster_capacity_resident call.  A refused call resets and replays the table and
+    // is made again per call, over GetNonSchedulableOverhead (defined after ResidentOverheadComputer).
+    std::vector<bool> DoesPodsExceedClusterCapacity(const std::vector<CapacityNode>& nodes, ResidentOverheadComputer& overhead,
+                                                    const std::unordered_map<std::string, int32_t>& nodeClass, int32_t nClasses,
+                                                    const std::vector<StaleDriver>& drivers) const;
 
     // The same sweep with each driver's node set = the nodes its required affinity matches (gp_exceeds_cluster_capacity_affinity):
     // the sets may overlap freely.  nodes: the node table with labels, every node in nodesSchedulingMetadata; programs: one
@@ -1388,26 +1402,68 @@ struct ReconcileResult {
     std::vector<std::string> ReservedNodeNames;
 };
 
+// The node table (minus its usage) and the stale drivers of one reconcile as gp_reconcile_find_nodes[_resident] take them,
+// and the results read back.  Holds pointers into its own vectors: not copied.
+struct ReconcileCall {
+    std::vector<int64_t> ac, am, ag, cr, ec, em, eg, off;
+    std::vector<int32_t> grp, count, dg, placed, exe;
+    std::vector<uint8_t> unsched, ready;
+    gp_reconcile_nodes nd{};
+    gp_apps a{};
+    gp_reconcile_results out{};
+    ReconcileCall(const std::vector<ReconcileNode>& nodes, const std::string& instanceGroupLabel, const std::vector<StaleDriver>& drivers) {
+        const size_t N = nodes.size(), Q = drivers.size();
+        std::unordered_map<std::string, int32_t> groupId;
+        auto intern = [&](const std::string& g) { return groupId.emplace(g, (int32_t)groupId.size()).first->second; };
+        ac.resize(N); am.resize(N); ag.resize(N); cr.resize(N); grp.resize(N); unsched.resize(N); ready.resize(N);
+        for (size_t i = 0; i < N; ++i) {
+            const ReconcileNode& n = nodes[i];
+            ac[i] = n.Allocatable.CPU; am[i] = n.Allocatable.Memory; ag[i] = n.Allocatable.NvidiaGPU;
+            auto l = n.Labels.find(instanceGroupLabel);
+            grp[i] = intern(l == n.Labels.end() ? std::string() : l->second);      // n.Labels[label]: "" when missing
+            unsched[i] = n.Unschedulable; ready[i] = n.Ready; cr[i] = n.CreationUnixNano;
+        }
+        ec.resize(Q); em.resize(Q); eg.resize(Q); off.assign(Q + 1, 0); count.resize(Q); dg.resize(Q);
+        for (size_t i = 0; i < Q; ++i) {
+            const StaleDriver& d = drivers[i];
+            ec[i] = d.ExecutorResources.CPU; em[i] = d.ExecutorResources.Memory; eg[i] = d.ExecutorResources.NvidiaGPU;
+            count[i] = std::max(0, d.MinExecutorCount - std::min(d.RunningExecutors, d.MinExecutorCount));   // :366
+            dg[i] = intern(d.InstanceGroup);
+            off[i + 1] = off[i] + count[i];
+        }
+        nd.n_groups = std::max<int32_t>(1, (int32_t)groupId.size());
+        nd.node_group = grp.data(); nd.creation = cr.data(); nd.unschedulable = unsched.data(); nd.ready = ready.data();
+        a.n_apps = (int32_t)Q;
+        a.exe_cpu_milli = ec.data(); a.exe_mem_bytes = em.data(); a.exe_gpu = eg.data();
+        a.exe_count = count.data(); a.group = dg.data(); a.exec_out_off = off.data();
+        placed.resize(std::max<size_t>(Q, 1)); exe.resize((size_t)std::max<int64_t>(off[Q], 1));
+        out.placed = placed.data(); out.executor_nodes = exe.data(); out.executor_nodes_cap = off[Q];
+    }
+    ReconcileCall(const ReconcileCall&) = delete;
+    ReconcileCall& operator=(const ReconcileCall&) = delete;
+    std::vector<ReconcileResult> Results(const std::vector<ReconcileNode>& nodes) const {
+        std::vector<ReconcileResult> res((size_t)a.n_apps);
+        for (size_t i = 0; i < res.size(); ++i) {
+            res[i].InstanceGroupFound = placed[i] >= 0;
+            for (int32_t j = 0; j < placed[i]; ++j) res[i].ReservedNodeNames.push_back(nodes[(size_t)exe[(size_t)off[i] + (size_t)j]].Name);
+        }
+        return res;
+    }
+};
+
 // nodes: the lister's nodes (their order is the tie order among equal creation times, DESIGN §2.3); rows: every RR and soft
 // reservation; overhead: GetOverhead by node name; drivers: in the order their RRs are written.
 inline std::vector<ReconcileResult> ReconcileFindNodes(const std::vector<ReconcileNode>& nodes, const std::vector<ReconcileRow>& rows,
                                                        const resources::NodeGroupResources& overhead, const std::string& instanceGroupLabel,
                                                        const std::vector<StaleDriver>& drivers) {
-    const size_t N = nodes.size(), R = rows.size(), Q = drivers.size();
-    std::unordered_map<std::string, int32_t> index, groupId;
-    auto intern = [&](const std::string& g) { return groupId.emplace(g, (int32_t)groupId.size()).first->second; };
-    std::vector<int64_t> ac(N), am(N), ag(N), oc(N), om(N), og(N), cr(N);
-    std::vector<int32_t> grp(N);
-    std::vector<uint8_t> unsched(N), ready(N);
+    const size_t N = nodes.size(), R = rows.size();
+    ReconcileCall call(nodes, instanceGroupLabel, drivers);
+    std::unordered_map<std::string, int32_t> index;
+    std::vector<int64_t> oc(N), om(N), og(N);
     for (size_t i = 0; i < N; ++i) {
-        const ReconcileNode& n = nodes[i];
-        index.emplace(n.Name, (int32_t)i);
-        ac[i] = n.Allocatable.CPU; am[i] = n.Allocatable.Memory; ag[i] = n.Allocatable.NvidiaGPU;
-        auto o = overhead.find(n.Name);
+        index.emplace(nodes[i].Name, (int32_t)i);
+        auto o = overhead.find(nodes[i].Name);
         if (o != overhead.end()) { oc[i] = o->second.CPU; om[i] = o->second.Memory; og[i] = o->second.NvidiaGPU; }
-        auto l = n.Labels.find(instanceGroupLabel);
-        grp[i] = intern(l == n.Labels.end() ? std::string() : l->second);      // n.Labels[label]: "" when missing
-        unsched[i] = n.Unschedulable; ready[i] = n.Ready; cr[i] = n.CreationUnixNano;
     }
     std::vector<int32_t> rn(R);
     std::vector<int64_t> rc(R), rm(R), rg(R);
@@ -1416,38 +1472,14 @@ inline std::vector<ReconcileResult> ReconcileFindNodes(const std::vector<Reconci
         rn[r] = it == index.end() ? -1 : it->second;
         rc[r] = rows[r].Resources.CPU; rm[r] = rows[r].Resources.Memory; rg[r] = rows[r].Resources.NvidiaGPU;
     }
-    std::vector<int64_t> ec(Q), em(Q), eg(Q), off(Q + 1, 0);
-    std::vector<int32_t> count(Q), dg(Q);
-    for (size_t i = 0; i < Q; ++i) {
-        const StaleDriver& d = drivers[i];
-        ec[i] = d.ExecutorResources.CPU; em[i] = d.ExecutorResources.Memory; eg[i] = d.ExecutorResources.NvidiaGPU;
-        count[i] = std::max(0, d.MinExecutorCount - std::min(d.RunningExecutors, d.MinExecutorCount));   // :366
-        dg[i] = intern(d.InstanceGroup);
-        off[i + 1] = off[i] + count[i];
-    }
     gp_usage_input u{};
     u.n_nodes = (int32_t)N;
-    u.alloc_cpu_milli = ac.data(); u.alloc_mem_bytes = am.data(); u.alloc_gpu = ag.data();
+    u.alloc_cpu_milli = call.ac.data(); u.alloc_mem_bytes = call.am.data(); u.alloc_gpu = call.ag.data();
     u.overhead_cpu_milli = oc.data(); u.overhead_mem_bytes = om.data(); u.overhead_gpu = og.data();
     u.n_reservations = (int64_t)R; u.res_node = rn.data(); u.res_cpu_milli = rc.data(); u.res_mem_bytes = rm.data(); u.res_gpu = rg.data();
-    gp_reconcile_nodes nd{};
-    nd.n_groups = std::max<int32_t>(1, (int32_t)groupId.size());
-    nd.node_group = grp.data(); nd.creation = cr.data(); nd.unschedulable = unsched.data(); nd.ready = ready.data();
-    gp_apps a{};
-    a.n_apps = (int32_t)Q;
-    a.exe_cpu_milli = ec.data(); a.exe_mem_bytes = em.data(); a.exe_gpu = eg.data();
-    a.exe_count = count.data(); a.group = dg.data(); a.exec_out_off = off.data();
-    std::vector<int32_t> placed(std::max<size_t>(Q, 1)), exe(std::max<int64_t>(off[Q], 1));
-    gp_reconcile_results out{};
-    out.placed = placed.data(); out.executor_nodes = exe.data(); out.executor_nodes_cap = off[Q];
     gangpack::Device& dev = gangpack::Device::Get();
-    dev.check(gp_reconcile_find_nodes(dev.ctx(), &u, &nd, &a, &out), "gp_reconcile_find_nodes");
-    std::vector<ReconcileResult> res(Q);
-    for (size_t i = 0; i < Q; ++i) {
-        res[i].InstanceGroupFound = placed[i] >= 0;
-        for (int32_t j = 0; j < placed[i]; ++j) res[i].ReservedNodeNames.push_back(nodes[(size_t)exe[(size_t)off[i] + (size_t)j]].Name);
-    }
-    return res;
+    dev.check(gp_reconcile_find_nodes(dev.ctx(), &u, &call.nd, &call.a, &call.out), "gp_reconcile_find_nodes");
+    return call.Results(nodes);
 }
 
 // The overhead computer (internal/extender/overhead.go): the event side on the host, the per-call side in one
@@ -1635,6 +1667,19 @@ public:
         soft_[app] = pods;
     }
     void DeleteSoftReservation(const std::string& app) { if (soft_.count(app)) dropSoft(app); }
+
+    // For the entries that read the table in place: send the pending delta (at most one update), the table's id of each node
+    // name (-1: no records, overhead zero), and a reset and replay of the whole state at the next flush (after a refusal).
+    void Flush(gangpack::Device& dev) { flush(dev); }
+    std::vector<int32_t> NodeIDs(const std::vector<std::string>& nodes) const {
+        std::vector<int32_t> ids(nodes.size(), -1);
+        for (size_t i = 0; i < nodes.size(); ++i) {
+            auto it = nodes_.id.find(nodes[i]);
+            if (it != nodes_.id.end()) ids[i] = it->second;
+        }
+        return ids;
+    }
+    void Replay() { replay_ = true; }
 
     resources::NodeGroupResources GetOverhead(const std::vector<std::string>& nodes) { return compute(nodes).first; }
     resources::NodeGroupResources GetNonSchedulableOverhead(const std::vector<std::string>& nodes) { return compute(nodes).second; }
@@ -1909,6 +1954,17 @@ public:
         return ids;
     }
 
+    // the next Flush resets the table and sends the whole state again (after a refused resident call)
+    void Replay() { replay_ = true; }
+    // GetReservedResources' rows as the per-call reconciler takes them
+    std::vector<ReconcileRow> Rows() const {
+        std::vector<ReconcileRow> rows;
+        for (const auto* store : {&rrs_, &soft_})
+            for (const auto& owner : *store)
+                for (const auto& e : owner.second) rows.push_back(ReconcileRow{e.second.Node, e.second.Res});
+        return rows;
+    }
+
     void Flush(gangpack::Device& dev) {
         auto grow = [&](int64_t& cap, int64_t need) { while (cap < need) { cap = std::max<int64_t>(2 * cap, 1); replay_ = true; } };
         int64_t caps[2] = {size_.n_slots, size_.n_node_ids};
@@ -2014,6 +2070,84 @@ private:
     std::vector<int32_t> nodeCount_, freeIds_;
     std::map<size_t, Row> dirty_;                                 // -> the row the table holds
 };
+
+// ReconcileFindNodes over the resident tables (gp_reconcile_find_nodes_resident): each table's pending delta is flushed once,
+// then one device call reads every reservation and GetOverhead in place.  A refused call resets and replays both tables and
+// is made again per call, over Rows() and GetOverhead, which answers or refuses as the per-call entry does.
+inline std::vector<ReconcileResult> ReconcileFindNodesResident(const std::vector<ReconcileNode>& nodes, ResidentReservations& reservations,
+                                                               ResidentOverheadComputer& overhead, const std::string& instanceGroupLabel,
+                                                               const std::vector<StaleDriver>& drivers) {
+    gangpack::Device& dev = gangpack::Device::Get();
+    reservations.Flush(dev);
+    overhead.Flush(dev);
+    std::vector<std::string> names;
+    for (const auto& n : nodes) names.push_back(n.Name);
+    const std::vector<int32_t> ids = reservations.NodeIDs(names), oids = overhead.NodeIDs(names);
+    ReconcileCall call(nodes, instanceGroupLabel, drivers);
+    gp_resident_usage u{};
+    u.n_nodes = (int32_t)nodes.size(); u.node_id = ids.data();
+    u.alloc_cpu_milli = call.ac.data(); u.alloc_mem_bytes = call.am.data(); u.alloc_gpu = call.ag.data();
+    u.overhead_node_id = oids.data();
+    if (gp_reconcile_find_nodes_resident(dev.ctx(), &u, &call.nd, &call.a, &call.out) == GP_OK) return call.Results(nodes);
+    reservations.Replay();
+    overhead.Replay();
+    reservations.Flush(dev);
+    return ReconcileFindNodes(nodes, reservations.Rows(), overhead.GetOverhead(names), instanceGroupLabel, drivers);
+}
+
+inline std::vector<bool> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(const std::vector<CapacityNode>& nodes,
+                                                                               ResidentOverheadComputer& overhead,
+                                                                               const std::unordered_map<std::string, int32_t>& nodeClass,
+                                                                               int32_t nClasses, const std::vector<StaleDriver>& drivers) const {
+    gangpack::Device& dev = gangpack::Device::Get();
+    overhead.Flush(dev);
+    const size_t N = nodes.size(), Q = drivers.size();
+    std::vector<std::string> names;
+    std::vector<int64_t> ac(N + 1), am(N + 1), ag(N + 1);
+    std::vector<int32_t> zone(N + 1), group(N + 1);
+    std::unordered_map<std::string, int32_t> zoneId;
+    for (size_t i = 0; i < N; ++i) {
+        names.push_back(nodes[i].Name);
+        ac[i] = nodes[i].Allocatable.CPU; am[i] = nodes[i].Allocatable.Memory; ag[i] = nodes[i].Allocatable.NvidiaGPU;
+        zone[i] = zoneId.emplace(nodes[i].ZoneLabel, (int32_t)zoneId.size()).first->second;
+        auto c = nodeClass.find(nodes[i].Name);
+        group[i] = c == nodeClass.end() ? -1 : c->second;
+    }
+    const std::vector<int32_t> oids = overhead.NodeIDs(names);
+    std::vector<int64_t> q[6];
+    std::vector<int32_t> count(Q + 1), cls(Q + 1);
+    for (auto& col : q) col.resize(Q + 1);
+    for (size_t i = 0; i < Q; ++i) {
+        const StaleDriver& d = drivers[i];
+        q[0][i] = d.DriverResources.CPU; q[1][i] = d.DriverResources.Memory; q[2][i] = d.DriverResources.NvidiaGPU;
+        q[3][i] = d.ExecutorResources.CPU; q[4][i] = d.ExecutorResources.Memory; q[5][i] = d.ExecutorResources.NvidiaGPU;
+        count[i] = d.MinExecutorCount; cls[i] = d.AffinityClass;
+    }
+    gp_capacity_nodes n{};
+    n.n_nodes = (int32_t)N;
+    n.alloc_cpu_milli = ac.data(); n.alloc_mem_bytes = am.data(); n.alloc_gpu = ag.data();
+    n.n_zones = std::max<int32_t>(1, (int32_t)zoneId.size()); n.zone_id = zone.data();
+    n.n_groups = std::max<int32_t>(1, nClasses); n.node_group = group.data();
+    gp_apps a{};
+    a.n_apps = (int32_t)Q;
+    a.drv_cpu_milli = q[0].data(); a.drv_mem_bytes = q[1].data(); a.drv_gpu = q[2].data();
+    a.exe_cpu_milli = q[3].data(); a.exe_mem_bytes = q[4].data(); a.exe_gpu = q[5].data();
+    a.exe_count = count.data(); a.group = cls.data();
+    std::vector<uint8_t> out(Q + 1);
+    if (gp_exceeds_cluster_capacity_resident(dev.ctx(), &n, oids.data(), &a, Packer(), out.data()) == GP_OK)
+        return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
+    overhead.Replay();
+    const resources::NodeGroupResources nonsched = overhead.GetNonSchedulableOverhead(names);
+    resources::NodeGroupSchedulingMetadata md;
+    for (const auto& node : nodes) {
+        resources::NodeSchedulingMetadata m;
+        m.SchedulableResources = node.Allocatable;
+        m.SchedulableResources.Sub(nonsched.at(node.Name));
+        m.ZoneLabel = node.ZoneLabel;
+        md[node.Name] = m;
+    }
+    return DoesPodsExceedClusterCapacity(md, nodeClass, nClasses, drivers);
+}
 
 }  // namespace extender
 

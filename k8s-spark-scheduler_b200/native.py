@@ -40,6 +40,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_node_overhead", "gp_overhead_table_reset", "gp_overhead_table_update", "gp_overhead_table_query",
            "gp_reservation_table_reset", "gp_reservation_table_update", "gp_prepare_cluster_groups_resident",
            "gp_prepare_cluster_zones_groups_resident", "gp_reschedule_from_reservations_resident",
+           "gp_reconcile_find_nodes_resident", "gp_exceeds_cluster_capacity_resident",
+           "gp_exceeds_cluster_capacity_affinity_resident",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -382,6 +384,16 @@ def load():
     L.gp_prepare_cluster_zones_groups_resident.restype = C.c_int
     L.gp_prepare_cluster_zones_groups_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input),
                                                            C.c_void_p, C.c_int32, C.POINTER(gp_instance_group_layout)]
+    L.gp_reconcile_find_nodes_resident.restype = C.c_int
+    L.gp_reconcile_find_nodes_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_reconcile_nodes),
+                                                   C.POINTER(gp_apps), C.POINTER(gp_reconcile_results)]
+    L.gp_exceeds_cluster_capacity_resident.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_resident.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.c_void_p, C.POINTER(gp_apps), C.c_int,
+                                                       C.c_void_p]
+    L.gp_exceeds_cluster_capacity_affinity_resident.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_affinity_resident.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.c_void_p,
+                                                                C.POINTER(gp_node_labels), C.POINTER(gp_node_affinities),
+                                                                C.POINTER(gp_apps), C.c_int, C.c_void_p, C.c_void_p]
     L.gp_reschedule_from_reservations_resident.restype = C.c_int
     L.gp_reschedule_from_reservations_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input),
                                                            C.POINTER(gp_reschedule_scope), C.POINTER(gp_reschedule), C.c_void_p,
@@ -479,6 +491,19 @@ def _resident_usage(node_id, alloc, overhead=None, overhead_node_id=None):
                            overhead_node_id=_p(oid), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]), overhead_gpu=_p(ov[2]))
     ru._keep = (ids, al, ov, oid)
     return ru
+
+
+def _capacity_nodes(alloc, overhead, zone_id, n_zones, node_group, n_groups):
+    """gp_capacity_nodes over (cpu, mem[, gpu]) triples; overhead may be None.  The struct keeps its arrays alive."""
+    al = [_np(v, np.int64) for v in alloc]
+    ov = [_np(v, np.int64) for v in overhead] if overhead is not None else [None, None, None]
+    zid, grp = _np(zone_id, np.int32), _np(node_group, np.int32)
+    nd = gp_capacity_nodes(n_nodes=len(al[0]), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]),
+                           alloc_gpu=_p(al[2] if len(al) > 2 else None), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]),
+                           overhead_gpu=_p(ov[2] if len(ov) > 2 else None), n_zones=int(n_zones), zone_id=_p(zid),
+                           n_groups=int(n_groups), node_group=_p(grp))
+    nd._keep = (al, ov, zid, grp)
+    return nd
 
 
 def _sort_input(n, n_zones, zone_id=None, name_rank=None, is_driver_candidate=None, unschedulable=None, ready=None,
@@ -1112,16 +1137,23 @@ class GangPacker:
         class per node, -1 = none (None = all 0).  apps: drv_*, exe_*, count and group (the driver's class, -1 = every node).
         -> uint8[n_apps], 1 = exceeds cluster capacity.  Leaves the context's snapshot and statistics untouched."""
         q = len(apps["count"])
-        al = [_np(v, np.int64) for v in alloc]
-        ov = [_np(v, np.int64) for v in overhead] if overhead is not None else [None, None, None]
-        zid, grp = _np(zone_id, np.int32), _np(node_group, np.int32)
-        nd = gp_capacity_nodes(n_nodes=len(al[0]), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]),
-                               alloc_gpu=_p(al[2] if len(al) > 2 else None), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]),
-                               overhead_gpu=_p(ov[2] if len(ov) > 2 else None), n_zones=int(n_zones), zone_id=_p(zid),
-                               n_groups=int(n_groups), node_group=_p(grp))
+        nd = _capacity_nodes(alloc, overhead, zone_id, n_zones, node_group, n_groups)
         a = _apps(apps, None, group=apps.get("group"))
         out = np.full(max(q, 1), 255, np.uint8)
         self._check(load().gp_exceeds_cluster_capacity(self._h, C.byref(nd), C.byref(a), int(packer), _p(out)))
+        return out[:q]
+
+    def exceeds_cluster_capacity_resident(self, alloc, overhead_node_id, apps: dict, packer: int, zone_id=None, n_zones=1,
+                                          node_group=None, n_groups=1) -> np.ndarray:
+        """exceeds_cluster_capacity with GetNonSchedulableOverhead from the resident overhead table
+        (gp_exceeds_cluster_capacity_resident): overhead_node_id[n] = each node's overhead-table id (distinct, -1 = no records).
+        Returns what exceeds_cluster_capacity returns with overhead = overhead_table_query(overhead_node_id)'s nonsched."""
+        q = len(apps["count"])
+        nd = _capacity_nodes(alloc, None, zone_id, n_zones, node_group, n_groups)
+        oid = _np(overhead_node_id, np.int32)
+        a = _apps(apps, None, group=apps.get("group"))
+        out = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity_resident(self._h, C.byref(nd), _p(oid), C.byref(a), int(packer), _p(out)))
         return out[:q]
 
     def match_node_affinity(self, enc: dict):
@@ -1142,19 +1174,28 @@ class GangPacker:
         (gp_exceeds_cluster_capacity_affinity): enc from affinity.encode(); apps["group"] = the driver's affinity id.
         -> (exceeds uint8[n_apps], affinity_error uint8[n_apps]); exceeds[i] is undefined where affinity_error[i] = 1."""
         q = len(apps["count"])
-        al = [_np(v, np.int64) for v in alloc]
-        ov = [_np(v, np.int64) for v in overhead] if overhead is not None else [None, None, None]
-        zid = _np(zone_id, np.int32)
-        nd = gp_capacity_nodes(n_nodes=len(al[0]), alloc_cpu_milli=_p(al[0]), alloc_mem_bytes=_p(al[1]),
-                               alloc_gpu=_p(al[2] if len(al) > 2 else None), overhead_cpu_milli=_p(ov[0]), overhead_mem_bytes=_p(ov[1]),
-                               overhead_gpu=_p(ov[2] if len(ov) > 2 else None), n_zones=int(n_zones), zone_id=_p(zid),
-                               n_groups=0, node_group=None)
+        nd = _capacity_nodes(alloc, overhead, zone_id, n_zones, None, 0)
         lab, aff = _affinity_input(enc)
         a = _apps(apps, None, group=apps.get("group"))
         out = np.full(max(q, 1), 255, np.uint8)
         err = np.full(max(q, 1), 255, np.uint8)
         self._check(load().gp_exceeds_cluster_capacity_affinity(self._h, C.byref(nd), C.byref(lab), C.byref(aff), C.byref(a),
                                                                 int(packer), _p(out), _p(err)))
+        return out[:q], err[:q]
+
+    def exceeds_cluster_capacity_affinity_resident(self, alloc, overhead_node_id, enc: dict, apps: dict, packer: int, zone_id=None,
+                                                   n_zones=1):
+        """exceeds_cluster_capacity_affinity with GetNonSchedulableOverhead from the resident overhead table
+        (gp_exceeds_cluster_capacity_affinity_resident), overhead_node_id as in exceeds_cluster_capacity_resident."""
+        q = len(apps["count"])
+        nd = _capacity_nodes(alloc, None, zone_id, n_zones, None, 0)
+        oid = _np(overhead_node_id, np.int32)
+        lab, aff = _affinity_input(enc)
+        a = _apps(apps, None, group=apps.get("group"))
+        out = np.full(max(q, 1), 255, np.uint8)
+        err = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity_affinity_resident(self._h, C.byref(nd), _p(oid), C.byref(lab), C.byref(aff),
+                                                                         C.byref(a), int(packer), _p(out), _p(err)))
         return out[:q], err[:q]
 
     def reconcile_find_nodes(self, alloc, overhead, res_node, res, node_group, creation, apps: dict, n_groups: int,
@@ -1165,7 +1206,18 @@ class GangPacker:
         (UnixNano); apps: exe_cpu, exe_mem, exe_gpu (optional), count = max(0, Min - running) and group, in call order.
         -> (placed[q] (-1 = instance group not found), executor_nodes (CSR by off), off[q + 1], (cpu, mem, gpu) availability after
         the loop or None).  Leaves the context's snapshot and statistics untouched."""
-        ui = _usage_input(alloc, overhead, res_node, res)
+        return self._reconcile(load().gp_reconcile_find_nodes, _usage_input(alloc, overhead, res_node, res), node_group, creation,
+                               apps, n_groups, unschedulable, ready, exec_cap, want_avail)
+
+    def reconcile_find_nodes_resident(self, node_id, alloc, overhead, node_group, creation, apps: dict, n_groups: int,
+                                      unschedulable=None, ready=None, exec_cap=None, want_avail=True, overhead_node_id=None):
+        """reconcile_find_nodes with the reservations from the resident reservation table (gp_reconcile_find_nodes_resident):
+        node_id, overhead and overhead_node_id as in reschedule_from_reservations_resident.  Returns what reconcile_find_nodes
+        returns on the equivalent rows, and leaves the context as it would."""
+        return self._reconcile(load().gp_reconcile_find_nodes_resident, _resident_usage(node_id, alloc, overhead, overhead_node_id),
+                               node_group, creation, apps, n_groups, unschedulable, ready, exec_cap, want_avail)
+
+    def _reconcile(self, fn, ui, node_group, creation, apps, n_groups, unschedulable, ready, exec_cap, want_avail):
         n = ui.n_nodes
         ng, cr = _np(node_group, np.int32), _np(creation, np.int64)
         fu, fr = _np(unschedulable, np.uint8), _np(ready, np.uint8)
@@ -1181,7 +1233,7 @@ class GangPacker:
         av = [np.empty(max(n, 1), np.int64) for _ in range(3)] if want_avail else [None] * 3
         r = gp_reconcile_results(placed=_p(placed), executor_nodes=_p(execn), executor_nodes_cap=cap,
                                  avail_cpu_milli=_p(av[0]), avail_mem_bytes=_p(av[1]), avail_gpu=_p(av[2]))
-        self._check(load().gp_reconcile_find_nodes(self._h, C.byref(ui), C.byref(nd), C.byref(a), C.byref(r)))
+        self._check(fn(self._h, C.byref(ui), C.byref(nd), C.byref(a), C.byref(r)))
         return placed[:q], execn[:int(off[q])], off, (tuple(x[:n] for x in av) if want_avail else None)
 
     def node_overhead(self, enc: dict):
