@@ -1136,6 +1136,71 @@ gp_status gp_exceeds_cluster_capacity_affinity_resident(gp_ctx* ctx, const gp_ca
                                                         const gp_apps* drivers, gp_binpacker packer, uint8_t* exceeds /* [n_apps] */,
                                                         uint8_t* affinity_error /* [n_apps] or NULL */);
 
+/* ---- the resident label table -------------------------------------------------------------------------------------------
+ * Every node's labels kept on the device and changed only by deltas, so a driver Predicate and the marker's affinity sweep no
+ * longer upload every label of every node (gp_node_labels) per call.  The state:
+ *   rows          [n_node_ids] fixed-stride rows: label-table node id r owns entries [r * max_labels, r * max_labels + count[r])
+ *                 of two columns, key id and value id, keys strictly ascending (node.Labels is a map); count 0 = no labels
+ *   value columns [n_values] val_int_ok / val_int: strconv.ParseInt(value, 10, 64) of each interned value string -- a
+ *                 function of the string, so kept per value id rather than per label
+ * Node, key and value ids are the caller's interned node names, label keys and label values.  A node with more labels than
+ * max_labels does not fit: the caller resets with a larger stride and replays.  The table belongs to the context (freed by
+ * gp_destroy); updates change no snapshot, layout, schedulable resources, held orders or statistics. */
+typedef struct {
+    int32_t n_node_ids;              /* rows */
+    int32_t max_labels;              /* row stride; n_node_ids * max_labels < 2^31 */
+    int32_t n_keys;                  /* label key ids 0..n_keys-1 */
+    int32_t n_values;                /* label value ids 0..n_values-1 */
+} gp_label_table_size;
+/* Replace the context's label table with an empty one: every row without labels, no value parses.  GP_ERR_INVALID: NULL
+ * size, a negative capacity or n_node_ids * max_labels >= 2^31 (the table held before is kept).  After a CUDA error the
+ * context holds no table. */
+gp_status gp_label_table_reset(gp_ctx* ctx, const gp_label_table_size* size);
+
+typedef struct {
+    int32_t n_rows;                  /* whole-row writes: the row's new labels replace all its old ones */
+    int32_t n_values;                /* value writes */
+    const int32_t* row_node;         /* [n_rows] distinct node ids < n_node_ids */
+    const int64_t* row_off;          /* [n_rows + 1] CSR: row_node[i]'s labels are [row_off[i], row_off[i+1]); row_off[0] = 0;
+                                        an empty run clears the row (a deleted node) */
+    const int32_t* label_key;        /* key ids, strictly ascending within a row */
+    const int32_t* label_val;        /* value ids */
+    const int32_t* value_id;         /* [n_values] distinct value ids < n_values */
+    const uint8_t* value_int_ok;     /* [n_values] ParseInt(value, 10, 64) succeeded */
+    const int64_t* value_int;        /* [n_values] its result where value_int_ok (ignored elsewhere) */
+} gp_label_delta;
+/* Apply one delta.  The whole delta is checked on the device before anything is written: a refused delta leaves the table
+ * exactly as it was.  One stream synchronise.  GP_ERR_INVALID: no table (gp_label_table_reset first), missing arrays, a
+ * negative count or row_off that does not start at 0 or decreases; a node or value id out of range or given twice; a row
+ * longer than max_labels; a key id out of range or the keys of a row not strictly ascending; a label value id out of range.
+ * A refusal, or a CUDA error while the delta is staged, leaves the table as it was; a CUDA error once the update writes the
+ * table leaves no table (GP_ERR_INVALID "no label table" until the next reset), and the caller resets and replays. */
+gp_status gp_label_table_update(gp_ctx* ctx, const gp_label_delta* delta);
+
+/* The node table of a resident match: for each node-table entry its label-table id, or -1 for a node without labels.  The
+ * ids may repeat: the call only reads the rows. */
+typedef struct {
+    int32_t n_nodes;
+    int32_t reserved;
+    const int32_t* node_id;          /* [n_nodes] in [-1, n_node_ids); NULL only with n_nodes == 0 */
+} gp_resident_labels;
+/* gp_match_node_affinity over the label table: member, n_match, n_error and the status are those of gp_match_node_affinity
+ * given the equivalent gp_node_labels -- n_nodes, the table's n_keys / n_values, node i's labels = row node_id[i] (none for
+ * -1), label_int_ok / label_int from the value columns.  Affinity key and value ids are checked against the table's n_keys /
+ * n_values, metadata.name node indices against labels->n_nodes.  Uploads: the node ids and the programs.  The context, the
+ * table included, is left alone; one stream synchronise.  Refusals: gp_match_node_affinity's for the programs, and
+ * GP_ERR_INVALID for no label table or a node id outside [-1, n_node_ids). */
+gp_status gp_match_node_affinity_resident(gp_ctx* ctx, const gp_resident_labels* labels, const gp_node_affinities* affinities,
+                                          gp_affinity_match* out);
+/* gp_exceeds_cluster_capacity_affinity_resident with the labels from the label table: its result -- exceeds, affinity_error
+ * and the status -- is that of gp_exceeds_cluster_capacity_affinity_resident given the equivalent gp_node_labels (as for
+ * gp_match_node_affinity_resident); labels->n_nodes = nodes->n_nodes.  Both tables are read in place and left as they were.
+ * Refusals: gp_exceeds_cluster_capacity_affinity_resident's and gp_match_node_affinity_resident's. */
+gp_status gp_exceeds_cluster_capacity_affinity_label_table(gp_ctx* ctx, const gp_capacity_nodes* nodes, const int32_t* overhead_node_id,
+                                                           const gp_resident_labels* labels, const gp_node_affinities* affinities,
+                                                           const gp_apps* drivers, gp_binpacker packer, uint8_t* exceeds /* [n_apps] */,
+                                                           uint8_t* affinity_error /* [n_apps] or NULL */);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

@@ -16,8 +16,15 @@
 //      skipped, a term matches when all its requirements do, and the first matching term is a match;
 //   4. otherwise no match, an error if some term recorded one.
 //
-// Kernel gp_aff_labels: thread per node, checks its labels (ids in range, keys strictly ascending) -- once per call, whatever
-// the number of affinities.
+// The labels come from one of two sources, a template parameter of aff_req / aff_outcome / gp_aff_match:
+//   AffLabelsIn        the per-call CSR of gp_node_labels, ParseInt per label entry;
+//   AffLabelsResident  the label table's fixed-stride rows (gangpack_label_table.cu), read through the call's node_id (-1: no
+//                      labels), ParseInt per value id.
+// Both give a node's labels as a range [lo, hi) of one key column and one value column, so the program runs unchanged.
+//
+// Kernel gp_aff_labels: thread per node, checks its per-call labels (ids in range, keys strictly ascending) -- once per call,
+// whatever the number of affinities.  The resident rows were checked when they were written; gp_aff_ids checks the call's
+// node ids against the table instead.
 // Kernel gp_aff_match: grid (node tiles, affinity).  The CTA stages its affinity's program in shared memory (or reads it
 // from global memory when it is larger than kAffSmem bytes); each thread runs the program on one node, finding each key by
 // binary search in the node's labels and each In / NotIn value by binary search in the requirement's values.  Bitmap words
@@ -44,6 +51,10 @@ enum : int {
     kAffErrLabelVal = 2,                  // a node's label value out of range
 };
 
+enum : int {
+    kAffErrNodeId = 4,                    // a resident node id outside [-1, n_node_ids)
+};
+
 struct AffLabelsIn {
     int32_t n, n_keys, n_values;
     const long long* off;                 // [n + 1]
@@ -51,6 +62,35 @@ struct AffLabelsIn {
     const int32_t* val;
     const uint8_t* int_ok;                // NULL: no value parses
     const long long* ival;
+    __device__ __forceinline__ void range(int32_t node, long long& lo, long long& hi) const { lo = off[node]; hi = off[node + 1]; }
+    __device__ __forceinline__ bool int_at(long long e, long long& v) const {
+        if (!int_ok || !int_ok[e]) return false;
+        v = ival[e];
+        return true;
+    }
+};
+
+// The label table's rows: node i's labels are entries [r * stride, r * stride + count[r]) of key / val, r = node_id[i]; an id
+// outside [0, n_rows) reads as no labels (gp_aff_ids refuses it)
+struct AffLabelsResident {
+    int32_t n, n_rows, stride;
+    const int32_t* node_id;               // [n]
+    const int32_t* count;                 // [n_rows]
+    const int32_t* key;                   // [n_rows * stride]
+    const int32_t* val;
+    const uint8_t* val_int_ok;            // [n_values] ParseInt of the value succeeded
+    const long long* val_int;             // [n_values]
+    __device__ __forceinline__ void range(int32_t node, long long& lo, long long& hi) const {
+        const int32_t r = node_id[node];
+        lo = hi = 0;
+        if (r >= 0 && r < n_rows) { lo = (long long)r * stride; hi = lo + count[r]; }
+    }
+    __device__ __forceinline__ bool int_at(long long e, long long& v) const {
+        const int32_t x = val[e];
+        if (!val_int_ok[x]) return false;
+        v = val_int[x];
+        return true;
+    }
 };
 
 struct AffProgIn {
@@ -98,7 +138,8 @@ __device__ __forceinline__ long long aff_find(const int32_t* __restrict__ keys, 
     return -1;
 }
 
-__device__ __forceinline__ bool aff_req(const AffView& p, long long r, const AffLabelsIn& L, long long lo, long long hi, int32_t node) {
+template <class Lab>
+__device__ __forceinline__ bool aff_req(const AffView& p, long long r, const Lab& L, long long lo, long long hi, int32_t node) {
     const int32_t op = p.req_op[r];
     if (op == kAffFieldNameIn) return (long long)node == p.req_int[r];
     if (op == kAffFieldNameNotIn) return (long long)node != p.req_int[r];
@@ -114,16 +155,19 @@ __device__ __forceinline__ bool aff_req(const AffView& p, long long r, const Aff
     case kAffDoesNotExist: return at < 0;
     case kAffGt:
     case kAffLt: {
-        if (at < 0 || !L.int_ok || !L.int_ok[at]) return false;          // ParseInt failed: no match, not an error
-        return op == kAffGt ? L.ival[at] > p.req_int[r] : L.ival[at] < p.req_int[r];
+        long long v;
+        if (at < 0 || !L.int_at(at, v)) return false;                    // ParseInt failed: no match, not an error
+        return op == kAffGt ? v > p.req_int[r] : v < p.req_int[r];
     }
     default: return false;
     }
 }
 
 // 0 no match, 1 match, 2 error
-__device__ __forceinline__ int aff_outcome(const AffView& p, const AffLabelsIn& L, int32_t node) {
-    const long long lo = L.off[node], hi = L.off[node + 1];
+template <class Lab>
+__device__ __forceinline__ int aff_outcome(const AffView& p, const Lab& L, int32_t node) {
+    long long lo, hi;
+    L.range(node, lo, hi);
     for (int32_t t = 0; t < p.n_sel; ++t) {
         const long long at = aff_find(L.key, lo, hi, p.sel_key[t]);
         if (at < 0 || L.val[at] != p.sel_val[t]) return 0;
@@ -162,8 +206,17 @@ __global__ void gp_aff_labels(AffLabelsIn L, int* err) {
     if (bad) atomicOr(err, bad);
 }
 
+// thread per node of a resident call: its label-table id in [-1, n_rows)
+__global__ void gp_aff_ids(AffLabelsResident L, int* err) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= L.n) return;
+    const int32_t r = L.node_id[i];
+    if (r < -1 || r >= L.n_rows) atomicOr(err, kAffErrNodeId);
+}
+
 // affinities a_base + blockIdx.y (gridDim.y <= 65535: more affinities take more launches)
-__global__ void __launch_bounds__(kAffThreads) gp_aff_match(AffLabelsIn L, AffProgIn P, AffOut out, int32_t a_base) {
+template <class Lab>
+__global__ void __launch_bounds__(kAffThreads) gp_aff_match(Lab L, AffProgIn P, AffOut out, int32_t a_base) {
     __shared__ __align__(16) unsigned char s_prog[kAffSmem];
     const int32_t a = a_base + (int32_t)blockIdx.y;
     const long long s0 = P.sel_off[a], s1 = P.sel_off[a + 1], t0 = P.term_off[a], t1 = P.term_off[a + 1];

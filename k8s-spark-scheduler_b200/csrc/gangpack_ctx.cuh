@@ -231,6 +231,14 @@ struct gp_ctx {
         uint32_t seq = 0;                         // the last update's stamp
     } rt;
 
+    // the resident label table (gangpack_label_table.cu); read by the *_resident affinity entries, changed only by its own
+    struct LabelTable {
+        bool live = false;                        // reset and not broken by a CUDA error since
+        gp_label_table_size size{};
+        DevBuf cols;                              // count, key, val, val_int, val_int_ok and the row / value stamps in one block
+        uint32_t seq = 0;                         // the last update's stamp
+    } lt;
+
     gp_stats last{};
 };
 
@@ -404,3 +412,10 @@ void enqueue_resident_dir(cudaStream_t st, int32_t n, const int32_t* ids, int32_
 // The live reservation table's columns on the device: node id [n_slots] (-1 = free) and cpu / mem / gpu [n_slots] each
 struct RtCols { const int32_t* node; const long long* v[3]; };
 RtCols rt_cols(gp_ctx* c);
+
+// ---- gangpack_label_table.cu -----------------------------------------------------------------------------------------
+
+// The live label table's columns on the device: count [n_node_ids], key / val [n_node_ids * max_labels], val_int / val_int_ok
+// [n_values]
+struct LtCols { const int32_t* count; const int32_t* key; const int32_t* val; const long long* vint; const uint8_t* vok; };
+LtCols lt_cols(gp_ctx* c);

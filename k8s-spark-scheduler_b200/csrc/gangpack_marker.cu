@@ -1,6 +1,7 @@
 // gangpack_marker.cu -- the unschedulable-pod marker's capacity checks (gp_exceeds_cluster_capacity, with required node
-// affinity gp_exceeds_cluster_capacity_affinity, and their *_resident forms over the overhead table), gp_match_node_affinity,
-// and the overhead computer (gp_node_overhead).
+// affinity gp_exceeds_cluster_capacity_affinity, their *_resident forms over the overhead table, and
+// gp_exceeds_cluster_capacity_affinity_label_table over both it and the label table), gp_match_node_affinity[_resident], and
+// the overhead computer (gp_node_overhead).
 #include "gangpack_ctx.cuh"
 #include "gangpack_affinity.cuh"
 #include "gangpack_capacity.cuh"
@@ -11,30 +12,28 @@
 #include <vector>
 
 // ---- required node affinity and the marker's capacity checks (gangpack_affinity.cuh, gangpack_capacity.cuh) ---------------
-// Host checks of the label offsets and of the affinity programs (small); each label entry is checked by gp_aff_match itself.
-static gp_status check_affinity(gp_ctx* c, const gp_node_labels* L, const gp_node_affinities* P, const char* who) {
+static bool csr_ok(const int64_t* off, int64_t n) {     // off[0] = 0, non-decreasing
+    if (off[0] != 0) return false;
+    for (int64_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
+    return true;
+}
+
+// Host checks of the affinity programs (small) against n nodes and the label id ranges n_keys / n_values
+static gp_status check_programs(gp_ctx* c, int32_t n, int32_t n_keys, int32_t n_values, const gp_node_affinities* P, const char* who) {
     auto bad = [&](const char* what) { return fail(c, GP_ERR_INVALID, who, what); };
-    if (!L || !P || L->n_nodes < 0 || L->n_keys < 0 || L->n_values < 0 || P->n_aff < 0 || !L->label_off || !P->sel_off ||
-        !P->term_off || !P->term_req_off || !P->req_val_off || (P->n_aff > 0 && !P->has_required) || (L->label_int_ok && !L->label_int))
+    if (!P || P->n_aff < 0 || !P->sel_off || !P->term_off || !P->term_req_off || !P->req_val_off || (P->n_aff > 0 && !P->has_required))
         return bad("missing arrays or negative sizes");
-    auto csr = [](const int64_t* off, int64_t n) {      // off[0] = 0, non-decreasing
-        if (off[0] != 0) return false;
-        for (int64_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
-        return true;
-    };
-    const int32_t n = L->n_nodes, A = P->n_aff;
-    if (!csr(L->label_off, n)) return bad("label_off does not start at 0 or decreases");
-    if (L->label_off[n] > 0 && (!L->label_key || !L->label_val)) return bad("missing arrays or negative sizes");
-    if (!csr(P->sel_off, A) || !csr(P->term_off, A)) return bad("sel_off or term_off does not start at 0 or decreases");
+    const int32_t A = P->n_aff;
+    if (!csr_ok(P->sel_off, A) || !csr_ok(P->term_off, A)) return bad("sel_off or term_off does not start at 0 or decreases");
     const int64_t ns = P->sel_off[A], nt = P->term_off[A];
-    if (!csr(P->term_req_off, nt)) return bad("term_req_off does not start at 0 or decreases");
+    if (!csr_ok(P->term_req_off, nt)) return bad("term_req_off does not start at 0 or decreases");
     const int64_t nr = P->term_req_off[nt];
-    if (!csr(P->req_val_off, nr)) return bad("req_val_off does not start at 0 or decreases");
+    if (!csr_ok(P->req_val_off, nr)) return bad("req_val_off does not start at 0 or decreases");
     const int64_t nv = P->req_val_off[nr];
     if ((ns > 0 && (!P->sel_key || !P->sel_val)) || (nr > 0 && (!P->req_op || !P->req_key || !P->req_int)) || (nv > 0 && !P->req_val))
         return bad("missing arrays or negative sizes");
     for (int64_t t = 0; t < ns; ++t)
-        if (P->sel_key[t] < 0 || P->sel_key[t] >= L->n_keys || P->sel_val[t] < 0 || P->sel_val[t] >= L->n_values)
+        if (P->sel_key[t] < 0 || P->sel_key[t] >= n_keys || P->sel_val[t] < 0 || P->sel_val[t] >= n_values)
             return bad("node selector key or value id out of range");
     for (int64_t r = 0; r < nr; ++r) {
         const int32_t op = P->req_op[r];
@@ -43,51 +42,82 @@ static gp_status check_affinity(gp_ctx* c, const gp_node_labels* L, const gp_nod
             if (P->req_int[r] < -1 || P->req_int[r] >= n) return bad("metadata.name node index out of range (-1 or 0..n_nodes-1)");
             continue;
         }
-        if (P->req_key[r] < 0 || P->req_key[r] >= L->n_keys) return bad("requirement key id out of range");
+        if (P->req_key[r] < 0 || P->req_key[r] >= n_keys) return bad("requirement key id out of range");
         for (int64_t v = P->req_val_off[r]; v < P->req_val_off[r + 1]; ++v) {
-            if (P->req_val[v] < 0 || P->req_val[v] >= L->n_values) return bad("requirement value id out of range");
+            if (P->req_val[v] < 0 || P->req_val[v] >= n_values) return bad("requirement value id out of range");
             if (v > P->req_val_off[r] && P->req_val[v] <= P->req_val[v - 1]) return bad("requirement values not strictly ascending");
         }
     }
     return GP_OK;
 }
 
+// Host checks of the per-call label offsets, then of the programs against them; each label entry is checked by
+// gp_aff_labels on the device
+static gp_status check_affinity(gp_ctx* c, const gp_node_labels* L, const gp_node_affinities* P, const char* who) {
+    if (!L || L->n_nodes < 0 || L->n_keys < 0 || L->n_values < 0 || !L->label_off || (L->label_int_ok && !L->label_int))
+        return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    const int32_t n = L->n_nodes;
+    if (!csr_ok(L->label_off, n)) return fail(c, GP_ERR_INVALID, who, "label_off does not start at 0 or decreases");
+    if (L->label_off[n] > 0 && (!L->label_key || !L->label_val)) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    return check_programs(c, n, L->n_keys, L->n_values, P, who);
+}
+
+// The same for a resident call: a live label table, the node ids present, the programs against the table's id ranges (each
+// node id is checked by gp_aff_ids on the device)
+static gp_status check_affinity(gp_ctx* c, const gp_resident_labels* L, const gp_node_affinities* P, const char* who) {
+    if (!L || L->n_nodes < 0 || (L->n_nodes > 0 && !L->node_id)) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    if (!c->lt.live) return fail(c, GP_ERR_INVALID, who, "no label table (gp_label_table_reset first)");
+    return check_programs(c, L->n_nodes, c->lt.size.n_keys, c->lt.size.n_values, P, who);
+}
+
 // The label check's status word (kAffErr* bits)
 static const Refusal kAffRefusals[] = {
     {kAffErrLabelKey, GP_ERR_INVALID, "label key id out of range or the keys of a node not strictly ascending"},
     {kAffErrLabelVal, GP_ERR_INVALID, "label value id out of range"},
+    {kAffErrNodeId, GP_ERR_INVALID, "a label-table node id outside [-1, n_node_ids)"},
 };
 
-// Device staging of the labels and programs, and the match launches
+// Device staging of the labels (per-call CSR, or the resident node ids: rl != NULL) and programs, and the match launches
 struct AffStage {
     Piece<long long> loff, lint, soff, toff, troff, rint, rvoff;
-    Piece<int32_t> lkey, lval, skey, sval, rop, rkey, rval, nm, ne;
+    Piece<int32_t> lkey, lval, skey, sval, rop, rkey, rval, nm, ne, rid;
     Piece<uint8_t> lok, hreq, terr;
     Piece<int> err;
     int32_t n, A, words;
+    bool resident = false;
     AffLabelsIn L{};
+    AffLabelsResident R{};
     AffProgIn P{};
 
-    void take(Arena& ar, const gp_node_labels* l, const gp_node_affinities* p) {
-        n = l->n_nodes; A = p->n_aff; words = (n + 31) / 32;
-        const size_t nl = l->label_off[n], ns = p->sel_off[A], nt = p->term_off[A], nr = p->term_req_off[nt], nv = p->req_val_off[nr];
-        const size_t N1 = (size_t)n + 1, A1 = (size_t)A + 1;
+    void take(Arena& ar, const gp_node_labels* l, const gp_resident_labels* rl, const gp_node_affinities* p) {
+        resident = rl != nullptr;
+        n = resident ? rl->n_nodes : l->n_nodes; A = p->n_aff; words = (n + 31) / 32;
+        const size_t nl = resident ? 0 : l->label_off[n], ns = p->sel_off[A], nt = p->term_off[A], nr = p->term_req_off[nt],
+                     nv = p->req_val_off[nr];
+        const size_t N1 = resident ? 0 : (size_t)n + 1, A1 = (size_t)A + 1;
         loff = ar.take<long long>(N1); lkey = ar.take<int32_t>(nl); lval = ar.take<int32_t>(nl); lok = ar.take<uint8_t>(nl);
-        lint = ar.take<long long>(nl);
+        lint = ar.take<long long>(nl); rid = ar.take<int32_t>(resident ? (size_t)n : 0);
         soff = ar.take<long long>(A1); skey = ar.take<int32_t>(ns); sval = ar.take<int32_t>(ns); hreq = ar.take<uint8_t>(A);
         toff = ar.take<long long>(A1); troff = ar.take<long long>(nt + 1); terr = ar.take<uint8_t>(nt);
         rop = ar.take<int32_t>(nr); rkey = ar.take<int32_t>(nr); rint = ar.take<long long>(nr); rvoff = ar.take<long long>(nr + 1);
         rval = ar.take<int32_t>(nv);
         nm = ar.take<int32_t>(A); ne = ar.take<int32_t>(A); err = ar.take<int>(2);
     }
-    // uploads (an absent column is zeroed), zeroes the counters and the error word, and checks the labels once, whatever
-    // the number of affinities
-    gp_status upload(gp_ctx* c, Arena& ar, const gp_node_labels* l, const gp_node_affinities* p) {
-        L.n = n; L.n_keys = l->n_keys; L.n_values = l->n_values;
-        L.off = ar.put_or_zero(loff, l->label_off); L.key = ar.put_or_zero(lkey, l->label_key); L.val = ar.put_or_zero(lval, l->label_val);
-        const uint8_t* int_ok = ar.put_or_zero(lok, l->label_int_ok);
-        L.int_ok = l->label_int_ok ? int_ok : nullptr;
-        L.ival = ar.put_or_zero(lint, l->label_int);
+    // uploads (an absent column is zeroed), zeroes the counters and the error word, and checks the labels (or the resident
+    // node ids) once, whatever the number of affinities
+    gp_status upload(gp_ctx* c, Arena& ar, const gp_node_labels* l, const gp_resident_labels* rl, const gp_node_affinities* p) {
+        if (resident) {
+            const LtCols t = lt_cols(c);
+            R.n = n; R.n_rows = c->lt.size.n_node_ids; R.stride = c->lt.size.max_labels;
+            R.count = t.count; R.key = t.key; R.val = t.val; R.val_int_ok = t.vok; R.val_int = t.vint;
+            R.node_id = ar.put(rid, rl->node_id);
+        } else {
+            L.n = n; L.n_keys = l->n_keys; L.n_values = l->n_values;
+            L.off = ar.put_or_zero(loff, l->label_off); L.key = ar.put_or_zero(lkey, l->label_key); L.val = ar.put_or_zero(lval, l->label_val);
+            const uint8_t* int_ok = ar.put_or_zero(lok, l->label_int_ok);
+            L.int_ok = l->label_int_ok ? int_ok : nullptr;
+            L.ival = ar.put_or_zero(lint, l->label_int);
+        }
         P.n_aff = A;
         P.sel_off = ar.put_or_zero(soff, p->sel_off); P.sel_key = ar.put_or_zero(skey, p->sel_key); P.sel_val = ar.put_or_zero(sval, p->sel_val);
         P.has_required = ar.put_or_zero(hreq, p->has_required); P.term_off = ar.put_or_zero(toff, p->term_off);
@@ -98,7 +128,9 @@ struct AffStage {
         ar.zero(ne);
         ar.zero(err);
         GP_TRY(ar.check(c));
-        if (n > 0) gp_aff_labels<<<(unsigned)((n + kAffThreads - 1) / kAffThreads), kAffThreads, 0, ar.st>>>(L, ar.ptr(err));
+        const unsigned blocks = (unsigned)((n + kAffThreads - 1) / kAffThreads);
+        if (n > 0 && resident) gp_aff_ids<<<blocks, kAffThreads, 0, ar.st>>>(R, ar.ptr(err));
+        else if (n > 0) gp_aff_labels<<<blocks, kAffThreads, 0, ar.st>>>(L, ar.ptr(err));
         return GP_OK;
     }
     // affinities [a0, a0 + k) into member rows 0..k-1
@@ -107,7 +139,8 @@ struct AffStage {
         AffOut out{member, ar.ptr(nm), ar.ptr(ne), words, a0};
         for (int32_t y = 0; y < k; y += 65535) {
             const dim3 grid((unsigned)((n + kAffThreads - 1) / kAffThreads), (unsigned)std::min(k - y, 65535));
-            gp_aff_match<<<grid, kAffThreads, 0, ar.st>>>(L, P, out, a0 + y);
+            if (resident) gp_aff_match<<<grid, kAffThreads, 0, ar.st>>>(R, P, out, a0 + y);
+            else gp_aff_match<<<grid, kAffThreads, 0, ar.st>>>(L, P, out, a0 + y);
         }
     }
 };
@@ -115,9 +148,11 @@ struct AffStage {
 // DoesPodExceedClusterCapacity for a batch of stale drivers, any packer; the node sets are the node_group classes (aff ==
 // NULL) or the affinities' matches.  The overhead is nodes->overhead_* (resident false) or, resident, GetNonSchedulableOverhead
 // of the overhead table's records on node id over_ids[i] (-1: none), summed into this call's scratch by the query's kernels.
+// The affinities' labels are the per-call labels, or with rlabels the label table's rows.
 static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
                               const gp_node_affinities* aff, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds,
-                              uint8_t* affinity_error, bool resident = false, const int32_t* over_ids = nullptr) {
+                              uint8_t* affinity_error, bool resident = false, const int32_t* over_ids = nullptr,
+                              const gp_resident_labels* rlabels = nullptr) {
     if (!aff) {
         if (!nodes || !a || nodes->n_nodes < 0 || a->n_apps < 0 || nodes->n_groups < 1 || (nodes->zone_id && nodes->n_zones < 1) ||
             (nodes->n_nodes > 0 && (!nodes->alloc_cpu_milli || !nodes->alloc_mem_bytes)) ||
@@ -130,8 +165,9 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
                                !a->group || !exceeds)))
             return fail(c, GP_ERR_INVALID, who, "missing arrays or bad sizes (group required; n_zones >= 1 with zone_id)");
         if (nodes->node_group) return fail(c, GP_ERR_INVALID, who, "node_group must be NULL: the node sets are the affinities' matches");
-        if (!labels || labels->n_nodes != nodes->n_nodes) return fail(c, GP_ERR_INVALID, who, "labels->n_nodes != nodes->n_nodes");
-        const gp_status s = check_affinity(c, labels, aff, who);
+        if (rlabels ? rlabels->n_nodes != nodes->n_nodes : (!labels || labels->n_nodes != nodes->n_nodes))
+            return fail(c, GP_ERR_INVALID, who, "labels->n_nodes != nodes->n_nodes");
+        const gp_status s = rlabels ? check_affinity(c, rlabels, aff, who) : check_affinity(c, labels, aff, who);
         if (s != GP_OK) return s;
     }
     if ((int)packer < GP_BP_TIGHTLY_PACK || (int)packer > GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) return fail(c, GP_ERR_INVALID, who, "unknown packer");
@@ -177,7 +213,7 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     const auto d_out = ar.take<uint8_t>(q1);
     AffStage as{};
     Piece<uint32_t> member{0, 0};
-    if (aff) { as.take(ar, labels, aff); member = ar.take<uint32_t>((size_t)K * (size_t)as.words); }
+    if (aff) { as.take(ar, labels, rlabels, aff); member = ar.take<uint32_t>((size_t)K * (size_t)as.words); }
     const size_t NR = resident ? N : 0;
     const auto oids = ar.take<int32_t>(NR), odir = ar.take<int32_t>(resident ? (size_t)c->oht.size.n_node_ids : 0);
     const auto oacc = ar.take<unsigned long long>(12 * NR), owarned = ar.take<unsigned long long>(resident ? 1 : 0);
@@ -189,7 +225,7 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         ar.fill(odir, 0xff);
         ar.fill(oacc, oerr, 0);
     }
-    if (aff) GP_TRY(as.upload(c, ar, labels, aff));
+    if (aff) GP_TRY(as.upload(c, ar, labels, rlabels, aff));
     CapScratch s{};
     s.key = ar.ptr(key); s.rank = ar.ptr(rank); s.zone = ar.ptr(zst); s.bucket_cnt = ar.ptr(bcnt);
     s.bucket_off = ar.ptr(boff); s.seg_off = ar.ptr(soff); s.ms_off = ar.ptr(moff);
@@ -323,21 +359,30 @@ gp_status gp_exceeds_cluster_capacity_affinity_resident(gp_ctx* c, const gp_capa
     return capacity_run(c, who, nodes, labels, affinities, a, packer, exceeds, affinity_error, true, overhead_node_id);
 }
 
-// GetRequiredNodeAffinity(...).Match for every (affinity, node); see gangpack_affinity.cuh
-gp_status gp_match_node_affinity(gp_ctx* c, const gp_node_labels* labels, const gp_node_affinities* affinities, gp_affinity_match* out) {
+// the same with the labels read in place from the label table
+gp_status gp_exceeds_cluster_capacity_affinity_label_table(gp_ctx* c, const gp_capacity_nodes* nodes, const int32_t* overhead_node_id,
+                                                           const gp_resident_labels* labels, const gp_node_affinities* affinities,
+                                                           const gp_apps* a, gp_binpacker packer, uint8_t* exceeds, uint8_t* affinity_error) {
     if (!enter(c)) return GP_ERR_INVALID;
-    static const char* who = "gp_match_node_affinity";
-    gp_status s = check_affinity(c, labels, affinities, who);
+    static const char* who = "gp_exceeds_cluster_capacity_affinity_label_table";
+    if (!affinities || !labels) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    return capacity_run(c, who, nodes, nullptr, affinities, a, packer, exceeds, affinity_error, true, overhead_node_id, labels);
+}
+
+// GetRequiredNodeAffinity(...).Match for every (affinity, node) over the per-call labels or (rl) the label table's rows
+static gp_status match_run(gp_ctx* c, const char* who, const gp_node_labels* labels, const gp_resident_labels* rl,
+                           const gp_node_affinities* affinities, gp_affinity_match* out) {
+    gp_status s = rl ? check_affinity(c, rl, affinities, who) : check_affinity(c, labels, affinities, who);
     if (s != GP_OK) return s;
     if (!out) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     Arena ar{c->callbuf, st};
     AffStage as{};
-    as.take(ar, labels, affinities);
+    as.take(ar, labels, rl, affinities);
     const auto member = ar.take<uint32_t>((size_t)as.A * (size_t)as.words);
     ar.reserve();
-    GP_TRY(as.upload(c, ar, labels, affinities));
+    GP_TRY(as.upload(c, ar, labels, rl, affinities));
     as.match(ar, ar.ptr(member), 0, as.A);
     GP_CUDA(c, cudaGetLastError());
     int aerr = 0;
@@ -347,6 +392,18 @@ gp_status gp_match_node_affinity(gp_ctx* c, const gp_node_labels* labels, const 
     ar.get(&aerr, ar.ptr(as.err), 1);
     GP_TRY(ar.sync(c));
     return refuse(c, aerr, kAffRefusals, who);
+}
+
+// see gangpack_affinity.cuh
+gp_status gp_match_node_affinity(gp_ctx* c, const gp_node_labels* labels, const gp_node_affinities* affinities, gp_affinity_match* out) {
+    if (!enter(c)) return GP_ERR_INVALID;
+    return match_run(c, "gp_match_node_affinity", labels, nullptr, affinities, out);
+}
+
+gp_status gp_match_node_affinity_resident(gp_ctx* c, const gp_resident_labels* labels, const gp_node_affinities* affinities,
+                                          gp_affinity_match* out) {
+    if (!enter(c)) return GP_ERR_INVALID;
+    return match_run(c, "gp_match_node_affinity_resident", nullptr, labels, affinities, out);
 }
 
 // The overhead kernels' status word (kOhErr* bits)

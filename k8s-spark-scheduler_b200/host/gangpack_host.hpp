@@ -761,6 +761,10 @@ struct Encoded {
     }
 };
 
+template <class KeyFn, class ValFn>
+inline void EncodePrograms(Encoded& e, const std::vector<Program>& programs, KeyFn key, ValFn val,
+                           const std::unordered_map<std::string, int32_t>& nodeIndex);
+
 inline Encoded Encode(const std::vector<Node>& nodes, const std::vector<Program>& programs) {
     Encoded e;
     std::unordered_map<std::string, int32_t> keys, vals, nodeIndex;
@@ -781,6 +785,15 @@ inline Encoded Encode(const std::vector<Node>& nodes, const std::vector<Program>
         }
         e.label_off.push_back((int64_t)e.label_key.size());
     }
+    EncodePrograms(e, programs, key, val, nodeIndex);
+    e.n_nodes = (int32_t)nodes.size(); e.n_keys = (int32_t)keys.size(); e.n_values = (int32_t)vals.size();
+    return e;
+}
+
+// The gp_node_affinities arrays of the programs into e, label keys and values mapped by key / val, metadata.name by nodeIndex
+template <class KeyFn, class ValFn>
+inline void EncodePrograms(Encoded& e, const std::vector<Program>& programs, KeyFn key, ValFn val,
+                           const std::unordered_map<std::string, int32_t>& nodeIndex) {
     auto addReq = [&](int32_t op, int32_t k, int64_t bound, std::vector<int32_t> vs) {
         std::sort(vs.begin(), vs.end());
         vs.erase(std::unique(vs.begin(), vs.end()), vs.end());
@@ -823,13 +836,11 @@ inline Encoded Encode(const std::vector<Node>& nodes, const std::vector<Program>
         }
         e.term_off.push_back((int64_t)e.term_parse_error.size());
     }
-    e.n_nodes = (int32_t)nodes.size(); e.n_keys = (int32_t)keys.size(); e.n_values = (int32_t)vals.size();
     e.n_aff = (int32_t)programs.size();
     // never hand a NULL pointer for an empty column
     for (auto* v : {&e.label_key, &e.label_val, &e.sel_key, &e.sel_val, &e.req_op, &e.req_key, &e.req_val}) v->reserve(1);
     for (auto* v : {&e.label_int, &e.req_int}) v->reserve(1);
     for (auto* v : {&e.label_int_ok, &e.has_required, &e.term_parse_error}) v->reserve(1);
-    return e;
 }
 
 // utils.ListWithPredicate(nodes, GetRequiredNodeAffinity(pod).Match) for every program at once (gp_match_node_affinity):
@@ -851,6 +862,171 @@ inline MatchResult MatchRequiredNodeAffinity(const std::vector<Node>& nodes, con
     for (size_t p = 0; p < A; ++p) {
         r.Failed[p] = nError[p] > 0;
         for (size_t i = 0; i < nodes.size(); ++i)
+            if ((member[p * words + i / 32] >> (i % 32)) & 1u) r.Matched[p].push_back((int32_t)i);
+    }
+    return r;
+}
+
+// Every node's labels as the resident label table (gp_label_table_*) keeps them, from the node informer: SetNode for AddFunc
+// and UpdateFunc (no write when the labels are unchanged), DeleteNode for DeleteFunc.  Keys and values are interned for good,
+// id 0 of each reserved for strings no node carries, so encoding a program never changes the table; node ids freed by a
+// delete go to the next new node.  Flush sends what changed since the last flush in one update, after a reset with doubled
+// capacities and the whole state when a capacity would be exceeded (or after Replay).
+class ResidentLabels {
+public:
+    explicit ResidentLabels(gp_label_table_size initial = {64, 16, 64, 256}) : size_(initial) {
+        parsed_.push_back({0, 0});                       // value id 0: reserved
+    }
+
+    void SetNode(const Node& n) {
+        auto it = labels_.find(n.Name);
+        if (it != labels_.end() && it->second == n.Labels) return;
+        labels_[n.Name] = n.Labels;
+        auto id = nodes_.find(n.Name);
+        int32_t at;
+        if (id != nodes_.end()) at = id->second;
+        else {
+            if (!free_.empty()) { at = free_.back(); free_.pop_back(); }
+            else { at = (int32_t)rows_.size(); rows_.emplace_back(); }
+            nodes_.emplace(n.Name, at);
+        }
+        std::vector<std::pair<int32_t, int32_t>> row;
+        for (const auto& kv : n.Labels) row.emplace_back(InternKey(kv.first), InternVal(kv.second));
+        std::sort(row.begin(), row.end());
+        rows_[(size_t)at] = std::move(row);
+        dirty_.insert(at);
+    }
+    void DeleteNode(const std::string& name) {
+        auto id = nodes_.find(name);
+        if (id == nodes_.end()) return;
+        rows_[(size_t)id->second].clear();
+        dirty_.insert(id->second);
+        free_.push_back(id->second);
+        nodes_.erase(id);
+        labels_.erase(name);
+    }
+
+    // the table's id of each node name, -1 for a node it does not know (no labels)
+    std::vector<int32_t> NodeIDs(const std::vector<std::string>& names) const {
+        std::vector<int32_t> ids(names.size(), -1);
+        for (size_t i = 0; i < names.size(); ++i) {
+            auto it = nodes_.find(names[i]);
+            if (it != nodes_.end()) ids[i] = it->second;
+        }
+        return ids;
+    }
+    // the nodes as the per-call Encode takes them (a node the table does not know has no labels)
+    std::vector<Node> Nodes(const std::vector<std::string>& names) const {
+        std::vector<Node> out;
+        for (const auto& nm : names) {
+            auto it = labels_.find(nm);
+            out.push_back(Node{nm, it == labels_.end() ? std::map<std::string, std::string>{} : it->second});
+        }
+        return out;
+    }
+    // the programs against this table's ids (gp_node_affinities of the returned object), metadata.name by index in names
+    Encoded EncodePrograms(const std::vector<std::string>& names, const std::vector<Program>& programs) const {
+        Encoded e;
+        std::unordered_map<std::string, int32_t> nodeIndex;
+        for (size_t i = 0; i < names.size(); ++i) nodeIndex.emplace(names[i], (int32_t)i);
+        auto key = [&](const std::string& k) { auto it = keyId_.find(k); return it == keyId_.end() ? 0 : it->second; };
+        auto val = [&](const std::string& v) { auto it = valId_.find(v); return it == valId_.end() ? 0 : it->second; };
+        affinity::EncodePrograms(e, programs, key, val, nodeIndex);
+        e.n_nodes = (int32_t)names.size(); e.n_keys = size_.n_keys; e.n_values = size_.n_values;
+        return e;
+    }
+
+    // the next Flush resets the table and sends the whole state again (after a refused resident call)
+    void Replay() { replay_ = true; }
+
+    void Flush(gangpack::Device& dev) {
+        int32_t longest = 0;
+        for (const auto& r : rows_) longest = std::max(longest, (int32_t)r.size());
+        auto grow = [&](int32_t& cap, int64_t need) { while (cap < need) { cap = std::max<int32_t>(2 * cap, 1); replay_ = true; } };
+        grow(size_.n_node_ids, (int64_t)rows_.size());
+        grow(size_.max_labels, longest);
+        grow(size_.n_keys, (int64_t)keyId_.size() + 1);
+        grow(size_.n_values, (int64_t)parsed_.size());
+        std::vector<int32_t> rowNode, key, val, valueId;
+        std::vector<int64_t> off{0}, valueInt;
+        std::vector<uint8_t> valueOk;
+        auto row = [&](int32_t at) {
+            rowNode.push_back(at);
+            for (const auto& kv : rows_[(size_t)at]) { key.push_back(kv.first); val.push_back(kv.second); }
+            off.push_back((int64_t)key.size());
+        };
+        auto value = [&](int32_t v) { valueId.push_back(v); valueOk.push_back(parsed_[(size_t)v].first); valueInt.push_back(parsed_[(size_t)v].second); };
+        if (replay_) {
+            for (int32_t at = 0; at < (int32_t)rows_.size(); ++at) if (!rows_[(size_t)at].empty()) row(at);
+            for (int32_t v = 1; v < (int32_t)parsed_.size(); ++v) value(v);
+        } else {
+            for (int32_t at : dirty_) row(at);
+            for (int32_t v : newVals_) value(v);
+        }
+        const bool reset = replay_;
+        replay_ = true;                            // until the table holds this state: a failed call replays next time
+        if (reset) dev.check(gp_label_table_reset(dev.ctx(), &size_), "gp_label_table_reset");
+        if (!rowNode.empty() || !valueId.empty()) {
+            for (auto* v : {&key, &val, &rowNode, &valueId}) v->reserve(1);
+            valueOk.reserve(1); valueInt.reserve(1);
+            gp_label_delta d{(int32_t)rowNode.size(), (int32_t)valueId.size(), rowNode.data(), off.data(), key.data(), val.data(),
+                             valueId.data(), valueOk.data(), valueInt.data()};
+            dev.check(gp_label_table_update(dev.ctx(), &d), "gp_label_table_update");
+        }
+        replay_ = false;
+        dirty_.clear();
+        newVals_.clear();
+    }
+
+private:
+    int32_t InternKey(const std::string& k) { return keyId_.emplace(k, (int32_t)keyId_.size() + 1).first->second; }
+    int32_t InternVal(const std::string& v) {
+        auto it = valId_.find(v);
+        if (it != valId_.end()) return it->second;
+        const int32_t id = (int32_t)parsed_.size();
+        int64_t x = 0;
+        const bool ok = ParseInt(v, &x);
+        parsed_.push_back({ok ? 1 : 0, ok ? x : 0});
+        valId_.emplace(v, id);
+        newVals_.push_back(id);
+        return id;
+    }
+
+    gp_label_table_size size_;
+    bool replay_ = true;
+    std::map<std::string, std::map<std::string, std::string>> labels_;
+    std::unordered_map<std::string, int32_t> nodes_, keyId_, valId_;   // key ids start at 1, value ids at 1
+    std::vector<std::pair<uint8_t, int64_t>> parsed_;             // per value id: ParseInt of the string
+    std::vector<std::vector<std::pair<int32_t, int32_t>>> rows_;  // per node id: (key id, value id) by key id
+    std::vector<int32_t> free_, newVals_;
+    std::set<int32_t> dirty_;
+};
+
+// MatchRequiredNodeAffinity over the resident label table (gp_match_node_affinity_resident): the table's pending delta is
+// flushed once, then one device call reads every label in place.  A refused call resets and replays the table and is made
+// again per call, over the table's labels (Encode + gp_match_node_affinity), which answers or refuses as it does.
+inline MatchResult MatchRequiredNodeAffinity(const std::vector<std::string>& nodeNames, ResidentLabels& labels,
+                                             const std::vector<Program>& programs) {
+    gangpack::Device& dev = gangpack::Device::Get();
+    labels.Flush(dev);
+    const std::vector<int32_t> ids = labels.NodeIDs(nodeNames);
+    const Encoded e = labels.EncodePrograms(nodeNames, programs);
+    const gp_node_affinities a = e.Programs();
+    const gp_resident_labels rl{(int32_t)nodeNames.size(), 0, ids.data()};
+    const size_t words = (nodeNames.size() + 31) / 32, A = programs.size();
+    std::vector<uint32_t> member(std::max<size_t>(A * words, 1));
+    std::vector<int32_t> nMatch(std::max<size_t>(A, 1)), nError(std::max<size_t>(A, 1));
+    gp_affinity_match out{member.data(), nMatch.data(), nError.data()};
+    if (gp_match_node_affinity_resident(dev.ctx(), &rl, &a, &out) != GP_OK) {
+        labels.Replay();
+        labels.Flush(dev);
+        return MatchRequiredNodeAffinity(labels.Nodes(nodeNames), programs);
+    }
+    MatchResult r;
+    r.Matched.resize(A); r.Failed.resize(A);
+    for (size_t p = 0; p < A; ++p) {
+        r.Failed[p] = nError[p] > 0;
+        for (size_t i = 0; i < nodeNames.size(); ++i)
             if ((member[p * words + i / 32] >> (i % 32)) & 1u) r.Matched[p].push_back((int32_t)i);
     }
     return r;
@@ -1363,6 +1539,14 @@ public:
         if (affinityError) affinityError->assign(err.begin(), err.begin() + (std::ptrdiff_t)Q);
         return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
     }
+
+    // The affinity sweep over both resident tables: GetNonSchedulableOverhead from the overhead table and every node's labels
+    // from the label table, each flushed once, then one gp_exceeds_cluster_capacity_affinity_label_table call.  A refused
+    // call resets and replays both tables and is made again per call, over the tables' labels and GetNonSchedulableOverhead
+    // (defined after ResidentOverheadComputer).
+    std::vector<bool> DoesPodsExceedClusterCapacity(const std::vector<CapacityNode>& nodes, ResidentOverheadComputer& overhead,
+                                                    affinity::ResidentLabels& labels, const std::vector<affinity::Program>& programs,
+                                                    const std::vector<AffinityStaleDriver>& drivers, std::vector<bool>* affinityError) const;
 
 private:
     gp_binpacker Packer() const {
@@ -2147,6 +2331,67 @@ inline std::vector<bool> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(c
         md[node.Name] = m;
     }
     return DoesPodsExceedClusterCapacity(md, nodeClass, nClasses, drivers);
+}
+
+inline std::vector<bool> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(const std::vector<CapacityNode>& nodes,
+                                                                               ResidentOverheadComputer& overhead,
+                                                                               affinity::ResidentLabels& labels,
+                                                                               const std::vector<affinity::Program>& programs,
+                                                                               const std::vector<AffinityStaleDriver>& drivers,
+                                                                               std::vector<bool>* affinityError) const {
+    gangpack::Device& dev = gangpack::Device::Get();
+    overhead.Flush(dev);
+    labels.Flush(dev);
+    const size_t N = nodes.size(), Q = drivers.size();
+    std::vector<std::string> names;
+    std::vector<int64_t> ac(N + 1), am(N + 1), ag(N + 1);
+    std::vector<int32_t> zone(N + 1);
+    std::unordered_map<std::string, int32_t> zoneId;
+    for (size_t i = 0; i < N; ++i) {
+        names.push_back(nodes[i].Name);
+        ac[i] = nodes[i].Allocatable.CPU; am[i] = nodes[i].Allocatable.Memory; ag[i] = nodes[i].Allocatable.NvidiaGPU;
+        zone[i] = zoneId.emplace(nodes[i].ZoneLabel, (int32_t)zoneId.size()).first->second;
+    }
+    const std::vector<int32_t> oids = overhead.NodeIDs(names), lids = labels.NodeIDs(names);
+    std::vector<int64_t> q[6];
+    std::vector<int32_t> count(Q + 1), prog(Q + 1);
+    for (auto& col : q) col.resize(Q + 1);
+    for (size_t i = 0; i < Q; ++i) {
+        const AffinityStaleDriver& d = drivers[i];
+        q[0][i] = d.DriverResources.CPU; q[1][i] = d.DriverResources.Memory; q[2][i] = d.DriverResources.NvidiaGPU;
+        q[3][i] = d.ExecutorResources.CPU; q[4][i] = d.ExecutorResources.Memory; q[5][i] = d.ExecutorResources.NvidiaGPU;
+        count[i] = d.MinExecutorCount; prog[i] = d.Affinity;
+    }
+    const affinity::Encoded e = labels.EncodePrograms(names, programs);
+    const gp_node_affinities p = e.Programs();
+    const gp_resident_labels rl{(int32_t)N, 0, lids.data()};
+    gp_capacity_nodes n{};
+    n.n_nodes = (int32_t)N;
+    n.alloc_cpu_milli = ac.data(); n.alloc_mem_bytes = am.data(); n.alloc_gpu = ag.data();
+    n.n_zones = std::max<int32_t>(1, (int32_t)zoneId.size()); n.zone_id = zone.data();
+    gp_apps a{};
+    a.n_apps = (int32_t)Q;
+    a.drv_cpu_milli = q[0].data(); a.drv_mem_bytes = q[1].data(); a.drv_gpu = q[2].data();
+    a.exe_cpu_milli = q[3].data(); a.exe_mem_bytes = q[4].data(); a.exe_gpu = q[5].data();
+    a.exe_count = count.data(); a.group = prog.data();
+    std::vector<uint8_t> out(Q + 1), err(Q + 1);
+    if (gp_exceeds_cluster_capacity_affinity_label_table(dev.ctx(), &n, oids.data(), &rl, &p, &a, Packer(), out.data(), err.data()) == GP_OK) {
+        if (affinityError) affinityError->assign(err.begin(), err.begin() + (std::ptrdiff_t)Q);
+        return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
+    }
+    overhead.Replay();
+    labels.Replay();
+    labels.Flush(dev);
+    const resources::NodeGroupResources nonsched = overhead.GetNonSchedulableOverhead(names);
+    resources::NodeGroupSchedulingMetadata md;
+    for (const auto& node : nodes) {
+        resources::NodeSchedulingMetadata m;
+        m.SchedulableResources = node.Allocatable;
+        m.SchedulableResources.Sub(nonsched.at(node.Name));
+        m.ZoneLabel = node.ZoneLabel;
+        md[node.Name] = m;
+    }
+    return DoesPodsExceedClusterCapacity(md, labels.Nodes(names), programs, drivers, affinityError);
 }
 
 }  // namespace extender

@@ -41,7 +41,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_reservation_table_reset", "gp_reservation_table_update", "gp_prepare_cluster_groups_resident",
            "gp_prepare_cluster_zones_groups_resident", "gp_reschedule_from_reservations_resident",
            "gp_reconcile_find_nodes_resident", "gp_exceeds_cluster_capacity_resident",
-           "gp_exceeds_cluster_capacity_affinity_resident",
+           "gp_exceeds_cluster_capacity_affinity_resident", "gp_label_table_reset", "gp_label_table_update",
+           "gp_match_node_affinity_resident", "gp_exceeds_cluster_capacity_affinity_label_table",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -272,6 +273,20 @@ class gp_resident_usage(C.Structure):
                 ("overhead_mem_bytes", C.c_void_p), ("overhead_gpu", C.c_void_p)]
 
 
+class gp_label_table_size(C.Structure):
+    _fields_ = [("n_node_ids", C.c_int32), ("max_labels", C.c_int32), ("n_keys", C.c_int32), ("n_values", C.c_int32)]
+
+
+class gp_label_delta(C.Structure):
+    _fields_ = [("n_rows", C.c_int32), ("n_values", C.c_int32), ("row_node", C.c_void_p), ("row_off", C.c_void_p),
+                ("label_key", C.c_void_p), ("label_val", C.c_void_p), ("value_id", C.c_void_p), ("value_int_ok", C.c_void_p),
+                ("value_int", C.c_void_p)]
+
+
+class gp_resident_labels(C.Structure):
+    _fields_ = [("n_nodes", C.c_int32), ("reserved", C.c_int32), ("node_id", C.c_void_p)]
+
+
 class gp_placement_record(C.Structure):
     _fields_ = [("collocation", C.c_int32), ("distinct_exec_nodes", C.c_int32), ("execs_per_node", C.c_int32), ("n_zones", C.c_int32),
                 ("cross_zone_pairs", C.c_int64), ("total_pairs", C.c_int64)]
@@ -394,6 +409,17 @@ def load():
     L.gp_exceeds_cluster_capacity_affinity_resident.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.c_void_p,
                                                                 C.POINTER(gp_node_labels), C.POINTER(gp_node_affinities),
                                                                 C.POINTER(gp_apps), C.c_int, C.c_void_p, C.c_void_p]
+    L.gp_label_table_reset.restype = C.c_int
+    L.gp_label_table_reset.argtypes = [C.c_void_p, C.POINTER(gp_label_table_size)]
+    L.gp_label_table_update.restype = C.c_int
+    L.gp_label_table_update.argtypes = [C.c_void_p, C.POINTER(gp_label_delta)]
+    L.gp_match_node_affinity_resident.restype = C.c_int
+    L.gp_match_node_affinity_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_labels), C.POINTER(gp_node_affinities),
+                                                  C.POINTER(gp_affinity_match)]
+    L.gp_exceeds_cluster_capacity_affinity_label_table.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_affinity_label_table.argtypes = [C.c_void_p, C.POINTER(gp_capacity_nodes), C.c_void_p,
+                                                                   C.POINTER(gp_resident_labels), C.POINTER(gp_node_affinities),
+                                                                   C.POINTER(gp_apps), C.c_int, C.c_void_p, C.c_void_p]
     L.gp_reschedule_from_reservations_resident.restype = C.c_int
     L.gp_reschedule_from_reservations_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input),
                                                            C.POINTER(gp_reschedule_scope), C.POINTER(gp_reschedule), C.c_void_p,
@@ -493,6 +519,13 @@ def _resident_usage(node_id, alloc, overhead=None, overhead_node_id=None):
     return ru
 
 
+def _resident_labels(node_id):
+    ids = _np(node_id, np.int32)
+    rl = gp_resident_labels(n_nodes=len(ids), node_id=_p(ids))
+    rl._keep = ids
+    return rl
+
+
 def _capacity_nodes(alloc, overhead, zone_id, n_zones, node_group, n_groups):
     """gp_capacity_nodes over (cpu, mem[, gpu]) triples; overhead may be None.  The struct keeps its arrays alive."""
     al = [_np(v, np.int64) for v in alloc]
@@ -572,6 +605,10 @@ _DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "req_cpu_milli": np.int64,
                "spark_scheduler": np.uint8, "rr_app_key": np.int32, "rr_exists": np.uint8, "member_kind": np.uint8,
                "member_app": np.int32, "member_name": np.int32, "member_present": np.uint8}
 
+# gp_label_delta's columns (affinity.LabelTable.delta() keys)
+_LT_DELTA_COLS = {"row_node": np.int32, "row_off": np.int64, "label_key": np.int32, "label_val": np.int32, "value_id": np.int32,
+                  "value_int_ok": np.uint8, "value_int": np.int64}
+
 # gp_reservation_delta's columns (reservations.ReservationTable.delta() keys)
 _RT_DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "cpu_milli": np.int64, "mem_bytes": np.int64, "gpu": np.int64}
 
@@ -585,13 +622,19 @@ def _affinity_input(enc: dict):
     """(gp_node_labels, gp_node_affinities) over the arrays of affinity.encode() (or the same keys given by hand; a missing
     optional column is NULL).  The structs keep their arrays alive."""
     lc = {k: _np(enc.get(k), t) for k, t in _LABEL_COLS.items()}
-    ac = {k: _np(enc.get(k), t) for k, t in _AFF_COLS.items()}
     n = int(enc["n_nodes"]) if "n_nodes" in enc else len(lc["label_off"]) - 1
     lab = gp_node_labels(n_nodes=n, n_keys=int(enc["n_keys"]), n_values=int(enc["n_values"]), **{k: _p(v) for k, v in lc.items()})
+    lab._keep = lc
+    return lab, _programs(enc)
+
+
+def _programs(enc: dict):
+    """gp_node_affinities over the program arrays of enc; the struct keeps its arrays alive."""
+    ac = {k: _np(enc.get(k), t) for k, t in _AFF_COLS.items()}
     n_aff = int(enc["n_aff"]) if "n_aff" in enc else len(ac["sel_off"]) - 1
     aff = gp_node_affinities(n_aff=n_aff, **{k: _p(v) for k, v in ac.items()})
-    lab._keep, aff._keep = lc, ac
-    return lab, aff
+    aff._keep = ac
+    return aff
 
 
 def compact_apps(apps: dict, mem_shift: int = 20):
@@ -1161,12 +1204,22 @@ class GangPacker:
         (gp_match_node_affinity).  -> (member uint32[n_aff][ceil(n / 32)], n_match int32[n_aff], n_error int32[n_aff]);
         a non-zero n_error is ListWithPredicate's error (the Predicate's failureInternal)."""
         lab, aff = _affinity_input(enc)
-        words = (lab.n_nodes + 31) // 32
+        return self._match(load().gp_match_node_affinity, lab, aff, lab.n_nodes)
+
+    def match_node_affinity_resident(self, node_id, enc: dict):
+        """match_node_affinity with the labels read in place from the label table (gp_match_node_affinity_resident): node_id
+        [n] the label-table id of each node (-1 = no labels), enc the programs of LabelTable.encode_affinities()."""
+        rl = _resident_labels(node_id)
+        aff = _programs(enc)
+        return self._match(load().gp_match_node_affinity_resident, rl, aff, rl.n_nodes)
+
+    def _match(self, fn, lab, aff, n):
+        words = (n + 31) // 32
         member = np.zeros((max(aff.n_aff, 1), max(words, 1)), np.uint32)
         n_match = np.zeros(max(aff.n_aff, 1), np.int32)
         n_error = np.zeros(max(aff.n_aff, 1), np.int32)
         out = gp_affinity_match(member=_p(member), n_match=_p(n_match), n_error=_p(n_error))
-        self._check(load().gp_match_node_affinity(self._h, C.byref(lab), C.byref(aff), C.byref(out)))
+        self._check(fn(self._h, C.byref(lab), C.byref(aff), C.byref(out)))
         return member[:aff.n_aff, :words], n_match[:aff.n_aff], n_error[:aff.n_aff]
 
     def exceeds_cluster_capacity_affinity(self, alloc, enc: dict, apps: dict, packer: int, overhead=None, zone_id=None, n_zones=1):
@@ -1196,6 +1249,22 @@ class GangPacker:
         err = np.full(max(q, 1), 255, np.uint8)
         self._check(load().gp_exceeds_cluster_capacity_affinity_resident(self._h, C.byref(nd), _p(oid), C.byref(lab), C.byref(aff),
                                                                          C.byref(a), int(packer), _p(out), _p(err)))
+        return out[:q], err[:q]
+
+    def exceeds_cluster_capacity_affinity_label_table(self, alloc, overhead_node_id, node_id, enc: dict, apps: dict, packer: int,
+                                                      zone_id=None, n_zones=1):
+        """exceeds_cluster_capacity_affinity_resident with the labels read in place from the label table
+        (gp_exceeds_cluster_capacity_affinity_label_table): node_id and enc as in match_node_affinity_resident."""
+        q = len(apps["count"])
+        nd = _capacity_nodes(alloc, None, zone_id, n_zones, None, 0)
+        oid = _np(overhead_node_id, np.int32)
+        rl = _resident_labels(node_id)
+        aff = _programs(enc)
+        a = _apps(apps, None, group=apps.get("group"))
+        out = np.full(max(q, 1), 255, np.uint8)
+        err = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity_affinity_label_table(self._h, C.byref(nd), _p(oid), C.byref(rl), C.byref(aff),
+                                                                            C.byref(a), int(packer), _p(out), _p(err)))
         return out[:q], err[:q]
 
     def reconcile_find_nodes(self, alloc, overhead, res_node, res, node_group, creation, apps: dict, n_groups: int,
@@ -1302,6 +1371,21 @@ class GangPacker:
         col = {k: _np(delta.get(k), t) for k, t in _RT_DELTA_COLS.items()}
         d = gp_reservation_delta(n_write=0 if col["slot"] is None else len(col["slot"]), **{k: _p(v) for k, v in col.items()})
         self._check(load().gp_reservation_table_update(self._h, C.byref(d)))
+
+    # ---- the resident label table (gp_label_table_*) ---------------------------------------------------------------------
+    def label_table_reset(self, n_node_ids, max_labels, n_keys, n_values):
+        """Replace the context's label table with an empty one of these capacities."""
+        z = gp_label_table_size(int(n_node_ids), int(max_labels), int(n_keys), int(n_values))
+        self._check(load().gp_label_table_reset(self._h, C.byref(z)))
+
+    def label_table_update(self, delta: dict):
+        """One gp_label_table_update over the arrays of affinity.LabelTable.delta() (row_node, row_off, label_key, label_val,
+        value_id, value_int_ok, value_int; a missing column is NULL; the "reset" entry is not read here)."""
+        col = {k: _np(delta.get(k), t) for k, t in _LT_DELTA_COLS.items()}
+        n = lambda k: 0 if col[k] is None else len(col[k])
+        d = gp_label_delta(n_rows=int(delta.get("n_rows", n("row_node"))), n_values=int(delta.get("n_values", n("value_id"))),
+                           **{k: _p(v) for k, v in col.items()})
+        self._check(load().gp_label_table_update(self._h, C.byref(d)))
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
