@@ -1201,6 +1201,98 @@ gp_status gp_exceeds_cluster_capacity_affinity_label_table(gp_ctx* ctx, const gp
                                                            const gp_apps* drivers, gp_binpacker packer, uint8_t* exceeds /* [n_apps] */,
                                                            uint8_t* affinity_error /* [n_apps] or NULL */);
 
+/* ---- the resident node table --------------------------------------------------------------------------------------------
+ * Every node's allocatable, Spec.Unschedulable, NodeReady condition and name order kept on the device and changed only by
+ * deltas from node events, so a Predicate no longer uploads those columns, nor sorts the node names on the host.  One row per
+ * node id; node ids are the label table's (one node informer interns both).  A row holds: present, alloc cpu / mem / gpu,
+ * unschedulable, ready, name_key, and name_rank -- the dense rank of name_key among the present rows, recomputed on the
+ * device by every update.  name_key is an order key the caller keeps: strictly increasing in the byte order of the node
+ * names, unique among present rows, below 2^63 - 1, and not necessarily dense (INTEGRATION.md: a new name takes the midpoint
+ * of its neighbours' keys; when no gap is left every node is relabelled in one delta).  A rank over the whole table orders
+ * any subset of it as the names do.  The table belongs to the context (freed by gp_destroy); updates change no snapshot,
+ * layout, schedulable resources, held orders or statistics. */
+typedef struct {
+    int32_t n_node_ids;              /* rows */
+    int32_t reserved;
+} gp_node_table_size;
+/* Replace the context's node table with an empty one (no row present).  GP_ERR_INVALID: NULL size or a negative capacity
+ * (the table held before is kept).  After a CUDA error the context holds no table. */
+gp_status gp_node_table_reset(gp_ctx* ctx, const gp_node_table_size* size);
+
+typedef struct {
+    int32_t n_write;                 /* whole-row writes */
+    int32_t reserved;
+    const int32_t* node_id;          /* [n_write] distinct node ids < n_node_ids */
+    const uint8_t* present;          /* [n_write] 0: the node is deleted (the row's other columns are ignored) */
+    const int64_t* alloc_cpu_milli;  /* [n_write] |v| < 2^61 on present rows */
+    const int64_t* alloc_mem_bytes;
+    const int64_t* alloc_gpu;        /* or NULL (= 0) */
+    const uint8_t* unschedulable;    /* [n_write] node.Spec.Unschedulable */
+    const uint8_t* ready;            /* [n_write] NodeReady == True */
+    const int64_t* name_key;         /* [n_write] the name's order key (see above) */
+} gp_node_delta;
+/* Apply one delta, then recompute name_rank.  The whole delta is checked on the device before anything is written: a refused
+ * delta leaves the table exactly as it was.  One stream synchronise.  GP_ERR_INVALID: no table (gp_node_table_reset first),
+ * missing arrays or a negative count; a node id out of range or given twice; two rows present after the delta with the same
+ * name_key, or a present row's name_key = 2^63 - 1.  GP_ERR_UNREPRESENTABLE: |alloc| >= 2^61 on a present row.  A refusal,
+ * or a CUDA error while the delta is staged, leaves the table as it was; a CUDA error once the update writes the table
+ * leaves no table (GP_ERR_INVALID "no node table" until the next reset), and the caller resets and replays. */
+gp_status gp_node_table_update(gp_ctx* ctx, const gp_node_delta* delta);
+
+/* The node list of a node-table Predicate entry.  Per listed node i: its node-table id, its reservation-table id and its
+ * overhead-table id -- the only per-node uploads, with is_driver_candidate when given.  Per call: how the zone, the instance
+ * group and the two label priority ranks are read from the label table's row node_table_id[i] (the reference's rules):
+ *   zone            label zone_key (failure-domain.beta.kubernetes.io/zone); the dense zone is the index of its value id in
+ *                   zone_value [n_zones]; a node without the label is in zone zone_missing (the "default" placeholder's
+ *                   dense id), or is refused when zone_missing = -1; a value not listed is refused.  zone_key = -1: one
+ *                   zone (zone_id NULL of gp_sort_input).
+ *   instance group  label instance_group_key; the index of its value id in instance_group_value [n_instance_groups of the
+ *                   entry]; a node without the label or with a value not listed is in no instance group (-1).  Ignored when
+ *                   the entry is given an instance_group array; key -1 without one: every node in instance group 0.
+ *   label ranks     label driver_rank_key / executor_rank_key; the rank is the index of the value id in the list
+ *                   (DescendingPriorityValues order, the last index of a repeated value); -1 without the label or for a
+ *                   value not listed (extractRank's false).  Key -1: not configured (the gp_sort_input column NULL). */
+typedef struct {
+    int32_t n_nodes;
+    int32_t reserved;
+    const int32_t* node_table_id;        /* [n_nodes] distinct, each a present row */
+    const int32_t* reservation_id;       /* [n_nodes] as gp_resident_usage.node_id */
+    const int32_t* overhead_node_id;     /* [n_nodes] as gp_resident_usage.overhead_node_id; required */
+    const uint8_t* is_driver_candidate;  /* [n_nodes] member of ExtenderArgs.NodeNames, or NULL (= all) */
+    int32_t zone_key;
+    int32_t n_zones;                     /* >= 1 */
+    const int32_t* zone_value;           /* [n_zones] distinct value ids, or NULL with zone_key = -1 */
+    int32_t zone_missing;                /* in [-1, n_zones) */
+    int32_t instance_group_key;
+    const int32_t* instance_group_value; /* [n_instance_groups] distinct value ids, or NULL with instance_group_key = -1 */
+    int32_t driver_rank_key;
+    int32_t n_driver_rank_values;
+    const int32_t* driver_rank_value;
+    int32_t executor_rank_key;
+    int32_t n_executor_rank_values;
+    const int32_t* executor_rank_value;
+    int32_t* undefined_ties;             /* out, or NULL: as gp_sort_input.undefined_ties */
+    int32_t* zone_id_out;                /* out [n_nodes], or NULL: the dense zone of each node (0 with zone_key = -1) */
+    int32_t* instance_group_out;         /* out [n_nodes], or NULL: the instance group of each node */
+} gp_node_table_nodes;
+/* The node-table forms of the three *_resident Predicate entries: a gp_node_table_nodes in place of both the
+ * gp_resident_usage and the gp_sort_input.  One kernel gathers, on the device, exactly the columns the *_resident entry would
+ * upload (allocatable, name_rank, unschedulable and ready from the node table; zone, instance group and label ranks from the
+ * label table), and the *_resident entry's stages then run unchanged.  So each returns what its *_resident entry returns --
+ * outputs bit for bit, status, and the context afterwards -- given node_id = reservation_id, overhead from the overhead
+ * table, and the columns above.  The node and label tables are read in place and left as they were.
+ * Checks, in order (a refused call replaces nothing): GP_ERR_INVALID for no node table, no label table, missing arrays
+ * (overhead_node_id included) or bad sizes, a zone_missing out of range, a value listed twice in zone_value or
+ * instance_group_value; then the *_resident entry's host checks; then, read in the one synchronise the entry makes before it
+ * writes the context, GP_ERR_INVALID for a node-table id out of range, absent or given twice, and for a zone label whose
+ * value is not in zone_value (or a node without it when zone_missing = -1); then the *_resident entry's device refusals. */
+gp_status gp_prepare_cluster_groups_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, const int32_t* instance_group,
+                                               int32_t n_instance_groups, gp_instance_group_orders* out);
+gp_status gp_prepare_cluster_zones_groups_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, const int32_t* instance_group,
+                                                     int32_t n_instance_groups, gp_instance_group_layout* layout);
+gp_status gp_reschedule_from_reservations_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, const gp_reschedule_scope* scope,
+                                                     const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

@@ -1,9 +1,10 @@
 // gangpack_cluster.cu -- the entry points driven by the reservations: node priority orders (gp_potential_nodes),
 // availability (gp_build_*availability), the prepared snapshots (gp_prepare_cluster[_groups], gp_prepare_cluster_zones[_groups]), executor
 // reschedule (gp_reschedule_executors, gp_reschedule_from_reservations) and the failover reconciler (gp_reconcile_find_nodes),
-// with the input checks and device staging they share; and the *_resident forms of gp_prepare_cluster_groups,
+// with the input checks and device staging they share; the *_resident forms of gp_prepare_cluster_groups,
 // gp_prepare_cluster_zones_groups, gp_reschedule_from_reservations and gp_reconcile_find_nodes, which take the reservations
-// from the resident table.
+// from the resident table; and the *_node_table forms of the first three, which take the node columns from the resident node
+// and label tables as well.
 #include "gangpack_ctx.cuh"
 #include "gangpack_sort.cuh"
 #include "gangpack_zonelayout.cuh"
@@ -48,12 +49,19 @@ static const Refusal kFeRefusals[] = {
 
 // Where an availability stage takes its usage from: the per-call rows of a gp_usage_input, or the resident reservation table
 // through a gp_resident_usage (the *_resident entries).  Everything else of the stage is the same for both.
+// The *_node_table entries pass a gp_resident_usage and a gp_sort_input whose node columns were gathered on the device
+// (nt_gather): gather_err, the gather's status word, marks them.
 struct UsageIn {
     const gp_usage_input* rows = nullptr;
     const gp_resident_usage* res = nullptr;
+    const int* gather_err = nullptr;
     UsageIn(const gp_usage_input* u) : rows(u) {}
-    UsageIn(const gp_resident_usage* r) : res(r) {}
+    UsageIn(const gp_resident_usage* r, const int* gathered = nullptr) : res(r), gather_err(gathered) {}
     bool given() const { return rows || res; }
+    // allocatable and the gp_sort_input columns other than is_driver_candidate are device pointers.  They are not checked on
+    // the host: the gather keeps every index in range and name_rank unique even for a call it refuses, and its status word is
+    // read in the entry's synchronise, before the context is written
+    bool on_device() const { return gather_err != nullptr; }
     int32_t n_nodes() const { return rows ? rows->n_nodes : res ? res->n_nodes : 0; }
     // overhead from the resident overhead table, on the device
     bool table_overhead() const { return res && res->overhead_node_id; }
@@ -169,7 +177,7 @@ static gp_status stage_availability(gp_ctx* c, const UsageIn& in, cudaStream_t s
     const long long* al[3];
     const long long* ov[3];
     for (int d = 0; d < 3; ++d) {
-        al[d] = ar.put(alloc.part(N * d, N), alloc_h[d]);
+        al[d] = in.on_device() ? (const long long*)alloc_h[d] : ar.put(alloc.part(N * d, N), alloc_h[d]);
         ov[d] = tab ? ar.ptr(over.part(N * d, N)) : ar.put(over.part(N * d, N), over_h[d]);
     }
     ar.fill(usage, err, 0);                             // the usage sums, the has-an-entry flags and the status words
@@ -241,9 +249,10 @@ static void launch_label_resort(int32_t n, const int32_t* cnt, const int32_t* li
 // f1 stage: d_cpu / d_mem / d_gpu are device arrays (NULL: uploaded from `in`; gpu optional); leaves the two orders,
 // counts[3] = {#driver candidates, #executor candidates, #undefined ties} and the zone ids (NULL: one zone) on the device.
 // ig (host, [n_nodes] in [-1, n_ig), or NULL): PotentialNodes per instance group, instance-group-major (the instance group
-// is the leading key; nodes in none are dropped).  The caller has run check_sort_ids and checked ig.
+// is the leading key; nodes in none are dropped).  The caller has run check_sort_ids and checked ig.  dev: ig and the columns
+// of `in` other than is_driver_candidate are device pointers (UsageIn::on_device).
 static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const int32_t* ig, int32_t n_ig, const long long* d_cpu, const long long* d_mem,
-                            const long long* d_gpu, cudaStream_t st, SortStage* out) {
+                            const long long* d_gpu, cudaStream_t st, SortStage* out, bool dev = false) {
     const int32_t n = in->n_nodes;
     const bool zoned = in->zone_id != nullptr && in->n_zones > 1;       // one zone: priority 0 for every node, nothing to total
     // one scratch block; the zone totals and priorities are per (instance group, zone) pair
@@ -266,15 +275,15 @@ static gp_status stage_sort(gp_ctx* c, const gp_sort_input* in, const int32_t* i
     if (!d_cpu) d_cpu = ar.put(cpu, in->avail_cpu_milli);
     if (!d_mem) d_mem = ar.put(mem, in->avail_mem_bytes);
     if (!d_gpu) d_gpu = ar.put(gpu, in->avail_gpu);
-    const int32_t* d_zone = zoned ? ar.put(zone, in->zone_id) : nullptr;
-    const int32_t* d_ig = ar.put(igp, ig);
+    const int32_t* d_zone = !zoned ? nullptr : dev ? in->zone_id : ar.put(zone, in->zone_id);
+    const int32_t* d_ig = dev ? ig : ar.put(igp, ig);
     int32_t* d_ties = ig ? ar.zero(ties) : nullptr;
-    const int32_t* d_nr = ar.put(nr, in->name_rank);
+    const int32_t* d_nr = dev ? in->name_rank : ar.put(nr, in->name_rank);
     const uint8_t* d_fc = ar.put(fc, in->is_driver_candidate);
-    const uint8_t* d_fu = ar.put(fu, in->unschedulable);
-    const uint8_t* d_fr = ar.put(fr, in->ready);
-    const int32_t* d_lrd = ar.put(lrd, in->driver_label_rank);
-    const int32_t* d_lre = ar.put(lre, in->executor_label_rank);
+    const uint8_t* d_fu = dev ? in->unschedulable : ar.put(fu, in->unschedulable);
+    const uint8_t* d_fr = dev ? in->ready : ar.put(fr, in->ready);
+    const int32_t* d_lrd = dev ? in->driver_label_rank : ar.put(lrd, in->driver_label_rank);
+    const int32_t* d_lre = dev ? in->executor_label_rank : ar.put(lre, in->executor_label_rank);
     if (zoned) ar.zero(tot);
     GP_TRY(ar.check(c));
     if (!c->sort_attr_set) {
@@ -324,15 +333,17 @@ static gp_status prepare_orders(gp_ctx* c, const UsageIn& usage, const gp_sort_i
     if (!sort || usage.n_nodes() != sort->n_nodes || sort->n_zones < 1)
         return fail(c, GP_ERR_INVALID, who, "missing arrays or mismatched sizes");
     if (usage.n_nodes() == 0) return fail(c, GP_ERR_INVALID, who, "empty node table");
-    GP_TRY(check_sort_ids(c, sort, who));
+    if (!usage.on_device()) GP_TRY(check_sort_ids(c, sort, who));
     GP_CUDA(c, cudaSetDevice(c->device));
     int* d_err = nullptr;
     GP_TRY(stage_availability(c, usage, c->stream, d_avail, d_sched, &d_err));
     const size_t N = (size_t)usage.n_nodes();
-    GP_TRY(stage_sort(c, sort, ig, n_ig, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so));
-    int err[2] = {0, 0};
+    GP_TRY(stage_sort(c, sort, ig, n_ig, *d_avail, *d_avail + N, *d_avail + 2 * N, c->stream, so, usage.on_device()));
+    int err[2] = {0, 0}, gather = 0;
     GP_CUDA(c, cudaMemcpyAsync(err, d_err, sizeof err, cudaMemcpyDeviceToHost, c->stream));
+    if (usage.on_device()) GP_CUDA(c, cudaMemcpyAsync(&gather, usage.gather_err, sizeof gather, cudaMemcpyDeviceToHost, c->stream));
     GP_CUDA(c, cudaStreamSynchronize(c->stream));
+    GP_TRY(nt_refusal(c, gather, who));
     return stage_refusal(c, err, who);
 }
 
@@ -365,7 +376,7 @@ static gp_status check_instance_groups(gp_ctx* c, const UsageIn& usage, const gp
     if (n_ig < 1) return fail(c, GP_ERR_INVALID, who, "n_instance_groups must be >= 1");
     if (sort && n_ig > 1 && (int64_t)n_ig * ((int64_t)sort->n_zones + 1) > kZoneLayoutMaxPairs)
         return fail(c, GP_ERR_INVALID, who, "n_instance_groups x (n_zones + 1) above 2^22");
-    if (ig && usage.given() && sort && usage.n_nodes() == sort->n_nodes)
+    if (ig && usage.given() && !usage.on_device() && sort && usage.n_nodes() == sort->n_nodes)
         for (int32_t i = 0; i < usage.n_nodes(); ++i)
             if (ig[i] < -1 || ig[i] >= n_ig) return fail(c, GP_ERR_INVALID, who, "instance_group outside [-1, n_instance_groups)");
     return GP_OK;
@@ -787,7 +798,7 @@ static gp_status reschedule_from_reservations(gp_ctx* c, const UsageIn& usage, c
                 return fail(c, GP_ERR_INVALID, who, "filterNodesToZone: a node has no topology.kubernetes.io/zone label (topology_zone == -1), "
                                                     "unable to make scheduling decisions based on AZ");
     }
-    GP_TRY(check_sort_ids(c, sort, who));
+    if (!usage.on_device()) GP_TRY(check_sort_ids(c, sort, who));
     const bool mf = in->min_frag != 0;
     const bool has_host = mf && in->host_off;
     GP_TRY(check_requests(c, q, in->exe_cpu_milli, in->exe_mem_bytes, in->exe_gpu, who));
@@ -816,11 +827,12 @@ static gp_status reschedule_from_reservations(gp_ctx* c, const UsageIn& usage, c
     const auto amb = ar.take<uint8_t>(Q);
     ar.reserve();
     RpNodeIn ni{};
-    ni.zone = zoned ? ar.put(zone, sort->zone_id) : nullptr;
-    ni.name_rank = ar.put(nr, sort->name_rank);
-    ni.unschedulable = ar.put(fu, sort->unschedulable);
-    ni.ready = ar.put(fr, sort->ready);
-    ni.label_rank = ar.put(lr, sort->executor_label_rank);
+    const bool dev = usage.on_device();
+    ni.zone = !zoned ? nullptr : dev ? sort->zone_id : ar.put(zone, sort->zone_id);
+    ni.name_rank = dev ? sort->name_rank : ar.put(nr, sort->name_rank);
+    ni.unschedulable = dev ? sort->unschedulable : ar.put(fu, sort->unschedulable);
+    ni.ready = dev ? sort->ready : ar.put(fr, sort->ready);
+    ni.label_rank = dev ? sort->executor_label_rank : ar.put(lr, sort->executor_label_rank);
     ni.tz = keep >= 0 ? ar.put(tz, scope->topology_zone) : nullptr;
     RpDecideIn di{};
     di.exe = ar.put(exe.part(0, Q), in->exe_cpu_milli);
@@ -855,9 +867,11 @@ static gp_status reschedule_from_reservations(gp_ctx* c, const UsageIn& usage, c
     GP_CUDA(c, cudaGetLastError());
     ar.get(node_out, d_out);
     ar.get(ambiguous, amb);
-    int err[2] = {0, 0};
+    int err[2] = {0, 0}, gather = 0;
     ar.get(err, d_err, 2);
+    if (dev) ar.get(&gather, usage.gather_err, 1);
     GP_TRY(ar.sync(c));
+    GP_TRY(nt_refusal(c, gather, who));
     return stage_refusal(c, err, who);                  // refused: node_out / ambiguous hold no decision
 }
 
@@ -1012,6 +1026,44 @@ gp_status gp_reconcile_find_nodes(gp_ctx* c, const gp_usage_input* usage, const 
 gp_status gp_reconcile_find_nodes_resident(gp_ctx* c, const gp_resident_usage* usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
                                            gp_reconcile_results* out) {
     return reconcile_find_nodes(c, usage, nodes, a, out, "gp_reconcile_find_nodes_resident");
+}
+
+}  // extern "C"
+
+// ---- the *_node_table forms: nt_gather fills the columns on the device, then the *_resident entry's own path runs ----
+
+extern "C" {
+
+gp_status gp_prepare_cluster_groups_node_table(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* instance_group,
+                                               int32_t n_instance_groups, gp_instance_group_orders* out) {
+    static const char* who = "gp_prepare_cluster_groups_node_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    NtGathered g{};
+    GP_TRY(nt_gather(c, nodes, instance_group, n_instance_groups, true, who, &g));
+    GP_TRY(check_instance_groups(c, UsageIn(&g.usage), &g.sort, instance_group, n_instance_groups, who));
+    GP_TRY(prepare_cluster_groups(c, UsageIn(&g.usage, g.err), &g.sort, g.ig, n_instance_groups, out, who));
+    return nt_outputs(c, nodes, g);
+}
+
+gp_status gp_prepare_cluster_zones_groups_node_table(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* instance_group,
+                                                     int32_t n_instance_groups, gp_instance_group_layout* layout) {
+    static const char* who = "gp_prepare_cluster_zones_groups_node_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    NtGathered g{};
+    GP_TRY(nt_gather(c, nodes, instance_group, n_instance_groups, true, who, &g));
+    GP_TRY(check_instance_groups(c, UsageIn(&g.usage), &g.sort, instance_group, n_instance_groups, who));
+    GP_TRY(prepare_cluster_zones_groups(c, UsageIn(&g.usage, g.err), &g.sort, g.ig, n_instance_groups, layout, who));
+    return nt_outputs(c, nodes, g);
+}
+
+gp_status gp_reschedule_from_reservations_node_table(gp_ctx* c, const gp_node_table_nodes* nodes, const gp_reschedule_scope* scope,
+                                                     const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous) {
+    static const char* who = "gp_reschedule_from_reservations_node_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    NtGathered g{};
+    GP_TRY(nt_gather(c, nodes, nullptr, 1, false, who, &g));
+    GP_TRY(reschedule_from_reservations(c, UsageIn(&g.usage, g.err), &g.sort, scope, in, node_out, ambiguous, who));
+    return nt_outputs(c, nodes, g);
 }
 
 }  // extern "C"

@@ -239,6 +239,15 @@ struct gp_ctx {
         uint32_t seq = 0;                         // the last update's stamp
     } lt;
 
+    // the resident node table (gangpack_node_table.cu); read by the *_node_table entries, changed only by its own
+    struct NodeTable {
+        bool live = false;                        // reset and not broken by a CUDA error since
+        gp_node_table_size size{};
+        DevBuf cols;                              // present, alloc [3], unschedulable, ready, name_key, name_rank, stamps in one block
+        DevBuf gather;                            // the columns one *_node_table call gathers, and its scratch
+        uint32_t seq = 0;                         // the last update's stamp
+    } nt;
+
     gp_stats last{};
 };
 
@@ -419,3 +428,23 @@ RtCols rt_cols(gp_ctx* c);
 // [n_values]
 struct LtCols { const int32_t* count; const int32_t* key; const int32_t* val; const long long* vint; const uint8_t* vok; };
 LtCols lt_cols(gp_ctx* c);
+
+// ---- gangpack_node_table.cu ------------------------------------------------------------------------------------------
+
+// What a *_node_table entry hands to the *_resident stages: a gp_resident_usage and a gp_sort_input over the listed nodes whose
+// columns (is_driver_candidate and the id arrays excepted) are device pointers into the context's gather buffer, the
+// instance groups (device, or NULL), and the gather's status word, read by the stage's one synchronise (nt_refusal).
+struct NtGathered {
+    gp_resident_usage usage;
+    gp_sort_input sort;
+    const int32_t* ig;
+    const int* err;
+};
+// The host checks of a *_node_table entry, then the gather enqueued on the context's stream.  ig_host (or NULL): the entry's
+// instance_group array, uploaded as is (checked by the *_resident entry); with_ig: read instance groups from the labels.
+gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* ig_host, int32_t n_ig, bool with_ig, const char* who,
+                    NtGathered* out);
+// The gather's refusal, once the stream has been synchronised
+gp_status nt_refusal(gp_ctx* c, int word, const char* who);
+// After the entry's synchronise: the optional zone_id_out / instance_group_out copies
+gp_status nt_outputs(gp_ctx* c, const gp_node_table_nodes* nodes, const NtGathered& g);

@@ -24,6 +24,7 @@
 #include <stdint.h>
 
 #include "gangpack_kernels.cuh"
+#include "gangpack_tilesort.cuh"
 
 namespace gp {
 
@@ -154,10 +155,7 @@ __global__ void gp_make_keys(int32_t n, const long long* __restrict__ cpu, const
     keys[i] = k;
 }
 
-// ---- sort primitive: tiles sorted in shared memory, ranks by binary search across tiles ---------------------------
-constexpr int kSortTile = 4096;
-constexpr int kSortThreads = 1024;
-
+// ---- sort primitive (gangpack_tilesort.cuh): keys of this file ----------------------------------------------------
 struct LabelKey {          // stable re-sort by label rank: (rank, position in the list) is unique
     uint32_t rank;
     int32_t pos;
@@ -176,55 +174,6 @@ __device__ __forceinline__ bool key_less(const SegLabelKey& a, const SegLabelKey
 __device__ __forceinline__ SortKey key_max(const SortKey*) { SortKey k; k.mem = 0x7fffffffffffffffLL; k.cpu = 0x7fffffffffffffffLL; k.az = 0x7fffffff; k.name_rank = 0x7fffffff; return k; }
 __device__ __forceinline__ LabelKey key_max(const LabelKey*) { LabelKey k; k.rank = 0xffffffffu; k.pos = 0x7fffffff; return k; }
 __device__ __forceinline__ SegLabelKey key_max(const SegLabelKey*) { SegLabelKey k; k.seg = 0xffffffffu; k.rank = 0xffffffffu; k.pos = 0x7fffffff; return k; }
-
-// (1) sorted[tile] = the tile's keys in ascending order.  count_ptr: the number of keys lives on the device (candidate
-// lists) or is `n` when NULL.  Dynamic shared memory: kSortTile * sizeof(K).
-template <class K>
-__global__ void __launch_bounds__(kSortThreads) gp_sort_tiles(int32_t n, const int32_t* __restrict__ count_ptr, const K* __restrict__ keys,
-                                                              K* __restrict__ sorted) {
-    extern __shared__ __align__(16) unsigned char sort_smem[];
-    K* t = reinterpret_cast<K*>(sort_smem);
-    if (count_ptr) n = *count_ptr;
-    const int32_t base = blockIdx.x * kSortTile;
-    if (base >= n) return;
-    const int32_t m = min(kSortTile, n - base);
-    for (int32_t i = threadIdx.x; i < kSortTile; i += blockDim.x) t[i] = i < m ? keys[base + i] : key_max((const K*)nullptr);
-    __syncthreads();
-    for (int32_t size = 2; size <= kSortTile; size <<= 1) {
-        for (int32_t stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int32_t p = threadIdx.x; p < kSortTile / 2; p += blockDim.x) {
-                const int32_t lo = 2 * p - (p & (stride - 1));          // index with bit `stride` clear
-                const int32_t hi = lo + stride;
-                const bool up = (lo & size) == 0;
-                const K a = t[lo], b = t[hi];
-                if (key_less(b, a) == up) { t[lo] = b; t[hi] = a; }
-            }
-            __syncthreads();
-        }
-    }
-    for (int32_t i = threadIdx.x; i < m; i += blockDim.x) sorted[base + i] = t[i];
-}
-
-// (2) pos[i] = #{ j : key_j < key_i } = sum over tiles of lower_bound(tile, key_i)
-template <class K>
-__global__ void __launch_bounds__(256) gp_rank_by_search(int32_t n, const int32_t* __restrict__ count_ptr, const K* __restrict__ keys,
-                                                         const K* __restrict__ sorted, int32_t* __restrict__ pos) {
-    if (count_ptr) n = *count_ptr;
-    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const K me = keys[i];
-    int32_t cnt = 0;
-    for (int32_t base = 0; base < n; base += kSortTile) {
-        const K* t = sorted + base;
-        int32_t lo = 0, hi = min(kSortTile, n - base);              // first index whose key is not < me
-        while (lo < hi) {
-            const int32_t mid = (lo + hi) >> 1;
-            if (key_less(t[mid], me)) lo = mid + 1; else hi = mid;
-        }
-        cnt += lo;
-    }
-    pos[i] = cnt;
-}
 
 __global__ void gp_scatter_order(int32_t n, const int32_t* __restrict__ pos, int32_t* __restrict__ order) {
     int32_t i = blockIdx.x * blockDim.x + threadIdx.x;

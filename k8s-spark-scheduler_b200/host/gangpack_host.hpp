@@ -936,6 +936,10 @@ public:
         return e;
     }
 
+    // the id of a label key / value string; 0, the reserved id no row holds, for a string no node carries
+    int32_t KeyID(const std::string& k) const { auto it = keyId_.find(k); return it == keyId_.end() ? 0 : it->second; }
+    int32_t ValueID(const std::string& v) const { auto it = valId_.find(v); return it == valId_.end() ? 0 : it->second; }
+
     // the next Flush resets the table and sends the whole state again (after a refused resident call)
     void Replay() { replay_ = true; }
 
@@ -1033,6 +1037,251 @@ inline MatchResult MatchRequiredNodeAffinity(const std::vector<std::string>& nod
 }
 
 }  // namespace affinity
+
+namespace resources {
+
+// Every node's allocatable, Spec.Unschedulable, NodeReady condition and name order as the resident node table
+// (gp_node_table_*) keeps them, from the node informer: SetNode for AddFunc and UpdateFunc, after the label table's SetNode,
+// which gives the node its id (no write when nothing changed); DeleteNode for DeleteFunc, before the label table's
+// DeleteNode, which frees the id.  name_key is kept here: strictly increasing in the byte order of the names, in
+// [0, 2^keyBits); a new name takes the midpoint of its neighbours' keys (-1 before the first, 2^keyBits after the last), and
+// when no gap is left every present node gets an evenly spaced key and the next delta carries every row.  Flush sends the
+// rows that differ from what the device holds as one gp_node_table_update, after a reset with a doubled capacity and the
+// whole state when a node id would not fit (or after Replay, or a failed flush).
+class ResidentNodes {
+public:
+    explicit ResidentNodes(const affinity::ResidentLabels& labels, int32_t nNodeIds = 64, int keyBits = 62)
+        : labels_(labels), size_{nNodeIds, 0}, keyHi_((int64_t)1 << keyBits) {}
+
+    void SetNode(const std::string& name, const Resources& allocatable, bool unschedulable, bool ready) {
+        const int32_t at = labels_.NodeIDs({name})[0];
+        if (at < 0) throw gangpack::Error(GP_ERR_INVALID, "ResidentNodes::SetNode: the label table does not know " + name + " (its SetNode first)");
+        auto held = nameAt_.find(at);
+        if (held != nameAt_.end() && held->second != name)
+            throw gangpack::Error(GP_ERR_INVALID, "ResidentNodes::SetNode: node id held by " + held->second + " (DeleteNode it first)");
+        auto cur = nodes_.find(name);
+        if (cur != nodes_.end() && cur->second.id != at)
+            throw gangpack::Error(GP_ERR_INVALID, "ResidentNodes::SetNode: " + name + " is held under another id (DeleteNode it before the label table's)");
+        const Row row{true, {allocatable.CPU, allocatable.Memory, allocatable.NvidiaGPU}, unschedulable, ready, 0};
+        if (cur != nodes_.end()) {
+            Row next = row;
+            next.key = cur->second.row.key;
+            if (next == cur->second.row) return;
+            cur->second.row = next;
+        } else {
+            const int64_t key = insert(name);
+            Row r = row;
+            r.key = key;
+            nodes_[name] = Held{at, r};
+            nameAt_[at] = name;
+        }
+        dirty_.insert(at);
+    }
+    void DeleteNode(const std::string& name) {
+        auto it = nodes_.find(name);
+        if (it == nodes_.end()) return;
+        dirty_.insert(it->second.id);
+        nameAt_.erase(it->second.id);
+        byName_.erase(name);
+        nodes_.erase(it);
+    }
+
+    // the table's id of each node name, -1 for a node it does not hold
+    std::vector<int32_t> NodeIDs(const std::vector<std::string>& names) const {
+        std::vector<int32_t> ids(names.size(), -1);
+        for (size_t i = 0; i < names.size(); ++i) {
+            auto it = nodes_.find(names[i]);
+            if (it != nodes_.end()) ids[i] = it->second.id;
+        }
+        return ids;
+    }
+    int64_t NameKey(const std::string& name) const { return nodes_.at(name).row.key; }
+    int Relabels() const { return relabels_; }
+
+    // the per-call columns the node-table entries stand for: allocatable, name_rank (the byte order of the listed names, a
+    // permutation of 0..n-1), unschedulable and ready
+    struct Columns {
+        std::vector<int64_t> alloc[3];
+        std::vector<int32_t> nameRank;
+        std::vector<uint8_t> unschedulable, ready;
+    };
+    Columns PerCall(const std::vector<std::string>& names) const {
+        Columns c;
+        std::vector<size_t> order(names.size());
+        for (size_t i = 0; i < names.size(); ++i) order[i] = i;
+        std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return names[a] < names[b]; });
+        c.nameRank.resize(names.size());
+        for (size_t r = 0; r < order.size(); ++r) c.nameRank[order[r]] = (int32_t)r;
+        for (const auto& nm : names) {
+            const Row& r = nodes_.at(nm).row;
+            for (int d = 0; d < 3; ++d) c.alloc[d].push_back(r.alloc[d]);
+            c.unschedulable.push_back(r.unschedulable);
+            c.ready.push_back(r.ready);
+        }
+        return c;
+    }
+
+    void Replay() { replay_ = true; }
+
+    void Flush(gangpack::Device& dev) {
+        const int32_t need = nameAt_.empty() ? 0 : nameAt_.rbegin()->first + 1;
+        while (size_.n_node_ids < need) { size_.n_node_ids = std::max<int32_t>(2 * size_.n_node_ids, 1); replay_ = true; }
+        std::vector<int32_t> id;
+        std::vector<uint8_t> present, uns, rdy;
+        std::vector<int64_t> v[3], key;
+        auto row = [&](int32_t at) {
+            const Row r = record(at);
+            id.push_back(at); present.push_back(r.present); uns.push_back(r.unschedulable); rdy.push_back(r.ready);
+            for (int d = 0; d < 3; ++d) v[d].push_back(r.alloc[d]);
+            key.push_back(r.key);
+        };
+        if (replay_) {
+            sent_.clear();
+            for (const auto& kv : nameAt_) row(kv.first);
+        } else {
+            for (int32_t at : dirty_) {
+                auto s = sent_.find(at);
+                if (!(record(at) == (s == sent_.end() ? Row{} : s->second))) row(at);
+            }
+        }
+        const bool reset = replay_;
+        replay_ = true;                            // until the table holds this state: a failed call replays next time
+        if (reset) dev.check(gp_node_table_reset(dev.ctx(), &size_), "gp_node_table_reset");
+        if (!id.empty()) {
+            gp_node_delta d{(int32_t)id.size(), 0, id.data(), present.data(), v[0].data(), v[1].data(), v[2].data(), uns.data(),
+                            rdy.data(), key.data()};
+            dev.check(gp_node_table_update(dev.ctx(), &d), "gp_node_table_update");
+        }
+        for (int32_t at : id) sent_[at] = record(at);
+        replay_ = false;
+        dirty_.clear();
+    }
+
+private:
+    struct Row {
+        bool present = false;
+        int64_t alloc[3] = {0, 0, 0};
+        bool unschedulable = false, ready = false;
+        int64_t key = 0;
+        bool operator==(const Row& o) const {
+            return present == o.present && alloc[0] == o.alloc[0] && alloc[1] == o.alloc[1] && alloc[2] == o.alloc[2] &&
+                   unschedulable == o.unschedulable && ready == o.ready && key == o.key;
+        }
+    };
+    struct Held { int32_t id; Row row; };
+
+    Row record(int32_t at) const {
+        auto n = nameAt_.find(at);
+        return n == nameAt_.end() ? Row{} : nodes_.at(n->second).row;
+    }
+    // name_key of a new name (byName_ holds the present names in byte order, std::string's operator<)
+    int64_t insert(const std::string& name) {
+        auto next = byName_.lower_bound(name);
+        const int64_t lo = next == byName_.begin() ? -1 : nodes_.at(*std::prev(next)).row.key;
+        const int64_t hi = next == byName_.end() ? keyHi_ : nodes_.at(*next).row.key;
+        if (hi - lo >= 2) { byName_.insert(name); return lo + (hi - lo) / 2; }
+        const int64_t n = (int64_t)byName_.size() + 1, step = keyHi_ / (n + 1);
+        if (step < 1) throw gangpack::Error(GP_ERR_CAPACITY, "ResidentNodes: more nodes than name keys");
+        byName_.insert(name);
+        int64_t j = 0, mine = 0;
+        for (const auto& nm : byName_) {                // relabel: the next delta carries every row
+            const int64_t k = step * ++j;
+            if (nm == name) { mine = k; continue; }
+            Held& h = nodes_.at(nm);
+            h.row.key = k;
+            dirty_.insert(h.id);
+        }
+        ++relabels_;
+        return mine;
+    }
+
+    const affinity::ResidentLabels& labels_;
+    gp_node_table_size size_;
+    int64_t keyHi_;
+    bool replay_ = true;
+    int relabels_ = 0;
+    std::unordered_map<std::string, Held> nodes_;
+    std::map<int32_t, std::string> nameAt_;
+    std::set<std::string> byName_;
+    std::set<int32_t> dirty_;
+    std::map<int32_t, Row> sent_;                 // node id -> the row the device holds
+};
+
+// The label part of a gp_node_table_nodes from the configuration's strings, against a ResidentLabels' ids: the zone label
+// (failure-domain.beta.kubernetes.io/zone) with the dense zones in order and "default" appended when not listed (a node
+// without the label is there, resources.go:78-81), instance-group-label with the instance groups in order, and the two
+// LabelPriorityOrder's (or none).  A string no node carries gets a value id no row holds.  Decode restates the same rules on
+// the label strings, for the *_resident form of the call.
+struct NodeTableLabels {
+    static constexpr const char* kZoneLabel = "failure-domain.beta.kubernetes.io/zone";
+
+    NodeTableLabels(const affinity::ResidentLabels& labels, std::vector<std::string> zones, std::string instanceGroupLabel,
+                    std::vector<std::string> instanceGroups, const sort::LabelPriorityOrder* driver = nullptr,
+                    const sort::LabelPriorityOrder* executor = nullptr)
+        : zones_(std::move(zones)), igLabel_(std::move(instanceGroupLabel)), groups_(std::move(instanceGroups)) {
+        if (std::find(zones_.begin(), zones_.end(), "default") == zones_.end()) zones_.push_back("default");
+        int32_t unknown = -1;
+        auto ids = [&](const std::vector<std::string>& v) {
+            std::vector<int32_t> out;
+            for (const auto& s : v) { const int32_t x = labels.ValueID(s); out.push_back(x ? x : unknown--); }
+            return out;
+        };
+        zoneKey_ = labels.KeyID(kZoneLabel);
+        zoneValue_ = ids(zones_);
+        igKey_ = labels.KeyID(igLabel_);
+        igValue_ = ids(groups_);
+        const sort::LabelPriorityOrder* pr[2] = {driver, executor};
+        for (int k = 0; k < 2; ++k)
+            if (pr[k]) { prio_[k] = *pr[k]; rankKey_[k] = labels.KeyID(pr[k]->Name); rankValue_[k] = ids(pr[k]->DescendingPriorityValues); }
+    }
+
+    void Fill(gp_node_table_nodes* n) const {
+        n->zone_key = zoneKey_; n->n_zones = (int32_t)zones_.size(); n->zone_value = zoneValue_.data();
+        n->zone_missing = (int32_t)(std::find(zones_.begin(), zones_.end(), "default") - zones_.begin());
+        n->instance_group_key = igKey_; n->instance_group_value = igValue_.data();
+        n->driver_rank_key = rankKey_[0]; n->n_driver_rank_values = (int32_t)rankValue_[0].size(); n->driver_rank_value = rankValue_[0].data();
+        n->executor_rank_key = rankKey_[1]; n->n_executor_rank_values = (int32_t)rankValue_[1].size();
+        n->executor_rank_value = rankValue_[1].data();
+    }
+    int32_t NumInstanceGroups() const { return (int32_t)groups_.size(); }
+    int32_t NumZones() const { return (int32_t)zones_.size(); }
+
+    // the per-call columns from the strings: zone (every value is listed: unknown zones are refused, false), instance group
+    // (-1: none), and the label ranks (-1: extractRank's false; empty: not configured)
+    struct Columns { std::vector<int32_t> zone, instanceGroup, driverRank, executorRank; };
+    bool Decode(const std::vector<affinity::Node>& nodes, Columns* c) const {
+        auto index = [](const std::vector<std::string>& v, const std::string& s, bool last) {
+            int32_t at = -1;
+            for (size_t i = 0; i < v.size(); ++i) if (v[i] == s) { at = (int32_t)i; if (!last) break; }
+            return at;
+        };
+        for (const auto& nd : nodes) {
+            auto z = nd.Labels.find(kZoneLabel);
+            const int32_t zone = index(zones_, z == nd.Labels.end() ? "default" : z->second, false);
+            if (zone < 0) return false;
+            c->zone.push_back(zone);
+            auto g = nd.Labels.find(igLabel_);
+            c->instanceGroup.push_back(g == nd.Labels.end() ? -1 : index(groups_, g->second, false));
+            std::vector<int32_t>* rank[2] = {&c->driverRank, &c->executorRank};
+            for (int k = 0; k < 2; ++k) {
+                if (rankKey_[k] < 0) continue;
+                auto l = nd.Labels.find(prio_[k].Name);
+                rank[k]->push_back(l == nd.Labels.end() ? -1 : index(prio_[k].DescendingPriorityValues, l->second, true));
+            }
+        }
+        return true;
+    }
+
+private:
+    std::vector<std::string> zones_;
+    std::string igLabel_;
+    std::vector<std::string> groups_;
+    sort::LabelPriorityOrder prio_[2];
+    int32_t zoneKey_ = -1, igKey_ = -1, rankKey_[2] = {-1, -1};
+    std::vector<int32_t> zoneValue_, igValue_, rankValue_[2];
+};
+
+}  // namespace resources
 
 namespace extender {
 

@@ -43,6 +43,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_reconcile_find_nodes_resident", "gp_exceeds_cluster_capacity_resident",
            "gp_exceeds_cluster_capacity_affinity_resident", "gp_label_table_reset", "gp_label_table_update",
            "gp_match_node_affinity_resident", "gp_exceeds_cluster_capacity_affinity_label_table",
+           "gp_node_table_reset", "gp_node_table_update", "gp_prepare_cluster_groups_node_table",
+           "gp_prepare_cluster_zones_groups_node_table", "gp_reschedule_from_reservations_node_table",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -287,6 +289,26 @@ class gp_resident_labels(C.Structure):
     _fields_ = [("n_nodes", C.c_int32), ("reserved", C.c_int32), ("node_id", C.c_void_p)]
 
 
+class gp_node_table_size(C.Structure):
+    _fields_ = [("n_node_ids", C.c_int32), ("reserved", C.c_int32)]
+
+
+class gp_node_delta(C.Structure):
+    _fields_ = [("n_write", C.c_int32), ("reserved", C.c_int32), ("node_id", C.c_void_p), ("present", C.c_void_p),
+                ("alloc_cpu_milli", C.c_void_p), ("alloc_mem_bytes", C.c_void_p), ("alloc_gpu", C.c_void_p),
+                ("unschedulable", C.c_void_p), ("ready", C.c_void_p), ("name_key", C.c_void_p)]
+
+
+class gp_node_table_nodes(C.Structure):
+    _fields_ = [("n_nodes", C.c_int32), ("reserved", C.c_int32), ("node_table_id", C.c_void_p), ("reservation_id", C.c_void_p),
+                ("overhead_node_id", C.c_void_p), ("is_driver_candidate", C.c_void_p), ("zone_key", C.c_int32), ("n_zones", C.c_int32),
+                ("zone_value", C.c_void_p), ("zone_missing", C.c_int32), ("instance_group_key", C.c_int32),
+                ("instance_group_value", C.c_void_p), ("driver_rank_key", C.c_int32), ("n_driver_rank_values", C.c_int32),
+                ("driver_rank_value", C.c_void_p), ("executor_rank_key", C.c_int32), ("n_executor_rank_values", C.c_int32),
+                ("executor_rank_value", C.c_void_p), ("undefined_ties", C.c_void_p), ("zone_id_out", C.c_void_p),
+                ("instance_group_out", C.c_void_p)]
+
+
 class gp_placement_record(C.Structure):
     _fields_ = [("collocation", C.c_int32), ("distinct_exec_nodes", C.c_int32), ("execs_per_node", C.c_int32), ("n_zones", C.c_int32),
                 ("cross_zone_pairs", C.c_int64), ("total_pairs", C.c_int64)]
@@ -424,6 +446,19 @@ def load():
     L.gp_reschedule_from_reservations_resident.argtypes = [C.c_void_p, C.POINTER(gp_resident_usage), C.POINTER(gp_sort_input),
                                                            C.POINTER(gp_reschedule_scope), C.POINTER(gp_reschedule), C.c_void_p,
                                                            C.c_void_p]
+    L.gp_node_table_reset.restype = C.c_int
+    L.gp_node_table_reset.argtypes = [C.c_void_p, C.POINTER(gp_node_table_size)]
+    L.gp_node_table_update.restype = C.c_int
+    L.gp_node_table_update.argtypes = [C.c_void_p, C.POINTER(gp_node_delta)]
+    L.gp_prepare_cluster_groups_node_table.restype = C.c_int
+    L.gp_prepare_cluster_groups_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.c_void_p, C.c_int32,
+                                                       C.POINTER(gp_instance_group_orders)]
+    L.gp_prepare_cluster_zones_groups_node_table.restype = C.c_int
+    L.gp_prepare_cluster_zones_groups_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.c_void_p, C.c_int32,
+                                                             C.POINTER(gp_instance_group_layout)]
+    L.gp_reschedule_from_reservations_node_table.restype = C.c_int
+    L.gp_reschedule_from_reservations_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.POINTER(gp_reschedule_scope),
+                                                             C.POINTER(gp_reschedule), C.c_void_p, C.c_void_p]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -526,6 +561,36 @@ def _resident_labels(node_id):
     return rl
 
 
+def _node_table_nodes(node_table_id, reservation_id, overhead_node_id, is_driver_candidate=None, zone_key=-1, zone_value=None,
+                      n_zones=1, zone_missing=-1, instance_group_key=-1, instance_group_value=None, driver_rank_key=-1,
+                      driver_rank_value=None, executor_rank_key=-1, executor_rank_value=None, zone_id_out=None,
+                      instance_group_out=None):
+    """gp_node_table_nodes (zone_id_out / instance_group_out: int32 arrays the call fills, or None).  The struct keeps its
+    arrays alive."""
+    tid, rid, oid = _np(node_table_id, np.int32), _np(reservation_id, np.int32), _np(overhead_node_id, np.int32)
+    cand = _np(is_driver_candidate, np.uint8)
+    zv, igv = _np(zone_value, np.int32), _np(instance_group_value, np.int32)
+    drv, exe = _np(driver_rank_value, np.int32), _np(executor_rank_value, np.int32)
+    nt = gp_node_table_nodes(n_nodes=len(tid), node_table_id=_p(tid), reservation_id=_p(rid), overhead_node_id=_p(oid),
+                             is_driver_candidate=_p(cand), zone_key=int(zone_key), n_zones=int(n_zones), zone_value=_p(zv),
+                             zone_missing=int(zone_missing), instance_group_key=int(instance_group_key), instance_group_value=_p(igv),
+                             driver_rank_key=int(driver_rank_key), n_driver_rank_values=0 if drv is None else len(drv),
+                             driver_rank_value=_p(drv), executor_rank_key=int(executor_rank_key),
+                             n_executor_rank_values=0 if exe is None else len(exe), executor_rank_value=_p(exe),
+                             zone_id_out=_p(zone_id_out), instance_group_out=_p(instance_group_out))
+    nt._keep = (tid, rid, oid, cand, zv, igv, drv, exe, zone_id_out, instance_group_out)
+    return nt
+
+
+def _node_table_entry(entry):
+    """The call of a *_node_table entry in the place of its *_resident entry's: the helpers pass (handle, gp_node_table_nodes,
+    gp_sort_input, rest...), and the gp_sort_input only lends its undefined_ties."""
+    def fn(h, nt_ref, si_ref, *rest):
+        nt_ref._obj.undefined_ties = si_ref._obj.undefined_ties
+        return entry(h, nt_ref, *rest)
+    return fn
+
+
 def _capacity_nodes(alloc, overhead, zone_id, n_zones, node_group, n_groups):
     """gp_capacity_nodes over (cpu, mem[, gpu]) triples; overhead may be None.  The struct keeps its arrays alive."""
     al = [_np(v, np.int64) for v in alloc]
@@ -608,6 +673,10 @@ _DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "req_cpu_milli": np.int64,
 # gp_label_delta's columns (affinity.LabelTable.delta() keys)
 _LT_DELTA_COLS = {"row_node": np.int32, "row_off": np.int64, "label_key": np.int32, "label_val": np.int32, "value_id": np.int32,
                   "value_int_ok": np.uint8, "value_int": np.int64}
+
+# gp_node_delta's columns (nodes.NodeTable.delta() keys)
+_NT_DELTA_COLS = {"node_id": np.int32, "present": np.uint8, "alloc_cpu_milli": np.int64, "alloc_mem_bytes": np.int64,
+                  "alloc_gpu": np.int64, "unschedulable": np.uint8, "ready": np.uint8, "name_key": np.int64}
 
 # gp_reservation_delta's columns (reservations.ReservationTable.delta() keys)
 _RT_DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "cpu_milli": np.int64, "mem_bytes": np.int64, "gpu": np.int64}
@@ -1386,6 +1455,44 @@ class GangPacker:
         d = gp_label_delta(n_rows=int(delta.get("n_rows", n("row_node"))), n_values=int(delta.get("n_values", n("value_id"))),
                            **{k: _p(v) for k, v in col.items()})
         self._check(load().gp_label_table_update(self._h, C.byref(d)))
+
+    # ---- the resident node table (gp_node_table_*) and the node-table Predicate entries ----------------------------------
+    def node_table_reset(self, n_node_ids):
+        """Replace the context's node table with an empty one of this capacity."""
+        self._check(load().gp_node_table_reset(self._h, C.byref(gp_node_table_size(int(n_node_ids), 0))))
+
+    def node_table_update(self, delta: dict):
+        """One gp_node_table_update over the arrays of nodes.NodeTable.delta() (node_id, present, alloc_cpu_milli,
+        alloc_mem_bytes, alloc_gpu, unschedulable, ready, name_key; a missing column is NULL; "reset" is not read here)."""
+        col = {k: _np(delta.get(k), t) for k, t in _NT_DELTA_COLS.items()}
+        d = gp_node_delta(n_write=0 if col["node_id"] is None else len(col["node_id"]), **{k: _p(v) for k, v in col.items()})
+        self._check(load().gp_node_table_update(self._h, C.byref(d)))
+
+    def prepare_cluster_groups_node_table(self, nodes: dict, instance_group, n_instance_groups, orders=True):
+        """prepare_cluster_groups_resident with the node columns from the node and label tables: nodes holds the keyword
+        arguments of the gp_node_table_nodes (node_table_id, reservation_id, overhead_node_id, is_driver_candidate, zone_key,
+        zone_value, n_zones, zone_missing, instance_group_key, instance_group_value, driver_rank_key, driver_rank_value,
+        executor_rank_key, executor_rank_value, zone_id_out, instance_group_out).  instance_group: an array, or None to take
+        the instance groups from the labels (or every node in 0 without instance_group_key).  Returns what
+        prepare_cluster_groups_resident returns on the equivalent columns."""
+        nt = _node_table_nodes(**nodes)
+        return self._prepare_groups(_node_table_entry(load().gp_prepare_cluster_groups_node_table), nt, instance_group,
+                                    n_instance_groups, None, int(nt.n_zones), None, None, None, None, None, None, orders)
+
+    def prepare_cluster_zones_groups_node_table(self, nodes: dict, instance_group, n_instance_groups, kind=LAYOUT_AZ_AWARE, layout=True):
+        """prepare_cluster_zones_groups_resident with the node columns from the node and label tables (nodes and
+        instance_group as in prepare_cluster_groups_node_table)."""
+        nt = _node_table_nodes(**nodes)
+        return self._prepare_zones_groups(_node_table_entry(load().gp_prepare_cluster_zones_groups_node_table), nt, instance_group,
+                                          n_instance_groups, None, int(nt.n_zones), None, None, None, None, None, None, kind, layout)
+
+    def reschedule_from_reservations_node_table(self, nodes: dict, exe, min_frag=False, hosting=None, keep_topology_zone=None,
+                                                topology_zone=None):
+        """reschedule_from_reservations_resident with the node columns from the node and label tables (nodes as in
+        prepare_cluster_groups_node_table; instance groups do not apply)."""
+        nt = _node_table_nodes(**nodes)
+        return self._reschedule(_node_table_entry(load().gp_reschedule_from_reservations_node_table), nt, exe, min_frag, hosting,
+                                None, int(nt.n_zones), None, None, None, None, keep_topology_zone, topology_zone)
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
