@@ -1205,8 +1205,8 @@ gp_status gp_exceeds_cluster_capacity_affinity_label_table(gp_ctx* ctx, const gp
  * Every node's allocatable, Spec.Unschedulable, NodeReady condition and name order kept on the device and changed only by
  * deltas from node events, so a Predicate no longer uploads those columns, nor sorts the node names on the host.  One row per
  * node id; node ids are the label table's (one node informer interns both).  A row holds: present, alloc cpu / mem / gpu,
- * unschedulable, ready, name_key, and name_rank -- the dense rank of name_key among the present rows, recomputed on the
- * device by every update.  name_key is an order key the caller keeps: strictly increasing in the byte order of the node
+ * unschedulable, ready, name_key, creation (the failover reconciler's newest-first order), and name_rank -- the dense rank
+ * of name_key among the present rows, recomputed on the device by every update.  name_key is an order key the caller keeps: strictly increasing in the byte order of the node
  * names, unique among present rows, below 2^63 - 1, and not necessarily dense (INTEGRATION.md: a new name takes the midpoint
  * of its neighbours' keys; when no gap is left every node is relabelled in one delta).  A rank over the whole table orders
  * any subset of it as the names do.  The table belongs to the context (freed by gp_destroy); updates change no snapshot,
@@ -1230,6 +1230,8 @@ typedef struct {
     const uint8_t* unschedulable;    /* [n_write] node.Spec.Unschedulable */
     const uint8_t* ready;            /* [n_write] NodeReady == True */
     const int64_t* name_key;         /* [n_write] the name's order key (see above) */
+    const int64_t* creation;         /* [n_write] metav1.Time as UnixNano (the order of gp_reconcile_nodes.creation), or NULL
+                                        (= 0 for every written row); no part of name_rank, no refusal */
 } gp_node_delta;
 /* Apply one delta, then recompute name_rank.  The whole delta is checked on the device before anything is written: a refused
  * delta leaves the table exactly as it was.  One stream synchronise.  GP_ERR_INVALID: no table (gp_node_table_reset first),
@@ -1256,7 +1258,7 @@ typedef struct {
     int32_t n_nodes;
     int32_t reserved;
     const int32_t* node_table_id;        /* [n_nodes] distinct, each a present row */
-    const int32_t* reservation_id;       /* [n_nodes] as gp_resident_usage.node_id */
+    const int32_t* reservation_id;       /* [n_nodes] as gp_resident_usage.node_id (NULL for the marker's entries) */
     const int32_t* overhead_node_id;     /* [n_nodes] as gp_resident_usage.overhead_node_id; required */
     const uint8_t* is_driver_candidate;  /* [n_nodes] member of ExtenderArgs.NodeNames, or NULL (= all) */
     int32_t zone_key;
@@ -1292,6 +1294,41 @@ gp_status gp_prepare_cluster_zones_groups_node_table(gp_ctx* ctx, const gp_node_
                                                      int32_t n_instance_groups, gp_instance_group_layout* layout);
 gp_status gp_reschedule_from_reservations_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, const gp_reschedule_scope* scope,
                                                      const gp_reschedule* in, int32_t* node_out, uint8_t* ambiguous);
+/* The failover reconciler's node-table form: gp_reconcile_find_nodes_resident with the node columns gathered on the device.
+ * It returns what gp_reconcile_find_nodes_resident returns -- placed, executor_nodes, the avail_* outputs, the status and
+ * the gp_last_error category -- and leaves the context as it does, given node_id = reservation_id, allocatable from the
+ * node table, overhead from the overhead table, and gp_reconcile_nodes{n_groups, node_group = the groups below, creation,
+ * unschedulable and ready from the node table}.  is_driver_candidate and the rank keys are ignored.
+ * The instance group follows the reference's instanceGroup(n.Labels[instanceGroupLabel]), where a missing label reads "":
+ *   instance_group_key >= 0   the index of the node's value id in instance_group_value [n_groups]; a node without the label
+ *                             is in instance_group_missing, the dense id of "" (list the value id of "" there, or -1 when no
+ *                             node carries ""), and is refused when instance_group_missing = -1; a value not listed is
+ *                             refused (every node must lie in [0, n_groups)).
+ *   instance_group_key = -1   every node in group 0.
+ * instance_group_out, when given, receives these groups.  Checks, in order (a refused call changes no state; its outputs
+ * are undefined): the gather's host checks (as for the entries above, and instance_group_missing outside [-1, n_groups)); then
+ * gp_reconcile_find_nodes_resident's host checks; then, read in its one synchronise, a node-table id out of range, absent
+ * or given twice, a zone refusal (zone_key >= 0), and an instance-group refusal; then its device refusals.  Like the
+ * resident form, a call with n_nodes = 0, or without stale drivers and avail_* outputs, returns before any device work is
+ * read. */
+gp_status gp_reconcile_find_nodes_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, int32_t n_groups,
+                                             int32_t instance_group_missing, const gp_apps* stale, gp_reconcile_results* out);
+/* The unschedulable-pod marker's node-table forms: gp_exceeds_cluster_capacity_resident and
+ * gp_exceeds_cluster_capacity_affinity_label_table with allocatable gathered from the node table, zone_id from the label
+ * table (zone_key, zone_value, zone_missing as above; NULL with zone_key = -1), overhead_node_id from nodes, and (affinity
+ * form) the label rows node_table_id.  Each returns what that entry returns -- exceeds, affinity_error and the status --
+ * and leaves the context as it does.  Unschedulable and not-ready nodes count, as in the marker.  reservation_id may be NULL;
+ * is_driver_candidate, the instance-group and rank keys are ignored.  node_group / n_groups: as gp_capacity_nodes'.
+ * Checks, in order: affinities missing (affinity form, as gp_exceeds_cluster_capacity_affinity_label_table checks first), the
+ * gather's host checks, the entry's host checks, then in its one synchronise the gather's refusals (a node-table id out of
+ * range, absent or given twice; a zone), then the entry's device refusals. */
+gp_status gp_exceeds_cluster_capacity_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, const int32_t* node_group,
+                                                 int32_t n_groups, const gp_apps* drivers, gp_binpacker packer,
+                                                 uint8_t* exceeds /* [n_apps] */);
+gp_status gp_exceeds_cluster_capacity_affinity_node_table(gp_ctx* ctx, const gp_node_table_nodes* nodes,
+                                                          const gp_node_affinities* affinities, const gp_apps* drivers,
+                                                          gp_binpacker packer, uint8_t* exceeds /* [n_apps] */,
+                                                          uint8_t* affinity_error /* [n_apps] or NULL */);
 
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets

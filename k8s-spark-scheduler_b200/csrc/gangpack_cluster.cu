@@ -892,7 +892,8 @@ gp_status gp_reschedule_from_reservations_resident(gp_ctx* c, const gp_resident_
 
 }  // extern "C"
 
-// gp_reconcile_find_nodes[_resident]
+// gp_reconcile_find_nodes[_resident|_node_table].  Gathered input (usage.on_device()): node_group, creation, unschedulable
+// and ready are device pointers too, kept in range by the gather, whose status word is read in the one synchronise.
 static gp_status reconcile_find_nodes(gp_ctx* c, const UsageIn& usage, const gp_reconcile_nodes* nodes, const gp_apps* a,
                                       gp_reconcile_results* out, const char* who) {
     if (!enter(c)) return GP_ERR_INVALID;
@@ -902,7 +903,8 @@ static gp_status reconcile_find_nodes(gp_ctx* c, const UsageIn& usage, const gp_
         (a->n_apps > 0 && (!a->exe_cpu_milli || !a->exe_mem_bytes || !a->exe_count || !out->placed)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or bad sizes (n_groups >= 1)");
     const int32_t q = a->n_apps, G = nodes->n_groups;
-    for (int32_t i = 0; i < n; ++i)
+    const bool dev = usage.on_device();
+    for (int32_t i = 0; i < (dev ? 0 : n); ++i)
         if (nodes->node_group[i] < 0 || nodes->node_group[i] >= G) return fail(c, GP_ERR_INVALID, who, "node_group out of range");
     GP_TRY(check_requests(c, q, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu, who));
     int64_t total = 0;
@@ -946,10 +948,10 @@ static gp_status reconcile_find_nodes(gp_ctx* c, const UsageIn& usage, const gp_
     const auto herr_p = ar.take<int>(1);
     const auto n_listed = ar.take<int32_t>(2);
     ar.reserve();
-    const int32_t* d_grp = ar.put(grp, nodes->node_group);
-    const long long* d_cre = ar.put(cre, nodes->creation);
-    const uint8_t* d_fu = ar.put(fu, nodes->unschedulable);
-    const uint8_t* d_fr = ar.put(fr, nodes->ready);
+    const int32_t* d_grp = dev ? nodes->node_group : ar.put(grp, nodes->node_group);
+    const long long* d_cre = dev ? (const long long*)nodes->creation : ar.put(cre, nodes->creation);
+    const uint8_t* d_fu = dev ? nodes->unschedulable : ar.put(fu, nodes->unschedulable);
+    const uint8_t* d_fr = dev ? nodes->ready : ar.put(fr, nodes->ready);
     ar.fill(claim, n_listed, 0);                        // claim counter, error word, listed drivers
     GP_TRY(ar.check(c));
     if (!c->recon_attr_set) {
@@ -1006,9 +1008,11 @@ static gp_status reconcile_find_nodes(gp_ctx* c, const UsageIn& usage, const gp_
     }
     int64_t* outs[3] = {out->avail_cpu_milli, out->avail_mem_bytes, out->avail_gpu};
     for (int d = 0; d < 3; ++d) ar.get(outs[d], d_avail + N * (size_t)d, N);
-    int uerr[2] = {0, 0};
+    int uerr[2] = {0, 0}, gather = 0;
     ar.get(uerr, d_err, 2);
+    if (dev) ar.get(&gather, usage.gather_err, 1);
     GP_TRY(ar.sync(c));
+    GP_TRY(nt_refusal(c, gather, who));
     GP_TRY(stage_refusal(c, uerr, who));
     return refuse(c, herr, kRcRefusals, who);
 }
@@ -1063,6 +1067,25 @@ gp_status gp_reschedule_from_reservations_node_table(gp_ctx* c, const gp_node_ta
     NtGathered g{};
     GP_TRY(nt_gather(c, nodes, nullptr, 1, false, who, &g));
     GP_TRY(reschedule_from_reservations(c, UsageIn(&g.usage, g.err), &g.sort, scope, in, node_out, ambiguous, who));
+    return nt_outputs(c, nodes, g);
+}
+
+// the failover reconciler: the gather adds creation and the reconciler's instance groups, then gp_reconcile_find_nodes_resident's
+// path runs on them
+gp_status gp_reconcile_find_nodes_node_table(gp_ctx* c, const gp_node_table_nodes* nodes, int32_t n_groups, int32_t instance_group_missing,
+                                             const gp_apps* a, gp_reconcile_results* out) {
+    static const char* who = "gp_reconcile_find_nodes_node_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    NtGathered g{};
+    const NtReconcile rc{instance_group_missing};
+    GP_TRY(nt_gather(c, nodes, nullptr, n_groups, true, who, &g, &rc));
+    gp_reconcile_nodes rn{};
+    rn.n_groups = n_groups;
+    rn.node_group = g.ig;
+    rn.creation = (const int64_t*)g.creation;
+    rn.unschedulable = g.sort.unschedulable;
+    rn.ready = g.sort.ready;
+    GP_TRY(reconcile_find_nodes(c, UsageIn(&g.usage, g.err), &rn, a, out, who));
     return nt_outputs(c, nodes, g);
 }
 

@@ -438,12 +438,20 @@ struct NtGathered {
     gp_resident_usage usage;
     gp_sort_input sort;
     const int32_t* ig;
+    const long long* creation;                // the failover reconciler's creation times (NtReconcile given), else NULL
     const int* err;
+};
+// The failover reconciler's instance groups: instanceGroup(n.Labels[key]) in [0, n_groups), a missing label in `missing`
+// (the dense id of "", -1 refused), a value not listed refused; key -1: every node in 0.  The gather then writes creation too.
+struct NtReconcile {
+    int32_t missing;
 };
 // The host checks of a *_node_table entry, then the gather enqueued on the context's stream.  ig_host (or NULL): the entry's
 // instance_group array, uploaded as is (checked by the *_resident entry); with_ig: read instance groups from the labels.
+// recon: the reconciler's rule over n_ig groups instead of the Predicates' (with_ig true, ig_host NULL).  reservations false:
+// reservation_id may be NULL (the marker's entries).
 gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* ig_host, int32_t n_ig, bool with_ig, const char* who,
-                    NtGathered* out);
+                    NtGathered* out, const NtReconcile* recon = nullptr, bool reservations = true);
 // The gather's refusal, once the stream has been synchronised
 gp_status nt_refusal(gp_ctx* c, int word, const char* who);
 // After the entry's synchronise: the optional zone_id_out / instance_group_out copies

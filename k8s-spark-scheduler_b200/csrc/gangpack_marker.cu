@@ -149,10 +149,12 @@ struct AffStage {
 // NULL) or the affinities' matches.  The overhead is nodes->overhead_* (resident false) or, resident, GetNonSchedulableOverhead
 // of the overhead table's records on node id over_ids[i] (-1: none), summed into this call's scratch by the query's kernels.
 // The affinities' labels are the per-call labels, or with rlabels the label table's rows.
+// gather_err (the *_node_table entries): nodes' allocatable and zone_id are device columns gathered from the node and label
+// tables, kept in range by the gather, whose status word is read in the one synchronise before the entry's own refusals.
 static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
                               const gp_node_affinities* aff, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds,
                               uint8_t* affinity_error, bool resident = false, const int32_t* over_ids = nullptr,
-                              const gp_resident_labels* rlabels = nullptr) {
+                              const gp_resident_labels* rlabels = nullptr, const int* gather_err = nullptr) {
     if (!aff) {
         if (!nodes || !a || nodes->n_nodes < 0 || a->n_apps < 0 || nodes->n_groups < 1 || (nodes->zone_id && nodes->n_zones < 1) ||
             (nodes->n_nodes > 0 && (!nodes->alloc_cpu_milli || !nodes->alloc_mem_bytes)) ||
@@ -239,11 +241,11 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         ni.n = n;
         const int64_t* cols[2][3] = {{nodes->alloc_cpu_milli, nodes->alloc_mem_bytes, nodes->alloc_gpu},
                                      {nodes->overhead_cpu_milli, nodes->overhead_mem_bytes, nodes->overhead_gpu}};
-        for (int d = 0; d < 3; ++d) ni.alloc[d] = ar.put(alloc.part(d * N, N), cols[0][d]);
+        for (int d = 0; d < 3; ++d) ni.alloc[d] = gather_err ? (const long long*)cols[0][d] : ar.put(alloc.part(d * N, N), cols[0][d]);
         if (!resident)
             for (int d = 0; d < 3; ++d) ni.over[d] = ar.put(over.part(d * N, N), cols[1][d]);
         const int32_t* d_oids = ar.put(oids, resident ? over_ids : nullptr);
-        ni.zone = ar.put(zone, nodes->zone_id);
+        ni.zone = gather_err ? nodes->zone_id : ar.put(zone, nodes->zone_id);
         ni.group = ar.put(grp, nodes->node_group);
         ci.group = ni.group;
         GP_TRY(ar.check(c));
@@ -298,7 +300,7 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     }
     if (Q > 0) gp_cc_decide<<<(unsigned)((q + T - 1) / T), T, 0, st>>>(Q, ai.count, ar.ptr(app_pair), ar.ptr(pairs), po, (int32_t)packer, ar.ptr(d_out));
     GP_CUDA(c, cudaGetLastError());
-    int herr = 0, aerr = 0, oerr_h[2] = {0, 0};
+    int herr = 0, aerr = 0, oerr_h[2] = {0, 0}, gather = 0;
     std::vector<int32_t> n_error(aff ? (size_t)G : 0);
     ar.get(exceeds, ar.ptr(d_out), q);
     ar.get(&herr, s.err, 1);
@@ -307,7 +309,9 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         ar.get(n_error.data(), as.ne);
     }
     ar.get(oerr_h, oerr);
+    if (gather_err) ar.get(&gather, gather_err, 1);
     GP_TRY(ar.sync(c));
+    GP_TRY(nt_refusal(c, gather, who));
     if (oerr_h[0]) return fail(c, GP_ERR_INVALID, who, "an overhead_node_id out of range or given twice");
     GP_TRY(oht_sum_refusal(c, oerr_h[1], who));
     if (aff) GP_TRY(refuse(c, aerr, kAffRefusals, who));
@@ -367,6 +371,44 @@ gp_status gp_exceeds_cluster_capacity_affinity_label_table(gp_ctx* c, const gp_c
     static const char* who = "gp_exceeds_cluster_capacity_affinity_label_table";
     if (!affinities || !labels) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
     return capacity_run(c, who, nodes, nullptr, affinities, a, packer, exceeds, affinity_error, true, overhead_node_id, labels);
+}
+
+// the node-table forms: nt_gather fills allocatable and zone_id on the device, then the resident / label-table path runs
+static gp_capacity_nodes gathered_nodes(const gp_node_table_nodes* nodes, const NtGathered& g, const int32_t* node_group, int32_t n_groups) {
+    gp_capacity_nodes cn{};
+    cn.n_nodes = g.usage.n_nodes;
+    cn.alloc_cpu_milli = g.usage.alloc_cpu_milli;
+    cn.alloc_mem_bytes = g.usage.alloc_mem_bytes;
+    cn.alloc_gpu = g.usage.alloc_gpu;
+    cn.n_zones = nodes->n_zones;
+    cn.zone_id = g.sort.zone_id;
+    cn.n_groups = n_groups;
+    cn.node_group = node_group;
+    return cn;
+}
+
+gp_status gp_exceeds_cluster_capacity_node_table(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* node_group, int32_t n_groups,
+                                                 const gp_apps* a, gp_binpacker packer, uint8_t* exceeds) {
+    static const char* who = "gp_exceeds_cluster_capacity_node_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    NtGathered g{};
+    GP_TRY(nt_gather(c, nodes, nullptr, 1, false, who, &g, nullptr, false));
+    const gp_capacity_nodes cn = gathered_nodes(nodes, g, node_group, n_groups);
+    GP_TRY(capacity_run(c, who, &cn, nullptr, nullptr, a, packer, exceeds, nullptr, true, nodes->overhead_node_id, nullptr, g.err));
+    return nt_outputs(c, nodes, g);
+}
+
+gp_status gp_exceeds_cluster_capacity_affinity_node_table(gp_ctx* c, const gp_node_table_nodes* nodes, const gp_node_affinities* affinities,
+                                                          const gp_apps* a, gp_binpacker packer, uint8_t* exceeds, uint8_t* affinity_error) {
+    static const char* who = "gp_exceeds_cluster_capacity_affinity_node_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    if (!affinities) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    NtGathered g{};
+    GP_TRY(nt_gather(c, nodes, nullptr, 1, false, who, &g, nullptr, false));
+    const gp_capacity_nodes cn = gathered_nodes(nodes, g, nullptr, 0);
+    const gp_resident_labels rl{nodes->n_nodes, 0, nodes->node_table_id};
+    GP_TRY(capacity_run(c, who, &cn, nullptr, affinities, a, packer, exceeds, affinity_error, true, nodes->overhead_node_id, &rl, g.err));
+    return nt_outputs(c, nodes, g);
 }
 
 // GetRequiredNodeAffinity(...).Match for every (affinity, node) over the per-call labels or (rl) the label table's rows

@@ -9,11 +9,13 @@
 //   gp_sort_tiles / gp_rank_by_search <NameKey>   pos[row] = the row's rank among all rows by (name_key, id)
 //   gp_nt_scatter + gp_nt_dups   the keys in rank order; two adjacent present keys that are equal refuse the delta
 //   gp_nt_apply     the row writes and name_rank[row] = pos[row] (-1 absent); nothing when the error word is set
+//   gp_nt_creation  the rows' creation times, under the same condition
 // so a refused delta leaves the table as it was, and only its stamps are written before the check is complete.
 //
 // The gather (gp_nt_gather, thread per listed node) writes exactly the columns a *_resident entry would upload: allocatable,
 // name_rank, unschedulable and ready from the node table, and zone, instance group and the two label ranks from the label
-// table's row of the same id, read through AffLabelsResident's row range and aff_find.
+// table's row of the same id, read through AffLabelsResident's row range and aff_find.  For the failover reconciler it also
+// writes creation, and reads the instance group under the reconciler's rule (a missing label is the group of "").
 #include "gangpack_ctx.cuh"
 #include "gangpack_labels.cuh"
 #include "gangpack_tilesort.cuh"
@@ -60,7 +62,7 @@ static const Refusal kNtRefusals[] = {
 
 struct NtPieces {
     Piece<uint8_t> present, unsched, ready;
-    Piece<long long> alloc, key;
+    Piece<long long> alloc, key, creation;
     Piece<int32_t> rank;
     Piece<uint32_t> stamp;
 };
@@ -74,6 +76,7 @@ static NtPieces take_cols(Arena& a, const gp_node_table_size& z) {
     p.ready = a.take<uint8_t>(R);
     p.alloc = a.take<long long>(3 * R);
     p.key = a.take<long long>(R);
+    p.creation = a.take<long long>(R);
     p.rank = a.take<int32_t>(R);
     p.stamp = a.take<uint32_t>(R);
     return p;
@@ -88,6 +91,7 @@ struct NtDelta {
     const uint8_t* unsched;
     const uint8_t* ready;
     const long long* key;
+    const long long* creation;        // NULL: 0
 };
 
 struct NtTable {
@@ -150,16 +154,28 @@ __global__ void gp_nt_apply(NtDelta D, NtTable T, const NameKey* __restrict__ ke
     }
 }
 
+// creation[row] of every write (0 for a deleted row), when the delta was accepted.  A kernel of its own, so that gp_nt_apply
+// is compiled as it was before the table kept creation times.
+__global__ void gp_nt_creation(NtDelta D, long long* __restrict__ creation, const int* __restrict__ err) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= D.n || *(volatile const int*)err) return;
+    creation[D.id[i]] = D.present[i] && D.creation ? D.creation[i] : 0;
+}
+
 // ---- the gather of the *_node_table entries ----
 
 enum : int {
     kNtgErrId = 1,              // a node-table id out of range, absent or given twice
     kNtgErrZone = 2,            // a zone value not listed, or a node without the zone label and zone_missing = -1
+    kNtgErrGroup = 4,           // the reconciler's rule: an instance-group value not listed
+    kNtgErrGroupMissing = 8,    // the reconciler's rule: a node without the instance-group label and instance_group_missing = -1
 };
 
 static const Refusal kNtgRefusals[] = {
     {kNtgErrId, GP_ERR_INVALID, "a node-table id out of range, absent or given twice"},
     {kNtgErrZone, GP_ERR_INVALID, "a zone label value not in zone_value, or a node without the zone label (zone_missing = -1)"},
+    {kNtgErrGroup, GP_ERR_INVALID, "an instance-group label value not in instance_group_value"},
+    {kNtgErrGroupMissing, GP_ERR_INVALID, "a node without the instance-group label (instance_group_missing = -1)"},
 };
 
 // A label key and the value ids it maps: map [n] sorted by value, .y = the dense id or rank.  key -1: not read.
@@ -175,12 +191,16 @@ struct NtGatherIn {
     const uint8_t* present; const uint8_t* unsched; const uint8_t* ready;
     const long long* alloc;           // [3][n_rows]
     const int32_t* rank;
+    const long long* creation;        // [n_rows]
     NtLabelMap zone, ig, lr[2];
     int32_t zone_missing;
+    int32_t ig_missing;               // the reconciler's rule (strict_ig): the group of a node without the label, -1 refused
+    bool strict_ig;
     int32_t* dir;                     // [n_rows] -1: no listed node has the id yet
     long long* alloc_out;             // [3][n]
     int32_t* rank_out; uint8_t* unsched_out; uint8_t* ready_out;
     int32_t* zone_out; int32_t* ig_out; int32_t* lr_out[2];
+    long long* creation_out;          // [n] or NULL: not asked for
     int* err;
 };
 
@@ -227,7 +247,17 @@ __global__ void gp_nt_gather(NtGatherIn G) {
         if (z < 0) { bad |= kNtgErrZone; z = 0; }
         G.zone_out[i] = z;
     }
-    if (G.ig.key >= 0) {
+    if (G.creation_out) G.creation_out[i] = ok ? G.creation[r] : 0;
+    if (G.strict_ig) {
+        // every node in [0, n_groups): a refused one takes 0, so that the reconciler's stages index in range
+        int32_t g = 0;
+        if (G.ig.key >= 0) {
+            const int32_t v = nt_label(G.L, i, G.ig.key);
+            g = v < 0 ? G.ig_missing : nt_lookup(G.ig, v);
+            if (g < 0) { bad |= v < 0 ? kNtgErrGroupMissing : kNtgErrGroup; g = 0; }
+        }
+        G.ig_out[i] = g;
+    } else if (G.ig.key >= 0) {
         const int32_t v = nt_label(G.L, i, G.ig.key);
         G.ig_out[i] = v < 0 ? -1 : nt_lookup(G.ig, v);
     }
@@ -261,17 +291,19 @@ static bool label_map(const int32_t* list, int32_t n, bool distinct, std::vector
 }
 
 gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nd, const int32_t* ig_host, int32_t n_ig, bool with_ig, const char* who,
-                    NtGathered* g) {
+                    NtGathered* g, const NtReconcile* recon, bool reservations) {
     auto& t = c->nt;
     if (!t.live) return no_table(c, who);
     if (!c->lt.live) return fail(c, GP_ERR_INVALID, who, "no label table (gp_label_table_reset first)");
     if (!nd || nd->n_nodes < 0 || nd->n_zones < 1 ||
-        (nd->n_nodes > 0 && (!nd->node_table_id || !nd->reservation_id || !nd->overhead_node_id)) ||
+        (nd->n_nodes > 0 && (!nd->node_table_id || (reservations && !nd->reservation_id) || !nd->overhead_node_id)) ||
         (nd->zone_key >= 0 && !nd->zone_value) || (with_ig && !ig_host && nd->instance_group_key >= 0 && n_ig > 0 && !nd->instance_group_value) ||
         (nd->driver_rank_key >= 0 && (nd->n_driver_rank_values < 0 || (nd->n_driver_rank_values > 0 && !nd->driver_rank_value))) ||
         (nd->executor_rank_key >= 0 && (nd->n_executor_rank_values < 0 || (nd->n_executor_rank_values > 0 && !nd->executor_rank_value))))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or bad sizes");
     if (nd->zone_missing < -1 || nd->zone_missing >= nd->n_zones) return fail(c, GP_ERR_INVALID, who, "zone_missing outside [-1, n_zones)");
+    if (recon && (recon->missing < -1 || recon->missing >= std::max(n_ig, 0)))
+        return fail(c, GP_ERR_INVALID, who, "instance_group_missing outside [-1, n_groups)");
     const bool label_ig = with_ig && !ig_host && nd->instance_group_key >= 0;
     std::vector<int2> maps[4];
     if (nd->zone_key >= 0 && !label_map(nd->zone_value, nd->n_zones, true, maps[0]))
@@ -290,6 +322,7 @@ gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nd, const int32_t* ig_
     const auto rank = ar.take<int32_t>(N), zone = ar.take<int32_t>(N), ig = ar.take<int32_t>(N), lrd = ar.take<int32_t>(N),
                lre = ar.take<int32_t>(N);
     const auto fu = ar.take<uint8_t>(N), fr = ar.take<uint8_t>(N);
+    const auto cre = ar.take<long long>(recon ? N : 0);
     const auto dir = ar.take<int32_t>(R);
     Piece<int2> mp[4];
     for (int k = 0; k < 4; ++k) mp[k] = ar.take<int2>(maps[k].size());
@@ -304,11 +337,14 @@ gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nd, const int32_t* ig_
     Arena tc{t.cols, st};
     const NtPieces p = take_cols(tc, t.size);
     G.present = tc.ptr(p.present); G.unsched = tc.ptr(p.unsched); G.ready = tc.ptr(p.ready);
-    G.alloc = tc.ptr(p.alloc); G.rank = tc.ptr(p.rank);
+    G.alloc = tc.ptr(p.alloc); G.rank = tc.ptr(p.rank); G.creation = tc.ptr(p.creation);
     const int32_t keys[4] = {nd->zone_key, label_ig ? nd->instance_group_key : -1, nd->driver_rank_key, nd->executor_rank_key};
     NtLabelMap* lm[4] = {&G.zone, &G.ig, &G.lr[0], &G.lr[1]};
     for (int k = 0; k < 4; ++k) *lm[k] = NtLabelMap{keys[k] >= 0 ? keys[k] : -1, (int32_t)maps[k].size(), ar.put(mp[k], maps[k].data())};
     G.zone_missing = nd->zone_missing;
+    G.strict_ig = recon != nullptr;
+    G.ig_missing = recon ? recon->missing : -1;
+    G.creation_out = recon ? ar.ptr(cre) : nullptr;
     G.dir = ar.fill(dir, 0xff);
     G.alloc_out = ar.ptr(alloc); G.rank_out = ar.ptr(rank); G.unsched_out = ar.ptr(fu); G.ready_out = ar.ptr(fr);
     G.zone_out = ar.ptr(zone); G.ig_out = ar.ptr(ig); G.lr_out[0] = ar.ptr(lrd); G.lr_out[1] = ar.ptr(lre);
@@ -339,7 +375,8 @@ gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nd, const int32_t* ig_
     s.driver_label_rank = nd->driver_rank_key >= 0 ? G.lr_out[0] : nullptr;
     s.executor_label_rank = nd->executor_rank_key >= 0 ? G.lr_out[1] : nullptr;
     s.undefined_ties = nd->undefined_ties;
-    g->ig = ig_host || label_ig ? G.ig_out : nullptr;
+    g->ig = ig_host || label_ig || recon ? G.ig_out : nullptr;
+    g->creation = G.creation_out;
     g->err = G.err;
     return GP_OK;
 }
@@ -394,7 +431,7 @@ gp_status gp_node_table_update(gp_ctx* c, const gp_node_delta* d) {
     Arena ar{c->callbuf, st};
     const auto id = ar.take<int32_t>(W);
     const auto on = ar.take<uint8_t>(W), fu = ar.take<uint8_t>(W), fr = ar.take<uint8_t>(W);
-    const auto al = ar.take<long long>(3 * W), key = ar.take<long long>(W);
+    const auto al = ar.take<long long>(3 * W), key = ar.take<long long>(W), cre = ar.take<long long>(W);
     const auto keys = ar.take<NameKey>(R), sorted = ar.take<NameKey>(R);
     const auto pos = ar.take<int32_t>(R);
     const auto skey = ar.take<long long>(R);
@@ -411,6 +448,7 @@ gp_status gp_node_table_update(gp_ctx* c, const gp_node_delta* d) {
     D.unsched = ar.put(fu, d->unschedulable);
     D.ready = ar.put(fr, d->ready);
     D.key = ar.put(key, d->name_key);
+    D.creation = ar.put(cre, d->creation);
     GP_TRY(ar.check(c));
     // From here on the table's own buffers are written: a CUDA error leaves no table (reset and replay)
     t.live = false;
@@ -436,6 +474,7 @@ gp_status gp_node_table_update(gp_ctx* c, const gp_node_delta* d) {
         const long long items = (long long)W + (long long)R;
         const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((items + T - 1) / T, (long long)c->sm_count * 8));
         gp_nt_apply<<<grid, T, 0, st>>>(D, tab, ar.ptr(keys), ar.ptr(pos), w);
+        if (W > 0) gp_nt_creation<<<(unsigned)((W + T - 1) / T), T, 0, st>>>(D, tc.ptr(p.creation), w);
     }
     GP_CUDA(c, cudaGetLastError());
     int hw = 0;

@@ -1040,7 +1040,7 @@ inline MatchResult MatchRequiredNodeAffinity(const std::vector<std::string>& nod
 
 namespace resources {
 
-// Every node's allocatable, Spec.Unschedulable, NodeReady condition and name order as the resident node table
+// Every node's allocatable, Spec.Unschedulable, NodeReady condition, creation time and name order as the resident node table
 // (gp_node_table_*) keeps them, from the node informer: SetNode for AddFunc and UpdateFunc, after the label table's SetNode,
 // which gives the node its id (no write when nothing changed); DeleteNode for DeleteFunc, before the label table's
 // DeleteNode, which frees the id.  name_key is kept here: strictly increasing in the byte order of the names, in
@@ -1053,7 +1053,8 @@ public:
     explicit ResidentNodes(const affinity::ResidentLabels& labels, int32_t nNodeIds = 64, int keyBits = 62)
         : labels_(labels), size_{nNodeIds, 0}, keyHi_((int64_t)1 << keyBits) {}
 
-    void SetNode(const std::string& name, const Resources& allocatable, bool unschedulable, bool ready) {
+    // creationUnixNano: metav1.Time as UnixNano (the failover reconciler's newest-first order)
+    void SetNode(const std::string& name, const Resources& allocatable, bool unschedulable, bool ready, int64_t creationUnixNano = 0) {
         const int32_t at = labels_.NodeIDs({name})[0];
         if (at < 0) throw gangpack::Error(GP_ERR_INVALID, "ResidentNodes::SetNode: the label table does not know " + name + " (its SetNode first)");
         auto held = nameAt_.find(at);
@@ -1062,7 +1063,7 @@ public:
         auto cur = nodes_.find(name);
         if (cur != nodes_.end() && cur->second.id != at)
             throw gangpack::Error(GP_ERR_INVALID, "ResidentNodes::SetNode: " + name + " is held under another id (DeleteNode it before the label table's)");
-        const Row row{true, {allocatable.CPU, allocatable.Memory, allocatable.NvidiaGPU}, unschedulable, ready, 0};
+        const Row row{true, {allocatable.CPU, allocatable.Memory, allocatable.NvidiaGPU}, unschedulable, ready, 0, creationUnixNano};
         if (cur != nodes_.end()) {
             Row next = row;
             next.key = cur->second.row.key;
@@ -1097,13 +1098,15 @@ public:
     }
     int64_t NameKey(const std::string& name) const { return nodes_.at(name).row.key; }
     int Relabels() const { return relabels_; }
+    int Replays() const { return replays_; }      // Replay calls: a host path's fallback after a refused device call is one
 
     // the per-call columns the node-table entries stand for: allocatable, name_rank (the byte order of the listed names, a
-    // permutation of 0..n-1), unschedulable and ready
+    // permutation of 0..n-1), unschedulable, ready and creation
     struct Columns {
         std::vector<int64_t> alloc[3];
         std::vector<int32_t> nameRank;
         std::vector<uint8_t> unschedulable, ready;
+        std::vector<int64_t> creation;
     };
     Columns PerCall(const std::vector<std::string>& names) const {
         Columns c;
@@ -1117,23 +1120,25 @@ public:
             for (int d = 0; d < 3; ++d) c.alloc[d].push_back(r.alloc[d]);
             c.unschedulable.push_back(r.unschedulable);
             c.ready.push_back(r.ready);
+            c.creation.push_back(r.creation);
         }
         return c;
     }
 
-    void Replay() { replay_ = true; }
+    void Replay() { replay_ = true; ++replays_; }
 
     void Flush(gangpack::Device& dev) {
         const int32_t need = nameAt_.empty() ? 0 : nameAt_.rbegin()->first + 1;
         while (size_.n_node_ids < need) { size_.n_node_ids = std::max<int32_t>(2 * size_.n_node_ids, 1); replay_ = true; }
         std::vector<int32_t> id;
         std::vector<uint8_t> present, uns, rdy;
-        std::vector<int64_t> v[3], key;
+        std::vector<int64_t> v[3], key, cre;
         auto row = [&](int32_t at) {
             const Row r = record(at);
             id.push_back(at); present.push_back(r.present); uns.push_back(r.unschedulable); rdy.push_back(r.ready);
             for (int d = 0; d < 3; ++d) v[d].push_back(r.alloc[d]);
             key.push_back(r.key);
+            cre.push_back(r.creation);
         };
         if (replay_) {
             sent_.clear();
@@ -1149,7 +1154,7 @@ public:
         if (reset) dev.check(gp_node_table_reset(dev.ctx(), &size_), "gp_node_table_reset");
         if (!id.empty()) {
             gp_node_delta d{(int32_t)id.size(), 0, id.data(), present.data(), v[0].data(), v[1].data(), v[2].data(), uns.data(),
-                            rdy.data(), key.data()};
+                            rdy.data(), key.data(), cre.data()};
             dev.check(gp_node_table_update(dev.ctx(), &d), "gp_node_table_update");
         }
         for (int32_t at : id) sent_[at] = record(at);
@@ -1163,9 +1168,10 @@ private:
         int64_t alloc[3] = {0, 0, 0};
         bool unschedulable = false, ready = false;
         int64_t key = 0;
+        int64_t creation = 0;
         bool operator==(const Row& o) const {
             return present == o.present && alloc[0] == o.alloc[0] && alloc[1] == o.alloc[1] && alloc[2] == o.alloc[2] &&
-                   unschedulable == o.unschedulable && ready == o.ready && key == o.key;
+                   unschedulable == o.unschedulable && ready == o.ready && key == o.key && creation == o.creation;
         }
     };
     struct Held { int32_t id; Row row; };
@@ -1200,6 +1206,7 @@ private:
     int64_t keyHi_;
     bool replay_ = true;
     int relabels_ = 0;
+    int replays_ = 0;
     std::unordered_map<std::string, Held> nodes_;
     std::map<int32_t, std::string> nameAt_;
     std::set<std::string> byName_;
@@ -1797,6 +1804,20 @@ public:
                                                     affinity::ResidentLabels& labels, const std::vector<affinity::Program>& programs,
                                                     const std::vector<AffinityStaleDriver>& drivers, std::vector<bool>* affinityError) const;
 
+    // The two resident sweeps with allocatable from the node table and the zone from the label table: names lists the nodes,
+    // zones the dense zones ("default" appended when not listed).  The overhead, label and node tables are flushed once,
+    // then one gp_exceeds_cluster_capacity[_affinity]_node_table call.  A refused call resets and replays the three tables and
+    // makes the resident sweep above over the columns the host decodes from them (defined after ResidentOverheadComputer).
+    std::vector<bool> DoesPodsExceedClusterCapacity(const std::vector<std::string>& names, resources::ResidentNodes& nodes,
+                                                    affinity::ResidentLabels& labels, ResidentOverheadComputer& overhead,
+                                                    const std::vector<std::string>& zones,
+                                                    const std::unordered_map<std::string, int32_t>& nodeClass, int32_t nClasses,
+                                                    const std::vector<StaleDriver>& drivers) const;
+    std::vector<bool> DoesPodsExceedClusterCapacity(const std::vector<std::string>& names, resources::ResidentNodes& nodes,
+                                                    affinity::ResidentLabels& labels, ResidentOverheadComputer& overhead,
+                                                    const std::vector<std::string>& zones, const std::vector<affinity::Program>& programs,
+                                                    const std::vector<AffinityStaleDriver>& drivers, std::vector<bool>* affinityError) const;
+
 private:
     gp_binpacker Packer() const {
         if (packer_.Name == binpacker::tightlyPack) return GP_BP_TIGHTLY_PACK;
@@ -1844,10 +1865,13 @@ struct ReconcileCall {
     gp_reconcile_nodes nd{};
     gp_apps a{};
     gp_reconcile_results out{};
-    ReconcileCall(const std::vector<ReconcileNode>& nodes, const std::string& instanceGroupLabel, const std::vector<StaleDriver>& drivers) {
+    // groups (or NULL): instance-group values that take ids 0, 1, .. before any node's or driver's
+    ReconcileCall(const std::vector<ReconcileNode>& nodes, const std::string& instanceGroupLabel, const std::vector<StaleDriver>& drivers,
+                  const std::vector<std::string>* groups = nullptr) {
         const size_t N = nodes.size(), Q = drivers.size();
         std::unordered_map<std::string, int32_t> groupId;
         auto intern = [&](const std::string& g) { return groupId.emplace(g, (int32_t)groupId.size()).first->second; };
+        if (groups) for (const auto& g : *groups) intern(g);
         ac.resize(N); am.resize(N); ag.resize(N); cr.resize(N); grp.resize(N); unsched.resize(N); ready.resize(N);
         for (size_t i = 0; i < N; ++i) {
             const ReconcileNode& n = nodes[i];
@@ -1875,10 +1899,15 @@ struct ReconcileCall {
     ReconcileCall(const ReconcileCall&) = delete;
     ReconcileCall& operator=(const ReconcileCall&) = delete;
     std::vector<ReconcileResult> Results(const std::vector<ReconcileNode>& nodes) const {
+        std::vector<std::string> names;
+        for (const auto& n : nodes) names.push_back(n.Name);
+        return Results(names);
+    }
+    std::vector<ReconcileResult> Results(const std::vector<std::string>& names) const {
         std::vector<ReconcileResult> res((size_t)a.n_apps);
         for (size_t i = 0; i < res.size(); ++i) {
             res[i].InstanceGroupFound = placed[i] >= 0;
-            for (int32_t j = 0; j < placed[i]; ++j) res[i].ReservedNodeNames.push_back(nodes[(size_t)exe[(size_t)off[i] + (size_t)j]].Name);
+            for (int32_t j = 0; j < placed[i]; ++j) res[i].ReservedNodeNames.push_back(names[(size_t)exe[(size_t)off[i] + (size_t)j]]);
         }
         return res;
     }
@@ -2641,6 +2670,178 @@ inline std::vector<bool> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(c
         md[node.Name] = m;
     }
     return DoesPodsExceedClusterCapacity(md, labels.Nodes(names), programs, drivers, affinityError);
+}
+
+// The CapacityNode list of the resident sweeps, decoded on the host from the node and label tables' own state
+inline std::vector<UnschedulablePodMarker::CapacityNode> CapacityNodesOf(const std::vector<std::string>& names,
+                                                                         const resources::ResidentNodes& nodes,
+                                                                         const affinity::ResidentLabels& labels) {
+    const resources::ResidentNodes::Columns c = nodes.PerCall(names);
+    const std::vector<affinity::Node> lab = labels.Nodes(names);
+    std::vector<UnschedulablePodMarker::CapacityNode> out(names.size());
+    for (size_t i = 0; i < names.size(); ++i) {
+        out[i].Name = names[i];
+        out[i].Allocatable = resources::Resources{c.alloc[0][i], c.alloc[1][i], c.alloc[2][i]};
+        auto z = lab[i].Labels.find(resources::NodeTableLabels::kZoneLabel);
+        if (z != lab[i].Labels.end()) out[i].ZoneLabel = z->second;
+    }
+    return out;
+}
+
+// The gp_node_table_nodes of a node-table marker sweep over these names (flushed tables; the zone arguments from z)
+struct MarkerNodeTable {
+    std::vector<int32_t> ids, oids;
+    gp_node_table_nodes nd{};
+    MarkerNodeTable(const std::vector<std::string>& names, const resources::ResidentNodes& nodes, ResidentOverheadComputer& overhead,
+                    const resources::NodeTableLabels& z)
+        : ids(nodes.NodeIDs(names)), oids(overhead.NodeIDs(names)) {
+        z.Fill(&nd);
+        nd.n_nodes = (int32_t)names.size();
+        nd.node_table_id = ids.data();
+        nd.overhead_node_id = oids.data();
+    }
+};
+
+inline std::vector<bool> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(const std::vector<std::string>& names,
+                                                                               resources::ResidentNodes& nodes,
+                                                                               affinity::ResidentLabels& labels,
+                                                                               ResidentOverheadComputer& overhead,
+                                                                               const std::vector<std::string>& zones,
+                                                                               const std::unordered_map<std::string, int32_t>& nodeClass,
+                                                                               int32_t nClasses, const std::vector<StaleDriver>& drivers) const {
+    gangpack::Device& dev = gangpack::Device::Get();
+    overhead.Flush(dev);
+    labels.Flush(dev);
+    nodes.Flush(dev);
+    const size_t N = names.size(), Q = drivers.size();
+    const resources::NodeTableLabels z(labels, zones, "", {});
+    MarkerNodeTable t(names, nodes, overhead, z);
+    std::vector<int32_t> group(N + 1);
+    for (size_t i = 0; i < N; ++i) {
+        auto c = nodeClass.find(names[i]);
+        group[i] = c == nodeClass.end() ? -1 : c->second;
+    }
+    std::vector<int64_t> q[6];
+    std::vector<int32_t> count(Q + 1), cls(Q + 1);
+    for (auto& col : q) col.resize(Q + 1);
+    for (size_t i = 0; i < Q; ++i) {
+        const StaleDriver& d = drivers[i];
+        q[0][i] = d.DriverResources.CPU; q[1][i] = d.DriverResources.Memory; q[2][i] = d.DriverResources.NvidiaGPU;
+        q[3][i] = d.ExecutorResources.CPU; q[4][i] = d.ExecutorResources.Memory; q[5][i] = d.ExecutorResources.NvidiaGPU;
+        count[i] = d.MinExecutorCount; cls[i] = d.AffinityClass;
+    }
+    gp_apps a{};
+    a.n_apps = (int32_t)Q;
+    a.drv_cpu_milli = q[0].data(); a.drv_mem_bytes = q[1].data(); a.drv_gpu = q[2].data();
+    a.exe_cpu_milli = q[3].data(); a.exe_mem_bytes = q[4].data(); a.exe_gpu = q[5].data();
+    a.exe_count = count.data(); a.group = cls.data();
+    std::vector<uint8_t> out(Q + 1);
+    if (gp_exceeds_cluster_capacity_node_table(dev.ctx(), &t.nd, group.data(), std::max<int32_t>(1, nClasses), &a, Packer(), out.data()) == GP_OK)
+        return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
+    overhead.Replay();
+    labels.Replay();
+    nodes.Replay();
+    labels.Flush(dev);
+    nodes.Flush(dev);
+    return DoesPodsExceedClusterCapacity(CapacityNodesOf(names, nodes, labels), overhead, nodeClass, nClasses, drivers);
+}
+
+inline std::vector<bool> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(const std::vector<std::string>& names,
+                                                                               resources::ResidentNodes& nodes,
+                                                                               affinity::ResidentLabels& labels,
+                                                                               ResidentOverheadComputer& overhead,
+                                                                               const std::vector<std::string>& zones,
+                                                                               const std::vector<affinity::Program>& programs,
+                                                                               const std::vector<AffinityStaleDriver>& drivers,
+                                                                               std::vector<bool>* affinityError) const {
+    gangpack::Device& dev = gangpack::Device::Get();
+    overhead.Flush(dev);
+    labels.Flush(dev);
+    nodes.Flush(dev);
+    const size_t Q = drivers.size();
+    const resources::NodeTableLabels z(labels, zones, "", {});
+    MarkerNodeTable t(names, nodes, overhead, z);
+    std::vector<int64_t> q[6];
+    std::vector<int32_t> count(Q + 1), prog(Q + 1);
+    for (auto& col : q) col.resize(Q + 1);
+    for (size_t i = 0; i < Q; ++i) {
+        const AffinityStaleDriver& d = drivers[i];
+        q[0][i] = d.DriverResources.CPU; q[1][i] = d.DriverResources.Memory; q[2][i] = d.DriverResources.NvidiaGPU;
+        q[3][i] = d.ExecutorResources.CPU; q[4][i] = d.ExecutorResources.Memory; q[5][i] = d.ExecutorResources.NvidiaGPU;
+        count[i] = d.MinExecutorCount; prog[i] = d.Affinity;
+    }
+    const affinity::Encoded e = labels.EncodePrograms(names, programs);
+    const gp_node_affinities p = e.Programs();
+    gp_apps a{};
+    a.n_apps = (int32_t)Q;
+    a.drv_cpu_milli = q[0].data(); a.drv_mem_bytes = q[1].data(); a.drv_gpu = q[2].data();
+    a.exe_cpu_milli = q[3].data(); a.exe_mem_bytes = q[4].data(); a.exe_gpu = q[5].data();
+    a.exe_count = count.data(); a.group = prog.data();
+    std::vector<uint8_t> out(Q + 1), err(Q + 1);
+    if (gp_exceeds_cluster_capacity_affinity_node_table(dev.ctx(), &t.nd, &p, &a, Packer(), out.data(), err.data()) == GP_OK) {
+        if (affinityError) affinityError->assign(err.begin(), err.begin() + (std::ptrdiff_t)Q);
+        return std::vector<bool>(out.begin(), out.begin() + (std::ptrdiff_t)Q);
+    }
+    overhead.Replay();
+    labels.Replay();
+    nodes.Replay();
+    nodes.Flush(dev);
+    return DoesPodsExceedClusterCapacity(CapacityNodesOf(names, nodes, labels), overhead, labels, programs, drivers, affinityError);
+}
+
+// ReconcileFindNodes over the four resident tables (gp_reconcile_find_nodes_node_table): names lists the lister's nodes (their
+// order is the tie order among equal creation times); instanceGroups the values of instanceGroupLabel in group order -- ""
+// (the group of a node without the label) and any driver's group not listed are appended.  Each table's pending delta is
+// flushed once, then one device call reads allocatable, flags, creation, the instance-group label, every reservation and
+// GetOverhead in place.  A refused call (a node whose instance group is not listed, for one) resets and replays the label
+// and node tables and makes ReconcileFindNodesResident over the columns the host decodes from them.  That costs a full
+// resend of both tables on every call while such a node exists: list every value the nodes carry for the key, not only
+// the groups Spark manages.
+inline std::vector<ReconcileResult> ReconcileFindNodesNodeTable(const std::vector<std::string>& names, resources::ResidentNodes& nodes,
+                                                                affinity::ResidentLabels& labels, ResidentReservations& reservations,
+                                                                ResidentOverheadComputer& overhead, const std::string& instanceGroupLabel,
+                                                                const std::vector<std::string>& instanceGroups,
+                                                                const std::vector<StaleDriver>& drivers) {
+    gangpack::Device& dev = gangpack::Device::Get();
+    labels.Flush(dev);
+    nodes.Flush(dev);
+    reservations.Flush(dev);
+    overhead.Flush(dev);
+    // every group id the call uses: the listed values, "", then the drivers' groups not listed (no node of the listed ones
+    // is in them; a value id no row holds, or the value's own id when some node carries it after all).  The value list
+    // and n_groups are the same list, so the gather reads exactly n_groups values.
+    std::vector<std::string> groups = instanceGroups;
+    if (std::find(groups.begin(), groups.end(), std::string()) == groups.end()) groups.push_back(std::string());
+    const int32_t missing = (int32_t)(std::find(groups.begin(), groups.end(), std::string()) - groups.begin());
+    for (const auto& d : drivers)
+        if (std::find(groups.begin(), groups.end(), d.InstanceGroup) == groups.end()) groups.push_back(d.InstanceGroup);
+    ReconcileCall call({}, instanceGroupLabel, drivers, &groups);
+    const resources::NodeTableLabels ig(labels, {}, instanceGroupLabel, groups);
+    const std::vector<int32_t> ids = nodes.NodeIDs(names), rids = reservations.NodeIDs(names), oids = overhead.NodeIDs(names);
+    gp_node_table_nodes nd{};
+    ig.Fill(&nd);
+    nd.zone_key = -1; nd.n_zones = 1; nd.zone_value = nullptr; nd.zone_missing = -1;
+    nd.driver_rank_key = -1; nd.executor_rank_key = -1;
+    nd.n_nodes = (int32_t)names.size();
+    nd.node_table_id = ids.data(); nd.reservation_id = rids.data(); nd.overhead_node_id = oids.data();
+    if (gp_reconcile_find_nodes_node_table(dev.ctx(), &nd, (int32_t)groups.size(), missing, &call.a, &call.out) == GP_OK)
+        return call.Results(names);
+    labels.Replay();
+    nodes.Replay();
+    labels.Flush(dev);
+    nodes.Flush(dev);
+    const resources::ResidentNodes::Columns c = nodes.PerCall(names);
+    const std::vector<affinity::Node> lab = labels.Nodes(names);
+    std::vector<ReconcileNode> rn(names.size());
+    for (size_t i = 0; i < names.size(); ++i) {
+        rn[i].Name = names[i];
+        rn[i].Allocatable = resources::Resources{c.alloc[0][i], c.alloc[1][i], c.alloc[2][i]};
+        rn[i].Labels.insert(lab[i].Labels.begin(), lab[i].Labels.end());
+        rn[i].Unschedulable = c.unschedulable[i] != 0;
+        rn[i].Ready = c.ready[i] != 0;
+        rn[i].CreationUnixNano = c.creation[i];
+    }
+    return ReconcileFindNodesResident(rn, reservations, overhead, instanceGroupLabel, drivers);
 }
 
 }  // namespace extender

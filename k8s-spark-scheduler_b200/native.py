@@ -45,6 +45,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_match_node_affinity_resident", "gp_exceeds_cluster_capacity_affinity_label_table",
            "gp_node_table_reset", "gp_node_table_update", "gp_prepare_cluster_groups_node_table",
            "gp_prepare_cluster_zones_groups_node_table", "gp_reschedule_from_reservations_node_table",
+           "gp_reconcile_find_nodes_node_table", "gp_exceeds_cluster_capacity_node_table",
+           "gp_exceeds_cluster_capacity_affinity_node_table",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -296,7 +298,7 @@ class gp_node_table_size(C.Structure):
 class gp_node_delta(C.Structure):
     _fields_ = [("n_write", C.c_int32), ("reserved", C.c_int32), ("node_id", C.c_void_p), ("present", C.c_void_p),
                 ("alloc_cpu_milli", C.c_void_p), ("alloc_mem_bytes", C.c_void_p), ("alloc_gpu", C.c_void_p),
-                ("unschedulable", C.c_void_p), ("ready", C.c_void_p), ("name_key", C.c_void_p)]
+                ("unschedulable", C.c_void_p), ("ready", C.c_void_p), ("name_key", C.c_void_p), ("creation", C.c_void_p)]
 
 
 class gp_node_table_nodes(C.Structure):
@@ -459,6 +461,15 @@ def load():
     L.gp_reschedule_from_reservations_node_table.restype = C.c_int
     L.gp_reschedule_from_reservations_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.POINTER(gp_reschedule_scope),
                                                              C.POINTER(gp_reschedule), C.c_void_p, C.c_void_p]
+    L.gp_reconcile_find_nodes_node_table.restype = C.c_int
+    L.gp_reconcile_find_nodes_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.c_int32, C.c_int32, C.POINTER(gp_apps),
+                                                     C.POINTER(gp_reconcile_results)]
+    L.gp_exceeds_cluster_capacity_node_table.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.c_void_p, C.c_int32,
+                                                         C.POINTER(gp_apps), C.c_int, C.c_void_p]
+    L.gp_exceeds_cluster_capacity_affinity_node_table.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_affinity_node_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.POINTER(gp_node_affinities),
+                                                                  C.POINTER(gp_apps), C.c_int, C.c_void_p, C.c_void_p]
     L.gp_pack_one.restype = C.c_int
     L.gp_pack_one.argtypes = [C.c_void_p, C.c_int] + [C.c_int64] * 6 + [C.c_int32, C.POINTER(C.c_int32),
                                                                           C.POINTER(C.c_int32), C.c_void_p]
@@ -676,7 +687,7 @@ _LT_DELTA_COLS = {"row_node": np.int32, "row_off": np.int64, "label_key": np.int
 
 # gp_node_delta's columns (nodes.NodeTable.delta() keys)
 _NT_DELTA_COLS = {"node_id": np.int32, "present": np.uint8, "alloc_cpu_milli": np.int64, "alloc_mem_bytes": np.int64,
-                  "alloc_gpu": np.int64, "unschedulable": np.uint8, "ready": np.uint8, "name_key": np.int64}
+                  "alloc_gpu": np.int64, "unschedulable": np.uint8, "ready": np.uint8, "name_key": np.int64, "creation": np.int64}
 
 # gp_reservation_delta's columns (reservations.ReservationTable.delta() keys)
 _RT_DELTA_COLS = {"slot": np.int32, "node_id": np.int32, "cpu_milli": np.int64, "mem_bytes": np.int64, "gpu": np.int64}
@@ -1463,7 +1474,8 @@ class GangPacker:
 
     def node_table_update(self, delta: dict):
         """One gp_node_table_update over the arrays of nodes.NodeTable.delta() (node_id, present, alloc_cpu_milli,
-        alloc_mem_bytes, alloc_gpu, unschedulable, ready, name_key; a missing column is NULL; "reset" is not read here)."""
+        alloc_mem_bytes, alloc_gpu, unschedulable, ready, name_key, creation; a missing column is NULL; "reset" is not read
+        here)."""
         col = {k: _np(delta.get(k), t) for k, t in _NT_DELTA_COLS.items()}
         d = gp_node_delta(n_write=0 if col["node_id"] is None else len(col["node_id"]), **{k: _p(v) for k, v in col.items()})
         self._check(load().gp_node_table_update(self._h, C.byref(d)))
@@ -1493,6 +1505,46 @@ class GangPacker:
         nt = _node_table_nodes(**nodes)
         return self._reschedule(_node_table_entry(load().gp_reschedule_from_reservations_node_table), nt, exe, min_frag, hosting,
                                 None, int(nt.n_zones), None, None, None, None, keep_topology_zone, topology_zone)
+
+    def reconcile_find_nodes_node_table(self, nodes: dict, apps: dict, n_groups: int, instance_group_missing: int, exec_cap=None,
+                                        want_avail=True):
+        """reconcile_find_nodes_resident with the node columns from the node and label tables
+        (gp_reconcile_find_nodes_node_table): nodes as in prepare_cluster_groups_node_table (is_driver_candidate and the rank
+        keys ignored); the instance group of a node is the index of its instance_group_key value in instance_group_value, a
+        node without the label is in instance_group_missing (the group of ""), and every node in 0 without instance_group_key.
+        Returns what reconcile_find_nodes_resident returns on the equivalent columns."""
+        if int(nodes.get("instance_group_key", -1)) >= 0 and len(nodes.get("instance_group_value", ())) != int(n_groups):
+            raise ValueError("instance_group_value must list exactly n_groups value ids (the call reads n_groups of them)")
+        nt = _node_table_nodes(**nodes)
+
+        def fn(h, nt_ref, nd_ref, *rest):
+            return load().gp_reconcile_find_nodes_node_table(h, nt_ref, int(n_groups), int(instance_group_missing), *rest)
+        return self._reconcile(fn, nt, None, None, apps, n_groups, None, None, exec_cap, want_avail)
+
+    def exceeds_cluster_capacity_node_table(self, nodes: dict, apps: dict, packer: int, node_group=None, n_groups=1) -> np.ndarray:
+        """exceeds_cluster_capacity_resident with allocatable from the node table, zone_id from the label table and
+        overhead_node_id from nodes (gp_exceeds_cluster_capacity_node_table); reservation_id may be omitted."""
+        q = len(apps["count"])
+        nt = _node_table_nodes(**dict({"reservation_id": None}, **nodes))
+        grp = _np(node_group, np.int32)
+        a = _apps(apps, None, group=apps.get("group"))
+        out = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity_node_table(self._h, C.byref(nt), _p(grp), int(n_groups), C.byref(a), int(packer),
+                                                                  _p(out)))
+        return out[:q]
+
+    def exceeds_cluster_capacity_affinity_node_table(self, nodes: dict, enc: dict, apps: dict, packer: int):
+        """exceeds_cluster_capacity_affinity_label_table with allocatable, zone_id and the label rows from nodes
+        (gp_exceeds_cluster_capacity_affinity_node_table); enc as in match_node_affinity_resident."""
+        q = len(apps["count"])
+        nt = _node_table_nodes(**dict({"reservation_id": None}, **nodes))
+        aff = _programs(enc)
+        a = _apps(apps, None, group=apps.get("group"))
+        out = np.full(max(q, 1), 255, np.uint8)
+        err = np.full(max(q, 1), 255, np.uint8)
+        self._check(load().gp_exceeds_cluster_capacity_affinity_node_table(self._h, C.byref(nt), C.byref(aff), C.byref(a), int(packer),
+                                                                           _p(out), _p(err)))
+        return out[:q], err[:q]
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)

@@ -1,15 +1,18 @@
 """The resident node table (gp_node_table_* of include/gangpack.h) from the node informer's events, and the per-call columns
 a node-table Predicate stands for.
 
-NodeTable keeps, per node, what the device's node table holds: allocatable, Spec.Unschedulable, the NodeReady condition and
-name_key, an order key of the node's name.  Node ids are those of an affinity.LabelTable, so one node event feeds both
+NodeTable keeps, per node, what the device's node table holds: allocatable, Spec.Unschedulable, the NodeReady condition,
+the creation time (metav1.Time as UnixNano, the failover reconciler's newest-first order) and name_key, an order key of the
+node's name.  Node ids are those of an affinity.LabelTable, so one node event feeds both
 tables.  name_key is strictly increasing in the byte order of the names: a new name takes the midpoint of its neighbours'
 keys, and when no gap is left every present node is relabelled with evenly spaced keys in one delta.  The device recomputes
 each row's dense rank from the keys, so no Predicate sorts names.
 
 label_columns() decodes zone, instance group and the two label priority ranks from an affinity.LabelMirror with the
 reference's rules (resources.go:78-81 for the zone and its "default" placeholder, nodesorting.go:161-189 for the ranks), and
-label_args() builds the per-call arguments of the node-table entries from the label strings.
+label_args() builds the per-call arguments of the node-table entries from the label strings.  reconcile_groups() and
+reconcile_label_args() do the same for the failover reconciler's instance groups, instanceGroup(n.Labels[label]), where a
+node without the label is in the group of "".
 """
 from __future__ import annotations
 
@@ -21,12 +24,12 @@ ZONE_LABEL = "failure-domain.beta.kubernetes.io/zone"
 DEFAULT_ZONE = "default"
 
 
-_ABSENT = (False, 0, 0, 0, False, False, 0)
+_ABSENT = (False, 0, 0, 0, False, False, 0, 0)
 
 
 class NodeTable:
-    """Every node's allocatable, unschedulable and ready flags and name order, as the resident node table keeps them:
-    set_node(name, allocatable, unschedulable, ready) for an add or an update (after the label table's set_node, which
+    """Every node's allocatable, unschedulable and ready flags, creation time and name order, as the resident node table keeps
+    them: set_node(name, allocatable, unschedulable, ready, creation) for an add or an update (after the label table's set_node, which
     gives the node its id; nothing changes when the values are the same), delete_node(name) (before the label table's
     delete_node, which frees the id).
 
@@ -41,6 +44,7 @@ class NodeTable:
         self.size = dict(n_node_ids=n_node_ids)
         self._key_hi = 1 << key_bits
         self.nodes = {}                                 # name -> (cpu, mem, gpu, unschedulable, ready)
+        self.creation = {}                              # name -> creation time (UnixNano)
         self._id, self._key = {}, {}                    # name -> node id, name -> name_key
         self._name_at = {}                              # node id -> name
         self._sorted = []                               # the present names' bytes, ascending
@@ -51,7 +55,7 @@ class NodeTable:
         self.mirror = NodeMirror()
 
     # ---- events
-    def set_node(self, name, allocatable, unschedulable, ready):
+    def set_node(self, name, allocatable, unschedulable, ready, creation=0):
         at = self.labels._node.get(name)
         if at is None:
             raise KeyError(f"node {name!r} has no label-table id: LabelTable.set_node first")
@@ -63,11 +67,12 @@ class NodeTable:
         cpu, mem = int(allocatable[0]), int(allocatable[1])
         gpu = int(allocatable[2]) if len(allocatable) > 2 and allocatable[2] is not None else 0
         row = (cpu, mem, gpu, bool(unschedulable), bool(ready))
-        if self.nodes.get(name) == row and self._id.get(name) == at:
+        if self.nodes.get(name) == row and self.creation.get(name) == int(creation) and self._id.get(name) == at:
             return
         if name not in self._id:
             self._insert(name)
         self.nodes[name] = row
+        self.creation[name] = int(creation)
         self._id[name] = at
         self._name_at[at] = name
         self._dirty.add(at)
@@ -76,7 +81,7 @@ class NodeTable:
         at = self._id.pop(name, None)
         if at is None:
             return
-        del self.nodes[name], self._name_at[at], self._key[name]
+        del self.nodes[name], self.creation[name], self._name_at[at], self._key[name]
         b = name.encode()
         del self._sorted[bisect.bisect_left(self._sorted, b)]
         self._dirty.add(at)
@@ -111,7 +116,7 @@ class NodeTable:
              "present": np.array([r[0] for r in rec], np.uint8), "alloc_cpu_milli": np.array([r[1] for r in rec], np.int64),
              "alloc_mem_bytes": np.array([r[2] for r in rec], np.int64), "alloc_gpu": np.array([r[3] for r in rec], np.int64),
              "unschedulable": np.array([r[4] for r in rec], np.uint8), "ready": np.array([r[5] for r in rec], np.uint8),
-             "name_key": np.array([r[6] for r in rec], np.int64)}
+             "name_key": np.array([r[6] for r in rec], np.int64), "creation": np.array([r[7] for r in rec], np.int64)}
         self._dirty = set()
         self._replay = False
         return d
@@ -135,7 +140,9 @@ class NodeTable:
     def _record(self, at):
         """the row of node id `at` as a delta writes it"""
         nm = self._name_at.get(at)
-        return _ABSENT if nm is None else (True, *self.nodes[nm][:3], *self.nodes[nm][3:], self._key[nm])
+        if nm is None:
+            return _ABSENT
+        return (True, *self.nodes[nm], self._key[nm], self.creation[nm])
 
     @staticmethod
     def _push(packer, d):
@@ -182,6 +189,7 @@ class NodeMirror:
             self.unschedulable = np.zeros(R, np.uint8)
             self.ready = np.zeros(R, np.uint8)
             self.name_key = np.zeros(R, np.int64)
+            self.creation = np.zeros(R, np.int64)
         ids = np.asarray(d["node_id"], np.int64)
         on = np.asarray(d["present"], np.uint8) != 0
         self.present[ids] = on
@@ -190,6 +198,8 @@ class NodeMirror:
         self.unschedulable[ids] = np.where(on, np.asarray(d["unschedulable"], np.uint8) != 0, 0)
         self.ready[ids] = np.where(on, np.asarray(d["ready"], np.uint8) != 0, 0)
         self.name_key[ids] = np.where(on, np.asarray(d["name_key"], np.int64), 0)
+        cre = d.get("creation")
+        self.creation[ids] = np.where(on, np.asarray(cre, np.int64), 0) if cre is not None else 0
         keys = np.where(self.present, self.name_key, np.iinfo(np.int64).max)
         order = np.lexsort((np.arange(len(keys)), keys))
         self.name_rank = np.full(len(keys), -1, np.int32)
@@ -198,14 +208,14 @@ class NodeMirror:
 
     def to_columns(self, node_table_id) -> dict:
         """the per-call columns of the listed nodes: alloc (cpu, mem, gpu), name_rank (a permutation of 0..n-1 in the order
-        of the table's ranks), unschedulable, ready"""
+        of the table's ranks), unschedulable, ready, creation"""
         ids = np.asarray(node_table_id, np.int64)
         if not self.present[ids].all():
             raise ValueError("a listed node is not in the node table")
         rank = np.empty(len(ids), np.int32)
         rank[np.argsort(self.name_rank[ids], kind="stable")] = np.arange(len(ids), dtype=np.int32)
         return dict(alloc=tuple(self.alloc[d, ids].copy() for d in range(3)), name_rank=rank,
-                    unschedulable=self.unschedulable[ids].copy(), ready=self.ready[ids].copy())
+                    unschedulable=self.unschedulable[ids].copy(), ready=self.ready[ids].copy(), creation=self.creation[ids].copy())
 
 
 def _value_of(mirror, ids, key):
@@ -282,3 +292,31 @@ def label_args(labels, zones=None, zone_label=ZONE_LABEL, instance_group_label=N
         if pr is not None:
             args.update({f"{pfx}_rank_key": max(key(pr[0]), 0), f"{pfx}_rank_value": vals(pr[1])})
     return args
+
+
+def reconcile_groups(mirror, node_table_id, instance_group_key=-1, instance_group_value=None, instance_group_missing=-1, **_):
+    """The failover reconciler's instance group of each listed node, as gp_reconcile_find_nodes_node_table reads it from an
+    affinity.LabelMirror: the index of its instance_group_key value in instance_group_value, instance_group_missing (the
+    group of "") for a node without the label, 0 for every node with instance_group_key -1.  A group the call would refuse
+    (a value not listed, or a missing label with instance_group_missing -1) raises ValueError."""
+    ids = np.asarray(node_table_id, np.int64)
+    if instance_group_key < 0:
+        return np.zeros(len(ids), np.int32)
+    v = _value_of(mirror, ids, instance_group_key)
+    g = np.where(v < 0, instance_group_missing, _index_of(v, instance_group_value)).astype(np.int32)
+    if (g < 0).any():
+        raise ValueError("an instance-group label value not in instance_group_value, or a node without the label "
+                         "(instance_group_missing = -1)")
+    return g
+
+
+def reconcile_label_args(labels, instance_group_label, instance_groups) -> dict:
+    """The instance-group arguments of reconcile_find_nodes_node_table from the strings: instance_groups, the label values
+    in instance-group order; "" (the group of a node without the label) is appended when not listed.  -> dict(
+    instance_group_key, instance_group_value, instance_group_missing, n_groups)."""
+    groups = list(instance_groups)
+    if "" not in groups:
+        groups.append("")
+    args = label_args(labels, instance_group_label=instance_group_label, instance_groups=groups)
+    return dict(instance_group_key=args["instance_group_key"], instance_group_value=args["instance_group_value"],
+                instance_group_missing=groups.index(""), n_groups=len(groups))
