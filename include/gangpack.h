@@ -1330,6 +1330,97 @@ gp_status gp_exceeds_cluster_capacity_affinity_node_table(gp_ctx* ctx, const gp_
                                                           gp_binpacker packer, uint8_t* exceeds /* [n_apps] */,
                                                           uint8_t* affinity_error /* [n_apps] or NULL */);
 
+/* ---- the resident driver table (pending drivers from the pod informer) --------------------------------------------------
+ * Every pending, parseable driver pod kept on the device and changed only by deltas from pod events, so that a FIFO
+ * Predicate no longer lists, sorts, parses and uploads the queue of earlier drivers (ListEarlierDrivers, EXT/sparkpods.go:54-71;
+ * sparkResources and shouldSkipDriverFifo, EXT/resource.go:224-270).  One row per slot; the host interns instance-group names
+ * (FindInstanceGroupFromPodSpec) and Spec.SchedulerName into dense ids.  A row holds: present, creation (CreationTimestamp as
+ * UnixNano), scheduler, group (-1: no instance group found -- MatchPodInstanceGroup is then false for every pair), the six
+ * quantities of sparkResources, min_executor_count (MinExecutorCount, the only count that packs) and exact (0: a quantity lies
+ * outside the exact-int64 model).  The host writes only pending drivers whose annotations parse: a driver that is bound,
+ * deleted, carries a DeletionTimestamp or no longer parses is cleared (EXT/resource.go:232-237 skips it).  The table belongs to
+ * the context (freed by gp_destroy); updates change no snapshot, layout, schedulable resources, held orders or statistics. */
+typedef struct {
+    int32_t n_slots;                 /* rows */
+    int32_t n_groups;                /* instance-group ids 0 .. n_groups-1 */
+    int32_t n_schedulers;            /* scheduler ids 0 .. n_schedulers-1 */
+    int32_t reserved;
+} gp_driver_table_size;
+/* Replace the context's driver table with an empty one (no row present).  GP_ERR_INVALID: NULL size or a negative capacity
+ * (the table held before is kept).  After a CUDA error the context holds no table. */
+gp_status gp_driver_table_reset(gp_ctx* ctx, const gp_driver_table_size* size);
+
+typedef struct {
+    int32_t n_write;                 /* whole-slot writes */
+    int32_t reserved;
+    const int32_t* slot;             /* [n_write] distinct slots < n_slots */
+    const uint8_t* present;          /* [n_write] 0: the slot is cleared (the other columns are ignored) */
+    const int64_t* creation;         /* [n_write] CreationTimestamp as UnixNano */
+    const int32_t* scheduler;        /* [n_write] in [0, n_schedulers) on present rows */
+    const int32_t* group;            /* [n_write] in [-1, n_groups) on present rows */
+    const int64_t* drv_cpu_milli;    /* [n_write] as gp_apps' columns; negative values are kept (the pack refuses them) */
+    const int64_t* drv_mem_bytes;
+    const int64_t* drv_gpu;          /* or NULL (= 0) */
+    const int64_t* exe_cpu_milli;
+    const int64_t* exe_mem_bytes;
+    const int64_t* exe_gpu;          /* or NULL (= 0) */
+    const int32_t* min_executor_count;
+    const uint8_t* exact;            /* [n_write] 0: a quantity is outside the exact-int64 model (the row queues, but a queue that
+                                        selects it is refused with GP_ERR_UNREPRESENTABLE) */
+} gp_driver_delta;
+/* Apply one delta.  The whole delta is checked on the device before anything is written: a refused delta leaves the table
+ * exactly as it was.  One stream synchronise.  GP_ERR_INVALID: no table (gp_driver_table_reset first), missing arrays or a
+ * negative count; a slot out of range or given twice; on a present row a scheduler or group out of range.
+ * GP_ERR_UNREPRESENTABLE: |quantity| >= 2^61 on a present row with exact = 1.  A refusal, or a CUDA error while the delta is
+ * staged, leaves the table as it was; a CUDA error once the update writes the table leaves no table (GP_ERR_INVALID "no
+ * driver table" until the next reset), and the caller resets and replays. */
+gp_status gp_driver_table_update(gp_ctx* ctx, const gp_driver_delta* delta);
+
+/* The FIFO queue one call selects from the driver table and orders on the device, and the gp_apps it packs.
+ *   Predicate form (requesting_slot >= 0): selectDriverNode's ListEarlierDrivers + fitEarlierDrivers + the driver's own
+ *     pack.  The queue is the present rows with the requesting row's scheduler, its group (group != -1) and a creation
+ *     strictly below the requesting row's, ordered by (creation, slot); then the requesting row itself with skip_if_no_fit 0.
+ *     Every entry packs in snapshot group predicate_group.  The requesting driver's driver_node is then -2
+ *     (failure-earlier-driver), -1 (failure-fit) or its driver node.
+ *   Drain form (requesting_slot = -1): every present row with scheduler `scheduler` and snapshot_group[row.group] >= 0, in
+ *     snapshot group snapshot_group[row.group], ordered by (snapshot group, creation, slot).
+ * skip_if_no_fit of a queued row = creation + enforce_after_ns[row.group] > now_unix_nano (shouldSkipDriverFifo), evaluated
+ * exactly (no overflow; a negative age is allowed).  Equal creation times (whole seconds in the API) leave the reference's
+ * sort.Slice order undefined: ties are broken by slot, and undefined_ties counts the adjacent entries of one queue with equal
+ * creation (a shim that wants the reference's own unspecified order falls back to Go).
+ * Outputs: queue_slot[i] = the slot of entry i, exec_out_off [n_queued + 1] = its ExecutorNodes offsets (the prefix sum of
+ * max(min_executor_count, 0)), *n_queued and *n_executors (= exec_out_off[n_queued]).
+ * Refusals, all before any pack work and changing nothing (the outputs above excepted): GP_ERR_INVALID for an absent requesting
+ * slot; GP_ERR_UNREPRESENTABLE for a queued row with exact = 0; GP_ERR_CAPACITY when n_queued > queue_cap or n_executors >
+ * executor_nodes_cap -- *n_queued and *n_executors then hold the sizes needed, so the caller can grow its buffers and retry. */
+typedef struct {
+    int32_t requesting_slot;         /* >= 0: Predicate form; -1: drain form */
+    int32_t scheduler;               /* drain form: the scheduler id drained (Predicate form: ignored, the requesting row's) */
+    int32_t predicate_group;         /* Predicate form: the snapshot group of every entry (normally 0) */
+    int32_t queue_cap;               /* entries of queue_slot and of the results' driver_node */
+    const int32_t* snapshot_group;   /* drain form: [n_groups] the snapshot group of each table group, -1 = not drained */
+    const int64_t* enforce_after_ns; /* [n_groups] the FIFO age of each table group (DefaultEnforceAfterPodAge unless overridden) */
+    int64_t now_unix_nano;
+    int32_t* queue_slot;             /* out [queue_cap] */
+    int64_t* exec_out_off;           /* out [queue_cap + 1], or NULL */
+    int32_t* n_queued;               /* out */
+    int64_t* n_executors;            /* out, or NULL */
+    int32_t* undefined_ties;         /* out, or NULL */
+} gp_driver_queue;
+/* gp_pack_batch(algo GP_TIGHTLY_PACK / GP_DISTRIBUTE_EVENLY, mode GP_MODE_FIFO_REFERENCE / GP_MODE_FIFO_EXACT) on the queue,
+ * over the held snapshot: driver_node [n_queued] and ExecutorNodes by exec_out_off, status, gp_last_error category, gp_last_stats
+ * and the snapshot left behind are what gp_pack_batch returns on the gp_apps the host would build from the same rows.  The
+ * driver table is read in place and left unchanged.  Checks: gp_pack_batch's argument checks; snapshot_group (drain form) and
+ * predicate_group outside [-1, snapshot groups) resp. [0, snapshot groups) are GP_ERR_INVALID; then the refusals above.  One
+ * stream synchronise after the queue stage (count, executor total and refusal word), one after the pack. */
+gp_status gp_pack_fifo_driver_table(gp_ctx* ctx, const gp_driver_queue* queue, gp_algo algo, gp_mode mode, gp_results* out);
+/* gp_pack_fifo_zones_groups(groups == NULL) on the queue: the snapshot groups are the instance groups of the layout
+ * gp_prepare_cluster_zones_groups[_node_table] left; zone, driver_node, ExecutorNodes, avg_efficiency, status, statistics and
+ * the snapshot left behind are what that entry returns on the host-built gp_apps.  Checks as gp_pack_fifo_zones_groups', with
+ * the snapshot-group ranges of gp_pack_fifo_driver_table, then the queue refusals. */
+gp_status gp_pack_fifo_zones_groups_driver_table(gp_ctx* ctx, const gp_driver_queue* queue, gp_binpacker packer, gp_mode mode,
+                                                 const gp_instance_groups* groups /* must be NULL */, gp_zone_results* out);
+
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets
  * that process use every GPU: one gp_ctx + one worker thread per entry of `devices` (an ordinal may repeat).

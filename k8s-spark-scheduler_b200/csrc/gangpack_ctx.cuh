@@ -248,6 +248,16 @@ struct gp_ctx {
         uint32_t seq = 0;                         // the last update's stamp
     } nt;
 
+    // the resident driver table (gangpack_driver_table.cu); read by the *_driver_table entries, changed only by its own
+    struct DriverTable {
+        bool live = false;                        // reset and not broken by a CUDA error since
+        gp_driver_table_size size{};
+        DevBuf cols;                              // present, exact, creation, scheduler, group, quantities [6], count, stamps in one block
+        DevBuf queue;                             // the queue one *_driver_table call selects, orders and packs, and its scratch
+        uint32_t seq = 0;                         // the last update's stamp
+        bool sort_attr_set = false;               // dynamic shared-memory opt-in of gp_sort_tiles<QueueKey> done on this device
+    } dt;
+
     gp_stats last{};
 };
 
@@ -456,3 +466,26 @@ gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* 
 gp_status nt_refusal(gp_ctx* c, int word, const char* who);
 // After the entry's synchronise: the optional zone_id_out / instance_group_out copies
 gp_status nt_outputs(gp_ctx* c, const gp_node_table_nodes* nodes, const NtGathered& g);
+
+// ---- gangpack_zones.cu -----------------------------------------------------------------------------------------------
+
+// The applications of one zone FIFO drain: host columns to upload (host, with group = their instance groups or NULL and off
+// = the offsets), or (host NULL) device columns already in instance-group order, queue order within each: q[6] the six
+// quantities (NULL = 0), count, off, skip and queue = the identity over the applications.
+struct ZoneFifoApps {
+    const gp_apps* host;
+    const int32_t* group;
+    const int64_t* off;
+    const int64_t* q[6];
+    const int32_t* count;
+    const uint8_t* skip;
+    const int32_t* queue;
+};
+// gp_pack_fifo_zones_groups' packer and mode checks: kind = GP_TIGHTLY_PACK / GP_MINIMAL_FRAGMENTATION / kZoneAzAware
+gp_status zone_fifo_kind(gp_ctx* c, gp_binpacker packer, gp_mode mode, const char* who, int* kind);
+// The layout gp_prepare_cluster_zones_groups left (groups == NULL), checked for the packer kind
+gp_status held_groups_layout(gp_ctx* c, int kind, const char* who, gp_instance_groups* held);
+// The zone FIFO drain over Q applications with `total` ExecutorNodes entries; c->zone_groups [n_instance_groups] holds each
+// instance group's application count in q_end and its largest exe_count in row_pitch
+gp_status fifo_zones_body(gp_ctx* c, int32_t Q, int64_t total, const ZoneFifoApps& src, int kind, gp_mode mode,
+                          const gp_instance_groups& ig, bool az_dev, gp_zone_results* out, const char* who);

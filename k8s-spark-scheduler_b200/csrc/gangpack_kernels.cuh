@@ -385,6 +385,8 @@ struct GatherSlots {
     int32_t ne, nd;
 };
 
+constexpr int kZoneAzAware = 3;               // ALGO of az-aware-tightly-pack (0 and 2 are the single-AZ packers)
+
 // One instance group of the zone FIFO loop (gp_pack_fifo_zones_cta, gangpack_zonefifo.cuh): CTA b runs the b-th
 struct ZoneFifoGroup {
     int64_t row_base;                 // its scratch rows start at entry row_base of the row arrays

@@ -37,7 +37,6 @@ namespace gp {
 constexpr int kZoneFifoWarps = 16;
 constexpr int kZoneFifoThreads = kZoneFifoWarps * 32;
 constexpr int kZoneFifoMaxZones = 64;
-constexpr int kZoneAzAware = 3;               // ALGO of az-aware-tightly-pack (0 and 2 are the single-AZ packers)
 
 struct ZoneFifoIn {
     const long long* sched[3];        // SchedulableResources, node-table order (gpu may be NULL = 0)

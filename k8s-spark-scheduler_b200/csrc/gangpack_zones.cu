@@ -286,17 +286,136 @@ static gp_status held_az_orders(gp_ctx* c, const gp_apps* a, const gp_zone_resul
     return GP_OK;
 }
 
+}  // extern "C"
+
+gp_status zone_fifo_kind(gp_ctx* c, gp_binpacker packer, gp_mode mode, const char* who, int* kind) {
+    if (packer == GP_BP_SINGLE_AZ_TIGHTLY_PACK) *kind = GP_TIGHTLY_PACK;
+    else if (packer == GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) *kind = GP_MINIMAL_FRAGMENTATION;
+    else if (packer == GP_BP_AZ_AWARE_TIGHTLY_PACK) *kind = kZoneAzAware;
+    else return fail(c, GP_ERR_INVALID, who, "packer must be GP_BP_SINGLE_AZ_TIGHTLY_PACK, GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION or "
+                                             "GP_BP_AZ_AWARE_TIGHTLY_PACK");
+    if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
+        return fail(c, GP_ERR_INVALID, who, "mode must be one of the FIFO modes");
+    return require(c, c->held.full_sched(), who);
+}
+
 // The FIFO loop over zones in one launch (gangpack_zonefifo.cuh), one CTA per instance group of `ig` (already validated),
 // shared by gp_pack_fifo_zones (kind = 0 tightly-pack, 2 minimal-fragmentation; one instance group whose zones are every
 // snapshot group), gp_pack_fifo_az_aware (kind = kZoneAzAware; one instance group, zones 0..n_zones-1, plus the undivided
-// orders of the fallback; az_dev: they are device arrays) and gp_pack_fifo_zones_groups (either, per instance group).
-// group: the instance group of every application, NULL = 0.  Argument checks common to all three are here.
+// orders of the fallback; az_dev: they are device arrays), gp_pack_fifo_zones_groups (either, per instance group) and
+// gp_pack_fifo_zones_groups_driver_table (its columns on the device).  c->zone_groups holds, per instance group, its
+// application count in q_end and its largest exe_count in row_pitch; total = the ExecutorNodes entries.
+gp_status fifo_zones_body(gp_ctx* c, int32_t Q, int64_t total, const ZoneFifoApps& src, int kind, gp_mode mode,
+                          const gp_instance_groups& ig, bool az_dev, gp_zone_results* out, const char* who) {
+    const bool azk = kind == kZoneAzAware;
+    const int32_t G = ig.n_instance_groups;
+    const gp_apps* a = src.host;
+    std::vector<ZoneFifoGroup>& grp = c->zone_groups;
+    if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, who, "executor_nodes_cap too small");
+    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, who, "executor_nodes is NULL");
+    // per instance group: its zones, its queue range and its scratch rows (n_zones, az-aware: + the fallback row)
+    int32_t qb = 0;
+    int64_t rows = 0;
+    for (int32_t b = 0; b < G; ++b) {
+        ZoneFifoGroup& g = grp[(size_t)b];
+        g.zone0 = ig.group_off[b];
+        g.n_zones = azk ? ig.n_zones[b] : ig.group_off[b + 1] - ig.group_off[b];
+        const int32_t n = g.q_end;
+        g.q_begin = g.q_end = qb;                          // q_end: the cursor of the fill below
+        qb += n;
+        g.row_pitch = (std::max<int64_t>(g.row_pitch, 1) + 3) & ~(int64_t)3;
+        g.row_base = rows;
+        rows += (int64_t)(g.n_zones + (azk ? 1 : 0)) * g.row_pitch;
+        if (azk) {
+            g.e0 = ig.exec_off[b]; g.ne = ig.exec_off[b + 1] - g.e0;
+            g.d0 = ig.drv_off[b]; g.nd = ig.drv_off[b + 1] - g.d0;
+        }
+    }
+    std::vector<int32_t>& queue = c->zone_queue;
+    if (a) {                                                // stable counting sort of the applications by instance group
+        queue.resize((size_t)Q);
+        for (int32_t i = 0; i < Q; ++i) queue[(size_t)grp[(size_t)(src.group ? src.group[i] : 0)].q_end++] = i;
+    } else {                                                // device columns: already in instance-group order (src.queue)
+        for (int32_t b = 0; b < G; ++b) grp[(size_t)b].q_end = b + 1 < G ? grp[(size_t)b + 1].q_begin : qb;
+    }
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)rows, qh = a ? q : 0;
+    Arena ar{c->zonebuf, st};
+    const auto in = ar.take<int64_t>(6 * qh);
+    const auto cnt = ar.take<int32_t>(qh);
+    const auto off_p = ar.take<int64_t>(a ? q + 1 : 0);
+    const auto skip = ar.take<uint8_t>(qh);
+    const auto gdesc = ar.take<ZoneFifoGroup>((size_t)G);
+    const auto qidx = ar.take<int32_t>(qh);
+    const auto rexe = ar.take<int32_t>(RP);
+    const auto rlist = ar.take<int2>(kind == GP_MINIMAL_FRAGMENTATION ? RP : 0);
+    const auto zone = ar.take<int32_t>(q), drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1);
+    const auto avg_p = ar.take<double>(4 * q);
+    ar.reserve();
+    GP_TRY(ar.check(c));
+    int2* unused = nullptr;
+    GP_TRY(pack_begin(c, Q, GP_TIGHTLY_PACK, mode, total, false, &unused, st));
+    AppColumns cols{};
+    SixCols six{};
+    for (int k = 0; k < 6; ++k) six.p[k] = src.q[k];
+    const int32_t* d_cnt = src.count;
+    const int64_t* d_off = src.off;
+    const uint8_t* d_skip = src.skip;
+    const int32_t* d_queue = src.queue;
+    if (a) {
+        six = upload_app_columns(ar, a, src.off, in, cnt, off_p);
+        d_cnt = ar.ptr(cnt); d_off = ar.ptr(off_p);
+        d_skip = ar.put(skip, a->skip_if_no_fit);
+        d_queue = ar.put(qidx, queue.data());
+    }
+    ar.put(gdesc, grp.data());
+    GP_TRY(ar.check(c));
+    for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
+    cols.count = d_cnt; cols.group = nullptr; cols.off = d_off; cols.bits = 64; cols.mem_shift = 0;
+    DevStatus* ds = c->status();
+    unsigned long long* d_stats = ds->head.stats;
+    PrepApp* prep = c->prep.as<PrepApp>();
+    gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
+        Q, cols, d_skip, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, &ds->head.err, &c->host_status()->err_word);
+    Snapshot snap = make_snapshot(c);
+    ZoneFifoIn zi{};
+    const size_t N = (size_t)c->n_nodes;
+    zi.sched[0] = c->sched.as<long long>(); zi.sched[1] = c->sched.as<long long>() + N; zi.sched[2] = c->sched.as<long long>() + 2 * N;
+    zi.node_slot = c->node_slot.as<int32_t>();
+    zi.row_exec = ar.ptr(rexe);
+    zi.row_list = kind == GP_MINIMAL_FRAGMENTATION ? ar.ptr(rlist) : nullptr;
+    zi.groups = ar.ptr(gdesc); zi.queue = d_queue;
+    double* avg = out->avg_efficiency ? ar.ptr(avg_p) : nullptr;
+    int32_t* zo = ar.ptr(zone); int32_t* dq = ar.ptr(drv); int32_t* eo = ar.ptr(exe);
+    GatherSlots fb{};
+    if (azk) GP_TRY(stage_fallback_view(c, ig, az_dev, st, &fb));
+    const unsigned ctas = (unsigned)G;                 // one per instance group
+    if (kind == GP_TIGHTLY_PACK) {
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+        else gp_pack_fifo_zones_cta<0, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+    } else if (kind == GP_MINIMAL_FRAGMENTATION) {
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<2, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+        else gp_pack_fifo_zones_cta<2, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
+    } else {
+        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<kZoneAzAware, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
+        else gp_pack_fifo_zones_cta<kZoneAzAware, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
+    }
+    GP_CUDA(c, cudaGetLastError());
+    c->last.kernel_launches += 2;
+    GP_TRY(refresh_views(c, st));                       // the compact view follows the charged slots
+    return finish_zone_results(c, ar, out, zone, drv, exe, avg_p, T);
+}
+
+extern "C" {
+
+// fifo_zones_body over host columns.  group: the instance group of every application, NULL = 0.  Argument checks common to
+// gp_pack_fifo_zones, gp_pack_fifo_az_aware and gp_pack_fifo_zones_groups are here.
 static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, const int32_t* group, int kind, gp_mode mode, const gp_instance_groups& ig,
                                 bool az_dev, gp_zone_results* out, const char* who) {
     const int32_t Q = a->n_apps;
     if (Q == 0) return GP_OK;
     if (!has_zone_arrays(a, out)) return fail(c, GP_ERR_INVALID, who, "missing app/result arrays");
-    const bool azk = kind == kZoneAzAware;
     const int32_t G = ig.n_instance_groups;
     // one pass over the queue: ExecutorNodes offsets, and per instance group its application count (in q_end) and its
     // largest exe_count (in row_pitch)
@@ -318,88 +437,9 @@ static gp_status fifo_zones_run(gp_ctx* c, const gp_apps* a, const int32_t* grou
     if (a->exec_out_off)
         for (int32_t i = 0; i <= Q; ++i)
             if (a->exec_out_off[i] != hoff[(size_t)i]) return fail(c, GP_ERR_INVALID, who, "exec_out_off must be the prefix sum of exe_count (or NULL)");
-    const int64_t total = acc;
-    if (total > out->executor_nodes_cap) return fail(c, GP_ERR_CAPACITY, who, "executor_nodes_cap too small");
-    if (total > 0 && !out->executor_nodes) return fail(c, GP_ERR_INVALID, who, "executor_nodes is NULL");
-    // per instance group: its zones, its queue range and its scratch rows (n_zones, az-aware: + the fallback row)
-    int32_t qb = 0;
-    int64_t rows = 0;
-    for (int32_t b = 0; b < G; ++b) {
-        ZoneFifoGroup& g = grp[(size_t)b];
-        g.zone0 = ig.group_off[b];
-        g.n_zones = azk ? ig.n_zones[b] : ig.group_off[b + 1] - ig.group_off[b];
-        const int32_t n = g.q_end;
-        g.q_begin = g.q_end = qb;                          // q_end: the cursor of the fill below
-        qb += n;
-        g.row_pitch = (std::max<int64_t>(g.row_pitch, 1) + 3) & ~(int64_t)3;
-        g.row_base = rows;
-        rows += (int64_t)(g.n_zones + (azk ? 1 : 0)) * g.row_pitch;
-        if (azk) {
-            g.e0 = ig.exec_off[b]; g.ne = ig.exec_off[b + 1] - g.e0;
-            g.d0 = ig.drv_off[b]; g.nd = ig.drv_off[b + 1] - g.d0;
-        }
-    }
-    std::vector<int32_t>& queue = c->zone_queue;            // stable counting sort of the applications by instance group
-    queue.resize((size_t)Q);
-    for (int32_t i = 0; i < Q; ++i) queue[(size_t)grp[(size_t)(group ? group[i] : 0)].q_end++] = i;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    cudaStream_t st = c->stream;
-    const size_t q = (size_t)Q, T = (size_t)total, RP = (size_t)rows;
-    Arena ar{c->zonebuf, st};
-    const auto in = ar.take<int64_t>(6 * q);
-    const auto cnt = ar.take<int32_t>(q);
-    const auto off_p = ar.take<int64_t>(q + 1);
-    const auto skip = ar.take<uint8_t>(q);
-    const auto gdesc = ar.take<ZoneFifoGroup>((size_t)G);
-    const auto qidx = ar.take<int32_t>(q);
-    const auto rexe = ar.take<int32_t>(RP);
-    const auto rlist = ar.take<int2>(kind == GP_MINIMAL_FRAGMENTATION ? RP : 0);
-    const auto zone = ar.take<int32_t>(q), drv = ar.take<int32_t>(q), exe = ar.take<int32_t>(T + 1);
-    const auto avg_p = ar.take<double>(4 * q);
-    ar.reserve();
-    GP_TRY(ar.check(c));
-    int2* unused = nullptr;
-    GP_TRY(pack_begin(c, Q, GP_TIGHTLY_PACK, mode, total, false, &unused, st));
-    AppColumns cols{};
-    const SixCols six = upload_app_columns(ar, a, hoff.data(), in, cnt, off_p);
-    const uint8_t* d_skip = ar.put(skip, a->skip_if_no_fit);
-    ar.put(gdesc, grp.data());
-    ar.put(qidx, queue.data());
-    GP_TRY(ar.check(c));
-    for (int k = 0; k < 6; ++k) cols.q[k] = six.p[k];
-    cols.count = ar.ptr(cnt); cols.group = nullptr; cols.off = ar.ptr(off_p); cols.bits = 64; cols.mem_shift = 0;
-    DevStatus* ds = c->status();
-    unsigned long long* d_stats = ds->head.stats;
-    PrepApp* prep = c->prep.as<PrepApp>();
-    gp_prep_apps<<<(Q + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, st>>>(
-        Q, cols, d_skip, c->n_groups, total, c->snap_flags.as<SnapMeta>(), nullptr, prep, &ds->head.err, &c->host_status()->err_word);
-    Snapshot snap = make_snapshot(c);
-    ZoneFifoIn zi{};
-    const size_t N = (size_t)c->n_nodes;
-    zi.sched[0] = c->sched.as<long long>(); zi.sched[1] = c->sched.as<long long>() + N; zi.sched[2] = c->sched.as<long long>() + 2 * N;
-    zi.node_slot = c->node_slot.as<int32_t>();
-    zi.row_exec = ar.ptr(rexe);
-    zi.row_list = kind == GP_MINIMAL_FRAGMENTATION ? ar.ptr(rlist) : nullptr;
-    zi.groups = ar.ptr(gdesc); zi.queue = ar.ptr(qidx);
-    double* avg = out->avg_efficiency ? ar.ptr(avg_p) : nullptr;
-    int32_t* zo = ar.ptr(zone); int32_t* dq = ar.ptr(drv); int32_t* eo = ar.ptr(exe);
-    GatherSlots fb{};
-    if (azk) GP_TRY(stage_fallback_view(c, ig, az_dev, st, &fb));
-    const unsigned ctas = (unsigned)G;                 // one per instance group
-    if (kind == GP_TIGHTLY_PACK) {
-        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<0, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-        else gp_pack_fifo_zones_cta<0, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-    } else if (kind == GP_MINIMAL_FRAGMENTATION) {
-        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<2, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-        else gp_pack_fifo_zones_cta<2, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats);
-    } else {
-        if (mode == GP_MODE_FIFO_REFERENCE) gp_pack_fifo_zones_cta<kZoneAzAware, 1><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
-        else gp_pack_fifo_zones_cta<kZoneAzAware, 2><<<ctas, kZoneFifoThreads, 0, st>>>(snap, prep, zi, zo, dq, eo, avg, d_stats, fb);
-    }
-    GP_CUDA(c, cudaGetLastError());
-    c->last.kernel_launches += 2;
-    GP_TRY(refresh_views(c, st));                       // the compact view follows the charged slots
-    return finish_zone_results(c, ar, out, zone, drv, exe, avg_p, T);
+    ZoneFifoApps src{};
+    src.host = a; src.group = group; src.off = hoff.data();
+    return fifo_zones_body(c, Q, acc, src, kind, mode, ig, az_dev, out, who);
 }
 
 // the FIFO loop with a single-AZ packer in one launch
@@ -435,16 +475,26 @@ gp_status gp_pack_fifo_az_aware(gp_ctx* c, const gp_apps* a, gp_mode mode, const
     return fifo_zones_run(c, a, nullptr, kZoneAzAware, mode, one.ig, held, out, "gp_pack_fifo_az_aware");
 }
 
+}  // extern "C"
+
 // gp_pack_fifo_zones_groups(groups == NULL): the layout gp_prepare_cluster_zones_groups left, from its host words and its
 // device orders (built by the library: no order check)
-static gp_status held_groups_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, gp_zone_results* out, const char* who) {
+gp_status held_groups_layout(gp_ctx* c, int kind, const char* who, gp_instance_groups* held) {
     const bool azk = kind == kZoneAzAware;
     GP_TRY(require(c, c->held.groups_layout(azk), who));
-    const gp_instance_groups held = c->held.groups();
-    for (int32_t b = 0; b < held.n_instance_groups; ++b)
-        if ((azk ? held.n_zones[b] : held.group_off[b + 1] - held.group_off[b]) > kZoneFifoMaxZones)
+    *held = c->held.groups();
+    for (int32_t b = 0; b < held->n_instance_groups; ++b)
+        if ((azk ? held->n_zones[b] : held->group_off[b + 1] - held->group_off[b]) > kZoneFifoMaxZones)
             return fail(c, GP_ERR_INVALID, who, "more than 64 candidate zones in an instance group");
-    return fifo_zones_run(c, a, a->group, kind, mode, held, azk, out, who);
+    return GP_OK;
+}
+
+extern "C" {
+
+static gp_status held_groups_run(gp_ctx* c, const gp_apps* a, int kind, gp_mode mode, gp_zone_results* out, const char* who) {
+    gp_instance_groups held{};
+    GP_TRY(held_groups_layout(c, kind, who, &held));
+    return fifo_zones_run(c, a, a->group, kind, mode, held, kind == kZoneAzAware, out, who);
 }
 
 // the FIFO loop of every instance group with a zone-aware packer, one CTA per instance group, in one launch
@@ -454,14 +504,7 @@ gp_status gp_pack_fifo_zones_groups(gp_ctx* c, const gp_apps* a, gp_binpacker pa
     if (!enter(c)) return GP_ERR_INVALID;
     GP_TRY(require(c, c->held.snapshot(), who));
     int kind;
-    if (packer == GP_BP_SINGLE_AZ_TIGHTLY_PACK) kind = GP_TIGHTLY_PACK;
-    else if (packer == GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) kind = GP_MINIMAL_FRAGMENTATION;
-    else if (packer == GP_BP_AZ_AWARE_TIGHTLY_PACK) kind = kZoneAzAware;
-    else return fail(c, GP_ERR_INVALID, who, "packer must be GP_BP_SINGLE_AZ_TIGHTLY_PACK, GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION or "
-                                             "GP_BP_AZ_AWARE_TIGHTLY_PACK");
-    if (mode != GP_MODE_FIFO_REFERENCE && mode != GP_MODE_FIFO_EXACT)
-        return fail(c, GP_ERR_INVALID, who, "mode must be one of the FIFO modes");
-    GP_TRY(require(c, c->held.full_sched(), who));
+    GP_TRY(zone_fifo_kind(c, packer, mode, who, &kind));
     if (!ig) {
         if (!a || !out || a->n_apps < 0) return fail(c, GP_ERR_INVALID, who, "NULL apps/results");
         return held_groups_run(c, a, kind, mode, out, who);

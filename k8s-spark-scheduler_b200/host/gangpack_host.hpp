@@ -11,6 +11,8 @@
 //   sort::NodeSorter::PotentialNodes              internal/sort/nodesorting.go:41-200
 //   extender::FitEarlierDrivers / SparkResourceUsage
 //        internal/extender/resource.go:224-262, internal/extender/sparkpods.go:139-146
+//   extender::ResidentDrivers / FitEarlierDriversDriverTable (pending drivers kept on the device, the FIFO step from them)
+//        internal/extender/sparkpods.go:45-137, internal/extender/resource.go:224-270
 //
 // Quantities are int64 (CPU millicores, memory bytes, GPU units) -- the exact-int64 model of
 // resource.Quantity.  There is no CPU packer here: if the device path fails the call throws
@@ -2842,6 +2844,259 @@ inline std::vector<ReconcileResult> ReconcileFindNodesNodeTable(const std::vecto
         rn[i].CreationUnixNano = c.creation[i];
     }
     return ReconcileFindNodesResident(rn, reservations, overhead, instanceGroupLabel, drivers);
+}
+
+// ---- the resident driver table (gp_driver_table_*) ------------------------------------------------------------------------
+
+// Every pending driver as the resident driver table keeps it, from the pod informer: SetDriver for a driver pod's add and
+// update events (a bound or terminating pod, or one whose annotations do not parse, is deleted: resource.go:232-237),
+// DeleteDriver for its delete.  Slots freed by a delete are reused, lowest first; scheduler names and instance groups are
+// interned into dense ids (no instance group: -1).  Flush sends the slots that differ from what the device holds as one
+// gp_driver_table_update, after a reset with doubled capacities and the whole state when a slot, group or scheduler id would
+// not fit (or after Replay, or a failed flush).  The host keeps every row, so a refused device call can fall back to
+// FilterToEarliestAndSort and the per-call FIFO batch over the same drivers (Pods, Pending).
+class ResidentDrivers {
+public:
+    explicit ResidentDrivers(gp_driver_table_size size = gp_driver_table_size{64, 4, 2, 0}) : size_(size) {}
+
+    void SetDriver(const QueuedDriverPod& pod, const std::map<std::string, std::string>& annotations) {
+        ParsedSparkResources r;
+        if (!pod.NodeName.empty() || pod.Deleting || !SparkResources(annotations, &r).empty()) {
+            DeleteDriver(pod.UID);
+            return;
+        }
+        Row row;
+        row.present = true;
+        row.creation = pod.CreationSeconds * 1000000000LL;
+        row.scheduler = intern(schedulers_, pod.SchedulerName);
+        row.group = pod.HasInstanceGroup ? intern(groups_, pod.InstanceGroup) : -1;
+        const int64_t q[6] = {r.DriverCPUMilli, r.DriverMemoryBytes, r.DriverNvidiaGPUs, r.ExecutorCPUMilli, r.ExecutorMemoryBytes,
+                              r.ExecutorNvidiaGPUs};
+        for (int k = 0; k < 6; ++k) row.q[k] = q[k];
+        row.count = (int32_t)r.MinExecutorCount;
+        row.exact = r.Exact;
+        auto it = held_.find(pod.UID);
+        if (it != held_.end() && it->second.row == row && it->second.pod.CreationSeconds == pod.CreationSeconds) return;
+        int32_t slot;
+        if (it != held_.end()) slot = it->second.slot;
+        else if (!free_.empty()) { slot = *free_.begin(); free_.erase(free_.begin()); }
+        else slot = next_++;
+        held_[pod.UID] = Held{slot, row, pod, r};
+        uidAt_[slot] = pod.UID;
+        dirty_.insert(slot);
+    }
+    void DeleteDriver(const std::string& uid) {
+        auto it = held_.find(uid);
+        if (it == held_.end()) return;
+        dirty_.insert(it->second.slot);
+        free_.insert(it->second.slot);
+        uidAt_.erase(it->second.slot);
+        held_.erase(it);
+    }
+
+    int32_t Slot(const std::string& uid) const { auto it = held_.find(uid); return it == held_.end() ? -1 : it->second.slot; }
+    bool Holds(const std::string& uid) const { return held_.count(uid) != 0; }
+    int Replays() const { return replays_; }
+    const gp_driver_table_size& Size() const { return size_; }
+    // enforce_after_ns of every group id: its instance group's override, else the default (DefaultEnforceAfterPodAge)
+    std::vector<int64_t> GroupAges(int64_t defaultNs, const std::map<std::string, int64_t>& overrides = {}) const {
+        std::vector<int64_t> ages((size_t)size_.n_groups, defaultNs);
+        for (const auto& g : groups_) {
+            auto o = overrides.find(g.first);
+            if (o != overrides.end()) ages[(size_t)g.second] = o->second;
+        }
+        return ages;
+    }
+    // the pending drivers as a lister lists them (slot order), and what fitEarlierDrivers reads off one of them
+    std::vector<QueuedDriverPod> Pods() const {
+        std::vector<QueuedDriverPod> out;
+        for (const auto& kv : uidAt_) out.push_back(held_.at(kv.second).pod);
+        return out;
+    }
+    PendingDriver Pending(const std::string& uid, bool skipIfNoFit) const {
+        const Held& h = held_.at(uid);
+        PendingDriver d;
+        d.Name = uid;
+        d.SkipIfNoFit = skipIfNoFit;
+        d.Resources.DriverResources = resources::CreateResources(h.parsed.DriverCPUMilli, h.parsed.DriverMemoryBytes, h.parsed.DriverNvidiaGPUs);
+        d.Resources.ExecutorResources = resources::CreateResources(h.parsed.ExecutorCPUMilli, h.parsed.ExecutorMemoryBytes, h.parsed.ExecutorNvidiaGPUs);
+        d.Resources.MinExecutorCount = (int)h.parsed.MinExecutorCount;
+        d.Resources.MaxExecutorCount = (int)h.parsed.MaxExecutorCount;
+        return d;
+    }
+    bool Exact(const std::string& uid) const { return held_.at(uid).row.exact; }
+    int32_t GroupID(const std::string& uid) const { return held_.at(uid).row.group; }
+
+    void Replay() { replay_ = true; ++replays_; }
+
+    void Flush(gangpack::Device& dev) {
+        auto grow = [&](int32_t& cap, int32_t need) { while (cap < need) { cap = std::max<int32_t>(2 * cap, 1); replay_ = true; } };
+        grow(size_.n_slots, next_);
+        grow(size_.n_groups, (int32_t)groups_.size());
+        grow(size_.n_schedulers, (int32_t)schedulers_.size());
+        std::vector<int32_t> slot, sched, group, count;
+        std::vector<uint8_t> present, exact;
+        std::vector<int64_t> creation, q[6];
+        auto row = [&](int32_t s) {
+            const Row r = record(s);
+            slot.push_back(s); present.push_back(r.present); exact.push_back(r.exact); creation.push_back(r.creation);
+            sched.push_back(r.scheduler); group.push_back(r.group); count.push_back(r.count);
+            for (int k = 0; k < 6; ++k) q[k].push_back(r.q[k]);
+        };
+        if (replay_) {
+            sent_.clear();
+            for (const auto& kv : uidAt_) row(kv.first);
+        } else {
+            for (int32_t s : dirty_) {
+                auto it = sent_.find(s);
+                if (!(record(s) == (it == sent_.end() ? Row{} : it->second))) row(s);
+            }
+        }
+        const bool reset = replay_;
+        replay_ = true;                            // until the table holds this state: a failed call replays next time
+        if (reset) dev.check(gp_driver_table_reset(dev.ctx(), &size_), "gp_driver_table_reset");
+        if (!slot.empty()) {
+            gp_driver_delta d{(int32_t)slot.size(), 0, slot.data(), present.data(), creation.data(), sched.data(), group.data(),
+                              q[0].data(), q[1].data(), q[2].data(), q[3].data(), q[4].data(), q[5].data(), count.data(), exact.data()};
+            dev.check(gp_driver_table_update(dev.ctx(), &d), "gp_driver_table_update");
+        }
+        for (int32_t s : slot) sent_[s] = record(s);
+        replay_ = false;
+        dirty_.clear();
+    }
+
+private:
+    struct Row {
+        bool present = false;
+        int64_t creation = 0;
+        int32_t scheduler = 0, group = -1;
+        int64_t q[6] = {0, 0, 0, 0, 0, 0};
+        int32_t count = 0;
+        bool exact = false;
+        bool operator==(const Row& o) const {
+            for (int k = 0; k < 6; ++k) if (q[k] != o.q[k]) return false;
+            return present == o.present && creation == o.creation && scheduler == o.scheduler && group == o.group && count == o.count &&
+                   exact == o.exact;
+        }
+    };
+    struct Held { int32_t slot; Row row; QueuedDriverPod pod; ParsedSparkResources parsed; };
+    static int32_t intern(std::map<std::string, int32_t>& t, const std::string& name) {
+        auto it = t.find(name);
+        if (it != t.end()) return it->second;
+        const int32_t id = (int32_t)t.size();
+        t.emplace(name, id);
+        return id;
+    }
+    Row record(int32_t s) const { auto it = uidAt_.find(s); return it == uidAt_.end() ? Row{} : held_.at(it->second).row; }
+
+    gp_driver_table_size size_;
+    std::map<std::string, Held> held_;
+    std::map<int32_t, std::string> uidAt_;       // slot -> uid, in slot order
+    std::set<int32_t> free_;
+    int32_t next_ = 0;
+    std::map<std::string, int32_t> schedulers_, groups_;
+    std::set<int32_t> dirty_;
+    std::map<int32_t, Row> sent_;
+    bool replay_ = true;
+    int replays_ = 0;
+};
+
+// What selectDriverNode's FIFO step decides for the requesting driver: fits (result = its packing), failure-fit (-1) or
+// failure-earlier-driver (-2); undefinedTies > 0: equal creation times whose order the reference leaves undefined.
+struct DriverQueueOutcome {
+    int32_t status = -1;                  // >= 0: fits; -1 failure-fit; -2 failure-earlier-driver
+    binpack::PackingResult result;
+    int32_t undefinedTies = 0;
+    bool fromTable = false;               // false: the per-call path answered (a refusal, or a packer the table entry does not take)
+};
+
+// fitEarlierDrivers (resource.go:224-262) followed by the requesting driver's own FIFO step, from the resident driver table:
+// one flush, one gp_pack_fifo_driver_table over the snapshot of `metadata`, which then holds the usage of every fitted driver
+// (the requesting one included).  The requesting driver must be held (SetDriver it from ExtenderArgs.Pod first: an informer
+// can lag).  A capacity refusal grows the buffers and calls again; any other refusal, of the flush or of the call, replays the
+// table and falls back to
+// FilterToEarliestAndSort over drivers.Pods() plus FitEarlierDrivers, the per-call FIFO batch, on the same metadata.  The
+// zone-aware packers, whose snapshot is laid out per zone, take that per-call path too.
+inline DriverQueueOutcome FitEarlierDriversDriverTable(const binpacker::Binpacker& packer, ResidentDrivers& drivers,
+                                                      const std::string& uid, int64_t defaultEnforceAfterNs,
+                                                      const std::map<std::string, int64_t>& enforceAfterOverrides,
+                                                      int64_t nowUnixNano, const std::vector<std::string>& nodeNames,
+                                                      const std::vector<std::string>& executorNodeNames,
+                                                      resources::NodeGroupSchedulingMetadata& metadata) {
+    gangpack::Device& d = gangpack::Device::Get();
+    DriverQueueOutcome out;
+    const bool tableForm = !packer.IsSingleAz && packer.Name != binpacker::azAwareTightlyPack;
+    bool flushed = false;
+    if (tableForm && drivers.Holds(uid)) {
+        try {
+            drivers.Flush(d);
+            flushed = true;
+        } catch (const gangpack::Error&) {
+        }
+    }
+    if (flushed) {
+        const std::vector<int64_t> enforceAfterNs = drivers.GroupAges(defaultEnforceAfterNs, enforceAfterOverrides);
+        d.SetSnapshot(metadata, nodeNames, executorNodeNames);
+        int32_t cap = (int32_t)drivers.Size().n_slots + 1, n = 0, ties = 0;
+        int64_t ecap = 4 * (int64_t)cap, ne = 0;
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            std::vector<int32_t> slots((size_t)cap), driver((size_t)cap), exec((size_t)std::max<int64_t>(ecap, 1));
+            std::vector<int64_t> off((size_t)cap + 1);
+            gp_driver_queue q{};
+            q.requesting_slot = drivers.Slot(uid);
+            q.queue_cap = cap;
+            q.enforce_after_ns = enforceAfterNs.data();
+            q.now_unix_nano = nowUnixNano;
+            q.queue_slot = slots.data(); q.exec_out_off = off.data(); q.n_queued = &n; q.n_executors = &ne; q.undefined_ties = &ties;
+            gp_results r{driver.data(), exec.data(), ecap};
+            const int st = gp_pack_fifo_driver_table(d.ctx(), &q, (gp_algo)packer.algo, GP_MODE_FIFO_REFERENCE, &r);
+            if (st == GP_ERR_CAPACITY && attempt == 0) { cap = std::max(cap, n); ecap = std::max(ecap, ne); continue; }
+            if (st != GP_OK) break;
+            std::vector<int64_t> cpu(d.n_nodes()), mem(d.n_nodes()), gpu(d.n_nodes());
+            d.check(gp_get_snapshot(d.ctx(), cpu.data(), mem.data(), gpu.data()), "gp_get_snapshot");
+            for (size_t i = 0; i < d.n_nodes(); ++i) {
+                auto& m = metadata.at(d.name((int32_t)i)).AvailableResources;
+                m.CPU = cpu[i]; m.Memory = mem[i]; m.NvidiaGPU = gpu[i];
+            }
+            const int32_t last = n - 1;
+            out.status = driver[(size_t)last];
+            out.undefinedTies = ties;
+            out.fromTable = true;
+            if (out.status >= 0) {
+                out.result.HasCapacity = true;
+                out.result.DriverNode = d.name(out.status);
+                for (int64_t t = off[(size_t)last]; t < off[(size_t)last + 1]; ++t) out.result.ExecutorNodes.push_back(d.name(exec[(size_t)t]));
+            }
+            return out;
+        }
+    }
+    if (tableForm && drivers.Holds(uid)) {       // refused (the update or the call): resend the whole table, then answer with
+        drivers.Replay();                        // the per-call path
+        drivers.Flush(d);
+    }
+    // the per-call path: FilterToEarliestAndSort over the listed drivers, shouldSkipDriverFifo, the FIFO batch
+    const std::vector<QueuedDriverPod> pods = drivers.Pods();
+    const QueuedDriverPod* me = nullptr;
+    for (const auto& p : pods) if (p.UID == uid) me = &p;
+    if (!me) throw gangpack::Error(GP_ERR_INVALID, "FitEarlierDriversDriverTable: the requesting driver is not held (SetDriver it first)");
+    const std::vector<int64_t> enforceAfterNs = drivers.GroupAges(defaultEnforceAfterNs, enforceAfterOverrides);
+    std::vector<PendingDriver> queue;
+    const std::vector<QueuedDriverPod> earlier = FilterToEarliestAndSort(*me, pods);
+    for (size_t j = 0; j < earlier.size(); ++j) {
+        const auto& p = earlier[j];
+        if (!drivers.Exact(p.UID)) throw gangpack::Error(GP_ERR_UNREPRESENTABLE, "FitEarlierDriversDriverTable: a queued driver is outside the exact-int64 model (run the Go loop)");
+        const int32_t g = drivers.GroupID(p.UID);
+        const __int128 created = (__int128)p.CreationSeconds * 1000000000LL;
+        queue.push_back(drivers.Pending(p.UID, created > (__int128)nowUnixNano - (__int128)enforceAfterNs.at((size_t)g)));
+        if (j > 0 && p.CreationSeconds == earlier[j - 1].CreationSeconds) ++out.undefinedTies;
+    }
+    if (!drivers.Exact(uid)) throw gangpack::Error(GP_ERR_UNREPRESENTABLE, "FitEarlierDriversDriverTable: the driver is outside the exact-int64 model (run the Go loop)");
+    if (!FitEarlierDrivers(packer, queue, nodeNames, executorNodeNames, metadata)) { out.status = -2; return out; }
+    std::vector<binpack::PackingResult> res;
+    FitEarlierDrivers(packer, {drivers.Pending(uid, false)}, nodeNames, executorNodeNames, metadata, &res);
+    out.result = res[0];
+    out.status = res[0].HasCapacity ? d.index(res[0].DriverNode) : -1;
+    return out;
 }
 
 }  // namespace extender

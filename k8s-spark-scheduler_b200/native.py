@@ -47,6 +47,8 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_prepare_cluster_zones_groups_node_table", "gp_reschedule_from_reservations_node_table",
            "gp_reconcile_find_nodes_node_table", "gp_exceeds_cluster_capacity_node_table",
            "gp_exceeds_cluster_capacity_affinity_node_table",
+           "gp_driver_table_reset", "gp_driver_table_update", "gp_pack_fifo_driver_table",
+           "gp_pack_fifo_zones_groups_driver_table",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -311,6 +313,24 @@ class gp_node_table_nodes(C.Structure):
                 ("instance_group_out", C.c_void_p)]
 
 
+class gp_driver_table_size(C.Structure):
+    _fields_ = [("n_slots", C.c_int32), ("n_groups", C.c_int32), ("n_schedulers", C.c_int32), ("reserved", C.c_int32)]
+
+
+class gp_driver_delta(C.Structure):
+    _fields_ = [("n_write", C.c_int32), ("reserved", C.c_int32), ("slot", C.c_void_p), ("present", C.c_void_p),
+                ("creation", C.c_void_p), ("scheduler", C.c_void_p), ("group", C.c_void_p), ("drv_cpu_milli", C.c_void_p),
+                ("drv_mem_bytes", C.c_void_p), ("drv_gpu", C.c_void_p), ("exe_cpu_milli", C.c_void_p), ("exe_mem_bytes", C.c_void_p),
+                ("exe_gpu", C.c_void_p), ("min_executor_count", C.c_void_p), ("exact", C.c_void_p)]
+
+
+class gp_driver_queue(C.Structure):
+    _fields_ = [("requesting_slot", C.c_int32), ("scheduler", C.c_int32), ("predicate_group", C.c_int32), ("queue_cap", C.c_int32),
+                ("snapshot_group", C.c_void_p), ("enforce_after_ns", C.c_void_p), ("now_unix_nano", C.c_int64),
+                ("queue_slot", C.c_void_p), ("exec_out_off", C.c_void_p), ("n_queued", C.c_void_p), ("n_executors", C.c_void_p),
+                ("undefined_ties", C.c_void_p)]
+
+
 class gp_placement_record(C.Structure):
     _fields_ = [("collocation", C.c_int32), ("distinct_exec_nodes", C.c_int32), ("execs_per_node", C.c_int32), ("n_zones", C.c_int32),
                 ("cross_zone_pairs", C.c_int64), ("total_pairs", C.c_int64)]
@@ -524,6 +544,15 @@ def load():
     L.gp_multi_get_snapshot.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.gp_multi_group_owner.restype = C.c_int
     L.gp_multi_group_owner.argtypes = [C.c_void_p, C.c_void_p]
+    L.gp_driver_table_reset.restype = C.c_int
+    L.gp_driver_table_reset.argtypes = [C.c_void_p, C.POINTER(gp_driver_table_size)]
+    L.gp_driver_table_update.restype = C.c_int
+    L.gp_driver_table_update.argtypes = [C.c_void_p, C.POINTER(gp_driver_delta)]
+    L.gp_pack_fifo_driver_table.restype = C.c_int
+    L.gp_pack_fifo_driver_table.argtypes = [C.c_void_p, C.POINTER(gp_driver_queue), C.c_int, C.c_int, C.POINTER(gp_results)]
+    L.gp_pack_fifo_zones_groups_driver_table.restype = C.c_int
+    L.gp_pack_fifo_zones_groups_driver_table.argtypes = [C.c_void_p, C.POINTER(gp_driver_queue), C.c_int, C.c_int, C.c_void_p,
+                                                         C.POINTER(gp_zone_results)]
     _lib = L
     return L
 
@@ -539,6 +568,11 @@ def _p(a):
 def _triple(t):
     """(cpu, mem[, gpu]) columns, the gpu one absent or None -> three int64 arrays (gpu None when not given)."""
     return [_np(t[i], np.int64) if i < len(t) else None for i in range(3)]
+
+
+_DT_DELTA_COLS = {"slot": np.int32, "present": np.uint8, "creation": np.int64, "scheduler": np.int32, "group": np.int32,
+                  "drv_cpu_milli": np.int64, "drv_mem_bytes": np.int64, "drv_gpu": np.int64, "exe_cpu_milli": np.int64,
+                  "exe_mem_bytes": np.int64, "exe_gpu": np.int64, "min_executor_count": np.int32, "exact": np.uint8}
 
 
 def _usage_input(alloc, overhead, res_node, res):
@@ -1545,6 +1579,85 @@ class GangPacker:
         self._check(load().gp_exceeds_cluster_capacity_affinity_node_table(self._h, C.byref(nt), C.byref(aff), C.byref(a), int(packer),
                                                                            _p(out), _p(err)))
         return out[:q], err[:q]
+
+    # ---- the resident driver table (gp_driver_table_*) and the driver-table FIFO entries ----------------------------------
+    def driver_table_reset(self, n_slots, n_groups, n_schedulers):
+        """Replace the context's driver table with an empty one of these capacities."""
+        self._check(load().gp_driver_table_reset(self._h, C.byref(gp_driver_table_size(int(n_slots), int(n_groups), int(n_schedulers), 0))))
+
+    def driver_table_update(self, delta: dict):
+        """One gp_driver_table_update over the arrays of drivers.DriverTable.delta() (slot, present, creation, scheduler, group,
+        the six quantity columns, min_executor_count, exact; a missing column is NULL; "reset" is not read here)."""
+        col = {k: _np(delta.get(k), t) for k, t in _DT_DELTA_COLS.items()}
+        d = gp_driver_delta(n_write=0 if col["slot"] is None else len(col["slot"]), **{k: _p(v) for k, v in col.items()})
+        self._check(load().gp_driver_table_update(self._h, C.byref(d)))
+
+    def _driver_queue(self, queue: dict, queue_cap):
+        """gp_driver_queue over queue = dict(requesting_slot=-1, scheduler=0, predicate_group=0, snapshot_group=None,
+        enforce_after_ns=None, now=0) with out arrays for queue_cap entries; -> (struct, outs dict)"""
+        sg, age = _np(queue.get("snapshot_group"), np.int32), _np(queue.get("enforce_after_ns"), np.int64)
+        outs = dict(queue_slot=np.empty(max(queue_cap, 1), np.int32), off=np.empty(queue_cap + 1, np.int64),
+                    n_queued=C.c_int32(-9), n_executors=C.c_int64(-9), ties=C.c_int32(-9))
+        dq = gp_driver_queue(requesting_slot=int(queue.get("requesting_slot", -1)), scheduler=int(queue.get("scheduler", 0)),
+                             predicate_group=int(queue.get("predicate_group", 0)), queue_cap=int(queue_cap), snapshot_group=_p(sg),
+                             enforce_after_ns=_p(age), now_unix_nano=int(queue.get("now", 0)), queue_slot=_p(outs["queue_slot"]),
+                             exec_out_off=_p(outs["off"]), n_queued=C.addressof(outs["n_queued"]),
+                             n_executors=C.addressof(outs["n_executors"]), undefined_ties=C.addressof(outs["ties"]))
+        dq._keep = (sg, age, outs)
+        return dq, outs
+
+    def _driver_table_call(self, queue, queue_cap, exec_cap, retry, call):
+        """call(gp_driver_queue, outs, exec_cap) -> status.  Default capacities: the table's slots + 1 and 4 executors per
+        entry; with retry, a GP_ERR_CAPACITY is retried once with the sizes the call wrote back."""
+        if queue_cap is None:
+            queue_cap = int(queue.get("n_slots", 0)) + 1
+        if exec_cap is None:
+            exec_cap = 4 * queue_cap
+        dq, outs = self._driver_queue(queue, queue_cap)
+        st = call(dq, outs, exec_cap)
+        if st == 5 and retry:
+            queue_cap = max(queue_cap, outs["n_queued"].value)
+            exec_cap = max(exec_cap, int(outs["n_executors"].value))
+            dq, outs = self._driver_queue(queue, queue_cap)
+            st = call(dq, outs, exec_cap)
+        self._check(st)
+        n = outs["n_queued"].value
+        return dict(queue_slot=outs["queue_slot"][:n].copy(), off=outs["off"][:n + 1].copy(), n_queued=n,
+                    n_executors=outs["n_executors"].value, undefined_ties=outs["ties"].value)
+
+    def pack_fifo_driver_table(self, queue: dict, algo: int, mode: int, queue_cap=None, exec_cap=None, retry=True) -> dict:
+        """gp_pack_fifo_driver_table: the FIFO queue selected and ordered from the driver table (queue as in _driver_queue,
+        plus n_slots for the default capacity), packed over the held snapshot.  -> dict with queue_slot, off, n_queued,
+        n_executors, undefined_ties, driver_node and executor_nodes."""
+        res = {}
+
+        def call(dq, outs, cap):
+            res["drv"] = np.empty(max(dq.queue_cap, 1), np.int32)
+            res["exe"] = np.empty(max(cap, 1), np.int32)      # defined for placed drivers only, as gp_results says
+            r = gp_results(driver_node=_p(res["drv"]), executor_nodes=_p(res["exe"]), executor_nodes_cap=int(cap))
+            return load().gp_pack_fifo_driver_table(self._h, C.byref(dq), int(algo), int(mode), C.byref(r))
+        out = self._driver_table_call(queue, queue_cap, exec_cap, retry, call)
+        out["driver_node"] = res["drv"][:out["n_queued"]].copy()
+        out["executor_nodes"] = res["exe"][:out["n_executors"]].copy()
+        return out
+
+    def pack_fifo_zones_groups_driver_table(self, queue: dict, packer: int, mode: int, queue_cap=None, exec_cap=None, retry=True) -> dict:
+        """gp_pack_fifo_zones_groups_driver_table over the layout prepare_cluster_zones_groups left: -> the dict of
+        pack_fifo_driver_table plus zone and avg_efficiency."""
+        res = {}
+
+        def call(dq, outs, cap):
+            q = max(dq.queue_cap, 1)
+            res.update(zone=np.empty(q, np.int32), drv=np.empty(q, np.int32), exe=np.empty(max(cap, 1), np.int32),
+                       avg=np.zeros((q, 4), np.float64))
+            r = gp_zone_results(zone=_p(res["zone"]), driver_node=_p(res["drv"]), executor_nodes=_p(res["exe"]), executor_nodes_cap=int(cap),
+                                avg_efficiency=_p(res["avg"]))
+            return load().gp_pack_fifo_zones_groups_driver_table(self._h, C.byref(dq), int(packer), int(mode), None, C.byref(r))
+        out = self._driver_table_call(queue, queue_cap, exec_cap, retry, call)
+        n = out["n_queued"]
+        out.update(zone=res["zone"][:n].copy(), driver_node=res["drv"][:n].copy(), executor_nodes=res["exe"][:out["n_executors"]].copy(),
+                   avg_efficiency=res["avg"][:n].copy())
+        return out
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
