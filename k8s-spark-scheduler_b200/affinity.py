@@ -23,6 +23,8 @@ import re
 
 import numpy as np
 
+from .resident import ResidentTable
+
 IN, NOT_IN, EXISTS, DOES_NOT_EXIST, GT, LT, FIELD_NAME_IN, FIELD_NAME_NOT_IN = range(8)
 _LABEL_OPS = {"In": IN, "NotIn": NOT_IN, "Exists": EXISTS, "DoesNotExist": DOES_NOT_EXIST, "Gt": GT, "Lt": LT}
 
@@ -229,20 +231,19 @@ def unpack_bits(member, n) -> np.ndarray:
 _UNKNOWN = 0                    # the key id and value id of a string no node carries: no row ever holds them
 
 
-class LabelTable:
+class LabelTable(ResidentTable):
     """Every node's labels as the resident label table keeps them, from the node informer's events: set_node(name, labels)
     for an add or an update (nothing changes when the labels are the same), delete_node(name).
 
     Key and value strings are interned for good (id 0 of each is reserved for strings no node carries, so encoding an
     affinity never changes the table); node names get ids that a deleted node hands to the next new one.  delta() -> the
     arrays of one gp_label_table_update: the rows of the nodes whose labels changed (a deleted node's row cleared) and the
-    ParseInt columns of the values interned since the last delta.  When it carries "reset" (the first one, whenever a
-    capacity would be exceeded: it is doubled and the whole state replayed, and after replay()),
-    gp_label_table_reset(**delta["reset"]) goes first.  flush(packer) does both and keeps `mirror`, a numpy copy of what the
-    device holds."""
+    ParseInt columns of the values interned since the last delta; see ResidentTable."""
+
+    name, writes = "label", ("row_node", "value_id")
 
     def __init__(self, n_node_ids=64, max_labels=16, n_keys=64, n_values=256):
-        self.size = dict(n_node_ids=n_node_ids, max_labels=max_labels, n_keys=n_keys, n_values=n_values)
+        super().__init__(LabelMirror(), n_node_ids=n_node_ids, max_labels=max_labels, n_keys=n_keys, n_values=n_values)
         self.labels = {}                                # node name -> {key: value}, as the events gave them
         self._keys, self._vals = _Ids({None: _UNKNOWN}), _Ids({None: _UNKNOWN})
         self._parsed = [(False, 0)]                     # per value id: ParseInt of the string
@@ -251,8 +252,6 @@ class LabelTable:
         self._free = []
         self._longest = 0                               # the most labels any row has held: a stride that fits every row
         self._dirty, self._new_vals = set(), []
-        self._replay = True
-        self.mirror = LabelMirror()
 
     # ---- events
     def set_node(self, name, labels: dict):
@@ -291,18 +290,15 @@ class LabelTable:
         val = lambda v: self._vals.get(v, _UNKNOWN)
         return _encode_programs(affinities, key, val, _node_index(list(node_names)))
 
-    # ---- updates
-    def replay(self):
-        """The next delta resets the table and resends the whole state (after an update that was refused or failed)."""
-        self._replay = True
+    def to_node_labels(self, node_ids) -> dict:
+        return self.mirror.to_node_labels(node_ids)
 
-    def delta(self) -> dict:
-        need = dict(n_node_ids=len(self._row), max_labels=self._longest, n_keys=len(self._keys), n_values=len(self._vals))
-        for k, b in need.items():
-            while self.size[k] < b:
-                self.size[k] = max(2 * self.size[k], 1)
-                self._replay = True
-        if self._replay:
+    # ---- internals
+    def _bounds(self):
+        return dict(n_node_ids=len(self._row), max_labels=self._longest, n_keys=len(self._keys), n_values=len(self._vals))
+
+    def _changes(self, replay):
+        if replay:
             rows = [at for at, r in enumerate(self._row) if r]
             vals = list(range(1, len(self._vals)))
         else:
@@ -310,38 +306,12 @@ class LabelTable:
         off = np.zeros(len(rows) + 1, np.int64)
         np.cumsum([len(self._row[at]) for at in rows], out=off[1:])
         pairs = [kv for at in rows for kv in self._row[at]]
-        d = {"reset": dict(self.size) if self._replay else None, "row_node": _i32(rows), "row_off": off,
+        d = {"row_node": _i32(rows), "row_off": off,
              "label_key": np.array([k for k, _ in pairs], np.int32), "label_val": np.array([v for _, v in pairs], np.int32),
              "value_id": _i32(vals), "value_int_ok": np.array([self._parsed[v][0] for v in vals], np.uint8),
              "value_int": np.array([self._parsed[v][1] for v in vals], np.int64)}
         self._dirty, self._new_vals = set(), []
-        self._replay = False
         return d
-
-    def flush(self, packer):
-        """One update of the device's table (none when nothing changed), preceded by a reset when the delta carries one; on
-        a refusal the whole state is reset and replayed once more, and a second refusal is raised."""
-        from .native import GangpackError
-        d = self.delta()
-        if d["reset"] is None and len(d["row_node"]) == 0 and len(d["value_id"]) == 0:
-            return
-        try:
-            self._push(packer, d)
-        except GangpackError:
-            self.replay()
-            d = self.delta()
-            self._push(packer, d)
-        self.mirror.apply(d)
-
-    def to_node_labels(self, node_ids) -> dict:
-        return self.mirror.to_node_labels(node_ids)
-
-    # ---- internals
-    @staticmethod
-    def _push(packer, d):
-        if d["reset"] is not None:
-            packer.label_table_reset(**d["reset"])
-        packer.label_table_update(d)
 
     def _key(self, k):
         return self._keys.id(k)

@@ -74,7 +74,7 @@ static gp_status check_source(gp_ctx* c, const UsageIn& u, const char* who) {
     const gp_resident_usage* r = u.res;
     if (r->n_nodes < 0 || (r->n_nodes > 0 && (!r->node_id || !r->alloc_cpu_milli || !r->alloc_mem_bytes)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or bad sizes");
-    if (!c->rt.live) return fail(c, GP_ERR_INVALID, who, "no reservation table (gp_reservation_table_reset first)");
+    GP_TRY(require(c, c->rt.need(), who));
     if (r->overhead_node_id && !c->oht.live) return fail(c, GP_ERR_INVALID, who, "overhead_node_id without an overhead table");
     return GP_OK;
 }

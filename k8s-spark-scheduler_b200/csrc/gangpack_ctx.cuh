@@ -135,6 +135,23 @@ static_assert(sizeof(DevStatus) == 4 * kStatusWords, "gp_decide_tables zeroes th
 // Pinned host block: the mirror of StatusHead (gp_last_stats) and the error word the kernels write through its mapping
 struct PinnedStatus { StatusHead head; volatile int err_word; };
 
+#define GP_CUDA(ctx, expr)                                                                     \
+    do {                                                                                       \
+        cudaError_t _e = (expr);                                                               \
+        if (_e != cudaSuccess) {                                                               \
+            (ctx)->err = std::string(#expr) + ": " + cudaGetErrorString(_e);                   \
+            return GP_ERR_CUDA;                                                                \
+        }                                                                                      \
+    } while (0)
+
+#define GP_TRY(expr)                                                                           \
+    do {                                                                                       \
+        const gp_status _s = (expr);                                                           \
+        if (_s != GP_OK) return _s;                                                            \
+    } while (0)
+
+#include "gangpack_resident.cuh"
+
 struct gp_ctx {
     int device = 0;
     int sm_count = 0;
@@ -211,70 +228,34 @@ struct gp_ctx {
     bool recon_attr_set = false;                  // dynamic shared-memory opt-in of gp_sort_tiles<ReconKey> done on this device
     bool fifo_attr_set[2] = {false, false};       // dynamic shared-memory opt-in of gp_pack_fifo_cta<ALGO,*> done on this device
 
-    // the resident overhead table (gangpack_overhead_table.cu); no other entry reads or changes it
-    struct OverheadTable {
-        bool live = false;                        // reset and not broken by a CUDA error since
-        gp_overhead_table_size size{};
-        DevBuf cols;                              // slot columns, RR flags and the duplicate stamps in one block
+    // the resident tables (gangpack_resident.cuh); each is read by its own entries and those named below, and changed only by
+    // its own reset and update
+    struct OverheadTable : ResidentTable<gp_overhead_table_size> {   // gangpack_overhead_table.cu; the columns hold the RR flags
+        using ResidentTable::ResidentTable;
         DevBuf set[2];                            // member set: set[cur] is live, the other the target of the next rehash
         int cur = 0;
         uint32_t cells = 0;                       // cells of set[cur], a power of two
         long long keys = 0, used = 0;             // live keys; cells holding a key or a tombstone
-        uint32_t seq = 0;                         // the last update's stamp
-    } oht;
-
-    // the resident reservation table (gangpack_reservation_table.cu); read by the *_resident entries, changed only by its own
-    struct ReservationTable {
-        bool live = false;                        // reset and not broken by a CUDA error since
-        gp_reservation_table_size size{};
-        DevBuf cols;                              // node id [n_slots], cpu / mem / gpu [3][n_slots], duplicate stamps [n_slots]
-        uint32_t seq = 0;                         // the last update's stamp
-    } rt;
-
-    // the resident label table (gangpack_label_table.cu); read by the *_resident affinity entries, changed only by its own
-    struct LabelTable {
-        bool live = false;                        // reset and not broken by a CUDA error since
-        gp_label_table_size size{};
-        DevBuf cols;                              // count, key, val, val_int, val_int_ok and the row / value stamps in one block
-        uint32_t seq = 0;                         // the last update's stamp
-    } lt;
-
-    // the resident node table (gangpack_node_table.cu); read by the *_node_table entries, changed only by its own
-    struct NodeTable {
-        bool live = false;                        // reset and not broken by a CUDA error since
-        gp_node_table_size size{};
-        DevBuf cols;                              // present, alloc [3], unschedulable, ready, name_key, name_rank, stamps in one block
+    } oht{"no overhead table (gp_overhead_table_reset first)"};
+    // gangpack_reservation_table.cu, read by the *_resident entries: node id [n_slots], cpu / mem / gpu [3][n_slots]
+    ResidentTable<gp_reservation_table_size> rt{"no reservation table (gp_reservation_table_reset first)"};
+    // gangpack_label_table.cu, read by the *_resident affinity entries: count, key, val, val_int and val_int_ok
+    ResidentTable<gp_label_table_size> lt{"no label table (gp_label_table_reset first)"};
+    // gangpack_node_table.cu, read by the *_node_table entries: present, alloc [3], unschedulable, ready, name_key, name_rank
+    struct NodeTable : ResidentTable<gp_node_table_size> {
+        using ResidentTable::ResidentTable;
         DevBuf gather;                            // the columns one *_node_table call gathers, and its scratch
-        uint32_t seq = 0;                         // the last update's stamp
-    } nt;
-
-    // the resident driver table (gangpack_driver_table.cu); read by the *_driver_table entries, changed only by its own
-    struct DriverTable {
-        bool live = false;                        // reset and not broken by a CUDA error since
-        gp_driver_table_size size{};
-        DevBuf cols;                              // present, exact, creation, scheduler, group, quantities [6], count, stamps in one block
+    } nt{"no node table (gp_node_table_reset first)"};
+    // gangpack_driver_table.cu, read by the *_driver_table entries: present, exact, creation, scheduler, group, quantities [6],
+    // count
+    struct DriverTable : ResidentTable<gp_driver_table_size> {
+        using ResidentTable::ResidentTable;
         DevBuf queue;                             // the queue one *_driver_table call selects, orders and packs, and its scratch
-        uint32_t seq = 0;                         // the last update's stamp
         bool sort_attr_set = false;               // dynamic shared-memory opt-in of gp_sort_tiles<QueueKey> done on this device
-    } dt;
+    } dt{"no driver table (gp_driver_table_reset first)"};
 
     gp_stats last{};
 };
-
-#define GP_CUDA(ctx, expr)                                                                     \
-    do {                                                                                       \
-        cudaError_t _e = (expr);                                                               \
-        if (_e != cudaSuccess) {                                                               \
-            (ctx)->err = std::string(#expr) + ": " + cudaGetErrorString(_e);                   \
-            return GP_ERR_CUDA;                                                                \
-        }                                                                                      \
-    } while (0)
-
-#define GP_TRY(expr)                                                                           \
-    do {                                                                                       \
-        const gp_status _s = (expr);                                                           \
-        if (_s != GP_OK) return _s;                                                            \
-    } while (0)
 
 gp_status fail(gp_ctx* ctx, gp_status st, const std::string& msg);
 static inline gp_status fail(gp_ctx* c, gp_status st, const char* who, const char* what) {

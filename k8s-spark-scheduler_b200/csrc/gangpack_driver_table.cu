@@ -2,10 +2,10 @@
 // that select, order and pack a FIFO queue from it (gp_pack_fifo_driver_table, gp_pack_fifo_zones_groups_driver_table).
 //
 // An update runs
-//   gp_dt_check     thread per slot write: slot range, duplicates (per-slot stamps holding the update's sequence number,
-//                   atomicExch), on present rows scheduler and group range and |quantity| < 2^61 when the row is exact
+//   gp_dt_check     thread per slot write: slot range, duplicates (per-slot stamps, stamped_twice), on present rows scheduler
+//                   and group range and |quantity| < 2^61 when the row is exact
 //   gp_dt_apply     the slot writes; nothing when the error word is set
-// so a refused delta leaves the table as it was, and only its stamps are written before the check is complete.
+// within the update protocol of gangpack_resident.cuh, so a refused delta leaves the table as it was.
 //
 // The queue stage of an entry writes, on the device, exactly the gp_apps columns the host would upload for the same pods
 // (filterToEarliestAndSort stable in slot order, sparkResources, shouldSkipDriverFifo):
@@ -125,7 +125,7 @@ __global__ void gp_dt_check(DtDelta D, uint32_t* __restrict__ stamp, uint32_t se
     if (i >= D.n) return;
     const int32_t r = D.slot[i];
     if (r < 0 || r >= D.n_rows) { atomicOr(err, kDtErrRange); return; }
-    int bad = atomicExch(stamp + r, seq) == seq ? kDtErrDuplicate : 0;
+    int bad = stamped_twice(stamp + r, seq) ? kDtErrDuplicate : 0;
     if (D.present[i]) {
         const int32_t s = D.sched[i], g = D.group[i];
         if (s < 0 || s >= D.n_sched || g < -1 || g >= D.n_groups) bad |= kDtErrId;
@@ -307,10 +307,6 @@ __global__ void __launch_bounds__(kDqFinishThreads) gp_dq_finish(int32_t req, Dq
     }
 }
 
-static gp_status no_table(gp_ctx* c, const char* who) {
-    return fail(c, GP_ERR_INVALID, who, "no driver table (gp_driver_table_reset first)");
-}
-
 // What an entry packs after the queue stage: device columns of n_queued entries, and the staging arena they live in
 struct QueueRun {
     int32_t n_queued;
@@ -324,7 +320,7 @@ struct QueueRun {
 static gp_status queue_stage(gp_ctx* c, const gp_driver_queue* dq, int32_t n_sg, bool zones, int64_t executor_cap, const char* who,
                              QueueRun* run) {
     auto& t = c->dt;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     const int32_t S = t.size.n_slots, NG = t.size.n_groups;
     if (!dq->n_queued || !dq->queue_slot || dq->queue_cap < 0 || (NG > 0 && !dq->enforce_after_ns) ||
         (dq->requesting_slot < 0 && NG > 0 && !dq->snapshot_group))
@@ -419,31 +415,24 @@ gp_status gp_driver_table_reset(gp_ctx* c, const gp_driver_table_size* z) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_driver_table_reset";
     if (!z || z->n_slots < 0 || z->n_groups < 0 || z->n_schedulers < 0) return fail(c, GP_ERR_INVALID, who, "NULL size or a negative capacity");
-    auto& t = c->dt;
-    t.live = false;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    Arena a{t.cols, c->stream};
-    const DtPieces p = take_cols(a, *z);
-    a.reserve();
-    a.fill(p.present, p.stamp, 0);
-    GP_TRY(a.sync(c));
-    t.size = *z;
-    t.seq = 0;
-    t.live = true;
-    return GP_OK;
+    return c->dt.reset(c, *z, [&](Arena& a) {
+        const DtPieces p = take_cols(a, *z);
+        a.reserve();
+        a.fill(p.present, p.stamp, 0);
+        return GP_OK;
+    });
 }
 
 gp_status gp_driver_table_update(gp_ctx* c, const gp_driver_delta* d) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_driver_table_update";
     auto& t = c->dt;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     if (!d || d->n_write < 0 ||
         (d->n_write > 0 && (!d->slot || !d->present || !d->creation || !d->scheduler || !d->group || !d->drv_cpu_milli ||
                             !d->drv_mem_bytes || !d->exe_cpu_milli || !d->exe_mem_bytes || !d->min_executor_count || !d->exact)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or a negative count");
     if (d->n_write > t.size.n_slots) return fail(c, GP_ERR_INVALID, who, "more writes than slots: a slot given twice or out of range");
-    if (d->n_write == 0) return GP_OK;
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const size_t W = (size_t)d->n_write;
@@ -466,26 +455,18 @@ gp_status gp_driver_table_update(gp_ctx* c, const gp_driver_delta* d) {
     D.count = ar.put(cnt, d->min_executor_count);
     D.exact = ar.put(ex, d->exact);
     GP_TRY(ar.check(c));
-    // From here on the table's own buffers are written: a CUDA error leaves no table (reset and replay)
-    t.live = false;
     Arena tc{t.cols, st};
     const DtPieces p = take_cols(tc, t.size);
-    if (++t.seq == 0) {                                      // the stamps wrapped: none may equal a later update's number
-        tc.zero(p.stamp);
-        t.seq = 1;
-    }
-    GP_TRY(tc.check(c));
+    GP_TRY(t.begin(c, tc, p.stamp, p.stamp));
     int* w = ar.ptr(word);
-    const int T = 256;
-    const unsigned wb = (unsigned)((W + T - 1) / T);
-    gp_dt_check<<<wb, T, 0, st>>>(D, tc.ptr(p.stamp), t.seq, w);
-    gp_dt_apply<<<wb, T, 0, st>>>(D, table_cols(c), w);
-    GP_CUDA(c, cudaGetLastError());
+    if (W > 0) {
+        const int T = 256;
+        const unsigned wb = (unsigned)((W + T - 1) / T);
+        gp_dt_check<<<wb, T, 0, st>>>(D, tc.ptr(p.stamp), t.seq, w);
+        gp_dt_apply<<<wb, T, 0, st>>>(D, table_cols(c), w);
+    }
     int hw = 0;
-    ar.get(&hw, word);
-    GP_TRY(ar.sync(c));
-    t.live = true;
-    return refuse(c, hw, kDtRefusals, who);
+    return t.commit(c, ar, word, &hw, kDtRefusals, who);
 }
 
 gp_status gp_pack_fifo_driver_table(gp_ctx* c, const gp_driver_queue* dq, gp_algo algo, gp_mode mode, gp_results* out) {

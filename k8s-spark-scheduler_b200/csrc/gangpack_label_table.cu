@@ -2,16 +2,13 @@
 // entries of gangpack_marker.cu read it through lt_cols() as gp_aff_match's AffLabelsResident source.
 //
 // An update runs
-//   gp_lt_check   thread per row write and per value write: node and value id ranges, duplicates (per-row and per-value stamps
-//                 holding the update's sequence number, atomicExch: a second writer sees its own update's number), row length
-//                 within the stride, key ids in range and strictly ascending, label value ids in range; sets the error word and
-//                 writes nothing else
+//   gp_lt_check   thread per row write and per value write: node and value id ranges, duplicates (per-row and per-value
+//                 stamps, stamped_twice), row length within the stride, key ids in range and strictly ascending, label value
+//                 ids in range; sets the error word and writes nothing but the stamps
 //   gp_lt_apply   the same threads: the whole row (count, keys, values) or the value's ParseInt columns; nothing when the
 //                 error word is set
-// so a refused delta leaves the table as it was.
+// within the update protocol of gangpack_resident.cuh, so a refused delta leaves the table as it was.
 #include "gangpack_ctx.cuh"
-
-#include <algorithm>
 
 enum : int {
     kLtErrRange = 1,            // a node or value id out of its range
@@ -71,7 +68,7 @@ __global__ void gp_lt_check(LtDelta D, uint32_t* __restrict__ rstamp, uint32_t* 
         if (i < D.n_rows) {
             const int32_t r = D.row_node[i];
             if (r < 0 || r >= D.n_node_ids) { bad |= kLtErrRange; continue; }
-            if (atomicExch(rstamp + r, seq) == seq) bad |= kLtErrDuplicate;
+            if (stamped_twice(rstamp + r, seq)) bad |= kLtErrDuplicate;
             const long long lo = D.row_off[i], hi = D.row_off[i + 1];
             if (hi - lo > D.stride) { bad |= kLtErrLength; continue; }
             for (long long e = lo; e < hi; ++e) {
@@ -82,7 +79,7 @@ __global__ void gp_lt_check(LtDelta D, uint32_t* __restrict__ rstamp, uint32_t* 
         } else {
             const int32_t v = D.value_id[i - D.n_rows];
             if (v < 0 || v >= D.n_values) { bad |= kLtErrRange; continue; }
-            if (atomicExch(vstamp + v, seq) == seq) bad |= kLtErrDuplicate;
+            if (stamped_twice(vstamp + v, seq)) bad |= kLtErrDuplicate;
         }
     }
     if (bad) atomicOr(err, bad);
@@ -108,10 +105,6 @@ __global__ void gp_lt_apply(LtDelta D, int32_t* __restrict__ count, int32_t* __r
     }
 }
 
-static gp_status no_table(gp_ctx* c, const char* who) {
-    return fail(c, GP_ERR_INVALID, who, "no label table (gp_label_table_reset first)");
-}
-
 LtCols lt_cols(gp_ctx* c) {
     auto& t = c->lt;
     Arena a{t.cols, c->stream};
@@ -127,26 +120,20 @@ gp_status gp_label_table_reset(gp_ctx* c, const gp_label_table_size* z) {
     if (!z || z->n_node_ids < 0 || z->max_labels < 0 || z->n_keys < 0 || z->n_values < 0)
         return fail(c, GP_ERR_INVALID, who, "NULL size or a negative capacity");
     if ((int64_t)z->n_node_ids * z->max_labels > INT32_MAX) return fail(c, GP_ERR_INVALID, who, "n_node_ids * max_labels must be below 2^31");
-    auto& t = c->lt;
-    t.live = false;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    Arena a{t.cols, c->stream};
-    const LtPieces p = take_cols(a, *z);
-    a.reserve();
-    a.zero(p.count);
-    a.fill(p.vint, p.vstamp, 0);
-    GP_TRY(a.sync(c));
-    t.size = *z;
-    t.seq = 0;
-    t.live = true;
-    return GP_OK;
+    return c->lt.reset(c, *z, [&](Arena& a) {
+        const LtPieces p = take_cols(a, *z);
+        a.reserve();
+        a.zero(p.count);
+        a.fill(p.vint, p.vstamp, 0);
+        return GP_OK;
+    });
 }
 
 gp_status gp_label_table_update(gp_ctx* c, const gp_label_delta* d) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_label_table_update";
     auto& t = c->lt;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     if (!d || d->n_rows < 0 || d->n_values < 0 || (d->n_rows > 0 && (!d->row_node || !d->row_off)) ||
         (d->n_values > 0 && (!d->value_id || !d->value_int_ok || !d->value_int)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or a negative count");
@@ -185,30 +172,19 @@ gp_status gp_label_table_update(gp_ctx* c, const gp_label_delta* d) {
     D.int_ok = ar.put(vok, d->value_int_ok);
     D.ival = ar.put(vint, d->value_int);
     GP_TRY(ar.check(c));
-    // From here on the table's own buffers are written: a CUDA error leaves no table (reset and replay)
-    t.live = false;
     Arena tc{t.cols, st};
     const LtPieces p = take_cols(tc, t.size);
-    if (++t.seq == 0) {                                      // the stamps wrapped: none may equal a later update's number
-        tc.zero(p.rstamp);
-        tc.zero(p.vstamp);
-        t.seq = 1;
-    }
-    GP_TRY(tc.check(c));
+    GP_TRY(t.begin(c, tc, p.rstamp, p.vstamp));
     int* w = ar.ptr(word);
     const long long items = (long long)Rw + (long long)Vw;
     if (items > 0) {
         const int T = 256;
-        const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((items + T - 1) / T, (long long)c->sm_count * 8));
+        const unsigned grid = update_grid(items, T, c->sm_count);
         gp_lt_check<<<grid, T, 0, st>>>(D, tc.ptr(p.rstamp), tc.ptr(p.vstamp), t.seq, w);
         gp_lt_apply<<<grid, T, 0, st>>>(D, tc.ptr(p.count), tc.ptr(p.key), tc.ptr(p.val), tc.ptr(p.vint), tc.ptr(p.vok), w);
     }
-    GP_CUDA(c, cudaGetLastError());
     int hw = 0;
-    ar.get(&hw, word);
-    GP_TRY(ar.sync(c));
-    t.live = true;
-    return refuse(c, hw, kLtRefusals, who);
+    return t.commit(c, ar, word, &hw, kLtRefusals, who);
 }
 
 }  // extern "C"

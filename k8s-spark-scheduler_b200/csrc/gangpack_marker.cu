@@ -66,7 +66,7 @@ static gp_status check_affinity(gp_ctx* c, const gp_node_labels* L, const gp_nod
 // node id is checked by gp_aff_ids on the device)
 static gp_status check_affinity(gp_ctx* c, const gp_resident_labels* L, const gp_node_affinities* P, const char* who) {
     if (!L || L->n_nodes < 0 || (L->n_nodes > 0 && !L->node_id)) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
-    if (!c->lt.live) return fail(c, GP_ERR_INVALID, who, "no label table (gp_label_table_reset first)");
+    GP_TRY(require(c, c->lt.need(), who));
     return check_programs(c, L->n_nodes, c->lt.size.n_keys, c->lt.size.n_values, P, who);
 }
 
@@ -178,7 +178,7 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     if (!aff && (int64_t)(G + 1) * Z > (int64_t)INT32_MAX / 2) return fail(c, GP_ERR_INVALID, who, "(n_groups + 1) * n_zones too large");
     if (aff && (int64_t)Z > (int64_t)INT32_MAX / 2) return fail(c, GP_ERR_INVALID, who, "n_zones too large");
     if (resident && n > 0 && !over_ids) return fail(c, GP_ERR_INVALID, who, "overhead_node_id missing");
-    if (resident && !c->oht.live) return fail(c, GP_ERR_INVALID, who, "no overhead table (gp_overhead_table_reset first)");
+    if (resident) GP_TRY(require(c, c->oht.need(), who));
     // classes per chunk: node_group -> its own class and the all-nodes class; affinities -> as many as keep K n and K Z
     // within kCapEntries (at least one)
     const int32_t K = !aff ? 2 : (int32_t)std::max<int64_t>(1, std::min<int64_t>(std::max(G, 1), kCapEntries / std::max<int64_t>({(int64_t)n, (int64_t)Z, 1})));

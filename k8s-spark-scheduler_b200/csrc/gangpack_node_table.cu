@@ -3,14 +3,14 @@
 //
 // An update runs
 //   gp_nt_keys      thread per row: the row's NameKey (name_key, id) as the table holds it, absent rows last
-//   gp_nt_check     thread per row write: node id range, duplicates (per-row stamps holding the update's sequence number,
-//                   atomicExch), |alloc| < 2^61 and name_key < 2^63 - 1 on present rows; then the write's key replaces its
-//                   row's key in the scratch, so the scratch holds the table as it will be after the delta
+//   gp_nt_check     thread per row write: node id range, duplicates (per-row stamps, stamped_twice), |alloc| < 2^61 and
+//                   name_key < 2^63 - 1 on present rows; then the write's key replaces its row's key in the scratch, so the
+//                   scratch holds the table as it will be after the delta
 //   gp_sort_tiles / gp_rank_by_search <NameKey>   pos[row] = the row's rank among all rows by (name_key, id)
 //   gp_nt_scatter + gp_nt_dups   the keys in rank order; two adjacent present keys that are equal refuse the delta
 //   gp_nt_apply     the row writes and name_rank[row] = pos[row] (-1 absent); nothing when the error word is set
 //   gp_nt_creation  the rows' creation times, under the same condition
-// so a refused delta leaves the table as it was, and only its stamps are written before the check is complete.
+// within the update protocol of gangpack_resident.cuh, so a refused delta leaves the table as it was.
 //
 // The gather (gp_nt_gather, thread per listed node) writes exactly the columns a *_resident entry would upload: allocatable,
 // name_rank, unschedulable and ready from the node table, and zone, instance group and the two label ranks from the label
@@ -111,7 +111,7 @@ __global__ void gp_nt_check(NtDelta D, uint32_t* __restrict__ stamp, uint32_t se
     if (i >= D.n) return;
     const int32_t r = D.id[i];
     if (r < 0 || r >= D.n_rows) { atomicOr(err, kNtErrRange); return; }
-    int bad = atomicExch(stamp + r, seq) == seq ? kNtErrDuplicate : 0;
+    int bad = stamped_twice(stamp + r, seq) ? kNtErrDuplicate : 0;
     const bool on = D.present[i] != 0;
     if (on) {
         for (int d = 0; d < 3; ++d)
@@ -269,10 +269,6 @@ __global__ void gp_nt_gather(NtGatherIn G) {
     if (bad) atomicOr(G.err, bad);
 }
 
-static gp_status no_table(gp_ctx* c, const char* who) {
-    return fail(c, GP_ERR_INVALID, who, "no node table (gp_node_table_reset first)");
-}
-
 // (value, dense id) of list[n] sorted by value; a value listed twice is refused (distinct) or keeps its last index (ranks)
 static bool label_map(const int32_t* list, int32_t n, bool distinct, std::vector<int2>& out) {
     out.clear();
@@ -293,8 +289,7 @@ static bool label_map(const int32_t* list, int32_t n, bool distinct, std::vector
 gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nd, const int32_t* ig_host, int32_t n_ig, bool with_ig, const char* who,
                     NtGathered* g, const NtReconcile* recon, bool reservations) {
     auto& t = c->nt;
-    if (!t.live) return no_table(c, who);
-    if (!c->lt.live) return fail(c, GP_ERR_INVALID, who, "no label table (gp_label_table_reset first)");
+    GP_TRY(require(c, t.need(), c->lt.need(), who));
     if (!nd || nd->n_nodes < 0 || nd->n_zones < 1 ||
         (nd->n_nodes > 0 && (!nd->node_table_id || (reservations && !nd->reservation_id) || !nd->overhead_node_id)) ||
         (nd->zone_key >= 0 && !nd->zone_value) || (with_ig && !ig_host && nd->instance_group_key >= 0 && n_ig > 0 && !nd->instance_group_value) ||
@@ -400,25 +395,19 @@ gp_status gp_node_table_reset(gp_ctx* c, const gp_node_table_size* z) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_node_table_reset";
     if (!z || z->n_node_ids < 0) return fail(c, GP_ERR_INVALID, who, "NULL size or a negative capacity");
-    auto& t = c->nt;
-    t.live = false;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    Arena a{t.cols, c->stream};
-    const NtPieces p = take_cols(a, *z);
-    a.reserve();
-    a.fill(p.present, p.stamp, 0);
-    GP_TRY(a.sync(c));
-    t.size = *z;
-    t.seq = 0;
-    t.live = true;
-    return GP_OK;
+    return c->nt.reset(c, *z, [&](Arena& a) {
+        const NtPieces p = take_cols(a, *z);
+        a.reserve();
+        a.fill(p.present, p.stamp, 0);
+        return GP_OK;
+    });
 }
 
 gp_status gp_node_table_update(gp_ctx* c, const gp_node_delta* d) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_node_table_update";
     auto& t = c->nt;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     if (!d || d->n_write < 0 ||
         (d->n_write > 0 && (!d->node_id || !d->present || !d->alloc_cpu_milli || !d->alloc_mem_bytes || !d->unschedulable ||
                             !d->ready || !d->name_key)))
@@ -450,15 +439,9 @@ gp_status gp_node_table_update(gp_ctx* c, const gp_node_delta* d) {
     D.key = ar.put(key, d->name_key);
     D.creation = ar.put(cre, d->creation);
     GP_TRY(ar.check(c));
-    // From here on the table's own buffers are written: a CUDA error leaves no table (reset and replay)
-    t.live = false;
     Arena tc{t.cols, st};
     const NtPieces p = take_cols(tc, t.size);
-    if (++t.seq == 0) {                                      // the stamps wrapped: none may equal a later update's number
-        tc.zero(p.stamp);
-        t.seq = 1;
-    }
-    GP_TRY(tc.check(c));
+    GP_TRY(t.begin(c, tc, p.stamp, p.stamp));
     int* w = ar.ptr(word);
     const int T = 256;
     if (R > 0) {
@@ -472,16 +455,11 @@ gp_status gp_node_table_update(gp_ctx* c, const gp_node_delta* d) {
         gp_nt_dups<<<rb, T, 0, st>>>(n_rows, ar.ptr(skey), w);
         const NtTable tab{tc.ptr(p.present), tc.ptr(p.unsched), tc.ptr(p.ready), tc.ptr(p.alloc), tc.ptr(p.key), tc.ptr(p.rank)};
         const long long items = (long long)W + (long long)R;
-        const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((items + T - 1) / T, (long long)c->sm_count * 8));
-        gp_nt_apply<<<grid, T, 0, st>>>(D, tab, ar.ptr(keys), ar.ptr(pos), w);
+        gp_nt_apply<<<update_grid(items, T, c->sm_count), T, 0, st>>>(D, tab, ar.ptr(keys), ar.ptr(pos), w);
         if (W > 0) gp_nt_creation<<<(unsigned)((W + T - 1) / T), T, 0, st>>>(D, tc.ptr(p.creation), w);
     }
-    GP_CUDA(c, cudaGetLastError());
     int hw = 0;
-    ar.get(&hw, word);
-    GP_TRY(ar.sync(c));
-    t.live = true;
-    return refuse(c, hw, kNtRefusals, who);
+    return t.commit(c, ar, word, &hw, kNtRefusals, who);
 }
 
 }  // extern "C"

@@ -320,8 +320,8 @@ struct OhtDelta {
 // Update bookkeeping, read back with the error word: cells claimed and tombstones written by this update
 struct OhtWord { int err, unused; unsigned long long inserted, removed; };
 
-// Duplicates: slots and app keys through per-table stamps (the update's sequence number, atomicExch: a second writer of the
-// same slot sees its own update's number); member triples through a scratch set of the delta's keys.
+// Duplicates: slots and app keys through per-table stamps (stamped_twice); member triples through a scratch set of the delta's
+// keys.
 static __global__ void gp_oht_check(OhtDelta D, uint32_t* slot_stamp, uint32_t* rr_stamp, uint32_t seq, OhtSet dup, OhtWord* w) {
     const long long total = D.n_write + D.n_rr + D.n_member;
     int bad = 0;
@@ -329,7 +329,7 @@ static __global__ void gp_oht_check(OhtDelta D, uint32_t* slot_stamp, uint32_t* 
         if (i < D.n_write) {
             const int32_t s = D.slot[i], node = D.node_id[i];
             if (s < 0 || s >= D.n_slots) { bad |= kOhtErrRange; continue; }
-            if (atomicExch(slot_stamp + s, seq) == seq) bad |= kOhtErrDuplicate;
+            if (stamped_twice(slot_stamp + s, seq)) bad |= kOhtErrDuplicate;
             if (node == -1) continue;                                  // a free slot: nothing else is read
             if (node < 0 || node >= D.n_node_ids) bad |= kOhtErrRange;
             for (int d = 0; d < 3; ++d) {
@@ -344,7 +344,7 @@ static __global__ void gp_oht_check(OhtDelta D, uint32_t* slot_stamp, uint32_t* 
         } else if (i < D.n_write + D.n_rr) {
             const int32_t k = D.rr_app_key[i - D.n_write];
             if (k < 0 || k >= D.n_app_keys) { bad |= kOhtErrRange; continue; }
-            if (atomicExch(rr_stamp + k, seq) == seq) bad |= kOhtErrDuplicate;
+            if (stamped_twice(rr_stamp + k, seq)) bad |= kOhtErrDuplicate;
         } else {
             const long long m = i - D.n_write - D.n_rr;
             const int kind = D.member_kind[m];

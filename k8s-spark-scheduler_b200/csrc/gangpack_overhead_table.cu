@@ -1,5 +1,6 @@
 // gangpack_overhead_table.cu -- the resident overhead table: gp_overhead_table_reset, gp_overhead_table_update and
-// gp_overhead_table_query.  The kernels are in gangpack_overhead.cuh, next to the per-call ones they share.
+// gp_overhead_table_query.  The kernels are in gangpack_overhead.cuh, next to the per-call ones they share.  An update runs
+// within the protocol of gangpack_resident.cuh, with the member set's rehash target staged before it starts.
 #include "gangpack_ctx.cuh"
 #include "gangpack_overhead.cuh"
 
@@ -60,8 +61,6 @@ static const Refusal kOhtQueryRefusals[] = {
     {kOhErrSum, GP_ERR_UNREPRESENTABLE, "a per-node sum >= 2^61"},
 };
 
-static gp_status no_table(gp_ctx* c, const char* who) { return fail(c, GP_ERR_INVALID, who, "no overhead table (gp_overhead_table_reset first)"); }
-
 static uint32_t pow2_at_least(long long n, uint32_t lo) {
     uint32_t h = lo;
     while ((long long)h < n) h <<= 1;
@@ -104,33 +103,26 @@ gp_status gp_overhead_table_reset(gp_ctx* c, const gp_overhead_table_size* z) {
         return fail(c, GP_ERR_INVALID, who, "NULL size or a negative capacity");
     if (z->n_slots > INT32_MAX) return fail(c, GP_ERR_INVALID, who, "n_slots must be below 2^31");
     auto& t = c->oht;
-    t.live = false;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    cudaStream_t st = c->stream;
-    Arena a{t.cols, st};
-    const OhtPieces p = take_cols(a, *z);
-    a.reserve();
-    a.fill(p.node, 0xff);
-    a.fill(p.req, p.rr_stamp, 0);
-    Arena s{t.set[t.cur], st};
-    const auto cells = s.take<unsigned long long>(kOhtInitialCells);
-    s.reserve();
-    s.fill(cells, 0xff);
-    GP_TRY(a.sync(c));
-    GP_TRY(s.check(c));
-    t.size = *z;
-    t.cells = kOhtInitialCells;
-    t.keys = t.used = 0;
-    t.seq = 0;
-    t.live = true;
-    return GP_OK;
+    return t.reset(c, *z, [&](Arena& a) {
+        const OhtPieces p = take_cols(a, *z);
+        a.reserve();
+        a.fill(p.node, 0xff);
+        a.fill(p.req, p.rr_stamp, 0);
+        Arena s{t.set[t.cur], a.st};
+        const auto cells = s.take<unsigned long long>(kOhtInitialCells);
+        s.reserve();
+        s.fill(cells, 0xff);
+        t.cells = kOhtInitialCells;
+        t.keys = t.used = 0;
+        return s.check(c);
+    });
 }
 
 gp_status gp_overhead_table_update(gp_ctx* c, const gp_overhead_delta* d) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_overhead_table_update";
     auto& t = c->oht;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     if (!d || d->n_write < 0 || d->n_rr < 0 || d->n_member < 0 ||
         (d->n_write > 0 && (!d->slot || !d->node_id || !d->req_cpu_milli || !d->req_mem_bytes || !d->app_key || !d->app_id || !d->name_id)) ||
         (d->n_rr > 0 && (!d->rr_app_key || !d->rr_exists)) ||
@@ -192,19 +184,12 @@ gp_status gp_overhead_table_update(gp_ctx* c, const gp_overhead_delta* d) {
         nx.fill(to, 0xff);
         GP_TRY(nx.check(c));
     }
-    // From here on the table's own buffers are written: a CUDA error leaves no table (reset and replay)
-    t.live = false;
     Arena tc{t.cols, st};
     const OhtPieces p = take_cols(tc, t.size);
-    if (++t.seq == 0) {                                      // the stamps wrapped: none may equal a later update's number
-        tc.zero(p.slot_stamp);
-        tc.zero(p.rr_stamp);
-        t.seq = 1;
-    }
-    GP_TRY(tc.check(c));
+    GP_TRY(t.begin(c, tc, p.slot_stamp, p.rr_stamp));
     OhtWord* w = ar.ptr(word);
-    const int T = 256, cap = c->sm_count * 8;
-    auto grid = [&](long long n) { return (unsigned)std::max<long long>(1, std::min<long long>((n + T - 1) / T, cap)); };
+    const int T = 256;
+    auto grid = [&](long long n) { return update_grid(n, T, c->sm_count); };
     const long long total = (long long)W + (long long)R + (long long)M;
     if (total > 0)
         gp_oht_check<<<grid(total), T, 0, st>>>(D, tc.ptr(p.slot_stamp), tc.ptr(p.rr_stamp), t.seq, OhtSet{ar.ptr(dup), dup_cells - 1}, w);
@@ -219,12 +204,8 @@ gp_status gp_overhead_table_update(gp_ctx* c, const gp_overhead_delta* d) {
     }
     if (total > 0) gp_oht_apply<<<grid(total), T, 0, st>>>(D, cols_of(tc, p, S), set, w);
     if (ins > 0) gp_oht_insert<<<grid((long long)M), T, 0, st>>>(D, set, w);
-    GP_CUDA(c, cudaGetLastError());
     OhtWord hw{};
-    ar.get(&hw, word);
-    GP_TRY(ar.sync(c));
-    t.live = true;
-    GP_TRY(refuse(c, hw.err, kOhtRefusals, who));
+    GP_TRY(t.commit(c, ar, word, &hw, kOhtRefusals, who));
     t.keys += (long long)hw.inserted - (long long)hw.removed;
     t.used += (long long)hw.inserted;
     return GP_OK;
@@ -234,7 +215,7 @@ gp_status gp_overhead_table_query(gp_ctx* c, int32_t n_nodes, const int32_t* nod
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_overhead_table_query";
     auto& t = c->oht;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     if (!out || n_nodes < 0 || (n_nodes > 0 && !node_ids)) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
     GP_CUDA(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream;

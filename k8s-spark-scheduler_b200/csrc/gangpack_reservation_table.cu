@@ -2,14 +2,11 @@
 // The *_resident entries of gangpack_cluster.cu read it through rt_cols().
 //
 // An update runs
-//   gp_rt_check   thread per write: slot and node id ranges, duplicate slots (per-slot stamps holding the update's sequence
-//                 number, atomicExch: a second writer of a slot sees its own update's number), |value| < 2^61; sets the error
-//                 word and writes nothing else
+//   gp_rt_check   thread per write: slot and node id ranges, duplicate slots (stamped_twice), |value| < 2^61; sets the error
+//                 word and writes nothing but the stamps
 //   gp_rt_apply   thread per write: the whole row; nothing when the error word is set
-// so a refused delta leaves the table as it was.
+// within the update protocol of gangpack_resident.cuh, so a refused delta leaves the table as it was.
 #include "gangpack_ctx.cuh"
-
-#include <algorithm>
 
 enum : int {
     kRtErrRange = 1,            // a slot or node id out of its range
@@ -53,7 +50,7 @@ __global__ void gp_rt_check(RtDelta D, uint32_t* __restrict__ stamp, uint32_t se
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < D.n; i += (long long)gridDim.x * blockDim.x) {
         const int32_t s = D.slot[i], node = D.node_id[i];
         if (s < 0 || s >= D.n_slots) { bad |= kRtErrRange; continue; }
-        if (atomicExch(stamp + s, seq) == seq) bad |= kRtErrDuplicate;
+        if (stamped_twice(stamp + s, seq)) bad |= kRtErrDuplicate;
         if (node == -1) continue;                                      // a free slot: its values are not read
         if (node < 0 || node >= D.n_node_ids) bad |= kRtErrRange;
         for (int d = 0; d < 3; ++d) {
@@ -74,10 +71,6 @@ __global__ void gp_rt_apply(RtDelta D, int32_t* __restrict__ node, long long* __
     }
 }
 
-static gp_status no_table(gp_ctx* c, const char* who) {
-    return fail(c, GP_ERR_INVALID, who, "no reservation table (gp_reservation_table_reset first)");
-}
-
 RtCols rt_cols(gp_ctx* c) {
     auto& t = c->rt;
     Arena a{t.cols, c->stream};
@@ -95,26 +88,20 @@ gp_status gp_reservation_table_reset(gp_ctx* c, const gp_reservation_table_size*
     static const char* who = "gp_reservation_table_reset";
     if (!z || z->n_slots < 0 || z->n_node_ids < 0) return fail(c, GP_ERR_INVALID, who, "NULL size or a negative capacity");
     if (z->n_slots > INT32_MAX) return fail(c, GP_ERR_INVALID, who, "n_slots must be below 2^31");
-    auto& t = c->rt;
-    t.live = false;
-    GP_CUDA(c, cudaSetDevice(c->device));
-    Arena a{t.cols, c->stream};
-    const RtPieces p = take_cols(a, *z);
-    a.reserve();
-    a.fill(p.node, 0xff);
-    a.fill(p.v, p.stamp, 0);
-    GP_TRY(a.sync(c));
-    t.size = *z;
-    t.seq = 0;
-    t.live = true;
-    return GP_OK;
+    return c->rt.reset(c, *z, [&](Arena& a) {
+        const RtPieces p = take_cols(a, *z);
+        a.reserve();
+        a.fill(p.node, 0xff);
+        a.fill(p.v, p.stamp, 0);
+        return GP_OK;
+    });
 }
 
 gp_status gp_reservation_table_update(gp_ctx* c, const gp_reservation_delta* d) {
     if (!enter(c)) return GP_ERR_INVALID;
     static const char* who = "gp_reservation_table_update";
     auto& t = c->rt;
-    if (!t.live) return no_table(c, who);
+    GP_TRY(require(c, t.need(), who));
     if (!d || d->n_write < 0 || (d->n_write > 0 && (!d->slot || !d->node_id || !d->cpu_milli || !d->mem_bytes)))
         return fail(c, GP_ERR_INVALID, who, "missing arrays or a negative count");
     if (d->n_write > t.size.n_slots) return fail(c, GP_ERR_INVALID, who, "more slot writes than slots: a slot given twice or out of range");
@@ -135,28 +122,18 @@ gp_status gp_reservation_table_update(gp_ctx* c, const gp_reservation_delta* d) 
     const int64_t* vals[3] = {d->cpu_milli, d->mem_bytes, d->gpu};
     for (int k = 0; k < 3; ++k) D.v[k] = ar.put(val.part(W * k, W), vals[k]);
     GP_TRY(ar.check(c));
-    // From here on the table's own buffers are written: a CUDA error leaves no table (reset and replay)
-    t.live = false;
     Arena tc{t.cols, st};
     const RtPieces p = take_cols(tc, t.size);
-    if (++t.seq == 0) {                                      // the stamps wrapped: none may equal a later update's number
-        tc.zero(p.stamp);
-        t.seq = 1;
-    }
-    GP_TRY(tc.check(c));
+    GP_TRY(t.begin(c, tc, p.stamp, p.stamp));
     int* w = ar.ptr(word);
     if (W > 0) {
         const int T = 256;
-        const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(((long long)W + T - 1) / T, (long long)c->sm_count * 8));
+        const unsigned grid = update_grid((long long)W, T, c->sm_count);
         gp_rt_check<<<grid, T, 0, st>>>(D, tc.ptr(p.stamp), t.seq, w);
         gp_rt_apply<<<grid, T, 0, st>>>(D, tc.ptr(p.node), tc.ptr(p.v), w);
     }
-    GP_CUDA(c, cudaGetLastError());
     int hw = 0;
-    ar.get(&hw, word);
-    GP_TRY(ar.sync(c));
-    t.live = true;
-    return refuse(c, hw, kRtRefusals, who);
+    return t.commit(c, ar, word, &hw, kRtRefusals, who);
 }
 
 }  // extern "C"

@@ -17,33 +17,31 @@ import heapq
 
 import numpy as np
 
+from .resident import ResidentTable
+
 QUANTITIES = ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")
 DELTA_COLUMNS = ("drv_cpu_milli", "drv_mem_bytes", "drv_gpu", "exe_cpu_milli", "exe_mem_bytes", "exe_gpu")
 _ABSENT = (False, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, False)
 
 
-class DriverTable:
+class DriverTable(ResidentTable):
     """Every pending driver as the resident driver table keeps it: set_driver(uid, creation, scheduler, group, resources,
     exact) for an add or an update (resources None: the annotations do not parse, so the driver is deleted), delete_driver(uid)
     when it is bound, deleted or terminating.  resources is sparkResources' dict ({"drv": [cpu, mem, gpu], "exe": [...],
     "min": MinExecutorCount}).
 
-    delta() -> the arrays of one gp_driver_table_update: the slots that changed.  When it carries "reset" (the first one,
-    whenever the slot, group or scheduler capacity would be exceeded -- it is doubled and the whole state replayed -- and after
-    replay()), gp_driver_table_reset(**delta["reset"]) goes first.  flush(packer) does both, replays once more after a refused
-    update, and keeps `mirror`."""
+    delta() -> the arrays of one gp_driver_table_update: the slots that changed; see ResidentTable."""
+
+    name, writes = "driver", ("slot",)
 
     def __init__(self, n_slots=64, n_groups=4, n_schedulers=2):
-        self.size = dict(n_slots=int(n_slots), n_groups=int(n_groups), n_schedulers=int(n_schedulers))
+        super().__init__(DriverMirror(), n_slots=int(n_slots), n_groups=int(n_groups), n_schedulers=int(n_schedulers))
         self.rows = {}                                  # uid -> the row as a delta writes it
         self._slot, self._uid_at = {}, {}               # uid -> slot, slot -> uid
         self._free, self._next = [], 0                  # freed slots (a heap), the first slot never used
         self.schedulers, self.groups = {}, {}           # interners: name -> id
         self._dirty = set()
         self._sent = {}                                 # slot -> the row the device holds
-        self._replay = True
-        self.replays = 0
-        self.mirror = DriverMirror()
 
     # ---- events
     def set_driver(self, uid, creation, scheduler, group, resources, exact=True):
@@ -97,52 +95,29 @@ class DriverTable:
                 sg[g] = int(group_index[name])
         return sg
 
-    # ---- updates
-    def replay(self):
-        """The next delta resets the table and resends the whole state (after an update that was refused or failed)."""
-        self._replay = True
+    # ---- internals
+    def _bounds(self):
+        return dict(n_slots=self._next, n_groups=len(self.groups), n_schedulers=len(self.schedulers))
 
-    def delta(self) -> dict:
-        for key, need in (("n_slots", self._next), ("n_groups", len(self.groups)), ("n_schedulers", len(self.schedulers))):
-            while self.size[key] < need:
-                self.size[key] = max(2 * self.size[key], 1)
-                self._replay = True
-        if self._replay:
+    def _changes(self, replay):
+        if replay:
             self._sent = {}
             slots = sorted(self._uid_at)
-            self.replays += 1
         else:                                           # a row changed and changed back (or added and deleted) is not sent
             slots = [s for s in sorted(self._dirty) if self._record(s) != self._sent.get(s, _ABSENT)]
         rec = [self._record(s) for s in slots]
         for s, r in zip(slots, rec):
             self._sent[s] = r
         col = lambda j, dt: np.array([r[j] for r in rec], dt)
-        d = {"reset": dict(self.size) if self._replay else None, "slot": np.array(slots, np.int32), "present": col(0, np.uint8),
+        d = {"slot": np.array(slots, np.int32), "present": col(0, np.uint8),
              "creation": col(1, np.int64), "scheduler": col(2, np.int32), "group": col(3, np.int32)}
         for j, k in enumerate(DELTA_COLUMNS):
             d[k] = col(4 + j, np.int64)
         d["min_executor_count"] = col(10, np.int32)
         d["exact"] = col(11, np.uint8)
         self._dirty = set()
-        self._replay = False
         return d
 
-    def flush(self, packer):
-        """One update of the device's table (none when nothing changed), preceded by a reset when the delta carries one; on
-        a refusal the whole state is reset and replayed once more, and a second refusal is raised."""
-        from .native import GangpackError
-        d = self.delta()
-        if d["reset"] is None and len(d["slot"]) == 0:
-            return
-        try:
-            self._push(packer, d)
-        except GangpackError:
-            self.replay()
-            d = self.delta()
-            self._push(packer, d)
-        self.mirror.apply(d)
-
-    # ---- internals
     def _take_new(self):
         s = self._next
         self._next += 1
@@ -157,12 +132,6 @@ class DriverTable:
     def _record(self, s):
         uid = self._uid_at.get(s)
         return _ABSENT if uid is None else self.rows[uid]
-
-    @staticmethod
-    def _push(packer, d):
-        if d["reset"] is not None:
-            packer.driver_table_reset(**d["reset"])
-        packer.driver_table_update(d)
 
 
 class DriverMirror:

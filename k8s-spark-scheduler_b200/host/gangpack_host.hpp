@@ -267,6 +267,40 @@ inline binpack::PackingResult PackOne(gp_algo algo, const resources::Resources& 
     }
 }
 
+// What the host side of every resident table (gp_*_table_*) shares: the size the table is reset with, capacities that double
+// and force a replay, and the step that sends a delta.  A Flush assembles its delta from the whole state while Replaying(),
+// else from what changed, and hands it to Send.
+template <class Size>
+class ResidentTable {
+public:
+    // the next Flush resets the table and sends the whole state again (after a refused resident call)
+    void Replay() { replay_ = true; ++replays_; }
+    int Replays() const { return replays_; }      // Replay calls: a host path's fallback after a refused device call is one
+
+protected:
+    explicit ResidentTable(Size initial) : size_(initial) {}
+    bool Replaying() const { return replay_; }
+    template <class T> void Grow(T& cap, int64_t need) {
+        while (cap < need) { cap = std::max<T>(2 * cap, 1); replay_ = true; }
+    }
+    // The reset when replaying, then the update of *d (none when d is NULL).  Until both calls return the next Flush replays:
+    // a call that throws leaves the device's table to be rebuilt.
+    template <class Reset, class Update, class Delta>
+    void Send(Device& dev, Reset reset, const char* resetName, Update update, const char* updateName, const Delta* d) {
+        const bool replaying = replay_;
+        replay_ = true;
+        if (replaying) dev.check(reset(dev.ctx(), &size_), resetName);
+        if (d) dev.check(update(dev.ctx(), d), updateName);
+        replay_ = false;
+    }
+
+    Size size_;
+
+private:
+    bool replay_ = true;
+    int replays_ = 0;
+};
+
 }  // namespace gangpack
 
 namespace binpack {
@@ -874,9 +908,9 @@ inline MatchResult MatchRequiredNodeAffinity(const std::vector<Node>& nodes, con
 // id 0 of each reserved for strings no node carries, so encoding a program never changes the table; node ids freed by a
 // delete go to the next new node.  Flush sends what changed since the last flush in one update, after a reset with doubled
 // capacities and the whole state when a capacity would be exceeded (or after Replay).
-class ResidentLabels {
+class ResidentLabels : public gangpack::ResidentTable<gp_label_table_size> {
 public:
-    explicit ResidentLabels(gp_label_table_size initial = {64, 16, 64, 256}) : size_(initial) {
+    explicit ResidentLabels(gp_label_table_size initial = {64, 16, 64, 256}) : ResidentTable(initial) {
         parsed_.push_back({0, 0});                       // value id 0: reserved
     }
 
@@ -942,17 +976,13 @@ public:
     int32_t KeyID(const std::string& k) const { auto it = keyId_.find(k); return it == keyId_.end() ? 0 : it->second; }
     int32_t ValueID(const std::string& v) const { auto it = valId_.find(v); return it == valId_.end() ? 0 : it->second; }
 
-    // the next Flush resets the table and sends the whole state again (after a refused resident call)
-    void Replay() { replay_ = true; }
-
     void Flush(gangpack::Device& dev) {
         int32_t longest = 0;
         for (const auto& r : rows_) longest = std::max(longest, (int32_t)r.size());
-        auto grow = [&](int32_t& cap, int64_t need) { while (cap < need) { cap = std::max<int32_t>(2 * cap, 1); replay_ = true; } };
-        grow(size_.n_node_ids, (int64_t)rows_.size());
-        grow(size_.max_labels, longest);
-        grow(size_.n_keys, (int64_t)keyId_.size() + 1);
-        grow(size_.n_values, (int64_t)parsed_.size());
+        Grow(size_.n_node_ids, (int64_t)rows_.size());
+        Grow(size_.max_labels, longest);
+        Grow(size_.n_keys, (int64_t)keyId_.size() + 1);
+        Grow(size_.n_values, (int64_t)parsed_.size());
         std::vector<int32_t> rowNode, key, val, valueId;
         std::vector<int64_t> off{0}, valueInt;
         std::vector<uint8_t> valueOk;
@@ -962,24 +992,19 @@ public:
             off.push_back((int64_t)key.size());
         };
         auto value = [&](int32_t v) { valueId.push_back(v); valueOk.push_back(parsed_[(size_t)v].first); valueInt.push_back(parsed_[(size_t)v].second); };
-        if (replay_) {
+        if (Replaying()) {
             for (int32_t at = 0; at < (int32_t)rows_.size(); ++at) if (!rows_[(size_t)at].empty()) row(at);
             for (int32_t v = 1; v < (int32_t)parsed_.size(); ++v) value(v);
         } else {
             for (int32_t at : dirty_) row(at);
             for (int32_t v : newVals_) value(v);
         }
-        const bool reset = replay_;
-        replay_ = true;                            // until the table holds this state: a failed call replays next time
-        if (reset) dev.check(gp_label_table_reset(dev.ctx(), &size_), "gp_label_table_reset");
-        if (!rowNode.empty() || !valueId.empty()) {
-            for (auto* v : {&key, &val, &rowNode, &valueId}) v->reserve(1);
-            valueOk.reserve(1); valueInt.reserve(1);
-            gp_label_delta d{(int32_t)rowNode.size(), (int32_t)valueId.size(), rowNode.data(), off.data(), key.data(), val.data(),
-                             valueId.data(), valueOk.data(), valueInt.data()};
-            dev.check(gp_label_table_update(dev.ctx(), &d), "gp_label_table_update");
-        }
-        replay_ = false;
+        for (auto* v : {&key, &val, &rowNode, &valueId}) v->reserve(1);
+        valueOk.reserve(1); valueInt.reserve(1);
+        gp_label_delta d{(int32_t)rowNode.size(), (int32_t)valueId.size(), rowNode.data(), off.data(), key.data(), val.data(),
+                         valueId.data(), valueOk.data(), valueInt.data()};
+        Send(dev, gp_label_table_reset, "gp_label_table_reset", gp_label_table_update, "gp_label_table_update",
+             rowNode.empty() && valueId.empty() ? nullptr : &d);
         dirty_.clear();
         newVals_.clear();
     }
@@ -998,8 +1023,6 @@ private:
         return id;
     }
 
-    gp_label_table_size size_;
-    bool replay_ = true;
     std::map<std::string, std::map<std::string, std::string>> labels_;
     std::unordered_map<std::string, int32_t> nodes_, keyId_, valId_;   // key ids start at 1, value ids at 1
     std::vector<std::pair<uint8_t, int64_t>> parsed_;             // per value id: ParseInt of the string
@@ -1050,10 +1073,10 @@ namespace resources {
 // when no gap is left every present node gets an evenly spaced key and the next delta carries every row.  Flush sends the
 // rows that differ from what the device holds as one gp_node_table_update, after a reset with a doubled capacity and the
 // whole state when a node id would not fit (or after Replay, or a failed flush).
-class ResidentNodes {
+class ResidentNodes : public gangpack::ResidentTable<gp_node_table_size> {
 public:
     explicit ResidentNodes(const affinity::ResidentLabels& labels, int32_t nNodeIds = 64, int keyBits = 62)
-        : labels_(labels), size_{nNodeIds, 0}, keyHi_((int64_t)1 << keyBits) {}
+        : ResidentTable({nNodeIds, 0}), labels_(labels), keyHi_((int64_t)1 << keyBits) {}
 
     // creationUnixNano: metav1.Time as UnixNano (the failover reconciler's newest-first order)
     void SetNode(const std::string& name, const Resources& allocatable, bool unschedulable, bool ready, int64_t creationUnixNano = 0) {
@@ -1100,7 +1123,6 @@ public:
     }
     int64_t NameKey(const std::string& name) const { return nodes_.at(name).row.key; }
     int Relabels() const { return relabels_; }
-    int Replays() const { return replays_; }      // Replay calls: a host path's fallback after a refused device call is one
 
     // the per-call columns the node-table entries stand for: allocatable, name_rank (the byte order of the listed names, a
     // permutation of 0..n-1), unschedulable, ready and creation
@@ -1127,11 +1149,8 @@ public:
         return c;
     }
 
-    void Replay() { replay_ = true; ++replays_; }
-
     void Flush(gangpack::Device& dev) {
-        const int32_t need = nameAt_.empty() ? 0 : nameAt_.rbegin()->first + 1;
-        while (size_.n_node_ids < need) { size_.n_node_ids = std::max<int32_t>(2 * size_.n_node_ids, 1); replay_ = true; }
+        Grow(size_.n_node_ids, nameAt_.empty() ? 0 : nameAt_.rbegin()->first + 1);
         std::vector<int32_t> id;
         std::vector<uint8_t> present, uns, rdy;
         std::vector<int64_t> v[3], key, cre;
@@ -1142,7 +1161,7 @@ public:
             key.push_back(r.key);
             cre.push_back(r.creation);
         };
-        if (replay_) {
+        if (Replaying()) {
             sent_.clear();
             for (const auto& kv : nameAt_) row(kv.first);
         } else {
@@ -1151,16 +1170,10 @@ public:
                 if (!(record(at) == (s == sent_.end() ? Row{} : s->second))) row(at);
             }
         }
-        const bool reset = replay_;
-        replay_ = true;                            // until the table holds this state: a failed call replays next time
-        if (reset) dev.check(gp_node_table_reset(dev.ctx(), &size_), "gp_node_table_reset");
-        if (!id.empty()) {
-            gp_node_delta d{(int32_t)id.size(), 0, id.data(), present.data(), v[0].data(), v[1].data(), v[2].data(), uns.data(),
-                            rdy.data(), key.data(), cre.data()};
-            dev.check(gp_node_table_update(dev.ctx(), &d), "gp_node_table_update");
-        }
+        gp_node_delta d{(int32_t)id.size(), 0, id.data(), present.data(), v[0].data(), v[1].data(), v[2].data(), uns.data(),
+                        rdy.data(), key.data(), cre.data()};
+        Send(dev, gp_node_table_reset, "gp_node_table_reset", gp_node_table_update, "gp_node_table_update", id.empty() ? nullptr : &d);
         for (int32_t at : id) sent_[at] = record(at);
-        replay_ = false;
         dirty_.clear();
     }
 
@@ -1204,11 +1217,8 @@ private:
     }
 
     const affinity::ResidentLabels& labels_;
-    gp_node_table_size size_;
     int64_t keyHi_;
-    bool replay_ = true;
     int relabels_ = 0;
-    int replays_ = 0;
     std::unordered_map<std::string, Held> nodes_;
     std::map<int32_t, std::string> nameAt_;
     std::set<std::string> byName_;
@@ -2086,9 +2096,9 @@ private:
 // one gp_overhead_table_query.  Ids come from reference-counted interners, so the ids of names that are gone are reused; a
 // capacity that would be exceeded is doubled and the whole state replayed after a reset.  The table belongs to the
 // device context, so one instance per context.
-class ResidentOverheadComputer {
+class ResidentOverheadComputer : public gangpack::ResidentTable<gp_overhead_table_size> {
 public:
-    explicit ResidentOverheadComputer(gp_overhead_table_size initial = {64, 64, 64, 64, 64}) : size_(initial) {}
+    explicit ResidentOverheadComputer(gp_overhead_table_size initial = {64, 64, 64, 64, 64}) : ResidentTable(initial) {}
     ResidentOverheadComputer(const ResidentOverheadComputer&) = delete;            // rows hold pointers to its interners
     ResidentOverheadComputer& operator=(const ResidentOverheadComputer&) = delete;
 
@@ -2143,7 +2153,6 @@ public:
         }
         return ids;
     }
-    void Replay() { replay_ = true; }
 
     resources::NodeGroupResources GetOverhead(const std::vector<std::string>& nodes) { return compute(nodes).first; }
     resources::NodeGroupResources GetNonSchedulableOverhead(const std::vector<std::string>& nodes) { return compute(nodes).second; }
@@ -2314,11 +2323,9 @@ private:
 
     // The changes since the last update (everything after a reset) as one gp_overhead_table_update
     void flush(gangpack::Device& dev) {
-        auto grow = [&](int64_t& cap, int64_t need) { while (cap < need) { cap = std::max<int64_t>(2 * cap, 1); replay_ = true; } };
-        int64_t caps[5] = {size_.n_slots, size_.n_node_ids, size_.n_app_keys, size_.n_app_ids, size_.n_names};
-        grow(caps[0], (int64_t)slots_.size());
-        grow(caps[1], nodes_.bound()); grow(caps[2], keys_.bound()); grow(caps[3], apps_.bound()); grow(caps[4], names_.bound());
-        size_ = gp_overhead_table_size{caps[0], (int32_t)caps[1], (int32_t)caps[2], (int32_t)caps[3], (int32_t)caps[4]};
+        Grow(size_.n_slots, (int64_t)slots_.size());
+        Grow(size_.n_node_ids, nodes_.bound()); Grow(size_.n_app_keys, keys_.bound()); Grow(size_.n_app_ids, apps_.bound());
+        Grow(size_.n_names, names_.bound());
         std::vector<int32_t> slot, node, ak, ai, nm, rrKey, mApp, mName;
         std::vector<int64_t> cpu, mem, gpu;
         std::vector<uint8_t> listed, exe, spark, rrOn, mKind, mPresent;
@@ -2333,7 +2340,7 @@ private:
             mKind.push_back((uint8_t)std::get<0>(m)); mApp.push_back(std::get<1>(m)); mName.push_back(std::get<2>(m));
             mPresent.push_back(present);
         };
-        if (replay_) {
+        if (Replaying()) {
             for (size_t i = 0; i < rows_.size(); ++i) if (rows_[i] != Row{}) row(i);
             for (int32_t k : flags_) { rrKey.push_back(k); rrOn.push_back(1); }
             for (const auto& kv : members_) member(kv.first, true);
@@ -2349,26 +2356,19 @@ private:
                 if (on != kv.second) member(kv.first, on);
             }
         }
-        const bool reset = replay_;
-        replay_ = true;                            // until the table holds this state: a failed call replays next time
-        if (reset) dev.check(gp_overhead_table_reset(dev.ctx(), &size_), "gp_overhead_table_reset");
-        if (reset || !slot.empty() || !rrKey.empty() || !mKind.empty()) {
-            gp_overhead_delta d{};
-            d.n_write = (int64_t)slot.size();
-            d.slot = slot.data(); d.node_id = node.data(); d.req_cpu_milli = cpu.data(); d.req_mem_bytes = mem.data(); d.req_gpu = gpu.data();
-            d.listed = listed.data(); d.app_key = ak.data(); d.app_id = ai.data(); d.name_id = nm.data();
-            d.is_executor = exe.data(); d.spark_scheduler = spark.data();
-            d.n_rr = (int32_t)rrKey.size(); d.rr_app_key = rrKey.data(); d.rr_exists = rrOn.data();
-            d.n_member = (int64_t)mKind.size();
-            d.member_kind = mKind.data(); d.member_app = mApp.data(); d.member_name = mName.data(); d.member_present = mPresent.data();
-            dev.check(gp_overhead_table_update(dev.ctx(), &d), "gp_overhead_table_update");
-        }
-        replay_ = false;
+        gp_overhead_delta d{};
+        d.n_write = (int64_t)slot.size();
+        d.slot = slot.data(); d.node_id = node.data(); d.req_cpu_milli = cpu.data(); d.req_mem_bytes = mem.data(); d.req_gpu = gpu.data();
+        d.listed = listed.data(); d.app_key = ak.data(); d.app_id = ai.data(); d.name_id = nm.data();
+        d.is_executor = exe.data(); d.spark_scheduler = spark.data();
+        d.n_rr = (int32_t)rrKey.size(); d.rr_app_key = rrKey.data(); d.rr_exists = rrOn.data();
+        d.n_member = (int64_t)mKind.size();
+        d.member_kind = mKind.data(); d.member_app = mApp.data(); d.member_name = mName.data(); d.member_present = mPresent.data();
+        Send(dev, gp_overhead_table_reset, "gp_overhead_table_reset", gp_overhead_table_update, "gp_overhead_table_update",
+             slot.empty() && rrKey.empty() && mKind.empty() ? nullptr : &d);
         dirty_.clear(); flagTouched_.clear(); memberTouched_.clear();
     }
 
-    gp_overhead_table_size size_;
-    bool replay_ = true;
     std::vector<Slot> slots_;
     std::vector<size_t> free_;
     std::map<std::pair<std::string, std::string>, size_t> at_;   // (node, UID) -> slot
@@ -2394,12 +2394,12 @@ private:
 // gp_reschedule_from_reservations_resident with NodeIDs(nodes).  Freed slots are reused and node ids are reference-counted;
 // a capacity that would be exceeded is doubled, and after a reset, a refused or a failed update the whole state is sent
 // again until an update succeeds.  The table belongs to the device context, so one instance per context.
-class ResidentReservations {
+class ResidentReservations : public gangpack::ResidentTable<gp_reservation_table_size> {
 public:
     struct Reservation { std::string Node; resources::Resources Res; };
     using Entries = std::map<std::string, Reservation>;           // name (reservation entry or pod) -> reservation
 
-    explicit ResidentReservations(gp_reservation_table_size initial = {64, 64}) : size_(initial) {}
+    explicit ResidentReservations(gp_reservation_table_size initial = {64, 64}) : ResidentTable(initial) {}
 
     // a ResourceReservation created, updated or rewritten by compaction (its Spec.Reservations), and its deletion
     void SetResourceReservation(const std::string& ns, const std::string& app, const Entries& e) { set(0, ns + '\x00' + app, e, rrs_); }
@@ -2418,8 +2418,6 @@ public:
         return ids;
     }
 
-    // the next Flush resets the table and sends the whole state again (after a refused resident call)
-    void Replay() { replay_ = true; }
     // GetReservedResources' rows as the per-call reconciler takes them
     std::vector<ReconcileRow> Rows() const {
         std::vector<ReconcileRow> rows;
@@ -2430,30 +2428,22 @@ public:
     }
 
     void Flush(gangpack::Device& dev) {
-        auto grow = [&](int64_t& cap, int64_t need) { while (cap < need) { cap = std::max<int64_t>(2 * cap, 1); replay_ = true; } };
-        int64_t caps[2] = {size_.n_slots, size_.n_node_ids};
-        grow(caps[0], (int64_t)rows_.size());
-        grow(caps[1], (int64_t)nodeCount_.size());
-        size_ = gp_reservation_table_size{caps[0], (int32_t)caps[1]};
+        Grow(size_.n_slots, (int64_t)rows_.size());
+        Grow(size_.n_node_ids, (int64_t)nodeCount_.size());
         std::vector<int32_t> slot, node;
         std::vector<int64_t> cpu, mem, gpu;
         auto row = [&](size_t i) {
             slot.push_back((int32_t)i); node.push_back(rows_[i].node);
             cpu.push_back(rows_[i].v[0]); mem.push_back(rows_[i].v[1]); gpu.push_back(rows_[i].v[2]);
         };
-        if (replay_) {
+        if (Replaying()) {
             for (size_t i = 0; i < rows_.size(); ++i) if (rows_[i].node != -1) row(i);
         } else {
             for (const auto& kv : dirty_) if (rows_[kv.first] != kv.second) row(kv.first);
         }
-        const bool reset = replay_;
-        replay_ = true;                            // until the table holds this state: a failed call replays next time
-        if (reset) dev.check(gp_reservation_table_reset(dev.ctx(), &size_), "gp_reservation_table_reset");
-        if (!slot.empty()) {
-            gp_reservation_delta d{(int64_t)slot.size(), slot.data(), node.data(), cpu.data(), mem.data(), gpu.data()};
-            dev.check(gp_reservation_table_update(dev.ctx(), &d), "gp_reservation_table_update");
-        }
-        replay_ = false;
+        gp_reservation_delta d{(int64_t)slot.size(), slot.data(), node.data(), cpu.data(), mem.data(), gpu.data()};
+        Send(dev, gp_reservation_table_reset, "gp_reservation_table_reset", gp_reservation_table_update, "gp_reservation_table_update",
+             slot.empty() ? nullptr : &d);
         dirty_.clear();
     }
 
@@ -2523,8 +2513,6 @@ private:
         if (--nodeCount_[(size_t)i] == 0) { nodes_.erase(it); freeIds_.push_back(i); }
     }
 
-    gp_reservation_table_size size_;
-    bool replay_ = true;
     std::map<std::string, Entries> rrs_, soft_;
     std::map<Key, size_t> slot_;
     std::vector<Row> rows_;
@@ -2855,9 +2843,9 @@ inline std::vector<ReconcileResult> ReconcileFindNodesNodeTable(const std::vecto
 // gp_driver_table_update, after a reset with doubled capacities and the whole state when a slot, group or scheduler id would
 // not fit (or after Replay, or a failed flush).  The host keeps every row, so a refused device call can fall back to
 // FilterToEarliestAndSort and the per-call FIFO batch over the same drivers (Pods, Pending).
-class ResidentDrivers {
+class ResidentDrivers : public gangpack::ResidentTable<gp_driver_table_size> {
 public:
-    explicit ResidentDrivers(gp_driver_table_size size = gp_driver_table_size{64, 4, 2, 0}) : size_(size) {}
+    explicit ResidentDrivers(gp_driver_table_size size = gp_driver_table_size{64, 4, 2, 0}) : ResidentTable(size) {}
 
     void SetDriver(const QueuedDriverPod& pod, const std::map<std::string, std::string>& annotations) {
         ParsedSparkResources r;
@@ -2896,7 +2884,6 @@ public:
 
     int32_t Slot(const std::string& uid) const { auto it = held_.find(uid); return it == held_.end() ? -1 : it->second.slot; }
     bool Holds(const std::string& uid) const { return held_.count(uid) != 0; }
-    int Replays() const { return replays_; }
     const gp_driver_table_size& Size() const { return size_; }
     // enforce_after_ns of every group id: its instance group's override, else the default (DefaultEnforceAfterPodAge)
     std::vector<int64_t> GroupAges(int64_t defaultNs, const std::map<std::string, int64_t>& overrides = {}) const {
@@ -2927,13 +2914,10 @@ public:
     bool Exact(const std::string& uid) const { return held_.at(uid).row.exact; }
     int32_t GroupID(const std::string& uid) const { return held_.at(uid).row.group; }
 
-    void Replay() { replay_ = true; ++replays_; }
-
     void Flush(gangpack::Device& dev) {
-        auto grow = [&](int32_t& cap, int32_t need) { while (cap < need) { cap = std::max<int32_t>(2 * cap, 1); replay_ = true; } };
-        grow(size_.n_slots, next_);
-        grow(size_.n_groups, (int32_t)groups_.size());
-        grow(size_.n_schedulers, (int32_t)schedulers_.size());
+        Grow(size_.n_slots, next_);
+        Grow(size_.n_groups, (int64_t)groups_.size());
+        Grow(size_.n_schedulers, (int64_t)schedulers_.size());
         std::vector<int32_t> slot, sched, group, count;
         std::vector<uint8_t> present, exact;
         std::vector<int64_t> creation, q[6];
@@ -2943,7 +2927,7 @@ public:
             sched.push_back(r.scheduler); group.push_back(r.group); count.push_back(r.count);
             for (int k = 0; k < 6; ++k) q[k].push_back(r.q[k]);
         };
-        if (replay_) {
+        if (Replaying()) {
             sent_.clear();
             for (const auto& kv : uidAt_) row(kv.first);
         } else {
@@ -2952,16 +2936,11 @@ public:
                 if (!(record(s) == (it == sent_.end() ? Row{} : it->second))) row(s);
             }
         }
-        const bool reset = replay_;
-        replay_ = true;                            // until the table holds this state: a failed call replays next time
-        if (reset) dev.check(gp_driver_table_reset(dev.ctx(), &size_), "gp_driver_table_reset");
-        if (!slot.empty()) {
-            gp_driver_delta d{(int32_t)slot.size(), 0, slot.data(), present.data(), creation.data(), sched.data(), group.data(),
-                              q[0].data(), q[1].data(), q[2].data(), q[3].data(), q[4].data(), q[5].data(), count.data(), exact.data()};
-            dev.check(gp_driver_table_update(dev.ctx(), &d), "gp_driver_table_update");
-        }
+        gp_driver_delta d{(int32_t)slot.size(), 0, slot.data(), present.data(), creation.data(), sched.data(), group.data(),
+                          q[0].data(), q[1].data(), q[2].data(), q[3].data(), q[4].data(), q[5].data(), count.data(), exact.data()};
+        Send(dev, gp_driver_table_reset, "gp_driver_table_reset", gp_driver_table_update, "gp_driver_table_update",
+             slot.empty() ? nullptr : &d);
         for (int32_t s : slot) sent_[s] = record(s);
-        replay_ = false;
         dirty_.clear();
     }
 
@@ -2989,7 +2968,6 @@ private:
     }
     Row record(int32_t s) const { auto it = uidAt_.find(s); return it == uidAt_.end() ? Row{} : held_.at(it->second).row; }
 
-    gp_driver_table_size size_;
     std::map<std::string, Held> held_;
     std::map<int32_t, std::string> uidAt_;       // slot -> uid, in slot order
     std::set<int32_t> free_;
@@ -2997,8 +2975,6 @@ private:
     std::map<std::string, int32_t> schedulers_, groups_;
     std::set<int32_t> dirty_;
     std::map<int32_t, Row> sent_;
-    bool replay_ = true;
-    int replays_ = 0;
 };
 
 // What selectDriverNode's FIFO step decides for the requesting driver: fits (result = its packing), failure-fit (-1) or

@@ -20,6 +20,8 @@ import bisect
 
 import numpy as np
 
+from .resident import ResidentTable
+
 ZONE_LABEL = "failure-domain.beta.kubernetes.io/zone"
 DEFAULT_ZONE = "default"
 
@@ -27,21 +29,21 @@ DEFAULT_ZONE = "default"
 _ABSENT = (False, 0, 0, 0, False, False, 0, 0)
 
 
-class NodeTable:
+class NodeTable(ResidentTable):
     """Every node's allocatable, unschedulable and ready flags, creation time and name order, as the resident node table keeps
     them: set_node(name, allocatable, unschedulable, ready, creation) for an add or an update (after the label table's set_node, which
     gives the node its id; nothing changes when the values are the same), delete_node(name) (before the label table's
     delete_node, which frees the id).
 
     delta() -> the arrays of one gp_node_table_update: the rows of the nodes that changed (a deleted node's row written
-    absent), or every present row after a relabel.  When it carries "reset" (the first one, whenever the id capacity would
-    be exceeded: it is doubled and the whole state replayed, and after replay()), gp_node_table_reset(**delta["reset"])
-    goes first.  flush(packer) does both and keeps `mirror`, a numpy copy of what the device holds.  key_bits bounds the
-    keys to [0, 2^key_bits); a smaller value makes relabels frequent (tests)."""
+    absent), or every present row after a relabel; see ResidentTable.  key_bits bounds the keys to [0, 2^key_bits); a
+    smaller value makes relabels frequent (tests)."""
+
+    name, writes = "node", ("node_id",)
 
     def __init__(self, labels, n_node_ids=64, key_bits=62):
+        super().__init__(NodeMirror(), n_node_ids=n_node_ids)
         self.labels = labels
-        self.size = dict(n_node_ids=n_node_ids)
         self._key_hi = 1 << key_bits
         self.nodes = {}                                 # name -> (cpu, mem, gpu, unschedulable, ready)
         self.creation = {}                              # name -> creation time (UnixNano)
@@ -50,9 +52,7 @@ class NodeTable:
         self._sorted = []                               # the present names' bytes, ascending
         self._dirty = set()
         self._sent = {}                                 # node id -> the row the device holds (as _record gives it)
-        self._replay = True
         self.relabels = 0
-        self.mirror = NodeMirror()
 
     # ---- events
     def set_node(self, name, allocatable, unschedulable, ready, creation=0):
@@ -94,17 +94,12 @@ class NodeTable:
     def name_key(self, name) -> int:
         return self._key[name]
 
-    # ---- updates
-    def replay(self):
-        """The next delta resets the table and resends the whole state (after an update that was refused or failed)."""
-        self._replay = True
+    # ---- internals
+    def _bounds(self):
+        return dict(n_node_ids=max(self._name_at, default=-1) + 1)
 
-    def delta(self) -> dict:
-        need = max(self._name_at, default=-1) + 1
-        while self.size["n_node_ids"] < need:
-            self.size["n_node_ids"] = max(2 * self.size["n_node_ids"], 1)
-            self._replay = True
-        if self._replay:
+    def _changes(self, replay):
+        if replay:
             self._sent = {}
             rows = sorted(self._name_at)
         else:                                           # a row changed and changed back (or added and deleted) is not sent
@@ -112,43 +107,20 @@ class NodeTable:
         rec = [self._record(at) for at in rows]
         for at, r in zip(rows, rec):
             self._sent[at] = r
-        d = {"reset": dict(self.size) if self._replay else None, "node_id": np.array(rows, np.int32),
+        d = {"node_id": np.array(rows, np.int32),
              "present": np.array([r[0] for r in rec], np.uint8), "alloc_cpu_milli": np.array([r[1] for r in rec], np.int64),
              "alloc_mem_bytes": np.array([r[2] for r in rec], np.int64), "alloc_gpu": np.array([r[3] for r in rec], np.int64),
              "unschedulable": np.array([r[4] for r in rec], np.uint8), "ready": np.array([r[5] for r in rec], np.uint8),
              "name_key": np.array([r[6] for r in rec], np.int64), "creation": np.array([r[7] for r in rec], np.int64)}
         self._dirty = set()
-        self._replay = False
         return d
 
-    def flush(self, packer):
-        """One update of the device's table (none when nothing changed), preceded by a reset when the delta carries one; on
-        a refusal the whole state is reset and replayed once more, and a second refusal is raised."""
-        from .native import GangpackError
-        d = self.delta()
-        if d["reset"] is None and len(d["node_id"]) == 0:
-            return
-        try:
-            self._push(packer, d)
-        except GangpackError:
-            self.replay()
-            d = self.delta()
-            self._push(packer, d)
-        self.mirror.apply(d)
-
-    # ---- internals
     def _record(self, at):
         """the row of node id `at` as a delta writes it"""
         nm = self._name_at.get(at)
         if nm is None:
             return _ABSENT
         return (True, *self.nodes[nm], self._key[nm], self.creation[nm])
-
-    @staticmethod
-    def _push(packer, d):
-        if d["reset"] is not None:
-            packer.node_table_reset(**d["reset"])
-        packer.node_table_update(d)
 
     def _insert(self, name):
         # keys lie in [0, 2^key_bits): -1 and 2^key_bits stand for the neighbours past either end

@@ -21,6 +21,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from .resident import ResidentTable
+
 SPARK_APP_ID_LABEL = "spark-app-id"
 SPARK_ROLE_LABEL = "spark-role"
 EXECUTOR = "executor"
@@ -295,7 +297,7 @@ class _CountedInterner:
         return len(self.count)
 
 
-class OverheadTable(PodRecords):
+class OverheadTable(PodRecords, ResidentTable):
     """The host side of the resident overhead table: PodRecords' slots (same numbering), the pod lister, the
     ResourceReservation cache and the soft store, kept as the shim's informer handlers see them, and turned into the deltas of
     gp_overhead_table_update.  Ids come from reference-counted interners over the slots' rows, the RR flags and the members,
@@ -303,13 +305,15 @@ class OverheadTable(PodRecords):
 
     Events: add / update / delete (the pod informer through the nodeName filter, as PodRecords), lister_set(pod) /
     lister_delete(namespace, name), rr_set((namespace, appID), Status.Pods values) / rr_delete, soft_set(appID, Reservations
-    keys) / soft_delete.  delta() -> the arrays of one update; when it carries "reset" (the first one, whenever a capacity
-    would be exceeded: it is doubled and the whole state replayed, and after replay()), gp_overhead_table_reset(**delta["reset"])
-    goes first."""
+    keys) / soft_delete.  delta() -> the arrays of one gp_overhead_table_update: what changed since the last delta (everything
+    after a reset); see ResidentTable.  A request >= 2^61 is refused when it arrives."""
+
+    name, writes = "overhead", ("slot", "rr_app_key", "member_kind")
 
     def __init__(self, n_slots=64, n_node_ids=64, n_app_keys=64, n_app_ids=64, n_names=64):
-        super().__init__()
-        self.size = dict(n_slots=n_slots, n_node_ids=n_node_ids, n_app_keys=n_app_keys, n_app_ids=n_app_ids, n_names=n_names)
+        PodRecords.__init__(self)
+        ResidentTable.__init__(self, TableMirror(), n_slots=n_slots, n_node_ids=n_node_ids, n_app_keys=n_app_keys,
+                               n_app_ids=n_app_ids, n_names=n_names)
         self.lister, self.rrs, self.soft = {}, {}, {}
         self._nodes, self._keys, self._apps, self._names = (_CountedInterner() for _ in range(4))
         self._row, self._refs = [], []                  # per slot: its row (ids), the interner references the row holds
@@ -317,7 +321,6 @@ class OverheadTable(PodRecords):
         self._flags = set()                              # app key ids with a ResourceReservation
         self._members = {}                               # (kind, app, name) ids -> holders (0: absent)
         self._dirty, self._flag_touched, self._member_touched = {}, {}, {}   # -> what the device holds since the last delta
-        self._replay = True
 
     # ---- pod records (PodRecords' add / update / delete land here)
     def _record(self, pod):
@@ -385,22 +388,13 @@ class OverheadTable(PodRecords):
             c[known] = v
         return tuple(cols[:3]), tuple(cols[3:]), has, warned
 
-    def replay(self):
-        """The next delta resets the table and resends the whole state.  delta() takes its changes as sent, so after an
-        update the library refused (a request >= 2^61 is refused when it arrives) or that failed, call this: otherwise the
-        host and the device disagree for good."""
-        self._replay = True
+    # ---- internals
+    def _bounds(self):
+        return dict(n_slots=len(self.slots), n_node_ids=self._nodes.bound, n_app_keys=self._keys.bound,
+                    n_app_ids=self._apps.bound, n_names=self._names.bound)
 
-    def delta(self) -> dict:
-        """The arrays of one gp_overhead_table_update: what changed since the last delta (everything after a reset).  The
-        changes count as sent; see replay() for an update that does not go through."""
-        bounds = dict(n_slots=len(self.slots), n_node_ids=self._nodes.bound, n_app_keys=self._keys.bound,
-                      n_app_ids=self._apps.bound, n_names=self._names.bound)
-        for k, b in bounds.items():
-            while self.size[k] < b:
-                self.size[k] = max(2 * self.size[k], 1)
-                self._replay = True
-        if self._replay:
+    def _changes(self, replay):
+        if replay:
             slots = [at for at, row in enumerate(self._row) if row != _FREE_ROW]
             flags = sorted(self._flags)
             members = sorted(t for t, n in self._members.items() if n)
@@ -409,7 +403,7 @@ class OverheadTable(PodRecords):
             flags = sorted(k for k, was in self._flag_touched.items() if (k in self._flags) != was)
             members = sorted(t for t, was in self._member_touched.items() if (self._members.get(t, 0) > 0) != was)
         rows = [self._row[at] for at in slots]
-        d = {"reset": dict(self.size) if self._replay else None, "slot": np.array(slots, np.int32)}
+        d = {"slot": np.array(slots, np.int32)}
         for j, (name, t) in enumerate(_ROW_COLS):
             d[name] = np.array([r[j] for r in rows], t)
         d["rr_app_key"] = np.array(flags, np.int32)
@@ -419,10 +413,8 @@ class OverheadTable(PodRecords):
         d["member_name"] = np.array([t[2] for t in members], np.int32)
         d["member_present"] = np.array([self._members.get(t, 0) > 0 for t in members], np.uint8)
         self._dirty, self._flag_touched, self._member_touched = {}, {}, {}
-        self._replay = False
         return d
 
-    # ---- internals
     def _refresh(self, at):
         while len(self._row) < len(self.slots):
             self._row.append(_FREE_ROW)

@@ -10,27 +10,28 @@ from __future__ import annotations
 import numpy as np
 
 from .overhead import _CountedInterner
+from .resident import ResidentTable
 
 _FREE = (-1, 0, 0, 0)          # node id, cpu, mem, gpu of a free slot
 
 
-class ReservationTable:
+class ReservationTable(ResidentTable):
     """Events: rr_set((namespace, appID), {name: (node, cpu, mem, gpu)}) for a create, an update and the compaction rewrite
     alike, rr_delete(key), soft_set(appID, {pod: (node, cpu, mem, gpu)}) and soft_delete(appID).  Each entry holds one slot;
     freed slots are reused, and node ids come from a reference-counted interner, so the id of a node no entry names any more
-    goes to the next new node.  delta() -> the arrays of one update; when it carries "reset" (the first one, whenever a
-    capacity would be exceeded: it is doubled and the whole state replayed, and after replay()),
-    gp_reservation_table_reset(**delta["reset"]) goes first."""
+    goes to the next new node.  delta() -> the arrays of one gp_reservation_table_update: what changed since the last delta
+    (every occupied slot after a reset); see ResidentTable.  |value| >= 2^61 is refused when it arrives."""
+
+    name, writes = "reservation", ("slot",)
 
     def __init__(self, n_slots=64, n_node_ids=64):
-        self.size = dict(n_slots=n_slots, n_node_ids=n_node_ids)
+        super().__init__(ReservationMirror(), n_slots=n_slots, n_node_ids=n_node_ids)
         self.rrs, self.soft = {}, {}                    # key -> {name: (node, cpu, mem, gpu)}, as the events gave them
         self._nodes = _CountedInterner()
         self._slot = {}                                 # (kind, key, name) -> slot
         self._row, self._node = [], []                  # per slot: (node id, cpu, mem, gpu), the node name it holds (or None)
         self._free = []
         self._dirty = {}                                # slot -> the row the device holds since the last delta
-        self._replay = True
 
     # ---- events
     def rr_set(self, key, reservations: dict):
@@ -50,32 +51,22 @@ class ReservationTable:
         """the table's ids of these node names; -1 for a node no reservation names (nothing is reserved on it)"""
         return np.array([self._nodes.ids.get(n, -1) for n in nodes], np.int32)
 
-    def replay(self):
-        """The next delta resets the table and resends the whole state.  delta() takes its changes as sent, so after an
-        update the library refused (|value| >= 2^61 is refused when it arrives) or that failed, call this: otherwise the
-        host and the device disagree for good."""
-        self._replay = True
+    # ---- internals
+    def _bounds(self):
+        return dict(n_slots=len(self._row), n_node_ids=self._nodes.bound)
 
-    def delta(self) -> dict:
-        """The arrays of one gp_reservation_table_update: what changed since the last delta (every occupied slot after a
-        reset).  The changes count as sent; see replay() for an update that does not go through."""
-        for k, b in (("n_slots", len(self._row)), ("n_node_ids", self._nodes.bound)):
-            while self.size[k] < b:
-                self.size[k] = max(2 * self.size[k], 1)
-                self._replay = True
-        if self._replay:
+    def _changes(self, replay):
+        if replay:
             slots = [at for at, row in enumerate(self._row) if row != _FREE]
         else:
             slots = sorted(at for at, was in self._dirty.items() if self._row[at] != was)
         rows = [self._row[at] for at in slots]
-        d = {"reset": dict(self.size) if self._replay else None, "slot": np.array(slots, np.int32)}
+        d = {"slot": np.array(slots, np.int32)}
         for j, name in enumerate(("node_id", "cpu_milli", "mem_bytes", "gpu")):
             d[name] = np.array([r[j] for r in rows], np.int32 if j == 0 else np.int64)
         self._dirty = {}
-        self._replay = False
         return d
 
-    # ---- internals
     def _set(self, kind, key, reservations, store):
         old = store.pop(key, {})
         if reservations:

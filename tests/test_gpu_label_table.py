@@ -202,9 +202,7 @@ def test_marker_equals_affinity_resident(packer, name):
     odrv = OverheadDriver(n_slots=4, n_node_ids=2, n_app_keys=2, n_app_ids=2, n_names=4)
     exceeded = fitted = 0
     for s, od in enumerate(overhead_churn(rng, odrv, n - 4, steps=4, per_step=12)):
-        if od["reset"] is not None:
-            packer.overhead_table_reset(**od["reset"])
-        packer.overhead_table_update(od)
+        odrv.table.push(packer, od)
         for nm in rng.choice(names, 6, replace=False):                 # relabels: keys dropped, a zone set
             kept = dict(list(t.labels[str(nm)].items())[:3])
             t.set_node(str(nm), dict(kept, zone=str(rng.integers(0, 3))))

@@ -98,14 +98,8 @@ class World:
     def flush(self, p):
         self.labels.flush(p)
         self.table.flush(p)
-        d = next(self.rstream)
-        if d["reset"] is not None:
-            p.reservation_table_reset(**d["reset"])
-        p.reservation_table_update(d)
-        od = next(self.ostream)
-        if od["reset"] is not None:
-            p.overhead_table_reset(**od["reset"])
-        p.overhead_table_update(od)
+        self.rdrv.table.push(p, next(self.rstream))
+        self.odrv.table.push(p, next(self.ostream))
 
     def listed(self, subset=True):
         names = list(self.table.nodes)

@@ -24,12 +24,6 @@ def packer(gangpack):
     p.close()
 
 
-def push(packer, d):
-    if d["reset"] is not None:
-        packer.overhead_table_reset(**d["reset"])
-    packer.overhead_table_update(d)
-
-
 def same(a, b):
     """two (overhead, nonsched, has_reservation, n_warned) answers, bit for bit"""
     assert lists(a[0]) == lists(b[0]) and lists(a[1]) == lists(b[1])
@@ -51,7 +45,7 @@ def device_check(packer, drv, nodes, restated=True):
 
 def step(packer, drv):
     d = drv.step()
-    push(packer, d)
+    drv.table.push(packer, d)
     return d
 
 
@@ -62,7 +56,7 @@ def test_random_churn_streams(packer, seed):
     drv = Driver(n_slots=4, n_node_ids=2, n_app_keys=2, n_app_ids=2, n_names=4)
     nodes = [f"n{i}" for i in range(n_nodes)]
     for d in churn(rng, drv, n_nodes, steps=30, per_step=1 + seed % 7):
-        push(packer, d)
+        drv.table.push(packer, d)
         device_check(packer, drv, nodes)
     assert drv.replays >= 2
 
@@ -149,7 +143,7 @@ def test_update_refusals_leave_the_table_unchanged(packer, gangpack):
     nodes = ["n1", "n2"]
     rng = np.random.default_rng(5)
     for d in churn(rng, drv, 2, steps=4, per_step=20):
-        push(packer, d)
+        drv.table.push(packer, d)
     size = drv.table.size
     before = device_check(packer, drv, nodes)
     ids = drv.table.node_ids(nodes)
@@ -260,7 +254,7 @@ def test_refused_reset_keeps_a_nonempty_table(gangpack):
             drv.pod_event("add", q)
             drv.table.lister_set(q)
         drv.table.rr_set(("a", "app"), [f"e-{k}" for k in range(0, 600, 3)])
-        push(p, drv.step())
+        drv.table.push(p, drv.step())
         ids = np.arange(5, dtype=np.int32)
         before = p.overhead_table_query(ids)
         assert len(before[2]) == 1000 and before[2].sum() == 200
@@ -315,7 +309,7 @@ def test_table_leaves_the_other_entries_alone(gangpack):
     try:
         drv = Driver()
         load_cluster(drv, names, pods, lister, rrs, soft)
-        push(with_table, drv.step())
+        drv.table.push(with_table, drv.step())
         ids = drv.table.node_ids(names)
         ids = ids[ids >= 0]
         before = with_table.overhead_table_query(ids)

@@ -31,12 +31,6 @@ def packer(gangpack):
     p.close()
 
 
-def push(p, d):
-    if d["reset"] is not None:
-        p.reservation_table_reset(**d["reset"])
-    p.reservation_table_update(d)
-
-
 def outcome(fn):
     """(status, result): GP_OK and the result, or the refusal's status and None"""
     try:
@@ -139,7 +133,7 @@ def test_random_streams_equivalence(packer, seed):
     rng = np.random.default_rng(seed)
     drv = Driver()
     for s, d in enumerate(stream(case, drv, rng, steps=8, per_step=1 + 3 * seed)):
-        push(packer, d)
+        drv.table.push(packer, d)
         present = rng.permutation(len(case.names))[: len(case.names) - 20] if s % 2 else None   # nodes leaving the table
         case.check(packer, drv, (seed, s), ig=seed != 3, present=present)
     assert drv.replays >= 2
@@ -153,10 +147,8 @@ def test_overhead_from_the_overhead_table(packer):
     odrv = OverheadDriver(n_slots=4, n_node_ids=2, n_app_keys=2, n_app_ids=2, n_names=4)
     drv = Driver()
     for s, (od, d) in enumerate(zip(overhead_churn(rng, odrv, 6, steps=10, per_step=3), stream(case, drv, rng, 10, 2))):
-        if od["reset"] is not None:
-            packer.overhead_table_reset(**od["reset"])
-        packer.overhead_table_update(od)
-        push(packer, d)
+        odrv.table.push(packer, od)
+        drv.table.push(packer, d)
         oids = odrv.table.node_ids(case.names)
         over = odrv.table.answer(case.names, packer.overhead_table_query)[0]
         case.check(packer, drv, ("host", s), overhead=over)                 # the query's output as host arrays on both sides
@@ -176,7 +168,7 @@ def test_full_size_with_churn(packer, n_nodes, n_rows):
     names = [f"node-{i}" for i in range(n_nodes)]
     drv = Driver(n_slots=2 * n_rows, n_node_ids=n_nodes)
     cluster_rows(rng, drv.table, names, n_rows)
-    push(packer, drv.step())
+    drv.table.push(packer, drv.step())
     alloc = [rng.integers(8, 65, n_nodes) * 1000, rng.integers(32, 513, n_nodes) * GIB, rng.integers(0, 9, n_nodes)]
     over = [rng.integers(0, 3, n_nodes) * 250, rng.integers(0, 3, n_nodes) * (1 << 28), np.zeros(n_nodes, np.int64)]
     ig = rng.integers(0, 4, n_nodes).astype(np.int32)
@@ -189,7 +181,7 @@ def test_full_size_with_churn(packer, n_nodes, n_rows):
         drv.table.rr_set(("ns", f"new-{s}"), {f"e{j}": (names[j], 500, 1 << 28, 0) for j in range(21)})
         d = drv.step()
         assert d["reset"] is None
-        push(packer, d)
+        drv.table.push(packer, d)
         ids = drv.table.node_ids(names)
         rnode, res = rv.to_usage_rows(drv.mirror, ids)
         want = packer.prepare_cluster_groups(alloc, over, rnode, res, ig, 4, zone_id=zid, n_zones=3, name_rank=rank)
@@ -354,7 +346,7 @@ def test_independence(gangpack):
         stats = p.stats()
         drv = Driver()
         for d in stream(case, drv, rng, steps=4, per_step=5):
-            push(p, d)
+            drv.table.push(p, d)
             assert p.stats() == stats
         same(snapshot_state(p, apps), held, "held")
         p.overhead_table_reset(n_slots=4, n_node_ids=4, n_app_keys=1, n_app_ids=1, n_names=1)

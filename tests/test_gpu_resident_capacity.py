@@ -34,12 +34,6 @@ def outcome(fn):
         return e.status, None
 
 
-def push_overhead(p, d):
-    if d["reset"] is not None:
-        p.overhead_table_reset(**d["reset"])
-    p.overhead_table_update(d)
-
-
 def pairs(p, names, odrv, alloc, zone, n_zones, group, n_groups, apps, enc, packer_id):
     """[(per-call, resident)] for the node_group form and, with enc, the affinity form"""
     oids = odrv.table.node_ids(names)
@@ -66,7 +60,7 @@ def test_random_overhead_streams(packer, name):
     odrv = OverheadDriver(n_slots=4, n_node_ids=2, n_app_keys=2, n_app_ids=2, n_names=4)
     exceeded = fitted = 0
     for s, od in enumerate(overhead_churn(rng, odrv, n - 4, steps=6, per_step=12)):
-        push_overhead(packer, od)
+        odrv.table.push(packer, od)
         apps = make_drivers(rng, q, n_groups)
         apps["count"] = rng.integers(0, 6, q).astype(np.int32)
         aff_apps = dict(apps, group=rng.integers(0, n_aff, q).astype(np.int32))
@@ -85,7 +79,7 @@ def test_without_zones_or_groups_and_no_nodes(packer):
     alloc, _, _, _ = make_nodes(rng, 20, 1, 1)
     odrv = OverheadDriver()
     for od in overhead_churn(rng, odrv, 18, steps=2, per_step=20):
-        push_overhead(packer, od)
+        odrv.table.push(packer, od)
     apps = make_drivers(rng, 30, 1, cls_lo=0)
     for a, b in pairs(packer, names, odrv, alloc, None, 1, None, 1, apps, None, 0):
         assert a[0] == 0 and a == b

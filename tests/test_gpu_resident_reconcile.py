@@ -78,18 +78,6 @@ class Nodes:
         return (a[0], defined(a[1])), (b[0], defined(b[1]))
 
 
-def push(p, d):
-    if d["reset"] is not None:
-        p.reservation_table_reset(**d["reset"])
-    p.reservation_table_update(d)
-
-
-def push_overhead(p, d):
-    if d["reset"] is not None:
-        p.overhead_table_reset(**d["reset"])
-    p.overhead_table_update(d)
-
-
 @pytest.mark.parametrize("seed", range(4))
 def test_random_streams(packer, seed):
     """after every flush of both tables: overhead from the host arrays and from the overhead table, all nodes and a subset"""
@@ -100,8 +88,8 @@ def test_random_streams(packer, seed):
     steps = zip(churn(rng, rdrv, names, 8, 2 + 3 * seed), overhead_churn(rng, odrv, 46, 8, 4))
     placed_somewhere = unplaced = 0
     for s, (d, od) in enumerate(steps):
-        push(packer, d)
-        push_overhead(packer, od)
+        rdrv.table.push(packer, d)
+        odrv.table.push(packer, od)
         apps = nodes.apps(rng, 30)
         present = np.sort(rng.permutation(48)[:36]) if s % 2 else None    # nodes leaving the node table
         sub = nodes.names if present is None else [nodes.names[i] for i in present]
@@ -120,7 +108,7 @@ def test_no_nodes_and_no_drivers(packer):
     nodes = Nodes(rng, 30, 3)
     rdrv = Driver()
     for d in churn(rng, rdrv, nodes.names, 2, 5):
-        push(packer, d)
+        rdrv.table.push(packer, d)
     apps = nodes.apps(rng, 12)
     a, b = nodes.pair(packer, rdrv, apps, present=np.zeros(0, np.int64))          # n_nodes == 0: every driver -1
     assert a == b and a[0] == 0 and a[1][0] == [-1] * 12
@@ -180,12 +168,12 @@ def test_refusals_leave_both_tables_and_the_snapshot(gangpack):
         assert call() == INVALID                                                    # no reservation table
         rdrv = Driver(n_slots=64, n_node_ids=40)
         for d in churn(rng, rdrv, nodes.names, 3, 6):
-            push(p, d)
+            rdrv.table.push(p, d)
         assert call() == 0
         assert call(oid=ids) == INVALID                                             # overhead_node_id without an overhead table
         odrv = OverheadDriver(n_slots=64, n_node_ids=48, n_app_keys=8, n_app_ids=8, n_names=64)
         for od in overhead_churn(rng, odrv, 38, 3, 8):
-            push_overhead(p, od)
+            odrv.table.push(p, od)
         oids = odrv.table.node_ids(nodes.names)
         assert call(node_id=rdrv.table.node_ids(nodes.names), oid=oids) == 0
         held = held_state(p, nodes.names, rdrv, odrv, nodes.alloc)
@@ -231,14 +219,14 @@ def test_full_size_with_churn(packer):
     for r in range(n_rows // 20):
         drv.table.rr_set(("ns", f"app-{r}"), {f"e{j}": (nodes.names[rng.integers(n)], int(rng.integers(1, 5)) * 250,
                                                          int(rng.integers(1, 9)) << 28, 0) for j in range(20)})
-    push(packer, drv.step())
+    drv.table.push(packer, drv.step())
     keys = list(drv.table.rrs)
     for s in range(2):
         for k in rng.choice(len(keys), len(keys) // 100, replace=False):           # 1 % of the rows rewritten
             drv.table.rr_set(keys[k], {e: (nodes.names[rng.integers(n)],) + r[1:] for e, r in drv.table.rrs[keys[k]].items()})
         d = drv.step()
         assert d["reset"] is None
-        push(packer, d)
+        drv.table.push(packer, d)
         apps = nodes.apps(rng, q)
         apps["count"] = rng.integers(0, 40, q).astype(np.int32)
         a, b = nodes.pair(packer, drv, apps)
