@@ -1367,6 +1367,10 @@ typedef struct {
     const int32_t* min_executor_count;
     const uint8_t* exact;            /* [n_write] 0: a quantity is outside the exact-int64 model (the row queues, but a queue that
                                         selects it is refused with GP_ERR_UNREPRESENTABLE) */
+    const int32_t* affinity;         /* [n_write] the driver's required-affinity id in the caller's affinity interner; -1: no
+                                        nodeSelector and no required node affinity (matches every node).  NULL writes -1.  Not
+                                        checked here: its range is the sweep's gp_node_affinities, checked by
+                                        gp_exceeds_cluster_capacity_driver_table.  The FIFO entries do not read it. */
 } gp_driver_delta;
 /* Apply one delta.  The whole delta is checked on the device before anything is written: a refused delta leaves the table
  * exactly as it was.  One stream synchronise.  GP_ERR_INVALID: no table (gp_driver_table_reset first), missing arrays or a
@@ -1420,6 +1424,38 @@ gp_status gp_pack_fifo_driver_table(gp_ctx* ctx, const gp_driver_queue* queue, g
  * the snapshot-group ranges of gp_pack_fifo_driver_table, then the queue refusals. */
 gp_status gp_pack_fifo_zones_groups_driver_table(gp_ctx* ctx, const gp_driver_queue* queue, gp_binpacker packer, gp_mode mode,
                                                  const gp_instance_groups* groups /* must be NULL */, gp_zone_results* out);
+
+/* The unschedulable-pod marker's whole sweep (scanForUnschedulablePods, EXT/unschedulablepods.go:93-166) from the driver
+ * table, the node table and the label table, in one call.
+ *   Stale rows: present, scheduler == `scheduler` and creation + timeout_ns < now_unix_nano (CreationTimestamp.Add(timeout)
+ *     .Before(now): strict), evaluated exactly in 128 bits.  Pending, not terminating and parseable hold by construction (the
+ *     host clears every other driver).  They are listed in (creation, slot) order: stale_slot[i] = the slot of entry i.
+ *   outcome[i] = 2 (outside the model): the row has exact = 0, a negative quantity or a negative min_executor_count -- what
+ *     gp_exceeds_cluster_capacity* would refuse for the whole call.  The caller answers it with DoesPodExceedClusterCapacity
+ *     on the host; exceeds[i] is 0.
+ *   Otherwise exceeds[i] and outcome[i] = 1 (the driver's affinity errors on some node: ListWithPredicate fails) or 0 are,
+ *     bit for bit, exceeds and affinity_error of gp_exceeds_cluster_capacity_affinity_node_table(nodes, affinities + one
+ *     appended program that matches every node, drivers) on the gp_apps built from the same rows: the six quantities,
+ *     exe_count = min_executor_count and group = the row's affinity id, -1 becoming the appended program.
+ * Refusals, in this order, each changing no state (the outputs excepted):
+ *   1. the host checks of gp_exceeds_cluster_capacity_affinity_node_table; NULL sweep or outputs, cap < 0 (GP_ERR_INVALID);
+ *      no driver table (gp_driver_table_reset first);
+ *   2. read in one stream synchronise after the selection: a stale row whose affinity id lies outside [-1, n_aff)
+ *      (GP_ERR_INVALID); then n_stale > cap (GP_ERR_CAPACITY, *n_stale holds the size needed: grow and retry);
+ *   3. the device refusals of gp_exceeds_cluster_capacity_affinity_node_table (node gather, overhead, labels, nodes).
+ * The driver, node and label tables are read in place and left unchanged.  Two stream synchronises. */
+typedef struct {
+    int32_t scheduler;               /* table id of the scheduler swept (spark-scheduler); -1: none (selects nothing) */
+    int32_t cap;                     /* entries of the outputs below */
+    int64_t timeout_ns;              /* unschedulablePodTimeoutDuration, used as given */
+    int64_t now_unix_nano;
+    int32_t* stale_slot;             /* out [cap] the stale drivers' slots in (creation, slot) order */
+    uint8_t* exceeds;                /* out [cap] !HasCapacity, where outcome = 0 */
+    uint8_t* outcome;                /* out [cap] 0 answered, 1 affinity error, 2 outside the model */
+    int32_t* n_stale;                /* out */
+} gp_stale_sweep;
+gp_status gp_exceeds_cluster_capacity_driver_table(gp_ctx* ctx, const gp_node_table_nodes* nodes, const gp_node_affinities* affinities,
+                                                   const gp_stale_sweep* sweep, gp_binpacker packer);
 
 /* ---- several GPUs of one box behind ONE host process (SURVEY 8e) -----------------------------------------------
  * The reference is a single process with a serial Predicate (internal/extender/resource.go:194-205); this handle lets

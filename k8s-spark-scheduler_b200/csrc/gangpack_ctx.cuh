@@ -247,7 +247,7 @@ struct gp_ctx {
         DevBuf gather;                            // the columns one *_node_table call gathers, and its scratch
     } nt{"no node table (gp_node_table_reset first)"};
     // gangpack_driver_table.cu, read by the *_driver_table entries: present, exact, creation, scheduler, group, quantities [6],
-    // count
+    // count, affinity
     struct DriverTable : ResidentTable<gp_driver_table_size> {
         using ResidentTable::ResidentTable;
         DevBuf queue;                             // the queue one *_driver_table call selects, orders and packs, and its scratch
@@ -447,6 +447,22 @@ gp_status nt_gather(gp_ctx* c, const gp_node_table_nodes* nodes, const int32_t* 
 gp_status nt_refusal(gp_ctx* c, int word, const char* who);
 // After the entry's synchronise: the optional zone_id_out / instance_group_out copies
 gp_status nt_outputs(gp_ctx* c, const gp_node_table_nodes* nodes, const NtGathered& g);
+
+// ---- gangpack_driver_table.cu ----------------------------------------------------------------------------------------
+
+// The stale drivers of one marker sweep as device columns in (creation, slot) order, in the driver table's queue buffer: the
+// six quantities, count and capacity group (the affinity id, -1 -> n_aff) of each, all zero for a row outside the model
+struct DtStale {
+    int32_t n;
+    const int64_t* q[6];
+    const int32_t* count;
+    const int32_t* group;
+};
+// The stale stage of gp_exceeds_cluster_capacity_driver_table over a live driver table: select, order and scatter, one
+// synchronise, then the refusals (an affinity id outside [-1, n_aff) on a stale row, then n_stale > cap with *n_stale
+// written).  stale_slot and outcome (0, or 2 outside the model) are downloaded on the stream: complete after the next
+// synchronise.
+gp_status dt_stale_stage(gp_ctx* c, const gp_stale_sweep* sw, int32_t n_aff, const char* who, DtStale* out);
 
 // ---- gangpack_zones.cu -----------------------------------------------------------------------------------------------
 

@@ -5,6 +5,7 @@
 //   gp_dt_check     thread per slot write: slot range, duplicates (per-slot stamps, stamped_twice), on present rows scheduler
 //                   and group range and |quantity| < 2^61 when the row is exact
 //   gp_dt_apply     the slot writes; nothing when the error word is set
+//   gp_dt_apply_aff the affinity column's writes, under the same error word
 // within the update protocol of gangpack_resident.cuh, so a refused delta leaves the table as it was.
 //
 // The queue stage of an entry writes, on the device, exactly the gp_apps columns the host would upload for the same pods
@@ -20,6 +21,15 @@
 // then one synchronise reads the count, the executor total and the refusal word, so every refusal comes before any pack
 // launch.  The existing FIFO bodies then run unchanged on these device columns: pack_begin + pack_device_range as
 // gp_pack_batch_device runs them, or fifo_zones_body (gangpack_zones.cu) in place of its upload.
+//
+// The unschedulable-pod marker's stale stage (dt_stale_stage, for gp_exceeds_cluster_capacity_driver_table) has the same shape:
+//   gp_ds_select    thread per slot: present, the swept scheduler and creation + timeout < now (exact, 128 bits), compacted
+//                   into QueueKeys (0, creation, slot) by the same block compaction; an affinity id outside [-1, n_aff) on a
+//                   stale row sets the refusal word
+//   gp_sort_tiles / gp_rank_by_search <QueueKey>   the (creation, slot) order
+//   gp_ds_scatter   thread per stale row: its slot, six quantities, count and capacity group (the affinity id, -1 -> n_aff) at
+//                   its position, or an all-zero placeholder with outcome 2 for a row outside the model
+// then one synchronise reads the count and the refusal word before the capacity kernels run on the columns.
 #include "gangpack_ctx.cuh"
 #include "gangpack_tilesort.cuh"
 
@@ -74,7 +84,7 @@ static const Refusal kDqRefusals[] = {
 struct DtPieces {
     Piece<uint8_t> present, exact;
     Piece<long long> creation, q;
-    Piece<int32_t> sched, group, count;
+    Piece<int32_t> sched, group, count, aff;
     Piece<uint32_t> stamp;
 };
 
@@ -89,6 +99,7 @@ static DtPieces take_cols(Arena& a, const gp_driver_table_size& z) {
     p.sched = a.take<int32_t>(S);
     p.group = a.take<int32_t>(S);
     p.count = a.take<int32_t>(S);
+    p.aff = a.take<int32_t>(S);
     p.stamp = a.take<uint32_t>(S);
     return p;
 }
@@ -105,6 +116,12 @@ static DtTable table_cols(gp_ctx* c) {
     Arena tc{c->dt.cols, c->stream};
     const DtPieces p = take_cols(tc, c->dt.size);
     return DtTable{tc.ptr(p.present), tc.ptr(p.exact), tc.ptr(p.creation), tc.ptr(p.q), tc.ptr(p.sched), tc.ptr(p.group), tc.ptr(p.count)};
+}
+
+// The affinity column [n_slots]: the marker's alone, so it stays out of DtTable (gp_dt_apply and the queue stage do not see it)
+static int32_t* table_aff(gp_ctx* c) {
+    Arena tc{c->dt.cols, c->stream};
+    return tc.ptr(take_cols(tc, c->dt.size).aff);
 }
 
 // One update, staged on the device
@@ -151,6 +168,14 @@ __global__ void gp_dt_apply(DtDelta D, DtTable T, const int* __restrict__ err) {
     for (int d = 0; d < 6; ++d) T.q[(size_t)d * S + r] = on && D.q[d] ? D.q[d][i] : 0;
 }
 
+// the affinity ids of the same writes (aff NULL: -1), after gp_dt_apply and under its error word
+__global__ void gp_dt_apply_aff(int32_t n, const int32_t* __restrict__ slot, const uint8_t* __restrict__ present,
+                                const int32_t* __restrict__ aff, int32_t* __restrict__ col, const int* __restrict__ err) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || *(volatile const int*)err) return;
+    col[slot[i]] = present[i] && aff ? aff[i] : -1;
+}
+
 // ---- the queue stage ----
 
 // The words the host reads after the queue stage
@@ -191,9 +216,26 @@ struct DqOut {
 
 constexpr int kDqThreads = 256;
 
-__global__ void __launch_bounds__(kDqThreads) gp_dq_select(DqIn in, QueueKey* __restrict__ keys, DqWords* __restrict__ w) {
-    __shared__ int32_t wsum[kDqThreads / 32];
+// The compacted index of this thread's entry among the selected ones of every block (meaningful where sel): a warp ballot, a
+// scan of the warp counts by one thread, and one atomicAdd on *cursor per block.  Every thread of the block calls it.
+template <int kThreads>
+__device__ __forceinline__ int32_t block_compact(bool sel, int32_t* cursor) {
+    __shared__ int32_t wsum[kThreads / 32];
     __shared__ int32_t base;
+    const unsigned m = __ballot_sync(0xffffffffu, sel);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) wsum[warp] = __popc(m);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int32_t acc = 0;
+        for (int k = 0; k < kThreads / 32; ++k) { const int32_t t = wsum[k]; wsum[k] = acc; acc += t; }
+        base = acc ? atomicAdd(cursor, acc) : 0;
+    }
+    __syncthreads();
+    return base + wsum[warp] + __popc(m & ((1u << lane) - 1u));
+}
+
+__global__ void __launch_bounds__(kDqThreads) gp_dq_select(DqIn in, QueueKey* __restrict__ keys, DqWords* __restrict__ w) {
     const int32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     bool sel = false;
     int32_t sg = 0;
@@ -211,19 +253,10 @@ __global__ void __launch_bounds__(kDqThreads) gp_dq_select(DqIn in, QueueKey* __
     int bad = sel && !in.exact[r] ? kDqErrInexact : 0;
     if (r == 0 && in.req >= 0) bad |= !in.present[in.req] ? kDqErrAbsent : (!in.exact[in.req] ? kDqErrInexact : 0);
     if (bad) atomicOr(&w->err, bad);
-    const unsigned m = __ballot_sync(0xffffffffu, sel);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (lane == 0) wsum[warp] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int32_t acc = 0;
-        for (int k = 0; k < kDqThreads / 32; ++k) { const int32_t t = wsum[k]; wsum[k] = acc; acc += t; }
-        base = acc ? atomicAdd(&w->selected, acc) : 0;
-    }
-    __syncthreads();
+    const int32_t at = block_compact<kDqThreads>(sel, &w->selected);
     if (sel) {
         QueueKey k; k.sg = sg; k.slot = r; k.creation = in.creation[r];
-        keys[base + wsum[warp] + __popc(m & ((1u << lane) - 1u))] = k;
+        keys[at] = k;
     }
 }
 
@@ -409,6 +442,120 @@ static gp_status queue_stage(gp_ctx* c, const gp_driver_queue* dq, int32_t n_sg,
     return GP_OK;
 }
 
+// ---- the marker's stale stage ----
+
+enum : int {
+    kDsErrAffinity = 1,         // a stale row's affinity id outside [-1, n_aff)
+};
+
+struct DsIn {
+    int32_t n_rows, scheduler, n_aff;
+    long long timeout, now;
+    const uint8_t* present; const uint8_t* exact;
+    const long long* creation;
+    const long long* q;               // [6][n_rows]
+    const int32_t* sched; const int32_t* count; const int32_t* aff;
+};
+
+// The stale rows' capacity columns, at their positions in (creation, slot) order; pitch n_rows
+struct DsOut {
+    int32_t cap;
+    int32_t* slot;
+    long long* q;                     // [6][cap]
+    int32_t* count; int32_t* group;
+    uint8_t* outcome;                 // 0, or 2: outside the model (the row is an all-zero placeholder)
+};
+
+__global__ void __launch_bounds__(kDqThreads) gp_ds_select(DsIn in, QueueKey* __restrict__ keys, DqWords* __restrict__ w) {
+    const int32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    bool sel = false;
+    // CreationTimestamp.Add(timeout).Before(now), exactly: creation + timeout < now in 128 bits
+    if (r < in.n_rows && in.present[r] && in.sched[r] == in.scheduler)
+        sel = (__int128)in.creation[r] + (__int128)in.timeout < (__int128)in.now;
+    if (sel && (in.aff[r] < -1 || in.aff[r] >= in.n_aff)) atomicOr(&w->err, kDsErrAffinity);
+    const int32_t at = block_compact<kDqThreads>(sel, &w->selected);
+    if (sel) {
+        QueueKey k; k.sg = 0; k.slot = r; k.creation = in.creation[r];
+        keys[at] = k;
+    }
+}
+
+__global__ void gp_ds_scatter(DsIn in, const QueueKey* __restrict__ keys, const int32_t* __restrict__ pos, const DqWords* __restrict__ w,
+                              DsOut o) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= w->selected) return;
+    const int32_t r = keys[i].slot, p = pos[i];
+    const size_t S = (size_t)in.n_rows, C = (size_t)o.cap;
+    // what gp_exceeds_cluster_capacity* refuses for a whole call: an inexact row, a negative quantity or count
+    bool outside = !in.exact[r] || in.count[r] < 0;
+    for (int d = 0; d < 6; ++d) outside |= in.q[(size_t)d * S + r] < 0;
+    o.slot[p] = r;
+    for (int d = 0; d < 6; ++d) o.q[(size_t)d * C + p] = outside ? 0 : in.q[(size_t)d * S + r];
+    o.count[p] = outside ? 0 : in.count[r];
+    const int32_t a = in.aff[r];
+    o.group[p] = outside || a == -1 ? in.n_aff : a;
+    o.outcome[p] = outside ? 2 : 0;
+}
+
+gp_status dt_stale_stage(gp_ctx* c, const gp_stale_sweep* sw, int32_t n_aff, const char* who, DtStale* out) {
+    auto& t = c->dt;
+    const int32_t S = t.size.n_slots;
+    GP_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    const size_t R = (size_t)S;
+    Arena ar{t.queue, st};
+    const auto keys = ar.take<QueueKey>(R), sorted = ar.take<QueueKey>(R);
+    const auto pos = ar.take<int32_t>(R), slot = ar.take<int32_t>(R), cnt = ar.take<int32_t>(R), grp = ar.take<int32_t>(R);
+    const auto cols = ar.take<long long>(6 * R);
+    const auto oc = ar.take<uint8_t>(R);
+    const auto words = ar.take<DqWords>(1);
+    ar.reserve();
+    ar.zero(words);
+    GP_TRY(ar.check(c));
+    Arena tc{t.cols, st};
+    const DtPieces p = take_cols(tc, t.size);
+    DsIn in{};
+    in.n_rows = S; in.scheduler = sw->scheduler; in.n_aff = n_aff; in.timeout = sw->timeout_ns; in.now = sw->now_unix_nano;
+    in.present = tc.ptr(p.present); in.exact = tc.ptr(p.exact); in.creation = tc.ptr(p.creation); in.q = tc.ptr(p.q);
+    in.sched = tc.ptr(p.sched); in.count = tc.ptr(p.count); in.aff = tc.ptr(p.aff);
+    DsOut o{};
+    o.cap = S;
+    o.slot = ar.ptr(slot); o.q = ar.ptr(cols); o.count = ar.ptr(cnt); o.group = ar.ptr(grp); o.outcome = ar.ptr(oc);
+    DqWords* w = ar.ptr(words);
+    if (!t.sort_attr_set) {
+        GP_CUDA(c, cudaFuncSetAttribute(gp_sort_tiles<QueueKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSortTile * sizeof(QueueKey))));
+        t.sort_attr_set = true;
+    }
+    if (S > 0) {
+        const int rb = (S + kDqThreads - 1) / kDqThreads;
+        gp_ds_select<<<rb, kDqThreads, 0, st>>>(in, ar.ptr(keys), w);
+        const int32_t* n_sel = &w->selected;
+        gp_sort_tiles<QueueKey><<<(S + kSortTile - 1) / kSortTile, kSortThreads, kSortTile * sizeof(QueueKey), st>>>(S, n_sel, ar.ptr(keys),
+                                                                                                                   ar.ptr(sorted));
+        gp_rank_by_search<QueueKey><<<rb, kDqThreads, 0, st>>>(S, n_sel, ar.ptr(keys), ar.ptr(sorted), ar.ptr(pos));
+        gp_ds_scatter<<<rb, kDqThreads, 0, st>>>(in, ar.ptr(keys), ar.ptr(pos), w, o);
+    }
+    GP_CUDA(c, cudaGetLastError());
+    DqWords hw{};
+    ar.get(&hw, words);
+    GP_TRY(ar.sync(c));
+    static const Refusal refusals[] = {{kDsErrAffinity, GP_ERR_INVALID, "a stale driver's affinity id outside [-1, n_aff)"}};
+    GP_TRY(refuse(c, hw.err, refusals, who));
+    *sw->n_stale = hw.selected;
+    if (hw.selected > sw->cap) return fail(c, GP_ERR_CAPACITY, who, "cap too small (*n_stale holds the size needed)");
+    // completed by the capacity call's synchronise
+    const size_t n = (size_t)hw.selected;
+    ar.get(sw->stale_slot, ar.ptr(slot), n);
+    ar.get(sw->outcome, ar.ptr(oc), n);
+    GP_TRY(ar.check(c));
+    *out = DtStale{};
+    out->n = hw.selected;
+    for (int d = 0; d < 6; ++d) out->q[d] = (const int64_t*)o.q + (size_t)d * R;
+    out->count = o.count;
+    out->group = o.group;
+    return GP_OK;
+}
+
 extern "C" {
 
 gp_status gp_driver_table_reset(gp_ctx* c, const gp_driver_table_size* z) {
@@ -438,6 +585,7 @@ gp_status gp_driver_table_update(gp_ctx* c, const gp_driver_delta* d) {
     const size_t W = (size_t)d->n_write;
     Arena ar{c->callbuf, st};
     const auto slot = ar.take<int32_t>(W), sched = ar.take<int32_t>(W), grp = ar.take<int32_t>(W), cnt = ar.take<int32_t>(W);
+    const auto aff = ar.take<int32_t>(W);
     const auto on = ar.take<uint8_t>(W), ex = ar.take<uint8_t>(W);
     const auto cre = ar.take<long long>(W), q = ar.take<long long>(6 * W);
     const auto word = ar.take<int>(1);
@@ -454,6 +602,7 @@ gp_status gp_driver_table_update(gp_ctx* c, const gp_driver_delta* d) {
     for (int k = 0; k < 6; ++k) D.q[k] = ar.put(q.part((size_t)k * W, W), hq[k]);
     D.count = ar.put(cnt, d->min_executor_count);
     D.exact = ar.put(ex, d->exact);
+    const int32_t* d_aff = ar.put(aff, d->affinity);
     GP_TRY(ar.check(c));
     Arena tc{t.cols, st};
     const DtPieces p = take_cols(tc, t.size);
@@ -464,6 +613,7 @@ gp_status gp_driver_table_update(gp_ctx* c, const gp_driver_delta* d) {
         const unsigned wb = (unsigned)((W + T - 1) / T);
         gp_dt_check<<<wb, T, 0, st>>>(D, tc.ptr(p.stamp), t.seq, w);
         gp_dt_apply<<<wb, T, 0, st>>>(D, table_cols(c), w);
+        gp_dt_apply_aff<<<wb, T, 0, st>>>(D.n, D.slot, D.present, d_aff, table_aff(c), w);
     }
     int hw = 0;
     return t.commit(c, ar, word, &hw, kDtRefusals, who);

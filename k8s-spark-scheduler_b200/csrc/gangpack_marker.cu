@@ -1,7 +1,8 @@
 // gangpack_marker.cu -- the unschedulable-pod marker's capacity checks (gp_exceeds_cluster_capacity, with required node
 // affinity gp_exceeds_cluster_capacity_affinity, their *_resident forms over the overhead table, and
-// gp_exceeds_cluster_capacity_affinity_label_table over both it and the label table), gp_match_node_affinity[_resident], and
-// the overhead computer (gp_node_overhead).
+// gp_exceeds_cluster_capacity_affinity_label_table over both it and the label table, the node-table forms, and
+// gp_exceeds_cluster_capacity_driver_table over the driver table's stale rows), gp_match_node_affinity[_resident], and the
+// overhead computer (gp_node_overhead).
 #include "gangpack_ctx.cuh"
 #include "gangpack_affinity.cuh"
 #include "gangpack_capacity.cuh"
@@ -151,10 +152,13 @@ struct AffStage {
 // The affinities' labels are the per-call labels, or with rlabels the label table's rows.
 // gather_err (the *_node_table entries): nodes' allocatable and zone_id are device columns gathered from the node and label
 // tables, kept in range by the gather, whose status word is read in the one synchronise before the entry's own refusals.
-static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
-                              const gp_node_affinities* aff, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds,
-                              uint8_t* affinity_error, bool resident = false, const int32_t* over_ids = nullptr,
-                              const gp_resident_labels* rlabels = nullptr, const int* gather_err = nullptr) {
+// apps_on_device (the driver-table entry): a's six quantities, exe_count and group are device columns (DtStale), used in place;
+// the groups are copied back with the results for affinity_error.
+// capacity_check: the host checks alone (capacity_run's first step), for an entry that has device work to do between them and
+// the run.
+static gp_status capacity_check(gp_ctx* c, const char* who, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
+                                const gp_node_affinities* aff, const gp_apps* a, gp_binpacker packer, bool resident,
+                                const int32_t* over_ids, const gp_resident_labels* rlabels, const uint8_t* exceeds) {
     if (!aff) {
         if (!nodes || !a || nodes->n_nodes < 0 || a->n_apps < 0 || nodes->n_groups < 1 || (nodes->zone_id && nodes->n_zones < 1) ||
             (nodes->n_nodes > 0 && (!nodes->alloc_cpu_milli || !nodes->alloc_mem_bytes)) ||
@@ -173,12 +177,22 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         if (s != GP_OK) return s;
     }
     if ((int)packer < GP_BP_TIGHTLY_PACK || (int)packer > GP_BP_SINGLE_AZ_MINIMAL_FRAGMENTATION) return fail(c, GP_ERR_INVALID, who, "unknown packer");
-    const int32_t n = nodes->n_nodes, Q = a->n_apps;
+    const int32_t n = nodes->n_nodes;
     const int32_t Z = nodes->zone_id ? nodes->n_zones : 1, G = aff ? aff->n_aff : nodes->n_groups;
     if (!aff && (int64_t)(G + 1) * Z > (int64_t)INT32_MAX / 2) return fail(c, GP_ERR_INVALID, who, "(n_groups + 1) * n_zones too large");
     if (aff && (int64_t)Z > (int64_t)INT32_MAX / 2) return fail(c, GP_ERR_INVALID, who, "n_zones too large");
     if (resident && n > 0 && !over_ids) return fail(c, GP_ERR_INVALID, who, "overhead_node_id missing");
     if (resident) GP_TRY(require(c, c->oht.need(), who));
+    return GP_OK;
+}
+
+static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_nodes* nodes, const gp_node_labels* labels,
+                              const gp_node_affinities* aff, const gp_apps* a, gp_binpacker packer, uint8_t* exceeds,
+                              uint8_t* affinity_error, bool resident = false, const int32_t* over_ids = nullptr,
+                              const gp_resident_labels* rlabels = nullptr, const int* gather_err = nullptr, bool apps_on_device = false) {
+    GP_TRY(capacity_check(c, who, nodes, labels, aff, a, packer, resident, over_ids, rlabels, exceeds));
+    const int32_t n = nodes->n_nodes, Q = a->n_apps;
+    const int32_t Z = nodes->zone_id ? nodes->n_zones : 1, G = aff ? aff->n_aff : nodes->n_groups;
     // classes per chunk: node_group -> its own class and the all-nodes class; affinities -> as many as keep K n and K Z
     // within kCapEntries (at least one)
     const int32_t K = !aff ? 2 : (int32_t)std::max<int64_t>(1, std::min<int64_t>(std::max(G, 1), kCapEntries / std::max<int64_t>({(int64_t)n, (int64_t)Z, 1})));
@@ -201,8 +215,9 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     const auto staged = ar.take<long long>(3 * N), sched = ar.take<long long>(3 * E);
     const auto bcnt = ar.take<int32_t>(B), boff = ar.take<int32_t>(B + 1), soff = ar.take<int32_t>(B + 1), moff = ar.take<int32_t>(B + 1);
     const auto segs = ar.take<CapSeg>(n_segs);
-    const auto qp = ar.take<long long>(6 * q);
-    const auto cnt = ar.take<int32_t>(q), ag = ar.take<int32_t>(q);
+    const size_t qh = apps_on_device ? 0 : q;           // host columns staged
+    const auto qp = ar.take<long long>(6 * qh);
+    const auto cnt = ar.take<int32_t>(qh), ag = ar.take<int32_t>(qh);
     const auto hash = ar.take<CapEntry>(H);
     const auto pairs = ar.take<CapPair>(q);
     const auto n_pairs = ar.take<int32_t>(2);
@@ -260,10 +275,16 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     CapAppsIn ai{};
     ai.n = Q;
     const int64_t* qcols[6] = {a->drv_cpu_milli, a->drv_mem_bytes, a->drv_gpu, a->exe_cpu_milli, a->exe_mem_bytes, a->exe_gpu};
-    for (int t = 0; t < 6; ++t) ai.q[t] = ar.put(qp.part(q * t, q), qcols[t]);
-    ar.put(cnt, a->exe_count);
-    ai.count = ar.ptr(cnt);
-    if (Q > 0) ai.group = ar.put(ag, a->group);
+    if (apps_on_device) {
+        for (int t = 0; t < 6; ++t) ai.q[t] = (const long long*)qcols[t];
+        ai.count = a->exe_count;
+        ai.group = a->group;
+    } else {
+        for (int t = 0; t < 6; ++t) ai.q[t] = ar.put(qp.part(q * t, q), qcols[t]);
+        ar.put(cnt, a->exe_count);
+        ai.count = ar.ptr(cnt);
+        if (Q > 0) ai.group = ar.put(ag, a->group);
+    }
     ai.n_groups = G;
     ai.min_group = aff ? 0 : -1;
     ai.hash_mask = (uint32_t)(H - 1);
@@ -302,6 +323,8 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
     GP_CUDA(c, cudaGetLastError());
     int herr = 0, aerr = 0, oerr_h[2] = {0, 0}, gather = 0;
     std::vector<int32_t> n_error(aff ? (size_t)G : 0);
+    std::vector<int32_t> dev_group(apps_on_device && aff && affinity_error ? q : 0);
+    ar.get(dev_group.data(), a->group, dev_group.size());
     ar.get(exceeds, ar.ptr(d_out), q);
     ar.get(&herr, s.err, 1);
     if (aff) {
@@ -323,8 +346,10 @@ static gp_status capacity_run(gp_ctx* c, const char* who, const gp_capacity_node
         {kCcErrUnrepresentable, GP_ERR_UNREPRESENTABLE, "request >= 2^61"},
         {kCcErrNodeQuantity, GP_ERR_UNREPRESENTABLE, "|allocatable| or |overhead| >= 2^61"}};
     GP_TRY(refuse(c, herr, cc_refusals, who));
-    if (aff && affinity_error)
-        for (int32_t i = 0; i < Q; ++i) affinity_error[i] = n_error[a->group[i]] > 0 ? 1 : 0;
+    if (aff && affinity_error) {
+        const int32_t* group = apps_on_device ? dev_group.data() : a->group;
+        for (int32_t i = 0; i < Q; ++i) affinity_error[i] = n_error[group[i]] > 0 ? 1 : 0;
+    }
     return GP_OK;
 }
 
@@ -408,6 +433,57 @@ gp_status gp_exceeds_cluster_capacity_affinity_node_table(gp_ctx* c, const gp_no
     const gp_capacity_nodes cn = gathered_nodes(nodes, g, nullptr, 0);
     const gp_resident_labels rl{nodes->n_nodes, 0, nodes->node_table_id};
     GP_TRY(capacity_run(c, who, &cn, nullptr, affinities, a, packer, exceeds, affinity_error, true, nodes->overhead_node_id, &rl, g.err));
+    return nt_outputs(c, nodes, g);
+}
+
+// The marker's whole sweep from the driver table (DESIGN §2.14): the host checks of the affinity node-table entry and the
+// sweep's own, the gather enqueued, the stale stage (one synchronise, its refusals), then the capacity run on the stale
+// columns in place over the caller's programs plus one that matches every node (the drivers without an affinity).
+gp_status gp_exceeds_cluster_capacity_driver_table(gp_ctx* c, const gp_node_table_nodes* nodes, const gp_node_affinities* affinities,
+                                                   const gp_stale_sweep* sw, gp_binpacker packer) {
+    static const char* who = "gp_exceeds_cluster_capacity_driver_table";
+    if (!enter(c)) return GP_ERR_INVALID;
+    if (!affinities) return fail(c, GP_ERR_INVALID, who, "missing arrays or negative sizes");
+    NtGathered g{};
+    GP_TRY(nt_gather(c, nodes, nullptr, 1, false, who, &g, nullptr, false));
+    const gp_capacity_nodes cn = gathered_nodes(nodes, g, nullptr, 0);
+    const gp_resident_labels rl{nodes->n_nodes, 0, nodes->node_table_id};
+    // the caller's programs and, appended, one with no nodeSelector and no required affinity (it matches every node); arrays
+    // the check would refuse are passed on as they are, so that it refuses them as the affinity node-table entry does
+    const gp_node_affinities* P = affinities;
+    gp_node_affinities ext = *P;
+    std::vector<int64_t> sel_off, term_off;
+    std::vector<uint8_t> has_required;
+    if (P->n_aff >= 0 && P->sel_off && P->term_off && (P->n_aff == 0 || P->has_required) && P->n_aff < INT32_MAX) {
+        const int32_t A = P->n_aff;
+        sel_off.assign(P->sel_off, P->sel_off + A + 1);
+        sel_off.push_back(sel_off[A]);
+        term_off.assign(P->term_off, P->term_off + A + 1);
+        term_off.push_back(term_off[A]);
+        has_required.assign(A + 1, 0);
+        if (A > 0) std::copy(P->has_required, P->has_required + A, has_required.begin());
+        ext.n_aff = A + 1;
+        ext.sel_off = sel_off.data(); ext.term_off = term_off.data(); ext.has_required = has_required.data();
+    }
+    const gp_apps none{};
+    GP_TRY(capacity_check(c, who, &cn, nullptr, &ext, &none, packer, true, nodes->overhead_node_id, &rl, nullptr));
+    if (!sw || !sw->stale_slot || !sw->exceeds || !sw->outcome || !sw->n_stale || sw->cap < 0)
+        return fail(c, GP_ERR_INVALID, who, "NULL sweep or outputs, or a negative cap");
+    GP_TRY(require(c, c->dt.need(), who));
+    DtStale ds{};
+    GP_TRY(dt_stale_stage(c, sw, P->n_aff, who, &ds));
+    gp_apps a{};
+    a.n_apps = ds.n;
+    a.drv_cpu_milli = ds.q[0]; a.drv_mem_bytes = ds.q[1]; a.drv_gpu = ds.q[2];
+    a.exe_cpu_milli = ds.q[3]; a.exe_mem_bytes = ds.q[4]; a.exe_gpu = ds.q[5];
+    a.exe_count = ds.count; a.group = ds.group;
+    std::vector<uint8_t> aff_err((size_t)ds.n);
+    GP_TRY(capacity_run(c, who, &cn, nullptr, &ext, &a, packer, sw->exceeds, aff_err.data(), true, nodes->overhead_node_id, &rl, g.err,
+                        true));
+    for (int32_t i = 0; i < ds.n; ++i) {           // outcome holds 2 (outside the model) or 0 from the stale stage
+        if (sw->outcome[i] == 2) sw->exceeds[i] = 0;
+        else sw->outcome[i] = aff_err[i] ? 1 : 0;
+    }
     return nt_outputs(c, nodes, g);
 }
 

@@ -3,13 +3,17 @@ queue a driver-table entry stands for.
 
 DriverTable keeps, per pending driver pod, what the device's driver table holds: the creation time (UnixNano), the
 scheduler and instance-group ids (the host interns Spec.SchedulerName and FindInstanceGroupFromPodSpec's group; -1 when no
-group is found), the six quantities of sparkResources, MinExecutorCount and whether every quantity is exact.  A driver is
+group is found), the six quantities of sparkResources, MinExecutorCount, whether every quantity is exact and the id of its
+required node affinity (interned by a canonical key; -1 for no nodeSelector and no required affinity).  A driver is
 written only while it is pending and its annotations parse; a bound, deleted or terminating driver, and one whose
 annotations no longer parse, is deleted.  Slots freed by a delete are reused, lowest first.
 
 DriverMirror is a numpy copy of what the device holds.  queue() decodes it into the gp_apps the per-call path builds:
 filterToEarliestAndSort (EXT/sparkpods.go:54-71, stable in slot order) for the Predicate form, every drained row in
-(snapshot group, creation, slot) order for the drain form, and shouldSkipDriverFifo for skip_if_no_fit.
+(snapshot group, creation, slot) order for the drain form, and shouldSkipDriverFifo for skip_if_no_fit.  stale() decodes it
+into what the unschedulable-pod marker's sweep selects (scanForUnschedulablePods, EXT/unschedulablepods.go:93-166): the
+drivers of one scheduler with creation + timeout < now, in (creation, slot) order, with their gp_apps columns and which of
+them lie outside the capacity check's model.
 """
 from __future__ import annotations
 
@@ -21,14 +25,32 @@ from .resident import ResidentTable
 
 QUANTITIES = ("drv_cpu", "drv_mem", "drv_gpu", "exe_cpu", "exe_mem", "exe_gpu")
 DELTA_COLUMNS = ("drv_cpu_milli", "drv_mem_bytes", "drv_gpu", "exe_cpu_milli", "exe_mem_bytes", "exe_gpu")
-_ABSENT = (False, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, False)
+_ABSENT = (False, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, False, -1)
+MATCH_ALL = {"nodeSelector": None, "required": None}
+
+
+def affinity_key(affinity):
+    """A canonical, hashable key of a required-affinity program in the form LabelTable.encode_affinities takes, or None for
+    one that matches every node (no nodeSelector and no required terms)"""
+    if affinity is None:
+        return None
+    sel = tuple(sorted((affinity.get("nodeSelector") or {}).items()))
+    terms = affinity.get("required")
+    if not sel and terms is None:
+        return None
+    req = None if terms is None else tuple(
+        tuple(tuple((k, op, tuple(vs)) for k, op, vs in (t.get(part) or ())) for part in ("matchExpressions", "matchFields"))
+        for t in terms)
+    return sel, req
 
 
 class DriverTable(ResidentTable):
     """Every pending driver as the resident driver table keeps it: set_driver(uid, creation, scheduler, group, resources,
-    exact) for an add or an update (resources None: the annotations do not parse, so the driver is deleted), delete_driver(uid)
-    when it is bound, deleted or terminating.  resources is sparkResources' dict ({"drv": [cpu, mem, gpu], "exe": [...],
-    "min": MinExecutorCount}).
+    exact, affinity) for an add or an update (resources None: the annotations do not parse, so the driver is deleted),
+    delete_driver(uid) when it is bound, deleted or terminating.  resources is sparkResources' dict ({"drv": [cpu, mem, gpu],
+    "exe": [...], "min": MinExecutorCount}); affinity the pod's required node affinity in the form
+    affinity.LabelTable.encode_affinities takes ({"nodeSelector": ..., "required": ...}), or None.  Distinct affinities are
+    interned by affinity_key with reference counts, a freed id reused lowest first; affinity_programs() lists them by id.
 
     delta() -> the arrays of one gp_driver_table_update: the slots that changed; see ResidentTable."""
 
@@ -40,19 +62,25 @@ class DriverTable(ResidentTable):
         self._slot, self._uid_at = {}, {}               # uid -> slot, slot -> uid
         self._free, self._next = [], 0                  # freed slots (a heap), the first slot never used
         self.schedulers, self.groups = {}, {}           # interners: name -> id
+        self._aff_id, self._aff_refs, self._aff_prog = {}, {}, {}   # affinity key -> id, id -> live rows, id -> program
+        self._aff_free, self._aff_next = [], 0
         self._dirty = set()
         self._sent = {}                                 # slot -> the row the device holds
 
     # ---- events
-    def set_driver(self, uid, creation, scheduler, group, resources, exact=True):
+    def set_driver(self, uid, creation, scheduler, group, resources, exact=True, affinity=None):
         if resources is None:
             self.delete_driver(uid)
             return
         sid = self._intern(self.schedulers, scheduler)
         gid = -1 if group is None else self._intern(self.groups, group)
         q = [int(v) for v in resources["drv"]] + [int(v) for v in resources["exe"]]
-        row = (True, int(creation), sid, gid, *q, int(resources["min"]), bool(exact))
-        if self.rows.get(uid) == row:
+        old = self.rows.get(uid)
+        aid = self._aff_acquire(affinity)
+        if old is not None:
+            self._aff_release(old[12])
+        row = (True, int(creation), sid, gid, *q, int(resources["min"]), bool(exact), aid)
+        if old == row:
             return
         if uid not in self._slot:
             s = heapq.heappop(self._free) if self._free else self._take_new()
@@ -65,6 +93,7 @@ class DriverTable(ResidentTable):
         s = self._slot.pop(uid, None)
         if s is None:
             return
+        self._aff_release(self.rows[uid][12])
         del self.rows[uid], self._uid_at[s]
         heapq.heappush(self._free, s)
         self._dirty.add(s)
@@ -73,6 +102,11 @@ class DriverTable(ResidentTable):
     def slot_of(self, uid) -> int:
         """the driver's slot, -1 when the table holds no row for it"""
         return self._slot.get(uid, -1)
+
+    def affinity_programs(self) -> list:
+        """the interned affinities by id (an id no live driver holds: a program that matches every node), for
+        affinity.LabelTable.encode_affinities; the gp_node_affinities of a marker sweep"""
+        return [self._aff_prog.get(a, MATCH_ALL) for a in range(self._aff_next)]
 
     def scheduler_id(self, name) -> int:
         """the id of a scheduler name, -1 for a name no driver has carried (a drain of it selects nothing)"""
@@ -115,6 +149,7 @@ class DriverTable(ResidentTable):
             d[k] = col(4 + j, np.int64)
         d["min_executor_count"] = col(10, np.int32)
         d["exact"] = col(11, np.uint8)
+        d["affinity"] = col(12, np.int32)
         self._dirty = set()
         return d
 
@@ -122,6 +157,26 @@ class DriverTable(ResidentTable):
         s = self._next
         self._next += 1
         return s
+
+    def _aff_acquire(self, affinity):
+        key = affinity_key(affinity)
+        if key is None:
+            return -1
+        a = self._aff_id.get(key)
+        if a is None:
+            a = heapq.heappop(self._aff_free) if self._aff_free else self._aff_next
+            self._aff_next = max(self._aff_next, a + 1)
+            self._aff_id[key], self._aff_prog[a], self._aff_refs[a] = a, affinity, 0
+        self._aff_refs[a] += 1
+        return a
+
+    def _aff_release(self, a):
+        if a < 0:
+            return
+        self._aff_refs[a] -= 1
+        if self._aff_refs[a] == 0:
+            del self._aff_refs[a], self._aff_id[affinity_key(self._aff_prog.pop(a))]
+            heapq.heappush(self._aff_free, a)
 
     @staticmethod
     def _intern(table, name):
@@ -151,6 +206,7 @@ class DriverMirror:
             self.group = np.full(S, -1, np.int32)
             self.q = np.zeros((6, S), np.int64)
             self.count = np.zeros(S, np.int32)
+            self.affinity = np.full(S, -1, np.int32)
         s = np.asarray(d["slot"], np.int64)
         on = np.asarray(d["present"], np.uint8) != 0
         self.present[s] = on
@@ -161,6 +217,8 @@ class DriverMirror:
         for j, k in enumerate(DELTA_COLUMNS):
             self.q[j, s] = np.where(on, np.asarray(d[k], np.int64), 0)
         self.count[s] = np.where(on, np.asarray(d["min_executor_count"], np.int32), 0)
+        aff = d.get("affinity")
+        self.affinity[s] = np.where(on, np.asarray(aff, np.int32), -1) if aff is not None else -1
 
     def queue(self, requesting_slot=-1, scheduler=0, predicate_group=0, snapshot_group=None, enforce_after_ns=None, now=0):
         """The per-call queue of one gp_driver_queue: -> (queue_slot, apps, undefined_ties, inexact), apps the gp_apps columns
@@ -198,6 +256,23 @@ class DriverMirror:
         ties = int(np.sum((cre[1:] == cre[:-1]) & (apps["group"][1:] == apps["group"][:-1]))) if len(o) > 1 else 0
         inexact = bool(len(o) and not self.exact[o].all())
         return o.astype(np.int32), apps, ties, inexact
+
+    def stale(self, scheduler, timeout_ns, now, n_aff=None):
+        """The marker's sweep restated per call: the present rows of `scheduler` with creation + timeout_ns < now (Python
+        integers: exact), in (creation, slot) order.  -> (slots, apps, outside): apps the gp_apps columns (QUANTITIES, count
+        and group = the affinity id, -1 replaced by n_aff when given) of every stale row, outside = the row has exact = 0, a
+        negative quantity or a negative count (what the capacity check refuses)."""
+        live = np.flatnonzero(self.present & (self.scheduler == scheduler))
+        keep = [int(s) for s in live if int(self.creation[s]) + int(timeout_ns) < int(now)]
+        o = np.array(sorted(keep, key=lambda s: (int(self.creation[s]), s)), np.int64)
+        apps = {k: self.q[j, o].copy() for j, k in enumerate(QUANTITIES)}
+        apps["count"] = self.count[o].copy()
+        g = self.affinity[o].copy()
+        if n_aff is not None:
+            g[g == -1] = n_aff
+        apps["group"] = g
+        outside = ~self.exact[o] | (self.q[:, o] < 0).any(axis=0) | (self.count[o] < 0)
+        return o.astype(np.int32), apps, outside
 
     def _young(self, s, ages, now):
         """shouldSkipDriverFifo: creation + enforce-after age > now, with Python integers (exact)"""

@@ -707,13 +707,7 @@ private:
 // label_int_ok / label_int, metadata.name becomes a node index.  The same rules as affinity.encode() of the Python package.
 namespace affinity {
 
-struct Requirement { std::string Key, Operator; std::vector<std::string> Values; };   // v1.NodeSelectorRequirement
-struct Term { std::vector<Requirement> MatchExpressions, MatchFields; };              // v1.NodeSelectorTerm
-struct Program {                                   // pod.Spec.NodeSelector + RequiredDuringSchedulingIgnoredDuringExecution
-    std::map<std::string, std::string> NodeSelector;
-    bool HasRequired = false;                      // the required node selector is not nil
-    std::vector<Term> Terms;
-};
+// Requirement, Term and Program: spark_resources.hpp (a pending driver's QueuedDriverPod carries its Program)
 struct Node { std::string Name; std::map<std::string, std::string> Labels; };
 
 // strconv.ParseInt(s, 10, 64): an optional sign, then one or more ASCII digits, within int64
@@ -1686,6 +1680,7 @@ inline RescheduleOutcome RescheduleExecutor(const binpacker::Binpacker& packer, 
 }
 
 class ResidentOverheadComputer;
+class ResidentDrivers;
 
 // The unschedulable-pod marker's capacity checks (scanForUnschedulablePods, internal/extender/unschedulablepods.go:93-129) for
 // ALL stale drivers in one device call (gp_exceeds_cluster_capacity) instead of one DoesPodExceedClusterCapacity (:132-166) each.
@@ -1830,6 +1825,25 @@ public:
                                                     const std::vector<std::string>& zones, const std::vector<affinity::Program>& programs,
                                                     const std::vector<AffinityStaleDriver>& drivers, std::vector<bool>* affinityError) const;
 
+    // The whole scan from the resident driver table too (gp_exceeds_cluster_capacity_driver_table): the stale drivers of
+    // schedulerName (creation + timeout < now) are selected, ordered by (creation, slot) and checked on the device against
+    // each one's required affinity, which the driver table interns.  The overhead, label, node and driver tables are flushed
+    // once, then one call; a capacity refusal grows the output and calls again.  Any other refusal replays the four tables
+    // and answers with the per-call node-table affinity sweep above over the stale drivers decoded from the held pods.
+    // -> one entry per stale driver: Outcome 0 answered (Exceeds), 1 its affinity errors (ListWithPredicate fails), 2 outside
+    // the exact-int64 model (inexact, a negative quantity or count: the caller answers it with DoesPodExceedClusterCapacity).
+    struct StaleOutcome {
+        std::string UID;
+        bool Exceeds = false;
+        int32_t Outcome = 0;
+    };
+    std::vector<StaleOutcome> DoesPodsExceedClusterCapacity(ResidentDrivers& drivers, const std::string& schedulerName, int64_t timeoutNs,
+                                                            int64_t nowUnixNano, const std::vector<std::string>& names,
+                                                            resources::ResidentNodes& nodes, affinity::ResidentLabels& labels,
+                                                            ResidentOverheadComputer& overhead, const std::vector<std::string>& zones) const;
+    // true when the last driver-table scan was answered by the per-call path
+    bool LastScanFellBack() const { return fellBack_; }
+
 private:
     gp_binpacker Packer() const {
         if (packer_.Name == binpacker::tightlyPack) return GP_BP_TIGHTLY_PACK;
@@ -1839,6 +1853,8 @@ private:
         return GP_BP_DISTRIBUTE_EVENLY;                 // SelectBinpacker's default
     }
     binpacker::Binpacker packer_;
+    mutable int32_t staleCap_ = 64;                    // the driver-table scan's output size, grown on a capacity refusal
+    mutable bool fellBack_ = false;
 };
 
 // The failover reconciler's node choice (syncResourceReservationsAndDemands, internal/extender/failover.go:43-82):
@@ -2863,8 +2879,13 @@ public:
         for (int k = 0; k < 6; ++k) row.q[k] = q[k];
         row.count = (int32_t)r.MinExecutorCount;
         row.exact = r.Exact;
+        row.affinity = acquire(pod.Affinity);
         auto it = held_.find(pod.UID);
-        if (it != held_.end() && it->second.row == row && it->second.pod.CreationSeconds == pod.CreationSeconds) return;
+        if (it != held_.end()) release(it->second.row.affinity);
+        if (it != held_.end() && it->second.row == row && it->second.pod.CreationSeconds == pod.CreationSeconds) {
+            it->second.pod.Affinity = pod.Affinity;
+            return;
+        }
         int32_t slot;
         if (it != held_.end()) slot = it->second.slot;
         else if (!free_.empty()) { slot = *free_.begin(); free_.erase(free_.begin()); }
@@ -2876,6 +2897,7 @@ public:
     void DeleteDriver(const std::string& uid) {
         auto it = held_.find(uid);
         if (it == held_.end()) return;
+        release(it->second.row.affinity);
         dirty_.insert(it->second.slot);
         free_.insert(it->second.slot);
         uidAt_.erase(it->second.slot);
@@ -2913,18 +2935,49 @@ public:
     }
     bool Exact(const std::string& uid) const { return held_.at(uid).row.exact; }
     int32_t GroupID(const std::string& uid) const { return held_.at(uid).row.group; }
+    // the id of a scheduler name, -1 for a name no driver has carried (a sweep of it selects nothing)
+    int32_t SchedulerID(const std::string& name) const { auto it = schedulers_.find(name); return it == schedulers_.end() ? -1 : it->second; }
+    // the interned required affinities by id (an id no driver holds: a program that matches every node), the programs of a
+    // marker sweep; a driver's id is -1 when its Program matches every node
+    std::vector<affinity::Program> AffinityPrograms() const {
+        std::vector<affinity::Program> out((size_t)affNext_);
+        for (const auto& kv : affProg_) out[(size_t)kv.first] = kv.second;
+        return out;
+    }
+    int32_t AffinityID(const std::string& uid) const { return held_.at(uid).row.affinity; }
+    const std::string& UIDAt(int32_t slot) const { return uidAt_.at(slot); }
+    // The marker's stale drivers restated on the host from the held pods: scheduler id `scheduler`, creation + timeout < now
+    // (exactly), in (creation, slot) order; outside = exact false, a negative quantity or count
+    struct StaleRow { std::string UID; int32_t Affinity; bool Outside; ParsedSparkResources Parsed; };
+    std::vector<StaleRow> Stale(int32_t scheduler, int64_t timeoutNs, int64_t nowUnixNano) const {
+        std::vector<std::pair<std::pair<int64_t, int32_t>, const Held*>> keep;
+        for (const auto& kv : held_) {
+            const Row& r = kv.second.row;
+            if (r.scheduler == scheduler && (__int128)r.creation + (__int128)timeoutNs < (__int128)nowUnixNano)
+                keep.push_back({{r.creation, kv.second.slot}, &kv.second});
+        }
+        std::sort(keep.begin(), keep.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+        std::vector<StaleRow> out;
+        for (const auto& k : keep) {
+            const Row& r = k.second->row;
+            bool outside = !r.exact || r.count < 0;
+            for (int d = 0; d < 6; ++d) outside = outside || r.q[d] < 0;
+            out.push_back(StaleRow{k.second->pod.UID, r.affinity, outside, k.second->parsed});
+        }
+        return out;
+    }
 
     void Flush(gangpack::Device& dev) {
         Grow(size_.n_slots, next_);
         Grow(size_.n_groups, (int64_t)groups_.size());
         Grow(size_.n_schedulers, (int64_t)schedulers_.size());
-        std::vector<int32_t> slot, sched, group, count;
+        std::vector<int32_t> slot, sched, group, count, aff;
         std::vector<uint8_t> present, exact;
         std::vector<int64_t> creation, q[6];
         auto row = [&](int32_t s) {
             const Row r = record(s);
             slot.push_back(s); present.push_back(r.present); exact.push_back(r.exact); creation.push_back(r.creation);
-            sched.push_back(r.scheduler); group.push_back(r.group); count.push_back(r.count);
+            sched.push_back(r.scheduler); group.push_back(r.group); count.push_back(r.count); aff.push_back(r.affinity);
             for (int k = 0; k < 6; ++k) q[k].push_back(r.q[k]);
         };
         if (Replaying()) {
@@ -2937,7 +2990,8 @@ public:
             }
         }
         gp_driver_delta d{(int32_t)slot.size(), 0, slot.data(), present.data(), creation.data(), sched.data(), group.data(),
-                          q[0].data(), q[1].data(), q[2].data(), q[3].data(), q[4].data(), q[5].data(), count.data(), exact.data()};
+                          q[0].data(), q[1].data(), q[2].data(), q[3].data(), q[4].data(), q[5].data(), count.data(), exact.data(),
+                          aff.data()};
         Send(dev, gp_driver_table_reset, "gp_driver_table_reset", gp_driver_table_update, "gp_driver_table_update",
              slot.empty() ? nullptr : &d);
         for (int32_t s : slot) sent_[s] = record(s);
@@ -2952,12 +3006,52 @@ private:
         int64_t q[6] = {0, 0, 0, 0, 0, 0};
         int32_t count = 0;
         bool exact = false;
+        int32_t affinity = -1;
         bool operator==(const Row& o) const {
             for (int k = 0; k < 6; ++k) if (q[k] != o.q[k]) return false;
             return present == o.present && creation == o.creation && scheduler == o.scheduler && group == o.group && count == o.count &&
-                   exact == o.exact;
+                   exact == o.exact && affinity == o.affinity;
         }
     };
+    // a canonical key of a Program ("" when it matches every node: no nodeSelector and no required affinity)
+    static std::string affinityKey(const affinity::Program& p) {
+        if (p.NodeSelector.empty() && !p.HasRequired) return "";
+        std::string k;
+        auto put = [&](const std::string& x) { k += std::to_string(x.size()); k += ':'; k += x; };
+        for (const auto& kv : p.NodeSelector) { put(kv.first); put(kv.second); }
+        k += p.HasRequired ? "|R" : "|N";
+        for (const auto& t : p.Terms) {
+            for (const auto* part : {&t.MatchExpressions, &t.MatchFields}) {
+                k += '[';
+                for (const auto& r : *part) { put(r.Key); put(r.Operator); k += '('; for (const auto& v : r.Values) put(v); k += ')'; }
+                k += ']';
+            }
+        }
+        return k;
+    }
+    // the program's id, interned with a reference count (the lowest free id reused); -1 for one that matches every node
+    int32_t acquire(const affinity::Program& p) {
+        const std::string key = affinityKey(p);
+        if (key.empty()) return -1;
+        auto it = affId_.find(key);
+        if (it == affId_.end()) {
+            int32_t a;
+            if (!affFree_.empty()) { a = *affFree_.begin(); affFree_.erase(affFree_.begin()); }
+            else a = affNext_++;
+            it = affId_.emplace(key, a).first;
+            affProg_[a] = p;
+            affRefs_[a] = 0;
+        }
+        ++affRefs_[it->second];
+        return it->second;
+    }
+    void release(int32_t a) {
+        if (a < 0 || --affRefs_[a] > 0) return;
+        affId_.erase(affinityKey(affProg_.at(a)));
+        affProg_.erase(a);
+        affRefs_.erase(a);
+        affFree_.insert(a);
+    }
     struct Held { int32_t slot; Row row; QueuedDriverPod pod; ParsedSparkResources parsed; };
     static int32_t intern(std::map<std::string, int32_t>& t, const std::string& name) {
         auto it = t.find(name);
@@ -2975,6 +3069,11 @@ private:
     std::map<std::string, int32_t> schedulers_, groups_;
     std::set<int32_t> dirty_;
     std::map<int32_t, Row> sent_;
+    std::map<std::string, int32_t> affId_;       // affinityKey -> id
+    std::map<int32_t, affinity::Program> affProg_;
+    std::map<int32_t, int32_t> affRefs_;
+    std::set<int32_t> affFree_;
+    int32_t affNext_ = 0;
 };
 
 // What selectDriverNode's FIFO step decides for the requesting driver: fits (result = its packing), failure-fit (-1) or
@@ -3072,6 +3171,69 @@ inline DriverQueueOutcome FitEarlierDriversDriverTable(const binpacker::Binpacke
     FitEarlierDrivers(packer, {drivers.Pending(uid, false)}, nodeNames, executorNodeNames, metadata, &res);
     out.result = res[0];
     out.status = res[0].HasCapacity ? d.index(res[0].DriverNode) : -1;
+    return out;
+}
+
+inline std::vector<UnschedulablePodMarker::StaleOutcome> UnschedulablePodMarker::DoesPodsExceedClusterCapacity(
+        ResidentDrivers& drivers, const std::string& schedulerName, int64_t timeoutNs, int64_t nowUnixNano,
+        const std::vector<std::string>& names, resources::ResidentNodes& nodes, affinity::ResidentLabels& labels,
+        ResidentOverheadComputer& overhead, const std::vector<std::string>& zones) const {
+    gangpack::Device& dev = gangpack::Device::Get();
+    overhead.Flush(dev);
+    labels.Flush(dev);
+    nodes.Flush(dev);
+    drivers.Flush(dev);
+    const std::vector<affinity::Program> programs = drivers.AffinityPrograms();
+    const int32_t scheduler = drivers.SchedulerID(schedulerName);
+    std::vector<StaleOutcome> out;
+    fellBack_ = false;
+    {
+        const resources::NodeTableLabels z(labels, zones, "", {});
+        MarkerNodeTable t(names, nodes, overhead, z);
+        const affinity::Encoded e = labels.EncodePrograms(names, programs);
+        const gp_node_affinities p = e.Programs();
+        for (;;) {
+            const int32_t cap = staleCap_;
+            std::vector<int32_t> slot((size_t)cap + 1);
+            std::vector<uint8_t> exceeds((size_t)cap + 1), outcome((size_t)cap + 1);
+            int32_t n = 0;
+            const gp_stale_sweep sw{scheduler, cap, timeoutNs, nowUnixNano, slot.data(), exceeds.data(), outcome.data(), &n};
+            const gp_status st = gp_exceeds_cluster_capacity_driver_table(dev.ctx(), &t.nd, &p, &sw, Packer());
+            if (st == GP_ERR_CAPACITY && n > cap) { staleCap_ = n; continue; }
+            if (st != GP_OK) break;
+            for (int32_t i = 0; i < n; ++i) out.push_back(StaleOutcome{drivers.UIDAt(slot[(size_t)i]), exceeds[(size_t)i] != 0, outcome[(size_t)i]});
+            return out;
+        }
+    }
+    // refused: replay the four tables and answer per call over the held pods
+    fellBack_ = true;
+    overhead.Replay();
+    labels.Replay();
+    nodes.Replay();
+    drivers.Replay();
+    drivers.Flush(dev);
+    const std::vector<ResidentDrivers::StaleRow> stale = drivers.Stale(scheduler, timeoutNs, nowUnixNano);
+    std::vector<affinity::Program> progs = programs;
+    progs.push_back(affinity::Program{});              // matches every node: the drivers with affinity -1
+    std::vector<AffinityStaleDriver> answered;
+    for (const auto& r : stale) {
+        if (r.Outside) continue;
+        AffinityStaleDriver d;
+        const ParsedSparkResources& x = r.Parsed;
+        d.DriverResources = resources::CreateResources(x.DriverCPUMilli, x.DriverMemoryBytes, x.DriverNvidiaGPUs);
+        d.ExecutorResources = resources::CreateResources(x.ExecutorCPUMilli, x.ExecutorMemoryBytes, x.ExecutorNvidiaGPUs);
+        d.MinExecutorCount = (int)x.MinExecutorCount;
+        d.Affinity = r.Affinity < 0 ? (int)programs.size() : r.Affinity;
+        answered.push_back(d);
+    }
+    std::vector<bool> err;
+    const std::vector<bool> exceeds = DoesPodsExceedClusterCapacity(names, nodes, labels, overhead, zones, progs, answered, &err);
+    size_t j = 0;
+    for (const auto& r : stale) {
+        if (r.Outside) { out.push_back(StaleOutcome{r.UID, false, 2}); continue; }
+        out.push_back(StaleOutcome{r.UID, exceeds[j], err[j] ? 1 : 0});
+        ++j;
+    }
     return out;
 }
 

@@ -136,6 +136,17 @@ inline ParseStatus ParseQuantityScaled(const std::string& str, int scale, int64_
 
 }  // namespace resource
 
+// A pod's required node affinity as the host keeps it (the device form is gangpack_host.hpp's affinity::Encoded)
+namespace affinity {
+struct Requirement { std::string Key, Operator; std::vector<std::string> Values; };   // v1.NodeSelectorRequirement
+struct Term { std::vector<Requirement> MatchExpressions, MatchFields; };              // v1.NodeSelectorTerm
+struct Program {                                   // pod.Spec.NodeSelector + RequiredDuringSchedulingIgnoredDuringExecution
+    std::map<std::string, std::string> NodeSelector;
+    bool HasRequired = false;                      // the required node selector is not nil
+    std::vector<Term> Terms;
+};
+}  // namespace affinity
+
 namespace extender {
 
 // internal/common/constants.go:31-50
@@ -220,6 +231,7 @@ struct QueuedDriverPod {
     bool HasInstanceGroup = false;        // FindInstanceGroupFromPodSpec succeeded (podspec.go:29-35)
     std::string InstanceGroup;
     bool Deleting = false;                // DeletionTimestamp != nil
+    affinity::Program Affinity;           // Spec.NodeSelector + the required node affinity (empty: matches every node)
 };
 
 // filterToEarliestAndSort (sparkpods.go:54-74): the drivers that must fit before `driver` may be scheduled -- unscheduled,

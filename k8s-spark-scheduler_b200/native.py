@@ -48,7 +48,7 @@ EXPORTS = ["gp_abi_version", "gp_create", "gp_destroy", "gp_last_error", "gp_bac
            "gp_reconcile_find_nodes_node_table", "gp_exceeds_cluster_capacity_node_table",
            "gp_exceeds_cluster_capacity_affinity_node_table",
            "gp_driver_table_reset", "gp_driver_table_update", "gp_pack_fifo_driver_table",
-           "gp_pack_fifo_zones_groups_driver_table",
+           "gp_pack_fifo_zones_groups_driver_table", "gp_exceeds_cluster_capacity_driver_table",
            "gp_pack_fifo_zones_groups", "gp_prepare_cluster_zones_groups",
            "gp_prepare_cluster_groups", "gp_packing_efficiency_groups", "gp_placement_metrics", "gp_placement_metrics_device",
            "gp_multi_create", "gp_multi_destroy", "gp_multi_last_error", "gp_multi_size", "gp_multi_ctx",
@@ -321,7 +321,7 @@ class gp_driver_delta(C.Structure):
     _fields_ = [("n_write", C.c_int32), ("reserved", C.c_int32), ("slot", C.c_void_p), ("present", C.c_void_p),
                 ("creation", C.c_void_p), ("scheduler", C.c_void_p), ("group", C.c_void_p), ("drv_cpu_milli", C.c_void_p),
                 ("drv_mem_bytes", C.c_void_p), ("drv_gpu", C.c_void_p), ("exe_cpu_milli", C.c_void_p), ("exe_mem_bytes", C.c_void_p),
-                ("exe_gpu", C.c_void_p), ("min_executor_count", C.c_void_p), ("exact", C.c_void_p)]
+                ("exe_gpu", C.c_void_p), ("min_executor_count", C.c_void_p), ("exact", C.c_void_p), ("affinity", C.c_void_p)]
 
 
 class gp_driver_queue(C.Structure):
@@ -329,6 +329,11 @@ class gp_driver_queue(C.Structure):
                 ("snapshot_group", C.c_void_p), ("enforce_after_ns", C.c_void_p), ("now_unix_nano", C.c_int64),
                 ("queue_slot", C.c_void_p), ("exec_out_off", C.c_void_p), ("n_queued", C.c_void_p), ("n_executors", C.c_void_p),
                 ("undefined_ties", C.c_void_p)]
+
+
+class gp_stale_sweep(C.Structure):
+    _fields_ = [("scheduler", C.c_int32), ("cap", C.c_int32), ("timeout_ns", C.c_int64), ("now_unix_nano", C.c_int64),
+                ("stale_slot", C.c_void_p), ("exceeds", C.c_void_p), ("outcome", C.c_void_p), ("n_stale", C.c_void_p)]
 
 
 class gp_placement_record(C.Structure):
@@ -553,6 +558,9 @@ def load():
     L.gp_pack_fifo_zones_groups_driver_table.restype = C.c_int
     L.gp_pack_fifo_zones_groups_driver_table.argtypes = [C.c_void_p, C.POINTER(gp_driver_queue), C.c_int, C.c_int, C.c_void_p,
                                                          C.POINTER(gp_zone_results)]
+    L.gp_exceeds_cluster_capacity_driver_table.restype = C.c_int
+    L.gp_exceeds_cluster_capacity_driver_table.argtypes = [C.c_void_p, C.POINTER(gp_node_table_nodes), C.POINTER(gp_node_affinities),
+                                                           C.POINTER(gp_stale_sweep), C.c_int]
     _lib = L
     return L
 
@@ -572,7 +580,8 @@ def _triple(t):
 
 _DT_DELTA_COLS = {"slot": np.int32, "present": np.uint8, "creation": np.int64, "scheduler": np.int32, "group": np.int32,
                   "drv_cpu_milli": np.int64, "drv_mem_bytes": np.int64, "drv_gpu": np.int64, "exe_cpu_milli": np.int64,
-                  "exe_mem_bytes": np.int64, "exe_gpu": np.int64, "min_executor_count": np.int32, "exact": np.uint8}
+                  "exe_mem_bytes": np.int64, "exe_gpu": np.int64, "min_executor_count": np.int32, "exact": np.uint8,
+                  "affinity": np.int32}
 
 
 def _usage_input(alloc, overhead, res_node, res):
@@ -1658,6 +1667,30 @@ class GangPacker:
         out.update(zone=res["zone"][:n].copy(), driver_node=res["drv"][:n].copy(), executor_nodes=res["exe"][:out["n_executors"]].copy(),
                    avg_efficiency=res["avg"][:n].copy())
         return out
+
+    def exceeds_cluster_capacity_driver_table(self, nodes: dict, enc: dict, scheduler: int, timeout_ns: int, now: int, packer: int,
+                                              cap=None, retry=True) -> dict:
+        """gp_exceeds_cluster_capacity_driver_table: the marker's sweep over the driver table's stale rows (scheduler id,
+        creation + timeout_ns < now), nodes as in exceeds_cluster_capacity_affinity_node_table and enc the programs the
+        table's affinity ids index (drivers.DriverTable.affinity_programs encoded).  cap defaults to 64; with retry a
+        GP_ERR_CAPACITY is retried once with the size the call wrote back.  -> dict with stale_slot, exceeds and
+        outcome (0 answered, 1 affinity error, 2 outside the model) in (creation, slot) order."""
+        nt = _node_table_nodes(**dict({"reservation_id": None}, **nodes))
+        aff = _programs(enc)
+        cap = 64 if cap is None else int(cap)
+
+        def call(cap):
+            o = dict(slot=np.full(max(cap, 1), -9, np.int32), exceeds=np.full(max(cap, 1), 255, np.uint8),
+                     outcome=np.full(max(cap, 1), 255, np.uint8), n=C.c_int32(-9))
+            sw = gp_stale_sweep(scheduler=int(scheduler), cap=int(cap), timeout_ns=int(timeout_ns), now_unix_nano=int(now),
+                                stale_slot=_p(o["slot"]), exceeds=_p(o["exceeds"]), outcome=_p(o["outcome"]), n_stale=C.addressof(o["n"]))
+            return load().gp_exceeds_cluster_capacity_driver_table(self._h, C.byref(nt), C.byref(aff), C.byref(sw), int(packer)), o
+        st, o = call(cap)
+        if st == 5 and retry:
+            st, o = call(max(cap, o["n"].value))
+        self._check(st)
+        n = o["n"].value
+        return dict(stale_slot=o["slot"][:n].copy(), exceeds=o["exceeds"][:n].copy(), outcome=o["outcome"][:n].copy())
 
     # ---- bound calls: what a shim does -- marshal the argument structs ONCE over its long-lived buffers, then one FFI call
     # per Predicate (the numpy / ctypes marshalling of set_snapshot() / pack_batch() costs more than a small batch's kernels)
